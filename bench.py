@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py - clips/s of the NISQA predict hot path (BASELINE.json metric) on N B200s.
+"""bench.py - clips/s of the NISQA predict hot path (BASELINE.json metric) on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|reference-gpu]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|reference-gpu] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (BASELINE.json configs[1]): predict_dir bs=64, synthetic 10 s 48 kHz PCM16 clips,
@@ -17,7 +17,12 @@ engine stream), `cpu_baseline` = the oracle port on the host cores on a bounded 
 clip-parallel on all host cores) and prints the same line with "impl": "reference".
 `--impl reference-gpu` (and the `reference_gpu` key of the default line at N=1) times the UNMODIFIED
 reference torch modules in PyTorch eager on this GPU (tools/reference_gpu.py; SURVEY.md 8d's "honest thing to
-beat"), when the reference package was installed under baseline/_ref by __graft_entry__.build().
+beat"), with the copy of the reference package that __graft_entry__.build() puts under oracle/_ref (recipe
+oracle/build_ref.py; without a reference checkout the leg reports itself unavailable).
+`--dump-outputs DIR` writes what the timed path returned in its last timed step as DIR/<name>.npy: for the
+device-resident call scores.npy ([64, 5] float32), n_segments.npy and status.npy ([64], float64); the same three with
+the suffix _e2e for the host-buffer call; at N > 1 also scores_gathered.npy, the [N, 64, 5] table every rank receives.
+The clips are seeded, so the same arguments give the same inputs on every run and every build.
 """
 import argparse
 import json
@@ -35,7 +40,7 @@ sys.path.insert(0, ROOT)
 METRIC = "clips/sec (48 kHz, 10 s) NISQA v2.0 predict"
 UNIT = "clips/s"
 BS, SECONDS, SR = 64, 10.0, 48000
-N_ROT = 4                      # rotating batches: 4 x 61 MB PCM16 = 245 MB > 126 MB L2
+N_ROT = 4                      # rotating batches: 4 x 61 MB PCM16 = 245 MB > 50 MB L2
 CKPT = os.path.join(ROOT, "weights", "nisqa.tar")
 
 # algorithmic FLOPs per segment of each conv layer (SURVEY.md 8a row a10 / BASELINE.md section 3)
@@ -51,12 +56,12 @@ ATT_FLOP_PER_CLIP = 31.2e6
 SA_LAYER_FLOP_PER_CLIP = 55.6e6
 
 
-def build_rooflines(kernel_ms, peaks, sm_max_mhz, traffic_tab, n_samples):
+def build_rooflines(kernel_ms, peaks, sm_max_mhz, traffic_tab, n_samples, n_sm=132):
     """Per-kernel rooflines from CUDA-event kernel times (ms per 64-clip step).  Returns (all, dominant):
     `dominant` is the kernel with the largest share of the step.  Pure function (tests/test_host_logic.py
     replays a recorded bench line through it)."""
     n_seg_step = BS * SEGS_PER_CLIP
-    fp32_peak = 148 * 128 * 2 * (sm_max_mhz or 1965.0) * 1e6 / 1e12
+    fp32_peak = n_sm * 128 * 2 * (sm_max_mhz or 1980.0) * 1e6 / 1e12
     tc_layers = ("conv12", "conv2", "conv3", "conv4", "conv5", "conv6")
     roofs = {}
     for k in ("conv1",) + tc_layers:
@@ -69,12 +74,12 @@ def build_rooflines(kernel_ms, peaks, sm_max_mhz, traffic_tab, n_samples):
              "peak_source": peaks["source"] + ", sustained 16-bit dense (kernel timed inside a long step)",
              "kernel_ms": kernel_ms[k], "algorithmic_flop_per_launch": flop}
         if k in tc_layers:
-            r["note"] = ("tcgen05 kind::f16 implicit GEMM with a two-term fp16 split: 3 MMAs per algorithmic MAC "
+            r["note"] = ("wgmma f16 implicit GEMM with a two-term fp16 split: 3 MMAs per algorithmic MAC "
                          "(parity: plain 16-bit operands move MOS by >1e-3), so the tensor pipe executes 3x `achieved`")
             r["executed_tflops"] = 3 * ach
             r["frac_executed"] = 3 * ach / peaks["bf16_tflops_sustained"]
             if k == "conv12":
-                r["note"] = ("conv1 + pool1 (fp32 FFMA, producer warps) fused with conv2 + pool2 (tcgen05, fp16 two-term split) in one "
+                r["note"] = ("conv1 + pool1 (fp32 FFMA) fused with conv2 + pool2 (wgmma, fp16 two-term split) in one "
                              "persistent kernel: the pool1 activations never reach HBM; algorithmic FLOPs of both layers")
         else:
             r["note"] = "conv1 (C_in=1, K=9) is direct fp32 FFMA; fraction of the fp32 FFMA peak in frac_fp32"
@@ -89,7 +94,7 @@ def build_rooflines(kernel_ms, peaks, sm_max_mhz, traffic_tab, n_samples):
     # 8d's "STFT-bandwidth roofline" is kept beside it: hbm_gbs / hbm_frac say how far it is from being a copy)
     roofs["frontend"] = {"kernel": "frontend", "bound": "fp32-issue", "achieved": fft_tf, "peak": fp32_peak, "unit": "TFLOP/s",
                          "frac": fft_tf / fp32_peak, "traffic": traffic_tab.get("frontend"),
-                         "peak_source": "fp32 FFMA peak 148 SM x 128 lanes x 2 x SM clock", "kernel_ms": kernel_ms["frontend"],
+                         "peak_source": "fp32 FFMA peak %d SM x 128 lanes x 2 x SM clock" % n_sm, "kernel_ms": kernel_ms["frontend"],
                          "algorithmic_flop_per_launch": 136.7e6 * BS, "algorithmic_bytes_per_launch": byts,
                          "hbm_gbs": hbm, "hbm_peak_gbs": peaks["hbm_gbs"], "hbm_frac": hbm / peaks["hbm_gbs"],
                          "hbm_peak_source": peaks["source"],
@@ -101,8 +106,8 @@ def build_rooflines(kernel_ms, peaks, sm_max_mhz, traffic_tab, n_samples):
         att = ATT_FLOP_PER_CLIP * BS / (ms / 1e3) / 1e12
         roofs["sa_layer"] = {"kernel": "sa_layer", "bound": "tensor", "achieved": att, "peak": fp32_peak, "unit": "TFLOP/s",
                              "frac": att / fp32_peak, "traffic": traffic_tab.get("sa_layer"),
-                             "peak_source": "fp32 FFMA peak 148 SM x 128 lanes x 2 x SM clock (the kernel runs on the FFMA pipe, "
-                                            "no tensor cores: fp32 parity)",
+                             "peak_source": ("fp32 FFMA peak %d SM x 128 lanes x 2 x SM clock (the kernel runs on the FFMA pipe, "
+                                             "no tensor cores: fp32 parity)" % n_sm),
                              "kernel_ms": ms, "algorithmic_flop_per_launch": ATT_FLOP_PER_CLIP * BS,
                              "note": "attention-FLOP roofline of SURVEY 8d(iii): QK^T + PV only; with out-proj + FFN the same "
                                      "launches do %.1f TFLOP/s" % (SA_LAYER_FLOP_PER_CLIP * BS / (ms / 1e3) / 1e12)}
@@ -174,8 +179,8 @@ def measured_peaks():
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0,
+            "source": "H100 SXM data sheet (dense, 700 W; not measured)"}
 
 
 class CpuPool(object):
@@ -253,7 +258,7 @@ def _host_info():
 
 
 def load_traffic_table():
-    """Per-launch DRAM traffic (ncu dram__bytes_read + write) of the kernels, measured by tools/profile_round.sh and
+    """Per-launch DRAM traffic (ncu dram__bytes_read + write) of the kernels, written by tools/ncu_summary.py from an ncu export and
     stamped with the digest of the kernel sources it was measured on (nisqa_b200/build.py _digest).  ncu cannot run
     inside the bench, so a table taken on OTHER sources is refused: traffic is then null, never stale."""
     tp = os.path.join(ROOT, "profiles", "roofline_traffic.json")
@@ -450,9 +455,11 @@ def run_ours(a, rank, world, local):
         eng.set_gather_target(glob.data_ptr(), BS)
         gather = True
 
+    dev_aux = {}                                 # host outputs of the latest device-resident call
+
     def step_dev(i, sync=False):
-        eng.predict_pcm_device(dev_batches[i % N_ROT].data_ptr(), offs, n_s, srs, E.FMT_S16,
-                               scores_ring[i % 3].data_ptr(), sync=sync)
+        dev_aux["nseg"], dev_aux["status"] = eng.predict_pcm_device(dev_batches[i % N_ROT].data_ptr(), offs, n_s, srs,
+                                                                    E.FMT_S16, scores_ring[i % 3].data_ptr(), sync=sync)
 
     # e2e: the public streaming API - submit batch i (pinned host PCM16 -> H2D -> kernels -> D2H of the
     # scores), then collect batch i-1; two batches in flight, every step's copies inside the timed region
@@ -526,10 +533,24 @@ def run_ours(a, rank, world, local):
     mark0 = sampler.mark()
     ms_dev, _ = timed(step_dev, a.steps)
     launches = eng.kernel_launches() - l0
+    # what the last timed step returned to its caller: score rows, segment counts, per-clip status (and, at N > 1, the
+    # gathered [world, 64, n_out] table every rank receives)
+    dumps = {"scores": scores_ring[(a.steps - 1) % 3].cpu().numpy().copy(),
+             "n_segments": dev_aux["nseg"].astype(np.float64), "status": dev_aux["status"].astype(np.float64)}
+    if world > 1:
+        dumps["scores_gathered"] = glob.cpu().numpy().copy()
     for i in range(max(a.warmup, 4)):
         step_e2e(i)
     drain_e2e()
     ms_e2e, wall_e2e = timed(step_e2e, a.steps, drain_e2e)
+    k_last = (a.steps - 1) % NF
+    dumps["scores_e2e"] = e2e_scores[k_last].copy()
+    dumps["n_segments_e2e"] = e2e_aux[k_last][0].astype(np.float64)
+    dumps["status_e2e"] = e2e_aux[k_last][1].astype(np.float64)
+    if a.dump_outputs and rank == 0:
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        for k, v in dumps.items():          # scores float32, integer outputs as (exact) float64
+            np.save(os.path.join(a.dump_outputs, k + ".npy"), np.ascontiguousarray(v))
     clocks = sampler.stop(mark0, sampler.mark()) if rank == 0 else None
 
     # ---- per-kernel durations (CUDA events on the engine stream), same workload
@@ -583,7 +604,7 @@ def run_ours(a, rank, world, local):
             "config": {"workload": "predict_dir bs=64, synthetic 10 s 48 kHz PCM16 clips, weights/nisqa.tar "
                                    "(BASELINE.json configs[1]); one step = 64 clips per GPU",
                        "clips_per_step_per_gpu": BS, "segments_per_clip": SEGS_PER_CLIP,
-                       "l2": "inputs rotate over %d resident batches (%.0f MB PCM16 > 126 MB L2); per-step "
+                       "l2": "inputs rotate over %d resident batches (%.0f MB PCM16 > 50 MB L2); per-step "
                              "activations ~730 MB stream through L2" % (N_ROT, N_ROT * BS * stride * 2 / 1e6),
                        "exchange": "1 ncclAllGather of [64,5] rows per step" if world > 1 else "none (N=1)"},
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(BS * int(n_s[0]) * 2),
@@ -609,9 +630,15 @@ def main():
     ap.add_argument("--warmup-seconds", dest="warmup_seconds", type=float, default=1.5,
                     help="minimum duration of the untimed warm-up (in addition to --warmup steps)")
     ap.add_argument("--skip-cpu", dest="skip_cpu", action="store_true", help="omit the cpu_baseline leg (profiling runs)")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write what the last timed step returned (scores, segment counts, status) as DIR/<name>.npy")
     a = ap.parse_args()
     if a.steps is None:
         a.steps = 200 if a.impl == "ours" else 20
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
+    if a.dump_outputs and a.impl != "ours":
+        ap.error("--dump-outputs applies to --impl ours (the engine's timed path)")
     a.warmup = max(a.warmup, 3) if a.impl == "ours" else max(a.warmup, 0)
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
     if a.impl == "reference":

@@ -1,4 +1,4 @@
-/* nisqa_b200.h - C ABI of the B200-native NISQA predict engine (libnisqa_b200.so).
+/* nisqa_b200.h - C ABI of the H100-native NISQA predict engine (libnisqa_b200.so).
  *
  * Drop-in boundary (SURVEY.md 8b): the reference has no FFI; its seam for this path is the
  * Python function boundary
@@ -8,7 +8,7 @@
  * that seam - get_librosa_melspec (lib:2284-2331) minus the file decode, segment_specs
  * (lib:2239-2282), Framewise/AdaptCNN/StandardCNN (lib:428-836), SelfAttention/LSTM
  * (lib:897-1040), PoolAttFF/PoolLastStepBi (lib:1099-1183) and the NISQA / NISQA_DIM
- * containers (lib:29-268) - runs inside this library as hand-written sm_100a CUDA.
+ * containers (lib:29-268) - runs inside this library as hand-written sm_90a CUDA.
  *
  * Plain C types only: pointers and sizes, no torch types.  All functions return 0 on
  * success and a negative nisqa_status on failure; nisqa_last_error() gives the message.
@@ -265,15 +265,11 @@ NISQA_API int     nisqa_join(nisqa_engine* e);
  * groups: "frontend", "cnn", "td", "pool" */
 NISQA_API int    nisqa_set_profiling(nisqa_engine* e, int on);
 /* kernel-variant switches for A/B measurements and the parity tests:
- *   "conv_tc"    bit mask of the conv layers (2..6) that run as tcgen05 implicit GEMMs with the fp16
- *                two-term split (default / 1 = all of them); a cleared bit selects the fp32 FFMA kernel.
- *   "conv_split" 1 (default): with all of conv2..6 on tcgen05, activations travel between the layers as
- *                fp16 hi/lo plane pairs (csrc/conv_split.cu); 0: fp32 channels-last activations and the
- *                register-staged kernels of csrc/conv_tc.cu.  Results are bit-identical.
- *   "conv12"     1 (default): conv1 + pool1 + conv2 + pool2 run as ONE persistent kernel (csrc/conv12.cu), the pool1
+ *   "conv_tc"    1 (default): conv2..6 run as wgmma implicit GEMMs with the fp16 two-term split, activations
+ *                travelling between the layers as fp16 hi/lo plane pairs (csrc/conv_split.cu); 0: fp32 FFMA kernels.
+ *   "conv12"     1 (default): conv1 + pool1 + conv2 + pool2 run as ONE kernel (csrc/conv_split.cu), the pool1
  *                activations never reach HBM (NISQA_STAGE_POOL1 is then not dumpable); 0: separate kernels.
- *   "conv_pipe"  bit mask of the conv layers (2..6) whose plane kernel runs as persistent warp-specialised CTAs
- *                (default / 1 = all); a cleared bit selects the one-tile-per-CTA kernel.  Bit-identical results.
+ *                Bit-identical results.
  *   "fe_ppc"     frame pairs per front-end CTA (0 = kernel default).
  *   "td_tiled"   1 (default): time-dependency block + pooling logits as register-tiled GEMM kernels
  *                (csrc/td_tiled.cu); 0: the one-thread-per-row kernels of csrc/td.cu.

@@ -1,5 +1,5 @@
 """Host-side mirror of the reference's predict seam (reference nisqa/NISQA_lib.py:1420-1467,
-2052-2236) with the hot path replaced by the B200 engine.
+2052-2236) with the hot path replaced by the engine.
 
 Same names, argument meaning and error behaviour as the reference so that
 ``nisqaModel.predict()`` reads the same:
@@ -43,7 +43,7 @@ class SpeechQualityDataset(object):
             # the reference indexes df[None] here (lib:2133) - predict_file / predict_dir have no reference column
             raise KeyError(filename_column_ref)
         if mos_column != "predict_only":
-            raise NotImplementedError("only predict_only datasets are on the B200 path")
+            raise NotImplementedError("only predict_only datasets are on the engine path")
         if transform is not None or to_memory:
             raise NotImplementedError("transform / to_memory are training-side options")
         self.df = df

@@ -1,4 +1,4 @@
-"""``nisqaModel`` for the B200 engine - the predict side of the reference driver class
+"""``nisqaModel`` for the engine - the predict side of the reference driver class
 (reference nisqa/NISQA_model.py:21-81, 732-847, 928-1051) with the same constructor argument
 dict, the same ``predict()`` surface (prints, ``NISQA_results.csv``, returned DataFrame) and the
 same precedence of checkpoint args vs. CLI args, but with the torch modules replaced by
@@ -41,7 +41,7 @@ class nisqaModel(object):
 
     # ------------------------------------------------------------------ out of scope
     def train(self):
-        raise NotImplementedError("training is outside the B200 predict path (SURVEY.md section 2, #15)")
+        raise NotImplementedError("training is outside the predict path (SURVEY.md section 2, #15)")
 
     # ------------------------------------------------------------------ evaluate (model:48-52, 572-715)
     def evaluate(self, mapping="first_order", do_print=True, do_plot=False):
@@ -111,7 +111,7 @@ class nisqaModel(object):
         elif mode == "predict_csv":
             self._loadDatasetsCSVpredict()
         elif mode == "main":
-            raise NotImplementedError("mode 'main' (training CSVs) is outside the B200 predict path")
+            raise NotImplementedError("mode 'main' (training CSVs) is outside the predict path")
         else:
             raise NotImplementedError("mode not available")
 
@@ -159,7 +159,7 @@ class nisqaModel(object):
     # ------------------------------------------------------------------ model (model:928-1030)
     def _loadModel(self):
         if not self.args.get("pretrained_model"):
-            raise NotImplementedError("the B200 engine only runs pretrained checkpoints")
+            raise NotImplementedError("the engine only runs pretrained checkpoints")
         if os.path.isabs(self.args["pretrained_model"]):
             model_path = os.path.join(self.args["pretrained_model"])
         else:
@@ -195,9 +195,9 @@ class nisqaModel(object):
     # ------------------------------------------------------------------ device (model:1032-1051)
     def _getDevice(self):
         if self.args.get("tr_device") == "cpu":
-            raise RuntimeError("the B200 engine has no CPU path (tr_device='cpu' requested)")
+            raise RuntimeError("the engine has no CPU path (tr_device='cpu' requested)")
         if not torch.cuda.is_available():
-            raise RuntimeError("no CUDA device available: the B200 engine has no CPU fallback")
+            raise RuntimeError("no CUDA device available: the engine has no CPU fallback")
         _, world, local = nb_dist.env_world()
         idx = local if world > 1 else torch.cuda.current_device()
         torch.cuda.set_device(idx)

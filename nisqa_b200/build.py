@@ -1,4 +1,4 @@
-"""Builds nisqa_b200/libnisqa_b200.so in-tree with nvcc for sm_100a (no GPU needed to build).
+"""Builds nisqa_b200/libnisqa_b200.so in-tree with nvcc for sm_90a (no GPU needed to build).
 
     python -m nisqa_b200.build [--force]
 """
@@ -12,8 +12,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libnisqa_b200.so")
 STAMP = os.path.join(HERE, ".libnisqa_b200.stamp")
-SOURCES = ["engine.cu", "frontend.cu", "cnn.cu", "conv_tc.cu", "conv_split.cu", "conv12.cu", "td.cu", "td_tiled.cu", "wavio.cpp", "flac.cpp", "resample.cpp", "resample_gpu.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+SOURCES = ["engine.cu", "frontend.cu", "cnn.cu", "conv_split.cu", "td.cu", "td_tiled.cu", "wavio.cpp", "flac.cpp", "resample.cpp", "resample_gpu.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--shared"]
 
 

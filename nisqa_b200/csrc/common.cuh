@@ -1,4 +1,4 @@
-// common.cuh - shared device structs / helpers for the sm_100a NISQA kernels.
+// common.cuh - shared device structs / helpers for the sm_90a NISQA kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

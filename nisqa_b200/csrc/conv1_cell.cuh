@@ -1,5 +1,5 @@
 // conv1_cell.cuh - conv1(1->16) + BN + ReLU fused with the first max-pool for ONE pooled cell of one segment (all 16
-// channels), shared by conv1_pool1_kernel (cnn.cu) and the fused conv1 + conv2 kernel (conv12.cu).
+// channels), shared by conv1_pool1_kernel (cnn.cu) and the fused conv1 + conv2 kernel (conv_split.cu).
 //   MODE 0 (adapt, reference lib:690-691): adaptive_max_pool2d 48x15 -> 24x7 : rows {2i,2i+1}, cols [2j,2j+3)
 //   MODE 1 (standard, lib:813-814): MaxPool2d(2, stride 2, padding (0,1)) -> 24x8 : cols {2j-1,2j}
 #pragma once
@@ -7,7 +7,7 @@
 #include "f32x2.cuh"
 
 #ifndef NISQA_C1_PK
-#define NISQA_C1_PK 1        // conv1 FMAs as packed FFMA2 (bit-identical to the scalar form)
+#define NISQA_C1_PK 1        // conv1 FMAs over channel pairs (f32x2.cuh; bit-identical to the scalar form)
 #endif
 
 namespace nisqa {
@@ -35,8 +35,7 @@ __device__ __forceinline__ void conv1_cell(const float* __restrict__ mel, int f0
     }
 
 #if NISQA_C1_PK
-  // 16 channels as 8 packed pairs (FFMA2: the same fp32 FMA per element and tap order as the scalar form, half the
-  // instructions - the producer warps of conv12 are issue bound)
+  // 16 channels as 8 pairs (the same fp32 FMA per element and tap order as the scalar form)
 #pragma unroll
   for (int cq_ = 0; cq_ < NCQ; ++cq_) {
     const int cq = cq0 + cq_;

@@ -32,22 +32,13 @@ void launch_conv1(cudaStream_t, int, const float*, const int*, const float*, con
                   const float*, float*, int, void*, void*);
 void launch_conv_layer(cudaStream_t, int, int, const float*, const float*, const float*, float*, int);
 void launch_nhwc_to_nchw(cudaStream_t, const float*, float*, long long, int, int);
-// conv_tc.cu
-void launch_conv_tc(cudaStream_t, int, int, const float*, const void*, const float*, float, float*, int);
 // conv_split.cu
 size_t split_plane_bytes(int std_mode, int layer, int n_seg);
 void launch_conv_split(cudaStream_t, int, int, const void*, const void*, const void*, const float*, float,
-                       void*, void*, float*, int, int);
+                       void*, void*, float*, int);
 void launch_unsplit(cudaStream_t, int, int, const void*, const void*, float*, int);
-// conv12.cu
 void launch_conv12(cudaStream_t, int, const float*, const int*, const float*, const float*, const float*, const void*,
                    const float*, float, void*, void*, int);
-#ifdef NISQA_TC_TIMING
-int tc_timing_read(long long*, int);
-int sp_timing_read(long long*, int);
-int pipe_timing_read(long long*, int, int);
-int c12_timing_read(long long*, int, int);
-#endif
 // td.cu
 struct SaLayerParams {
   const float* WoT; const float* bo; const float* W1T; const float* b1; const float* W2T;
@@ -200,15 +191,12 @@ struct nisqa_engine {
   bool weights_loaded = false;
   bool profiling = false;
   int fe_ppc = 0;          // frame pairs per front-end CTA (0: kernel default)
-  int conv12 = 1;          // conv1 + pool1 + conv2 + pool2 in one persistent kernel (conv12.cu): pool1 never reaches HBM
+  int conv12 = 1;          // conv1 + pool1 + conv2 + pool2 in one kernel (conv_split.cu): pool1 never reaches HBM
   bool last_conv12 = false;
-  int conv_pipe = 0x78;    // bit l (conv2's small tiles are faster one per CTA, four CTAs per SM): conv2..6 plane kernels as persistent warp-specialised CTAs (conv_pipe_kernel); 0: one tile per CTA
-  int conv_split = 1;      // conv2..6 exchange activations as fp16 hi/lo plane pairs (conv_split.cu); needs conv_tc == 0x7c
-  int tc_timing_layer = 0; // NISQA_TC_TIMING builds: the layer whose CTAs record their phase stamps
   bool last_split = false; // the last pass ran the plane pipeline (stage dumps convert back to fp32)
   int lstm_batched = 1;    // BiLSTM: NB clips per CTA in lock step (td.cu lstm_batched_kernel); 0: one CTA per (clip, direction)
   int keep_td_out = 0;     // standard arch: also write the per-step LSTM outputs [n_seg][256] (only the stage dump reads them)
-  int conv_tc = 0x7c;      // bit l set: conv layer l (2..6) runs on tcgen05 (fp16 two-term split); else fp32 FFMA
+  int conv_tc = 1;         // 1: conv2..6 on the tensor cores (fp16 two-term split, fp16 plane pairs between the layers); 0: fp32 FFMA
   std::vector<TimerSlot> timers;
 
   // weights arena (device) + offsets
@@ -540,7 +528,7 @@ int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
   }
   for (int i = 1; conv_net && i <= 6; ++i)
     if (!pack_conv(P, i, cin[i], cout[i])) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-  // conv2..conv6 for the tcgen05 path: [tap][ci/8][hi co | lo co][8] fp16 two-term split of w * 2^S
+  // conv2..conv6 for the tensor-core path: [tap][ci/8][hi co | lo co][8] fp16 two-term split of w * 2^S
   for (int i = 2; conv_net && i <= 6; ++i) {
     char k1[32], k2[32];
     snprintf(k1, sizeof k1, "conv%d.w", i); snprintf(k2, sizeof k2, "conv%d.wtc", i);
@@ -909,7 +897,7 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
     const int FEAT = std_mode ? 768 : 384;
     CK(LN.mel.reserve((size_t)n_frames * kMels * 4));
     CK(LN.segtab.reserve((size_t)n_seg * 12));
-    const bool split = e->conv_split && e->conv_tc == 0x7c;
+    const bool split = e->conv_tc != 0;
     e->last_split = split;
     const bool conv_net = c.cnn_kind == NISQA_CNN_CONV;
     if (!conv_net) {
@@ -989,10 +977,7 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
         if (split)
           launch_conv_split(st, std_mode, l, plane_hi(l), plane_lo(l), W(e, kt), W(e, kb), e->tc_scale[l],
                             l < 6 ? plane_hi(l + 1) : nullptr, l < 6 ? plane_lo(l + 1) : nullptr,
-                            l == 6 ? LN.feats.as<float>() : nullptr, n_seg,
-                            (e->tc_timing_layer == l ? 2 : 0) | (((e->conv_pipe >> l) & 1) ? 4 : 0));
-        else if (e->conv_tc & (1 << l))
-          launch_conv_tc(st, std_mode, l, cin_[l], W(e, kt), W(e, kb), e->tc_scale[l], cout_[l], n_seg);
+                            l == 6 ? LN.feats.as<float>() : nullptr, n_seg);
         else
           launch_conv_layer(st, std_mode, l, cin_[l], W(e, kw), W(e, kb), cout_[l], n_seg);
       }
@@ -1151,8 +1136,8 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
     for (int i = 0; i < n_clips; i += 2)
       if (!plan[i].run || !plan[i + 1].run) plan[i].run = plan[i + 1].run = 0;      // the pair scores NaN
   }
-  // segments per internal pass: 131072 segments keep ~8 GB of activation planes per compute lane (sized for the
-  // 180 GB of a B200) and give the BiLSTM >= 128 clips per launch at configs[3]; one 64-clip batch is 15 808
+  // segments per internal pass: 131072 segments keep ~8 GB of activation planes per compute lane (three lanes stay
+  // well inside the 80 GB of an H100) and give the BiLSTM >= 128 clips per launch at configs[3]; one 64-clip batch is 15 808
   const int max_seg = e->cfg.max_chunk_segments > 0 ? e->cfg.max_chunk_segments : 131072;
   float* scores_all = scores_dev;
   if (!scores_all) {
@@ -1281,7 +1266,7 @@ int nisqa_create(nisqa_engine** out, int device, const nisqa_config* cfg) {
   CK(cudaSetDevice(device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major < 10) return fail(e, NISQA_ERR_CUDA, "libnisqa_b200 is compiled for sm_100a only");
+  if (prop.major != 9 || prop.minor != 0) return fail(e, NISQA_ERR_CUDA, "libnisqa_b200 is compiled for sm_90a (H100) only");
   CK(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
   for (auto& l : e->lanes) CK(cudaStreamCreateWithFlags(&l.stream, cudaStreamNonBlocking));
   for (auto& g : e->stages) {
@@ -1583,14 +1568,11 @@ int nisqa_join(nisqa_engine* e) {
 
 int nisqa_set_option(nisqa_engine* e, const char* name, int value) {
   if (!e || !name) return NISQA_ERR_INVALID;
-  if (strcmp(name, "conv_tc") == 0) { e->conv_tc = (value == 1) ? 0x7c : (value & 0x7c); return 0; }
+  if (strcmp(name, "conv_tc") == 0) { e->conv_tc = value != 0; return 0; }
   if (strcmp(name, "fe_ppc") == 0) { e->fe_ppc = value; return 0; }
   if (strcmp(name, "lstm_batched") == 0) { e->lstm_batched = value != 0; return 0; }
   if (strcmp(name, "keep_td_out") == 0) { e->keep_td_out = value != 0; return 0; }
   if (strcmp(name, "conv12") == 0) { e->conv12 = value != 0; return 0; }
-  if (strcmp(name, "conv_split") == 0) { e->conv_split = value != 0; return 0; }
-  if (strcmp(name, "conv_pipe") == 0) { e->conv_pipe = (value == 1) ? 0x78 : (value & 0x7c); return 0; }
-  if (strcmp(name, "tc_timing_layer") == 0) { e->tc_timing_layer = value; return 0; }
   return fail(e, NISQA_ERR_INVALID, std::string("unknown option ") + name);
 }
 
@@ -1717,18 +1699,3 @@ int nisqa_gather_nccl(nisqa_engine* e, void* nccl_comm, const float* local_dev, 
 }
 
 }  // extern "C"
-
-#ifdef NISQA_TC_TIMING
-extern "C" __attribute__((visibility("default"))) int nisqa_debug_tc_timing(long long* host, int n) {
-  return nisqa::tc_timing_read(host, n);
-}
-extern "C" __attribute__((visibility("default"))) int nisqa_debug_sp_timing(long long* host, int n) {
-  return nisqa::sp_timing_read(host, n);
-}
-extern "C" __attribute__((visibility("default"))) int nisqa_debug_pipe_timing(long long* host, int n, int reset) {
-  return nisqa::pipe_timing_read(host, n, reset);
-}
-extern "C" __attribute__((visibility("default"))) int nisqa_debug_c12_timing(long long* host, int n, int reset) {
-  return nisqa::c12_timing_read(host, n, reset);
-}
-#endif

@@ -1,16 +1,13 @@
-// f32x2.cuh - packed fp32 arithmetic of sm_100 (PTX fma/add/sub/mul.rn.f32x2 -> SASS FFMA2 / FADD2 / FMUL2): two
-// independent IEEE fp32 operations per instruction on an aligned register pair.  The fp32 pipe's lane rate is unchanged
-// (measured 122 of 128 FMA lanes / clk / SM with FFMA2 vs 100 with scalar FFMA, profiles/r02o_ffma2_probe.txt) but
-// every packed instruction frees an issue slot, which is what bounds the front-end FFT, conv1 and the fp32 tile GEMMs
-// of the time-dependency block.  Every lane result is the correctly rounded fp32 result of the same scalar operation:
-// a kernel that replaces fmaf(a, b, c) pairs by fma2 is bit-identical.  ptxas folds a pair built from one scalar
-// (`pk(a, a)`) into the instruction's scalar-broadcast operand form (`R.F32`): no extra moves.
+// f32x2.cuh - pairs of fp32 values carried in one 64-bit register pair (.x in the low register, .y in the high one):
+// the front-end FFT, conv1 and the fp32 tile GEMMs of the time-dependency block are written over such pairs.  sm_90
+// has no packed fp32 instructions, so every pair operation is two scalar IEEE fp32 operations: each lane result is
+// the correctly rounded fp32 result of the same scalar operation, exactly as a kernel written with fmaf directly.
 #pragma once
 #include <cuda_runtime.h>
 
 namespace nisqa {
 
-typedef unsigned long long f2;      // two packed floats: .x in the low register, .y in the high one
+typedef unsigned long long f2;      // two floats: .x in the low register, .y in the high one
 
 __device__ __forceinline__ f2 pk(float lo, float hi) {
   f2 r;
@@ -25,23 +22,32 @@ __device__ __forceinline__ float2 upk(f2 v) {
   return r;
 }
 __device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) {
-  f2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  const float2 x = upk(a), y = upk(b), z = upk(c);
+  return pk(fmaf(x.x, y.x, z.x), fmaf(x.y, y.y, z.y));
 }
 __device__ __forceinline__ f2 mul2(f2 a, f2 b) {
-  f2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  const float2 x = upk(a), y = upk(b);
+  return pk(__fmul_rn(x.x, y.x), __fmul_rn(x.y, y.y));
 }
 __device__ __forceinline__ f2 add2(f2 a, f2 b) {
-  f2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  const float2 x = upk(a), y = upk(b);
+  return pk(__fadd_rn(x.x, y.x), __fadd_rn(x.y, y.y));
 }
 __device__ __forceinline__ f2 sub2(f2 a, f2 b) {
+  const float2 x = upk(a), y = upk(b);
+  return pk(__fsub_rn(x.x, y.x), __fsub_rn(x.y, y.y));
+}
+
+// c ? a : b as a register select.  Written as `c ? x[i] : x[j]` on two array elements, the compiler may turn the choice
+// into a load from a computed address, which keeps the whole array in local memory.
+__device__ __forceinline__ f2 sel(bool c, f2 a, f2 b) {
   f2 r;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
+  asm("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %3, 0;\n\tselp.b64 %0, %1, %2, p;\n\t}" : "=l"(r) : "l"(a), "l"(b), "r"((int)c));
+  return r;
+}
+__device__ __forceinline__ float sel(bool c, float a, float b) {
+  float r;
+  asm("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %3, 0;\n\tselp.f32 %0, %1, %2, p;\n\t}" : "=f"(r) : "f"(a), "f"(b), "r"((int)c));
   return r;
 }
 

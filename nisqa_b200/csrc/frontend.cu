@@ -14,8 +14,7 @@
 #include "common.cuh"
 #include "f32x2.cuh"
 
-// experiment switches (tools/tc_ab_build.sh builds variant libraries); defaults = the measured winners, profiles/r02q_ab_kernels.txt:
-// packing the FFT butterflies made the kernel 5 % slower (it is latency bound at five warps per scheduler, not issue bound)
+// experiment switches (-DNAME=value when building a variant library); the defaults are the variants the kernel is tuned with
 #ifndef NISQA_FE_PK_FFT
 #define NISQA_FE_PK_FFT 0      // butterflies / twiddle products as packed FADD2 / FMUL2 / FFMA2
 #endif
@@ -100,9 +99,11 @@ __device__ __forceinline__ void fft32(f2 (&x)[32]) {
 // The same transform as decimation in TIME: input n sits at x[rev5(n)], X[k] ends up in x[k].  A butterfly with a
 // non-trivial twiddle is out1 = a + w b (4 FMAs), out2 = 2 a - out1 (2 FMAs) instead of add, subtract and a 4-instruction
 // complex product; 34 of the 80 butterflies of a 32-point transform have one.
-__device__ __forceinline__ void fft32_dit(f2 (&x)[32]) {
-#pragma unroll
-  for (int half = 1; half <= 16; half <<= 1) {
+// One stage per template instance: every loop has a compile-time trip count, so the array indices are constants and
+// `x` stays in registers (a stage loop over `half` is not fully unrolled by the sm_90 compiler, which puts x in local memory).
+template <int HALF>
+__device__ __forceinline__ void fft32_dit_stage(f2 (&x)[32]) {
+  constexpr int half = HALF;
 #pragma unroll
     for (int base = 0; base < 32; base += 2 * half) {
 #pragma unroll
@@ -124,7 +125,13 @@ __device__ __forceinline__ void fft32_dit(f2 (&x)[32]) {
         }
       }
     }
-  }
+}
+__device__ __forceinline__ void fft32_dit(f2 (&x)[32]) {
+  fft32_dit_stage<1>(x);
+  fft32_dit_stage<2>(x);
+  fft32_dit_stage<4>(x);
+  fft32_dit_stage<8>(x);
+  fft32_dit_stage<16>(x);
 }
 
 // slot of input / output index i in the register array handed to the 32-point transform
@@ -147,6 +154,28 @@ __device__ __forceinline__ int reflect_index(int i, int n) {
   int m = i % period;
   if (m < 0) m += period;
   return (m < n) ? m : period - m;
+}
+
+// One step of a multi-value butterfly reduction across the lanes: lane L keeps slot i or i + O (bit O of L / S) and sends
+// the other to its partner at lane distance O * S.  A template per step keeps the trip counts constant, so that `v`
+// stays in registers (a loop over O is not fully unrolled by the sm_90 compiler, which puts v in local memory).
+template <int O, int S = 1, int N>
+__device__ __forceinline__ void fold_step(float (&v)[N], int lane) {
+  const bool up = (lane & (O * S)) != 0;
+#pragma unroll
+  for (int i = 0; i < O; ++i) {
+    const float lo = v[i], hi = v[i + O];
+    v[i] = sel(up, hi, lo) + __shfl_xor_sync(0xffffffffu, sel(up, lo, hi), O * S);
+  }
+}
+template <int O, int S = 1, int N>
+__device__ __forceinline__ void fold_step(f2 (&v)[N], int lane) {
+  const bool up = (lane & (O * S)) != 0;
+#pragma unroll
+  for (int i = 0; i < O; ++i) {
+    const f2 lo = v[i], hi = v[i + O];
+    v[i] = add2(sel(up, hi, lo), __shfl_xor_sync(0xffffffffu, sel(up, lo, hi), O * S));
+  }
 }
 
 template <typename T> __device__ __forceinline__ float sample_to_float(T v);
@@ -238,16 +267,7 @@ __device__ __forceinline__ float mel_bands(const float2* scratch, const int* ban
     v[2 * slot] = s0;
     v[2 * slot + 1] = s1;
   }
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) {
-    const bool up = (lane & o) != 0;
-#pragma unroll
-    for (int i = 0; i < o; ++i) {
-      const float keep = up ? v[i + o] : v[i];
-      const float send = up ? v[i] : v[i + o];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
-    }
-  }
+  fold_step<16>(v, lane); fold_step<8>(v, lane); fold_step<4>(v, lane); fold_step<2>(v, lane); fold_step<1>(v, lane);
   float out = -INFINITY;
   const int my_slot = lane >> 1, f = lane & 1;
   if (lane < 2 * (kMels / 4) && (f == 0 || validB)) {
@@ -334,16 +354,7 @@ __device__ __forceinline__ float mel_bands_staged(const float2* scratch, const i
   }
   // multi-value butterfly over the 12 (padded to 16) packed values: after the steps with lane offsets 16, 8, 4, 2 lane L
   // holds the value of slot (L >> 1) & ... summed over 16 lanes; the last step adds the partner lane (L ^ 1)
-#pragma unroll
-  for (int o = 8; o >= 1; o >>= 1) {
-    const bool up = (lane & (2 * o)) != 0;
-#pragma unroll
-    for (int i = 0; i < o; ++i) {
-      const f2 keep = up ? v[i + o] : v[i];
-      const f2 send = up ? v[i] : v[i + o];
-      v[i] = add2(keep, __shfl_xor_sync(0xffffffffu, send, 2 * o));
-    }
-  }
+  fold_step<8, 2>(v, lane); fold_step<4, 2>(v, lane); fold_step<2, 2>(v, lane); fold_step<1, 2>(v, lane);
   const float2 tot = upk(add2(v[0], __shfl_xor_sync(0xffffffffu, v[0], 1)));
   // lane L now holds slot s(L) = bit-reversal free index: bits 4..1 of L select the slot (offset 16 -> +8, 8 -> +4, ...)
   float out = -INFINITY;

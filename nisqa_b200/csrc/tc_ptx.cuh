@@ -1,12 +1,11 @@
-// tc_ptx.cuh - PTX wrappers shared by the tcgen05 conv kernels (mbarrier, cp.async.bulk, tcgen05
-// alloc / mma / commit / ld, shared-memory matrix descriptors) and the two-term fp16 split.
+// tc_ptx.cuh - PTX wrappers shared by the tensor-core conv kernels (mbarrier, cp.async.bulk, ldmatrix, Hopper
+// wgmma with the A operand in registers and B through a shared-memory matrix descriptor) and the two-term fp16 split.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
 
 namespace nisqa {
 
-// ------------------------------------------------------------------ PTX helpers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -30,99 +29,63 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if (!done && ++spins > (1u << 26)) __trap();
   } while (!done);
 }
-// The same wait for roles whose wake-up latency is not on the critical path (whole warps of producers / epilogue that poll
-// together): a failed poll is followed by a short sleep, so that waiting warps leave the issue slots of their scheduler to
-// the warps that have work (NISQA_MBAR_SLEEP ns; 0 = plain polling).
-#ifndef NISQA_MBAR_SLEEP
-#define NISQA_MBAR_SLEEP 0
-#endif
-__device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity) {
-#if NISQA_MBAR_SLEEP > 0
-  uint32_t done;
-  uint32_t spins = 0;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    if (!done) {
-      __nanosleep(NISQA_MBAR_SLEEP);
-      if (++spins > (1u << 24)) __trap();
-    }
-  } while (!done);
-#else
-  mbar_wait(bar, parity);
-#endif
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// named barrier over a subset of the CTA's warps (id 1..15; 0 is __syncthreads)
-__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n_threads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n_threads) : "memory");
-}
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
-// shared -> global bulk store (bulk async-group completion); sizes / addresses are multiples of 16 bytes
-__device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// generic-proxy accesses of this thread -> ordered before later async-proxy (bulk copy) accesses of the same memory
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (fp16 inputs, fp32 accumulate), one thread
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// 32 lanes x 32 columns of fp32 accumulators -> 32 registers per thread
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+// four 8x8 b16 matrices; lane l supplies the row address of matrix l / 8, row l % 8
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
 }
 
-// 32 lanes x 16 columns, no wait (pair with tmem_ld_wait)
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// two-term fp16 split of 8 consecutive channels -> two 16-byte core-matrix rows
+// B operand: K-major, no swizzle: core matrices of 8 rows x 16 bytes, rows 16 B apart, 8-row groups SBO = 128 B apart
+// along N, K-adjacent core matrices LBO bytes apart
+__device__ __forceinline__ uint64_t make_desc_b(uint32_t saddr, uint32_t lbo_bytes) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(128u >> 4) << 32);
+}
+
+// D[64 x N] (fp32, registers of the warpgroup) += A[64 x 16] (fp16, registers: the mma.m16n8k16 A fragment of the
+// warp's 16 rows) * B[16 x N] (fp16, shared memory descriptor)
+template <int N>
+__device__ __forceinline__ void wgmma_rs(float* d, const uint32_t (&a)[4], uint64_t b_desc);
+template <> __device__ __forceinline__ void wgmma_rs<32>(float* d, const uint32_t (&a)[4], uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15"
+      "}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
+}
+
+template <> __device__ __forceinline__ void wgmma_rs<64>(float* d, const uint32_t (&a)[4], uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
+      "}, {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
+}
+
+
+// two-term fp16 split of 8 consecutive channels -> two 16-byte rows
 __device__ __forceinline__ void split8(const float4& a, const float4& b, uint4& hi, uint4& lo) {
   const float x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
   uint32_t h[4], l[4];
@@ -136,22 +99,6 @@ __device__ __forceinline__ void split8(const float4& a, const float4& b, uint4& 
   }
   hi = make_uint4(h[0], h[1], h[2], h[3]);
   lo = make_uint4(l[0], l[1], l[2], l[3]);
-}
-
-// K-major, no swizzle: ((8,m),(8,2)):((16B,SBO),(2B,LBO)); version 1 (sm_100)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) |
-         ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46);
-}
-
-
-// K-major with the hardware swizzle: rows of ROWB = 32 / 64 / 128 bytes, 8-row groups at SBO = 8 * ROWB;
-// layout type 6 / 4 / 2 = SWIZZLE_32B / 64B / 128B in bits 61..63, LBO unused (a K-step of 32 bytes never
-// leaves the swizzle atom).  The XOR is a function of the absolute shared-memory address (measured: a
-// start address shifted by whole rows or by 32 bytes addresses the same tile, base_offset stays 0).
-__device__ __forceinline__ uint64_t make_desc_swz(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-         (1ull << 46) | ((uint64_t)layout << 61);
 }
 
 }  // namespace nisqa

@@ -543,19 +543,23 @@ void launch_pool_simple(cudaStream_t st, const float* x, int D, const ClipDesc* 
 template <int NB> constexpr int lstm_batched_smem() { return (2 * 64 * 256 + 2 * NB * 128 + 2 * NB * 32 + NB * 128) * 4; }
 
 // `order`: device array of the pass's clip indices sorted by decreasing n_seg (host-built, run_pass); the batch
-// width follows the number of sequences per SM: 148 SMs x NB sequences per direction pair of CTAs in one wave
+// width follows the number of sequences per SM: n_SM x NB sequences per direction pair of CTAs in one wave
 void launch_lstm_batched(cudaStream_t st, const float* feats20, const ClipDesc* clips, const int* order, int n_clips,
                          const LstmParams& P, float* td_out, float* partial, float pool_bias, float* scores) {
   static unsigned long long cfg = 0;
+  static int n_sm = 132;
   if (first_launch_on_device(cfg)) {
     cudaFuncSetAttribute(lstm_batched_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm_batched_smem<1>());
     cudaFuncSetAttribute(lstm_batched_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm_batched_smem<2>());
     cudaFuncSetAttribute(lstm_batched_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm_batched_smem<4>());
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   }
   const int seqs = 2 * n_clips;
-  if (seqs <= 148)
+  if (seqs <= n_sm)
     lstm_batched_kernel<1><<<2 * n_clips, 256, lstm_batched_smem<1>(), st>>>(feats20, clips, order, n_clips, P, td_out, partial);
-  else if (seqs <= 2 * 148)
+  else if (seqs <= 2 * n_sm)
     lstm_batched_kernel<2><<<2 * ((n_clips + 1) / 2), 256, lstm_batched_smem<2>(), st>>>(feats20, clips, order, n_clips, P, td_out, partial);
   else
     lstm_batched_kernel<4><<<2 * ((n_clips + 3) / 4), 256, lstm_batched_smem<4>(), st>>>(feats20, clips, order, n_clips, P, td_out, partial);

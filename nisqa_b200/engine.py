@@ -148,7 +148,7 @@ def config_from_args(args, max_chunk_segments=0):
     kernels do not implement (no fallback)."""
     cnn, td, pool = args.get("cnn_model"), args.get("td"), args.get("pool")
     if args.get("model") not in ("NISQA", "NISQA_DIM", "NISQA_DE"):
-        raise NotImplementedError("Model not available in the B200 engine: %r" % args.get("model"))
+        raise NotImplementedError("Model not available in the engine: %r" % args.get("model"))
     de = args.get("model") == "NISQA_DE"
     pool_mode = {"avg": POOL_AVG, "max": POOL_MAX, "last_step": POOL_LAST_STEP, "last_step_bi": POOL_LAST_STEP_BI}.get(pool)
     if pool == "att":
@@ -157,9 +157,9 @@ def config_from_args(args, max_chunk_segments=0):
         elif args.get("pool_att_h") in (None, 0):
             pool_mode = POOL_ATT
         else:
-            raise NotImplementedError("pool_att_h=%r is not implemented by the B200 engine (128 or None)" % args.get("pool_att_h"))
+            raise NotImplementedError("pool_att_h=%r is not implemented by the engine (128 or None)" % args.get("pool_att_h"))
     if pool_mode is None:
-        raise NotImplementedError("Pool option not available in the B200 engine: %r" % pool)
+        raise NotImplementedError("Pool option not available in the engine: %r" % pool)
     cnn_kind, cnn_fc = CNN_CONV, 0
     if (cnn, td) == ("adapt", "self_att") and pool_mode != POOL_LAST_STEP_BI:
         arch = ARCH_ADAPT_SA_ATTFF
@@ -168,7 +168,7 @@ def config_from_args(args, max_chunk_segments=0):
               and args["td_sa_d_model"] == 64 and args["td_sa_nhead"] == 1 and args["td_sa_h"] == 64)
         cnn_fc = int(args.get("cnn_fc_out_h") or 0)           # optional Linear behind conv6 (lib:682-684)
         if cnn_fc % 64 != 0:
-            raise NotImplementedError("cnn_fc_out_h=%d: the B200 engine needs a multiple of 64" % cnn_fc)
+            raise NotImplementedError("cnn_fc_out_h=%d: the engine needs a multiple of 64" % cnn_fc)
     elif cnn in (None, "skip", "dff") and td == "self_att" and pool_mode != POOL_LAST_STEP_BI:
         # framewise models without convolutions (lib:504-583) in front of the self-attention stack
         arch = ARCH_ADAPT_SA_ATTFF
@@ -177,7 +177,7 @@ def config_from_args(args, max_chunk_segments=0):
         if cnn_kind == CNN_DFF and cnn_fc == 0:
             cnn_fc = 4096                                   # DFF's default hidden width (lib:544)
         if cnn_fc % 64 != 0:
-            raise NotImplementedError("cnn_fc_out_h=%d: the B200 engine needs a multiple of 64" % cnn_fc)
+            raise NotImplementedError("cnn_fc_out_h=%d: the engine needs a multiple of 64" % cnn_fc)
         ok = args["td_sa_d_model"] == 64 and args["td_sa_nhead"] == 1 and args["td_sa_h"] == 64
     elif (cnn, td) == ("standard", "lstm") and pool_mode in (POOL_LAST_STEP_BI, POOL_AVG, POOL_MAX, POOL_LAST_STEP):
         arch = ARCH_STD_LSTM_LASTBI
@@ -186,7 +186,7 @@ def config_from_args(args, max_chunk_segments=0):
               and args["model"] == "NISQA")
     else:
         raise NotImplementedError(
-            "architecture cnn=%r td=%r pool=%r is not implemented by the B200 engine" % (cnn, td, pool))
+            "architecture cnn=%r td=%r pool=%r is not implemented by the engine" % (cnn, td, pool))
     ks = args.get("cnn_kernel_size")
     ok = ok and (ks == 3 or tuple(ks) == (3, 3))
     if de:
@@ -195,11 +195,11 @@ def config_from_args(args, max_chunk_segments=0):
         if arch != ARCH_ADAPT_SA_ATTFF:
             raise NotImplementedError("NISQA_DE is implemented for cnn_model='adapt', td='self_att'")
         if args.get("de_align") not in DE_ALIGN:
-            raise NotImplementedError("de_align=%r is not implemented by the B200 engine (dot, cosine, distance, luong, bahd)" % (args.get("de_align"),))
+            raise NotImplementedError("de_align=%r is not implemented by the engine (dot, cosine, distance, luong, bahd)" % (args.get("de_align"),))
         if args.get("de_align_apply") not in DE_APPLY or args.get("de_fuse") not in DE_FUSE:
             raise NotImplementedError("de_align_apply / de_fuse option not available: %r / %r" % (args.get("de_align_apply"), args.get("de_fuse")))
         if args.get("de_fuse_dim") and int(args["de_fuse_dim"]) % 64 != 0:
-            raise NotImplementedError("de_fuse_dim=%r: the B200 engine needs a multiple of 64" % (args.get("de_fuse_dim"),))
+            raise NotImplementedError("de_fuse_dim=%r: the engine needs a multiple of 64" % (args.get("de_fuse_dim"),))
         ok = ok and args.get("td_2") == "self_att" and args.get("td_2_sa_d_model") == 64 and args.get("td_2_sa_nhead") == 1 \
             and args.get("td_2_sa_h") == 64
     elif args.get("td_2") == "self_att":

@@ -6,7 +6,7 @@ reference`` legs may import it, and only as the checker / the thing timed as the
 CPU baseline.
 
 PARITY UNPINNED (front-end half).  The arithmetic restated here lives in a
-third-party dependency that is not vendored under ``/root/reference``:
+third-party dependency that is not vendored in the reference project:
 ``librosa==0.8.1`` (reference ``env.yml:16``; with ``numpy==1.20.3`` FFT,
 ``scipy=1.7.3`` ``get_window``, ``libsndfile=1.0.31``).  It cannot be installed in
 this environment and the reference ships no golden vectors / tests for this

@@ -1,7 +1,7 @@
 """Generate tests/golden/eval_golden.json from the UNMODIFIED reference statistics functions
 (``nisqa.NISQA_lib.eval_results`` and helpers, reference lib:1469-1852); runs only in the build container.
 
-    python -m oracle.make_eval_golden            # needs /root/reference (read-only)
+    python -m oracle.make_eval_golden            # needs the reference checkout ($NISQA_REFERENCE_DIR, read-only)
 
 Inputs: a seeded synthetic listening-test table (3 databases with 4-6 conditions, per-file and
 per-condition MOS / dimension labels with confidence intervals, predictions = labels + noise + a
@@ -19,7 +19,9 @@ import sys
 import numpy as np
 import pandas as pd
 
-REF = "/root/reference"
+from oracle.build_ref import reference_dir
+
+REF = reference_dir()     # the reference checkout ($NISQA_REFERENCE_DIR); exits with a message when absent
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import librosa_compat  # noqa: E402

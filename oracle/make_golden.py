@@ -1,8 +1,8 @@
 """Generate tests/golden/*.npz from the UNMODIFIED reference (runs only in the build container).
 
-    python -m oracle.make_golden            # needs /root/reference (read-only)
+    python -m oracle.make_golden            # needs the reference checkout ($NISQA_REFERENCE_DIR, read-only)
 
-The reference package is imported as-is from /root/reference with ``librosa`` replaced by
+The reference package is imported as-is from $NISQA_REFERENCE_DIR with ``librosa`` replaced by
 ``oracle/librosa_compat.py`` (real librosa 0.8.1 is not installable offline - the front-end
 half therefore stays "parity unpinned") and a ``matplotlib.pyplot`` stub.  Everything
 downstream of the mel-dB tensor - ``segment_specs``, ``SpeechQualityDataset``, the
@@ -18,7 +18,9 @@ import tempfile
 import numpy as np
 import torch
 
-REF = "/root/reference"
+from oracle.build_ref import reference_dir
+
+REF = reference_dir()     # the reference checkout ($NISQA_REFERENCE_DIR); exits with a message when absent
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 

@@ -1,6 +1,6 @@
 """tests/golden/variants.npz and variants_de.npz from the UNMODIFIED reference modules (runs only in the build container).
 
-    python -m oracle.make_variant_golden            # needs /root/reference (read-only)
+    python -m oracle.make_variant_golden            # needs the reference checkout ($NISQA_REFERENCE_DIR, read-only)
 
 For every variant of oracle/variants.py a temporary checkpoint ({'args', 'model_state_dict'}) is written and scored by
 the reference's own ``nisqaModel(args).predict()`` (strict ``load_state_dict`` into the reference's NISQA / NISQA_DIM
@@ -14,7 +14,9 @@ import tempfile
 import numpy as np
 import torch
 
-REF = "/root/reference"
+from oracle.build_ref import reference_dir
+
+REF = reference_dir()     # the reference checkout ($NISQA_REFERENCE_DIR); exits with a message when absent
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 

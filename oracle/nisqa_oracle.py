@@ -10,7 +10,7 @@ function citing the reference ``file:line`` it follows (``lib`` = nisqa/NISQA_li
 
 Pinning status
   * model half (segments -> scores): PINNED against the unmodified reference modules imported
-    from ``/root/reference`` (``oracle/make_golden.py`` -> ``tests/golden/*.npz``,
+    from the reference checkout (``oracle/make_golden.py`` -> ``tests/golden/*.npz``,
     checked by ``tests/test_oracle_golden.py``).
   * front-end half (samples -> mel dB): PARITY UNPINNED - see ``oracle/librosa_compat.py``.
 

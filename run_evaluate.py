@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""Scores a labelled corpus with the B200 engine and prints the reference's evaluation statistics
+"""Scores a labelled corpus with the engine and prints the reference's evaluation statistics
 (reference run_evaluate.py: predict_csv, then per-database Pearson / RMSE / mapped RMSE / RMSE*).
 
     python run_evaluate.py --pretrained_model weights/nisqa.tar --data_dir corpus --csv_file NISQA_corpus_file.csv \
@@ -15,7 +15,7 @@ from nisqa_b200.NISQA_model import nisqaModel
 
 
 def parse_args(argv=None):
-    ap = argparse.ArgumentParser(description="NISQA evaluation on B200")
+    ap = argparse.ArgumentParser(description="NISQA evaluation on H100")
     ap.add_argument("--pretrained_model", required=True)
     ap.add_argument("--data_dir", required=True)
     ap.add_argument("--csv_file", required=True, help="per-file table (paths + labels)")

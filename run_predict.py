@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""Command line of the B200 NISQA engine.
+"""Command line of the H100 NISQA engine.
 
 Flag-compatible with the reference CLI (reference run_predict.py:8-43): the three predict modes
 and the same option names, so existing invocations keep working:
@@ -37,7 +37,7 @@ _NEEDS = {
 
 
 def parse_args(argv=None):
-    parser = argparse.ArgumentParser(description="NISQA speech quality prediction on B200")
+    parser = argparse.ArgumentParser(description="NISQA speech quality prediction on H100")
     for name, (typ, default, text) in _OPTIONS.items():
         parser.add_argument("--" + name, type=typ, default=default, required=name in _REQUIRED, help=text)
     args = vars(parser.parse_args(argv))

@@ -12,7 +12,7 @@ WEIGHTS = os.path.join(ROOT, "weights")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100")
 
 
 @pytest.fixture(scope="session")

@@ -1,4 +1,4 @@
-"""CPU-side checks of the C-ABI boundary: the library builds for sm_100a, loads, exports every
+"""CPU-side checks of the C-ABI boundary: the library builds for sm_90a, loads, exports every
 symbol include/nisqa_b200.h declares, its pure-host entry points agree with the oracle, and the
 product path fails loudly without a GPU (no CPU fallback)."""
 import ctypes

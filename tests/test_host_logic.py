@@ -8,7 +8,7 @@ import sys
 import numpy as np
 import pytest
 
-from conftest import ROOT
+from conftest import GOLDEN, ROOT
 from nisqa_b200 import dist as nb_dist
 from nisqa_b200 import wav
 from oracle import librosa_compat as lb
@@ -328,15 +328,16 @@ def test_bench_reference_arm_contract():
 
 
 def test_bench_rooflines_replay_recorded_line():
-    """bench.build_rooflines is a pure function of the per-kernel CUDA-event times: replaying the recorded
-    r01e line (profiles/r01e_bench_n1.json, measured on a B200) must reproduce its roofline entries, name the
-    same dominant kernel, and carry the attention-FLOP roofline of SURVEY 8d(iii)."""
+    """bench.build_rooflines is a pure function of the per-kernel CUDA-event times: replaying a fixed bench line
+    (tests/golden/bench_line_replay.json: synthetic kernel times, roofline entries computed from the algorithmic FLOP /
+    byte counts) must reproduce its roofline entries, name the same dominant kernel, and carry the attention-FLOP
+    roofline of SURVEY 8d(iii)."""
     import importlib.util
     import json
     spec = importlib.util.spec_from_file_location("nisqa_bench", os.path.join(ROOT, "bench.py"))
     bench = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(bench)
-    rec = json.load(open(os.path.join(ROOT, "profiles", "r01e_bench_n1.json")))
+    rec = json.load(open(os.path.join(GOLDEN, "bench_line_replay.json")))
     peaks = {"hbm_gbs": rec["roofline"]["peak"], "bf16_tflops_sustained": rec["roofline_kernels"]["conv4"]["peak"],
              "bf16_tflops": 0.0, "source": "measured (MEASURED_PEAKS.json)"}
     traffic = {k: v["traffic"] for k, v in rec["roofline_kernels"].items()}

@@ -4,8 +4,8 @@ lib:1441-1467) with the rows sharded over the ranks (``dist.shard_rows``) and ON
 rows through the engine (``_predict_all`` -> ``dist.all_gather_scores`` -> ``nisqa_gather_nccl``).
 
 The gathered table must be BIT-identical to the single-process run (clips are independent units; sharding only
-changes which GPU computes a row) and within 1e-4 of the oracle.  Needs >= 2 GPUs on the box
-(``gpurun --gpus 2 -- 'python -m pytest tests/test_multi_gpu.py -m gpu -q'``); the world_size-2 ``gloo`` twin of the
+changes which GPU computes a row) and within 1e-4 of the oracle.  Needs >= 2 GPUs
+(``python -m pytest tests/test_multi_gpu.py -m gpu -q``); the world_size-2 ``gloo`` twin of the
 host logic runs on the CPU in tests/test_host_logic.py.
 """
 import os
@@ -39,7 +39,7 @@ def _run(cmd, timeout=150):       # (a hang must fail fast: GPU-box minutes are 
     return r
 
 
-@pytest.mark.skipif(_n_gpus() < 2, reason="needs two GPUs on the box (gpurun --gpus 2)")
+@pytest.mark.skipif(_n_gpus() < 2, reason="needs two GPUs")
 def test_predict_csv_sharded_equals_single_rank(tmp_path, built_lib):
     from oracle import nisqa_oracle as O
     rng = np.random.default_rng(3)

@@ -1,5 +1,5 @@
 """Pins the oracle's model half to the UNMODIFIED reference modules: tests/golden/*.npz were
-produced by oracle/make_golden.py running /root/reference's nisqaModel.predict() (reference
+produced by oracle/make_golden.py running the reference's nisqaModel.predict() (reference
 nisqa/NISQA_model.py:54-81) with forward hooks on model.cnn / model.time_dependency."""
 import os
 

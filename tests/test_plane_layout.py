@@ -1,11 +1,11 @@
-"""Executable specification of the fp16 plane layout that carries activations between the tcgen05 conv layers
+"""Executable specification of the fp16 plane layout that carries activations between the tensor-core conv layers
 (csrc/conv_split.cu) - a NumPy emulation of the index arithmetic of those kernels, checked
 against torch's conv2d on the CPU:
 
   * plane row / swizzle addressing, hi/lo split and its round trip (what conv1 / the epilogues write and
     launch_unsplit reads back),
   * a CTA's tile = one contiguous byte range of a plane, placed at row offset g0 & 7 of a 1024-byte aligned
-    buffer, read back through the absolute-address swizzle the UMMA descriptors apply (measured on B200),
+    buffer, read back through the same absolute-address swizzle the kernel applies to its ldmatrix addresses,
   * the implicit GEMM over row-shifted tiles (9 taps) == conv2d(padding=1), positions x channels, with the
     epilogue's row <-> (segment, h, w) map, pooling and the centre-column pick of conv6.
 

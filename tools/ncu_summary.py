@@ -1,4 +1,4 @@
-"""Turns an `ncu --page raw --csv` export of one bench step (tools/profile_round.sh) into the tracked
+"""Turns an `ncu --page raw --csv` export of one bench step (`ncu --page raw --csv python bench.py --steps 1`) into the tracked
 summary profiles/<tag>_ncu_full_one_step.csv and refreshes profiles/roofline_traffic.json.
 
     python tools/ncu_summary.py gpurun_out/r01d_full_raw.csv r01d

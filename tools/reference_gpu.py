@@ -1,4 +1,4 @@
-"""The reference's OWN torch modules on the B200 (PyTorch eager, ``dev=cuda``) - SURVEY.md 8(d)'s "reference on
+"""The reference's OWN torch modules on this GPU (PyTorch eager, ``dev=cuda``) - SURVEY.md 8(d)'s "reference on
 this GPU" row, the honest thing the hand-written engine has to beat.
 
     python tools/reference_gpu.py [--clips 64] [--workers N]        (prints one JSON object)
@@ -7,9 +7,8 @@ this GPU" row, the honest thing the hand-written engine has to beat.
 What runs is the UNMODIFIED reference package (``nisqa/NISQA_model.py`` + ``nisqa/NISQA_lib.py``) through its own
 public API ``nisqaModel(args).predict()`` -> ``NL.predict_dim(model, ds, bs, dev, num_workers)`` (reference
 lib:1441-1467) with the device it picks itself (CUDA when available, model:1036-1045).  The package is not part of
-this repository: ``__graft_entry__.build()`` installs a copy of ``/root/reference/nisqa`` under ``baseline/_ref/``
-(git-ignored, travels to the GPU box with the snapshot) when ``/root/reference`` exists; without it this module
-reports ``{"unavailable": ...}``.  ``librosa`` is not installable offline, so the reference's
+this repository: ``__graft_entry__.build()`` copies it to ``oracle/_ref/nisqa`` (recipe ``oracle/build_ref.py``,
+git-ignored) where a reference checkout exists; without it this module reports ``{"unavailable": ...}``.  ``librosa`` is not installable offline, so the reference's
 ``lb.load / melspectrogram / amplitude_to_db`` calls land in ``oracle/librosa_compat.py`` (NumPy restatement of
 librosa 0.8.1) - stated in the output.  Nothing of the product (engine, kernels, native wav reader) is on this path.
 
@@ -32,23 +31,9 @@ import time
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
-
-
-def install_reference(src="/root/reference"):
-    """Copy of the reference package for the GPU box (pure Python, no build metadata: `pip install --target`
-    has nothing to build, the package directory IS the install).  No-op without the source tree."""
-    pkg = os.path.join(src, "nisqa")
-    if not os.path.isdir(pkg):
-        return False
-    dst = os.path.join(REF_DIR, "nisqa")
-    os.makedirs(REF_DIR, exist_ok=True)
-    if os.path.isdir(dst):
-        shutil.rmtree(dst)
-    shutil.copytree(pkg, dst)          # as it lies: a namespace package (no __init__.py), nothing added or edited
-    return True
 
 
 def available():
@@ -111,7 +96,7 @@ def measure(n_clips=64, bs=64, seconds=10.0, sr=48000, workers=None, ckpt=None, 
     """-> dict (see module docstring).  ``ours``: optional callable(list of wav paths) -> [n, 5] scores of the
     engine on the same files, for the |delta| column."""
     if not available():
-        return {"unavailable": "baseline/_ref/nisqa is absent (installed by __graft_entry__.build() where /root/reference exists)"}
+        return {"unavailable": "oracle/_ref/nisqa is absent (made by __graft_entry__.build() where a reference checkout exists)"}
     import torch
     cuda = torch.cuda.is_available()
     if not cuda and not allow_cpu:           # allow_cpu: plumbing test of this module in the build container
@@ -216,11 +201,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--clips", type=int, default=64)
     ap.add_argument("--workers", type=int, default=None)
-    ap.add_argument("--install", action="store_true", help="copy /root/reference/nisqa to baseline/_ref and exit")
     a = ap.parse_args()
-    if a.install:
-        print(json.dumps({"installed": install_reference()}))
-        return
     print(json.dumps(measure(n_clips=a.clips, workers=a.workers)))
 
 

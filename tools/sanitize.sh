@@ -1,9 +1,9 @@
 #!/bin/bash
 # GPU-box memory / race / init check of every kernel on the default path (SURVEY.md section 5: the reference has no
 # sanitizer story; this is ours): compute-sanitizer memcheck over __graft_entry__.smoke() (nisqa.tar, two
-# short clips at 48 / 16 kHz: front-end, conv1, the five tcgen05 conv layers with their bulk copies /
-# mbarriers / TMEM, self-attention, pooling) and over a short nisqa_tts.tar call (StandardCNN, BiLSTM).
-#   gpurun --timeout 300 -- 'bash tools/sanitize.sh r01e'
+# short clips at 48 / 16 kHz: front-end, conv1, the five wgmma conv layers with their bulk copies /
+# mbarriers, self-attention, pooling) and over a short nisqa_tts.tar call (StandardCNN, BiLSTM).
+#   bash tools/sanitize.sh TAG
 TAG=${1:-rXX}
 OUT=gpurun_out
 mkdir -p $OUT
