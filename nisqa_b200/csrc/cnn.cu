@@ -30,7 +30,8 @@ __global__ void __launch_bounds__(256)
 conv1_pool1_kernel(const float* __restrict__ mel, const int* __restrict__ seg_frame0,
                    const float* __restrict__ seg_thr, const float* __restrict__ w1 /*[9][16]*/,
                    const float* __restrict__ b1 /*[16]*/, float* __restrict__ out,
-                   unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo, int n_seg) {
+                   unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo,
+                   float store_scale /*2^-e1*/, int n_seg) {
   constexpr int PW = (MODE == 0) ? 7 : 8;
   __shared__ __align__(16) float ws[9 * 16 + 16];
   for (int i = threadIdx.x; i < 9 * 16 + 16; i += blockDim.x)
@@ -53,7 +54,7 @@ conv1_pool1_kernel(const float* __restrict__ mel, const int* __restrict__ seg_fr
     for (int c = 0; c < 2; ++c) {
       uint4 hi, lo;
       split8(make_float4(res[8 * c], res[8 * c + 1], res[8 * c + 2], res[8 * c + 3]),
-             make_float4(res[8 * c + 4], res[8 * c + 5], res[8 * c + 6], res[8 * c + 7]), hi, lo);
+             make_float4(res[8 * c + 4], res[8 * c + 5], res[8 * c + 6], res[8 * c + 7]), store_scale, hi, lo);
       size_t o = (size_t)g * 32 + (size_t)c * 16;
       o ^= (o >> 3) & 16;                          // Swizzle<1,4,3>
       *reinterpret_cast<uint4*>(out_hi + o) = hi;
@@ -267,18 +268,19 @@ static void launch_conv(cudaStream_t st, const float* in, const float* w, const 
 
 void launch_conv1(cudaStream_t st, int std_mode, const float* mel, const int* seg_frame0,
                   const float* seg_thr, const float* w1, const float* b1, float* out, int n_seg,
-                  void* out_hi, void* out_lo) {
+                  void* out_hi, void* out_lo, float store_scale) {
   const int cells = std_mode ? 24 * 8 : 24 * 7;
   const long long total = (long long)n_seg * cells;
   const int grid = (int)((total + 255) / 256);
   unsigned char* oh = static_cast<unsigned char*>(out_hi);
   unsigned char* ol = static_cast<unsigned char*>(out_lo);
+  const float s = store_scale;
   if (out_hi) {
-    if (std_mode) conv1_pool1_kernel<1, true><<<grid, 256, 0, st>>>(mel, seg_frame0, seg_thr, w1, b1, out, oh, ol, n_seg);
-    else conv1_pool1_kernel<0, true><<<grid, 256, 0, st>>>(mel, seg_frame0, seg_thr, w1, b1, out, oh, ol, n_seg);
+    if (std_mode) conv1_pool1_kernel<1, true><<<grid, 256, 0, st>>>(mel, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
+    else conv1_pool1_kernel<0, true><<<grid, 256, 0, st>>>(mel, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
   } else {
-    if (std_mode) conv1_pool1_kernel<1, false><<<grid, 256, 0, st>>>(mel, seg_frame0, seg_thr, w1, b1, out, oh, ol, n_seg);
-    else conv1_pool1_kernel<0, false><<<grid, 256, 0, st>>>(mel, seg_frame0, seg_thr, w1, b1, out, oh, ol, n_seg);
+    if (std_mode) conv1_pool1_kernel<1, false><<<grid, 256, 0, st>>>(mel, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
+    else conv1_pool1_kernel<0, false><<<grid, 256, 0, st>>>(mel, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
   }
 }
 

@@ -6,7 +6,10 @@
 //      a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi          (dropped a_lo*b_lo ~ 2^-22 |a b|)
 // The main accumulator only ever sees the hi*hi products; hi*lo and lo*hi go to a second, small accumulator, and the
 // epilogue adds the two.  The weights are pre-scaled by 2^S on the host (S chosen per layer so that max|w| 2^S <= 1024)
-// to keep b_lo out of the fp16 subnormal range; the epilogue multiplies by 2^-S (exact).
+// to keep b_lo out of the fp16 subnormal range; the epilogue multiplies by 2^-S (exact).  Activations are stored
+// multiplied by 2^-e (e per layer, from its folded BatchNorm) for the same reason; the consuming layer's epilogue
+// multiplies by 2^(e_in - S).  Every stored fp16 value is therefore unchanged when a checkpoint is rescaled by
+// powers of two (BatchNorm i times 2^k, conv i+1 times 2^-k), and so is every score.
 //
 // The activations travel BETWEEN the layers already in the form the GEMM consumes: two fp16 planes (hi, lo), laid out
 // in HBM as the exact shared-memory image of the A tile:
@@ -47,11 +50,12 @@ template <class C, int FUSE>
 __global__ void __launch_bounds__(C::NT, 1)
 conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* __restrict__ in_lo,
                   const __half* __restrict__ wtc /*[9][CIN/8][hi co | lo co][8] fp16, scaled by 2^S*/,
-                  const float* __restrict__ bias, float out_scale /*2^-S*/,
+                  const float* __restrict__ bias, float out_scale /*2^(e_in - S)*/, float store_scale /*2^-e_out*/,
                   unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo,
                   float* __restrict__ out_f32 /*last layer only*/, int n_seg,
                   const float* __restrict__ mel, const int* __restrict__ seg_frame0, const float* __restrict__ seg_thr,
-                  const float* __restrict__ w1 /*[9][16]*/, const float* __restrict__ b1 /*[16]*/) {
+                  const float* __restrict__ w1 /*[9][16]*/, const float* __restrict__ b1 /*[16]*/,
+                  float c1_scale /*2^-e1: conv1's activation scale, fused kernel only*/) {
   constexpr int H = C::H, W = C::W, CIN = C::CIN, COUT = C::COUT, P = C::P, BLK = C::BLK, G = C::G;
   constexpr int HALO = C::HALO, ROWB = C::ROWB, NT = C::NT, SS = C::STG_STRIDE;
   static_assert(FUSE == 0 || (G == 1 && CIN == 16 && !C::ALIAS), "fused conv1: one segment per tile, conv2 geometry");
@@ -112,7 +116,7 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
         for (int c = 0; c < 2; ++c) {
           uint4 hi, lo;
           split8(make_float4(res[8 * c], res[8 * c + 1], res[8 * c + 2], res[8 * c + 3]),
-                 make_float4(res[8 * c + 4], res[8 * c + 5], res[8 * c + 6], res[8 * c + 7]), hi, lo);
+                 make_float4(res[8 * c + 4], res[8 * c + 5], res[8 * c + 6], res[8 * c + 7]), c1_scale, hi, lo);
           const uint32_t o = (uint32_t)split_off<ROWB>(row, c);
           *reinterpret_cast<uint4*>(smem + C::OFF_A_HI + o) = hi;
           *reinterpret_cast<uint4*>(smem + C::OFF_A_LO + o) = lo;
@@ -195,7 +199,7 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
             mb.x = fmaxf(mb.x, tb.x); mb.y = fmaxf(mb.y, tb.y); mb.z = fmaxf(mb.z, tb.z); mb.w = fmaxf(mb.w, tb.w);
           }
         uint4 hi, lo;
-        split8(ma, mb, hi, lo);
+        split8(ma, mb, store_scale, hi, lo);
         const int g = kSplitLead + (seg0 + s) * C::OBLK + (ph + 1) * C::OP + (pw + 1);
         const size_t o = split_off<C::OROWB>(g, c8);
         *reinterpret_cast<uint4*>(out_hi + o) = hi;
@@ -210,7 +214,7 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
         uint4 hi = make_uint4(0u, 0u, 0u, 0u), lo = hi;
         if (hh >= 1 && ww >= 1) {
           const float4* tp = reinterpret_cast<const float4*>(stg + r * SS + c8 * 8);
-          split8(tp[0], tp[1], hi, lo);
+          split8(tp[0], tp[1], store_scale, hi, lo);
         }
         const size_t o = split_off<C::OROWB>(kSplitLead + seg0 * BLK + r, c8);
         *reinterpret_cast<uint4*>(out_hi + o) = hi;
@@ -235,10 +239,11 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
   }
 }
 
-// planes -> fp32 channels-last [seg][H][W][C] (stage dumps for the parity tests; x_hi + x_lo == x to 2^-22)
+// planes -> fp32 channels-last [seg][H][W][C] (stage dumps for the parity tests; x_hi + x_lo == x 2^-e to 2^-22,
+// unit = 2^e undoes the activation scale exactly)
 template <int ROWB>
 __global__ void unsplit_kernel(const unsigned char* __restrict__ hi, const unsigned char* __restrict__ lo,
-                               float* __restrict__ out, long long n_items, int H, int W) {
+                               float* __restrict__ out, long long n_items, int H, int W, float unit) {
   constexpr int C8 = ROWB / 16;
   const int P = W + 1, BLK = (H + 1) * P;
   for (long long it = (long long)blockIdx.x * blockDim.x + threadIdx.x; it < n_items; it += (long long)gridDim.x * blockDim.x) {
@@ -256,7 +261,7 @@ __global__ void unsplit_kernel(const unsigned char* __restrict__ hi, const unsig
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const float2 x = __half22float2(ah[i]), y = __half22float2(bh[i]);
-      r[2 * i] = x.x + y.x; r[2 * i + 1] = x.y + y.y;
+      r[2 * i] = (x.x + y.x) * unit; r[2 * i + 1] = (x.y + y.y) * unit;
     }
     float4* dst = reinterpret_cast<float4*>(out + it * 8);
     dst[0] = make_float4(r[0], r[1], r[2], r[3]);
@@ -273,9 +278,10 @@ static int device_sms() {
 
 template <class C, int FUSE>
 static void launch_sp(cudaStream_t st, const unsigned char* in_hi, const unsigned char* in_lo, const __half* wtc,
-                      const float* b, float scale, unsigned char* out_hi, unsigned char* out_lo, float* out_f32,
-                      int n_seg, const float* mel = nullptr, const int* seg_frame0 = nullptr,
-                      const float* seg_thr = nullptr, const float* w1 = nullptr, const float* b1 = nullptr) {
+                      const float* b, float scale, float store_scale, unsigned char* out_hi, unsigned char* out_lo,
+                      float* out_f32, int n_seg, const float* mel = nullptr, const int* seg_frame0 = nullptr,
+                      const float* seg_thr = nullptr, const float* w1 = nullptr, const float* b1 = nullptr,
+                      float c1_scale = 1.f) {
   static unsigned long long configured = 0;
   static int n_sm = 0;
   if (first_launch_on_device(configured)) {
@@ -284,8 +290,8 @@ static void launch_sp(cudaStream_t st, const unsigned char* in_hi, const unsigne
   }
   const int n_tiles = (n_seg + C::G - 1) / C::G;
   const int grid = std::min(n_tiles, n_sm);              // one persistent CTA per SM
-  conv_split_kernel<C, FUSE><<<grid, C::NT, C::SMEM_BYTES, st>>>(in_hi, in_lo, wtc, b, scale, out_hi, out_lo, out_f32,
-                                                                 n_seg, mel, seg_frame0, seg_thr, w1, b1);
+  conv_split_kernel<C, FUSE><<<grid, C::NT, C::SMEM_BYTES, st>>>(in_hi, in_lo, wtc, b, scale, store_scale, out_hi, out_lo,
+                                                                 out_f32, n_seg, mel, seg_frame0, seg_thr, w1, b1, c1_scale);
 }
 
 // Geometry of the plane pair that feeds conv layer `layer` (2..6): rows of the padded image per segment,
@@ -305,8 +311,8 @@ size_t split_plane_bytes(int std_mode, int layer, int n_seg) {
 // conv layer 2..6 on planes; the last layer (6) writes the fp32 CNN features (adapt: [seg][6][64];
 // standard: [seg][6][2][64])
 void launch_conv_split(cudaStream_t st, int std_mode, int layer, const void* in_hi, const void* in_lo,
-                       const void* wtc, const float* b, float out_scale, void* out_hi, void* out_lo,
-                       float* out_f32, int n_seg) {
+                       const void* wtc, const float* b, float out_scale, float store_scale, void* out_hi,
+                       void* out_lo, float* out_f32, int n_seg) {
   const __half* w = reinterpret_cast<const __half*>(wtc);
   const unsigned char* ih = static_cast<const unsigned char*>(in_hi);
   const unsigned char* il = static_cast<const unsigned char*>(in_lo);
@@ -314,44 +320,49 @@ void launch_conv_split(cudaStream_t st, int std_mode, int layer, const void* in_
   unsigned char* ol = static_cast<unsigned char*>(out_lo);
   if (!std_mode) {
     switch (layer) {
-      case 2: launch_sp<SpConv2A, 0>(st, ih, il, w, b, out_scale, oh, ol, out_f32, n_seg); break;
-      case 3: launch_sp<SpConv3A, 0>(st, ih, il, w, b, out_scale, oh, ol, out_f32, n_seg); break;
-      case 4: launch_sp<SpConv4A, 0>(st, ih, il, w, b, out_scale, oh, ol, out_f32, n_seg); break;
-      case 5: launch_sp<SpConv5A, 0>(st, ih, il, w, b, out_scale, oh, ol, out_f32, n_seg); break;
-      default: launch_sp<SpConv6A, 0>(st, ih, il, w, b, out_scale, oh, ol, out_f32, n_seg); break;
+      case 2: launch_sp<SpConv2A, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 3: launch_sp<SpConv3A, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 4: launch_sp<SpConv4A, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 5: launch_sp<SpConv5A, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      default: launch_sp<SpConv6A, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
     }
   } else {
     switch (layer) {
-      case 2: launch_sp<SpConv2S, 0>(st, ih, il, w, b, out_scale, oh, ol, out_f32, n_seg); break;
-      case 3: launch_sp<SpConv3S, 0>(st, ih, il, w, b, out_scale, oh, ol, out_f32, n_seg); break;
-      case 4: launch_sp<SpConv4S, 0>(st, ih, il, w, b, out_scale, oh, ol, out_f32, n_seg); break;
-      case 5: launch_sp<SpConv5S, 0>(st, ih, il, w, b, out_scale, oh, ol, out_f32, n_seg); break;
-      default: launch_sp<SpConv6S, 0>(st, ih, il, w, b, out_scale, oh, ol, out_f32, n_seg); break;
+      case 2: launch_sp<SpConv2S, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 3: launch_sp<SpConv3S, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 4: launch_sp<SpConv4S, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 5: launch_sp<SpConv5S, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      default: launch_sp<SpConv6S, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
     }
   }
 }
 
 // conv1 + pool1 + conv2 + pool2 in one kernel: mel segments -> the plane pair feeding conv3
 void launch_conv12(cudaStream_t st, int std_mode, const float* mel, const int* seg_frame0, const float* seg_thr,
-                   const float* w1, const float* b1, const void* wtc2, const float* bias2, float scale2,
-                   void* out_hi, void* out_lo, int n_seg) {
+                   const float* w1, const float* b1, float c1_scale, const void* wtc2, const float* bias2,
+                   float scale2, float store_scale, void* out_hi, void* out_lo, int n_seg) {
   const __half* w = reinterpret_cast<const __half*>(wtc2);
   unsigned char* oh = static_cast<unsigned char*>(out_hi);
   unsigned char* ol = static_cast<unsigned char*>(out_lo);
-  if (std_mode) launch_sp<SpConv2S, 2>(st, nullptr, nullptr, w, bias2, scale2, oh, ol, nullptr, n_seg, mel, seg_frame0, seg_thr, w1, b1);
-  else launch_sp<SpConv2A, 1>(st, nullptr, nullptr, w, bias2, scale2, oh, ol, nullptr, n_seg, mel, seg_frame0, seg_thr, w1, b1);
+  if (std_mode)
+    launch_sp<SpConv2S, 2>(st, nullptr, nullptr, w, bias2, scale2, store_scale, oh, ol, nullptr, n_seg, mel, seg_frame0,
+                           seg_thr, w1, b1, c1_scale);
+  else
+    launch_sp<SpConv2A, 1>(st, nullptr, nullptr, w, bias2, scale2, store_scale, oh, ol, nullptr, n_seg, mel, seg_frame0,
+                           seg_thr, w1, b1, c1_scale);
 }
 
-void launch_unsplit(cudaStream_t st, int std_mode, int layer, const void* hi, const void* lo, float* out, int n_seg) {
+void launch_unsplit(cudaStream_t st, int std_mode, int layer, const void* hi, const void* lo, float unit, float* out,
+                    int n_seg) {
   int H, W, C;
   split_geometry(std_mode, layer, &H, &W, &C);
   const long long items = (long long)n_seg * H * W * (C / 8);
   const unsigned char* h = static_cast<const unsigned char*>(hi);
   const unsigned char* l = static_cast<const unsigned char*>(lo);
   const int grid = (int)std::min<long long>((items + 255) / 256, (long long)device_sms() * 16);
-  if (C == 16) unsplit_kernel<32><<<grid, 256, 0, st>>>(h, l, out, items, H, W);
-  else if (C == 32) unsplit_kernel<64><<<grid, 256, 0, st>>>(h, l, out, items, H, W);
-  else unsplit_kernel<128><<<grid, 256, 0, st>>>(h, l, out, items, H, W);
+  if (C == 16) unsplit_kernel<32><<<grid, 256, 0, st>>>(h, l, out, items, H, W, unit);
+  else if (C == 32) unsplit_kernel<64><<<grid, 256, 0, st>>>(h, l, out, items, H, W, unit);
+  else unsplit_kernel<128><<<grid, 256, 0, st>>>(h, l, out, items, H, W, unit);
 }
 
 }  // namespace nisqa

@@ -13,6 +13,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <map>
 #include <string>
 #include <vector>
@@ -29,16 +30,16 @@ void launch_seg_table(cudaStream_t, const ClipDesc*, int, const int*, const unsi
 void launch_mel_dump(cudaStream_t, const float*, const ClipDesc*, int, const unsigned*, float*);
 // cnn.cu
 void launch_conv1(cudaStream_t, int, const float*, const int*, const float*, const float*,
-                  const float*, float*, int, void*, void*);
+                  const float*, float*, int, void*, void*, float);
 void launch_conv_layer(cudaStream_t, int, int, const float*, const float*, const float*, float*, int);
 void launch_nhwc_to_nchw(cudaStream_t, const float*, float*, long long, int, int);
 // conv_split.cu
 size_t split_plane_bytes(int std_mode, int layer, int n_seg);
-void launch_conv_split(cudaStream_t, int, int, const void*, const void*, const void*, const float*, float,
+void launch_conv_split(cudaStream_t, int, int, const void*, const void*, const void*, const float*, float, float,
                        void*, void*, float*, int);
-void launch_unsplit(cudaStream_t, int, int, const void*, const void*, float*, int);
-void launch_conv12(cudaStream_t, int, const float*, const int*, const float*, const float*, const float*, const void*,
-                   const float*, float, void*, void*, int);
+void launch_unsplit(cudaStream_t, int, int, const void*, const void*, float, float*, int);
+void launch_conv12(cudaStream_t, int, const float*, const int*, const float*, const float*, const float*, float,
+                   const void*, const float*, float, float, void*, void*, int);
 // td.cu
 struct SaLayerParams {
   const float* WoT; const float* bo; const float* W1T; const float* b1; const float* W2T;
@@ -206,7 +207,9 @@ struct nisqa_engine {
   int rs_nwin = 0, rs_num_table = 0;
   std::map<std::string, size_t> woff;   // float offsets into warena
   float pool_bias_std = 0.f;
-  float tc_scale[8] = {1, 1, 1, 1, 1, 1, 1, 1};   // 2^-S of the fp16 weight pre-scale, per conv layer
+  float tc_scale[8] = {1, 1, 1, 1, 1, 1, 1, 1};   // 2^(e_{i-1} - S_i): undoes the activation and weight pre-scales of conv i
+  int act_exp[8] = {0, 0, 0, 0, 0, 0, 0, 0};      // e_i: conv i's activations are stored as fp16 planes of v * 2^-e_i
+  float act_store(int i) const { return ldexpf(1.f, -act_exp[i]); }
 
   // front-end tables
   std::vector<FbEntry*> fbs;
@@ -439,7 +442,7 @@ struct Packer {
   }
 };
 
-bool pack_conv(Packer& P, int idx, int cin, int cout) {
+bool pack_conv(Packer& P, int idx, int cin, int cout, int* act_exp) {
   char nm[96];
   auto name = [&](const char* fmt) { snprintf(nm, sizeof nm, fmt, idx); return std::string(nm); };
   const TensorView* w = P.get(name("cnn.model.conv%d.weight"), {cout, cin, 3, 3});
@@ -449,6 +452,11 @@ bool pack_conv(Packer& P, int idx, int cin, int cout) {
   const TensorView* mu = P.get(name("cnn.model.bn%d.running_mean"), {cout});
   const TensorView* var = P.get(name("cnn.model.bn%d.running_var"), {cout});
   if (!w || !b || !g || !be || !mu || !var) return false;
+  // activation exponent: max_c |beta_c| + 3 |gamma_c| (the BN output at three standard deviations) -> [2.8, 5.7) 2^e.
+  // It moves by exactly k when BatchNorm's weight and bias are multiplied by 2^k.
+  double E = 0.0;
+  for (int co = 0; co < cout; ++co) E = std::max(E, fabs((double)be->d[co]) + 3.0 * fabs((double)g->d[co]));
+  *act_exp = (E > 0.0 && std::isfinite(E)) ? ilogb(E * sqrt(2.0) / 4.0) : 0;
   const size_t wo = P.alloc(name("conv%d.w"), (size_t)cin * 9 * cout);
   const size_t bo = P.alloc(name("conv%d.b"), cout);
   for (int co = 0; co < cout; ++co) {
@@ -527,8 +535,9 @@ int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
     if (!ok) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
   }
   for (int i = 1; conv_net && i <= 6; ++i)
-    if (!pack_conv(P, i, cin[i], cout[i])) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-  // conv2..conv6 for the tensor-core path: [tap][ci/8][hi co | lo co][8] fp16 two-term split of w * 2^S
+    if (!pack_conv(P, i, cin[i], cout[i], &e->act_exp[i])) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
+  // conv2..conv6 for the tensor-core path: [tap][ci/8][hi co | lo co][8] fp16 two-term split of w * 2^S, S chosen so
+  // that max|w| 2^S lies in (512, 1024] whatever the weights' range (b_lo stays out of the fp16 subnormals)
   for (int i = 2; conv_net && i <= 6; ++i) {
     char k1[32], k2[32];
     snprintf(k1, sizeof k1, "conv%d.w", i); snprintf(k2, sizeof k2, "conv%d.wtc", i);
@@ -537,14 +546,17 @@ int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
     float wmax = 0.f;
     for (size_t j = 0; j < (size_t)ci_n * 9 * co_n; ++j) wmax = std::max(wmax, fabsf(P.arena[src + j]));
     int S = 0;
-    while (S < 14 && wmax * (float)(2 << S) <= 1024.f) ++S;        // max|w| * 2^S <= 1024
-    e->tc_scale[i] = 1.0f / (float)(1 << S);
+    if (wmax > 0.f && std::isfinite(wmax)) {
+      S = 9 - ilogbf(wmax);                                         // max|w| 2^S in [512, 1024)
+      if (ldexpf(wmax, S) == 512.f) ++S;                            // a power of two: 1024 itself
+    }
+    e->tc_scale[i] = ldexpf(1.f, e->act_exp[i - 1] - S);
     const size_t n_half = (size_t)9 * 2 * ci_n * co_n;
     const size_t dst = P.alloc(k2, (n_half + 1) / 2);              // fp16 payload inside the float arena
     for (int tap = 0; tap < 9; ++tap)
       for (int ci = 0; ci < ci_n; ++ci)
         for (int co = 0; co < co_n; ++co) {
-          const float w = P.arena[src + ((size_t)ci * 9 + tap) * co_n + co] * (float)(1 << S);
+          const float w = ldexpf(P.arena[src + ((size_t)ci * 9 + tap) * co_n + co], S);
           const __half hi = __float2half_rn(w);
           const __half lo = __float2half_rn(w - __half2float(hi));
           __half* base = reinterpret_cast<__half*>(&P.arena[dst]) + (size_t)tap * 2 * ci_n * co_n;
@@ -957,12 +969,13 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
     } else if (fused12) {
       Scope s(e, "conv12");
       launch_conv12(st, std_mode, LN.mel.as<float>(), seg_frame0, seg_thr, W(e, "conv1.w"), W(e, "conv1.b"),
-                    W(e, "conv2.wtc"), W(e, "conv2.b"), e->tc_scale[2], plane_hi(3), plane_lo(3), n_seg);
+                    e->act_store(1), W(e, "conv2.wtc"), W(e, "conv2.b"), e->tc_scale[2], e->act_store(2),
+                    plane_hi(3), plane_lo(3), n_seg);
     } else {
       Scope s(e, "conv1");
       launch_conv1(st, std_mode, LN.mel.as<float>(), seg_frame0, seg_thr, W(e, "conv1.w"),
                    W(e, "conv1.b"), split ? nullptr : LN.act1.as<float>(), n_seg,
-                   split ? plane_hi(2) : nullptr, split ? plane_lo(2) : nullptr);
+                   split ? plane_hi(2) : nullptr, split ? plane_lo(2) : nullptr, e->act_store(1));
     }
     if (conv_net) {
       const float* cin_[7] = {nullptr, nullptr, LN.act1.as<float>(), LN.act2.as<float>(), LN.act3.as<float>(),
@@ -976,7 +989,7 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
         Scope s(e, nm);
         if (split)
           launch_conv_split(st, std_mode, l, plane_hi(l), plane_lo(l), W(e, kt), W(e, kb), e->tc_scale[l],
-                            l < 6 ? plane_hi(l + 1) : nullptr, l < 6 ? plane_lo(l + 1) : nullptr,
+                            e->act_store(l), l < 6 ? plane_hi(l + 1) : nullptr, l < 6 ? plane_lo(l + 1) : nullptr,
                             l == 6 ? LN.feats.as<float>() : nullptr, n_seg);
         else
           launch_conv_layer(st, std_mode, l, cin_[l], W(e, kw), W(e, kb), cout_[l], n_seg);
@@ -1516,7 +1529,8 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
       DevBuf* tmp[7] = {nullptr, nullptr, &LN.act1, &LN.act2, &LN.act3, &LN.act4, &LN.act5};
       CK(tmp[plane_layer]->reserve((size_t)count * 4));
       launch_unsplit(st, std_mode, plane_layer, LN.planes[plane_layer].as<char>(),
-                     LN.planes[plane_layer].as<char>() + LN.plane_bytes[plane_layer], tmp[plane_layer]->as<float>(), (int)ns);
+                     LN.planes[plane_layer].as<char>() + LN.plane_bytes[plane_layer],
+                     ldexpf(1.f, e->act_exp[plane_layer - 1]), tmp[plane_layer]->as<float>(), (int)ns);
       src = tmp[plane_layer]->as<float>();
     }
     CK(e->dump.reserve((size_t)count * 4));

@@ -10,7 +10,9 @@ against torch's conv2d on the CPU:
     epilogue's row <-> (segment, h, w) map, pooling and the centre-column pick of conv6.
 
 No GPU and no library call: this pins the layout contract the CUDA kernels implement (their numerical parity is
-tests/test_gpu_parity.py's job).
+tests/test_gpu_parity.py's and tests/test_gpu_layers.py's job).  The last tests run the per-stage float64 checker of
+tests/test_gpu_layers.py on this emulation: it passes the correct three-term split and catches each of three
+plausible kernel faults.
 """
 import numpy as np
 import pytest
@@ -39,9 +41,10 @@ def swz(off, rowb):
     return off ^ ((off >> 3) & (rowb - 16))
 
 
-def split(x):
-    """split8 of csrc/tc_ptx.cuh: x >= 0 -> (hi, lo) fp16 with hi + lo == x to 2^-22."""
-    x = np.minimum(x.astype(np.float32), np.float32(60000.0))
+def split(x, e=0):
+    """split8 of csrc/tc_ptx.cuh with the layer's activation exponent e: x >= 0 -> (hi, lo) fp16 with
+    hi + lo == x 2^-e to 2^-22 (values of x 2^-e in [2^-3, 60000]; the product with 2^-e is exact)."""
+    x = np.minimum(np.ldexp(x.astype(np.float32), -e).astype(np.float32), np.float32(60000.0))
     hi = x.astype(np.float16)
     lo = (x - hi.astype(np.float32)).astype(np.float16)
     return hi, lo
@@ -206,3 +209,74 @@ def test_implicit_gemm_over_shifted_tiles_is_conv2d(name, H, W, C, pool, pow_, c
                         rows = [s * g.BLK + (hy + 1) * g.P + (x + 1) for hy in (2 * ph, 2 * ph + 1) for x in range(x0, x1)]
                         v = np.maximum(D[rows] + bias, 0.0).max(axis=0)
                         np.testing.assert_allclose(v, ref[seg0 + s, ph, pw], rtol=0, atol=tol)
+
+
+def test_split_is_invariant_under_power_of_two_rescaling():
+    """With e shifted by k, the planes of x 2^k are the planes of x bit for bit (pack_weights moves e with the
+    checkpoint's BatchNorm), over a range far beyond the fixed window [2^-3, 60000] of an unscaled split."""
+    rng = np.random.default_rng(5)
+    x = (np.abs(rng.standard_normal(4096)) * 3).astype(np.float32)
+    hi, lo = split(x)
+    for k in (-24, -16, -12, 12, 16, 24):
+        h2, l2 = split(np.ldexp(x, k).astype(np.float32), k)
+        np.testing.assert_array_equal(h2.view(np.uint16), hi.view(np.uint16))
+        np.testing.assert_array_equal(l2.view(np.uint16), lo.view(np.uint16))
+        back = np.ldexp(h2.astype(np.float64) + l2.astype(np.float64), k)
+        big = x >= 0.125
+        assert np.all(np.abs(back - np.ldexp(x, k).astype(np.float64))[big] <= 2.0 ** -22 * np.ldexp(x, k)[big])
+
+
+def _plane_conv(x, wgt, bias, g, fault=None):
+    """conv_split.cu's GEMM on the planes of x, in float64 over the fp16 parts: A_hi B_hi + A_hi B_lo + A_lo B_hi,
+    + bias, ReLU; returns [seg][H][W][co].  `fault` emulates a broken kernel."""
+    n_seg = x.shape[0]
+    hi_p, lo_p = pack_planes(x, g)
+    w_hi = wgt.astype(np.float16)
+    w_lo = (wgt - w_hi.astype(np.float32)).astype(np.float16)
+    out = np.zeros((n_seg, g.H, g.W, wgt.shape[0]))
+    for seg0 in range(0, n_seg, g.G):
+        Xs = []
+        for plane in (hi_p, lo_p):
+            read, _ = load_tile(plane, g, seg0)
+            Xs.append(np.array([[v for c8 in range(g.C // 8) for v in read(r, c8)] for r in range(g.AROWS)], np.float64))
+        Xh, Xl = Xs
+        if fault == "halo_lo":            # lo plane ignored on the image rows next to each segment's zero rows
+            for r in range(g.AROWS):
+                hh = ((r - g.HALO) % g.BLK) // g.P
+                if hh in (1, g.H):
+                    Xl[r] = 0.0
+        D = np.zeros((256, wgt.shape[0]))
+        for t in range(9):
+            ky, kx = t // 3, t % 3
+            off = (ky - 1) * g.P + (kx - 1) + (1 if fault == "tap_shift" and t == 4 else 0)
+            a_h, a_l = Xh[g.HALO + off:g.HALO + off + 256], Xl[g.HALO + off:g.HALO + off + 256]
+            bh = w_hi[:, :, ky, kx].astype(np.float64).T
+            bl = w_lo[:, :, ky, kx].astype(np.float64).T
+            D += a_h @ bh + a_h @ bl
+            if fault != "drop_lohi":
+                D += a_l @ bh
+        for s in range(min(g.G, n_seg - seg0)):
+            for h in range(g.H):
+                for w in range(g.W):
+                    out[seg0 + s, h, w] = np.maximum(D[s * g.BLK + (h + 1) * g.P + (w + 1)] + bias, 0.0)
+    return out
+
+
+@pytest.mark.parametrize("fault", [None, "drop_lohi", "halo_lo", "tap_shift"])
+def test_stage_checker_passes_the_split_gemm_and_catches_faults(fault):
+    import stage_ref as R
+    g = Geom(12, 5, 32)                                                      # conv3 of the AdaptCNN, G = 3
+    rng = np.random.default_rng(21)
+    n_seg = 2 * g.G + 1                                                      # the last tile holds one segment
+    x = (np.abs(rng.standard_normal((n_seg, g.H, g.W, g.C))) * 2).astype(np.float32)
+    wgt = (rng.standard_normal((64, g.C, 3, 3)) * 0.1).astype(np.float32)
+    bias = (rng.standard_normal(64) * 0.1).astype(np.float32)
+    got = _plane_conv(x, wgt, bias, g, fault)
+    xs = torch.from_numpy(unpack_planes(*pack_planes(x, g), g, n_seg)).permute(0, 3, 1, 2).double()
+    ref, bound = R.conv_stage(xs, None, torch.from_numpy(wgt).double(), torch.from_numpy(bias).double(), 1, None, True)
+    r = R.ratio(torch.from_numpy(got).permute(0, 3, 1, 2), ref, bound)
+    print("%s: max |got - ref| / bound = %.3g" % (fault, r))
+    if fault is None:
+        assert r <= 1.0
+    else:
+        assert r > 10.0
