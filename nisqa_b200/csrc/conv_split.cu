@@ -31,10 +31,12 @@
 //   (all nine weight taps, resident for the CTA's life) through shared-memory descriptors, accumulators in
 //   registers.  CTAs are persistent: the weights are loaded once per CTA, the tiles are walked with a grid stride.
 //   Epilogue: registers -> bias / ReLU -> fp32 staging tile -> (max-pool) -> split -> planes of the next layer.
+//   For CIN <= 32 one tap is kept in flight (its A fragments load while the previous tap's wgmmas run); where the
+//   staging tile does not alias the A tile, the A tile is double-buffered (conv_split_kernel).
 //
-// The fused variant (FUSE = 1 + MODE) also computes conv1 + BN + ReLU + pool1 (conv1_cell.cuh, the same fp32
-// arithmetic as conv1_pool1_kernel) of the tile's segment straight into the A tile, so pool1 never reaches HBM; its
-// conv2 GEMM is the same code on the same values: results are bit-identical to the separate kernels.
+// The fused kernel (conv12_kernel) also computes conv1 + BN + ReLU + pool1 of the tile's segment straight into the A
+// tile, so pool1 never reaches HBM; two warpgroups run the GEMM while the other two compute conv1 of the next tile
+// and the epilogue of the previous one.
 #include <cuda_fp16.h>
 
 #include <algorithm>
@@ -46,42 +48,215 @@
 
 namespace nisqa {
 
-template <class C, int FUSE>
+// ---- pieces shared by the two kernels ----
+
+// A fragments of one tap for this warpgroup's NB m64 blocks: block b reads tile rows row + 64 b
+template <class C, int NB>
+__device__ __forceinline__ void load_tap(uint32_t a_hi, uint32_t a_lo, int row, int lchunk,
+                                         uint32_t (&ah)[NB][C::CIN / 16][4], uint32_t (&al)[NB][C::CIN / 16][4]) {
+#pragma unroll
+  for (int b = 0; b < NB; ++b)
+#pragma unroll
+    for (int ks = 0; ks < C::CIN / 16; ++ks) {
+      const uint32_t ao = (uint32_t)split_off<C::ROWB>(row + 64 * b, 2 * ks + lchunk);
+      ldsm_x4(a_hi + ao, ah[b][ks]);
+      ldsm_x4(a_lo + ao, al[b][ks]);
+    }
+}
+
+// the wgmmas of one tap (weights at bst) for NB m64 blocks; no fence / commit
+template <class C, int NB>
+__device__ __forceinline__ void mma_tap(float (&acc_m)[NB][C::COUT / 2], float (&acc_s)[NB][C::COUT / 2],
+                                        const uint32_t (&ah)[NB][C::CIN / 16][4], const uint32_t (&al)[NB][C::CIN / 16][4],
+                                        uint32_t bst) {
+  constexpr int COUT = C::COUT;
+#pragma unroll
+  for (int b = 0; b < NB; ++b)
+#pragma unroll
+    for (int ks = 0; ks < C::CIN / 16; ++ks) {
+      const uint32_t bk = bst + (uint32_t)(2 * ks) * (2 * COUT * 16);
+      const uint64_t dbh = make_desc_b(bk, 2 * COUT * 16), dbl = make_desc_b(bk + COUT * 16, 2 * COUT * 16);
+      wgmma_rs<COUT>(acc_m[b], ah[b][ks], dbh);
+      wgmma_rs<COUT>(acc_s[b], ah[b][ks], dbl);
+      wgmma_rs<COUT>(acc_s[b], al[b][ks], dbh);
+    }
+}
+
+// The GEMM of one tile for this warpgroup's NB m64 blocks: acc_m[b] = hi*hi, acc_s[b] = hi*lo + lo*hi over the nine
+// taps, in tap order.  `row` is this lane's ldmatrix row of block 0 at tap offset 0.
+template <class C, int NB>
+__device__ __forceinline__ void tile_gemm(float (&acc_m)[NB][C::COUT / 2], float (&acc_s)[NB][C::COUT / 2], uint32_t a_hi,
+                                          uint32_t a_lo, uint32_t b_base, uint32_t bar_w, int row, int lchunk) {
+  constexpr int P = C::P, KS = C::CIN / 16;
+#pragma unroll
+  for (int b = 0; b < NB; ++b)
+#pragma unroll
+    for (int i = 0; i < C::COUT / 2; ++i) { acc_m[b][i] = 0.f; acc_s[b][i] = 0.f; }
+  if constexpr (C::CIN <= 32) {
+    // one tap in flight: tap t + 1's fragments load into the other register set while tap t's wgmmas run.  All nine
+    // weight taps are waited for up front: a wait loop between in-flight wgmmas makes ptxas serialize them.
+    for (int t = 0; t < 9; ++t) mbar_wait(bar_w + 8 * t, 0);
+    uint32_t ah[2][NB][KS][4], al[2][NB][KS][4];
+    load_tap<C, NB>(a_hi, a_lo, row - P - 1, lchunk, ah[0], al[0]);
+#pragma unroll
+    for (int t = 0; t < 9; ++t) {
+      wgmma_fence();
+      mma_tap<C, NB>(acc_m, acc_s, ah[t & 1], al[t & 1], b_base + t * C::B_STAGE);
+      wgmma_commit();
+      if (t < 8) {
+        wgmma_wait<1>();                         // tap t - 1 is done with the set that tap t + 1 loads into
+        const int u = t + 1;
+        load_tap<C, NB>(a_hi, a_lo, row + (u / 3 - 1) * P + (u % 3 - 1), lchunk, ah[u & 1], al[u & 1]);
+      }
+    }
+    wgmma_wait<0>();
+  } else {
+    static_assert(NB == 1, "CIN 64: one m64 block per warpgroup");
+#pragma unroll 1
+    for (int t = 0; t < 9; ++t) {
+      mbar_wait(bar_w + 8 * t, 0);
+      const int tapoff = (t / 3 - 1) * P + (t % 3 - 1);
+      uint32_t ah[1][KS][4], al[1][KS][4];
+      load_tap<C, 1>(a_hi, a_lo, row + tapoff, lchunk, ah, al);
+      wgmma_fence();
+      mma_tap<C, 1>(acc_m, acc_s, ah, al, b_base + t * C::B_STAGE);
+      wgmma_commit();
+      wgmma_wait<0>();                           // the A fragments are overwritten by the next tap's loads
+    }
+  }
+}
+
+// epilogue part 1 for one m64 block: accumulators -> bias + ReLU -> staging rows arow0 and arow0 + 8
+template <class C>
+__device__ __forceinline__ void stage_rows(const float (&acc_m)[C::COUT / 2], const float (&acc_s)[C::COUT / 2], int arow0,
+                                           int acol, int seg0, int n_seg, const float* __restrict__ bias, float out_scale,
+                                           float* stg) {
+  constexpr int P = C::P, BLK = C::BLK, SS = C::STG_STRIDE;
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    const int r = arow0 + 8 * half;
+    const int s = r / BLK, q = r - s * BLK;
+    const int hh = q / P, ww = q - hh * P;
+    bool valid = (s < C::G) && (seg0 + s < n_seg) && hh >= 1 && ww >= 1;
+    if (C::CENTER) valid = valid && (ww == 2);
+    if (valid) {
+#pragma unroll
+      for (int j = 0; j < C::COUT / 8; ++j) {
+        const int col = 8 * j + acol;
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + col));
+        const float v0 = fmaxf(fmaf(acc_m[4 * j + 2 * half] + acc_s[4 * j + 2 * half], out_scale, bb.x), 0.f);
+        const float v1 = fmaxf(fmaf(acc_m[4 * j + 2 * half + 1] + acc_s[4 * j + 2 * half + 1], out_scale, bb.y), 0.f);
+        *reinterpret_cast<float2*>(stg + r * SS + col) = make_float2(v0, v1);
+      }
+    }
+  }
+}
+
+// epilogue part 2 (threads t0, t0 + nthr, ...): staging tile -> max-pool / split / store of the tile's nvalid segments
+template <class C>
+__device__ __forceinline__ void store_tile(const float* stg, int seg0, int nvalid, int t0, int nthr, float store_scale,
+                                           unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo,
+                                           float* __restrict__ out_f32) {
+  constexpr int H = C::H, W = C::W, COUT = C::COUT, P = C::P, BLK = C::BLK, SS = C::STG_STRIDE;
+  if constexpr (C::POOL != SP_POOL_NONE) {
+    constexpr int POW = C::POW, HO = H / 2, C8 = COUT / 8;
+    for (int i = t0; i < nvalid * HO * POW * C8; i += nthr) {
+      const int c8 = i % C8;
+      int rest = i / C8;
+      const int pw = rest % POW; rest /= POW;
+      const int ph = rest % HO;
+      const int s = rest / HO;
+      int x0, x1;
+      if (C::POOL == SP_POOL_ADAPT) { x0 = (pw * W) / POW; x1 = ((pw + 1) * W + POW - 1) / POW; }
+      else { x0 = 2 * pw; x1 = 2 * pw + 2; }
+      float4 ma = make_float4(0.f, 0.f, 0.f, 0.f), mb = ma;       // post-ReLU values are >= 0
+      for (int hy = 2 * ph; hy < 2 * ph + 2; ++hy)
+        for (int x = x0; x < x1; ++x) {
+          const float4* tp = reinterpret_cast<const float4*>(stg + (s * BLK + (hy + 1) * P + (x + 1)) * SS + c8 * 8);
+          const float4 ta = tp[0], tb = tp[1];
+          ma.x = fmaxf(ma.x, ta.x); ma.y = fmaxf(ma.y, ta.y); ma.z = fmaxf(ma.z, ta.z); ma.w = fmaxf(ma.w, ta.w);
+          mb.x = fmaxf(mb.x, tb.x); mb.y = fmaxf(mb.y, tb.y); mb.z = fmaxf(mb.z, tb.z); mb.w = fmaxf(mb.w, tb.w);
+        }
+      uint4 hi, lo;
+      split8(ma, mb, store_scale, hi, lo);
+      const int g = kSplitLead + (seg0 + s) * C::OBLK + (ph + 1) * C::OP + (pw + 1);
+      const size_t o = split_off<C::OROWB>(g, c8);
+      *reinterpret_cast<uint4*>(out_hi + o) = hi;
+      *reinterpret_cast<uint4*>(out_lo + o) = lo;
+    }
+  } else if constexpr (C::OUT_SPLIT) {
+    // the whole image of the tile's segments, zero row / column positions included (as zeros)
+    constexpr int C8 = COUT / 8;
+    for (int i = t0; i < nvalid * BLK * C8; i += nthr) {
+      const int c8 = i % C8, r = i / C8;
+      const int q = r % BLK, hh = q / P, ww = q - hh * P;
+      uint4 hi = make_uint4(0u, 0u, 0u, 0u), lo = hi;
+      if (hh >= 1 && ww >= 1) {
+        const float4* tp = reinterpret_cast<const float4*>(stg + r * SS + c8 * 8);
+        split8(tp[0], tp[1], store_scale, hi, lo);
+      }
+      const size_t o = split_off<C::OROWB>(kSplitLead + seg0 * BLK + r, c8);
+      *reinterpret_cast<uint4*>(out_hi + o) = hi;
+      *reinterpret_cast<uint4*>(out_lo + o) = lo;
+    }
+  } else {
+    // fp32 CNN features, channels-last [seg][HO][WO][COUT]
+    constexpr int HO = C::HO, WO = C::WO, C4 = COUT / 4;
+    for (int i = t0; i < nvalid * HO * WO * C4; i += nthr) {
+      const int c4 = i % C4;
+      int rest = i / C4;
+      const int w = rest % WO; rest /= WO;
+      const int h = rest % HO;
+      const int s = rest / HO;
+      const int r = s * BLK + (h + 1) * P + (C::CENTER ? 2 : w + 1);
+      *reinterpret_cast<float4*>(out_f32 + ((size_t)(seg0 + s) * (HO * WO) + h * WO + w) * COUT + c4 * 4) =
+          *reinterpret_cast<const float4*>(stg + r * SS + c4 * 4);
+    }
+  }
+}
+
+// ---- conv2..conv6 on planes ----
+// Four warpgroups own 64 rows each and run GEMM, epilogue part 1, part 2 in turn.  Without aliasing (conv2, conv3)
+// the activation tile is double-buffered: one thread issues the next tile's copy into the other buffer as soon as
+// that buffer's readers (the previous tile's GEMM) have arrived on its empty barrier.
+template <class C>
 __global__ void __launch_bounds__(C::NT, 1)
 conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* __restrict__ in_lo,
                   const __half* __restrict__ wtc /*[9][CIN/8][hi co | lo co][8] fp16, scaled by 2^S*/,
                   const float* __restrict__ bias, float out_scale /*2^(e_in - S)*/, float store_scale /*2^-e_out*/,
                   unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo,
-                  float* __restrict__ out_f32 /*last layer only*/, int n_seg,
-                  const float* __restrict__ mel, const int* __restrict__ seg_frame0, const float* __restrict__ seg_thr,
-                  const float* __restrict__ w1 /*[9][16]*/, const float* __restrict__ b1 /*[16]*/,
-                  float c1_scale /*2^-e1: conv1's activation scale, fused kernel only*/) {
-  constexpr int H = C::H, W = C::W, CIN = C::CIN, COUT = C::COUT, P = C::P, BLK = C::BLK, G = C::G;
-  constexpr int HALO = C::HALO, ROWB = C::ROWB, NT = C::NT, SS = C::STG_STRIDE;
-  static_assert(FUSE == 0 || (G == 1 && CIN == 16 && !C::ALIAS), "fused conv1: one segment per tile, conv2 geometry");
+                  float* __restrict__ out_f32 /*last layer only*/, int n_seg) {
+  constexpr int G = C::G, BLK = C::BLK, HALO = C::HALO, ROWB = C::ROWB, NT = C::NT;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // swizzle atoms repeat every 1024 B
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t a_hi = sbase + C::OFF_A_HI, a_lo = sbase + C::OFF_A_LO, b_base = sbase + C::OFF_B;
-  const uint32_t bar_w = sbase + C::OFF_BAR, bar_a = bar_w + 8 * 9;
+  const uint32_t b_base = sbase + C::OFF_B;
+  const uint32_t bar_w = sbase + C::OFF_BAR, bar_full = bar_w + 8 * 9, bar_empty = bar_full + 8 * C::A_BUFS;
   float* stg = reinterpret_cast<float*>(smem + C::OFF_STG);
-  float* ws = reinterpret_cast<float*>(smem + C::OFF_W1);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const int n_tiles = (n_seg + G - 1) / G;
 
-  if constexpr (FUSE != 0) {
-    // the zero row / zero column / halo rows of the A tile are never written again
-    for (int i = tid; i < 2 * C::A_BYTES / 16; i += NT) reinterpret_cast<uint4*>(smem + C::OFF_A_HI)[i] = make_uint4(0u, 0u, 0u, 0u);
-    for (int i = tid; i < 9 * 16 + 16; i += NT) ws[i] = (i < 144) ? __ldg(w1 + i) : __ldg(b1 + i - 144);
-  }
+  // one thread: both planes of tile `tile` into activation buffer b, placed at row g0 & 7 (tile row == plane row mod 8)
+  auto issue_tile = [&](int tile, int b) {
+    constexpr uint32_t A_COPY = (uint32_t)C::AROWS * ROWB;
+    const int g0 = kSplitLead + tile * G * BLK - HALO;
+    const uint32_t dst = sbase + C::OFF_A_HI + b * C::A_BUF + (uint32_t)(g0 & 7) * ROWB;
+    mbar_expect_tx(bar_full + 8 * b, 2 * A_COPY);
+    bulk_g2s(dst, in_hi + (size_t)g0 * ROWB, A_COPY, bar_full + 8 * b);
+    bulk_g2s(dst + C::A_BYTES, in_lo + (size_t)g0 * ROWB, A_COPY, bar_full + 8 * b);
+  };
+
   if (tid == 0) {
     for (int t = 0; t < 9; ++t) mbar_init(bar_w + 8 * t, 1);
-    mbar_init(bar_a, 1);
+    for (int b = 0; b < C::A_BUFS; ++b) mbar_init(bar_full + 8 * b, 1);
+    if constexpr (!C::ALIAS)
+      for (int b = 0; b < C::A_BUFS; ++b) mbar_init(bar_empty + 8 * b, NT);
     fence_barrier_init();
     for (int t = 0; t < 9; ++t) {                // all nine taps stay resident; tap t's MMAs start once it has landed
       mbar_expect_tx(bar_w + 8 * t, C::B_STAGE);
       bulk_g2s(b_base + t * C::B_STAGE, wtc + (size_t)t * (C::B_STAGE / 2), C::B_STAGE, bar_w + 8 * t);
     }
+    if constexpr (!C::ALIAS) issue_tile(blockIdx.x, 0);
   }
   __syncthreads();
 
@@ -95,147 +270,139 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
     const int seg0 = tile * G;
     const int g0 = kSplitLead + seg0 * BLK - HALO;         // first plane row of this tile
-    const uint32_t sh = FUSE ? 0u : (uint32_t)(g0 & 7);    // tile row == plane row (mod 8)
-    if constexpr (FUSE == 0) {
-      if (tid == 0) {
-        constexpr uint32_t A_COPY = (uint32_t)C::AROWS * ROWB;
-        mbar_expect_tx(bar_a, 2 * A_COPY);
-        bulk_g2s(a_hi + sh * ROWB, in_hi + (size_t)g0 * ROWB, A_COPY, bar_a);
-        bulk_g2s(a_lo + sh * ROWB, in_lo + (size_t)g0 * ROWB, A_COPY, bar_a);
-      }
-      mbar_wait(bar_a, it & 1);
+    const int ab = C::ALIAS ? 0 : (it & 1);
+    if constexpr (C::ALIAS) {
+      if (tid == 0) issue_tile(tile, 0);
+      mbar_wait(bar_full, it & 1);
     } else {
-      // conv1 + BN + ReLU + pool1 of segment `tile`: one thread per pooled cell, all 16 channels
-      constexpr int PW = W, NCELL = 24 * PW;
-      if (tid < NCELL) {
-        const int ph = tid / PW, pw = tid - ph * PW;
-        float res[16];
-        conv1_cell<FUSE - 1>(mel, __ldg(seg_frame0 + tile), __ldg(seg_thr + tile), ws, ph, pw, res);
-        const int row = HALO + (ph + 1) * P + (pw + 1);
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          uint4 hi, lo;
-          split8(make_float4(res[8 * c], res[8 * c + 1], res[8 * c + 2], res[8 * c + 3]),
-                 make_float4(res[8 * c + 4], res[8 * c + 5], res[8 * c + 6], res[8 * c + 7]), c1_scale, hi, lo);
-          const uint32_t o = (uint32_t)split_off<ROWB>(row, c);
-          *reinterpret_cast<uint4*>(smem + C::OFF_A_HI + o) = hi;
-          *reinterpret_cast<uint4*>(smem + C::OFF_A_LO + o) = lo;
-        }
+      const int next = tile + gridDim.x;
+      if (tid == 0 && next < n_tiles) {
+        const int nb = (it + 1) & 1;
+        mbar_wait(bar_empty + 8 * nb, (((it + 1) >> 1) & 1) ^ 1);   // tile it - 1's GEMM is done with buffer nb
+        issue_tile(next, nb);
       }
-      __syncthreads();
+      mbar_wait(bar_full + 8 * ab, (it >> 1) & 1);
     }
 
     // ===== GEMM: warpgroup wg, rows 64 wg .. 64 wg + 63 =====
-    float acc_m[COUT / 2], acc_s[COUT / 2];      // hi*hi ; hi*lo + lo*hi
-#pragma unroll
-    for (int i = 0; i < COUT / 2; ++i) { acc_m[i] = 0.f; acc_s[i] = 0.f; }
-#pragma unroll 1
-    for (int t = 0; t < 9; ++t) {
-      mbar_wait(bar_w + 8 * t, 0);
-      const int tapoff = (t / 3 - 1) * P + (t % 3 - 1);
-      const int row = (int)sh + HALO + tapoff + lrow;
-      const uint32_t bst = b_base + t * C::B_STAGE;
-      uint32_t ah[CIN / 16][4], al[CIN / 16][4];
-#pragma unroll
-      for (int ks = 0; ks < CIN / 16; ++ks) {
-        const uint32_t ao = (uint32_t)split_off<ROWB>(row, 2 * ks + lchunk);
-        ldsm_x4(a_hi + ao, ah[ks]);
-        ldsm_x4(a_lo + ao, al[ks]);
-      }
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < CIN / 16; ++ks) {
-        const uint32_t bk = bst + (uint32_t)(2 * ks) * (2 * COUT * 16);
-        const uint64_t dbh = make_desc_b(bk, 2 * COUT * 16), dbl = make_desc_b(bk + COUT * 16, 2 * COUT * 16);
-        wgmma_rs<COUT>(acc_m, ah[ks], dbh);
-        wgmma_rs<COUT>(acc_s, ah[ks], dbl);
-        wgmma_rs<COUT>(acc_s, al[ks], dbh);
-      }
-      wgmma_commit();
-      wgmma_wait0();                             // the A fragments are overwritten by the next tap's loads
-    }
-    __syncthreads();                             // every warpgroup is done with the A tile (the staging tile may alias it)
+    const uint32_t a_hi = sbase + C::OFF_A_HI + ab * C::A_BUF, a_lo = a_hi + C::A_BYTES;
+    float acc_m[1][C::COUT / 2], acc_s[1][C::COUT / 2];      // hi*hi ; hi*lo + lo*hi
+    tile_gemm<C, 1>(acc_m, acc_s, a_hi, a_lo, b_base, bar_w, (g0 & 7) + HALO + lrow, lchunk);
+    if constexpr (!C::ALIAS) mbar_arrive(bar_empty + 8 * ab);
+    __syncthreads();                             // ALIAS: every warpgroup is done with the A tile the staging tile
+                                                 // overwrites; otherwise the previous tile's part 2 is done with it
 
     // ===== epilogue part 1: accumulators -> bias + ReLU -> staging row r =====
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      const int r = arow0 + 8 * half;
-      const int s = r / BLK, q = r - s * BLK;
-      const int hh = q / P, ww = q - hh * P;
-      bool valid = (s < G) && (seg0 + s < n_seg) && hh >= 1 && ww >= 1;
-      if (C::CENTER) valid = valid && (ww == 2);
-      if (valid) {
-#pragma unroll
-        for (int j = 0; j < COUT / 8; ++j) {
-          const int col = 8 * j + acol;
-          const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + col));
-          const float v0 = fmaxf(fmaf(acc_m[4 * j + 2 * half] + acc_s[4 * j + 2 * half], out_scale, bb.x), 0.f);
-          const float v1 = fmaxf(fmaf(acc_m[4 * j + 2 * half + 1] + acc_s[4 * j + 2 * half + 1], out_scale, bb.y), 0.f);
-          *reinterpret_cast<float2*>(stg + r * SS + col) = make_float2(v0, v1);
-        }
-      }
-    }
+    stage_rows<C>(acc_m[0], acc_s[0], arow0, acol, seg0, n_seg, bias, out_scale, stg);
     __syncthreads();
 
     // ===== epilogue part 2 (all threads): max-pool / split / store =====
-    const int nvalid = min(G, n_seg - seg0);
-    if constexpr (C::POOL != SP_POOL_NONE) {
-      constexpr int POW = C::POW, HO = H / 2, C8 = COUT / 8;
-      for (int i = tid; i < nvalid * HO * POW * C8; i += NT) {
-        const int c8 = i % C8;
-        int rest = i / C8;
-        const int pw = rest % POW; rest /= POW;
-        const int ph = rest % HO;
-        const int s = rest / HO;
-        int x0, x1;
-        if (C::POOL == SP_POOL_ADAPT) { x0 = (pw * W) / POW; x1 = ((pw + 1) * W + POW - 1) / POW; }
-        else { x0 = 2 * pw; x1 = 2 * pw + 2; }
-        float4 ma = make_float4(0.f, 0.f, 0.f, 0.f), mb = ma;       // post-ReLU values are >= 0
-        for (int hy = 2 * ph; hy < 2 * ph + 2; ++hy)
-          for (int x = x0; x < x1; ++x) {
-            const float4* tp = reinterpret_cast<const float4*>(stg + (s * BLK + (hy + 1) * P + (x + 1)) * SS + c8 * 8);
-            const float4 ta = tp[0], tb = tp[1];
-            ma.x = fmaxf(ma.x, ta.x); ma.y = fmaxf(ma.y, ta.y); ma.z = fmaxf(ma.z, ta.z); ma.w = fmaxf(ma.w, ta.w);
-            mb.x = fmaxf(mb.x, tb.x); mb.y = fmaxf(mb.y, tb.y); mb.z = fmaxf(mb.z, tb.z); mb.w = fmaxf(mb.w, tb.w);
-          }
-        uint4 hi, lo;
-        split8(ma, mb, store_scale, hi, lo);
-        const int g = kSplitLead + (seg0 + s) * C::OBLK + (ph + 1) * C::OP + (pw + 1);
-        const size_t o = split_off<C::OROWB>(g, c8);
-        *reinterpret_cast<uint4*>(out_hi + o) = hi;
-        *reinterpret_cast<uint4*>(out_lo + o) = lo;
-      }
-    } else if constexpr (C::OUT_SPLIT) {
-      // the whole image of the tile's segments, zero row / column positions included (as zeros)
-      constexpr int C8 = COUT / 8;
-      for (int i = tid; i < nvalid * BLK * C8; i += NT) {
-        const int c8 = i % C8, r = i / C8;
-        const int q = r % BLK, hh = q / P, ww = q - hh * P;
-        uint4 hi = make_uint4(0u, 0u, 0u, 0u), lo = hi;
-        if (hh >= 1 && ww >= 1) {
-          const float4* tp = reinterpret_cast<const float4*>(stg + r * SS + c8 * 8);
-          split8(tp[0], tp[1], store_scale, hi, lo);
-        }
-        const size_t o = split_off<C::OROWB>(kSplitLead + seg0 * BLK + r, c8);
-        *reinterpret_cast<uint4*>(out_hi + o) = hi;
-        *reinterpret_cast<uint4*>(out_lo + o) = lo;
-      }
-    } else {
-      // fp32 CNN features, channels-last [seg][HO][WO][COUT]
-      constexpr int HO = C::HO, WO = C::WO, C4 = COUT / 4;
-      for (int i = tid; i < nvalid * HO * WO * C4; i += NT) {
-        const int c4 = i % C4;
-        int rest = i / C4;
-        const int w = rest % WO; rest /= WO;
-        const int h = rest % HO;
-        const int s = rest / HO;
-        const int r = s * BLK + (h + 1) * P + (C::CENTER ? 2 : w + 1);
-        *reinterpret_cast<float4*>(out_f32 + ((size_t)(seg0 + s) * (HO * WO) + h * WO + w) * COUT + c4 * 4) =
-            *reinterpret_cast<const float4*>(stg + r * SS + c4 * 4);
-      }
+    store_tile<C>(stg, seg0, min(G, n_seg - seg0), tid, NT, store_scale, out_hi, out_lo, out_f32);
+    if constexpr (C::ALIAS) {
+      fence_proxy_async();                       // staging stores (generic proxy) before the next tile's bulk copy
+      __syncthreads();
     }
-    fence_proxy_async();                         // staging stores (generic proxy) before the next tile's bulk copy
-    __syncthreads();
+  }
+}
+
+// ---- conv1 + pool1 + conv2 + pool2 ----
+// conv1 + BN + ReLU + pool1 (conv1_cell.cuh, the same fp32 arithmetic as conv1_pool1_kernel) of one segment per tile
+// goes straight into the A tile; the conv2 GEMM and epilogue are the same code on the same values as conv_split_kernel,
+// so results are bit-identical to the separate kernels.  The persistent CTA splits into two roles:
+//   warpgroups 0, 1 (MMA):   wait A full[i & 1]; GEMM of rows 128 wg .. 128 wg + 127 (two m64 blocks); arrive A
+//                            empty[i & 1]; bias + ReLU into staging tile i & 1; named barrier of the 256 MMA threads;
+//                            max-pool / split / store of tile i
+//   warpgroups 2, 3 (conv1): conv1 of tile i + 1 into A buffer (i + 1) & 1 (after its empty barrier), arrive A full
+// so conv1 of the next tile runs while the tensor cores work on this one.  conv1 is the longer of the two roles, so the
+// epilogue stays with the MMA warpgroups.  The A barriers count the 256 threads of the role that arrives on them;
+// buffer b's k-th use waits on parity k & 1 (full) or (k & 1) ^ 1 (empty: a fresh barrier's "previous phase" counts as
+// complete).  Staging tile i & 1 is next written at tile i + 2, after the named barrier of tile i + 1, which every MMA
+// thread reaches only after its part of tile i's store.
+template <class C, int MODE>
+__global__ void __launch_bounds__(C::NT, 1)
+conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, float out_scale, float store_scale,
+              unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo, int n_seg,
+              const float* __restrict__ mel, const int* __restrict__ seg_frame0, const float* __restrict__ seg_thr,
+              const float* __restrict__ w1 /*[9][16]*/, const float* __restrict__ b1 /*[16]*/,
+              float c1_scale /*2^-e1: conv1's activation scale*/) {
+  using L = SpFused<C>;
+  constexpr int W = C::W, P = C::P, HALO = C::HALO, ROWB = C::ROWB, NT = C::NT, NR = NT / 2;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  const uint32_t sbase = smem_u32(smem);
+  const uint32_t b_base = sbase + L::OFF_B;
+  const uint32_t bar_w = sbase + L::OFF_BAR, a_full = bar_w + 8 * 9, a_empty = a_full + 16;
+  float* ws = reinterpret_cast<float*>(smem + L::OFF_W1);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);   // warp-uniform as far as ptxas can tell: the role branch
+                                                           // below must not count as divergent around the wgmmas
+  const int n_tiles = n_seg;                     // G == 1
+
+  // the zero row / zero column / halo rows of both A buffers are never written again
+  for (int i = tid; i < 2 * C::A_BUF / 16; i += NT) reinterpret_cast<uint4*>(smem + L::OFF_A)[i] = make_uint4(0u, 0u, 0u, 0u);
+  for (int i = tid; i < 9 * 16 + 16; i += NT) ws[i] = (i < 144) ? __ldg(w1 + i) : __ldg(b1 + i - 144);
+  if (tid == 0) {
+    for (int t = 0; t < 9; ++t) mbar_init(bar_w + 8 * t, 1);
+    for (int b = 0; b < 4; ++b) mbar_init(a_full + 8 * b, NR);
+    fence_barrier_init();
+    for (int t = 0; t < 9; ++t) {
+      mbar_expect_tx(bar_w + 8 * t, C::B_STAGE);
+      bulk_g2s(b_base + t * C::B_STAGE, wtc + (size_t)t * (C::B_STAGE / 2), C::B_STAGE, bar_w + 8 * t);
+    }
+  }
+  __syncthreads();
+
+  // registers: 64 accumulators and two fragment sets per MMA thread; 2 x 128 x (160 + 96) = the whole register file
+  if (wg < 2) {
+    // ===== MMA warpgroups: block b of warpgroup wg = tile rows 128 wg + 64 b .. + 63 =====
+    setmaxnreg_inc<160>();
+    const int lrow = wg * 128 + (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+    const int lchunk = lane >> 4;
+    const int arow0 = wg * 128 + (warp & 3) * 16 + (lane >> 2);
+    const int acol = 2 * (lane & 3);
+    int it = 0;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+      const int ab = it & 1;
+      const uint32_t par = (uint32_t)(it >> 1) & 1u;
+      mbar_wait(a_full + 8 * ab, par);
+      const uint32_t a_hi = sbase + L::OFF_A + ab * C::A_BUF, a_lo = a_hi + C::A_BYTES;
+      float acc_m[2][C::COUT / 2], acc_s[2][C::COUT / 2];
+      tile_gemm<C, 2>(acc_m, acc_s, a_hi, a_lo, b_base, bar_w, HALO + lrow, lchunk);
+      mbar_arrive(a_empty + 8 * ab);
+      float* stg = reinterpret_cast<float*>(smem + L::OFF_STG + ab * C::STG_BYTES);
+#pragma unroll
+      for (int b = 0; b < 2; ++b) stage_rows<C>(acc_m[b], acc_s[b], arow0 + 64 * b, acol, tile, n_seg, bias, out_scale, stg);
+      named_bar_sync<1, NR>();
+      store_tile<C>(stg, tile, 1, tid, NR, store_scale, out_hi, out_lo, nullptr);
+    }
+  } else {
+    // ===== worker warpgroups =====
+    setmaxnreg_dec<96>();
+    const int wt = tid - NR;
+    // conv1 + BN + ReLU + pool1 of segment `seg` into A buffer j & 1 (j: the CTA's tile index): one item per
+    // pooled cell and channel half (conv1_cell's channel quads 2c, 2c + 1 -> 16-byte chunk c of the cell's row)
+    auto fill = [&](int seg, int j) {
+      constexpr int NCELL = 24 * W;
+      const int b = j & 1;
+      mbar_wait(a_empty + 8 * b, ((uint32_t)(j >> 1) & 1u) ^ 1u);
+      unsigned char* a = smem + L::OFF_A + b * C::A_BUF;
+      const int f0 = __ldg(seg_frame0 + seg);
+      const float thr = __ldg(seg_thr + seg);
+      for (int i = wt; i < 2 * NCELL; i += NR) {
+        const int cell = i >> 1, c = i & 1;
+        const int ph = cell / W, pw = cell - ph * W;
+        float res[8];
+        conv1_cell<MODE, true, kMels, 2>(mel, f0, thr, ws, ph, pw, res, 2 * c);
+        uint4 hi, lo;
+        split8(make_float4(res[0], res[1], res[2], res[3]), make_float4(res[4], res[5], res[6], res[7]), c1_scale, hi, lo);
+        const uint32_t o = (uint32_t)split_off<ROWB>(HALO + (ph + 1) * P + (pw + 1), c);
+        *reinterpret_cast<uint4*>(a + o) = hi;
+        *reinterpret_cast<uint4*>(a + C::A_BYTES + o) = lo;
+      }
+      mbar_arrive(a_full + 8 * b);
+    };
+    int it = 0;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) fill(tile, it);
   }
 }
 
@@ -276,22 +443,35 @@ static int device_sms() {
   return n > 0 ? n : 1;
 }
 
-template <class C, int FUSE>
+template <class C>
 static void launch_sp(cudaStream_t st, const unsigned char* in_hi, const unsigned char* in_lo, const __half* wtc,
                       const float* b, float scale, float store_scale, unsigned char* out_hi, unsigned char* out_lo,
-                      float* out_f32, int n_seg, const float* mel = nullptr, const int* seg_frame0 = nullptr,
-                      const float* seg_thr = nullptr, const float* w1 = nullptr, const float* b1 = nullptr,
-                      float c1_scale = 1.f) {
+                      float* out_f32, int n_seg) {
   static unsigned long long configured = 0;
   static int n_sm = 0;
   if (first_launch_on_device(configured)) {
-    cudaFuncSetAttribute(conv_split_kernel<C, FUSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    cudaFuncSetAttribute(conv_split_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     n_sm = device_sms();
   }
   const int n_tiles = (n_seg + C::G - 1) / C::G;
   const int grid = std::min(n_tiles, n_sm);              // one persistent CTA per SM
-  conv_split_kernel<C, FUSE><<<grid, C::NT, C::SMEM_BYTES, st>>>(in_hi, in_lo, wtc, b, scale, store_scale, out_hi, out_lo,
-                                                                 out_f32, n_seg, mel, seg_frame0, seg_thr, w1, b1, c1_scale);
+  conv_split_kernel<C><<<grid, C::NT, C::SMEM_BYTES, st>>>(in_hi, in_lo, wtc, b, scale, store_scale, out_hi, out_lo,
+                                                           out_f32, n_seg);
+}
+
+template <class C, int MODE>
+static void launch_c12(cudaStream_t st, const __half* wtc, const float* b, float scale, float store_scale,
+                       unsigned char* out_hi, unsigned char* out_lo, int n_seg, const float* mel, const int* seg_frame0,
+                       const float* seg_thr, const float* w1, const float* b1, float c1_scale) {
+  static unsigned long long configured = 0;
+  static int n_sm = 0;
+  if (first_launch_on_device(configured)) {
+    cudaFuncSetAttribute(conv12_kernel<C, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SpFused<C>::SMEM_BYTES);
+    n_sm = device_sms();
+  }
+  const int grid = std::min(n_seg, n_sm);                // one persistent CTA per SM, one segment per tile
+  conv12_kernel<C, MODE><<<grid, C::NT, SpFused<C>::SMEM_BYTES, st>>>(wtc, b, scale, store_scale, out_hi, out_lo, n_seg,
+                                                                      mel, seg_frame0, seg_thr, w1, b1, c1_scale);
 }
 
 // Geometry of the plane pair that feeds conv layer `layer` (2..6): rows of the padded image per segment,
@@ -320,19 +500,19 @@ void launch_conv_split(cudaStream_t st, int std_mode, int layer, const void* in_
   unsigned char* ol = static_cast<unsigned char*>(out_lo);
   if (!std_mode) {
     switch (layer) {
-      case 2: launch_sp<SpConv2A, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 3: launch_sp<SpConv3A, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 4: launch_sp<SpConv4A, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 5: launch_sp<SpConv5A, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      default: launch_sp<SpConv6A, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 2: launch_sp<SpConv2A>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 3: launch_sp<SpConv3A>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 4: launch_sp<SpConv4A>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 5: launch_sp<SpConv5A>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      default: launch_sp<SpConv6A>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
     }
   } else {
     switch (layer) {
-      case 2: launch_sp<SpConv2S, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 3: launch_sp<SpConv3S, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 4: launch_sp<SpConv4S, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 5: launch_sp<SpConv5S, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      default: launch_sp<SpConv6S, 0>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 2: launch_sp<SpConv2S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 3: launch_sp<SpConv3S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 4: launch_sp<SpConv4S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 5: launch_sp<SpConv5S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      default: launch_sp<SpConv6S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
     }
   }
 }
@@ -345,11 +525,9 @@ void launch_conv12(cudaStream_t st, int std_mode, const float* mel, const int* s
   unsigned char* oh = static_cast<unsigned char*>(out_hi);
   unsigned char* ol = static_cast<unsigned char*>(out_lo);
   if (std_mode)
-    launch_sp<SpConv2S, 2>(st, nullptr, nullptr, w, bias2, scale2, store_scale, oh, ol, nullptr, n_seg, mel, seg_frame0,
-                           seg_thr, w1, b1, c1_scale);
+    launch_c12<SpConv2S, 1>(st, w, bias2, scale2, store_scale, oh, ol, n_seg, mel, seg_frame0, seg_thr, w1, b1, c1_scale);
   else
-    launch_sp<SpConv2A, 1>(st, nullptr, nullptr, w, bias2, scale2, store_scale, oh, ol, nullptr, n_seg, mel, seg_frame0,
-                           seg_thr, w1, b1, c1_scale);
+    launch_c12<SpConv2A, 0>(st, w, bias2, scale2, store_scale, oh, ol, n_seg, mel, seg_frame0, seg_thr, w1, b1, c1_scale);
 }
 
 void launch_unsplit(cudaStream_t st, int std_mode, int layer, const void* hi, const void* lo, float unit, float* out,

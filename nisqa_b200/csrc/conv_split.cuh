@@ -45,14 +45,22 @@ struct SpCfg {
   // the staging tile reuses the activation tile when both do not fit beside the nine resident weight taps
   static constexpr int SMEM_BUDGET = 227 * 1024 - 2048;
   static constexpr bool ALIAS = 2 * A_BYTES + STG_BYTES + 9 * B_STAGE > SMEM_BUDGET;
+  // without aliasing the activation tile is double-buffered: the next tile's copy lands during this tile's GEMM and
+  // epilogue.  Buffer b: hi plane at b * A_BUF, lo plane at b * A_BUF + A_BYTES.
+  static constexpr int A_BUFS = ALIAS ? 1 : 2;
+  static constexpr int A_BUF = 2 * A_BYTES;
   static constexpr int OFF_A_HI = 0;
   static constexpr int OFF_A_LO = A_BYTES;
-  static constexpr int OFF_STG = ALIAS ? 0 : 2 * A_BYTES;
-  static constexpr int OFF_B = ((ALIAS ? (2 * A_BYTES > STG_BYTES ? 2 * A_BYTES : STG_BYTES) : 2 * A_BYTES + STG_BYTES) + 1023) & ~1023;
+  static constexpr int OFF_STG = ALIAS ? 0 : A_BUFS * A_BUF;
+  static constexpr int OFF_B = ((ALIAS ? (A_BUF > STG_BYTES ? A_BUF : STG_BYTES) : A_BUFS * A_BUF + STG_BYTES) + 1023) & ~1023;
   static constexpr int OFF_W1 = OFF_B + 9 * B_STAGE;      // conv1 weights [9][16] + biases [16] (fused conv1 + conv2 only)
-  static constexpr int OFF_BAR = OFF_W1 + 1024;           // 9 weight-tap barriers + the activation-tile barrier
-  static constexpr int SMEM_BYTES = OFF_BAR + 8 * 10 + 1024;    // + slack: the tile is aligned to 1024 B
+  // 9 weight-tap barriers, then a full barrier per activation buffer, then (double-buffered) an empty barrier per buffer
+  static constexpr int OFF_BAR = OFF_W1 + 1024;
+  static constexpr int NBAR = ALIAS ? 10 : 13;
+  static constexpr int SMEM_BYTES = OFF_BAR + 8 * NBAR + 1024;    // + slack: the tile is aligned to 1024 B
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
+  static_assert(ALIAS || A_BUFS * A_BUF + STG_BYTES + 9 * B_STAGE <= SMEM_BUDGET,
+                "both activation buffers fit beside the staging tile and the weights");
   static_assert(B_STAGE % 16 == 0 && CIN % 16 == 0 && (COUT == 32 || COUT == 64), "shape");
   static_assert(ROWB == 32 || ROWB == 64 || ROWB == 128, "rows are 32 / 64 / 128 bytes (one swizzle atom)");
   static_assert(HALO <= kSplitLead, "kSplitLead");
@@ -73,5 +81,21 @@ using SpConv3S = SpCfg<12, 4, 32, 64, SP_POOL_NONE, 0>;
 using SpConv4S = SpCfg<12, 4, 64, 64, SP_POOL_2X2, 2>;
 using SpConv5S = SpCfg<6, 2, 64, 64, SP_POOL_NONE, 0>;
 using SpConv6S = SpCfg<6, 2, 64, 64, SP_POOL_NONE, 0, true>;
+
+// Shared memory of the fused conv1 + conv2 kernel (conv12_kernel) on the conv2 geometry C: two activation buffers
+// (conv1 fills one while the GEMM reads the other) and two staging tiles (tile i's is written while stragglers of the
+// MMA warpgroups may still read tile i - 1's).
+template <class C>
+struct SpFused {
+  static constexpr int OFF_A = 0;                         // buffer b at b * C::A_BUF (1024-aligned: A_BYTES is)
+  static constexpr int OFF_STG = 2 * C::A_BUF;            // staging tile b at OFF_STG + b * C::STG_BYTES
+  static constexpr int OFF_B = (OFF_STG + 2 * C::STG_BYTES + 1023) & ~1023;
+  static constexpr int OFF_W1 = OFF_B + 9 * C::B_STAGE;   // conv1 weights [9][16] + biases [16]
+  // 9 weight-tap barriers, then A full[2], A empty[2]
+  static constexpr int OFF_BAR = OFF_W1 + 1024;
+  static constexpr int SMEM_BYTES = OFF_BAR + 8 * 13 + 1024;
+  static_assert(!C::ALIAS && C::G == 1 && C::CIN == 16, "conv2 geometry");
+  static_assert(SMEM_BYTES <= C::SMEM_BUDGET, "shared memory budget");
+};
 
 }  // namespace nisqa

@@ -29,6 +29,10 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if (!done && ++spins > (1u << 26)) __trap();
   } while (!done);
 }
+// one arrival (release semantics: this thread's earlier shared-memory accesses are ordered before the phase completes)
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
@@ -45,7 +49,16 @@ __device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// barrier ID among the first N threads that reach it (N a multiple of 32; ID 0 is __syncthreads)
+template <int ID, int N> __device__ __forceinline__ void named_bar_sync() { asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(N) : "memory"); }
+
+// per-thread register budget of the calling warpgroup, raised (waits for registers released by others) or lowered
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// wait until at most N committed wgmma groups of this warpgroup are still pending
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // B operand: K-major, no swizzle: core matrices of 8 rows x 16 bytes, rows 16 B apart, 8-row groups SBO = 128 B apart
 // along N, K-adjacent core matrices LBO bytes apart
