@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define NISQA_B200_ABI_VERSION 3
+#define NISQA_B200_ABI_VERSION 4   /* nisqa_create also accepts 3: the struct without the self-attention widths */
 
 #if defined(__GNUC__)
 #define NISQA_API __attribute__((visibility("default")))
@@ -85,8 +85,9 @@ enum nisqa_stage {
   NISQA_STAGE_POOL3    = 4, /* [n_seg, 64, 6, W3]                                            */
   NISQA_STAGE_CONV5    = 5, /* [n_seg, 64, 6, W3]                                            */
   NISQA_STAGE_CNN_FEAT = 6, /* [n_seg, 384] (adapt, index c*6+h) or [n_seg, 20] (standard)   */
-  NISQA_STAGE_TD_IN    = 7, /* adapt only: LayerNorm(Linear 384->64) [n_seg, 64]             */
-  NISQA_STAGE_TD_OUT   = 8  /* [n_seg, 64] (self-attention) or [n_seg, 256] (BiLSTM fwd||bwd) */
+  NISQA_STAGE_TD_IN    = 7, /* adapt only: LayerNorm(Linear 384->D) [n_seg, D], D = sa_d_model */
+  NISQA_STAGE_TD_OUT   = 8  /* [n_seg, D] (output of the last self-attention stack: td2_d_model when td_2 runs, else
+                             * sa_d_model) or [n_seg, 256] (BiLSTM fwd||bwd)                                          */
 };
 
 /* Mirrors the checkpoint 'args' the hot path consumes (SURVEY.md Appendix A). */
@@ -113,7 +114,7 @@ typedef struct nisqa_config {
   int32_t de_align;      /* enum nisqa_de_align */
   int32_t de_align_apply;/* enum nisqa_de_apply */
   int32_t de_fuse;       /* enum nisqa_de_fuse */
-  int32_t td2_layers;    /* td_2 = 'self_att' (d_model 64, one head, h 64): number of layers; 0 = td_2 'skip'.  NISQA_DE needs >= 1;
+  int32_t td2_layers;    /* td_2 = 'self_att' (one head, width td2_d_model, feed-forward td2_ff): number of layers; 0 = td_2 'skip'.  NISQA_DE needs >= 1;
                           * NISQA / NISQA_DIM run it as a second stack behind the first (lib:114-141, 236-268) */
   int32_t td2_pos_enc;   /* td_2_sa_pos_enc */
   /* framewise model in front of the self-attention stack (arch NISQA_ARCH_ADAPT_SA_ATTFF): */
@@ -122,6 +123,12 @@ typedef struct nisqa_config {
                           * hidden width of DFF; a multiple of 64 */
   int32_t de_fuse_dim;   /* NISQA_DE: Linear(fused features -> de_fuse_dim) behind the fusion (lib:1399-1401, 1414-1415); 0 = none;
                           * a multiple of 64 */
+  /* ABI 4: widths of the self-attention stacks (one head; lib:945-1040).  0 = 64.  d_model: 64, 128, 192 or 256 (NISQA_DE:
+   * 64 only); feed-forward width (td_sa_h / td_2_sa_h): a multiple of 64 up to 4096 */
+  int32_t sa_d_model;    /* td_sa_d_model */
+  int32_t sa_ff;         /* td_sa_h */
+  int32_t td2_d_model;   /* td_2_sa_d_model */
+  int32_t td2_ff;        /* td_2_sa_h */
 } nisqa_config;
 
 /* One state_dict entry, passed straight through: name as in the checkpoint

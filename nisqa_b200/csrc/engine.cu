@@ -50,7 +50,7 @@ struct LstmParams { const float* w_ih; const float* w_hh; const float* b; const 
 void launch_fc20(cudaStream_t, const float*, const float*, const float*, float*, int);
 void launch_lstm(cudaStream_t, const float*, const ClipDesc*, int, const LstmParams&, float*, float*, float, float*);
 void launch_lstm_batched(cudaStream_t, const float*, const ClipDesc*, const int*, int, const LstmParams&, float*, float*, float, float*);
-void launch_pool_final(cudaStream_t, const float*, const float*, const ClipDesc*, int, const PoolHeadParams&, int, int, float*);
+void launch_pool_final(cudaStream_t, const float*, int, const float*, const ClipDesc*, int, const PoolHeadParams&, int, int, float*);
 // td_tiled.cu
 struct ResampleClip { long long in_off, out_off, time_off; int n_in, n_out, n_fix, copy; double ratio; };
 void launch_resample(cudaStream_t, const void*, int, const ResampleClip*, int, int, double*, const double*, int, int, float*);
@@ -60,12 +60,12 @@ void launch_de_align(cudaStream_t, const float*, const ClipDesc*, int, const int
 void launch_de_finalize(cudaStream_t, const ClipDesc*, int, int, float*);
 void launch_seg_feats(cudaStream_t, const float*, const int*, const float*, const float*, int, float*);
 void launch_linear_tile(cudaStream_t, const float*, int, const float*, const float*, int, float*, int, int, int, int);
-void launch_td_in(cudaStream_t, const float*, const float*, int, const float*, const float*, const float*,
-                  const float*, const float*, const float*, const int*, const ClipDesc*, float*, float*, int);
+void launch_td_in(cudaStream_t, int, const float*, const float*, int, const float*, const float*, const float*,
+                  const float*, const float*, float, const float*, const int*, const ClipDesc*, float*, float*, int);
 struct PoolSimpleParams { const float* a1; const float* a1b; const float* w3; const float* b3; };
 void launch_pool_simple(cudaStream_t, const float*, int, const ClipDesc*, int, int, const PoolSimpleParams&, int, int, float*);
-void launch_td_sa(cudaStream_t, const float*, const float*, const ClipDesc*, int, const int*, int, const SaLayerParams&,
-                  float*, const float*, const float*, float*, const PoolHeadParams&, int, float*);
+void launch_td_sa(cudaStream_t, int, const float*, const float*, const ClipDesc*, int, const int*, int, const SaLayerParams&, int,
+                  float*, const float*, const float*, float, float*, const PoolHeadParams&, int, float*);
 }  // namespace nisqa
 
 using namespace nisqa;
@@ -210,6 +210,12 @@ struct nisqa_engine {
   float tc_scale[8] = {1, 1, 1, 1, 1, 1, 1, 1};   // 2^(e_{i-1} - S_i): undoes the activation and weight pre-scales of conv i
   int act_exp[8] = {0, 0, 0, 0, 0, 0, 0, 0};      // e_i: conv i's activations are stored as fp16 planes of v * 2^-e_i
   float act_store(int i) const { return ldexpf(1.f, -act_exp[i]); }
+  // widths of the self-attention stacks (0 in the config = 64) and of the rows the pooling module reads
+  int sa_d() const { return cfg.sa_d_model ? cfg.sa_d_model : 64; }
+  int sa_f() const { return cfg.sa_ff ? cfg.sa_ff : 64; }
+  int td2_d() const { return cfg.td2_d_model ? cfg.td2_d_model : 64; }
+  int td2_f() const { return cfg.td2_ff ? cfg.td2_ff : 64; }
+  int pool_d() const { return cfg.td2_layers > 0 ? td2_d() : sa_d(); }
 
   // front-end tables
   std::vector<FbEntry*> fbs;
@@ -234,6 +240,7 @@ struct nisqa_engine {
   int last_n_seg = 0, last_n_frames = 0, last_passes = 0;
   const float* last_td_in = nullptr;
   const float* last_td_out = nullptr;
+  int last_td_out_d = 64;       // row width of last_td_out
 
   // engine-owned NCCL communicator (multi-GPU gather, SURVEY.md 8e)
   void* nccl_comm = nullptr;
@@ -477,6 +484,20 @@ void pack_linear_T(Packer& P, size_t off, const TensorView* w, int n_out, int n_
     for (int j = 0; j < n_out; ++j) P.arena[off + (size_t)k * n_out + j] = w->d[(size_t)j * n_in + k] * scale;
 }
 
+// W^T of an nn.Linear(n_in -> n_out) in 64-column chunks (the layout of the td_tiled.cu kernels): chunk n is the k-major
+// [k_pad][64] block at n k_pad 64; engine input row k reads checkpoint input column col(k); rows >= n_in stay zero
+template <class Col>
+void pack_linear_chunked(Packer& P, size_t off, const TensorView* w, int n_out, int n_in, int k_pad, Col col) {
+  for (int n = 0; n < n_out / 64; ++n)
+    for (int k = 0; k < n_in; ++k)
+      for (int j = 0; j < 64; ++j) P.arena[off + ((size_t)n * k_pad + k) * 64 + j] = w->d[(size_t)(n * 64 + j) * n_in + col(k)];
+}
+
+// nn.MultiheadAttention scales q by D^-1/2 after the in-projection: folded into the packed q weights where that is a power
+// of two (exact), otherwise applied by the kernels to the projected q (qscale)
+float q_fold(int D) { return D == 64 ? 0.125f : D == 256 ? 0.0625f : 1.f; }
+float q_scale(int D) { return q_fold(D) == 1.f ? (float)(1.0 / std::sqrt((double)D)) : 1.f; }
+
 int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
   Packer P; P.e = e;
   for (int i = 0; i < n; ++i) {
@@ -570,69 +591,66 @@ int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
 
   if (e->cfg.arch == NISQA_ARCH_ADAPT_SA_ATTFF) {
     const std::string td = "time_dependency.model.";
-    // one SelfAttention stack (lib:945-1040): Linear(in -> 64) + LayerNorm + `layers` encoder layers.  `kp` prefixes the
-    // arena keys ("" = time_dependency, "2" = time_dependency_2 of the double-ended model)
-    auto pack_sa_stack = [&](const std::string& ck, const std::string& kp, int in_dim, int layers, bool cnn_order) -> bool {
-      const TensorView* lw = P.get(ck + "linear.weight", {64, in_dim});
-      const TensorView* lb = P.get(ck + "linear.bias", {64});
-      const TensorView* ng = P.get(ck + "norm1.weight", {64});
-      const TensorView* nb = P.get(ck + "norm1.bias", {64});
+    // one SelfAttention stack (lib:945-1040) of width D and feed-forward width F: Linear(in -> D) + LayerNorm + `layers`
+    // encoder layers.  `kp` prefixes the arena keys ("" = time_dependency, "2" = time_dependency_2)
+    auto pack_sa_stack = [&](const std::string& ck, const std::string& kp, int in_dim, int layers, bool cnn_order, int D,
+                             int F) -> bool {
+      const size_t vb = (size_t)D * 4;
+      const TensorView* lw = P.get(ck + "linear.weight", {D, in_dim});
+      const TensorView* lb = P.get(ck + "linear.bias", {D});
+      const TensorView* ng = P.get(ck + "norm1.weight", {D});
+      const TensorView* nb = P.get(ck + "norm1.bias", {D});
       if (!lw || !lb || !ng || !nb) return false;
-      size_t o = P.alloc("lin" + kp + ".wT", (size_t)((in_dim + 63) / 64 * 64) * 64);      // (rows beyond in_dim stay zero)
-      if (cnn_order) {
-        // engine feature order k' = h*64 + c  <->  reference view(-1, 64*6) order c*6 + h (lib:706)
-        for (int h = 0; h < 6; ++h)
-          for (int c = 0; c < 64; ++c)
-            for (int j = 0; j < 64; ++j) P.arena[o + ((size_t)h * 64 + c) * 64 + j] = lw->d[(size_t)j * 384 + c * 6 + h];
-      } else {
-        pack_linear_T(P, o, lw, 64, in_dim);
-      }
-      o = P.alloc("lin" + kp + ".b", 64); memcpy(&P.arena[o], lb->d, 256);
-      o = P.alloc("ln" + kp + "0.g", 64); memcpy(&P.arena[o], ng->d, 256);
-      o = P.alloc("ln" + kp + "0.b", 64); memcpy(&P.arena[o], nb->d, 256);
+      const int k_pad = (in_dim + 63) / 64 * 64;
+      size_t o = P.alloc("lin" + kp + ".wT", (size_t)k_pad * D);
+      if (cnn_order)      // engine feature order k' = h*64 + c  <->  reference view(-1, 64*6) order c*6 + h (lib:706)
+        pack_linear_chunked(P, o, lw, D, in_dim, k_pad, [](int k) { return (k & 63) * 6 + (k >> 6); });
+      else
+        pack_linear_chunked(P, o, lw, D, in_dim, k_pad, [](int k) { return k; });
+      o = P.alloc("lin" + kp + ".b", D); memcpy(&P.arena[o], lb->d, vb);
+      o = P.alloc("ln" + kp + "0.g", D); memcpy(&P.arena[o], ng->d, vb);
+      o = P.alloc("ln" + kp + "0.b", D); memcpy(&P.arena[o], nb->d, vb);
+      const auto id = [](int k) { return k; };
       for (int l = 0; l < layers; ++l) {
         char pf[96]; snprintf(pf, sizeof pf, "layers.%d.", l);
         char key[64];
         const std::string p = ck + pf;
-        const TensorView* iw = P.get(p + "self_attn.in_proj_weight", {192, 64});
-        const TensorView* ib = P.get(p + "self_attn.in_proj_bias", {192});
-        const TensorView* ow = P.get(p + "self_attn.out_proj.weight", {64, 64});
-        const TensorView* ob = P.get(p + "self_attn.out_proj.bias", {64});
-        const TensorView* w1 = P.get(p + "linear1.weight", {64, 64});
-        const TensorView* b1 = P.get(p + "linear1.bias", {64});
-        const TensorView* w2 = P.get(p + "linear2.weight", {64, 64});
-        const TensorView* b2 = P.get(p + "linear2.bias", {64});
-        const TensorView* g1 = P.get(p + "norm1.weight", {64});
-        const TensorView* e1 = P.get(p + "norm1.bias", {64});
-        const TensorView* g2 = P.get(p + "norm2.weight", {64});
-        const TensorView* e2 = P.get(p + "norm2.bias", {64});
+        const TensorView* iw = P.get(p + "self_attn.in_proj_weight", {3 * D, D});
+        const TensorView* ib = P.get(p + "self_attn.in_proj_bias", {3 * D});
+        const TensorView* ow = P.get(p + "self_attn.out_proj.weight", {D, D});
+        const TensorView* ob = P.get(p + "self_attn.out_proj.bias", {D});
+        const TensorView* w1 = P.get(p + "linear1.weight", {F, D});
+        const TensorView* b1 = P.get(p + "linear1.bias", {F});
+        const TensorView* w2 = P.get(p + "linear2.weight", {D, F});
+        const TensorView* b2 = P.get(p + "linear2.bias", {D});
+        const TensorView* g1 = P.get(p + "norm1.weight", {D});
+        const TensorView* e1 = P.get(p + "norm1.bias", {D});
+        const TensorView* g2 = P.get(p + "norm2.weight", {D});
+        const TensorView* e2 = P.get(p + "norm2.bias", {D});
         if (!iw || !ib || !ow || !ob || !w1 || !b1 || !w2 || !b2 || !g1 || !e1 || !g2 || !e2) return false;
         auto K = [&](const char* s2) { snprintf(key, sizeof key, "sa%s%d.%s", kp.c_str(), l, s2); return std::string(key); };
-        o = P.alloc(K("qkvT"), 3 * 4096);
-        for (int part = 0; part < 3; ++part) {
-          const float sc = part == 0 ? 0.125f : 1.f;      // q * 1/sqrt(64): exact power of two
-          for (int k = 0; k < 64; ++k)
-            for (int j = 0; j < 64; ++j)
-              P.arena[o + part * 4096 + k * 64 + j] = iw->d[(size_t)(part * 64 + j) * 64 + k] * sc;
-        }
-        o = P.alloc(K("qkvb"), 192);
-        for (int j = 0; j < 192; ++j) P.arena[o + j] = ib->d[j] * (j < 64 ? 0.125f : 1.f);
-        o = P.alloc(K("woT"), 4096); pack_linear_T(P, o, ow, 64, 64);
-        o = P.alloc(K("bo"), 64); memcpy(&P.arena[o], ob->d, 256);
-        o = P.alloc(K("w1T"), 4096); pack_linear_T(P, o, w1, 64, 64);
-        o = P.alloc(K("b1"), 64); memcpy(&P.arena[o], b1->d, 256);
-        o = P.alloc(K("w2T"), 4096); pack_linear_T(P, o, w2, 64, 64);
-        o = P.alloc(K("b2"), 64); memcpy(&P.arena[o], b2->d, 256);
-        o = P.alloc(K("ln1g"), 64); memcpy(&P.arena[o], g1->d, 256);
-        o = P.alloc(K("ln1b"), 64); memcpy(&P.arena[o], e1->d, 256);
-        o = P.alloc(K("ln2g"), 64); memcpy(&P.arena[o], g2->d, 256);
-        o = P.alloc(K("ln2b"), 64); memcpy(&P.arena[o], e2->d, 256);
+        const float qf = q_fold(D);
+        o = P.alloc(K("qkvT"), (size_t)3 * D * D);
+        pack_linear_chunked(P, o, iw, 3 * D, D, D, id);
+        for (size_t i = 0; i < (size_t)D * D; ++i) P.arena[o + i] *= qf;          // the q chunks come first
+        o = P.alloc(K("qkvb"), 3 * D);
+        for (int j = 0; j < 3 * D; ++j) P.arena[o + j] = ib->d[j] * (j < D ? qf : 1.f);
+        o = P.alloc(K("woT"), (size_t)D * D); pack_linear_chunked(P, o, ow, D, D, D, id);
+        o = P.alloc(K("bo"), D); memcpy(&P.arena[o], ob->d, vb);
+        o = P.alloc(K("w1T"), (size_t)F * D); pack_linear_chunked(P, o, w1, F, D, D, id);
+        o = P.alloc(K("b1"), F); memcpy(&P.arena[o], b1->d, (size_t)F * 4);
+        o = P.alloc(K("w2T"), (size_t)D * F); pack_linear_chunked(P, o, w2, D, F, F, id);
+        o = P.alloc(K("b2"), D); memcpy(&P.arena[o], b2->d, vb);
+        o = P.alloc(K("ln1g"), D); memcpy(&P.arena[o], g1->d, vb);
+        o = P.alloc(K("ln1b"), D); memcpy(&P.arena[o], e1->d, vb);
+        o = P.alloc(K("ln2g"), D); memcpy(&P.arena[o], g2->d, vb);
+        o = P.alloc(K("ln2b"), D); memcpy(&P.arena[o], e2->d, vb);
       }
       return true;
     };
-    auto pack_pos_enc = [&](const std::string& ck, const std::string& key) -> int {
-      auto it = P.t.find(ck + "pos_encoder.pe");                  // registered buffer [max_len, 1, 64] (lib:1051-1058)
-      if (it == P.t.end() || it->second.nd != 3 || it->second.dims[1] != 1 || it->second.dims[2] != 64)
+    auto pack_pos_enc = [&](const std::string& ck, const std::string& key, int D) -> int {
+      auto it = P.t.find(ck + "pos_encoder.pe");                  // registered buffer [max_len, 1, D] (lib:1051-1058)
+      if (it == P.t.end() || it->second.nd != 3 || it->second.dims[1] != 1 || it->second.dims[2] != D)
         return fail(e, NISQA_ERR_WEIGHTS, "missing tensor " + ck + "pos_encoder.pe");
       if (e->cfg.max_segments > 0 && it->second.dims[0] < e->cfg.max_segments)
         return fail(e, NISQA_ERR_WEIGHTS, "positional encoding shorter than ms_max_segments");
@@ -655,12 +673,13 @@ int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
           for (int j = 0; j < H; ++j) P.arena[ow + ((size_t)h * 64 + c) * H + j] = w->d[(size_t)j * 384 + c * 6 + h];
       memcpy(&P.arena[ob], b->d, (size_t)H * 4);
     }
-    if (!pack_sa_stack(td, "", feat_dim, e->cfg.sa_layers, conv_net && e->cfg.cnn_fc == 0)) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
+    if (!pack_sa_stack(td, "", feat_dim, e->cfg.sa_layers, conv_net && e->cfg.cnn_fc == 0, e->sa_d(), e->sa_f()))
+      return fail(e, NISQA_ERR_WEIGHTS, P.missing);
     if (e->cfg.double_ended || e->cfg.td2_layers > 0) {
       // time_dependency_2: behind the fusion of the double-ended model (input 192 / 128), or a second stack behind the
-      // first one in NISQA / NISQA_DIM (lib:114-141, 236-268; input 64)
+      // first one in NISQA / NISQA_DIM (lib:114-141, 236-268; input: the first stack's width)
       const std::string td2 = "time_dependency_2.model.";
-      int fdim = !e->cfg.double_ended ? 64 : (e->cfg.de_fuse == NISQA_DE_FUSE_XY_MINUS ? 192 : 128);
+      int fdim = !e->cfg.double_ended ? e->sa_d() : (e->cfg.de_fuse == NISQA_DE_FUSE_XY_MINUS ? 192 : 128);
       if (e->cfg.double_ended && e->cfg.de_fuse_dim > 0) {        // Fusion.lin_fusion (lib:1399-1401)
         const int D = e->cfg.de_fuse_dim;
         const TensorView* w = P.get("fuse.lin_fusion.weight", {D, fdim});
@@ -671,8 +690,8 @@ int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
         memcpy(&P.arena[ob], b->d, (size_t)D * 4);
         fdim = D;
       }
-      if (!pack_sa_stack(td2, "2", fdim, e->cfg.td2_layers, false)) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-      if (e->cfg.td2_pos_enc) { int rc = pack_pos_enc(td2, "pe2"); if (rc) return rc; }
+      if (!pack_sa_stack(td2, "2", fdim, e->cfg.td2_layers, false, e->td2_d(), e->td2_f())) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
+      if (e->cfg.td2_pos_enc) { int rc = pack_pos_enc(td2, "pe2", e->td2_d()); if (rc) return rc; }
       if (e->cfg.de_align == NISQA_DE_ALIGN_LUONG) {            // AttLuong: W = Linear(y_dim -> q_dim), lib:1348-1351
         const TensorView* w = P.get("align.att.W.weight", {64, 64});
         const TensorView* b = P.get("align.att.W.bias", {64});
@@ -701,41 +720,42 @@ int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
       else snprintf(pf, sizeof pf, "pool_layers.%d.model.", h);   // head order mos,noi,dis,col,loud (lib:1461-1465)
       return std::string(pf);
     };
-    if (e->cfg.pos_enc) { int rc = pack_pos_enc(td, "pe"); if (rc) return rc; }
+    if (e->cfg.pos_enc) { int rc = pack_pos_enc(td, "pe", e->sa_d()); if (rc) return rc; }
+    const int Dp = e->pool_d();        // width of the rows the pooling module reads
     if (e->cfg.pool == NISQA_POOL_ATT_FF) {
-    const size_t oW1 = P.alloc("pool.w1T", (size_t)nh * 64 * 128), ob1 = P.alloc("pool.b1", nh * 128),
+    const size_t oW1 = P.alloc("pool.w1T", (size_t)nh * Dp * 128), ob1 = P.alloc("pool.b1", nh * 128),
                  ow2 = P.alloc("pool.w2", nh * 128), ob2 = P.alloc("pool.b2", nh),
-                 ow3 = P.alloc("pool.w3", nh * 64), ob3 = P.alloc("pool.b3", nh);
+                 ow3 = P.alloc("pool.w3", nh * Dp), ob3 = P.alloc("pool.b3", nh);
     for (int h = 0; h < nh; ++h) {
       const std::string p = head_prefix(h);
-      const TensorView* w1 = P.get(p + "linear1.weight", {128, 64});
+      const TensorView* w1 = P.get(p + "linear1.weight", {128, Dp});
       const TensorView* b1 = P.get(p + "linear1.bias", {128});
       const TensorView* w2 = P.get(p + "linear2.weight", {1, 128});
       const TensorView* b2 = P.get(p + "linear2.bias", {1});
-      const TensorView* w3 = P.get(p + "linear3.weight", {1, 64});
+      const TensorView* w3 = P.get(p + "linear3.weight", {1, Dp});
       const TensorView* b3 = P.get(p + "linear3.bias", {1});
       if (!w1 || !b1 || !w2 || !b2 || !w3 || !b3) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-      pack_linear_T(P, oW1 + (size_t)h * 64 * 128, w1, 128, 64);
+      pack_linear_T(P, oW1 + (size_t)h * Dp * 128, w1, 128, Dp);          // [head][D][128]
       memcpy(&P.arena[ob1 + h * 128], b1->d, 512);
       memcpy(&P.arena[ow2 + h * 128], w2->d, 512);
       P.arena[ob2 + h] = b2->d[0];
-      memcpy(&P.arena[ow3 + h * 64], w3->d, 256);
+      memcpy(&P.arena[ow3 + h * Dp], w3->d, (size_t)Dp * 4);
       P.arena[ob3 + h] = b3->d[0];
     }
     } else {
-      // PoolAtt: linear1 (64 -> 1 attention logit) + linear2 (64 -> 1); PoolAvg / PoolMax / PoolLastStep: linear (64 -> 1)
+      // PoolAtt: linear1 (D -> 1 attention logit) + linear2 (D -> 1); PoolAvg / PoolMax / PoolLastStep: linear (D -> 1)
       const bool att = e->cfg.pool == NISQA_POOL_ATT;
-      const size_t oa1 = P.alloc("pool.a1", nh * 64), oa1b = P.alloc("pool.a1b", nh),
-                   ow3 = P.alloc("pool.w3", nh * 64), ob3 = P.alloc("pool.b3", nh);
+      const size_t oa1 = P.alloc("pool.a1", nh * Dp), oa1b = P.alloc("pool.a1b", nh),
+                   ow3 = P.alloc("pool.w3", nh * Dp), ob3 = P.alloc("pool.b3", nh);
       for (int h = 0; h < nh; ++h) {
         const std::string p = head_prefix(h);
-        const TensorView* a1 = att ? P.get(p + "linear1.weight", {1, 64}) : nullptr;
+        const TensorView* a1 = att ? P.get(p + "linear1.weight", {1, Dp}) : nullptr;
         const TensorView* a1b = att ? P.get(p + "linear1.bias", {1}) : nullptr;
-        const TensorView* w3 = P.get(p + (att ? "linear2.weight" : "linear.weight"), {1, 64});
+        const TensorView* w3 = P.get(p + (att ? "linear2.weight" : "linear.weight"), {1, Dp});
         const TensorView* b3 = P.get(p + (att ? "linear2.bias" : "linear.bias"), {1});
         if ((att && (!a1 || !a1b)) || !w3 || !b3) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-        if (att) { memcpy(&P.arena[oa1 + h * 64], a1->d, 256); P.arena[oa1b + h] = a1b->d[0]; }
-        memcpy(&P.arena[ow3 + h * 64], w3->d, 256);
+        if (att) { memcpy(&P.arena[oa1 + h * Dp], a1->d, (size_t)Dp * 4); P.arena[oa1b + h] = a1b->d[0]; }
+        memcpy(&P.arena[ow3 + h * Dp], w3->d, (size_t)Dp * 4);
         P.arena[ob3 + h] = b3->d[0];
       }
     }
@@ -1003,11 +1023,12 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
       sa_in = LN.ffb.as<float>(); sa_nk = c.cnn_fc / 64;
     }
     if (!std_mode) {
-      CK(LN.xa.reserve((size_t)n_seg * 64 * 4));
-      CK(LN.xb.reserve((size_t)n_seg * 64 * 4));
-      CK(LN.qkv.reserve((size_t)n_seg * 192 * 4));
+      const int D1 = e->sa_d(), D2 = c.td2_layers > 0 ? e->td2_d() : 0, Dm = std::max(D1, D2);
+      CK(LN.xa.reserve((size_t)n_seg * Dm * 4));
+      CK(LN.xb.reserve((size_t)n_seg * Dm * 4));
+      CK(LN.qkv.reserve((size_t)n_seg * 3 * Dm * 4));
       CK(LN.logits.reserve((size_t)n_seg * n_out * 4));
-      CK(LN.tdout.reserve((size_t)n_seg * 64 * 4));
+      CK(LN.tdout.reserve((size_t)n_seg * D1 * 4));
       const bool attff = c.pool == NISQA_POOL_ATT_FF;
       PoolHeadParams H = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
       if (attff) {
@@ -1020,13 +1041,15 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
       // Linear+LN (+positional encoding, +QKV of layer 0) | per layer: attention + out_proj + FFN + LNs (+ next QKV, or
       // the PoolAttFF logits behind the last layer) | per-clip pooling.  qkv ping-pongs between two buffers: a layer's
       // CTAs read keys / values of rows whose next-layer projection other CTAs are already writing.
-      CK(LN.qkv2.reserve((size_t)n_seg * 192 * 4));
+      CK(LN.qkv2.reserve((size_t)n_seg * 3 * Dm * 4));
       float* qk[2] = {LN.qkv.as<float>(), LN.qkv2.as<float>()};
       const bool de = c.double_ended != 0;
       // one SelfAttention stack; `kp` = "" (time_dependency) or "2" (time_dependency_2); the stack that feeds the pooling
       // module computes the PoolAttFF logits behind its last layer
       auto sa_stack = [&](const std::string& kp, const float* in_rows, int nk, int layers, bool pos_enc, bool feeds_pool,
-                          float* x0) -> const float* {
+                          float* x0, int D, int F) -> const float* {
+        const int nc = D / 64;
+        const float qs = q_scale(D);
         auto key = [&](int l, const char* s2) { char k[40]; snprintf(k, sizeof k, "sa%s%d.%s", kp.c_str(), l, s2); return std::string(k); };
         auto params = [&](int l) {
           SaLayerParams P;
@@ -1036,25 +1059,25 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
           return P;
         };
         { Scope s(e, "lin_ln");
-          launch_td_in(st, in_rows, W(e, "lin" + kp + ".wT"), nk, W(e, "lin" + kp + ".b"), W(e, "ln" + kp + "0.g"), W(e, "ln" + kp + "0.b"),
-                       W(e, key(0, "qkvT")), W(e, key(0, "qkvb")), pos_enc ? W(e, kp.empty() ? "pe" : "pe2") : nullptr, seg_clip, d_clips,
-                       x0, qk[0], n_seg); }
+          launch_td_in(st, nc, in_rows, W(e, "lin" + kp + ".wT"), nk, W(e, "lin" + kp + ".b"), W(e, "ln" + kp + "0.g"),
+                       W(e, "ln" + kp + "0.b"), W(e, key(0, "qkvT")), W(e, key(0, "qkvb")), qs,
+                       pos_enc ? W(e, kp.empty() ? "pe" : "pe2") : nullptr, seg_clip, d_clips, x0, qk[0], n_seg); }
         const float* cur2 = x0;
         for (int l = 0; l < layers; ++l) {
           const bool last = l + 1 == layers;
           Scope s(e, "sa_layer");
-          launch_td_sa(st, cur2, qk[l & 1], d_clips, n, d_qt64, n_qt64, params(l), pp[l & 1],
-                       last ? nullptr : W(e, key(l + 1, "qkvT")), last ? nullptr : W(e, key(l + 1, "qkvb")),
+          launch_td_sa(st, nc, cur2, qk[l & 1], d_clips, n, d_qt64, n_qt64, params(l), F, pp[l & 1],
+                       last ? nullptr : W(e, key(l + 1, "qkvT")), last ? nullptr : W(e, key(l + 1, "qkvb")), qs,
                        qk[(l + 1) & 1], H, (feeds_pool && attff) ? n_out : 0, LN.logits.as<float>());
           cur2 = pp[l & 1];
         }
         return cur2;
       };
       const bool td2_single = !de && c.td2_layers > 0;      // NISQA / NISQA_DIM with td_2 = 'self_att'
-      cur = sa_stack("", sa_in, sa_nk, c.sa_layers, c.pos_enc != 0, !de && !td2_single, LN.tdout.as<float>());
+      cur = sa_stack("", sa_in, sa_nk, c.sa_layers, c.pos_enc != 0, !de && !td2_single, LN.tdout.as<float>(), D1, e->sa_f());
       if (td2_single) {
-        CK(LN.td2in.reserve((size_t)n_seg * 64 * 4));
-        cur = sa_stack("2", cur, 1, c.td2_layers, c.td2_pos_enc != 0, true, LN.td2in.as<float>());
+        CK(LN.td2in.reserve((size_t)n_seg * D2 * 4));
+        cur = sa_stack("2", cur, D1 / 64, c.td2_layers, c.td2_pos_enc != 0, true, LN.td2in.as<float>(), D2, e->td2_f());
       }
       if (de) {
         // NISQA_DE (lib:404-424): align the reference clip's rows to the degraded clip's, fuse, second time-dependency stack
@@ -1079,14 +1102,15 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
                              n_seg, 64 * nf, c.de_fuse_dim);
           td2_rows = LN.ffa.as<float>(); td2_nk = c.de_fuse_dim / 64;
         }
-        cur = sa_stack("2", td2_rows, td2_nk, c.td2_layers, c.td2_pos_enc != 0, true, LN.td2in.as<float>());
+        cur = sa_stack("2", td2_rows, td2_nk, c.td2_layers, c.td2_pos_enc != 0, true, LN.td2in.as<float>(), D2, e->td2_f());
       }
       e->last_td_out = cur;
+      e->last_td_out_d = e->pool_d();
       { Scope s(e, "pool");
-        if (attff) launch_pool_final(st, cur, LN.logits.as<float>(), d_clips, n, H, n_out, max_n_seg, scores);
+        if (attff) launch_pool_final(st, cur, e->pool_d(), LN.logits.as<float>(), d_clips, n, H, n_out, max_n_seg, scores);
         else {
           PoolSimpleParams Q = {W(e, "pool.a1"), W(e, "pool.a1b"), W(e, "pool.w3"), W(e, "pool.b3")};
-          launch_pool_simple(st, cur, 64, d_clips, n, c.pool, Q, n_out, max_n_seg, scores);
+          launch_pool_simple(st, cur, e->pool_d(), d_clips, n, c.pool, Q, n_out, max_n_seg, scores);
         }
         if (de) launch_de_finalize(st, d_clips, n, n_out, scores); }
     } else {
@@ -1112,6 +1136,7 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
       }
       e->last_td_in = nullptr;
       e->last_td_out = (e->lstm_batched && !keep) ? nullptr : LN.tdout.as<float>();
+      e->last_td_out_d = 256;
     }
   }
   CK(cudaGetLastError());
@@ -1151,7 +1176,9 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
   }
   // segments per internal pass: 131072 segments keep ~8 GB of activation planes per compute lane (three lanes stay
   // well inside the 80 GB of an H100) and give the BiLSTM >= 128 clips per launch at configs[3]; one 64-clip batch is 15 808
-  const int max_seg = e->cfg.max_chunk_segments > 0 ? e->cfg.max_chunk_segments : 131072;
+  // (scaled down for self-attention stacks wider than 64: their activation rows grow with d_model)
+  const int d_max = std::max(e->sa_d(), e->cfg.td2_layers > 0 ? e->td2_d() : 64);
+  const int max_seg = e->cfg.max_chunk_segments > 0 ? e->cfg.max_chunk_segments : 131072 / (d_max / 64);
   float* scores_all = scores_dev;
   if (!scores_all) {
     DevBuf& sb = ticket_out ? e->tickets[e->next_ticket % kStages].scores : e->scores;
@@ -1238,9 +1265,13 @@ int nisqa_create(nisqa_engine** out, int device, const nisqa_config* cfg) {
   if (!out || !cfg) return NISQA_ERR_INVALID;
   *out = nullptr;
   nisqa_engine* e = new nisqa_engine();
-  e->cfg = *cfg; e->device = device;
+  e->device = device;
   *out = e;     // returned even on failure so that nisqa_last_error() can be read
-  if (cfg->abi_version != NISQA_B200_ABI_VERSION) return fail(e, NISQA_ERR_INVALID, "abi_version mismatch");
+  // ABI 3 callers pass the smaller struct without the self-attention widths: never read past it (their widths are 64)
+  if (cfg->abi_version != 3 && cfg->abi_version != NISQA_B200_ABI_VERSION) return fail(e, NISQA_ERR_INVALID, "abi_version mismatch");
+  memset(&e->cfg, 0, sizeof e->cfg);
+  memcpy(&e->cfg, cfg, cfg->abi_version == 3 ? offsetof(nisqa_config, sa_d_model) : sizeof(nisqa_config));
+  cfg = &e->cfg;
   if (cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF && cfg->arch != NISQA_ARCH_STD_LSTM_LASTBI)
     return fail(e, NISQA_ERR_INVALID, "unsupported architecture");
   if (cfg->n_fft != kNfft || cfg->n_mels != kMels || cfg->seg_len != kSegLen)
@@ -1263,6 +1294,18 @@ int nisqa_create(nisqa_engine** out, int device, const nisqa_config* cfg) {
     return fail(e, NISQA_ERR_INVALID, "cnn_kind / cnn_fc: SkipCNN and DFF feed the self-attention architecture; cnn_fc_out_h a multiple of 64");
   if (cfg->td2_layers < 0 || cfg->td2_layers > 8 || (cfg->td2_layers > 0 && cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF))
     return fail(e, NISQA_ERR_INVALID, "td_2 = 'self_att' needs the self-attention architecture (td2_layers 0..8)");
+  {
+    const int32_t w[4] = {cfg->sa_d_model, cfg->sa_ff, cfg->td2_d_model, cfg->td2_ff};
+    const char* nm[4] = {"sa_d_model", "sa_ff", "td2_d_model", "td2_ff"};
+    for (int i = 0; i < 4; ++i) {
+      const int lim = (i & 1) ? 4096 : 256;        // d_model 64..256, feed-forward width 64..4096, multiples of 64 (0 = 64)
+      if (w[i] < 0 || w[i] % 64 != 0 || w[i] > lim || (w[i] != 0 && cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF))
+        return fail(e, NISQA_ERR_INVALID, std::string(nm[i]) + " = " + std::to_string(w[i]) +
+                                              ": the self-attention kernels take d_model 64..256 and h 64..4096, multiples of 64");
+    }
+    if (cfg->double_ended && (e->sa_d() != 64 || e->td2_d() != 64))
+      return fail(e, NISQA_ERR_INVALID, "NISQA_DE: the alignment and fusion kernels are 64 wide (sa_d_model = td2_d_model = 64)");
+  }
   if (cfg->double_ended) {
     if (cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF || cfg->n_out != 1)
       return fail(e, NISQA_ERR_INVALID, "NISQA_DE: AdaptCNN + self-attention, one output");
@@ -1495,10 +1538,10 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
       break;
     case NISQA_STAGE_TD_IN:
       if (std_mode || !e->last_td_in) return fail(e, NISQA_ERR_INVALID, "stage not available for this architecture");
-      src = e->last_td_in; count = ns * 64; break;
+      src = e->last_td_in; count = ns * e->sa_d(); break;
     case NISQA_STAGE_TD_OUT:
       if (!e->last_td_out) return fail(e, NISQA_ERR_STATE, "the per-step BiLSTM outputs were not kept: nisqa_set_option(\"keep_td_out\", 1) before the predict call");
-      src = e->last_td_out; count = ns * (std_mode ? 256 : 64); break;
+      src = e->last_td_out; count = ns * e->last_td_out_d; break;
     default: return fail(e, NISQA_ERR_INVALID, "unknown stage");
   }
   if (ch > 0) count = ns * hw * ch;

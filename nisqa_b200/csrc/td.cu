@@ -97,22 +97,22 @@ struct SaLayerParams {
   const float* WoT; const float* bo; const float* W1T; const float* b1; const float* W2T;
   const float* b2; const float* ln1_g; const float* ln1_b; const float* ln2_g; const float* ln2_b;
 };
-// PoolAttFF (lib:1156-1183): the logits w2_h . relu(W1_h x + b1_h) + b2_h come out of td_sa_kernel's fused tail
+// PoolAttFF (lib:1156-1183): the logits w2_h . relu(W1_h x + b1_h) + b2_h come out of td_sa_kernel's fused tail; x is D wide
 struct PoolHeadParams {      // device pointers, heads concatenated
-  const float* W1T;   // [n_heads][64 k][128 j]
+  const float* W1T;   // [n_heads][D k][128 j]
   const float* b1;    // [n_heads][128]
   const float* w2;    // [n_heads][128]
   const float* b2;    // [n_heads]
-  const float* w3;    // [n_heads][64]
+  const float* w3;    // [n_heads][D]
   const float* b3;    // [n_heads]
 };
 
-// softmax over the clip's time steps, weighted sum of x, Linear 64->1   (lib:1177-1181)
-// grid = n_clips, block = 64 * n_heads; thread (h, d).  The softmax numerators are formed once per (head, step) into shared
+// softmax over the clip's time steps, weighted sum of x, Linear D->1   (lib:1177-1181)
+// grid = n_clips, block = 64 * n_heads; thread (h, d) owns features d, d + 64, .. < D.  The softmax numerators are formed once per (head, step) into shared
 // memory; the weighted sum keeps ONE accumulator per thread in step order (the result does not depend on the unrolling) with
 // eight independent loads in flight.
 __global__ void pool_final_kernel(const float* __restrict__ x, const float* __restrict__ logits,
-                                  const ClipDesc* __restrict__ clips, PoolHeadParams P, int n_heads, int max_seg,
+                                  const ClipDesc* __restrict__ clips, PoolHeadParams P, int n_heads, int max_seg, int D,
                                   float* __restrict__ scores) {
   __shared__ float red[5 * 64];
   extern __shared__ float pnum[];                       // [n_heads][max_seg] softmax numerators
@@ -136,19 +136,23 @@ __global__ void pool_final_kernel(const float* __restrict__ x, const float* __re
   for (int o = 32; o > 0; o >>= 1) { if (d < o) red[threadIdx.x] += red[threadIdx.x + o]; __syncthreads(); }
   sum = red[h * 64];
   __syncthreads();
-  const float* xb = x + (size_t)cd.seg_off * 64 + d;
-  float acc = 0.f;
-  int t = 0;
-  for (; t + 8 <= S; t += 8) {
-    float xv[8];
+  float tot = 0.f;
+  for (int c = 0; c < D; c += 64) {
+    const float* xb = x + (size_t)cd.seg_off * D + c + d;
+    float acc = 0.f;
+    int t = 0;
+    for (; t + 8 <= S; t += 8) {
+      float xv[8];
 #pragma unroll
-    for (int u = 0; u < 8; ++u) xv[u] = __ldg(xb + (size_t)(t + u) * 64);
+      for (int u = 0; u < 8; ++u) xv[u] = __ldg(xb + (size_t)(t + u) * D);
 #pragma unroll
-    for (int u = 0; u < 8; ++u) acc = fmaf(pn[t + u], xv[u], acc);
+      for (int u = 0; u < 8; ++u) acc = fmaf(pn[t + u], xv[u], acc);
+    }
+    for (; t < S; ++t) acc = fmaf(pn[t], __ldg(xb + (size_t)t * D), acc);
+    acc = (acc / sum) * __ldg(P.w3 + h * D + c + d);
+    tot = c ? tot + acc : acc;
   }
-  for (; t < S; ++t) acc = fmaf(pn[t], __ldg(xb + (size_t)t * 64), acc);
-  acc = (acc / sum) * __ldg(P.w3 + h * 64 + d);
-  red[threadIdx.x] = acc;
+  red[threadIdx.x] = tot;
   __syncthreads();
   for (int o = 32; o > 0; o >>= 1) { if (d < o) red[threadIdx.x] += red[threadIdx.x + o]; __syncthreads(); }
   if (d == 0) scores[blockIdx.x * n_heads + h] = red[h * 64] + __ldg(P.b3 + h);
@@ -156,7 +160,7 @@ __global__ void pool_final_kernel(const float* __restrict__ x, const float* __re
 
 // ---------------------------------------------------------------------------------------
 // The other pooling modules of the reference (user-trained checkpoints, SURVEY.md 8f.4), one CTA per clip, D threads
-// (thread d owns feature d; D = 64 after self-attention, 256 after the BiLSTM):
+// (thread d owns feature d; D = 64..256 after self-attention, 256 after the BiLSTM):
 //   mode 1 PoolAtt       (lib:1131-1154): att_t = a1 . x_t + a1b, softmax over the clip's steps, sum_t att_t x_t, Linear
 //   mode 2 PoolAvg       (lib:1185-1204): mean over the clip's steps, Linear
 //   mode 3 PoolMax       (lib:1206-1225): max over the clip's steps, Linear
@@ -188,7 +192,7 @@ __device__ __forceinline__ float block_max(float v, float* red) {
 }
 
 template <int D>
-__global__ void __launch_bounds__(D)
+__global__ void __launch_bounds__(D, 1)
 pool_simple_kernel(const float* __restrict__ x /*[n_seg][D]*/, const ClipDesc* __restrict__ clips, int mode,
                    PoolSimpleParams P, int n_heads, float* __restrict__ scores) {
   extern __shared__ __align__(16) float slog[];          // mode 1: softmax numerators of the clip's steps
@@ -513,11 +517,11 @@ constexpr int kRowSmem20 = (kRows * kXS + 64 * 20) * 4;
 void launch_fc20(cudaStream_t st, const float* feats, const float* WT, const float* b, float* out, int n_rows) {
   linear_rows_kernel<20, false><<<(n_rows + kRows - 1) / kRows, kRows, kRowSmem20, st>>>(feats, 768, WT, b, nullptr, nullptr, out, n_rows);
 }
-void launch_pool_final(cudaStream_t st, const float* x, const float* logits, const ClipDesc* clips, int n_clips,
+void launch_pool_final(cudaStream_t st, const float* x, int D, const float* logits, const ClipDesc* clips, int n_clips,
                        const PoolHeadParams& P, int n_heads, int max_seg, float* scores) {
   const int smem = n_heads * std::max(max_seg, 1) * 4;          // <= 5 x 1300 x 4 bytes at ms_max_segments = 1300
   if (smem > 40 * 1024) cudaFuncSetAttribute(pool_final_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  pool_final_kernel<<<n_clips, 64 * n_heads, smem, st>>>(x, logits, clips, P, n_heads, std::max(max_seg, 1), scores);
+  pool_final_kernel<<<n_clips, 64 * n_heads, smem, st>>>(x, logits, clips, P, n_heads, std::max(max_seg, 1), D, scores);
 }
 void launch_lstm(cudaStream_t st, const float* feats20, const ClipDesc* clips, int n_clips,
                  const LstmParams& P, float* td_out, float* partial, float pool_bias, float* scores) {
@@ -528,15 +532,20 @@ void launch_lstm(cudaStream_t st, const float* feats20, const ClipDesc* clips, i
   if (scores) lastbi_final_kernel<<<(n_clips + 127) / 128, 128, 0, st>>>(partial, clips, pool_bias, scores, n_clips);
 }
 
+template <int D>
+void pool_simple_instance(cudaStream_t st, const float* x, const ClipDesc* clips, int n_clips, int mode, const PoolSimpleParams& P,
+                          int n_heads, int smem, float* scores) {
+  if (smem > 48 * 1024) cudaFuncSetAttribute(pool_simple_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  pool_simple_kernel<D><<<n_clips, D, smem, st>>>(x, clips, mode, P, n_heads, scores);
+}
 void launch_pool_simple(cudaStream_t st, const float* x, int D, const ClipDesc* clips, int n_clips, int mode,
                         const PoolSimpleParams& P, int n_heads, int max_seg, float* scores) {
   const int smem = (mode == 1 ? max_seg : 0) * 4 + 16;
-  if (D == 64) {
-    if (smem > 48 * 1024) cudaFuncSetAttribute(pool_simple_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    pool_simple_kernel<64><<<n_clips, 64, smem, st>>>(x, clips, mode, P, n_heads, scores);
-  } else {
-    if (smem > 48 * 1024) cudaFuncSetAttribute(pool_simple_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    pool_simple_kernel<256><<<n_clips, 256, smem, st>>>(x, clips, mode, P, n_heads, scores);
+  switch (D) {
+    case 64: pool_simple_instance<64>(st, x, clips, n_clips, mode, P, n_heads, smem, scores); break;
+    case 128: pool_simple_instance<128>(st, x, clips, n_clips, mode, P, n_heads, smem, scores); break;
+    case 192: pool_simple_instance<192>(st, x, clips, n_clips, mode, P, n_heads, smem, scores); break;
+    case 256: pool_simple_instance<256>(st, x, clips, n_clips, mode, P, n_heads, smem, scores); break;
   }
 }
 

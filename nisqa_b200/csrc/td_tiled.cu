@@ -1,12 +1,14 @@
 // td_tiled.cu - time-dependency block + attention-pool logits of the adapt architecture as register-tiled fp32
-// GEMMs (round 2; replaces the one-thread-per-row kernels of td.cu, which ran at 6 % occupancy):
+// GEMMs (round 2; replaces the one-thread-per-row kernels of td.cu, which ran at 6 % occupancy), for self-attention
+// widths D = 64 NC, NC = 1..4 (one template instance each) and any feed-forward width F (a multiple of 64):
 //
-//   td_in_kernel   : Linear 384->64 + LayerNorm (reference nisqa/NISQA_lib.py:989-991) and, fused behind it, the
+//   td_in_kernel   : Linear in->D + LayerNorm (reference nisqa/NISQA_lib.py:989-991) and, fused behind it, the
 //                    QKV projection of encoder layer 0 (in_proj of nn.MultiheadAttention, lib:1032)
 //   td_sa_kernel   : one encoder layer for 64 queries of one clip (lib:1025-1040): softmax(q k^T) v over the clip's
-//                    own keys (flash-style, keys in blocks of 64, online max / sum), out_proj, +x, LN1, FFN(ReLU),
-//                    +, LN2 - and, fused behind it, either the NEXT layer's QKV projection or (last layer) the
-//                    PoolAttFF logits of all heads  w2_h . relu(W1_h x + b1_h) + b2_h  (lib:1173)
+//                    own keys (flash-style, keys in blocks of 64, online max / sum), out_proj, +x, LN1, FFN(ReLU)
+//                    streamed over F in chunks of 64, +, LN2 - and, fused behind it, either the NEXT layer's QKV
+//                    projection or (last layer) the PoolAttFF logits of all heads  w2_h . relu(W1_h x + b1_h) + b2_h
+//                    (lib:1173)
 //
 // Every matrix product is a 64 x 64 x 64 tile product on the FFMA pipe: 256 threads = 16 (ty) x 16 (tx), a thread
 // owns rows 4ty..4ty+3 and four columns, operands sit in shared memory, the A operand always row-major
@@ -14,10 +16,10 @@
 //   gemm_nn : B k-major [k][n]  (weights as packed by the engine, V), columns 4tx..4tx+3, LDS.128 along n
 //   gemm_nt : B row-major [n][k] (K of q k^T), columns tx, tx+16, tx+32, tx+48 - consecutive lanes read consecutive
 //             rows of pitch 68 floats = 4 banks apart: conflict-free LDS.128 along k
-// A row's 64 columns live in the 16 lanes of one half-warp, so softmax / LayerNorm reductions are four xor-shuffles,
-// and P (the softmax numerators) is written and re-read by the same half-warp: no block barrier inside a key block.
-// Weights stream through two shared-memory buffers with cp.async (16 KB chunks, L2 resident), the next chunk in
-// flight while the current one is multiplied.  fp32 throughout (parity: +-1e-4 on the scores).
+// A row's D columns live in the 16 lanes of one half-warp (4 NC per lane), so softmax / LayerNorm reductions are four
+// xor-shuffles, and P (the softmax numerators) is written and re-read by the same half-warp: no block barrier inside a
+// key block.  Operand tiles (16 KB, L2 resident) stream through a ring of shared-memory slots with cp.async, the next
+// ones in flight while the current one is multiplied.  fp32 throughout (parity: +-1e-4 on the scores).
 #include "common.cuh"
 #include "f32x2.cuh"
 
@@ -197,133 +199,197 @@ __device__ __forceinline__ float row_max(float v) {
   return v;
 }
 
-// nn.LayerNorm(64) (biased variance, eps 1e-5) of the rows held as v[i][0..3] = columns 4tx..4tx+3
-__device__ __forceinline__ void layernorm_rows(float (&v)[4][4], const float* __restrict__ gamma,
-                                               const float* __restrict__ beta, int tx) {
-  const float4 g = __ldg(reinterpret_cast<const float4*>(gamma) + tx), be = __ldg(reinterpret_cast<const float4*>(beta) + tx);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float mean = row_sum((v[i][0] + v[i][1]) + (v[i][2] + v[i][3])) * (1.0f / 64.0f);
-    const float d0 = v[i][0] - mean, d1 = v[i][1] - mean, d2 = v[i][2] - mean, d3 = v[i][3] - mean;
-    const float var = row_sum(fmaf(d0, d0, d1 * d1) + fmaf(d2, d2, d3 * d3)) * (1.0f / 64.0f);
-    const float rstd = 1.0f / sqrtf(var + 1e-5f);
-    v[i][0] = d0 * rstd * g.x + be.x; v[i][1] = d1 * rstd * g.y + be.y;
-    v[i][2] = d2 * rstd * g.z + be.z; v[i][3] = d3 * rstd * g.w + be.w;
-  }
-}
-
 __device__ __forceinline__ void store_rows_smem(float* X, const float (&v)[4][4], int ty, int tx) {
 #pragma unroll
   for (int i = 0; i < 4; ++i)
     *reinterpret_cast<float4*>(X + (4 * ty + i) * kLd + 4 * tx) = make_float4(v[i][0], v[i][1], v[i][2], v[i][3]);
 }
 
-// QKV projection of a 64-row tile X (shared, row-major) -> qkv[row0 + r][192]; Wbuf: two [64][64] buffers, the
-// first chunk (part 0) must already be in flight into Wbuf[b0] as the most recent cp.async group.
-__device__ __forceinline__ void qkv_tail(const float* X, float* Wbuf, const float* __restrict__ WT3,
-                                         const float* __restrict__ b3, float* __restrict__ qkv, long long row0,
-                                         int rows_valid, int tid, int ty, int tx, int b0 = 0) {
-#pragma unroll 1
-  for (int part_ = 0; part_ < 3; ++part_) {
-    const int part = part_;
-    if (part + 1 < 3) tile_load_async(Wbuf + ((part + 1 + b0) & 1) * 4096, 64, WT3 + (part + 1) * 4096, 64, 64, tid);
-    cp_commit();
-    cp_wait<1>();
-    __syncthreads();
-    float acc[4][4];
-    const float4 bb = __ldg(reinterpret_cast<const float4*>(b3 + part * 64) + tx);
+// Tiles stream through a ring of RS shared-memory slots of SLOT floats.  src(t, slot) issues the cp.async copies of the
+// stream's tile t (nothing past its end); acquire() returns the slot of the next tile once it has landed for every
+// thread.  One block barrier per tile: tile t + RS - 1 goes into the slot of tile t - 1 right after the barrier of tile
+// t, when every thread is done with tile t - 1.  The barrier also publishes every shared-memory store made before it.
+template <int RS, int SLOT, class Src>
+struct TileStream {
+  float* ring;
+  const Src& src;
+  int t = 0;
+  __device__ __forceinline__ TileStream(float* r, const Src& s) : ring(r), src(s) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) { acc[i][0] = bb.x; acc[i][1] = bb.y; acc[i][2] = bb.z; acc[i][3] = bb.w; }
-    gemm_nn(acc, X, Wbuf + ((part + b0) & 1) * 4096, 64, ty, tx);
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-      if (4 * ty + i < rows_valid)
-        *reinterpret_cast<float4*>(qkv + (row0 + 4 * ty + i) * 192 + part * 64 + 4 * tx) =
-            make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
-    __syncthreads();                        // buffer (part & 1) is refilled by the next iteration's prefetch
+    for (int i = 0; i < RS - 1; ++i) { src(i, ring + i * SLOT); cp_commit(); }
   }
+  __device__ __forceinline__ float* acquire() {
+    cp_wait<RS - 2>();
+    __syncthreads();
+    src(t + RS - 1, ring + ((t + RS - 1) % RS) * SLOT);
+    cp_commit();
+    return ring + (t++ % RS) * SLOT;
+  }
+};
+
+__device__ __forceinline__ void bias_rows(float (&acc)[4][4], const float* __restrict__ b, int tx) {
+  const float4 bb = __ldg(reinterpret_cast<const float4*>(b) + tx);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) { acc[i][0] = bb.x; acc[i][1] = bb.y; acc[i][2] = bb.z; acc[i][3] = bb.w; }
+}
+
+// nn.LayerNorm(64 NC) (biased variance, eps 1e-5) of the rows held as v[n][i][0..3] = columns 64 n + 4tx .. 64 n + 4tx + 3:
+// the chunks are summed in order before the xor-shuffles
+template <int NC>
+__device__ __forceinline__ void layernorm_rows(float (&v)[NC][4][4], const float* __restrict__ gamma,
+                                               const float* __restrict__ beta, int tx) {
+  constexpr float inv_d = 1.0f / (64.0f * NC);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    float s = (v[0][i][0] + v[0][i][1]) + (v[0][i][2] + v[0][i][3]);
+#pragma unroll
+    for (int n = 1; n < NC; ++n) s += (v[n][i][0] + v[n][i][1]) + (v[n][i][2] + v[n][i][3]);
+    const float mean = row_sum(s) * inv_d;
+    float q = 0.f;
+#pragma unroll
+    for (int n = 0; n < NC; ++n) {
+      const float d0 = v[n][i][0] - mean, d1 = v[n][i][1] - mean, d2 = v[n][i][2] - mean, d3 = v[n][i][3] - mean;
+      const float qn = fmaf(d0, d0, d1 * d1) + fmaf(d2, d2, d3 * d3);
+      q = n ? q + qn : qn;
+      v[n][i][0] = d0; v[n][i][1] = d1; v[n][i][2] = d2; v[n][i][3] = d3;
+    }
+    const float var = row_sum(q) * inv_d;
+    const float rstd = 1.0f / sqrtf(var + 1e-5f);
+#pragma unroll
+    for (int n = 0; n < NC; ++n) {
+      const float4 g = __ldg(reinterpret_cast<const float4*>(gamma + 64 * n) + tx);
+      const float4 be = __ldg(reinterpret_cast<const float4*>(beta + 64 * n) + tx);
+      v[n][i][0] = v[n][i][0] * rstd * g.x + be.x; v[n][i][1] = v[n][i][1] * rstd * g.y + be.y;
+      v[n][i][2] = v[n][i][2] * rstd * g.z + be.z; v[n][i][3] = v[n][i][3] * rstd * g.w + be.w;
+    }
+  }
+}
+
+// rows 4ty..4ty+3 of a [64][ld] row block, columns 4tx..4tx+3, rows >= rows_valid not written
+__device__ __forceinline__ void store_rows_global(float* __restrict__ dst, long long ld, const float (&v)[4][4], int rows_valid,
+                                                  int ty, int tx) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    if (4 * ty + i < rows_valid)
+      *reinterpret_cast<float4*>(dst + (4 * ty + i) * ld + 4 * tx) = make_float4(v[i][0], v[i][1], v[i][2], v[i][3]);
 }
 
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------
-constexpr int kInSmemFloats = 2 * kTileF + 2 * 4096 + kTileF;
+// The time-dependency kernels are templates on NC = d_model / 64 (1..4).  A thread holds 4 rows x 4 NC columns: chunk n
+// is columns 64 n + 4tx .. 64 n + 4tx + 3.  A transposed weight W^T [K][N] is packed in 64-column chunks: chunk n is the
+// k-major [K][64] block at n K 64, so tile (k chunk c, column chunk n) is the contiguous [64][64] block (n K / 64 + c) 4096.
+// Activations are row-major: x [n][D], qkv [n][3D] = q | k | v.  q is scaled by D^-1/2 after the projection (qscale) or,
+// where that is a power of two, by the packed weights (qscale = 1).
+template <int NC> struct TdShape {
+  static constexpr int kMinBlocks = NC == 1 ? 2 : 1;     // CTAs per SM the register budget is sized for (NC 2 spills at 128)
+  static constexpr int kRing = 4;                        // td_sa ring slots: 102 KB (NC 1), 119 KB (2), 136 KB (3), 153 KB (4)
+  static constexpr int kSaFloats = NC * kTileF + kTileF + kRing * kTileF;
+  static constexpr int kInSlot = kTileF + 4096;          // td_in ring slot: input tile | weight tile
+  static constexpr int kInFloats = NC * kTileF + 2 * kInSlot;
+};
 
-__global__ void __launch_bounds__(kNT, 2)
-td_in_kernel(const float* __restrict__ feats /*[n][64 nk]*/, const float* __restrict__ WT /*[64 nk][64]*/, int nk,
+// Linear(64 nk -> D) + LayerNorm (reference nisqa/NISQA_lib.py:989-991), the positional encoding, and the QKV projection
+// of encoder layer 0 (in_proj of nn.MultiheadAttention, lib:1032) for 64 rows.  Per column chunk n: acc[n] = b + sum_c
+// A_c W(c, n), A_c re-read for every n (one ring slot carries A_c and W(c, n)).
+template <int NC>
+__global__ void __launch_bounds__(kNT, TdShape<NC>::kMinBlocks)
+td_in_kernel(const float* __restrict__ feats /*[n][64 nk]*/, const float* __restrict__ WT /*[NC][64 nk][64]*/, int nk,
              const float* __restrict__ bias, const float* __restrict__ gamma, const float* __restrict__ beta,
-             const float* __restrict__ qkvT /*[3][64][64]*/, const float* __restrict__ qkvb /*[192]*/,
-             const float* __restrict__ pe /*[max_len][64] positional encoding or nullptr*/,
+             const float* __restrict__ qkvT /*[3 NC][D][64]*/, const float* __restrict__ qkvb /*[3D]*/, float qscale,
+             const float* __restrict__ pe /*[max_len][D] positional encoding or nullptr*/,
              const int* __restrict__ seg_clip, const ClipDesc* __restrict__ clips,
-             float* __restrict__ x0 /*[n][64]*/, float* __restrict__ qkv /*[n][192]*/, int n_rows) {
+             float* __restrict__ x0 /*[n][D]*/, float* __restrict__ qkv /*[n][3D]*/, int n_rows) {
+  constexpr int D = 64 * NC, SLOT = TdShape<NC>::kInSlot;
   extern __shared__ __align__(16) float sm[];
-  float* As = sm;                       // [2][64][68]
-  float* Ws = sm + 2 * kTileF;          // [2][64][64]
-  float* Xs = Ws + 2 * 4096;            // [64][68]
+  float* Xs = sm;                               // [NC][64][68] LayerNorm output, input of the QKV projection
+  float* ring = sm + NC * kTileF;               // 2 x (A tile [64][68] | weight tile [64][64])
   const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
   const long long row0 = (long long)blockIdx.x * kT;
   const int rows_valid = (int)min((long long)kT, (long long)n_rows - row0);
-  const int ld = 64 * nk;                 // 384 CNN features, or the 192 / 128 fused features of the double-ended model
-  const float* src = feats + row0 * ld;
-
-  tile_load_async(As, kLd, src, ld, rows_valid, tid);
-  tile_load_async(Ws, 64, WT, 64, 64, tid);
-  cp_commit();
-  float acc[4][4];
-  {
-    const float4 bb = __ldg(reinterpret_cast<const float4*>(bias) + tx);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { acc[i][0] = bb.x; acc[i][1] = bb.y; acc[i][2] = bb.z; acc[i][3] = bb.w; }
-  }
-#pragma unroll 1
-  for (int c = 0; c < nk; ++c) {
-    if (c + 1 < nk) {
-      tile_load_async(As + ((c + 1) & 1) * kTileF, kLd, src + (c + 1) * 64, ld, rows_valid, tid);
-      tile_load_async(Ws + ((c + 1) & 1) * 4096, 64, WT + (size_t)(c + 1) * 4096, 64, 64, tid);
-    } else {
-      tile_load_async(Ws + ((c + 1) & 1) * 4096, 64, qkvT, 64, 64, tid);       // first QKV chunk rides behind the last k chunk
+  const int ld = 64 * nk;                       // 384 CNN features, cnn_fc_out_h, the fused features, or the first stack's D
+  const float* rows = feats + row0 * ld;
+  const int t_lin = NC * nk;
+  auto src = [&](int t, float* dst) {
+    if (t < t_lin) {
+      const int n = t / nk, c = t - n * nk;
+      tile_load_async(dst, kLd, rows + c * 64, ld, rows_valid, tid);
+      tile_load_async(dst + kTileF, 64, WT + (size_t)t * 4096, 64, 64, tid);        // tile (c, n) = (n nk + c) 4096
+    } else if (t < t_lin + 3 * NC * NC) {
+      tile_load_async(dst + kTileF, 64, qkvT + (size_t)(t - t_lin) * 4096, 64, 64, tid);
     }
-    cp_commit();
-    cp_wait<1>();
-    __syncthreads();
-    gemm_nn(acc, As + (c & 1) * kTileF, Ws + (c & 1) * 4096, 64, ty, tx);
-    __syncthreads();
+  };
+  TileStream<2, SLOT, decltype(src)> st(ring, src);
+  float acc[NC][4][4];
+#pragma unroll
+  for (int n = 0; n < NC; ++n) {
+    bias_rows(acc[n], bias + 64 * n, tx);
+#pragma unroll 1
+    for (int c = 0; c < nk; ++c) {
+      const float* s = st.acquire();
+      gemm_nn(acc[n], s, s + kTileF, 64, ty, tx);
+    }
   }
-  layernorm_rows(acc, gamma, beta, tx);
+  layernorm_rows<NC>(acc, gamma, beta, tx);
   if (pe != nullptr) {
     // PositionalEncoding (lib:1042-1062): x[t] += pe[t], t = position of the segment inside its clip
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const long long row = row0 + min(4 * ty + i, rows_valid - 1);
       const int t = (int)(row - clips[__ldg(seg_clip + row)].seg_off);
-      const float4 pv = __ldg(reinterpret_cast<const float4*>(pe + (size_t)t * 64) + tx);
-      acc[i][0] += pv.x; acc[i][1] += pv.y; acc[i][2] += pv.z; acc[i][3] += pv.w;
+#pragma unroll
+      for (int n = 0; n < NC; ++n) {
+        const float4 pv = __ldg(reinterpret_cast<const float4*>(pe + (size_t)t * D + 64 * n) + tx);
+        acc[n][i][0] += pv.x; acc[n][i][1] += pv.y; acc[n][i][2] += pv.z; acc[n][i][3] += pv.w;
+      }
     }
   }
-  store_rows_smem(Xs, acc, ty, tx);
 #pragma unroll
-  for (int i = 0; i < 4; ++i)
-    if (4 * ty + i < rows_valid)
-      *reinterpret_cast<float4*>(x0 + (row0 + 4 * ty + i) * 64 + 4 * tx) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
-  // QKV of layer 0: its first weight chunk is in flight into Ws[nk & 1]; qkv_tail syncs before reading Xs
-  qkv_tail(Xs, Ws, qkvT, qkvb, qkv, row0, rows_valid, tid, ty, tx, nk & 1);
+  for (int n = 0; n < NC; ++n) {
+    store_rows_smem(Xs + n * kTileF, acc[n], ty, tx);
+    store_rows_global(x0 + row0 * D + 64 * n, D, acc[n], rows_valid, ty, tx);
+  }
+  // QKV of layer 0: output chunk p = b + sum_c X_c W(c, p); the stream's next acquire publishes Xs
+#pragma unroll 1
+  for (int p = 0; p < 3 * NC; ++p) {
+    float q[4][4];
+    bias_rows(q, qkvb + 64 * p, tx);
+#pragma unroll 1
+    for (int c = 0; c < NC; ++c) {
+      const float* s = st.acquire();
+      gemm_nn(q, Xs + c * kTileF, s + kTileF, 64, ty, tx);
+    }
+    if (p < NC && qscale != 1.f) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) q[i][j] *= qscale;
+    }
+    store_rows_global(qkv + row0 * (3 * D) + 64 * p, 3 * D, q, rows_valid, ty, tx);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// shared memory: Qs | Ps | Kb[2] | Vb[2]  (Kb/Vb double as weight buffers after the attention loop)
-constexpr int kSaSmemFloats = 2 * kTileF + 2 * kTileF + 2 * 4096;
-
-__global__ void __launch_bounds__(kNT, 2)
+// One encoder layer for 64 queries of one clip (lib:1025-1040): softmax(q k^T) v over the clip's own keys (flash-style,
+// keys in blocks of 64, online max / sum), out_proj, +x, LN1, FFN(ReLU) streamed over the hidden width F in chunks of 64
+// (out += relu(X W1[:, f] + b1_f) W2[f, :]: the hidden layer is never held whole), +, LN2 - and, fused behind it, either
+// the NEXT layer's QKV projection or (last layer) the PoolAttFF logits of all heads  w2_h . relu(W1_h x + b1_h) + b2_h
+// (lib:1173).  Every operand tile after Q - K and V chunks of each key block, then the weight tiles - comes through
+// one TileStream, so the loads of the next phase are in flight while the current one computes.
+// shared memory: Qs [NC][64][68] | Ps [64][68] | ring [kRing][64][68]
+template <int NC>
+__global__ void __launch_bounds__(kNT, TdShape<NC>::kMinBlocks)
 td_sa_kernel(const float* __restrict__ x_in, const float* __restrict__ qkv, const ClipDesc* __restrict__ clips,
-             int n_clips, const int* __restrict__ qtile_prefix /*64-row tiles*/, SaLayerParams P,
+             int n_clips, const int* __restrict__ qtile_prefix /*64-row tiles*/, SaLayerParams P, int F,
              float* __restrict__ x_out,
-             const float* __restrict__ next_qkvT, const float* __restrict__ next_qkvb, float* __restrict__ qkv_next,
+             const float* __restrict__ next_qkvT, const float* __restrict__ next_qkvb, float qscale, float* __restrict__ qkv_next,
              PoolHeadParams H, int n_heads, float* __restrict__ logits) {
+  constexpr int D = 64 * NC;
   extern __shared__ __align__(16) float sm[];
-  float* Qs = sm;                          // [64][68]  queries, later the row tile fed to the linears
-  float* Ps = sm + kTileF;                 // [64][68]  softmax numerators, later scratch row tile
-  float* Kb = Ps + kTileF;                 // [2][64][68]
-  float* Vb = Kb + 2 * kTileF;             // [2][64][64]
+  float* Qs = sm;                          // queries -> attention output -> LN1 output (FFN input) -> layer output
+  float* Ps = sm + NC * kTileF;            // softmax numerators -> FFN hidden chunk
+  float* ring = Ps + kTileF;
   const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
   const int c = upper_slot(qtile_prefix, n_clips, blockIdx.x);
   const ClipDesc cd = clips[c];
@@ -331,34 +397,52 @@ td_sa_kernel(const float* __restrict__ x_in, const float* __restrict__ qkv, cons
   const int q0 = (blockIdx.x - __ldg(qtile_prefix + c)) * kT;
   const int rows_valid = min(kT, S - q0);
   const long long row0 = (long long)cd.seg_off + q0;
-  const float* kv_base = qkv + (long long)cd.seg_off * 192;
+  const float* kv_base = qkv + (long long)cd.seg_off * (3 * D);
+  const int n_kb = (S + kT - 1) / kT, FC = F / 64;
+  const bool last = next_qkvT == nullptr;
+  // the layer's tile stream: per key block K chunks 0..NC-1 (row-major [key][d], pitch 68) then V chunks 0..NC-1
+  // (k-major, pitch 64); out_proj tiles (c, n); per hidden chunk f the W1 tiles (c, f), then the W2 tiles (f, n); then
+  // the next layer's QKV tiles (c, p) or the PoolAttFF W1 tiles (c) of every (head, half) of W1T [head][D][128]
+  const int t_att = 2 * NC * n_kb, t_out = t_att + NC * NC, t_ffn = t_out + 2 * NC * FC;
+  auto src = [&](int t, float* dst) {
+    if (t < t_att) {
+      const int kb = t / (2 * NC), r = t - kb * 2 * NC;
+      const float* kv = kv_base + (long long)kb * kT * (3 * D) + D;
+      const int nv = min(kT, S - kb * kT);
+      if (r < NC) tile_load_async(dst, kLd, kv + 64 * r, 3 * D, nv, tid);
+      else tile_load_async(dst, 64, kv + D + 64 * (r - NC), 3 * D, nv, tid);
+    } else if (t < t_out) {
+      tile_load_async(dst, 64, P.WoT + (size_t)(t - t_att) * 4096, 64, 64, tid);                   // WoT [NC][D][64]
+    } else if (t < t_ffn) {
+      const int u = t - t_out, f = u / (2 * NC), r = u - f * 2 * NC;
+      if (r < NC) tile_load_async(dst, 64, P.W1T + ((size_t)f * NC + r) * 4096, 64, 64, tid);      // W1T [F/64][D][64]
+      else tile_load_async(dst, 64, P.W2T + ((size_t)(r - NC) * FC + f) * 4096, 64, 64, tid);     // W2T [NC][F][64]
+    } else if (!last) {
+      const int u = t - t_ffn;
+      if (u < 3 * NC * NC) tile_load_async(dst, 64, next_qkvT + (size_t)u * 4096, 64, 64, tid);   // [3 NC][D][64]
+    } else {
+      const int u = t - t_ffn, q = u / NC, k = u - q * NC;                                         // q = 2 head + half
+      if (q < 2 * n_heads) tile_load_async(dst, 64, H.W1T + ((size_t)(q >> 1) * D + 64 * k) * 128 + (q & 1) * 64, 128, 64, tid);
+    }
+  };
 
-  // ---- attention: Q tile, then key blocks of 64 (K row-major [key][d], V k-major [key][d])
-  tile_load_async(Qs, kLd, qkv + row0 * 192, 192, rows_valid, tid);
-  tile_load_async(Kb, kLd, kv_base + 64, 192, min(kT, S), tid);
-  tile_load_async(Vb, 64, kv_base + 128, 192, min(kT, S), tid);
-  cp_commit();
-  float o[4][4];
-  zero_acc(o);
+  // ---- attention
+#pragma unroll
+  for (int n = 0; n < NC; ++n) tile_load_async(Qs + n * kTileF, kLd, qkv + row0 * (3 * D) + 64 * n, 3 * D, rows_valid, tid);
+  TileStream<TdShape<NC>::kRing, kTileF, decltype(src)> st(ring, src);      // (its first group carries Q)
+  float o[NC][4][4];
+#pragma unroll
+  for (int n = 0; n < NC; ++n) zero_acc(o[n]);
   float m[4], l[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) { m[i] = -INFINITY; l[i] = 0.f; }
-  const int n_kb = (S + kT - 1) / kT;
 #pragma unroll 1
   for (int kb = 0; kb < n_kb; ++kb) {
-    const int j0 = kb * kT;
-    if (kb + 1 < n_kb) {
-      const int nv = min(kT, S - (j0 + kT));
-      tile_load_async(Kb + ((kb + 1) & 1) * kTileF, kLd, kv_base + (long long)(j0 + kT) * 192 + 64, 192, nv, tid);
-      tile_load_async(Vb + ((kb + 1) & 1) * 4096, 64, kv_base + (long long)(j0 + kT) * 192 + 128, 192, nv, tid);
-    }
-    cp_commit();
-    cp_wait<1>();
-    __syncthreads();                               // K/V block kb (and Q) landed for every thread
     float s[4][4];
     zero_acc(s);
-    gemm_nt(s, Qs, Kb + (kb & 1) * kTileF, ty, tx);           // s[i][j]: query 4ty+i, key j0 + tx + 16j
-    const int nk = S - j0;                                     // keys >= nk of this block do not exist
+#pragma unroll 1
+    for (int k = 0; k < NC; ++k) gemm_nt(s, Qs + k * kTileF, st.acquire(), ty, tx);   // s[i][j]: query 4ty+i, key 64 kb + tx + 16j
+    const int nk = S - kb * kT;                                                      // keys >= nk of this block do not exist
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       float bm = -INFINITY;
@@ -376,126 +460,104 @@ td_sa_kernel(const float* __restrict__ x_in, const float* __restrict__ qkv, cons
       }
       l[i] = l[i] * sc + row_sum(ps);
       m[i] = mn;
-      o[i][0] *= sc; o[i][1] *= sc; o[i][2] *= sc; o[i][3] *= sc;
+#pragma unroll
+      for (int n = 0; n < NC; ++n) { o[n][i][0] *= sc; o[n][i][1] *= sc; o[n][i][2] *= sc; o[n][i][3] *= sc; }
     }
     __syncwarp();                                  // P rows 4ty..4ty+3 are written and read by this half-warp only
-    gemm_nn(o, Ps, Vb + (kb & 1) * 4096, 64, ty, tx);         // o[i][j]: query 4ty+i, d = 4tx + j
-    __syncthreads();                               // block kb consumed: its buffers are the prefetch target of kb + 2
+#pragma unroll
+    for (int n = 0; n < NC; ++n) gemm_nn(o[n], Ps, st.acquire(), 64, ty, tx);   // o[n][i][j]: query 4ty+i, d = 64 n + 4tx + j
   }
-  // ---- out_proj + residual + LN1, FFN + residual + LN2; weights stream through Kb (as [64][64] chunks)
-  float* Wb = Kb;                                  // two [64][64] weight buffers inside the K region (2 x 4096 <= 2 x kTileF)
-  tile_load_async(Wb, 64, P.WoT, 64, 64, tid);
-  cp_commit();
+  // the attention output replaces Q: every thread has read Q for the last time before the barrier of the last V chunk
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const float inv = 1.0f / l[i];
-    o[i][0] *= inv; o[i][1] *= inv; o[i][2] *= inv; o[i][3] *= inv;
-  }
-  store_rows_smem(Qs, o, ty, tx);                  // attention output tile (Q is no longer needed)
-  tile_load_async(Wb + 4096, 64, P.W1T, 64, 64, tid);
-  cp_commit();
-  cp_wait<1>();
-  __syncthreads();
-  float v[4][4];
-  {
-    const float4 bb = __ldg(reinterpret_cast<const float4*>(P.bo) + tx);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) { v[i][0] = bb.x; v[i][1] = bb.y; v[i][2] = bb.z; v[i][3] = bb.w; }
+    for (int n = 0; n < NC; ++n) { o[n][i][0] *= inv; o[n][i][1] *= inv; o[n][i][2] *= inv; o[n][i][3] *= inv; }
   }
-  gemm_nn(v, Qs, Wb, 64, ty, tx);
+#pragma unroll
+  for (int n = 0; n < NC; ++n) store_rows_smem(Qs + n * kTileF, o[n], ty, tx);
+
+  // ---- out_proj + residual + LN1
+  float v[NC][4][4];
+#pragma unroll
+  for (int n = 0; n < NC; ++n) {
+    bias_rows(v[n], P.bo + 64 * n, tx);
+#pragma unroll 1
+    for (int k = 0; k < NC; ++k) gemm_nn(v[n], Qs + k * kTileF, st.acquire(), 64, ty, tx);
+  }
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int r = min(4 * ty + i, rows_valid - 1);                             // rows beyond the clip: any valid row
-    const float4 xr = __ldg(reinterpret_cast<const float4*>(x_in + (row0 + r) * 64) + tx);
-    v[i][0] += xr.x; v[i][1] += xr.y; v[i][2] += xr.z; v[i][3] += xr.w;
+#pragma unroll
+    for (int n = 0; n < NC; ++n) {
+      const float4 xr = __ldg(reinterpret_cast<const float4*>(x_in + (row0 + r) * D + 64 * n) + tx);
+      v[n][i][0] += xr.x; v[n][i][1] += xr.y; v[n][i][2] += xr.z; v[n][i][3] += xr.w;
+    }
   }
-  layernorm_rows(v, P.ln1_g, P.ln1_b, tx);
-  store_rows_smem(Ps, v, ty, tx);                  // LN1 output: FFN input (and residual, kept in v)
-  __syncthreads();                                 // Wb[0] (Wo) consumed, Ps complete
-  tile_load_async(Wb, 64, P.W2T, 64, 64, tid);
-  cp_commit();
-  cp_wait<1>();                                    // W1 landed
-  __syncthreads();
-  float h[4][4];
-  {
-    const float4 bb = __ldg(reinterpret_cast<const float4*>(P.b1) + tx);
+  layernorm_rows<NC>(v, P.ln1_g, P.ln1_b, tx);
+  __syncthreads();                                 // every thread is done with the attention output
 #pragma unroll
-    for (int i = 0; i < 4; ++i) { h[i][0] = bb.x; h[i][1] = bb.y; h[i][2] = bb.z; h[i][3] = bb.w; }
+  for (int n = 0; n < NC; ++n) store_rows_smem(Qs + n * kTileF, v[n], ty, tx);   // FFN input and residual
+
+  // ---- FFN over hidden chunks of 64
+#pragma unroll
+  for (int n = 0; n < NC; ++n) bias_rows(v[n], P.b2 + 64 * n, tx);           // v now accumulates the FFN output
+#pragma unroll 1
+  for (int f = 0; f < FC; ++f) {
+    float h[4][4];
+    bias_rows(h, P.b1 + 64 * f, tx);
+#pragma unroll 1
+    for (int k = 0; k < NC; ++k) gemm_nn(h, Qs + k * kTileF, st.acquire(), 64, ty, tx);
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) h[i][j] = fmaxf(h[i][j], 0.f);
+    store_rows_smem(Ps, h, ty, tx);                // (every thread is done with the previous chunk: barrier of W1 tile k = 0)
+#pragma unroll
+    for (int n = 0; n < NC; ++n) gemm_nn(v[n], Ps, st.acquire(), 64, ty, tx);
   }
-  gemm_nn(h, Ps, Wb + 4096, 64, ty, tx);
 #pragma unroll
-  for (int i = 0; i < 4; ++i)
+  for (int n = 0; n < NC; ++n)
 #pragma unroll
-    for (int j = 0; j < 4; ++j) h[i][j] = fmaxf(h[i][j], 0.f);
-  store_rows_smem(Qs, h, ty, tx);                  // FFN hidden tile
-  __syncthreads();                                 // Wb[1] (W1) consumed, Qs complete
-  const bool last = next_qkvT == nullptr;
-  // first chunk of the fused tail rides behind W2
-  if (!last) tile_load_async(Wb + 4096, 64, next_qkvT, 64, 64, tid);
-  else if (n_heads > 0) tile_load_async(Wb + 4096, 64, H.W1T, 128, 64, tid);      // (n_heads == 0: another pooling module follows)
-  cp_commit();
-  cp_wait<1>();                                    // W2 landed
-  __syncthreads();
-  {
-    const float4 bb = __ldg(reinterpret_cast<const float4*>(P.b2) + tx);
+    for (int i = 0; i < 4; ++i) {                  // + residual: this thread's own elements of the FFN input
+      const float4 xr = *reinterpret_cast<const float4*>(Qs + n * kTileF + (4 * ty + i) * kLd + 4 * tx);
+      v[n][i][0] = xr.x + v[n][i][0]; v[n][i][1] = xr.y + v[n][i][1];
+      v[n][i][2] = xr.z + v[n][i][2]; v[n][i][3] = xr.w + v[n][i][3];
+    }
+  layernorm_rows<NC>(v, P.ln2_g, P.ln2_b, tx);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) { h[i][0] = bb.x; h[i][1] = bb.y; h[i][2] = bb.z; h[i][3] = bb.w; }
+  for (int n = 0; n < NC; ++n) {
+    store_rows_global(x_out + row0 * D + 64 * n, D, v[n], rows_valid, ty, tx);
+    store_rows_smem(Qs + n * kTileF, v[n], ty, tx);   // input of the fused tail (the FFN input was last read before the W2 barriers)
   }
-  gemm_nn(h, Qs, Wb, 64, ty, tx);
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) v[i][j] += h[i][j];
-  layernorm_rows(v, P.ln2_g, P.ln2_b, tx);
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-    if (4 * ty + i < rows_valid)
-      *reinterpret_cast<float4*>(x_out + (row0 + 4 * ty + i) * 64 + 4 * tx) = make_float4(v[i][0], v[i][1], v[i][2], v[i][3]);
-  store_rows_smem(Ps, v, ty, tx);                  // layer output tile: input of the fused tail
-  __syncthreads();                                 // Wb[0] (W2) consumed, Ps complete
 
   if (!last) {
-    // ---- next layer's QKV projection (its part 0 is in flight into Wb[1])
+    // ---- next layer's QKV projection
 #pragma unroll 1
-    for (int part = 0; part < 3; ++part) {
-      const int cur = (part + 1) & 1;
-      if (part + 1 < 3) tile_load_async(Wb + (cur ^ 1) * 4096, 64, next_qkvT + (part + 1) * 4096, 64, 64, tid);
-      cp_commit();
-      cp_wait<1>();
-      __syncthreads();
+    for (int p = 0; p < 3 * NC; ++p) {
       float acc[4][4];
-      const float4 bb = __ldg(reinterpret_cast<const float4*>(next_qkvb + part * 64) + tx);
+      bias_rows(acc, next_qkvb + 64 * p, tx);
+#pragma unroll 1
+      for (int k = 0; k < NC; ++k) gemm_nn(acc, Qs + k * kTileF, st.acquire(), 64, ty, tx);
+      if (p < NC && qscale != 1.f) {
 #pragma unroll
-      for (int i = 0; i < 4; ++i) { acc[i][0] = bb.x; acc[i][1] = bb.y; acc[i][2] = bb.z; acc[i][3] = bb.w; }
-      gemm_nn(acc, Ps, Wb + cur * 4096, 64, ty, tx);
+        for (int i = 0; i < 4; ++i)
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
-        if (4 * ty + i < rows_valid)
-          *reinterpret_cast<float4*>(qkv_next + (row0 + 4 * ty + i) * 192 + part * 64 + 4 * tx) =
-              make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
-      __syncthreads();
+          for (int j = 0; j < 4; ++j) acc[i][j] *= qscale;
+      }
+      store_rows_global(qkv_next + row0 * (3 * D) + 64 * p, 3 * D, acc, rows_valid, ty, tx);
     }
   } else {
-    // ---- PoolAttFF logits of every head: chunk q = (head, half) of W1T [head][64 k][128 j]; chunk 0 is in flight
-    const int n_chunks = 2 * n_heads;
+    // ---- PoolAttFF logits of every head (n_heads == 0: another pooling module follows)
     float part_logit[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll 1
-    for (int q = 0; q < n_chunks; ++q) {
-      const int cur = (q + 1) & 1;
-      if (q + 1 < n_chunks) {
-        const int hn = (q + 1) >> 1, halfn = (q + 1) & 1;
-        tile_load_async(Wb + (cur ^ 1) * 4096, 64, H.W1T + (size_t)hn * 64 * 128 + halfn * 64, 128, 64, tid);
-      }
-      cp_commit();
-      cp_wait<1>();
-      __syncthreads();
+    for (int q = 0; q < 2 * n_heads; ++q) {
       const int hd = q >> 1, half = q & 1;
       float acc[4][4];
-      const float4 bb = __ldg(reinterpret_cast<const float4*>(H.b1 + hd * 128 + half * 64) + tx);
+      bias_rows(acc, H.b1 + hd * 128 + half * 64, tx);
       const float4 w2 = __ldg(reinterpret_cast<const float4*>(H.w2 + hd * 128 + half * 64) + tx);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) { acc[i][0] = bb.x; acc[i][1] = bb.y; acc[i][2] = bb.z; acc[i][3] = bb.w; }
-      gemm_nn(acc, Ps, Wb + cur * 4096, 64, ty, tx);
+#pragma unroll 1
+      for (int k = 0; k < NC; ++k) gemm_nn(acc, Qs + k * kTileF, st.acquire(), 64, ty, tx);
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         float t = part_logit[i];
@@ -512,11 +574,10 @@ td_sa_kernel(const float* __restrict__ x_in, const float* __restrict__ qkv, cons
           part_logit[i] = 0.f;
         }
       }
-      __syncthreads();
     }
   }
+  cp_wait<0>();                                    // (only empty groups can be pending here)
 }
-
 
 // ---------------------------------------------------------------------------------------------------------------
 // Double-ended model (NISQA_DE, reference lib:272-424): time alignment of the reference clip's features to the degraded
@@ -858,13 +919,26 @@ linear_tile_kernel(const float* __restrict__ X, int ldx, const float* __restrict
 }
 
 // ------------------------------------------------------------------ host launchers
-void launch_td_in(cudaStream_t st, const float* feats, const float* WT, int nk, const float* b, const float* g, const float* be,
-                  const float* qkvT, const float* qkvb, const float* pe, const int* seg_clip, const ClipDesc* clips,
-                  float* x0, float* qkv, int n_rows) {
+// d_model = 64 nc, nc in 1..4
+template <int NC>
+void td_in_instance(cudaStream_t st, const float* feats, const float* WT, int nk, const float* b, const float* g, const float* be,
+                    const float* qkvT, const float* qkvb, float qscale, const float* pe, const int* seg_clip, const ClipDesc* clips,
+                    float* x0, float* qkv, int n_rows) {
   static unsigned long long cfg = 0;
-  const int smem = kInSmemFloats * 4;
-  if (first_launch_on_device(cfg)) cudaFuncSetAttribute(td_in_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  td_in_kernel<<<(n_rows + kT - 1) / kT, kNT, smem, st>>>(feats, WT, nk, b, g, be, qkvT, qkvb, pe, seg_clip, clips, x0, qkv, n_rows);
+  const int smem = TdShape<NC>::kInFloats * 4;
+  if (first_launch_on_device(cfg)) cudaFuncSetAttribute(td_in_kernel<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  td_in_kernel<NC><<<(n_rows + kT - 1) / kT, kNT, smem, st>>>(feats, WT, nk, b, g, be, qkvT, qkvb, qscale, pe, seg_clip, clips,
+                                                              x0, qkv, n_rows);
+}
+void launch_td_in(cudaStream_t st, int nc, const float* feats, const float* WT, int nk, const float* b, const float* g,
+                  const float* be, const float* qkvT, const float* qkvb, float qscale, const float* pe, const int* seg_clip,
+                  const ClipDesc* clips, float* x0, float* qkv, int n_rows) {
+  switch (nc) {
+    case 1: td_in_instance<1>(st, feats, WT, nk, b, g, be, qkvT, qkvb, qscale, pe, seg_clip, clips, x0, qkv, n_rows); break;
+    case 2: td_in_instance<2>(st, feats, WT, nk, b, g, be, qkvT, qkvb, qscale, pe, seg_clip, clips, x0, qkv, n_rows); break;
+    case 3: td_in_instance<3>(st, feats, WT, nk, b, g, be, qkvT, qkvb, qscale, pe, seg_clip, clips, x0, qkv, n_rows); break;
+    case 4: td_in_instance<4>(st, feats, WT, nk, b, g, be, qkvT, qkvb, qscale, pe, seg_clip, clips, x0, qkv, n_rows); break;
+  }
 }
 
 void launch_de_align(cudaStream_t st, const float* x_td, const ClipDesc* clips, int n_clips, const int* qtile64_prefix,
@@ -894,15 +968,27 @@ void launch_de_finalize(cudaStream_t st, const ClipDesc* clips, int n_clips, int
   de_finalize_kernel<<<(n_clips + 127) / 128, 128, 0, st>>>(clips, n_clips, n_out, scores);
 }
 
-void launch_td_sa(cudaStream_t st, const float* x_in, const float* qkv, const ClipDesc* clips, int n_clips,
-                  const int* qtile64_prefix, int n_qtiles, const SaLayerParams& P, float* x_out,
-                  const float* next_qkvT, const float* next_qkvb, float* qkv_next,
-                  const PoolHeadParams& H, int n_heads, float* logits) {
+template <int NC>
+void td_sa_instance(cudaStream_t st, const float* x_in, const float* qkv, const ClipDesc* clips, int n_clips,
+                    const int* qtile64_prefix, int n_qtiles, const SaLayerParams& P, int F, float* x_out,
+                    const float* next_qkvT, const float* next_qkvb, float qscale, float* qkv_next,
+                    const PoolHeadParams& H, int n_heads, float* logits) {
   static unsigned long long cfg = 0;
-  const int smem = kSaSmemFloats * 4;
-  if (first_launch_on_device(cfg)) cudaFuncSetAttribute(td_sa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  td_sa_kernel<<<n_qtiles, kNT, smem, st>>>(x_in, qkv, clips, n_clips, qtile64_prefix, P, x_out,
-                                            next_qkvT, next_qkvb, qkv_next, H, n_heads, logits);
+  const int smem = TdShape<NC>::kSaFloats * 4;
+  if (first_launch_on_device(cfg)) cudaFuncSetAttribute(td_sa_kernel<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  td_sa_kernel<NC><<<n_qtiles, kNT, smem, st>>>(x_in, qkv, clips, n_clips, qtile64_prefix, P, F, x_out,
+                                                next_qkvT, next_qkvb, qscale, qkv_next, H, n_heads, logits);
+}
+void launch_td_sa(cudaStream_t st, int nc, const float* x_in, const float* qkv, const ClipDesc* clips, int n_clips,
+                  const int* qtile64_prefix, int n_qtiles, const SaLayerParams& P, int F, float* x_out,
+                  const float* next_qkvT, const float* next_qkvb, float qscale, float* qkv_next,
+                  const PoolHeadParams& H, int n_heads, float* logits) {
+  switch (nc) {
+    case 1: td_sa_instance<1>(st, x_in, qkv, clips, n_clips, qtile64_prefix, n_qtiles, P, F, x_out, next_qkvT, next_qkvb, qscale, qkv_next, H, n_heads, logits); break;
+    case 2: td_sa_instance<2>(st, x_in, qkv, clips, n_clips, qtile64_prefix, n_qtiles, P, F, x_out, next_qkvT, next_qkvb, qscale, qkv_next, H, n_heads, logits); break;
+    case 3: td_sa_instance<3>(st, x_in, qkv, clips, n_clips, qtile64_prefix, n_qtiles, P, F, x_out, next_qkvT, next_qkvb, qscale, qkv_next, H, n_heads, logits); break;
+    case 4: td_sa_instance<4>(st, x_in, qkv, clips, n_clips, qtile64_prefix, n_qtiles, P, F, x_out, next_qkvT, next_qkvb, qscale, qkv_next, H, n_heads, logits); break;
+  }
 }
 
 }  // namespace nisqa

@@ -13,7 +13,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libnisqa_b200.so")
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 MAX_IN_FLIGHT = 6          # staging slots of the engine (nisqa_submit_pcm)
 ARCH_ADAPT_SA_ATTFF, ARCH_STD_LSTM_LASTBI = 0, 1
 FMT_S16, FMT_F32 = 0, 1
@@ -48,7 +48,25 @@ class NisqaConfig(C.Structure):
                 ("max_chunk_segments", C.c_int32), ("pool", C.c_int32), ("pos_enc", C.c_int32),
                 ("double_ended", C.c_int32), ("de_align", C.c_int32), ("de_align_apply", C.c_int32),
                 ("de_fuse", C.c_int32), ("td2_layers", C.c_int32), ("td2_pos_enc", C.c_int32),
-                ("cnn_kind", C.c_int32), ("cnn_fc", C.c_int32), ("de_fuse_dim", C.c_int32)]
+                ("cnn_kind", C.c_int32), ("cnn_fc", C.c_int32), ("de_fuse_dim", C.c_int32),
+                ("sa_d_model", C.c_int32), ("sa_ff", C.c_int32), ("td2_d_model", C.c_int32), ("td2_ff", C.c_int32)]
+
+SA_D_MODELS = (64, 128, 192, 256)     # self-attention widths the kernels are instantiated for (one head)
+SA_FF_MAX = 4096                      # feed-forward width: a multiple of 64 up to this
+
+
+def _sa_widths(args, prefix, de=False):
+    """(d_model, feed-forward width) of a self-attention stack's args ('td_sa' / 'td_2_sa'); refuses what the kernels do
+    not implement, naming the value."""
+    d, h, nhead = args.get(prefix + "_d_model"), args.get(prefix + "_h"), args.get(prefix + "_nhead")
+    if nhead != 1:
+        raise NotImplementedError("%s_nhead=%r: the engine runs one-head self-attention" % (prefix, nhead))
+    if d not in SA_D_MODELS or (de and d != 64):
+        raise NotImplementedError("%s_d_model=%r: the engine runs d_model %s%s" % (
+            prefix, d, "64" if de else "64, 128, 192 or 256", " in NISQA_DE" if de else ""))
+    if h is None or int(h) != h or h <= 0 or h % 64 != 0 or h > SA_FF_MAX:
+        raise NotImplementedError("%s_h=%r: the engine needs a positive multiple of 64 up to %d" % (prefix, h, SA_FF_MAX))
+    return int(d), int(h)
 
 
 class NisqaTensor(C.Structure):
@@ -164,8 +182,7 @@ def config_from_args(args, max_chunk_segments=0):
     if (cnn, td) == ("adapt", "self_att") and pool_mode != POOL_LAST_STEP_BI:
         arch = ARCH_ADAPT_SA_ATTFF
         ok = (list(args["cnn_pool_1"]) == [24, 7] and list(args["cnn_pool_2"]) == [12, 5]
-              and list(args["cnn_pool_3"]) == [6, 3]
-              and args["td_sa_d_model"] == 64 and args["td_sa_nhead"] == 1 and args["td_sa_h"] == 64)
+              and list(args["cnn_pool_3"]) == [6, 3])
         cnn_fc = int(args.get("cnn_fc_out_h") or 0)           # optional Linear behind conv6 (lib:682-684)
         if cnn_fc % 64 != 0:
             raise NotImplementedError("cnn_fc_out_h=%d: the engine needs a multiple of 64" % cnn_fc)
@@ -178,7 +195,7 @@ def config_from_args(args, max_chunk_segments=0):
             cnn_fc = 4096                                   # DFF's default hidden width (lib:544)
         if cnn_fc % 64 != 0:
             raise NotImplementedError("cnn_fc_out_h=%d: the engine needs a multiple of 64" % cnn_fc)
-        ok = args["td_sa_d_model"] == 64 and args["td_sa_nhead"] == 1 and args["td_sa_h"] == 64
+        ok = True
     elif (cnn, td) == ("standard", "lstm") and pool_mode in (POOL_LAST_STEP_BI, POOL_AVG, POOL_MAX, POOL_LAST_STEP):
         arch = ARCH_STD_LSTM_LASTBI
         ok = (args.get("cnn_fc_out_h") == 20 and args["td_lstm_h"] == 128
@@ -200,18 +217,25 @@ def config_from_args(args, max_chunk_segments=0):
             raise NotImplementedError("de_align_apply / de_fuse option not available: %r / %r" % (args.get("de_align_apply"), args.get("de_fuse")))
         if args.get("de_fuse_dim") and int(args["de_fuse_dim"]) % 64 != 0:
             raise NotImplementedError("de_fuse_dim=%r: the engine needs a multiple of 64" % (args.get("de_fuse_dim"),))
-        ok = ok and args.get("td_2") == "self_att" and args.get("td_2_sa_d_model") == 64 and args.get("td_2_sa_nhead") == 1 \
-            and args.get("td_2_sa_h") == 64
+        ok = ok and args.get("td_2") == "self_att"
     elif args.get("td_2") == "self_att":
         # a second self-attention stack behind the first one (lib:114-141, 236-268)
-        ok = ok and arch == ARCH_ADAPT_SA_ATTFF and args.get("td_2_sa_d_model") == 64 and args.get("td_2_sa_nhead") == 1 \
-            and args.get("td_2_sa_h") == 64
+        ok = ok and arch == ARCH_ADAPT_SA_ATTFF
     else:
         ok = ok and args.get("td_2") in (None, "skip")
     ok = ok and (cnn_kind != CNN_CONV or (args["cnn_c_out_1"], args["cnn_c_out_2"], args["cnn_c_out_3"]) == (16, 32, 64))
     ok = ok and args["ms_n_fft"] == 4096 and args["ms_n_mels"] == 48 and args["ms_seg_length"] == 15
     if not ok:
         raise NotImplementedError("checkpoint hyper-parameters outside the shipped NISQA configurations")
+    sa = td2 = (0, 0)
+    if arch == ARCH_ADAPT_SA_ATTFF:
+        sa = _sa_widths(args, "td_sa", de)
+        if args.get("td_2") == "self_att":
+            td2 = _sa_widths(args, "td_2_sa", de)
+            if args["model"] == "NISQA_DIM" and td2[0] != sa[0]:
+                # NISQA_DIM builds its pooling heads for the first stack's width (lib:247-253): td_2 must keep it
+                raise NotImplementedError("NISQA_DIM with td_2_sa_d_model=%d != td_sa_d_model=%d: the reference model cannot "
+                                          "run it" % (td2[0], sa[0]))
     # ms_sr != None: the ingest converts every clip to that rate (nisqa_b200/resample.py) before the engine sees it
     cfg = NisqaConfig()
     cfg.abi_version = ABI_VERSION
@@ -228,6 +252,8 @@ def config_from_args(args, max_chunk_segments=0):
     cfg.pool = pool_mode
     cfg.pos_enc = 1 if (arch == ARCH_ADAPT_SA_ATTFF and args.get("td_sa_pos_enc")) else 0
     cfg.cnn_kind, cfg.cnn_fc = cnn_kind, cnn_fc
+    cfg.sa_d_model, cfg.sa_ff = sa
+    cfg.td2_d_model, cfg.td2_ff = td2
     if args.get("td_2") == "self_att":
         cfg.td2_layers = int(args["td_2_sa_num_layers"])
         cfg.td2_pos_enc = 1 if args.get("td_2_sa_pos_enc") else 0
