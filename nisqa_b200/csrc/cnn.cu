@@ -15,6 +15,7 @@
 #include "common.cuh"
 #include "tc_ptx.cuh"
 #include "conv1_cell.cuh"
+#include "launch.cuh"
 
 namespace nisqa {
 
@@ -253,6 +254,10 @@ using Conv3S = ConvCfg<12, 4, 32, 64, 1, POOL_NONE, 0, 4, 1, 6, 3>;   // -> [12]
 using Conv4S = ConvCfg<12, 4, 64, 64, 1, POOL_2X2, 2, 4, 1, 6, 3>;     // -> [6][2][64]
 using Conv5S = ConvCfg<6, 2, 64, 64, 1, POOL_NONE, 0, 6, 2, 8, 2>;    // -> [6][2][64]
 using Conv6S = Conv5S;
+
+static_assert(input_is<Conv2A>(0, 2) && input_is<Conv3A>(0, 3) && input_is<Conv4A>(0, 4) && input_is<Conv5A>(0, 5) &&
+              input_is<Conv6A>(0, 6) && input_is<Conv2S>(1, 2) && input_is<Conv3S>(1, 3) && input_is<Conv4S>(1, 4) &&
+              input_is<Conv5S>(1, 5) && input_is<Conv6S>(1, 6), "ConvCfg geometry differs from split_geometry");
 
 template <class C>
 static void launch_conv(cudaStream_t st, const float* in, const float* w, const float* b,

@@ -44,6 +44,7 @@
 #include "common.cuh"
 #include "conv1_cell.cuh"
 #include "conv_split.cuh"
+#include "launch.cuh"
 #include "tc_ptx.cuh"
 
 namespace nisqa {
@@ -474,18 +475,17 @@ static void launch_c12(cudaStream_t st, const __half* wtc, const float* b, float
                                                                       mel, seg_frame0, seg_thr, w1, b1, c1_scale);
 }
 
-// Geometry of the plane pair that feeds conv layer `layer` (2..6): rows of the padded image per segment,
-// bytes per row, and the bytes of one plane for n_seg segments (tile over-read included).
-void split_geometry(int std_mode, int layer, int* H, int* W, int* C) {
-  static const int ha[7] = {0, 0, 24, 12, 12, 6, 6}, ca[7] = {0, 0, 16, 32, 64, 64, 64};
-  static const int wa[7] = {0, 0, 7, 5, 5, 3, 3}, ws[7] = {0, 0, 8, 4, 4, 2, 2};
-  *H = ha[layer]; *C = ca[layer]; *W = std_mode ? ws[layer] : wa[layer];
-}
+static_assert(input_is<SpConv2A>(0, 2) && input_is<SpConv3A>(0, 3) && input_is<SpConv4A>(0, 4) &&
+              input_is<SpConv5A>(0, 5) && input_is<SpConv6A>(0, 6) && input_is<SpConv2S>(1, 2) &&
+              input_is<SpConv3S>(1, 3) && input_is<SpConv4S>(1, 4) && input_is<SpConv5S>(1, 5) &&
+              input_is<SpConv6S>(1, 6), "SpCfg geometry differs from split_geometry");
+
+// Bytes of one plane of the pair that feeds conv layer `layer` (2..6) for n_seg segments: per segment (H + 1) rows of
+// W + 1 pixels (shared zero row / column), the zero lead rows and the tile over-read.
 size_t split_plane_bytes(int std_mode, int layer, int n_seg) {
-  int H, W, C;
-  split_geometry(std_mode, layer, &H, &W, &C);
-  const size_t rows = (size_t)kSplitLead + (size_t)n_seg * (H + 1) * (W + 1) + 256 + 32;
-  return (rows * (size_t)C * 2 + 1023) & ~(size_t)1023;
+  const ConvGeom g = split_geometry(std_mode, layer);
+  const size_t rows = (size_t)kSplitLead + (size_t)n_seg * (g.H + 1) * (g.W + 1) + 256 + 32;
+  return (rows * (size_t)g.C * 2 + 1023) & ~(size_t)1023;
 }
 
 // conv layer 2..6 on planes; the last layer (6) writes the fp32 CNN features (adapt: [seg][6][64];
@@ -532,15 +532,14 @@ void launch_conv12(cudaStream_t st, int std_mode, const float* mel, const int* s
 
 void launch_unsplit(cudaStream_t st, int std_mode, int layer, const void* hi, const void* lo, float unit, float* out,
                     int n_seg) {
-  int H, W, C;
-  split_geometry(std_mode, layer, &H, &W, &C);
-  const long long items = (long long)n_seg * H * W * (C / 8);
+  const ConvGeom g = split_geometry(std_mode, layer);
+  const long long items = (long long)n_seg * g.H * g.W * (g.C / 8);
   const unsigned char* h = static_cast<const unsigned char*>(hi);
   const unsigned char* l = static_cast<const unsigned char*>(lo);
   const int grid = (int)std::min<long long>((items + 255) / 256, (long long)device_sms() * 16);
-  if (C == 16) unsplit_kernel<32><<<grid, 256, 0, st>>>(h, l, out, items, H, W, unit);
-  else if (C == 32) unsplit_kernel<64><<<grid, 256, 0, st>>>(h, l, out, items, H, W, unit);
-  else unsplit_kernel<128><<<grid, 256, 0, st>>>(h, l, out, items, H, W, unit);
+  if (g.C == 16) unsplit_kernel<32><<<grid, 256, 0, st>>>(h, l, out, items, g.H, g.W, unit);
+  else if (g.C == 32) unsplit_kernel<64><<<grid, 256, 0, st>>>(h, l, out, items, g.H, g.W, unit);
+  else unsplit_kernel<128><<<grid, 256, 0, st>>>(h, l, out, items, g.H, g.W, unit);
 }
 
 }  // namespace nisqa

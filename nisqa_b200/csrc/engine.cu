@@ -20,53 +20,7 @@
 
 #include "../../include/nisqa_b200.h"
 #include "common.cuh"
-
-namespace nisqa {
-// frontend.cu
-void launch_frontend(cudaStream_t, const void*, int, const ClipDesc*, int, int,
-                     const FbTables*, const float2*, float*, unsigned*, int, int, int);
-void launch_seg_table(cudaStream_t, const ClipDesc*, int, const int*, const unsigned*, int, int,
-                      int*, float*, int*);
-void launch_mel_dump(cudaStream_t, const float*, const ClipDesc*, int, const unsigned*, float*);
-// cnn.cu
-void launch_conv1(cudaStream_t, int, const float*, const int*, const float*, const float*,
-                  const float*, float*, int, void*, void*, float);
-void launch_conv_layer(cudaStream_t, int, int, const float*, const float*, const float*, float*, int);
-void launch_nhwc_to_nchw(cudaStream_t, const float*, float*, long long, int, int);
-// conv_split.cu
-size_t split_plane_bytes(int std_mode, int layer, int n_seg);
-void launch_conv_split(cudaStream_t, int, int, const void*, const void*, const void*, const float*, float, float,
-                       void*, void*, float*, int);
-void launch_unsplit(cudaStream_t, int, int, const void*, const void*, float, float*, int);
-void launch_conv12(cudaStream_t, int, const float*, const int*, const float*, const float*, const float*, float,
-                   const void*, const float*, float, float, void*, void*, int);
-// td.cu
-struct SaLayerParams {
-  const float* WoT; const float* bo; const float* W1T; const float* b1; const float* W2T;
-  const float* b2; const float* ln1_g; const float* ln1_b; const float* ln2_g; const float* ln2_b;
-};
-struct PoolHeadParams { const float* W1T; const float* b1; const float* w2; const float* b2; const float* w3; const float* b3; };
-struct LstmParams { const float* w_ih; const float* w_hh; const float* b; const float* w_pool; };
-void launch_fc20(cudaStream_t, const float*, const float*, const float*, float*, int);
-void launch_lstm(cudaStream_t, const float*, const ClipDesc*, int, const LstmParams&, float*, float*, float, float*);
-void launch_lstm_batched(cudaStream_t, const float*, const ClipDesc*, const int*, int, const LstmParams&, float*, float*, float, float*);
-void launch_pool_final(cudaStream_t, const float*, int, const float*, const ClipDesc*, int, const PoolHeadParams&, int, int, float*);
-// td_tiled.cu
-struct ResampleClip { long long in_off, out_off, time_off; int n_in, n_out, n_fix, copy; double ratio; };
-void launch_resample(cudaStream_t, const void*, int, const ResampleClip*, int, int, double*, const double*, int, int, float*);
-bool resample_table(std::vector<double>*, int*);
-struct DeAlignParams { const float* wT; const float* b; const float* wqT; const float* bq; const float* wyT; const float* by; const float* v; };
-void launch_de_align(cudaStream_t, const float*, const ClipDesc*, int, const int*, int, int, int, int, const DeAlignParams&, float*);
-void launch_de_finalize(cudaStream_t, const ClipDesc*, int, int, float*);
-void launch_seg_feats(cudaStream_t, const float*, const int*, const float*, const float*, int, float*);
-void launch_linear_tile(cudaStream_t, const float*, int, const float*, const float*, int, float*, int, int, int, int);
-void launch_td_in(cudaStream_t, int, const float*, const float*, int, const float*, const float*, const float*,
-                  const float*, const float*, float, const float*, const int*, const ClipDesc*, float*, float*, int);
-struct PoolSimpleParams { const float* a1; const float* a1b; const float* w3; const float* b3; };
-void launch_pool_simple(cudaStream_t, const float*, int, const ClipDesc*, int, int, const PoolSimpleParams&, int, int, float*);
-void launch_td_sa(cudaStream_t, int, const float*, const float*, const ClipDesc*, int, const int*, int, const SaLayerParams&, int,
-                  float*, const float*, const float*, float, float*, const PoolHeadParams&, int, float*);
-}  // namespace nisqa
+#include "launch.cuh"
 
 using namespace nisqa;
 
@@ -146,13 +100,15 @@ constexpr int kLanes = NISQA_LANES;
 constexpr int kStages = 6;     // staging slots / submissions in flight (uploads run ahead of the lanes)
 struct Lane {
   cudaStream_t stream = nullptr;
-  DevBuf mel, segtab, act1, act2, act3, act4, act5, feats, xa, xb, qkv, qkv2, logits, feats20, tdout, partial, fused, td2in, ffa, ffb;
+  DevBuf mel, segtab, feats, xa, xb, qkv, qkv2, logits, feats20, tdout, partial, fused, td2in, ffa, ffb;
+  DevBuf act[7];           // act[l]: fp32 channels-last map feeding conv layer l (2..6) on the FFMA path (and stage dumps)
   DevBuf planes[7];        // planes[l]: fp16 hi | lo plane pair feeding conv layer l (2..6), conv_split.cu
   size_t plane_bytes[7] = {0, 0, 0, 0, 0, 0, 0};   // offset of the lo plane inside planes[l] (half of the allocation)
   void release() {
+    for (auto& b : act) b.release();
     for (auto& b : planes) b.release();
-    DevBuf* all[] = {&mel, &segtab, &act1, &act2, &act3, &act4, &act5,
-                     &feats, &xa, &xb, &qkv, &qkv2, &logits, &feats20, &tdout, &partial, &fused, &td2in, &ffa, &ffb};
+    DevBuf* all[] = {&mel, &segtab, &feats, &xa, &xb, &qkv, &qkv2, &logits, &feats20, &tdout, &partial, &fused, &td2in,
+                     &ffa, &ffb};
     for (auto* b : all) b->release();
     if (stream) cudaStreamDestroy(stream);
   }
@@ -181,6 +137,37 @@ struct TimerSlot {
   int launches = 0;
 };
 
+// The packed weights: device pointers into the weights arena, set by pack_weights on every load.  A weight that the
+// checkpoint's architecture does not use stays nullptr.
+struct Linear { const float* wT = nullptr; const float* b = nullptr; };    // k-major weight, bias
+struct ConvWeights {
+  const float* w = nullptr;      // [ci][tap][co] fp32, BatchNorm folded in (conv1, and conv2..6 on the FFMA path)
+  const float* b = nullptr;      // [co]
+  const float* wtc = nullptr;    // conv2..6 on the tensor cores: fp16 hi / lo split (pack_conv_tc)
+};
+constexpr int kMaxSaLayers = 8;  // nisqa_create's limit on sa_layers / td2_layers
+struct SaStackWeights {
+  Linear in;                     // Linear(in -> D), 64-column chunks
+  const float* ln_g = nullptr;   // the LayerNorm behind it
+  const float* ln_b = nullptr;
+  const float* pe = nullptr;     // positional encoding [max_len][D], when the stack has one
+  SaLayerParams layer[kMaxSaLayers] = {};
+  Linear qkv[kMaxSaLayers];      // in_proj of each layer (q pre-scaled by q_fold)
+};
+struct Weights {
+  ConvWeights conv[7];           // conv1..conv6
+  const float* ff_bn = nullptr;  // SkipCNN / DFF: BatchNorm2d(1) as (scale, shift)
+  Linear ff[4];                  // SkipCNN's Linear, or DFF's four, BatchNorm1d folded in
+  Linear ffc;                    // AdaptCNN's Linear behind conv6 (cnn_fc_out_h)
+  SaStackWeights sa[2];          // time_dependency, time_dependency_2
+  Linear defuse;                 // NISQA_DE Fusion.lin_fusion
+  DeAlignParams de = {};
+  PoolHeadParams pool_head = {};       // PoolAttFF
+  PoolSimpleParams pool_simple = {};   // the other pooling modules
+  Linear fc;                     // StandardCNN fc_out 768 -> 20
+  LstmParams lstm = {};
+};
+
 }  // namespace
 
 struct nisqa_engine {
@@ -200,12 +187,12 @@ struct nisqa_engine {
   int conv_tc = 1;         // 1: conv2..6 on the tensor cores (fp16 two-term split, fp16 plane pairs between the layers); 0: fp32 FFMA
   std::vector<TimerSlot> timers;
 
-  // weights arena (device) + offsets
+  // weights arena (device) and the pointers into it
   DevBuf warena;
+  Weights w;
   DevBuf rs_raw, rs_out, rs_clips, rs_times, rs_win;   // device resampler of the ingest (resample_gpu.cu)
   HostBuf rs_host;
   int rs_nwin = 0, rs_num_table = 0;
-  std::map<std::string, size_t> woff;   // float offsets into warena
   float pool_bias_std = 0.f;
   float tc_scale[8] = {1, 1, 1, 1, 1, 1, 1, 1};   // 2^(e_{i-1} - S_i): undoes the activation and weight pre-scales of conv i
   int act_exp[8] = {0, 0, 0, 0, 0, 0, 0, 0};      // e_i: conv i's activations are stored as fp16 planes of v * 2^-e_i
@@ -427,45 +414,50 @@ int build_fb(nisqa_engine* e, int sr, int hop, int win, int* id_out) {
 struct TensorView { const float* d; int nd; int64_t dims[4]; int64_t numel; };
 
 struct Packer {
-  nisqa_engine* e;
   std::map<std::string, TensorView> t;
   std::vector<float> arena;
-  std::string missing;
+  Weights w;                                               // its pointers are set by pack_weights once `arena` is uploaded
+  std::vector<std::pair<const float**, size_t>> slots;     // (member of w, float offset of its block in arena)
+  std::string err;
+  bool fail(const std::string& msg) { if (err.empty()) err = msg; return false; }
   const TensorView* get(const std::string& name, std::initializer_list<int64_t> shape) {
     auto it = t.find(name);
-    if (it == t.end()) { if (missing.empty()) missing = "missing tensor " + name; return nullptr; }
+    if (it == t.end()) { fail("missing tensor " + name); return nullptr; }
     const TensorView& v = it->second;
     bool ok = v.nd == (int)shape.size();
     int i = 0;
     for (int64_t s : shape) { if (ok && v.dims[i] != s) ok = false; ++i; }
-    if (!ok) { if (missing.empty()) missing = "bad shape for tensor " + name; return nullptr; }
+    if (!ok) { fail("bad shape for tensor " + name); return nullptr; }
     return &v;
   }
-  size_t alloc(const std::string& key, size_t n) {
-    size_t off = (arena.size() + 63) / 64 * 64;     // 256-byte aligned blocks
+  // a zero-filled block of n floats for `dst`, 256-byte aligned (the conv kernels read their weights with 16-byte cp.async
+  // and bulk copies); returns its offset in arena
+  size_t alloc(const float*& dst, size_t n) {
+    const size_t off = (arena.size() + 63) / 64 * 64;
     arena.resize(off + n, 0.f);
-    e->woff[key] = off;
+    slots.push_back({&dst, off});
     return off;
   }
+  void copy(const float*& dst, const float* src, size_t n) { memcpy(&arena[alloc(dst, n)], src, n * 4); }
 };
 
-bool pack_conv(Packer& P, int idx, int cin, int cout, int* act_exp) {
-  char nm[96];
-  auto name = [&](const char* fmt) { snprintf(nm, sizeof nm, fmt, idx); return std::string(nm); };
-  const TensorView* w = P.get(name("cnn.model.conv%d.weight"), {cout, cin, 3, 3});
-  const TensorView* b = P.get(name("cnn.model.conv%d.bias"), {cout});
-  const TensorView* g = P.get(name("cnn.model.bn%d.weight"), {cout});
-  const TensorView* be = P.get(name("cnn.model.bn%d.bias"), {cout});
-  const TensorView* mu = P.get(name("cnn.model.bn%d.running_mean"), {cout});
-  const TensorView* var = P.get(name("cnn.model.bn%d.running_var"), {cout});
+// conv<idx> with bn<idx> folded in, as [ci][tap][co] (conv1: [tap][16]); *w_off: the offset of the weights in the arena
+bool pack_conv(Packer& P, int idx, int cin, int cout, int* act_exp, size_t* w_off) {
+  const std::string cv = "cnn.model.conv" + std::to_string(idx) + ".", bn = "cnn.model.bn" + std::to_string(idx) + ".";
+  const TensorView* w = P.get(cv + "weight", {cout, cin, 3, 3});
+  const TensorView* b = P.get(cv + "bias", {cout});
+  const TensorView* g = P.get(bn + "weight", {cout});
+  const TensorView* be = P.get(bn + "bias", {cout});
+  const TensorView* mu = P.get(bn + "running_mean", {cout});
+  const TensorView* var = P.get(bn + "running_var", {cout});
   if (!w || !b || !g || !be || !mu || !var) return false;
   // activation exponent: max_c |beta_c| + 3 |gamma_c| (the BN output at three standard deviations) -> [2.8, 5.7) 2^e.
   // It moves by exactly k when BatchNorm's weight and bias are multiplied by 2^k.
   double E = 0.0;
   for (int co = 0; co < cout; ++co) E = std::max(E, fabs((double)be->d[co]) + 3.0 * fabs((double)g->d[co]));
   *act_exp = (E > 0.0 && std::isfinite(E)) ? ilogb(E * sqrt(2.0) / 4.0) : 0;
-  const size_t wo = P.alloc(name("conv%d.w"), (size_t)cin * 9 * cout);
-  const size_t bo = P.alloc(name("conv%d.b"), cout);
+  const size_t wo = P.alloc(P.w.conv[idx].w, (size_t)cin * 9 * cout);
+  const size_t bo = P.alloc(P.w.conv[idx].b, cout);
   for (int co = 0; co < cout; ++co) {
     // eval-mode BatchNorm2d (eps 1e-5) folded into the convolution (SURVEY.md Appendix A)
     const double s = (double)g->d[co] / sqrt((double)var->d[co] + 1e-5);
@@ -475,7 +467,36 @@ bool pack_conv(Packer& P, int idx, int cin, int cout, int* act_exp) {
         P.arena[wo + ((size_t)ci * 9 + tap) * cout + co] =
             (float)((double)w->d[((size_t)co * cin + ci) * 9 + tap] * s);
   }
+  *w_off = wo;
   return true;
+}
+
+// conv2..conv6 for the tensor-core path, from the folded fp32 weights at `src`: [tap][ci/8][hi co | lo co][8] fp16
+// two-term split of w * 2^S, S chosen so that max|w| 2^S lies in (512, 1024] whatever the weights' range (b_lo stays out
+// of the fp16 subnormals)
+void pack_conv_tc(Packer& P, int idx, int ci_n, int co_n, size_t src, int act_exp_in, float* tc_scale) {
+  float wmax = 0.f;
+  for (size_t j = 0; j < (size_t)ci_n * 9 * co_n; ++j) wmax = std::max(wmax, fabsf(P.arena[src + j]));
+  int S = 0;
+  if (wmax > 0.f && std::isfinite(wmax)) {
+    S = 9 - ilogbf(wmax);                                         // max|w| 2^S in [512, 1024)
+    if (ldexpf(wmax, S) == 512.f) ++S;                            // a power of two: 1024 itself
+  }
+  *tc_scale = ldexpf(1.f, act_exp_in - S);
+  const size_t n_half = (size_t)9 * 2 * ci_n * co_n;
+  const size_t dst = P.alloc(P.w.conv[idx].wtc, (n_half + 1) / 2);   // fp16 payload inside the float arena
+  for (int tap = 0; tap < 9; ++tap)
+    for (int ci = 0; ci < ci_n; ++ci)
+      for (int co = 0; co < co_n; ++co) {
+        const float w = ldexpf(P.arena[src + ((size_t)ci * 9 + tap) * co_n + co], S);
+        const __half hi = __float2half_rn(w);
+        const __half lo = __float2half_rn(w - __half2float(hi));
+        __half* base = reinterpret_cast<__half*>(&P.arena[dst]) + (size_t)tap * 2 * ci_n * co_n;
+        // per 16-byte K chunk: rows [0,co_n) = hi, rows [co_n, 2 co_n) = lo  (one N = 2*C_out operand)
+        const size_t off = ((size_t)(ci / 8) * (2 * co_n) + co) * 8 + (ci & 7);
+        base[off] = hi;
+        base[off + (size_t)co_n * 8] = lo;
+      }
 }
 
 // dst[k][j] = src[j][perm(k)] for a [n_out][n_in] PyTorch Linear weight
@@ -498,243 +519,189 @@ void pack_linear_chunked(Packer& P, size_t off, const TensorView* w, int n_out, 
 float q_fold(int D) { return D == 64 ? 0.125f : D == 256 ? 0.0625f : 1.f; }
 float q_scale(int D) { return q_fold(D) == 1.f ? (float)(1.0 / std::sqrt((double)D)) : 1.f; }
 
-int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
-  Packer P; P.e = e;
-  for (int i = 0; i < n; ++i) {
-    if (!tensors[i].name || !tensors[i].data) continue;
-    TensorView v; v.d = tensors[i].data; v.nd = tensors[i].ndim; v.numel = 1;
-    for (int d = 0; d < 4; ++d) { v.dims[d] = d < v.nd ? tensors[i].dims[d] : 1; v.numel *= v.dims[d]; }
-    P.t[tensors[i].name] = v;
-  }
-  e->woff.clear();
-  const int cin[7] = {0, 1, 16, 32, 64, 64, 64}, cout[7] = {0, 16, 32, 64, 64, 64, 64};
-  const bool conv_net = e->cfg.cnn_kind == NISQA_CNN_CONV;
-  if (!conv_net) {
-    // SkipCNN / DFF (lib:504-583): the BatchNorm2d(1) in front as a scalar affine map (applied by seg_feats_kernel, so
-    // that the Linear layers see what the reference's see), Linear layers k-major, DFF's BatchNorm1d folded into them
-    const bool dff = e->cfg.cnn_kind == NISQA_CNN_DFF;
-    const std::string p = "cnn.model.";
-    const std::string bn = dff ? "bn1." : "bn.";
-    const TensorView* g = P.get(p + bn + "weight", {1});
-    const TensorView* be = P.get(p + bn + "bias", {1});
-    const TensorView* mu = P.get(p + bn + "running_mean", {1});
-    const TensorView* var = P.get(p + bn + "running_var", {1});
-    if (!g || !be || !mu || !var) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-    const double a = (double)g->d[0] / sqrt((double)var->d[0] + 1e-5);
-    size_t o = P.alloc("ff.bn", 2);
-    P.arena[o] = (float)a; P.arena[o + 1] = (float)((double)be->d[0] - (double)mu->d[0] * a);
-    const int H = e->cfg.cnn_fc;
-    auto pack_lin = [&](const std::string& wname, const std::string& bnname, int n_in, int n_in_pad, int n_out, const std::string& key) -> bool {
-      const TensorView* w = P.get(p + wname + ".weight", {n_out, n_in});
-      const TensorView* b = P.get(p + wname + ".bias", {n_out});
-      if (!w || !b) return false;
-      std::vector<double> sc(n_out, 1.0), sh(n_out, 0.0);
-      if (!bnname.empty()) {            // eval-mode BatchNorm1d (eps 1e-5) folded into the Linear in front of it
-        const TensorView* g2 = P.get(p + bnname + ".weight", {n_out});
-        const TensorView* b2 = P.get(p + bnname + ".bias", {n_out});
-        const TensorView* m2 = P.get(p + bnname + ".running_mean", {n_out});
-        const TensorView* v2 = P.get(p + bnname + ".running_var", {n_out});
-        if (!g2 || !b2 || !m2 || !v2) return false;
-        for (int j = 0; j < n_out; ++j) {
-          sc[j] = (double)g2->d[j] / sqrt((double)v2->d[j] + 1e-5);
-          sh[j] = (double)b2->d[j] - (double)m2->d[j] * sc[j];
-        }
-      }
-      const size_t ow = P.alloc(key + ".wT", (size_t)n_in_pad * n_out), ob = P.alloc(key + ".b", n_out);
-      for (int k = 0; k < n_in; ++k)
-        for (int j = 0; j < n_out; ++j) P.arena[ow + (size_t)k * n_out + j] = (float)((double)w->d[(size_t)j * n_in + k] * sc[j]);
-      for (int j = 0; j < n_out; ++j) P.arena[ob + j] = (float)((double)b->d[j] * sc[j] + sh[j]);
-      return true;
-    };
-    bool ok = true;
-    if (dff) {
-      ok = pack_lin("lin1", "bn2", 720, 768, H, "ff1") && pack_lin("lin2", "bn3", H, H, H, "ff2") &&
-           pack_lin("lin3", "bn4", H, H, H, "ff3") && pack_lin("lin4", "bn5", H, H, H, "ff4");
-    } else if (H > 0) {
-      ok = pack_lin("linear", "", 720, 768, H, "ff1");
+// SkipCNN / DFF Linear `name` (n_in -> n_out) k-major with n_in_pad rows, the eval-mode BatchNorm1d `bn` behind it
+// (eps 1e-5; none when empty) folded in
+bool pack_ff_linear(Packer& P, Linear& dst, const std::string& name, const std::string& bn, int n_in, int n_in_pad, int n_out) {
+  const std::string p = "cnn.model.";
+  const TensorView* w = P.get(p + name + ".weight", {n_out, n_in});
+  const TensorView* b = P.get(p + name + ".bias", {n_out});
+  if (!w || !b) return false;
+  std::vector<double> sc(n_out, 1.0), sh(n_out, 0.0);
+  if (!bn.empty()) {
+    const TensorView* g2 = P.get(p + bn + ".weight", {n_out});
+    const TensorView* b2 = P.get(p + bn + ".bias", {n_out});
+    const TensorView* m2 = P.get(p + bn + ".running_mean", {n_out});
+    const TensorView* v2 = P.get(p + bn + ".running_var", {n_out});
+    if (!g2 || !b2 || !m2 || !v2) return false;
+    for (int j = 0; j < n_out; ++j) {
+      sc[j] = (double)g2->d[j] / sqrt((double)v2->d[j] + 1e-5);
+      sh[j] = (double)b2->d[j] - (double)m2->d[j] * sc[j];
     }
-    if (!ok) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
   }
-  for (int i = 1; conv_net && i <= 6; ++i)
-    if (!pack_conv(P, i, cin[i], cout[i], &e->act_exp[i])) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-  // conv2..conv6 for the tensor-core path: [tap][ci/8][hi co | lo co][8] fp16 two-term split of w * 2^S, S chosen so
-  // that max|w| 2^S lies in (512, 1024] whatever the weights' range (b_lo stays out of the fp16 subnormals)
-  for (int i = 2; conv_net && i <= 6; ++i) {
-    char k1[32], k2[32];
-    snprintf(k1, sizeof k1, "conv%d.w", i); snprintf(k2, sizeof k2, "conv%d.wtc", i);
-    const int ci_n = cin[i], co_n = cout[i], nch = ci_n / 8;
-    const size_t src = e->woff.at(k1);
-    float wmax = 0.f;
-    for (size_t j = 0; j < (size_t)ci_n * 9 * co_n; ++j) wmax = std::max(wmax, fabsf(P.arena[src + j]));
-    int S = 0;
-    if (wmax > 0.f && std::isfinite(wmax)) {
-      S = 9 - ilogbf(wmax);                                         // max|w| 2^S in [512, 1024)
-      if (ldexpf(wmax, S) == 512.f) ++S;                            // a power of two: 1024 itself
-    }
-    e->tc_scale[i] = ldexpf(1.f, e->act_exp[i - 1] - S);
-    const size_t n_half = (size_t)9 * 2 * ci_n * co_n;
-    const size_t dst = P.alloc(k2, (n_half + 1) / 2);              // fp16 payload inside the float arena
-    for (int tap = 0; tap < 9; ++tap)
-      for (int ci = 0; ci < ci_n; ++ci)
-        for (int co = 0; co < co_n; ++co) {
-          const float w = ldexpf(P.arena[src + ((size_t)ci * 9 + tap) * co_n + co], S);
-          const __half hi = __float2half_rn(w);
-          const __half lo = __float2half_rn(w - __half2float(hi));
-          __half* base = reinterpret_cast<__half*>(&P.arena[dst]) + (size_t)tap * 2 * ci_n * co_n;
-          // per 16-byte K chunk: rows [0,co_n) = hi, rows [co_n, 2 co_n) = lo  (one N = 2*C_out operand)
-          const size_t off = ((size_t)(ci / 8) * (2 * co_n) + co) * 8 + (ci & 7);
-          base[off] = hi;
-          base[off + (size_t)co_n * 8] = lo;
-          (void)nch;
-        }
-  }
+  const size_t ow = P.alloc(dst.wT, (size_t)n_in_pad * n_out), ob = P.alloc(dst.b, n_out);
+  for (int k = 0; k < n_in; ++k)
+    for (int j = 0; j < n_out; ++j) P.arena[ow + (size_t)k * n_out + j] = (float)((double)w->d[(size_t)j * n_in + k] * sc[j]);
+  for (int j = 0; j < n_out; ++j) P.arena[ob + j] = (float)((double)b->d[j] * sc[j] + sh[j]);
+  return true;
+}
 
-  if (e->cfg.arch == NISQA_ARCH_ADAPT_SA_ATTFF) {
-    const std::string td = "time_dependency.model.";
-    // one SelfAttention stack (lib:945-1040) of width D and feed-forward width F: Linear(in -> D) + LayerNorm + `layers`
-    // encoder layers.  `kp` prefixes the arena keys ("" = time_dependency, "2" = time_dependency_2)
-    auto pack_sa_stack = [&](const std::string& ck, const std::string& kp, int in_dim, int layers, bool cnn_order, int D,
-                             int F) -> bool {
-      const size_t vb = (size_t)D * 4;
-      const TensorView* lw = P.get(ck + "linear.weight", {D, in_dim});
-      const TensorView* lb = P.get(ck + "linear.bias", {D});
-      const TensorView* ng = P.get(ck + "norm1.weight", {D});
-      const TensorView* nb = P.get(ck + "norm1.bias", {D});
-      if (!lw || !lb || !ng || !nb) return false;
-      const int k_pad = (in_dim + 63) / 64 * 64;
-      size_t o = P.alloc("lin" + kp + ".wT", (size_t)k_pad * D);
-      if (cnn_order)      // engine feature order k' = h*64 + c  <->  reference view(-1, 64*6) order c*6 + h (lib:706)
-        pack_linear_chunked(P, o, lw, D, in_dim, k_pad, [](int k) { return (k & 63) * 6 + (k >> 6); });
-      else
-        pack_linear_chunked(P, o, lw, D, in_dim, k_pad, [](int k) { return k; });
-      o = P.alloc("lin" + kp + ".b", D); memcpy(&P.arena[o], lb->d, vb);
-      o = P.alloc("ln" + kp + "0.g", D); memcpy(&P.arena[o], ng->d, vb);
-      o = P.alloc("ln" + kp + "0.b", D); memcpy(&P.arena[o], nb->d, vb);
-      const auto id = [](int k) { return k; };
-      for (int l = 0; l < layers; ++l) {
-        char pf[96]; snprintf(pf, sizeof pf, "layers.%d.", l);
-        char key[64];
-        const std::string p = ck + pf;
-        const TensorView* iw = P.get(p + "self_attn.in_proj_weight", {3 * D, D});
-        const TensorView* ib = P.get(p + "self_attn.in_proj_bias", {3 * D});
-        const TensorView* ow = P.get(p + "self_attn.out_proj.weight", {D, D});
-        const TensorView* ob = P.get(p + "self_attn.out_proj.bias", {D});
-        const TensorView* w1 = P.get(p + "linear1.weight", {F, D});
-        const TensorView* b1 = P.get(p + "linear1.bias", {F});
-        const TensorView* w2 = P.get(p + "linear2.weight", {D, F});
-        const TensorView* b2 = P.get(p + "linear2.bias", {D});
-        const TensorView* g1 = P.get(p + "norm1.weight", {D});
-        const TensorView* e1 = P.get(p + "norm1.bias", {D});
-        const TensorView* g2 = P.get(p + "norm2.weight", {D});
-        const TensorView* e2 = P.get(p + "norm2.bias", {D});
-        if (!iw || !ib || !ow || !ob || !w1 || !b1 || !w2 || !b2 || !g1 || !e1 || !g2 || !e2) return false;
-        auto K = [&](const char* s2) { snprintf(key, sizeof key, "sa%s%d.%s", kp.c_str(), l, s2); return std::string(key); };
-        const float qf = q_fold(D);
-        o = P.alloc(K("qkvT"), (size_t)3 * D * D);
-        pack_linear_chunked(P, o, iw, 3 * D, D, D, id);
-        for (size_t i = 0; i < (size_t)D * D; ++i) P.arena[o + i] *= qf;          // the q chunks come first
-        o = P.alloc(K("qkvb"), 3 * D);
-        for (int j = 0; j < 3 * D; ++j) P.arena[o + j] = ib->d[j] * (j < D ? qf : 1.f);
-        o = P.alloc(K("woT"), (size_t)D * D); pack_linear_chunked(P, o, ow, D, D, D, id);
-        o = P.alloc(K("bo"), D); memcpy(&P.arena[o], ob->d, vb);
-        o = P.alloc(K("w1T"), (size_t)F * D); pack_linear_chunked(P, o, w1, F, D, D, id);
-        o = P.alloc(K("b1"), F); memcpy(&P.arena[o], b1->d, (size_t)F * 4);
-        o = P.alloc(K("w2T"), (size_t)D * F); pack_linear_chunked(P, o, w2, D, F, F, id);
-        o = P.alloc(K("b2"), D); memcpy(&P.arena[o], b2->d, vb);
-        o = P.alloc(K("ln1g"), D); memcpy(&P.arena[o], g1->d, vb);
-        o = P.alloc(K("ln1b"), D); memcpy(&P.arena[o], e1->d, vb);
-        o = P.alloc(K("ln2g"), D); memcpy(&P.arena[o], g2->d, vb);
-        o = P.alloc(K("ln2b"), D); memcpy(&P.arena[o], e2->d, vb);
-      }
-      return true;
-    };
-    auto pack_pos_enc = [&](const std::string& ck, const std::string& key, int D) -> int {
-      auto it = P.t.find(ck + "pos_encoder.pe");                  // registered buffer [max_len, 1, D] (lib:1051-1058)
-      if (it == P.t.end() || it->second.nd != 3 || it->second.dims[1] != 1 || it->second.dims[2] != D)
-        return fail(e, NISQA_ERR_WEIGHTS, "missing tensor " + ck + "pos_encoder.pe");
-      if (e->cfg.max_segments > 0 && it->second.dims[0] < e->cfg.max_segments)
-        return fail(e, NISQA_ERR_WEIGHTS, "positional encoding shorter than ms_max_segments");
-      const size_t o2 = P.alloc(key, (size_t)it->second.numel);
-      memcpy(&P.arena[o2], it->second.d, (size_t)it->second.numel * 4);
-      return 0;
-    };
-    // framewise features feeding the first stack: 384 (AdaptCNN, engine order), 720 (SkipCNN without Linear: padded to 768
-    // with zero rows) or cnn_fc_out_h
-    const int feat_dim = e->cfg.cnn_fc > 0 ? e->cfg.cnn_fc : (conv_net ? 384 : 720);
-    if (conv_net && e->cfg.cnn_fc > 0) {
-      // AdaptCNN's optional Linear (lib:682-684, 708-709): k-major, rows in the engine's feature order h*64 + c
-      const int H = e->cfg.cnn_fc;
-      const TensorView* w = P.get("cnn.model.fc.weight", {H, 384});
-      const TensorView* b = P.get("cnn.model.fc.bias", {H});
-      if (!w || !b) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-      const size_t ow = P.alloc("ffc.wT", (size_t)384 * H), ob = P.alloc("ffc.b", H);
-      for (int h = 0; h < 6; ++h)
-        for (int c = 0; c < 64; ++c)
-          for (int j = 0; j < H; ++j) P.arena[ow + ((size_t)h * 64 + c) * H + j] = w->d[(size_t)j * 384 + c * 6 + h];
-      memcpy(&P.arena[ob], b->d, (size_t)H * 4);
-    }
-    if (!pack_sa_stack(td, "", feat_dim, e->cfg.sa_layers, conv_net && e->cfg.cnn_fc == 0, e->sa_d(), e->sa_f()))
-      return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-    if (e->cfg.double_ended || e->cfg.td2_layers > 0) {
-      // time_dependency_2: behind the fusion of the double-ended model (input 192 / 128), or a second stack behind the
-      // first one in NISQA / NISQA_DIM (lib:114-141, 236-268; input: the first stack's width)
-      const std::string td2 = "time_dependency_2.model.";
-      int fdim = !e->cfg.double_ended ? e->sa_d() : (e->cfg.de_fuse == NISQA_DE_FUSE_XY_MINUS ? 192 : 128);
-      if (e->cfg.double_ended && e->cfg.de_fuse_dim > 0) {        // Fusion.lin_fusion (lib:1399-1401)
-        const int D = e->cfg.de_fuse_dim;
-        const TensorView* w = P.get("fuse.lin_fusion.weight", {D, fdim});
-        const TensorView* b = P.get("fuse.lin_fusion.bias", {D});
-        if (!w || !b) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-        const size_t ow = P.alloc("defuse.wT", (size_t)fdim * D), ob = P.alloc("defuse.b", D);
-        pack_linear_T(P, ow, w, D, fdim);
-        memcpy(&P.arena[ob], b->d, (size_t)D * 4);
-        fdim = D;
-      }
-      if (!pack_sa_stack(td2, "2", fdim, e->cfg.td2_layers, false, e->td2_d(), e->td2_f())) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-      if (e->cfg.td2_pos_enc) { int rc = pack_pos_enc(td2, "pe2", e->td2_d()); if (rc) return rc; }
-      if (e->cfg.de_align == NISQA_DE_ALIGN_LUONG) {            // AttLuong: W = Linear(y_dim -> q_dim), lib:1348-1351
-        const TensorView* w = P.get("align.att.W.weight", {64, 64});
-        const TensorView* b = P.get("align.att.W.bias", {64});
-        if (!w || !b) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-        size_t o = P.alloc("de.wT", 4096); pack_linear_T(P, o, w, 64, 64);
-        o = P.alloc("de.b", 64); memcpy(&P.arena[o], b->d, 256);
-      }
-      if (e->cfg.de_align == NISQA_DE_ALIGN_BAHDANAU) {         // AttBahdanau: Wq, Wy (-> att_dim 128), v, lib:1329-1337
-        const TensorView* wq = P.get("align.att.Wq.weight", {128, 64});
-        const TensorView* bq = P.get("align.att.Wq.bias", {128});
-        const TensorView* wy = P.get("align.att.Wy.weight", {128, 64});
-        const TensorView* by = P.get("align.att.Wy.bias", {128});
-        const TensorView* v = P.get("align.att.v.weight", {1, 128});
-        if (!wq || !bq || !wy || !by || !v) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-        size_t o = P.alloc("de.wqT", 64 * 128); pack_linear_T(P, o, wq, 128, 64);
-        o = P.alloc("de.bq", 128); memcpy(&P.arena[o], bq->d, 512);
-        o = P.alloc("de.wyT", 64 * 128); pack_linear_T(P, o, wy, 128, 64);
-        o = P.alloc("de.by", 128); memcpy(&P.arena[o], by->d, 512);
-        o = P.alloc("de.v", 128); memcpy(&P.arena[o], v->d, 512);
-      }
-    }
-    const int nh = e->cfg.n_out;
-    auto head_prefix = [&](int h) {
-      char pf[64];
-      if (nh == 1) snprintf(pf, sizeof pf, "pool.model.");
-      else snprintf(pf, sizeof pf, "pool_layers.%d.model.", h);   // head order mos,noi,dis,col,loud (lib:1461-1465)
-      return std::string(pf);
-    };
-    if (e->cfg.pos_enc) { int rc = pack_pos_enc(td, "pe", e->sa_d()); if (rc) return rc; }
-    const int Dp = e->pool_d();        // width of the rows the pooling module reads
-    if (e->cfg.pool == NISQA_POOL_ATT_FF) {
-    const size_t oW1 = P.alloc("pool.w1T", (size_t)nh * Dp * 128), ob1 = P.alloc("pool.b1", nh * 128),
-                 ow2 = P.alloc("pool.w2", nh * 128), ob2 = P.alloc("pool.b2", nh),
-                 ow3 = P.alloc("pool.w3", nh * Dp), ob3 = P.alloc("pool.b3", nh);
+// SkipCNN / DFF (lib:504-583): the BatchNorm2d(1) in front as a scalar affine map (applied by seg_feats_kernel, so
+// that the Linear layers see what the reference's see), Linear layers k-major, DFF's BatchNorm1d folded into them
+bool pack_ffnet(Packer& P, const nisqa_config& c) {
+  const bool dff = c.cnn_kind == NISQA_CNN_DFF;
+  const std::string bn = dff ? "cnn.model.bn1." : "cnn.model.bn.";
+  const TensorView* g = P.get(bn + "weight", {1});
+  const TensorView* be = P.get(bn + "bias", {1});
+  const TensorView* mu = P.get(bn + "running_mean", {1});
+  const TensorView* var = P.get(bn + "running_var", {1});
+  if (!g || !be || !mu || !var) return false;
+  const double a = (double)g->d[0] / sqrt((double)var->d[0] + 1e-5);
+  const size_t o = P.alloc(P.w.ff_bn, 2);
+  P.arena[o] = (float)a; P.arena[o + 1] = (float)((double)be->d[0] - (double)mu->d[0] * a);
+  const int H = c.cnn_fc;
+  if (dff)
+    return pack_ff_linear(P, P.w.ff[0], "lin1", "bn2", 720, 768, H) && pack_ff_linear(P, P.w.ff[1], "lin2", "bn3", H, H, H) &&
+           pack_ff_linear(P, P.w.ff[2], "lin3", "bn4", H, H, H) && pack_ff_linear(P, P.w.ff[3], "lin4", "bn5", H, H, H);
+  return H == 0 || pack_ff_linear(P, P.w.ff[0], "linear", "", 720, 768, H);
+}
+
+// The framewise model: AdaptCNN / StandardCNN (fp32 and tensor-core weights, activation scales) with AdaptCNN's optional
+// Linear, or SkipCNN / DFF
+bool pack_framewise(Packer& P, nisqa_engine* e) {
+  const nisqa_config& c = e->cfg;
+  if (c.cnn_kind != NISQA_CNN_CONV) return pack_ffnet(P, c);
+  const int cin[7] = {0, 1, 16, 32, 64, 64, 64}, cout[7] = {0, 16, 32, 64, 64, 64, 64};
+  for (int i = 1; i <= 6; ++i) {
+    size_t w_off = 0;
+    if (!pack_conv(P, i, cin[i], cout[i], &e->act_exp[i], &w_off)) return false;
+    if (i >= 2) pack_conv_tc(P, i, cin[i], cout[i], w_off, e->act_exp[i - 1], &e->tc_scale[i]);
+  }
+  if (c.cnn_fc > 0) {
+    // AdaptCNN's optional Linear (lib:682-684, 708-709): k-major, rows in the engine's feature order h*64 + c
+    const int H = c.cnn_fc;
+    const TensorView* w = P.get("cnn.model.fc.weight", {H, 384});
+    const TensorView* b = P.get("cnn.model.fc.bias", {H});
+    if (!w || !b) return false;
+    const size_t ow = P.alloc(P.w.ffc.wT, (size_t)384 * H);
+    for (int h = 0; h < 6; ++h)
+      for (int ch = 0; ch < 64; ++ch)
+        for (int j = 0; j < H; ++j) P.arena[ow + ((size_t)h * 64 + ch) * H + j] = w->d[(size_t)j * 384 + ch * 6 + h];
+    P.copy(P.w.ffc.b, b->d, H);
+  }
+  return true;
+}
+
+// One SelfAttention stack (lib:945-1040) of width D and feed-forward width F, checkpoint prefix `ck`: Linear(in -> D) +
+// LayerNorm + `layers` encoder layers.  cnn_order: the input rows are AdaptCNN features in the engine's order.
+bool pack_sa_stack(Packer& P, SaStackWeights& S, const std::string& ck, int in_dim, int layers, bool cnn_order, int D, int F) {
+  const TensorView* lw = P.get(ck + "linear.weight", {D, in_dim});
+  const TensorView* lb = P.get(ck + "linear.bias", {D});
+  const TensorView* ng = P.get(ck + "norm1.weight", {D});
+  const TensorView* nb = P.get(ck + "norm1.bias", {D});
+  if (!lw || !lb || !ng || !nb) return false;
+  const int k_pad = (in_dim + 63) / 64 * 64;
+  const size_t o = P.alloc(S.in.wT, (size_t)k_pad * D);
+  if (cnn_order)      // engine feature order k' = h*64 + c  <->  reference view(-1, 64*6) order c*6 + h (lib:706)
+    pack_linear_chunked(P, o, lw, D, in_dim, k_pad, [](int k) { return (k & 63) * 6 + (k >> 6); });
+  else
+    pack_linear_chunked(P, o, lw, D, in_dim, k_pad, [](int k) { return k; });
+  P.copy(S.in.b, lb->d, D);
+  P.copy(S.ln_g, ng->d, D);
+  P.copy(S.ln_b, nb->d, D);
+  const auto id = [](int k) { return k; };
+  for (int l = 0; l < layers; ++l) {
+    const std::string p = ck + "layers." + std::to_string(l) + ".";
+    const TensorView* iw = P.get(p + "self_attn.in_proj_weight", {3 * D, D});
+    const TensorView* ib = P.get(p + "self_attn.in_proj_bias", {3 * D});
+    const TensorView* ow = P.get(p + "self_attn.out_proj.weight", {D, D});
+    const TensorView* ob = P.get(p + "self_attn.out_proj.bias", {D});
+    const TensorView* w1 = P.get(p + "linear1.weight", {F, D});
+    const TensorView* b1 = P.get(p + "linear1.bias", {F});
+    const TensorView* w2 = P.get(p + "linear2.weight", {D, F});
+    const TensorView* b2 = P.get(p + "linear2.bias", {D});
+    const TensorView* g1 = P.get(p + "norm1.weight", {D});
+    const TensorView* e1 = P.get(p + "norm1.bias", {D});
+    const TensorView* g2 = P.get(p + "norm2.weight", {D});
+    const TensorView* e2 = P.get(p + "norm2.bias", {D});
+    if (!iw || !ib || !ow || !ob || !w1 || !b1 || !w2 || !b2 || !g1 || !e1 || !g2 || !e2) return false;
+    const float qf = q_fold(D);
+    const size_t oq = P.alloc(S.qkv[l].wT, (size_t)3 * D * D);
+    pack_linear_chunked(P, oq, iw, 3 * D, D, D, id);
+    for (size_t i = 0; i < (size_t)D * D; ++i) P.arena[oq + i] *= qf;          // the q chunks come first
+    const size_t oqb = P.alloc(S.qkv[l].b, 3 * D);
+    for (int j = 0; j < 3 * D; ++j) P.arena[oqb + j] = ib->d[j] * (j < D ? qf : 1.f);
+    SaLayerParams& L = S.layer[l];
+    pack_linear_chunked(P, P.alloc(L.WoT, (size_t)D * D), ow, D, D, D, id);
+    P.copy(L.bo, ob->d, D);
+    pack_linear_chunked(P, P.alloc(L.W1T, (size_t)F * D), w1, F, D, D, id);
+    P.copy(L.b1, b1->d, F);
+    pack_linear_chunked(P, P.alloc(L.W2T, (size_t)D * F), w2, D, F, F, id);
+    P.copy(L.b2, b2->d, D);
+    P.copy(L.ln1_g, g1->d, D);
+    P.copy(L.ln1_b, e1->d, D);
+    P.copy(L.ln2_g, g2->d, D);
+    P.copy(L.ln2_b, e2->d, D);
+  }
+  return true;
+}
+
+// the positional encoding of the stack under `ck`: registered buffer [max_len, 1, D] (lib:1051-1058)
+bool pack_pos_enc(Packer& P, const nisqa_config& c, const std::string& ck, SaStackWeights& S, int D) {
+  auto it = P.t.find(ck + "pos_encoder.pe");
+  if (it == P.t.end() || it->second.nd != 3 || it->second.dims[1] != 1 || it->second.dims[2] != D)
+    return P.fail("missing tensor " + ck + "pos_encoder.pe");
+  if (c.max_segments > 0 && it->second.dims[0] < c.max_segments)
+    return P.fail("positional encoding shorter than ms_max_segments");
+  P.copy(S.pe, it->second.d, (size_t)it->second.numel);
+  return true;
+}
+
+// NISQA_DE's learned alignment: AttLuong W = Linear(y_dim -> q_dim) (lib:1348-1351), AttBahdanau Wq, Wy (-> att_dim 128)
+// and v (lib:1329-1337)
+bool pack_de_align(Packer& P, const nisqa_config& c) {
+  DeAlignParams& A = P.w.de;
+  if (c.de_align == NISQA_DE_ALIGN_LUONG) {
+    const TensorView* w = P.get("align.att.W.weight", {64, 64});
+    const TensorView* b = P.get("align.att.W.bias", {64});
+    if (!w || !b) return false;
+    pack_linear_T(P, P.alloc(A.wT, 4096), w, 64, 64);
+    P.copy(A.b, b->d, 64);
+  }
+  if (c.de_align == NISQA_DE_ALIGN_BAHDANAU) {
+    const TensorView* wq = P.get("align.att.Wq.weight", {128, 64});
+    const TensorView* bq = P.get("align.att.Wq.bias", {128});
+    const TensorView* wy = P.get("align.att.Wy.weight", {128, 64});
+    const TensorView* by = P.get("align.att.Wy.bias", {128});
+    const TensorView* v = P.get("align.att.v.weight", {1, 128});
+    if (!wq || !bq || !wy || !by || !v) return false;
+    pack_linear_T(P, P.alloc(A.wqT, 64 * 128), wq, 128, 64);
+    P.copy(A.bq, bq->d, 128);
+    pack_linear_T(P, P.alloc(A.wyT, 64 * 128), wy, 128, 64);
+    P.copy(A.by, by->d, 128);
+    P.copy(A.v, v->d, 128);
+  }
+  return true;
+}
+
+// The pooling module behind self-attention, one head per output (order mos, noi, dis, col, loud: lib:1461-1465), reading
+// Dp-wide rows: PoolAttFF, or PoolAtt / PoolAvg / PoolMax / PoolLastStep
+bool pack_pool_heads(Packer& P, const nisqa_config& c, int Dp) {
+  const int nh = c.n_out;
+  auto prefix = [&](int h) { return nh == 1 ? std::string("pool.model.") : "pool_layers." + std::to_string(h) + ".model."; };
+  if (c.pool == NISQA_POOL_ATT_FF) {
+    PoolHeadParams& H = P.w.pool_head;
+    const size_t oW1 = P.alloc(H.W1T, (size_t)nh * Dp * 128), ob1 = P.alloc(H.b1, nh * 128),
+                 ow2 = P.alloc(H.w2, nh * 128), ob2 = P.alloc(H.b2, nh),
+                 ow3 = P.alloc(H.w3, nh * Dp), ob3 = P.alloc(H.b3, nh);
     for (int h = 0; h < nh; ++h) {
-      const std::string p = head_prefix(h);
+      const std::string p = prefix(h);
       const TensorView* w1 = P.get(p + "linear1.weight", {128, Dp});
       const TensorView* b1 = P.get(p + "linear1.bias", {128});
       const TensorView* w2 = P.get(p + "linear2.weight", {1, 128});
       const TensorView* b2 = P.get(p + "linear2.bias", {1});
       const TensorView* w3 = P.get(p + "linear3.weight", {1, Dp});
       const TensorView* b3 = P.get(p + "linear3.bias", {1});
-      if (!w1 || !b1 || !w2 || !b2 || !w3 || !b3) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
+      if (!w1 || !b1 || !w2 || !b2 || !w3 || !b3) return false;
       pack_linear_T(P, oW1 + (size_t)h * Dp * 128, w1, 128, Dp);          // [head][D][128]
       memcpy(&P.arena[ob1 + h * 128], b1->d, 512);
       memcpy(&P.arena[ow2 + h * 128], w2->d, 512);
@@ -742,64 +709,109 @@ int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
       memcpy(&P.arena[ow3 + h * Dp], w3->d, (size_t)Dp * 4);
       P.arena[ob3 + h] = b3->d[0];
     }
-    } else {
-      // PoolAtt: linear1 (D -> 1 attention logit) + linear2 (D -> 1); PoolAvg / PoolMax / PoolLastStep: linear (D -> 1)
-      const bool att = e->cfg.pool == NISQA_POOL_ATT;
-      const size_t oa1 = P.alloc("pool.a1", nh * Dp), oa1b = P.alloc("pool.a1b", nh),
-                   ow3 = P.alloc("pool.w3", nh * Dp), ob3 = P.alloc("pool.b3", nh);
-      for (int h = 0; h < nh; ++h) {
-        const std::string p = head_prefix(h);
-        const TensorView* a1 = att ? P.get(p + "linear1.weight", {1, Dp}) : nullptr;
-        const TensorView* a1b = att ? P.get(p + "linear1.bias", {1}) : nullptr;
-        const TensorView* w3 = P.get(p + (att ? "linear2.weight" : "linear.weight"), {1, Dp});
-        const TensorView* b3 = P.get(p + (att ? "linear2.bias" : "linear.bias"), {1});
-        if ((att && (!a1 || !a1b)) || !w3 || !b3) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-        if (att) { memcpy(&P.arena[oa1 + h * Dp], a1->d, (size_t)Dp * 4); P.arena[oa1b + h] = a1b->d[0]; }
-        memcpy(&P.arena[ow3 + h * Dp], w3->d, (size_t)Dp * 4);
-        P.arena[ob3 + h] = b3->d[0];
-      }
-    }
-  } else {
-    const TensorView* fw = P.get("cnn.model.fc_out.weight", {20, 768});
-    const TensorView* fb = P.get("cnn.model.fc_out.bias", {20});
-    if (!fw || !fb) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-    size_t o = P.alloc("fc.wT", 768 * 20);
-    // engine order k' = (h*2 + w)*64 + c  <->  reference view order c*12 + h*2 + w (lib:830)
-    for (int hw = 0; hw < 12; ++hw)
-      for (int c = 0; c < 64; ++c)
-        for (int j = 0; j < 20; ++j) P.arena[o + ((size_t)hw * 64 + c) * 20 + j] = fw->d[(size_t)j * 768 + c * 12 + hw];
-    o = P.alloc("fc.b", 32); memcpy(&P.arena[o], fb->d, 80);
-    const std::string p = "time_dependency.model.lstm.";
-    const size_t owi = P.alloc("lstm.wih", 2 * 512 * 20), owh = P.alloc("lstm.whh", 2 * 512 * 128),
-                 obb = P.alloc("lstm.b", 2 * 512);
-    for (int d = 0; d < 2; ++d) {
-      const std::string sfx = d ? "_reverse" : "";
-      const TensorView* wi = P.get(p + "weight_ih_l0" + sfx, {512, 20});
-      const TensorView* wh = P.get(p + "weight_hh_l0" + sfx, {512, 128});
-      const TensorView* bi = P.get(p + "bias_ih_l0" + sfx, {512});
-      const TensorView* bh = P.get(p + "bias_hh_l0" + sfx, {512});
-      if (!wi || !wh || !bi || !bh) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-      memcpy(&P.arena[owi + (size_t)d * 512 * 20], wi->d, 512 * 20 * 4);
-      memcpy(&P.arena[owh + (size_t)d * 512 * 128], wh->d, 512 * 128 * 4);
-      for (int g = 0; g < 512; ++g) P.arena[obb + d * 512 + g] = bi->d[g] + bh->d[g];
-    }
-    const TensorView* pw = P.get("pool.model.linear.weight", {1, 256});      // every pooling module of this arch: Linear(256 -> 1)
-    const TensorView* pb = P.get("pool.model.linear.bias", {1});
-    if (!pw || !pb) return fail(e, NISQA_ERR_WEIGHTS, P.missing);
-    o = P.alloc("lastbi.w", 256); memcpy(&P.arena[o], pw->d, 1024);
-    e->pool_bias_std = pb->d[0];
-    o = P.alloc("pool.w3", 256); memcpy(&P.arena[o], pw->d, 1024);
-    o = P.alloc("pool.b3", 1); P.arena[o] = pb->d[0];
-    P.alloc("pool.a1", 1); P.alloc("pool.a1b", 1);
+    return true;
   }
-  // conv1 is stored as [tap][16]: same as the generic [ci=1][tap][cout] packing.
-  CK(e->warena.reserve(P.arena.size() * 4));
-  CK(cudaMemcpy(e->warena.p, P.arena.data(), P.arena.size() * 4, cudaMemcpyHostToDevice));
-  return 0;
+  // PoolAtt: linear1 (D -> 1 attention logit) + linear2 (D -> 1); PoolAvg / PoolMax / PoolLastStep: linear (D -> 1)
+  PoolSimpleParams& Q = P.w.pool_simple;
+  const bool att = c.pool == NISQA_POOL_ATT;
+  const size_t oa1 = att ? P.alloc(Q.a1, nh * Dp) : 0, oa1b = att ? P.alloc(Q.a1b, nh) : 0;
+  const size_t ow3 = P.alloc(Q.w3, nh * Dp), ob3 = P.alloc(Q.b3, nh);
+  for (int h = 0; h < nh; ++h) {
+    const std::string p = prefix(h);
+    const TensorView* a1 = att ? P.get(p + "linear1.weight", {1, Dp}) : nullptr;
+    const TensorView* a1b = att ? P.get(p + "linear1.bias", {1}) : nullptr;
+    const TensorView* w3 = P.get(p + (att ? "linear2.weight" : "linear.weight"), {1, Dp});
+    const TensorView* b3 = P.get(p + (att ? "linear2.bias" : "linear.bias"), {1});
+    if ((att && (!a1 || !a1b)) || !w3 || !b3) return false;
+    if (att) { memcpy(&P.arena[oa1 + h * Dp], a1->d, (size_t)Dp * 4); P.arena[oa1b + h] = a1b->d[0]; }
+    memcpy(&P.arena[ow3 + h * Dp], w3->d, (size_t)Dp * 4);
+    P.arena[ob3 + h] = b3->d[0];
+  }
+  return true;
 }
 
-const float* W(nisqa_engine* e, const std::string& key) {
-  return e->warena.as<float>() + e->woff.at(key);
+// The self-attention architecture behind the framewise model: time_dependency, then (NISQA_DE's fusion and alignment, or
+// NISQA / NISQA_DIM's second stack) time_dependency_2, and the pooling module
+bool pack_sa_model(Packer& P, nisqa_engine* e) {
+  const nisqa_config& c = e->cfg;
+  const std::string td = "time_dependency.model.", td2 = "time_dependency_2.model.";
+  // framewise features feeding the first stack: 384 (AdaptCNN, engine order), 720 (SkipCNN without Linear: padded to 768
+  // with zero rows) or cnn_fc_out_h
+  const bool conv_net = c.cnn_kind == NISQA_CNN_CONV;
+  const int feat_dim = c.cnn_fc > 0 ? c.cnn_fc : (conv_net ? 384 : 720);
+  if (!pack_sa_stack(P, P.w.sa[0], td, feat_dim, c.sa_layers, conv_net && c.cnn_fc == 0, e->sa_d(), e->sa_f())) return false;
+  if (c.double_ended || c.td2_layers > 0) {
+    // time_dependency_2: behind the fusion of the double-ended model (input 192 / 128), or a second stack behind the
+    // first one in NISQA / NISQA_DIM (lib:114-141, 236-268; input: the first stack's width)
+    int fdim = !c.double_ended ? e->sa_d() : (c.de_fuse == NISQA_DE_FUSE_XY_MINUS ? 192 : 128);
+    if (c.double_ended && c.de_fuse_dim > 0) {        // Fusion.lin_fusion (lib:1399-1401)
+      const int D = c.de_fuse_dim;
+      const TensorView* w = P.get("fuse.lin_fusion.weight", {D, fdim});
+      const TensorView* b = P.get("fuse.lin_fusion.bias", {D});
+      if (!w || !b) return false;
+      pack_linear_T(P, P.alloc(P.w.defuse.wT, (size_t)fdim * D), w, D, fdim);
+      P.copy(P.w.defuse.b, b->d, D);
+      fdim = D;
+    }
+    if (!pack_sa_stack(P, P.w.sa[1], td2, fdim, c.td2_layers, false, e->td2_d(), e->td2_f())) return false;
+    if (c.td2_pos_enc && !pack_pos_enc(P, c, td2, P.w.sa[1], e->td2_d())) return false;
+    if (!pack_de_align(P, c)) return false;
+  }
+  if (c.pos_enc && !pack_pos_enc(P, c, td, P.w.sa[0], e->sa_d())) return false;
+  return pack_pool_heads(P, c, e->pool_d());
+}
+
+// The StandardCNN architecture behind the convolutions: fc_out 768 -> 20, the BiLSTM and its pooling module
+bool pack_lstm_model(Packer& P, nisqa_engine* e) {
+  const TensorView* fw = P.get("cnn.model.fc_out.weight", {20, 768});
+  const TensorView* fb = P.get("cnn.model.fc_out.bias", {20});
+  if (!fw || !fb) return false;
+  const size_t o = P.alloc(P.w.fc.wT, 768 * 20);
+  // engine order k' = (h*2 + w)*64 + c  <->  reference view order c*12 + h*2 + w (lib:830)
+  for (int hw = 0; hw < 12; ++hw)
+    for (int c = 0; c < 64; ++c)
+      for (int j = 0; j < 20; ++j) P.arena[o + ((size_t)hw * 64 + c) * 20 + j] = fw->d[(size_t)j * 768 + c * 12 + hw];
+  memcpy(&P.arena[P.alloc(P.w.fc.b, 32)], fb->d, 80);
+  const std::string p = "time_dependency.model.lstm.";
+  LstmParams& L = P.w.lstm;
+  const size_t owi = P.alloc(L.w_ih, 2 * 512 * 20), owh = P.alloc(L.w_hh, 2 * 512 * 128), obb = P.alloc(L.b, 2 * 512);
+  for (int d = 0; d < 2; ++d) {
+    const std::string sfx = d ? "_reverse" : "";
+    const TensorView* wi = P.get(p + "weight_ih_l0" + sfx, {512, 20});
+    const TensorView* wh = P.get(p + "weight_hh_l0" + sfx, {512, 128});
+    const TensorView* bi = P.get(p + "bias_ih_l0" + sfx, {512});
+    const TensorView* bh = P.get(p + "bias_hh_l0" + sfx, {512});
+    if (!wi || !wh || !bi || !bh) return false;
+    memcpy(&P.arena[owi + (size_t)d * 512 * 20], wi->d, 512 * 20 * 4);
+    memcpy(&P.arena[owh + (size_t)d * 512 * 128], wh->d, 512 * 128 * 4);
+    for (int g = 0; g < 512; ++g) P.arena[obb + d * 512 + g] = bi->d[g] + bh->d[g];
+  }
+  const TensorView* pw = P.get("pool.model.linear.weight", {1, 256});      // every pooling module of this arch: Linear(256 -> 1)
+  const TensorView* pb = P.get("pool.model.linear.bias", {1});
+  if (!pw || !pb) return false;
+  P.copy(L.w_pool, pw->d, 256);
+  e->pool_bias_std = pb->d[0];
+  P.copy(P.w.pool_simple.w3, pw->d, 256);
+  P.copy(P.w.pool_simple.b3, pb->d, 1);
+  return true;
+}
+
+int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
+  Packer P;
+  for (int i = 0; i < n; ++i) {
+    if (!tensors[i].name || !tensors[i].data) continue;
+    TensorView v; v.d = tensors[i].data; v.nd = tensors[i].ndim; v.numel = 1;
+    for (int d = 0; d < 4; ++d) { v.dims[d] = d < v.nd ? tensors[i].dims[d] : 1; v.numel *= v.dims[d]; }
+    P.t[tensors[i].name] = v;
+  }
+  const bool ok = pack_framewise(P, e) &&
+                  (e->cfg.arch == NISQA_ARCH_ADAPT_SA_ATTFF ? pack_sa_model(P, e) : pack_lstm_model(P, e));
+  if (!ok) return fail(e, NISQA_ERR_WEIGHTS, P.err);
+  CK(e->warena.reserve(P.arena.size() * 4));
+  CK(cudaMemcpy(e->warena.p, P.arena.data(), P.arena.size() * 4, cudaMemcpyHostToDevice));
+  for (auto& s : P.slots) *s.first = e->warena.as<float>() + s.second;
+  e->w = P.w;
+  return 0;
 }
 
 // ---------------------------------------------------------------- one pass over a run of clips
@@ -818,330 +830,374 @@ struct PassInput {
 
 int lane_allgather(nisqa_engine* e, const float* src, float* dst, size_t count, cudaStream_t st);
 
-int run_pass(nisqa_engine* e, const PassInput& in) {
-  const nisqa_config& c = e->cfg;
-  const int n = in.n_clips;
-  const int std_mode = c.arch == NISQA_ARCH_STD_LSTM_LASTBI;
-  const size_t esz = in.fmt == NISQA_FMT_F32 ? 4 : 2;
-  // ---- tables
+// A pass while it is enqueued: where it runs, its device tables and its sizes
+struct Pass {
+  nisqa_engine* e;
+  const nisqa_config& c;
+  const Weights& w;
+  Lane& LN;                    // compute lane: stream and activation workspaces
+  Stage& SG;                   // staging slot: tables and PCM
+  cudaStream_t st;
+  bool std_mode;
+  float* scores;               // [n][n_out]
+  int n;
+  int n_frames = 0, n_seg = 0, n_qt64 = 0, max_n_seg = 0;
+  int max_pairs = 0, Q = 1, max_span = 0;     // launch shape of the front end
+  const void* pcm = nullptr;                  // packed PCM on the device
+  const ClipDesc* clips = nullptr;            // device tables (staging slot)
+  unsigned* clipmax = nullptr;
+  const int* seg_prefix = nullptr;
+  const int* qt64_prefix = nullptr;
+  const int* by_len = nullptr;
+  int* seg_frame0 = nullptr;                  // segment table (lane, seg_table_kernel)
+  float* seg_thr = nullptr;
+  int* seg_clip = nullptr;
+  Pass(nisqa_engine* e_, const PassInput& in)
+      : e(e_), c(e_->cfg), w(e_->w), LN(e_->lanes[in.slot]), SG(e_->stages[in.stage]), st(LN.stream),
+        std_mode(c.arch == NISQA_ARCH_STD_LSTM_LASTBI), scores(in.scores_dev_out), n(in.n_clips) {}
+};
+
+// [n_seg][64 nk] rows that feed a time-dependency block
+struct Rows { const float* x; int nk; };
+
+// The pass's host tables - ClipDesc rows, prefix sums of frame pairs, segments, 128- and 64-row query tiles, the clips by
+// decreasing length (batched BiLSTM groups) - and, when it has segments, its PCM: uploaded on the copy stream, which the
+// lane's stream then waits for
+int upload_inputs(Pass& p, const PassInput& in) {
+  nisqa_engine* e = p.e;
+  const nisqa_config& c = p.c;
+  const int n = p.n;
   std::vector<ClipDesc>& cl = e->last_clips;
   cl.assign(n, ClipDesc());
-  std::vector<int> pair_prefix(n + 1, 0), seg_prefix(n + 1, 0), qt_prefix(n + 1, 0), qt64_prefix(n + 1, 0), by_len(n + 1, 0);
+  const size_t np = (size_t)n + 1;
+  std::vector<int> pre(5 * np, 0);             // pair | seg | qt | qt64 prefixes | by_len, [n + 1] each
+  int* pair_prefix = &pre[0]; int* seg_prefix = &pre[np]; int* qt_prefix = &pre[2 * np]; int* qt64_prefix = &pre[3 * np];
+  int* by_len = &pre[4 * np];
   long long pcm_elems = 0;
-  int n_frames = 0, n_seg = 0, n_pairs = 0, n_qt = 0, n_qt64 = 0, Q = 1, max_pairs = 0, max_span = 0, max_n_seg = 0;
+  int n_pairs = 0, n_qt = 0;
   for (int i = 0; i < n; ++i) {
-    const ClipPlan& p = in.plan[i];
+    const ClipPlan& pl = in.plan[i];
     ClipDesc& d = cl[i];
-    const bool ok = p.run != 0;
+    const bool ok = pl.run != 0;
     d.n_samples = (int)in.n_samples[i];
-    d.fb_id = ok ? p.fb_id : 0;
-    d.hop = p.hop; d.win = p.win;
-    d.s0 = (c.n_fft - p.win) / 2 - c.n_fft / 2;      // pad_center lpad minus the reflect pad
-    d.n_frames = ok ? p.n_frames : 0;
-    d.n_seg = ok ? p.n_seg : 0;
-    d.frame_off = n_frames; d.seg_off = n_seg; d.pair_off = n_pairs;
+    d.fb_id = ok ? pl.fb_id : 0;
+    d.hop = pl.hop; d.win = pl.win;
+    d.s0 = (c.n_fft - pl.win) / 2 - c.n_fft / 2;      // pad_center lpad minus the reflect pad
+    d.n_frames = ok ? pl.n_frames : 0;
+    d.n_seg = ok ? pl.n_seg : 0;
+    d.frame_off = p.n_frames; d.seg_off = p.n_seg; d.pair_off = n_pairs;
     if (in.host_pcm) { d.pcm_off = pcm_elems; pcm_elems += ((long long)in.n_samples[i] + 15) / 16 * 16; }
     else d.pcm_off = in.dev_off[i];
-    pair_prefix[i] = n_pairs; seg_prefix[i] = n_seg; qt_prefix[i] = n_qt; qt64_prefix[i] = n_qt64;
-    n_frames += d.n_frames; n_seg += d.n_seg;
+    pair_prefix[i] = n_pairs; seg_prefix[i] = p.n_seg; qt_prefix[i] = n_qt; qt64_prefix[i] = p.n_qt64;
+    p.n_frames += d.n_frames; p.n_seg += d.n_seg;
     n_pairs += (d.n_frames + 1) / 2;
-    max_pairs = std::max(max_pairs, (d.n_frames + 1) / 2);
+    p.max_pairs = std::max(p.max_pairs, (d.n_frames + 1) / 2);
     n_qt += (d.n_seg + 127) / 128;
-    n_qt64 += (d.n_seg + 63) / 64;
-    max_n_seg = std::max(max_n_seg, d.n_seg);
-    if (ok) { Q = std::max(Q, (p.win + 1023) / 1024); max_span = std::max(max_span, p.hop + p.win); }
+    p.n_qt64 += (d.n_seg + 63) / 64;
+    p.max_n_seg = std::max(p.max_n_seg, d.n_seg);
+    if (ok) { p.Q = std::max(p.Q, (pl.win + 1023) / 1024); p.max_span = std::max(p.max_span, pl.hop + pl.win); }
   }
-  pair_prefix[n] = n_pairs; seg_prefix[n] = n_seg; qt_prefix[n] = n_qt; qt64_prefix[n] = n_qt64;
-  for (int i = 0; i < n; ++i) by_len[i] = i;          // clips by decreasing length (batched BiLSTM groups)
-  std::stable_sort(by_len.begin(), by_len.begin() + n, [&](int a, int b) { return cl[a].n_seg > cl[b].n_seg; });
-  e->last_n_seg = n_seg; e->last_n_frames = n_frames;
-  const int n_out = c.n_out;
+  pair_prefix[n] = n_pairs; seg_prefix[n] = p.n_seg; qt_prefix[n] = n_qt; qt64_prefix[n] = p.n_qt64;
+  for (int i = 0; i < n; ++i) by_len[i] = i;
+  std::stable_sort(by_len, by_len + n, [&](int a, int b) { return cl[a].n_seg > cl[b].n_seg; });
+  e->last_n_seg = p.n_seg; e->last_n_frames = p.n_frames;
 
-  float* scores = in.scores_dev_out;
-  Lane& LN = e->lanes[in.slot];
-  Stage& SG = e->stages[in.stage];
-  cudaStream_t st = LN.stream, cs = e->copy_stream;
-  e->cur_stream = st;
   // the staging slot (pinned tables, device tables, PCM buffer) is reused every kStages-th pass; the
   // lane's activation workspaces are protected by stream order alone
+  Stage& SG = p.SG;
+  cudaStream_t cs = e->copy_stream;
   if (SG.busy) { CK(cudaEventSynchronize(SG.ev_done)); SG.busy = false; }
   SG.lane = in.slot;
-
-  // ---- upload tables (one pinned block: ClipDesc[n] | 4 prefix arrays | clips by length)
-  const size_t tb_clips = (size_t)n * sizeof(ClipDesc);
-  const size_t tb_pref = (size_t)(n + 1) * 4;
-  CK(SG.h_tables.reserve(tb_clips + 5 * tb_pref));
+  // one pinned block: ClipDesc[n] | the prefix arrays
+  const size_t tb_clips = (size_t)n * sizeof(ClipDesc), tb_pref = pre.size() * 4;
+  CK(SG.h_tables.reserve(tb_clips + tb_pref));
   char* ht = SG.h_tables.as<char>();
   memcpy(ht, cl.data(), tb_clips);
-  memcpy(ht + tb_clips, pair_prefix.data(), tb_pref);
-  memcpy(ht + tb_clips + tb_pref, seg_prefix.data(), tb_pref);
-  memcpy(ht + tb_clips + 2 * tb_pref, qt_prefix.data(), tb_pref);
-  memcpy(ht + tb_clips + 3 * tb_pref, qt64_prefix.data(), tb_pref);
-  memcpy(ht + tb_clips + 4 * tb_pref, by_len.data(), tb_pref);
+  memcpy(ht + tb_clips, pre.data(), tb_pref);
   CK(SG.clips.reserve(tb_clips));
-  CK(SG.prefixes.reserve(5 * tb_pref));
+  CK(SG.prefixes.reserve(tb_pref));
   CK(SG.clipmax.reserve((size_t)n * 4));
   CK(cudaMemcpyAsync(SG.clips.p, ht, tb_clips, cudaMemcpyHostToDevice, cs));
-  CK(cudaMemcpyAsync(SG.prefixes.p, ht + tb_clips, 5 * tb_pref, cudaMemcpyHostToDevice, cs));
+  CK(cudaMemcpyAsync(SG.prefixes.p, ht + tb_clips, tb_pref, cudaMemcpyHostToDevice, cs));
   CK(cudaMemsetAsync(SG.clipmax.p, 0, (size_t)n * 4, cs));
-  const ClipDesc* d_clips = SG.clips.as<ClipDesc>();
-  unsigned* d_clipmax = SG.clipmax.as<unsigned>();
-  const int* d_pair = SG.prefixes.as<int>();
-  (void)d_pair;
+  p.clips = SG.clips.as<ClipDesc>();
+  p.clipmax = SG.clipmax.as<unsigned>();
+  p.seg_prefix = SG.prefixes.as<int>() + np;
+  p.qt64_prefix = SG.prefixes.as<int>() + 3 * np;
+  p.by_len = SG.prefixes.as<int>() + 4 * np;
   e->last_lane = in.slot;
   e->last_stage = in.stage;
-  const int* d_seg = d_pair + (n + 1);
-  const int* d_qt = d_pair + 2 * (n + 1);
-  const int* d_qt64 = d_pair + 3 * (n + 1);
-  const int* d_by_len = d_pair + 4 * (n + 1);
 
-  if (n_seg == 0) {   // nothing valid in this pass: NaN scores
-    CK(cudaEventRecord(SG.ev_copied, cs));
-    CK(cudaStreamWaitEvent(st, SG.ev_copied, 0));
-    CK(cudaMemsetAsync(scores, 0xFF, (size_t)n * n_out * 4, st));
+  p.pcm = in.dev_pcm;
+  if (p.n_seg > 0 && in.host_pcm) {
+    const size_t esz = in.fmt == NISQA_FMT_F32 ? 4 : 2;
+    CK(SG.pcm.reserve((size_t)pcm_elems * esz));
+    // clips that are back to back in host memory with the same 16-element alignment as the
+    // device packing travel as ONE copy (a pinned batch buffer becomes a single large DMA)
+    for (int i = 0; i < n;) {
+      if (cl[i].n_frames <= 0) { ++i; continue; }
+      const char* h0 = static_cast<const char*>(in.host_pcm[i]);
+      const long long o0 = cl[i].pcm_off;
+      size_t bytes = (size_t)in.n_samples[i] * esz;
+      int j = i + 1;
+      while (j < n && cl[j].n_frames > 0 &&
+             static_cast<const char*>(in.host_pcm[j]) == h0 + (size_t)(cl[j].pcm_off - o0) * esz) {
+        bytes = (size_t)(cl[j].pcm_off - o0) * esz + (size_t)in.n_samples[j] * esz;
+        ++j;
+      }
+      CK(cudaMemcpyAsync(SG.pcm.as<char>() + (size_t)o0 * esz, h0, bytes, cudaMemcpyHostToDevice, cs));
+      i = j;
+    }
+    p.pcm = SG.pcm.p;
+  }
+  CK(cudaEventRecord(SG.ev_copied, cs));
+  CK(cudaStreamWaitEvent(p.st, SG.ev_copied, 0));
+  return 0;
+}
+
+// AdaptCNN / StandardCNN: conv1 (fused with conv2 on the tensor-core path), then conv2..conv6 on fp16 plane pairs
+// (conv_split.cu) or as fp32 FFMA convolutions (cnn.cu); conv6 writes the features to LN.feats
+void conv_layers(Pass& p) {
+  nisqa_engine* e = p.e;
+  Lane& LN = p.LN;
+  const Weights& w = p.w;
+  const bool split = e->conv_tc != 0, fused12 = split && e->conv12;
+  auto plane_hi = [&](int l) { return LN.planes[l].as<char>(); };
+  auto plane_lo = [&](int l) { return LN.planes[l].as<char>() + LN.plane_bytes[l]; };
+  if (fused12) {
+    Scope s(e, "conv12");
+    launch_conv12(p.st, p.std_mode, LN.mel.as<float>(), p.seg_frame0, p.seg_thr, w.conv[1].w, w.conv[1].b,
+                  e->act_store(1), w.conv[2].wtc, w.conv[2].b, e->tc_scale[2], e->act_store(2),
+                  plane_hi(3), plane_lo(3), p.n_seg);
   } else {
-    // ---- PCM (copy stream), then hand over to the compute stream
-    const void* d_pcm = in.dev_pcm;
-    if (in.host_pcm) {
-      CK(SG.pcm.reserve((size_t)pcm_elems * esz));
-      // clips that are back to back in host memory with the same 16-element alignment as the
-      // device packing travel as ONE copy (a pinned batch buffer becomes a single large DMA)
-      for (int i = 0; i < n;) {
-        if (cl[i].n_frames <= 0) { ++i; continue; }
-        const char* h0 = static_cast<const char*>(in.host_pcm[i]);
-        const long long o0 = cl[i].pcm_off;
-        size_t bytes = (size_t)in.n_samples[i] * esz;
-        int j = i + 1;
-        while (j < n && cl[j].n_frames > 0 &&
-               static_cast<const char*>(in.host_pcm[j]) == h0 + (size_t)(cl[j].pcm_off - o0) * esz) {
-          bytes = (size_t)(cl[j].pcm_off - o0) * esz + (size_t)in.n_samples[j] * esz;
-          ++j;
-        }
-        CK(cudaMemcpyAsync(SG.pcm.as<char>() + (size_t)o0 * esz, h0, bytes, cudaMemcpyHostToDevice, cs));
-        i = j;
-      }
-      d_pcm = SG.pcm.p;
-    }
-    CK(cudaEventRecord(SG.ev_copied, cs));
-    CK(cudaStreamWaitEvent(st, SG.ev_copied, 0));
-    // ---- workspaces
-    const int W1 = std_mode ? 8 : 7, W2 = std_mode ? 4 : 5, W3 = std_mode ? 2 : 3;
-    const int FEAT = std_mode ? 768 : 384;
-    CK(LN.mel.reserve((size_t)n_frames * kMels * 4));
-    CK(LN.segtab.reserve((size_t)n_seg * 12));
-    const bool split = e->conv_tc != 0;
-    e->last_split = split;
-    const bool conv_net = c.cnn_kind == NISQA_CNN_CONV;
-    if (!conv_net) {
-    } else if (split) {
-      for (int l = (e->conv12 ? 3 : 2); l <= 6; ++l) {
-        // the lo plane sits at a fixed offset of the ALLOCATION (not of this pass's n_seg): the zero rows /
-        // columns of both planes must stay where they were when the buffer was cleared
-        CK(LN.planes[l].reserve_zeroed(2 * split_plane_bytes(std_mode, l, n_seg), st));
-        LN.plane_bytes[l] = (LN.planes[l].cap / 2) & ~(size_t)1023;
-      }
-    } else {
-      CK(LN.act1.reserve((size_t)n_seg * 24 * W1 * 16 * 4));
-      CK(LN.act2.reserve((size_t)n_seg * 12 * W2 * 32 * 4));
-      CK(LN.act3.reserve((size_t)n_seg * 12 * W2 * 64 * 4));
-      CK(LN.act4.reserve((size_t)n_seg * 6 * W3 * 64 * 4));
-      CK(LN.act5.reserve((size_t)n_seg * 6 * W3 * 64 * 4));
-    }
-    CK(LN.feats.reserve((size_t)n_seg * FEAT * 4));
-    int* seg_frame0 = LN.segtab.as<int>();
-    float* seg_thr = reinterpret_cast<float*>(seg_frame0 + n_seg);
-    int* seg_clip = seg_frame0 + 2 * (size_t)n_seg;
+    Scope s(e, "conv1");
+    launch_conv1(p.st, p.std_mode, LN.mel.as<float>(), p.seg_frame0, p.seg_thr, w.conv[1].w,
+                 w.conv[1].b, split ? nullptr : LN.act[2].as<float>(), p.n_seg,
+                 split ? plane_hi(2) : nullptr, split ? plane_lo(2) : nullptr, e->act_store(1));
+  }
+  static const char* const names[7] = {"", "", "conv2", "conv3", "conv4", "conv5", "conv6"};
+  for (int l = fused12 ? 3 : 2; l <= 6; ++l) {
+    Scope s(e, names[l]);
+    if (split)
+      launch_conv_split(p.st, p.std_mode, l, plane_hi(l), plane_lo(l), w.conv[l].wtc, w.conv[l].b, e->tc_scale[l],
+                        e->act_store(l), l < 6 ? plane_hi(l + 1) : nullptr, l < 6 ? plane_lo(l + 1) : nullptr,
+                        l == 6 ? LN.feats.as<float>() : nullptr, p.n_seg);
+    else
+      launch_conv_layer(p.st, p.std_mode, l, LN.act[l].as<float>(), w.conv[l].w, w.conv[l].b,
+                        l < 6 ? LN.act[l + 1].as<float>() : LN.feats.as<float>(), p.n_seg);
+  }
+}
 
-    { Scope s(e, "frontend");
-      launch_frontend(st, d_pcm, in.fmt == NISQA_FMT_F32, d_clips, n, max_pairs,
-                      e->fb_table.as<FbTables>(), e->tw4096.as<float2>(), LN.mel.as<float>(),
-                      d_clipmax, Q, max_span, e->fe_ppc); }
-    { Scope s(e, "seg_table");
-      launch_seg_table(st, d_clips, n, d_seg, d_clipmax, c.seg_hop, n_seg,
-                       seg_frame0, seg_thr, seg_clip); }
-    auto plane_hi = [&](int l) { return LN.planes[l].as<char>(); };
-    auto plane_lo = [&](int l) { return LN.planes[l].as<char>() + LN.plane_bytes[l]; };
-    const bool fused12 = split && e->conv12;
-    e->last_conv12 = fused12;
-    const float* sa_in = LN.feats.as<float>();       // rows fed to the first self-attention stack
-    int sa_nk = 6;                                   // ... in 64-wide chunks
-    if (!conv_net) {
-      // SkipCNN / DFF (lib:504-583): BN + flatten (+ Linear layers), no convolution
-      Scope s(e, "framewise", 5);
-      const int H = c.cnn_fc;
-      CK(LN.ffa.reserve((size_t)n_seg * std::max(768, H) * 4));
-      launch_seg_feats(st, LN.mel.as<float>(), seg_frame0, seg_thr, W(e, "ff.bn"), n_seg, LN.ffa.as<float>());
-      sa_in = LN.ffa.as<float>(); sa_nk = 12;
-      if (H > 0) {
-        CK(LN.ffb.reserve((size_t)n_seg * H * 4));
-        const bool dff = c.cnn_kind == NISQA_CNN_DFF;
-        launch_linear_tile(st, LN.ffa.as<float>(), 768, W(e, "ff1.wT"), W(e, "ff1.b"), dff, LN.ffb.as<float>(), H, n_seg, 768, H);
-        sa_in = LN.ffb.as<float>(); sa_nk = H / 64;
-        if (dff) {
-          float* pp2[2] = {LN.ffa.as<float>(), LN.ffb.as<float>()};
-          const char* keys[3] = {"ff2", "ff3", "ff4"};
-          for (int l = 0; l < 3; ++l)       // ffb -> ffa -> ffb -> ffa
-            launch_linear_tile(st, pp2[(l + 1) & 1], H, W(e, std::string(keys[l]) + ".wT"), W(e, std::string(keys[l]) + ".b"), 1,
-                               pp2[l & 1], H, n_seg, H, H);
-          sa_in = LN.ffa.as<float>();
-        }
-      }
-    } else if (fused12) {
-      Scope s(e, "conv12");
-      launch_conv12(st, std_mode, LN.mel.as<float>(), seg_frame0, seg_thr, W(e, "conv1.w"), W(e, "conv1.b"),
-                    e->act_store(1), W(e, "conv2.wtc"), W(e, "conv2.b"), e->tc_scale[2], e->act_store(2),
-                    plane_hi(3), plane_lo(3), n_seg);
-    } else {
-      Scope s(e, "conv1");
-      launch_conv1(st, std_mode, LN.mel.as<float>(), seg_frame0, seg_thr, W(e, "conv1.w"),
-                   W(e, "conv1.b"), split ? nullptr : LN.act1.as<float>(), n_seg,
-                   split ? plane_hi(2) : nullptr, split ? plane_lo(2) : nullptr, e->act_store(1));
-    }
-    if (conv_net) {
-      const float* cin_[7] = {nullptr, nullptr, LN.act1.as<float>(), LN.act2.as<float>(), LN.act3.as<float>(),
-                              LN.act4.as<float>(), LN.act5.as<float>()};
-      float* cout_[7] = {nullptr, nullptr, LN.act2.as<float>(), LN.act3.as<float>(), LN.act4.as<float>(),
-                         LN.act5.as<float>(), LN.feats.as<float>()};
-      for (int l = fused12 ? 3 : 2; l <= 6; ++l) {
-        char nm[16], kw[24], kt[24], kb[24];
-        snprintf(nm, sizeof nm, "conv%d", l); snprintf(kw, sizeof kw, "conv%d.w", l);
-        snprintf(kt, sizeof kt, "conv%d.wtc", l); snprintf(kb, sizeof kb, "conv%d.b", l);
-        Scope s(e, nm);
-        if (split)
-          launch_conv_split(st, std_mode, l, plane_hi(l), plane_lo(l), W(e, kt), W(e, kb), e->tc_scale[l],
-                            e->act_store(l), l < 6 ? plane_hi(l + 1) : nullptr, l < 6 ? plane_lo(l + 1) : nullptr,
-                            l == 6 ? LN.feats.as<float>() : nullptr, n_seg);
-        else
-          launch_conv_layer(st, std_mode, l, cin_[l], W(e, kw), W(e, kb), cout_[l], n_seg);
-      }
-    }
+// SkipCNN / DFF (lib:504-583): BN + flatten (+ Linear layers), no convolution
+int ff_layers(Pass& p, Rows* out) {
+  nisqa_engine* e = p.e;
+  Lane& LN = p.LN;
+  const Weights& w = p.w;
+  Scope s(e, "framewise", 5);
+  const int H = p.c.cnn_fc, n_seg = p.n_seg;
+  CK(LN.ffa.reserve((size_t)n_seg * std::max(768, H) * 4));
+  float* ffa = LN.ffa.as<float>();
+  launch_seg_feats(p.st, LN.mel.as<float>(), p.seg_frame0, p.seg_thr, w.ff_bn, n_seg, ffa);
+  *out = {ffa, 12};
+  if (H == 0) return 0;
+  CK(LN.ffb.reserve((size_t)n_seg * H * 4));
+  float* ffb = LN.ffb.as<float>();
+  const bool dff = p.c.cnn_kind == NISQA_CNN_DFF;
+  launch_linear_tile(p.st, ffa, 768, w.ff[0].wT, w.ff[0].b, dff, ffb, H, n_seg, 768, H);
+  *out = {ffb, H / 64};
+  if (!dff) return 0;
+  float* pp[2] = {ffa, ffb};
+  for (int l = 1; l <= 3; ++l)       // ffb -> ffa -> ffb -> ffa
+    launch_linear_tile(p.st, pp[l & 1], H, w.ff[l].wT, w.ff[l].b, 1, pp[(l + 1) & 1], H, n_seg, H, H);
+  *out = {ffa, H / 64};
+  return 0;
+}
 
-    if (conv_net && c.cnn_fc > 0) {      // AdaptCNN's Linear behind conv6 (lib:708-709)
-      Scope s(e, "framewise");
-      CK(LN.ffb.reserve((size_t)n_seg * c.cnn_fc * 4));
-      launch_linear_tile(st, LN.feats.as<float>(), 384, W(e, "ffc.wT"), W(e, "ffc.b"), 0, LN.ffb.as<float>(), c.cnn_fc, n_seg, 384, c.cnn_fc);
-      sa_in = LN.ffb.as<float>(); sa_nk = c.cnn_fc / 64;
-    }
-    if (!std_mode) {
-      const int D1 = e->sa_d(), D2 = c.td2_layers > 0 ? e->td2_d() : 0, Dm = std::max(D1, D2);
-      CK(LN.xa.reserve((size_t)n_seg * Dm * 4));
-      CK(LN.xb.reserve((size_t)n_seg * Dm * 4));
-      CK(LN.qkv.reserve((size_t)n_seg * 3 * Dm * 4));
-      CK(LN.logits.reserve((size_t)n_seg * n_out * 4));
-      CK(LN.tdout.reserve((size_t)n_seg * D1 * 4));
-      const bool attff = c.pool == NISQA_POOL_ATT_FF;
-      PoolHeadParams H = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-      if (attff) {
-        H.W1T = W(e, "pool.w1T"); H.b1 = W(e, "pool.b1"); H.w2 = W(e, "pool.w2"); H.b2 = W(e, "pool.b2");
-      }
-      H.w3 = W(e, "pool.w3"); H.b3 = W(e, "pool.b3");
-      e->last_td_in = LN.tdout.as<float>();
-      const float* cur = LN.tdout.as<float>();
-      float* pp[2] = {LN.xa.as<float>(), LN.xb.as<float>()};
-      // Linear+LN (+positional encoding, +QKV of layer 0) | per layer: attention + out_proj + FFN + LNs (+ next QKV, or
-      // the PoolAttFF logits behind the last layer) | per-clip pooling.  qkv ping-pongs between two buffers: a layer's
-      // CTAs read keys / values of rows whose next-layer projection other CTAs are already writing.
-      CK(LN.qkv2.reserve((size_t)n_seg * 3 * Dm * 4));
-      float* qk[2] = {LN.qkv.as<float>(), LN.qkv2.as<float>()};
-      const bool de = c.double_ended != 0;
-      // one SelfAttention stack; `kp` = "" (time_dependency) or "2" (time_dependency_2); the stack that feeds the pooling
-      // module computes the PoolAttFF logits behind its last layer
-      auto sa_stack = [&](const std::string& kp, const float* in_rows, int nk, int layers, bool pos_enc, bool feeds_pool,
-                          float* x0, int D, int F) -> const float* {
-        const int nc = D / 64;
-        const float qs = q_scale(D);
-        auto key = [&](int l, const char* s2) { char k[40]; snprintf(k, sizeof k, "sa%s%d.%s", kp.c_str(), l, s2); return std::string(k); };
-        auto params = [&](int l) {
-          SaLayerParams P;
-          P.WoT = W(e, key(l, "woT")); P.bo = W(e, key(l, "bo")); P.W1T = W(e, key(l, "w1T")); P.b1 = W(e, key(l, "b1"));
-          P.W2T = W(e, key(l, "w2T")); P.b2 = W(e, key(l, "b2")); P.ln1_g = W(e, key(l, "ln1g")); P.ln1_b = W(e, key(l, "ln1b"));
-          P.ln2_g = W(e, key(l, "ln2g")); P.ln2_b = W(e, key(l, "ln2b"));
-          return P;
-        };
-        { Scope s(e, "lin_ln");
-          launch_td_in(st, nc, in_rows, W(e, "lin" + kp + ".wT"), nk, W(e, "lin" + kp + ".b"), W(e, "ln" + kp + "0.g"),
-                       W(e, "ln" + kp + "0.b"), W(e, key(0, "qkvT")), W(e, key(0, "qkvb")), qs,
-                       pos_enc ? W(e, kp.empty() ? "pe" : "pe2") : nullptr, seg_clip, d_clips, x0, qk[0], n_seg); }
-        const float* cur2 = x0;
-        for (int l = 0; l < layers; ++l) {
-          const bool last = l + 1 == layers;
-          Scope s(e, "sa_layer");
-          launch_td_sa(st, nc, cur2, qk[l & 1], d_clips, n, d_qt64, n_qt64, params(l), F, pp[l & 1],
-                       last ? nullptr : W(e, key(l + 1, "qkvT")), last ? nullptr : W(e, key(l + 1, "qkvb")), qs,
-                       qk[(l + 1) & 1], H, (feeds_pool && attff) ? n_out : 0, LN.logits.as<float>());
-          cur2 = pp[l & 1];
-        }
-        return cur2;
-      };
-      const bool td2_single = !de && c.td2_layers > 0;      // NISQA / NISQA_DIM with td_2 = 'self_att'
-      cur = sa_stack("", sa_in, sa_nk, c.sa_layers, c.pos_enc != 0, !de && !td2_single, LN.tdout.as<float>(), D1, e->sa_f());
-      if (td2_single) {
-        CK(LN.td2in.reserve((size_t)n_seg * D2 * 4));
-        cur = sa_stack("2", cur, D1 / 64, c.td2_layers, c.td2_pos_enc != 0, true, LN.td2in.as<float>(), D2, e->td2_f());
-      }
-      if (de) {
-        // NISQA_DE (lib:404-424): align the reference clip's rows to the degraded clip's, fuse, second time-dependency stack
-        const int nf = c.de_fuse == NISQA_DE_FUSE_XY_MINUS ? 3 : 2;
-        CK(LN.fused.reserve((size_t)n_seg * 64 * nf * 4));
-        CK(LN.td2in.reserve((size_t)n_seg * 64 * 4));
-        CK(cudaMemsetAsync(LN.fused.p, 0, (size_t)n_seg * 64 * nf * 4, st));      // rows of the reference clips stay zero
-        DeAlignParams AP = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-        if (c.de_align == NISQA_DE_ALIGN_LUONG) { AP.wT = W(e, "de.wT"); AP.b = W(e, "de.b"); }
-        if (c.de_align == NISQA_DE_ALIGN_BAHDANAU) {
-          AP.wqT = W(e, "de.wqT"); AP.bq = W(e, "de.bq"); AP.wyT = W(e, "de.wyT"); AP.by = W(e, "de.by"); AP.v = W(e, "de.v");
-        }
-        { Scope s(e, "de_align");
-          launch_de_align(st, cur, d_clips, n, d_qt64, n_qt64, c.de_align, c.de_align_apply == NISQA_DE_APPLY_SOFT, c.de_fuse,
-                          AP, LN.fused.as<float>()); }
-        const float* td2_rows = LN.fused.as<float>();
-        int td2_nk = nf;
-        if (c.de_fuse_dim > 0) {         // Fusion.lin_fusion (lib:1414-1415)
-          Scope s(e, "de_align");
-          CK(LN.ffa.reserve((size_t)n_seg * c.de_fuse_dim * 4));
-          launch_linear_tile(st, LN.fused.as<float>(), 64 * nf, W(e, "defuse.wT"), W(e, "defuse.b"), 0, LN.ffa.as<float>(), c.de_fuse_dim,
-                             n_seg, 64 * nf, c.de_fuse_dim);
-          td2_rows = LN.ffa.as<float>(); td2_nk = c.de_fuse_dim / 64;
-        }
-        cur = sa_stack("2", td2_rows, td2_nk, c.td2_layers, c.td2_pos_enc != 0, true, LN.td2in.as<float>(), D2, e->td2_f());
-      }
-      e->last_td_out = cur;
-      e->last_td_out_d = e->pool_d();
-      { Scope s(e, "pool");
-        if (attff) launch_pool_final(st, cur, e->pool_d(), LN.logits.as<float>(), d_clips, n, H, n_out, max_n_seg, scores);
-        else {
-          PoolSimpleParams Q = {W(e, "pool.a1"), W(e, "pool.a1b"), W(e, "pool.w3"), W(e, "pool.b3")};
-          launch_pool_simple(st, cur, e->pool_d(), d_clips, n, c.pool, Q, n_out, max_n_seg, scores);
-        }
-        if (de) launch_de_finalize(st, d_clips, n, n_out, scores); }
+// The framewise model: workspaces, front end, segment table, then the CNN (+ AdaptCNN's Linear) or SkipCNN / DFF.
+// `out`: the rows that feed the time-dependency block.
+int framewise(Pass& p, int fmt, Rows* out) {
+  nisqa_engine* e = p.e;
+  const nisqa_config& c = p.c;
+  Lane& LN = p.LN;
+  const int n_seg = p.n_seg;
+  const bool conv_net = c.cnn_kind == NISQA_CNN_CONV, split = e->conv_tc != 0;
+  CK(LN.mel.reserve((size_t)p.n_frames * kMels * 4));
+  CK(LN.segtab.reserve((size_t)n_seg * 12));
+  e->last_split = split;
+  for (int l = split && e->conv12 ? 3 : 2; conv_net && l <= 6; ++l) {
+    if (split) {
+      // the lo plane sits at a fixed offset of the ALLOCATION (not of this pass's n_seg): the zero rows /
+      // columns of both planes must stay where they were when the buffer was cleared
+      CK(LN.planes[l].reserve_zeroed(2 * split_plane_bytes(p.std_mode, l, n_seg), p.st));
+      LN.plane_bytes[l] = (LN.planes[l].cap / 2) & ~(size_t)1023;
     } else {
-      CK(LN.feats20.reserve((size_t)n_seg * 20 * 4));
-      CK(LN.tdout.reserve((size_t)n_seg * 256 * 4));
-      CK(LN.partial.reserve((size_t)n * 2 * 4));
-      { Scope s(e, "fc_out"); launch_fc20(st, LN.feats.as<float>(), W(e, "fc.wT"), W(e, "fc.b"), LN.feats20.as<float>(), n_seg); }
-      LstmParams L;
-      L.w_ih = W(e, "lstm.wih"); L.w_hh = W(e, "lstm.whh"); L.b = W(e, "lstm.b"); L.w_pool = W(e, "lastbi.w");
-      const bool lastbi = c.pool == NISQA_POOL_LAST_STEP_BI;
-      const bool keep = e->keep_td_out || !lastbi;        // the other pooling modules read every step's output
-      { Scope s(e, "lstm", 2);
-        if (e->lstm_batched)
-          launch_lstm_batched(st, LN.feats20.as<float>(), d_clips, d_by_len, n, L, keep ? LN.tdout.as<float>() : nullptr,
-                              LN.partial.as<float>(), e->pool_bias_std, lastbi ? scores : nullptr);
-        else
-          launch_lstm(st, LN.feats20.as<float>(), d_clips, n, L, LN.tdout.as<float>(), LN.partial.as<float>(), e->pool_bias_std,
-                      lastbi ? scores : nullptr); }
-      if (!lastbi) {
-        Scope s(e, "pool");
-        PoolSimpleParams Q = {W(e, "pool.a1"), W(e, "pool.a1b"), W(e, "pool.w3"), W(e, "pool.b3")};
-        launch_pool_simple(st, LN.tdout.as<float>(), 256, d_clips, n, c.pool, Q, 1, max_n_seg, scores);
-      }
-      e->last_td_in = nullptr;
-      e->last_td_out = (e->lstm_batched && !keep) ? nullptr : LN.tdout.as<float>();
-      e->last_td_out_d = 256;
+      const ConvGeom g = split_geometry(p.std_mode, l);
+      CK(LN.act[l].reserve((size_t)n_seg * g.H * g.W * g.C * 4));
     }
   }
+  CK(LN.feats.reserve((size_t)n_seg * (p.std_mode ? 768 : 384) * 4));
+  p.seg_frame0 = LN.segtab.as<int>();
+  p.seg_thr = reinterpret_cast<float*>(p.seg_frame0 + n_seg);
+  p.seg_clip = p.seg_frame0 + 2 * (size_t)n_seg;
+
+  { Scope s(e, "frontend");
+    launch_frontend(p.st, p.pcm, fmt == NISQA_FMT_F32, p.clips, p.n, p.max_pairs, e->fb_table.as<FbTables>(),
+                    e->tw4096.as<float2>(), LN.mel.as<float>(), p.clipmax, p.Q, p.max_span, e->fe_ppc); }
+  { Scope s(e, "seg_table");
+    launch_seg_table(p.st, p.clips, p.n, p.seg_prefix, p.clipmax, c.seg_hop, n_seg, p.seg_frame0, p.seg_thr, p.seg_clip); }
+  e->last_conv12 = split && e->conv12;
+  if (!conv_net) return ff_layers(p, out);
+  conv_layers(p);
+  *out = {LN.feats.as<float>(), 6};
+  if (c.cnn_fc > 0) {      // AdaptCNN's Linear behind conv6 (lib:708-709)
+    Scope s(e, "framewise");
+    CK(LN.ffb.reserve((size_t)n_seg * c.cnn_fc * 4));
+    launch_linear_tile(p.st, LN.feats.as<float>(), 384, p.w.ffc.wT, p.w.ffc.b, 0, LN.ffb.as<float>(), c.cnn_fc, n_seg, 384,
+                       c.cnn_fc);
+    *out = {LN.ffb.as<float>(), c.cnn_fc / 64};
+  }
+  return 0;
+}
+
+// One SelfAttention stack (k = 0: time_dependency, 1: time_dependency_2) over `in`, written to x0 first: Linear + LayerNorm
+// (+ positional encoding, + QKV of layer 0) | per layer: attention + out_proj + FFN + LNs (+ next QKV, or - in the stack
+// that feeds the pooling module - the PoolAttFF logits behind the last layer).  qkv ping-pongs between two buffers: a
+// layer's CTAs read keys / values of rows whose next-layer projection other CTAs are already writing.  Returns the output.
+const float* sa_stack(Pass& p, int k, Rows in, bool feeds_pool, float* x0) {
+  nisqa_engine* e = p.e;
+  const nisqa_config& c = p.c;
+  Lane& LN = p.LN;
+  const SaStackWeights& S = p.w.sa[k];
+  const int D = k ? e->td2_d() : e->sa_d(), F = k ? e->td2_f() : e->sa_f(), layers = k ? c.td2_layers : c.sa_layers;
+  const int nc = D / 64;
+  const float qs = q_scale(D);
+  const int n_heads = (feeds_pool && c.pool == NISQA_POOL_ATT_FF) ? c.n_out : 0;
+  float* pp[2] = {LN.xa.as<float>(), LN.xb.as<float>()};
+  float* qk[2] = {LN.qkv.as<float>(), LN.qkv2.as<float>()};
+  { Scope s(e, "lin_ln");
+    launch_td_in(p.st, nc, in.x, S.in.wT, in.nk, S.in.b, S.ln_g, S.ln_b, S.qkv[0].wT, S.qkv[0].b, qs, S.pe, p.seg_clip,
+                 p.clips, x0, qk[0], p.n_seg); }
+  const float* cur = x0;
+  for (int l = 0; l < layers; ++l) {
+    const bool last = l + 1 == layers;
+    Scope s(e, "sa_layer");
+    launch_td_sa(p.st, nc, cur, qk[l & 1], p.clips, p.n, p.qt64_prefix, p.n_qt64, S.layer[l], F, pp[l & 1],
+                 last ? nullptr : S.qkv[l + 1].wT, last ? nullptr : S.qkv[l + 1].b, qs, qk[(l + 1) & 1], p.w.pool_head,
+                 n_heads, LN.logits.as<float>());
+    cur = pp[l & 1];
+  }
+  return cur;
+}
+
+// NISQA_DE (lib:404-424): align the reference clip's rows to the degraded clip's and fuse them (+ Fusion.lin_fusion,
+// lib:1414-1415).  `out`: the rows that feed time_dependency_2.
+int de_fuse(Pass& p, const float* td_rows, Rows* out) {
+  nisqa_engine* e = p.e;
+  const nisqa_config& c = p.c;
+  Lane& LN = p.LN;
+  const int n_seg = p.n_seg, nf = c.de_fuse == NISQA_DE_FUSE_XY_MINUS ? 3 : 2;
+  CK(LN.fused.reserve((size_t)n_seg * 64 * nf * 4));
+  CK(LN.td2in.reserve((size_t)n_seg * 64 * 4));
+  CK(cudaMemsetAsync(LN.fused.p, 0, (size_t)n_seg * 64 * nf * 4, p.st));      // rows of the reference clips stay zero
+  { Scope s(e, "de_align");
+    launch_de_align(p.st, td_rows, p.clips, p.n, p.qt64_prefix, p.n_qt64, c.de_align, c.de_align_apply == NISQA_DE_APPLY_SOFT,
+                    c.de_fuse, p.w.de, LN.fused.as<float>()); }
+  *out = {LN.fused.as<float>(), nf};
+  if (c.de_fuse_dim > 0) {
+    Scope s(e, "de_align");
+    CK(LN.ffa.reserve((size_t)n_seg * c.de_fuse_dim * 4));
+    launch_linear_tile(p.st, LN.fused.as<float>(), 64 * nf, p.w.defuse.wT, p.w.defuse.b, 0, LN.ffa.as<float>(), c.de_fuse_dim,
+                       n_seg, 64 * nf, c.de_fuse_dim);
+    *out = {LN.ffa.as<float>(), c.de_fuse_dim / 64};
+  }
+  return 0;
+}
+
+// The self-attention time-dependency block - one stack, two stacks (td_2), or NISQA_DE's stack, alignment and second
+// stack - and its pooling module
+int sa_head(Pass& p, Rows rows) {
+  nisqa_engine* e = p.e;
+  const nisqa_config& c = p.c;
+  Lane& LN = p.LN;
+  const int n_seg = p.n_seg, n_out = c.n_out;
+  const int D1 = e->sa_d(), D2 = c.td2_layers > 0 ? e->td2_d() : 0, Dm = std::max(D1, D2);
+  CK(LN.xa.reserve((size_t)n_seg * Dm * 4));
+  CK(LN.xb.reserve((size_t)n_seg * Dm * 4));
+  CK(LN.qkv.reserve((size_t)n_seg * 3 * Dm * 4));
+  CK(LN.logits.reserve((size_t)n_seg * n_out * 4));
+  CK(LN.tdout.reserve((size_t)n_seg * D1 * 4));
+  CK(LN.qkv2.reserve((size_t)n_seg * 3 * Dm * 4));
+  e->last_td_in = LN.tdout.as<float>();
+  const bool de = c.double_ended != 0;
+  const bool td2_single = !de && c.td2_layers > 0;      // NISQA / NISQA_DIM with td_2 = 'self_att'
+  const float* cur = sa_stack(p, 0, rows, !de && !td2_single, LN.tdout.as<float>());
+  if (td2_single) {
+    CK(LN.td2in.reserve((size_t)n_seg * D2 * 4));
+    cur = sa_stack(p, 1, {cur, D1 / 64}, true, LN.td2in.as<float>());
+  }
+  if (de) {
+    Rows fused;
+    const int rc = de_fuse(p, cur, &fused);
+    if (rc) return rc;
+    cur = sa_stack(p, 1, fused, true, LN.td2in.as<float>());
+  }
+  e->last_td_out = cur;
+  e->last_td_out_d = e->pool_d();
+  { Scope s(e, "pool");
+    if (c.pool == NISQA_POOL_ATT_FF)
+      launch_pool_final(p.st, cur, e->pool_d(), LN.logits.as<float>(), p.clips, p.n, p.w.pool_head, n_out, p.max_n_seg, p.scores);
+    else
+      launch_pool_simple(p.st, cur, e->pool_d(), p.clips, p.n, c.pool, p.w.pool_simple, n_out, p.max_n_seg, p.scores);
+    if (de) launch_de_finalize(p.st, p.clips, p.n, n_out, p.scores); }
+  return 0;
+}
+
+// The StandardCNN architecture's fc_out 768 -> 20, BiLSTM and pooling (PoolLastStepBi fused into the BiLSTM launch)
+int lstm_head(Pass& p) {
+  nisqa_engine* e = p.e;
+  const nisqa_config& c = p.c;
+  Lane& LN = p.LN;
+  const Weights& w = p.w;
+  const int n_seg = p.n_seg;
+  CK(LN.feats20.reserve((size_t)n_seg * 20 * 4));
+  CK(LN.tdout.reserve((size_t)n_seg * 256 * 4));
+  CK(LN.partial.reserve((size_t)p.n * 2 * 4));
+  { Scope s(e, "fc_out"); launch_fc20(p.st, LN.feats.as<float>(), w.fc.wT, w.fc.b, LN.feats20.as<float>(), n_seg); }
+  const bool lastbi = c.pool == NISQA_POOL_LAST_STEP_BI;
+  const bool keep = e->keep_td_out || !lastbi;        // the other pooling modules read every step's output
+  { Scope s(e, "lstm", 2);
+    if (e->lstm_batched)
+      launch_lstm_batched(p.st, LN.feats20.as<float>(), p.clips, p.by_len, p.n, w.lstm, keep ? LN.tdout.as<float>() : nullptr,
+                          LN.partial.as<float>(), e->pool_bias_std, lastbi ? p.scores : nullptr);
+    else
+      launch_lstm(p.st, LN.feats20.as<float>(), p.clips, p.n, w.lstm, LN.tdout.as<float>(), LN.partial.as<float>(),
+                  e->pool_bias_std, lastbi ? p.scores : nullptr); }
+  if (!lastbi) {
+    Scope s(e, "pool");
+    launch_pool_simple(p.st, LN.tdout.as<float>(), 256, p.clips, p.n, c.pool, w.pool_simple, 1, p.max_n_seg, p.scores);
+  }
+  e->last_td_in = nullptr;
+  e->last_td_out = (e->lstm_batched && !keep) ? nullptr : LN.tdout.as<float>();
+  e->last_td_out_d = 256;
+  return 0;
+}
+
+int run_pass(nisqa_engine* e, const PassInput& in) {
+  Pass p(e, in);
+  e->cur_stream = p.st;
+  int rc = upload_inputs(p, in);
+  if (rc) return rc;
+  if (p.n_seg == 0) {   // nothing valid in this pass: NaN scores
+    CK(cudaMemsetAsync(p.scores, 0xFF, (size_t)p.n * p.c.n_out * 4, p.st));
+  } else {
+    Rows rows;
+    rc = framewise(p, in.fmt, &rows);
+    if (!rc) rc = p.std_mode ? lstm_head(p) : sa_head(p, rows);
+    if (rc) return rc;
+  }
   CK(cudaGetLastError());
-  CK(cudaEventRecord(SG.ev_done, st));
-  SG.busy = true;
+  CK(cudaEventRecord(p.SG.ev_done, p.st));
+  p.SG.busy = true;
   return 0;
 }
 
@@ -1367,6 +1423,7 @@ int nisqa_load_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
   if (!e->stream) return fail(e, NISQA_ERR_STATE, "engine was not created successfully");
   CK(cudaSetDevice(e->device));
   CK(cudaDeviceSynchronize());
+  e->weights_loaded = false;      // a failed load may have freed the previous arena
   int rc = pack_weights(e, tensors, n);
   if (rc) return rc;
   e->weights_loaded = true;
@@ -1518,20 +1575,21 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
   Lane& LN = e->lanes[e->last_lane];
   Stage& SG = e->stages[e->last_stage];
   const int std_mode = e->cfg.arch == NISQA_ARCH_STD_LSTM_LASTBI;
-  const int W1 = std_mode ? 8 : 7, W2 = std_mode ? 4 : 5, W3 = std_mode ? 2 : 3;
   const int64_t ns = e->last_n_seg;
   if (e->cfg.cnn_kind != NISQA_CNN_CONV && stage >= NISQA_STAGE_POOL1 && stage <= NISQA_STAGE_CNN_FEAT)
     return fail(e, NISQA_ERR_INVALID, "stage not available: this checkpoint has no convolutional framewise model");
+  const bool conv_map = stage >= NISQA_STAGE_POOL1 && stage <= NISQA_STAGE_CONV5;
+  const int layer = stage - NISQA_STAGE_POOL1 + 2;      // POOL1 .. CONV5: the map that feeds conv layer 2 .. 6
   int64_t count = 0;
   const float* src = nullptr;
   int hw = 0, ch = 0;    // NHWC -> NCHW conversion when ch > 0
+  if (conv_map) {
+    const ConvGeom g = split_geometry(std_mode, layer);
+    src = LN.act[layer].as<float>(); hw = g.H * g.W; ch = g.C;
+  }
   switch (stage) {
     case NISQA_STAGE_MEL_DB: count = (int64_t)e->last_n_frames * kMels; break;
-    case NISQA_STAGE_POOL1: src = LN.act1.as<float>(); hw = 24 * W1; ch = 16; break;
-    case NISQA_STAGE_POOL2: src = LN.act2.as<float>(); hw = 12 * W2; ch = 32; break;
-    case NISQA_STAGE_CONV3: src = LN.act3.as<float>(); hw = 12 * W2; ch = 64; break;
-    case NISQA_STAGE_POOL3: src = LN.act4.as<float>(); hw = 6 * W3; ch = 64; break;
-    case NISQA_STAGE_CONV5: src = LN.act5.as<float>(); hw = 6 * W3; ch = 64; break;
+    case NISQA_STAGE_POOL1: case NISQA_STAGE_POOL2: case NISQA_STAGE_CONV3: case NISQA_STAGE_POOL3: case NISQA_STAGE_CONV5: break;
     case NISQA_STAGE_CNN_FEAT:
       if (std_mode) { src = LN.feats20.as<float>(); count = ns * 20; }
       else { src = LN.feats.as<float>(); hw = 6; ch = 64; }     // [h][c] -> c*6+h
@@ -1546,19 +1604,9 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
   }
   if (ch > 0) count = ns * hw * ch;
   if (!out) return count;
-  int plane_layer = 0;          // stage lives in the plane pair feeding this conv layer
-  if (e->last_split) {
-    if (stage == NISQA_STAGE_POOL1 && e->last_conv12)
-      return fail(e, NISQA_ERR_STATE, "pool1 lives only in shared memory on the fused conv1+conv2 path: nisqa_set_option(\"conv12\", 0) before the predict call");
-    switch (stage) {
-      case NISQA_STAGE_POOL1: plane_layer = 2; break;
-      case NISQA_STAGE_POOL2: plane_layer = 3; break;
-      case NISQA_STAGE_CONV3: plane_layer = 4; break;
-      case NISQA_STAGE_POOL3: plane_layer = 5; break;
-      case NISQA_STAGE_CONV5: plane_layer = 6; break;
-      default: break;
-    }
-  }
+  const bool from_planes = conv_map && e->last_split;     // the map lives in the plane pair planes[layer]
+  if (from_planes && stage == NISQA_STAGE_POOL1 && e->last_conv12)
+    return fail(e, NISQA_ERR_STATE, "pool1 lives only in shared memory on the fused conv1+conv2 path: nisqa_set_option(\"conv12\", 0) before the predict call");
   if (cap < count) return fail(e, NISQA_ERR_INVALID, "stage dump buffer too small");
   if (count == 0) return 0;
   cudaStream_t st = LN.stream;
@@ -1568,13 +1616,11 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
                     SG.clipmax.as<unsigned>(), e->dump.as<float>());
     src = e->dump.as<float>();
   } else if (ch > 0) {
-    if (plane_layer) {
-      DevBuf* tmp[7] = {nullptr, nullptr, &LN.act1, &LN.act2, &LN.act3, &LN.act4, &LN.act5};
-      CK(tmp[plane_layer]->reserve((size_t)count * 4));
-      launch_unsplit(st, std_mode, plane_layer, LN.planes[plane_layer].as<char>(),
-                     LN.planes[plane_layer].as<char>() + LN.plane_bytes[plane_layer],
-                     ldexpf(1.f, e->act_exp[plane_layer - 1]), tmp[plane_layer]->as<float>(), (int)ns);
-      src = tmp[plane_layer]->as<float>();
+    if (from_planes) {
+      CK(LN.act[layer].reserve((size_t)count * 4));
+      launch_unsplit(st, std_mode, layer, LN.planes[layer].as<char>(), LN.planes[layer].as<char>() + LN.plane_bytes[layer],
+                     ldexpf(1.f, e->act_exp[layer - 1]), LN.act[layer].as<float>(), (int)ns);
+      src = LN.act[layer].as<float>();
     }
     CK(e->dump.reserve((size_t)count * 4));
     launch_nhwc_to_nchw(st, src, e->dump.as<float>(), ns, hw, ch);

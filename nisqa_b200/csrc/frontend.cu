@@ -13,6 +13,7 @@
 // Grid: x = frame pair, y = clip.
 #include "common.cuh"
 #include "f32x2.cuh"
+#include "launch.cuh"
 
 // experiment switches (-DNAME=value when building a variant library); the defaults are the variants the kernel is tuned with
 #ifndef NISQA_FE_PK_FFT

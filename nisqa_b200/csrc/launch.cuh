@@ -1,0 +1,126 @@
+// launch.cuh - the boundary between the host runtime (engine.cu) and the kernel files: the parameter structs the
+// kernels take by value and the host launchers each kernel file defines.  Every file that defines one of them
+// includes this header, so a definition that drifts from its declaration is a compile or link error.
+// Plain host C++ (resample.cpp includes it too): the device structs of common.cuh are only named here.
+#pragma once
+#include <cuda_runtime.h>
+#include <stddef.h>
+
+#include <vector>
+
+namespace nisqa {
+
+struct ClipDesc;
+struct FbTables;
+
+// Geometry of one segment's activation map that feeds conv layer `layer` (2..6), i.e. the output of layer - 1:
+// H rows, W columns, C channels.  AdaptCNN pools to widths 7 / 5 / 3 (adaptive max-pool), StandardCNN to 8 / 4 / 2
+// (MaxPool2d(2)).  The fp16 plane pairs (conv_split.cu), the fp32 FFMA activations and the stage dumps all use it.
+struct ConvGeom { int H, W, C; };
+constexpr ConvGeom split_geometry(int std_mode, int layer) {
+  return {layer == 2 ? 24 : layer <= 4 ? 12 : 6,
+          std_mode ? (layer == 2 ? 8 : layer <= 4 ? 4 : 2) : (layer == 2 ? 7 : layer <= 4 ? 5 : 3),
+          layer == 2 ? 16 : layer == 3 ? 32 : 64};
+}
+// true when the layer configuration C (cnn.cu ConvCfg, conv_split.cuh SpCfg) reads that geometry
+template <class C>
+constexpr bool input_is(int std_mode, int layer) {
+  return split_geometry(std_mode, layer).H == C::H && split_geometry(std_mode, layer).W == C::W &&
+         split_geometry(std_mode, layer).C == C::CIN;
+}
+
+// ---------------------------------------------------------------- parameter structs (device pointers)
+// One post-norm encoder layer of a self-attention stack, weights k-major in 64-column chunks (td_tiled.cu)
+struct SaLayerParams {
+  const float* WoT; const float* bo; const float* W1T; const float* b1; const float* W2T;
+  const float* b2; const float* ln1_g; const float* ln1_b; const float* ln2_g; const float* ln2_b;
+};
+// PoolAttFF (lib:1156-1183): the logits w2_h . relu(W1_h x + b1_h) + b2_h come out of td_sa_kernel's fused tail; x is D wide
+struct PoolHeadParams {      // heads concatenated
+  const float* W1T;   // [n_heads][D k][128 j]
+  const float* b1;    // [n_heads][128]
+  const float* w2;    // [n_heads][128]
+  const float* b2;    // [n_heads]
+  const float* w3;    // [n_heads][D]
+  const float* b3;    // [n_heads]
+};
+// PoolAtt (a1, a1b: the attention logit) / PoolAvg / PoolMax / PoolLastStep: one Linear(D -> 1) per head (td.cu)
+struct PoolSimpleParams { const float* a1; const float* a1b; const float* w3; const float* b3; };
+struct LstmParams {
+  const float* w_ih;   // [2][512][20]
+  const float* w_hh;   // [2][512][128]
+  const float* b;      // [2][512]   (bias_ih + bias_hh)
+  const float* w_pool; // [256]
+};
+// learned weights of AttLuong (wT [64][64] k-major, b [64]) / AttBahdanau (wqT, wyT [64][128] k-major, bq, by, v [128])
+struct DeAlignParams { const float* wT; const float* b; const float* wqT; const float* bq; const float* wyT; const float* by; const float* v; };
+struct ResampleClip {
+  long long in_off;      // element offset of the clip in the raw input buffer (float32, or int16 scaled by 1/32768)
+  long long out_off;     // element offset in the packed float32 output buffer
+  long long time_off;    // first entry of the clip in the chunk-start time register table
+  int n_in;              // input samples
+  int n_out;             // resampy's int(n_in * ratio)
+  int n_fix;             // librosa fix_length: ceil(n_in * ratio) (zero padded / trimmed)
+  int copy;              // 1: sr_orig == sr_new, plain conversion / copy
+  double ratio;          // sr_new / sr_orig
+};
+
+// ---------------------------------------------------------------- frontend.cu
+void launch_frontend(cudaStream_t st, const void* pcm, int fmt_f32, const ClipDesc* clips, int n_clips, int max_pairs,
+                     const FbTables* fbs, const float2* tw, float* mel, unsigned* clipmax, int Q, int max_span, int ppc);
+void launch_seg_table(cudaStream_t st, const ClipDesc* clips, int n_clips, const int* seg_prefix, const unsigned* clipmax,
+                      int seg_hop, int n_seg, int* seg_frame0, float* seg_thr, int* seg_clip);
+void launch_mel_dump(cudaStream_t st, const float* mel, const ClipDesc* clips, int n_clips, const unsigned* clipmax, float* out);
+
+// ---------------------------------------------------------------- cnn.cu (fp32 FFMA convolutions)
+void launch_conv1(cudaStream_t st, int std_mode, const float* mel, const int* seg_frame0, const float* seg_thr,
+                  const float* w1, const float* b1, float* out, int n_seg, void* out_hi, void* out_lo, float store_scale);
+void launch_conv_layer(cudaStream_t st, int std_mode, int layer, const float* in, const float* w, const float* b, float* out,
+                       int n_seg);
+void launch_nhwc_to_nchw(cudaStream_t st, const float* in, float* out, long long n, int hw, int ch);
+
+// ---------------------------------------------------------------- conv_split.cu (tensor-core convolutions on fp16 planes)
+size_t split_plane_bytes(int std_mode, int layer, int n_seg);
+void launch_conv_split(cudaStream_t st, int std_mode, int layer, const void* in_hi, const void* in_lo, const void* wtc,
+                       const float* b, float out_scale, float store_scale, void* out_hi, void* out_lo, float* out_f32, int n_seg);
+void launch_conv12(cudaStream_t st, int std_mode, const float* mel, const int* seg_frame0, const float* seg_thr,
+                   const float* w1, const float* b1, float c1_scale, const void* wtc2, const float* bias2, float scale2,
+                   float store_scale, void* out_hi, void* out_lo, int n_seg);
+void launch_unsplit(cudaStream_t st, int std_mode, int layer, const void* hi, const void* lo, float unit, float* out, int n_seg);
+
+// ---------------------------------------------------------------- td.cu (fc_out, BiLSTM, pooling)
+void launch_fc20(cudaStream_t st, const float* feats, const float* WT, const float* b, float* out, int n_rows);
+void launch_lstm(cudaStream_t st, const float* feats20, const ClipDesc* clips, int n_clips, const LstmParams& P,
+                 float* td_out, float* partial, float pool_bias, float* scores);
+void launch_lstm_batched(cudaStream_t st, const float* feats20, const ClipDesc* clips, const int* order, int n_clips,
+                         const LstmParams& P, float* td_out, float* partial, float pool_bias, float* scores);
+void launch_pool_final(cudaStream_t st, const float* x, int D, const float* logits, const ClipDesc* clips, int n_clips,
+                       const PoolHeadParams& P, int n_heads, int max_seg, float* scores);
+void launch_pool_simple(cudaStream_t st, const float* x, int D, const ClipDesc* clips, int n_clips, int mode,
+                        const PoolSimpleParams& P, int n_heads, int max_seg, float* scores);
+
+// ---------------------------------------------------------------- td_tiled.cu (self-attention, NISQA_DE, SkipCNN / DFF)
+void launch_td_in(cudaStream_t st, int nc, const float* feats, const float* WT, int nk, const float* b, const float* g,
+                  const float* be, const float* qkvT, const float* qkvb, float qscale, const float* pe, const int* seg_clip,
+                  const ClipDesc* clips, float* x0, float* qkv, int n_rows);
+void launch_td_sa(cudaStream_t st, int nc, const float* x_in, const float* qkv, const ClipDesc* clips, int n_clips,
+                  const int* qtile64_prefix, int n_qtiles, const SaLayerParams& P, int F, float* x_out,
+                  const float* next_qkvT, const float* next_qkvb, float qscale, float* qkv_next,
+                  const PoolHeadParams& H, int n_heads, float* logits);
+void launch_de_align(cudaStream_t st, const float* x_td, const ClipDesc* clips, int n_clips, const int* qtile64_prefix,
+                     int n_qtiles, int align, int soft, int fuse, const DeAlignParams& A, float* fused);
+void launch_de_finalize(cudaStream_t st, const ClipDesc* clips, int n_clips, int n_out, float* scores);
+void launch_seg_feats(cudaStream_t st, const float* mel, const int* seg_frame0, const float* seg_thr, const float* bn, int n_seg,
+                      float* out);
+void launch_linear_tile(cudaStream_t st, const float* X, int ldx, const float* WT, const float* bias, int relu, float* Y, int ldy,
+                        int n_rows, int K, int N);
+
+// ---------------------------------------------------------------- resample_gpu.cu
+void launch_resample(cudaStream_t st, const void* raw, int fmt_f32, const ResampleClip* clips, int n_clips, int max_fix,
+                     double* t_start, const double* win, int nwin, int num_table, float* out);
+
+// ---------------------------------------------------------------- resample.cpp
+// the interpolation table of the resampler (set by nisqa_resample_set_filter); false before that call
+bool resample_table(std::vector<double>* win, int* num_table);
+
+}  // namespace nisqa

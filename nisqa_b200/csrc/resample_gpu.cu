@@ -12,19 +12,9 @@
 // 2 table loads per tap out of a 262 KB L2-resident table.  A 10 s clip takes ~2 ms of one SM's time instead of
 // 0.28 s of a host core.
 #include "common.cuh"
+#include "launch.cuh"
 
 namespace nisqa {
-
-struct ResampleClip {
-  long long in_off;      // element offset of the clip in the raw input buffer (float32, or int16 scaled by 1/32768)
-  long long out_off;     // element offset in the packed float32 output buffer
-  long long time_off;    // first entry of the clip in the chunk-start time register table
-  int n_in;              // input samples
-  int n_out;             // resampy's int(n_in * ratio)
-  int n_fix;             // librosa fix_length: ceil(n_in * ratio) (zero padded / trimmed)
-  int copy;              // 1: sr_orig == sr_new, plain conversion / copy
-  double ratio;          // sr_new / sr_orig
-};
 
 constexpr int kRsChunk = 256;
 

@@ -1,17 +1,14 @@
-// td.cu - time-dependency + pooling kernels.
-//   adapt arch  : Linear 384->64 + LayerNorm (reference nisqa/NISQA_lib.py:989-991),
-//                 2x post-norm encoder layer with 1-head attention (lib:1025-1040),
-//                 5 (or 1) PoolAttFF heads (lib:1171-1183, fan-out lib:260-268).
-//   standard    : fc_out 768->20 (lib:832-834), BiLSTM (lib:925-943), PoolLastStepBi
-//                 (lib:1107-1115).
-// All of it is row-local fp32 work on [n_seg, 64] matrices (3.5 % of the FLOPs of a clip):
-// one thread owns one time step (row); weights sit in shared memory as [k][out] so the
-// inner loop is a warp-broadcast LDS.128 per 4 FMAs.  Clips are ragged: every kernel works
-// on the valid rows only, so no key-padding mask exists (masked keys in the reference
-// contribute exactly 0 after softmax).
+// td.cu - the time-dependency and pooling kernels that are not register-tiled GEMMs (the self-attention stacks live in
+// td_tiled.cu):
+//   standard arch : fc_out 768->20 (reference nisqa/NISQA_lib.py:832-834, linear_rows_kernel), BiLSTM (lib:925-943, one
+//                   CTA per sequence or NB sequences per CTA in lock step), PoolLastStepBi (lib:1107-1115)
+//   both archs    : the pooling modules - PoolAttFF (lib:1156-1183) behind self-attention, whose logits td_sa_kernel
+//                   computes, and PoolAtt / PoolAvg / PoolMax / PoolLastStep behind either time-dependency block
+// Clips are ragged: every kernel works on the clip's valid rows only, so no key-padding mask exists.
 #include <algorithm>
 
 #include "common.cuh"
+#include "launch.cuh"
 
 namespace nisqa {
 
@@ -37,33 +34,17 @@ __device__ __forceinline__ void rowgemm(float (&acc)[NCOL], const float* xrow, c
   }
 }
 
-// nn.LayerNorm(64): biased variance, eps 1e-5
-__device__ __forceinline__ void layernorm64(float (&v)[64], const float* __restrict__ gamma,
-                                            const float* __restrict__ beta) {
-  float mean = 0.f;
-#pragma unroll
-  for (int j = 0; j < 64; ++j) mean += v[j];
-  mean *= (1.0f / 64.0f);
-  float var = 0.f;
-#pragma unroll
-  for (int j = 0; j < 64; ++j) { const float d = v[j] - mean; var = fmaf(d, d, var); }
-  const float rstd = 1.0f / sqrtf(var * (1.0f / 64.0f) + 1e-5f);
-#pragma unroll
-  for (int j = 0; j < 64; ++j) v[j] = (v[j] - mean) * rstd * __ldg(gamma + j) + __ldg(beta + j);
-}
-
 __device__ __forceinline__ void stage_f4(float* dst, const float* __restrict__ src, int n_floats) {
   const float4* s = reinterpret_cast<const float4*>(src);
   for (int i = threadIdx.x; i < n_floats / 4; i += blockDim.x) reinterpret_cast<float4*>(dst)[i] = __ldg(s + i);
 }
 
 // ---------------------------------------------------------------------------------------
-// out[row][0..NOUT) = (LN?)( in[row][0..K) @ WT[K][NOUT] + bias )   K % 64 == 0
-template <int NOUT, bool LN>
+// out[row][0..NOUT) = in[row][0..K) @ WT[K][NOUT] + bias   K % 64 == 0; one thread per row
+template <int NOUT>
 __global__ void __launch_bounds__(kRows)
 linear_rows_kernel(const float* __restrict__ in, int K, const float* __restrict__ WT,
-                   const float* __restrict__ bias, const float* __restrict__ gamma,
-                   const float* __restrict__ beta, float* __restrict__ out, int n_rows) {
+                   const float* __restrict__ bias, float* __restrict__ out, int n_rows) {
   extern __shared__ __align__(16) float sm[];
   float* xs = sm;                       // [kRows][kXS]
   float* ws = sm + kRows * kXS;         // [64][NOUT]
@@ -82,10 +63,6 @@ linear_rows_kernel(const float* __restrict__ in, int K, const float* __restrict_
     rowgemm<NOUT>(acc, xs + tid * kXS, ws, 64);
   }
   if (row0 + tid >= n_rows) return;
-  if constexpr (LN) {
-    static_assert(!LN || NOUT == 64, "LayerNorm width");
-    layernorm64(acc, gamma, beta);
-  }
   float* o = out + (size_t)(row0 + tid) * NOUT;
 #pragma unroll
   for (int q = 0; q < NOUT / 4; ++q)
@@ -93,21 +70,7 @@ linear_rows_kernel(const float* __restrict__ in, int K, const float* __restrict_
 }
 
 // ---------------------------------------------------------------------------------------
-struct SaLayerParams {
-  const float* WoT; const float* bo; const float* W1T; const float* b1; const float* W2T;
-  const float* b2; const float* ln1_g; const float* ln1_b; const float* ln2_g; const float* ln2_b;
-};
-// PoolAttFF (lib:1156-1183): the logits w2_h . relu(W1_h x + b1_h) + b2_h come out of td_sa_kernel's fused tail; x is D wide
-struct PoolHeadParams {      // device pointers, heads concatenated
-  const float* W1T;   // [n_heads][D k][128 j]
-  const float* b1;    // [n_heads][128]
-  const float* w2;    // [n_heads][128]
-  const float* b2;    // [n_heads]
-  const float* w3;    // [n_heads][D]
-  const float* b3;    // [n_heads]
-};
-
-// softmax over the clip's time steps, weighted sum of x, Linear D->1   (lib:1177-1181)
+// PoolAttFF: softmax over the clip's time steps, weighted sum of x, Linear D->1   (lib:1177-1181)
 // grid = n_clips, block = 64 * n_heads; thread (h, d) owns features d, d + 64, .. < D.  The softmax numerators are formed once per (head, step) into shared
 // memory; the weighted sum keeps ONE accumulator per thread in step order (the result does not depend on the unrolling) with
 // eight independent loads in flight.
@@ -166,7 +129,6 @@ __global__ void pool_final_kernel(const float* __restrict__ x, const float* __re
 //   mode 3 PoolMax       (lib:1206-1225): max over the clip's steps, Linear
 //   mode 4 PoolLastStep  (lib:1117-1129): x at the last valid step, Linear
 // One Linear(D -> 1) per head (NISQA_DIM: five heads with their own weights, lib:260-268).
-struct PoolSimpleParams { const float* a1; const float* a1b; const float* w3; const float* b3; };
 
 template <int D>
 __device__ __forceinline__ float block_sum(float v, float* red) {
@@ -242,12 +204,6 @@ pool_simple_kernel(const float* __restrict__ x /*[n_seg][D]*/, const ClipDesc* _
 // so the gate exchange is four shuffles, the cell update is replicated in the quad, and a step
 // needs ONE barrier (h and x are double buffered).  W_hh row: first 64 taps in registers, last 64
 // in shared memory [k][512].
-struct LstmParams {
-  const float* w_ih;   // [2][512][20]
-  const float* w_hh;   // [2][512][128]
-  const float* b;      // [2][512]   (bias_ih + bias_hh)
-  const float* w_pool; // [256]
-};
 constexpr int kLstmSmemFloats = 64 * 512 + 2 * 128 + 2 * 32 + 128;
 
 __global__ void __launch_bounds__(512, 1)
@@ -515,7 +471,7 @@ __global__ void lastbi_final_kernel(const float* __restrict__ partial, const Cli
 constexpr int kRowSmem20 = (kRows * kXS + 64 * 20) * 4;
 
 void launch_fc20(cudaStream_t st, const float* feats, const float* WT, const float* b, float* out, int n_rows) {
-  linear_rows_kernel<20, false><<<(n_rows + kRows - 1) / kRows, kRows, kRowSmem20, st>>>(feats, 768, WT, b, nullptr, nullptr, out, n_rows);
+  linear_rows_kernel<20><<<(n_rows + kRows - 1) / kRows, kRows, kRowSmem20, st>>>(feats, 768, WT, b, out, n_rows);
 }
 void launch_pool_final(cudaStream_t st, const float* x, int D, const float* logits, const ClipDesc* clips, int n_clips,
                        const PoolHeadParams& P, int n_heads, int max_seg, float* scores) {

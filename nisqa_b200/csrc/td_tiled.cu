@@ -20,20 +20,16 @@
 // xor-shuffles, and P (the softmax numerators) is written and re-read by the same half-warp: no block barrier inside a
 // key block.  Operand tiles (16 KB, L2 resident) stream through a ring of shared-memory slots with cp.async, the next
 // ones in flight while the current one is multiplied.  fp32 throughout (parity: +-1e-4 on the scores).
+#include "../../include/nisqa_b200.h"
 #include "common.cuh"
 #include "f32x2.cuh"
+#include "launch.cuh"
 
 #ifndef NISQA_TD_PK
 #define NISQA_TD_PK 0        // tile GEMMs with packed FFMA2 (same FMAs in the same order)
 #endif
 
 namespace nisqa {
-
-struct SaLayerParams {
-  const float* WoT; const float* bo; const float* W1T; const float* b1; const float* W2T;
-  const float* b2; const float* ln1_g; const float* ln1_b; const float* ln2_g; const float* ln2_b;
-};
-struct PoolHeadParams { const float* W1T; const float* b1; const float* w2; const float* b2; const float* w3; const float* b3; };
 
 namespace {
 
@@ -591,8 +587,6 @@ td_sa_kernel(const float* __restrict__ x_in, const float* __restrict__ qkv, cons
 //   soft        : y_al[i] = softmax_j(score[i]) . y (ApplySoftAttention, lib:1370-1378), online max / sum over key blocks
 //   fuse        : [x, y_al, x - y_al] | [x + y_al, x - y_al] | [x, y_al]  ->  fused[row][64 * nf]
 // Same 64 x 64 register tiling as td_sa_kernel; the y block serves as K (row-major, pitch 68) and as V.
-enum { DE_ALIGN_DOT = 1, DE_ALIGN_COSINE = 2, DE_ALIGN_DISTANCE = 3, DE_ALIGN_LUONG = 4, DE_ALIGN_BAHD = 5 };      // = enum nisqa_de_align
-enum { DE_FUSE_XY_MINUS = 0, DE_FUSE_PLUS_MINUS = 1, DE_FUSE_XY = 2 };
 
 // s[i][j] -= sum_k |A[4ty+i][k] - B[tx+16j][k]|
 __device__ __forceinline__ void absdiff_nt(float (&s)[4][4], const float* __restrict__ A, const float* __restrict__ B, int ty, int tx) {
@@ -617,8 +611,6 @@ constexpr int kDeSmemFloats = 2 * kTileF + 2 * kTileF + 2 * kT;      // Qs | Ps 
 constexpr int kBhLd = 132;                                            // pitch of the [64][128] projections (AttBahdanau)
 constexpr int kDeLuongFloats = 4096 + kTileF;                          // W^T | projected keys
 constexpr int kDeBahdFloats = 64 * 128 + 2 * 64 * kBhLd;               // Wy^T | Wq x + bq | Wy y + by
-// learned weights of AttLuong (wT [64][64] k-major, b [64]) / AttBahdanau (wqT, wyT [64][128] k-major, bq, by, v [128])
-struct DeAlignParams { const float* wT; const float* b; const float* wqT; const float* bq; const float* wyT; const float* by; const float* v; };
 
 __global__ void __launch_bounds__(kNT, 2)
 de_align_kernel(const float* __restrict__ x_td /*[n_seg][64]*/, const ClipDesc* __restrict__ clips, int n_clips,
@@ -640,17 +632,17 @@ de_align_kernel(const float* __restrict__ x_td /*[n_seg][64]*/, const ClipDesc* 
   const int rows_valid = min(kT, Sx - q0);
   const long long row0 = (long long)cd.seg_off + q0;
   const float* y_base = x_td + (long long)cr.seg_off * 64;
-  const int nf = fuse == DE_FUSE_XY_MINUS ? 3 : 2;
+  const int nf = fuse == NISQA_DE_FUSE_XY_MINUS ? 3 : 2;
 
   tile_load_async(Qs, kLd, x_td + row0 * 64, 64, rows_valid, tid);
   tile_load_async(Yb, kLd, y_base, 64, min(kT, Sy), tid);
   cp_commit();
-  if (align == DE_ALIGN_LUONG) tile_load_async(Ex, 64, A.wT, 64, 64, tid);
-  if (align == DE_ALIGN_BAHD) { tile_load_async(Ex, 128, A.wyT, 128, 64, tid); tile_load_async(Ex + 64, 128, A.wyT + 64, 128, 64, tid); }
+  if (align == NISQA_DE_ALIGN_LUONG) tile_load_async(Ex, 64, A.wT, 64, 64, tid);
+  if (align == NISQA_DE_ALIGN_BAHDANAU) { tile_load_async(Ex, 128, A.wyT, 128, 64, tid); tile_load_async(Ex + 64, 128, A.wyT + 64, 128, 64, tid); }
   cp_commit();
   float o[4][4];
   zero_acc(o);
-  if (align == DE_ALIGN_BAHD) {
+  if (align == NISQA_DE_ALIGN_BAHDANAU) {
     // XQ = Wq x + bq for the CTA's 64 degraded steps: two 64-column halves, Wq^T staged through Ps
     float* XQ = Ex + 64 * 128;
     cp_wait<0>();
@@ -686,7 +678,7 @@ de_align_kernel(const float* __restrict__ x_td /*[n_seg][64]*/, const ClipDesc* 
       cp_wait<1>();
       __syncthreads();
       const float* Y = Yb + (kb & 1) * kTileF;
-      if (align == DE_ALIGN_COSINE) {
+      if (align == NISQA_DE_ALIGN_COSINE) {
         // nn.CosineSimilarity: x . y / (max(|x|, eps) max(|y|, eps)); four threads per key row, 16 features each
         const int r = tid >> 2, qd = tid & 3;
         float ss = 0.f;
@@ -711,7 +703,7 @@ de_align_kernel(const float* __restrict__ x_td /*[n_seg][64]*/, const ClipDesc* 
       }
       float s[4][4];
       zero_acc(s);
-      if (align == DE_ALIGN_LUONG) {
+      if (align == NISQA_DE_ALIGN_LUONG) {
         // y' = W y + b for the block's keys, then x . y'
         float* Yp = Ex + 4096;
         float acc[4][4];
@@ -722,7 +714,7 @@ de_align_kernel(const float* __restrict__ x_td /*[n_seg][64]*/, const ClipDesc* 
         store_rows_smem(Yp, acc, ty, tx);
         __syncthreads();
         gemm_nt(s, Qs, Yp, ty, tx);
-      } else if (align == DE_ALIGN_BAHD) {
+      } else if (align == NISQA_DE_ALIGN_BAHDANAU) {
         const float* WyT = Ex;
         const float* XQ = Ex + 64 * 128;
         float* YK = Ex + 64 * 128 + 64 * kBhLd;
@@ -756,7 +748,7 @@ de_align_kernel(const float* __restrict__ x_td /*[n_seg][64]*/, const ClipDesc* 
               s[i][j] = t;
             }
         }
-      } else if (align == DE_ALIGN_DISTANCE) {
+      } else if (align == NISQA_DE_ALIGN_DISTANCE) {
         absdiff_nt(s, Qs, Y, ty, tx);
 #pragma unroll
         for (int i = 0; i < 4; ++i)
@@ -764,7 +756,7 @@ de_align_kernel(const float* __restrict__ x_td /*[n_seg][64]*/, const ClipDesc* 
           for (int j = 0; j < 4; ++j) s[i][j] *= (1.0f / 64.0f);
       } else {
         gemm_nt(s, Qs, Y, ty, tx);
-        if (align == DE_ALIGN_COSINE) {
+        if (align == NISQA_DE_ALIGN_COSINE) {
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             const float ry = Yn[(kb & 1) * kT + tx + 16 * j];
@@ -835,8 +827,8 @@ de_align_kernel(const float* __restrict__ x_td /*[n_seg][64]*/, const ClipDesc* 
     const float4 yv = make_float4(o[i][0], o[i][1], o[i][2], o[i][3]);
     const float4 df = make_float4(xv.x - yv.x, xv.y - yv.y, xv.z - yv.z, xv.w - yv.w);
     float4* dst = reinterpret_cast<float4*>(fused + (row0 + 4 * ty + i) * (64 * nf)) + tx;
-    if (fuse == DE_FUSE_XY_MINUS) { dst[0] = xv; dst[16] = yv; dst[32] = df; }
-    else if (fuse == DE_FUSE_PLUS_MINUS) { dst[0] = make_float4(xv.x + yv.x, xv.y + yv.y, xv.z + yv.z, xv.w + yv.w); dst[16] = df; }
+    if (fuse == NISQA_DE_FUSE_XY_MINUS) { dst[0] = xv; dst[16] = yv; dst[32] = df; }
+    else if (fuse == NISQA_DE_FUSE_PLUS_MINUS) { dst[0] = make_float4(xv.x + yv.x, xv.y + yv.y, xv.z + yv.z, xv.w + yv.w); dst[16] = df; }
     else { dst[0] = xv; dst[16] = yv; }
   }
 }
@@ -946,7 +938,7 @@ void launch_de_align(cudaStream_t st, const float* x_td, const ClipDesc* clips, 
   static unsigned long long cfg = 0;
   if (first_launch_on_device(cfg))
     cudaFuncSetAttribute(de_align_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (kDeSmemFloats + kDeBahdFloats) * 4);
-  const int smem = (kDeSmemFloats + (align == DE_ALIGN_LUONG ? kDeLuongFloats : align == DE_ALIGN_BAHD ? kDeBahdFloats : 0)) * 4;
+  const int smem = (kDeSmemFloats + (align == NISQA_DE_ALIGN_LUONG ? kDeLuongFloats : align == NISQA_DE_ALIGN_BAHDANAU ? kDeBahdFloats : 0)) * 4;
   de_align_kernel<<<n_qtiles, kNT, smem, st>>>(x_td, clips, n_clips, qtile64_prefix, align, soft, fuse, A, fused);
 }
 

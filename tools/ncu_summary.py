@@ -26,7 +26,7 @@ STALL_NAMES = ["long_scoreboard", "short_scoreboard", "barrier", "math_pipe_thro
 
 def short(name, seen):
     table = [("conv12", "conv12"), ("frontend", "frontend"), ("seg_table", "seg_table"), ("conv1_pool1", "conv1"),
-             ("linear_rows_kernel<64", "lin_ln"), ("linear_rows_kernel<20", "fc_out"), ("qkv", "qkv"),
+             ("linear_rows_kernel<20", "fc_out"), ("qkv", "qkv"),
              ("sa_layer", "sa_layer"), ("pool_logits", "pool_logits"), ("pool_final", "pool_final"),
              ("lstm", "lstm"), ("lastbi", "lastbi")]
     name = name.replace("(int)", "").replace("(bool)", "")
