@@ -26,13 +26,15 @@
 // exists.  The 9 taps are the same tile read at row-shifted addresses: im2col is never materialised.
 //
 // GEMM view:  D[pos, co] = sum_{tap, ci} X[pos + off(tap), ci] * W[tap][co][ci]
-//   M = 256 tile rows (G segments), N = C_out, K = 9 * C_in.  Four warpgroups own 64 rows each: A fragments come
-//   from the swizzled tile with ldmatrix (conflict free: 8 consecutive rows hit 8 distinct 16-byte bank groups), B
+//   M = the interior output positions of G segments (SpCfg::gemm_row: GEMM row -> plane row; the zero row / column
+//   positions are not computed), N = C_out, K = 9 * C_in.  Warpgroup b < NBLK owns GEMM rows 64 b .. 64 b + 63: A
+//   fragments come from the swizzled tile with ldmatrix, one gathered row address per lane (8 rows of distinct
+//   plane row mod 8 hit 8 distinct 16-byte bank groups; a group that crosses a zero column may repeat one), B
 //   (all nine weight taps, resident for the CTA's life) through shared-memory descriptors, accumulators in
 //   registers.  CTAs are persistent: the weights are loaded once per CTA, the tiles are walked with a grid stride.
 //   Epilogue: registers -> bias / ReLU -> fp32 staging tile -> (max-pool) -> split -> planes of the next layer.
-//   For CIN <= 32 one tap is kept in flight (its A fragments load while the previous tap's wgmmas run); where the
-//   staging tile does not alias the A tile, the A tile is double-buffered (conv_split_kernel).
+//   One tap (CIN <= 32) or half a tap (CIN 64) is kept in flight: its A fragments load while the previous unit's
+//   wgmmas run.  Where the staging tile does not alias the A tile, the A tile is double-buffered (conv_split_kernel).
 //
 // The fused kernel (conv12_kernel) also computes conv1 + BN + ReLU + pool1 of the tile's segment straight into the A
 // tile, so pool1 never reaches HBM; two warpgroups run the GEMM while the other two compute conv1 of the next tile
@@ -51,31 +53,39 @@ namespace nisqa {
 
 // ---- pieces shared by the two kernels ----
 
-// A fragments of one tap for this warpgroup's NB m64 blocks: block b reads tile rows row + 64 b
+// The K steps of one tap go to the tensor cores in units of UK k16 steps: a whole tap for CIN <= 32, half a tap for
+// CIN 64 (two fragment sets of a whole 64-channel tap do not fit beside the accumulators in 128 registers).
+template <class C>
+struct TapUnits {
+  static constexpr int KS = C::CIN / 16, UK = KS < 2 ? KS : 2, PER_TAP = KS / UK, N = 9 * PER_TAP;
+};
+
+// A fragments of K steps k0 .. k0 + UK - 1 of one tap (row offset tapoff) for this warpgroup's NB m64 blocks: block b
+// reads tile row row[b] + tapoff
 template <class C, int NB>
-__device__ __forceinline__ void load_tap(uint32_t a_hi, uint32_t a_lo, int row, int lchunk,
-                                         uint32_t (&ah)[NB][C::CIN / 16][4], uint32_t (&al)[NB][C::CIN / 16][4]) {
+__device__ __forceinline__ void load_unit(uint32_t a_hi, uint32_t a_lo, const int (&row)[NB], int tapoff, int k0, int lchunk,
+                                          uint32_t (&ah)[NB][TapUnits<C>::UK][4], uint32_t (&al)[NB][TapUnits<C>::UK][4]) {
 #pragma unroll
   for (int b = 0; b < NB; ++b)
 #pragma unroll
-    for (int ks = 0; ks < C::CIN / 16; ++ks) {
-      const uint32_t ao = (uint32_t)split_off<C::ROWB>(row + 64 * b, 2 * ks + lchunk);
+    for (int ks = 0; ks < TapUnits<C>::UK; ++ks) {
+      const uint32_t ao = (uint32_t)split_off<C::ROWB>(row[b] + tapoff, 2 * (k0 + ks) + lchunk);
       ldsm_x4(a_hi + ao, ah[b][ks]);
       ldsm_x4(a_lo + ao, al[b][ks]);
     }
 }
 
-// the wgmmas of one tap (weights at bst) for NB m64 blocks; no fence / commit
+// the wgmmas of K steps k0 .. k0 + UK - 1 of one tap (weights at bst) for NB m64 blocks; no fence / commit
 template <class C, int NB>
-__device__ __forceinline__ void mma_tap(float (&acc_m)[NB][C::COUT / 2], float (&acc_s)[NB][C::COUT / 2],
-                                        const uint32_t (&ah)[NB][C::CIN / 16][4], const uint32_t (&al)[NB][C::CIN / 16][4],
-                                        uint32_t bst) {
+__device__ __forceinline__ void mma_unit(float (&acc_m)[NB][C::COUT / 2], float (&acc_s)[NB][C::COUT / 2],
+                                         const uint32_t (&ah)[NB][TapUnits<C>::UK][4],
+                                         const uint32_t (&al)[NB][TapUnits<C>::UK][4], uint32_t bst, int k0) {
   constexpr int COUT = C::COUT;
 #pragma unroll
   for (int b = 0; b < NB; ++b)
 #pragma unroll
-    for (int ks = 0; ks < C::CIN / 16; ++ks) {
-      const uint32_t bk = bst + (uint32_t)(2 * ks) * (2 * COUT * 16);
+    for (int ks = 0; ks < TapUnits<C>::UK; ++ks) {
+      const uint32_t bk = bst + (uint32_t)(2 * (k0 + ks)) * (2 * COUT * 16);
       const uint64_t dbh = make_desc_b(bk, 2 * COUT * 16), dbl = make_desc_b(bk + COUT * 16, 2 * COUT * 16);
       wgmma_rs<COUT>(acc_m[b], ah[b][ks], dbh);
       wgmma_rs<COUT>(acc_s[b], ah[b][ks], dbl);
@@ -84,63 +94,48 @@ __device__ __forceinline__ void mma_tap(float (&acc_m)[NB][C::COUT / 2], float (
 }
 
 // The GEMM of one tile for this warpgroup's NB m64 blocks: acc_m[b] = hi*hi, acc_s[b] = hi*lo + lo*hi over the nine
-// taps, in tap order.  `row` is this lane's ldmatrix row of block 0 at tap offset 0.
+// taps, in tap order.  row[b] is this lane's ldmatrix row of block b at tap offset 0.
 template <class C, int NB>
 __device__ __forceinline__ void tile_gemm(float (&acc_m)[NB][C::COUT / 2], float (&acc_s)[NB][C::COUT / 2], uint32_t a_hi,
-                                          uint32_t a_lo, uint32_t b_base, uint32_t bar_w, int row, int lchunk) {
-  constexpr int P = C::P, KS = C::CIN / 16;
+                                          uint32_t a_lo, uint32_t b_base, uint32_t bar_w, const int (&row)[NB], int lchunk) {
+  using U = TapUnits<C>;
+  constexpr int P = C::P, UK = U::UK, PT = U::PER_TAP;
+  static_assert(C::CIN <= 32 || NB == 1, "CIN 64: one m64 block per warpgroup");
 #pragma unroll
   for (int b = 0; b < NB; ++b)
 #pragma unroll
     for (int i = 0; i < C::COUT / 2; ++i) { acc_m[b][i] = 0.f; acc_s[b][i] = 0.f; }
-  if constexpr (C::CIN <= 32) {
-    // one tap in flight: tap t + 1's fragments load into the other register set while tap t's wgmmas run.  All nine
-    // weight taps are waited for up front: a wait loop between in-flight wgmmas makes ptxas serialize them.
-    for (int t = 0; t < 9; ++t) mbar_wait(bar_w + 8 * t, 0);
-    uint32_t ah[2][NB][KS][4], al[2][NB][KS][4];
-    load_tap<C, NB>(a_hi, a_lo, row - P - 1, lchunk, ah[0], al[0]);
+  // one unit in flight: unit u + 1's fragments load into the other register set while unit u's wgmmas run.  All nine
+  // weight taps are waited for up front: a wait loop between in-flight wgmmas makes ptxas serialize them.
+  for (int t = 0; t < 9; ++t) mbar_wait(bar_w + 8 * t, 0);
+  uint32_t ah[2][NB][UK][4], al[2][NB][UK][4];
+  load_unit<C, NB>(a_hi, a_lo, row, -P - 1, 0, lchunk, ah[0], al[0]);
 #pragma unroll
-    for (int t = 0; t < 9; ++t) {
-      wgmma_fence();
-      mma_tap<C, NB>(acc_m, acc_s, ah[t & 1], al[t & 1], b_base + t * C::B_STAGE);
-      wgmma_commit();
-      if (t < 8) {
-        wgmma_wait<1>();                         // tap t - 1 is done with the set that tap t + 1 loads into
-        const int u = t + 1;
-        load_tap<C, NB>(a_hi, a_lo, row + (u / 3 - 1) * P + (u % 3 - 1), lchunk, ah[u & 1], al[u & 1]);
-      }
-    }
-    wgmma_wait<0>();
-  } else {
-    static_assert(NB == 1, "CIN 64: one m64 block per warpgroup");
-#pragma unroll 1
-    for (int t = 0; t < 9; ++t) {
-      mbar_wait(bar_w + 8 * t, 0);
-      const int tapoff = (t / 3 - 1) * P + (t % 3 - 1);
-      uint32_t ah[1][KS][4], al[1][KS][4];
-      load_tap<C, 1>(a_hi, a_lo, row + tapoff, lchunk, ah, al);
-      wgmma_fence();
-      mma_tap<C, 1>(acc_m, acc_s, ah, al, b_base + t * C::B_STAGE);
-      wgmma_commit();
-      wgmma_wait<0>();                           // the A fragments are overwritten by the next tap's loads
+  for (int u = 0; u < U::N; ++u) {
+    wgmma_fence();
+    mma_unit<C, NB>(acc_m, acc_s, ah[u & 1], al[u & 1], b_base + (u / PT) * C::B_STAGE, (u % PT) * UK);
+    wgmma_commit();
+    if (u + 1 < U::N) {
+      wgmma_wait<1>();                           // unit u - 1 is done with the set that unit u + 1 loads into
+      const int v = u + 1, t = v / PT;
+      load_unit<C, NB>(a_hi, a_lo, row, (t / 3 - 1) * P + (t % 3 - 1), (v % PT) * UK, lchunk, ah[v & 1], al[v & 1]);
     }
   }
+  wgmma_wait<0>();
 }
 
-// epilogue part 1 for one m64 block: accumulators -> bias + ReLU -> staging rows arow0 and arow0 + 8
+// epilogue part 1 for one m64 block: accumulators of GEMM rows m0 and m0 + 8 -> bias + ReLU -> the staging rows of
+// their plane positions (every interior position of the tile's live segments is written: store_tile reads them all)
 template <class C>
-__device__ __forceinline__ void stage_rows(const float (&acc_m)[C::COUT / 2], const float (&acc_s)[C::COUT / 2], int arow0,
+__device__ __forceinline__ void stage_rows(const float (&acc_m)[C::COUT / 2], const float (&acc_s)[C::COUT / 2], int m0,
                                            int acol, int seg0, int n_seg, const float* __restrict__ bias, float out_scale,
                                            float* stg) {
-  constexpr int P = C::P, BLK = C::BLK, SS = C::STG_STRIDE;
+  constexpr int SS = C::STG_STRIDE;
 #pragma unroll
   for (int half = 0; half < 2; ++half) {
-    const int r = arow0 + 8 * half;
-    const int s = r / BLK, q = r - s * BLK;
-    const int hh = q / P, ww = q - hh * P;
-    bool valid = (s < C::G) && (seg0 + s < n_seg) && hh >= 1 && ww >= 1;
-    if (C::CENTER) valid = valid && (ww == 2);
-    if (valid) {
+    const int m = m0 + 8 * half;
+    if (m < C::KEPT && seg0 + m / C::SEG_ROWS < n_seg) {
+      const int r = C::gemm_row(m);
 #pragma unroll
       for (int j = 0; j < C::COUT / 8; ++j) {
         const int col = 8 * j + acol;
@@ -217,7 +212,8 @@ __device__ __forceinline__ void store_tile(const float* stg, int seg0, int nvali
 }
 
 // ---- conv2..conv6 on planes ----
-// Four warpgroups own 64 rows each and run GEMM, epilogue part 1, part 2 in turn.  Without aliasing (conv2, conv3)
+// Warpgroup b < NBLK owns m64 block b (3 blocks, 1 for conv6A) and runs GEMM and epilogue part 1; all four run part 2.
+// One warpgroup's wgmmas already use the tensor cores of all four SM sub-partitions.  Without aliasing (conv2, conv3)
 // the activation tile is double-buffered: one thread issues the next tile's copy into the other buffer as soon as
 // that buffer's readers (the previous tile's GEMM) have arrived on its empty barrier.
 template <class C>
@@ -261,8 +257,8 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
   }
   __syncthreads();
 
-  // this lane's ldmatrix row (within its warp's 16 rows) and K chunk; its accumulator rows
-  const int lrow = wg * 64 + (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+  // this lane's ldmatrix row (the tile row of GEMM row m within its warp's 16 rows) and K chunk; its accumulator rows
+  const int lrow = HALO + C::gemm_row(wg * 64 + (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8);
   const int lchunk = lane >> 4;
   const int arow0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const int acol = 2 * (lane & 3);
@@ -285,16 +281,23 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
       mbar_wait(bar_full + 8 * ab, (it >> 1) & 1);
     }
 
-    // ===== GEMM: warpgroup wg, rows 64 wg .. 64 wg + 63 =====
+    // ===== GEMM: warpgroup wg < NBLK, GEMM rows 64 wg .. 64 wg + 63; the others have no rows and wait =====
     const uint32_t a_hi = sbase + C::OFF_A_HI + ab * C::A_BUF, a_lo = a_hi + C::A_BYTES;
+    // The accumulators are defined on both sides of the branch and its condition is broadcast from lane 0: without
+    // either, ptxas spills (CIN 64) or serializes the wgmmas (CIN <= 32).
     float acc_m[1][C::COUT / 2], acc_s[1][C::COUT / 2];      // hi*hi ; hi*lo + lo*hi
-    tile_gemm<C, 1>(acc_m, acc_s, a_hi, a_lo, b_base, bar_w, (g0 & 7) + HALO + lrow, lchunk);
+#pragma unroll
+    for (int i = 0; i < C::COUT / 2; ++i) { acc_m[0][i] = 0.f; acc_s[0][i] = 0.f; }
+    if (__shfl_sync(0xffffffffu, wg < C::NBLK, 0)) {
+      const int row[1] = {(g0 & 7) + lrow};
+      tile_gemm<C, 1>(acc_m, acc_s, a_hi, a_lo, b_base, bar_w, row, lchunk);
+    }
     if constexpr (!C::ALIAS) mbar_arrive(bar_empty + 8 * ab);
     __syncthreads();                             // ALIAS: every warpgroup is done with the A tile the staging tile
                                                  // overwrites; otherwise the previous tile's part 2 is done with it
 
-    // ===== epilogue part 1: accumulators -> bias + ReLU -> staging row r =====
-    stage_rows<C>(acc_m[0], acc_s[0], arow0, acol, seg0, n_seg, bias, out_scale, stg);
+    // ===== epilogue part 1: accumulators -> bias + ReLU -> staging row of each GEMM row's plane position =====
+    stage_rows<C>(acc_m[0], acc_s[0], arow0, acol, seg0, n_seg, bias, out_scale, stg);   // (no rows past block NBLK - 1)
     __syncthreads();
 
     // ===== epilogue part 2 (all threads): max-pool / split / store =====
@@ -355,9 +358,10 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
 
   // registers: 64 accumulators and two fragment sets per MMA thread; 2 x 128 x (160 + 96) = the whole register file
   if (wg < 2) {
-    // ===== MMA warpgroups: block b of warpgroup wg = tile rows 128 wg + 64 b .. + 63 =====
+    // ===== MMA warpgroups: block b of warpgroup wg = GEMM rows 128 wg + 64 b .. + 63 =====
     setmaxnreg_inc<160>();
-    const int lrow = wg * 128 + (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+    const int lm = wg * 128 + (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+    const int lrow[2] = {HALO + C::gemm_row(lm), HALO + C::gemm_row(lm + 64)};
     const int lchunk = lane >> 4;
     const int arow0 = wg * 128 + (warp & 3) * 16 + (lane >> 2);
     const int acol = 2 * (lane & 3);
@@ -368,7 +372,7 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
       mbar_wait(a_full + 8 * ab, par);
       const uint32_t a_hi = sbase + L::OFF_A + ab * C::A_BUF, a_lo = a_hi + C::A_BYTES;
       float acc_m[2][C::COUT / 2], acc_s[2][C::COUT / 2];
-      tile_gemm<C, 2>(acc_m, acc_s, a_hi, a_lo, b_base, bar_w, HALO + lrow, lchunk);
+      tile_gemm<C, 2>(acc_m, acc_s, a_hi, a_lo, b_base, bar_w, lrow, lchunk);
       mbar_arrive(a_empty + 8 * ab);
       float* stg = reinterpret_cast<float*>(smem + L::OFF_STG + ab * C::STG_BYTES);
 #pragma unroll

@@ -20,7 +20,7 @@ __device__ __forceinline__ size_t split_off(int g, int c) {
 
 template <int H_, int W_, int CIN_, int COUT_, int POOL_, int POW_, bool F32OUT_ = false, bool CENTER_ = false>
 struct SpCfg {
-  static constexpr int NT = 4 * 128;             // four warpgroups, 64 GEMM rows each
+  static constexpr int NT = 4 * 128;             // four warpgroups; warpgroup b < NBLK runs m64 block b
   static constexpr int H = H_, W = W_, CIN = CIN_, COUT = COUT_, POOL = POOL_, POW = POW_;
   static constexpr bool CENTER = CENTER_;         // conv6 of the AdaptCNN: kernel (3,3), padding (1,0) on a
                                                   // 3-wide map == the padded conv evaluated at column 1 only
@@ -30,6 +30,19 @@ struct SpCfg {
   static constexpr int G = 256 / BLK;             // segments per tile (256 GEMM rows)
   static constexpr int HALO = P + 1;              // |row offset| of the farthest tap
   static constexpr int AROWS = 256 + 2 * HALO;    // rows of the tile (copied)
+  // GEMM rows: only the tile's interior output positions, in (segment, h, w) order (conv6A: the centre column only),
+  // packed into NBLK m64 blocks.  GEMM row m reads its taps around tile row HALO + gemm_row(m).
+  static constexpr int KW = CENTER ? 1 : W;       // output columns per row
+  static constexpr int SEG_ROWS = H * KW;         // GEMM rows per segment
+  static constexpr int KEPT = G * SEG_ROWS;
+  static constexpr int NBLK = (KEPT + 63) / 64;
+  // plane row of GEMM row m, counted from the zero row of the tile's first segment.  Rows m >= KEPT read that zero row;
+  // the rows of segments past the end of a short last tile read the copied range as it lies.  Neither is staged.
+  __host__ __device__ static constexpr int gemm_row(int m) {
+    if (m >= KEPT) return 0;
+    const int s = m / SEG_ROWS, q = m - s * SEG_ROWS, h = q / KW, w = q - h * KW;
+    return s * BLK + (h + 1) * P + (CENTER ? 2 : w + 1);
+  }
   static constexpr int ROWB = CIN * 2;            // bytes per row
   static constexpr int A_BYTES = ((AROWS + 7) * ROWB + 1023) & ~1023;     // + placement shift (g0 & 7 rows)
   static constexpr int NCH = CIN / 8;             // 16-byte K chunks (8 halves)
@@ -67,6 +80,7 @@ struct SpCfg {
   static_assert(!CENTER || F32OUT_, "the centre-column variant only exists as the last layer");
   static_assert(OUT_SPLIT || POOL == SP_POOL_NONE, "fp32 output is not pooled");
   static_assert(G >= 1, "tile");
+  static_assert(NBLK <= 4 && (!CENTER || W == 3), "GEMM rows");
 };
 
 // layers 2..6; std_mode selects the StandardCNN geometry (W 8/4/2, MaxPool2d(2))
