@@ -37,7 +37,9 @@ typedef struct nisqa_engine nisqa_engine;
 /* architectures of the shipped checkpoints (SURVEY.md 0.4) */
 enum nisqa_arch {
   NISQA_ARCH_ADAPT_SA_ATTFF  = 0, /* nisqa.tar, nisqa_mos_only.tar: AdaptCNN + SelfAttention + PoolAttFF */
-  NISQA_ARCH_STD_LSTM_LASTBI = 1  /* nisqa_tts.tar: StandardCNN + BiLSTM + PoolLastStepBi            */
+  NISQA_ARCH_STD_LSTM_LASTBI = 1  /* nisqa_tts.tar: StandardCNN + BiLSTM + PoolLastStepBi; also any other
+                                   * StandardCNN + LSTM checkpoint: its LSTM shape is read from the tensors given to
+                                   * nisqa_load_weights (weight_hh_l{k}[_reverse], cnn.model.fc_out.*)            */
 };
 
 /* pooling over time (reference lib:1066-1225).  The shipped checkpoints use ATT_FF (nisqa*.tar) and LAST_STEP_BI
@@ -84,10 +86,11 @@ enum nisqa_stage {
   NISQA_STAGE_CONV3    = 3, /* [n_seg, 64, 12, W2]                                           */
   NISQA_STAGE_POOL3    = 4, /* [n_seg, 64, 6, W3]                                            */
   NISQA_STAGE_CONV5    = 5, /* [n_seg, 64, 6, W3]                                            */
-  NISQA_STAGE_CNN_FEAT = 6, /* [n_seg, 384] (adapt, index c*6+h) or [n_seg, 20] (standard)   */
+  NISQA_STAGE_CNN_FEAT = 6, /* [n_seg, 384] (adapt, index c*6+h) or [n_seg, F] (standard: fc_out's width F, or 768 in
+                             * index c*12+h*2+w without fc_out)                                                        */
   NISQA_STAGE_TD_IN    = 7, /* adapt only: LayerNorm(Linear 384->D) [n_seg, D], D = sa_d_model */
   NISQA_STAGE_TD_OUT   = 8  /* [n_seg, D] (output of the last self-attention stack: td2_d_model when td_2 runs, else
-                             * sa_d_model) or [n_seg, 256] (BiLSTM fwd||bwd)                                          */
+                             * sa_d_model) or [n_seg, dirs*H] (the last LSTM layer, fwd||bwd)                          */
 };
 
 /* Mirrors the checkpoint 'args' the hot path consumes (SURVEY.md Appendix A). */
@@ -282,7 +285,7 @@ NISQA_API int    nisqa_set_profiling(nisqa_engine* e, int on);
  *                (csrc/td_tiled.cu); 0: the one-thread-per-row kernels of csrc/td.cu.
  *   "lstm_batched" 1 (default): BiLSTM advances up to four clips per CTA in lock step; 0: one CTA per
  *                (clip, direction).
- *   "keep_td_out" standard architecture: 1 = also store the per-step BiLSTM outputs so that
+ *   "keep_td_out" nisqa_tts.tar's LSTM shape: 1 = also store the per-step BiLSTM outputs so that
  *                NISQA_STAGE_TD_OUT can be dumped (default 0: only the final states are needed, lib:1107-1115). */
 NISQA_API int    nisqa_set_option(nisqa_engine* e, const char* name, int value);
 NISQA_API double nisqa_group_ms(const nisqa_engine* e, const char* group);

@@ -100,7 +100,7 @@ constexpr int kLanes = NISQA_LANES;
 constexpr int kStages = 6;     // staging slots / submissions in flight (uploads run ahead of the lanes)
 struct Lane {
   cudaStream_t stream = nullptr;
-  DevBuf mel, segtab, feats, xa, xb, qkv, qkv2, logits, feats20, tdout, partial, fused, td2in, ffa, ffb;
+  DevBuf mel, segtab, feats, xa, xb, qkv, qkv2, logits, feats20, tdout, partial, fused, td2in, ffa, ffb, gx, atth;
   DevBuf act[7];           // act[l]: fp32 channels-last map feeding conv layer l (2..6) on the FFMA path (and stage dumps)
   DevBuf planes[7];        // planes[l]: fp16 hi | lo plane pair feeding conv layer l (2..6), conv_split.cu
   size_t plane_bytes[7] = {0, 0, 0, 0, 0, 0, 0};   // offset of the lo plane inside planes[l] (half of the allocation)
@@ -108,7 +108,7 @@ struct Lane {
     for (auto& b : act) b.release();
     for (auto& b : planes) b.release();
     DevBuf* all[] = {&mel, &segtab, &feats, &xa, &xb, &qkv, &qkv2, &logits, &feats20, &tdout, &partial, &fused, &td2in,
-                     &ffa, &ffb};
+                     &ffa, &ffb, &gx, &atth};
     for (auto* b : all) b->release();
     if (stream) cudaStreamDestroy(stream);
   }
@@ -164,8 +164,14 @@ struct Weights {
   DeAlignParams de = {};
   PoolHeadParams pool_head = {};       // PoolAttFF
   PoolSimpleParams pool_simple = {};   // the other pooling modules
-  Linear fc;                     // StandardCNN fc_out 768 -> 20
+  Linear fc;                     // StandardCNN fc_out 768 -> 20 (any width on the stacked-LSTM path: 64-column padded)
   LstmParams lstm = {};
+  // The LSTM's shape, read from the checkpoint's tensors.  `stacked`: every shape but the shipped one (fc_out 20, one
+  // bidirectional layer of 128, one output, no attention pooling), which keeps lstm_batched_kernel.
+  struct LstmShape { bool stacked = false; int fc = 0, H = 0, layers = 0, dirs = 0; } lstm_shape;
+  Linear lstm_ih[4];             // stacked path: W_ih^T of each layer k-major [K pad 64][dirs 4H], bias b_ih + b_hh
+  const float* lstm_hh[4] = {};  // [dirs][4H][H]
+  Linear lstm_att;               // PoolAttFF behind the LSTM: linear1 of every head, k-major [D pad 64][n_heads 128]
 };
 
 }  // namespace
@@ -228,6 +234,7 @@ struct nisqa_engine {
   const float* last_td_in = nullptr;
   const float* last_td_out = nullptr;
   int last_td_out_d = 64;       // row width of last_td_out
+  int last_td_out_ld = 0;       // its row stride (0: the width)
 
   // engine-owned NCCL communicator (multi-GPU gather, SURVEY.md 8e)
   void* nccl_comm = nullptr;
@@ -683,14 +690,19 @@ bool pack_de_align(Packer& P, const nisqa_config& c) {
   return true;
 }
 
-// The pooling module behind self-attention, one head per output (order mos, noi, dis, col, loud: lib:1461-1465), reading
-// Dp-wide rows: PoolAttFF, or PoolAtt / PoolAvg / PoolMax / PoolLastStep
-bool pack_pool_heads(Packer& P, const nisqa_config& c, int Dp) {
+int round64(int n) { return (n + 63) / 64 * 64; }
+
+// The pooling module behind the time-dependency block, one head per output (order mos, noi, dis, col, loud:
+// lib:1461-1465), reading Dp-wide rows: PoolAttFF, or PoolAtt / PoolAvg / PoolMax / PoolLastStep / PoolLastStepBi.
+// PoolAttFF's linear1: [head][Dp][128] for td_sa_kernel's fused tail (self-attention), or - behind an LSTM - k-major
+// [Dp padded to 64][head 128] for the tile GEMM (lstm_att)
+bool pack_pool_heads(Packer& P, const nisqa_config& c, int Dp, bool lstm = false) {
   const int nh = c.n_out;
   auto prefix = [&](int h) { return nh == 1 ? std::string("pool.model.") : "pool_layers." + std::to_string(h) + ".model."; };
   if (c.pool == NISQA_POOL_ATT_FF) {
     PoolHeadParams& H = P.w.pool_head;
-    const size_t oW1 = P.alloc(H.W1T, (size_t)nh * Dp * 128), ob1 = P.alloc(H.b1, nh * 128),
+    const size_t oW1 = lstm ? P.alloc(P.w.lstm_att.wT, (size_t)round64(Dp) * nh * 128) : P.alloc(H.W1T, (size_t)nh * Dp * 128),
+                 ob1 = lstm ? P.alloc(P.w.lstm_att.b, nh * 128) : P.alloc(H.b1, nh * 128),
                  ow2 = P.alloc(H.w2, nh * 128), ob2 = P.alloc(H.b2, nh),
                  ow3 = P.alloc(H.w3, nh * Dp), ob3 = P.alloc(H.b3, nh);
     for (int h = 0; h < nh; ++h) {
@@ -702,7 +714,12 @@ bool pack_pool_heads(Packer& P, const nisqa_config& c, int Dp) {
       const TensorView* w3 = P.get(p + "linear3.weight", {1, Dp});
       const TensorView* b3 = P.get(p + "linear3.bias", {1});
       if (!w1 || !b1 || !w2 || !b2 || !w3 || !b3) return false;
-      pack_linear_T(P, oW1 + (size_t)h * Dp * 128, w1, 128, Dp);          // [head][D][128]
+      if (lstm) {
+        for (int k = 0; k < Dp; ++k)
+          for (int j = 0; j < 128; ++j) P.arena[oW1 + (size_t)k * nh * 128 + h * 128 + j] = w1->d[(size_t)j * Dp + k];
+      } else {
+        pack_linear_T(P, oW1 + (size_t)h * Dp * 128, w1, 128, Dp);        // [head][D][128]
+      }
       memcpy(&P.arena[ob1 + h * 128], b1->d, 512);
       memcpy(&P.arena[ow2 + h * 128], w2->d, 512);
       P.arena[ob2 + h] = b2->d[0];
@@ -761,8 +778,8 @@ bool pack_sa_model(Packer& P, nisqa_engine* e) {
   return pack_pool_heads(P, c, e->pool_d());
 }
 
-// The StandardCNN architecture behind the convolutions: fc_out 768 -> 20, the BiLSTM and its pooling module
-bool pack_lstm_model(Packer& P, nisqa_engine* e) {
+// The shipped StandardCNN + LSTM shape (nisqa_tts.tar): fc_out 768 -> 20, the BiLSTM(20 -> 128) and its pooling module
+bool pack_bilstm128(Packer& P, nisqa_engine* e) {
   const TensorView* fw = P.get("cnn.model.fc_out.weight", {20, 768});
   const TensorView* fb = P.get("cnn.model.fc_out.bias", {20});
   if (!fw || !fb) return false;
@@ -794,6 +811,77 @@ bool pack_lstm_model(Packer& P, nisqa_engine* e) {
   P.copy(P.w.pool_simple.w3, pw->d, 256);
   P.copy(P.w.pool_simple.b3, pb->d, 1);
   return true;
+}
+
+// Any other StandardCNN + LSTM shape: fc_out 768 -> F (or none), `layers` LSTM layers of H units in `dirs` directions,
+// W_ih and W_hh of each layer, and the pooling module over D = dirs H.  Input rows of layer 0 are fc_out's (padded to a
+// multiple of 64 with zero columns) or conv6's 768 features in the engine's order; those of layer l > 0 are layer l - 1's
+// outputs, padded the same way.  Zero weights in the padding keep every product exact.
+bool pack_lstm_stack(Packer& P, nisqa_engine* e, const Weights::LstmShape& L) {
+  const std::string p = "time_dependency.model.lstm.";
+  const int H = L.H, N = L.dirs * 4 * H, D = L.dirs * H;
+  if (L.fc > 0) {
+    const TensorView* fw = P.get("cnn.model.fc_out.weight", {L.fc, 768});
+    const TensorView* fb = P.get("cnn.model.fc_out.bias", {L.fc});
+    if (!fw || !fb) return false;
+    const int Fp = round64(L.fc);
+    const size_t o = P.alloc(P.w.fc.wT, (size_t)768 * Fp);
+    for (int hw = 0; hw < 12; ++hw)            // engine order k' = (h*2 + w)*64 + c <-> reference view order c*12 + h*2 + w
+      for (int c = 0; c < 64; ++c)
+        for (int j = 0; j < L.fc; ++j) P.arena[o + ((size_t)hw * 64 + c) * Fp + j] = fw->d[(size_t)j * 768 + c * 12 + hw];
+    memcpy(&P.arena[P.alloc(P.w.fc.b, Fp)], fb->d, (size_t)L.fc * 4);
+  }
+  for (int l = 0; l < L.layers; ++l) {
+    const int in = l ? D : (L.fc ? L.fc : 768), K = round64(in);
+    const size_t owi = P.alloc(P.w.lstm_ih[l].wT, (size_t)K * N), ob = P.alloc(P.w.lstm_ih[l].b, N);
+    const size_t owh = P.alloc(P.w.lstm_hh[l], (size_t)L.dirs * 4 * H * H);
+    for (int d = 0; d < L.dirs; ++d) {
+      const std::string sfx = "_l" + std::to_string(l) + (d ? "_reverse" : "");
+      const TensorView* wi = P.get(p + "weight_ih" + sfx, {4 * H, in});
+      const TensorView* wh = P.get(p + "weight_hh" + sfx, {4 * H, H});
+      const TensorView* bi = P.get(p + "bias_ih" + sfx, {4 * H});
+      const TensorView* bh = P.get(p + "bias_hh" + sfx, {4 * H});
+      if (!wi || !wh || !bi || !bh) return false;
+      for (int k = 0; k < in; ++k) {
+        // layer 0 without fc_out reads conv6's features in the engine's order (see above)
+        const int kc = (l == 0 && L.fc == 0) ? (k & 63) * 12 + (k >> 6) : k;
+        for (int g = 0; g < 4 * H; ++g) P.arena[owi + (size_t)k * N + d * 4 * H + g] = wi->d[(size_t)g * in + kc];
+      }
+      for (int g = 0; g < 4 * H; ++g) P.arena[ob + d * 4 * H + g] = bi->d[g] + bh->d[g];
+      memcpy(&P.arena[owh + (size_t)d * 4 * H * H], wh->d, (size_t)4 * H * H * 4);
+    }
+  }
+  return pack_pool_heads(P, e->cfg, D, true);
+}
+
+// The StandardCNN architecture behind the convolutions: its LSTM's shape comes from the tensors (the weight_hh_l{k}
+// [_reverse] shapes give H, the layer count and the directions; cnn.model.fc_out.* present or not gives fc_out's width)
+bool pack_lstm_model(Packer& P, nisqa_engine* e) {
+  const nisqa_config& c = e->cfg;
+  const std::string p = "time_dependency.model.lstm.";
+  Weights::LstmShape L;
+  auto it = P.t.find(p + "weight_hh_l0");
+  if (it == P.t.end()) return P.fail("missing tensor " + p + "weight_hh_l0");
+  L.H = it->second.nd == 2 ? (int)it->second.dims[1] : 0;
+  if (!lstm_layer_supported(L.H) || it->second.dims[0] != 4 * L.H)
+    return P.fail("tensor " + p + "weight_hh_l0: hidden size " + std::to_string(L.H) +
+                  " is not implemented by the engine (td_lstm_h 32, 64, 96, 128, 192 or 256)");
+  while (P.t.count(p + "weight_hh_l" + std::to_string(L.layers))) ++L.layers;
+  if (L.layers > 4)
+    return P.fail("tensor " + p + "weight_hh_l4: the engine runs 1 to 4 LSTM layers");
+  L.dirs = P.t.count(p + "weight_hh_l0_reverse") ? 2 : 1;
+  if (c.pool == NISQA_POOL_LAST_STEP_BI && L.dirs != 2)
+    return P.fail("missing tensor " + p + "weight_hh_l0_reverse: PoolLastStepBi needs a bidirectional LSTM");
+  auto fc = P.t.find("cnn.model.fc_out.weight");
+  if (fc != P.t.end()) {
+    L.fc = fc->second.nd == 2 ? (int)fc->second.dims[0] : 0;
+    if (L.fc < 1 || L.fc > 1024)
+      return P.fail("tensor cnn.model.fc_out.weight: width " + std::to_string(L.fc) + " outside 1..1024");
+  }
+  L.stacked = !(L.fc == 20 && L.H == 128 && L.layers == 1 && L.dirs == 2 && c.n_out == 1 && c.pool != NISQA_POOL_ATT &&
+                c.pool != NISQA_POOL_ATT_FF);
+  P.w.lstm_shape = L;
+  return L.stacked ? pack_lstm_stack(P, e, L) : pack_bilstm128(P, e);
 }
 
 int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
@@ -1143,16 +1231,71 @@ int sa_head(Pass& p, Rows rows) {
   }
   e->last_td_out = cur;
   e->last_td_out_d = e->pool_d();
+  e->last_td_out_ld = e->pool_d();
   { Scope s(e, "pool");
     if (c.pool == NISQA_POOL_ATT_FF)
-      launch_pool_final(p.st, cur, e->pool_d(), LN.logits.as<float>(), p.clips, p.n, p.w.pool_head, n_out, p.max_n_seg, p.scores);
+      launch_pool_final(p.st, cur, e->pool_d(), e->pool_d(), LN.logits.as<float>(), p.clips, p.n, p.w.pool_head, n_out, p.max_n_seg,
+                        p.scores);
     else
-      launch_pool_simple(p.st, cur, e->pool_d(), p.clips, p.n, c.pool, p.w.pool_simple, n_out, p.max_n_seg, p.scores);
+      launch_pool_simple(p.st, cur, e->pool_d(), e->pool_d(), p.clips, p.n, c.pool, p.w.pool_simple, n_out, p.max_n_seg, p.scores);
     if (de) launch_de_finalize(p.st, p.clips, p.n, n_out, p.scores); }
   return 0;
 }
 
-// The StandardCNN architecture's fc_out 768 -> 20, BiLSTM and pooling (PoolLastStepBi fused into the BiLSTM launch)
+// Any other LSTM shape: fc_out (tile GEMM), then per layer the input projection of every step and direction (tile GEMM)
+// and the recurrence (lstm_layer_kernel); the pooling module reads the last layer's rows.  Rows are padded to a multiple
+// of 64 floats with zero columns (the next GEMM's K).
+int lstm_stack_head(Pass& p) {
+  nisqa_engine* e = p.e;
+  const nisqa_config& c = p.c;
+  Lane& LN = p.LN;
+  const Weights& w = p.w;
+  const Weights::LstmShape& L = w.lstm_shape;
+  const int n_seg = p.n_seg, H = L.H, N = L.dirs * 4 * H, D = L.dirs * H, Dp = round64(D), Fp = round64(L.fc);
+  CK(LN.gx.reserve((size_t)n_seg * N * 4));
+  CK(LN.tdout.reserve((size_t)n_seg * Dp * 4));
+  const float* x = LN.feats.as<float>();
+  int ldx = 768;
+  if (L.fc > 0) {
+    Scope s(e, "fc_out");
+    CK(LN.feats20.reserve((size_t)n_seg * Fp * 4));
+    launch_linear_tile(p.st, x, 768, w.fc.wT, w.fc.b, 0, LN.feats20.as<float>(), Fp, n_seg, 768, Fp);
+    x = LN.feats20.as<float>(); ldx = Fp;
+  }
+  float* inter[2] = {nullptr, nullptr};
+  for (int l = 0; l + 1 < L.layers && l < 2; ++l) {
+    DevBuf& b = l ? LN.xb : LN.xa;
+    CK(b.reserve((size_t)n_seg * Dp * 4));
+    inter[l] = b.as<float>();
+  }
+  for (int l = 0; l < L.layers; ++l) {
+    float* out = l + 1 == L.layers ? LN.tdout.as<float>() : inter[l & 1];
+    if (Dp != D) CK(cudaMemsetAsync(out, 0, (size_t)n_seg * Dp * 4, p.st));     // the padding columns the next GEMM reads
+    Scope s(e, "lstm", 2);
+    launch_linear_tile(p.st, x, ldx, w.lstm_ih[l].wT, w.lstm_ih[l].b, 0, LN.gx.as<float>(), N, n_seg, ldx, N);
+    const LstmLayerParams P = {LN.gx.as<float>(), N, w.lstm_hh[l], out, Dp};
+    launch_lstm_layer(p.st, H, L.dirs, p.clips, p.by_len, p.n, P);
+    x = out; ldx = Dp;
+  }
+  { Scope s(e, "pool", c.pool == NISQA_POOL_ATT_FF ? 3 : 1);
+    if (c.pool == NISQA_POOL_ATT_FF) {
+      const int nh = c.n_out;
+      CK(LN.atth.reserve((size_t)n_seg * nh * 128 * 4));
+      CK(LN.logits.reserve((size_t)n_seg * nh * 4));
+      launch_linear_tile(p.st, x, Dp, w.lstm_att.wT, w.lstm_att.b, 1, LN.atth.as<float>(), nh * 128, n_seg, Dp, nh * 128);
+      launch_att_logits(p.st, LN.atth.as<float>(), w.pool_head.w2, w.pool_head.b2, nh, n_seg, LN.logits.as<float>());
+      launch_pool_final(p.st, x, D, Dp, LN.logits.as<float>(), p.clips, p.n, w.pool_head, nh, p.max_n_seg, p.scores);
+    } else {
+      launch_pool_simple(p.st, x, D, Dp, p.clips, p.n, c.pool, w.pool_simple, c.n_out, p.max_n_seg, p.scores);
+    } }
+  e->last_td_in = nullptr;
+  e->last_td_out = x;
+  e->last_td_out_d = D;
+  e->last_td_out_ld = Dp;
+  return 0;
+}
+
+// The shipped shape's fc_out 768 -> 20, BiLSTM and pooling (PoolLastStepBi fused into the BiLSTM launch)
 int lstm_head(Pass& p) {
   nisqa_engine* e = p.e;
   const nisqa_config& c = p.c;
@@ -1174,11 +1317,12 @@ int lstm_head(Pass& p) {
                   e->pool_bias_std, lastbi ? p.scores : nullptr); }
   if (!lastbi) {
     Scope s(e, "pool");
-    launch_pool_simple(p.st, LN.tdout.as<float>(), 256, p.clips, p.n, c.pool, w.pool_simple, 1, p.max_n_seg, p.scores);
+    launch_pool_simple(p.st, LN.tdout.as<float>(), 256, 256, p.clips, p.n, c.pool, w.pool_simple, 1, p.max_n_seg, p.scores);
   }
   e->last_td_in = nullptr;
   e->last_td_out = (e->lstm_batched && !keep) ? nullptr : LN.tdout.as<float>();
   e->last_td_out_d = 256;
+  e->last_td_out_ld = 256;
   return 0;
 }
 
@@ -1192,7 +1336,7 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
   } else {
     Rows rows;
     rc = framewise(p, in.fmt, &rows);
-    if (!rc) rc = p.std_mode ? lstm_head(p) : sa_head(p, rows);
+    if (!rc) rc = !p.std_mode ? sa_head(p, rows) : p.w.lstm_shape.stacked ? lstm_stack_head(p) : lstm_head(p);
     if (rc) return rc;
   }
   CK(cudaGetLastError());
@@ -1333,14 +1477,12 @@ int nisqa_create(nisqa_engine** out, int device, const nisqa_config* cfg) {
   if (cfg->n_fft != kNfft || cfg->n_mels != kMels || cfg->seg_len != kSegLen)
     return fail(e, NISQA_ERR_INVALID, "engine is built for n_fft=4096, n_mels=48, seg_length=15");
   if (cfg->n_out != 1 && cfg->n_out != 5) return fail(e, NISQA_ERR_INVALID, "n_out must be 1 or 5");
-  if (cfg->arch == NISQA_ARCH_STD_LSTM_LASTBI && cfg->n_out != 1) return fail(e, NISQA_ERR_INVALID, "n_out");
   if (cfg->seg_hop < 1 || cfg->hop_s <= 0 || cfg->win_s <= 0 || cfg->fmax <= 0)
     return fail(e, NISQA_ERR_INVALID, "bad front-end parameters");
   if (cfg->arch == NISQA_ARCH_ADAPT_SA_ATTFF && (cfg->sa_layers < 1 || cfg->sa_layers > 8))
     return fail(e, NISQA_ERR_INVALID, "sa_layers");
   if (cfg->pool < NISQA_POOL_ATT_FF || cfg->pool > NISQA_POOL_LAST_STEP_BI ||
-      (cfg->arch == NISQA_ARCH_ADAPT_SA_ATTFF && cfg->pool == NISQA_POOL_LAST_STEP_BI) ||
-      (cfg->arch == NISQA_ARCH_STD_LSTM_LASTBI && (cfg->pool == NISQA_POOL_ATT_FF || cfg->pool == NISQA_POOL_ATT)))
+      (cfg->arch == NISQA_ARCH_ADAPT_SA_ATTFF && cfg->pool == NISQA_POOL_LAST_STEP_BI))
     return fail(e, NISQA_ERR_INVALID, "pooling module not available for this architecture");
   if (cfg->pos_enc && cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF) return fail(e, NISQA_ERR_INVALID, "pos_enc needs the self-attention architecture");
   if (cfg->cnn_kind < NISQA_CNN_CONV || cfg->cnn_kind > NISQA_CNN_DFF || cfg->cnn_fc < 0 || cfg->cnn_fc % 64 != 0 || cfg->cnn_fc > 8192 ||
@@ -1583,6 +1725,7 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
   int64_t count = 0;
   const float* src = nullptr;
   int hw = 0, ch = 0;    // NHWC -> NCHW conversion when ch > 0
+  int width = 0, ld = 0; // rows of `width` floats at a stride of `ld` (a padded row layout)
   if (conv_map) {
     const ConvGeom g = split_geometry(std_mode, layer);
     src = LN.act[layer].as<float>(); hw = g.H * g.W; ch = g.C;
@@ -1591,15 +1734,22 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
     case NISQA_STAGE_MEL_DB: count = (int64_t)e->last_n_frames * kMels; break;
     case NISQA_STAGE_POOL1: case NISQA_STAGE_POOL2: case NISQA_STAGE_CONV3: case NISQA_STAGE_POOL3: case NISQA_STAGE_CONV5: break;
     case NISQA_STAGE_CNN_FEAT:
-      if (std_mode) { src = LN.feats20.as<float>(); count = ns * 20; }
-      else { src = LN.feats.as<float>(); hw = 6; ch = 64; }     // [h][c] -> c*6+h
+      if (std_mode && e->w.lstm_shape.stacked && e->w.lstm_shape.fc > 0) {
+        src = LN.feats20.as<float>(); width = e->w.lstm_shape.fc; ld = round64(width); count = ns * width;
+      } else if (std_mode && e->w.lstm_shape.stacked) {
+        src = LN.feats.as<float>(); hw = 12; ch = 64;           // [h*2+w][c] -> c*12+h*2+w
+      } else if (std_mode) {
+        src = LN.feats20.as<float>(); count = ns * 20;
+      } else {
+        src = LN.feats.as<float>(); hw = 6; ch = 64;            // [h][c] -> c*6+h
+      }
       break;
     case NISQA_STAGE_TD_IN:
       if (std_mode || !e->last_td_in) return fail(e, NISQA_ERR_INVALID, "stage not available for this architecture");
       src = e->last_td_in; count = ns * e->sa_d(); break;
     case NISQA_STAGE_TD_OUT:
       if (!e->last_td_out) return fail(e, NISQA_ERR_STATE, "the per-step BiLSTM outputs were not kept: nisqa_set_option(\"keep_td_out\", 1) before the predict call");
-      src = e->last_td_out; count = ns * e->last_td_out_d; break;
+      src = e->last_td_out; count = ns * e->last_td_out_d; width = e->last_td_out_d; ld = e->last_td_out_ld; break;
     default: return fail(e, NISQA_ERR_INVALID, "unknown stage");
   }
   if (ch > 0) count = ns * hw * ch;
@@ -1627,7 +1777,10 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
     src = e->dump.as<float>();
   }
   if (!src) return fail(e, NISQA_ERR_STATE, "stage was not produced");
-  CK(cudaMemcpyAsync(out, src, (size_t)count * 4, cudaMemcpyDeviceToHost, st));
+  if (ld > width)
+    CK(cudaMemcpy2DAsync(out, (size_t)width * 4, src, (size_t)ld * 4, (size_t)width * 4, (size_t)ns, cudaMemcpyDeviceToHost, st));
+  else
+    CK(cudaMemcpyAsync(out, src, (size_t)count * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return count;
 }

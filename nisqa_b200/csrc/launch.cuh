@@ -52,6 +52,15 @@ struct LstmParams {
   const float* b;      // [2][512]   (bias_ih + bias_hh)
   const float* w_pool; // [256]
 };
+// One layer of a stacked LSTM of any accepted shape (td.cu lstm_layer_kernel): the input projection
+// gx = x W_ih^T + b_ih + b_hh of every step and direction comes precomputed from the tile GEMM
+struct LstmLayerParams {
+  const float* gx;     // [n_seg][ldg]: direction d's gate rows at columns d 4H .. d 4H + 4H (PyTorch order i, f, g, o)
+  int ldg;             // dirs 4H
+  const float* w_hh;   // [dirs][4H][H]
+  float* out;          // [n_seg][ldo]: direction d's hidden state at columns d H .. d H + H
+  int ldo;
+};
 // learned weights of AttLuong (wT [64][64] k-major, b [64]) / AttBahdanau (wqT, wyT [64][128] k-major, bq, by, v [128])
 struct DeAlignParams { const float* wT; const float* b; const float* wqT; const float* bq; const float* wyT; const float* by; const float* v; };
 struct ResampleClip {
@@ -94,9 +103,17 @@ void launch_lstm(cudaStream_t st, const float* feats20, const ClipDesc* clips, i
                  float* td_out, float* partial, float pool_bias, float* scores);
 void launch_lstm_batched(cudaStream_t st, const float* feats20, const ClipDesc* clips, const int* order, int n_clips,
                          const LstmParams& P, float* td_out, float* partial, float pool_bias, float* scores);
-void launch_pool_final(cudaStream_t st, const float* x, int D, const float* logits, const ClipDesc* clips, int n_clips,
+// one layer of a stacked LSTM, H in {32, 64, 96, 128, 192, 256}, dirs 1 or 2 (H 192 / 256: clusters of H / 64 CTAs)
+bool lstm_layer_supported(int H);
+void launch_lstm_layer(cudaStream_t st, int H, int dirs, const ClipDesc* clips, const int* order, int n_clips,
+                       const LstmLayerParams& P);
+// PoolAttFF logits of rows whose hidden layer relu(W1 x + b1) is already computed: [n_rows][n_heads 128] -> [n_rows][n_heads]
+void launch_att_logits(cudaStream_t st, const float* hid, const float* w2, const float* b2, int n_heads, int n_rows,
+                       float* logits);
+// x: rows of D features at a row stride of ldx floats
+void launch_pool_final(cudaStream_t st, const float* x, int D, int ldx, const float* logits, const ClipDesc* clips, int n_clips,
                        const PoolHeadParams& P, int n_heads, int max_seg, float* scores);
-void launch_pool_simple(cudaStream_t st, const float* x, int D, const ClipDesc* clips, int n_clips, int mode,
+void launch_pool_simple(cudaStream_t st, const float* x, int D, int ldx, const ClipDesc* clips, int n_clips, int mode,
                         const PoolSimpleParams& P, int n_heads, int max_seg, float* scores);
 
 // ---------------------------------------------------------------- td_tiled.cu (self-attention, NISQA_DE, SkipCNN / DFF)

@@ -71,11 +71,11 @@ linear_rows_kernel(const float* __restrict__ in, int K, const float* __restrict_
 
 // ---------------------------------------------------------------------------------------
 // PoolAttFF: softmax over the clip's time steps, weighted sum of x, Linear D->1   (lib:1177-1181)
-// grid = n_clips, block = 64 * n_heads; thread (h, d) owns features d, d + 64, .. < D.  The softmax numerators are formed once per (head, step) into shared
+// grid = n_clips, block = 64 * n_heads; thread (h, d) owns features d, d + 64, .. < D (rows ldx floats apart).  The softmax numerators are formed once per (head, step) into shared
 // memory; the weighted sum keeps ONE accumulator per thread in step order (the result does not depend on the unrolling) with
 // eight independent loads in flight.
 __global__ void pool_final_kernel(const float* __restrict__ x, const float* __restrict__ logits,
-                                  const ClipDesc* __restrict__ clips, PoolHeadParams P, int n_heads, int max_seg, int D,
+                                  const ClipDesc* __restrict__ clips, PoolHeadParams P, int n_heads, int max_seg, int D, int ldx,
                                   float* __restrict__ scores) {
   __shared__ float red[5 * 64];
   extern __shared__ float pnum[];                       // [n_heads][max_seg] softmax numerators
@@ -101,18 +101,20 @@ __global__ void pool_final_kernel(const float* __restrict__ x, const float* __re
   __syncthreads();
   float tot = 0.f;
   for (int c = 0; c < D; c += 64) {
-    const float* xb = x + (size_t)cd.seg_off * D + c + d;
     float acc = 0.f;
-    int t = 0;
-    for (; t + 8 <= S; t += 8) {
-      float xv[8];
+    if (c + d < D) {                  // (D = 32 / 96 behind an LSTM: the last chunk is partial)
+      const float* xb = x + (size_t)cd.seg_off * ldx + c + d;
+      int t = 0;
+      for (; t + 8 <= S; t += 8) {
+        float xv[8];
 #pragma unroll
-      for (int u = 0; u < 8; ++u) xv[u] = __ldg(xb + (size_t)(t + u) * D);
+        for (int u = 0; u < 8; ++u) xv[u] = __ldg(xb + (size_t)(t + u) * ldx);
 #pragma unroll
-      for (int u = 0; u < 8; ++u) acc = fmaf(pn[t + u], xv[u], acc);
+        for (int u = 0; u < 8; ++u) acc = fmaf(pn[t + u], xv[u], acc);
+      }
+      for (; t < S; ++t) acc = fmaf(pn[t], __ldg(xb + (size_t)t * ldx), acc);
+      acc = (acc / sum) * __ldg(P.w3 + h * D + c + d);
     }
-    for (; t < S; ++t) acc = fmaf(pn[t], __ldg(xb + (size_t)t * D), acc);
-    acc = (acc / sum) * __ldg(P.w3 + h * D + c + d);
     tot = c ? tot + acc : acc;
   }
   red[threadIdx.x] = tot;
@@ -123,11 +125,12 @@ __global__ void pool_final_kernel(const float* __restrict__ x, const float* __re
 
 // ---------------------------------------------------------------------------------------
 // The other pooling modules of the reference (user-trained checkpoints, SURVEY.md 8f.4), one CTA per clip, D threads
-// (thread d owns feature d; D = 64..256 after self-attention, 256 after the BiLSTM):
+// (thread d owns feature d; D = 64..256 after self-attention, dirs H = 32..512 after an LSTM; rows ldx floats apart):
 //   mode 1 PoolAtt       (lib:1131-1154): att_t = a1 . x_t + a1b, softmax over the clip's steps, sum_t att_t x_t, Linear
 //   mode 2 PoolAvg       (lib:1185-1204): mean over the clip's steps, Linear
 //   mode 3 PoolMax       (lib:1206-1225): max over the clip's steps, Linear
 //   mode 4 PoolLastStep  (lib:1117-1129): x at the last valid step, Linear
+//   mode 5 PoolLastStepBi (lib:1107-1115): the forward half at the last valid step, the backward half at step 0, Linear
 // One Linear(D -> 1) per head (NISQA_DIM: five heads with their own weights, lib:260-268).
 
 template <int D>
@@ -155,30 +158,32 @@ __device__ __forceinline__ float block_max(float v, float* red) {
 
 template <int D>
 __global__ void __launch_bounds__(D, 1)
-pool_simple_kernel(const float* __restrict__ x /*[n_seg][D]*/, const ClipDesc* __restrict__ clips, int mode,
+pool_simple_kernel(const float* __restrict__ x /*[n_seg][ldx]*/, int ldx, const ClipDesc* __restrict__ clips, int mode,
                    PoolSimpleParams P, int n_heads, float* __restrict__ scores) {
   extern __shared__ __align__(16) float slog[];          // mode 1: softmax numerators of the clip's steps
   __shared__ float red[D / 32];
   const ClipDesc cd = clips[blockIdx.x];
   const int S = cd.n_seg, d = threadIdx.x, lane = d & 31, warp = d >> 5;
   if (S <= 0) { if (d < n_heads) scores[blockIdx.x * n_heads + d] = __int_as_float(0x7fc00000); return; }
-  const float* xb = x + (size_t)cd.seg_off * D;
+  const float* xb = x + (size_t)cd.seg_off * ldx;
   float pooled = 0.f;
   if (mode == 2) {
-    for (int t = 0; t < S; ++t) pooled += __ldg(xb + (size_t)t * D + d);
+    for (int t = 0; t < S; ++t) pooled += __ldg(xb + (size_t)t * ldx + d);
     pooled = pooled / (float)S;
   } else if (mode == 3) {
     pooled = -INFINITY;
-    for (int t = 0; t < S; ++t) pooled = fmaxf(pooled, __ldg(xb + (size_t)t * D + d));
+    for (int t = 0; t < S; ++t) pooled = fmaxf(pooled, __ldg(xb + (size_t)t * ldx + d));
   } else if (mode == 4) {
-    pooled = __ldg(xb + (size_t)(S - 1) * D + d);
+    pooled = __ldg(xb + (size_t)(S - 1) * ldx + d);
+  } else if (mode == 5) {
+    pooled = __ldg(xb + (size_t)(d < D / 2 ? S - 1 : 0) * ldx + d);
   }
   for (int h = 0; h < n_heads; ++h) {
     if (mode == 1) {
       __syncthreads();                                    // slog of the previous head consumed
       for (int t = warp; t < S; t += D / 32) {
         float a = 0.f;
-        for (int k = lane; k < D; k += 32) a = fmaf(__ldg(xb + (size_t)t * D + k), __ldg(P.a1 + h * D + k), a);
+        for (int k = lane; k < D; k += 32) a = fmaf(__ldg(xb + (size_t)t * ldx + k), __ldg(P.a1 + h * D + k), a);
         a = warp_sum(a);
         if (lane == 0) slog[t] = a + __ldg(P.a1b + h);
       }
@@ -190,7 +195,7 @@ pool_simple_kernel(const float* __restrict__ x /*[n_seg][D]*/, const ClipDesc* _
       for (int t = d; t < S; t += D) { const float e = expf(slog[t] - mx); slog[t] = e; sum += e; }
       sum = block_sum<D>(sum, red);                       // (its barriers also publish the numerators)
       float acc = 0.f;
-      for (int t = 0; t < S; ++t) acc = fmaf(slog[t], __ldg(xb + (size_t)t * D + d), acc);
+      for (int t = 0; t < S; ++t) acc = fmaf(slog[t], __ldg(xb + (size_t)t * ldx + d), acc);
       pooled = acc / sum;
     }
     const float tot = block_sum<D>(pooled * __ldg(P.w3 + h * D + d), red);
@@ -467,17 +472,174 @@ __global__ void lastbi_final_kernel(const float* __restrict__ partial, const Cli
                                    : __int_as_float(0x7fc00000);
 }
 
+// ---------------------------------------------------------------------------------------
+// One layer of a stacked LSTM of any accepted shape (checkpoints trained with other td_lstm_h / td_lstm_num_layers /
+// td_lstm_bidirectional / cnn_fc_out_h, reference lib:925-943).  The input projection gx = x W_ih^T + b of every step and
+// direction is one tile GEMM before this launch, so a step is the recurrence alone: pre = gx[t] + W_hh h.
+// A direction's 4H gate rows are split over C = H / 64 CTAs of a thread-block cluster for H = 192 / 256 (W_hh is 576 KB /
+// 1 MB in fp32) and held by one CTA (C = 1) for H <= 128.  Each CTA owns U = H / C hidden units with 2U threads:
+// thread t owns unit u = t >> 1 and the gate pair gp = t & 1 ((i, f) or (g, o)), i.e. two rows of W_hh, of which the
+// first min(H, 64) taps live in registers and the rest in shared memory, like lstm_batched_kernel.  NB sequences of one
+// direction advance in lock step (group g = clips order[NB g .. NB g + NB)); a finished sequence keeps its state.
+// Each CTA holds the whole h of the step (double buffered): with C > 1 every CTA stores its U new values into every CTA's
+// next buffer through distributed shared memory, and one cluster barrier (release / acquire) ends the step.
+// gx of the next step is loaded while the current step computes.  Every row keeps two partial sums (even / odd taps)
+// whatever NB is, so a clip's result does not depend on NB or on the clips that share its CTA.
+__device__ __forceinline__ unsigned cluster_ctarank() {
+  unsigned r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_barrier() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// store v into the shared-memory word `local` (a shared-window address of this CTA's layout) of cluster CTA `rank`
+__device__ __forceinline__ void st_cluster(unsigned local, unsigned rank, float v) {
+  unsigned remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local), "r"(rank));
+  asm volatile("st.shared::cluster.f32 [%0], %1;" :: "r"(remote), "f"(v) : "memory");
+}
+
+template <int H, int NB, int C>
+struct LstmLayerShape {
+  static constexpr int U = H / C;                    // hidden units per CTA
+  static constexpr int T = 2 * U;                    // threads
+  static constexpr int KR = H < 64 ? H : 64;         // taps per row in registers
+  static constexpr int KS = H - KR;                  // taps per row in shared memory
+  static constexpr int kSmemBytes = (KS * T * 2 + 2 * NB * H) * 4;
+  static_assert(H % (4 * C) == 0 && KR % 4 == 0 && KS % 4 == 0, "shape");
+};
+
+template <int H, int NB, int C>
+__global__ void __launch_bounds__(LstmLayerShape<H, NB, C>::T, 1)
+lstm_layer_kernel(const ClipDesc* __restrict__ clips, const int* __restrict__ order, int n_clips, LstmLayerParams P) {
+  using L = LstmLayerShape<H, NB, C>;
+  extern __shared__ __align__(16) float sm[];
+  float2* whs = reinterpret_cast<float2*>(sm);       // [KS k][T t]: taps KR.. of this thread's two rows
+  float* hbuf = sm + L::KS * L::T * 2;               // [2][NB][H]
+  const int t = threadIdx.x, u = t >> 1, gp = t & 1;
+  const unsigned rank = C > 1 ? cluster_ctarank() : 0;
+  const int gu = (int)rank * L::U + u;               // this thread's hidden unit
+  const int dir = blockIdx.y, g0 = blockIdx.z * NB;
+  int S[NB];
+  size_t seg_off[NB];
+  int maxS = 0;
+#pragma unroll
+  for (int b = 0; b < NB; ++b) {
+    const int clip = (g0 + b < n_clips) ? __ldg(order + g0 + b) : -1;
+    S[b] = 0; seg_off[b] = 0;
+    if (clip >= 0) { const ClipDesc cd = clips[clip]; S[b] = cd.n_seg; seg_off[b] = (size_t)cd.seg_off; }
+    maxS = max(maxS, S[b]);
+  }
+  const int rowA = (2 * gp) * H + gu, rowB = rowA + H;
+  float wrA[L::KR], wrB[L::KR];
+  {
+    const float* ra = P.w_hh + ((size_t)dir * 4 * H + rowA) * H;
+    const float* rb = P.w_hh + ((size_t)dir * 4 * H + rowB) * H;
+#pragma unroll
+    for (int k = 0; k < L::KR; ++k) { wrA[k] = __ldg(ra + k); wrB[k] = __ldg(rb + k); }
+    for (int k = 0; k < L::KS; ++k) whs[k * L::T + t] = make_float2(__ldg(ra + L::KR + k), __ldg(rb + L::KR + k));
+  }
+  for (int i = t; i < 2 * NB * H; i += L::T) hbuf[i] = 0.f;
+  const float* gxd = P.gx + (size_t)dir * 4 * H;
+  // gx of (sequence b, step) for this thread's two rows
+  auto gx_row = [&](int b, int step) { return gxd + (seg_off[b] + (size_t)(dir ? S[b] - 1 - step : step)) * P.ldg; };
+  float gA[NB], gB[NB], cst[NB], hl[NB];
+#pragma unroll
+  for (int b = 0; b < NB; ++b) {
+    cst[b] = 0.f; hl[b] = 0.f; gA[b] = 0.f; gB[b] = 0.f;
+    if (S[b] > 0) { gA[b] = __ldg(gx_row(b, 0) + rowA); gB[b] = __ldg(gx_row(b, 0) + rowB); }
+  }
+  if (C > 1) cluster_barrier(); else __syncthreads();        // every CTA's h buffers are cleared before anyone stores
+
+  for (int step = 0; step < maxS; ++step) {
+    const float* h = hbuf + (step & 1) * NB * H;
+    float nA[NB], nB[NB];
+#pragma unroll
+    for (int b = 0; b < NB; ++b) {
+      nA[b] = 0.f; nB[b] = 0.f;
+      if (step + 1 < S[b]) { nA[b] = __ldg(gx_row(b, step + 1) + rowA); nB[b] = __ldg(gx_row(b, step + 1) + rowB); }
+    }
+    float pA[NB][2], pB[NB][2];
+#pragma unroll
+    for (int b = 0; b < NB; ++b) { pA[b][0] = gA[b]; pA[b][1] = 0.f; pB[b][0] = gB[b]; pB[b][1] = 0.f; }
+#pragma unroll
+    for (int k = 0; k < L::KR; k += 4) {
+#pragma unroll
+      for (int b = 0; b < NB; ++b) {
+        const float4 hv = *reinterpret_cast<const float4*>(h + b * H + k);
+        pA[b][0] = fmaf(wrA[k], hv.x, pA[b][0]); pA[b][1] = fmaf(wrA[k + 1], hv.y, pA[b][1]);
+        pA[b][0] = fmaf(wrA[k + 2], hv.z, pA[b][0]); pA[b][1] = fmaf(wrA[k + 3], hv.w, pA[b][1]);
+        pB[b][0] = fmaf(wrB[k], hv.x, pB[b][0]); pB[b][1] = fmaf(wrB[k + 1], hv.y, pB[b][1]);
+        pB[b][0] = fmaf(wrB[k + 2], hv.z, pB[b][0]); pB[b][1] = fmaf(wrB[k + 3], hv.w, pB[b][1]);
+      }
+    }
+#pragma unroll 4
+    for (int k = 0; k < L::KS; k += 4) {
+      const float2 w0 = whs[k * L::T + t], w1 = whs[(k + 1) * L::T + t], w2 = whs[(k + 2) * L::T + t],
+                   w3 = whs[(k + 3) * L::T + t];
+#pragma unroll
+      for (int b = 0; b < NB; ++b) {
+        const float4 hv = *reinterpret_cast<const float4*>(h + b * H + L::KR + k);
+        pA[b][0] = fmaf(w0.x, hv.x, pA[b][0]); pA[b][1] = fmaf(w1.x, hv.y, pA[b][1]);
+        pA[b][0] = fmaf(w2.x, hv.z, pA[b][0]); pA[b][1] = fmaf(w3.x, hv.w, pA[b][1]);
+        pB[b][0] = fmaf(w0.y, hv.x, pB[b][0]); pB[b][1] = fmaf(w1.y, hv.y, pB[b][1]);
+        pB[b][0] = fmaf(w2.y, hv.z, pB[b][0]); pB[b][1] = fmaf(w3.y, hv.w, pB[b][1]);
+      }
+    }
+    float* hn = hbuf + ((step + 1) & 1) * NB * H;
+#pragma unroll
+    for (int b = 0; b < NB; ++b) {
+      const float aA = pA[b][0] + pA[b][1], aB = pB[b][0] + pB[b][1];
+      // gp == 0: (aA, aB) = pre-activations of (i, f); gp == 1: of (g, o)
+      const float actA = gp ? tanhf(aA) : 1.0f / (1.0f + expf(-aA));
+      const float actB = 1.0f / (1.0f + expf(-aB));
+      const float qA = __shfl_xor_sync(0xffffffffu, actA, 1), qB = __shfl_xor_sync(0xffffffffu, actB, 1);
+      const float ig = gp ? qA : actA, fg = gp ? qB : actB, gg = gp ? actA : qA, og = gp ? actB : qB;
+      if (step < S[b]) {                       // uniform over the CTA: S[b] is the same for every thread
+        cst[b] = fmaf(fg, cst[b], ig * gg);
+        hl[b] = og * tanhf(cst[b]);
+        if (gp == 0) P.out[(seg_off[b] + (size_t)(dir ? S[b] - 1 - step : step)) * P.ldo + dir * H + gu] = hl[b];
+      }
+      if (gp == 0) {                           // (a finished sequence: its state carried along unchanged)
+        if (C == 1) {
+          hn[b * H + gu] = hl[b];
+        } else {
+          const unsigned a = (unsigned)__cvta_generic_to_shared(hn + b * H + gu);
+#pragma unroll
+          for (int r = 0; r < C; ++r) st_cluster(a, r, hl[b]);
+        }
+      }
+      gA[b] = nA[b]; gB[b] = nB[b];
+    }
+    if (C > 1) cluster_barrier(); else __syncthreads();
+  }
+}
+
+// PoolAttFF logits behind an LSTM: one warp per (row, head), logit = w2_h . hid[row][h 128 ..] + b2_h
+__global__ void att_logits_kernel(const float* __restrict__ hid, const float* __restrict__ w2, const float* __restrict__ b2,
+                                  int n_heads, int n_rows, float* __restrict__ logits) {
+  const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (wid >= n_rows * n_heads) return;
+  const int row = wid / n_heads, h = wid - row * n_heads;
+  const float4 x = __ldg(reinterpret_cast<const float4*>(hid + ((size_t)row * n_heads + h) * 128) + lane);
+  const float4 w = __ldg(reinterpret_cast<const float4*>(w2 + h * 128) + lane);
+  float a = fmaf(x.x, w.x, fmaf(x.y, w.y, fmaf(x.z, w.z, x.w * w.w)));
+  a = warp_sum(a);
+  if (lane == 0) logits[wid] = a + __ldg(b2 + h);
+}
+
 // ------------------------------------------------------------------ host launchers
 constexpr int kRowSmem20 = (kRows * kXS + 64 * 20) * 4;
 
 void launch_fc20(cudaStream_t st, const float* feats, const float* WT, const float* b, float* out, int n_rows) {
   linear_rows_kernel<20><<<(n_rows + kRows - 1) / kRows, kRows, kRowSmem20, st>>>(feats, 768, WT, b, out, n_rows);
 }
-void launch_pool_final(cudaStream_t st, const float* x, int D, const float* logits, const ClipDesc* clips, int n_clips,
+void launch_pool_final(cudaStream_t st, const float* x, int D, int ldx, const float* logits, const ClipDesc* clips, int n_clips,
                        const PoolHeadParams& P, int n_heads, int max_seg, float* scores) {
   const int smem = n_heads * std::max(max_seg, 1) * 4;          // <= 5 x 1300 x 4 bytes at ms_max_segments = 1300
   if (smem > 40 * 1024) cudaFuncSetAttribute(pool_final_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  pool_final_kernel<<<n_clips, 64 * n_heads, smem, st>>>(x, logits, clips, P, n_heads, std::max(max_seg, 1), D, scores);
+  pool_final_kernel<<<n_clips, 64 * n_heads, smem, st>>>(x, logits, clips, P, n_heads, std::max(max_seg, 1), D, ldx, scores);
 }
 void launch_lstm(cudaStream_t st, const float* feats20, const ClipDesc* clips, int n_clips,
                  const LstmParams& P, float* td_out, float* partial, float pool_bias, float* scores) {
@@ -489,19 +651,23 @@ void launch_lstm(cudaStream_t st, const float* feats20, const ClipDesc* clips, i
 }
 
 template <int D>
-void pool_simple_instance(cudaStream_t st, const float* x, const ClipDesc* clips, int n_clips, int mode, const PoolSimpleParams& P,
-                          int n_heads, int smem, float* scores) {
+void pool_simple_instance(cudaStream_t st, const float* x, int ldx, const ClipDesc* clips, int n_clips, int mode,
+                          const PoolSimpleParams& P, int n_heads, int smem, float* scores) {
   if (smem > 48 * 1024) cudaFuncSetAttribute(pool_simple_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  pool_simple_kernel<D><<<n_clips, D, smem, st>>>(x, clips, mode, P, n_heads, scores);
+  pool_simple_kernel<D><<<n_clips, D, smem, st>>>(x, ldx, clips, mode, P, n_heads, scores);
 }
-void launch_pool_simple(cudaStream_t st, const float* x, int D, const ClipDesc* clips, int n_clips, int mode,
+void launch_pool_simple(cudaStream_t st, const float* x, int D, int ldx, const ClipDesc* clips, int n_clips, int mode,
                         const PoolSimpleParams& P, int n_heads, int max_seg, float* scores) {
   const int smem = (mode == 1 ? max_seg : 0) * 4 + 16;
   switch (D) {
-    case 64: pool_simple_instance<64>(st, x, clips, n_clips, mode, P, n_heads, smem, scores); break;
-    case 128: pool_simple_instance<128>(st, x, clips, n_clips, mode, P, n_heads, smem, scores); break;
-    case 192: pool_simple_instance<192>(st, x, clips, n_clips, mode, P, n_heads, smem, scores); break;
-    case 256: pool_simple_instance<256>(st, x, clips, n_clips, mode, P, n_heads, smem, scores); break;
+    case 32: pool_simple_instance<32>(st, x, ldx, clips, n_clips, mode, P, n_heads, smem, scores); break;
+    case 64: pool_simple_instance<64>(st, x, ldx, clips, n_clips, mode, P, n_heads, smem, scores); break;
+    case 96: pool_simple_instance<96>(st, x, ldx, clips, n_clips, mode, P, n_heads, smem, scores); break;
+    case 128: pool_simple_instance<128>(st, x, ldx, clips, n_clips, mode, P, n_heads, smem, scores); break;
+    case 192: pool_simple_instance<192>(st, x, ldx, clips, n_clips, mode, P, n_heads, smem, scores); break;
+    case 256: pool_simple_instance<256>(st, x, ldx, clips, n_clips, mode, P, n_heads, smem, scores); break;
+    case 384: pool_simple_instance<384>(st, x, ldx, clips, n_clips, mode, P, n_heads, smem, scores); break;
+    case 512: pool_simple_instance<512>(st, x, ldx, clips, n_clips, mode, P, n_heads, smem, scores); break;
   }
 }
 
@@ -529,6 +695,52 @@ void launch_lstm_batched(cudaStream_t st, const float* feats20, const ClipDesc* 
   else
     lstm_batched_kernel<4><<<2 * ((n_clips + 3) / 4), 256, lstm_batched_smem<4>(), st>>>(feats20, clips, order, n_clips, P, td_out, partial);
   if (scores) lastbi_final_kernel<<<(n_clips + 127) / 128, 128, 0, st>>>(partial, clips, pool_bias, scores, n_clips);
+}
+
+template <int H, int C>
+void lstm_layer_instance(cudaStream_t st, int dirs, const ClipDesc* clips, const int* order, int n_clips, const LstmLayerParams& P) {
+  static unsigned long long cfg = 0;
+  static int n_sm = 132;
+  if (first_launch_on_device(cfg)) {
+    cudaFuncSetAttribute(lstm_layer_kernel<H, 1, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, LstmLayerShape<H, 1, C>::kSmemBytes);
+    cudaFuncSetAttribute(lstm_layer_kernel<H, 2, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, LstmLayerShape<H, 2, C>::kSmemBytes);
+    cudaFuncSetAttribute(lstm_layer_kernel<H, 4, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, LstmLayerShape<H, 4, C>::kSmemBytes);
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+  }
+  // the fewest sequences per CTA that still put every CTA of the launch on the chip at once
+  const int ctas = dirs * n_clips * C;
+  const int nb = ctas <= n_sm ? 1 : ctas <= 2 * n_sm ? 2 : 4;
+  cudaLaunchConfig_t lc = {};
+  lc.gridDim = dim3(C, dirs, (n_clips + nb - 1) / nb);
+  lc.blockDim = dim3(LstmLayerShape<H, 1, C>::T);
+  lc.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = C; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  lc.attrs = attr;
+  lc.numAttrs = C > 1 ? 1 : 0;
+  if (nb == 1) { lc.dynamicSmemBytes = LstmLayerShape<H, 1, C>::kSmemBytes; cudaLaunchKernelEx(&lc, lstm_layer_kernel<H, 1, C>, clips, order, n_clips, P); }
+  else if (nb == 2) { lc.dynamicSmemBytes = LstmLayerShape<H, 2, C>::kSmemBytes; cudaLaunchKernelEx(&lc, lstm_layer_kernel<H, 2, C>, clips, order, n_clips, P); }
+  else { lc.dynamicSmemBytes = LstmLayerShape<H, 4, C>::kSmemBytes; cudaLaunchKernelEx(&lc, lstm_layer_kernel<H, 4, C>, clips, order, n_clips, P); }
+}
+bool lstm_layer_supported(int H) { return H == 32 || H == 64 || H == 96 || H == 128 || H == 192 || H == 256; }
+void launch_lstm_layer(cudaStream_t st, int H, int dirs, const ClipDesc* clips, const int* order, int n_clips,
+                       const LstmLayerParams& P) {
+  switch (H) {
+    case 32: lstm_layer_instance<32, 1>(st, dirs, clips, order, n_clips, P); break;
+    case 64: lstm_layer_instance<64, 1>(st, dirs, clips, order, n_clips, P); break;
+    case 96: lstm_layer_instance<96, 1>(st, dirs, clips, order, n_clips, P); break;
+    case 128: lstm_layer_instance<128, 1>(st, dirs, clips, order, n_clips, P); break;
+    case 192: lstm_layer_instance<192, 3>(st, dirs, clips, order, n_clips, P); break;
+    case 256: lstm_layer_instance<256, 4>(st, dirs, clips, order, n_clips, P); break;
+  }
+}
+void launch_att_logits(cudaStream_t st, const float* hid, const float* w2, const float* b2, int n_heads, int n_rows,
+                       float* logits) {
+  const long long warps = (long long)n_rows * n_heads;
+  if (warps > 0) att_logits_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(hid, w2, b2, n_heads, n_rows, logits);
 }
 
 }  // namespace nisqa

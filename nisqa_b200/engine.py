@@ -53,6 +53,9 @@ class NisqaConfig(C.Structure):
 
 SA_D_MODELS = (64, 128, 192, 256)     # self-attention widths the kernels are instantiated for (one head)
 SA_FF_MAX = 4096                      # feed-forward width: a multiple of 64 up to this
+LSTM_H = (32, 64, 96, 128, 192, 256)  # LSTM hidden sizes the kernels are instantiated for
+LSTM_LAYERS_MAX = 4
+CNN_FC_OUT_MAX = 1024                 # StandardCNN's fc_out width (None: the LSTM reads the 768 conv6 features)
 
 
 def _sa_widths(args, prefix, de=False):
@@ -67,6 +70,29 @@ def _sa_widths(args, prefix, de=False):
     if h is None or int(h) != h or h <= 0 or h % 64 != 0 or h > SA_FF_MAX:
         raise NotImplementedError("%s_h=%r: the engine needs a positive multiple of 64 up to %d" % (prefix, h, SA_FF_MAX))
     return int(d), int(h)
+
+
+def _check_lstm(args, pool_mode):
+    """Refuses the StandardCNN + LSTM hyper-parameters the kernels do not implement, naming the value.  The engine reads
+    the LSTM's shape from the checkpoint's tensors (nisqa_load_weights); nothing of it goes into nisqa_config."""
+    h, nl, fc = args.get("td_lstm_h"), args.get("td_lstm_num_layers"), args.get("cnn_fc_out_h")
+    if h not in LSTM_H:
+        raise NotImplementedError("td_lstm_h=%r: the engine runs LSTM hidden sizes %s" % (h, ", ".join(map(str, LSTM_H))))
+    if nl is None or int(nl) != nl or not 1 <= nl <= LSTM_LAYERS_MAX:
+        raise NotImplementedError("td_lstm_num_layers=%r: the engine runs 1 to %d LSTM layers" % (nl, LSTM_LAYERS_MAX))
+    if pool_mode == POOL_LAST_STEP_BI and not args.get("td_lstm_bidirectional"):
+        raise NotImplementedError("pool='last_step_bi' with td_lstm_bidirectional=%r: PoolLastStepBi needs a bidirectional LSTM"
+                                  % (args.get("td_lstm_bidirectional"),))
+    if fc and (int(fc) != fc or not 1 <= fc <= CNN_FC_OUT_MAX):
+        raise NotImplementedError("cnn_fc_out_h=%r: the engine runs fc_out widths 1 to %d (or None)" % (fc, CNN_FC_OUT_MAX))
+    if args.get("td_2") not in (None, "skip"):
+        raise NotImplementedError("td_2=%r behind an LSTM is not implemented by the engine" % (args.get("td_2"),))
+    ch = (args.get("cnn_c_out_1"), args.get("cnn_c_out_2"), args.get("cnn_c_out_3"))
+    if ch != (16, 32, 64):
+        raise NotImplementedError("cnn_c_out_1/2/3=%r: the engine runs StandardCNN with 16, 32, 64 channels" % (ch,))
+    ks = args.get("cnn_kernel_size")
+    if not (ks == 3 or (isinstance(ks, (list, tuple)) and tuple(ks) == (3, 3))):
+        raise NotImplementedError("cnn_kernel_size=%r: the engine runs 3x3 convolutions" % (ks,))
 
 
 class NisqaTensor(C.Structure):
@@ -196,11 +222,11 @@ def config_from_args(args, max_chunk_segments=0):
         if cnn_fc % 64 != 0:
             raise NotImplementedError("cnn_fc_out_h=%d: the engine needs a multiple of 64" % cnn_fc)
         ok = True
-    elif (cnn, td) == ("standard", "lstm") and pool_mode in (POOL_LAST_STEP_BI, POOL_AVG, POOL_MAX, POOL_LAST_STEP):
+    elif (cnn, td) == ("standard", "lstm"):
+        # any LSTM width, depth and direction behind StandardCNN (lib:811-836, 925-943), every pooling module
         arch = ARCH_STD_LSTM_LASTBI
-        ok = (args.get("cnn_fc_out_h") == 20 and args["td_lstm_h"] == 128
-              and args["td_lstm_num_layers"] == 1 and bool(args["td_lstm_bidirectional"])
-              and args["model"] == "NISQA")
+        _check_lstm(args, pool_mode)
+        ok = True
     else:
         raise NotImplementedError(
             "architecture cnn=%r td=%r pool=%r is not implemented by the engine" % (cnn, td, pool))
