@@ -118,4 +118,66 @@ __device__ __forceinline__ void conv1_cell(const float* __restrict__ mel, int f0
 }
 #endif
 
+// Pooled cells PW0 .. PW1 - 1 of pooled row ph for the 4 channels of one quad, with every conv1 output position computed
+// once (AdaptCNN: a column shared by two overlapping windows feeds both maxima instead of being computed twice).  Each
+// position is the same fmaf chain as in conv1_cell (zero start, taps 0..8), each cell the same max, + bias, ReLU, so the
+// results are bit-identical to conv1_cell's.  mel: the segment's frames (f0 = 0), PITCH floats apart; wq / bq: the
+// quad's folded weights and biases.  emit(pw, res) receives each cell as soon as its last column is done.
+template <int MODE, int PW0, int PW1, int PITCH, class Emit>
+__device__ __forceinline__ void conv1_strip(const float* mel, float thr, const float (&wq)[9][4], const float (&bq)[4],
+                                            int ph, Emit&& emit) {
+  constexpr int NC = PW1 - PW0;
+  // conv columns of cell pw: [lo(pw), hi(pw)] (MODE 1: the padding column -1 and column 15 do not exist)
+  auto lo = [](int pw) { return MODE == 0 ? 2 * pw : (2 * pw - 1 < 0 ? 0 : 2 * pw - 1); };
+  auto hi = [](int pw) { return MODE == 0 ? 2 * pw + 2 : (2 * pw < kSegLen - 1 ? 2 * pw : kSegLen - 1); };
+  constexpr int X0 = MODE == 0 ? 2 * PW0 : (2 * PW0 - 1 < 0 ? 0 : 2 * PW0 - 1);
+  constexpr int X1 = MODE == 0 ? 2 * (PW1 - 1) + 2 : (2 * (PW1 - 1) < kSegLen - 1 ? 2 * (PW1 - 1) : kSegLen - 1);
+  const int r0 = 2 * ph - 1;                     // first mel row of the 3x3 windows of conv rows 2 ph, 2 ph + 1
+  // mel frame t, rows r0 .. r0 + 3 (clamped at thr; zero outside the segment)
+  auto load_frame = [&](int t, float (&v)[4]) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int r = r0 + i;
+      v[i] = 0.f;
+      if (t >= 0 && t < kSegLen && r >= 0 && r < kMels) v[i] = fmaxf(mel[t * PITCH + r], thr);
+    }
+  };
+  float fr[3][4];                                // frames x - 1, x, x + 1 at fr[(t - X0 + 1) % 3]
+  load_frame(X0 - 1, fr[0]);
+  load_frame(X0, fr[1]);
+  float mx[NC][4];
+#pragma unroll
+  for (int p = 0; p < NC; ++p)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) mx[p][c] = -INFINITY;
+#pragma unroll
+  for (int x = X0; x <= X1; ++x) {
+    load_frame(x + 1, fr[(x - X0 + 2) % 3]);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float acc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+      for (int tap = 0; tap < 9; ++tap) {
+        const int ky = tap / 3, kx = tap % 3;
+        const float a = fr[(x - 1 + kx - X0 + 1) % 3][i + ky];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) acc[c] = fmaf(a, wq[tap][c], acc[c]);
+      }
+#pragma unroll
+      for (int p = 0; p < NC; ++p)
+        if (x >= lo(PW0 + p) && x <= hi(PW0 + p))
+#pragma unroll
+          for (int c = 0; c < 4; ++c) mx[p][c] = fmaxf(mx[p][c], acc[c]);
+    }
+#pragma unroll
+    for (int p = 0; p < NC; ++p)
+      if (x == hi(PW0 + p)) {
+        float res[4];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) res[c] = fmaxf(mx[p][c] + bq[c], 0.f);   // bias + ReLU commute with max
+        emit(PW0 + p, res);
+      }
+  }
+}
+
 }  // namespace nisqa

@@ -42,6 +42,7 @@
 #include <cuda_fp16.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 #include "conv1_cell.cuh"
@@ -93,11 +94,18 @@ __device__ __forceinline__ void mma_unit(float (&acc_m)[NB][C::COUT / 2], float 
     }
 }
 
+// All nine weight taps have landed.  Called before tile_gemm, never between its in-flight wgmmas: a wait loop there
+// makes ptxas serialize them.
+__device__ __forceinline__ void wait_weights(uint32_t bar_w) {
+  for (int t = 0; t < 9; ++t) mbar_wait(bar_w + 8 * t, 0);
+}
+
 // The GEMM of one tile for this warpgroup's NB m64 blocks: acc_m[b] = hi*hi, acc_s[b] = hi*lo + lo*hi over the nine
-// taps, in tap order.  row[b] is this lane's ldmatrix row of block b at tap offset 0.
+// taps, in tap order.  row[b] is this lane's ldmatrix row of block b at tap offset 0.  The weights must have landed
+// (wait_weights).
 template <class C, int NB>
 __device__ __forceinline__ void tile_gemm(float (&acc_m)[NB][C::COUT / 2], float (&acc_s)[NB][C::COUT / 2], uint32_t a_hi,
-                                          uint32_t a_lo, uint32_t b_base, uint32_t bar_w, const int (&row)[NB], int lchunk) {
+                                          uint32_t a_lo, uint32_t b_base, const int (&row)[NB], int lchunk) {
   using U = TapUnits<C>;
   constexpr int P = C::P, UK = U::UK, PT = U::PER_TAP;
   static_assert(C::CIN <= 32 || NB == 1, "CIN 64: one m64 block per warpgroup");
@@ -105,9 +113,7 @@ __device__ __forceinline__ void tile_gemm(float (&acc_m)[NB][C::COUT / 2], float
   for (int b = 0; b < NB; ++b)
 #pragma unroll
     for (int i = 0; i < C::COUT / 2; ++i) { acc_m[b][i] = 0.f; acc_s[b][i] = 0.f; }
-  // one unit in flight: unit u + 1's fragments load into the other register set while unit u's wgmmas run.  All nine
-  // weight taps are waited for up front: a wait loop between in-flight wgmmas makes ptxas serialize them.
-  for (int t = 0; t < 9; ++t) mbar_wait(bar_w + 8 * t, 0);
+  // one unit in flight: unit u + 1's fragments load into the other register set while unit u's wgmmas run
   uint32_t ah[2][NB][UK][4], al[2][NB][UK][4];
   load_unit<C, NB>(a_hi, a_lo, row, -P - 1, 0, lchunk, ah[0], al[0]);
 #pragma unroll
@@ -124,11 +130,19 @@ __device__ __forceinline__ void tile_gemm(float (&acc_m)[NB][C::COUT / 2], float
   wgmma_wait<0>();
 }
 
-// epilogue part 1 for one m64 block: accumulators of GEMM rows m0 and m0 + 8 -> bias + ReLU -> the staging rows of
-// their plane positions (every interior position of the tile's live segments is written: store_tile reads them all)
+// this lane's accumulator columns of the bias: bb[j] = bias[8 j + acol], bias[8 j + acol + 1]
+template <class C>
+__device__ __forceinline__ void load_bias(const float* __restrict__ bias, int acol, float2 (&bb)[C::COUT / 8]) {
+#pragma unroll
+  for (int j = 0; j < C::COUT / 8; ++j) bb[j] = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + acol));
+}
+
+// epilogue part 1 for one m64 block: accumulators of GEMM rows m0 and m0 + 8 -> bias (load_bias) + ReLU -> the staging
+// rows of their plane positions (every interior position of the tile's live segments is written: store_tile reads them
+// all)
 template <class C>
 __device__ __forceinline__ void stage_rows(const float (&acc_m)[C::COUT / 2], const float (&acc_s)[C::COUT / 2], int m0,
-                                           int acol, int seg0, int n_seg, const float* __restrict__ bias, float out_scale,
+                                           int acol, int seg0, int n_seg, const float2 (&bb)[C::COUT / 8], float out_scale,
                                            float* stg) {
   constexpr int SS = C::STG_STRIDE;
 #pragma unroll
@@ -139,9 +153,8 @@ __device__ __forceinline__ void stage_rows(const float (&acc_m)[C::COUT / 2], co
 #pragma unroll
       for (int j = 0; j < C::COUT / 8; ++j) {
         const int col = 8 * j + acol;
-        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + col));
-        const float v0 = fmaxf(fmaf(acc_m[4 * j + 2 * half] + acc_s[4 * j + 2 * half], out_scale, bb.x), 0.f);
-        const float v1 = fmaxf(fmaf(acc_m[4 * j + 2 * half + 1] + acc_s[4 * j + 2 * half + 1], out_scale, bb.y), 0.f);
+        const float v0 = fmaxf(fmaf(acc_m[4 * j + 2 * half] + acc_s[4 * j + 2 * half], out_scale, bb[j].x), 0.f);
+        const float v1 = fmaxf(fmaf(acc_m[4 * j + 2 * half + 1] + acc_s[4 * j + 2 * half + 1], out_scale, bb[j].y), 0.f);
         *reinterpret_cast<float2*>(stg + r * SS + col) = make_float2(v0, v1);
       }
     }
@@ -290,14 +303,17 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
     for (int i = 0; i < C::COUT / 2; ++i) { acc_m[0][i] = 0.f; acc_s[0][i] = 0.f; }
     if (__shfl_sync(0xffffffffu, wg < C::NBLK, 0)) {
       const int row[1] = {(g0 & 7) + lrow};
-      tile_gemm<C, 1>(acc_m, acc_s, a_hi, a_lo, b_base, bar_w, row, lchunk);
+      wait_weights(bar_w);
+      tile_gemm<C, 1>(acc_m, acc_s, a_hi, a_lo, b_base, row, lchunk);
     }
     if constexpr (!C::ALIAS) mbar_arrive(bar_empty + 8 * ab);
     __syncthreads();                             // ALIAS: every warpgroup is done with the A tile the staging tile
                                                  // overwrites; otherwise the previous tile's part 2 is done with it
 
     // ===== epilogue part 1: accumulators -> bias + ReLU -> staging row of each GEMM row's plane position =====
-    stage_rows<C>(acc_m[0], acc_s[0], arow0, acol, seg0, n_seg, bias, out_scale, stg);   // (no rows past block NBLK - 1)
+    float2 bb[C::COUT / 8];
+    load_bias<C>(bias, acol, bb);
+    stage_rows<C>(acc_m[0], acc_s[0], arow0, acol, seg0, n_seg, bb, out_scale, stg);   // (no rows past block NBLK - 1)
     __syncthreads();
 
     // ===== epilogue part 2 (all threads): max-pool / split / store =====
@@ -313,15 +329,17 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
 // conv1 + BN + ReLU + pool1 (conv1_cell.cuh, the same fp32 arithmetic as conv1_pool1_kernel) of one segment per tile
 // goes straight into the A tile; the conv2 GEMM and epilogue are the same code on the same values as conv_split_kernel,
 // so results are bit-identical to the separate kernels.  The persistent CTA splits into two roles:
-//   warpgroups 0, 1 (MMA):   wait A full[i & 1]; GEMM of rows 128 wg .. 128 wg + 127 (two m64 blocks); arrive A
-//                            empty[i & 1]; bias + ReLU into staging tile i & 1; named barrier of the 256 MMA threads;
-//                            max-pool / split / store of tile i
-//   warpgroups 2, 3 (conv1): conv1 of tile i + 1 into A buffer (i + 1) & 1 (after its empty barrier), arrive A full
-// so conv1 of the next tile runs while the tensor cores work on this one.  conv1 is the longer of the two roles, so the
-// epilogue stays with the MMA warpgroups.  The A barriers count the 256 threads of the role that arrives on them;
-// buffer b's k-th use waits on parity k & 1 (full) or (k & 1) ^ 1 (empty: a fresh barrier's "previous phase" counts as
-// complete).  Staging tile i & 1 is next written at tile i + 2, after the named barrier of tile i + 1, which every MMA
-// thread reaches only after its part of tile i's store.
+//   warpgroups 0, 1 (MMA):   wait A full[i & 1]; GEMM of m64 blocks 0, 1 (warpgroup 0) or block 2 (warpgroup 1);
+//                            arrive A empty[i & 1]; bias + ReLU into staging tile i & 1; named barrier of the 256 MMA
+//                            threads; max-pool / split / store of tile i
+//   warpgroups 2, 3 (conv1): one thread copies the mel block of tile i + 3 into the mel ring; wait mel full[(i + 1) % 4]
+//                            and A empty[(i + 1) & 1]; conv1 of tile i + 1 from the ring into A buffer (i + 1) & 1;
+//                            arrive mel empty and A full
+// so conv1 of the next tile runs while the tensor cores work on this one, and its mel reads never wait for global
+// memory.  The A and mel empty barriers count the 256 threads of the role that arrives on them (mel full: the copying
+// thread, plus the copy's bytes); a barrier's k-th use waits on parity k & 1 (full) or (k & 1) ^ 1 (empty: a fresh
+// barrier's "previous phase" counts as complete).  Staging tile i & 1 is next written at tile i + 2, after the named
+// barrier of tile i + 1, which every MMA thread reaches only after its part of tile i's store.
 template <class C, int MODE>
 __global__ void __launch_bounds__(C::NT, 1)
 conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, float out_scale, float store_scale,
@@ -336,6 +354,7 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
   const uint32_t sbase = smem_u32(smem);
   const uint32_t b_base = sbase + L::OFF_B;
   const uint32_t bar_w = sbase + L::OFF_BAR, a_full = bar_w + 8 * 9, a_empty = a_full + 16;
+  const uint32_t mel_full = a_empty + 16, mel_empty = mel_full + 8 * L::MEL_R;
   float* ws = reinterpret_cast<float*>(smem + L::OFF_W1);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);   // warp-uniform as far as ptxas can tell: the role branch
@@ -348,6 +367,10 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
   if (tid == 0) {
     for (int t = 0; t < 9; ++t) mbar_init(bar_w + 8 * t, 1);
     for (int b = 0; b < 4; ++b) mbar_init(a_full + 8 * b, NR);
+    for (int s = 0; s < L::MEL_R; ++s) {
+      mbar_init(mel_full + 8 * s, 1);
+      mbar_init(mel_empty + 8 * s, NR);
+    }
     fence_barrier_init();
     for (int t = 0; t < 9; ++t) {
       mbar_expect_tx(bar_w + 8 * t, C::B_STAGE);
@@ -358,56 +381,112 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
 
   // registers: 64 accumulators and two fragment sets per MMA thread; 2 x 128 x (160 + 96) = the whole register file
   if (wg < 2) {
-    // ===== MMA warpgroups: block b of warpgroup wg = GEMM rows 128 wg + 64 b .. + 63 =====
+    // ===== MMA warpgroups: warpgroup 0 runs m64 blocks 0 and 1 (GEMM rows 0 .. 127), warpgroup 1 block 2 (rows
+    // 128 .. 191); block 3 would hold only rows m >= KEPT, which are never staged =====
     setmaxnreg_inc<160>();
-    const int lm = wg * 128 + (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-    const int lrow[2] = {HALO + C::gemm_row(lm), HALO + C::gemm_row(lm + 64)};
+    const int lm = (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;   // ldmatrix row within an m64 block
+    const int am = (warp & 3) * 16 + (lane >> 2);                          // accumulator row within an m64 block
     const int lchunk = lane >> 4;
-    const int arow0 = wg * 128 + (warp & 3) * 16 + (lane >> 2);
     const int acol = 2 * (lane & 3);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-      const int ab = it & 1;
-      const uint32_t par = (uint32_t)(it >> 1) & 1u;
-      mbar_wait(a_full + 8 * ab, par);
-      const uint32_t a_hi = sbase + L::OFF_A + ab * C::A_BUF, a_lo = a_hi + C::A_BYTES;
-      float acc_m[2][C::COUT / 2], acc_s[2][C::COUT / 2];
-      tile_gemm<C, 2>(acc_m, acc_s, a_hi, a_lo, b_base, bar_w, lrow, lchunk);
-      mbar_arrive(a_empty + 8 * ab);
-      float* stg = reinterpret_cast<float*>(smem + L::OFF_STG + ab * C::STG_BYTES);
+    // the whole tile loop of a warpgroup that owns NB blocks from block b0 on: the branch between the two instances is
+    // taken once, outside the loop, on the warp-uniform wg
+    float2 bb[C::COUT / 8];
+    load_bias<C>(bias, acol, bb);
+    wait_weights(bar_w);
+    auto mma_role = [&](auto nb, int b0) {
+      constexpr int NB = decltype(nb)::value;
+      int lrow[NB];
 #pragma unroll
-      for (int b = 0; b < 2; ++b) stage_rows<C>(acc_m[b], acc_s[b], arow0 + 64 * b, acol, tile, n_seg, bias, out_scale, stg);
-      named_bar_sync<1, NR>();
-      store_tile<C>(stg, tile, 1, tid, NR, store_scale, out_hi, out_lo, nullptr);
-    }
+      for (int b = 0; b < NB; ++b) lrow[b] = HALO + C::gemm_row(lm + 64 * (b0 + b));
+      int it = 0;
+      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+        const int ab = it & 1;
+        const uint32_t par = (uint32_t)(it >> 1) & 1u;
+        mbar_wait(a_full + 8 * ab, par);
+        const uint32_t a_hi = sbase + L::OFF_A + ab * C::A_BUF, a_lo = a_hi + C::A_BYTES;
+        float acc_m[NB][C::COUT / 2], acc_s[NB][C::COUT / 2];
+        tile_gemm<C, NB>(acc_m, acc_s, a_hi, a_lo, b_base, lrow, lchunk);
+        mbar_arrive(a_empty + 8 * ab);
+        float* stg = reinterpret_cast<float*>(smem + L::OFF_STG + ab * C::STG_BYTES);
+#pragma unroll
+        for (int b = 0; b < NB; ++b)
+          stage_rows<C>(acc_m[b], acc_s[b], am + 64 * (b0 + b), acol, tile, n_seg, bb, out_scale, stg);
+        named_bar_sync<1, NR>();
+        store_tile<C>(stg, tile, 1, tid, NR, store_scale, out_hi, out_lo, nullptr);
+      }
+    };
+    if (wg == 0) mma_role(std::integral_constant<int, 2>(), 0);
+    else mma_role(std::integral_constant<int, 1>(), 2);
   } else {
     // ===== worker warpgroups =====
     setmaxnreg_dec<96>();
     const int wt = tid - NR;
-    // conv1 + BN + ReLU + pool1 of segment `seg` into A buffer j & 1 (j: the CTA's tile index): one item per
-    // pooled cell and channel half (conv1_cell's channel quads 2c, 2c + 1 -> 16-byte chunk c of the cell's row)
-    auto fill = [&](int seg, int j) {
-      constexpr int NCELL = 24 * W;
-      const int b = j & 1;
+    constexpr int R = L::MEL_R, MEL_FLOATS = L::MEL_BYTES / 4;
+    const float* ring = reinterpret_cast<const float*>(smem + L::OFF_MEL);
+    float* ring_thr = reinterpret_cast<float*>(smem + L::OFF_THR);
+    // Mel ring, thread wt == 0 only: the CTA's k-th segment goes to slot k % R once every worker has arrived on the
+    // slot's empty barrier for segment k - R.  The segment's 15 frames are one contiguous block of 2880 bytes at
+    // mel + kMels f0: the mel workspace comes from cudaMalloc (256-byte aligned) and kMels * 4 = 192 bytes per frame,
+    // so the source is 16-byte aligned for any f0.  seg_frame0 / seg_thr of the next segment to copy are loaded one
+    // copy ahead, so the thread that issues never waits for them.
+    int nf0 = 0;
+    float nthr = 0.f;
+    auto prefetch_seg = [&](int k) {
+      const int seg = blockIdx.x + k * gridDim.x;
+      if (seg < n_tiles) { nf0 = __ldg(seg_frame0 + seg); nthr = __ldg(seg_thr + seg); }
+    };
+    auto issue_mel = [&](int k) {
+      if (blockIdx.x + k * gridDim.x >= n_tiles) return;
+      const int s = k % R;
+      mbar_wait(mel_empty + 8 * s, ((uint32_t)(k / R) & 1u) ^ 1u);
+      ring_thr[s] = nthr;                        // published by the arrive below (release) to the full barrier's waiters
+      mbar_expect_tx(mel_full + 8 * s, L::MEL_BYTES);
+      bulk_g2s(sbase + L::OFF_MEL + s * L::MEL_BYTES, mel + (size_t)nf0 * kMels, L::MEL_BYTES, mel_full + 8 * s);
+      prefetch_seg(k + 1);
+    };
+    if (wt == 0) {
+      prefetch_seg(0);
+      for (int k = 0; k < R - 2; ++k) issue_mel(k);
+    }
+    // conv1 + BN + ReLU + pool1 of the CTA's j-th segment (mel ring slot j % R) into A buffer j & 1.  Thread wt < 192
+    // owns one strip for the kernel's life: pooled row ph, channel quad cq, and the left (pw < W / 2) or right half of
+    // the pooled cells (warp-uniform: 96 strips = 3 warps per half); conv1_strip computes each conv1 output position
+    // of the strip once.  The quad's weights and biases stay in registers.  A warp's lanes run over cq, then ph: its 8
+    // distinct mel addresses are rows 2 apart, on distinct banks.  Each cell -> one 8-byte half of a 16-byte chunk.
+    constexpr int NSTRIP = 2 * 4 * 24;
+    const int cq = wt & 3, ph = (wt >> 2) % 24;
+    const bool right = __shfl_sync(0xffffffffu, wt >= NSTRIP / 2, 0);
+    float wq[9][4], bq[4];
+#pragma unroll
+    for (int t = 0; t < 9; ++t)
+#pragma unroll
+      for (int c = 0; c < 4; ++c) wq[t][c] = ws[t * 16 + cq * 4 + c];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) bq[c] = ws[144 + cq * 4 + c];
+    auto fill = [&](int j) {
+      const int b = j & 1, s = j % R;
+      if (wt == 0) issue_mel(j + R - 2);         // its slot held segment j - 2
       mbar_wait(a_empty + 8 * b, ((uint32_t)(j >> 1) & 1u) ^ 1u);
+      mbar_wait(mel_full + 8 * s, (uint32_t)(j / R) & 1u);
       unsigned char* a = smem + L::OFF_A + b * C::A_BUF;
-      const int f0 = __ldg(seg_frame0 + seg);
-      const float thr = __ldg(seg_thr + seg);
-      for (int i = wt; i < 2 * NCELL; i += NR) {
-        const int cell = i >> 1, c = i & 1;
-        const int ph = cell / W, pw = cell - ph * W;
-        float res[8];
-        conv1_cell<MODE, true, kMels, 2>(mel, f0, thr, ws, ph, pw, res, 2 * c);
-        uint4 hi, lo;
-        split8(make_float4(res[0], res[1], res[2], res[3]), make_float4(res[4], res[5], res[6], res[7]), c1_scale, hi, lo);
-        const uint32_t o = (uint32_t)split_off<ROWB>(HALO + (ph + 1) * P + (pw + 1), c);
-        *reinterpret_cast<uint4*>(a + o) = hi;
-        *reinterpret_cast<uint4*>(a + C::A_BYTES + o) = lo;
+      const float* slot = ring + s * MEL_FLOATS;
+      const float thr = ring_thr[s];
+      auto emit = [&](int pw, const float (&res)[4]) {
+        uint2 hi, lo;
+        split4(make_float4(res[0], res[1], res[2], res[3]), c1_scale, hi, lo);
+        const uint32_t o = (uint32_t)split_off<ROWB>(HALO + (ph + 1) * P + (pw + 1), cq >> 1) + 8 * (cq & 1);
+        *reinterpret_cast<uint2*>(a + o) = hi;
+        *reinterpret_cast<uint2*>(a + C::A_BYTES + o) = lo;
+      };
+      if (wt < NSTRIP) {
+        if (right) conv1_strip<MODE, W / 2, W, kMels>(slot, thr, wq, bq, ph, emit);
+        else conv1_strip<MODE, 0, W / 2, kMels>(slot, thr, wq, bq, ph, emit);
       }
+      mbar_arrive(mel_empty + 8 * s);
       mbar_arrive(a_full + 8 * b);
     };
     int it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) fill(tile, it);
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) fill(it);
   }
 }
 

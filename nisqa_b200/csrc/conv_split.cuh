@@ -97,18 +97,25 @@ using SpConv5S = SpCfg<6, 2, 64, 64, SP_POOL_NONE, 0>;
 using SpConv6S = SpCfg<6, 2, 64, 64, SP_POOL_NONE, 0, true>;
 
 // Shared memory of the fused conv1 + conv2 kernel (conv12_kernel) on the conv2 geometry C: two activation buffers
-// (conv1 fills one while the GEMM reads the other) and two staging tiles (tile i's is written while stragglers of the
-// MMA warpgroups may still read tile i - 1's).
+// (conv1 fills one while the GEMM reads the other), two staging tiles (tile i's is written while stragglers of the
+// MMA warpgroups may still read tile i - 1's) and a ring of MEL_R mel blocks (one segment's kSegLen frames x kMels,
+// copied whole by one cp.async.bulk; 16-byte aligned like its source) with the segment's clamp threshold beside each.
 template <class C>
 struct SpFused {
   static constexpr int OFF_A = 0;                         // buffer b at b * C::A_BUF (1024-aligned: A_BYTES is)
   static constexpr int OFF_STG = 2 * C::A_BUF;            // staging tile b at OFF_STG + b * C::STG_BYTES
   static constexpr int OFF_B = (OFF_STG + 2 * C::STG_BYTES + 1023) & ~1023;
   static constexpr int OFF_W1 = OFF_B + 9 * C::B_STAGE;   // conv1 weights [9][16] + biases [16]
-  // 9 weight-tap barriers, then A full[2], A empty[2]
-  static constexpr int OFF_BAR = OFF_W1 + 1024;
-  static constexpr int SMEM_BYTES = OFF_BAR + 8 * 13 + 1024;
+  static constexpr int MEL_R = 4;                         // ring slots: tile j + 2's copy lands while tile j computes
+  static constexpr int MEL_BYTES = kSegLen * kMels * 4;   // 2880
+  static constexpr int OFF_MEL = OFF_W1 + 1024;           // slot s at OFF_MEL + s * MEL_BYTES
+  static constexpr int OFF_THR = OFF_MEL + MEL_R * MEL_BYTES;   // float [MEL_R]
+  // 9 weight-tap barriers, then A full[2], A empty[2], mel full[MEL_R], mel empty[MEL_R]
+  static constexpr int OFF_BAR = OFF_THR + 4 * MEL_R;
+  static constexpr int SMEM_BYTES = OFF_BAR + 8 * (13 + 2 * MEL_R) + 1024;
   static_assert(!C::ALIAS && C::G == 1 && C::CIN == 16, "conv2 geometry");
+  static_assert(C::NBLK == 3, "the MMA warpgroups run m64 blocks {0, 1} and {2}");
+  static_assert(MEL_BYTES % 16 == 0 && OFF_MEL % 16 == 0 && OFF_BAR % 8 == 0, "bulk copy / mbarrier alignment");
   static_assert(SMEM_BYTES <= C::SMEM_BUDGET, "shared memory budget");
 };
 

@@ -102,11 +102,12 @@ template <> __device__ __forceinline__ void wgmma_rs<64>(float* d, const uint32_
 // pack_weights) -> two 16-byte rows.  hi + lo keeps 22 significant bits of x s while 2^-3 <= x s <= 60000; below
 // 2^-3 lo is subnormal (absolute error <= 2^-25), above 60000 the value is clamped.  With e chosen from the folded
 // BatchNorm (E = max_c |beta_c| + 3 |gamma_c| maps to [2.8, 5.7)) that is 1e4 times the BN output estimate.
-__device__ __forceinline__ void split8(const float4& a, const float4& b, float s, uint4& hi, uint4& lo) {
-  const float x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-  uint32_t h[4], l[4];
+// split4: the same for 4 consecutive channels (one 8-byte half of a row chunk); split8 is two of them.
+__device__ __forceinline__ void split4(const float4& a, float s, uint2& hi, uint2& lo) {
+  const float x[4] = {a.x, a.y, a.z, a.w};
+  uint32_t h[2], l[2];
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
+  for (int i = 0; i < 2; ++i) {
     // post-ReLU inputs (>= 0); x * 2^-e is exact
     const float x0 = fminf(x[2 * i] * s, 60000.f), x1 = fminf(x[2 * i + 1] * s, 60000.f);
     const __half h0 = __float2half_rn(x0), h1 = __float2half_rn(x1);
@@ -114,8 +115,15 @@ __device__ __forceinline__ void split8(const float4& a, const float4& b, float s
     h[i] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
     l[i] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
   }
-  hi = make_uint4(h[0], h[1], h[2], h[3]);
-  lo = make_uint4(l[0], l[1], l[2], l[3]);
+  hi = make_uint2(h[0], h[1]);
+  lo = make_uint2(l[0], l[1]);
+}
+__device__ __forceinline__ void split8(const float4& a, const float4& b, float s, uint4& hi, uint4& lo) {
+  uint2 ha, la, hb, lb;
+  split4(a, s, ha, la);
+  split4(b, s, hb, lb);
+  hi = make_uint4(ha.x, ha.y, hb.x, hb.y);
+  lo = make_uint4(la.x, la.y, lb.x, lb.y);
 }
 
 }  // namespace nisqa
