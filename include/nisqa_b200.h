@@ -34,23 +34,30 @@ extern "C" {
 
 typedef struct nisqa_engine nisqa_engine;
 
-/* architectures of the shipped checkpoints (SURVEY.md 0.4) */
+/* time-dependency models behind the framewise model (td, then td_2; lib:839-895).  The two shipped architectures are 0
+ * and 1; 2 and 3 add an LSTM as td_2.  A self-attention td_2 is td2_layers > 0 with arch 0 or 1. */
 enum nisqa_arch {
-  NISQA_ARCH_ADAPT_SA_ATTFF  = 0, /* nisqa.tar, nisqa_mos_only.tar: AdaptCNN + SelfAttention + PoolAttFF */
-  NISQA_ARCH_STD_LSTM_LASTBI = 1  /* nisqa_tts.tar: StandardCNN + BiLSTM + PoolLastStepBi; also any other
+  NISQA_ARCH_ADAPT_SA_ATTFF  = 0, /* nisqa.tar, nisqa_mos_only.tar: AdaptCNN + SelfAttention + PoolAttFF; in general any
+                                   * framewise model (cnn_kind) + self-attention td, td_2 skip or self-attention          */
+  NISQA_ARCH_STD_LSTM_LASTBI = 1, /* nisqa_tts.tar: StandardCNN + BiLSTM + PoolLastStepBi; also any other
                                    * StandardCNN + LSTM checkpoint: its LSTM shape is read from the tensors given to
-                                   * nisqa_load_weights (weight_hh_l{k}[_reverse], cnn.model.fc_out.*)            */
+                                   * nisqa_load_weights (weight_hh_l{k}[_reverse], cnn.model.fc_out.*); td_2 skip or
+                                   * self-attention                                                                        */
+  NISQA_ARCH_SA_LSTM         = 2, /* any framewise model (cnn_kind) + self-attention td + LSTM td_2                        */
+  NISQA_ARCH_LSTM_LSTM       = 3  /* StandardCNN + LSTM td + LSTM td_2.  A td_2 LSTM's shape is read from
+                                   * time_dependency_2.model.lstm.weight_hh_l{k}[_reverse], like td's                      */
 };
 
-/* pooling over time (reference lib:1066-1225).  The shipped checkpoints use ATT_FF (nisqa*.tar) and LAST_STEP_BI
- * (nisqa_tts.tar); the others are reachable through user-trained checkpoints (SURVEY.md 8f.4). */
+/* pooling over time (reference lib:1066-1225) over the last time-dependency stage's rows.  The shipped checkpoints use
+ * ATT_FF (nisqa*.tar) and LAST_STEP_BI (nisqa_tts.tar); the others are reachable through user-trained checkpoints
+ * (SURVEY.md 8f.4). */
 enum nisqa_pool {
   NISQA_POOL_ATT_FF       = 0, /* PoolAttFF, h = 128 (lib:1156-1183)                  */
   NISQA_POOL_ATT          = 1, /* PoolAtt (lib:1131-1154)                             */
   NISQA_POOL_AVG          = 2, /* PoolAvg (lib:1185-1204)                             */
   NISQA_POOL_MAX          = 3, /* PoolMax (lib:1206-1225)                             */
   NISQA_POOL_LAST_STEP    = 4, /* PoolLastStep (lib:1117-1129)                        */
-  NISQA_POOL_LAST_STEP_BI = 5  /* PoolLastStepBi (lib:1099-1115), BiLSTM only         */
+  NISQA_POOL_LAST_STEP_BI = 5  /* PoolLastStepBi (lib:1099-1115), behind a bidirectional LSTM only */
 };
 
 /* double-ended model NISQA_DE (reference lib:272-424; train_nisqa_double_ended.yaml): time alignment of the reference
@@ -61,7 +68,9 @@ enum nisqa_de_align { NISQA_DE_ALIGN_DOT = 1, NISQA_DE_ALIGN_COSINE = 2, NISQA_D
 enum nisqa_de_apply { NISQA_DE_APPLY_HARD = 0, NISQA_DE_APPLY_SOFT = 1 };
 enum nisqa_de_fuse  { NISQA_DE_FUSE_XY_MINUS = 0 /* 'x/y/-' */, NISQA_DE_FUSE_PLUS_MINUS = 1 /* '+/-' */, NISQA_DE_FUSE_XY = 2 /* 'x/y' */ };
 
-enum nisqa_cnn_kind { NISQA_CNN_CONV = 0, NISQA_CNN_SKIP = 1, NISQA_CNN_DFF = 2 };
+/* framewise model in front of a self-attention td (arch 0 and 2; behind an LSTM td the CNN is always StandardCNN):
+ * CONV = AdaptCNN, STANDARD = StandardCNN (lib:811-836; its fc_out width is read from cnn.model.fc_out.*, cnn_fc stays 0) */
+enum nisqa_cnn_kind { NISQA_CNN_CONV = 0, NISQA_CNN_SKIP = 1, NISQA_CNN_DFF = 2, NISQA_CNN_STANDARD = 3 };
 
 enum nisqa_sample_fmt { NISQA_FMT_S16 = 0, NISQA_FMT_F32 = 1 };
 
@@ -88,9 +97,11 @@ enum nisqa_stage {
   NISQA_STAGE_CONV5    = 5, /* [n_seg, 64, 6, W3]                                            */
   NISQA_STAGE_CNN_FEAT = 6, /* [n_seg, 384] (adapt, index c*6+h) or [n_seg, F] (standard: fc_out's width F, or 768 in
                              * index c*12+h*2+w without fc_out)                                                        */
-  NISQA_STAGE_TD_IN    = 7, /* adapt only: LayerNorm(Linear 384->D) [n_seg, D], D = sa_d_model */
-  NISQA_STAGE_TD_OUT   = 8  /* [n_seg, D] (output of the last self-attention stack: td2_d_model when td_2 runs, else
-                             * sa_d_model) or [n_seg, dirs*H] (the last LSTM layer, fwd||bwd)                          */
+  NISQA_STAGE_TD_IN    = 7, /* the input LayerNorm output of the first self-attention stack that runs (td's, or td_2's
+                             * behind an LSTM td): LayerNorm(Linear(in -> D)) [n_seg, D]; not available without one     */
+  NISQA_STAGE_TD_OUT   = 8, /* output of the last time-dependency stage: [n_seg, D] (a self-attention stack: td2_d_model
+                             * when td_2 runs, else sa_d_model) or [n_seg, dirs*H] (the last LSTM layer, fwd||bwd)       */
+  NISQA_STAGE_TD1_OUT  = 9  /* NISQA / NISQA_DIM with a td_2 stage: td's output rows [n_seg, td fan_out] (D or dirs*H)   */
 };
 
 /* Mirrors the checkpoint 'args' the hot path consumes (SURVEY.md Appendix A). */
@@ -106,7 +117,7 @@ typedef struct nisqa_config {
   double  hop_s;         /* ms_hop_length seconds: hop = (int)(sr*hop_s), lib:2308 */
   double  win_s;         /* ms_win_length seconds: win = (int)(sr*win_s), lib:2309 */
   double  fmax;          /* ms_fmax Hz */
-  int32_t sa_layers;     /* td_sa_num_layers (adapt arch), else 0 */
+  int32_t sa_layers;     /* td_sa_num_layers (self-attention td: arch 0 and 2), else 0 */
   int32_t max_chunk_segments; /* 0 = default; upper bound on segments processed per internal pass */
   int32_t pool;          /* enum nisqa_pool */
   int32_t pos_enc;       /* td_sa_pos_enc: add the checkpoint's positional-encoding buffer after the input LayerNorm (lib:1042-1062) */
@@ -117,11 +128,11 @@ typedef struct nisqa_config {
   int32_t de_align;      /* enum nisqa_de_align */
   int32_t de_align_apply;/* enum nisqa_de_apply */
   int32_t de_fuse;       /* enum nisqa_de_fuse */
-  int32_t td2_layers;    /* td_2 = 'self_att' (one head, width td2_d_model, feed-forward td2_ff): number of layers; 0 = td_2 'skip'.  NISQA_DE needs >= 1;
-                          * NISQA / NISQA_DIM run it as a second stack behind the first (lib:114-141, 236-268) */
+  int32_t td2_layers;    /* td_2 = 'self_att' (one head, width td2_d_model, feed-forward td2_ff): number of layers; 0 = no such stack.  NISQA_DE needs >= 1;
+                          * NISQA / NISQA_DIM (arch 0 and 1) run it behind td (lib:114-141, 236-268); arch 2 and 3 keep 0 */
   int32_t td2_pos_enc;   /* td_2_sa_pos_enc */
-  /* framewise model in front of the self-attention stack (arch NISQA_ARCH_ADAPT_SA_ATTFF): */
-  int32_t cnn_kind;      /* enum nisqa_cnn_kind: 0 = the convolutional networks, 1 = SkipCNN (lib:504-534), 2 = DFF (lib:536-583) */
+  /* framewise model in front of a self-attention td (arch NISQA_ARCH_ADAPT_SA_ATTFF / NISQA_ARCH_SA_LSTM): */
+  int32_t cnn_kind;      /* enum nisqa_cnn_kind: 0 = AdaptCNN, 1 = SkipCNN (lib:504-534), 2 = DFF (lib:536-583), 3 = StandardCNN */
   int32_t cnn_fc;        /* cnn_fc_out_h: Linear behind the AdaptCNN (lib:682-684, 708-709), of SkipCNN (0 = none: 720 features),
                           * hidden width of DFF; a multiple of 64 */
   int32_t de_fuse_dim;   /* NISQA_DE: Linear(fused features -> de_fuse_dim) behind the fusion (lib:1399-1401, 1414-1415); 0 = none;

@@ -100,15 +100,17 @@ constexpr int kLanes = NISQA_LANES;
 constexpr int kStages = 6;     // staging slots / submissions in flight (uploads run ahead of the lanes)
 struct Lane {
   cudaStream_t stream = nullptr;
-  DevBuf mel, segtab, feats, xa, xb, qkv, qkv2, logits, feats20, tdout, partial, fused, td2in, ffa, ffb, gx, atth;
+  // td's stage works in tdout (self-attention: its TD_IN rows; LSTM: its output) and xa / xb, td_2's in td2in (its TD_IN
+  // rows), td2out (an LSTM's output) and ya / yb, so that td's output is still there after td_2 (NISQA_STAGE_TD1_OUT)
+  DevBuf mel, segtab, feats, xa, xb, ya, yb, qkv, qkv2, logits, feats20, tdout, td2out, partial, fused, td2in, ffa, ffb, gx, atth;
   DevBuf act[7];           // act[l]: fp32 channels-last map feeding conv layer l (2..6) on the FFMA path (and stage dumps)
   DevBuf planes[7];        // planes[l]: fp16 hi | lo plane pair feeding conv layer l (2..6), conv_split.cu
   size_t plane_bytes[7] = {0, 0, 0, 0, 0, 0, 0};   // offset of the lo plane inside planes[l] (half of the allocation)
   void release() {
     for (auto& b : act) b.release();
     for (auto& b : planes) b.release();
-    DevBuf* all[] = {&mel, &segtab, &feats, &xa, &xb, &qkv, &qkv2, &logits, &feats20, &tdout, &partial, &fused, &td2in,
-                     &ffa, &ffb, &gx, &atth};
+    DevBuf* all[] = {&mel, &segtab, &feats, &xa, &xb, &ya, &yb, &qkv, &qkv2, &logits, &feats20, &tdout, &td2out, &partial,
+                     &fused, &td2in, &ffa, &ffb, &gx, &atth};
     for (auto* b : all) b->release();
     if (stream) cudaStreamDestroy(stream);
   }
@@ -164,14 +166,18 @@ struct Weights {
   DeAlignParams de = {};
   PoolHeadParams pool_head = {};       // PoolAttFF
   PoolSimpleParams pool_simple = {};   // the other pooling modules
-  Linear fc;                     // StandardCNN fc_out 768 -> 20 (any width on the stacked-LSTM path: 64-column padded)
+  Linear fc;                     // StandardCNN fc_out 768 -> 20 (any other path: any width, 64-column padded)
+  int std_fc = 0;                // StandardCNN's fc_out width, read from cnn.model.fc_out.weight (0: none, 768 features)
+  // The shipped StandardCNN + LSTM shape (fc_out 20, one bidirectional layer of 128, one output, no attention pooling, no
+  // td_2) keeps lstm_batched_kernel and its LstmParams; every other LSTM runs as a stack of lstm_layer_kernel layers.
+  bool lstm_shipped = false;
   LstmParams lstm = {};
-  // The LSTM's shape, read from the checkpoint's tensors.  `stacked`: every shape but the shipped one (fc_out 20, one
-  // bidirectional layer of 128, one output, no attention pooling), which keeps lstm_batched_kernel.
-  struct LstmShape { bool stacked = false; int fc = 0, H = 0, layers = 0, dirs = 0; } lstm_shape;
-  Linear lstm_ih[4];             // stacked path: W_ih^T of each layer k-major [K pad 64][dirs 4H], bias b_ih + b_hh
-  const float* lstm_hh[4] = {};  // [dirs][4H][H]
-  Linear lstm_att;               // PoolAttFF behind the LSTM: linear1 of every head, k-major [D pad 64][n_heads 128]
+  // A stacked LSTM (td or td_2), its shape read from the checkpoint's tensors: W_ih^T of each layer k-major
+  // [K pad 64][dirs 4H], bias b_ih + b_hh, and W_hh [dirs][4H][H]
+  struct LstmShape { int H = 0, layers = 0, dirs = 0; };
+  struct LstmStack { LstmShape s; Linear ih[4]; const float* hh[4] = {}; };
+  LstmStack lstm_st[2];          // time_dependency, time_dependency_2
+  Linear lstm_att;               // PoolAttFF behind an LSTM: linear1 of every head, k-major [D pad 64][n_heads 128]
 };
 
 }  // namespace
@@ -208,6 +214,12 @@ struct nisqa_engine {
   int sa_f() const { return cfg.sa_ff ? cfg.sa_ff : 64; }
   int td2_d() const { return cfg.td2_d_model ? cfg.td2_d_model : 64; }
   int td2_f() const { return cfg.td2_ff ? cfg.td2_ff : 64; }
+  // which time-dependency model each stage runs, and the CNN geometry (StandardCNN: W 8/4/2, 768 features)
+  bool td_lstm() const { return cfg.arch == NISQA_ARCH_STD_LSTM_LASTBI || cfg.arch == NISQA_ARCH_LSTM_LSTM; }
+  bool td2_lstm() const { return cfg.arch == NISQA_ARCH_SA_LSTM || cfg.arch == NISQA_ARCH_LSTM_LSTM; }
+  bool td2_runs() const { return cfg.td2_layers > 0 || td2_lstm(); }
+  bool std_cnn() const { return td_lstm() || cfg.cnn_kind == NISQA_CNN_STANDARD; }
+  bool conv_net() const { return cfg.cnn_kind == NISQA_CNN_CONV || cfg.cnn_kind == NISQA_CNN_STANDARD; }
   int pool_d() const { return cfg.td2_layers > 0 ? td2_d() : sa_d(); }
 
   // front-end tables
@@ -235,6 +247,8 @@ struct nisqa_engine {
   const float* last_td_out = nullptr;
   int last_td_out_d = 64;       // row width of last_td_out
   int last_td_out_ld = 0;       // its row stride (0: the width)
+  const float* last_td1_out = nullptr;    // td's output when a td_2 stage ran (NISQA_STAGE_TD1_OUT)
+  int last_td1_out_d = 0, last_td1_out_ld = 0;
 
   // engine-owned NCCL communicator (multi-GPU gather, SURVEY.md 8e)
   void* nccl_comm = nullptr;
@@ -576,7 +590,7 @@ bool pack_ffnet(Packer& P, const nisqa_config& c) {
 // Linear, or SkipCNN / DFF
 bool pack_framewise(Packer& P, nisqa_engine* e) {
   const nisqa_config& c = e->cfg;
-  if (c.cnn_kind != NISQA_CNN_CONV) return pack_ffnet(P, c);
+  if (!e->conv_net()) return pack_ffnet(P, c);
   const int cin[7] = {0, 1, 16, 32, 64, 64, 64}, cout[7] = {0, 16, 32, 64, 64, 64, 64};
   for (int i = 1; i <= 6; ++i) {
     size_t w_off = 0;
@@ -598,9 +612,17 @@ bool pack_framewise(Packer& P, nisqa_engine* e) {
   return true;
 }
 
+// The rows that feed a time-dependency stage: `dim` features, padded with zero columns to a multiple of 64, in the order
+// of the checkpoint's Linear (PLAIN) or - conv6's features - in the engine's order: AdaptCNN k' = h*64 + c <-> reference
+// view(-1, 64*6) order c*6 + h (lib:706), StandardCNN k' = (h*2 + w)*64 + c <-> c*12 + h*2 + w (lib:830)
+enum InOrder { IN_PLAIN, IN_ADAPT_CONV, IN_STD_CONV };
+struct InRows { int dim; InOrder order; };
+int in_col(InOrder o, int k) { return o == IN_ADAPT_CONV ? (k & 63) * 6 + (k >> 6) : o == IN_STD_CONV ? (k & 63) * 12 + (k >> 6) : k; }
+
 // One SelfAttention stack (lib:945-1040) of width D and feed-forward width F, checkpoint prefix `ck`: Linear(in -> D) +
-// LayerNorm + `layers` encoder layers.  cnn_order: the input rows are AdaptCNN features in the engine's order.
-bool pack_sa_stack(Packer& P, SaStackWeights& S, const std::string& ck, int in_dim, int layers, bool cnn_order, int D, int F) {
+// LayerNorm + `layers` encoder layers.  The Linear's rows beyond in.dim (the padding of the input rows) stay zero.
+bool pack_sa_stack(Packer& P, SaStackWeights& S, const std::string& ck, InRows in, int layers, int D, int F) {
+  const int in_dim = in.dim;
   const TensorView* lw = P.get(ck + "linear.weight", {D, in_dim});
   const TensorView* lb = P.get(ck + "linear.bias", {D});
   const TensorView* ng = P.get(ck + "norm1.weight", {D});
@@ -608,10 +630,7 @@ bool pack_sa_stack(Packer& P, SaStackWeights& S, const std::string& ck, int in_d
   if (!lw || !lb || !ng || !nb) return false;
   const int k_pad = (in_dim + 63) / 64 * 64;
   const size_t o = P.alloc(S.in.wT, (size_t)k_pad * D);
-  if (cnn_order)      // engine feature order k' = h*64 + c  <->  reference view(-1, 64*6) order c*6 + h (lib:706)
-    pack_linear_chunked(P, o, lw, D, in_dim, k_pad, [](int k) { return (k & 63) * 6 + (k >> 6); });
-  else
-    pack_linear_chunked(P, o, lw, D, in_dim, k_pad, [](int k) { return k; });
+  pack_linear_chunked(P, o, lw, D, in_dim, k_pad, [&](int k) { return in_col(in.order, k); });
   P.copy(S.in.b, lb->d, D);
   P.copy(S.ln_g, ng->d, D);
   P.copy(S.ln_b, nb->d, D);
@@ -747,37 +766,6 @@ bool pack_pool_heads(Packer& P, const nisqa_config& c, int Dp, bool lstm = false
   return true;
 }
 
-// The self-attention architecture behind the framewise model: time_dependency, then (NISQA_DE's fusion and alignment, or
-// NISQA / NISQA_DIM's second stack) time_dependency_2, and the pooling module
-bool pack_sa_model(Packer& P, nisqa_engine* e) {
-  const nisqa_config& c = e->cfg;
-  const std::string td = "time_dependency.model.", td2 = "time_dependency_2.model.";
-  // framewise features feeding the first stack: 384 (AdaptCNN, engine order), 720 (SkipCNN without Linear: padded to 768
-  // with zero rows) or cnn_fc_out_h
-  const bool conv_net = c.cnn_kind == NISQA_CNN_CONV;
-  const int feat_dim = c.cnn_fc > 0 ? c.cnn_fc : (conv_net ? 384 : 720);
-  if (!pack_sa_stack(P, P.w.sa[0], td, feat_dim, c.sa_layers, conv_net && c.cnn_fc == 0, e->sa_d(), e->sa_f())) return false;
-  if (c.double_ended || c.td2_layers > 0) {
-    // time_dependency_2: behind the fusion of the double-ended model (input 192 / 128), or a second stack behind the
-    // first one in NISQA / NISQA_DIM (lib:114-141, 236-268; input: the first stack's width)
-    int fdim = !c.double_ended ? e->sa_d() : (c.de_fuse == NISQA_DE_FUSE_XY_MINUS ? 192 : 128);
-    if (c.double_ended && c.de_fuse_dim > 0) {        // Fusion.lin_fusion (lib:1399-1401)
-      const int D = c.de_fuse_dim;
-      const TensorView* w = P.get("fuse.lin_fusion.weight", {D, fdim});
-      const TensorView* b = P.get("fuse.lin_fusion.bias", {D});
-      if (!w || !b) return false;
-      pack_linear_T(P, P.alloc(P.w.defuse.wT, (size_t)fdim * D), w, D, fdim);
-      P.copy(P.w.defuse.b, b->d, D);
-      fdim = D;
-    }
-    if (!pack_sa_stack(P, P.w.sa[1], td2, fdim, c.td2_layers, false, e->td2_d(), e->td2_f())) return false;
-    if (c.td2_pos_enc && !pack_pos_enc(P, c, td2, P.w.sa[1], e->td2_d())) return false;
-    if (!pack_de_align(P, c)) return false;
-  }
-  if (c.pos_enc && !pack_pos_enc(P, c, td, P.w.sa[0], e->sa_d())) return false;
-  return pack_pool_heads(P, c, e->pool_d());
-}
-
 // The shipped StandardCNN + LSTM shape (nisqa_tts.tar): fc_out 768 -> 20, the BiLSTM(20 -> 128) and its pooling module
 bool pack_bilstm128(Packer& P, nisqa_engine* e) {
   const TensorView* fw = P.get("cnn.model.fc_out.weight", {20, 768});
@@ -813,28 +801,55 @@ bool pack_bilstm128(Packer& P, nisqa_engine* e) {
   return true;
 }
 
-// Any other StandardCNN + LSTM shape: fc_out 768 -> F (or none), `layers` LSTM layers of H units in `dirs` directions,
-// W_ih and W_hh of each layer, and the pooling module over D = dirs H.  Input rows of layer 0 are fc_out's (padded to a
-// multiple of 64 with zero columns) or conv6's 768 features in the engine's order; those of layer l > 0 are layer l - 1's
-// outputs, padded the same way.  Zero weights in the padding keep every product exact.
-bool pack_lstm_stack(Packer& P, nisqa_engine* e, const Weights::LstmShape& L) {
-  const std::string p = "time_dependency.model.lstm.";
+// StandardCNN's fc_out (lib:811-836): its width from cnn.model.fc_out.weight (absent: none, 0)
+bool read_std_fc(Packer& P, int* fc) {
+  *fc = 0;
+  auto it = P.t.find("cnn.model.fc_out.weight");
+  if (it == P.t.end()) return true;
+  *fc = it->second.nd == 2 ? (int)it->second.dims[0] : 0;
+  if (*fc < 1 || *fc > 1024) return P.fail("tensor cnn.model.fc_out.weight: width " + std::to_string(*fc) + " outside 1..1024");
+  return true;
+}
+
+// fc_out 768 -> F k-major with F padded to a multiple of 64 (zero columns), rows in the engine's conv6 order
+bool pack_std_fc(Packer& P, int F) {
+  const TensorView* fw = P.get("cnn.model.fc_out.weight", {F, 768});
+  const TensorView* fb = P.get("cnn.model.fc_out.bias", {F});
+  if (!fw || !fb) return false;
+  const int Fp = round64(F);
+  const size_t o = P.alloc(P.w.fc.wT, (size_t)768 * Fp);
+  for (int k = 0; k < 768; ++k)
+    for (int j = 0; j < F; ++j) P.arena[o + (size_t)k * Fp + j] = fw->d[(size_t)j * 768 + in_col(IN_STD_CONV, k)];
+  memcpy(&P.arena[P.alloc(P.w.fc.b, Fp)], fb->d, (size_t)F * 4);
+  return true;
+}
+
+// The shape of the LSTM under prefix `p` from its tensors: the weight_hh_l{k}[_reverse] shapes give H, the layer count and
+// the directions.  `arg` names the checkpoint argument in the refusal (td_lstm_h / td_2_lstm_h).
+bool read_lstm_shape(Packer& P, const std::string& p, const char* arg, Weights::LstmShape* L) {
+  auto it = P.t.find(p + "weight_hh_l0");
+  if (it == P.t.end()) return P.fail("missing tensor " + p + "weight_hh_l0");
+  L->H = it->second.nd == 2 ? (int)it->second.dims[1] : 0;
+  if (!lstm_layer_supported(L->H) || it->second.dims[0] != 4 * L->H)
+    return P.fail("tensor " + p + "weight_hh_l0: hidden size " + std::to_string(L->H) + " is not implemented by the engine (" +
+                  arg + " 32, 64, 96, 128, 192 or 256)");
+  L->layers = 0;
+  while (P.t.count(p + "weight_hh_l" + std::to_string(L->layers))) ++L->layers;
+  if (L->layers > 4) return P.fail("tensor " + p + "weight_hh_l4: the engine runs 1 to 4 LSTM layers");
+  L->dirs = P.t.count(p + "weight_hh_l0_reverse") ? 2 : 1;
+  return true;
+}
+
+// A stacked LSTM of any accepted shape under prefix `p`: W_ih and W_hh of each layer.  Layer 0 reads `in` (its padding
+// rows of W_ih stay zero); layer l > 0 reads layer l - 1's dirs H outputs, padded the same way.  Zero weights in the
+// padding keep every product exact.
+bool pack_lstm_stack(Packer& P, Weights::LstmStack& S, const std::string& p, InRows in0) {
+  const Weights::LstmShape& L = S.s;
   const int H = L.H, N = L.dirs * 4 * H, D = L.dirs * H;
-  if (L.fc > 0) {
-    const TensorView* fw = P.get("cnn.model.fc_out.weight", {L.fc, 768});
-    const TensorView* fb = P.get("cnn.model.fc_out.bias", {L.fc});
-    if (!fw || !fb) return false;
-    const int Fp = round64(L.fc);
-    const size_t o = P.alloc(P.w.fc.wT, (size_t)768 * Fp);
-    for (int hw = 0; hw < 12; ++hw)            // engine order k' = (h*2 + w)*64 + c <-> reference view order c*12 + h*2 + w
-      for (int c = 0; c < 64; ++c)
-        for (int j = 0; j < L.fc; ++j) P.arena[o + ((size_t)hw * 64 + c) * Fp + j] = fw->d[(size_t)j * 768 + c * 12 + hw];
-    memcpy(&P.arena[P.alloc(P.w.fc.b, Fp)], fb->d, (size_t)L.fc * 4);
-  }
   for (int l = 0; l < L.layers; ++l) {
-    const int in = l ? D : (L.fc ? L.fc : 768), K = round64(in);
-    const size_t owi = P.alloc(P.w.lstm_ih[l].wT, (size_t)K * N), ob = P.alloc(P.w.lstm_ih[l].b, N);
-    const size_t owh = P.alloc(P.w.lstm_hh[l], (size_t)L.dirs * 4 * H * H);
+    const int in = l ? D : in0.dim, K = round64(in);
+    const size_t owi = P.alloc(S.ih[l].wT, (size_t)K * N), ob = P.alloc(S.ih[l].b, N);
+    const size_t owh = P.alloc(S.hh[l], (size_t)L.dirs * 4 * H * H);
     for (int d = 0; d < L.dirs; ++d) {
       const std::string sfx = "_l" + std::to_string(l) + (d ? "_reverse" : "");
       const TensorView* wi = P.get(p + "weight_ih" + sfx, {4 * H, in});
@@ -843,45 +858,80 @@ bool pack_lstm_stack(Packer& P, nisqa_engine* e, const Weights::LstmShape& L) {
       const TensorView* bh = P.get(p + "bias_hh" + sfx, {4 * H});
       if (!wi || !wh || !bi || !bh) return false;
       for (int k = 0; k < in; ++k) {
-        // layer 0 without fc_out reads conv6's features in the engine's order (see above)
-        const int kc = (l == 0 && L.fc == 0) ? (k & 63) * 12 + (k >> 6) : k;
+        const int kc = l == 0 ? in_col(in0.order, k) : k;
         for (int g = 0; g < 4 * H; ++g) P.arena[owi + (size_t)k * N + d * 4 * H + g] = wi->d[(size_t)g * in + kc];
       }
       for (int g = 0; g < 4 * H; ++g) P.arena[ob + d * 4 * H + g] = bi->d[g] + bh->d[g];
       memcpy(&P.arena[owh + (size_t)d * 4 * H * H], wh->d, (size_t)4 * H * H * 4);
     }
   }
-  return pack_pool_heads(P, e->cfg, D, true);
+  return true;
 }
 
-// The StandardCNN architecture behind the convolutions: its LSTM's shape comes from the tensors (the weight_hh_l{k}
-// [_reverse] shapes give H, the layer count and the directions; cnn.model.fc_out.* present or not gives fc_out's width)
-bool pack_lstm_model(Packer& P, nisqa_engine* e) {
+// The time-dependency model behind the framewise model - td (self-attention or LSTM), then td_2 (NISQA_DE's fusion,
+// alignment and stack, or NISQA / NISQA_DIM's self-attention or LSTM stage, lib:114-141, 236-268) - and the pooling
+// module over the last stage's rows
+bool pack_td_model(Packer& P, nisqa_engine* e) {
   const nisqa_config& c = e->cfg;
-  const std::string p = "time_dependency.model.lstm.";
-  Weights::LstmShape L;
-  auto it = P.t.find(p + "weight_hh_l0");
-  if (it == P.t.end()) return P.fail("missing tensor " + p + "weight_hh_l0");
-  L.H = it->second.nd == 2 ? (int)it->second.dims[1] : 0;
-  if (!lstm_layer_supported(L.H) || it->second.dims[0] != 4 * L.H)
-    return P.fail("tensor " + p + "weight_hh_l0: hidden size " + std::to_string(L.H) +
-                  " is not implemented by the engine (td_lstm_h 32, 64, 96, 128, 192 or 256)");
-  while (P.t.count(p + "weight_hh_l" + std::to_string(L.layers))) ++L.layers;
-  if (L.layers > 4)
-    return P.fail("tensor " + p + "weight_hh_l4: the engine runs 1 to 4 LSTM layers");
-  L.dirs = P.t.count(p + "weight_hh_l0_reverse") ? 2 : 1;
-  if (c.pool == NISQA_POOL_LAST_STEP_BI && L.dirs != 2)
-    return P.fail("missing tensor " + p + "weight_hh_l0_reverse: PoolLastStepBi needs a bidirectional LSTM");
-  auto fc = P.t.find("cnn.model.fc_out.weight");
-  if (fc != P.t.end()) {
-    L.fc = fc->second.nd == 2 ? (int)fc->second.dims[0] : 0;
-    if (L.fc < 1 || L.fc > 1024)
-      return P.fail("tensor cnn.model.fc_out.weight: width " + std::to_string(L.fc) + " outside 1..1024");
+  Weights& W = P.w;
+  const std::string td = "time_dependency.model.", td2 = "time_dependency_2.model.";
+  // the rows feeding td: AdaptCNN's 384 (engine order), SkipCNN's 720 (padded to 768 with zero rows), cnn_fc_out_h, or
+  // StandardCNN's fc_out / 768 conv6 features (engine order)
+  InRows in;
+  if (e->std_cnn()) {
+    if (!read_std_fc(P, &W.std_fc)) return false;
+    in = W.std_fc ? InRows{W.std_fc, IN_PLAIN} : InRows{768, IN_STD_CONV};
+  } else {
+    const bool conv_net = c.cnn_kind == NISQA_CNN_CONV;
+    in = {c.cnn_fc > 0 ? c.cnn_fc : (conv_net ? 384 : 720), conv_net && c.cnn_fc == 0 ? IN_ADAPT_CONV : IN_PLAIN};
   }
-  L.stacked = !(L.fc == 20 && L.H == 128 && L.layers == 1 && L.dirs == 2 && c.n_out == 1 && c.pool != NISQA_POOL_ATT &&
-                c.pool != NISQA_POOL_ATT_FF);
-  P.w.lstm_shape = L;
-  return L.stacked ? pack_lstm_stack(P, e, L) : pack_bilstm128(P, e);
+  const Weights::LstmShape* last_lstm = nullptr;      // the last stage, when it is an LSTM
+  int d1;                                             // td's fan_out
+  if (e->td_lstm()) {
+    Weights::LstmShape& L = W.lstm_st[0].s;
+    if (!read_lstm_shape(P, td + "lstm.", "td_lstm_h", &L)) return false;
+    W.lstm_shipped = W.std_fc == 20 && L.H == 128 && L.layers == 1 && L.dirs == 2 && c.n_out == 1 && c.pool != NISQA_POOL_ATT &&
+                     c.pool != NISQA_POOL_ATT_FF && !e->td2_runs();
+    if (W.lstm_shipped) return pack_bilstm128(P, e);
+    if (W.std_fc > 0 && !pack_std_fc(P, W.std_fc)) return false;
+    if (!pack_lstm_stack(P, W.lstm_st[0], td + "lstm.", in)) return false;
+    d1 = L.dirs * L.H;
+    last_lstm = &L;
+  } else {
+    if (W.std_fc > 0 && !pack_std_fc(P, W.std_fc)) return false;
+    if (!pack_sa_stack(P, W.sa[0], td, in, c.sa_layers, e->sa_d(), e->sa_f())) return false;
+    d1 = e->sa_d();
+  }
+  int dp = d1;                                        // width of the rows the pooling module reads
+  if (c.double_ended || c.td2_layers > 0) {
+    // time_dependency_2: behind the fusion of the double-ended model (input 192 / 128), or a second stack behind td in
+    // NISQA / NISQA_DIM (input: td's fan_out)
+    int fdim = !c.double_ended ? d1 : (c.de_fuse == NISQA_DE_FUSE_XY_MINUS ? 192 : 128);
+    if (c.double_ended && c.de_fuse_dim > 0) {        // Fusion.lin_fusion (lib:1399-1401)
+      const int D = c.de_fuse_dim;
+      const TensorView* w = P.get("fuse.lin_fusion.weight", {D, fdim});
+      const TensorView* b = P.get("fuse.lin_fusion.bias", {D});
+      if (!w || !b) return false;
+      pack_linear_T(P, P.alloc(W.defuse.wT, (size_t)fdim * D), w, D, fdim);
+      P.copy(W.defuse.b, b->d, D);
+      fdim = D;
+    }
+    if (!pack_sa_stack(P, W.sa[1], td2, {fdim, IN_PLAIN}, c.td2_layers, e->td2_d(), e->td2_f())) return false;
+    if (c.td2_pos_enc && !pack_pos_enc(P, c, td2, W.sa[1], e->td2_d())) return false;
+    if (!pack_de_align(P, c)) return false;
+    dp = e->td2_d();
+    last_lstm = nullptr;
+  } else if (e->td2_lstm()) {
+    Weights::LstmShape& L2 = W.lstm_st[1].s;
+    if (!read_lstm_shape(P, td2 + "lstm.", "td_2_lstm_h", &L2)) return false;
+    if (!pack_lstm_stack(P, W.lstm_st[1], td2 + "lstm.", {d1, IN_PLAIN})) return false;
+    dp = L2.dirs * L2.H;
+    last_lstm = &L2;
+  }
+  if (!e->td_lstm() && c.pos_enc && !pack_pos_enc(P, c, td, W.sa[0], e->sa_d())) return false;
+  if (c.pool == NISQA_POOL_LAST_STEP_BI && (!last_lstm || last_lstm->dirs != 2))
+    return P.fail("missing tensor " + (e->td2_lstm() ? td2 : td) + "lstm.weight_hh_l0_reverse: PoolLastStepBi needs a bidirectional LSTM");
+  return pack_pool_heads(P, c, dp, last_lstm != nullptr);
 }
 
 int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
@@ -892,8 +942,7 @@ int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
     for (int d = 0; d < 4; ++d) { v.dims[d] = d < v.nd ? tensors[i].dims[d] : 1; v.numel *= v.dims[d]; }
     P.t[tensors[i].name] = v;
   }
-  const bool ok = pack_framewise(P, e) &&
-                  (e->cfg.arch == NISQA_ARCH_ADAPT_SA_ATTFF ? pack_sa_model(P, e) : pack_lstm_model(P, e));
+  const bool ok = pack_framewise(P, e) && pack_td_model(P, e);
   if (!ok) return fail(e, NISQA_ERR_WEIGHTS, P.err);
   CK(e->warena.reserve(P.arena.size() * 4));
   CK(cudaMemcpy(e->warena.p, P.arena.data(), P.arena.size() * 4, cudaMemcpyHostToDevice));
@@ -942,7 +991,7 @@ struct Pass {
   int* seg_clip = nullptr;
   Pass(nisqa_engine* e_, const PassInput& in)
       : e(e_), c(e_->cfg), w(e_->w), LN(e_->lanes[in.slot]), SG(e_->stages[in.stage]), st(LN.stream),
-        std_mode(c.arch == NISQA_ARCH_STD_LSTM_LASTBI), scores(in.scores_dev_out), n(in.n_clips) {}
+        std_mode(e_->std_cnn()), scores(in.scores_dev_out), n(in.n_clips) {}
 };
 
 // [n_seg][64 nk] rows that feed a time-dependency block
@@ -1101,14 +1150,14 @@ int ff_layers(Pass& p, Rows* out) {
   return 0;
 }
 
-// The framewise model: workspaces, front end, segment table, then the CNN (+ AdaptCNN's Linear) or SkipCNN / DFF.
-// `out`: the rows that feed the time-dependency block.
+// The framewise model: workspaces, front end, segment table, then the CNN (+ AdaptCNN's Linear or StandardCNN's fc_out)
+// or SkipCNN / DFF.  `out`: the rows that feed the time-dependency block (the shipped LSTM shape reads LN.feats itself).
 int framewise(Pass& p, int fmt, Rows* out) {
   nisqa_engine* e = p.e;
   const nisqa_config& c = p.c;
   Lane& LN = p.LN;
   const int n_seg = p.n_seg;
-  const bool conv_net = c.cnn_kind == NISQA_CNN_CONV, split = e->conv_tc != 0;
+  const bool conv_net = e->conv_net(), split = e->conv_tc != 0;
   CK(LN.mel.reserve((size_t)p.n_frames * kMels * 4));
   CK(LN.segtab.reserve((size_t)n_seg * 12));
   e->last_split = split;
@@ -1136,7 +1185,14 @@ int framewise(Pass& p, int fmt, Rows* out) {
   e->last_conv12 = split && e->conv12;
   if (!conv_net) return ff_layers(p, out);
   conv_layers(p);
-  *out = {LN.feats.as<float>(), 6};
+  *out = {LN.feats.as<float>(), p.std_mode ? 12 : 6};
+  if (p.std_mode && p.w.std_fc > 0 && !p.w.lstm_shipped) {      // StandardCNN's fc_out (lib:830-835), 64-column padded
+    Scope s(e, "fc_out");
+    const int Fp = round64(p.w.std_fc);
+    CK(LN.feats20.reserve((size_t)n_seg * Fp * 4));
+    launch_linear_tile(p.st, LN.feats.as<float>(), 768, p.w.fc.wT, p.w.fc.b, 0, LN.feats20.as<float>(), Fp, n_seg, 768, Fp);
+    *out = {LN.feats20.as<float>(), Fp / 64};
+  }
   if (c.cnn_fc > 0) {      // AdaptCNN's Linear behind conv6 (lib:708-709)
     Scope s(e, "framewise");
     CK(LN.ffb.reserve((size_t)n_seg * c.cnn_fc * 4));
@@ -1160,7 +1216,7 @@ const float* sa_stack(Pass& p, int k, Rows in, bool feeds_pool, float* x0) {
   const int nc = D / 64;
   const float qs = q_scale(D);
   const int n_heads = (feeds_pool && c.pool == NISQA_POOL_ATT_FF) ? c.n_out : 0;
-  float* pp[2] = {LN.xa.as<float>(), LN.xb.as<float>()};
+  float* pp[2] = {(k ? LN.ya : LN.xa).as<float>(), (k ? LN.yb : LN.xb).as<float>()};
   float* qk[2] = {LN.qkv.as<float>(), LN.qkv2.as<float>()};
   { Scope s(e, "lin_ln");
     launch_td_in(p.st, nc, in.x, S.in.wT, in.nk, S.in.b, S.ln_g, S.ln_b, S.qkv[0].wT, S.qkv[0].b, qs, S.pe, p.seg_clip,
@@ -1201,98 +1257,124 @@ int de_fuse(Pass& p, const float* td_rows, Rows* out) {
   return 0;
 }
 
-// The self-attention time-dependency block - one stack, two stacks (td_2), or NISQA_DE's stack, alignment and second
-// stack - and its pooling module
-int sa_head(Pass& p, Rows rows) {
+// One LSTM stage (k = 0: time_dependency, 1: time_dependency_2) of any accepted shape over `in`: per layer the input
+// projection of every step and direction (tile GEMM into gx) and the recurrence (lstm_layer_kernel).  Intermediate layers
+// alternate between two workspaces, the last one writes `dst`.  Rows are padded to a multiple of 64 floats with zero
+// columns (the next GEMM's K).  `out`: the last layer's rows.
+int lstm_stage(Pass& p, int k, Rows in, float* dst, Rows* out) {
   nisqa_engine* e = p.e;
-  const nisqa_config& c = p.c;
   Lane& LN = p.LN;
-  const int n_seg = p.n_seg, n_out = c.n_out;
-  const int D1 = e->sa_d(), D2 = c.td2_layers > 0 ? e->td2_d() : 0, Dm = std::max(D1, D2);
-  CK(LN.xa.reserve((size_t)n_seg * Dm * 4));
-  CK(LN.xb.reserve((size_t)n_seg * Dm * 4));
-  CK(LN.qkv.reserve((size_t)n_seg * 3 * Dm * 4));
-  CK(LN.logits.reserve((size_t)n_seg * n_out * 4));
-  CK(LN.tdout.reserve((size_t)n_seg * D1 * 4));
-  CK(LN.qkv2.reserve((size_t)n_seg * 3 * Dm * 4));
-  e->last_td_in = LN.tdout.as<float>();
-  const bool de = c.double_ended != 0;
-  const bool td2_single = !de && c.td2_layers > 0;      // NISQA / NISQA_DIM with td_2 = 'self_att'
-  const float* cur = sa_stack(p, 0, rows, !de && !td2_single, LN.tdout.as<float>());
-  if (td2_single) {
-    CK(LN.td2in.reserve((size_t)n_seg * D2 * 4));
-    cur = sa_stack(p, 1, {cur, D1 / 64}, true, LN.td2in.as<float>());
+  const Weights::LstmStack& S = p.w.lstm_st[k];
+  const Weights::LstmShape& L = S.s;
+  const int n_seg = p.n_seg, H = L.H, N = L.dirs * 4 * H, D = L.dirs * H, Dp = round64(D);
+  float* inter[2] = {(k ? LN.ya : LN.xa).as<float>(), (k ? LN.yb : LN.xb).as<float>()};
+  const float* x = in.x;
+  int ldx = 64 * in.nk;
+  for (int l = 0; l < L.layers; ++l) {
+    float* o = l + 1 == L.layers ? dst : inter[l & 1];
+    if (Dp != D) CK(cudaMemsetAsync(o, 0, (size_t)n_seg * Dp * 4, p.st));     // the padding columns the next GEMM reads
+    Scope s(e, "lstm", 2);
+    launch_linear_tile(p.st, x, ldx, S.ih[l].wT, S.ih[l].b, 0, LN.gx.as<float>(), N, n_seg, ldx, N);
+    const LstmLayerParams P = {LN.gx.as<float>(), N, S.hh[l], o, Dp};
+    launch_lstm_layer(p.st, H, L.dirs, p.clips, p.by_len, p.n, P);
+    x = o; ldx = Dp;
   }
-  if (de) {
-    Rows fused;
-    const int rc = de_fuse(p, cur, &fused);
-    if (rc) return rc;
-    cur = sa_stack(p, 1, fused, true, LN.td2in.as<float>());
-  }
-  e->last_td_out = cur;
-  e->last_td_out_d = e->pool_d();
-  e->last_td_out_ld = e->pool_d();
-  { Scope s(e, "pool");
-    if (c.pool == NISQA_POOL_ATT_FF)
-      launch_pool_final(p.st, cur, e->pool_d(), e->pool_d(), LN.logits.as<float>(), p.clips, p.n, p.w.pool_head, n_out, p.max_n_seg,
-                        p.scores);
-    else
-      launch_pool_simple(p.st, cur, e->pool_d(), e->pool_d(), p.clips, p.n, c.pool, p.w.pool_simple, n_out, p.max_n_seg, p.scores);
-    if (de) launch_de_finalize(p.st, p.clips, p.n, n_out, p.scores); }
+  *out = {x, Dp / 64};
   return 0;
 }
 
-// Any other LSTM shape: fc_out (tile GEMM), then per layer the input projection of every step and direction (tile GEMM)
-// and the recurrence (lstm_layer_kernel); the pooling module reads the last layer's rows.  Rows are padded to a multiple
-// of 64 floats with zero columns (the next GEMM's K).
-int lstm_stack_head(Pass& p) {
+// The pooling module over the last stage's rows x (D features at a stride of ld).  Behind a self-attention stack the
+// PoolAttFF logits come out of its last td_sa layer; behind an LSTM they are a tile GEMM + att_logits.
+int pool_rows(Pass& p, const float* x, int D, int ld, bool after_lstm) {
   nisqa_engine* e = p.e;
   const nisqa_config& c = p.c;
   Lane& LN = p.LN;
   const Weights& w = p.w;
-  const Weights::LstmShape& L = w.lstm_shape;
-  const int n_seg = p.n_seg, H = L.H, N = L.dirs * 4 * H, D = L.dirs * H, Dp = round64(D), Fp = round64(L.fc);
-  CK(LN.gx.reserve((size_t)n_seg * N * 4));
-  CK(LN.tdout.reserve((size_t)n_seg * Dp * 4));
-  const float* x = LN.feats.as<float>();
-  int ldx = 768;
-  if (L.fc > 0) {
-    Scope s(e, "fc_out");
-    CK(LN.feats20.reserve((size_t)n_seg * Fp * 4));
-    launch_linear_tile(p.st, x, 768, w.fc.wT, w.fc.b, 0, LN.feats20.as<float>(), Fp, n_seg, 768, Fp);
-    x = LN.feats20.as<float>(); ldx = Fp;
+  const int n_seg = p.n_seg, nh = c.n_out;
+  if (!after_lstm) {
+    Scope s(e, "pool");
+    if (c.pool == NISQA_POOL_ATT_FF)
+      launch_pool_final(p.st, x, D, ld, LN.logits.as<float>(), p.clips, p.n, w.pool_head, nh, p.max_n_seg, p.scores);
+    else
+      launch_pool_simple(p.st, x, D, ld, p.clips, p.n, c.pool, w.pool_simple, nh, p.max_n_seg, p.scores);
+    if (c.double_ended) launch_de_finalize(p.st, p.clips, p.n, nh, p.scores);
+    return 0;
   }
-  float* inter[2] = {nullptr, nullptr};
-  for (int l = 0; l + 1 < L.layers && l < 2; ++l) {
-    DevBuf& b = l ? LN.xb : LN.xa;
-    CK(b.reserve((size_t)n_seg * Dp * 4));
-    inter[l] = b.as<float>();
+  Scope s(e, "pool", c.pool == NISQA_POOL_ATT_FF ? 3 : 1);
+  if (c.pool == NISQA_POOL_ATT_FF) {
+    CK(LN.atth.reserve((size_t)n_seg * nh * 128 * 4));
+    CK(LN.logits.reserve((size_t)n_seg * nh * 4));
+    launch_linear_tile(p.st, x, ld, w.lstm_att.wT, w.lstm_att.b, 1, LN.atth.as<float>(), nh * 128, n_seg, ld, nh * 128);
+    launch_att_logits(p.st, LN.atth.as<float>(), w.pool_head.w2, w.pool_head.b2, nh, n_seg, LN.logits.as<float>());
+    launch_pool_final(p.st, x, D, ld, LN.logits.as<float>(), p.clips, p.n, w.pool_head, nh, p.max_n_seg, p.scores);
+  } else {
+    launch_pool_simple(p.st, x, D, ld, p.clips, p.n, c.pool, w.pool_simple, nh, p.max_n_seg, p.scores);
   }
-  for (int l = 0; l < L.layers; ++l) {
-    float* out = l + 1 == L.layers ? LN.tdout.as<float>() : inter[l & 1];
-    if (Dp != D) CK(cudaMemsetAsync(out, 0, (size_t)n_seg * Dp * 4, p.st));     // the padding columns the next GEMM reads
-    Scope s(e, "lstm", 2);
-    launch_linear_tile(p.st, x, ldx, w.lstm_ih[l].wT, w.lstm_ih[l].b, 0, LN.gx.as<float>(), N, n_seg, ldx, N);
-    const LstmLayerParams P = {LN.gx.as<float>(), N, w.lstm_hh[l], out, Dp};
-    launch_lstm_layer(p.st, H, L.dirs, p.clips, p.by_len, p.n, P);
-    x = out; ldx = Dp;
-  }
-  { Scope s(e, "pool", c.pool == NISQA_POOL_ATT_FF ? 3 : 1);
-    if (c.pool == NISQA_POOL_ATT_FF) {
-      const int nh = c.n_out;
-      CK(LN.atth.reserve((size_t)n_seg * nh * 128 * 4));
-      CK(LN.logits.reserve((size_t)n_seg * nh * 4));
-      launch_linear_tile(p.st, x, Dp, w.lstm_att.wT, w.lstm_att.b, 1, LN.atth.as<float>(), nh * 128, n_seg, Dp, nh * 128);
-      launch_att_logits(p.st, LN.atth.as<float>(), w.pool_head.w2, w.pool_head.b2, nh, n_seg, LN.logits.as<float>());
-      launch_pool_final(p.st, x, D, Dp, LN.logits.as<float>(), p.clips, p.n, w.pool_head, nh, p.max_n_seg, p.scores);
-    } else {
-      launch_pool_simple(p.st, x, D, Dp, p.clips, p.n, c.pool, w.pool_simple, c.n_out, p.max_n_seg, p.scores);
-    } }
-  e->last_td_in = nullptr;
-  e->last_td_out = x;
-  e->last_td_out_d = D;
-  e->last_td_out_ld = Dp;
   return 0;
+}
+
+// The time-dependency model - td, then td_2 when it runs (NISQA_DE: alignment, fusion and a stack) - and the pooling module
+// over the last stage's rows.  A self-attention stage is sa_stack (the PoolAttFF logits fused into its last layer when it
+// feeds the pooling module), an LSTM stage is lstm_stage.  td works in tdout / xa / xb, td_2 in td2in / td2out / ya / yb:
+// td's output stays readable after td_2 (NISQA_STAGE_TD1_OUT).
+int td_stages(Pass& p, Rows rows) {
+  nisqa_engine* e = p.e;
+  const nisqa_config& c = p.c;
+  Lane& LN = p.LN;
+  const Weights& w = p.w;
+  const int n_seg = p.n_seg;
+  const bool de = c.double_ended != 0, sa1 = !e->td_lstm(), sa2 = c.td2_layers > 0, lstm2 = e->td2_lstm();
+  const Weights::LstmShape &L1 = w.lstm_st[0].s, &L2 = w.lstm_st[1].s;
+  auto res = [&](DevBuf& b, size_t floats) { return b.reserve(floats * 4); };
+  // workspaces of both stages, reserved before the first launch
+  const size_t D1 = sa1 ? e->sa_d() : round64(L1.dirs * L1.H), D2 = sa2 ? e->td2_d() : lstm2 ? round64(L2.dirs * L2.H) : 0;
+  size_t qkv = 0, gx = 0;
+  if (sa1) qkv = 3 * D1; else gx = (size_t)L1.dirs * 4 * L1.H;
+  if (sa2) qkv = std::max(qkv, 3 * D2);
+  if (lstm2) gx = std::max(gx, (size_t)L2.dirs * 4 * L2.H);
+  if (sa1 || L1.layers > 1) { CK(res(LN.xa, n_seg * D1)); CK(res(LN.xb, n_seg * D1)); }
+  if (sa2 || (lstm2 && L2.layers > 1)) { CK(res(LN.ya, n_seg * D2)); CK(res(LN.yb, n_seg * D2)); }
+  if (qkv) {
+    CK(res(LN.qkv, n_seg * qkv));
+    CK(res(LN.qkv2, n_seg * qkv));
+    CK(res(LN.logits, (size_t)n_seg * c.n_out));
+  }
+  if (gx) CK(res(LN.gx, n_seg * gx));
+  CK(res(LN.tdout, n_seg * D1));
+  if (sa2) CK(res(LN.td2in, n_seg * D2));
+  if (lstm2) CK(res(LN.td2out, n_seg * D2));
+
+  Rows cur;
+  e->last_td_in = nullptr;
+  if (sa1) {
+    e->last_td_in = LN.tdout.as<float>();
+    cur = {sa_stack(p, 0, rows, !e->td2_runs(), LN.tdout.as<float>()), e->sa_d() / 64};
+  } else {
+    const int rc = lstm_stage(p, 0, rows, LN.tdout.as<float>(), &cur);
+    if (rc) return rc;
+  }
+  int D = sa1 ? e->sa_d() : L1.dirs * L1.H;           // width of cur's rows
+  e->last_td1_out = nullptr;
+  if (e->td2_runs() && !de) { e->last_td1_out = cur.x; e->last_td1_out_d = D; e->last_td1_out_ld = 64 * cur.nk; }
+  if (de) {
+    Rows fused;
+    const int rc = de_fuse(p, cur.x, &fused);
+    if (rc) return rc;
+    cur = {sa_stack(p, 1, fused, true, LN.td2in.as<float>()), e->td2_d() / 64};
+    D = e->td2_d();
+  } else if (sa2) {
+    if (!e->last_td_in) e->last_td_in = LN.td2in.as<float>();
+    cur = {sa_stack(p, 1, cur, true, LN.td2in.as<float>()), e->td2_d() / 64};
+    D = e->td2_d();
+  } else if (lstm2) {
+    const int rc = lstm_stage(p, 1, cur, LN.td2out.as<float>(), &cur);
+    if (rc) return rc;
+    D = L2.dirs * L2.H;
+  }
+  e->last_td_out = cur.x;
+  e->last_td_out_d = D;
+  e->last_td_out_ld = 64 * cur.nk;
+  return pool_rows(p, cur.x, D, 64 * cur.nk, lstm2 || (!sa1 && !sa2));
 }
 
 // The shipped shape's fc_out 768 -> 20, BiLSTM and pooling (PoolLastStepBi fused into the BiLSTM launch)
@@ -1320,6 +1402,7 @@ int lstm_head(Pass& p) {
     launch_pool_simple(p.st, LN.tdout.as<float>(), 256, 256, p.clips, p.n, c.pool, w.pool_simple, 1, p.max_n_seg, p.scores);
   }
   e->last_td_in = nullptr;
+  e->last_td1_out = nullptr;
   e->last_td_out = (e->lstm_batched && !keep) ? nullptr : LN.tdout.as<float>();
   e->last_td_out_d = 256;
   e->last_td_out_ld = 256;
@@ -1336,7 +1419,7 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
   } else {
     Rows rows;
     rc = framewise(p, in.fmt, &rows);
-    if (!rc) rc = !p.std_mode ? sa_head(p, rows) : p.w.lstm_shape.stacked ? lstm_stack_head(p) : lstm_head(p);
+    if (!rc) rc = p.w.lstm_shipped ? lstm_head(p) : td_stages(p, rows);
     if (rc) return rc;
   }
   CK(cudaGetLastError());
@@ -1472,32 +1555,34 @@ int nisqa_create(nisqa_engine** out, int device, const nisqa_config* cfg) {
   memset(&e->cfg, 0, sizeof e->cfg);
   memcpy(&e->cfg, cfg, cfg->abi_version == 3 ? offsetof(nisqa_config, sa_d_model) : sizeof(nisqa_config));
   cfg = &e->cfg;
-  if (cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF && cfg->arch != NISQA_ARCH_STD_LSTM_LASTBI)
+  if (cfg->arch < NISQA_ARCH_ADAPT_SA_ATTFF || cfg->arch > NISQA_ARCH_LSTM_LSTM)
     return fail(e, NISQA_ERR_INVALID, "unsupported architecture");
+  const bool sa_td = !e->td_lstm();          // a self-attention td: arch 0 and 2
+  const bool last_sa = sa_td ? !e->td2_lstm() : cfg->td2_layers > 0;      // the pooling module reads self-attention rows
   if (cfg->n_fft != kNfft || cfg->n_mels != kMels || cfg->seg_len != kSegLen)
     return fail(e, NISQA_ERR_INVALID, "engine is built for n_fft=4096, n_mels=48, seg_length=15");
   if (cfg->n_out != 1 && cfg->n_out != 5) return fail(e, NISQA_ERR_INVALID, "n_out must be 1 or 5");
   if (cfg->seg_hop < 1 || cfg->hop_s <= 0 || cfg->win_s <= 0 || cfg->fmax <= 0)
     return fail(e, NISQA_ERR_INVALID, "bad front-end parameters");
-  if (cfg->arch == NISQA_ARCH_ADAPT_SA_ATTFF && (cfg->sa_layers < 1 || cfg->sa_layers > 8))
+  if (sa_td && (cfg->sa_layers < 1 || cfg->sa_layers > 8))
     return fail(e, NISQA_ERR_INVALID, "sa_layers");
-  if (cfg->pool < NISQA_POOL_ATT_FF || cfg->pool > NISQA_POOL_LAST_STEP_BI ||
-      (cfg->arch == NISQA_ARCH_ADAPT_SA_ATTFF && cfg->pool == NISQA_POOL_LAST_STEP_BI))
-    return fail(e, NISQA_ERR_INVALID, "pooling module not available for this architecture");
-  if (cfg->pos_enc && cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF) return fail(e, NISQA_ERR_INVALID, "pos_enc needs the self-attention architecture");
-  if (cfg->cnn_kind < NISQA_CNN_CONV || cfg->cnn_kind > NISQA_CNN_DFF || cfg->cnn_fc < 0 || cfg->cnn_fc % 64 != 0 || cfg->cnn_fc > 8192 ||
-      (cfg->cnn_kind == NISQA_CNN_DFF && cfg->cnn_fc == 0) || (cfg->cnn_fc != 0 && cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF) ||
-      (cfg->cnn_kind != NISQA_CNN_CONV && cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF) ||
+  if (cfg->pool < NISQA_POOL_ATT_FF || cfg->pool > NISQA_POOL_LAST_STEP_BI || (last_sa && cfg->pool == NISQA_POOL_LAST_STEP_BI))
+    return fail(e, NISQA_ERR_INVALID, "pooling module not available for this architecture (PoolLastStepBi needs an LSTM as the last stage)");
+  if (cfg->pos_enc && !sa_td) return fail(e, NISQA_ERR_INVALID, "pos_enc needs a self-attention td");
+  if (cfg->cnn_kind < NISQA_CNN_CONV || cfg->cnn_kind > NISQA_CNN_STANDARD || cfg->cnn_fc < 0 || cfg->cnn_fc % 64 != 0 || cfg->cnn_fc > 8192 ||
+      (cfg->cnn_kind == NISQA_CNN_DFF && cfg->cnn_fc == 0) || (cfg->cnn_fc != 0 && (!sa_td || cfg->cnn_kind == NISQA_CNN_STANDARD)) ||
+      (cfg->cnn_kind != NISQA_CNN_CONV && !sa_td) ||
       cfg->de_fuse_dim < 0 || cfg->de_fuse_dim % 64 != 0 || cfg->de_fuse_dim > 8192 || (cfg->de_fuse_dim != 0 && !cfg->double_ended))
-    return fail(e, NISQA_ERR_INVALID, "cnn_kind / cnn_fc: SkipCNN and DFF feed the self-attention architecture; cnn_fc_out_h a multiple of 64");
-  if (cfg->td2_layers < 0 || cfg->td2_layers > 8 || (cfg->td2_layers > 0 && cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF))
-    return fail(e, NISQA_ERR_INVALID, "td_2 = 'self_att' needs the self-attention architecture (td2_layers 0..8)");
+    return fail(e, NISQA_ERR_INVALID, "cnn_kind / cnn_fc: SkipCNN, DFF and StandardCNN (cnn_kind) feed a self-attention td; cnn_fc_out_h a "
+                                      "multiple of 64 (StandardCNN's fc_out comes from the weights)");
+  if (cfg->td2_layers < 0 || cfg->td2_layers > 8 || (cfg->td2_layers > 0 && e->td2_lstm()))
+    return fail(e, NISQA_ERR_INVALID, "td_2 = 'self_att' needs arch 0 or 1 (td2_layers 0..8)");
   {
     const int32_t w[4] = {cfg->sa_d_model, cfg->sa_ff, cfg->td2_d_model, cfg->td2_ff};
     const char* nm[4] = {"sa_d_model", "sa_ff", "td2_d_model", "td2_ff"};
     for (int i = 0; i < 4; ++i) {
       const int lim = (i & 1) ? 4096 : 256;        // d_model 64..256, feed-forward width 64..4096, multiples of 64 (0 = 64)
-      if (w[i] < 0 || w[i] % 64 != 0 || w[i] > lim || (w[i] != 0 && cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF))
+      if (w[i] < 0 || w[i] % 64 != 0 || w[i] > lim || (w[i] != 0 && (i < 2 ? !sa_td : cfg->td2_layers == 0)))
         return fail(e, NISQA_ERR_INVALID, std::string(nm[i]) + " = " + std::to_string(w[i]) +
                                               ": the self-attention kernels take d_model 64..256 and h 64..4096, multiples of 64");
     }
@@ -1505,7 +1590,7 @@ int nisqa_create(nisqa_engine** out, int device, const nisqa_config* cfg) {
       return fail(e, NISQA_ERR_INVALID, "NISQA_DE: the alignment and fusion kernels are 64 wide (sa_d_model = td2_d_model = 64)");
   }
   if (cfg->double_ended) {
-    if (cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF || cfg->n_out != 1)
+    if (cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF || cfg->cnn_kind == NISQA_CNN_STANDARD || cfg->n_out != 1)
       return fail(e, NISQA_ERR_INVALID, "NISQA_DE: AdaptCNN + self-attention, one output");
     if (cfg->de_align < NISQA_DE_ALIGN_DOT || cfg->de_align > NISQA_DE_ALIGN_BAHDANAU)
       return fail(e, NISQA_ERR_INVALID, "de_align: dot, cosine, distance, luong or bahd");
@@ -1716,9 +1801,9 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
   cudaSetDevice(e->device);
   Lane& LN = e->lanes[e->last_lane];
   Stage& SG = e->stages[e->last_stage];
-  const int std_mode = e->cfg.arch == NISQA_ARCH_STD_LSTM_LASTBI;
+  const int std_mode = e->std_cnn();
   const int64_t ns = e->last_n_seg;
-  if (e->cfg.cnn_kind != NISQA_CNN_CONV && stage >= NISQA_STAGE_POOL1 && stage <= NISQA_STAGE_CNN_FEAT)
+  if (!e->conv_net() && stage >= NISQA_STAGE_POOL1 && stage <= NISQA_STAGE_CNN_FEAT)
     return fail(e, NISQA_ERR_INVALID, "stage not available: this checkpoint has no convolutional framewise model");
   const bool conv_map = stage >= NISQA_STAGE_POOL1 && stage <= NISQA_STAGE_CONV5;
   const int layer = stage - NISQA_STAGE_POOL1 + 2;      // POOL1 .. CONV5: the map that feeds conv layer 2 .. 6
@@ -1734,19 +1819,22 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
     case NISQA_STAGE_MEL_DB: count = (int64_t)e->last_n_frames * kMels; break;
     case NISQA_STAGE_POOL1: case NISQA_STAGE_POOL2: case NISQA_STAGE_CONV3: case NISQA_STAGE_POOL3: case NISQA_STAGE_CONV5: break;
     case NISQA_STAGE_CNN_FEAT:
-      if (std_mode && e->w.lstm_shape.stacked && e->w.lstm_shape.fc > 0) {
-        src = LN.feats20.as<float>(); width = e->w.lstm_shape.fc; ld = round64(width); count = ns * width;
-      } else if (std_mode && e->w.lstm_shape.stacked) {
-        src = LN.feats.as<float>(); hw = 12; ch = 64;           // [h*2+w][c] -> c*12+h*2+w
-      } else if (std_mode) {
+      if (std_mode && e->w.lstm_shipped) {
         src = LN.feats20.as<float>(); count = ns * 20;
+      } else if (std_mode && e->w.std_fc > 0) {
+        src = LN.feats20.as<float>(); width = e->w.std_fc; ld = round64(width); count = ns * width;
+      } else if (std_mode) {
+        src = LN.feats.as<float>(); hw = 12; ch = 64;           // [h*2+w][c] -> c*12+h*2+w
       } else {
         src = LN.feats.as<float>(); hw = 6; ch = 64;            // [h][c] -> c*6+h
       }
       break;
     case NISQA_STAGE_TD_IN:
-      if (std_mode || !e->last_td_in) return fail(e, NISQA_ERR_INVALID, "stage not available for this architecture");
-      src = e->last_td_in; count = ns * e->sa_d(); break;
+      if (!e->last_td_in) return fail(e, NISQA_ERR_INVALID, "stage not available for this architecture");
+      src = e->last_td_in; count = ns * (e->td_lstm() ? e->td2_d() : e->sa_d()); break;
+    case NISQA_STAGE_TD1_OUT:
+      if (!e->last_td1_out) return fail(e, NISQA_ERR_INVALID, "stage not available: no td_2 stage ran");
+      src = e->last_td1_out; count = ns * e->last_td1_out_d; width = e->last_td1_out_d; ld = e->last_td1_out_ld; break;
     case NISQA_STAGE_TD_OUT:
       if (!e->last_td_out) return fail(e, NISQA_ERR_STATE, "the per-step BiLSTM outputs were not kept: nisqa_set_option(\"keep_td_out\", 1) before the predict call");
       src = e->last_td_out; count = ns * e->last_td_out_d; width = e->last_td_out_d; ld = e->last_td_out_ld; break;

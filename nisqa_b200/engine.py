@@ -15,17 +15,18 @@ LIB_PATH = os.path.join(_HERE, "libnisqa_b200.so")
 
 ABI_VERSION = 4
 MAX_IN_FLIGHT = 6          # staging slots of the engine (nisqa_submit_pcm)
-ARCH_ADAPT_SA_ATTFF, ARCH_STD_LSTM_LASTBI = 0, 1
+# enum nisqa_arch: td self-attention (0) or LSTM (1) with td_2 skip or self-attention; td_2 LSTM behind either (2, 3)
+ARCH_ADAPT_SA_ATTFF, ARCH_STD_LSTM_LASTBI, ARCH_SA_LSTM, ARCH_LSTM_LSTM = 0, 1, 2, 3
 FMT_S16, FMT_F32 = 0, 1
 CLIP_OK, CLIP_TOO_SHORT, CLIP_TOO_LONG = 0, 1, 2
 POOL_ATT_FF, POOL_ATT, POOL_AVG, POOL_MAX, POOL_LAST_STEP, POOL_LAST_STEP_BI = range(6)
 # NISQA_DE options (enum nisqa_de_align / nisqa_de_apply / nisqa_de_fuse)
-CNN_CONV, CNN_SKIP, CNN_DFF = 0, 1, 2
+CNN_CONV, CNN_SKIP, CNN_DFF, CNN_STANDARD = 0, 1, 2, 3
 DE_ALIGN = {"dot": 1, "cosine": 2, "distance": 3, "luong": 4, "bahd": 5}
 DE_APPLY = {"hard": 0, "soft": 1}
 DE_FUSE = {"x/y/-": 0, "+/-": 1, "x/y": 2}
 (STAGE_MEL_DB, STAGE_POOL1, STAGE_POOL2, STAGE_CONV3, STAGE_POOL3, STAGE_CONV5, STAGE_CNN_FEAT,
- STAGE_TD_IN, STAGE_TD_OUT) = range(9)
+ STAGE_TD_IN, STAGE_TD_OUT, STAGE_TD1_OUT) = range(10)
 
 # every symbol include/nisqa_b200.h declares (checked by tests/test_abi.py)
 EXPORTS = [
@@ -72,21 +73,25 @@ def _sa_widths(args, prefix, de=False):
     return int(d), int(h)
 
 
-def _check_lstm(args, pool_mode):
-    """Refuses the StandardCNN + LSTM hyper-parameters the kernels do not implement, naming the value.  The engine reads
-    the LSTM's shape from the checkpoint's tensors (nisqa_load_weights); nothing of it goes into nisqa_config."""
-    h, nl, fc = args.get("td_lstm_h"), args.get("td_lstm_num_layers"), args.get("cnn_fc_out_h")
+def _check_lstm(args, key):
+    """Refuses the LSTM hyper-parameters ('td_lstm' / 'td_2_lstm') the kernels do not implement, naming the value; returns
+    the LSTM's fan_out.  The engine reads the LSTM's shape from the checkpoint's tensors (nisqa_load_weights); nothing of
+    it goes into nisqa_config."""
+    where = "td_2='lstm' with " if key == "td_2_lstm" else ""
+    h, nl = args.get(key + "_h"), args.get(key + "_num_layers")
     if h not in LSTM_H:
-        raise NotImplementedError("td_lstm_h=%r: the engine runs LSTM hidden sizes %s" % (h, ", ".join(map(str, LSTM_H))))
+        raise NotImplementedError("%s%s_h=%r: the engine runs LSTM hidden sizes %s" % (where, key, h, ", ".join(map(str, LSTM_H))))
     if nl is None or int(nl) != nl or not 1 <= nl <= LSTM_LAYERS_MAX:
-        raise NotImplementedError("td_lstm_num_layers=%r: the engine runs 1 to %d LSTM layers" % (nl, LSTM_LAYERS_MAX))
-    if pool_mode == POOL_LAST_STEP_BI and not args.get("td_lstm_bidirectional"):
-        raise NotImplementedError("pool='last_step_bi' with td_lstm_bidirectional=%r: PoolLastStepBi needs a bidirectional LSTM"
-                                  % (args.get("td_lstm_bidirectional"),))
+        raise NotImplementedError("%s%s_num_layers=%r: the engine runs 1 to %d LSTM layers" % (where, key, nl, LSTM_LAYERS_MAX))
+    return (2 if args.get(key + "_bidirectional") else 1) * h
+
+
+def _check_standard_cnn(args):
+    """Refuses the StandardCNN hyper-parameters the kernels do not implement, naming the value.  Its fc_out width comes
+    from the checkpoint's tensors."""
+    fc = args.get("cnn_fc_out_h")
     if fc and (int(fc) != fc or not 1 <= fc <= CNN_FC_OUT_MAX):
         raise NotImplementedError("cnn_fc_out_h=%r: the engine runs fc_out widths 1 to %d (or None)" % (fc, CNN_FC_OUT_MAX))
-    if args.get("td_2") not in (None, "skip"):
-        raise NotImplementedError("td_2=%r behind an LSTM is not implemented by the engine" % (args.get("td_2"),))
     ch = (args.get("cnn_c_out_1"), args.get("cnn_c_out_2"), args.get("cnn_c_out_3"))
     if ch != (16, 32, 64):
         raise NotImplementedError("cnn_c_out_1/2/3=%r: the engine runs StandardCNN with 16, 32, 64 channels" % (ch,))
@@ -205,14 +210,20 @@ def config_from_args(args, max_chunk_segments=0):
     if pool_mode is None:
         raise NotImplementedError("Pool option not available in the engine: %r" % pool)
     cnn_kind, cnn_fc = CNN_CONV, 0
-    if (cnn, td) == ("adapt", "self_att") and pool_mode != POOL_LAST_STEP_BI:
+    td2 = args.get("td_2") or "skip"
+    if td2 not in ("skip", "self_att", "lstm"):
+        raise NotImplementedError("td_2=%r is not implemented by the engine (skip, self_att or lstm)" % (args.get("td_2"),))
+    if de and td2 != "self_att":
+        # (NISQA_DE fuses two self-attention outputs into a self-attention td_2, lib:404-424)
+        raise NotImplementedError("NISQA_DE with td_2=%r: the engine runs NISQA_DE with td_2='self_att'" % (args.get("td_2"),))
+    if cnn == "adapt" and td == "self_att":
         arch = ARCH_ADAPT_SA_ATTFF
         ok = (list(args["cnn_pool_1"]) == [24, 7] and list(args["cnn_pool_2"]) == [12, 5]
               and list(args["cnn_pool_3"]) == [6, 3])
         cnn_fc = int(args.get("cnn_fc_out_h") or 0)           # optional Linear behind conv6 (lib:682-684)
         if cnn_fc % 64 != 0:
             raise NotImplementedError("cnn_fc_out_h=%d: the engine needs a multiple of 64" % cnn_fc)
-    elif cnn in (None, "skip", "dff") and td == "self_att" and pool_mode != POOL_LAST_STEP_BI:
+    elif cnn in (None, "skip", "dff") and td == "self_att":
         # framewise models without convolutions (lib:504-583) in front of the self-attention stack
         arch = ARCH_ADAPT_SA_ATTFF
         cnn_kind = CNN_DFF if cnn == "dff" else CNN_SKIP
@@ -222,14 +233,33 @@ def config_from_args(args, max_chunk_segments=0):
         if cnn_fc % 64 != 0:
             raise NotImplementedError("cnn_fc_out_h=%d: the engine needs a multiple of 64" % cnn_fc)
         ok = True
+    elif (cnn, td) == ("standard", "self_att") and not de:
+        # StandardCNN (lib:811-836) in front of the self-attention stack; fc_out's width comes from the weights
+        arch, cnn_kind = ARCH_ADAPT_SA_ATTFF, CNN_STANDARD
+        _check_standard_cnn(args)
+        ok = True
     elif (cnn, td) == ("standard", "lstm"):
         # any LSTM width, depth and direction behind StandardCNN (lib:811-836, 925-943), every pooling module
         arch = ARCH_STD_LSTM_LASTBI
-        _check_lstm(args, pool_mode)
+        _check_standard_cnn(args)
         ok = True
     else:
         raise NotImplementedError(
             "architecture cnn=%r td=%r pool=%r is not implemented by the engine" % (cnn, td, pool))
+    if td2 == "lstm":
+        arch = ARCH_LSTM_LSTM if arch == ARCH_STD_LSTM_LASTBI else ARCH_SA_LSTM
+    # fan_out of each stage (lib:839-895): the pooling module reads the last one's rows
+    td_lstm = arch in (ARCH_STD_LSTM_LASTBI, ARCH_LSTM_LSTM)
+    fan1 = _check_lstm(args, "td_lstm") if td_lstm else None
+    fan2 = _check_lstm(args, "td_2_lstm") if td2 == "lstm" else None
+    if pool_mode == POOL_LAST_STEP_BI:
+        key = "td_2_lstm" if td2 == "lstm" else "td_lstm" if td2 == "skip" and td_lstm else None
+        if key is None:
+            raise NotImplementedError("pool='last_step_bi' behind td=%r, td_2=%r: PoolLastStepBi needs a bidirectional LSTM as the "
+                                      "last time-dependency stage" % (td, args.get("td_2")))
+        if not args.get(key + "_bidirectional"):
+            raise NotImplementedError("pool='last_step_bi' with %s_bidirectional=%r: PoolLastStepBi needs a bidirectional LSTM"
+                                      % (key, args.get(key + "_bidirectional")))
     ks = args.get("cnn_kernel_size")
     ok = ok and (ks == 3 or tuple(ks) == (3, 3))
     if de:
@@ -243,25 +273,24 @@ def config_from_args(args, max_chunk_segments=0):
             raise NotImplementedError("de_align_apply / de_fuse option not available: %r / %r" % (args.get("de_align_apply"), args.get("de_fuse")))
         if args.get("de_fuse_dim") and int(args["de_fuse_dim"]) % 64 != 0:
             raise NotImplementedError("de_fuse_dim=%r: the engine needs a multiple of 64" % (args.get("de_fuse_dim"),))
-        ok = ok and args.get("td_2") == "self_att"
-    elif args.get("td_2") == "self_att":
-        # a second self-attention stack behind the first one (lib:114-141, 236-268)
-        ok = ok and arch == ARCH_ADAPT_SA_ATTFF
-    else:
-        ok = ok and args.get("td_2") in (None, "skip")
     ok = ok and (cnn_kind != CNN_CONV or (args["cnn_c_out_1"], args["cnn_c_out_2"], args["cnn_c_out_3"]) == (16, 32, 64))
     ok = ok and args["ms_n_fft"] == 4096 and args["ms_n_mels"] == 48 and args["ms_seg_length"] == 15
     if not ok:
         raise NotImplementedError("checkpoint hyper-parameters outside the shipped NISQA configurations")
-    sa = td2 = (0, 0)
-    if arch == ARCH_ADAPT_SA_ATTFF:
+    sa = td2w = (0, 0)
+    if not td_lstm:
         sa = _sa_widths(args, "td_sa", de)
-        if args.get("td_2") == "self_att":
-            td2 = _sa_widths(args, "td_2_sa", de)
-            if args["model"] == "NISQA_DIM" and td2[0] != sa[0]:
-                # NISQA_DIM builds its pooling heads for the first stack's width (lib:247-253): td_2 must keep it
-                raise NotImplementedError("NISQA_DIM with td_2_sa_d_model=%d != td_sa_d_model=%d: the reference model cannot "
-                                          "run it" % (td2[0], sa[0]))
+        fan1 = sa[0]
+    if td2 == "self_att":
+        td2w = _sa_widths(args, "td_2_sa", de)
+        fan2 = td2w[0]
+    if args["model"] == "NISQA_DIM" and fan2 is not None and fan2 != fan1:
+        # NISQA_DIM builds its pooling heads for td's fan_out (lib:247-253): td_2 must keep it
+        if td2 == "self_att" and not td_lstm:
+            raise NotImplementedError("NISQA_DIM with td_2_sa_d_model=%d != td_sa_d_model=%d: the reference model cannot "
+                                      "run it" % (fan2, fan1))
+        raise NotImplementedError("NISQA_DIM with td_2 fan_out %d (%s) != td fan_out %d (%s): the reference model cannot run it" % (
+            fan2, _fan_out_args(args, "td_2"), fan1, _fan_out_args(args, "td")))
     # ms_sr != None: the ingest converts every clip to that rate (nisqa_b200/resample.py) before the engine sees it
     cfg = NisqaConfig()
     cfg.abi_version = ABI_VERSION
@@ -272,15 +301,15 @@ def config_from_args(args, max_chunk_segments=0):
     cfg.max_segments = int(args["ms_max_segments"]) if args.get("ms_max_segments") else 0
     cfg.hop_s, cfg.win_s = float(args["ms_hop_length"]), float(args["ms_win_length"])
     cfg.fmax = float(args["ms_fmax"])
-    cfg.sa_layers = int(args["td_sa_num_layers"]) if arch == ARCH_ADAPT_SA_ATTFF else 0
+    cfg.sa_layers = 0 if td_lstm else int(args["td_sa_num_layers"])
     # NISQA_MAX_CHUNK: experiment knob (segments per internal pass) for A/B runs of the pass size
     cfg.max_chunk_segments = int(max_chunk_segments) or int(os.environ.get("NISQA_MAX_CHUNK", "0"))
     cfg.pool = pool_mode
-    cfg.pos_enc = 1 if (arch == ARCH_ADAPT_SA_ATTFF and args.get("td_sa_pos_enc")) else 0
+    cfg.pos_enc = 1 if (not td_lstm and args.get("td_sa_pos_enc")) else 0
     cfg.cnn_kind, cfg.cnn_fc = cnn_kind, cnn_fc
     cfg.sa_d_model, cfg.sa_ff = sa
-    cfg.td2_d_model, cfg.td2_ff = td2
-    if args.get("td_2") == "self_att":
+    cfg.td2_d_model, cfg.td2_ff = td2w
+    if td2 == "self_att":
         cfg.td2_layers = int(args["td_2_sa_num_layers"])
         cfg.td2_pos_enc = 1 if args.get("td_2_sa_pos_enc") else 0
     if de:
@@ -288,6 +317,14 @@ def config_from_args(args, max_chunk_segments=0):
         cfg.de_fuse_dim = int(args.get("de_fuse_dim") or 0)
         cfg.de_align, cfg.de_align_apply, cfg.de_fuse = DE_ALIGN[args["de_align"]], DE_APPLY[args["de_align_apply"]], DE_FUSE[args["de_fuse"]]
     return cfg
+
+
+def _fan_out_args(args, stage):
+    """the args that set a time-dependency stage's fan_out, for refusals"""
+    if args.get(stage) == "lstm":
+        return "%s_lstm_h=%r, %s_lstm_bidirectional=%r" % (stage, args.get(stage + "_lstm_h"), stage,
+                                                           args.get(stage + "_lstm_bidirectional"))
+    return "%s_sa_d_model=%r" % (stage, args.get(stage + "_sa_d_model"))
 
 
 def segment_counts(cfg, n_samples, sample_rate):
