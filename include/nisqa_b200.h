@@ -35,7 +35,8 @@ extern "C" {
 typedef struct nisqa_engine nisqa_engine;
 
 /* time-dependency models behind the framewise model (td, then td_2; lib:839-895).  The two shipped architectures are 0
- * and 1; 2 and 3 add an LSTM as td_2.  A self-attention td_2 is td2_layers > 0 with arch 0 or 1. */
+ * and 1; 2 and 3 add an LSTM as td_2; 4 and 5 have no td (td = 'skip').  A self-attention td_2 is td2_layers > 0 with
+ * arch 0, 1 or 4. */
 enum nisqa_arch {
   NISQA_ARCH_ADAPT_SA_ATTFF  = 0, /* nisqa.tar, nisqa_mos_only.tar: AdaptCNN + SelfAttention + PoolAttFF; in general any
                                    * framewise model (cnn_kind) + self-attention td, td_2 skip or self-attention          */
@@ -44,8 +45,13 @@ enum nisqa_arch {
                                    * nisqa_load_weights (weight_hh_l{k}[_reverse], cnn.model.fc_out.*); td_2 skip or
                                    * self-attention                                                                        */
   NISQA_ARCH_SA_LSTM         = 2, /* any framewise model (cnn_kind) + self-attention td + LSTM td_2                        */
-  NISQA_ARCH_LSTM_LSTM       = 3  /* StandardCNN + LSTM td + LSTM td_2.  A td_2 LSTM's shape is read from
+  NISQA_ARCH_LSTM_LSTM       = 3, /* StandardCNN + LSTM td + LSTM td_2.  A td_2 LSTM's shape is read from
                                    * time_dependency_2.model.lstm.weight_hh_l{k}[_reverse], like td's                      */
+  NISQA_ARCH_SKIP            = 4, /* no td: the framewise model's rows (cnn_kind) go to a self-attention td_2 when
+                                   * td2_layers > 0, or straight to the pooling module (any but PoolLastStepBi)             */
+  NISQA_ARCH_SKIP_LSTM       = 5  /* StandardCNN (cnn_kind NISQA_CNN_STANDARD), no td, then an LSTM td_2 read from
+                                   * time_dependency_2.model.lstm.*, as for arch 3.  Arch 4 and 5 keep sa_layers, sa_d_model,
+                                   * sa_ff and pos_enc at 0                                                                 */
 };
 
 /* pooling over time (reference lib:1066-1225) over the last time-dependency stage's rows.  The shipped checkpoints use
@@ -68,7 +74,8 @@ enum nisqa_de_align { NISQA_DE_ALIGN_DOT = 1, NISQA_DE_ALIGN_COSINE = 2, NISQA_D
 enum nisqa_de_apply { NISQA_DE_APPLY_HARD = 0, NISQA_DE_APPLY_SOFT = 1 };
 enum nisqa_de_fuse  { NISQA_DE_FUSE_XY_MINUS = 0 /* 'x/y/-' */, NISQA_DE_FUSE_PLUS_MINUS = 1 /* '+/-' */, NISQA_DE_FUSE_XY = 2 /* 'x/y' */ };
 
-/* framewise model in front of a self-attention td (arch 0 and 2; behind an LSTM td the CNN is always StandardCNN):
+/* framewise model in front of a self-attention td or of no td (arch 0, 2 and 4; arch 5 and behind an LSTM td the CNN is
+ * always StandardCNN):
  * CONV = AdaptCNN, STANDARD = StandardCNN (lib:811-836; its fc_out width is read from cnn.model.fc_out.*, cnn_fc stays 0) */
 enum nisqa_cnn_kind { NISQA_CNN_CONV = 0, NISQA_CNN_SKIP = 1, NISQA_CNN_DFF = 2, NISQA_CNN_STANDARD = 3 };
 
@@ -98,10 +105,13 @@ enum nisqa_stage {
   NISQA_STAGE_CNN_FEAT = 6, /* [n_seg, 384] (adapt, index c*6+h) or [n_seg, F] (standard: fc_out's width F, or 768 in
                              * index c*12+h*2+w without fc_out)                                                        */
   NISQA_STAGE_TD_IN    = 7, /* the input LayerNorm output of the first self-attention stack that runs (td's, or td_2's
-                             * behind an LSTM td): LayerNorm(Linear(in -> D)) [n_seg, D]; not available without one     */
-  NISQA_STAGE_TD_OUT   = 8, /* output of the last time-dependency stage: [n_seg, D] (a self-attention stack: td2_d_model
-                             * when td_2 runs, else sa_d_model) or [n_seg, dirs*H] (the last LSTM layer, fwd||bwd)       */
-  NISQA_STAGE_TD1_OUT  = 9  /* NISQA / NISQA_DIM with a td_2 stage: td's output rows [n_seg, td fan_out] (D or dirs*H)   */
+                             * behind an LSTM td or no td): LayerNorm(Linear(in -> D)) [n_seg, D]; not available without one */
+  NISQA_STAGE_TD_OUT   = 8, /* the rows the pooling module reads.  Output of the last time-dependency stage: [n_seg, D] (a
+                             * self-attention stack: td2_d_model when td_2 runs, else sa_d_model) or [n_seg, dirs*H] (the
+                             * last LSTM layer, fwd||bwd); arch 4 without td_2: the framewise output [n_seg, fan_out] in
+                             * the reference's column order (AdaptCNN c*6+h, StandardCNN c*12+h*2+w, or the Linear's) */
+  NISQA_STAGE_TD1_OUT  = 9  /* NISQA / NISQA_DIM with a td and a td_2 stage: td's output rows [n_seg, td fan_out] (D or
+                             * dirs*H); not available without a td (arch 4, 5)                                          */
 };
 
 /* Mirrors the checkpoint 'args' the hot path consumes (SURVEY.md Appendix A). */
@@ -129,9 +139,11 @@ typedef struct nisqa_config {
   int32_t de_align_apply;/* enum nisqa_de_apply */
   int32_t de_fuse;       /* enum nisqa_de_fuse */
   int32_t td2_layers;    /* td_2 = 'self_att' (one head, width td2_d_model, feed-forward td2_ff): number of layers; 0 = no such stack.  NISQA_DE needs >= 1;
-                          * NISQA / NISQA_DIM (arch 0 and 1) run it behind td (lib:114-141, 236-268); arch 2 and 3 keep 0 */
+                          * NISQA / NISQA_DIM (arch 0 and 1) run it behind td (lib:114-141, 236-268), arch 4 behind the
+                          * framewise model; arch 2, 3 and 5 keep 0 */
   int32_t td2_pos_enc;   /* td_2_sa_pos_enc */
-  /* framewise model in front of a self-attention td (arch NISQA_ARCH_ADAPT_SA_ATTFF / NISQA_ARCH_SA_LSTM): */
+  /* framewise model in front of a self-attention td (arch NISQA_ARCH_ADAPT_SA_ATTFF / NISQA_ARCH_SA_LSTM) or of no td
+   * (NISQA_ARCH_SKIP; NISQA_ARCH_SKIP_LSTM: NISQA_CNN_STANDARD): */
   int32_t cnn_kind;      /* enum nisqa_cnn_kind: 0 = AdaptCNN, 1 = SkipCNN (lib:504-534), 2 = DFF (lib:536-583), 3 = StandardCNN */
   int32_t cnn_fc;        /* cnn_fc_out_h: Linear behind the AdaptCNN (lib:682-684, 708-709), of SkipCNN (0 = none: 720 features),
                           * hidden width of DFF; a multiple of 64 */

@@ -216,7 +216,11 @@ struct nisqa_engine {
   int td2_f() const { return cfg.td2_ff ? cfg.td2_ff : 64; }
   // which time-dependency model each stage runs, and the CNN geometry (StandardCNN: W 8/4/2, 768 features)
   bool td_lstm() const { return cfg.arch == NISQA_ARCH_STD_LSTM_LASTBI || cfg.arch == NISQA_ARCH_LSTM_LSTM; }
-  bool td2_lstm() const { return cfg.arch == NISQA_ARCH_SA_LSTM || cfg.arch == NISQA_ARCH_LSTM_LSTM; }
+  bool td_skip() const { return cfg.arch == NISQA_ARCH_SKIP || cfg.arch == NISQA_ARCH_SKIP_LSTM; }     // no td stage
+  bool td_sa() const { return !td_lstm() && !td_skip(); }
+  bool td2_lstm() const {
+    return cfg.arch == NISQA_ARCH_SA_LSTM || cfg.arch == NISQA_ARCH_LSTM_LSTM || cfg.arch == NISQA_ARCH_SKIP_LSTM;
+  }
   bool td2_runs() const { return cfg.td2_layers > 0 || td2_lstm(); }
   bool std_cnn() const { return td_lstm() || cfg.cnn_kind == NISQA_CNN_STANDARD; }
   bool conv_net() const { return cfg.cnn_kind == NISQA_CNN_CONV || cfg.cnn_kind == NISQA_CNN_STANDARD; }
@@ -247,6 +251,7 @@ struct nisqa_engine {
   const float* last_td_out = nullptr;
   int last_td_out_d = 64;       // row width of last_td_out
   int last_td_out_ld = 0;       // its row stride (0: the width)
+  int last_td_out_hw = 0;       // td = 'skip': conv6 features in the engine's order [hw][64] (6 / 12); 0: the reference's
   const float* last_td1_out = nullptr;    // td's output when a td_2 stage ran (NISQA_STAGE_TD1_OUT)
   int last_td1_out_d = 0, last_td1_out_ld = 0;
 
@@ -712,16 +717,21 @@ bool pack_de_align(Packer& P, const nisqa_config& c) {
 int round64(int n) { return (n + 63) / 64 * 64; }
 
 // The pooling module behind the time-dependency block, one head per output (order mos, noi, dis, col, loud:
-// lib:1461-1465), reading Dp-wide rows: PoolAttFF, or PoolAtt / PoolAvg / PoolMax / PoolLastStep / PoolLastStepBi.
-// PoolAttFF's linear1: [head][Dp][128] for td_sa_kernel's fused tail (self-attention), or - behind an LSTM - k-major
-// [Dp padded to 64][head 128] for the tile GEMM (lstm_att)
-bool pack_pool_heads(Packer& P, const nisqa_config& c, int Dp, bool lstm = false) {
-  const int nh = c.n_out;
+// lib:1461-1465), reading rows of in.dim features: PoolAttFF, or PoolAtt / PoolAvg / PoolMax / PoolLastStep /
+// PoolLastStepBi.  Every vector over the features is laid out in the rows' column order (in_col: the framewise rows of
+// td = 'skip' hold conv6 features in the engine's order); a plain description packs the checkpoint's order unchanged.
+// PoolAttFF's linear1: [head][Dp][128] for td_sa_kernel's fused tail (self-attention), or - behind an LSTM or the
+// framewise model - k-major [Dp padded to 64][head 128] for the tile GEMM (lstm_att), zero in the padding rows
+bool pack_pool_heads(Packer& P, const nisqa_config& c, InRows in, bool gemm = false) {
+  const int nh = c.n_out, Dp = in.dim;
   auto prefix = [&](int h) { return nh == 1 ? std::string("pool.model.") : "pool_layers." + std::to_string(h) + ".model."; };
+  auto put_row = [&](size_t o, const TensorView* v) {          // one [1, Dp] weight in the rows' column order
+    for (int k = 0; k < Dp; ++k) P.arena[o + k] = v->d[in_col(in.order, k)];
+  };
   if (c.pool == NISQA_POOL_ATT_FF) {
     PoolHeadParams& H = P.w.pool_head;
-    const size_t oW1 = lstm ? P.alloc(P.w.lstm_att.wT, (size_t)round64(Dp) * nh * 128) : P.alloc(H.W1T, (size_t)nh * Dp * 128),
-                 ob1 = lstm ? P.alloc(P.w.lstm_att.b, nh * 128) : P.alloc(H.b1, nh * 128),
+    const size_t oW1 = gemm ? P.alloc(P.w.lstm_att.wT, (size_t)round64(Dp) * nh * 128) : P.alloc(H.W1T, (size_t)nh * Dp * 128),
+                 ob1 = gemm ? P.alloc(P.w.lstm_att.b, nh * 128) : P.alloc(H.b1, nh * 128),
                  ow2 = P.alloc(H.w2, nh * 128), ob2 = P.alloc(H.b2, nh),
                  ow3 = P.alloc(H.w3, nh * Dp), ob3 = P.alloc(H.b3, nh);
     for (int h = 0; h < nh; ++h) {
@@ -733,16 +743,18 @@ bool pack_pool_heads(Packer& P, const nisqa_config& c, int Dp, bool lstm = false
       const TensorView* w3 = P.get(p + "linear3.weight", {1, Dp});
       const TensorView* b3 = P.get(p + "linear3.bias", {1});
       if (!w1 || !b1 || !w2 || !b2 || !w3 || !b3) return false;
-      if (lstm) {
-        for (int k = 0; k < Dp; ++k)
-          for (int j = 0; j < 128; ++j) P.arena[oW1 + (size_t)k * nh * 128 + h * 128 + j] = w1->d[(size_t)j * Dp + k];
+      if (gemm) {
+        for (int k = 0; k < Dp; ++k) {
+          const int kc = in_col(in.order, k);
+          for (int j = 0; j < 128; ++j) P.arena[oW1 + (size_t)k * nh * 128 + h * 128 + j] = w1->d[(size_t)j * Dp + kc];
+        }
       } else {
-        pack_linear_T(P, oW1 + (size_t)h * Dp * 128, w1, 128, Dp);        // [head][D][128]
+        pack_linear_T(P, oW1 + (size_t)h * Dp * 128, w1, 128, Dp);        // [head][D][128] (self-attention rows: plain)
       }
       memcpy(&P.arena[ob1 + h * 128], b1->d, 512);
       memcpy(&P.arena[ow2 + h * 128], w2->d, 512);
       P.arena[ob2 + h] = b2->d[0];
-      memcpy(&P.arena[ow3 + h * Dp], w3->d, (size_t)Dp * 4);
+      put_row(ow3 + (size_t)h * Dp, w3);
       P.arena[ob3 + h] = b3->d[0];
     }
     return true;
@@ -759,8 +771,8 @@ bool pack_pool_heads(Packer& P, const nisqa_config& c, int Dp, bool lstm = false
     const TensorView* w3 = P.get(p + (att ? "linear2.weight" : "linear.weight"), {1, Dp});
     const TensorView* b3 = P.get(p + (att ? "linear2.bias" : "linear.bias"), {1});
     if ((att && (!a1 || !a1b)) || !w3 || !b3) return false;
-    if (att) { memcpy(&P.arena[oa1 + h * Dp], a1->d, (size_t)Dp * 4); P.arena[oa1b + h] = a1b->d[0]; }
-    memcpy(&P.arena[ow3 + h * Dp], w3->d, (size_t)Dp * 4);
+    if (att) { put_row(oa1 + (size_t)h * Dp, a1); P.arena[oa1b + h] = a1b->d[0]; }
+    put_row(ow3 + (size_t)h * Dp, w3);
     P.arena[ob3 + h] = b3->d[0];
   }
   return true;
@@ -887,6 +899,24 @@ bool pack_td_model(Packer& P, nisqa_engine* e) {
   }
   const Weights::LstmShape* last_lstm = nullptr;      // the last stage, when it is an LSTM
   int d1;                                             // td's fan_out
+  if (e->td_skip()) {
+    // no td (TimeDependency._skip, lib:839-895): td_2 or the pooling module reads the framewise rows themselves
+    if (W.std_fc > 0 && !pack_std_fc(P, W.std_fc)) return false;
+    if (c.td2_layers > 0) {
+      if (!pack_sa_stack(P, W.sa[1], td2, in, c.td2_layers, e->td2_d(), e->td2_f())) return false;
+      if (c.td2_pos_enc && !pack_pos_enc(P, c, td2, W.sa[1], e->td2_d())) return false;
+      return pack_pool_heads(P, c, {e->td2_d(), IN_PLAIN});
+    }
+    if (e->td2_lstm()) {
+      Weights::LstmShape& L2 = W.lstm_st[1].s;
+      if (!read_lstm_shape(P, td2 + "lstm.", "td_2_lstm_h", &L2)) return false;
+      if (!pack_lstm_stack(P, W.lstm_st[1], td2 + "lstm.", in)) return false;
+      if (c.pool == NISQA_POOL_LAST_STEP_BI && L2.dirs != 2)
+        return P.fail("missing tensor " + td2 + "lstm.weight_hh_l0_reverse: PoolLastStepBi needs a bidirectional LSTM");
+      return pack_pool_heads(P, c, {L2.dirs * L2.H, IN_PLAIN}, true);
+    }
+    return pack_pool_heads(P, c, in, true);
+  }
   if (e->td_lstm()) {
     Weights::LstmShape& L = W.lstm_st[0].s;
     if (!read_lstm_shape(P, td + "lstm.", "td_lstm_h", &L)) return false;
@@ -931,7 +961,7 @@ bool pack_td_model(Packer& P, nisqa_engine* e) {
   if (!e->td_lstm() && c.pos_enc && !pack_pos_enc(P, c, td, W.sa[0], e->sa_d())) return false;
   if (c.pool == NISQA_POOL_LAST_STEP_BI && (!last_lstm || last_lstm->dirs != 2))
     return P.fail("missing tensor " + (e->td2_lstm() ? td2 : td) + "lstm.weight_hh_l0_reverse: PoolLastStepBi needs a bidirectional LSTM");
-  return pack_pool_heads(P, c, dp, last_lstm != nullptr);
+  return pack_pool_heads(P, c, {dp, IN_PLAIN}, last_lstm != nullptr);
 }
 
 int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
@@ -1313,9 +1343,34 @@ int pool_rows(Pass& p, const float* x, int D, int ld, bool after_lstm) {
   return 0;
 }
 
-// The time-dependency model - td, then td_2 when it runs (NISQA_DE: alignment, fusion and a stack) - and the pooling module
-// over the last stage's rows.  A self-attention stage is sa_stack (the PoolAttFF logits fused into its last layer when it
-// feeds the pooling module), an LSTM stage is lstm_stage.  td works in tdout / xa / xb, td_2 in td2in / td2out / ya / yb:
+// The pooling module over the framewise rows of a checkpoint without td and td_2 (x: D real features at a stride of ld):
+// launch_pool_wide, the PoolAttFF logits from the tile GEMM + att_logits as behind an LSTM
+int pool_framewise(Pass& p, const float* x, int D, int ld) {
+  nisqa_engine* e = p.e;
+  const nisqa_config& c = p.c;
+  Lane& LN = p.LN;
+  const Weights& w = p.w;
+  const int n_seg = p.n_seg, nh = c.n_out;
+  const bool attff = c.pool == NISQA_POOL_ATT_FF, att = c.pool == NISQA_POOL_ATT;
+  Scope s(e, "pool", attff ? 4 : att ? 3 : 2);
+  if (attff || att) CK(LN.logits.reserve((size_t)n_seg * nh * 4));
+  CK(LN.partial.reserve((size_t)p.n * pool_wide_slabs(D) * nh * 4));
+  PoolSimpleParams P = w.pool_simple;
+  if (attff) {
+    CK(LN.atth.reserve((size_t)n_seg * nh * 128 * 4));
+    launch_linear_tile(p.st, x, ld, w.lstm_att.wT, w.lstm_att.b, 1, LN.atth.as<float>(), nh * 128, n_seg, ld, nh * 128);
+    launch_att_logits(p.st, LN.atth.as<float>(), w.pool_head.w2, w.pool_head.b2, nh, n_seg, LN.logits.as<float>());
+    P.w3 = w.pool_head.w3;
+    P.b3 = w.pool_head.b3;
+  }
+  launch_pool_wide(p.st, x, D, ld, c.pool, P, nh, LN.logits.as<float>(), n_seg, p.clips, p.n, LN.partial.as<float>(), p.scores);
+  return 0;
+}
+
+// The time-dependency model - td (none for td = 'skip'), then td_2 when it runs (NISQA_DE: alignment, fusion and a
+// stack) - and the pooling module over the last stage's rows, or over the framewise rows when neither runs.  A
+// self-attention stage is sa_stack (the PoolAttFF logits fused into its last layer when it feeds the pooling module),
+// an LSTM stage is lstm_stage.  td works in tdout / xa / xb, td_2 in td2in / td2out / ya / yb:
 // td's output stays readable after td_2 (NISQA_STAGE_TD1_OUT).
 int td_stages(Pass& p, Rows rows) {
   nisqa_engine* e = p.e;
@@ -1323,11 +1378,11 @@ int td_stages(Pass& p, Rows rows) {
   Lane& LN = p.LN;
   const Weights& w = p.w;
   const int n_seg = p.n_seg;
-  const bool de = c.double_ended != 0, sa1 = !e->td_lstm(), sa2 = c.td2_layers > 0, lstm2 = e->td2_lstm();
-  const Weights::LstmShape &L1 = w.lstm_st[0].s, &L2 = w.lstm_st[1].s;
+  const bool de = c.double_ended != 0, skip = e->td_skip(), sa1 = e->td_sa(), sa2 = c.td2_layers > 0, lstm2 = e->td2_lstm();
+  const Weights::LstmShape &L1 = w.lstm_st[0].s, &L2 = w.lstm_st[1].s;      // (L1: all zero without an LSTM td)
   auto res = [&](DevBuf& b, size_t floats) { return b.reserve(floats * 4); };
-  // workspaces of both stages, reserved before the first launch
-  const size_t D1 = sa1 ? e->sa_d() : round64(L1.dirs * L1.H), D2 = sa2 ? e->td2_d() : lstm2 ? round64(L2.dirs * L2.H) : 0;
+  // workspaces of the stages that run, reserved before the first launch
+  const size_t D1 = skip ? 0 : sa1 ? e->sa_d() : round64(L1.dirs * L1.H), D2 = sa2 ? e->td2_d() : lstm2 ? round64(L2.dirs * L2.H) : 0;
   size_t qkv = 0, gx = 0;
   if (sa1) qkv = 3 * D1; else gx = (size_t)L1.dirs * 4 * L1.H;
   if (sa2) qkv = std::max(qkv, 3 * D2);
@@ -1340,22 +1395,27 @@ int td_stages(Pass& p, Rows rows) {
     CK(res(LN.logits, (size_t)n_seg * c.n_out));
   }
   if (gx) CK(res(LN.gx, n_seg * gx));
-  CK(res(LN.tdout, n_seg * D1));
+  if (D1) CK(res(LN.tdout, n_seg * D1));
   if (sa2) CK(res(LN.td2in, n_seg * D2));
   if (lstm2) CK(res(LN.td2out, n_seg * D2));
 
   Rows cur;
+  int D;                                              // width of cur's rows
   e->last_td_in = nullptr;
-  if (sa1) {
+  if (skip) {
+    cur = rows;
+    D = p.std_mode ? (w.std_fc ? w.std_fc : 768) : c.cnn_fc ? c.cnn_fc : c.cnn_kind == NISQA_CNN_CONV ? 384 : 720;
+  } else if (sa1) {
     e->last_td_in = LN.tdout.as<float>();
     cur = {sa_stack(p, 0, rows, !e->td2_runs(), LN.tdout.as<float>()), e->sa_d() / 64};
+    D = e->sa_d();
   } else {
     const int rc = lstm_stage(p, 0, rows, LN.tdout.as<float>(), &cur);
     if (rc) return rc;
+    D = L1.dirs * L1.H;
   }
-  int D = sa1 ? e->sa_d() : L1.dirs * L1.H;           // width of cur's rows
   e->last_td1_out = nullptr;
-  if (e->td2_runs() && !de) { e->last_td1_out = cur.x; e->last_td1_out_d = D; e->last_td1_out_ld = 64 * cur.nk; }
+  if (e->td2_runs() && !de && !skip) { e->last_td1_out = cur.x; e->last_td1_out_d = D; e->last_td1_out_ld = 64 * cur.nk; }
   if (de) {
     Rows fused;
     const int rc = de_fuse(p, cur.x, &fused);
@@ -1374,6 +1434,11 @@ int td_stages(Pass& p, Rows rows) {
   e->last_td_out = cur.x;
   e->last_td_out_d = D;
   e->last_td_out_ld = 64 * cur.nk;
+  e->last_td_out_hw = 0;
+  if (skip && !e->td2_runs()) {
+    if (cur.x == LN.feats.as<float>()) e->last_td_out_hw = p.std_mode ? 12 : 6;      // conv6 features, engine order
+    return pool_framewise(p, cur.x, D, 64 * cur.nk);
+  }
   return pool_rows(p, cur.x, D, 64 * cur.nk, lstm2 || (!sa1 && !sa2));
 }
 
@@ -1555,10 +1620,16 @@ int nisqa_create(nisqa_engine** out, int device, const nisqa_config* cfg) {
   memset(&e->cfg, 0, sizeof e->cfg);
   memcpy(&e->cfg, cfg, cfg->abi_version == 3 ? offsetof(nisqa_config, sa_d_model) : sizeof(nisqa_config));
   cfg = &e->cfg;
-  if (cfg->arch < NISQA_ARCH_ADAPT_SA_ATTFF || cfg->arch > NISQA_ARCH_LSTM_LSTM)
+  if (cfg->arch < NISQA_ARCH_ADAPT_SA_ATTFF || cfg->arch > NISQA_ARCH_SKIP_LSTM)
     return fail(e, NISQA_ERR_INVALID, "unsupported architecture");
-  const bool sa_td = !e->td_lstm();          // a self-attention td: arch 0 and 2
-  const bool last_sa = sa_td ? !e->td2_lstm() : cfg->td2_layers > 0;      // the pooling module reads self-attention rows
+  const bool sa_td = e->td_sa();             // a self-attention td: arch 0 and 2
+  // the pooling module reads the rows of an LSTM (PoolLastStepBi needs it)
+  const bool last_lstm = e->td2_lstm() || (e->td_lstm() && cfg->td2_layers == 0);
+  const bool any_cnn = sa_td || cfg->arch == NISQA_ARCH_SKIP;       // every framewise model (cnn_kind, cnn_fc) may feed td
+  if (e->td_skip() && (cfg->sa_layers != 0 || cfg->sa_d_model != 0 || cfg->sa_ff != 0 || cfg->pos_enc != 0))
+    return fail(e, NISQA_ERR_INVALID, "sa_layers / sa_d_model / sa_ff / pos_enc: arch 4 and 5 have no td (keep them 0)");
+  if (cfg->arch == NISQA_ARCH_SKIP_LSTM && cfg->cnn_kind != NISQA_CNN_STANDARD)
+    return fail(e, NISQA_ERR_INVALID, "cnn_kind: arch 5 (an LSTM td_2 behind no td) needs StandardCNN");
   if (cfg->n_fft != kNfft || cfg->n_mels != kMels || cfg->seg_len != kSegLen)
     return fail(e, NISQA_ERR_INVALID, "engine is built for n_fft=4096, n_mels=48, seg_length=15");
   if (cfg->n_out != 1 && cfg->n_out != 5) return fail(e, NISQA_ERR_INVALID, "n_out must be 1 or 5");
@@ -1566,17 +1637,17 @@ int nisqa_create(nisqa_engine** out, int device, const nisqa_config* cfg) {
     return fail(e, NISQA_ERR_INVALID, "bad front-end parameters");
   if (sa_td && (cfg->sa_layers < 1 || cfg->sa_layers > 8))
     return fail(e, NISQA_ERR_INVALID, "sa_layers");
-  if (cfg->pool < NISQA_POOL_ATT_FF || cfg->pool > NISQA_POOL_LAST_STEP_BI || (last_sa && cfg->pool == NISQA_POOL_LAST_STEP_BI))
+  if (cfg->pool < NISQA_POOL_ATT_FF || cfg->pool > NISQA_POOL_LAST_STEP_BI || (!last_lstm && cfg->pool == NISQA_POOL_LAST_STEP_BI))
     return fail(e, NISQA_ERR_INVALID, "pooling module not available for this architecture (PoolLastStepBi needs an LSTM as the last stage)");
   if (cfg->pos_enc && !sa_td) return fail(e, NISQA_ERR_INVALID, "pos_enc needs a self-attention td");
   if (cfg->cnn_kind < NISQA_CNN_CONV || cfg->cnn_kind > NISQA_CNN_STANDARD || cfg->cnn_fc < 0 || cfg->cnn_fc % 64 != 0 || cfg->cnn_fc > 8192 ||
-      (cfg->cnn_kind == NISQA_CNN_DFF && cfg->cnn_fc == 0) || (cfg->cnn_fc != 0 && (!sa_td || cfg->cnn_kind == NISQA_CNN_STANDARD)) ||
-      (cfg->cnn_kind != NISQA_CNN_CONV && !sa_td) ||
+      (cfg->cnn_kind == NISQA_CNN_DFF && cfg->cnn_fc == 0) || (cfg->cnn_fc != 0 && (!any_cnn || cfg->cnn_kind == NISQA_CNN_STANDARD)) ||
+      (cfg->cnn_kind != NISQA_CNN_CONV && !any_cnn && cfg->arch != NISQA_ARCH_SKIP_LSTM) ||
       cfg->de_fuse_dim < 0 || cfg->de_fuse_dim % 64 != 0 || cfg->de_fuse_dim > 8192 || (cfg->de_fuse_dim != 0 && !cfg->double_ended))
-    return fail(e, NISQA_ERR_INVALID, "cnn_kind / cnn_fc: SkipCNN, DFF and StandardCNN (cnn_kind) feed a self-attention td; cnn_fc_out_h a "
+    return fail(e, NISQA_ERR_INVALID, "cnn_kind / cnn_fc: SkipCNN, DFF and StandardCNN (cnn_kind) feed a self-attention td or no td; cnn_fc_out_h a "
                                       "multiple of 64 (StandardCNN's fc_out comes from the weights)");
   if (cfg->td2_layers < 0 || cfg->td2_layers > 8 || (cfg->td2_layers > 0 && e->td2_lstm()))
-    return fail(e, NISQA_ERR_INVALID, "td_2 = 'self_att' needs arch 0 or 1 (td2_layers 0..8)");
+    return fail(e, NISQA_ERR_INVALID, "td_2 = 'self_att' needs arch 0, 1 or 4 (td2_layers 0..8)");
   {
     const int32_t w[4] = {cfg->sa_d_model, cfg->sa_ff, cfg->td2_d_model, cfg->td2_ff};
     const char* nm[4] = {"sa_d_model", "sa_ff", "td2_d_model", "td2_ff"};
@@ -1831,13 +1902,15 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
       break;
     case NISQA_STAGE_TD_IN:
       if (!e->last_td_in) return fail(e, NISQA_ERR_INVALID, "stage not available for this architecture");
-      src = e->last_td_in; count = ns * (e->td_lstm() ? e->td2_d() : e->sa_d()); break;
+      src = e->last_td_in; count = ns * (e->td_sa() ? e->sa_d() : e->td2_d()); break;
     case NISQA_STAGE_TD1_OUT:
       if (!e->last_td1_out) return fail(e, NISQA_ERR_INVALID, "stage not available: no td_2 stage ran");
       src = e->last_td1_out; count = ns * e->last_td1_out_d; width = e->last_td1_out_d; ld = e->last_td1_out_ld; break;
     case NISQA_STAGE_TD_OUT:
       if (!e->last_td_out) return fail(e, NISQA_ERR_STATE, "the per-step BiLSTM outputs were not kept: nisqa_set_option(\"keep_td_out\", 1) before the predict call");
-      src = e->last_td_out; count = ns * e->last_td_out_d; width = e->last_td_out_d; ld = e->last_td_out_ld; break;
+      src = e->last_td_out; count = ns * e->last_td_out_d; width = e->last_td_out_d; ld = e->last_td_out_ld;
+      if (e->last_td_out_hw) { hw = e->last_td_out_hw; ch = 64; }       // conv6 features: [hw][c] -> c*hw + hw index
+      break;
     default: return fail(e, NISQA_ERR_INVALID, "unknown stage");
   }
   if (ch > 0) count = ns * hw * ch;

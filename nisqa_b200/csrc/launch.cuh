@@ -115,6 +115,14 @@ void launch_pool_final(cudaStream_t st, const float* x, int D, int ldx, const fl
                        const PoolHeadParams& P, int n_heads, int max_seg, float* scores);
 void launch_pool_simple(cudaStream_t st, const float* x, int D, int ldx, const ClipDesc* clips, int n_clips, int mode,
                         const PoolSimpleParams& P, int n_heads, int max_seg, float* scores);
+// Pooling over wide rows (td = 'skip': the framewise rows, D real columns at a stride of ldx, a multiple of 64), one CTA
+// per (clip, column slab of kPoolWideSlab).  mode: enum nisqa_pool except PoolLastStepBi; P.w3 / P.b3: each head's score
+// Linear [n_heads][D] (columns in the rows' order); logits [n_seg][n_heads]: PoolAttFF's, computed by the caller, or -
+// PoolAtt - written here from P.a1 [n_heads][D] / P.a1b.  partial: [n_clips][pool_wide_slabs(D)][n_heads] floats.
+constexpr int kPoolWideSlab = 128;
+constexpr int pool_wide_slabs(int D) { return (D + kPoolWideSlab - 1) / kPoolWideSlab; }
+void launch_pool_wide(cudaStream_t st, const float* x, int D, int ldx, int mode, const PoolSimpleParams& P, int n_heads,
+                      float* logits, int n_seg, const ClipDesc* clips, int n_clips, float* partial, float* scores);
 
 // ---------------------------------------------------------------- td_tiled.cu (self-attention, NISQA_DE, SkipCNN / DFF)
 void launch_td_in(cudaStream_t st, int nc, const float* feats, const float* WT, int nk, const float* b, const float* g,

@@ -629,6 +629,178 @@ __global__ void att_logits_kernel(const float* __restrict__ hid, const float* __
   if (lane == 0) logits[wid] = a + __ldg(b2 + h);
 }
 
+// ---------------------------------------------------------------------------------------
+// Pooling over wide rows: the framewise rows of a checkpoint without a time-dependency model (td = 'skip'), D real
+// columns (up to 4096) at a row stride of ldx floats, every pooling module but PoolLastStepBi, 1 or 5 heads.
+// grid = (column slab of kPoolWideSlab, clip), kPoolWarps warps: lane l of warp g owns the slab's columns 4l..4l+3 over
+// the clip's steps t = g, g + kPoolWarps, .., one accumulator per head and column updated in step order, so x is read
+// from HBM once for every head.  PoolAtt / PoolAttFF: the softmax numerators exp(logit - max) of the precomputed logits
+// [n_seg][NH] are staged kPoolChunk steps at a time; every slab CTA forms the clip's max and sum in the same fixed order.
+// The warps' sums are added in warp order, dotted with each head's Linear over the slab's columns and written to
+// partial[clip][slab][head]; pool_wide_finish_kernel adds the slabs in slab order plus the bias.  Every sum's order
+// depends only on D and the clip's own steps (not on the batch or the pass split); columns >= D are never read.
+constexpr int kPoolWarps = 4, kPoolChunk = 256;
+enum { PW_ATT = 0, PW_AVG = 1, PW_MAX = 2, PW_LAST = 3 };
+static_assert(kPoolWideSlab == 128, "one float4 of columns per lane");
+
+__device__ __forceinline__ float4 ld_cols(const float* __restrict__ p, int nv) {      // the first nv (<= 4) of 4 columns
+  if (nv >= 4) return __ldg(reinterpret_cast<const float4*>(p));
+  float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (nv > 0) v.x = __ldg(p);
+  if (nv > 1) v.y = __ldg(p + 1);
+  if (nv > 2) v.z = __ldg(p + 2);
+  return v;
+}
+
+template <int NH, int MODE>
+__global__ void __launch_bounds__(kPoolWarps * 32)
+pool_wide_kernel(const float* __restrict__ x, int D, int ldx, const float* __restrict__ logits,
+                 const ClipDesc* __restrict__ clips, const float* __restrict__ w3, float* __restrict__ partial) {
+  constexpr int NA = MODE == PW_ATT ? NH : 1;           // accumulators per column
+  __shared__ float pn[MODE == PW_ATT ? NH * kPoolChunk : 1];
+  __shared__ float red[kPoolWarps][NA][kPoolWideSlab];
+  __shared__ float wred[kPoolWarps][NH];
+  __shared__ float mx[NH], sum[NH];
+  const ClipDesc cd = clips[blockIdx.y];
+  const int S = cd.n_seg;
+  if (S <= 0) return;                                   // (pool_wide_finish_kernel writes NaN)
+  const int tid = threadIdx.x, lane = tid & 31, g = tid >> 5, c0 = blockIdx.x * kPoolWideSlab;
+  const float* lg = logits + (size_t)cd.seg_off * NH;
+  if constexpr (MODE == PW_ATT) {
+    for (int h = 0; h < NH; ++h) {
+      float m = -INFINITY;
+      for (int t = tid; t < S; t += kPoolWarps * 32) m = fmaxf(m, __ldg(lg + (size_t)t * NH + h));
+      m = warp_max(m);
+      if (lane == 0) wred[g][h] = m;
+    }
+    __syncthreads();
+    if (tid < NH) {
+      float m = wred[0][tid];
+      for (int w = 1; w < kPoolWarps; ++w) m = fmaxf(m, wred[w][tid]);
+      mx[tid] = m;
+    }
+    __syncthreads();
+    for (int h = 0; h < NH; ++h) {
+      float s = 0.f;
+      for (int t = tid; t < S; t += kPoolWarps * 32) s += expf(__ldg(lg + (size_t)t * NH + h) - mx[h]);
+      s = warp_sum(s);
+      if (lane == 0) wred[g][h] = s;
+    }
+    __syncthreads();
+    if (tid < NH) {
+      float s = wred[0][tid];
+      for (int w = 1; w < kPoolWarps; ++w) s += wred[w][tid];
+      sum[tid] = s;
+    }
+  }
+  if constexpr (MODE != PW_LAST) {
+    const int nv = D - (c0 + 4 * lane);
+    const float* xb = x + (size_t)cd.seg_off * ldx + c0 + 4 * lane;
+    float acc[NA][4];
+#pragma unroll
+    for (int a = 0; a < NA; ++a)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) acc[a][i] = MODE == PW_MAX ? -INFINITY : 0.f;
+    auto step = [&](const float4 v, int tc) {           // tc: the step's index in the chunk
+      const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int a = 0; a < NA; ++a) {
+        const float p = MODE == PW_ATT ? pn[a * kPoolChunk + tc] : 0.f;
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          acc[a][i] = MODE == PW_ATT ? fmaf(p, e[i], acc[a][i]) : MODE == PW_MAX ? fmaxf(acc[a][i], e[i]) : acc[a][i] + e[i];
+      }
+    };
+    for (int t0 = 0; t0 < S; t0 += kPoolChunk) {
+      const int n = min(kPoolChunk, S - t0);
+      if constexpr (MODE == PW_ATT) {
+        __syncthreads();                                // (the previous chunk's numerators consumed; mx published)
+        for (int i = tid; i < n * NH; i += kPoolWarps * 32) {
+          const int t = i / NH, h = i - t * NH;
+          pn[h * kPoolChunk + t] = expf(__ldg(lg + (size_t)(t0 + t) * NH + h) - mx[h]);
+        }
+        __syncthreads();
+      }
+      if (nv > 0) {
+        int t = g;
+        for (; t + 7 * kPoolWarps < n; t += 8 * kPoolWarps) {      // eight steps in flight
+          float4 v[8];
+#pragma unroll
+          for (int u = 0; u < 8; ++u) v[u] = ld_cols(xb + (size_t)(t0 + t + u * kPoolWarps) * ldx, nv);
+#pragma unroll
+          for (int u = 0; u < 8; ++u) step(v[u], t + u * kPoolWarps);
+        }
+        for (; t < n; t += kPoolWarps) step(ld_cols(xb + (size_t)(t0 + t) * ldx, nv), t);
+      }
+    }
+#pragma unroll
+    for (int a = 0; a < NA; ++a)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) red[g][a][4 * lane + i] = acc[a][i];
+  }
+  __syncthreads();
+  // thread tid: column c0 + tid of the slab, the warps' sums in warp order, then each head's Linear
+  const int c = c0 + tid;
+  float last = 0.f;
+  if constexpr (MODE == PW_LAST) last = c < D ? __ldg(x + ((size_t)cd.seg_off + S - 1) * ldx + c) : 0.f;
+#pragma unroll
+  for (int h = 0; h < NH; ++h) {
+    float pooled;
+    if constexpr (MODE == PW_LAST) {
+      pooled = last;
+    } else {
+      const int a = MODE == PW_ATT ? h : 0;
+      pooled = red[0][a][tid];
+      for (int w = 1; w < kPoolWarps; ++w) pooled = MODE == PW_MAX ? fmaxf(pooled, red[w][a][tid]) : pooled + red[w][a][tid];
+      if (MODE == PW_ATT) pooled = pooled / sum[h];
+      if (MODE == PW_AVG) pooled = pooled / (float)S;
+    }
+    const float v = warp_sum(c < D ? pooled * __ldg(w3 + (size_t)h * D + c) : 0.f);
+    if (lane == 0) wred[g][h] = v;
+  }
+  __syncthreads();
+  if (tid < NH) {
+    float s = wred[0][tid];
+    for (int w = 1; w < kPoolWarps; ++w) s += wred[w][tid];
+    partial[((size_t)blockIdx.y * gridDim.x + blockIdx.x) * NH + tid] = s;
+  }
+}
+
+// scores[clip][h] = sum over the slabs in slab order + b3[h]; NaN for a clip without segments
+__global__ void pool_wide_finish_kernel(const float* __restrict__ partial, int n_slabs, const ClipDesc* __restrict__ clips,
+                                        int n_clips, int n_heads, const float* __restrict__ b3, float* __restrict__ scores) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_clips * n_heads) return;
+  const int clip = i / n_heads, h = i - clip * n_heads;
+  if (clips[clip].n_seg <= 0) { scores[i] = __int_as_float(0x7fc00000); return; }
+  float s = 0.f;
+  for (int k = 0; k < n_slabs; ++k) s += partial[((size_t)clip * n_slabs + k) * n_heads + h];
+  scores[i] = s + __ldg(b3 + h);
+}
+
+// PoolAtt's logits over wide rows, one warp per row: logits[row][h] = a1_h . x[row][0..D) + a1b_h (lanes over the columns)
+template <int NH>
+__global__ void pool_att_logits_kernel(const float* __restrict__ x, int D, int ldx, const float* __restrict__ a1,
+                                       const float* __restrict__ a1b, int n_rows, float* __restrict__ logits) {
+  const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (row >= n_rows) return;
+  const float* xr = x + (size_t)row * ldx;
+  float a[NH];
+#pragma unroll
+  for (int h = 0; h < NH; ++h) a[h] = 0.f;
+  for (int k = lane; k < D; k += 32) {
+    const float v = __ldg(xr + k);
+#pragma unroll
+    for (int h = 0; h < NH; ++h) a[h] = fmaf(v, __ldg(a1 + (size_t)h * D + k), a[h]);
+  }
+#pragma unroll
+  for (int h = 0; h < NH; ++h) {
+    const float s = warp_sum(a[h]);
+    if (lane == 0) logits[row * NH + h] = s + __ldg(a1b + h);
+  }
+}
+
 // ------------------------------------------------------------------ host launchers
 constexpr int kRowSmem20 = (kRows * kXS + 64 * 20) * 4;
 
@@ -741,6 +913,26 @@ void launch_att_logits(cudaStream_t st, const float* hid, const float* w2, const
                        float* logits) {
   const long long warps = (long long)n_rows * n_heads;
   if (warps > 0) att_logits_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(hid, w2, b2, n_heads, n_rows, logits);
+}
+
+template <int NH>
+void pool_wide_instance(cudaStream_t st, const float* x, int D, int ldx, int mode, const PoolSimpleParams& P, float* logits,
+                        int n_seg, const ClipDesc* clips, int n_clips, float* partial, float* scores) {
+  const int slabs = pool_wide_slabs(D);
+  if (mode == 1 && n_seg > 0)
+    pool_att_logits_kernel<NH><<<(unsigned)(((long long)n_seg + 7) / 8), 256, 0, st>>>(x, D, ldx, P.a1, P.a1b, n_seg, logits);
+  const dim3 grid(slabs, n_clips), block(kPoolWarps * 32);
+  if (mode <= 1) pool_wide_kernel<NH, PW_ATT><<<grid, block, 0, st>>>(x, D, ldx, logits, clips, P.w3, partial);
+  else if (mode == 2) pool_wide_kernel<NH, PW_AVG><<<grid, block, 0, st>>>(x, D, ldx, logits, clips, P.w3, partial);
+  else if (mode == 3) pool_wide_kernel<NH, PW_MAX><<<grid, block, 0, st>>>(x, D, ldx, logits, clips, P.w3, partial);
+  else pool_wide_kernel<NH, PW_LAST><<<grid, block, 0, st>>>(x, D, ldx, logits, clips, P.w3, partial);
+  pool_wide_finish_kernel<<<(n_clips * NH + 127) / 128, 128, 0, st>>>(partial, slabs, clips, n_clips, NH, P.b3, scores);
+}
+void launch_pool_wide(cudaStream_t st, const float* x, int D, int ldx, int mode, const PoolSimpleParams& P, int n_heads,
+                      float* logits, int n_seg, const ClipDesc* clips, int n_clips, float* partial, float* scores) {
+  if (n_clips <= 0) return;
+  if (n_heads == 5) pool_wide_instance<5>(st, x, D, ldx, mode, P, logits, n_seg, clips, n_clips, partial, scores);
+  else pool_wide_instance<1>(st, x, D, ldx, mode, P, logits, n_seg, clips, n_clips, partial, scores);
 }
 
 }  // namespace nisqa

@@ -15,8 +15,9 @@ LIB_PATH = os.path.join(_HERE, "libnisqa_b200.so")
 
 ABI_VERSION = 4
 MAX_IN_FLIGHT = 6          # staging slots of the engine (nisqa_submit_pcm)
-# enum nisqa_arch: td self-attention (0) or LSTM (1) with td_2 skip or self-attention; td_2 LSTM behind either (2, 3)
-ARCH_ADAPT_SA_ATTFF, ARCH_STD_LSTM_LASTBI, ARCH_SA_LSTM, ARCH_LSTM_LSTM = 0, 1, 2, 3
+# enum nisqa_arch: td self-attention (0) or LSTM (1) with td_2 skip or self-attention; td_2 LSTM behind either (2, 3);
+# no td (td='skip') with td_2 skip or self-attention (4), or StandardCNN with an LSTM td_2 (5)
+ARCH_ADAPT_SA_ATTFF, ARCH_STD_LSTM_LASTBI, ARCH_SA_LSTM, ARCH_LSTM_LSTM, ARCH_SKIP, ARCH_SKIP_LSTM = 0, 1, 2, 3, 4, 5
 FMT_S16, FMT_F32 = 0, 1
 CLIP_OK, CLIP_TOO_SHORT, CLIP_TOO_LONG = 0, 1, 2
 POOL_ATT_FF, POOL_ATT, POOL_AVG, POOL_MAX, POOL_LAST_STEP, POOL_LAST_STEP_BI = range(6)
@@ -98,6 +99,24 @@ def _check_standard_cnn(args):
     ks = args.get("cnn_kernel_size")
     if not (ks == 3 or (isinstance(ks, (list, tuple)) and tuple(ks) == (3, 3))):
         raise NotImplementedError("cnn_kernel_size=%r: the engine runs 3x3 convolutions" % (ks,))
+
+
+def _framewise(args):
+    """(cnn_kind, cnn_fc, ok) of the framewise model in front of a self-attention td or of no td; refuses the
+    hyper-parameters the kernels do not implement, naming the value (ok: AdaptCNN's pools are the shipped ones)."""
+    cnn = args.get("cnn_model")
+    if cnn == "standard":
+        _check_standard_cnn(args)
+        return CNN_STANDARD, 0, True
+    cnn_kind = CNN_CONV if cnn == "adapt" else CNN_DFF if cnn == "dff" else CNN_SKIP
+    cnn_fc = int(args.get("cnn_fc_out_h") or 0)         # AdaptCNN's optional Linear behind conv6 (lib:682-684), SkipCNN's
+    if cnn_kind == CNN_DFF and cnn_fc == 0:
+        cnn_fc = 4096                                   # DFF's default hidden width (lib:544)
+    if cnn_fc % 64 != 0:
+        raise NotImplementedError("cnn_fc_out_h=%d: the engine needs a multiple of 64" % cnn_fc)
+    ok = cnn != "adapt" or (list(args["cnn_pool_1"]) == [24, 7] and list(args["cnn_pool_2"]) == [12, 5]
+                            and list(args["cnn_pool_3"]) == [6, 3])
+    return cnn_kind, cnn_fc, ok
 
 
 class NisqaTensor(C.Structure):
@@ -216,41 +235,39 @@ def config_from_args(args, max_chunk_segments=0):
     if de and td2 != "self_att":
         # (NISQA_DE fuses two self-attention outputs into a self-attention td_2, lib:404-424)
         raise NotImplementedError("NISQA_DE with td_2=%r: the engine runs NISQA_DE with td_2='self_att'" % (args.get("td_2"),))
-    if cnn == "adapt" and td == "self_att":
+    if cnn in ("adapt", None, "skip", "dff") and td == "self_att":
+        # AdaptCNN, or a framewise model without convolutions (lib:504-583), in front of the self-attention stack
         arch = ARCH_ADAPT_SA_ATTFF
-        ok = (list(args["cnn_pool_1"]) == [24, 7] and list(args["cnn_pool_2"]) == [12, 5]
-              and list(args["cnn_pool_3"]) == [6, 3])
-        cnn_fc = int(args.get("cnn_fc_out_h") or 0)           # optional Linear behind conv6 (lib:682-684)
-        if cnn_fc % 64 != 0:
-            raise NotImplementedError("cnn_fc_out_h=%d: the engine needs a multiple of 64" % cnn_fc)
-    elif cnn in (None, "skip", "dff") and td == "self_att":
-        # framewise models without convolutions (lib:504-583) in front of the self-attention stack
-        arch = ARCH_ADAPT_SA_ATTFF
-        cnn_kind = CNN_DFF if cnn == "dff" else CNN_SKIP
-        cnn_fc = int(args.get("cnn_fc_out_h") or 0)
-        if cnn_kind == CNN_DFF and cnn_fc == 0:
-            cnn_fc = 4096                                   # DFF's default hidden width (lib:544)
-        if cnn_fc % 64 != 0:
-            raise NotImplementedError("cnn_fc_out_h=%d: the engine needs a multiple of 64" % cnn_fc)
-        ok = True
+        cnn_kind, cnn_fc, ok = _framewise(args)
     elif (cnn, td) == ("standard", "self_att") and not de:
         # StandardCNN (lib:811-836) in front of the self-attention stack; fc_out's width comes from the weights
-        arch, cnn_kind = ARCH_ADAPT_SA_ATTFF, CNN_STANDARD
-        _check_standard_cnn(args)
-        ok = True
+        arch = ARCH_ADAPT_SA_ATTFF
+        cnn_kind, cnn_fc, ok = _framewise(args)
     elif (cnn, td) == ("standard", "lstm"):
         # any LSTM width, depth and direction behind StandardCNN (lib:811-836, 925-943), every pooling module
         arch = ARCH_STD_LSTM_LASTBI
         _check_standard_cnn(args)
         ok = True
+    elif cnn in ("adapt", None, "skip", "dff", "standard") and td in (None, "skip"):
+        # no time-dependency model (TimeDependency._skip, lib:839-895): td_2, or the pooling module, reads the framewise rows
+        if de:
+            raise NotImplementedError("NISQA_DE with td=%r: the engine runs NISQA_DE with td='self_att'" % (td,))
+        if td2 == "lstm" and cnn != "standard":
+            raise NotImplementedError("td_2='lstm' behind td=%r and cnn_model=%r: the engine runs an LSTM td_2 behind no td "
+                                      "for cnn_model='standard' only" % (td, cnn))
+        arch = ARCH_SKIP
+        cnn_kind, cnn_fc, ok = _framewise(args)
     else:
         raise NotImplementedError(
             "architecture cnn=%r td=%r pool=%r is not implemented by the engine" % (cnn, td, pool))
     if td2 == "lstm":
-        arch = ARCH_LSTM_LSTM if arch == ARCH_STD_LSTM_LASTBI else ARCH_SA_LSTM
+        arch = {ARCH_STD_LSTM_LASTBI: ARCH_LSTM_LSTM, ARCH_SKIP: ARCH_SKIP_LSTM}.get(arch, ARCH_SA_LSTM)
     # fan_out of each stage (lib:839-895): the pooling module reads the last one's rows
     td_lstm = arch in (ARCH_STD_LSTM_LASTBI, ARCH_LSTM_LSTM)
+    skip = arch in (ARCH_SKIP, ARCH_SKIP_LSTM)
     fan1 = _check_lstm(args, "td_lstm") if td_lstm else None
+    if skip:
+        fan1 = int(args.get("cnn_fc_out_h") or 768) if cnn == "standard" else (cnn_fc or (384 if cnn == "adapt" else 720))
     fan2 = _check_lstm(args, "td_2_lstm") if td2 == "lstm" else None
     if pool_mode == POOL_LAST_STEP_BI:
         key = "td_2_lstm" if td2 == "lstm" else "td_lstm" if td2 == "skip" and td_lstm else None
@@ -278,7 +295,7 @@ def config_from_args(args, max_chunk_segments=0):
     if not ok:
         raise NotImplementedError("checkpoint hyper-parameters outside the shipped NISQA configurations")
     sa = td2w = (0, 0)
-    if not td_lstm:
+    if not td_lstm and not skip:
         sa = _sa_widths(args, "td_sa", de)
         fan1 = sa[0]
     if td2 == "self_att":
@@ -286,7 +303,7 @@ def config_from_args(args, max_chunk_segments=0):
         fan2 = td2w[0]
     if args["model"] == "NISQA_DIM" and fan2 is not None and fan2 != fan1:
         # NISQA_DIM builds its pooling heads for td's fan_out (lib:247-253): td_2 must keep it
-        if td2 == "self_att" and not td_lstm:
+        if td2 == "self_att" and not td_lstm and not skip:
             raise NotImplementedError("NISQA_DIM with td_2_sa_d_model=%d != td_sa_d_model=%d: the reference model cannot "
                                       "run it" % (fan2, fan1))
         raise NotImplementedError("NISQA_DIM with td_2 fan_out %d (%s) != td fan_out %d (%s): the reference model cannot run it" % (
@@ -301,11 +318,11 @@ def config_from_args(args, max_chunk_segments=0):
     cfg.max_segments = int(args["ms_max_segments"]) if args.get("ms_max_segments") else 0
     cfg.hop_s, cfg.win_s = float(args["ms_hop_length"]), float(args["ms_win_length"])
     cfg.fmax = float(args["ms_fmax"])
-    cfg.sa_layers = 0 if td_lstm else int(args["td_sa_num_layers"])
+    cfg.sa_layers = 0 if td_lstm or skip else int(args["td_sa_num_layers"])
     # NISQA_MAX_CHUNK: experiment knob (segments per internal pass) for A/B runs of the pass size
     cfg.max_chunk_segments = int(max_chunk_segments) or int(os.environ.get("NISQA_MAX_CHUNK", "0"))
     cfg.pool = pool_mode
-    cfg.pos_enc = 1 if (not td_lstm and args.get("td_sa_pos_enc")) else 0
+    cfg.pos_enc = 1 if (not td_lstm and not skip and args.get("td_sa_pos_enc")) else 0
     cfg.cnn_kind, cfg.cnn_fc = cnn_kind, cnn_fc
     cfg.sa_d_model, cfg.sa_ff = sa
     cfg.td2_d_model, cfg.td2_ff = td2w
@@ -324,6 +341,9 @@ def _fan_out_args(args, stage):
     if args.get(stage) == "lstm":
         return "%s_lstm_h=%r, %s_lstm_bidirectional=%r" % (stage, args.get(stage + "_lstm_h"), stage,
                                                            args.get(stage + "_lstm_bidirectional"))
+    if args.get(stage) in (None, "skip"):
+        return "%s=%r: the framewise fan_out of cnn_model=%r, cnn_fc_out_h=%r" % (
+            stage, args.get(stage), args.get("cnn_model"), args.get("cnn_fc_out_h"))
     return "%s_sa_d_model=%r" % (stage, args.get(stage + "_sa_d_model"))
 
 
