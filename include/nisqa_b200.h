@@ -119,9 +119,9 @@ typedef struct nisqa_config {
   int32_t abi_version;   /* NISQA_B200_ABI_VERSION */
   int32_t arch;          /* enum nisqa_arch */
   int32_t n_out;         /* 1 (NISQA) or 5 (NISQA_DIM: mos,noi,dis,col,loud - lib:1461-1465) */
-  int32_t n_fft;         /* ms_n_fft = 4096 */
-  int32_t n_mels;        /* ms_n_mels = 48  */
-  int32_t seg_len;       /* ms_seg_length = 15 */
+  int32_t n_fft;         /* ms_n_fft: 4096 only */
+  int32_t n_mels;        /* ms_n_mels: 32, 40, 48, 64, 80, 96 or 128 (StandardCNN: 48) */
+  int32_t seg_len;       /* ms_seg_length: odd, 3 .. 31 (StandardCNN: 15) */
   int32_t seg_hop;       /* ms_seg_hop_length (4 | 1) */
   int32_t max_segments;  /* ms_max_segments (1300 | 6000) */
   double  hop_s;         /* ms_hop_length seconds: hop = (int)(sr*hop_s), lib:2308 */
@@ -145,7 +145,7 @@ typedef struct nisqa_config {
   /* framewise model in front of a self-attention td (arch NISQA_ARCH_ADAPT_SA_ATTFF / NISQA_ARCH_SA_LSTM) or of no td
    * (NISQA_ARCH_SKIP; NISQA_ARCH_SKIP_LSTM: NISQA_CNN_STANDARD): */
   int32_t cnn_kind;      /* enum nisqa_cnn_kind: 0 = AdaptCNN, 1 = SkipCNN (lib:504-534), 2 = DFF (lib:536-583), 3 = StandardCNN */
-  int32_t cnn_fc;        /* cnn_fc_out_h: Linear behind the AdaptCNN (lib:682-684, 708-709), of SkipCNN (0 = none: 720 features),
+  int32_t cnn_fc;        /* cnn_fc_out_h: Linear behind the AdaptCNN (lib:682-684, 708-709), of SkipCNN (0 = none: n_mels * seg_len features),
                           * hidden width of DFF; a multiple of 64 */
   int32_t de_fuse_dim;   /* NISQA_DE: Linear(fused features -> de_fuse_dim) behind the fusion (lib:1399-1401, 1414-1415); 0 = none;
                           * a multiple of 64 */

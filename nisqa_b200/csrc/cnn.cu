@@ -1,7 +1,7 @@
 // cnn.cu - framewise CNN over mel segments (reference nisqa/NISQA_lib.py:688-710 AdaptCNN,
 // lib:811-836 StandardCNN; eval-mode BatchNorm folded into the conv weights on the host).
 //
-// Segments are never materialised: segment s is the view mel[frame0(s) .. frame0(s)+15][48]
+// Segments are never materialised: segment s is the view mel[frame0(s) .. frame0(s)+seg_len][n_mels]
 // (x[i,0,m,t] = spec[m, i*seg_hop + t], lib:2266-2273).  Activations between layers live in
 // HBM/L2 as channels-last [segment][h][w][c] fp32.
 //
@@ -20,15 +20,17 @@
 namespace nisqa {
 
 // ----------------------------------------------------------------------------------------
-// conv1 + BN + ReLU + pool1
-//   MODE 0 (adapt, lib:690-691): adaptive_max_pool2d 48x15 -> 24x7 : rows {2i,2i+1}, cols [2j,2j+3)
-//   MODE 1 (standard, lib:813-814): MaxPool2d(2, stride 2, padding (0,1)) -> 24x8 : cols {2j-1,2j}
+// conv1 + BN + ReLU + pool1 of segments of n_mels x seg_len cells (mel rows n_mels floats apart)
+//   MODE 0 (adapt, lib:690-691): adaptive_max_pool2d n_mels x seg_len -> 24x7 (conv1_adapt_cell; 48x15: rows {2i,2i+1},
+//          cols [2j,2j+3))
+//   MODE 1 (standard, lib:813-814): MaxPool2d(2, stride 2, padding (0,1)) -> 24x8 : cols {2j-1,2j} (48 x 15 only)
 // thread = one pooled cell of one segment, all 16 channels.
 // SPLIT: the output goes out as the two fp16 planes conv2's tensor-core kernel consumes (conv_split.cu:
 // padded rows of 16 halves = 32 bytes, 32-byte swizzle) instead of fp32 channels-last.
+// (__launch_bounds__ minimum of 2 CTAs: without it ptxas holds the AdaptCNN cell at 80 registers and spills)
 template <int MODE, bool SPLIT>
-__global__ void __launch_bounds__(256)
-conv1_pool1_kernel(const float* __restrict__ mel, const int* __restrict__ seg_frame0,
+__global__ void __launch_bounds__(256, 2)
+conv1_pool1_kernel(const float* __restrict__ mel, int n_mels, int seg_len, const int* __restrict__ seg_frame0,
                    const float* __restrict__ seg_thr, const float* __restrict__ w1 /*[9][16]*/,
                    const float* __restrict__ b1 /*[16]*/, float* __restrict__ out,
                    unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo,
@@ -48,7 +50,8 @@ conv1_pool1_kernel(const float* __restrict__ mel, const int* __restrict__ seg_fr
   const float thr = __ldg(seg_thr + seg);
 
   float res[16];
-  conv1_cell<MODE>(mel, f0, thr, ws, ph, pw, res);
+  if constexpr (MODE == 0) conv1_adapt_cell(mel + (size_t)f0 * n_mels, n_mels, seg_len, thr, ws, ph, pw, res);
+  else conv1_cell<MODE>(mel, f0, thr, ws, ph, pw, res);
   if constexpr (SPLIT) {
     const int g = kSplitLead + seg * (25 * (PW + 1)) + (ph + 1) * (PW + 1) + (pw + 1);
 #pragma unroll
@@ -271,21 +274,22 @@ static void launch_conv(cudaStream_t st, const float* in, const float* w, const 
   conv3x3_kernel<C><<<grid, C::NT, C::SMEM_BYTES, st>>>(in, w, b, out, n_seg);
 }
 
-void launch_conv1(cudaStream_t st, int std_mode, const float* mel, const int* seg_frame0,
-                  const float* seg_thr, const float* w1, const float* b1, float* out, int n_seg,
-                  void* out_hi, void* out_lo, float store_scale) {
+void launch_conv1(cudaStream_t st, int std_mode, const float* mel, int n_mels, int seg_len, const int* seg_frame0,
+                  const float* seg_thr, const float* w1, const float* b1, float* out, int n_seg, void* out_hi, void* out_lo,
+                  float store_scale) {
   const int cells = std_mode ? 24 * 8 : 24 * 7;
   const long long total = (long long)n_seg * cells;
   const int grid = (int)((total + 255) / 256);
   unsigned char* oh = static_cast<unsigned char*>(out_hi);
   unsigned char* ol = static_cast<unsigned char*>(out_lo);
   const float s = store_scale;
+  const int H = n_mels, W = seg_len;
   if (out_hi) {
-    if (std_mode) conv1_pool1_kernel<1, true><<<grid, 256, 0, st>>>(mel, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
-    else conv1_pool1_kernel<0, true><<<grid, 256, 0, st>>>(mel, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
+    if (std_mode) conv1_pool1_kernel<1, true><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
+    else conv1_pool1_kernel<0, true><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
   } else {
-    if (std_mode) conv1_pool1_kernel<1, false><<<grid, 256, 0, st>>>(mel, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
-    else conv1_pool1_kernel<0, false><<<grid, 256, 0, st>>>(mel, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
+    if (std_mode) conv1_pool1_kernel<1, false><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
+    else conv1_pool1_kernel<0, false><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
   }
 }
 

@@ -5,7 +5,9 @@
 
 namespace nisqa {
 
-constexpr int kMels = 48;        // ms_n_mels (asserted on the host)
+// The shipped Mel-spectrogram shape: the only one the fused conv1 + conv2 kernel (conv_split.cu) and StandardCNN take.
+// Every other kernel takes n_mels / seg_len from the engine (frontend.cu: one instance per band count).
+constexpr int kMels = 48;        // ms_n_mels
 constexpr int kSegLen = 15;      // ms_seg_length
 constexpr int kNfft = 4096;      // ms_n_fft
 constexpr int kBins = kNfft / 2 + 1;
@@ -19,7 +21,7 @@ struct ClipDesc {
   int hop, win;        // (int)(sr*hop_s), (int)(sr*win_s)  - reference lib:2308-2309
   int s0;              // sample index of window tap 0 of frame 0: lpad - n_fft/2
   int n_frames;        // 1 + n_samples / hop    (0 when the clip is skipped)
-  int frame_off;       // first row of this clip in the mel buffer [total_frames][48]
+  int frame_off;       // first row of this clip in the mel buffer [total_frames][n_mels]
   int pair_off;        // first frame-pair work item of this clip
   int n_seg;           // segments ("n_wins" after seg_hop, lib:2271-2273)
   int seg_off;         // first segment row of this clip in the segment-major buffers
@@ -29,8 +31,8 @@ struct ClipDesc {
 // Per-sample-rate front-end tables (device pointers).
 struct FbTables {
   const float* window;     // [win] periodic Hann (float32 of scipy's float64 values)
-  const int*   band_start; // [49] prefix offsets into weights
-  const int*   band_k0;    // [48] first FFT bin of each band
+  const int*   band_start; // [n_mels + 1] prefix offsets into weights
+  const int*   band_k0;    // [n_mels] first FFT bin of each band
   const float* weights;    // concatenated non-zero runs, band-major
   const float2* wtab;      // [4][1024] window[n] * W_4096^(r n) (0 for n >= win): window and residue twiddle in one load
   int n_mag;               // bins 0 .. n_mag-1 carry a non-zero filterbank weight (magnitudes are formed for these only)

@@ -224,6 +224,11 @@ struct nisqa_engine {
   bool td2_runs() const { return cfg.td2_layers > 0 || td2_lstm(); }
   bool std_cnn() const { return td_lstm() || cfg.cnn_kind == NISQA_CNN_STANDARD; }
   bool conv_net() const { return cfg.cnn_kind == NISQA_CNN_CONV || cfg.cnn_kind == NISQA_CNN_STANDARD; }
+  // SkipCNN / DFF rows: n_mels * seg_len features (x.view(-1, fan_in), lib:520 / 556), zero-padded to a multiple of 64
+  int ff_fan_in() const { return cfg.n_mels * cfg.seg_len; }
+  int ff_fan_in_pad() const { return (ff_fan_in() + 63) / 64 * 64; }
+  // conv1 + conv2 in one kernel (conv_split.cu): tensor-core path, the shipped 48 x 15 segments only
+  bool fused12() const { return conv_tc != 0 && conv12 != 0 && cfg.n_mels == kMels && cfg.seg_len == kSegLen; }
   int pool_d() const { return cfg.td2_layers > 0 ? td2_d() : sa_d(); }
 
   // front-end tables
@@ -574,6 +579,7 @@ bool pack_ff_linear(Packer& P, Linear& dst, const std::string& name, const std::
 // SkipCNN / DFF (lib:504-583): the BatchNorm2d(1) in front as a scalar affine map (applied by seg_feats_kernel, so
 // that the Linear layers see what the reference's see), Linear layers k-major, DFF's BatchNorm1d folded into them
 bool pack_ffnet(Packer& P, const nisqa_config& c) {
+  const int fan_in = c.n_mels * c.seg_len, fan_pad = (fan_in + 63) / 64 * 64;
   const bool dff = c.cnn_kind == NISQA_CNN_DFF;
   const std::string bn = dff ? "cnn.model.bn1." : "cnn.model.bn.";
   const TensorView* g = P.get(bn + "weight", {1});
@@ -586,9 +592,9 @@ bool pack_ffnet(Packer& P, const nisqa_config& c) {
   P.arena[o] = (float)a; P.arena[o + 1] = (float)((double)be->d[0] - (double)mu->d[0] * a);
   const int H = c.cnn_fc;
   if (dff)
-    return pack_ff_linear(P, P.w.ff[0], "lin1", "bn2", 720, 768, H) && pack_ff_linear(P, P.w.ff[1], "lin2", "bn3", H, H, H) &&
+    return pack_ff_linear(P, P.w.ff[0], "lin1", "bn2", fan_in, fan_pad, H) && pack_ff_linear(P, P.w.ff[1], "lin2", "bn3", H, H, H) &&
            pack_ff_linear(P, P.w.ff[2], "lin3", "bn4", H, H, H) && pack_ff_linear(P, P.w.ff[3], "lin4", "bn5", H, H, H);
-  return H == 0 || pack_ff_linear(P, P.w.ff[0], "linear", "", 720, 768, H);
+  return H == 0 || pack_ff_linear(P, P.w.ff[0], "linear", "", fan_in, fan_pad, H);
 }
 
 // The framewise model: AdaptCNN / StandardCNN (fp32 and tensor-core weights, activation scales) with AdaptCNN's optional
@@ -887,7 +893,8 @@ bool pack_td_model(Packer& P, nisqa_engine* e) {
   const nisqa_config& c = e->cfg;
   Weights& W = P.w;
   const std::string td = "time_dependency.model.", td2 = "time_dependency_2.model.";
-  // the rows feeding td: AdaptCNN's 384 (engine order), SkipCNN's 720 (padded to 768 with zero rows), cnn_fc_out_h, or
+  // the rows feeding td: AdaptCNN's 384 (engine order), SkipCNN's n_mels * seg_len (padded to a multiple of 64 with zero
+  // rows: 720 -> 768 at 48 x 15), cnn_fc_out_h, or
   // StandardCNN's fc_out / 768 conv6 features (engine order)
   InRows in;
   if (e->std_cnn()) {
@@ -895,7 +902,7 @@ bool pack_td_model(Packer& P, nisqa_engine* e) {
     in = W.std_fc ? InRows{W.std_fc, IN_PLAIN} : InRows{768, IN_STD_CONV};
   } else {
     const bool conv_net = c.cnn_kind == NISQA_CNN_CONV;
-    in = {c.cnn_fc > 0 ? c.cnn_fc : (conv_net ? 384 : 720), conv_net && c.cnn_fc == 0 ? IN_ADAPT_CONV : IN_PLAIN};
+    in = {c.cnn_fc > 0 ? c.cnn_fc : (conv_net ? 384 : e->ff_fan_in()), conv_net && c.cnn_fc == 0 ? IN_ADAPT_CONV : IN_PLAIN};
   }
   const Weights::LstmShape* last_lstm = nullptr;      // the last stage, when it is an LSTM
   int d1;                                             // td's fan_out
@@ -1128,7 +1135,7 @@ void conv_layers(Pass& p) {
   nisqa_engine* e = p.e;
   Lane& LN = p.LN;
   const Weights& w = p.w;
-  const bool split = e->conv_tc != 0, fused12 = split && e->conv12;
+  const bool split = e->conv_tc != 0, fused12 = e->fused12();
   auto plane_hi = [&](int l) { return LN.planes[l].as<char>(); };
   auto plane_lo = [&](int l) { return LN.planes[l].as<char>() + LN.plane_bytes[l]; };
   if (fused12) {
@@ -1138,7 +1145,7 @@ void conv_layers(Pass& p) {
                   plane_hi(3), plane_lo(3), p.n_seg);
   } else {
     Scope s(e, "conv1");
-    launch_conv1(p.st, p.std_mode, LN.mel.as<float>(), p.seg_frame0, p.seg_thr, w.conv[1].w,
+    launch_conv1(p.st, p.std_mode, LN.mel.as<float>(), p.c.n_mels, p.c.seg_len, p.seg_frame0, p.seg_thr, w.conv[1].w,
                  w.conv[1].b, split ? nullptr : LN.act[2].as<float>(), p.n_seg,
                  split ? plane_hi(2) : nullptr, split ? plane_lo(2) : nullptr, e->act_store(1));
   }
@@ -1161,16 +1168,16 @@ int ff_layers(Pass& p, Rows* out) {
   Lane& LN = p.LN;
   const Weights& w = p.w;
   Scope s(e, "framewise", 5);
-  const int H = p.c.cnn_fc, n_seg = p.n_seg;
-  CK(LN.ffa.reserve((size_t)n_seg * std::max(768, H) * 4));
+  const int H = p.c.cnn_fc, n_seg = p.n_seg, K = e->ff_fan_in_pad();
+  CK(LN.ffa.reserve((size_t)n_seg * std::max(K, H) * 4));
   float* ffa = LN.ffa.as<float>();
-  launch_seg_feats(p.st, LN.mel.as<float>(), p.seg_frame0, p.seg_thr, w.ff_bn, n_seg, ffa);
-  *out = {ffa, 12};
+  launch_seg_feats(p.st, LN.mel.as<float>(), p.c.n_mels, p.c.seg_len, K, p.seg_frame0, p.seg_thr, w.ff_bn, n_seg, ffa);
+  *out = {ffa, K / 64};
   if (H == 0) return 0;
   CK(LN.ffb.reserve((size_t)n_seg * H * 4));
   float* ffb = LN.ffb.as<float>();
   const bool dff = p.c.cnn_kind == NISQA_CNN_DFF;
-  launch_linear_tile(p.st, ffa, 768, w.ff[0].wT, w.ff[0].b, dff, ffb, H, n_seg, 768, H);
+  launch_linear_tile(p.st, ffa, K, w.ff[0].wT, w.ff[0].b, dff, ffb, H, n_seg, K, H);
   *out = {ffb, H / 64};
   if (!dff) return 0;
   float* pp[2] = {ffa, ffb};
@@ -1188,10 +1195,10 @@ int framewise(Pass& p, int fmt, Rows* out) {
   Lane& LN = p.LN;
   const int n_seg = p.n_seg;
   const bool conv_net = e->conv_net(), split = e->conv_tc != 0;
-  CK(LN.mel.reserve((size_t)p.n_frames * kMels * 4));
+  CK(LN.mel.reserve((size_t)p.n_frames * c.n_mels * 4));
   CK(LN.segtab.reserve((size_t)n_seg * 12));
   e->last_split = split;
-  for (int l = split && e->conv12 ? 3 : 2; conv_net && l <= 6; ++l) {
+  for (int l = e->fused12() ? 3 : 2; conv_net && l <= 6; ++l) {
     if (split) {
       // the lo plane sits at a fixed offset of the ALLOCATION (not of this pass's n_seg): the zero rows /
       // columns of both planes must stay where they were when the buffer was cleared
@@ -1208,11 +1215,11 @@ int framewise(Pass& p, int fmt, Rows* out) {
   p.seg_clip = p.seg_frame0 + 2 * (size_t)n_seg;
 
   { Scope s(e, "frontend");
-    launch_frontend(p.st, p.pcm, fmt == NISQA_FMT_F32, p.clips, p.n, p.max_pairs, e->fb_table.as<FbTables>(),
+    launch_frontend(p.st, c.n_mels, p.pcm, fmt == NISQA_FMT_F32, p.clips, p.n, p.max_pairs, e->fb_table.as<FbTables>(),
                     e->tw4096.as<float2>(), LN.mel.as<float>(), p.clipmax, p.Q, p.max_span, e->fe_ppc); }
   { Scope s(e, "seg_table");
     launch_seg_table(p.st, p.clips, p.n, p.seg_prefix, p.clipmax, c.seg_hop, n_seg, p.seg_frame0, p.seg_thr, p.seg_clip); }
-  e->last_conv12 = split && e->conv12;
+  e->last_conv12 = e->fused12();
   if (!conv_net) return ff_layers(p, out);
   conv_layers(p);
   *out = {LN.feats.as<float>(), p.std_mode ? 12 : 6};
@@ -1404,7 +1411,7 @@ int td_stages(Pass& p, Rows rows) {
   e->last_td_in = nullptr;
   if (skip) {
     cur = rows;
-    D = p.std_mode ? (w.std_fc ? w.std_fc : 768) : c.cnn_fc ? c.cnn_fc : c.cnn_kind == NISQA_CNN_CONV ? 384 : 720;
+    D = p.std_mode ? (w.std_fc ? w.std_fc : 768) : c.cnn_fc ? c.cnn_fc : c.cnn_kind == NISQA_CNN_CONV ? 384 : e->ff_fan_in();
   } else if (sa1) {
     e->last_td_in = LN.tdout.as<float>();
     cur = {sa_stack(p, 0, rows, !e->td2_runs(), LN.tdout.as<float>()), e->sa_d() / 64};
@@ -1630,8 +1637,15 @@ int nisqa_create(nisqa_engine** out, int device, const nisqa_config* cfg) {
     return fail(e, NISQA_ERR_INVALID, "sa_layers / sa_d_model / sa_ff / pos_enc: arch 4 and 5 have no td (keep them 0)");
   if (cfg->arch == NISQA_ARCH_SKIP_LSTM && cfg->cnn_kind != NISQA_CNN_STANDARD)
     return fail(e, NISQA_ERR_INVALID, "cnn_kind: arch 5 (an LSTM td_2 behind no td) needs StandardCNN");
-  if (cfg->n_fft != kNfft || cfg->n_mels != kMels || cfg->seg_len != kSegLen)
-    return fail(e, NISQA_ERR_INVALID, "engine is built for n_fft=4096, n_mels=48, seg_length=15");
+  if (cfg->n_fft != kNfft)
+    return fail(e, NISQA_ERR_INVALID, "n_fft = " + std::to_string(cfg->n_fft) + ": the front end runs n_fft 4096");
+  if (!frontend_supports_mels(cfg->n_mels))
+    return fail(e, NISQA_ERR_INVALID, "n_mels = " + std::to_string(cfg->n_mels) + ": the front end runs 32, 40, 48, 64, 80, 96 or 128 bands");
+  if (cfg->seg_len < 3 || cfg->seg_len > 31 || cfg->seg_len % 2 == 0)
+    return fail(e, NISQA_ERR_INVALID, "seg_len = " + std::to_string(cfg->seg_len) + ": the engine runs odd segment lengths of 3 to 31 frames");
+  if (e->std_cnn() && (cfg->n_mels != kMels || cfg->seg_len != kSegLen))
+    return fail(e, NISQA_ERR_INVALID, "n_mels = " + std::to_string(cfg->n_mels) + ", seg_len = " + std::to_string(cfg->seg_len) +
+                                          ": StandardCNN is built for 48 x 15 segments");
   if (cfg->n_out != 1 && cfg->n_out != 5) return fail(e, NISQA_ERR_INVALID, "n_out must be 1 or 5");
   if (cfg->seg_hop < 1 || cfg->hop_s <= 0 || cfg->win_s <= 0 || cfg->fmax <= 0)
     return fail(e, NISQA_ERR_INVALID, "bad front-end parameters");
@@ -1887,7 +1901,7 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
     src = LN.act[layer].as<float>(); hw = g.H * g.W; ch = g.C;
   }
   switch (stage) {
-    case NISQA_STAGE_MEL_DB: count = (int64_t)e->last_n_frames * kMels; break;
+    case NISQA_STAGE_MEL_DB: count = (int64_t)e->last_n_frames * e->cfg.n_mels; break;
     case NISQA_STAGE_POOL1: case NISQA_STAGE_POOL2: case NISQA_STAGE_CONV3: case NISQA_STAGE_POOL3: case NISQA_STAGE_CONV5: break;
     case NISQA_STAGE_CNN_FEAT:
       if (std_mode && e->w.lstm_shipped) {
@@ -1924,7 +1938,7 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
   if (stage == NISQA_STAGE_MEL_DB) {
     CK(e->dump.reserve((size_t)count * 4));
     launch_mel_dump(st, LN.mel.as<float>(), SG.clips.as<ClipDesc>(), (int)e->last_clips.size(),
-                    SG.clipmax.as<unsigned>(), e->dump.as<float>());
+                    SG.clipmax.as<unsigned>(), e->cfg.n_mels, e->dump.as<float>());
     src = e->dump.as<float>();
   } else if (ch > 0) {
     if (from_planes) {

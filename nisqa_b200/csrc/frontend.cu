@@ -224,27 +224,29 @@ __device__ __forceinline__ void fft1024_plane(f2 (&x)[32], float2* tile_, int la
   for (int p = 0; p < 32; ++p) tile[lane + 32 * p] = x[fe_out(p)];
 }
 
-// Fused unpack of the two real spectra, |.|, sparse mel, dB for the 12 bands of this warp
+// Fused unpack of the two real spectra, |.|, sparse mel, dB for the MELS / 4 bands of this warp
 // (b = warp + 4*slot).  Lanes stride over a band's bins and keep one partial sum per (slot, frame);
-// the 24 partials are reduced across the warp with ONE multi-value butterfly (31 shuffles instead of
-// 24 x 5): at the step with offset o the 2*o live values are paired (i, i+o), a lane whose bit o is set
+// the partials of up to 16 slots (32 values: one round) are reduced across the warp with ONE multi-value butterfly (31
+// shuffles instead of 32 x 5): at the step with offset o the 2*o live values are paired (i, i+o), a lane whose bit o is set
 // keeps the upper one and sends the lower one, so lane L ends up with the total of value index L =
-// (slot L>>1, frame L&1) and one log10f serves the whole warp.  A bin belongs to two adjacent
-// triangles, so its magnitudes are formed twice - cheaper than a shared-memory round trip.
-// Returns this lane's dB value (or -inf) for the clip maximum.
-__device__ __forceinline__ float mel_bands(const float2* scratch, const int* band_meta,
-                                           const float* __restrict__ weights, int warp, int lane,
-                                           bool validB, float* __restrict__ mel_row0 /*frame A row*/) {
+// (slot L>>1, frame L&1) and one log10f serves the whole warp.  More than 64 bands (80 / 96 / 128) take a second round
+// over slots 16 .. 31.  A bin belongs to two adjacent triangles, so its magnitudes are formed twice - cheaper than a
+// shared-memory round trip.  Returns this lane's dB value (or -inf) for the clip maximum.
+template <int MELS, int S0>
+__device__ __forceinline__ float mel_bands_round(const float2* scratch, const int* band_meta,
+                                                 const float* __restrict__ weights, int warp, int lane,
+                                                 bool validB, float* __restrict__ mel_row0 /*frame A row*/) {
+  constexpr int NS = (MELS / 4 - S0) < 16 ? (MELS / 4 - S0) : 16;     // slots of this round
   float v[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) v[i] = 0.f;
 #pragma unroll
-  for (int slot = 0; slot < kMels / 4; ++slot) {
-    const int b = warp + slot * 4;
+  for (int slot = 0; slot < NS; ++slot) {
+    const int b = warp + (S0 + slot) * 4;
     // band rows are zero-padded to a multiple of 32 weights (engine build_fb): warp-uniform trip
     // count, no divergence, every lane loads unconditionally (the padded bins stay inside the planes)
     const int beg = band_meta[b], iters = (band_meta[b + 1] - beg) >> 5;
-    const int k = band_meta[kMels + 1 + b] + lane;
+    const int k = band_meta[MELS + 1 + b] + lane;
     const int kk = (kNfft - k) & (kNfft - 1);
     // Z planes: bin k lives at plane (k & 3), slot (k >> 2); k advances by 32 per iteration,
     // so both indices move by +-8 and the plane never changes.
@@ -271,12 +273,21 @@ __device__ __forceinline__ float mel_bands(const float2* scratch, const int* ban
   fold_step<16>(v, lane); fold_step<8>(v, lane); fold_step<4>(v, lane); fold_step<2>(v, lane); fold_step<1>(v, lane);
   float out = -INFINITY;
   const int my_slot = lane >> 1, f = lane & 1;
-  if (lane < 2 * (kMels / 4) && (f == 0 || validB)) {
+  if (lane < 2 * NS && (f == 0 || validB)) {
     const float sv = 0.5f * v[0];                          // the 1/2 of the real-pair unpacking
     const float p = sv * sv;
-    out = 10.0f * log10f(fmaxf(p, 1e-8f));
-    mel_row0[(size_t)f * kMels + warp + my_slot * 4] = out;
+    out = 10.0f * log10f(fmaxf(p, 1e-8f));                 // (an empty band of a low rate: 0 -> the -80 dB floor)
+    mel_row0[(size_t)f * MELS + warp + (S0 + my_slot) * 4] = out;
   }
+  return out;
+}
+template <int MELS>
+__device__ __forceinline__ float mel_bands(const float2* scratch, const int* band_meta,
+                                           const float* __restrict__ weights, int warp, int lane,
+                                           bool validB, float* __restrict__ mel_row0) {
+  float out = mel_bands_round<MELS, 0>(scratch, band_meta, weights, warp, lane, validB, mel_row0);
+  if constexpr (MELS / 4 > 16)
+    out = fmaxf(out, mel_bands_round<MELS, 16>(scratch, band_meta, weights, warp, lane, validB, mel_row0));
   return out;
 }
 
@@ -313,21 +324,24 @@ __device__ __forceinline__ void mag_stage(float2* scratch, int n_mag, int tid) {
   }
 }
 
-// Stage B: the 12 bands of this warp as weighted sums of the staged magnitudes, then the same multi-value butterfly
-// reduction and dB as mel_bands.  `pscale` = 2^-30 for PCM16 input fed as raw integers (|X| scales by 2^15 exactly).
-__device__ __forceinline__ float mel_bands_staged(const float2* scratch, const int* band_meta,
-                                                  const float* __restrict__ weights, int warp, int lane,
-                                                  bool validB, float pscale, float* __restrict__ mel_row0) {
+// Stage B: the MELS / 4 bands of this warp as weighted sums of the staged magnitudes, then the same multi-value butterfly
+// reduction and dB as mel_bands, in rounds of up to 16 slots.  `pscale` = 2^-30 for PCM16 input fed as raw integers
+// (|X| scales by 2^15 exactly).
+template <int MELS, int S0>
+__device__ __forceinline__ float mel_bands_staged_round(const float2* scratch, const int* band_meta,
+                                                        const float* __restrict__ weights, int warp, int lane,
+                                                        bool validB, float pscale, float* __restrict__ mel_row0) {
+  constexpr int NS = (MELS / 4 - S0) < 16 ? (MELS / 4 - S0) : 16;     // slots of this round
   // v[i]: packed (frame A, frame B) partial sums of slot i in this lane.  The band loop is kept rolled: one weight load,
-  // one magnitude pair, one FFMA2 per 32 bins and lane; trip counts (1 .. ~10 rows per band) are warp uniform.
+  // one magnitude pair, one FFMA2 per 32 bins and lane; trip counts (0 .. ~10 rows per band) are warp uniform.
   f2 v[16];
 #pragma unroll
   for (int i = 0; i < 16; ++i) v[i] = 0ull;
 #pragma unroll
-  for (int slot = 0; slot < kMels / 4; ++slot) {
-    const int b = warp + slot * 4;
+  for (int slot = 0; slot < NS; ++slot) {
+    const int b = warp + (S0 + slot) * 4;
     const int beg = band_meta[b], end = band_meta[b + 1];
-    const int k = band_meta[kMels + 1 + b] + lane;
+    const int k = band_meta[MELS + 1 + b] + lane;
     const f2* pm = reinterpret_cast<const f2*>(scratch + (k & 3) * kScratchPerWarp + (k >> 2));
     const float* wt = weights + beg + lane;
     // padded bins (weight 0) may hold raw spectrum values: finite, times 0
@@ -353,24 +367,47 @@ __device__ __forceinline__ float mel_bands_staged(const float2* scratch, const i
     v[slot] = acc;
 #endif
   }
-  // multi-value butterfly over the 12 (padded to 16) packed values: after the steps with lane offsets 16, 8, 4, 2 lane L
+  // multi-value butterfly over the NS (padded to 16) packed values: after the steps with lane offsets 16, 8, 4, 2 lane L
   // holds the value of slot (L >> 1) & ... summed over 16 lanes; the last step adds the partner lane (L ^ 1)
   fold_step<8, 2>(v, lane); fold_step<4, 2>(v, lane); fold_step<2, 2>(v, lane); fold_step<1, 2>(v, lane);
   const float2 tot = upk(add2(v[0], __shfl_xor_sync(0xffffffffu, v[0], 1)));
   // lane L now holds slot s(L) = bit-reversal free index: bits 4..1 of L select the slot (offset 16 -> +8, 8 -> +4, ...)
   float out = -INFINITY;
   const int my_slot = lane >> 1, f = lane & 1;
-  if (my_slot < kMels / 4 && (f == 0 || validB)) {
+  if (my_slot < NS && (f == 0 || validB)) {
     const float sv = 0.5f * (f == 0 ? tot.x : tot.y);
     const float p = (sv * sv) * pscale;
-    out = 10.0f * log10f(fmaxf(p, 1e-8f));
-    mel_row0[(size_t)f * kMels + warp + my_slot * 4] = out;
+    out = 10.0f * log10f(fmaxf(p, 1e-8f));                 // (an empty band of a low rate: 0 -> the -80 dB floor)
+    mel_row0[(size_t)f * MELS + warp + (S0 + my_slot) * 4] = out;
   }
   return out;
 }
+template <int MELS>
+__device__ __forceinline__ float mel_bands_staged(const float2* scratch, const int* band_meta,
+                                                  const float* __restrict__ weights, int warp, int lane,
+                                                  bool validB, float pscale, float* __restrict__ mel_row0) {
+  float out = mel_bands_staged_round<MELS, 0>(scratch, band_meta, weights, warp, lane, validB, pscale, mel_row0);
+  if constexpr (MELS / 4 > 16)
+    out = fmaxf(out, mel_bands_staged_round<MELS, 16>(scratch, band_meta, weights, warp, lane, validB, pscale, mel_row0));
+  return out;
+}
+
+// band_meta[0 .. MELS]: CSR offsets of the bands, [MELS + 1 .. 2 MELS]: first bin of each band (one pass of the CTA's
+// 128 threads up to 63 bands, a strided loop beyond)
+template <int MELS>
+__device__ __forceinline__ void load_band_meta(int* band_meta, const FbTables& fb, int tid) {
+  if constexpr (2 * MELS + 1 <= kFeThreads) {
+    if (tid <= MELS) band_meta[tid] = __ldg(fb.band_start + tid);
+    else if (tid < 2 * MELS + 1) band_meta[tid] = __ldg(fb.band_k0 + tid - MELS - 1);
+  } else {
+    for (int i = tid; i < 2 * MELS + 1; i += kFeThreads)
+      band_meta[i] = i <= MELS ? __ldg(fb.band_start + i) : __ldg(fb.band_k0 + i - MELS - 1);
+  }
+}
 
 // ---- generic kernel: one CTA per frame pair, any window length (win <= 1024*Q <= n_fft) ------
-template <typename T>
+// One instance per band count MELS (the mel rows are MELS floats apart).
+template <typename T, int MELS>
 __global__ void __launch_bounds__(kFeThreads, 5)
 frontend_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips, int n_clips,
                 const FbTables* __restrict__ fbs,
@@ -380,7 +417,7 @@ frontend_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips, i
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float2* zin = reinterpret_cast<float2*>(smem_raw);                     // [1024*Q] packed input
   float2* scratch = reinterpret_cast<float2*>(smem_raw + fe_region0_bytes(Q));
-  __shared__ int band_meta[2 * kMels + 1];        // [0..48] CSR offsets, [49..96] first bin per band
+  __shared__ int band_meta[2 * MELS + 1];         // [0..MELS] CSR offsets, [MELS+1..2 MELS] first bin per band
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   // grid: x = frame pair within the clip, y = clip (no search, no dependent loads)
@@ -392,8 +429,7 @@ frontend_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips, i
   const int tB = tA + 1;
   const bool validB = tB < cd.n_frames;
   const T* y = pcm + cd.pcm_off;
-  if (tid <= kMels) band_meta[tid] = __ldg(fb.band_start + tid);
-  else if (tid < 2 * kMels + 1) band_meta[tid] = __ldg(fb.band_k0 + tid - kMels - 1);
+  load_band_meta<MELS>(band_meta, fb, tid);
 
   // ---- a. windowed, reflect-padded frame pair -> zin  (8 elements per thread per 1024 chunk,
   //         all loads of a chunk issued before they are consumed)
@@ -442,8 +478,8 @@ frontend_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips, i
   __syncthreads();
 
   // ---- c. mel + dB + clip max
-  float wmax = mel_bands(scratch, band_meta, fb.weights, warp, lane, validB,
-                         mel + (size_t)(cd.frame_off + tA) * kMels);
+  float wmax = mel_bands<MELS>(scratch, band_meta, fb.weights, warp, lane, validB,
+                               mel + (size_t)(cd.frame_off + tA) * MELS);
   wmax = warp_max(wmax);
   if (lane == 0 && wmax > -INFINITY) atomicMax(clipmax + c, f2key(wmax));
 }
@@ -486,7 +522,7 @@ __device__ __forceinline__ void pp_issue_pair(const T* __restrict__ y, int a, in
   asm volatile("cp.async.commit_group;" ::: "memory");
 }
 
-template <typename T>
+template <typename T, int MELS>
 __global__ void __launch_bounds__(kFeThreads, (sizeof(T) == 2 && NISQA_FE_CTAS >= 6) ? 6 : 5)
 frontend_pp_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips,
                    const FbTables* __restrict__ fbs, const float2* __restrict__ tw1,
@@ -495,7 +531,7 @@ frontend_pp_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips
   extern __shared__ __align__(16) unsigned char smem_raw[];
   constexpr int NSLOT = pp_slots<T>();
   float2* scratch = reinterpret_cast<float2*>(smem_raw + NSLOT * pp_slot_bytes<T>());
-  __shared__ int band_meta[2 * kMels + 1];
+  __shared__ int band_meta[2 * MELS + 1];
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int c = blockIdx.y;
@@ -508,8 +544,7 @@ frontend_pp_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips
   const int span = cd.hop + cd.win;
   pp_issue_pair<T>(y, cd.s0 + 2 * p0 * cd.hop, span, cd.n_samples, reinterpret_cast<T*>(smem_raw), tid);
   const FbTables fb = fbs[cd.fb_id];
-  if (tid <= kMels) band_meta[tid] = __ldg(fb.band_start + tid);
-  else if (tid < 2 * kMels + 1) band_meta[tid] = __ldg(fb.band_k0 + tid - kMels - 1);
+  load_band_meta<MELS>(band_meta, fb, tid);
 
   const int r = warp;
   float wmax = -INFINITY;
@@ -558,9 +593,9 @@ frontend_pp_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips
       pp_issue_pair<T>(y, a + 2 * cd.hop, span, cd.n_samples, reinterpret_cast<T*>(smem_raw), tid);
     mag_stage(scratch, fb.n_mag, tid);
     __syncthreads();                    // magnitudes staged
-    wmax = fmaxf(wmax, mel_bands_staged(scratch, band_meta, fb.weights, warp, lane, validB,
-                                        sizeof(T) == 2 ? 9.313225746154785e-10f : 1.0f,
-                                        mel + (size_t)(cd.frame_off + 2 * p) * kMels));
+    wmax = fmaxf(wmax, mel_bands_staged<MELS>(scratch, band_meta, fb.weights, warp, lane, validB,
+                                              sizeof(T) == 2 ? 9.313225746154785e-10f : 1.0f,
+                                              mel + (size_t)(cd.frame_off + 2 * p) * MELS));
   }
   wmax = warp_max(wmax);
   if (lane == 0 && wmax > -INFINITY) atomicMax(clipmax + c, f2key(wmax));
@@ -582,39 +617,40 @@ __global__ void seg_table_kernel(const ClipDesc* __restrict__ clips, int n_clips
   seg_clip[s] = c;
 }
 
-// stage dump helper: mel[frame][48] -> per clip [48][n_frames] with the top_db clamp applied
+// stage dump helper: mel[frame][n_mels] -> per clip [n_mels][n_frames] with the top_db clamp applied
 __global__ void mel_dump_kernel(const float* __restrict__ mel, const ClipDesc* __restrict__ clips,
-                                int n_clips, const unsigned* __restrict__ clipmax,
+                                int n_clips, const unsigned* __restrict__ clipmax, int n_mels,
                                 float* __restrict__ out) {
   const int c = blockIdx.y;
   const ClipDesc cd = clips[c];
   const float thr = key2f(clipmax[c]) - 80.0f;
-  const int n = cd.n_frames * kMels;
-  float* o = out + (size_t)cd.frame_off * kMels;
+  const int n = cd.n_frames * n_mels;
+  float* o = out + (size_t)cd.frame_off * n_mels;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const int b = i / cd.n_frames, t = i - b * cd.n_frames;
-    o[i] = fmaxf(mel[(size_t)(cd.frame_off + t) * kMels + b], thr);
+    o[i] = fmaxf(mel[(size_t)(cd.frame_off + t) * n_mels + b], thr);
   }
 }
 
 // ------------------------------------------------------------------ host launchers
-void launch_frontend(cudaStream_t st, const void* pcm, int fmt_f32, const ClipDesc* clips,
-                     int n_clips, int max_pairs, const FbTables* fbs,
-                     const float2* tw, float* mel, unsigned* clipmax, int Q, int max_span, int ppc) {
+template <int MELS>
+static void launch_frontend_mels(cudaStream_t st, const void* pcm, int fmt_f32, const ClipDesc* clips,
+                                 int n_clips, int max_pairs, const FbTables* fbs,
+                                 const float2* tw, float* mel, unsigned* clipmax, int Q, int max_span, int ppc) {
   const float2* tw1 = tw;               // [3][32][32]
   const float4* tw2 = reinterpret_cast<const float4*>(tw + 4 * 1024);    // [32][32] (x, y, -y, x)
   if (Q == 1 && max_span <= kSpanMax) { // the pipelined multi-pair kernel
     static unsigned long long configured = 0;
     if (first_launch_on_device(configured)) {
-      cudaFuncSetAttribute(frontend_pp_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, pp_smem_bytes<float>());
-      cudaFuncSetAttribute(frontend_pp_kernel<short>, cudaFuncAttributeMaxDynamicSharedMemorySize, pp_smem_bytes<short>());
+      cudaFuncSetAttribute(frontend_pp_kernel<float, MELS>, cudaFuncAttributeMaxDynamicSharedMemorySize, pp_smem_bytes<float>());
+      cudaFuncSetAttribute(frontend_pp_kernel<short, MELS>, cudaFuncAttributeMaxDynamicSharedMemorySize, pp_smem_bytes<short>());
     }
     if (ppc < 1) ppc = kPairsPerCta;
     const dim3 grid((max_pairs + ppc - 1) / ppc, n_clips);
     if (fmt_f32)
-      frontend_pp_kernel<float><<<grid, kFeThreads, pp_smem_bytes<float>(), st>>>((const float*)pcm, clips, fbs, tw1, tw2, mel, clipmax, ppc);
+      frontend_pp_kernel<float, MELS><<<grid, kFeThreads, pp_smem_bytes<float>(), st>>>((const float*)pcm, clips, fbs, tw1, tw2, mel, clipmax, ppc);
     else
-      frontend_pp_kernel<short><<<grid, kFeThreads, pp_smem_bytes<short>(), st>>>((const short*)pcm, clips, fbs, tw1, tw2, mel, clipmax, ppc);
+      frontend_pp_kernel<short, MELS><<<grid, kFeThreads, pp_smem_bytes<short>(), st>>>((const short*)pcm, clips, fbs, tw1, tw2, mel, clipmax, ppc);
     return;
   }
   const int smem = frontend_smem_bytes(Q);
@@ -622,16 +658,35 @@ void launch_frontend(cudaStream_t st, const void* pcm, int fmt_f32, const ClipDe
   // for the largest window this kernel supports (Q = 4: win up to n_fft)
   static unsigned long long configured = 0;
   if (first_launch_on_device(configured)) {
-    cudaFuncSetAttribute(frontend_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, frontend_smem_bytes(4));
-    cudaFuncSetAttribute(frontend_kernel<short>, cudaFuncAttributeMaxDynamicSharedMemorySize, frontend_smem_bytes(4));
+    cudaFuncSetAttribute(frontend_kernel<float, MELS>, cudaFuncAttributeMaxDynamicSharedMemorySize, frontend_smem_bytes(4));
+    cudaFuncSetAttribute(frontend_kernel<short, MELS>, cudaFuncAttributeMaxDynamicSharedMemorySize, frontend_smem_bytes(4));
   }
   const dim3 grid(max_pairs, n_clips);
   if (fmt_f32) {
-    frontend_kernel<float><<<grid, kFeThreads, smem, st>>>(
+    frontend_kernel<float, MELS><<<grid, kFeThreads, smem, st>>>(
         (const float*)pcm, clips, n_clips, fbs, tw1, tw2, mel, clipmax, Q);
   } else {
-    frontend_kernel<short><<<grid, kFeThreads, smem, st>>>(
+    frontend_kernel<short, MELS><<<grid, kFeThreads, smem, st>>>(
         (const short*)pcm, clips, n_clips, fbs, tw1, tw2, mel, clipmax, Q);
+  }
+}
+
+bool frontend_supports_mels(int n_mels) {
+  switch (n_mels) {
+    case 32: case 40: case 48: case 64: case 80: case 96: case 128: return true;
+    default: return false;
+  }
+}
+
+void launch_frontend(cudaStream_t st, int n_mels, const void* pcm, int fmt_f32, const ClipDesc* clips,
+                     int n_clips, int max_pairs, const FbTables* fbs,
+                     const float2* tw, float* mel, unsigned* clipmax, int Q, int max_span, int ppc) {
+  switch (n_mels) {       // (nisqa_create accepts these only: frontend_supports_mels)
+#define NISQA_FE_CASE(M) \
+    case M: launch_frontend_mels<M>(st, pcm, fmt_f32, clips, n_clips, max_pairs, fbs, tw, mel, clipmax, Q, max_span, ppc); break;
+    NISQA_FE_CASE(32) NISQA_FE_CASE(40) NISQA_FE_CASE(48) NISQA_FE_CASE(64) NISQA_FE_CASE(80) NISQA_FE_CASE(96) NISQA_FE_CASE(128)
+#undef NISQA_FE_CASE
+    default: break;
   }
 }
 
@@ -644,9 +699,9 @@ void launch_seg_table(cudaStream_t st, const ClipDesc* clips, int n_clips, const
 }
 
 void launch_mel_dump(cudaStream_t st, const float* mel, const ClipDesc* clips, int n_clips,
-                     const unsigned* clipmax, float* out) {
+                     const unsigned* clipmax, int n_mels, float* out) {
   dim3 grid(8, n_clips);
-  mel_dump_kernel<<<grid, 256, 0, st>>>(mel, clips, n_clips, clipmax, out);
+  mel_dump_kernel<<<grid, 256, 0, st>>>(mel, clips, n_clips, clipmax, n_mels, out);
 }
 
 }  // namespace nisqa

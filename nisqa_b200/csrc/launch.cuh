@@ -75,15 +75,21 @@ struct ResampleClip {
 };
 
 // ---------------------------------------------------------------- frontend.cu
-void launch_frontend(cudaStream_t st, const void* pcm, int fmt_f32, const ClipDesc* clips, int n_clips, int max_pairs,
+// mel: [frames][n_mels]; one kernel instance per band count, n_mels in {32, 40, 48, 64, 80, 96, 128} (frontend_supports_mels)
+bool frontend_supports_mels(int n_mels);
+void launch_frontend(cudaStream_t st, int n_mels, const void* pcm, int fmt_f32, const ClipDesc* clips, int n_clips, int max_pairs,
                      const FbTables* fbs, const float2* tw, float* mel, unsigned* clipmax, int Q, int max_span, int ppc);
 void launch_seg_table(cudaStream_t st, const ClipDesc* clips, int n_clips, const int* seg_prefix, const unsigned* clipmax,
                       int seg_hop, int n_seg, int* seg_frame0, float* seg_thr, int* seg_clip);
-void launch_mel_dump(cudaStream_t st, const float* mel, const ClipDesc* clips, int n_clips, const unsigned* clipmax, float* out);
+void launch_mel_dump(cudaStream_t st, const float* mel, const ClipDesc* clips, int n_clips, const unsigned* clipmax, int n_mels,
+                     float* out);
 
 // ---------------------------------------------------------------- cnn.cu (fp32 FFMA convolutions)
-void launch_conv1(cudaStream_t st, int std_mode, const float* mel, const int* seg_frame0, const float* seg_thr,
-                  const float* w1, const float* b1, float* out, int n_seg, void* out_hi, void* out_lo, float store_scale);
+// conv1 + pool1 of segments of n_mels x seg_len mel cells (rows n_mels floats apart): AdaptCNN any accepted shape ->
+// 24 x 7, StandardCNN 48 x 15 only -> 24 x 8
+void launch_conv1(cudaStream_t st, int std_mode, const float* mel, int n_mels, int seg_len, const int* seg_frame0,
+                  const float* seg_thr, const float* w1, const float* b1, float* out, int n_seg, void* out_hi, void* out_lo,
+                  float store_scale);
 void launch_conv_layer(cudaStream_t st, int std_mode, int layer, const float* in, const float* w, const float* b, float* out,
                        int n_seg);
 void launch_nhwc_to_nchw(cudaStream_t st, const float* in, float* out, long long n, int hw, int ch);
@@ -135,8 +141,9 @@ void launch_td_sa(cudaStream_t st, int nc, const float* x_in, const float* qkv, 
 void launch_de_align(cudaStream_t st, const float* x_td, const ClipDesc* clips, int n_clips, const int* qtile64_prefix,
                      int n_qtiles, int align, int soft, int fuse, const DeAlignParams& A, float* fused);
 void launch_de_finalize(cudaStream_t st, const ClipDesc* clips, int n_clips, int n_out, float* scores);
-void launch_seg_feats(cudaStream_t st, const float* mel, const int* seg_frame0, const float* seg_thr, const float* bn, int n_seg,
-                      float* out);
+// SkipCNN / DFF rows: n_mels * seg_len features at index m * seg_len + t, zero up to the row stride ld (a multiple of 64)
+void launch_seg_feats(cudaStream_t st, const float* mel, int n_mels, int seg_len, int ld, const int* seg_frame0,
+                      const float* seg_thr, const float* bn, int n_seg, float* out);
 void launch_linear_tile(cudaStream_t st, const float* X, int ldx, const float* WT, const float* bias, int relu, float* Y, int ldy,
                         int n_rows, int K, int N);
 

@@ -845,24 +845,25 @@ __global__ void de_finalize_kernel(const ClipDesc* __restrict__ clips, int n_cli
 // ---------------------------------------------------------------------------------------------------------------
 // Framewise models without convolutions (reference lib:504-583, user checkpoints): SkipCNN = BatchNorm2d(1) + flatten
 // (+ Linear), DFF = BatchNorm2d(1) + flatten + 4 x (Linear + BatchNorm1d + ReLU).
-//   seg_feats_kernel  : segment s -> row [768]: a * max(mel[frame0 + t][m], thr) + c at index m * 15 + t (x.view(-1, 720),
-//                       lib:531 / 572), columns 720..767 zero (the rows feed 64-wide k chunks)
+//   seg_feats_kernel  : segment s -> row [ld]: a * max(mel[frame0 + t][m], thr) + c at index m * seg_len + t
+//                       (x.view(-1, fan_in), fan_in = n_mels * seg_len, lib:531 / 572), columns fan_in .. ld - 1 zero
+//                       (ld: fan_in rounded up to 64, the rows feed 64-wide k chunks)
 //   linear_tile_kernel: Y[n][N] = act(X[n][K] W^T + b), 64 x 64 output tiles, K in chunks of 64 (K, N multiples of 64),
 //                       the same register-tiled fp32 product as the time-dependency block
-__global__ void seg_feats_kernel(const float* __restrict__ mel, const int* __restrict__ seg_frame0,
-                                 const float* __restrict__ seg_thr, const float* __restrict__ bn /*a, c*/, int n_seg,
-                                 float* __restrict__ out /*[n_seg][768]*/) {
+__global__ void seg_feats_kernel(const float* __restrict__ mel, int n_mels, int seg_len, int ld,
+                                 const int* __restrict__ seg_frame0, const float* __restrict__ seg_thr,
+                                 const float* __restrict__ bn /*a, c*/, int n_seg, float* __restrict__ out /*[n_seg][ld]*/) {
   const int s = blockIdx.x;
   if (s >= n_seg) return;
-  const float* src = mel + (size_t)__ldg(seg_frame0 + s) * kMels;
+  const float* src = mel + (size_t)__ldg(seg_frame0 + s) * n_mels;
   const float thr = __ldg(seg_thr + s), a = __ldg(bn), c = __ldg(bn + 1);
-  for (int j = threadIdx.x; j < 768; j += blockDim.x) {
+  for (int j = threadIdx.x; j < ld; j += blockDim.x) {
     float v = 0.f;
-    if (j < kMels * kSegLen) {
-      const int m = j / kSegLen, t = j - m * kSegLen;
-      v = fmaf(a, fmaxf(__ldg(src + t * kMels + m), thr), c);
+    if (j < n_mels * seg_len) {
+      const int m = j / seg_len, t = j - m * seg_len;
+      v = fmaf(a, fmaxf(__ldg(src + t * n_mels + m), thr), c);
     }
-    out[(size_t)s * 768 + j] = v;
+    out[(size_t)s * ld + j] = v;
   }
 }
 
@@ -942,9 +943,9 @@ void launch_de_align(cudaStream_t st, const float* x_td, const ClipDesc* clips, 
   de_align_kernel<<<n_qtiles, kNT, smem, st>>>(x_td, clips, n_clips, qtile64_prefix, align, soft, fuse, A, fused);
 }
 
-void launch_seg_feats(cudaStream_t st, const float* mel, const int* seg_frame0, const float* seg_thr, const float* bn, int n_seg,
-                      float* out) {
-  if (n_seg > 0) seg_feats_kernel<<<n_seg, 256, 0, st>>>(mel, seg_frame0, seg_thr, bn, n_seg, out);
+void launch_seg_feats(cudaStream_t st, const float* mel, int n_mels, int seg_len, int ld, const int* seg_frame0,
+                      const float* seg_thr, const float* bn, int n_seg, float* out) {
+  if (n_seg > 0) seg_feats_kernel<<<n_seg, 256, 0, st>>>(mel, n_mels, seg_len, ld, seg_frame0, seg_thr, bn, n_seg, out);
 }
 
 void launch_linear_tile(cudaStream_t st, const float* X, int ldx, const float* WT, const float* bias, int relu, float* Y, int ldy,

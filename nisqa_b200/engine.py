@@ -58,6 +58,8 @@ SA_FF_MAX = 4096                      # feed-forward width: a multiple of 64 up 
 LSTM_H = (32, 64, 96, 128, 192, 256)  # LSTM hidden sizes the kernels are instantiated for
 LSTM_LAYERS_MAX = 4
 CNN_FC_OUT_MAX = 1024                 # StandardCNN's fc_out width (None: the LSTM reads the 768 conv6 features)
+N_MELS = (32, 40, 48, 64, 80, 96, 128)   # ms_n_mels: one front-end kernel instance per band count
+SEG_LEN_MIN, SEG_LEN_MAX = 3, 31      # ms_seg_length, odd (128 x 31 bounds SkipCNN's / DFF's fan_in at 3968 < 4096)
 
 
 def _sa_widths(args, prefix, de=False):
@@ -267,7 +269,8 @@ def config_from_args(args, max_chunk_segments=0):
     skip = arch in (ARCH_SKIP, ARCH_SKIP_LSTM)
     fan1 = _check_lstm(args, "td_lstm") if td_lstm else None
     if skip:
-        fan1 = int(args.get("cnn_fc_out_h") or 768) if cnn == "standard" else (cnn_fc or (384 if cnn == "adapt" else 720))
+        fan1 = int(args.get("cnn_fc_out_h") or 768) if cnn == "standard" else (
+            cnn_fc or (384 if cnn == "adapt" else int(args.get("ms_n_mels") or 0) * int(args.get("ms_seg_length") or 0)))
     fan2 = _check_lstm(args, "td_2_lstm") if td2 == "lstm" else None
     if pool_mode == POOL_LAST_STEP_BI:
         key = "td_2_lstm" if td2 == "lstm" else "td_lstm" if td2 == "skip" and td_lstm else None
@@ -291,9 +294,9 @@ def config_from_args(args, max_chunk_segments=0):
         if args.get("de_fuse_dim") and int(args["de_fuse_dim"]) % 64 != 0:
             raise NotImplementedError("de_fuse_dim=%r: the engine needs a multiple of 64" % (args.get("de_fuse_dim"),))
     ok = ok and (cnn_kind != CNN_CONV or (args["cnn_c_out_1"], args["cnn_c_out_2"], args["cnn_c_out_3"]) == (16, 32, 64))
-    ok = ok and args["ms_n_fft"] == 4096 and args["ms_n_mels"] == 48 and args["ms_seg_length"] == 15
     if not ok:
         raise NotImplementedError("checkpoint hyper-parameters outside the shipped NISQA configurations")
+    n_mels, seg_len = _check_mel_shape(args, td_lstm or cnn_kind == CNN_STANDARD)
     sa = td2w = (0, 0)
     if not td_lstm and not skip:
         sa = _sa_widths(args, "td_sa", de)
@@ -313,7 +316,7 @@ def config_from_args(args, max_chunk_segments=0):
     cfg.abi_version = ABI_VERSION
     cfg.arch = arch
     cfg.n_out = 5 if args["model"] == "NISQA_DIM" else 1
-    cfg.n_fft, cfg.n_mels, cfg.seg_len = 4096, 48, 15
+    cfg.n_fft, cfg.n_mels, cfg.seg_len = 4096, n_mels, seg_len
     cfg.seg_hop = int(args["ms_seg_hop_length"])
     cfg.max_segments = int(args["ms_max_segments"]) if args.get("ms_max_segments") else 0
     cfg.hop_s, cfg.win_s = float(args["ms_hop_length"]), float(args["ms_win_length"])
@@ -334,6 +337,26 @@ def config_from_args(args, max_chunk_segments=0):
         cfg.de_fuse_dim = int(args.get("de_fuse_dim") or 0)
         cfg.de_align, cfg.de_align_apply, cfg.de_fuse = DE_ALIGN[args["de_align"]], DE_APPLY[args["de_align_apply"]], DE_FUSE[args["de_fuse"]]
     return cfg
+
+
+def _check_mel_shape(args, standard):
+    """(n_mels, seg_len) of the checkpoint's Mel-spectrogram segments; refuses what the kernels do not implement, naming
+    the value"""
+    n_fft, n_mels, seg_len = args.get("ms_n_fft"), args.get("ms_n_mels"), args.get("ms_seg_length")
+    if n_fft != 4096:
+        raise NotImplementedError("ms_n_fft=%r: the engine's front end runs n_fft 4096 (four 1024-point FFTs)" % (n_fft,))
+    if n_mels not in N_MELS or int(n_mels) != n_mels:
+        raise NotImplementedError("ms_n_mels=%r: the engine runs %s Mel bands" % (n_mels, ", ".join(map(str, N_MELS))))
+    if seg_len is None or int(seg_len) != seg_len or not SEG_LEN_MIN <= seg_len <= SEG_LEN_MAX:
+        raise NotImplementedError("ms_seg_length=%r: the engine runs segments of %d to %d frames" % (seg_len, SEG_LEN_MIN, SEG_LEN_MAX))
+    if seg_len % 2 == 0:
+        raise NotImplementedError("ms_seg_length=%r: the reference's segment_specs refuses even segment lengths "
+                                  "(seg_length must be odd)" % (seg_len,))
+    if standard and (n_mels, seg_len) != (48, 15):
+        raise NotImplementedError("ms_n_mels=%r, ms_seg_length=%r with cnn_model='standard': the reference's StandardCNN "
+                                  "hard-codes output_height = 6, output_width = 2 (48 x 15 segments); use cnn_model='adapt'"
+                                  % (n_mels, seg_len))
+    return int(n_mels), int(seg_len)
 
 
 def _fan_out_args(args, stage):
