@@ -97,12 +97,13 @@ enum nisqa_status {
 /* stages readable through nisqa_stage_dump after a predict call (parity tests) */
 enum nisqa_stage {
   NISQA_STAGE_MEL_DB   = 0, /* per clip [n_mels, n_frames] row-major, clamped (lib:2330), clips concatenated */
-  NISQA_STAGE_POOL1    = 1, /* [n_seg, 16, 24, W1] NCHW like the reference tensors           */
-  NISQA_STAGE_POOL2    = 2, /* [n_seg, 32, 12, W2]                                           */
-  NISQA_STAGE_CONV3    = 3, /* [n_seg, 64, 12, W2]                                           */
-  NISQA_STAGE_POOL3    = 4, /* [n_seg, 64, 6, W3]                                            */
-  NISQA_STAGE_CONV5    = 5, /* [n_seg, 64, 6, W3]                                            */
-  NISQA_STAGE_CNN_FEAT = 6, /* [n_seg, 384] (adapt, index c*6+h) or [n_seg, F] (standard: fc_out's width F, or 768 in
+  NISQA_STAGE_POOL1    = 1, /* [n_seg, c1, 24, W1] NCHW like the reference tensors (c1..c3: cnn_c_out_1..3,
+                             * read from the weights; StandardCNN 16, 32, 64)                                          */
+  NISQA_STAGE_POOL2    = 2, /* [n_seg, c2, 12, W2]                                           */
+  NISQA_STAGE_CONV3    = 3, /* [n_seg, c3, 12, W2]                                           */
+  NISQA_STAGE_POOL3    = 4, /* [n_seg, c3, 6, W3]                                            */
+  NISQA_STAGE_CONV5    = 5, /* [n_seg, c3, 6, W3]                                            */
+  NISQA_STAGE_CNN_FEAT = 6, /* [n_seg, 6*c3] (adapt, index c*6+h) or [n_seg, F] (standard: fc_out's width F, or 768 in
                              * index c*12+h*2+w without fc_out)                                                        */
   NISQA_STAGE_TD_IN    = 7, /* the input LayerNorm output of the first self-attention stack that runs (td's, or td_2's
                              * behind an LSTM td or no td): LayerNorm(Linear(in -> D)) [n_seg, D]; not available without one */

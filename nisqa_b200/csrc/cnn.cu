@@ -15,6 +15,7 @@
 #include "common.cuh"
 #include "tc_ptx.cuh"
 #include "conv1_cell.cuh"
+#include "conv_split.cuh"
 #include "launch.cuh"
 
 namespace nisqa {
@@ -24,21 +25,22 @@ namespace nisqa {
 //   MODE 0 (adapt, lib:690-691): adaptive_max_pool2d n_mels x seg_len -> 24x7 (conv1_adapt_cell; 48x15: rows {2i,2i+1},
 //          cols [2j,2j+3))
 //   MODE 1 (standard, lib:813-814): MaxPool2d(2, stride 2, padding (0,1)) -> 24x8 : cols {2j-1,2j} (48 x 15 only)
-// thread = one pooled cell of one segment, all 16 channels.
+// thread = one pooled cell of one segment, all C1 channels (16, 32 or 64 for AdaptCNN, in groups of 16).
 // SPLIT: the output goes out as the two fp16 planes conv2's tensor-core kernel consumes (conv_split.cu:
-// padded rows of 16 halves = 32 bytes, 32-byte swizzle) instead of fp32 channels-last.
+// padded rows of C1 halves = 2 C1 bytes, swizzled) instead of fp32 channels-last (C1 = 16 only).
 // (__launch_bounds__ minimum of 2 CTAs: without it ptxas holds the AdaptCNN cell at 80 registers and spills)
-template <int MODE, bool SPLIT>
+template <int MODE, bool SPLIT, int C1 = 16>
 __global__ void __launch_bounds__(256, 2)
 conv1_pool1_kernel(const float* __restrict__ mel, int n_mels, int seg_len, const int* __restrict__ seg_frame0,
-                   const float* __restrict__ seg_thr, const float* __restrict__ w1 /*[9][16]*/,
-                   const float* __restrict__ b1 /*[16]*/, float* __restrict__ out,
+                   const float* __restrict__ seg_thr, const float* __restrict__ w1 /*[9][C1]*/,
+                   const float* __restrict__ b1 /*[C1]*/, float* __restrict__ out,
                    unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo,
                    float store_scale /*2^-e1*/, int n_seg) {
+  static_assert(C1 == 16 || (MODE == 0 && SPLIT), "StandardCNN and the fp32 output: 16 channels");
   constexpr int PW = (MODE == 0) ? 7 : 8;
-  __shared__ __align__(16) float ws[9 * 16 + 16];
-  for (int i = threadIdx.x; i < 9 * 16 + 16; i += blockDim.x)
-    ws[i] = (i < 144) ? __ldg(w1 + i) : __ldg(b1 + i - 144);
+  __shared__ __align__(16) float ws[9 * C1 + C1];
+  for (int i = threadIdx.x; i < 9 * C1 + C1; i += blockDim.x)
+    ws[i] = (i < 9 * C1) ? __ldg(w1 + i) : __ldg(b1 + i - 9 * C1);
   __syncthreads();
 
   const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -49,22 +51,30 @@ conv1_pool1_kernel(const float* __restrict__ mel, int n_mels, int seg_len, const
   const int f0 = __ldg(seg_frame0 + seg);
   const float thr = __ldg(seg_thr + seg);
 
-  float res[16];
-  if constexpr (MODE == 0) conv1_adapt_cell(mel + (size_t)f0 * n_mels, n_mels, seg_len, thr, ws, ph, pw, res);
-  else conv1_cell<MODE>(mel, f0, thr, ws, ph, pw, res);
-  if constexpr (SPLIT) {
+  // channels 16 cg .. 16 cg + 15 -> the two 16-byte chunks 2 cg, 2 cg + 1 of the cell's plane row
+  auto store_split = [&](const float (&res)[16], int cg) {
     const int g = kSplitLead + seg * (25 * (PW + 1)) + (ph + 1) * (PW + 1) + (pw + 1);
 #pragma unroll
     for (int c = 0; c < 2; ++c) {
       uint4 hi, lo;
       split8(make_float4(res[8 * c], res[8 * c + 1], res[8 * c + 2], res[8 * c + 3]),
              make_float4(res[8 * c + 4], res[8 * c + 5], res[8 * c + 6], res[8 * c + 7]), store_scale, hi, lo);
-      size_t o = (size_t)g * 32 + (size_t)c * 16;
-      o ^= (o >> 3) & 16;                          // Swizzle<1,4,3>
+      const size_t o = split_off<2 * C1>(g, 2 * cg + c);
       *reinterpret_cast<uint4*>(out_hi + o) = hi;
       *reinterpret_cast<uint4*>(out_lo + o) = lo;
     }
+  };
+  float res[16];
+  if constexpr (MODE == 0) {
+    for (int cg = 0; cg < C1 / 16; ++cg) {     // one group of 16 channels at a time (the registers of one cell)
+      conv1_adapt_cell<C1>(mel + (size_t)f0 * n_mels, n_mels, seg_len, thr, ws, ph, pw, 16 * cg, res);
+      if constexpr (SPLIT) store_split(res, cg);
+    }
   } else {
+    conv1_cell<MODE>(mel, f0, thr, ws, ph, pw, res);
+    if constexpr (SPLIT) store_split(res, 0);
+  }
+  if constexpr (!SPLIT) {
     float4* o = reinterpret_cast<float4*>(out + ((size_t)seg * 24 * PW + ph * PW + pw) * 16);
 #pragma unroll
     for (int q = 0; q < 4; ++q)
@@ -232,8 +242,8 @@ conv3x3_kernel(const float* __restrict__ in, const float* __restrict__ wpack /*[
   }
 }
 
-// NHWC [n][HW][C] -> NCHW [n][C][HW] (stage dumps only; matches the reference tensor layout)
-__global__ void nhwc_to_nchw_kernel(const float* __restrict__ in, float* __restrict__ out,
+// NHWC [n][HW][C] (rows of ld floats) -> NCHW [n][C][HW] (stage dumps only; matches the reference tensor layout)
+__global__ void nhwc_to_nchw_kernel(const float* __restrict__ in, int ld, float* __restrict__ out,
                                     long long n, int hw, int ch) {
   const long long total = n * hw * ch;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -241,7 +251,7 @@ __global__ void nhwc_to_nchw_kernel(const float* __restrict__ in, float* __restr
     const int p = (int)(i % hw);
     const int c = (int)((i / hw) % ch);
     const long long s = i / ((long long)hw * ch);
-    out[i] = in[(s * hw + p) * ch + c];
+    out[i] = in[s * ld + p * ch + c];
   }
 }
 
@@ -274,9 +284,10 @@ static void launch_conv(cudaStream_t st, const float* in, const float* w, const 
   conv3x3_kernel<C><<<grid, C::NT, C::SMEM_BYTES, st>>>(in, w, b, out, n_seg);
 }
 
-void launch_conv1(cudaStream_t st, int std_mode, const float* mel, int n_mels, int seg_len, const int* seg_frame0,
+bool launch_conv1(cudaStream_t st, int std_mode, int c1, const float* mel, int n_mels, int seg_len, const int* seg_frame0,
                   const float* seg_thr, const float* w1, const float* b1, float* out, int n_seg, void* out_hi, void* out_lo,
                   float store_scale) {
+  if (c1 != 16 && (std_mode || !out_hi || (c1 != 32 && c1 != 64))) return false;
   const int cells = std_mode ? 24 * 8 : 24 * 7;
   const long long total = (long long)n_seg * cells;
   const int grid = (int)((total + 255) / 256);
@@ -286,11 +297,14 @@ void launch_conv1(cudaStream_t st, int std_mode, const float* mel, int n_mels, i
   const int H = n_mels, W = seg_len;
   if (out_hi) {
     if (std_mode) conv1_pool1_kernel<1, true><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
+    else if (c1 == 32) conv1_pool1_kernel<0, true, 32><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
+    else if (c1 == 64) conv1_pool1_kernel<0, true, 64><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
     else conv1_pool1_kernel<0, true><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
   } else {
     if (std_mode) conv1_pool1_kernel<1, false><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
     else conv1_pool1_kernel<0, false><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
   }
+  return true;
 }
 
 // layer = 2..6
@@ -315,8 +329,8 @@ void launch_conv_layer(cudaStream_t st, int std_mode, int layer, const float* in
   }
 }
 
-void launch_nhwc_to_nchw(cudaStream_t st, const float* in, float* out, long long n, int hw, int ch) {
-  nhwc_to_nchw_kernel<<<1024, 256, 0, st>>>(in, out, n, hw, ch);
+void launch_nhwc_to_nchw(cudaStream_t st, const float* in, int ld, float* out, long long n, int hw, int ch) {
+  nhwc_to_nchw_kernel<<<1024, 256, 0, st>>>(in, ld, out, n, hw, ch);
 }
 
 }  // namespace nisqa

@@ -1,5 +1,6 @@
 // conv1_cell.cuh - conv1(1->16) + BN + ReLU fused with the first max-pool for ONE pooled cell of one segment (all 16
 // channels), for conv1_pool1_kernel (cnn.cu), and the strip form of the fused conv1 + conv2 kernel (conv_split.cu).
+// conv1_adapt_cell takes 16 of the C1 = 16 / 32 / 64 channels of an AdaptCNN conv1 (cnn_c_out_1) at a time.
 //   MODE 0 (adapt, reference lib:690-691): adaptive_max_pool2d 48x15 -> 24x7 : rows {2i,2i+1}, cols [2j,2j+3)
 //   MODE 1 (standard, lib:813-814): MaxPool2d(2, stride 2, padding (0,1)) -> 24x8 : cols {2j-1,2j}
 //   conv1_adapt_cell: AdaptCNN at any n_mels x seg_len (adaptive windows from the runtime shape)
@@ -119,13 +120,14 @@ __device__ __forceinline__ void conv1_cell(const float* __restrict__ mel, int f0
 }
 #endif
 
-// AdaptCNN conv1 + BN + ReLU + adaptive_max_pool2d to 24 x 7 for one pooled cell (ph, pw), all 16 channels, of a segment
-// of H mel rows x W frames (seg: its frame 0, rows H floats apart).  The cell's window (F.adaptive_max_pool2d) is conv rows
+// AdaptCNN conv1 + BN + ReLU + adaptive_max_pool2d to 24 x 7 for one pooled cell (ph, pw), channels c0 .. c0 + 15 of C1,
+// of a segment of H mel rows x W frames (seg: its frame 0, rows H floats apart; ws: [9][C1] weights, then C1 biases).  The cell's window (F.adaptive_max_pool2d) is conv rows
 // [floor(ph H / 24), ceil((ph + 1) H / 24)) x columns [floor(pw W / 7), ceil((pw + 1) W / 7)).  Each conv position is the
 // fmaf chain of conv1_cell (zero start, taps 0..8, inputs clamped at thr, zero outside the segment), each cell the max,
 // + bias, ReLU: at 48 x 15 the windows are conv1_cell<0>'s and the results bit-identical to it and to conv1_strip.
+template <int C1>
 __device__ __forceinline__ void conv1_adapt_cell(const float* __restrict__ seg, int H, int W, float thr, const float* ws,
-                                                 int ph, int pw, float (&res)[16]) {
+                                                 int ph, int pw, int c0, float (&res)[16]) {
   const int y0 = (ph * H) / 24, y1 = ((ph + 1) * H + 23) / 24;
   const int x0 = (pw * W) / 7, x1 = ((pw + 1) * W + 6) / 7;
   float mx[16];
@@ -145,12 +147,12 @@ __device__ __forceinline__ void conv1_adapt_cell(const float* __restrict__ seg, 
 #pragma unroll
       for (int tap = 0; tap < 9; ++tap)
 #pragma unroll
-        for (int c = 0; c < 16; ++c) acc[c] = fmaf(a[tap], ws[tap * 16 + c], acc[c]);
+        for (int c = 0; c < 16; ++c) acc[c] = fmaf(a[tap], ws[tap * C1 + c0 + c], acc[c]);
 #pragma unroll
       for (int c = 0; c < 16; ++c) mx[c] = fmaxf(mx[c], acc[c]);
     }
 #pragma unroll
-  for (int c = 0; c < 16; ++c) res[c] = fmaxf(mx[c] + ws[144 + c], 0.f);   // bias + ReLU commute with max
+  for (int c = 0; c < 16; ++c) res[c] = fmaxf(mx[c] + ws[9 * C1 + c0 + c], 0.f);   // bias + ReLU commute with max
 }
 
 // Pooled cells PW0 .. PW1 - 1 of pooled row ph for the 4 channels of one quad, with every conv1 output position computed

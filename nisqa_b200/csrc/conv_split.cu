@@ -55,10 +55,12 @@ namespace nisqa {
 // ---- pieces shared by the two kernels ----
 
 // The K steps of one tap go to the tensor cores in units of UK k16 steps: a whole tap for CIN <= 32, half a tap for
-// CIN 64 (two fragment sets of a whole 64-channel tap do not fit beside the accumulators in 128 registers).
+// CIN 64 (two fragment sets of a whole 64-channel tap do not fit beside the accumulators in 128 registers).  conv2 at
+// 64 output channels (24 x 7 maps) takes one k16 step per unit: with two, ptxas spills (CIN 32: 16 bytes, CIN 64: 72).
 template <class C>
 struct TapUnits {
-  static constexpr int KS = C::CIN / 16, UK = KS < 2 ? KS : 2, PER_TAP = KS / UK, N = 9 * PER_TAP;
+  static constexpr int KS = C::CIN / 16, UK = (KS < 2 || (C::H == 24 && C::COUT == 64)) ? 1 : 2, PER_TAP = KS / UK,
+                       N = 9 * PER_TAP;
 };
 
 // A fragments of K steps k0 .. k0 + UK - 1 of one tap (row offset tapoff) for this warpgroup's NB m64 blocks: block b
@@ -209,7 +211,7 @@ __device__ __forceinline__ void store_tile(const float* stg, int seg0, int nvali
       *reinterpret_cast<uint4*>(out_lo + o) = lo;
     }
   } else {
-    // fp32 CNN features, channels-last [seg][HO][WO][COUT]
+    // fp32 CNN features, channels-last [seg][HO][WO][COUT] in rows of OUT_LD floats
     constexpr int HO = C::HO, WO = C::WO, C4 = COUT / 4;
     for (int i = t0; i < nvalid * HO * WO * C4; i += nthr) {
       const int c4 = i % C4;
@@ -218,17 +220,26 @@ __device__ __forceinline__ void store_tile(const float* stg, int seg0, int nvali
       const int h = rest % HO;
       const int s = rest / HO;
       const int r = s * BLK + (h + 1) * P + (C::CENTER ? 2 : w + 1);
-      *reinterpret_cast<float4*>(out_f32 + ((size_t)(seg0 + s) * (HO * WO) + h * WO + w) * COUT + c4 * 4) =
-          *reinterpret_cast<const float4*>(stg + r * SS + c4 * 4);
+      float* dst = C::OUT_LD == C::OUT_COLS ? out_f32 + ((size_t)(seg0 + s) * (HO * WO) + h * WO + w) * COUT + c4 * 4
+                                            : out_f32 + (size_t)(seg0 + s) * C::OUT_LD + (h * WO + w) * COUT + c4 * 4;
+      *reinterpret_cast<float4*>(dst) = *reinterpret_cast<const float4*>(stg + r * SS + c4 * 4);
+    }
+    if constexpr (C::OUT_LD > C::OUT_COLS) {
+      // the padding columns are written as zeros: the Linear behind reads them (against zero weights)
+      constexpr int PAD4 = (C::OUT_LD - C::OUT_COLS) / 4;
+      for (int i = t0; i < nvalid * PAD4; i += nthr)
+        *reinterpret_cast<float4*>(out_f32 + (size_t)(seg0 + i / PAD4) * C::OUT_LD + C::OUT_COLS + (i % PAD4) * 4) =
+            make_float4(0.f, 0.f, 0.f, 0.f);
     }
   }
 }
 
 // ---- conv2..conv6 on planes ----
 // Warpgroup b < NBLK owns m64 block b (3 blocks, 1 for conv6A) and runs GEMM and epilogue part 1; all four run part 2.
-// One warpgroup's wgmmas already use the tensor cores of all four SM sub-partitions.  Without aliasing (conv2, conv3)
-// the activation tile is double-buffered: one thread issues the next tile's copy into the other buffer as soon as
-// that buffer's readers (the previous tile's GEMM) have arrived on its empty barrier.
+// One warpgroup's wgmmas already use the tensor cores of all four SM sub-partitions.  With two activation buffers (the
+// shipped conv2, conv3) one thread issues the next tile's copy into the other buffer as soon as that buffer's readers
+// (the previous tile's GEMM) have arrived on its empty barrier; with one unaliased buffer (CIN 64 -> COUT 32) it issues
+// the copy once this tile's GEMM is done, so that it lands during the epilogue.
 template <class C>
 __global__ void __launch_bounds__(C::NT, 1)
 conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* __restrict__ in_lo,
@@ -259,8 +270,8 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
   if (tid == 0) {
     for (int t = 0; t < 9; ++t) mbar_init(bar_w + 8 * t, 1);
     for (int b = 0; b < C::A_BUFS; ++b) mbar_init(bar_full + 8 * b, 1);
-    if constexpr (!C::ALIAS)
-      for (int b = 0; b < C::A_BUFS; ++b) mbar_init(bar_empty + 8 * b, NT);
+    if constexpr (C::A_BUFS == 2)
+      for (int b = 0; b < 2; ++b) mbar_init(bar_empty + 8 * b, NT);
     fence_barrier_init();
     for (int t = 0; t < 9; ++t) {                // all nine taps stay resident; tap t's MMAs start once it has landed
       mbar_expect_tx(bar_w + 8 * t, C::B_STAGE);
@@ -280,10 +291,12 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
     const int seg0 = tile * G;
     const int g0 = kSplitLead + seg0 * BLK - HALO;         // first plane row of this tile
-    const int ab = C::ALIAS ? 0 : (it & 1);
+    const int ab = C::A_BUFS == 1 ? 0 : (it & 1);
     if constexpr (C::ALIAS) {
       if (tid == 0) issue_tile(tile, 0);
       mbar_wait(bar_full, it & 1);
+    } else if constexpr (C::A_BUFS == 1) {
+      mbar_wait(bar_full, it & 1);               // issued by the prologue or the previous tile
     } else {
       const int next = tile + gridDim.x;
       if (tid == 0 && next < n_tiles) {
@@ -306,9 +319,12 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
       wait_weights(bar_w);
       tile_gemm<C, 1>(acc_m, acc_s, a_hi, a_lo, b_base, row, lchunk);
     }
-    if constexpr (!C::ALIAS) mbar_arrive(bar_empty + 8 * ab);
+    if constexpr (C::A_BUFS == 2) mbar_arrive(bar_empty + 8 * ab);
     __syncthreads();                             // ALIAS: every warpgroup is done with the A tile the staging tile
                                                  // overwrites; otherwise the previous tile's part 2 is done with it
+    if constexpr (!C::ALIAS && C::A_BUFS == 1) {
+      if (tid == 0 && tile + (int)gridDim.x < n_tiles) issue_tile(tile + gridDim.x, 0);   // the GEMM is done with it
+    }
 
     // ===== epilogue part 1: accumulators -> bias + ReLU -> staging row of each GEMM row's plane position =====
     float2 bb[C::COUT / 8];
@@ -558,22 +574,27 @@ static void launch_c12(cudaStream_t st, const __half* wtc, const float* b, float
                                                                       mel, seg_frame0, seg_thr, w1, b1, c1_scale);
 }
 
-static_assert(input_is<SpConv2A>(0, 2) && input_is<SpConv3A>(0, 3) && input_is<SpConv4A>(0, 4) &&
-              input_is<SpConv5A>(0, 5) && input_is<SpConv6A>(0, 6) && input_is<SpConv2S>(1, 2) &&
-              input_is<SpConv3S>(1, 3) && input_is<SpConv4S>(1, 4) && input_is<SpConv5S>(1, 5) &&
+#define NISQA_SP_GEOM(L, CI, CO) static_assert(input_is<SpAdapt<L, CI, CO>>(0, L), "SpCfg geometry differs from split_geometry");
+NISQA_SP_ADAPT_LAYERS(NISQA_SP_GEOM)
+#undef NISQA_SP_GEOM
+static_assert(input_is<SpConv2S>(1, 2) && input_is<SpConv3S>(1, 3) && input_is<SpConv4S>(1, 4) && input_is<SpConv5S>(1, 5) &&
               input_is<SpConv6S>(1, 6), "SpCfg geometry differs from split_geometry");
 
-// Bytes of one plane of the pair that feeds conv layer `layer` (2..6) for n_seg segments: per segment (H + 1) rows of
-// W + 1 pixels (shared zero row / column), the zero lead rows and the tile over-read.
-size_t split_plane_bytes(int std_mode, int layer, int n_seg) {
-  const ConvGeom g = split_geometry(std_mode, layer);
+// Bytes of one plane of the pair that feeds conv layer `layer` (2..6) with C channels for n_seg segments: per segment
+// (H + 1) rows of W + 1 pixels (shared zero row / column), the zero lead rows and the tile over-read.
+size_t split_plane_bytes(int std_mode, int layer, int C, int n_seg) {
+  const ConvGeom g = split_geometry(std_mode, layer, C);
   const size_t rows = (size_t)kSplitLead + (size_t)n_seg * (g.H + 1) * (g.W + 1) + 256 + 32;
   return (rows * (size_t)g.C * 2 + 1023) & ~(size_t)1023;
 }
 
-// conv layer 2..6 on planes; the last layer (6) writes the fp32 CNN features (adapt: [seg][6][64];
-// standard: [seg][6][2][64])
-void launch_conv_split(cudaStream_t st, int std_mode, int layer, const void* in_hi, const void* in_lo,
+bool conv_split_supported(int cin, int cout) {
+  return (cin == 16 || cin == 32 || cin == 64) && (cout == 16 || cout == 32 || cout == 64);
+}
+
+// conv layer 2..6 (cin -> cout channels) on planes; the last layer (6) writes the fp32 CNN features (adapt:
+// [seg][6][c3] in rows padded to a multiple of 64 floats; standard: [seg][6][2][64]).  false: no instance for the shape.
+bool launch_conv_split(cudaStream_t st, int std_mode, int layer, int cin, int cout, const void* in_hi, const void* in_lo,
                        const void* wtc, const float* b, float out_scale, float store_scale, void* out_hi,
                        void* out_lo, float* out_f32, int n_seg) {
   const __half* w = reinterpret_cast<const __half*>(wtc);
@@ -582,26 +603,30 @@ void launch_conv_split(cudaStream_t st, int std_mode, int layer, const void* in_
   unsigned char* oh = static_cast<unsigned char*>(out_hi);
   unsigned char* ol = static_cast<unsigned char*>(out_lo);
   if (!std_mode) {
-    switch (layer) {
-      case 2: launch_sp<SpConv2A>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 3: launch_sp<SpConv3A>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 4: launch_sp<SpConv4A>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 5: launch_sp<SpConv5A>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      default: launch_sp<SpConv6A>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+#define NISQA_SP_LAUNCH(L, CI, CO)                                                                           \
+    if (layer == L && cin == CI && cout == CO) {                                                              \
+      launch_sp<SpAdapt<L, CI, CO>>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg);        \
+      return true;                                                                                            \
     }
-  } else {
-    switch (layer) {
-      case 2: launch_sp<SpConv2S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 3: launch_sp<SpConv3S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 4: launch_sp<SpConv4S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 5: launch_sp<SpConv5S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      default: launch_sp<SpConv6S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-    }
+    NISQA_SP_ADAPT_LAYERS(NISQA_SP_LAUNCH)
+#undef NISQA_SP_LAUNCH
+    return false;
   }
+  if (cin != split_geometry(1, layer, 0).C || cout != (layer == 2 ? 32 : 64)) return false;
+  switch (layer) {
+    case 2: launch_sp<SpConv2S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+    case 3: launch_sp<SpConv3S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+    case 4: launch_sp<SpConv4S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+    case 5: launch_sp<SpConv5S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+    default: launch_sp<SpConv6S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+  }
+  return true;
 }
 
-// conv1 + pool1 + conv2 + pool2 in one kernel: mel segments -> the plane pair feeding conv3
-void launch_conv12(cudaStream_t st, int std_mode, const float* mel, const int* seg_frame0, const float* seg_thr,
+bool conv12_supported(int std_mode, int c1, int c2) { return c1 == 16 && (c2 == 32 || (!std_mode && c2 == 16)); }
+
+// conv1 + pool1 + conv2 + pool2 in one kernel: mel segments -> the plane pair feeding conv3 (conv12_supported shapes)
+void launch_conv12(cudaStream_t st, int std_mode, int c2, const float* mel, const int* seg_frame0, const float* seg_thr,
                    const float* w1, const float* b1, float c1_scale, const void* wtc2, const float* bias2,
                    float scale2, float store_scale, void* out_hi, void* out_lo, int n_seg) {
   const __half* w = reinterpret_cast<const __half*>(wtc2);
@@ -609,13 +634,15 @@ void launch_conv12(cudaStream_t st, int std_mode, const float* mel, const int* s
   unsigned char* ol = static_cast<unsigned char*>(out_lo);
   if (std_mode)
     launch_c12<SpConv2S, 1>(st, w, bias2, scale2, store_scale, oh, ol, n_seg, mel, seg_frame0, seg_thr, w1, b1, c1_scale);
+  else if (c2 == 16)
+    launch_c12<SpAdapt<2, 16, 16>, 0>(st, w, bias2, scale2, store_scale, oh, ol, n_seg, mel, seg_frame0, seg_thr, w1, b1, c1_scale);
   else
     launch_c12<SpConv2A, 0>(st, w, bias2, scale2, store_scale, oh, ol, n_seg, mel, seg_frame0, seg_thr, w1, b1, c1_scale);
 }
 
-void launch_unsplit(cudaStream_t st, int std_mode, int layer, const void* hi, const void* lo, float unit, float* out,
+void launch_unsplit(cudaStream_t st, int std_mode, int layer, int C, const void* hi, const void* lo, float unit, float* out,
                     int n_seg) {
-  const ConvGeom g = split_geometry(std_mode, layer);
+  const ConvGeom g = split_geometry(std_mode, layer, C);
   const long long items = (long long)n_seg * g.H * g.W * (g.C / 8);
   const unsigned char* h = static_cast<const unsigned char*>(hi);
   const unsigned char* l = static_cast<const unsigned char*>(lo);

@@ -3,6 +3,8 @@
 #pragma once
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "tc_ptx.cuh"
 
@@ -52,16 +54,20 @@ struct SpCfg {
   static constexpr int HO = (POOL == SP_POOL_NONE) ? H : H / 2;
   static constexpr int WO = (POOL == SP_POOL_NONE) ? (CENTER ? 1 : W) : POW;
   static constexpr int OP = WO + 1, OBLK = (HO + 1) * OP, OROWB = COUT * 2;
+  // fp32 output (the CNN features): one row per segment, zero-padded to a multiple of 64 columns (6 x 16 -> 128)
+  static constexpr int OUT_COLS = HO * WO * COUT, OUT_LD = (OUT_COLS + 63) / 64 * 64;
   // epilogue staging: one fp32 row per GEMM row (bias + ReLU applied)
   static constexpr int STG_STRIDE = COUT + 4;
   static constexpr int STG_BYTES = 256 * STG_STRIDE * 4;
-  // the staging tile reuses the activation tile when both do not fit beside the nine resident weight taps
+  // Three ways to fit beside the nine resident weight taps, the first that fits: the activation tile double-buffered
+  // (the next tile's copy lands during this tile's GEMM and epilogue), one activation buffer beside the staging tile (the
+  // next tile's copy lands during this tile's epilogue), or one buffer that the staging tile reuses (ALIAS: the copy
+  // waits for the epilogue).  Buffer b: hi plane at b * A_BUF, lo plane at b * A_BUF + A_BYTES.
   static constexpr int SMEM_BUDGET = 227 * 1024 - 2048;
-  static constexpr bool ALIAS = 2 * A_BYTES + STG_BYTES + 9 * B_STAGE > SMEM_BUDGET;
-  // without aliasing the activation tile is double-buffered: the next tile's copy lands during this tile's GEMM and
-  // epilogue.  Buffer b: hi plane at b * A_BUF, lo plane at b * A_BUF + A_BYTES.
-  static constexpr int A_BUFS = ALIAS ? 1 : 2;
   static constexpr int A_BUF = 2 * A_BYTES;
+  static constexpr int ONE_BUF = A_BUF + STG_BYTES + 9 * B_STAGE;     // one unaliased activation buffer
+  static constexpr bool ALIAS = ONE_BUF > SMEM_BUDGET;
+  static constexpr int A_BUFS = (ALIAS || ONE_BUF + A_BUF > SMEM_BUDGET) ? 1 : 2;
   static constexpr int OFF_A_HI = 0;
   static constexpr int OFF_A_LO = A_BYTES;
   static constexpr int OFF_STG = ALIAS ? 0 : A_BUFS * A_BUF;
@@ -69,12 +75,12 @@ struct SpCfg {
   static constexpr int OFF_W1 = OFF_B + 9 * B_STAGE;      // conv1 weights [9][16] + biases [16] (fused conv1 + conv2 only)
   // 9 weight-tap barriers, then a full barrier per activation buffer, then (double-buffered) an empty barrier per buffer
   static constexpr int OFF_BAR = OFF_W1 + 1024;
-  static constexpr int NBAR = ALIAS ? 10 : 13;
+  static constexpr int NBAR = 9 + 2 * A_BUFS;
   static constexpr int SMEM_BYTES = OFF_BAR + 8 * NBAR + 1024;    // + slack: the tile is aligned to 1024 B
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
   static_assert(ALIAS || A_BUFS * A_BUF + STG_BYTES + 9 * B_STAGE <= SMEM_BUDGET,
-                "both activation buffers fit beside the staging tile and the weights");
-  static_assert(B_STAGE % 16 == 0 && CIN % 16 == 0 && (COUT == 32 || COUT == 64), "shape");
+                "the activation buffers fit beside the staging tile and the weights");
+  static_assert(B_STAGE % 16 == 0 && CIN % 16 == 0 && (COUT == 16 || COUT == 32 || COUT == 64), "shape");
   static_assert(ROWB == 32 || ROWB == 64 || ROWB == 128, "rows are 32 / 64 / 128 bytes (one swizzle atom)");
   static_assert(HALO <= kSplitLead, "kSplitLead");
   static_assert(!CENTER || F32OUT_, "the centre-column variant only exists as the last layer");
@@ -83,13 +89,32 @@ struct SpCfg {
   static_assert(NBLK <= 4 && (!CENTER || W == 3), "GEMM rows");
 };
 
-// layers 2..6; std_mode selects the StandardCNN geometry (W 8/4/2, MaxPool2d(2))
-//                     H   W  CIN COUT POOL           POW F32OUT CENTER
+// Layers 2..6.  AdaptCNN: one instance per (layer, CIN, COUT) that cnn_c_out_1/2/3 in {16, 32, 64} reach - conv2
+// c1 -> c2, conv3 c2 -> c3, conv4..conv6 c3 -> c3 (NISQA_SP_ADAPT_LAYERS lists them, conv_split.cu instantiates them).
+// StandardCNN: the shipped 16 / 32 / 64 channels, std_mode selects its geometry (W 8/4/2, MaxPool2d(2)).
+template <int L, int CIN, int COUT> struct SpAdaptLayer;
+//                                                                H   W  CIN COUT POOL           POW F32OUT CENTER
+template <int CIN, int COUT> struct SpAdaptLayer<2, CIN, COUT> { using T = SpCfg<24, 7, CIN, COUT, SP_POOL_ADAPT, 5>; };
+template <int CIN, int COUT> struct SpAdaptLayer<3, CIN, COUT> { using T = SpCfg<12, 5, CIN, COUT, SP_POOL_NONE, 0>; };
+template <int CIN, int COUT> struct SpAdaptLayer<4, CIN, COUT> { using T = SpCfg<12, 5, CIN, COUT, SP_POOL_ADAPT, 3>; };
+template <int CIN, int COUT> struct SpAdaptLayer<5, CIN, COUT> { using T = SpCfg<6, 3, CIN, COUT, SP_POOL_NONE, 0>; };
+template <int CIN, int COUT> struct SpAdaptLayer<6, CIN, COUT> { using T = SpCfg<6, 3, CIN, COUT, SP_POOL_NONE, 0, true, true>; };
+template <int L, int CIN, int COUT> using SpAdapt = typename SpAdaptLayer<L, CIN, COUT>::T;
+// X(layer, CIN, COUT) for every AdaptCNN instance
+#define NISQA_SP_ANY_TO(X, L, CO) X(L, 16, CO) X(L, 32, CO) X(L, 64, CO)
+#define NISQA_SP_ADAPT_LAYERS(X)                                                                   \
+  NISQA_SP_ANY_TO(X, 2, 16) NISQA_SP_ANY_TO(X, 2, 32) NISQA_SP_ANY_TO(X, 2, 64)                   \
+  NISQA_SP_ANY_TO(X, 3, 16) NISQA_SP_ANY_TO(X, 3, 32) NISQA_SP_ANY_TO(X, 3, 64)                   \
+  X(4, 16, 16) X(4, 32, 32) X(4, 64, 64) X(5, 16, 16) X(5, 32, 32) X(5, 64, 64) X(6, 16, 16) X(6, 32, 32) X(6, 64, 64)
+// the shipped 16 / 32 / 64 AdaptCNN (the same types as SpAdapt's)
 using SpConv2A = SpCfg<24, 7, 16, 32, SP_POOL_ADAPT, 5>;
 using SpConv3A = SpCfg<12, 5, 32, 64, SP_POOL_NONE, 0>;
 using SpConv4A = SpCfg<12, 5, 64, 64, SP_POOL_ADAPT, 3>;
 using SpConv5A = SpCfg<6, 3, 64, 64, SP_POOL_NONE, 0>;
 using SpConv6A = SpCfg<6, 3, 64, 64, SP_POOL_NONE, 0, true, true>;
+static_assert(std::is_same<SpConv2A, SpAdapt<2, 16, 32>>::value && std::is_same<SpConv3A, SpAdapt<3, 32, 64>>::value &&
+              std::is_same<SpConv4A, SpAdapt<4, 64, 64>>::value && std::is_same<SpConv5A, SpAdapt<5, 64, 64>>::value &&
+              std::is_same<SpConv6A, SpAdapt<6, 64, 64>>::value, "shipped AdaptCNN layers");
 using SpConv2S = SpCfg<24, 8, 16, 32, SP_POOL_2X2, 4>;
 using SpConv3S = SpCfg<12, 4, 32, 64, SP_POOL_NONE, 0>;
 using SpConv4S = SpCfg<12, 4, 64, 64, SP_POOL_2X2, 2>;

@@ -106,6 +106,7 @@ struct Lane {
   DevBuf act[7];           // act[l]: fp32 channels-last map feeding conv layer l (2..6) on the FFMA path (and stage dumps)
   DevBuf planes[7];        // planes[l]: fp16 hi | lo plane pair feeding conv layer l (2..6), conv_split.cu
   size_t plane_bytes[7] = {0, 0, 0, 0, 0, 0, 0};   // offset of the lo plane inside planes[l] (half of the allocation)
+  int plane_c[7] = {0, 0, 0, 0, 0, 0, 0};          // channels per row planes[l] was zeroed for (its zero rows / columns)
   void release() {
     for (auto& b : act) b.release();
     for (auto& b : planes) b.release();
@@ -158,6 +159,12 @@ struct SaStackWeights {
 };
 struct Weights {
   ConvWeights conv[7];           // conv1..conv6
+  // output channels of conv1..conv6 (cnn_c[0]: the one input channel), read from the checkpoint's tensors: AdaptCNN
+  // c1 / c2 / c3 / c3 / c3 / c3 with each in {16, 32, 64}, StandardCNN 16 / 32 / 64 / 64 / 64 / 64
+  int cnn_c[7] = {1, 16, 32, 64, 64, 64, 64};
+  bool shipped_channels() const { return cnn_c[1] == 16 && cnn_c[2] == 32 && cnn_c[3] == 64; }
+  int feat_cols() const { return 6 * cnn_c[6]; }                  // AdaptCNN's framewise fan-out (lib:706)
+  int feat_ld() const { return (feat_cols() + 63) / 64 * 64; }    // its row stride: zero columns up to a multiple of 64
   const float* ff_bn = nullptr;  // SkipCNN / DFF: BatchNorm2d(1) as (scale, shift)
   Linear ff[4];                  // SkipCNN's Linear, or DFF's four, BatchNorm1d folded in
   Linear ffc;                    // AdaptCNN's Linear behind conv6 (cnn_fc_out_h)
@@ -227,8 +234,11 @@ struct nisqa_engine {
   // SkipCNN / DFF rows: n_mels * seg_len features (x.view(-1, fan_in), lib:520 / 556), zero-padded to a multiple of 64
   int ff_fan_in() const { return cfg.n_mels * cfg.seg_len; }
   int ff_fan_in_pad() const { return (ff_fan_in() + 63) / 64 * 64; }
-  // conv1 + conv2 in one kernel (conv_split.cu): tensor-core path, the shipped 48 x 15 segments only
-  bool fused12() const { return conv_tc != 0 && conv12 != 0 && cfg.n_mels == kMels && cfg.seg_len == kSegLen; }
+  // conv1 + conv2 in one kernel (conv_split.cu): tensor-core path, the shipped 48 x 15 segments, conv1 16 channels wide
+  bool fused12() const {
+    return conv_tc != 0 && conv12 != 0 && cfg.n_mels == kMels && cfg.seg_len == kSegLen &&
+           conv12_supported(std_cnn(), w.cnn_c[1], w.cnn_c[2]);
+  }
   int pool_d() const { return cfg.td2_layers > 0 ? td2_d() : sa_d(); }
 
   // front-end tables
@@ -256,7 +266,7 @@ struct nisqa_engine {
   const float* last_td_out = nullptr;
   int last_td_out_d = 64;       // row width of last_td_out
   int last_td_out_ld = 0;       // its row stride (0: the width)
-  int last_td_out_hw = 0;       // td = 'skip': conv6 features in the engine's order [hw][64] (6 / 12); 0: the reference's
+  int last_td_out_hw = 0;       // td = 'skip': conv6 features in the engine's order [hw][c3] (6 / 12); 0: the reference's
   const float* last_td1_out = nullptr;    // td's output when a td_2 stage ran (NISQA_STAGE_TD1_OUT)
   int last_td1_out_d = 0, last_td1_out_ld = 0;
 
@@ -597,38 +607,60 @@ bool pack_ffnet(Packer& P, const nisqa_config& c) {
   return H == 0 || pack_ff_linear(P, P.w.ff[0], "linear", "", fan_in, fan_pad, H);
 }
 
+// AdaptCNN's channel counts from its tensors: conv1..conv3's output channels c1, c2, c3 (cnn_c_out_1/2/3), each 16, 32
+// or 64 (one fp16 row of a plane pair is one 32 / 64 / 128-byte swizzle atom and a whole number of k16 steps);
+// conv4..conv6 stay at c3 (pack_conv checks their shapes)
+bool read_cnn_channels(Packer& P, int* cc) {
+  for (int i = 1; i <= 3; ++i) {
+    const std::string name = "cnn.model.conv" + std::to_string(i) + ".weight";
+    auto it = P.t.find(name);
+    if (it == P.t.end()) return P.fail("missing tensor " + name);
+    const int co = it->second.nd == 4 ? (int)it->second.dims[0] : 0;
+    if (co != 16 && co != 32 && co != 64)
+      return P.fail("tensor " + name + ": " + std::to_string(co) + " output channels (cnn_c_out_" + std::to_string(i) +
+                    "): the engine runs AdaptCNN channel counts 16, 32 or 64");
+    cc[i] = co;
+  }
+  cc[4] = cc[5] = cc[6] = cc[3];
+  return true;
+}
+
 // The framewise model: AdaptCNN / StandardCNN (fp32 and tensor-core weights, activation scales) with AdaptCNN's optional
 // Linear, or SkipCNN / DFF
 bool pack_framewise(Packer& P, nisqa_engine* e) {
   const nisqa_config& c = e->cfg;
   if (!e->conv_net()) return pack_ffnet(P, c);
-  const int cin[7] = {0, 1, 16, 32, 64, 64, 64}, cout[7] = {0, 16, 32, 64, 64, 64, 64};
+  int* cc = P.w.cnn_c;
+  if (!e->std_cnn() && !read_cnn_channels(P, cc)) return false;
   for (int i = 1; i <= 6; ++i) {
     size_t w_off = 0;
-    if (!pack_conv(P, i, cin[i], cout[i], &e->act_exp[i], &w_off)) return false;
-    if (i >= 2) pack_conv_tc(P, i, cin[i], cout[i], w_off, e->act_exp[i - 1], &e->tc_scale[i]);
+    if (!pack_conv(P, i, cc[i - 1], cc[i], &e->act_exp[i], &w_off)) return false;
+    if (i >= 2) pack_conv_tc(P, i, cc[i - 1], cc[i], w_off, e->act_exp[i - 1], &e->tc_scale[i]);
   }
   if (c.cnn_fc > 0) {
-    // AdaptCNN's optional Linear (lib:682-684, 708-709): k-major, rows in the engine's feature order h*64 + c
-    const int H = c.cnn_fc;
-    const TensorView* w = P.get("cnn.model.fc.weight", {H, 384});
+    // AdaptCNN's optional Linear (lib:682-684, 708-709): k-major, rows in the engine's feature order h*c3 + c, zero rows
+    // up to the padded feature width
+    const int H = c.cnn_fc, C3 = cc[6], K = P.w.feat_cols();
+    const TensorView* w = P.get("cnn.model.fc.weight", {H, K});
     const TensorView* b = P.get("cnn.model.fc.bias", {H});
     if (!w || !b) return false;
-    const size_t ow = P.alloc(P.w.ffc.wT, (size_t)384 * H);
+    const size_t ow = P.alloc(P.w.ffc.wT, (size_t)P.w.feat_ld() * H);
     for (int h = 0; h < 6; ++h)
-      for (int ch = 0; ch < 64; ++ch)
-        for (int j = 0; j < H; ++j) P.arena[ow + ((size_t)h * 64 + ch) * H + j] = w->d[(size_t)j * 384 + ch * 6 + h];
+      for (int ch = 0; ch < C3; ++ch)
+        for (int j = 0; j < H; ++j) P.arena[ow + ((size_t)h * C3 + ch) * H + j] = w->d[(size_t)j * K + ch * 6 + h];
     P.copy(P.w.ffc.b, b->d, H);
   }
   return true;
 }
 
 // The rows that feed a time-dependency stage: `dim` features, padded with zero columns to a multiple of 64, in the order
-// of the checkpoint's Linear (PLAIN) or - conv6's features - in the engine's order: AdaptCNN k' = h*64 + c <-> reference
-// view(-1, 64*6) order c*6 + h (lib:706), StandardCNN k' = (h*2 + w)*64 + c <-> c*12 + h*2 + w (lib:830)
+// of the checkpoint's Linear (PLAIN) or - conv6's `ch` channels - in the engine's order: AdaptCNN k' = h*ch + c <->
+// reference view(-1, ch*6) order c*6 + h (lib:706), StandardCNN k' = (h*2 + w)*64 + c <-> c*12 + h*2 + w (lib:830)
 enum InOrder { IN_PLAIN, IN_ADAPT_CONV, IN_STD_CONV };
-struct InRows { int dim; InOrder order; };
-int in_col(InOrder o, int k) { return o == IN_ADAPT_CONV ? (k & 63) * 6 + (k >> 6) : o == IN_STD_CONV ? (k & 63) * 12 + (k >> 6) : k; }
+struct InRows { int dim; InOrder order; int ch = 64; };
+int in_col(const InRows& in, int k) {
+  return in.order == IN_ADAPT_CONV ? (k % in.ch) * 6 + k / in.ch : in.order == IN_STD_CONV ? (k & 63) * 12 + (k >> 6) : k;
+}
 
 // One SelfAttention stack (lib:945-1040) of width D and feed-forward width F, checkpoint prefix `ck`: Linear(in -> D) +
 // LayerNorm + `layers` encoder layers.  The Linear's rows beyond in.dim (the padding of the input rows) stay zero.
@@ -641,7 +673,7 @@ bool pack_sa_stack(Packer& P, SaStackWeights& S, const std::string& ck, InRows i
   if (!lw || !lb || !ng || !nb) return false;
   const int k_pad = (in_dim + 63) / 64 * 64;
   const size_t o = P.alloc(S.in.wT, (size_t)k_pad * D);
-  pack_linear_chunked(P, o, lw, D, in_dim, k_pad, [&](int k) { return in_col(in.order, k); });
+  pack_linear_chunked(P, o, lw, D, in_dim, k_pad, [&](int k) { return in_col(in, k); });
   P.copy(S.in.b, lb->d, D);
   P.copy(S.ln_g, ng->d, D);
   P.copy(S.ln_b, nb->d, D);
@@ -732,7 +764,7 @@ bool pack_pool_heads(Packer& P, const nisqa_config& c, InRows in, bool gemm = fa
   const int nh = c.n_out, Dp = in.dim;
   auto prefix = [&](int h) { return nh == 1 ? std::string("pool.model.") : "pool_layers." + std::to_string(h) + ".model."; };
   auto put_row = [&](size_t o, const TensorView* v) {          // one [1, Dp] weight in the rows' column order
-    for (int k = 0; k < Dp; ++k) P.arena[o + k] = v->d[in_col(in.order, k)];
+    for (int k = 0; k < Dp; ++k) P.arena[o + k] = v->d[in_col(in, k)];
   };
   if (c.pool == NISQA_POOL_ATT_FF) {
     PoolHeadParams& H = P.w.pool_head;
@@ -751,7 +783,7 @@ bool pack_pool_heads(Packer& P, const nisqa_config& c, InRows in, bool gemm = fa
       if (!w1 || !b1 || !w2 || !b2 || !w3 || !b3) return false;
       if (gemm) {
         for (int k = 0; k < Dp; ++k) {
-          const int kc = in_col(in.order, k);
+          const int kc = in_col(in, k);
           for (int j = 0; j < 128; ++j) P.arena[oW1 + (size_t)k * nh * 128 + h * 128 + j] = w1->d[(size_t)j * Dp + kc];
         }
       } else {
@@ -837,7 +869,7 @@ bool pack_std_fc(Packer& P, int F) {
   const int Fp = round64(F);
   const size_t o = P.alloc(P.w.fc.wT, (size_t)768 * Fp);
   for (int k = 0; k < 768; ++k)
-    for (int j = 0; j < F; ++j) P.arena[o + (size_t)k * Fp + j] = fw->d[(size_t)j * 768 + in_col(IN_STD_CONV, k)];
+    for (int j = 0; j < F; ++j) P.arena[o + (size_t)k * Fp + j] = fw->d[(size_t)j * 768 + in_col({768, IN_STD_CONV}, k)];
   memcpy(&P.arena[P.alloc(P.w.fc.b, Fp)], fb->d, (size_t)F * 4);
   return true;
 }
@@ -876,7 +908,7 @@ bool pack_lstm_stack(Packer& P, Weights::LstmStack& S, const std::string& p, InR
       const TensorView* bh = P.get(p + "bias_hh" + sfx, {4 * H});
       if (!wi || !wh || !bi || !bh) return false;
       for (int k = 0; k < in; ++k) {
-        const int kc = l == 0 ? in_col(in0.order, k) : k;
+        const int kc = l == 0 ? in_col(in0, k) : k;
         for (int g = 0; g < 4 * H; ++g) P.arena[owi + (size_t)k * N + d * 4 * H + g] = wi->d[(size_t)g * in + kc];
       }
       for (int g = 0; g < 4 * H; ++g) P.arena[ob + d * 4 * H + g] = bi->d[g] + bh->d[g];
@@ -893,8 +925,8 @@ bool pack_td_model(Packer& P, nisqa_engine* e) {
   const nisqa_config& c = e->cfg;
   Weights& W = P.w;
   const std::string td = "time_dependency.model.", td2 = "time_dependency_2.model.";
-  // the rows feeding td: AdaptCNN's 384 (engine order), SkipCNN's n_mels * seg_len (padded to a multiple of 64 with zero
-  // rows: 720 -> 768 at 48 x 15), cnn_fc_out_h, or
+  // the rows feeding td: AdaptCNN's 6 c3 (engine order; 96 padded to 128 at c3 = 16), SkipCNN's n_mels * seg_len (padded
+  // to a multiple of 64 with zero rows: 720 -> 768 at 48 x 15), cnn_fc_out_h, or
   // StandardCNN's fc_out / 768 conv6 features (engine order)
   InRows in;
   if (e->std_cnn()) {
@@ -902,7 +934,8 @@ bool pack_td_model(Packer& P, nisqa_engine* e) {
     in = W.std_fc ? InRows{W.std_fc, IN_PLAIN} : InRows{768, IN_STD_CONV};
   } else {
     const bool conv_net = c.cnn_kind == NISQA_CNN_CONV;
-    in = {c.cnn_fc > 0 ? c.cnn_fc : (conv_net ? 384 : e->ff_fan_in()), conv_net && c.cnn_fc == 0 ? IN_ADAPT_CONV : IN_PLAIN};
+    in = {c.cnn_fc > 0 ? c.cnn_fc : (conv_net ? W.feat_cols() : e->ff_fan_in()), conv_net && c.cnn_fc == 0 ? IN_ADAPT_CONV : IN_PLAIN,
+          W.cnn_c[6]};
   }
   const Weights::LstmShape* last_lstm = nullptr;      // the last stage, when it is an LSTM
   int d1;                                             // td's fan_out
@@ -1131,35 +1164,44 @@ int upload_inputs(Pass& p, const PassInput& in) {
 
 // AdaptCNN / StandardCNN: conv1 (fused with conv2 on the tensor-core path), then conv2..conv6 on fp16 plane pairs
 // (conv_split.cu) or as fp32 FFMA convolutions (cnn.cu); conv6 writes the features to LN.feats
-void conv_layers(Pass& p) {
+int conv_layers(Pass& p) {
   nisqa_engine* e = p.e;
   Lane& LN = p.LN;
   const Weights& w = p.w;
+  const int* cc = w.cnn_c;
   const bool split = e->conv_tc != 0, fused12 = e->fused12();
   auto plane_hi = [&](int l) { return LN.planes[l].as<char>(); };
   auto plane_lo = [&](int l) { return LN.planes[l].as<char>() + LN.plane_bytes[l]; };
+  auto no_kernel = [&](int l) {
+    return fail(e, NISQA_ERR_STATE, "no conv" + std::to_string(l) + " kernel for " + std::to_string(cc[l - 1]) + " -> " +
+                                        std::to_string(cc[l]) + " channels");
+  };
   if (fused12) {
     Scope s(e, "conv12");
-    launch_conv12(p.st, p.std_mode, LN.mel.as<float>(), p.seg_frame0, p.seg_thr, w.conv[1].w, w.conv[1].b,
+    launch_conv12(p.st, p.std_mode, cc[2], LN.mel.as<float>(), p.seg_frame0, p.seg_thr, w.conv[1].w, w.conv[1].b,
                   e->act_store(1), w.conv[2].wtc, w.conv[2].b, e->tc_scale[2], e->act_store(2),
                   plane_hi(3), plane_lo(3), p.n_seg);
   } else {
     Scope s(e, "conv1");
-    launch_conv1(p.st, p.std_mode, LN.mel.as<float>(), p.c.n_mels, p.c.seg_len, p.seg_frame0, p.seg_thr, w.conv[1].w,
-                 w.conv[1].b, split ? nullptr : LN.act[2].as<float>(), p.n_seg,
-                 split ? plane_hi(2) : nullptr, split ? plane_lo(2) : nullptr, e->act_store(1));
+    if (!launch_conv1(p.st, p.std_mode, cc[1], LN.mel.as<float>(), p.c.n_mels, p.c.seg_len, p.seg_frame0, p.seg_thr,
+                      w.conv[1].w, w.conv[1].b, split ? nullptr : LN.act[2].as<float>(), p.n_seg,
+                      split ? plane_hi(2) : nullptr, split ? plane_lo(2) : nullptr, e->act_store(1)))
+      return no_kernel(1);
   }
   static const char* const names[7] = {"", "", "conv2", "conv3", "conv4", "conv5", "conv6"};
   for (int l = fused12 ? 3 : 2; l <= 6; ++l) {
     Scope s(e, names[l]);
-    if (split)
-      launch_conv_split(p.st, p.std_mode, l, plane_hi(l), plane_lo(l), w.conv[l].wtc, w.conv[l].b, e->tc_scale[l],
-                        e->act_store(l), l < 6 ? plane_hi(l + 1) : nullptr, l < 6 ? plane_lo(l + 1) : nullptr,
-                        l == 6 ? LN.feats.as<float>() : nullptr, p.n_seg);
-    else
+    if (split) {
+      if (!launch_conv_split(p.st, p.std_mode, l, cc[l - 1], cc[l], plane_hi(l), plane_lo(l), w.conv[l].wtc, w.conv[l].b,
+                             e->tc_scale[l], e->act_store(l), l < 6 ? plane_hi(l + 1) : nullptr,
+                             l < 6 ? plane_lo(l + 1) : nullptr, l == 6 ? LN.feats.as<float>() : nullptr, p.n_seg))
+        return no_kernel(l);
+    } else {
       launch_conv_layer(p.st, p.std_mode, l, LN.act[l].as<float>(), w.conv[l].w, w.conv[l].b,
                         l < 6 ? LN.act[l + 1].as<float>() : LN.feats.as<float>(), p.n_seg);
+    }
   }
+  return 0;
 }
 
 // SkipCNN / DFF (lib:504-583): BN + flatten (+ Linear layers), no convolution
@@ -1201,15 +1243,21 @@ int framewise(Pass& p, int fmt, Rows* out) {
   for (int l = e->fused12() ? 3 : 2; conv_net && l <= 6; ++l) {
     if (split) {
       // the lo plane sits at a fixed offset of the ALLOCATION (not of this pass's n_seg): the zero rows /
-      // columns of both planes must stay where they were when the buffer was cleared
-      CK(LN.planes[l].reserve_zeroed(2 * split_plane_bytes(p.std_mode, l, n_seg), p.st));
+      // columns of both planes must stay where they were when the buffer was cleared.  No kernel writes them, so a
+      // buffer cleared for another row width (weights of other channel counts loaded since) is cleared again.
+      const int C = p.w.cnn_c[l - 1];
+      if (LN.plane_c[l] != C) {
+        LN.planes[l].release();
+        LN.plane_c[l] = C;
+      }
+      CK(LN.planes[l].reserve_zeroed(2 * split_plane_bytes(p.std_mode, l, C, n_seg), p.st));
       LN.plane_bytes[l] = (LN.planes[l].cap / 2) & ~(size_t)1023;
     } else {
-      const ConvGeom g = split_geometry(p.std_mode, l);
+      const ConvGeom g = split_geometry(p.std_mode, l, p.w.cnn_c[l - 1]);
       CK(LN.act[l].reserve((size_t)n_seg * g.H * g.W * g.C * 4));
     }
   }
-  CK(LN.feats.reserve((size_t)n_seg * (p.std_mode ? 768 : 384) * 4));
+  CK(LN.feats.reserve((size_t)n_seg * (p.std_mode ? 768 : p.w.feat_ld()) * 4));
   p.seg_frame0 = LN.segtab.as<int>();
   p.seg_thr = reinterpret_cast<float*>(p.seg_frame0 + n_seg);
   p.seg_clip = p.seg_frame0 + 2 * (size_t)n_seg;
@@ -1221,8 +1269,9 @@ int framewise(Pass& p, int fmt, Rows* out) {
     launch_seg_table(p.st, p.clips, p.n, p.seg_prefix, p.clipmax, c.seg_hop, n_seg, p.seg_frame0, p.seg_thr, p.seg_clip); }
   e->last_conv12 = e->fused12();
   if (!conv_net) return ff_layers(p, out);
-  conv_layers(p);
-  *out = {LN.feats.as<float>(), p.std_mode ? 12 : 6};
+  const int rc = conv_layers(p);
+  if (rc) return rc;
+  *out = {LN.feats.as<float>(), p.std_mode ? 12 : p.w.feat_ld() / 64};
   if (p.std_mode && p.w.std_fc > 0 && !p.w.lstm_shipped) {      // StandardCNN's fc_out (lib:830-835), 64-column padded
     Scope s(e, "fc_out");
     const int Fp = round64(p.w.std_fc);
@@ -1233,7 +1282,8 @@ int framewise(Pass& p, int fmt, Rows* out) {
   if (c.cnn_fc > 0) {      // AdaptCNN's Linear behind conv6 (lib:708-709)
     Scope s(e, "framewise");
     CK(LN.ffb.reserve((size_t)n_seg * c.cnn_fc * 4));
-    launch_linear_tile(p.st, LN.feats.as<float>(), 384, p.w.ffc.wT, p.w.ffc.b, 0, LN.ffb.as<float>(), c.cnn_fc, n_seg, 384,
+    const int K = p.w.feat_ld();
+    launch_linear_tile(p.st, LN.feats.as<float>(), K, p.w.ffc.wT, p.w.ffc.b, 0, LN.ffb.as<float>(), c.cnn_fc, n_seg, K,
                        c.cnn_fc);
     *out = {LN.ffb.as<float>(), c.cnn_fc / 64};
   }
@@ -1411,7 +1461,7 @@ int td_stages(Pass& p, Rows rows) {
   e->last_td_in = nullptr;
   if (skip) {
     cur = rows;
-    D = p.std_mode ? (w.std_fc ? w.std_fc : 768) : c.cnn_fc ? c.cnn_fc : c.cnn_kind == NISQA_CNN_CONV ? 384 : e->ff_fan_in();
+    D = p.std_mode ? (w.std_fc ? w.std_fc : 768) : c.cnn_fc ? c.cnn_fc : c.cnn_kind == NISQA_CNN_CONV ? w.feat_cols() : e->ff_fan_in();
   } else if (sa1) {
     e->last_td_in = LN.tdout.as<float>();
     cur = {sa_stack(p, 0, rows, !e->td2_runs(), LN.tdout.as<float>()), e->sa_d() / 64};
@@ -1506,6 +1556,10 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
                    int32_t* status_out, int sync, int64_t* ticket_out = nullptr) {
   if (!e) return NISQA_ERR_INVALID;
   if (!e->weights_loaded) return fail(e, NISQA_ERR_STATE, "nisqa_load_weights has not been called");
+  if (!e->conv_tc && e->conv_net() && !e->w.shipped_channels())
+    return fail(e, NISQA_ERR_STATE, "conv_tc=0: the fp32 FFMA convolutions run AdaptCNN channel counts 16 / 32 / 64 only, this "
+                                    "checkpoint has " + std::to_string(e->w.cnn_c[1]) + " / " + std::to_string(e->w.cnn_c[2]) +
+                                    " / " + std::to_string(e->w.cnn_c[3]) + " (nisqa_set_option(\"conv_tc\", 1))");
   if (n_clips < 0 || (n_clips > 0 && (!n_samples || !sample_rate)))
     return fail(e, NISQA_ERR_INVALID, "null argument");
   if (fmt != NISQA_FMT_S16 && fmt != NISQA_FMT_F32) return fail(e, NISQA_ERR_INVALID, "sample_fmt");
@@ -1736,8 +1790,12 @@ int nisqa_load_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
   CK(cudaSetDevice(e->device));
   CK(cudaDeviceSynchronize());
   e->weights_loaded = false;      // a failed load may have freed the previous arena
+  int prev_c[7];
+  memcpy(prev_c, e->w.cnn_c, sizeof prev_c);
   int rc = pack_weights(e, tensors, n);
   if (rc) return rc;
+  // the last pass's maps were laid out for the previous channel counts: its stage dumps are gone with them
+  if (memcmp(prev_c, e->w.cnn_c, sizeof prev_c) != 0) e->last_passes = 0;
   e->weights_loaded = true;
   return 0;
 }
@@ -1894,10 +1952,12 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
   const int layer = stage - NISQA_STAGE_POOL1 + 2;      // POOL1 .. CONV5: the map that feeds conv layer 2 .. 6
   int64_t count = 0;
   const float* src = nullptr;
-  int hw = 0, ch = 0;    // NHWC -> NCHW conversion when ch > 0
+  int hw = 0, ch = 0;    // NHWC -> NCHW conversion when ch > 0 (rows of hw_ld floats; 0: hw * ch)
+  int hw_ld = 0;
   int width = 0, ld = 0; // rows of `width` floats at a stride of `ld` (a padded row layout)
+  const int* cc = e->w.cnn_c;
   if (conv_map) {
-    const ConvGeom g = split_geometry(std_mode, layer);
+    const ConvGeom g = split_geometry(std_mode, layer, cc[layer - 1]);
     src = LN.act[layer].as<float>(); hw = g.H * g.W; ch = g.C;
   }
   switch (stage) {
@@ -1911,7 +1971,7 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
       } else if (std_mode) {
         src = LN.feats.as<float>(); hw = 12; ch = 64;           // [h*2+w][c] -> c*12+h*2+w
       } else {
-        src = LN.feats.as<float>(); hw = 6; ch = 64;            // [h][c] -> c*6+h
+        src = LN.feats.as<float>(); hw = 6; ch = cc[6]; hw_ld = e->w.feat_ld();    // [h][c] -> c*6+h
       }
       break;
     case NISQA_STAGE_TD_IN:
@@ -1923,7 +1983,7 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
     case NISQA_STAGE_TD_OUT:
       if (!e->last_td_out) return fail(e, NISQA_ERR_STATE, "the per-step BiLSTM outputs were not kept: nisqa_set_option(\"keep_td_out\", 1) before the predict call");
       src = e->last_td_out; count = ns * e->last_td_out_d; width = e->last_td_out_d; ld = e->last_td_out_ld;
-      if (e->last_td_out_hw) { hw = e->last_td_out_hw; ch = 64; }       // conv6 features: [hw][c] -> c*hw + hw index
+      if (e->last_td_out_hw) { hw = e->last_td_out_hw; ch = cc[6]; hw_ld = ld; }   // conv6 features: [hw][c] -> c*hw + hw index
       break;
     default: return fail(e, NISQA_ERR_INVALID, "unknown stage");
   }
@@ -1943,13 +2003,14 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
   } else if (ch > 0) {
     if (from_planes) {
       CK(LN.act[layer].reserve((size_t)count * 4));
-      launch_unsplit(st, std_mode, layer, LN.planes[layer].as<char>(), LN.planes[layer].as<char>() + LN.plane_bytes[layer],
+      launch_unsplit(st, std_mode, layer, ch, LN.planes[layer].as<char>(), LN.planes[layer].as<char>() + LN.plane_bytes[layer],
                      ldexpf(1.f, e->act_exp[layer - 1]), LN.act[layer].as<float>(), (int)ns);
       src = LN.act[layer].as<float>();
     }
     CK(e->dump.reserve((size_t)count * 4));
-    launch_nhwc_to_nchw(st, src, e->dump.as<float>(), ns, hw, ch);
+    launch_nhwc_to_nchw(st, src, hw_ld ? hw_ld : hw * ch, e->dump.as<float>(), ns, hw, ch);
     src = e->dump.as<float>();
+    ld = 0;                                               // (the converted rows are contiguous)
   }
   if (!src) return fail(e, NISQA_ERR_STATE, "stage was not produced");
   if (ld > width)

@@ -15,18 +15,21 @@ struct FbTables;
 
 // Geometry of one segment's activation map that feeds conv layer `layer` (2..6), i.e. the output of layer - 1:
 // H rows, W columns, C channels.  AdaptCNN pools to widths 7 / 5 / 3 (adaptive max-pool), StandardCNN to 8 / 4 / 2
-// (MaxPool2d(2)).  The fp16 plane pairs (conv_split.cu), the fp32 FFMA activations and the stage dumps all use it.
+// (MaxPool2d(2)).  C is the checkpoint's (conv layer - 1's output channels, read from its weights; StandardCNN: 16 / 32 /
+// 64); C = 0 asks for StandardCNN's.  The fp16 plane pairs (conv_split.cu), the fp32 FFMA activations and the stage
+// dumps all use it.
 struct ConvGeom { int H, W, C; };
-constexpr ConvGeom split_geometry(int std_mode, int layer) {
+constexpr ConvGeom split_geometry(int std_mode, int layer, int C) {
   return {layer == 2 ? 24 : layer <= 4 ? 12 : 6,
           std_mode ? (layer == 2 ? 8 : layer <= 4 ? 4 : 2) : (layer == 2 ? 7 : layer <= 4 ? 5 : 3),
-          layer == 2 ? 16 : layer == 3 ? 32 : 64};
+          C ? C : layer == 2 ? 16 : layer == 3 ? 32 : 64};
 }
-// true when the layer configuration C (cnn.cu ConvCfg, conv_split.cuh SpCfg) reads that geometry
+// true when the layer configuration C (cnn.cu ConvCfg, conv_split.cuh SpCfg) reads that geometry (StandardCNN: with its
+// shipped input channels too; AdaptCNN's come from the weights)
 template <class C>
 constexpr bool input_is(int std_mode, int layer) {
-  return split_geometry(std_mode, layer).H == C::H && split_geometry(std_mode, layer).W == C::W &&
-         split_geometry(std_mode, layer).C == C::CIN;
+  return split_geometry(std_mode, layer, C::CIN).H == C::H && split_geometry(std_mode, layer, C::CIN).W == C::W &&
+         (!std_mode || split_geometry(std_mode, layer, 0).C == C::CIN);
 }
 
 // ---------------------------------------------------------------- parameter structs (device pointers)
@@ -86,22 +89,31 @@ void launch_mel_dump(cudaStream_t st, const float* mel, const ClipDesc* clips, i
 
 // ---------------------------------------------------------------- cnn.cu (fp32 FFMA convolutions)
 // conv1 + pool1 of segments of n_mels x seg_len mel cells (rows n_mels floats apart): AdaptCNN any accepted shape ->
-// 24 x 7, StandardCNN 48 x 15 only -> 24 x 8
-void launch_conv1(cudaStream_t st, int std_mode, const float* mel, int n_mels, int seg_len, const int* seg_frame0,
+// 24 x 7, StandardCNN 48 x 15 only -> 24 x 8.  c1 output channels: 16, 32 or 64 into the planes (out_hi), 16 into fp32
+// `out`.  false: no instance for the shape.
+bool launch_conv1(cudaStream_t st, int std_mode, int c1, const float* mel, int n_mels, int seg_len, const int* seg_frame0,
                   const float* seg_thr, const float* w1, const float* b1, float* out, int n_seg, void* out_hi, void* out_lo,
                   float store_scale);
 void launch_conv_layer(cudaStream_t st, int std_mode, int layer, const float* in, const float* w, const float* b, float* out,
                        int n_seg);
-void launch_nhwc_to_nchw(cudaStream_t st, const float* in, float* out, long long n, int hw, int ch);
+// rows of `ld` floats (>= hw * ch)
+void launch_nhwc_to_nchw(cudaStream_t st, const float* in, int ld, float* out, long long n, int hw, int ch);
 
 // ---------------------------------------------------------------- conv_split.cu (tensor-core convolutions on fp16 planes)
-size_t split_plane_bytes(int std_mode, int layer, int n_seg);
-void launch_conv_split(cudaStream_t st, int std_mode, int layer, const void* in_hi, const void* in_lo, const void* wtc,
-                       const float* b, float out_scale, float store_scale, void* out_hi, void* out_lo, float* out_f32, int n_seg);
-void launch_conv12(cudaStream_t st, int std_mode, const float* mel, const int* seg_frame0, const float* seg_thr,
+size_t split_plane_bytes(int std_mode, int layer, int C, int n_seg);
+// AdaptCNN conv2..conv6 take cin, cout in {16, 32, 64} (the pairs cnn_c_out_1/2/3 reach); StandardCNN its shipped ones.
+// The fp32 features of conv6 go out in rows of (6 cout + 63) / 64 * 64 floats (AdaptCNN), zero-padded.
+bool conv_split_supported(int cin, int cout);
+bool launch_conv_split(cudaStream_t st, int std_mode, int layer, int cin, int cout, const void* in_hi, const void* in_lo,
+                       const void* wtc, const float* b, float out_scale, float store_scale, void* out_hi, void* out_lo,
+                       float* out_f32, int n_seg);
+// the fused conv1 + conv2 kernel: 48 x 15 segments, c1 = 16, c2 = 32 (AdaptCNN also 16)
+bool conv12_supported(int std_mode, int c1, int c2);
+void launch_conv12(cudaStream_t st, int std_mode, int c2, const float* mel, const int* seg_frame0, const float* seg_thr,
                    const float* w1, const float* b1, float c1_scale, const void* wtc2, const float* bias2, float scale2,
                    float store_scale, void* out_hi, void* out_lo, int n_seg);
-void launch_unsplit(cudaStream_t st, int std_mode, int layer, const void* hi, const void* lo, float unit, float* out, int n_seg);
+void launch_unsplit(cudaStream_t st, int std_mode, int layer, int C, const void* hi, const void* lo, float unit, float* out,
+                    int n_seg);
 
 // ---------------------------------------------------------------- td.cu (fc_out, BiLSTM, pooling)
 void launch_fc20(cudaStream_t st, const float* feats, const float* WT, const float* b, float* out, int n_rows);

@@ -70,7 +70,15 @@ __device__ __forceinline__ uint64_t make_desc_b(uint32_t saddr, uint32_t lbo_byt
 // warp's 16 rows) * B[16 x N] (fp16, shared memory descriptor)
 template <int N>
 __device__ __forceinline__ void wgmma_rs(float* d, const uint32_t (&a)[4], uint64_t b_desc);
-template <> __device__ __forceinline__ void wgmma_rs<32>(float* d, const uint32_t (&a)[4], uint64_t b_desc) {
+template <> __device__ __forceinline__ void wgmma_rs<16>(float* d, const uint32_t (&a)[4], uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
+}
+template <>__device__ __forceinline__ void wgmma_rs<32>(float* d, const uint32_t (&a)[4], uint64_t b_desc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "

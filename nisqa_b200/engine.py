@@ -60,6 +60,7 @@ LSTM_LAYERS_MAX = 4
 CNN_FC_OUT_MAX = 1024                 # StandardCNN's fc_out width (None: the LSTM reads the 768 conv6 features)
 N_MELS = (32, 40, 48, 64, 80, 96, 128)   # ms_n_mels: one front-end kernel instance per band count
 SEG_LEN_MIN, SEG_LEN_MAX = 3, 31      # ms_seg_length, odd (128 x 31 bounds SkipCNN's / DFF's fan_in at 3968 < 4096)
+CNN_CHANNELS = (16, 32, 64)           # AdaptCNN cnn_c_out_1/2/3: one fp16 plane row is one 32 / 64 / 128-byte swizzle atom
 
 
 def _sa_widths(args, prefix, de=False):
@@ -111,6 +112,12 @@ def _framewise(args):
         _check_standard_cnn(args)
         return CNN_STANDARD, 0, True
     cnn_kind = CNN_CONV if cnn == "adapt" else CNN_DFF if cnn == "dff" else CNN_SKIP
+    if cnn == "adapt":
+        # (the engine reads the channel counts from the conv / bn tensors in nisqa_load_weights)
+        for i in (1, 2, 3):
+            c = args.get("cnn_c_out_%d" % i)
+            if c not in CNN_CHANNELS or int(c) != c:
+                raise NotImplementedError("cnn_c_out_%d=%r: the engine runs AdaptCNN channel counts 16, 32 or 64" % (i, c))
     cnn_fc = int(args.get("cnn_fc_out_h") or 0)         # AdaptCNN's optional Linear behind conv6 (lib:682-684), SkipCNN's
     if cnn_kind == CNN_DFF and cnn_fc == 0:
         cnn_fc = 4096                                   # DFF's default hidden width (lib:544)
@@ -270,7 +277,8 @@ def config_from_args(args, max_chunk_segments=0):
     fan1 = _check_lstm(args, "td_lstm") if td_lstm else None
     if skip:
         fan1 = int(args.get("cnn_fc_out_h") or 768) if cnn == "standard" else (
-            cnn_fc or (384 if cnn == "adapt" else int(args.get("ms_n_mels") or 0) * int(args.get("ms_seg_length") or 0)))
+            cnn_fc or (6 * int(args["cnn_c_out_3"]) if cnn == "adapt"
+                       else int(args.get("ms_n_mels") or 0) * int(args.get("ms_seg_length") or 0)))
     fan2 = _check_lstm(args, "td_2_lstm") if td2 == "lstm" else None
     if pool_mode == POOL_LAST_STEP_BI:
         key = "td_2_lstm" if td2 == "lstm" else "td_lstm" if td2 == "skip" and td_lstm else None
@@ -293,7 +301,6 @@ def config_from_args(args, max_chunk_segments=0):
             raise NotImplementedError("de_align_apply / de_fuse option not available: %r / %r" % (args.get("de_align_apply"), args.get("de_fuse")))
         if args.get("de_fuse_dim") and int(args["de_fuse_dim"]) % 64 != 0:
             raise NotImplementedError("de_fuse_dim=%r: the engine needs a multiple of 64" % (args.get("de_fuse_dim"),))
-    ok = ok and (cnn_kind != CNN_CONV or (args["cnn_c_out_1"], args["cnn_c_out_2"], args["cnn_c_out_3"]) == (16, 32, 64))
     if not ok:
         raise NotImplementedError("checkpoint hyper-parameters outside the shipped NISQA configurations")
     n_mels, seg_len = _check_mel_shape(args, td_lstm or cnn_kind == CNN_STANDARD)
