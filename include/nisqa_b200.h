@@ -175,6 +175,14 @@ NISQA_API const char* nisqa_last_error(const nisqa_engine* e);
  * folds eval-mode BatchNorm into the convolutions, repacks to the kernel layouts, uploads. */
 NISQA_API int  nisqa_load_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n);
 
+/* AdaptCNN's adaptive max-pool output sizes cnn_pool_1 / cnn_pool_2 / cnn_pool_3 as h1 w1 h2 w2 h3 w3 (lib:586-710).
+ * Call it between nisqa_create and nisqa_load_weights: it takes effect at the next load.  An engine that never calls it
+ * runs the shipped pools 24 7 12 5 6 3.  Accepted: every [h, w] with h, w >= 1, w <= 14 and (h + 1) * (w + 1) <= 256,
+ * and w3 <= 3; anything else returns NISQA_ERR_INVALID naming the field (as does a pool other than the shipped one on a
+ * StandardCNN, SkipCNN or DFF engine).  nisqa_load_weights then checks that cnn.model.conv6.weight is (c3, c3, 3, w3),
+ * that c3 * h3 <= 4096 and that the Linear behind the CNN reads c3 * h3 features (NISQA_ERR_WEIGHTS naming the tensor). */
+NISQA_API int  nisqa_set_cnn_pools(nisqa_engine* e, const int32_t pools[6]);  /* h1 w1 h2 w2 h3 w3 */
+
 /* replaces the body of predict_dim / predict_mos for n_clips clips given as mono PCM in HOST
  * memory (already channel-selected / mono-mixed by the caller, lib:2298-2304).
  *   pcm[i]         : n_samples[i] samples of sample_fmt

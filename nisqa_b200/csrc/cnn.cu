@@ -22,8 +22,8 @@ namespace nisqa {
 
 // ----------------------------------------------------------------------------------------
 // conv1 + BN + ReLU + pool1 of segments of n_mels x seg_len cells (mel rows n_mels floats apart)
-//   MODE 0 (adapt, lib:690-691): adaptive_max_pool2d n_mels x seg_len -> 24x7 (conv1_adapt_cell; 48x15: rows {2i,2i+1},
-//          cols [2j,2j+3))
+//   MODE 0 (adapt, lib:690-691): adaptive_max_pool2d n_mels x seg_len -> PH x PW = cnn_pool_1 (conv1_adapt_cell; 48x15 ->
+//          24 x 7: rows {2i,2i+1}, cols [2j,2j+3))
 //   MODE 1 (standard, lib:813-814): MaxPool2d(2, stride 2, padding (0,1)) -> 24x8 : cols {2j-1,2j} (48 x 15 only)
 // thread = one pooled cell of one segment, all C1 channels (16, 32 or 64 for AdaptCNN, in groups of 16).
 // SPLIT: the output goes out as the two fp16 planes conv2's tensor-core kernel consumes (conv_split.cu:
@@ -35,25 +35,24 @@ conv1_pool1_kernel(const float* __restrict__ mel, int n_mels, int seg_len, const
                    const float* __restrict__ seg_thr, const float* __restrict__ w1 /*[9][C1]*/,
                    const float* __restrict__ b1 /*[C1]*/, float* __restrict__ out,
                    unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo,
-                   float store_scale /*2^-e1*/, int n_seg) {
+                   float store_scale /*2^-e1*/, int n_seg, int PH, int PW) {
   static_assert(C1 == 16 || (MODE == 0 && SPLIT), "StandardCNN and the fp32 output: 16 channels");
-  constexpr int PW = (MODE == 0) ? 7 : 8;
   __shared__ __align__(16) float ws[9 * C1 + C1];
   for (int i = threadIdx.x; i < 9 * C1 + C1; i += blockDim.x)
     ws[i] = (i < 9 * C1) ? __ldg(w1 + i) : __ldg(b1 + i - 9 * C1);
   __syncthreads();
 
   const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const int seg = (int)(gid / (24 * PW));
+  const int seg = (int)(gid / (PH * PW));
   if (seg >= n_seg) return;
-  const int cell = (int)(gid - (long long)seg * (24 * PW));
-  const int ph = cell % 24, pw = cell / 24;      // lanes run along mel rows: coalesced reads
+  const int cell = (int)(gid - (long long)seg * (PH * PW));
+  const int ph = cell % PH, pw = cell / PH;      // lanes run along mel rows: coalesced reads
   const int f0 = __ldg(seg_frame0 + seg);
   const float thr = __ldg(seg_thr + seg);
 
   // channels 16 cg .. 16 cg + 15 -> the two 16-byte chunks 2 cg, 2 cg + 1 of the cell's plane row
   auto store_split = [&](const float (&res)[16], int cg) {
-    const int g = kSplitLead + seg * (25 * (PW + 1)) + (ph + 1) * (PW + 1) + (pw + 1);
+    const int g = kSplitLead + seg * ((PH + 1) * (PW + 1)) + (ph + 1) * (PW + 1) + (pw + 1);
 #pragma unroll
     for (int c = 0; c < 2; ++c) {
       uint4 hi, lo;
@@ -67,7 +66,7 @@ conv1_pool1_kernel(const float* __restrict__ mel, int n_mels, int seg_len, const
   float res[16];
   if constexpr (MODE == 0) {
     for (int cg = 0; cg < C1 / 16; ++cg) {     // one group of 16 channels at a time (the registers of one cell)
-      conv1_adapt_cell<C1>(mel + (size_t)f0 * n_mels, n_mels, seg_len, thr, ws, ph, pw, 16 * cg, res);
+      conv1_adapt_cell<C1>(mel + (size_t)f0 * n_mels, n_mels, seg_len, PH, PW, thr, ws, ph, pw, 16 * cg, res);
       if constexpr (SPLIT) store_split(res, cg);
     }
   } else {
@@ -75,7 +74,7 @@ conv1_pool1_kernel(const float* __restrict__ mel, int n_mels, int seg_len, const
     if constexpr (SPLIT) store_split(res, 0);
   }
   if constexpr (!SPLIT) {
-    float4* o = reinterpret_cast<float4*>(out + ((size_t)seg * 24 * PW + ph * PW + pw) * 16);
+    float4* o = reinterpret_cast<float4*>(out + ((size_t)seg * PH * PW + ph * PW + pw) * 16);
 #pragma unroll
     for (int q = 0; q < 4; ++q)
       o[q] = make_float4(res[q * 4], res[q * 4 + 1], res[q * 4 + 2], res[q * 4 + 3]);
@@ -286,23 +285,23 @@ static void launch_conv(cudaStream_t st, const float* in, const float* w, const 
 
 bool launch_conv1(cudaStream_t st, int std_mode, int c1, const float* mel, int n_mels, int seg_len, const int* seg_frame0,
                   const float* seg_thr, const float* w1, const float* b1, float* out, int n_seg, void* out_hi, void* out_lo,
-                  float store_scale) {
+                  float store_scale, int ph, int pw) {
   if (c1 != 16 && (std_mode || !out_hi || (c1 != 32 && c1 != 64))) return false;
-  const int cells = std_mode ? 24 * 8 : 24 * 7;
-  const long long total = (long long)n_seg * cells;
+  if (std_mode) { ph = 24; pw = 8; }
+  const long long total = (long long)n_seg * ph * pw;
   const int grid = (int)((total + 255) / 256);
   unsigned char* oh = static_cast<unsigned char*>(out_hi);
   unsigned char* ol = static_cast<unsigned char*>(out_lo);
   const float s = store_scale;
   const int H = n_mels, W = seg_len;
   if (out_hi) {
-    if (std_mode) conv1_pool1_kernel<1, true><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
-    else if (c1 == 32) conv1_pool1_kernel<0, true, 32><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
-    else if (c1 == 64) conv1_pool1_kernel<0, true, 64><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
-    else conv1_pool1_kernel<0, true><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
+    if (std_mode) conv1_pool1_kernel<1, true><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg, ph, pw);
+    else if (c1 == 32) conv1_pool1_kernel<0, true, 32><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg, ph, pw);
+    else if (c1 == 64) conv1_pool1_kernel<0, true, 64><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg, ph, pw);
+    else conv1_pool1_kernel<0, true><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg, ph, pw);
   } else {
-    if (std_mode) conv1_pool1_kernel<1, false><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
-    else conv1_pool1_kernel<0, false><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg);
+    if (std_mode) conv1_pool1_kernel<1, false><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg, ph, pw);
+    else conv1_pool1_kernel<0, false><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg, ph, pw);
   }
   return true;
 }

@@ -120,16 +120,17 @@ __device__ __forceinline__ void conv1_cell(const float* __restrict__ mel, int f0
 }
 #endif
 
-// AdaptCNN conv1 + BN + ReLU + adaptive_max_pool2d to 24 x 7 for one pooled cell (ph, pw), channels c0 .. c0 + 15 of C1,
-// of a segment of H mel rows x W frames (seg: its frame 0, rows H floats apart; ws: [9][C1] weights, then C1 biases).  The cell's window (F.adaptive_max_pool2d) is conv rows
-// [floor(ph H / 24), ceil((ph + 1) H / 24)) x columns [floor(pw W / 7), ceil((pw + 1) W / 7)).  Each conv position is the
-// fmaf chain of conv1_cell (zero start, taps 0..8, inputs clamped at thr, zero outside the segment), each cell the max,
-// + bias, ReLU: at 48 x 15 the windows are conv1_cell<0>'s and the results bit-identical to it and to conv1_strip.
+// AdaptCNN conv1 + BN + ReLU + adaptive_max_pool2d to PH x PW (cnn_pool_1, shipped 24 x 7) for one pooled cell (ph, pw),
+// channels c0 .. c0 + 15 of C1, of a segment of H mel rows x W frames (seg: its frame 0, rows H floats apart; ws: [9][C1]
+// weights, then C1 biases).  The cell's window (F.adaptive_max_pool2d) is conv rows [floor(ph H / PH), ceil((ph + 1) H / PH))
+// x columns [floor(pw W / PW), ceil((pw + 1) W / PW)).  Each conv position is the fmaf chain of conv1_cell (zero start, taps
+// 0..8, inputs clamped at thr, zero outside the segment), each cell the max, + bias, ReLU: at 48 x 15 -> 24 x 7 the windows
+// are conv1_cell<0>'s and the results bit-identical to it and to conv1_strip.
 template <int C1>
-__device__ __forceinline__ void conv1_adapt_cell(const float* __restrict__ seg, int H, int W, float thr, const float* ws,
-                                                 int ph, int pw, int c0, float (&res)[16]) {
-  const int y0 = (ph * H) / 24, y1 = ((ph + 1) * H + 23) / 24;
-  const int x0 = (pw * W) / 7, x1 = ((pw + 1) * W + 6) / 7;
+__device__ __forceinline__ void conv1_adapt_cell(const float* __restrict__ seg, int H, int W, int PH, int PW, float thr,
+                                                 const float* ws, int ph, int pw, int c0, float (&res)[16]) {
+  const int y0 = (ph * H) / PH, y1 = ((ph + 1) * H + PH - 1) / PH;
+  const int x0 = (pw * W) / PW, x1 = ((pw + 1) * W + PW - 1) / PW;
   float mx[16];
 #pragma unroll
   for (int c = 0; c < 16; ++c) mx[c] = -INFINITY;

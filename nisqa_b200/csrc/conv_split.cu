@@ -59,8 +59,8 @@ namespace nisqa {
 // 64 output channels (24 x 7 maps) takes one k16 step per unit: with two, ptxas spills (CIN 32: 16 bytes, CIN 64: 72).
 template <class C>
 struct TapUnits {
-  static constexpr int KS = C::CIN / 16, UK = (KS < 2 || (C::H == 24 && C::COUT == 64)) ? 1 : 2, PER_TAP = KS / UK,
-                       N = 9 * PER_TAP;
+  static constexpr int KS = C::CIN / 16, UK = (KS < 2 || C::ONE_STEP_UNITS) ? 1 : 2, PER_TAP = KS / UK,
+                       N = C::NTAP * PER_TAP;
 };
 
 // A fragments of K steps k0 .. k0 + UK - 1 of one tap (row offset tapoff) for this warpgroup's NB m64 blocks: block b
@@ -341,6 +341,213 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
   }
 }
 
+// ---- conv2..conv6 of an AdaptCNN with other pools: the same kernel on a run-time geometry ----
+// The pieces below are tile_gemm / stage_rows / store_tile with SpGeom's sizes in place of SpCfg's: the same tap order, the
+// same split and the same scales, so at equal sizes the values are those of conv_split_kernel.
+
+// tile_gemm over C::NTAP taps: tap t = 3 x KX position (t / KX, t % KX) reads tile row offset (t / KX - 1) P + t % KX - PADX
+template <class C>
+__device__ __forceinline__ void tile_gemm_rt(float (&acc_m)[1][C::COUT / 2], float (&acc_s)[1][C::COUT / 2], uint32_t a_hi,
+                                             uint32_t a_lo, uint32_t b_base, const int (&row)[1], int lchunk, int P) {
+  using U = TapUnits<C>;
+  constexpr int UK = U::UK, PT = U::PER_TAP;
+#pragma unroll
+  for (int i = 0; i < C::COUT / 2; ++i) { acc_m[0][i] = 0.f; acc_s[0][i] = 0.f; }
+  uint32_t ah[2][1][UK][4], al[2][1][UK][4];
+  load_unit<C, 1>(a_hi, a_lo, row, -P - C::PADX, 0, lchunk, ah[0], al[0]);
+#pragma unroll
+  for (int u = 0; u < U::N; ++u) {
+    wgmma_fence();
+    mma_unit<C, 1>(acc_m, acc_s, ah[u & 1], al[u & 1], b_base + (u / PT) * C::B_STAGE, (u % PT) * UK);
+    wgmma_commit();
+    if (u + 1 < U::N) {
+      wgmma_wait<1>();
+      const int v = u + 1, t = v / PT;
+      load_unit<C, 1>(a_hi, a_lo, row, (t / C::KX - 1) * P + (t % C::KX - C::PADX), (v % PT) * UK, lchunk, ah[v & 1], al[v & 1]);
+    }
+  }
+  wgmma_wait<0>();
+}
+
+template <class C>
+__device__ __forceinline__ void stage_rows_rt(const SpGeom& g, const float (&acc_m)[C::COUT / 2], const float (&acc_s)[C::COUT / 2],
+                                              int m0, int acol, int seg0, int n_seg, const float2 (&bb)[C::COUT / 8],
+                                              float out_scale, float* stg) {
+  constexpr int SS = C::STG_STRIDE;
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    const int m = m0 + 8 * half;
+    if (m < g.KEPT && seg0 + m / g.SEG_ROWS < n_seg) {
+      const int r = g.gemm_row(m);
+#pragma unroll
+      for (int j = 0; j < C::COUT / 8; ++j) {
+        const int col = 8 * j + acol;
+        const float v0 = fmaxf(fmaf(acc_m[4 * j + 2 * half] + acc_s[4 * j + 2 * half], out_scale, bb[j].x), 0.f);
+        const float v1 = fmaxf(fmaf(acc_m[4 * j + 2 * half + 1] + acc_s[4 * j + 2 * half + 1], out_scale, bb[j].y), 0.f);
+        *reinterpret_cast<float2*>(stg + r * SS + col) = make_float2(v0, v1);
+      }
+    }
+  }
+}
+
+// store_tile on a run-time geometry.  The pooling layers run F.adaptive_max_pool2d in both dimensions: cell (ph, pw) is the
+// maximum over rows [floor(ph H / HO), ceil((ph + 1) H / HO)) x columns [floor(pw W / WO), ceil((pw + 1) W / WO)) - windows
+// that may overlap, or repeat a row / column when the output is larger than the input.
+template <class C>
+__device__ __forceinline__ void store_tile_rt(const SpGeom& g, const float* stg, int seg0, int nvalid, int t0, int nthr,
+                                              float store_scale, unsigned char* __restrict__ out_hi,
+                                              unsigned char* __restrict__ out_lo, float* __restrict__ out_f32) {
+  constexpr int COUT = C::COUT, SS = C::STG_STRIDE;
+  const int H = g.H, W = g.W, P = g.P, BLK = g.BLK;
+  if constexpr (C::POOLED) {
+    constexpr int C8 = COUT / 8;
+    const int HO = g.HO, WO = g.WO;
+    for (int i = t0; i < nvalid * HO * WO * C8; i += nthr) {
+      const int c8 = i % C8;
+      int rest = i / C8;
+      const int pw = rest % WO; rest /= WO;
+      const int ph = rest % HO;
+      const int s = rest / HO;
+      const int y0 = (ph * H) / HO, y1 = ((ph + 1) * H + HO - 1) / HO;
+      const int x0 = (pw * W) / WO, x1 = ((pw + 1) * W + WO - 1) / WO;
+      float4 ma = make_float4(0.f, 0.f, 0.f, 0.f), mb = ma;       // post-ReLU values are >= 0
+      for (int hy = y0; hy < y1; ++hy)
+        for (int x = x0; x < x1; ++x) {
+          const float4* tp = reinterpret_cast<const float4*>(stg + (s * BLK + (hy + 1) * P + (x + 1)) * SS + c8 * 8);
+          const float4 ta = tp[0], tb = tp[1];
+          ma.x = fmaxf(ma.x, ta.x); ma.y = fmaxf(ma.y, ta.y); ma.z = fmaxf(ma.z, ta.z); ma.w = fmaxf(ma.w, ta.w);
+          mb.x = fmaxf(mb.x, tb.x); mb.y = fmaxf(mb.y, tb.y); mb.z = fmaxf(mb.z, tb.z); mb.w = fmaxf(mb.w, tb.w);
+        }
+      uint4 hi, lo;
+      split8(ma, mb, store_scale, hi, lo);
+      const int gr = kSplitLead + (seg0 + s) * g.OBLK + (ph + 1) * g.OP + (pw + 1);
+      const size_t o = split_off<COUT * 2>(gr, c8);
+      *reinterpret_cast<uint4*>(out_hi + o) = hi;
+      *reinterpret_cast<uint4*>(out_lo + o) = lo;
+    }
+  } else if constexpr (C::OUT_SPLIT) {
+    constexpr int C8 = COUT / 8;
+    for (int i = t0; i < nvalid * BLK * C8; i += nthr) {
+      const int c8 = i % C8, r = i / C8;
+      const int q = r % BLK, hh = q / P, ww = q - hh * P;
+      uint4 hi = make_uint4(0u, 0u, 0u, 0u), lo = hi;
+      if (hh >= 1 && ww >= 1) {
+        const float4* tp = reinterpret_cast<const float4*>(stg + r * SS + c8 * 8);
+        split8(tp[0], tp[1], store_scale, hi, lo);
+      }
+      const size_t o = split_off<COUT * 2>(kSplitLead + seg0 * BLK + r, c8);
+      *reinterpret_cast<uint4*>(out_hi + o) = hi;
+      *reinterpret_cast<uint4*>(out_lo + o) = lo;
+    }
+  } else {
+    // conv6: fp32 CNN features [seg][H][COUT] in rows of OUT_LD floats, zero padding columns
+    constexpr int C4 = COUT / 4;
+    for (int i = t0; i < nvalid * H * C4; i += nthr) {
+      const int c4 = i % C4, rest = i / C4, h = rest % H, s = rest / H;
+      *reinterpret_cast<float4*>(out_f32 + (size_t)(seg0 + s) * g.OUT_LD + h * COUT + c4 * 4) =
+          *reinterpret_cast<const float4*>(stg + (s * BLK + (h + 1) * P + 1) * SS + c4 * 4);
+    }
+    const int pad4 = (g.OUT_LD - g.OUT_COLS) / 4;
+    for (int i = t0; i < nvalid * pad4; i += nthr)
+      *reinterpret_cast<float4*>(out_f32 + (size_t)(seg0 + i / pad4) * g.OUT_LD + g.OUT_COLS + (i % pad4) * 4) =
+          make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+}
+
+// conv_split_kernel with SpGeom's sizes: the same persistent CTA, tile copies, barriers and roles
+template <class C>
+__global__ void __launch_bounds__(C::NT, 1)
+conv_split_rt_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* __restrict__ in_lo,
+                     const __half* __restrict__ wtc, const float* __restrict__ bias, float out_scale, float store_scale,
+                     unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo, float* __restrict__ out_f32,
+                     int n_seg, const SpGeom g) {
+  constexpr int ROWB = C::ROWB, NT = C::NT, NTAP = C::NTAP;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  const uint32_t sbase = smem_u32(smem);
+  const uint32_t b_base = sbase + C::OFF_B;
+  const uint32_t bar_w = sbase + C::OFF_BAR, bar_full = bar_w + 8 * NTAP, bar_empty = bar_full + 8 * C::A_BUFS;
+  float* stg = reinterpret_cast<float*>(smem + C::OFF_STG);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  const int G = g.G, BLK = g.BLK, HALO = g.HALO;
+  const int n_tiles = (n_seg + G - 1) / G;
+
+  auto issue_tile = [&](int tile, int b) {
+    const uint32_t a_copy = (uint32_t)(256 + 2 * HALO) * ROWB;
+    const int g0 = kSplitLead + tile * G * BLK - HALO;
+    const uint32_t dst = sbase + C::OFF_A_HI + b * C::A_BUF + (uint32_t)(g0 & 7) * ROWB;
+    mbar_expect_tx(bar_full + 8 * b, 2 * a_copy);
+    bulk_g2s(dst, in_hi + (size_t)g0 * ROWB, a_copy, bar_full + 8 * b);
+    bulk_g2s(dst + C::A_BYTES, in_lo + (size_t)g0 * ROWB, a_copy, bar_full + 8 * b);
+  };
+
+  if (tid == 0) {
+    for (int t = 0; t < NTAP; ++t) mbar_init(bar_w + 8 * t, 1);
+    for (int b = 0; b < C::A_BUFS; ++b) mbar_init(bar_full + 8 * b, 1);
+    if constexpr (C::A_BUFS == 2)
+      for (int b = 0; b < 2; ++b) mbar_init(bar_empty + 8 * b, NT);
+    fence_barrier_init();
+    for (int t = 0; t < NTAP; ++t) {
+      mbar_expect_tx(bar_w + 8 * t, C::B_STAGE);
+      bulk_g2s(b_base + t * C::B_STAGE, wtc + (size_t)t * (C::B_STAGE / 2), C::B_STAGE, bar_w + 8 * t);
+    }
+    if constexpr (!C::ALIAS) issue_tile(blockIdx.x, 0);
+  }
+  __syncthreads();
+
+  const int lrow = HALO + g.gemm_row(wg * 64 + (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8);
+  const int lchunk = lane >> 4;
+  const int arow0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int acol = 2 * (lane & 3);
+
+  int it = 0;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+    const int seg0 = tile * G;
+    const int g0 = kSplitLead + seg0 * BLK - HALO;
+    const int ab = C::A_BUFS == 1 ? 0 : (it & 1);
+    if constexpr (C::ALIAS) {
+      if (tid == 0) issue_tile(tile, 0);
+      mbar_wait(bar_full, it & 1);
+    } else if constexpr (C::A_BUFS == 1) {
+      mbar_wait(bar_full, it & 1);
+    } else {
+      const int next = tile + gridDim.x;
+      if (tid == 0 && next < n_tiles) {
+        const int nb = (it + 1) & 1;
+        mbar_wait(bar_empty + 8 * nb, (((it + 1) >> 1) & 1) ^ 1);
+        issue_tile(next, nb);
+      }
+      mbar_wait(bar_full + 8 * ab, (it >> 1) & 1);
+    }
+
+    const uint32_t a_hi = sbase + C::OFF_A_HI + ab * C::A_BUF, a_lo = a_hi + C::A_BYTES;
+    float acc_m[1][C::COUT / 2], acc_s[1][C::COUT / 2];
+#pragma unroll
+    for (int i = 0; i < C::COUT / 2; ++i) { acc_m[0][i] = 0.f; acc_s[0][i] = 0.f; }
+    if (__shfl_sync(0xffffffffu, wg < g.NBLK, 0)) {
+      const int row[1] = {(g0 & 7) + lrow};
+      for (int t = 0; t < NTAP; ++t) mbar_wait(bar_w + 8 * t, 0);
+      tile_gemm_rt<C>(acc_m, acc_s, a_hi, a_lo, b_base, row, lchunk, g.P);
+    }
+    if constexpr (C::A_BUFS == 2) mbar_arrive(bar_empty + 8 * ab);
+    __syncthreads();
+    if constexpr (!C::ALIAS && C::A_BUFS == 1) {
+      if (tid == 0 && tile + (int)gridDim.x < n_tiles) issue_tile(tile + gridDim.x, 0);
+    }
+
+    float2 bb[C::COUT / 8];
+    load_bias<C>(bias, acol, bb);
+    stage_rows_rt<C>(g, acc_m[0], acc_s[0], arow0, acol, seg0, n_seg, bb, out_scale, stg);
+    __syncthreads();
+
+    store_tile_rt<C>(g, stg, seg0, min(G, n_seg - seg0), tid, NT, store_scale, out_hi, out_lo, out_f32);
+    if constexpr (C::ALIAS) {
+      fence_proxy_async();
+      __syncthreads();
+    }
+  }
+}
+
 // ---- conv1 + pool1 + conv2 + pool2 ----
 // conv1 + BN + ReLU + pool1 (conv1_cell.cuh, the same fp32 arithmetic as conv1_pool1_kernel) of one segment per tile
 // goes straight into the A tile; the conv2 GEMM and epilogue are the same code on the same values as conv_split_kernel,
@@ -574,16 +781,34 @@ static void launch_c12(cudaStream_t st, const __half* wtc, const float* b, float
                                                                       mel, seg_frame0, seg_thr, w1, b1, c1_scale);
 }
 
+template <class C>
+static void launch_sp_rt(cudaStream_t st, const unsigned char* in_hi, const unsigned char* in_lo, const __half* wtc,
+                         const float* b, float scale, float store_scale, unsigned char* out_hi, unsigned char* out_lo,
+                         float* out_f32, int n_seg, const SpGeom& g) {
+  static unsigned long long configured = 0;
+  static int n_sm = 0;
+  if (first_launch_on_device(configured)) {
+    cudaFuncSetAttribute(conv_split_rt_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    n_sm = device_sms();
+  }
+  const int n_tiles = (n_seg + g.G - 1) / g.G;
+  const int grid = std::min(n_tiles, n_sm);
+  conv_split_rt_kernel<C><<<grid, C::NT, C::SMEM_BYTES, st>>>(in_hi, in_lo, wtc, b, scale, store_scale, out_hi, out_lo,
+                                                              out_f32, n_seg, g);
+}
+
 #define NISQA_SP_GEOM(L, CI, CO) static_assert(input_is<SpAdapt<L, CI, CO>>(0, L), "SpCfg geometry differs from split_geometry");
 NISQA_SP_ADAPT_LAYERS(NISQA_SP_GEOM)
 #undef NISQA_SP_GEOM
 static_assert(input_is<SpConv2S>(1, 2) && input_is<SpConv3S>(1, 3) && input_is<SpConv4S>(1, 4) && input_is<SpConv5S>(1, 5) &&
               input_is<SpConv6S>(1, 6), "SpCfg geometry differs from split_geometry");
+static_assert(kMaxPoolW + 2 <= kSplitLead && kMaxPoolCells <= 256,
+              "the run-time geometry kernels: a halo of at most kSplitLead rows, one segment per 256-row tile at least");
 
 // Bytes of one plane of the pair that feeds conv layer `layer` (2..6) with C channels for n_seg segments: per segment
 // (H + 1) rows of W + 1 pixels (shared zero row / column), the zero lead rows and the tile over-read.
-size_t split_plane_bytes(int std_mode, int layer, int C, int n_seg) {
-  const ConvGeom g = split_geometry(std_mode, layer, C);
+size_t split_plane_bytes(int std_mode, int layer, int C, int n_seg, const CnnPools& pools) {
+  const ConvGeom g = split_geometry(std_mode, layer, C, pools);
   const size_t rows = (size_t)kSplitLead + (size_t)n_seg * (g.H + 1) * (g.W + 1) + 256 + 32;
   return (rows * (size_t)g.C * 2 + 1023) & ~(size_t)1023;
 }
@@ -593,15 +818,31 @@ bool conv_split_supported(int cin, int cout) {
 }
 
 // conv layer 2..6 (cin -> cout channels) on planes; the last layer (6) writes the fp32 CNN features (adapt:
-// [seg][6][c3] in rows padded to a multiple of 64 floats; standard: [seg][6][2][64]).  false: no instance for the shape.
+// [seg][pool_3 h][c3] in rows padded to a multiple of 64 floats; standard: [seg][6][2][64]).  AdaptCNN layers whose input
+// map and output pooling are the shipped ones run the compile-time instances, every other one the run-time geometry
+// kernel.  false: no instance for the shape.
 bool launch_conv_split(cudaStream_t st, int std_mode, int layer, int cin, int cout, const void* in_hi, const void* in_lo,
                        const void* wtc, const float* b, float out_scale, float store_scale, void* out_hi,
-                       void* out_lo, float* out_f32, int n_seg) {
+                       void* out_lo, float* out_f32, int n_seg, const CnnPools& pools) {
   const __half* w = reinterpret_cast<const __half*>(wtc);
   const unsigned char* ih = static_cast<const unsigned char*>(in_hi);
   const unsigned char* il = static_cast<const unsigned char*>(in_lo);
   unsigned char* oh = static_cast<unsigned char*>(out_hi);
   unsigned char* ol = static_cast<unsigned char*>(out_lo);
+  if (!std_mode && !shipped_layer_geometry(layer, pools)) {
+    const ConvGeom in = split_geometry(0, layer, cin, pools);
+    const ConvGeom out = layer < 6 ? split_geometry(0, layer + 1, cout, pools) : ConvGeom{in.H, 1, cout};
+    const SpGeom g = sp_geom(layer, in.H, in.W, out.H, out.W, cout);
+    const int ntap = layer == 6 ? 3 * in.W : 9;
+#define NISQA_SP_RT_LAUNCH(L, CI, CO, NT)                                                                    \
+    if (layer == L && cin == CI && cout == CO && ntap == NT) {                                                \
+      launch_sp_rt<SpRt<L, CI, CO, NT>>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg, g);  \
+      return true;                                                                                            \
+    }
+    NISQA_SP_RT_LAYERS(NISQA_SP_RT_LAUNCH)
+#undef NISQA_SP_RT_LAUNCH
+    return false;
+  }
   if (!std_mode) {
 #define NISQA_SP_LAUNCH(L, CI, CO)                                                                           \
     if (layer == L && cin == CI && cout == CO) {                                                              \
@@ -641,8 +882,8 @@ void launch_conv12(cudaStream_t st, int std_mode, int c2, const float* mel, cons
 }
 
 void launch_unsplit(cudaStream_t st, int std_mode, int layer, int C, const void* hi, const void* lo, float unit, float* out,
-                    int n_seg) {
-  const ConvGeom g = split_geometry(std_mode, layer, C);
+                    int n_seg, const CnnPools& pools) {
+  const ConvGeom g = split_geometry(std_mode, layer, C, pools);
   const long long items = (long long)n_seg * g.H * g.W * (g.C / 8);
   const unsigned char* h = static_cast<const unsigned char*>(hi);
   const unsigned char* l = static_cast<const unsigned char*>(lo);

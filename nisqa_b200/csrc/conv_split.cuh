@@ -24,6 +24,8 @@ template <int H_, int W_, int CIN_, int COUT_, int POOL_, int POW_, bool F32OUT_
 struct SpCfg {
   static constexpr int NT = 4 * 128;             // four warpgroups; warpgroup b < NBLK runs m64 block b
   static constexpr int H = H_, W = W_, CIN = CIN_, COUT = COUT_, POOL = POOL_, POW = POW_;
+  static constexpr int NTAP = 9;                  // weight taps (3 x 3)
+  static constexpr bool ONE_STEP_UNITS = H == 24 && COUT == 64;   // conv2 at 64 output channels (TapUnits)
   static constexpr bool CENTER = CENTER_;         // conv6 of the AdaptCNN: kernel (3,3), padding (1,0) on a
                                                   // 3-wide map == the padded conv evaluated at column 1 only
   static constexpr bool OUT_SPLIT = !F32OUT_;     // the last layer writes the CNN features as fp32 channels-last
@@ -120,6 +122,77 @@ using SpConv3S = SpCfg<12, 4, 32, 64, SP_POOL_NONE, 0>;
 using SpConv4S = SpCfg<12, 4, 64, 64, SP_POOL_2X2, 2>;
 using SpConv5S = SpCfg<6, 2, 64, 64, SP_POOL_NONE, 0>;
 using SpConv6S = SpCfg<6, 2, 64, 64, SP_POOL_NONE, 0, true>;
+
+// ---- AdaptCNN layers whose map sizes come from the checkpoint's pools (cnn_pool_1/2/3) ----
+// Run-time geometry of one such layer (conv_split_rt_kernel): the members of SpCfg that depend on H and W.
+//   conv2..conv5: 3 x 3 taps, padding 1, output H x W, then (conv2, conv4) adaptive max-pool to HO x WO.
+//   conv6: kernel (3, W), padding (1, 0): output H x 1, written as the fp32 CNN features [seg][H][COUT].
+// GEMM row m reads its taps around plane row HALO + gemm_row(m), at column w + 1 (conv6: column 1).
+struct SpGeom {
+  int H, W, P, BLK, G, HALO, KW, SEG_ROWS, KEPT, NBLK;
+  int HO, WO, OP, OBLK;      // the output map (the next layer's input): pooled, H x W, or H x 1 (conv6)
+  int OUT_COLS, OUT_LD;      // conv6: H COUT features in rows of OUT_LD floats (a multiple of 64, zero-padded)
+  __host__ __device__ int gemm_row(int m) const {
+    if (m >= KEPT) return 0;
+    const int s = m / SEG_ROWS, q = m - s * SEG_ROWS, h = q / KW, w = q - h * KW;
+    return s * BLK + (h + 1) * P + w + 1;
+  }
+};
+// (H, W) input -> (HO, WO) output of conv layer `layer` (2..6) with COUT output channels
+inline SpGeom sp_geom(int layer, int H, int W, int HO, int WO, int cout) {
+  SpGeom g;
+  g.H = H; g.W = W; g.P = W + 1; g.BLK = (H + 1) * g.P; g.G = 256 / g.BLK; g.HALO = g.P + 1;
+  g.KW = layer == 6 ? 1 : W;
+  g.SEG_ROWS = H * g.KW; g.KEPT = g.G * g.SEG_ROWS; g.NBLK = (g.KEPT + 63) / 64;
+  g.HO = layer == 6 ? H : HO; g.WO = layer == 6 ? 1 : WO;
+  g.OP = g.WO + 1; g.OBLK = (g.HO + 1) * g.OP;
+  g.OUT_COLS = g.HO * g.WO * cout; g.OUT_LD = (g.OUT_COLS + 63) / 64 * 64;
+  return g;
+}
+
+// Compile-time part of a run-time geometry layer L (2..6) with CIN -> COUT channels and NTAP = 3 x KX weight taps (conv6:
+// KX = its input width 1..3; the others 3 x 3 with padding 1).  Shared memory is sized for the largest accepted map, a
+// 256-row tile whose halo is kSplitLead rows; otherwise the layout rules are SpCfg's.
+template <int L, int CIN_, int COUT_, int NTAP_ = 9>
+struct SpRt {
+  static constexpr int NT = 4 * 128;
+  static constexpr int CIN = CIN_, COUT = COUT_, NTAP = NTAP_, KX = NTAP / 3, PADX = L == 6 ? 0 : 1;
+  static constexpr bool ONE_STEP_UNITS = L == 2 && COUT == 64;
+  static constexpr bool POOLED = L == 2 || L == 4, OUT_SPLIT = L != 6;
+  static constexpr int AROWS = 256 + 2 * kSplitLead;
+  static constexpr int ROWB = CIN * 2;
+  static constexpr int A_BYTES = ((AROWS + 7) * ROWB + 1023) & ~1023;
+  static constexpr int NCH = CIN / 8;
+  static constexpr int B_HALF = NCH * COUT * 16;
+  static constexpr int B_STAGE = 2 * B_HALF;
+  static constexpr int STG_STRIDE = COUT + 4;
+  static constexpr int STG_BYTES = 256 * STG_STRIDE * 4;
+  static constexpr int SMEM_BUDGET = 227 * 1024 - 2048;
+  static constexpr int A_BUF = 2 * A_BYTES;
+  static constexpr int ONE_BUF = A_BUF + STG_BYTES + NTAP * B_STAGE;
+  static constexpr bool ALIAS = ONE_BUF > SMEM_BUDGET;
+  static constexpr int A_BUFS = (ALIAS || ONE_BUF + A_BUF > SMEM_BUDGET) ? 1 : 2;
+  static constexpr int OFF_A_HI = 0;
+  static constexpr int OFF_A_LO = A_BYTES;
+  static constexpr int OFF_STG = ALIAS ? 0 : A_BUFS * A_BUF;
+  static constexpr int OFF_B = ((ALIAS ? (A_BUF > STG_BYTES ? A_BUF : STG_BYTES) : A_BUFS * A_BUF + STG_BYTES) + 1023) & ~1023;
+  static constexpr int OFF_BAR = OFF_B + NTAP * B_STAGE;
+  static constexpr int NBAR = NTAP + 2 * A_BUFS;
+  static constexpr int SMEM_BYTES = OFF_BAR + 8 * NBAR + 1024;
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
+  static_assert(ALIAS || A_BUFS * A_BUF + STG_BYTES + NTAP * B_STAGE <= SMEM_BUDGET, "buffers");
+  static_assert(CIN % 16 == 0 && (COUT == 16 || COUT == 32 || COUT == 64), "shape");
+  static_assert(NTAP % 3 == 0 && (L == 6 || NTAP == 9), "taps");
+};
+// X(layer, CIN, COUT, NTAP) for every run-time geometry instance: the (layer, CIN, COUT) of NISQA_SP_ADAPT_LAYERS for
+// conv2..conv5, conv6 per width and tap count 3, 6, 9 (pool_3 widths 1, 2, 3)
+#define NISQA_SP_RT_TO(X, L, CO) X(L, 16, CO, 9) X(L, 32, CO, 9) X(L, 64, CO, 9)
+#define NISQA_SP_RT_C6(X, C) X(6, C, C, 3) X(6, C, C, 6) X(6, C, C, 9)
+#define NISQA_SP_RT_LAYERS(X)                                                                          \
+  NISQA_SP_RT_TO(X, 2, 16) NISQA_SP_RT_TO(X, 2, 32) NISQA_SP_RT_TO(X, 2, 64)                           \
+  NISQA_SP_RT_TO(X, 3, 16) NISQA_SP_RT_TO(X, 3, 32) NISQA_SP_RT_TO(X, 3, 64)                           \
+  X(4, 16, 16, 9) X(4, 32, 32, 9) X(4, 64, 64, 9) X(5, 16, 16, 9) X(5, 32, 32, 9) X(5, 64, 64, 9)     \
+  NISQA_SP_RT_C6(X, 16) NISQA_SP_RT_C6(X, 32) NISQA_SP_RT_C6(X, 64)
 
 // Shared memory of the fused conv1 + conv2 kernel (conv12_kernel) on the conv2 geometry C: two activation buffers
 // (conv1 fills one while the GEMM reads the other), two staging tiles (tile i's is written while stragglers of the

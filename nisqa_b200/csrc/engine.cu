@@ -106,7 +106,7 @@ struct Lane {
   DevBuf act[7];           // act[l]: fp32 channels-last map feeding conv layer l (2..6) on the FFMA path (and stage dumps)
   DevBuf planes[7];        // planes[l]: fp16 hi | lo plane pair feeding conv layer l (2..6), conv_split.cu
   size_t plane_bytes[7] = {0, 0, 0, 0, 0, 0, 0};   // offset of the lo plane inside planes[l] (half of the allocation)
-  int plane_c[7] = {0, 0, 0, 0, 0, 0, 0};          // channels per row planes[l] was zeroed for (its zero rows / columns)
+  ConvGeom plane_g[7] = {};                        // the map planes[l] was zeroed for (its zero rows / columns)
   void release() {
     for (auto& b : act) b.release();
     for (auto& b : planes) b.release();
@@ -163,7 +163,8 @@ struct Weights {
   // c1 / c2 / c3 / c3 / c3 / c3 with each in {16, 32, 64}, StandardCNN 16 / 32 / 64 / 64 / 64 / 64
   int cnn_c[7] = {1, 16, 32, 64, 64, 64, 64};
   bool shipped_channels() const { return cnn_c[1] == 16 && cnn_c[2] == 32 && cnn_c[3] == 64; }
-  int feat_cols() const { return 6 * cnn_c[6]; }                  // AdaptCNN's framewise fan-out (lib:706)
+  CnnPools pools = kShippedPools;  // AdaptCNN's cnn_pool_1/2/3 (nisqa_set_cnn_pools before the load)
+  int feat_cols() const { return pools.p[4] * cnn_c[6]; }         // AdaptCNN's framewise fan-out c3 h3 (lib:706)
   int feat_ld() const { return (feat_cols() + 63) / 64 * 64; }    // its row stride: zero columns up to a multiple of 64
   const float* ff_bn = nullptr;  // SkipCNN / DFF: BatchNorm2d(1) as (scale, shift)
   Linear ff[4];                  // SkipCNN's Linear, or DFF's four, BatchNorm1d folded in
@@ -204,6 +205,7 @@ struct nisqa_engine {
   int lstm_batched = 1;    // BiLSTM: NB clips per CTA in lock step (td.cu lstm_batched_kernel); 0: one CTA per (clip, direction)
   int keep_td_out = 0;     // standard arch: also write the per-step LSTM outputs [n_seg][256] (only the stage dump reads them)
   int conv_tc = 1;         // 1: conv2..6 on the tensor cores (fp16 two-term split, fp16 plane pairs between the layers); 0: fp32 FFMA
+  CnnPools pools_next = kShippedPools;   // AdaptCNN pools of the next nisqa_load_weights (nisqa_set_cnn_pools)
   std::vector<TimerSlot> timers;
 
   // weights arena (device) and the pointers into it
@@ -234,10 +236,11 @@ struct nisqa_engine {
   // SkipCNN / DFF rows: n_mels * seg_len features (x.view(-1, fan_in), lib:520 / 556), zero-padded to a multiple of 64
   int ff_fan_in() const { return cfg.n_mels * cfg.seg_len; }
   int ff_fan_in_pad() const { return (ff_fan_in() + 63) / 64 * 64; }
-  // conv1 + conv2 in one kernel (conv_split.cu): tensor-core path, the shipped 48 x 15 segments, conv1 16 channels wide
+  // conv1 + conv2 in one kernel (conv_split.cu): tensor-core path, the shipped 48 x 15 segments, pool_1 and pool_2, conv1
+  // 16 channels wide
   bool fused12() const {
     return conv_tc != 0 && conv12 != 0 && cfg.n_mels == kMels && cfg.seg_len == kSegLen &&
-           conv12_supported(std_cnn(), w.cnn_c[1], w.cnn_c[2]);
+           (std_cnn() || shipped_layer_geometry(2, w.pools)) && conv12_supported(std_cnn(), w.cnn_c[1], w.cnn_c[2]);
   }
   int pool_d() const { return cfg.td2_layers > 0 ? td2_d() : sa_d(); }
 
@@ -266,7 +269,7 @@ struct nisqa_engine {
   const float* last_td_out = nullptr;
   int last_td_out_d = 64;       // row width of last_td_out
   int last_td_out_ld = 0;       // its row stride (0: the width)
-  int last_td_out_hw = 0;       // td = 'skip': conv6 features in the engine's order [hw][c3] (6 / 12); 0: the reference's
+  int last_td_out_hw = 0;       // td = 'skip': conv6 features in the engine's order [hw][c3] (pool_3 h / 12); 0: the reference's
   const float* last_td1_out = nullptr;    // td's output when a td_2 stage ran (NISQA_STAGE_TD1_OUT)
   int last_td1_out_d = 0, last_td1_out_ld = 0;
 
@@ -482,10 +485,12 @@ struct Packer {
   void copy(const float*& dst, const float* src, size_t n) { memcpy(&arena[alloc(dst, n)], src, n * 4); }
 };
 
-// conv<idx> with bn<idx> folded in, as [ci][tap][co] (conv1: [tap][16]); *w_off: the offset of the weights in the arena
-bool pack_conv(Packer& P, int idx, int cin, int cout, int* act_exp, size_t* w_off) {
+// conv<idx> (kernel 3 x kw: AdaptCNN's conv6 is 3 x pool_3[1]) with bn<idx> folded in, as [ci][tap][co] (conv1: [tap][16]),
+// tap = ky kw + kx; *w_off: the offset of the weights in the arena
+bool pack_conv(Packer& P, int idx, int cin, int cout, int* act_exp, size_t* w_off, int kw = 3) {
   const std::string cv = "cnn.model.conv" + std::to_string(idx) + ".", bn = "cnn.model.bn" + std::to_string(idx) + ".";
-  const TensorView* w = P.get(cv + "weight", {cout, cin, 3, 3});
+  const int ntap = 3 * kw;
+  const TensorView* w = P.get(cv + "weight", {cout, cin, 3, kw});
   const TensorView* b = P.get(cv + "bias", {cout});
   const TensorView* g = P.get(bn + "weight", {cout});
   const TensorView* be = P.get(bn + "bias", {cout});
@@ -497,39 +502,39 @@ bool pack_conv(Packer& P, int idx, int cin, int cout, int* act_exp, size_t* w_of
   double E = 0.0;
   for (int co = 0; co < cout; ++co) E = std::max(E, fabs((double)be->d[co]) + 3.0 * fabs((double)g->d[co]));
   *act_exp = (E > 0.0 && std::isfinite(E)) ? ilogb(E * sqrt(2.0) / 4.0) : 0;
-  const size_t wo = P.alloc(P.w.conv[idx].w, (size_t)cin * 9 * cout);
+  const size_t wo = P.alloc(P.w.conv[idx].w, (size_t)cin * ntap * cout);
   const size_t bo = P.alloc(P.w.conv[idx].b, cout);
   for (int co = 0; co < cout; ++co) {
     // eval-mode BatchNorm2d (eps 1e-5) folded into the convolution (SURVEY.md Appendix A)
     const double s = (double)g->d[co] / sqrt((double)var->d[co] + 1e-5);
     P.arena[bo + co] = (float)(((double)b->d[co] - (double)mu->d[co]) * s + (double)be->d[co]);
     for (int ci = 0; ci < cin; ++ci)
-      for (int tap = 0; tap < 9; ++tap)
-        P.arena[wo + ((size_t)ci * 9 + tap) * cout + co] =
-            (float)((double)w->d[((size_t)co * cin + ci) * 9 + tap] * s);
+      for (int tap = 0; tap < ntap; ++tap)
+        P.arena[wo + ((size_t)ci * ntap + tap) * cout + co] =
+            (float)((double)w->d[((size_t)co * cin + ci) * ntap + tap] * s);
   }
   *w_off = wo;
   return true;
 }
 
-// conv2..conv6 for the tensor-core path, from the folded fp32 weights at `src`: [tap][ci/8][hi co | lo co][8] fp16
-// two-term split of w * 2^S, S chosen so that max|w| 2^S lies in (512, 1024] whatever the weights' range (b_lo stays out
-// of the fp16 subnormals)
-void pack_conv_tc(Packer& P, int idx, int ci_n, int co_n, size_t src, int act_exp_in, float* tc_scale) {
+// conv2..conv6 for the tensor-core path, from the folded fp32 weights at `src` (ntap taps): [tap][ci/8][hi co | lo co][8]
+// fp16 two-term split of w * 2^S, S chosen so that max|w| 2^S lies in (512, 1024] whatever the weights' range (b_lo stays
+// out of the fp16 subnormals)
+void pack_conv_tc(Packer& P, int idx, int ci_n, int co_n, size_t src, int act_exp_in, float* tc_scale, int ntap = 9) {
   float wmax = 0.f;
-  for (size_t j = 0; j < (size_t)ci_n * 9 * co_n; ++j) wmax = std::max(wmax, fabsf(P.arena[src + j]));
+  for (size_t j = 0; j < (size_t)ci_n * ntap * co_n; ++j) wmax = std::max(wmax, fabsf(P.arena[src + j]));
   int S = 0;
   if (wmax > 0.f && std::isfinite(wmax)) {
     S = 9 - ilogbf(wmax);                                         // max|w| 2^S in [512, 1024)
     if (ldexpf(wmax, S) == 512.f) ++S;                            // a power of two: 1024 itself
   }
   *tc_scale = ldexpf(1.f, act_exp_in - S);
-  const size_t n_half = (size_t)9 * 2 * ci_n * co_n;
+  const size_t n_half = (size_t)ntap * 2 * ci_n * co_n;
   const size_t dst = P.alloc(P.w.conv[idx].wtc, (n_half + 1) / 2);   // fp16 payload inside the float arena
-  for (int tap = 0; tap < 9; ++tap)
+  for (int tap = 0; tap < ntap; ++tap)
     for (int ci = 0; ci < ci_n; ++ci)
       for (int co = 0; co < co_n; ++co) {
-        const float w = ldexpf(P.arena[src + ((size_t)ci * 9 + tap) * co_n + co], S);
+        const float w = ldexpf(P.arena[src + ((size_t)ci * ntap + tap) * co_n + co], S);
         const __half hi = __float2half_rn(w);
         const __half lo = __float2half_rn(w - __half2float(hi));
         __half* base = reinterpret_cast<__half*>(&P.arena[dst]) + (size_t)tap * 2 * ci_n * co_n;
@@ -632,10 +637,17 @@ bool pack_framewise(Packer& P, nisqa_engine* e) {
   if (!e->conv_net()) return pack_ffnet(P, c);
   int* cc = P.w.cnn_c;
   if (!e->std_cnn() && !read_cnn_channels(P, cc)) return false;
+  if (!e->std_cnn()) P.w.pools = e->pools_next;
+  const int h3 = P.w.pools.p[4], w3 = e->std_cnn() ? 3 : P.w.pools.p[5];
+  if (!e->std_cnn() && h3 * cc[6] > kMaxCnnFeatures)
+    return P.fail("tensor cnn.model.conv6.weight: " + std::to_string(cc[6]) + " channels x pool_3 height " + std::to_string(h3) +
+                  " = " + std::to_string(h3 * cc[6]) + " features (cnn_c_out_3 x cnn_pool_3[0]): the engine runs up to " +
+                  std::to_string(kMaxCnnFeatures));
   for (int i = 1; i <= 6; ++i) {
     size_t w_off = 0;
-    if (!pack_conv(P, i, cc[i - 1], cc[i], &e->act_exp[i], &w_off)) return false;
-    if (i >= 2) pack_conv_tc(P, i, cc[i - 1], cc[i], w_off, e->act_exp[i - 1], &e->tc_scale[i]);
+    const int kw = i == 6 ? w3 : 3;        // conv6: kernel (3, pool_3[1]), padding (1, 0) (lib:674-678)
+    if (!pack_conv(P, i, cc[i - 1], cc[i], &e->act_exp[i], &w_off, kw)) return false;
+    if (i >= 2) pack_conv_tc(P, i, cc[i - 1], cc[i], w_off, e->act_exp[i - 1], &e->tc_scale[i], 3 * kw);
   }
   if (c.cnn_fc > 0) {
     // AdaptCNN's optional Linear (lib:682-684, 708-709): k-major, rows in the engine's feature order h*c3 + c, zero rows
@@ -645,21 +657,21 @@ bool pack_framewise(Packer& P, nisqa_engine* e) {
     const TensorView* b = P.get("cnn.model.fc.bias", {H});
     if (!w || !b) return false;
     const size_t ow = P.alloc(P.w.ffc.wT, (size_t)P.w.feat_ld() * H);
-    for (int h = 0; h < 6; ++h)
+    for (int h = 0; h < h3; ++h)
       for (int ch = 0; ch < C3; ++ch)
-        for (int j = 0; j < H; ++j) P.arena[ow + ((size_t)h * C3 + ch) * H + j] = w->d[(size_t)j * K + ch * 6 + h];
+        for (int j = 0; j < H; ++j) P.arena[ow + ((size_t)h * C3 + ch) * H + j] = w->d[(size_t)j * K + ch * h3 + h];
     P.copy(P.w.ffc.b, b->d, H);
   }
   return true;
 }
 
 // The rows that feed a time-dependency stage: `dim` features, padded with zero columns to a multiple of 64, in the order
-// of the checkpoint's Linear (PLAIN) or - conv6's `ch` channels - in the engine's order: AdaptCNN k' = h*ch + c <->
-// reference view(-1, ch*6) order c*6 + h (lib:706), StandardCNN k' = (h*2 + w)*64 + c <-> c*12 + h*2 + w (lib:830)
+// of the checkpoint's Linear (PLAIN) or - conv6's `ch` channels over `h` rows - in the engine's order: AdaptCNN k' = h*ch + c
+// <-> reference view(-1, ch*h3) order c*h3 + h (lib:706), StandardCNN k' = (h*2 + w)*64 + c <-> c*12 + h*2 + w (lib:830)
 enum InOrder { IN_PLAIN, IN_ADAPT_CONV, IN_STD_CONV };
-struct InRows { int dim; InOrder order; int ch = 64; };
+struct InRows { int dim; InOrder order; int ch = 64; int h = 6; };
 int in_col(const InRows& in, int k) {
-  return in.order == IN_ADAPT_CONV ? (k % in.ch) * 6 + k / in.ch : in.order == IN_STD_CONV ? (k & 63) * 12 + (k >> 6) : k;
+  return in.order == IN_ADAPT_CONV ? (k % in.ch) * in.h + k / in.ch : in.order == IN_STD_CONV ? (k & 63) * 12 + (k >> 6) : k;
 }
 
 // One SelfAttention stack (lib:945-1040) of width D and feed-forward width F, checkpoint prefix `ck`: Linear(in -> D) +
@@ -925,7 +937,7 @@ bool pack_td_model(Packer& P, nisqa_engine* e) {
   const nisqa_config& c = e->cfg;
   Weights& W = P.w;
   const std::string td = "time_dependency.model.", td2 = "time_dependency_2.model.";
-  // the rows feeding td: AdaptCNN's 6 c3 (engine order; 96 padded to 128 at c3 = 16), SkipCNN's n_mels * seg_len (padded
+  // the rows feeding td: AdaptCNN's h3 c3 (engine order; 96 padded to 128 at 6 x 16), SkipCNN's n_mels * seg_len (padded
   // to a multiple of 64 with zero rows: 720 -> 768 at 48 x 15), cnn_fc_out_h, or
   // StandardCNN's fc_out / 768 conv6 features (engine order)
   InRows in;
@@ -935,7 +947,7 @@ bool pack_td_model(Packer& P, nisqa_engine* e) {
   } else {
     const bool conv_net = c.cnn_kind == NISQA_CNN_CONV;
     in = {c.cnn_fc > 0 ? c.cnn_fc : (conv_net ? W.feat_cols() : e->ff_fan_in()), conv_net && c.cnn_fc == 0 ? IN_ADAPT_CONV : IN_PLAIN,
-          W.cnn_c[6]};
+          W.cnn_c[6], W.pools.p[4]};
   }
   const Weights::LstmShape* last_lstm = nullptr;      // the last stage, when it is an LSTM
   int d1;                                             // td's fan_out
@@ -1185,7 +1197,8 @@ int conv_layers(Pass& p) {
     Scope s(e, "conv1");
     if (!launch_conv1(p.st, p.std_mode, cc[1], LN.mel.as<float>(), p.c.n_mels, p.c.seg_len, p.seg_frame0, p.seg_thr,
                       w.conv[1].w, w.conv[1].b, split ? nullptr : LN.act[2].as<float>(), p.n_seg,
-                      split ? plane_hi(2) : nullptr, split ? plane_lo(2) : nullptr, e->act_store(1)))
+                      split ? plane_hi(2) : nullptr, split ? plane_lo(2) : nullptr, e->act_store(1), w.pools.p[0],
+                      w.pools.p[1]))
       return no_kernel(1);
   }
   static const char* const names[7] = {"", "", "conv2", "conv3", "conv4", "conv5", "conv6"};
@@ -1194,7 +1207,7 @@ int conv_layers(Pass& p) {
     if (split) {
       if (!launch_conv_split(p.st, p.std_mode, l, cc[l - 1], cc[l], plane_hi(l), plane_lo(l), w.conv[l].wtc, w.conv[l].b,
                              e->tc_scale[l], e->act_store(l), l < 6 ? plane_hi(l + 1) : nullptr,
-                             l < 6 ? plane_lo(l + 1) : nullptr, l == 6 ? LN.feats.as<float>() : nullptr, p.n_seg))
+                             l < 6 ? plane_lo(l + 1) : nullptr, l == 6 ? LN.feats.as<float>() : nullptr, p.n_seg, w.pools))
         return no_kernel(l);
     } else {
       launch_conv_layer(p.st, p.std_mode, l, LN.act[l].as<float>(), w.conv[l].w, w.conv[l].b,
@@ -1244,13 +1257,14 @@ int framewise(Pass& p, int fmt, Rows* out) {
     if (split) {
       // the lo plane sits at a fixed offset of the ALLOCATION (not of this pass's n_seg): the zero rows /
       // columns of both planes must stay where they were when the buffer was cleared.  No kernel writes them, so a
-      // buffer cleared for another row width (weights of other channel counts loaded since) is cleared again.
-      const int C = p.w.cnn_c[l - 1];
-      if (LN.plane_c[l] != C) {
+      // buffer cleared for another row width or map size (weights of other channel counts or pools loaded since) is
+      // cleared again.
+      const ConvGeom g = split_geometry(p.std_mode, l, p.w.cnn_c[l - 1], p.w.pools);
+      if (LN.plane_g[l].C != g.C || LN.plane_g[l].H != g.H || LN.plane_g[l].W != g.W) {
         LN.planes[l].release();
-        LN.plane_c[l] = C;
+        LN.plane_g[l] = g;
       }
-      CK(LN.planes[l].reserve_zeroed(2 * split_plane_bytes(p.std_mode, l, C, n_seg), p.st));
+      CK(LN.planes[l].reserve_zeroed(2 * split_plane_bytes(p.std_mode, l, g.C, n_seg, p.w.pools), p.st));
       LN.plane_bytes[l] = (LN.planes[l].cap / 2) & ~(size_t)1023;
     } else {
       const ConvGeom g = split_geometry(p.std_mode, l, p.w.cnn_c[l - 1]);
@@ -1493,7 +1507,7 @@ int td_stages(Pass& p, Rows rows) {
   e->last_td_out_ld = 64 * cur.nk;
   e->last_td_out_hw = 0;
   if (skip && !e->td2_runs()) {
-    if (cur.x == LN.feats.as<float>()) e->last_td_out_hw = p.std_mode ? 12 : 6;      // conv6 features, engine order
+    if (cur.x == LN.feats.as<float>()) e->last_td_out_hw = p.std_mode ? 12 : w.pools.p[4];   // conv6 features, engine order
     return pool_framewise(p, cur.x, D, 64 * cur.nk);
   }
   return pool_rows(p, cur.x, D, 64 * cur.nk, lstm2 || (!sa1 && !sa2));
@@ -1560,6 +1574,13 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
     return fail(e, NISQA_ERR_STATE, "conv_tc=0: the fp32 FFMA convolutions run AdaptCNN channel counts 16 / 32 / 64 only, this "
                                     "checkpoint has " + std::to_string(e->w.cnn_c[1]) + " / " + std::to_string(e->w.cnn_c[2]) +
                                     " / " + std::to_string(e->w.cnn_c[3]) + " (nisqa_set_option(\"conv_tc\", 1))");
+  if (!e->conv_tc && e->conv_net() && e->w.pools != kShippedPools) {
+    const int* q = e->w.pools.p;
+    char buf[160];
+    snprintf(buf, sizeof buf, "[%d, %d] [%d, %d] [%d, %d]", q[0], q[1], q[2], q[3], q[4], q[5]);
+    return fail(e, NISQA_ERR_STATE, std::string("conv_tc=0: the fp32 FFMA convolutions run the AdaptCNN pools [24, 7] [12, 5] [6, 3] "
+                                                "only, this checkpoint has ") + buf + " (nisqa_set_option(\"conv_tc\", 1))");
+  }
   if (n_clips < 0 || (n_clips > 0 && (!n_samples || !sample_rate)))
     return fail(e, NISQA_ERR_INVALID, "null argument");
   if (fmt != NISQA_FMT_S16 && fmt != NISQA_FMT_F32) return fail(e, NISQA_ERR_INVALID, "sample_fmt");
@@ -1792,10 +1813,11 @@ int nisqa_load_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
   e->weights_loaded = false;      // a failed load may have freed the previous arena
   int prev_c[7];
   memcpy(prev_c, e->w.cnn_c, sizeof prev_c);
+  const CnnPools prev_pools = e->w.pools;
   int rc = pack_weights(e, tensors, n);
   if (rc) return rc;
-  // the last pass's maps were laid out for the previous channel counts: its stage dumps are gone with them
-  if (memcmp(prev_c, e->w.cnn_c, sizeof prev_c) != 0) e->last_passes = 0;
+  // the last pass's maps were laid out for the previous channel counts and pools: its stage dumps are gone with them
+  if (memcmp(prev_c, e->w.cnn_c, sizeof prev_c) != 0 || prev_pools != e->w.pools) e->last_passes = 0;
   e->weights_loaded = true;
   return 0;
 }
@@ -1957,7 +1979,7 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
   int width = 0, ld = 0; // rows of `width` floats at a stride of `ld` (a padded row layout)
   const int* cc = e->w.cnn_c;
   if (conv_map) {
-    const ConvGeom g = split_geometry(std_mode, layer, cc[layer - 1]);
+    const ConvGeom g = split_geometry(std_mode, layer, cc[layer - 1], e->w.pools);
     src = LN.act[layer].as<float>(); hw = g.H * g.W; ch = g.C;
   }
   switch (stage) {
@@ -1971,7 +1993,7 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
       } else if (std_mode) {
         src = LN.feats.as<float>(); hw = 12; ch = 64;           // [h*2+w][c] -> c*12+h*2+w
       } else {
-        src = LN.feats.as<float>(); hw = 6; ch = cc[6]; hw_ld = e->w.feat_ld();    // [h][c] -> c*6+h
+        src = LN.feats.as<float>(); hw = e->w.pools.p[4]; ch = cc[6]; hw_ld = e->w.feat_ld();    // [h][c] -> c*h3+h
       }
       break;
     case NISQA_STAGE_TD_IN:
@@ -2004,7 +2026,7 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
     if (from_planes) {
       CK(LN.act[layer].reserve((size_t)count * 4));
       launch_unsplit(st, std_mode, layer, ch, LN.planes[layer].as<char>(), LN.planes[layer].as<char>() + LN.plane_bytes[layer],
-                     ldexpf(1.f, e->act_exp[layer - 1]), LN.act[layer].as<float>(), (int)ns);
+                     ldexpf(1.f, e->act_exp[layer - 1]), LN.act[layer].as<float>(), (int)ns, e->w.pools);
       src = LN.act[layer].as<float>();
     }
     CK(e->dump.reserve((size_t)count * 4));
@@ -2066,6 +2088,26 @@ int nisqa_set_option(nisqa_engine* e, const char* name, int value) {
   if (strcmp(name, "keep_td_out") == 0) { e->keep_td_out = value != 0; return 0; }
   if (strcmp(name, "conv12") == 0) { e->conv12 = value != 0; return 0; }
   return fail(e, NISQA_ERR_INVALID, std::string("unknown option ") + name);
+}
+
+int nisqa_set_cnn_pools(nisqa_engine* e, const int32_t pools[6]) {
+  if (!e || !pools) return NISQA_ERR_INVALID;
+  static const char* const names[3] = {"cnn_pool_1", "cnn_pool_2", "cnn_pool_3"};
+  CnnPools q;
+  for (int i = 0; i < 3; ++i) {
+    const int h = pools[2 * i], w = pools[2 * i + 1];
+    const std::string v = std::string(names[i]) + "=[" + std::to_string(h) + ", " + std::to_string(w) + "]: ";
+    if (h < 1 || w < 1 || w > kMaxPoolW || (h + 1) * (w + 1) > kMaxPoolCells)
+      return fail(e, NISQA_ERR_INVALID, v + "the engine runs AdaptCNN pool sizes [h, w] with w <= " + std::to_string(kMaxPoolW) +
+                                            " and (h + 1) * (w + 1) <= " + std::to_string(kMaxPoolCells));
+    if (i == 2 && w > kMaxPool3W)
+      return fail(e, NISQA_ERR_INVALID, v + "the engine runs pool_3 widths 1 to 3 (conv6's kernel is 3 x pool_3[1])");
+    q.p[2 * i] = h; q.p[2 * i + 1] = w;
+  }
+  if (q != kShippedPools && !(e->conv_net() && !e->std_cnn()))
+    return fail(e, NISQA_ERR_INVALID, "cnn_pool_1/2/3: only AdaptCNN takes other pool sizes");
+  e->pools_next = q;
+  return 0;
 }
 
 int nisqa_set_profiling(nisqa_engine* e, int on) {

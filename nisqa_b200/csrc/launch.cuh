@@ -13,16 +13,38 @@ namespace nisqa {
 struct ClipDesc;
 struct FbTables;
 
+// AdaptCNN's adaptive max-pool output sizes cnn_pool_1 / 2 / 3 as h1 w1 h2 w2 h3 w3 (lib:586-710), shipped 24 x 7, 12 x 5,
+// 6 x 3.  The tensor-core kernels take any [h, w] with w <= kMaxPoolW and (h + 1) (w + 1) <= kMaxPoolCells (one
+// segment's padded map in one 256-row GEMM tile, the tap halo w + 2 within kSplitLead), pool_3 widths 1..3 (conv6's
+// 3 x w3 weight taps stay resident), and c3 h3 <= kMaxCnnFeatures framewise features.
+struct CnnPools { int p[6]; };
+constexpr CnnPools kShippedPools = {{24, 7, 12, 5, 6, 3}};
+constexpr int kMaxPoolW = 14, kMaxPoolCells = 256, kMaxPool3W = 3, kMaxCnnFeatures = 4096;
+inline bool operator==(const CnnPools& a, const CnnPools& b) {
+  for (int i = 0; i < 6; ++i) if (a.p[i] != b.p[i]) return false;
+  return true;
+}
+inline bool operator!=(const CnnPools& a, const CnnPools& b) { return !(a == b); }
+
 // Geometry of one segment's activation map that feeds conv layer `layer` (2..6), i.e. the output of layer - 1:
-// H rows, W columns, C channels.  AdaptCNN pools to widths 7 / 5 / 3 (adaptive max-pool), StandardCNN to 8 / 4 / 2
-// (MaxPool2d(2)).  C is the checkpoint's (conv layer - 1's output channels, read from its weights; StandardCNN: 16 / 32 /
-// 64); C = 0 asks for StandardCNN's.  The fp16 plane pairs (conv_split.cu), the fp32 FFMA activations and the stage
-// dumps all use it.
+// H rows, W columns, C channels.  AdaptCNN pools to cnn_pool_1 / 2 / 3 (adaptive max-pool; shipped widths 7 / 5 / 3),
+// StandardCNN to 24 x 8, 12 x 4, 6 x 2 (MaxPool2d(2)).  C is the checkpoint's (conv layer - 1's output channels, read
+// from its weights; StandardCNN: 16 / 32 / 64); C = 0 asks for StandardCNN's.  The fp16 plane pairs (conv_split.cu),
+// the fp32 FFMA activations and the stage dumps all use it.
 struct ConvGeom { int H, W, C; };
-constexpr ConvGeom split_geometry(int std_mode, int layer, int C) {
-  return {layer == 2 ? 24 : layer <= 4 ? 12 : 6,
-          std_mode ? (layer == 2 ? 8 : layer <= 4 ? 4 : 2) : (layer == 2 ? 7 : layer <= 4 ? 5 : 3),
+constexpr ConvGeom split_geometry(int std_mode, int layer, int C, const CnnPools& pools = kShippedPools) {
+  return {std_mode ? (layer == 2 ? 24 : layer <= 4 ? 12 : 6) : pools.p[layer == 2 ? 0 : layer <= 4 ? 2 : 4],
+          std_mode ? (layer == 2 ? 8 : layer <= 4 ? 4 : 2) : pools.p[layer == 2 ? 1 : layer <= 4 ? 3 : 5],
           C ? C : layer == 2 ? 16 : layer == 3 ? 32 : 64};
+}
+// true when AdaptCNN conv layer `layer` (2..6) reads the shipped input map and writes the shipped output map under `pools`:
+// it runs the compile-time SpCfg instance (conv2: pool_1 and pool_2, conv3: pool_2, conv4: pool_2 and pool_3, conv5 and
+// conv6: pool_3)
+inline bool shipped_layer_geometry(int layer, const CnnPools& pools) {
+  const int k0 = layer == 2 ? 0 : layer <= 4 ? 2 : 4, k1 = (layer == 2 || layer == 4) ? k0 + 2 : k0;
+  for (int k = k0; k <= k1 + 1; ++k)
+    if (pools.p[k] != kShippedPools.p[k]) return false;
+  return true;
 }
 // true when the layer configuration C (cnn.cu ConvCfg, conv_split.cuh SpCfg) reads that geometry (StandardCNN: with its
 // shipped input channels too; AdaptCNN's come from the weights)
@@ -89,31 +111,32 @@ void launch_mel_dump(cudaStream_t st, const float* mel, const ClipDesc* clips, i
 
 // ---------------------------------------------------------------- cnn.cu (fp32 FFMA convolutions)
 // conv1 + pool1 of segments of n_mels x seg_len mel cells (rows n_mels floats apart): AdaptCNN any accepted shape ->
-// 24 x 7, StandardCNN 48 x 15 only -> 24 x 8.  c1 output channels: 16, 32 or 64 into the planes (out_hi), 16 into fp32
-// `out`.  false: no instance for the shape.
+// ph x pw (cnn_pool_1), StandardCNN 48 x 15 only -> 24 x 8.  c1 output channels: 16, 32 or 64 into the planes (out_hi),
+// 16 into fp32 `out`.  false: no instance for the shape.
 bool launch_conv1(cudaStream_t st, int std_mode, int c1, const float* mel, int n_mels, int seg_len, const int* seg_frame0,
                   const float* seg_thr, const float* w1, const float* b1, float* out, int n_seg, void* out_hi, void* out_lo,
-                  float store_scale);
+                  float store_scale, int ph, int pw);
 void launch_conv_layer(cudaStream_t st, int std_mode, int layer, const float* in, const float* w, const float* b, float* out,
                        int n_seg);
 // rows of `ld` floats (>= hw * ch)
 void launch_nhwc_to_nchw(cudaStream_t st, const float* in, int ld, float* out, long long n, int hw, int ch);
 
 // ---------------------------------------------------------------- conv_split.cu (tensor-core convolutions on fp16 planes)
-size_t split_plane_bytes(int std_mode, int layer, int C, int n_seg);
-// AdaptCNN conv2..conv6 take cin, cout in {16, 32, 64} (the pairs cnn_c_out_1/2/3 reach); StandardCNN its shipped ones.
-// The fp32 features of conv6 go out in rows of (6 cout + 63) / 64 * 64 floats (AdaptCNN), zero-padded.
+size_t split_plane_bytes(int std_mode, int layer, int C, int n_seg, const CnnPools& pools);
+// AdaptCNN conv2..conv6 take cin, cout in {16, 32, 64} (the pairs cnn_c_out_1/2/3 reach) and any accepted pools;
+// StandardCNN its shipped ones.  The fp32 features of conv6 go out in rows of (h3 cout + 63) / 64 * 64 floats (AdaptCNN),
+// zero-padded.
 bool conv_split_supported(int cin, int cout);
 bool launch_conv_split(cudaStream_t st, int std_mode, int layer, int cin, int cout, const void* in_hi, const void* in_lo,
                        const void* wtc, const float* b, float out_scale, float store_scale, void* out_hi, void* out_lo,
-                       float* out_f32, int n_seg);
+                       float* out_f32, int n_seg, const CnnPools& pools);
 // the fused conv1 + conv2 kernel: 48 x 15 segments, c1 = 16, c2 = 32 (AdaptCNN also 16)
 bool conv12_supported(int std_mode, int c1, int c2);
 void launch_conv12(cudaStream_t st, int std_mode, int c2, const float* mel, const int* seg_frame0, const float* seg_thr,
                    const float* w1, const float* b1, float c1_scale, const void* wtc2, const float* bias2, float scale2,
                    float store_scale, void* out_hi, void* out_lo, int n_seg);
 void launch_unsplit(cudaStream_t st, int std_mode, int layer, int C, const void* hi, const void* lo, float unit, float* out,
-                    int n_seg);
+                    int n_seg, const CnnPools& pools);
 
 // ---------------------------------------------------------------- td.cu (fc_out, BiLSTM, pooling)
 void launch_fc20(cudaStream_t st, const float* feats, const float* WT, const float* b, float* out, int n_rows);

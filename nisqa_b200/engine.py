@@ -38,7 +38,7 @@ EXPORTS = [
     "nisqa_submit_pcm", "nisqa_wait", "nisqa_drain", "nisqa_join", "nisqa_set_gather_target",
     "nisqa_wav_probe", "nisqa_wav_decode", "nisqa_wav_probe_batch", "nisqa_wav_decode_batch",
     "nisqa_resample_set_filter", "nisqa_resample_out_len", "nisqa_resample_f32",
-    "nisqa_resample_device", "nisqa_predict_pcm_resampled",
+    "nisqa_resample_device", "nisqa_predict_pcm_resampled", "nisqa_set_cnn_pools",
 ]
 
 
@@ -61,6 +61,11 @@ CNN_FC_OUT_MAX = 1024                 # StandardCNN's fc_out width (None: the LS
 N_MELS = (32, 40, 48, 64, 80, 96, 128)   # ms_n_mels: one front-end kernel instance per band count
 SEG_LEN_MIN, SEG_LEN_MAX = 3, 31      # ms_seg_length, odd (128 x 31 bounds SkipCNN's / DFF's fan_in at 3968 < 4096)
 CNN_CHANNELS = (16, 32, 64)           # AdaptCNN cnn_c_out_1/2/3: one fp16 plane row is one 32 / 64 / 128-byte swizzle atom
+# AdaptCNN cnn_pool_1/2/3 [h, w]: one segment's padded (h + 1) x (w + 1) map fits a 256-row GEMM tile and the tap halo
+# w + 2 stays within the 16 lead rows of a plane; conv6's 3 x pool_3[1] weight taps stay resident (w3 <= 3); the
+# framewise fan-out c3 * h3 is at most 4096
+SHIPPED_POOLS = ((24, 7), (12, 5), (6, 3))
+POOL_W_MAX, POOL_CELLS_MAX, POOL3_W_MAX, CNN_FEATURES_MAX = 14, 256, 3, 4096
 
 
 def _sa_widths(args, prefix, de=False):
@@ -99,33 +104,60 @@ def _check_standard_cnn(args):
     ch = (args.get("cnn_c_out_1"), args.get("cnn_c_out_2"), args.get("cnn_c_out_3"))
     if ch != (16, 32, 64):
         raise NotImplementedError("cnn_c_out_1/2/3=%r: the engine runs StandardCNN with 16, 32, 64 channels" % (ch,))
+    _check_kernel_size(args)
+
+
+def _check_kernel_size(args):
     ks = args.get("cnn_kernel_size")
     if not (ks == 3 or (isinstance(ks, (list, tuple)) and tuple(ks) == (3, 3))):
         raise NotImplementedError("cnn_kernel_size=%r: the engine runs 3x3 convolutions" % (ks,))
 
 
+def _check_adapt_pools(args):
+    """AdaptCNN's (cnn_pool_1, cnn_pool_2, cnn_pool_3) as ((h, w), ...); refuses what the kernels do not implement, naming
+    the field and value."""
+    pools = []
+    for i in (1, 2, 3):
+        key = "cnn_pool_%d" % i
+        p = args.get(key)
+        ok = isinstance(p, (list, tuple)) and len(p) == 2 and all(isinstance(v, int) and v >= 1 for v in p)
+        if not ok or p[1] > POOL_W_MAX or (p[0] + 1) * (p[1] + 1) > POOL_CELLS_MAX:
+            raise NotImplementedError("%s=%r: the engine runs AdaptCNN pool sizes [h, w] with w <= %d and (h + 1) * (w + 1) "
+                                      "<= %d" % (key, p, POOL_W_MAX, POOL_CELLS_MAX))
+        if i == 3 and p[1] > POOL3_W_MAX:
+            raise NotImplementedError("%s=%r: the engine runs pool_3 widths 1 to %d (conv6's kernel is 3 x pool_3[1])"
+                                      % (key, p, POOL3_W_MAX))
+        pools.append((int(p[0]), int(p[1])))
+    c3 = int(args["cnn_c_out_3"])
+    if c3 * pools[2][0] > CNN_FEATURES_MAX:
+        raise NotImplementedError("cnn_c_out_3=%d, cnn_pool_3=%r: the engine runs up to %d framewise features "
+                                  "(cnn_c_out_3 * cnn_pool_3[0] = %d)" % (c3, args["cnn_pool_3"], CNN_FEATURES_MAX, c3 * pools[2][0]))
+    return tuple(pools)
+
+
 def _framewise(args):
-    """(cnn_kind, cnn_fc, ok) of the framewise model in front of a self-attention td or of no td; refuses the
-    hyper-parameters the kernels do not implement, naming the value (ok: AdaptCNN's pools are the shipped ones)."""
+    """(cnn_kind, cnn_fc, pools) of the framewise model in front of a self-attention td or of no td; refuses the
+    hyper-parameters the kernels do not implement, naming the value (pools: AdaptCNN's cnn_pool_1/2/3, else None)."""
     cnn = args.get("cnn_model")
     if cnn == "standard":
         _check_standard_cnn(args)
-        return CNN_STANDARD, 0, True
+        return CNN_STANDARD, 0, None
     cnn_kind = CNN_CONV if cnn == "adapt" else CNN_DFF if cnn == "dff" else CNN_SKIP
+    pools = None
     if cnn == "adapt":
         # (the engine reads the channel counts from the conv / bn tensors in nisqa_load_weights)
         for i in (1, 2, 3):
             c = args.get("cnn_c_out_%d" % i)
             if c not in CNN_CHANNELS or int(c) != c:
                 raise NotImplementedError("cnn_c_out_%d=%r: the engine runs AdaptCNN channel counts 16, 32 or 64" % (i, c))
+        _check_kernel_size(args)
+        pools = _check_adapt_pools(args)
     cnn_fc = int(args.get("cnn_fc_out_h") or 0)         # AdaptCNN's optional Linear behind conv6 (lib:682-684), SkipCNN's
     if cnn_kind == CNN_DFF and cnn_fc == 0:
         cnn_fc = 4096                                   # DFF's default hidden width (lib:544)
     if cnn_fc % 64 != 0:
         raise NotImplementedError("cnn_fc_out_h=%d: the engine needs a multiple of 64" % cnn_fc)
-    ok = cnn != "adapt" or (list(args["cnn_pool_1"]) == [24, 7] and list(args["cnn_pool_2"]) == [12, 5]
-                            and list(args["cnn_pool_3"]) == [6, 3])
-    return cnn_kind, cnn_fc, ok
+    return cnn_kind, cnn_fc, pools
 
 
 class NisqaTensor(C.Structure):
@@ -213,6 +245,8 @@ def load_library(path=None):
     lib.nisqa_set_profiling.restype = C.c_int
     lib.nisqa_set_option.argtypes = [vp, C.c_char_p, C.c_int]
     lib.nisqa_set_option.restype = C.c_int
+    lib.nisqa_set_cnn_pools.argtypes = [vp, i32p]
+    lib.nisqa_set_cnn_pools.restype = C.c_int
     lib.nisqa_group_ms.argtypes = [vp, C.c_char_p]
     lib.nisqa_group_ms.restype = C.c_double
     if path is None:
@@ -237,7 +271,7 @@ def config_from_args(args, max_chunk_segments=0):
             raise NotImplementedError("pool_att_h=%r is not implemented by the engine (128 or None)" % args.get("pool_att_h"))
     if pool_mode is None:
         raise NotImplementedError("Pool option not available in the engine: %r" % pool)
-    cnn_kind, cnn_fc = CNN_CONV, 0
+    cnn_kind, cnn_fc, pools = CNN_CONV, 0, None
     td2 = args.get("td_2") or "skip"
     if td2 not in ("skip", "self_att", "lstm"):
         raise NotImplementedError("td_2=%r is not implemented by the engine (skip, self_att or lstm)" % (args.get("td_2"),))
@@ -247,16 +281,15 @@ def config_from_args(args, max_chunk_segments=0):
     if cnn in ("adapt", None, "skip", "dff") and td == "self_att":
         # AdaptCNN, or a framewise model without convolutions (lib:504-583), in front of the self-attention stack
         arch = ARCH_ADAPT_SA_ATTFF
-        cnn_kind, cnn_fc, ok = _framewise(args)
+        cnn_kind, cnn_fc, pools = _framewise(args)
     elif (cnn, td) == ("standard", "self_att") and not de:
         # StandardCNN (lib:811-836) in front of the self-attention stack; fc_out's width comes from the weights
         arch = ARCH_ADAPT_SA_ATTFF
-        cnn_kind, cnn_fc, ok = _framewise(args)
+        cnn_kind, cnn_fc, pools = _framewise(args)
     elif (cnn, td) == ("standard", "lstm"):
         # any LSTM width, depth and direction behind StandardCNN (lib:811-836, 925-943), every pooling module
         arch = ARCH_STD_LSTM_LASTBI
         _check_standard_cnn(args)
-        ok = True
     elif cnn in ("adapt", None, "skip", "dff", "standard") and td in (None, "skip"):
         # no time-dependency model (TimeDependency._skip, lib:839-895): td_2, or the pooling module, reads the framewise rows
         if de:
@@ -265,7 +298,7 @@ def config_from_args(args, max_chunk_segments=0):
             raise NotImplementedError("td_2='lstm' behind td=%r and cnn_model=%r: the engine runs an LSTM td_2 behind no td "
                                       "for cnn_model='standard' only" % (td, cnn))
         arch = ARCH_SKIP
-        cnn_kind, cnn_fc, ok = _framewise(args)
+        cnn_kind, cnn_fc, pools = _framewise(args)
     else:
         raise NotImplementedError(
             "architecture cnn=%r td=%r pool=%r is not implemented by the engine" % (cnn, td, pool))
@@ -277,7 +310,7 @@ def config_from_args(args, max_chunk_segments=0):
     fan1 = _check_lstm(args, "td_lstm") if td_lstm else None
     if skip:
         fan1 = int(args.get("cnn_fc_out_h") or 768) if cnn == "standard" else (
-            cnn_fc or (6 * int(args["cnn_c_out_3"]) if cnn == "adapt"
+            cnn_fc or (pools[2][0] * int(args["cnn_c_out_3"]) if cnn == "adapt"
                        else int(args.get("ms_n_mels") or 0) * int(args.get("ms_seg_length") or 0)))
     fan2 = _check_lstm(args, "td_2_lstm") if td2 == "lstm" else None
     if pool_mode == POOL_LAST_STEP_BI:
@@ -288,8 +321,6 @@ def config_from_args(args, max_chunk_segments=0):
         if not args.get(key + "_bidirectional"):
             raise NotImplementedError("pool='last_step_bi' with %s_bidirectional=%r: PoolLastStepBi needs a bidirectional LSTM"
                                       % (key, args.get(key + "_bidirectional")))
-    ks = args.get("cnn_kernel_size")
-    ok = ok and (ks == 3 or tuple(ks) == (3, 3))
     if de:
         # double-ended model (reference lib:272-424, config/train_nisqa_double_ended.yaml): AdaptCNN + self-attention on
         # both signals, alignment without learned weights, fusion without the optional Linear, td_2 = self-attention
@@ -301,8 +332,6 @@ def config_from_args(args, max_chunk_segments=0):
             raise NotImplementedError("de_align_apply / de_fuse option not available: %r / %r" % (args.get("de_align_apply"), args.get("de_fuse")))
         if args.get("de_fuse_dim") and int(args["de_fuse_dim"]) % 64 != 0:
             raise NotImplementedError("de_fuse_dim=%r: the engine needs a multiple of 64" % (args.get("de_fuse_dim"),))
-    if not ok:
-        raise NotImplementedError("checkpoint hyper-parameters outside the shipped NISQA configurations")
     n_mels, seg_len = _check_mel_shape(args, td_lstm or cnn_kind == CNN_STANDARD)
     sa = td2w = (0, 0)
     if not td_lstm and not skip:
@@ -343,6 +372,9 @@ def config_from_args(args, max_chunk_segments=0):
         cfg.double_ended = 1
         cfg.de_fuse_dim = int(args.get("de_fuse_dim") or 0)
         cfg.de_align, cfg.de_align_apply, cfg.de_fuse = DE_ALIGN[args["de_align"]], DE_APPLY[args["de_align_apply"]], DE_FUSE[args["de_fuse"]]
+    if pools is not None and pools != SHIPPED_POOLS:
+        # (nisqa_config has no room for them: Engine applies them with nisqa_set_cnn_pools before the weights load)
+        cfg.cnn_pools = pools
     return cfg
 
 
@@ -403,6 +435,9 @@ class Engine(object):
                 self.h = C.c_void_p()
             raise EngineError("nisqa_create failed (%d): %s" % (rc, msg))
         self.device = int(device)
+        pools = getattr(cfg, "cnn_pools", None)
+        if pools is not None:
+            self.set_cnn_pools(pools)
 
     def _err(self):
         m = self.lib.nisqa_last_error(self.h)
@@ -631,6 +666,11 @@ class Engine(object):
 
     def set_option(self, name, value):
         self._check(self.lib.nisqa_set_option(self.h, name.encode(), int(value)), "nisqa_set_option")
+
+    def set_cnn_pools(self, pools):
+        """AdaptCNN's cnn_pool_1/2/3 ((h1, w1), (h2, w2), (h3, w3)) for the next load_state_dict"""
+        flat = (C.c_int32 * 6)(*[int(v) for p in pools for v in p])
+        self._check(self.lib.nisqa_set_cnn_pools(self.h, flat), "nisqa_set_cnn_pools")
 
     def group_ms(self, group):
         return float(self.lib.nisqa_group_ms(self.h, group.encode()))
