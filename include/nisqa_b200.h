@@ -223,6 +223,43 @@ NISQA_API int  nisqa_predict_pcm_device(nisqa_engine* e, int n_clips,
                               int sample_fmt, float* scores_dev,
                               int32_t* n_segments_out, int32_t* status_out, int sync);
 
+/* A batch of clips the caller holds in DEVICE memory as a strided [n_clips][n_channels][length] array: sample t of
+ * channel c of clip b is element b * clip_stride + c * channel_stride + t of `data` (samples contiguous). */
+typedef struct nisqa_device_batch {
+  const void* data;          /* device memory owned by the caller                                                    */
+  int32_t sample_fmt;        /* NISQA_FMT_S16 | NISQA_FMT_F32                                                        */
+  int32_t n_clips;
+  int32_t n_channels;        /* >= 1                                                                                 */
+  int32_t channel;           /* -1: mono mix, the rule of the file ingest (int16 scaled by 1/32768, float32 sum in
+                              * channel order, then divided by n_channels); else that channel (ignored when
+                              * n_channels == 1)                                                                     */
+  int64_t length;            /* samples per channel row                                                              */
+  int64_t clip_stride;       /* in elements                                                                          */
+  int64_t channel_stride;    /* in elements                                                                          */
+  const int64_t* n_samples;  /* HOST [n_clips]: samples of each clip, 1 .. length                                    */
+  int32_t sample_rate;       /* of every clip of the batch                                                           */
+} nisqa_device_batch;
+
+/* nisqa_predict_pcm for audio already on the GPU, ordered on the caller's CUDA stream (cuda_stream; NULL = the legacy
+ * default stream).  The engine's lanes wait for the work enqueued on cuda_stream before the call, and cuda_stream waits
+ * for the call's kernels before anything enqueued after it: the input may be freed or overwritten, and scores_dev read,
+ * in stream order as soon as the call returns.  The call never waits on the host for its own work (it only waits, like
+ * nisqa_submit_pcm, for a call six passes back to release the staging slot it reuses, and an ms_sr call for the ms_sr
+ * call two conversions back to release the conversion buffers it reuses).
+ *   deg            : the clips to score; its channel applies (a one-channel batch is read as is)
+ *   ref            : NISQA_DE only (else NULL): the reference clips, deg->n_clips of them, always mono-mixed (the file
+ *                    ingest reads a double-ended row's reference without ms_channel).  Clip p of deg and clip p of ref
+ *                    form pair p, which the engine runs as clips 2p and 2p + 1 (see nisqa_config.double_ended).
+ *   target_sr      : ms_sr of the checkpoint (every clip converted to that rate on the device first), 0 = none; needs
+ *                    the interpolation table (nisqa_resample_set_filter), even when every clip is at target_sr already
+ *   scores_dev     : device [rows][n_out] fp32, rows = deg->n_clips (NISQA_DE: 2 deg->n_clips, row 2p holds pair p's
+ *                    score, row 2p + 1 is NaN); NaN rows for clips whose status != OK
+ *   n_segments_out, status_out : host [rows] int32, valid on return (host arithmetic on n_samples, after ms_sr)
+ * Mono int16 input (one channel, or a picked channel) runs as NISQA_FMT_S16, anything mixed or float32 as F32. */
+NISQA_API int  nisqa_predict_device_batch(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                                          const nisqa_device_batch* ref, int32_t target_sr, float* scores_dev,
+                                          int32_t* n_segments_out, int32_t* status_out);
+
 /* Copy an intermediate of the LAST predict call to host memory (parity tests).  Only valid
  * when that call fitted in one internal pass.  Returns the number of floats written (>=0)
  * or a negative status; with out == NULL returns the required count. */

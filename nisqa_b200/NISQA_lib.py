@@ -93,17 +93,10 @@ class SpeechQualityDataset(object):
 
 
 def _raise_for_status(ds, engine, index, n_samples, sr, n_seg, status):
-    path = ds.file_path(index)
-    if status == nb_engine.CLIP_TOO_SHORT:
-        hop = int(sr * ds.ms_hop_length)
-        width = 1 + n_samples // hop if hop > 0 else 0
-        raise ValueError(
-            "Sample too short. Only {} windows available but seg_length={}. "
-            "Consider zero padding the audio sample. File: {}".format(width, ds.seg_length, path))
-    if status == nb_engine.CLIP_TOO_LONG:
-        raise ValueError(
-            "n_wins {} > max_length {} --- {}. Increase max window length ms_max_segments!".format(
-                n_seg, ds.max_length, path))
+    err = nb_engine.clip_status_error(status, ds.file_path(index), n_samples, sr, n_seg, ds.ms_hop_length, ds.seg_length,
+                                      ds.max_length)
+    if err is not None:
+        raise err
 
 
 class _PinnedPool(object):

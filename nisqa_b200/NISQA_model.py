@@ -23,7 +23,7 @@ import torch
 from . import NISQA_lib as NL
 from . import evaluate as EV
 from . import dist as nb_dist
-from .engine import Engine, config_from_args
+from .engine import engine_from_checkpoint, load_checkpoint
 
 
 class nisqaModel(object):
@@ -164,10 +164,8 @@ class nisqaModel(object):
             model_path = os.path.join(self.args["pretrained_model"])
         else:
             model_path = os.path.join(os.getcwd(), self.args["pretrained_model"])
-        checkpoint = torch.load(model_path, map_location="cpu", weights_only=False)
         # checkpoint hyper-parameters, overridden by the caller's dict (model:941-942)
-        checkpoint["args"].update(self.args)
-        self.args = checkpoint["args"]
+        self.args, state_dict = load_checkpoint(model_path, self.args)
 
         if self.args["model"] == "NISQA_DIM":
             self.args["dim"] = True
@@ -186,9 +184,7 @@ class nisqaModel(object):
         chatty = nb_dist.env_world()[0] == 0
         if chatty:
             print("Model architecture: " + self.args["model"])
-        cfg = config_from_args(self.args, max_chunk_segments=self.args.get("b200_max_chunk_segments", 0))
-        self.model = Engine(cfg, device=self.dev.index if self.dev.index is not None else 0)
-        self.model.load_state_dict(checkpoint["model_state_dict"])   # strict: the engine names what is missing
+        self.model = engine_from_checkpoint(self.args, state_dict, device=self.dev.index if self.dev.index is not None else 0)
         if chatty:
             print("Loaded pretrained model from " + self.args["pretrained_model"])
 

@@ -133,6 +133,25 @@ struct Stage {
   }
 };
 
+// Conversion buffers of the device resampler (ms_sr, resample_gpu.cu): the raw packed input, the converted PCM, the
+// clip and time-register tables.  A device-batch call leaves its slot in use until its last pass is done (done, busy);
+// the calls rotate over kRsSlots of them, so the host can enqueue the next ms_sr call while the previous one runs.
+constexpr int kRsSlots = 2;
+struct RsSlot {
+  DevBuf raw, out, clips, times;
+  HostBuf host;                  // pinned copy of the clip table
+  cudaEvent_t ready = nullptr;   // the converted PCM is in `out` (recorded on the converting stream)
+  cudaEvent_t done = nullptr;    // the call that used the slot last is done with it
+  bool busy = false;
+  void release() {
+    DevBuf* all[] = {&raw, &out, &clips, &times};
+    for (auto* b : all) b->release();
+    host.release();
+    if (ready) cudaEventDestroy(ready);
+    if (done) cudaEventDestroy(done);
+  }
+};
+
 struct TimerSlot {
   std::string name;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev;
@@ -211,9 +230,13 @@ struct nisqa_engine {
   // weights arena (device) and the pointers into it
   DevBuf warena;
   Weights w;
-  DevBuf rs_raw, rs_out, rs_clips, rs_times, rs_win;   // device resampler of the ingest (resample_gpu.cu)
-  HostBuf rs_host;
+  DevBuf rs_win;                 // device resampler of the ingest (resample_gpu.cu): its interpolation table ...
   int rs_nwin = 0, rs_num_table = 0;
+  RsSlot rs[kRsSlots];           // ... and its conversion buffers, used in turn
+  int64_t rs_next = 0;
+  // nisqa_predict_device_batch: ev_in is recorded on the caller's stream (the lanes wait for it), ev_out behind the
+  // call's last pass (the caller's stream waits for it)
+  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
   float pool_bias_std = 0.f;
   float tc_scale[8] = {1, 1, 1, 1, 1, 1, 1, 1};   // 2^(e_{i-1} - S_i): undoes the activation and weight pre-scales of conv i
   int act_exp[8] = {0, 0, 0, 0, 0, 0, 0, 0};      // e_i: conv i's activations are stored as fp16 planes of v * 2^-e_i
@@ -281,8 +304,8 @@ struct nisqa_engine {
 
   ~nisqa_engine() {
     for (auto* f : fbs) { f->window.release(); f->band_start.release(); f->band_k0.release(); f->weights.release(); f->wtab.release(); delete f; }
-    DevBuf* all[] = {&warena, &fb_table, &tw4096, &scores, &dump, &rs_raw, &rs_out, &rs_clips, &rs_times, &rs_win};
-    rs_host.release();
+    DevBuf* all[] = {&warena, &fb_table, &tw4096, &scores, &dump, &rs_win};
+    for (auto& r : rs) r.release();
     for (auto* b : all) b->release();
     h_scores.release();
     for (auto& tk : tickets) { tk.pinned.release(); tk.scores.release(); if (tk.done) cudaEventDestroy(tk.done); }
@@ -291,6 +314,7 @@ struct nisqa_engine {
     for (auto& g : stages) g.release();
     stream = nullptr;
     for (auto& t : timers) for (auto& e : t.ev) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
+    for (cudaEvent_t ev : {ev_in, ev_out}) if (ev) cudaEventDestroy(ev);
   }
 };
 
@@ -1038,9 +1062,11 @@ struct PassInput {
   int n_clips;
   const ClipPlan* plan;               // [n_clips]
   const int64_t* n_samples;           // [n_clips]
-  // exactly one of the two sources:
+  // exactly one of the three sources:
   const void* const* host_pcm;        // per-clip host pointers, or
-  const void* dev_pcm; const int64_t* dev_off;   // packed device buffer + element offsets
+  const void* dev_pcm; const int64_t* dev_off;   // packed device buffer + element offsets, or
+  const IngestSources* ingest; int first_clip;   // the caller's strided device batch (clips first_clip.. of the call)
+  cudaEvent_t ready;                  // when set, the lane waits for it before it reads the input or writes scores
   int fmt;
   float* scores_dev_out;              // device destination [n_clips][n_out]
   int slot;                           // compute lane
@@ -1092,7 +1118,7 @@ int upload_inputs(Pass& p, const PassInput& in) {
   std::vector<int> pre(5 * np, 0);             // pair | seg | qt | qt64 prefixes | by_len, [n + 1] each
   int* pair_prefix = &pre[0]; int* seg_prefix = &pre[np]; int* qt_prefix = &pre[2 * np]; int* qt64_prefix = &pre[3 * np];
   int* by_len = &pre[4 * np];
-  long long pcm_elems = 0;
+  long long pcm_elems = 0, max_run_samples = 0;
   int n_pairs = 0, n_qt = 0;
   for (int i = 0; i < n; ++i) {
     const ClipPlan& pl = in.plan[i];
@@ -1105,8 +1131,9 @@ int upload_inputs(Pass& p, const PassInput& in) {
     d.n_frames = ok ? pl.n_frames : 0;
     d.n_seg = ok ? pl.n_seg : 0;
     d.frame_off = p.n_frames; d.seg_off = p.n_seg; d.pair_off = n_pairs;
-    if (in.host_pcm) { d.pcm_off = pcm_elems; pcm_elems += ((long long)in.n_samples[i] + 15) / 16 * 16; }
+    if (in.host_pcm || in.ingest) { d.pcm_off = pcm_elems; pcm_elems += ((long long)in.n_samples[i] + 15) / 16 * 16; }
     else d.pcm_off = in.dev_off[i];
+    if (ok) max_run_samples = std::max<long long>(max_run_samples, in.n_samples[i]);
     pair_prefix[i] = n_pairs; seg_prefix[i] = p.n_seg; qt_prefix[i] = n_qt; qt64_prefix[i] = p.n_qt64;
     p.n_frames += d.n_frames; p.n_seg += d.n_seg;
     n_pairs += (d.n_frames + 1) / 2;
@@ -1171,6 +1198,14 @@ int upload_inputs(Pass& p, const PassInput& in) {
   }
   CK(cudaEventRecord(SG.ev_copied, cs));
   CK(cudaStreamWaitEvent(p.st, SG.ev_copied, 0));
+  if (in.ready) CK(cudaStreamWaitEvent(p.st, in.ready, 0));
+  if (p.n_seg > 0 && in.ingest) {
+    // the caller's batch -> packed mono PCM in the staging slot, on the lane (behind `ready`: the caller's stream order)
+    CK(SG.pcm.reserve((size_t)pcm_elems * (in.fmt == NISQA_FMT_F32 ? 4 : 2)));
+    Scope sc(e, "ingest");
+    launch_ingest(p.st, *in.ingest, in.first_clip, p.clips, n, max_run_samples, in.fmt == NISQA_FMT_F32, SG.pcm.p);
+    p.pcm = SG.pcm.p;
+  }
   return 0;
 }
 
@@ -1567,7 +1602,8 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
 int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, const void* dev_pcm,
                    const int64_t* dev_off, const int64_t* n_samples, const int32_t* sample_rate,
                    int fmt, float* scores_host, float* scores_dev, int32_t* n_seg_out,
-                   int32_t* status_out, int sync, int64_t* ticket_out = nullptr) {
+                   int32_t* status_out, int sync, int64_t* ticket_out = nullptr,
+                   const IngestSources* ingest = nullptr, cudaEvent_t ready = nullptr, cudaStream_t* fin_out = nullptr) {
   if (!e) return NISQA_ERR_INVALID;
   if (!e->weights_loaded) return fail(e, NISQA_ERR_STATE, "nisqa_load_weights has not been called");
   if (!e->conv_tc && e->conv_net() && !e->w.shipped_channels())
@@ -1630,6 +1666,8 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
     in.n_clips = i1 - i0; in.plan = plan.data() + i0; in.n_samples = n_samples + i0;
     in.host_pcm = host_pcm ? host_pcm + i0 : nullptr;
     in.dev_pcm = dev_pcm; in.dev_off = dev_off ? dev_off + i0 : nullptr;
+    in.ingest = ingest; in.first_clip = i0;
+    in.ready = ready;
     in.fmt = fmt;
     in.scores_dev_out = scores_all + (size_t)i0 * e->cfg.n_out;
     in.slot = e->profiling ? 0 : (int)(e->pass_counter % kLanes);
@@ -1652,6 +1690,7 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
     if (rc) return rc;
     CK(cudaEventRecord(e->stages[e->last_stage].ev_done, fin));
   }
+  if (fin_out) *fin_out = fin;
   if (ticket_out) {
     // asynchronous completion: scores land in the ticket's pinned block; nisqa_wait hands them over
     Ticket& tk = e->tickets[e->next_ticket % kStages];
@@ -1772,6 +1811,11 @@ int nisqa_create(nisqa_engine** out, int device, const nisqa_config* cfg) {
     CK(cudaEventCreateWithFlags(&g.ev_copied, cudaEventDisableTiming));
     CK(cudaEventCreateWithFlags(&g.ev_done, cudaEventDisableTiming));
   }
+  for (cudaEvent_t* ev : {&e->ev_in, &e->ev_out}) CK(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
+  for (auto& r : e->rs) {
+    CK(cudaEventCreateWithFlags(&r.ready, cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(&r.done, cudaEventDisableTiming));
+  }
   e->stream = e->lanes[0].stream;
   e->cur_stream = e->stream;
   // twiddles laid out per lane so that every warp load is coalesced:
@@ -1862,6 +1906,7 @@ int nisqa_drain(nisqa_engine* e) {
   cudaError_t err = cudaDeviceSynchronize();
   for (auto& tk : e->tickets) { tk.active = false; tk.user_scores = nullptr; }
   for (auto& g : e->stages) g.busy = false;
+  for (auto& r : e->rs) r.busy = false;
   if (err != cudaSuccess) return fail(e, NISQA_ERR_CUDA, std::string("cudaDeviceSynchronize: ") + cudaGetErrorString(err));
   return 0;
 }
@@ -1876,15 +1921,17 @@ int nisqa_predict_pcm_device(nisqa_engine* e, int n_clips, const void* pcm_dev, 
 }
 
 
-// ---- device resampler of the ingest (SURVEY.md 8f.2): host clips at their own rates -> packed float32 PCM at
-// `target` Hz in e->rs_out (clip i at element offset offs[i], n_fix[i] samples), on lane 0's stream (synchronised).
-static int resample_to_device(nisqa_engine* e, int n_clips, const void* const* pcm, const int64_t* n_samples,
-                              const int32_t* sample_rate, int fmt, int32_t target, std::vector<int64_t>* offs,
-                              std::vector<int64_t>* n_fix) {
+// ---- device resampler of the ingest (SURVEY.md 8f.2): clips at their own rates -> packed float32 PCM at `target` Hz
+// in the `out` buffer of the next conversion slot, *slot_out (clip i at element offset offs[i], n_fix[i] samples), on
+// stream st.  The clips come from host memory (pcm: copied in, st synchronised before the return) or from the caller's
+// device batch (ingest: packed by the ingest kernel, nothing synchronised: the call that enqueued it records the slot's
+// `done` behind its last use of the slot and marks it busy).  A busy slot is waited for before it is reused.
+static int resample_to_device(nisqa_engine* e, cudaStream_t st, int n_clips, const void* const* pcm,
+                              const IngestSources* ingest, const int64_t* n_samples, const int32_t* sample_rate, int fmt,
+                              int32_t target, std::vector<int64_t>* offs, std::vector<int64_t>* n_fix, RsSlot** slot_out) {
   if (fmt != NISQA_FMT_S16 && fmt != NISQA_FMT_F32) return fail(e, NISQA_ERR_INVALID, "sample_fmt");
   if (target <= 0) return fail(e, NISQA_ERR_INVALID, "target sample rate");
   CK(cudaSetDevice(e->device));
-  cudaStream_t st = e->lanes[0].stream;
   if (!e->rs_nwin) {
     std::vector<double> win;
     int num_table = 0;
@@ -1915,22 +1962,32 @@ static int resample_to_device(nisqa_engine* e, int n_clips, const void* const* p
     (*offs)[i] = c.out_off; (*n_fix)[i] = c.n_fix;
     max_fix = std::max(max_fix, c.n_fix);
   }
+  RsSlot& S = e->rs[e->rs_next++ % kRsSlots];
+  *slot_out = &S;
   if (n_clips == 0) return 0;
-  CK(e->rs_raw.reserve((size_t)std::max<long long>(in_elems, 16) * esz));
-  CK(e->rs_out.reserve((size_t)std::max<long long>(out_elems, 16) * 4));
-  CK(e->rs_times.reserve((size_t)t_entries * 8));
-  CK(e->rs_clips.reserve(rc.size() * sizeof(ResampleClip)));
-  CK(e->rs_host.reserve(rc.size() * sizeof(ResampleClip)));
-  memcpy(e->rs_host.p, rc.data(), rc.size() * sizeof(ResampleClip));
-  CK(cudaMemcpyAsync(e->rs_clips.p, e->rs_host.p, rc.size() * sizeof(ResampleClip), cudaMemcpyHostToDevice, st));
-  for (int i = 0; i < n_clips; ++i)
-    if (rc[i].n_in > 0)
-      CK(cudaMemcpyAsync(e->rs_raw.as<char>() + (size_t)rc[i].in_off * esz, pcm[i], (size_t)rc[i].n_in * esz, cudaMemcpyHostToDevice, st));
+  if (S.busy) { CK(cudaEventSynchronize(S.done)); S.busy = false; }     // the device-batch call kRsSlots conversions back
+  CK(S.raw.reserve((size_t)std::max<long long>(in_elems, 16) * esz));
+  CK(S.out.reserve((size_t)std::max<long long>(out_elems, 16) * 4));
+  CK(S.times.reserve((size_t)t_entries * 8));
+  CK(S.clips.reserve(rc.size() * sizeof(ResampleClip)));
+  CK(S.host.reserve(rc.size() * sizeof(ResampleClip)));
+  memcpy(S.host.p, rc.data(), rc.size() * sizeof(ResampleClip));
+  CK(cudaMemcpyAsync(S.clips.p, S.host.p, rc.size() * sizeof(ResampleClip), cudaMemcpyHostToDevice, st));
+  if (ingest) {
+    long long max_in = 0;
+    for (const ResampleClip& c : rc) max_in = std::max<long long>(max_in, c.n_in);
+    e->launches += 1;
+    launch_ingest(st, *ingest, 0, S.clips.as<ResampleClip>(), n_clips, max_in, fmt == NISQA_FMT_F32, S.raw.p);
+  } else {
+    for (int i = 0; i < n_clips; ++i)
+      if (rc[i].n_in > 0)
+        CK(cudaMemcpyAsync(S.raw.as<char>() + (size_t)rc[i].in_off * esz, pcm[i], (size_t)rc[i].n_in * esz, cudaMemcpyHostToDevice, st));
+  }
   e->launches += 2;
-  launch_resample(st, e->rs_raw.p, fmt == NISQA_FMT_F32, e->rs_clips.as<ResampleClip>(), n_clips, max_fix, e->rs_times.as<double>(),
-                  e->rs_win.as<double>(), e->rs_nwin, e->rs_num_table, e->rs_out.as<float>());
+  launch_resample(st, S.raw.p, fmt == NISQA_FMT_F32, S.clips.as<ResampleClip>(), n_clips, max_fix, S.times.as<double>(),
+                  e->rs_win.as<double>(), e->rs_nwin, e->rs_num_table, S.out.as<float>());
   CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(st));
+  if (!ingest) CK(cudaStreamSynchronize(st));
   return 0;
 }
 
@@ -1939,10 +1996,11 @@ int nisqa_resample_device(nisqa_engine* e, const void* x, int64_t n, int sample_
   if (!e || !x || !y) return NISQA_ERR_INVALID;
   std::vector<int64_t> offs, n_fix;
   const void* ptrs[1] = {x};
-  int rc = resample_to_device(e, 1, ptrs, &n, &sr_orig, sample_fmt, sr_new, &offs, &n_fix);
+  RsSlot* S = nullptr;
+  int rc = resample_to_device(e, e->lanes[0].stream, 1, ptrs, nullptr, &n, &sr_orig, sample_fmt, sr_new, &offs, &n_fix, &S);
   if (rc) return rc;
   if (n_fix[0] > cap) return fail(e, NISQA_ERR_INVALID, "resample: output buffer too small");
-  CK(cudaMemcpy(y, e->rs_out.as<float>() + offs[0], (size_t)n_fix[0] * 4, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(y, S->out.as<float>() + offs[0], (size_t)n_fix[0] * 4, cudaMemcpyDeviceToHost));
   return (int)n_fix[0];
 }
 
@@ -1952,12 +2010,103 @@ int nisqa_predict_pcm_resampled(nisqa_engine* e, int n_clips, const void* const*
   if (!e) return NISQA_ERR_INVALID;
   if (n_clips > 0 && (!pcm || !n_samples || !sample_rate || !scores_out)) return fail(e, NISQA_ERR_INVALID, "null argument");
   std::vector<int64_t> offs, n_fix;
-  int rc = resample_to_device(e, n_clips, pcm, n_samples, sample_rate, sample_fmt, target_sr, &offs, &n_fix);
+  RsSlot* S = nullptr;
+  int rc = resample_to_device(e, e->lanes[0].stream, n_clips, pcm, nullptr, n_samples, sample_rate, sample_fmt, target_sr, &offs,
+                              &n_fix, &S);
   if (rc) return rc;
   std::vector<int32_t> srs(n_clips, target_sr);
   // the converted clips are ordinary float32 PCM resident in HBM: the device entry of the predict path takes over
-  return predict_common(e, n_clips, nullptr, e->rs_out.p, offs.data(), n_fix.data(), srs.data(), NISQA_FMT_F32,
+  return predict_common(e, n_clips, nullptr, S->out.p, offs.data(), n_fix.data(), srs.data(), NISQA_FMT_F32,
                         scores_out, nullptr, n_segments_out, status_out, 1);
+}
+
+// The device work of nisqa_predict_device_batch once its arguments are checked: the lanes wait for the caller's stream,
+// the clips are packed (and converted to target_sr), the passes run, and the caller's stream waits for the last pass.
+// *slot_out: the conversion slot the call uses (ms_sr), also when it fails.
+static int enqueue_device_batch(nisqa_engine* e, cudaStream_t caller, int n_clips, const IngestSources& ing,
+                                const int64_t* ns, const int32_t* sr, int fmt, int32_t target_sr, float* scores_dev,
+                                int32_t* n_segments_out, int32_t* status_out, RsSlot** slot_out) {
+  CK(cudaEventRecord(e->ev_in, caller));
+  cudaStream_t fin = nullptr;
+  if (target_sr > 0) {
+    // convert on the lane of the call's first pass; every pass waits for the slot's `ready`
+    cudaStream_t st = e->lanes[e->profiling ? 0 : (int)(e->pass_counter % kLanes)].stream;
+    CK(cudaStreamWaitEvent(st, e->ev_in, 0));
+    std::vector<int64_t> offs, n_fix;
+    int rc = resample_to_device(e, st, n_clips, nullptr, &ing, ns, sr, fmt, target_sr, &offs, &n_fix, slot_out);
+    if (rc) return rc;
+    RsSlot& S = **slot_out;
+    CK(cudaEventRecord(S.ready, st));
+    std::vector<int32_t> srs(n_clips, target_sr);
+    rc = predict_common(e, n_clips, nullptr, S.out.p, offs.data(), n_fix.data(), srs.data(), NISQA_FMT_F32, nullptr,
+                        scores_dev, n_segments_out, status_out, 0, nullptr, nullptr, S.ready, &fin);
+    if (rc) return rc;
+    CK(cudaEventRecord(S.done, fin));
+    S.busy = n_clips > 0;
+  } else {
+    int rc = predict_common(e, n_clips, nullptr, nullptr, nullptr, ns, sr, fmt, nullptr, scores_dev, n_segments_out,
+                            status_out, 0, nullptr, &ing, e->ev_in, &fin);
+    if (rc) return rc;
+  }
+  // the last pass's lane has joined the call's other lanes: the caller's stream continues behind all of them
+  CK(cudaEventRecord(e->ev_out, fin));
+  CK(cudaStreamWaitEvent(caller, e->ev_out, 0));
+  return 0;
+}
+
+int nisqa_predict_device_batch(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                               const nisqa_device_batch* ref, int32_t target_sr, float* scores_dev,
+                               int32_t* n_segments_out, int32_t* status_out) {
+  if (!e) return NISQA_ERR_INVALID;
+  if (!e->stream) return fail(e, NISQA_ERR_STATE, "engine was not created successfully");
+  if (!deg) return fail(e, NISQA_ERR_INVALID, "deg: null argument");
+  if (e->cfg.double_ended && !ref) return fail(e, NISQA_ERR_INVALID, "ref: a double-ended engine needs the reference batch");
+  if (!e->cfg.double_ended && ref) return fail(e, NISQA_ERR_INVALID, "ref: only a double-ended engine takes a reference batch");
+  if (target_sr < 0) return fail(e, NISQA_ERR_INVALID, "target_sr");
+  const nisqa_device_batch* src[2] = {deg, ref};
+  const int n_src = ref ? 2 : 1;
+  IngestSources ing = {};
+  ing.n_src = n_src;
+  bool out_f32 = false;
+  for (int k = 0; k < n_src; ++k) {
+    const nisqa_device_batch& b = *src[k];
+    const std::string nm = k ? "ref." : "deg.";
+    const int ch = k ? -1 : b.channel;        // the reference of a pair is always the mono mix
+    if (b.sample_fmt != NISQA_FMT_S16 && b.sample_fmt != NISQA_FMT_F32) return fail(e, NISQA_ERR_INVALID, nm + "sample_fmt");
+    if (b.n_clips < 0 || b.n_clips != deg->n_clips) return fail(e, NISQA_ERR_INVALID, nm + "n_clips");
+    if (b.n_channels < 1) return fail(e, NISQA_ERR_INVALID, nm + "n_channels");
+    if (b.n_channels > 1 && (ch < -1 || ch >= b.n_channels)) return fail(e, NISQA_ERR_INVALID, nm + "channel out of range");
+    if (b.length < 1 || b.clip_stride < 0 || b.channel_stride < 0) return fail(e, NISQA_ERR_INVALID, nm + "length / strides");
+    if (b.sample_rate <= 0) return fail(e, NISQA_ERR_INVALID, nm + "sample_rate");
+    if (b.n_clips > 0 && (!b.data || !b.n_samples)) return fail(e, NISQA_ERR_INVALID, nm + "data / n_samples: null argument");
+    for (int i = 0; i < b.n_clips; ++i)
+      if (b.n_samples[i] < 1 || b.n_samples[i] > b.length)
+        return fail(e, NISQA_ERR_INVALID, nm + "n_samples[" + std::to_string(i) + "] = " + std::to_string(b.n_samples[i]) +
+                                              ": not within 1 .. length (" + std::to_string(b.length) + ")");
+    const bool mix = b.n_channels > 1 && ch < 0;
+    ing.s[k] = {b.data, b.clip_stride, b.channel_stride, b.n_channels, ch, b.sample_fmt == NISQA_FMT_F32 ? 1 : 0};
+    out_f32 = out_f32 || b.sample_fmt == NISQA_FMT_F32 || mix;
+  }
+  const int n_clips = deg->n_clips * n_src;
+  if (n_clips > 0 && !scores_dev) return fail(e, NISQA_ERR_INVALID, "scores_dev: null argument");
+  // the engine's clip order: clip g is clip g / n_src of source g % n_src (NISQA_DE: degraded, reference pairs)
+  std::vector<int64_t> ns(n_clips);
+  std::vector<int32_t> sr(n_clips);
+  for (int g = 0; g < n_clips; ++g) { ns[g] = src[g % n_src]->n_samples[g / n_src]; sr[g] = src[g % n_src]->sample_rate; }
+  const int fmt = out_f32 ? NISQA_FMT_F32 : NISQA_FMT_S16;
+  CK(cudaSetDevice(e->device));
+  cudaStream_t caller = static_cast<cudaStream_t>(cuda_stream);
+  RsSlot* S = nullptr;
+  const int rc = enqueue_device_batch(e, caller, n_clips, ing, ns.data(), sr.data(), fmt, target_sr, scores_dev,
+                                      n_segments_out, status_out, &S);
+  if (rc) {
+    // whatever was enqueued before the failure may still read the caller's input or the conversion slot: the caller's
+    // stream waits for every lane, and the slot stays in use until then (best effort: the error is already reported)
+    for (auto& l : e->lanes)
+      if (cudaEventRecord(e->ev_out, l.stream) == cudaSuccess) cudaStreamWaitEvent(caller, e->ev_out, 0);
+    if (S && cudaEventRecord(S->done, caller) == cudaSuccess) S->busy = true;
+  }
+  return rc;
 }
 
 int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {

@@ -186,6 +186,26 @@ void launch_linear_tile(cudaStream_t st, const float* X, int ldx, const float* W
 void launch_resample(cudaStream_t st, const void* raw, int fmt_f32, const ResampleClip* clips, int n_clips, int max_fix,
                      double* t_start, const double* win, int nwin, int num_table, float* out);
 
+// ---------------------------------------------------------------- ingest.cu (nisqa_predict_device_batch)
+// One caller-owned strided [clips][channels][length] device array (nisqa_device_batch)
+struct IngestSrc {
+  const void* data;
+  long long clip_stride, channel_stride;   // elements
+  int n_channels;
+  int channel;                             // -1: mono mix; else that channel (ignored for one channel)
+  int f32;                                 // 1: float32 samples, 0: int16
+};
+// The clips of a call in the engine's order: clip g (of the whole call) is clip g / n_src of source g % n_src (NISQA_DE:
+// source 0 the degraded batch, source 1 the reference batch)
+struct IngestSources { IngestSrc s[2]; int n_src; };
+// Packed mono PCM of clips first_clip .. first_clip + n_clips - 1 of the call, written where the table says: the pass's
+// ClipDesc rows (pcm_off, n_samples; skipped clips are not read) or the resampler's ResampleClip rows (in_off, n_in).
+// out_f32 0: int16 out (every source int16 and mono or picked); 1: float32 out (int16 scaled by 1/32768).
+void launch_ingest(cudaStream_t st, const IngestSources& src, int first_clip, const ClipDesc* clips, int n_clips,
+                   long long max_n, int out_f32, void* out);
+void launch_ingest(cudaStream_t st, const IngestSources& src, int first_clip, const ResampleClip* clips, int n_clips,
+                   long long max_n, int out_f32, void* out);
+
 // ---------------------------------------------------------------- resample.cpp
 // the interpolation table of the resampler (set by nisqa_resample_set_filter); false before that call
 bool resample_table(std::vector<double>* win, int* num_table);

@@ -38,7 +38,7 @@ EXPORTS = [
     "nisqa_submit_pcm", "nisqa_wait", "nisqa_drain", "nisqa_join", "nisqa_set_gather_target",
     "nisqa_wav_probe", "nisqa_wav_decode", "nisqa_wav_probe_batch", "nisqa_wav_decode_batch",
     "nisqa_resample_set_filter", "nisqa_resample_out_len", "nisqa_resample_f32",
-    "nisqa_resample_device", "nisqa_predict_pcm_resampled", "nisqa_set_cnn_pools",
+    "nisqa_resample_device", "nisqa_predict_pcm_resampled", "nisqa_set_cnn_pools", "nisqa_predict_device_batch",
 ]
 
 
@@ -160,6 +160,13 @@ def _framewise(args):
     return cnn_kind, cnn_fc, pools
 
 
+class NisqaDeviceBatch(C.Structure):
+    """nisqa_device_batch: clips in device memory as a strided [n_clips][n_channels][length] array"""
+    _fields_ = [("data", C.c_void_p), ("sample_fmt", C.c_int32), ("n_clips", C.c_int32), ("n_channels", C.c_int32),
+                ("channel", C.c_int32), ("length", C.c_int64), ("clip_stride", C.c_int64), ("channel_stride", C.c_int64),
+                ("n_samples", C.POINTER(C.c_int64)), ("sample_rate", C.c_int32)]
+
+
 class NisqaTensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", C.POINTER(C.c_float)), ("ndim", C.c_int32),
                 ("dims", C.c_int64 * 4)]
@@ -225,6 +232,9 @@ def load_library(path=None):
     lib.nisqa_drain.restype = C.c_int
     lib.nisqa_predict_pcm_device.argtypes = [vp, C.c_int, vp, i64p, i64p, i32p, C.c_int, vp, i32p, i32p, C.c_int]
     lib.nisqa_predict_pcm_device.restype = C.c_int
+    dbp = C.POINTER(NisqaDeviceBatch)
+    lib.nisqa_predict_device_batch.argtypes = [vp, vp, dbp, dbp, C.c_int32, vp, i32p, i32p]
+    lib.nisqa_predict_device_batch.restype = C.c_int
     lib.nisqa_stage_dump.argtypes = [vp, C.c_int, f32p, C.c_int64]
     lib.nisqa_stage_dump.restype = C.c_int64
     lib.nisqa_segment_counts.argtypes = [C.POINTER(NisqaConfig), C.c_int64, C.c_int32, i32p, i32p, i32p]
@@ -407,6 +417,48 @@ def _fan_out_args(args, stage):
         return "%s=%r: the framewise fan_out of cnn_model=%r, cnn_fc_out_h=%r" % (
             stage, args.get(stage), args.get("cnn_model"), args.get("cnn_fc_out_h"))
     return "%s_sa_d_model=%r" % (stage, args.get(stage + "_sa_d_model"))
+
+
+def device_batch(data_ptr, sample_fmt, n_samples, n_channels, channel, length, clip_stride, channel_stride, sample_rate):
+    """-> (NisqaDeviceBatch, its host n_samples array): one argument of Engine.predict_device_batch (element strides)"""
+    ns = np.ascontiguousarray(n_samples, dtype=np.int64)
+    b = NisqaDeviceBatch(data=data_ptr, sample_fmt=sample_fmt, n_clips=len(ns), n_channels=n_channels, channel=channel,
+                         length=length, clip_stride=clip_stride, channel_stride=channel_stride,
+                         n_samples=ns.ctypes.data_as(C.POINTER(C.c_int64)), sample_rate=sample_rate)
+    return b, ns
+
+
+def load_checkpoint(model_path, overrides=None):
+    """-> (args, state_dict) of a checkpoint file, its ``args`` updated with ``overrides`` (the caller's dict takes
+    precedence, reference model:941-942)."""
+    import torch
+    checkpoint = torch.load(model_path, map_location="cpu", weights_only=False)
+    checkpoint["args"].update(overrides or {})
+    return checkpoint["args"], checkpoint["model_state_dict"]
+
+
+def engine_from_checkpoint(args, state_dict, device=0):
+    """An Engine on ``device`` running the checkpoint: nisqa_config from its args, then its weights (strict: the engine
+    names what is missing)."""
+    cfg = config_from_args(args, max_chunk_segments=args.get("b200_max_chunk_segments", 0))
+    eng = Engine(cfg, device=device)
+    eng.load_state_dict(state_dict)
+    return eng
+
+
+def clip_status_error(status, where, n_samples, sample_rate, n_seg, hop_length, seg_length, max_length):
+    """The reference's ValueError for a clip whose status is not CLIP_OK (lib:2259-2263 "Sample too short",
+    lib:2276-2277 "n_wins > max_length"), else None.  ``where`` names the clip: a file path, or an argument and index."""
+    if status == CLIP_TOO_SHORT:
+        hop = int(sample_rate * hop_length)
+        width = 1 + n_samples // hop if hop > 0 else 0
+        return ValueError(
+            "Sample too short. Only {} windows available but seg_length={}. "
+            "Consider zero padding the audio sample. File: {}".format(width, seg_length, where))
+    if status == CLIP_TOO_LONG:
+        return ValueError(
+            "n_wins {} > max_length {} --- {}. Increase max window length ms_max_segments!".format(n_seg, max_length, where))
+    return None
 
 
 def segment_counts(cfg, n_samples, sample_rate):
@@ -631,6 +683,25 @@ class Engine(object):
             fmt, C.c_void_p(scores_dev_ptr), nseg.ctypes.data_as(C.POINTER(C.c_int32)),
             status.ctypes.data_as(C.POINTER(C.c_int32)), 1 if sync else 0)
         self._check(rc, "nisqa_predict_pcm_device")
+        return nseg, status
+
+    def predict_device_batch(self, stream, deg, scores_dev_ptr, ref=None, target_sr=0):
+        """Clips already in device memory, ordered on the CUDA stream ``stream`` (a cudaStream_t as an int; 0: the
+        legacy default stream): ``deg`` / ``ref`` are :func:`device_batch` tuples (``ref``: NISQA_DE only), ``target_sr``
+        the checkpoint's ``ms_sr`` (0: none; every clip is converted to it on the device), the scores
+        go to ``scores_dev_ptr`` ([rows, n_out] fp32 device memory; rows = n_clips, NISQA_DE 2 n_clips).  Returns
+        (n_segments int32[rows], status int32[rows]), valid on return; the scores are valid in ``stream``'s order."""
+        rows = deg[0].n_clips * (2 if ref is not None else 1)
+        if target_sr:
+            from . import resample as _rs
+            _rs.out_len(1, 1, 1)                                      # the interpolation table is set once
+        nseg = np.empty(rows, dtype=np.int32)
+        status = np.empty(rows, dtype=np.int32)
+        rc = self.lib.nisqa_predict_device_batch(
+            self.h, C.c_void_p(stream or None), C.byref(deg[0]), C.byref(ref[0]) if ref is not None else None,
+            int(target_sr or 0), C.c_void_p(scores_dev_ptr), nseg.ctypes.data_as(C.POINTER(C.c_int32)),
+            status.ctypes.data_as(C.POINTER(C.c_int32)))
+        self._check(rc, "nisqa_predict_device_batch")
         return nseg, status
 
     # ------------------------------------------------------------------ introspection

@@ -1,0 +1,137 @@
+"""``Scorer``: NISQA scores of waveforms that are already on the GPU, in the caller's CUDA stream order.
+
+    scorer = Scorer("weights/nisqa.tar")
+    scores = scorer(wave, 48000)            # wave: [T], [B, T] or [B, C, T] int16 / float32 CUDA tensor
+    dict(zip(scorer.columns, scores[0].tolist()))
+
+The audio never leaves the device: the engine packs it with its own ingest kernel (``nisqa_predict_device_batch``)
+and the scores come back as a CUDA tensor, written in the order of ``torch.cuda.current_stream()``.  Nothing waits for
+the GPU: ``wave`` may be freed or reused in stream order as soon as the call returns.
+"""
+import numbers
+
+import numpy as np
+import torch
+
+from . import engine as E
+
+DIM_COLUMNS = ["mos_pred", "noi_pred", "dis_pred", "col_pred", "loud_pred"]     # NISQA_DIM's outputs (lib:1461-1465)
+
+
+class Scorer(object):
+    """A checkpoint loaded onto one GPU.  ``overrides`` update the checkpoint's args like the caller's dict of
+    ``nisqaModel`` (e.g. ``ms_sr``, ``b200_max_chunk_segments``)."""
+
+    def __init__(self, pretrained_model, device=None, **overrides):
+        if not torch.cuda.is_available():
+            raise RuntimeError("no CUDA device available: the engine has no CPU fallback")
+        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if dev.type != "cuda":
+            raise ValueError("device: the engine runs on a CUDA device, not %r" % (device,))
+        args, state_dict = E.load_checkpoint(pretrained_model, overrides)
+        self._configure(args, torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device()))
+        self.engine = E.engine_from_checkpoint(args, state_dict, device=self.device.index)
+
+    def _configure(self, args, device):
+        """The host side of a scorer: what its arguments are checked against"""
+        self.args, self.device = args, device
+        self.cfg = E.config_from_args(args, max_chunk_segments=args.get("b200_max_chunk_segments", 0))
+        self.double_ended = args["model"] == "NISQA_DE"
+        self.columns = list(DIM_COLUMNS) if args["model"] == "NISQA_DIM" else ["mos_pred"]
+        self.target_sr = int(args["ms_sr"]) if args.get("ms_sr") else 0
+
+    def close(self):
+        self.engine.close()
+
+    def __call__(self, wave, sample_rate, lengths=None, channel=None, reference=None, reference_lengths=None,
+                 reference_sample_rate=None):
+        """Scores of a batch -> float32 [B, len(columns)] on ``wave.device``.
+
+        wave        : [T], [B, T] or [B, C, T] int16 / float32 CUDA tensor on the scorer's device, any batch and channel
+                      strides, samples contiguous
+        sample_rate : of every clip
+        lengths     : host ints, samples of each clip (default T)
+        channel     : None = the mono mix (mean over channels, as the file ingest), else that channel
+        reference   : NISQA_DE only: the reference clips, one per clip of ``wave``, always mixed to mono; with their own
+                      ``reference_lengths`` and ``reference_sample_rate`` (default: ``sample_rate``)
+        A clip too short or too long for the checkpoint raises the file ingest's ValueError before anything is enqueued.
+        """
+        if self.double_ended and reference is None:
+            raise ValueError("reference: a double-ended (NISQA_DE) checkpoint scores (wave, reference) pairs")
+        if not self.double_ended and reference is not None:
+            raise ValueError("reference: only a double-ended (NISQA_DE) checkpoint takes reference clips")
+        deg = self._batch("wave", wave, sample_rate, lengths, channel)
+        ref = None
+        if reference is not None:
+            ref = self._batch("reference", reference, sample_rate if reference_sample_rate is None else reference_sample_rate,
+                              reference_lengths, None)
+            if ref[0].n_clips != deg[0].n_clips:
+                raise ValueError("reference: %d clips for %d clips of wave" % (ref[0].n_clips, deg[0].n_clips))
+        for name, b in (("wave", deg), ("reference", ref)):
+            if b is not None:
+                self._check_segments(name, b[1], b[0].sample_rate)
+        n = deg[0].n_clips * (2 if ref is not None else 1)
+        out = torch.empty((n, len(self.columns)), dtype=torch.float32, device=self.device)
+        if n:
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            self.engine.predict_device_batch(stream, deg, out.data_ptr(), ref=ref, target_sr=self.target_sr)
+        # (NISQA_DE: row 2p holds pair p's score, row 2p + 1 is the reference clip's NaN row)
+        return out[0::2].contiguous() if ref is not None else out
+
+    # ------------------------------------------------------------------ arguments
+    def _batch(self, name, x, sample_rate, lengths, channel):
+        """-> engine.device_batch(...) of one batch argument, after the argument checks"""
+        if not isinstance(x, torch.Tensor):
+            raise TypeError("%s: a torch.Tensor on the GPU, not %s" % (name, type(x).__name__))
+        if x.dtype not in (torch.int16, torch.float32):
+            raise TypeError("%s: dtype %s; the engine reads int16 or float32 samples (convert with .float())" % (name, x.dtype))
+        if x.device != self.device:
+            raise ValueError("%s: on %s, the scorer runs on %s" % (name, x.device, self.device))
+        if x.dim() not in (1, 2, 3):
+            raise ValueError("%s: shape %s; expected [T], [B, T] or [B, C, T]" % (name, tuple(x.shape)))
+        if isinstance(sample_rate, bool) or not isinstance(sample_rate, numbers.Integral) or sample_rate <= 0:
+            raise ValueError("%s: sample_rate must be a positive int, not %r" % (name, sample_rate))
+        x3 = x.reshape(1, 1, -1) if x.dim() == 1 else x.unsqueeze(1) if x.dim() == 2 else x
+        B, C, T = x3.shape
+        if T < 1:
+            raise ValueError("%s: no samples" % name)
+        if T > 1 and x3.stride(2) != 1:
+            raise ValueError("%s: samples must be contiguous (stride 1 along the last dimension, got %d)" % (name, x3.stride(2)))
+        if channel is None:
+            ch = -1
+        elif isinstance(channel, bool) or not isinstance(channel, numbers.Integral):
+            raise TypeError("channel: an int or None, not %r" % (channel,))
+        elif not 0 <= channel < C:
+            raise ValueError("channel: %d is out of range for %d channel(s)" % (channel, C))
+        else:
+            ch = int(channel)
+        what = "reference_lengths" if name == "reference" else "lengths"
+        if lengths is None:
+            ns = np.full(B, T, dtype=np.int64)
+        else:
+            if isinstance(lengths, torch.Tensor) and lengths.device.type != "cpu":
+                raise TypeError("%s: host integers (a list, NumPy array or CPU tensor), not a CUDA tensor" % what)
+            ns = np.asarray(lengths.tolist() if isinstance(lengths, torch.Tensor) else lengths)
+            if ns.ndim != 1 or (ns.size and not np.issubdtype(ns.dtype, np.integer)):
+                raise TypeError("%s: one int per clip" % what)
+            ns = ns.astype(np.int64)
+            if ns.shape[0] != B:
+                raise ValueError("%s: %d entries for %d clips" % (what, ns.shape[0], B))
+            bad = np.nonzero((ns < 1) | (ns > T))[0]
+            if bad.size:
+                raise ValueError("%s[%d] = %d: not within 1 .. %d samples" % (what, bad[0], ns[bad[0]], T))
+        fmt = E.FMT_S16 if x.dtype == torch.int16 else E.FMT_F32
+        return E.device_batch(x3.data_ptr(), fmt, ns, C, ch, T, x3.stride(0), x3.stride(1), int(sample_rate))
+
+    def _check_segments(self, name, n_samples, sample_rate):
+        """The file ingest's too-short / too-long errors (NISQA_lib._raise_for_status), on the host, before any launch"""
+        from . import resample as RS
+        rate = self.target_sr or sample_rate
+        a = self.args
+        for i, n in enumerate(n_samples):
+            n = int(n) if rate == sample_rate else RS.out_len(int(n), sample_rate, rate)
+            _, n_seg, status = E.segment_counts(self.cfg, n, rate)
+            err = E.clip_status_error(status, "%s[%d]" % (name, i), n, rate, n_seg, a["ms_hop_length"], a["ms_seg_length"],
+                                      a["ms_max_segments"])
+            if err is not None:
+                raise err

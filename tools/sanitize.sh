@@ -2,7 +2,8 @@
 # GPU-box memory / race / init check of every kernel on the default path (SURVEY.md section 5: the reference has no
 # sanitizer story; this is ours): compute-sanitizer memcheck over __graft_entry__.smoke() (nisqa.tar, two
 # short clips at 48 / 16 kHz: front-end, conv1, the five wgmma conv layers with their bulk copies /
-# mbarriers, self-attention, pooling) and over a short nisqa_tts.tar call (StandardCNN, BiLSTM).
+# mbarriers, self-attention, pooling), over a short nisqa_tts.tar call (StandardCNN, BiLSTM) and over device-batch
+# calls (the ingest kernel, with and without ms_sr).
 #   bash tools/sanitize.sh TAG
 TAG=${1:-rXX}
 OUT=gpurun_out
@@ -44,8 +45,18 @@ for so, sn in ((48000, 16000), (16000, 44100)):
     assert np.array_equal(e3.resample_device(xs, so, sn), RS.resample(xs, so, sn))
 print("resample ok", e3.predict_pcm_resampled([x, synth.synth_speech_pcm16(11, 0.5, 48000)], [16000, 48000], 16000)[0].tolist())
 e3.close()
+# device-batch ingest (csrc/ingest.cu): int16 channel pick, float32 mix of strided channels, ms_sr into a conversion slot
+import torch
+from nisqa_b200.scorer import Scorer
+w = torch.from_numpy(np.stack([synth.synth_speech_pcm16(12 + c, 0.7, 48000) for c in range(2)])[None]).cuda()   # [1, 2, T]
+s4 = Scorer(os.path.join("weights", "nisqa.tar"))
+print("ingest", s4(w, 48000, channel=1).tolist(), s4(w.float() / 32768, 48000).tolist())
+s4.close()
+s5 = Scorer(os.path.join("weights", "nisqa_mos_only.tar"), ms_sr=16000)
+print("ingest ms_sr", s5(w[0], 48000, lengths=[30000, w.shape[-1]]).tolist())
+s5.close()
 PY
-timeout 280 compute-sanitizer --tool memcheck --error-exitcode 7 --log-file $OUT/${TAG}_memcheck.log python /tmp/san_run.py > $OUT/${TAG}_memcheck_stdout.log 2>&1
+timeout 400 compute-sanitizer --tool memcheck --error-exitcode 7 --log-file $OUT/${TAG}_memcheck.log python /tmp/san_run.py > $OUT/${TAG}_memcheck_stdout.log 2>&1
 echo "memcheck exit $?"
 tail -5 $OUT/${TAG}_memcheck.log; tail -3 $OUT/${TAG}_memcheck_stdout.log
 # shared-memory hazards (racecheck) and uninitialised device reads (initcheck) of the same run (RACE=1)
