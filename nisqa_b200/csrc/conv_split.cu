@@ -26,11 +26,11 @@
 // exists.  The 9 taps are the same tile read at row-shifted addresses: im2col is never materialised.
 //
 // GEMM view:  D[pos, co] = sum_{tap, ci} X[pos + off(tap), ci] * W[tap][co][ci]
-//   M = the interior output positions of G segments (SpCfg::gemm_row: GEMM row -> plane row; the zero row / column
-//   positions are not computed), N = C_out, K = 9 * C_in.  Warpgroup b < NBLK owns GEMM rows 64 b .. 64 b + 63: A
+//   M = the interior output positions of G segments (gemm_row: GEMM row -> plane row; the zero row / column
+//   positions are not computed), N = C_out, K = NTAP * C_in.  Warpgroup b < NBLK owns GEMM rows 64 b .. 64 b + 63: A
 //   fragments come from the swizzled tile with ldmatrix, one gathered row address per lane (8 rows of distinct
 //   plane row mod 8 hit 8 distinct 16-byte bank groups; a group that crosses a zero column may repeat one), B
-//   (all nine weight taps, resident for the CTA's life) through shared-memory descriptors, accumulators in
+//   (all NTAP weight taps, resident for the CTA's life) through shared-memory descriptors, accumulators in
 //   registers.  CTAs are persistent: the weights are loaded once per CTA, the tiles are walked with a grid stride.
 //   Epilogue: registers -> bias / ReLU -> fp32 staging tile -> (max-pool) -> split -> planes of the next layer.
 //   One tap (CIN <= 32) or half a tap (CIN 64) is kept in flight: its A fragments load while the previous unit's
@@ -96,20 +96,22 @@ __device__ __forceinline__ void mma_unit(float (&acc_m)[NB][C::COUT / 2], float 
     }
 }
 
-// All nine weight taps have landed.  Called before tile_gemm, never between its in-flight wgmmas: a wait loop there
+// All NTAP weight taps have landed.  Called before tile_gemm, never between its in-flight wgmmas: a wait loop there
 // makes ptxas serialize them.
+template <class C>
 __device__ __forceinline__ void wait_weights(uint32_t bar_w) {
-  for (int t = 0; t < 9; ++t) mbar_wait(bar_w + 8 * t, 0);
+  for (int t = 0; t < C::NTAP; ++t) mbar_wait(bar_w + 8 * t, 0);
 }
 
-// The GEMM of one tile for this warpgroup's NB m64 blocks: acc_m[b] = hi*hi, acc_s[b] = hi*lo + lo*hi over the nine
-// taps, in tap order.  row[b] is this lane's ldmatrix row of block b at tap offset 0.  The weights must have landed
+// The GEMM of one tile for this warpgroup's NB m64 blocks: acc_m[b] = hi*hi, acc_s[b] = hi*lo + lo*hi over the NTAP
+// taps, in tap order: tap t = 3 x KX position (t / KX, t % KX) reads tile row offset (t / KX - 1) P + t % KX - PADX.
+// row[b] is this lane's ldmatrix row of block b at tap offset 0, P the row pitch.  The weights must have landed
 // (wait_weights).
 template <class C, int NB>
 __device__ __forceinline__ void tile_gemm(float (&acc_m)[NB][C::COUT / 2], float (&acc_s)[NB][C::COUT / 2], uint32_t a_hi,
-                                          uint32_t a_lo, uint32_t b_base, const int (&row)[NB], int lchunk) {
+                                          uint32_t a_lo, uint32_t b_base, const int (&row)[NB], int lchunk, int P) {
   using U = TapUnits<C>;
-  constexpr int P = C::P, UK = U::UK, PT = U::PER_TAP;
+  constexpr int UK = U::UK, PT = U::PER_TAP;
   static_assert(C::CIN <= 32 || NB == 1, "CIN 64: one m64 block per warpgroup");
 #pragma unroll
   for (int b = 0; b < NB; ++b)
@@ -117,7 +119,7 @@ __device__ __forceinline__ void tile_gemm(float (&acc_m)[NB][C::COUT / 2], float
     for (int i = 0; i < C::COUT / 2; ++i) { acc_m[b][i] = 0.f; acc_s[b][i] = 0.f; }
   // one unit in flight: unit u + 1's fragments load into the other register set while unit u's wgmmas run
   uint32_t ah[2][NB][UK][4], al[2][NB][UK][4];
-  load_unit<C, NB>(a_hi, a_lo, row, -P - 1, 0, lchunk, ah[0], al[0]);
+  load_unit<C, NB>(a_hi, a_lo, row, -P - C::PADX, 0, lchunk, ah[0], al[0]);
 #pragma unroll
   for (int u = 0; u < U::N; ++u) {
     wgmma_fence();
@@ -126,7 +128,8 @@ __device__ __forceinline__ void tile_gemm(float (&acc_m)[NB][C::COUT / 2], float
     if (u + 1 < U::N) {
       wgmma_wait<1>();                           // unit u - 1 is done with the set that unit u + 1 loads into
       const int v = u + 1, t = v / PT;
-      load_unit<C, NB>(a_hi, a_lo, row, (t / 3 - 1) * P + (t % 3 - 1), (v % PT) * UK, lchunk, ah[v & 1], al[v & 1]);
+      load_unit<C, NB>(a_hi, a_lo, row, (t / C::KX - 1) * P + (t % C::KX - C::PADX), (v % PT) * UK, lchunk, ah[v & 1],
+                       al[v & 1]);
     }
   }
   wgmma_wait<0>();
@@ -142,16 +145,16 @@ __device__ __forceinline__ void load_bias(const float* __restrict__ bias, int ac
 // epilogue part 1 for one m64 block: accumulators of GEMM rows m0 and m0 + 8 -> bias (load_bias) + ReLU -> the staging
 // rows of their plane positions (every interior position of the tile's live segments is written: store_tile reads them
 // all)
-template <class C>
-__device__ __forceinline__ void stage_rows(const float (&acc_m)[C::COUT / 2], const float (&acc_s)[C::COUT / 2], int m0,
-                                           int acol, int seg0, int n_seg, const float2 (&bb)[C::COUT / 8], float out_scale,
-                                           float* stg) {
+template <class C, class Geo>
+__device__ __forceinline__ void stage_rows(const Geo& g, const float (&acc_m)[C::COUT / 2], const float (&acc_s)[C::COUT / 2],
+                                           int m0, int acol, int seg0, int n_seg, const float2 (&bb)[C::COUT / 8],
+                                           float out_scale, float* stg) {
   constexpr int SS = C::STG_STRIDE;
 #pragma unroll
   for (int half = 0; half < 2; ++half) {
     const int m = m0 + 8 * half;
-    if (m < C::KEPT && seg0 + m / C::SEG_ROWS < n_seg) {
-      const int r = C::gemm_row(m);
+    if (m < g.KEPT && seg0 + m / g.SEG_ROWS < n_seg) {
+      const int r = gemm_row(g, m);
 #pragma unroll
       for (int j = 0; j < C::COUT / 8; ++j) {
         const int col = 8 * j + acol;
@@ -164,24 +167,31 @@ __device__ __forceinline__ void stage_rows(const float (&acc_m)[C::COUT / 2], co
 }
 
 // epilogue part 2 (threads t0, t0 + nthr, ...): staging tile -> max-pool / split / store of the tile's nvalid segments
-template <class C>
-__device__ __forceinline__ void store_tile(const float* stg, int seg0, int nvalid, int t0, int nthr, float store_scale,
-                                           unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo,
-                                           float* __restrict__ out_f32) {
-  constexpr int H = C::H, W = C::W, COUT = C::COUT, P = C::P, BLK = C::BLK, SS = C::STG_STRIDE;
+template <class C, class Geo>
+__device__ __forceinline__ void store_tile(const Geo& g, const float* stg, int seg0, int nvalid, int t0, int nthr,
+                                           float store_scale, unsigned char* __restrict__ out_hi,
+                                           unsigned char* __restrict__ out_lo, float* __restrict__ out_f32) {
+  constexpr int COUT = C::COUT, SS = C::STG_STRIDE;
+  const int H = g.H, W = g.W, P = g.P, BLK = g.BLK;
   if constexpr (C::POOL != SP_POOL_NONE) {
-    constexpr int POW = C::POW, HO = H / 2, C8 = COUT / 8;
-    for (int i = t0; i < nvalid * HO * POW * C8; i += nthr) {
+    constexpr int C8 = COUT / 8;
+    const int HO = g.HO, WO = g.WO;
+    for (int i = t0; i < nvalid * HO * WO * C8; i += nthr) {
       const int c8 = i % C8;
       int rest = i / C8;
-      const int pw = rest % POW; rest /= POW;
+      const int pw = rest % WO; rest /= WO;
       const int ph = rest % HO;
       const int s = rest / HO;
-      int x0, x1;
-      if (C::POOL == SP_POOL_ADAPT) { x0 = (pw * W) / POW; x1 = ((pw + 1) * W + POW - 1) / POW; }
+      // cell (ph, pw) is the maximum over rows [y0, y1) x columns [x0, x1).  MaxPool2d(2): 2 x 2.
+      // F.adaptive_max_pool2d: rows [floor(ph H / HO), ceil((ph + 1) H / HO)) x columns [floor(pw W / WO),
+      // ceil((pw + 1) W / WO)) - windows that may overlap, or repeat a row / column when the output is larger than the
+      // input.  The shipped maps halve the rows (H = 2 HO).
+      int y0 = 2 * ph, y1 = 2 * ph + 2, x0, x1;
+      if constexpr (C::RT) { y0 = (ph * H) / HO; y1 = ((ph + 1) * H + HO - 1) / HO; }
+      if (C::POOL == SP_POOL_ADAPT) { x0 = (pw * W) / WO; x1 = ((pw + 1) * W + WO - 1) / WO; }
       else { x0 = 2 * pw; x1 = 2 * pw + 2; }
       float4 ma = make_float4(0.f, 0.f, 0.f, 0.f), mb = ma;       // post-ReLU values are >= 0
-      for (int hy = 2 * ph; hy < 2 * ph + 2; ++hy)
+      for (int hy = y0; hy < y1; ++hy)
         for (int x = x0; x < x1; ++x) {
           const float4* tp = reinterpret_cast<const float4*>(stg + (s * BLK + (hy + 1) * P + (x + 1)) * SS + c8 * 8);
           const float4 ta = tp[0], tb = tp[1];
@@ -190,8 +200,8 @@ __device__ __forceinline__ void store_tile(const float* stg, int seg0, int nvali
         }
       uint4 hi, lo;
       split8(ma, mb, store_scale, hi, lo);
-      const int g = kSplitLead + (seg0 + s) * C::OBLK + (ph + 1) * C::OP + (pw + 1);
-      const size_t o = split_off<C::OROWB>(g, c8);
+      const int gr = kSplitLead + (seg0 + s) * g.OBLK + (ph + 1) * g.OP + (pw + 1);
+      const size_t o = split_off<C::OROWB>(gr, c8);
       *reinterpret_cast<uint4*>(out_hi + o) = hi;
       *reinterpret_cast<uint4*>(out_lo + o) = lo;
     }
@@ -211,24 +221,34 @@ __device__ __forceinline__ void store_tile(const float* stg, int seg0, int nvali
       *reinterpret_cast<uint4*>(out_lo + o) = lo;
     }
   } else {
-    // fp32 CNN features, channels-last [seg][HO][WO][COUT] in rows of OUT_LD floats
-    constexpr int HO = C::HO, WO = C::WO, C4 = COUT / 4;
-    for (int i = t0; i < nvalid * HO * WO * C4; i += nthr) {
-      const int c4 = i % C4;
-      int rest = i / C4;
-      const int w = rest % WO; rest /= WO;
-      const int h = rest % HO;
-      const int s = rest / HO;
-      const int r = s * BLK + (h + 1) * P + (C::CENTER ? 2 : w + 1);
-      float* dst = C::OUT_LD == C::OUT_COLS ? out_f32 + ((size_t)(seg0 + s) * (HO * WO) + h * WO + w) * COUT + c4 * 4
-                                            : out_f32 + (size_t)(seg0 + s) * C::OUT_LD + (h * WO + w) * COUT + c4 * 4;
-      *reinterpret_cast<float4*>(dst) = *reinterpret_cast<const float4*>(stg + r * SS + c4 * 4);
+    // fp32 CNN features, channels-last [seg][HO][WO][COUT] in rows of OUT_LD floats (the last layer does not pool)
+    constexpr int C4 = COUT / 4;
+    if constexpr (C::RT) {
+      // conv6 of a run-time geometry: one column, [seg][H][COUT]
+      for (int i = t0; i < nvalid * H * C4; i += nthr) {
+        const int c4 = i % C4, rest = i / C4, h = rest % H, s = rest / H;
+        *reinterpret_cast<float4*>(out_f32 + (size_t)(seg0 + s) * g.OUT_LD + h * COUT + c4 * 4) =
+            *reinterpret_cast<const float4*>(stg + (s * BLK + (h + 1) * P + g.X0) * SS + c4 * 4);
+      }
+    } else {
+      constexpr int HO = C::HO, WO = C::WO;
+      for (int i = t0; i < nvalid * HO * WO * C4; i += nthr) {
+        const int c4 = i % C4;
+        int rest = i / C4;
+        const int w = rest % WO; rest /= WO;
+        const int h = rest % HO;
+        const int s = rest / HO;
+        const int r = s * BLK + (h + 1) * P + (w + g.X0);
+        float* dst = g.OUT_LD == g.OUT_COLS ? out_f32 + ((size_t)(seg0 + s) * (HO * WO) + h * WO + w) * COUT + c4 * 4
+                                            : out_f32 + (size_t)(seg0 + s) * g.OUT_LD + (h * WO + w) * COUT + c4 * 4;
+        *reinterpret_cast<float4*>(dst) = *reinterpret_cast<const float4*>(stg + r * SS + c4 * 4);
+      }
     }
-    if constexpr (C::OUT_LD > C::OUT_COLS) {
-      // the padding columns are written as zeros: the Linear behind reads them (against zero weights)
-      constexpr int PAD4 = (C::OUT_LD - C::OUT_COLS) / 4;
-      for (int i = t0; i < nvalid * PAD4; i += nthr)
-        *reinterpret_cast<float4*>(out_f32 + (size_t)(seg0 + i / PAD4) * C::OUT_LD + C::OUT_COLS + (i % PAD4) * 4) =
+    // the padding columns are written as zeros: the Linear behind reads them (against zero weights)
+    if (C::RT || g.OUT_LD > g.OUT_COLS) {       // (a compile-time map's are known)
+      const int pad4 = (g.OUT_LD - g.OUT_COLS) / 4;
+      for (int i = t0; i < nvalid * pad4; i += nthr)
+        *reinterpret_cast<float4*>(out_f32 + (size_t)(seg0 + i / pad4) * g.OUT_LD + g.OUT_COLS + (i % pad4) * 4) =
             make_float4(0.f, 0.f, 0.f, 0.f);
     }
   }
@@ -239,41 +259,44 @@ __device__ __forceinline__ void store_tile(const float* stg, int seg0, int nvali
 // One warpgroup's wgmmas already use the tensor cores of all four SM sub-partitions.  With two activation buffers (the
 // shipped conv2, conv3) one thread issues the next tile's copy into the other buffer as soon as that buffer's readers
 // (the previous tile's GEMM) have arrived on its empty barrier; with one unaliased buffer (CIN 64 -> COUT 32) it issues
-// the copy once this tile's GEMM is done, so that it lands during the epilogue.
+// the copy once this tile's GEMM is done, so that it lands during the epilogue.  C::geom(geo) is the layer's geometry:
+// a compile-time type's constants (geo unused) or a run-time geometry type's argument.
 template <class C>
 __global__ void __launch_bounds__(C::NT, 1)
 conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* __restrict__ in_lo,
-                  const __half* __restrict__ wtc /*[9][CIN/8][hi co | lo co][8] fp16, scaled by 2^S*/,
+                  const __half* __restrict__ wtc /*[NTAP][CIN/8][hi co | lo co][8] fp16, scaled by 2^S*/,
                   const float* __restrict__ bias, float out_scale /*2^(e_in - S)*/, float store_scale /*2^-e_out*/,
                   unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo,
-                  float* __restrict__ out_f32 /*last layer only*/, int n_seg) {
-  constexpr int G = C::G, BLK = C::BLK, HALO = C::HALO, ROWB = C::ROWB, NT = C::NT;
+                  float* __restrict__ out_f32 /*last layer only*/, int n_seg, const SpGeom geo) {
+  constexpr int ROWB = C::ROWB, NT = C::NT, NTAP = C::NTAP;
+  const auto g = C::geom(geo);
+  const int G = g.G, BLK = g.BLK, HALO = g.HALO;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // swizzle atoms repeat every 1024 B
   const uint32_t sbase = smem_u32(smem);
   const uint32_t b_base = sbase + C::OFF_B;
-  const uint32_t bar_w = sbase + C::OFF_BAR, bar_full = bar_w + 8 * 9, bar_empty = bar_full + 8 * C::A_BUFS;
+  const uint32_t bar_w = sbase + C::OFF_BAR, bar_full = bar_w + 8 * NTAP, bar_empty = bar_full + 8 * C::A_BUFS;
   float* stg = reinterpret_cast<float*>(smem + C::OFF_STG);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const int n_tiles = (n_seg + G - 1) / G;
 
   // one thread: both planes of tile `tile` into activation buffer b, placed at row g0 & 7 (tile row == plane row mod 8)
   auto issue_tile = [&](int tile, int b) {
-    constexpr uint32_t A_COPY = (uint32_t)C::AROWS * ROWB;
+    const uint32_t a_copy = (uint32_t)(256 + 2 * HALO) * ROWB;
     const int g0 = kSplitLead + tile * G * BLK - HALO;
     const uint32_t dst = sbase + C::OFF_A_HI + b * C::A_BUF + (uint32_t)(g0 & 7) * ROWB;
-    mbar_expect_tx(bar_full + 8 * b, 2 * A_COPY);
-    bulk_g2s(dst, in_hi + (size_t)g0 * ROWB, A_COPY, bar_full + 8 * b);
-    bulk_g2s(dst + C::A_BYTES, in_lo + (size_t)g0 * ROWB, A_COPY, bar_full + 8 * b);
+    mbar_expect_tx(bar_full + 8 * b, 2 * a_copy);
+    bulk_g2s(dst, in_hi + (size_t)g0 * ROWB, a_copy, bar_full + 8 * b);
+    bulk_g2s(dst + C::A_BYTES, in_lo + (size_t)g0 * ROWB, a_copy, bar_full + 8 * b);
   };
 
   if (tid == 0) {
-    for (int t = 0; t < 9; ++t) mbar_init(bar_w + 8 * t, 1);
+    for (int t = 0; t < NTAP; ++t) mbar_init(bar_w + 8 * t, 1);
     for (int b = 0; b < C::A_BUFS; ++b) mbar_init(bar_full + 8 * b, 1);
     if constexpr (C::A_BUFS == 2)
       for (int b = 0; b < 2; ++b) mbar_init(bar_empty + 8 * b, NT);
     fence_barrier_init();
-    for (int t = 0; t < 9; ++t) {                // all nine taps stay resident; tap t's MMAs start once it has landed
+    for (int t = 0; t < NTAP; ++t) {             // all taps stay resident; tap t's MMAs start once it has landed
       mbar_expect_tx(bar_w + 8 * t, C::B_STAGE);
       bulk_g2s(b_base + t * C::B_STAGE, wtc + (size_t)t * (C::B_STAGE / 2), C::B_STAGE, bar_w + 8 * t);
     }
@@ -282,7 +305,7 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
   __syncthreads();
 
   // this lane's ldmatrix row (the tile row of GEMM row m within its warp's 16 rows) and K chunk; its accumulator rows
-  const int lrow = HALO + C::gemm_row(wg * 64 + (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8);
+  const int lrow = HALO + gemm_row(g, wg * 64 + (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8);
   const int lchunk = lane >> 4;
   const int arow0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const int acol = 2 * (lane & 3);
@@ -314,10 +337,10 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
     float acc_m[1][C::COUT / 2], acc_s[1][C::COUT / 2];      // hi*hi ; hi*lo + lo*hi
 #pragma unroll
     for (int i = 0; i < C::COUT / 2; ++i) { acc_m[0][i] = 0.f; acc_s[0][i] = 0.f; }
-    if (__shfl_sync(0xffffffffu, wg < C::NBLK, 0)) {
+    if (__shfl_sync(0xffffffffu, wg < g.NBLK, 0)) {
       const int row[1] = {(g0 & 7) + lrow};
-      wait_weights(bar_w);
-      tile_gemm<C, 1>(acc_m, acc_s, a_hi, a_lo, b_base, row, lchunk);
+      wait_weights<C>(bar_w);
+      tile_gemm<C, 1>(acc_m, acc_s, a_hi, a_lo, b_base, row, lchunk, g.P);
     }
     if constexpr (C::A_BUFS == 2) mbar_arrive(bar_empty + 8 * ab);
     __syncthreads();                             // ALIAS: every warpgroup is done with the A tile the staging tile
@@ -329,220 +352,13 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
     // ===== epilogue part 1: accumulators -> bias + ReLU -> staging row of each GEMM row's plane position =====
     float2 bb[C::COUT / 8];
     load_bias<C>(bias, acol, bb);
-    stage_rows<C>(acc_m[0], acc_s[0], arow0, acol, seg0, n_seg, bb, out_scale, stg);   // (no rows past block NBLK - 1)
+    stage_rows<C>(g, acc_m[0], acc_s[0], arow0, acol, seg0, n_seg, bb, out_scale, stg);   // (no rows past block NBLK - 1)
     __syncthreads();
 
     // ===== epilogue part 2 (all threads): max-pool / split / store =====
-    store_tile<C>(stg, seg0, min(G, n_seg - seg0), tid, NT, store_scale, out_hi, out_lo, out_f32);
+    store_tile<C>(g, stg, seg0, min(G, n_seg - seg0), tid, NT, store_scale, out_hi, out_lo, out_f32);
     if constexpr (C::ALIAS) {
       fence_proxy_async();                       // staging stores (generic proxy) before the next tile's bulk copy
-      __syncthreads();
-    }
-  }
-}
-
-// ---- conv2..conv6 of an AdaptCNN with other pools: the same kernel on a run-time geometry ----
-// The pieces below are tile_gemm / stage_rows / store_tile with SpGeom's sizes in place of SpCfg's: the same tap order, the
-// same split and the same scales, so at equal sizes the values are those of conv_split_kernel.
-
-// tile_gemm over C::NTAP taps: tap t = 3 x KX position (t / KX, t % KX) reads tile row offset (t / KX - 1) P + t % KX - PADX
-template <class C>
-__device__ __forceinline__ void tile_gemm_rt(float (&acc_m)[1][C::COUT / 2], float (&acc_s)[1][C::COUT / 2], uint32_t a_hi,
-                                             uint32_t a_lo, uint32_t b_base, const int (&row)[1], int lchunk, int P) {
-  using U = TapUnits<C>;
-  constexpr int UK = U::UK, PT = U::PER_TAP;
-#pragma unroll
-  for (int i = 0; i < C::COUT / 2; ++i) { acc_m[0][i] = 0.f; acc_s[0][i] = 0.f; }
-  uint32_t ah[2][1][UK][4], al[2][1][UK][4];
-  load_unit<C, 1>(a_hi, a_lo, row, -P - C::PADX, 0, lchunk, ah[0], al[0]);
-#pragma unroll
-  for (int u = 0; u < U::N; ++u) {
-    wgmma_fence();
-    mma_unit<C, 1>(acc_m, acc_s, ah[u & 1], al[u & 1], b_base + (u / PT) * C::B_STAGE, (u % PT) * UK);
-    wgmma_commit();
-    if (u + 1 < U::N) {
-      wgmma_wait<1>();
-      const int v = u + 1, t = v / PT;
-      load_unit<C, 1>(a_hi, a_lo, row, (t / C::KX - 1) * P + (t % C::KX - C::PADX), (v % PT) * UK, lchunk, ah[v & 1], al[v & 1]);
-    }
-  }
-  wgmma_wait<0>();
-}
-
-template <class C>
-__device__ __forceinline__ void stage_rows_rt(const SpGeom& g, const float (&acc_m)[C::COUT / 2], const float (&acc_s)[C::COUT / 2],
-                                              int m0, int acol, int seg0, int n_seg, const float2 (&bb)[C::COUT / 8],
-                                              float out_scale, float* stg) {
-  constexpr int SS = C::STG_STRIDE;
-#pragma unroll
-  for (int half = 0; half < 2; ++half) {
-    const int m = m0 + 8 * half;
-    if (m < g.KEPT && seg0 + m / g.SEG_ROWS < n_seg) {
-      const int r = g.gemm_row(m);
-#pragma unroll
-      for (int j = 0; j < C::COUT / 8; ++j) {
-        const int col = 8 * j + acol;
-        const float v0 = fmaxf(fmaf(acc_m[4 * j + 2 * half] + acc_s[4 * j + 2 * half], out_scale, bb[j].x), 0.f);
-        const float v1 = fmaxf(fmaf(acc_m[4 * j + 2 * half + 1] + acc_s[4 * j + 2 * half + 1], out_scale, bb[j].y), 0.f);
-        *reinterpret_cast<float2*>(stg + r * SS + col) = make_float2(v0, v1);
-      }
-    }
-  }
-}
-
-// store_tile on a run-time geometry.  The pooling layers run F.adaptive_max_pool2d in both dimensions: cell (ph, pw) is the
-// maximum over rows [floor(ph H / HO), ceil((ph + 1) H / HO)) x columns [floor(pw W / WO), ceil((pw + 1) W / WO)) - windows
-// that may overlap, or repeat a row / column when the output is larger than the input.
-template <class C>
-__device__ __forceinline__ void store_tile_rt(const SpGeom& g, const float* stg, int seg0, int nvalid, int t0, int nthr,
-                                              float store_scale, unsigned char* __restrict__ out_hi,
-                                              unsigned char* __restrict__ out_lo, float* __restrict__ out_f32) {
-  constexpr int COUT = C::COUT, SS = C::STG_STRIDE;
-  const int H = g.H, W = g.W, P = g.P, BLK = g.BLK;
-  if constexpr (C::POOLED) {
-    constexpr int C8 = COUT / 8;
-    const int HO = g.HO, WO = g.WO;
-    for (int i = t0; i < nvalid * HO * WO * C8; i += nthr) {
-      const int c8 = i % C8;
-      int rest = i / C8;
-      const int pw = rest % WO; rest /= WO;
-      const int ph = rest % HO;
-      const int s = rest / HO;
-      const int y0 = (ph * H) / HO, y1 = ((ph + 1) * H + HO - 1) / HO;
-      const int x0 = (pw * W) / WO, x1 = ((pw + 1) * W + WO - 1) / WO;
-      float4 ma = make_float4(0.f, 0.f, 0.f, 0.f), mb = ma;       // post-ReLU values are >= 0
-      for (int hy = y0; hy < y1; ++hy)
-        for (int x = x0; x < x1; ++x) {
-          const float4* tp = reinterpret_cast<const float4*>(stg + (s * BLK + (hy + 1) * P + (x + 1)) * SS + c8 * 8);
-          const float4 ta = tp[0], tb = tp[1];
-          ma.x = fmaxf(ma.x, ta.x); ma.y = fmaxf(ma.y, ta.y); ma.z = fmaxf(ma.z, ta.z); ma.w = fmaxf(ma.w, ta.w);
-          mb.x = fmaxf(mb.x, tb.x); mb.y = fmaxf(mb.y, tb.y); mb.z = fmaxf(mb.z, tb.z); mb.w = fmaxf(mb.w, tb.w);
-        }
-      uint4 hi, lo;
-      split8(ma, mb, store_scale, hi, lo);
-      const int gr = kSplitLead + (seg0 + s) * g.OBLK + (ph + 1) * g.OP + (pw + 1);
-      const size_t o = split_off<COUT * 2>(gr, c8);
-      *reinterpret_cast<uint4*>(out_hi + o) = hi;
-      *reinterpret_cast<uint4*>(out_lo + o) = lo;
-    }
-  } else if constexpr (C::OUT_SPLIT) {
-    constexpr int C8 = COUT / 8;
-    for (int i = t0; i < nvalid * BLK * C8; i += nthr) {
-      const int c8 = i % C8, r = i / C8;
-      const int q = r % BLK, hh = q / P, ww = q - hh * P;
-      uint4 hi = make_uint4(0u, 0u, 0u, 0u), lo = hi;
-      if (hh >= 1 && ww >= 1) {
-        const float4* tp = reinterpret_cast<const float4*>(stg + r * SS + c8 * 8);
-        split8(tp[0], tp[1], store_scale, hi, lo);
-      }
-      const size_t o = split_off<COUT * 2>(kSplitLead + seg0 * BLK + r, c8);
-      *reinterpret_cast<uint4*>(out_hi + o) = hi;
-      *reinterpret_cast<uint4*>(out_lo + o) = lo;
-    }
-  } else {
-    // conv6: fp32 CNN features [seg][H][COUT] in rows of OUT_LD floats, zero padding columns
-    constexpr int C4 = COUT / 4;
-    for (int i = t0; i < nvalid * H * C4; i += nthr) {
-      const int c4 = i % C4, rest = i / C4, h = rest % H, s = rest / H;
-      *reinterpret_cast<float4*>(out_f32 + (size_t)(seg0 + s) * g.OUT_LD + h * COUT + c4 * 4) =
-          *reinterpret_cast<const float4*>(stg + (s * BLK + (h + 1) * P + 1) * SS + c4 * 4);
-    }
-    const int pad4 = (g.OUT_LD - g.OUT_COLS) / 4;
-    for (int i = t0; i < nvalid * pad4; i += nthr)
-      *reinterpret_cast<float4*>(out_f32 + (size_t)(seg0 + i / pad4) * g.OUT_LD + g.OUT_COLS + (i % pad4) * 4) =
-          make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-}
-
-// conv_split_kernel with SpGeom's sizes: the same persistent CTA, tile copies, barriers and roles
-template <class C>
-__global__ void __launch_bounds__(C::NT, 1)
-conv_split_rt_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* __restrict__ in_lo,
-                     const __half* __restrict__ wtc, const float* __restrict__ bias, float out_scale, float store_scale,
-                     unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo, float* __restrict__ out_f32,
-                     int n_seg, const SpGeom g) {
-  constexpr int ROWB = C::ROWB, NT = C::NT, NTAP = C::NTAP;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const uint32_t sbase = smem_u32(smem);
-  const uint32_t b_base = sbase + C::OFF_B;
-  const uint32_t bar_w = sbase + C::OFF_BAR, bar_full = bar_w + 8 * NTAP, bar_empty = bar_full + 8 * C::A_BUFS;
-  float* stg = reinterpret_cast<float*>(smem + C::OFF_STG);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
-  const int G = g.G, BLK = g.BLK, HALO = g.HALO;
-  const int n_tiles = (n_seg + G - 1) / G;
-
-  auto issue_tile = [&](int tile, int b) {
-    const uint32_t a_copy = (uint32_t)(256 + 2 * HALO) * ROWB;
-    const int g0 = kSplitLead + tile * G * BLK - HALO;
-    const uint32_t dst = sbase + C::OFF_A_HI + b * C::A_BUF + (uint32_t)(g0 & 7) * ROWB;
-    mbar_expect_tx(bar_full + 8 * b, 2 * a_copy);
-    bulk_g2s(dst, in_hi + (size_t)g0 * ROWB, a_copy, bar_full + 8 * b);
-    bulk_g2s(dst + C::A_BYTES, in_lo + (size_t)g0 * ROWB, a_copy, bar_full + 8 * b);
-  };
-
-  if (tid == 0) {
-    for (int t = 0; t < NTAP; ++t) mbar_init(bar_w + 8 * t, 1);
-    for (int b = 0; b < C::A_BUFS; ++b) mbar_init(bar_full + 8 * b, 1);
-    if constexpr (C::A_BUFS == 2)
-      for (int b = 0; b < 2; ++b) mbar_init(bar_empty + 8 * b, NT);
-    fence_barrier_init();
-    for (int t = 0; t < NTAP; ++t) {
-      mbar_expect_tx(bar_w + 8 * t, C::B_STAGE);
-      bulk_g2s(b_base + t * C::B_STAGE, wtc + (size_t)t * (C::B_STAGE / 2), C::B_STAGE, bar_w + 8 * t);
-    }
-    if constexpr (!C::ALIAS) issue_tile(blockIdx.x, 0);
-  }
-  __syncthreads();
-
-  const int lrow = HALO + g.gemm_row(wg * 64 + (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8);
-  const int lchunk = lane >> 4;
-  const int arow0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  const int acol = 2 * (lane & 3);
-
-  int it = 0;
-  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-    const int seg0 = tile * G;
-    const int g0 = kSplitLead + seg0 * BLK - HALO;
-    const int ab = C::A_BUFS == 1 ? 0 : (it & 1);
-    if constexpr (C::ALIAS) {
-      if (tid == 0) issue_tile(tile, 0);
-      mbar_wait(bar_full, it & 1);
-    } else if constexpr (C::A_BUFS == 1) {
-      mbar_wait(bar_full, it & 1);
-    } else {
-      const int next = tile + gridDim.x;
-      if (tid == 0 && next < n_tiles) {
-        const int nb = (it + 1) & 1;
-        mbar_wait(bar_empty + 8 * nb, (((it + 1) >> 1) & 1) ^ 1);
-        issue_tile(next, nb);
-      }
-      mbar_wait(bar_full + 8 * ab, (it >> 1) & 1);
-    }
-
-    const uint32_t a_hi = sbase + C::OFF_A_HI + ab * C::A_BUF, a_lo = a_hi + C::A_BYTES;
-    float acc_m[1][C::COUT / 2], acc_s[1][C::COUT / 2];
-#pragma unroll
-    for (int i = 0; i < C::COUT / 2; ++i) { acc_m[0][i] = 0.f; acc_s[0][i] = 0.f; }
-    if (__shfl_sync(0xffffffffu, wg < g.NBLK, 0)) {
-      const int row[1] = {(g0 & 7) + lrow};
-      for (int t = 0; t < NTAP; ++t) mbar_wait(bar_w + 8 * t, 0);
-      tile_gemm_rt<C>(acc_m, acc_s, a_hi, a_lo, b_base, row, lchunk, g.P);
-    }
-    if constexpr (C::A_BUFS == 2) mbar_arrive(bar_empty + 8 * ab);
-    __syncthreads();
-    if constexpr (!C::ALIAS && C::A_BUFS == 1) {
-      if (tid == 0 && tile + (int)gridDim.x < n_tiles) issue_tile(tile + gridDim.x, 0);
-    }
-
-    float2 bb[C::COUT / 8];
-    load_bias<C>(bias, acol, bb);
-    stage_rows_rt<C>(g, acc_m[0], acc_s[0], arow0, acol, seg0, n_seg, bb, out_scale, stg);
-    __syncthreads();
-
-    store_tile_rt<C>(g, stg, seg0, min(G, n_seg - seg0), tid, NT, store_scale, out_hi, out_lo, out_f32);
-    if constexpr (C::ALIAS) {
-      fence_proxy_async();
       __syncthreads();
     }
   }
@@ -571,6 +387,7 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
               const float* __restrict__ w1 /*[9][16]*/, const float* __restrict__ b1 /*[16]*/,
               float c1_scale /*2^-e1: conv1's activation scale*/) {
   using L = SpFused<C>;
+  constexpr C g{};
   constexpr int W = C::W, P = C::P, HALO = C::HALO, ROWB = C::ROWB, NT = C::NT, NR = NT / 2;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -615,12 +432,12 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
     // taken once, outside the loop, on the warp-uniform wg
     float2 bb[C::COUT / 8];
     load_bias<C>(bias, acol, bb);
-    wait_weights(bar_w);
+    wait_weights<C>(bar_w);
     auto mma_role = [&](auto nb, int b0) {
       constexpr int NB = decltype(nb)::value;
       int lrow[NB];
 #pragma unroll
-      for (int b = 0; b < NB; ++b) lrow[b] = HALO + C::gemm_row(lm + 64 * (b0 + b));
+      for (int b = 0; b < NB; ++b) lrow[b] = HALO + gemm_row(g, lm + 64 * (b0 + b));
       int it = 0;
       for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
         const int ab = it & 1;
@@ -628,14 +445,14 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
         mbar_wait(a_full + 8 * ab, par);
         const uint32_t a_hi = sbase + L::OFF_A + ab * C::A_BUF, a_lo = a_hi + C::A_BYTES;
         float acc_m[NB][C::COUT / 2], acc_s[NB][C::COUT / 2];
-        tile_gemm<C, NB>(acc_m, acc_s, a_hi, a_lo, b_base, lrow, lchunk);
+        tile_gemm<C, NB>(acc_m, acc_s, a_hi, a_lo, b_base, lrow, lchunk, P);
         mbar_arrive(a_empty + 8 * ab);
         float* stg = reinterpret_cast<float*>(smem + L::OFF_STG + ab * C::STG_BYTES);
 #pragma unroll
         for (int b = 0; b < NB; ++b)
-          stage_rows<C>(acc_m[b], acc_s[b], am + 64 * (b0 + b), acol, tile, n_seg, bb, out_scale, stg);
+          stage_rows<C>(g, acc_m[b], acc_s[b], am + 64 * (b0 + b), acol, tile, n_seg, bb, out_scale, stg);
         named_bar_sync<1, NR>();
-        store_tile<C>(stg, tile, 1, tid, NR, store_scale, out_hi, out_lo, nullptr);
+        store_tile<C>(g, stg, tile, 1, tid, NR, store_scale, out_hi, out_lo, nullptr);
       }
     };
     if (wg == 0) mma_role(std::integral_constant<int, 2>(), 0);
@@ -750,20 +567,21 @@ static int device_sms() {
   return n > 0 ? n : 1;
 }
 
+// geo: a run-time geometry type's geometry (compile-time types have theirs)
 template <class C>
 static void launch_sp(cudaStream_t st, const unsigned char* in_hi, const unsigned char* in_lo, const __half* wtc,
                       const float* b, float scale, float store_scale, unsigned char* out_hi, unsigned char* out_lo,
-                      float* out_f32, int n_seg) {
+                      float* out_f32, int n_seg, const SpGeom& geo = SpGeom{}) {
   static unsigned long long configured = 0;
   static int n_sm = 0;
   if (first_launch_on_device(configured)) {
     cudaFuncSetAttribute(conv_split_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     n_sm = device_sms();
   }
-  const int n_tiles = (n_seg + C::G - 1) / C::G;
+  const int n_tiles = (n_seg + C::geom(geo).G - 1) / C::geom(geo).G;
   const int grid = std::min(n_tiles, n_sm);              // one persistent CTA per SM
   conv_split_kernel<C><<<grid, C::NT, C::SMEM_BYTES, st>>>(in_hi, in_lo, wtc, b, scale, store_scale, out_hi, out_lo,
-                                                           out_f32, n_seg);
+                                                           out_f32, n_seg, geo);
 }
 
 template <class C, int MODE>
@@ -779,22 +597,6 @@ static void launch_c12(cudaStream_t st, const __half* wtc, const float* b, float
   const int grid = std::min(n_seg, n_sm);                // one persistent CTA per SM, one segment per tile
   conv12_kernel<C, MODE><<<grid, C::NT, SpFused<C>::SMEM_BYTES, st>>>(wtc, b, scale, store_scale, out_hi, out_lo, n_seg,
                                                                       mel, seg_frame0, seg_thr, w1, b1, c1_scale);
-}
-
-template <class C>
-static void launch_sp_rt(cudaStream_t st, const unsigned char* in_hi, const unsigned char* in_lo, const __half* wtc,
-                         const float* b, float scale, float store_scale, unsigned char* out_hi, unsigned char* out_lo,
-                         float* out_f32, int n_seg, const SpGeom& g) {
-  static unsigned long long configured = 0;
-  static int n_sm = 0;
-  if (first_launch_on_device(configured)) {
-    cudaFuncSetAttribute(conv_split_rt_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
-    n_sm = device_sms();
-  }
-  const int n_tiles = (n_seg + g.G - 1) / g.G;
-  const int grid = std::min(n_tiles, n_sm);
-  conv_split_rt_kernel<C><<<grid, C::NT, C::SMEM_BYTES, st>>>(in_hi, in_lo, wtc, b, scale, store_scale, out_hi, out_lo,
-                                                              out_f32, n_seg, g);
 }
 
 #define NISQA_SP_GEOM(L, CI, CO) static_assert(input_is<SpAdapt<L, CI, CO>>(0, L), "SpCfg geometry differs from split_geometry");
@@ -818,9 +620,9 @@ bool conv_split_supported(int cin, int cout) {
 }
 
 // conv layer 2..6 (cin -> cout channels) on planes; the last layer (6) writes the fp32 CNN features (adapt:
-// [seg][pool_3 h][c3] in rows padded to a multiple of 64 floats; standard: [seg][6][2][64]).  AdaptCNN layers whose input
-// map and output pooling are the shipped ones run the compile-time instances, every other one the run-time geometry
-// kernel.  false: no instance for the shape.
+// [seg][pool_3 h][c3] in rows padded to a multiple of 64 floats; standard: [seg][6][2][64]).  StandardCNN layers and
+// AdaptCNN layers whose input map and output pooling are the shipped ones run the compile-time instances, every other
+// one a run-time geometry instance.  false: no instance for the shape.
 bool launch_conv_split(cudaStream_t st, int std_mode, int layer, int cin, int cout, const void* in_hi, const void* in_lo,
                        const void* wtc, const float* b, float out_scale, float store_scale, void* out_hi,
                        void* out_lo, float* out_f32, int n_seg, const CnnPools& pools) {
@@ -829,21 +631,18 @@ bool launch_conv_split(cudaStream_t st, int std_mode, int layer, int cin, int co
   const unsigned char* il = static_cast<const unsigned char*>(in_lo);
   unsigned char* oh = static_cast<unsigned char*>(out_hi);
   unsigned char* ol = static_cast<unsigned char*>(out_lo);
-  if (!std_mode && !shipped_layer_geometry(layer, pools)) {
-    const ConvGeom in = split_geometry(0, layer, cin, pools);
-    const ConvGeom out = layer < 6 ? split_geometry(0, layer + 1, cout, pools) : ConvGeom{in.H, 1, cout};
-    const SpGeom g = sp_geom(layer, in.H, in.W, out.H, out.W, cout);
-    const int ntap = layer == 6 ? 3 * in.W : 9;
-#define NISQA_SP_RT_LAUNCH(L, CI, CO, NT)                                                                    \
-    if (layer == L && cin == CI && cout == CO && ntap == NT) {                                                \
-      launch_sp_rt<SpRt<L, CI, CO, NT>>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg, g);  \
-      return true;                                                                                            \
+  if (std_mode) {
+    if (cin != split_geometry(1, layer, 0).C || cout != (layer == 2 ? 32 : 64)) return false;
+    switch (layer) {
+      case 2: launch_sp<SpConv2S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 3: launch_sp<SpConv3S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 4: launch_sp<SpConv4S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 5: launch_sp<SpConv5S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      default: launch_sp<SpConv6S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
     }
-    NISQA_SP_RT_LAYERS(NISQA_SP_RT_LAUNCH)
-#undef NISQA_SP_RT_LAUNCH
-    return false;
+    return true;
   }
-  if (!std_mode) {
+  if (shipped_layer_geometry(layer, pools)) {
 #define NISQA_SP_LAUNCH(L, CI, CO)                                                                           \
     if (layer == L && cin == CI && cout == CO) {                                                              \
       launch_sp<SpAdapt<L, CI, CO>>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg);        \
@@ -853,15 +652,19 @@ bool launch_conv_split(cudaStream_t st, int std_mode, int layer, int cin, int co
 #undef NISQA_SP_LAUNCH
     return false;
   }
-  if (cin != split_geometry(1, layer, 0).C || cout != (layer == 2 ? 32 : 64)) return false;
-  switch (layer) {
-    case 2: launch_sp<SpConv2S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-    case 3: launch_sp<SpConv3S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-    case 4: launch_sp<SpConv4S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-    case 5: launch_sp<SpConv5S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-    default: launch_sp<SpConv6S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+  // conv6 reads its whole input width (3 x W taps) and writes one column
+  const ConvGeom in = split_geometry(0, layer, cin, pools);
+  const ConvGeom out = layer < 6 ? split_geometry(0, layer + 1, cout, pools) : ConvGeom{in.H, 1, cout};
+  const SpGeom g = sp_geom(in.H, in.W, layer == 6 ? 1 : in.W, 1, out.H, out.W, cout);
+  const int ntap = layer == 6 ? 3 * in.W : 9;
+#define NISQA_SP_RT_LAUNCH(L, CI, CO, NT)                                                                    \
+  if (layer == L && cin == CI && cout == CO && ntap == NT) {                                                  \
+    launch_sp<SpRt<L, CI, CO, NT>>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg, g);      \
+    return true;                                                                                              \
   }
-  return true;
+  NISQA_SP_RT_LAYERS(NISQA_SP_RT_LAUNCH)
+#undef NISQA_SP_RT_LAUNCH
+  return false;
 }
 
 bool conv12_supported(int std_mode, int c1, int c2) { return c1 == 16 && (c2 == 32 || (!std_mode && c2 == 16)); }
