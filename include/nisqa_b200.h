@@ -111,8 +111,12 @@ enum nisqa_stage {
                              * self-attention stack: td2_d_model when td_2 runs, else sa_d_model) or [n_seg, dirs*H] (the
                              * last LSTM layer, fwd||bwd); arch 4 without td_2: the framewise output [n_seg, fan_out] in
                              * the reference's column order (AdaptCNN c*6+h, StandardCNN c*12+h*2+w, or the Linear's) */
-  NISQA_STAGE_TD1_OUT  = 9  /* NISQA / NISQA_DIM with a td and a td_2 stage: td's output rows [n_seg, td fan_out] (D or
-                             * dirs*H); not available without a td (arch 4, 5)                                          */
+  NISQA_STAGE_TD1_OUT  = 9, /* a td and a td_2 stage (NISQA / NISQA_DIM; NISQA_DE: the rows the alignment reads, of both
+                             * clips of every pair): td's output rows [n_seg, td fan_out] (D or dirs*H); not available
+                             * without a td (arch 4, 5)                                                                 */
+  NISQA_STAGE_DE_FUSED = 10 /* NISQA_DE: the alignment + fusion output [n_seg, 64*nf] (nf = 3 for de_fuse 'x/y/-', else
+                             * 2) before Fusion.lin_fusion; the rows of the reference clips are zero.  Not available for
+                             * a single-ended model                                                                      */
 };
 
 /* Mirrors the checkpoint 'args' the hot path consumes (SURVEY.md Appendix A). */

@@ -295,6 +295,8 @@ struct nisqa_engine {
   int last_td_out_hw = 0;       // td = 'skip': conv6 features in the engine's order [hw][c3] (pool_3 h / 12); 0: the reference's
   const float* last_td1_out = nullptr;    // td's output when a td_2 stage ran (NISQA_STAGE_TD1_OUT)
   int last_td1_out_d = 0, last_td1_out_ld = 0;
+  const float* last_de_fused = nullptr;   // de_align_kernel's output (NISQA_STAGE_DE_FUSED)
+  int last_de_fused_d = 0;
 
   // engine-owned NCCL communicator (multi-GPU gather, SURVEY.md 8e)
   void* nccl_comm = nullptr;
@@ -1383,6 +1385,8 @@ int de_fuse(Pass& p, const float* td_rows, Rows* out) {
     launch_de_align(p.st, td_rows, p.clips, p.n, p.qt64_prefix, p.n_qt64, c.de_align, c.de_align_apply == NISQA_DE_APPLY_SOFT,
                     c.de_fuse, p.w.de, LN.fused.as<float>()); }
   *out = {LN.fused.as<float>(), nf};
+  e->last_de_fused = LN.fused.as<float>();      // (nothing behind the alignment writes fused: lin_fusion writes ffa, td_2 its own buffers)
+  e->last_de_fused_d = 64 * nf;
   if (c.de_fuse_dim > 0) {
     Scope s(e, "de_align");
     CK(LN.ffa.reserve((size_t)n_seg * c.de_fuse_dim * 4));
@@ -1521,7 +1525,8 @@ int td_stages(Pass& p, Rows rows) {
     D = L1.dirs * L1.H;
   }
   e->last_td1_out = nullptr;
-  if (e->td2_runs() && !de && !skip) { e->last_td1_out = cur.x; e->last_td1_out_d = D; e->last_td1_out_ld = 64 * cur.nk; }
+  e->last_de_fused = nullptr;
+  if (e->td2_runs() && !skip) { e->last_td1_out = cur.x; e->last_td1_out_d = D; e->last_td1_out_ld = 64 * cur.nk; }
   if (de) {
     Rows fused;
     const int rc = de_fuse(p, cur.x, &fused);
@@ -1574,6 +1579,7 @@ int lstm_head(Pass& p) {
   }
   e->last_td_in = nullptr;
   e->last_td1_out = nullptr;
+  e->last_de_fused = nullptr;
   e->last_td_out = (e->lstm_batched && !keep) ? nullptr : LN.tdout.as<float>();
   e->last_td_out_d = 256;
   e->last_td_out_ld = 256;
@@ -2151,6 +2157,9 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
     case NISQA_STAGE_TD1_OUT:
       if (!e->last_td1_out) return fail(e, NISQA_ERR_INVALID, "stage not available: no td_2 stage ran");
       src = e->last_td1_out; count = ns * e->last_td1_out_d; width = e->last_td1_out_d; ld = e->last_td1_out_ld; break;
+    case NISQA_STAGE_DE_FUSED:
+      if (!e->last_de_fused) return fail(e, NISQA_ERR_INVALID, "stage not available: only a double-ended model aligns and fuses");
+      src = e->last_de_fused; count = ns * e->last_de_fused_d; break;
     case NISQA_STAGE_TD_OUT:
       if (!e->last_td_out) return fail(e, NISQA_ERR_STATE, "the per-step BiLSTM outputs were not kept: nisqa_set_option(\"keep_td_out\", 1) before the predict call");
       src = e->last_td_out; count = ns * e->last_td_out_d; width = e->last_td_out_d; ld = e->last_td_out_ld;

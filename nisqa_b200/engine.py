@@ -27,7 +27,7 @@ DE_ALIGN = {"dot": 1, "cosine": 2, "distance": 3, "luong": 4, "bahd": 5}
 DE_APPLY = {"hard": 0, "soft": 1}
 DE_FUSE = {"x/y/-": 0, "+/-": 1, "x/y": 2}
 (STAGE_MEL_DB, STAGE_POOL1, STAGE_POOL2, STAGE_CONV3, STAGE_POOL3, STAGE_CONV5, STAGE_CNN_FEAT,
- STAGE_TD_IN, STAGE_TD_OUT, STAGE_TD1_OUT) = range(10)
+ STAGE_TD_IN, STAGE_TD_OUT, STAGE_TD1_OUT, STAGE_DE_FUSED) = range(11)
 
 # every symbol include/nisqa_b200.h declares (checked by tests/test_abi.py)
 EXPORTS = [

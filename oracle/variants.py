@@ -89,9 +89,10 @@ def td2_weights(sd, args, in_dim, rng):
         sd["time_dependency_2.model.pos_encoder.pe"] = positional_encoding()
 
 
-def de_checkpoint(name, base_args, base_sd):
-    """-> (args, state_dict) of a double-ended variant built on nisqa_mos_only.tar."""
-    over = DE_VARIANTS[name]
+def de_checkpoint(name, base_args, base_sd, over=None):
+    """-> (args, state_dict) of a double-ended variant built on nisqa_mos_only.tar: a DE_VARIANTS entry, or `over` (an
+    entry of the same form, seeded by `name`)."""
+    over = DE_VARIANTS[name] if over is None else over
     args = dict(base_args)
     args.update({"model": "NISQA_DE", "td_2": "self_att", "td_2_sa_d_model": 64, "td_2_sa_nhead": 1, "td_2_sa_pos_enc": None,
                  "td_2_sa_num_layers": 2, "td_2_sa_h": 64, "td_2_sa_dropout": 0.1, "td_2_lstm_h": None,

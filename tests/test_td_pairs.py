@@ -91,15 +91,15 @@ def test_config_refuses_pairings_outside_the_kernels():
 def test_header_enums_equal_the_binding(tmp_path):
     src = tmp_path / "enums.c"
     names = ["NISQA_CNN_STANDARD", "NISQA_ARCH_ADAPT_SA_ATTFF", "NISQA_ARCH_STD_LSTM_LASTBI", "NISQA_ARCH_SA_LSTM",
-             "NISQA_ARCH_LSTM_LSTM", "NISQA_STAGE_TD_IN", "NISQA_STAGE_TD_OUT", "NISQA_STAGE_TD1_OUT"]
+             "NISQA_ARCH_LSTM_LSTM", "NISQA_STAGE_TD_IN", "NISQA_STAGE_TD_OUT", "NISQA_STAGE_TD1_OUT", "NISQA_STAGE_DE_FUSED"]
     src.write_text('#include <stdio.h>\n#include "nisqa_b200.h"\nint main(void){printf("%zu' + " %d" * len(names)
                    + '\\n", sizeof(nisqa_config), ' + ", ".join(names) + ");return 0;}\n")
     exe = tmp_path / "enums"
     subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
     out = [int(x) for x in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
     assert out == [ctypes.sizeof(E.NisqaConfig), E.CNN_STANDARD, E.ARCH_ADAPT_SA_ATTFF, E.ARCH_STD_LSTM_LASTBI, E.ARCH_SA_LSTM,
-                   E.ARCH_LSTM_LSTM, E.STAGE_TD_IN, E.STAGE_TD_OUT, E.STAGE_TD1_OUT]
-    assert out[1:] == [3, 0, 1, 2, 3, 7, 8, 9]
+                   E.ARCH_LSTM_LSTM, E.STAGE_TD_IN, E.STAGE_TD_OUT, E.STAGE_TD1_OUT, E.STAGE_DE_FUSED]
+    assert out[1:] == [3, 0, 1, 2, 3, 7, 8, 9, 10]
 
 
 def test_oracle_matches_reference_modules_on_the_pair_variants():

@@ -3,7 +3,7 @@
 # sanitizer story; this is ours): compute-sanitizer memcheck over __graft_entry__.smoke() (nisqa.tar, two
 # short clips at 48 / 16 kHz: front-end, conv1, the five wgmma conv layers with their bulk copies /
 # mbarriers, self-attention, pooling), over a short nisqa_tts.tar call (StandardCNN, BiLSTM) and over device-batch
-# calls (the ingest kernel, with and without ms_sr).
+# calls (the ingest kernel, with and without ms_sr); racecheck over the double-ended alignment's multi-block path.
 #   bash tools/sanitize.sh TAG
 TAG=${1:-rXX}
 OUT=gpurun_out
@@ -34,6 +34,9 @@ for name in ("de_cosine_hard", "de_distance_soft_xy"):
     got = e2.predict_pcm([d, r], [srd, srr])[0]
     ref = O.predict_pcm_de(a2, s2, d.astype(np.float32) / 32768.0, srd, r.astype(np.float32) / 32768.0, srr)[0]
     assert abs(float(got[0, 0]) - float(ref[0])) <= 5e-4, (name, got, ref)
+    # a reference of 130 steps (three key blocks, the last with 2 keys) behind a 70-step degraded clip
+    d2, r2 = synth.synth_speech_pcm16(13, 2.9, 16000), synth.synth_speech_pcm16(14, 5.3, 16000)
+    assert e2.predict_pcm([d2, r2], [16000, 16000])[1].tolist() == [70, 130]
     e2.close()
 a3, s3 = V.variant_checkpoint("mos_td2_sa_pos_enc", bargs, bsd)
 e3 = E.Engine(E.config_from_args(a3), 0); e3.load_state_dict(s3)
@@ -59,7 +62,25 @@ PY
 timeout 400 compute-sanitizer --tool memcheck --error-exitcode 7 --log-file $OUT/${TAG}_memcheck.log python /tmp/san_run.py > $OUT/${TAG}_memcheck_stdout.log 2>&1
 echo "memcheck exit $?"
 tail -5 $OUT/${TAG}_memcheck.log; tail -3 $OUT/${TAG}_memcheck_stdout.log
-# shared-memory hazards (racecheck) and uninitialised device reads (initcheck) of the same run (RACE=1)
+# shared-memory hazards of de_align_kernel's key-block loop (Yb / Yn / Yp / YK reused across blocks): one soft and one
+# hard call whose reference spans three key blocks
+cat > /tmp/san_de.py <<'PY'
+import os, sys
+sys.path.insert(0, os.getcwd())
+from nisqa_b200 import engine as E, synth
+from oracle import nisqa_oracle as O, variants as V
+bargs, bsd = O.load_checkpoint(os.path.join("weights", "nisqa_mos_only.tar"))
+d, r = synth.synth_speech_pcm16(13, 2.9, 16000), synth.synth_speech_pcm16(14, 5.3, 16000)
+for name, over in (("de_luong_soft", None), ("de_bahd_hard", {"de_align": "bahd", "de_align_apply": "hard", "de_fuse": "+/-"})):
+    a, s = V.de_checkpoint(name, bargs, bsd, over)
+    e = E.Engine(E.config_from_args(a), 0); e.load_state_dict(s)
+    print(name, e.predict_pcm([d, r], [16000, 16000])[:2])
+    e.close()
+PY
+timeout 300 compute-sanitizer --tool racecheck --error-exitcode 7 --log-file $OUT/${TAG}_de_racecheck.log python /tmp/san_de.py > $OUT/${TAG}_de_racecheck_stdout.log 2>&1
+echo "de racecheck exit $?"
+tail -4 $OUT/${TAG}_de_racecheck.log; tail -2 $OUT/${TAG}_de_racecheck_stdout.log
+# shared-memory hazards (racecheck) and uninitialised device reads (initcheck) of the whole run (RACE=1)
 [ -z "$RACE" ] && exit 0
 timeout 400 compute-sanitizer --tool racecheck --error-exitcode 7 --log-file $OUT/${TAG}_racecheck.log python /tmp/san_run.py > $OUT/${TAG}_racecheck_stdout.log 2>&1
 echo "racecheck exit $?"
