@@ -114,9 +114,11 @@ enum nisqa_stage {
   NISQA_STAGE_TD1_OUT  = 9, /* a td and a td_2 stage (NISQA / NISQA_DIM; NISQA_DE: the rows the alignment reads, of both
                              * clips of every pair): td's output rows [n_seg, td fan_out] (D or dirs*H); not available
                              * without a td (arch 4, 5)                                                                 */
-  NISQA_STAGE_DE_FUSED = 10 /* NISQA_DE: the alignment + fusion output [n_seg, 64*nf] (nf = 3 for de_fuse 'x/y/-', else
-                             * 2) before Fusion.lin_fusion; the rows of the reference clips are zero.  Not available for
-                             * a single-ended model                                                                      */
+  NISQA_STAGE_DE_FUSED = 10 /* NISQA_DE: the alignment + fusion output before Fusion.lin_fusion, in the engine's PADDED
+                             * layout [n_seg, nf*Wp] (nf = 3 for de_fuse 'x/y/-', else 2; W = td's fan_out, Wp = W
+                             * rounded up to a multiple of 64): part p of the reference's compact [n_seg, nf*W] row
+                             * sits at columns p*Wp .. p*Wp + W - 1, the pad columns are zero.  W = 64: [n_seg, 64*nf].
+                             * The rows of the reference clips are zero.  Not available for a single-ended model       */
 };
 
 /* Mirrors the checkpoint 'args' the hot path consumes (SURVEY.md Appendix A). */
@@ -136,7 +138,9 @@ typedef struct nisqa_config {
   int32_t max_chunk_segments; /* 0 = default; upper bound on segments processed per internal pass */
   int32_t pool;          /* enum nisqa_pool */
   int32_t pos_enc;       /* td_sa_pos_enc: add the checkpoint's positional-encoding buffer after the input LayerNorm (lib:1042-1062) */
-  /* NISQA_DE (arch NISQA_ARCH_ADAPT_SA_ATTFF, n_out 1).  A double-ended engine takes its clips in PAIRS: clip 2p is the
+  /* NISQA_DE (n_out 1, td2_layers >= 1): arch NISQA_ARCH_ADAPT_SA_ATTFF (any framewise model + a self-attention td of
+   * d_model 64) or NISQA_ARCH_STD_LSTM_LASTBI (StandardCNN + an LSTM td of any accepted shape: the alignment and fusion
+   * run at its fan_out dirs*H, 32 .. 512).  A double-ended engine takes its clips in PAIRS: clip 2p is the
    * degraded signal, clip 2p + 1 its reference (csv_deg / csv_ref of one dataset row, lib:2132-2156); n_clips must be
    * even; scores_out row 2p holds the pair's score, row 2p + 1 is NaN; a pair with a skipped clip scores NaN. */
   int32_t double_ended;  /* 1: NISQA_DE */

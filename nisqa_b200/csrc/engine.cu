@@ -103,6 +103,7 @@ struct Lane {
   // td's stage works in tdout (self-attention: its TD_IN rows; LSTM: its output) and xa / xb, td_2's in td2in (its TD_IN
   // rows), td2out (an LSTM's output) and ya / yb, so that td's output is still there after td_2 (NISQA_STAGE_TD1_OUT)
   DevBuf mel, segtab, feats, xa, xb, ya, yb, qkv, qkv2, logits, feats20, tdout, td2out, partial, fused, td2in, ffa, ffb, gx, atth;
+  DevBuf dework;           // NISQA_DE: the alignment's projections / norms (de_align_work_floats)
   DevBuf act[7];           // act[l]: fp32 channels-last map feeding conv layer l (2..6) on the FFMA path (and stage dumps)
   DevBuf planes[7];        // planes[l]: fp16 hi | lo plane pair feeding conv layer l (2..6), conv_split.cu
   size_t plane_bytes[7] = {0, 0, 0, 0, 0, 0, 0};   // offset of the lo plane inside planes[l] (half of the allocation)
@@ -111,7 +112,7 @@ struct Lane {
     for (auto& b : act) b.release();
     for (auto& b : planes) b.release();
     DevBuf* all[] = {&mel, &segtab, &feats, &xa, &xb, &ya, &yb, &qkv, &qkv2, &logits, &feats20, &tdout, &td2out, &partial,
-                     &fused, &td2in, &ffa, &ffb, &gx, &atth};
+                     &fused, &td2in, &ffa, &ffb, &gx, &atth, &dework};
     for (auto* b : all) b->release();
     if (stream) cudaStreamDestroy(stream);
   }
@@ -578,12 +579,17 @@ void pack_linear_T(Packer& P, size_t off, const TensorView* w, int n_out, int n_
 }
 
 // W^T of an nn.Linear(n_in -> n_out) in 64-column chunks (the layout of the td_tiled.cu kernels): chunk n is the k-major
-// [k_pad][64] block at n k_pad 64; engine input row k reads checkpoint input column col(k); rows >= n_in stay zero
+// [k_pad][64] block at n k_pad 64; engine input row k < k_rows (default n_in) reads checkpoint input column col(k); rows
+// with col(k) < 0 and rows >= k_rows stay zero
 template <class Col>
-void pack_linear_chunked(Packer& P, size_t off, const TensorView* w, int n_out, int n_in, int k_pad, Col col) {
+void pack_linear_chunked(Packer& P, size_t off, const TensorView* w, int n_out, int n_in, int k_pad, Col col, int k_rows = -1) {
+  if (k_rows < 0) k_rows = n_in;
   for (int n = 0; n < n_out / 64; ++n)
-    for (int k = 0; k < n_in; ++k)
-      for (int j = 0; j < 64; ++j) P.arena[off + ((size_t)n * k_pad + k) * 64 + j] = w->d[(size_t)(n * 64 + j) * n_in + col(k)];
+    for (int k = 0; k < k_rows; ++k) {
+      const int kc = col(k);
+      if (kc < 0) continue;
+      for (int j = 0; j < 64; ++j) P.arena[off + ((size_t)n * k_pad + k) * 64 + j] = w->d[(size_t)(n * 64 + j) * n_in + kc];
+    }
 }
 
 // nn.MultiheadAttention scales q by D^-1/2 after the in-projection: folded into the packed q weights where that is a power
@@ -693,12 +699,17 @@ bool pack_framewise(Packer& P, nisqa_engine* e) {
 
 // The rows that feed a time-dependency stage: `dim` features, padded with zero columns to a multiple of 64, in the order
 // of the checkpoint's Linear (PLAIN) or - conv6's `ch` channels over `h` rows - in the engine's order: AdaptCNN k' = h*ch + c
-// <-> reference view(-1, ch*h3) order c*h3 + h (lib:706), StandardCNN k' = (h*2 + w)*64 + c <-> c*12 + h*2 + w (lib:830)
-enum InOrder { IN_PLAIN, IN_ADAPT_CONV, IN_STD_CONV };
+// <-> reference view(-1, ch*h3) order c*h3 + h (lib:706), StandardCNN k' = (h*2 + w)*64 + c <-> c*12 + h*2 + w (lib:830).
+// NISQA_DE's fused rows (IN_DE_FUSED): `dim` = nf W reference columns, part p of W columns at engine row p h (h = W padded
+// to a multiple of 64, ch = W); in_col is -1 on the pad rows.
+enum InOrder { IN_PLAIN, IN_ADAPT_CONV, IN_STD_CONV, IN_DE_FUSED };
 struct InRows { int dim; InOrder order; int ch = 64; int h = 6; };
 int in_col(const InRows& in, int k) {
+  if (in.order == IN_DE_FUSED) return k % in.h < in.ch ? (k / in.h) * in.ch + k % in.h : -1;
   return in.order == IN_ADAPT_CONV ? (k % in.ch) * in.h + k / in.ch : in.order == IN_STD_CONV ? (k & 63) * 12 + (k >> 6) : k;
 }
+// engine rows of `in`: the padded fused layout, or dim rounded up to a multiple of 64
+int in_rows(const InRows& in) { return in.order == IN_DE_FUSED ? in.dim / in.ch * in.h : (in.dim + 63) / 64 * 64; }
 
 // One SelfAttention stack (lib:945-1040) of width D and feed-forward width F, checkpoint prefix `ck`: Linear(in -> D) +
 // LayerNorm + `layers` encoder layers.  The Linear's rows beyond in.dim (the padding of the input rows) stay zero.
@@ -709,9 +720,9 @@ bool pack_sa_stack(Packer& P, SaStackWeights& S, const std::string& ck, InRows i
   const TensorView* ng = P.get(ck + "norm1.weight", {D});
   const TensorView* nb = P.get(ck + "norm1.bias", {D});
   if (!lw || !lb || !ng || !nb) return false;
-  const int k_pad = (in_dim + 63) / 64 * 64;
+  const int k_pad = in_rows(in);
   const size_t o = P.alloc(S.in.wT, (size_t)k_pad * D);
-  pack_linear_chunked(P, o, lw, D, in_dim, k_pad, [&](int k) { return in_col(in, k); });
+  pack_linear_chunked(P, o, lw, D, in_dim, k_pad, [&](int k) { return in_col(in, k); }, in.order == IN_DE_FUSED ? k_pad : in_dim);
   P.copy(S.in.b, lb->d, D);
   P.copy(S.ln_g, ng->d, D);
   P.copy(S.ln_b, nb->d, D);
@@ -763,34 +774,43 @@ bool pack_pos_enc(Packer& P, const nisqa_config& c, const std::string& ck, SaSta
   return true;
 }
 
-// NISQA_DE's learned alignment: AttLuong W = Linear(y_dim -> q_dim) (lib:1348-1351), AttBahdanau Wq, Wy (-> att_dim 128)
-// and v (lib:1329-1337)
-bool pack_de_align(Packer& P, const nisqa_config& c) {
+int round64(int n) { return (n + 63) / 64 * 64; }
+
+// NISQA_DE's learned alignment at td's fan_out W (q_dim = y_dim = W, lib:404-410): AttLuong W = Linear(y_dim -> q_dim)
+// (lib:1348-1351), AttBahdanau Wq, Wy (-> att_dim 128) and v (lib:1329-1337); k-major with W padded to a multiple of 64
+// by zero rows (and, for AttLuong, zero columns and bias), so that the projections of the padded td rows are exact and
+// their pad columns zero
+bool pack_de_align(Packer& P, const nisqa_config& c, int W) {
   DeAlignParams& A = P.w.de;
+  const int ld = round64(W);
   if (c.de_align == NISQA_DE_ALIGN_LUONG) {
-    const TensorView* w = P.get("align.att.W.weight", {64, 64});
-    const TensorView* b = P.get("align.att.W.bias", {64});
+    const TensorView* w = P.get("align.att.W.weight", {W, W});
+    const TensorView* b = P.get("align.att.W.bias", {W});
     if (!w || !b) return false;
-    pack_linear_T(P, P.alloc(A.wT, 4096), w, 64, 64);
-    P.copy(A.b, b->d, 64);
+    const size_t o = P.alloc(A.wT, (size_t)ld * ld);
+    for (int k = 0; k < W; ++k)
+      for (int j = 0; j < W; ++j) P.arena[o + (size_t)k * ld + j] = w->d[(size_t)j * W + k];
+    memcpy(&P.arena[P.alloc(A.b, ld)], b->d, (size_t)W * 4);
   }
   if (c.de_align == NISQA_DE_ALIGN_BAHDANAU) {
-    const TensorView* wq = P.get("align.att.Wq.weight", {128, 64});
+    const TensorView* wq = P.get("align.att.Wq.weight", {128, W});
     const TensorView* bq = P.get("align.att.Wq.bias", {128});
-    const TensorView* wy = P.get("align.att.Wy.weight", {128, 64});
+    const TensorView* wy = P.get("align.att.Wy.weight", {128, W});
     const TensorView* by = P.get("align.att.Wy.bias", {128});
     const TensorView* v = P.get("align.att.v.weight", {1, 128});
     if (!wq || !bq || !wy || !by || !v) return false;
-    pack_linear_T(P, P.alloc(A.wqT, 64 * 128), wq, 128, 64);
-    P.copy(A.bq, bq->d, 128);
-    pack_linear_T(P, P.alloc(A.wyT, 64 * 128), wy, 128, 64);
-    P.copy(A.by, by->d, 128);
+    const size_t o = P.alloc(A.wqyT, (size_t)ld * 256), ob = P.alloc(A.bqy, 256);
+    for (int k = 0; k < W; ++k)
+      for (int j = 0; j < 128; ++j) {
+        P.arena[o + (size_t)k * 256 + j] = wq->d[(size_t)j * W + k];
+        P.arena[o + (size_t)k * 256 + 128 + j] = wy->d[(size_t)j * W + k];
+      }
+    memcpy(&P.arena[ob], bq->d, 512);
+    memcpy(&P.arena[ob + 128], by->d, 512);
     P.copy(A.v, v->d, 128);
   }
   return true;
 }
-
-int round64(int n) { return (n + 63) / 64 * 64; }
 
 // The pooling module behind the time-dependency block, one head per output (order mos, noi, dis, col, loud:
 // lib:1461-1465), reading rows of in.dim features: PoolAttFF, or PoolAtt / PoolAvg / PoolMax / PoolLastStep /
@@ -999,7 +1019,7 @@ bool pack_td_model(Packer& P, nisqa_engine* e) {
     Weights::LstmShape& L = W.lstm_st[0].s;
     if (!read_lstm_shape(P, td + "lstm.", "td_lstm_h", &L)) return false;
     W.lstm_shipped = W.std_fc == 20 && L.H == 128 && L.layers == 1 && L.dirs == 2 && c.n_out == 1 && c.pool != NISQA_POOL_ATT &&
-                     c.pool != NISQA_POOL_ATT_FF && !e->td2_runs();
+                     c.pool != NISQA_POOL_ATT_FF && !e->td2_runs() && !c.double_ended;
     if (W.lstm_shipped) return pack_bilstm128(P, e);
     if (W.std_fc > 0 && !pack_std_fc(P, W.std_fc)) return false;
     if (!pack_lstm_stack(P, W.lstm_st[0], td + "lstm.", in)) return false;
@@ -1012,21 +1032,26 @@ bool pack_td_model(Packer& P, nisqa_engine* e) {
   }
   int dp = d1;                                        // width of the rows the pooling module reads
   if (c.double_ended || c.td2_layers > 0) {
-    // time_dependency_2: behind the fusion of the double-ended model (input 192 / 128), or a second stack behind td in
-    // NISQA / NISQA_DIM (input: td's fan_out)
-    int fdim = !c.double_ended ? d1 : (c.de_fuse == NISQA_DE_FUSE_XY_MINUS ? 192 : 128);
+    // time_dependency_2: behind the fusion of the double-ended model (input nf d1, in the padded fused layout: part p
+    // at engine row p round64(d1)), or a second stack behind td in NISQA / NISQA_DIM (input: td's fan_out)
+    const int nf = c.de_fuse == NISQA_DE_FUSE_XY_MINUS ? 3 : 2;
+    InRows fin = !c.double_ended ? InRows{d1, IN_PLAIN} : InRows{nf * d1, IN_DE_FUSED, d1, round64(d1)};
     if (c.double_ended && c.de_fuse_dim > 0) {        // Fusion.lin_fusion (lib:1399-1401)
-      const int D = c.de_fuse_dim;
-      const TensorView* w = P.get("fuse.lin_fusion.weight", {D, fdim});
+      const int D = c.de_fuse_dim, K = fin.dim, rows = in_rows(fin);
+      const TensorView* w = P.get("fuse.lin_fusion.weight", {D, K});
       const TensorView* b = P.get("fuse.lin_fusion.bias", {D});
       if (!w || !b) return false;
-      pack_linear_T(P, P.alloc(W.defuse.wT, (size_t)fdim * D), w, D, fdim);
+      const size_t o = P.alloc(W.defuse.wT, (size_t)rows * D);
+      for (int k = 0; k < rows; ++k) {
+        const int kc = in_col(fin, k);
+        if (kc >= 0) for (int j = 0; j < D; ++j) P.arena[o + (size_t)k * D + j] = w->d[(size_t)j * K + kc];
+      }
       P.copy(W.defuse.b, b->d, D);
-      fdim = D;
+      fin = {D, IN_PLAIN};
     }
-    if (!pack_sa_stack(P, W.sa[1], td2, {fdim, IN_PLAIN}, c.td2_layers, e->td2_d(), e->td2_f())) return false;
+    if (!pack_sa_stack(P, W.sa[1], td2, fin, c.td2_layers, e->td2_d(), e->td2_f())) return false;
     if (c.td2_pos_enc && !pack_pos_enc(P, c, td2, W.sa[1], e->td2_d())) return false;
-    if (!pack_de_align(P, c)) return false;
+    if (c.double_ended && !pack_de_align(P, c, d1)) return false;
     dp = e->td2_d();
     last_lstm = nullptr;
   } else if (e->td2_lstm()) {
@@ -1372,26 +1397,29 @@ const float* sa_stack(Pass& p, int k, Rows in, bool feeds_pool, float* x0) {
 }
 
 // NISQA_DE (lib:404-424): align the reference clip's rows to the degraded clip's and fuse them (+ Fusion.lin_fusion,
-// lib:1414-1415).  `out`: the rows that feed time_dependency_2.
-int de_fuse(Pass& p, const float* td_rows, Rows* out) {
+// lib:1414-1415).  td_rows: td's output, W real columns at a pitch of round64(W) with zero pad columns.  The fused rows
+// are [x, y_al, x - y_al] / [x + y_al, x - y_al] / [x, y_al] with part p at column p round64(W), pad columns zero.
+// `out`: the rows that feed time_dependency_2.
+int de_fuse(Pass& p, const float* td_rows, int W, Rows* out) {
   nisqa_engine* e = p.e;
   const nisqa_config& c = p.c;
   Lane& LN = p.LN;
-  const int n_seg = p.n_seg, nf = c.de_fuse == NISQA_DE_FUSE_XY_MINUS ? 3 : 2;
-  CK(LN.fused.reserve((size_t)n_seg * 64 * nf * 4));
-  CK(LN.td2in.reserve((size_t)n_seg * 64 * 4));
-  CK(cudaMemsetAsync(LN.fused.p, 0, (size_t)n_seg * 64 * nf * 4, p.st));      // rows of the reference clips stay zero
-  { Scope s(e, "de_align");
-    launch_de_align(p.st, td_rows, p.clips, p.n, p.qt64_prefix, p.n_qt64, c.de_align, c.de_align_apply == NISQA_DE_APPLY_SOFT,
-                    c.de_fuse, p.w.de, LN.fused.as<float>()); }
-  *out = {LN.fused.as<float>(), nf};
+  const int n_seg = p.n_seg, nf = c.de_fuse == NISQA_DE_FUSE_XY_MINUS ? 3 : 2, fd = nf * round64(W);
+  const size_t work = de_align_work_floats(W, c.de_align, n_seg);
+  CK(LN.fused.reserve((size_t)n_seg * fd * 4));
+  if (work) CK(LN.dework.reserve(work * 4));
+  CK(cudaMemsetAsync(LN.fused.p, 0, (size_t)n_seg * fd * 4, p.st));      // rows of the reference clips stay zero
+  { Scope s(e, "de_align", de_align_launches(c.de_align));
+    launch_de_align(p.st, td_rows, W, n_seg, p.clips, p.n, p.qt64_prefix, p.n_qt64, c.de_align,
+                    c.de_align_apply == NISQA_DE_APPLY_SOFT, c.de_fuse, p.w.de, LN.dework.as<float>(), LN.fused.as<float>()); }
+  *out = {LN.fused.as<float>(), fd / 64};
   e->last_de_fused = LN.fused.as<float>();      // (nothing behind the alignment writes fused: lin_fusion writes ffa, td_2 its own buffers)
-  e->last_de_fused_d = 64 * nf;
+  e->last_de_fused_d = fd;
   if (c.de_fuse_dim > 0) {
     Scope s(e, "de_align");
     CK(LN.ffa.reserve((size_t)n_seg * c.de_fuse_dim * 4));
-    launch_linear_tile(p.st, LN.fused.as<float>(), 64 * nf, p.w.defuse.wT, p.w.defuse.b, 0, LN.ffa.as<float>(), c.de_fuse_dim,
-                       n_seg, 64 * nf, c.de_fuse_dim);
+    launch_linear_tile(p.st, LN.fused.as<float>(), fd, p.w.defuse.wT, p.w.defuse.b, 0, LN.ffa.as<float>(), c.de_fuse_dim,
+                       n_seg, fd, c.de_fuse_dim);
     *out = {LN.ffa.as<float>(), c.de_fuse_dim / 64};
   }
   return 0;
@@ -1529,7 +1557,7 @@ int td_stages(Pass& p, Rows rows) {
   if (e->td2_runs() && !skip) { e->last_td1_out = cur.x; e->last_td1_out_d = D; e->last_td1_out_ld = 64 * cur.nk; }
   if (de) {
     Rows fused;
-    const int rc = de_fuse(p, cur.x, &fused);
+    const int rc = de_fuse(p, cur.x, D, &fused);
     if (rc) return rc;
     cur = {sa_stack(p, 1, fused, true, LN.td2in.as<float>()), e->td2_d() / 64};
     D = e->td2_d();
@@ -1792,11 +1820,13 @@ int nisqa_create(nisqa_engine** out, int device, const nisqa_config* cfg) {
                                               ": the self-attention kernels take d_model 64..256 and h 64..4096, multiples of 64");
     }
     if (cfg->double_ended && (e->sa_d() != 64 || e->td2_d() != 64))
-      return fail(e, NISQA_ERR_INVALID, "NISQA_DE: the alignment and fusion kernels are 64 wide (sa_d_model = td2_d_model = 64)");
+      return fail(e, NISQA_ERR_INVALID, "NISQA_DE: the engine runs its self-attention stacks at d_model 64 (sa_d_model = td2_d_model = 64)");
   }
   if (cfg->double_ended) {
-    if (cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF || cfg->cnn_kind == NISQA_CNN_STANDARD || cfg->n_out != 1)
-      return fail(e, NISQA_ERR_INVALID, "NISQA_DE: AdaptCNN + self-attention, one output");
+    // td: self-attention behind any framewise model, or an LSTM behind StandardCNN (arch 1); td_2: self-attention
+    if ((cfg->arch != NISQA_ARCH_ADAPT_SA_ATTFF && cfg->arch != NISQA_ARCH_STD_LSTM_LASTBI) || cfg->n_out != 1)
+      return fail(e, NISQA_ERR_INVALID, "NISQA_DE: a self-attention td behind any framewise model or an LSTM td behind "
+                                        "StandardCNN (arch 0 or 1), one output");
     if (cfg->de_align < NISQA_DE_ALIGN_DOT || cfg->de_align > NISQA_DE_ALIGN_BAHDANAU)
       return fail(e, NISQA_ERR_INVALID, "de_align: dot, cosine, distance, luong or bahd");
     if (cfg->de_align_apply != NISQA_DE_APPLY_HARD && cfg->de_align_apply != NISQA_DE_APPLY_SOFT)

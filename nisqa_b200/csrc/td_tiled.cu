@@ -578,15 +578,22 @@ td_sa_kernel(const float* __restrict__ x_in, const float* __restrict__ qkv, cons
 // ---------------------------------------------------------------------------------------------------------------
 // Double-ended model (NISQA_DE, reference lib:272-424): time alignment of the reference clip's features to the degraded
 // clip's (Alignment, lib:1228-1285) and feature fusion (Fusion, lib:1380-1417), for 64 degraded steps of one pair.
-//   x = time_dependency output of the degraded clip (clip 2p), y = of the reference clip (clip 2p + 1)
-//   score[i][j] : dot  x_i . y_j (AttDot, lib:1287-1296) | cosine similarity (AttCosine, lib:1298-1308, eps 1e-8) |
-//                 -mean_d |x_id - y_jd| (AttDistance with its default norms, lib:1310-1323) | x_i . (W y_j + b) (AttLuong,
-//                 lib:1344-1357) | v . tanh(Wq x_i + bq + Wy y_j + by) (AttBahdanau, att_dim 128, lib:1325-1342; its
-//                 output bias shifts every score of a row alike and drops out of softmax / argmax); keys j >= n_wins_y masked
+//   x = time_dependency output of the degraded clip (clip 2p), y = of the reference clip (clip 2p + 1): rows of W real
+//   columns (td's fan_out) at a pitch of ld = 64 NC (NC = 1..8), the pad columns zero - so they add nothing to a dot
+//   product, a distance or a norm
+//   score[i][j] : dot  x_i . y_j (AttDot, lib:1287-1296) | cosine similarity x_i . y_j rx_i ry_j, r = 1 / max(|row|, 1e-8)
+//                 (AttCosine, lib:1298-1308) | -(1/W) sum_d |x_id - y_jd| (AttDistance with its default norms,
+//                 lib:1310-1323) | x_i . yp_j, yp = W y + b (AttLuong, lib:1344-1357) | v . tanh(xq_i + yk_j), xq = Wq x + bq,
+//                 yk = Wy y + by (AttBahdanau, att_dim 128, lib:1325-1342; its output bias shifts every score of a row
+//                 alike and drops out of softmax / argmax); keys j >= n_wins_y masked.  The projections yp, xq | yk and
+//                 the reciprocal norms r come from launch_de_align's tile GEMM / row_rnorm_kernel over all rows of the pass.
 //   hard        : y_al[i] = y[argmax_j softmax(score[i])] = y[first maximal score] (ApplyHardAttention, lib:1359-1368)
 //   soft        : y_al[i] = softmax_j(score[i]) . y (ApplySoftAttention, lib:1370-1378), online max / sum over key blocks
-//   fuse        : [x, y_al, x - y_al] | [x + y_al, x - y_al] | [x, y_al]  ->  fused[row][64 * nf]
-// Same 64 x 64 register tiling as td_sa_kernel; the y block serves as K (row-major, pitch 68) and as V.
+//   fuse        : [x, y_al, x - y_al] | [x + y_al, x - y_al] | [x, y_al]  ->  fused[row][nf ld], part p at column p ld
+// Same 64 x 64 register tiling as td_sa_kernel.  The query operand (x, or xq for AttBahdanau) of the CTA's 64 steps stays
+// resident; per key block the n_sc score chunks of the keys (row-major, pitch 68) and - soft - the value chunks of y the
+// CTA outputs (k-major, pitch 64) stream through one TileStream.  A soft CTA outputs a group of at most G column chunks
+// (blockIdx.y: the group) and recomputes the scores for it, so at most 4 output chunks sit in registers.
 
 // s[i][j] -= sum_k |A[4ty+i][k] - B[tx+16j][k]|
 __device__ __forceinline__ void absdiff_nt(float (&s)[4][4], const float* __restrict__ A, const float* __restrict__ B, int ty, int tx) {
@@ -607,21 +614,60 @@ __device__ __forceinline__ void absdiff_nt(float (&s)[4][4], const float* __rest
   }
 }
 
-constexpr int kDeSmemFloats = 2 * kTileF + 2 * kTileF + 2 * kT;      // Qs | Ps | Yb[2] | 1 / |y| of the two blocks
-constexpr int kBhLd = 132;                                            // pitch of the [64][128] projections (AttBahdanau)
-constexpr int kDeLuongFloats = 4096 + kTileF;                          // W^T | projected keys
-constexpr int kDeBahdFloats = 64 * 128 + 2 * 64 * kBhLd;               // Wy^T | Wq x + bq | Wy y + by
+// s[i][j] += sum_k v[k] tanh(A[4ty+i][k] + B[tx+16j][k])
+__device__ __forceinline__ void tanh_nt(float (&s)[4][4], const float* __restrict__ A, const float* __restrict__ B,
+                                        const float* __restrict__ v, int ty, int tx) {
+  const float* a0 = A + (4 * ty) * kLd;
+  const float* b0 = B + tx * kLd;
+#pragma unroll 1
+  for (int k = 0; k < kT; k += 4) {
+    const float4 vv = __ldg(reinterpret_cast<const float4*>(v + k));
+    float4 a[4], b[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) a[i] = *reinterpret_cast<const float4*>(a0 + i * kLd + k);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) b[j] = *reinterpret_cast<const float4*>(b0 + (16 * j) * kLd + k);
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        float t = s[i][j];
+        t = fmaf(vv.x, tanhf(a[i].x + b[j].x), t); t = fmaf(vv.y, tanhf(a[i].y + b[j].y), t);
+        t = fmaf(vv.z, tanhf(a[i].z + b[j].z), t); t = fmaf(vv.w, tanhf(a[i].w + b[j].w), t);
+        s[i][j] = t;
+      }
+  }
+}
 
-__global__ void __launch_bounds__(kNT, 2)
-de_align_kernel(const float* __restrict__ x_td /*[n_seg][64]*/, const ClipDesc* __restrict__ clips, int n_clips,
-                const int* __restrict__ qtile_prefix /*64-row tiles*/, int align, int soft, int fuse, DeAlignParams A,
-                float* __restrict__ fused /*[n_seg][64 nf]*/) {
+// Fusion (lib:1402-1417) of four columns at `col` of one row; part p of the row starts at column p ld
+__device__ __forceinline__ void fuse_store(float* __restrict__ dst, int ld, int col, float4 xv, float4 yv, int fuse) {
+  const float4 df = make_float4(xv.x - yv.x, xv.y - yv.y, xv.z - yv.z, xv.w - yv.w);
+  if (fuse == NISQA_DE_FUSE_XY_MINUS) {
+    *reinterpret_cast<float4*>(dst + col) = xv; *reinterpret_cast<float4*>(dst + ld + col) = yv;
+    *reinterpret_cast<float4*>(dst + 2 * ld + col) = df;
+  } else if (fuse == NISQA_DE_FUSE_PLUS_MINUS) {
+    *reinterpret_cast<float4*>(dst + col) = make_float4(xv.x + yv.x, xv.y + yv.y, xv.z + yv.z, xv.w + yv.w);
+    *reinterpret_cast<float4*>(dst + ld + col) = df;
+  } else {
+    *reinterpret_cast<float4*>(dst + col) = xv; *reinterpret_cast<float4*>(dst + ld + col) = yv;
+  }
+}
+
+constexpr int kDeRing = 3;              // de_align_kernel ring slots
+// shared memory of de_align_kernel: Qs [n_sc][64][68] | Ps [64][68] | ring [kDeRing][64][68]; n_sc <= 8: 204 KB
+constexpr int de_smem_bytes(int n_sc) { return (n_sc + 1 + kDeRing) * kTileF * 4; }
+
+// G: output chunks per soft CTA (hard application runs G = 1 and writes every chunk of y[best])
+template <int G>
+__global__ void __launch_bounds__(kNT, G <= 2 ? 2 : 1)
+de_align_kernel(const float* __restrict__ x_td /*[n_seg][ld]*/, int ld, int W, const ClipDesc* __restrict__ clips, int n_clips,
+                const int* __restrict__ qtile_prefix /*64-row tiles*/, int align, int soft, int fuse,
+                const float* __restrict__ qsrc, const float* __restrict__ ksrc, int pld, int n_sc,
+                const float* __restrict__ rnorm, const float* __restrict__ v, float* __restrict__ fused /*[n_seg][nf ld]*/) {
   extern __shared__ __align__(16) float sm[];
-  float* Qs = sm;                          // [64][68] degraded rows x
-  float* Ps = sm + kTileF;                 // [64][68] softmax numerators (soft attention)
-  float* Yb = Ps + kTileF;                 // [2][64][68] reference rows y
-  float* Yn = Yb + 2 * kTileF;             // [2][64] 1 / max(|y_j|, eps)
-  float* Ex = Yn + 2 * kT;                 // AttLuong: W^T [64][64] | W y + b [64][68];  AttBahdanau: Wy^T [64][128] | XQ | YK [64][132]
+  float* Qs = sm;                          // [n_sc][64][68] query operand of the CTA's degraded steps
+  float* Ps = sm + n_sc * kTileF;          // [64][68] softmax numerators (soft attention)
+  float* ring = Ps + kTileF;
   const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
   const int c = upper_slot(qtile_prefix, n_clips, blockIdx.x);
   if (c & 1) return;                       // reference clips are keys only
@@ -630,207 +676,138 @@ de_align_kernel(const float* __restrict__ x_td /*[n_seg][64]*/, const ClipDesc* 
   if (Sx <= 0 || Sy <= 0) return;
   const int q0 = (blockIdx.x - __ldg(qtile_prefix + c)) * kT;
   const int rows_valid = min(kT, Sx - q0);
-  const long long row0 = (long long)cd.seg_off + q0;
-  const float* y_base = x_td + (long long)cr.seg_off * 64;
-  const int nf = fuse == NISQA_DE_FUSE_XY_MINUS ? 3 : 2;
-
-  tile_load_async(Qs, kLd, x_td + row0 * 64, 64, rows_valid, tid);
-  tile_load_async(Yb, kLd, y_base, 64, min(kT, Sy), tid);
-  cp_commit();
-  if (align == NISQA_DE_ALIGN_LUONG) tile_load_async(Ex, 64, A.wT, 64, 64, tid);
-  if (align == NISQA_DE_ALIGN_BAHDANAU) { tile_load_async(Ex, 128, A.wyT, 128, 64, tid); tile_load_async(Ex + 64, 128, A.wyT + 64, 128, 64, tid); }
-  cp_commit();
-  float o[4][4];
-  zero_acc(o);
-  if (align == NISQA_DE_ALIGN_BAHDANAU) {
-    // XQ = Wq x + bq for the CTA's 64 degraded steps: two 64-column halves, Wq^T staged through Ps
-    float* XQ = Ex + 64 * 128;
-    cp_wait<0>();
-    __syncthreads();
+  const long long row0 = (long long)cd.seg_off + q0, yrow0 = cr.seg_off;
+  const int NC = ld / 64, nf = fuse == NISQA_DE_FUSE_XY_MINUS ? 3 : 2;
+  const int c0 = blockIdx.y * G, ng = soft ? min(G, NC - c0) : 0;       // the CTA's output chunks c0 .. c0 + ng - 1
+  const int n_kb = (Sy + kT - 1) / kT, per_kb = n_sc + ng;
+  // the tile stream: per key block its n_sc score chunks, then (soft) its value chunks c0 .. c0 + ng - 1
+  auto src = [&](int t, float* dst) {
+    if (t >= n_kb * per_kb) return;
+    const int kb = t / per_kb, r = t - kb * per_kb;
+    const int nv = min(kT, Sy - kb * kT);
+    const long long j0 = yrow0 + (long long)kb * kT;
+    if (r < n_sc) tile_load_async(dst, kLd, ksrc + j0 * pld + 64 * r, pld, nv, tid);
+    else tile_load_async(dst, 64, x_td + j0 * ld + 64 * (c0 + r - n_sc), ld, nv, tid);
+  };
 #pragma unroll 1
-    for (int half = 0; half < 2; ++half) {
-      tile_load_async(Ps, 64, A.wqT + half * 64, 128, 64, tid);
-      cp_commit();
-      cp_wait<0>();
-      __syncthreads();
-      float acc[4][4];
-      const float4 bb = __ldg(reinterpret_cast<const float4*>(A.bq + half * 64) + tx);
+  for (int k = 0; k < n_sc; ++k) tile_load_async(Qs + k * kTileF, kLd, qsrc + row0 * pld + 64 * k, pld, rows_valid, tid);
+  TileStream<kDeRing, kTileF, decltype(src)> st(ring, src);      // (its first group carries the query operand)
+  const float wf = (float)W;
+  float o[G][4][4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) { acc[i][0] = bb.x; acc[i][1] = bb.y; acc[i][2] = bb.z; acc[i][3] = bb.w; }
-      gemm_nn(acc, Qs, Ps, 64, ty, tx);
+  for (int n = 0; n < G; ++n) zero_acc(o[n]);
+  float m[4], l[4];
+  int best[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) { m[i] = -INFINITY; l[i] = 0.f; best[i] = 0; }
+#pragma unroll 1
+  for (int kb = 0; kb < n_kb; ++kb) {
+    const int j0 = kb * kT, nkeys = Sy - j0;            // keys >= nkeys of this block do not exist
+    float s[4][4];
+    zero_acc(s);
+#pragma unroll 1
+    for (int k = 0; k < n_sc; ++k) {                    // s[i][j]: query 4ty+i, key j0 + tx + 16j
+      const float* K = st.acquire();
+      if (align == NISQA_DE_ALIGN_BAHDANAU) tanh_nt(s, Qs + k * kTileF, K, v + 64 * k, ty, tx);
+      else if (align == NISQA_DE_ALIGN_DISTANCE) absdiff_nt(s, Qs + k * kTileF, K, ty, tx);
+      else gemm_nt(s, Qs + k * kTileF, K, ty, tx);
+    }
+    if (align == NISQA_DE_ALIGN_DISTANCE) {
 #pragma unroll
       for (int i = 0; i < 4; ++i)
-        *reinterpret_cast<float4*>(XQ + (4 * ty + i) * kBhLd + half * 64 + 4 * tx) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
-      __syncthreads();
+#pragma unroll
+        for (int j = 0; j < 4; ++j) s[i][j] /= wf;
+    } else if (align == NISQA_DE_ALIGN_COSINE) {
+      float rq[4], ry[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) rq[i] = __ldg(rnorm + row0 + min(4 * ty + i, rows_valid - 1));
+#pragma unroll
+      for (int j = 0; j < 4; ++j) ry[j] = __ldg(rnorm + yrow0 + j0 + min(tx + 16 * j, nkeys - 1));
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) s[i][j] = s[i][j] * rq[i] * ry[j];
+    }
+    if (!soft) {
+      // first maximal score of the row: columns of a thread ascend with j and with the block; ties between threads
+      // are resolved towards the smaller key index
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        float bv = -INFINITY; int bi = 0x7fffffff;
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (tx + 16 * j < nkeys && s[i][j] > bv) { bv = s[i][j]; bi = j0 + tx + 16 * j; }
+#pragma unroll
+        for (int of = 8; of > 0; of >>= 1) {
+          const float ov = __shfl_xor_sync(0xffffffffu, bv, of);
+          const int oi = __shfl_xor_sync(0xffffffffu, bi, of);
+          if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+        }
+        if (bv > m[i]) { m[i] = bv; best[i] = bi; }       // (strictly greater: an earlier block keeps a tie)
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        float bm = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { if (tx + 16 * j >= nkeys) s[i][j] = -INFINITY; bm = fmaxf(bm, s[i][j]); }
+        bm = row_max(bm);
+        const float mn = fmaxf(m[i], bm);
+        const float sc = expf(m[i] - mn);
+        float ps = 0.f;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float p = expf(s[i][j] - mn);
+          ps += p;
+          Ps[(4 * ty + i) * kLd + tx + 16 * j] = p;
+        }
+        l[i] = l[i] * sc + row_sum(ps);
+        m[i] = mn;
+#pragma unroll
+        for (int n = 0; n < G; ++n) { o[n][i][0] *= sc; o[n][i][1] *= sc; o[n][i][2] *= sc; o[n][i][3] *= sc; }
+      }
+      __syncwarp();                                  // P rows 4ty..4ty+3 are written and read by this half-warp only
+#pragma unroll
+      for (int n = 0; n < G; ++n)
+        if (n < ng) gemm_nn(o[n], Ps, st.acquire(), 64, ty, tx);   // o[n][i][d] += sum_j p[i][j] y[j][64 (c0 + n) + d]
     }
   }
-  {
-    float m[4], l[4], rq[4];
-    int best[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { m[i] = -INFINITY; l[i] = 0.f; best[i] = 0; rq[i] = 1.f; }
-    const int n_kb = (Sy + kT - 1) / kT;
-#pragma unroll 1
-    for (int kb = 0; kb < n_kb; ++kb) {
-      const int j0 = kb * kT;
-      if (kb + 1 < n_kb) tile_load_async(Yb + ((kb + 1) & 1) * kTileF, kLd, y_base + (long long)(j0 + kT) * 64, 64, min(kT, Sy - (j0 + kT)), tid);
-      cp_commit();
-      cp_wait<1>();
-      __syncthreads();
-      const float* Y = Yb + (kb & 1) * kTileF;
-      if (align == NISQA_DE_ALIGN_COSINE) {
-        // nn.CosineSimilarity: x . y / (max(|x|, eps) max(|y|, eps)); four threads per key row, 16 features each
-        const int r = tid >> 2, qd = tid & 3;
-        float ss = 0.f;
-#pragma unroll
-        for (int k = 0; k < 16; k += 4) {
-          const float4 v = *reinterpret_cast<const float4*>(Y + r * kLd + qd * 16 + k);
-          ss = fmaf(v.x, v.x, ss); ss = fmaf(v.y, v.y, ss); ss = fmaf(v.z, v.z, ss); ss = fmaf(v.w, v.w, ss);
-        }
-        ss += __shfl_xor_sync(0xffffffffu, ss, 1);
-        ss += __shfl_xor_sync(0xffffffffu, ss, 2);
-        if (qd == 0) Yn[(kb & 1) * kT + r] = 1.0f / fmaxf(sqrtf(ss), 1e-8f);
-        if (kb == 0) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            float qs = 0.f;
-            const float4 v = *reinterpret_cast<const float4*>(Qs + (4 * ty + i) * kLd + 4 * tx);
-            qs = fmaf(v.x, v.x, qs); qs = fmaf(v.y, v.y, qs); qs = fmaf(v.z, v.z, qs); qs = fmaf(v.w, v.w, qs);
-            rq[i] = 1.0f / fmaxf(sqrtf(row_sum(qs)), 1e-8f);
-          }
-        }
-        __syncthreads();
-      }
-      float s[4][4];
-      zero_acc(s);
-      if (align == NISQA_DE_ALIGN_LUONG) {
-        // y' = W y + b for the block's keys, then x . y'
-        float* Yp = Ex + 4096;
-        float acc[4][4];
-        const float4 bb = __ldg(reinterpret_cast<const float4*>(A.b) + tx);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) { acc[i][0] = bb.x; acc[i][1] = bb.y; acc[i][2] = bb.z; acc[i][3] = bb.w; }
-        gemm_nn(acc, Y, Ex, 64, ty, tx);
-        store_rows_smem(Yp, acc, ty, tx);
-        __syncthreads();
-        gemm_nt(s, Qs, Yp, ty, tx);
-      } else if (align == NISQA_DE_ALIGN_BAHDANAU) {
-        const float* WyT = Ex;
-        const float* XQ = Ex + 64 * 128;
-        float* YK = Ex + 64 * 128 + 64 * kBhLd;
-#pragma unroll 1
-        for (int half = 0; half < 2; ++half) {                 // YK = Wy y + by for the block's keys
-          float acc[4][4];
-          const float4 bb = __ldg(reinterpret_cast<const float4*>(A.by + half * 64) + tx);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) { acc[i][0] = bb.x; acc[i][1] = bb.y; acc[i][2] = bb.z; acc[i][3] = bb.w; }
-          gemm_nn(acc, Y, WyT + half * 64, 128, ty, tx);
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            *reinterpret_cast<float4*>(YK + (4 * ty + i) * kBhLd + half * 64 + 4 * tx) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
-        }
-        __syncthreads();
-#pragma unroll 1
-        for (int a = 0; a < 128; a += 4) {
-          const float4 vv = __ldg(reinterpret_cast<const float4*>(A.v + a));
-          float4 xq[4], yk[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) xq[i] = *reinterpret_cast<const float4*>(XQ + (4 * ty + i) * kBhLd + a);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) yk[j] = *reinterpret_cast<const float4*>(YK + (tx + 16 * j) * kBhLd + a);
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              float t = s[i][j];
-              t = fmaf(vv.x, tanhf(xq[i].x + yk[j].x), t); t = fmaf(vv.y, tanhf(xq[i].y + yk[j].y), t);
-              t = fmaf(vv.z, tanhf(xq[i].z + yk[j].z), t); t = fmaf(vv.w, tanhf(xq[i].w + yk[j].w), t);
-              s[i][j] = t;
-            }
-        }
-      } else if (align == NISQA_DE_ALIGN_DISTANCE) {
-        absdiff_nt(s, Qs, Y, ty, tx);
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) s[i][j] *= (1.0f / 64.0f);
-      } else {
-        gemm_nt(s, Qs, Y, ty, tx);
-        if (align == NISQA_DE_ALIGN_COSINE) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float ry = Yn[(kb & 1) * kT + tx + 16 * j];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) s[i][j] = s[i][j] * rq[i] * ry;
-          }
-        }
-      }
-      const int nkeys = Sy - j0;
-      if (!soft) {
-        // first maximal score of the row: columns of a thread ascend with j and with the block; ties between threads
-        // are resolved towards the smaller key index
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          float bv = -INFINITY; int bi = 0x7fffffff;
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (tx + 16 * j < nkeys && s[i][j] > bv) { bv = s[i][j]; bi = j0 + tx + 16 * j; }
-#pragma unroll
-          for (int of = 8; of > 0; of >>= 1) {
-            const float ov = __shfl_xor_sync(0xffffffffu, bv, of);
-            const int oi = __shfl_xor_sync(0xffffffffu, bi, of);
-            if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-          }
-          if (bv > m[i]) { m[i] = bv; best[i] = bi; }       // (strictly greater: an earlier block keeps a tie)
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          float bm = -INFINITY;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) { if (tx + 16 * j >= nkeys) s[i][j] = -INFINITY; bm = fmaxf(bm, s[i][j]); }
-          bm = row_max(bm);
-          const float mn = fmaxf(m[i], bm);
-          const float sc = expf(m[i] - mn);
-          float ps = 0.f;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float p = expf(s[i][j] - mn);
-            ps += p;
-            Ps[(4 * ty + i) * kLd + tx + 16 * j] = p;
-          }
-          l[i] = l[i] * sc + row_sum(ps);
-          m[i] = mn;
-          o[i][0] *= sc; o[i][1] *= sc; o[i][2] *= sc; o[i][3] *= sc;
-        }
-        __syncwarp();
-        gemm_nn(o, Ps, Y, kLd, ty, tx);                      // o[i][d] += sum_j p[i][j] y[j][d]
-      }
-      __syncthreads();                                       // block kb consumed
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      if (!soft) {
-        const float4 v = __ldg(reinterpret_cast<const float4*>(y_base + (long long)best[i] * 64) + tx);
-        o[i][0] = v.x; o[i][1] = v.y; o[i][2] = v.z; o[i][3] = v.w;
-      } else {
-        const float inv = 1.0f / l[i];
-        o[i][0] *= inv; o[i][1] *= inv; o[i][2] *= inv; o[i][3] *= inv;
-      }
-    }
-  }
-  // ---- fusion (lib:1402-1417)
+  // ---- fusion (lib:1402-1417): x from the td rows, y_al from y[best] (hard) or the accumulators (soft)
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     if (4 * ty + i >= rows_valid) continue;
-    const float4 xv = *reinterpret_cast<const float4*>(Qs + (4 * ty + i) * kLd + 4 * tx);
-    const float4 yv = make_float4(o[i][0], o[i][1], o[i][2], o[i][3]);
-    const float4 df = make_float4(xv.x - yv.x, xv.y - yv.y, xv.z - yv.z, xv.w - yv.w);
-    float4* dst = reinterpret_cast<float4*>(fused + (row0 + 4 * ty + i) * (64 * nf)) + tx;
-    if (fuse == NISQA_DE_FUSE_XY_MINUS) { dst[0] = xv; dst[16] = yv; dst[32] = df; }
-    else if (fuse == NISQA_DE_FUSE_PLUS_MINUS) { dst[0] = make_float4(xv.x + yv.x, xv.y + yv.y, xv.z + yv.z, xv.w + yv.w); dst[16] = df; }
-    else { dst[0] = xv; dst[16] = yv; }
+    const float* xr = x_td + (row0 + 4 * ty + i) * ld;
+    float* dst = fused + (row0 + 4 * ty + i) * (long long)(nf * ld);
+    if (!soft) {
+      const float* yr = x_td + (yrow0 + best[i]) * ld;
+#pragma unroll 1
+      for (int n = 0; n < NC; ++n) {
+        const int col = 64 * n + 4 * tx;
+        fuse_store(dst, ld, col, __ldg(reinterpret_cast<const float4*>(xr + col)), __ldg(reinterpret_cast<const float4*>(yr + col)), fuse);
+      }
+    } else {
+      const float inv = 1.0f / l[i];
+#pragma unroll
+      for (int n = 0; n < G; ++n) {
+        if (n >= ng) continue;
+        const int col = 64 * (c0 + n) + 4 * tx;
+        fuse_store(dst, ld, col, __ldg(reinterpret_cast<const float4*>(xr + col)),
+                   make_float4(o[n][i][0] * inv, o[n][i][1] * inv, o[n][i][2] * inv, o[n][i][3] * inv), fuse);
+      }
+    }
   }
+  cp_wait<0>();                                    // (only empty groups can be pending here)
+}
+
+// 1 / max(|x_r|, 1e-8) over the W real columns of every row (AttCosine's norms), one warp per row
+__global__ void row_rnorm_kernel(const float* __restrict__ x, int ld, int W, int n_rows, float* __restrict__ out) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= n_rows) return;
+  float ss = 0.f;
+  for (int k = lane; k < W; k += 32) { const float v = __ldg(x + (size_t)row * ld + k); ss = fmaf(v, v, ss); }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+  if (lane == 0) out[row] = 1.0f / fmaxf(sqrtf(ss), 1e-8f);
 }
 
 // scores of a double-ended pass: row 2p = the pair's score (NaN when either clip was skipped), row 2p + 1 = NaN
@@ -934,13 +911,51 @@ void launch_td_in(cudaStream_t st, int nc, const float* feats, const float* WT, 
   }
 }
 
-void launch_de_align(cudaStream_t st, const float* x_td, const ClipDesc* clips, int n_clips, const int* qtile64_prefix,
-                     int n_qtiles, int align, int soft, int fuse, const DeAlignParams& A, float* fused) {
+template <int G>
+void de_align_instance(cudaStream_t st, dim3 grid, int smem, const float* x_td, int ld, int W, const ClipDesc* clips,
+                       int n_clips, const int* qtile64_prefix, int align, int soft, int fuse, const float* q, const float* k,
+                       int pld, int n_sc, const float* rnorm, const float* v, float* fused) {
   static unsigned long long cfg = 0;
   if (first_launch_on_device(cfg))
-    cudaFuncSetAttribute(de_align_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (kDeSmemFloats + kDeBahdFloats) * 4);
-  const int smem = (kDeSmemFloats + (align == NISQA_DE_ALIGN_LUONG ? kDeLuongFloats : align == NISQA_DE_ALIGN_BAHDANAU ? kDeBahdFloats : 0)) * 4;
-  de_align_kernel<<<n_qtiles, kNT, smem, st>>>(x_td, clips, n_clips, qtile64_prefix, align, soft, fuse, A, fused);
+    cudaFuncSetAttribute(de_align_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, de_smem_bytes(8));
+  de_align_kernel<G><<<grid, kNT, smem, st>>>(x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc,
+                                              rnorm, v, fused);
+}
+
+size_t de_align_work_floats(int W, int align, int n_rows) {
+  const int ld = (W + 63) / 64 * 64;
+  return (size_t)n_rows * (align == NISQA_DE_ALIGN_LUONG ? ld : align == NISQA_DE_ALIGN_BAHDANAU ? 256 : align == NISQA_DE_ALIGN_COSINE ? 1 : 0);
+}
+
+int de_align_launches(int align) {
+  return align == NISQA_DE_ALIGN_LUONG || align == NISQA_DE_ALIGN_BAHDANAU || align == NISQA_DE_ALIGN_COSINE ? 2 : 1;
+}
+
+void launch_de_align(cudaStream_t st, const float* x_td, int W, int n_rows, const ClipDesc* clips, int n_clips,
+                     const int* qtile64_prefix, int n_qtiles, int align, int soft, int fuse, const DeAlignParams& A,
+                     float* work, float* fused) {
+  const int NC = (W + 63) / 64, ld = 64 * NC;
+  const float *q = x_td, *k = x_td;
+  int pld = ld, n_sc = NC;
+  if (align == NISQA_DE_ALIGN_LUONG) {               // yp = W y + b for every row
+    launch_linear_tile(st, x_td, ld, A.wT, A.b, 0, work, ld, n_rows, ld, ld);
+    k = work;
+  } else if (align == NISQA_DE_ALIGN_BAHDANAU) {     // xq | yk = Wq x + bq | Wy y + by for every row
+    launch_linear_tile(st, x_td, ld, A.wqyT, A.bqy, 0, work, 256, n_rows, ld, 256);
+    q = work; k = work + 128; pld = 256; n_sc = 2;
+  } else if (align == NISQA_DE_ALIGN_COSINE) {
+    row_rnorm_kernel<<<(n_rows + 7) / 8, 256, 0, st>>>(x_td, ld, W, n_rows, work);
+  }
+  // output chunks per soft CTA: NC up to 4 in one group, 5..8 in two
+  const int G = !soft ? 1 : NC <= 4 ? NC : (NC + 1) / 2;
+  const dim3 grid(n_qtiles, soft ? (NC + G - 1) / G : 1);
+  const int smem = de_smem_bytes(n_sc);
+  switch (G) {
+    case 1: de_align_instance<1>(st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, work, A.v, fused); break;
+    case 2: de_align_instance<2>(st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, work, A.v, fused); break;
+    case 3: de_align_instance<3>(st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, work, A.v, fused); break;
+    default: de_align_instance<4>(st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, work, A.v, fused); break;
+  }
 }
 
 void launch_seg_feats(cudaStream_t st, const float* mel, int n_mels, int seg_len, int ld, const int* seg_frame0,

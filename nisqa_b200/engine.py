@@ -292,7 +292,7 @@ def config_from_args(args, max_chunk_segments=0):
         # AdaptCNN, or a framewise model without convolutions (lib:504-583), in front of the self-attention stack
         arch = ARCH_ADAPT_SA_ATTFF
         cnn_kind, cnn_fc, pools = _framewise(args)
-    elif (cnn, td) == ("standard", "self_att") and not de:
+    elif (cnn, td) == ("standard", "self_att"):
         # StandardCNN (lib:811-836) in front of the self-attention stack; fc_out's width comes from the weights
         arch = ARCH_ADAPT_SA_ATTFF
         cnn_kind, cnn_fc, pools = _framewise(args)
@@ -332,9 +332,10 @@ def config_from_args(args, max_chunk_segments=0):
             raise NotImplementedError("pool='last_step_bi' with %s_bidirectional=%r: PoolLastStepBi needs a bidirectional LSTM"
                                       % (key, args.get(key + "_bidirectional")))
     if de:
-        # double-ended model (reference lib:272-424, config/train_nisqa_double_ended.yaml): AdaptCNN + self-attention on
-        # both signals, alignment without learned weights, fusion without the optional Linear, td_2 = self-attention
-        if arch != ARCH_ADAPT_SA_ATTFF:
+        # double-ended model (reference lib:272-424, config/train_nisqa_double_ended.yaml): any framewise model + a
+        # self-attention td, or StandardCNN + an LSTM td, on both signals; alignment and fusion at td's fan_out; td_2 =
+        # self-attention
+        if arch not in (ARCH_ADAPT_SA_ATTFF, ARCH_STD_LSTM_LASTBI):
             raise NotImplementedError("NISQA_DE is implemented for cnn_model='adapt', td='self_att'")
         if args.get("de_align") not in DE_ALIGN:
             raise NotImplementedError("de_align=%r is not implemented by the engine (dot, cosine, distance, luong, bahd)" % (args.get("de_align"),))
