@@ -8,10 +8,6 @@
 #include "common.cuh"
 #include "f32x2.cuh"
 
-#ifndef NISQA_C1_PK
-#define NISQA_C1_PK 1        // conv1 FMAs over channel pairs (f32x2.cuh; bit-identical to the scalar form)
-#endif
-
 namespace nisqa {
 
 // ws: [9][16] folded conv1 weights followed by the 16 biases (shared memory).  LDG: `mel` is global memory read through
@@ -36,8 +32,7 @@ __device__ __forceinline__ void conv1_cell(const float* __restrict__ mel, int f0
       patch[i][j] = v;
     }
 
-#if NISQA_C1_PK
-  // 16 channels as 8 pairs (the same fp32 FMA per element and tap order as the scalar form)
+  // 16 channels as 8 pairs (f32x2.cuh: the same fp32 FMA per element and tap order as one fmaf per channel)
 #pragma unroll
   for (int cq_ = 0; cq_ < NCQ; ++cq_) {
     const int cq = cq0 + cq_;
@@ -78,47 +73,6 @@ __device__ __forceinline__ void conv1_cell(const float* __restrict__ mel, int f0
     }
   }
 }
-#else
-#pragma unroll
-  for (int cq_ = 0; cq_ < NCQ; ++cq_) {
-    const int cq = cq0 + cq_;
-    float acc[2][NWC][4];
-#pragma unroll
-    for (int i = 0; i < 2; ++i)
-#pragma unroll
-      for (int j = 0; j < NWC; ++j)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) acc[i][j][c] = 0.f;
-#pragma unroll
-    for (int tap = 0; tap < 9; ++tap) {
-      const float4 w = *reinterpret_cast<const float4*>(ws + tap * 16 + cq * 4);
-      const int ky = tap / 3, kx = tap % 3;
-#pragma unroll
-      for (int i = 0; i < 2; ++i)
-#pragma unroll
-        for (int j = 0; j < NWC; ++j) {
-          const float a = patch[i + ky][j + kx];
-          acc[i][j][0] = fmaf(a, w.x, acc[i][j][0]);
-          acc[i][j][1] = fmaf(a, w.y, acc[i][j][1]);
-          acc[i][j][2] = fmaf(a, w.z, acc[i][j][2]);
-          acc[i][j][3] = fmaf(a, w.w, acc[i][j][3]);
-        }
-    }
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      float m = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < 2; ++i)
-#pragma unroll
-        for (int j = 0; j < NWC; ++j) {
-          const int col = c0 + 1 + j;            // conv output column of this window slot
-          if (MODE == 0 || (col >= 0 && col < kSegLen)) m = fmaxf(m, acc[i][j][c]);
-        }
-      res[cq_ * 4 + c] = fmaxf(m + ws[144 + cq * 4 + c], 0.f);   // bias + ReLU commute with max
-    }
-  }
-}
-#endif
 
 // AdaptCNN conv1 + BN + ReLU + adaptive_max_pool2d to PH x PW (cnn_pool_1, shipped 24 x 7) for one pooled cell (ph, pw),
 // channels c0 .. c0 + 15 of C1, of a segment of H mel rows x W frames (seg: its frame 0, rows H floats apart; ws: [9][C1]

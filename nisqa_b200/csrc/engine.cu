@@ -93,10 +93,7 @@ struct Ticket {          // one asynchronous nisqa_submit_pcm call
 // submissions run on different streams: wave tails and the small low-occupancy kernels of one
 // pass are filled with CTAs of another (+8..12 % throughput measured, tools/two_engines.py), and
 // the upload of the next pass (copy stream) overlaps compute.
-#ifndef NISQA_LANES
-#define NISQA_LANES 3
-#endif
-constexpr int kLanes = NISQA_LANES;
+constexpr int kLanes = 3;
 constexpr int kStages = 6;     // staging slots / submissions in flight (uploads run ahead of the lanes)
 struct Lane {
   cudaStream_t stream = nullptr;
@@ -271,7 +268,7 @@ struct nisqa_engine {
   // front-end tables
   std::vector<FbEntry*> fbs;
   DevBuf fb_table;       // FbTables[]
-  DevBuf tw4096;         // float2[6144] (twiddle tables of the front-end)
+  DevBuf tw4096;         // float2[4096] (twiddle tables of the front-end)
 
   // per-pass state lives in the lanes; `stream` aliases lane 0's stream (nisqa_stream)
   Lane lanes[kLanes];
@@ -1856,7 +1853,7 @@ int nisqa_create(nisqa_engine** out, int device, const nisqa_config* cfg) {
   e->cur_stream = e->stream;
   // twiddles laid out per lane so that every warp load is coalesced:
   //   tw1[r-1][j][lane] = W_4096^(r*(lane+32j)),  tw2[q][lane] = W_1024^(lane*q)
-  std::vector<float2> tw(6 * 1024);     // tw1 [3][32][32], tw2 [32][32], then tw2 again as (x, y, -y, x) float4 [32][32]
+  std::vector<float2> tw(4 * 1024);     // tw1 [3][32][32], tw2 [32][32]
   auto w4096 = [](long k) {
     const double a = -2.0 * M_PI * (double)(k & 4095) / 4096.0;
     return make_float2((float)cos(a), (float)sin(a));
@@ -1865,12 +1862,7 @@ int nisqa_create(nisqa_engine** out, int device, const nisqa_config* cfg) {
     for (int j = 0; j < 32; ++j)
       for (int l = 0; l < 32; ++l) tw[((r - 1) * 32 + j) * 32 + l] = w4096((long)r * (l + 32 * j));
   for (int q = 0; q < 32; ++q)
-    for (int l = 0; l < 32; ++l) {
-      const float2 t = w4096(4L * l * q);
-      tw[3 * 1024 + q * 32 + l] = t;
-      tw[4 * 1024 + 2 * (q * 32 + l)] = t;
-      tw[4 * 1024 + 2 * (q * 32 + l) + 1] = make_float2(-t.y, t.x);
-    }
+    for (int l = 0; l < 32; ++l) tw[3 * 1024 + q * 32 + l] = w4096(4L * l * q);
   CK(e->tw4096.reserve(tw.size() * sizeof(float2)));
   CK(cudaMemcpy(e->tw4096.p, tw.data(), tw.size() * sizeof(float2), cudaMemcpyHostToDevice));
   return 0;

@@ -15,20 +15,6 @@
 #include "f32x2.cuh"
 #include "launch.cuh"
 
-// experiment switches (-DNAME=value when building a variant library); the defaults are the variants the kernel is tuned with
-#ifndef NISQA_FE_PK_FFT
-#define NISQA_FE_PK_FFT 0      // butterflies / twiddle products as packed FADD2 / FMUL2 / FFMA2
-#endif
-#ifndef NISQA_FE_PK_MAG
-#define NISQA_FE_PK_MAG 0      // magnitude stage with packed adds
-#endif
-#ifndef NISQA_FE_DIT
-#define NISQA_FE_DIT 1         // 32-point transforms as decimation in time with fused twiddle butterflies (6 FMAs instead of 8 FP instructions)
-#endif
-#ifndef NISQA_FE_MEL
-#define NISQA_FE_MEL 2         // 0: scalar band loop unrolled by 4, 1: rolled packed loop, 2: packed loop unrolled by 4
-#endif
-
 namespace nisqa {
 
 // e^{-2 pi i k / 32}, k = 0..15
@@ -61,45 +47,10 @@ __device__ __forceinline__ float2 cmul(float2 a, float2 b) {
   return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x);
 }
 
-// In-register 32-point forward DFT, decimation in frequency: X[rev5(i)] ends up in x[i].  Complex values are packed
-// (re, im) register pairs (f32x2.cuh): a butterfly's sum / difference is one FADD2 each, a twiddle product FMUL2 + FFMA2;
-// the -i products are formed from the scalar halves (two FADDs, no multiply).
-__device__ __forceinline__ void fft32(f2 (&x)[32]) {
-#pragma unroll
-  for (int half = 16; half >= 1; half >>= 1) {
-#pragma unroll
-    for (int base = 0; base < 32; base += 2 * half) {
-#pragma unroll
-      for (int j = 0; j < half; ++j) {
-        const int k = j * (16 / half);
-#if NISQA_FE_PK_FFT
-        const f2 a = x[base + j], b = x[base + j + half];
-        x[base + j] = add2(a, b);
-        if (k == 0) {
-          x[base + j + half] = sub2(a, b);
-        } else if (k == 8) {                       // (a - b) * (-i) = (d.y, -d.x)
-          const float2 af = upk(a), bf = upk(b);
-          x[base + j + half] = pk(af.y - bf.y, bf.x - af.x);
-        } else {
-          const float2 w = w32(k);
-          x[base + j + half] = cmul2(sub2(a, b), pk(w.x, w.y), pk(-w.y, w.x));
-        }
-#else
-        const float2 a = upk(x[base + j]), b = upk(x[base + j + half]);
-        x[base + j] = pk(a.x + b.x, a.y + b.y);
-        const float2 d = make_float2(a.x - b.x, a.y - b.y);
-        if (k == 0) x[base + j + half] = pk(d);
-        else if (k == 8) x[base + j + half] = pk(d.y, -d.x);
-        else x[base + j + half] = pk(cmul(d, w32(k)));
-#endif
-      }
-    }
-  }
-}
-
-// The same transform as decimation in TIME: input n sits at x[rev5(n)], X[k] ends up in x[k].  A butterfly with a
-// non-trivial twiddle is out1 = a + w b (4 FMAs), out2 = 2 a - out1 (2 FMAs) instead of add, subtract and a 4-instruction
-// complex product; 34 of the 80 butterflies of a 32-point transform have one.
+// In-register 32-point forward DFT, decimation in time, over (re, im) register pairs (f32x2.cuh): input n sits at
+// x[rev5(n)], X[k] ends up in x[k].  A butterfly with a non-trivial twiddle is out1 = a + w b (4 FMAs), out2 = 2 a - out1
+// (2 FMAs) instead of add, subtract and a 4-instruction complex product; 34 of the 80 butterflies of a 32-point transform
+// have one.
 // One stage per template instance: every loop has a compile-time trip count, so the array indices are constants and
 // `x` stays in registers (a stage loop over `half` is not fully unrolled by the sm_90 compiler, which puts x in local memory).
 template <int HALF>
@@ -127,23 +78,12 @@ __device__ __forceinline__ void fft32_dit_stage(f2 (&x)[32]) {
       }
     }
 }
-__device__ __forceinline__ void fft32_dit(f2 (&x)[32]) {
+__device__ __forceinline__ void fft32(f2 (&x)[32]) {
   fft32_dit_stage<1>(x);
   fft32_dit_stage<2>(x);
   fft32_dit_stage<4>(x);
   fft32_dit_stage<8>(x);
   fft32_dit_stage<16>(x);
-}
-
-// slot of input / output index i in the register array handed to the 32-point transform
-__host__ __device__ constexpr int fe_in(int i) { return NISQA_FE_DIT ? rev5(i) : i; }
-__host__ __device__ constexpr int fe_out(int i) { return NISQA_FE_DIT ? i : rev5(i); }
-__device__ __forceinline__ void fe_fft32(f2 (&x)[32]) {
-#if NISQA_FE_DIT
-  fft32_dit(x);
-#else
-  fft32(x);
-#endif
 }
 
 __device__ __forceinline__ int reflect_index(int i, int n) {
@@ -194,34 +134,28 @@ int frontend_smem_bytes(int Q) { return fe_region0_bytes(Q) + 4 * kScratchPerWar
 
 // ---- shared pieces of the two front-end kernels ---------------------------------------------
 // 1024-point FFT of one residue plane: x[j] = input n = lane + 32 j (already twiddled by
-// W_4096^(r n)); result Z_r[m] is left in tile[m] (m = 0..1023).  tw2x[q][lane] = (t.x, t.y, -t.y, t.x), t = W_1024^(lane q):
-// both operand forms of the packed complex product in one 16-byte load.
+// W_4096^(r n)); result Z_r[m] is left in tile[m] (m = 0..1023).  tw2_end points one past the float2 table
+// tw2[32][32], tw2[q][lane] = W_1024^(lane q).  It is passed as a float4 pointer: with a float2 pointer to the table's
+// start the pipelined kernel's registers are allocated differently and bench.py measured 0.7 % fewer clips/s
+// (H100 80GB HBM3, 700 W).
 __device__ __forceinline__ void fft1024_plane(f2 (&x)[32], float2* tile_, int lane,
-                                              const float4* __restrict__ tw2x) {
-  // x[fe_in(j)] = input n = lane + 32 j on entry
+                                              const float4* __restrict__ tw2_end) {
+  // x[rev5(j)] = input n = lane + 32 j on entry
   f2* tile = reinterpret_cast<f2*>(tile_);
-  fe_fft32(x);                                   // A_l[q] at x[fe_out(q)]
+  fft32(x);                                      // A_l[q] at x[q]
 #pragma unroll
   for (int q = 0; q < 32; ++q) {
-    f2 v = x[fe_out(q)];
-    if (q != 0) {
-#if NISQA_FE_PK_FFT
-      const float4 t = __ldg(tw2x + q * 32 + lane);                        // W_1024^(l q), coalesced
-      v = cmul2(v, pk(t.x, t.y), pk(t.z, t.w));
-#else
-      const float2 t = __ldg(reinterpret_cast<const float2*>(tw2x) - 1024 + q * 32 + lane);   // the float2 table sits in front
-      v = pk(cmul(upk(v), t));
-#endif
-    }
+    f2 v = x[q];
+    if (q != 0) v = pk(cmul(upk(v), __ldg(reinterpret_cast<const float2*>(tw2_end) - 1024 + q * 32 + lane)));      // coalesced
     tile[lane * 33 + q] = v;
   }
   __syncwarp();
 #pragma unroll
-  for (int l = 0; l < 32; ++l) x[fe_in(l)] = tile[l * 33 + lane];
+  for (int l = 0; l < 32; ++l) x[rev5(l)] = tile[l * 33 + lane];
   __syncwarp();
-  fe_fft32(x);                                   // Z_r[lane + 32 p] at x[fe_out(p)]
+  fft32(x);                                      // Z_r[lane + 32 p] at x[p]
 #pragma unroll
-  for (int p = 0; p < 32; ++p) tile[lane + 32 * p] = x[fe_out(p)];
+  for (int p = 0; p < 32; ++p) tile[lane + 32 * p] = x[p];
 }
 
 // Fused unpack of the two real spectra, |.|, sparse mel, dB for the MELS / 4 bands of this warp
@@ -291,7 +225,7 @@ __device__ __forceinline__ float mel_bands(const float2* scratch, const int* ban
   return out;
 }
 
-// ---- two-stage variant used by the pipelined kernel (round 2) ---------------------------------------------------
+// ---- two-stage variant used by the pipelined kernel ------------------------------------------------------------
 // Stage A (whole CTA): |X_a[k]|, |X_b[k]| of the two packed real frames for the bins that carry a filterbank weight
 // (k < n_mag), each formed ONCE and written over Z[k] in its plane (Z[k] is read by the owner of bin k and, as a mirror,
 // by the owner of bin 4096 - k >= 2048 > n_mag - 1 only: in place is race free; k = 2048 mirrors itself).
@@ -302,38 +236,32 @@ __device__ __forceinline__ void mag_stage(float2* scratch, int n_mag, int tid) {
   const f2* pn = reinterpret_cast<const f2*>(scratch + (kk0 & 3) * kScratchPerWarp + (kk0 >> 2));
   for (int k = tid; k < n_mag; k += kFeThreads) {
     const f2 zk = *pk_, zn = *pn;
+    const float2 k_ = upk(zk), n_ = upk(zn);
+    const float ar = k_.x + n_.x, ai = k_.y - n_.y;        // 2 * X_a[k]
+    const float br = k_.y + n_.y, bi = k_.x - n_.x;        // 2 * X_b[k] (up to a unit factor)
     float ma, mb;
-#if NISQA_FE_PK_MAG
-    const f2 sm = add2(zk, zn);                            // (2 Re X_a[k], 2 Re X_b[k])
-    const float2 df = upk(sub2(zk, zn));                   // (-+2 Im X_b[k], 2 Im X_a[k])
-    const float2 pw = upk(mul2(sm, sm));
-    asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(ma) : "f"(fmaf(df.y, df.y, pw.x)));
-    asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(mb) : "f"(fmaf(df.x, df.x, pw.y)));
-#else
-    {
-      const float2 k_ = upk(zk), n_ = upk(zn);
-      const float ar = k_.x + n_.x, ai = k_.y - n_.y;      // 2 * X_a[k]
-      const float br = k_.y + n_.y, bi = k_.x - n_.x;      // 2 * X_b[k] (up to a unit factor)
-      asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(ma) : "f"(fmaf(ar, ar, ai * ai)));
-      asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(mb) : "f"(fmaf(br, br, bi * bi)));
-    }
-#endif
+    asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(ma) : "f"(fmaf(ar, ar, ai * ai)));
+    asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(mb) : "f"(fmaf(br, br, bi * bi)));
     *pk_ = pk(ma, mb);
     pk_ += 32; pn -= 32;                                    // (tid = 0, it = 0: k = kk = 0 reads the same slot twice)
     if (k == 0) pn += 1024;                                 // 4096 - 0 wraps to bin 0; from k = 128 on the mirror is 3968 - ...
   }
 }
 
-// Stage B: the MELS / 4 bands of this warp as weighted sums of the staged magnitudes, then the same multi-value butterfly
-// reduction and dB as mel_bands, in rounds of up to 16 slots.  `pscale` = 2^-30 for PCM16 input fed as raw integers
-// (|X| scales by 2^15 exactly).
+// Stage B: the MELS / 4 bands of this warp (b = warp + 4 slot) as weighted sums of the staged magnitudes, then dB.
+// Lanes stride over a band's bins and keep one packed (frame A, frame B) partial sum per slot; the partials of up to 16
+// slots (one round) are reduced across the warp with ONE multi-value butterfly (31 shuffles instead of 32 x 5), so lane L
+// ends up with the total of (slot L >> 1, frame L & 1) and one log10f serves the whole warp.  More than 64 bands
+// (80 / 96 / 128) take a second round over slots 16 .. 31.  `pscale` = 2^-30 for PCM16 input fed as raw integers (|X|
+// scales by 2^15 exactly), 1 for float input.  Returns this lane's dB value (or -inf) for the clip maximum.
 template <int MELS, int S0>
 __device__ __forceinline__ float mel_bands_staged_round(const float2* scratch, const int* band_meta,
                                                         const float* __restrict__ weights, int warp, int lane,
                                                         bool validB, float pscale, float* __restrict__ mel_row0) {
   constexpr int NS = (MELS / 4 - S0) < 16 ? (MELS / 4 - S0) : 16;     // slots of this round
-  // v[i]: packed (frame A, frame B) partial sums of slot i in this lane.  The band loop is kept rolled: one weight load,
-  // one magnitude pair, one FFMA2 per 32 bins and lane; trip counts (0 .. ~10 rows per band) are warp uniform.
+  // v[i]: packed (frame A, frame B) partial sums of slot i in this lane: one weight load, one magnitude pair, one FFMA2
+  // per 32 bins and lane.  Band rows are zero-padded to a multiple of 32 weights (engine build_fb): trip counts (0 .. ~10
+  // rows per band) are warp uniform and every lane loads unconditionally (the padded bins stay inside the planes).
   f2 v[16];
 #pragma unroll
   for (int i = 0; i < 16; ++i) v[i] = 0ull;
@@ -345,27 +273,10 @@ __device__ __forceinline__ float mel_bands_staged_round(const float2* scratch, c
     const f2* pm = reinterpret_cast<const f2*>(scratch + (k & 3) * kScratchPerWarp + (k >> 2));
     const float* wt = weights + beg + lane;
     // padded bins (weight 0) may hold raw spectrum values: finite, times 0
-#if NISQA_FE_MEL == 0
-    float s0 = 0.f, s1 = 0.f;
-#pragma unroll 4
-    for (int it = (end - beg) >> 5; it > 0; --it, wt += 32, pm += 8) {
-      const float w = __ldg(wt);
-      const float2 m = upk(*pm);
-      s0 = fmaf(w, m.x, s0);
-      s1 = fmaf(w, m.y, s1);
-    }
-    v[slot] = pk(s0, s1);
-#elif NISQA_FE_MEL == 1
-    f2 acc = 0ull;
-#pragma unroll 1
-    for (int it = (end - beg) >> 5; it > 0; --it, wt += 32, pm += 8) acc = fma2(bc(__ldg(wt)), *pm, acc);
-    v[slot] = acc;
-#else
     f2 acc = 0ull;
 #pragma unroll 4
     for (int it = (end - beg) >> 5; it > 0; --it, wt += 32, pm += 8) acc = fma2(bc(__ldg(wt)), *pm, acc);
     v[slot] = acc;
-#endif
   }
   // multi-value butterfly over the NS (padded to 16) packed values: after the steps with lane offsets 16, 8, 4, 2 lane L
   // holds the value of slot (L >> 1) & ... summed over 16 lanes; the last step adds the partner lane (L ^ 1)
@@ -412,7 +323,7 @@ __global__ void __launch_bounds__(kFeThreads, 5)
 frontend_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips, int n_clips,
                 const FbTables* __restrict__ fbs,
                 const float2* __restrict__ tw1 /*[3][32][32]: W4096^(r*(lane+32j))*/,
-                const float4* __restrict__ tw2 /*[32][32]: W1024^(lane*q) as (x, y, -y, x)*/, float* __restrict__ mel,
+                const float4* __restrict__ tw2_end /*end of [32][32]: W1024^(lane*q)*/, float* __restrict__ mel,
                 unsigned* __restrict__ clipmax, int Q) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float2* zin = reinterpret_cast<float2*>(smem_raw);                     // [1024*Q] packed input
@@ -471,9 +382,9 @@ frontend_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips, i
         }
       }
       if (r != 0) v = cmul(v, __ldg(tw1 + ((r - 1) * 32 + j) * 32 + lane));   // coalesced per-lane table
-      x[fe_in(j)] = pk(v);
+      x[rev5(j)] = pk(v);
     }
-    fft1024_plane(x, scratch + r * kScratchPerWarp, lane, tw2);
+    fft1024_plane(x, scratch + r * kScratchPerWarp, lane, tw2_end);
   }
   __syncthreads();
 
@@ -497,12 +408,10 @@ constexpr int kSpanMax = 1536;                    // hop + win limit of this ker
 template <typename T> __host__ __device__ constexpr int pp_slot_bytes() {
   return ((kSpanMax + 16 / (int)sizeof(T)) * (int)sizeof(T) + 15) / 16 * 16;
 }
-#ifndef NISQA_FE_CTAS
-#define NISQA_FE_CTAS 6        // PCM16 input: resident CTAs per SM the kernel is built for (6 = one sample slot, <= 80 registers)
-#endif
-// PCM16 with six CTAs per SM: ONE sample slot (the slot is only live during the input stage: the next pair's copy is issued
-// behind the barrier that follows the FFT, still a whole mel stage ahead of its use) - 37.4 KB of shared memory per CTA
-template <typename T> __host__ __device__ constexpr int pp_slots() { return (sizeof(T) == 2 && NISQA_FE_CTAS >= 6) ? 1 : 2; }
+// PCM16 with six CTAs per SM (<= 80 registers): ONE sample slot (the slot is only live during the input stage: the next
+// pair's copy is issued behind the barrier that follows the FFT, still a whole mel stage ahead of its use) - 37.4 KB of
+// shared memory per CTA
+template <typename T> __host__ __device__ constexpr int pp_slots() { return sizeof(T) == 2 ? 1 : 2; }
 template <typename T> constexpr int pp_smem_bytes() { return pp_slots<T>() * pp_slot_bytes<T>() + 4 * kScratchPerWarp * 8; }
 
 template <typename T>
@@ -523,10 +432,10 @@ __device__ __forceinline__ void pp_issue_pair(const T* __restrict__ y, int a, in
 }
 
 template <typename T, int MELS>
-__global__ void __launch_bounds__(kFeThreads, (sizeof(T) == 2 && NISQA_FE_CTAS >= 6) ? 6 : 5)
+__global__ void __launch_bounds__(kFeThreads, sizeof(T) == 2 ? 6 : 5)
 frontend_pp_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips,
-                   const FbTables* __restrict__ fbs, const float2* __restrict__ tw1,
-                   const float4* __restrict__ tw2, float* __restrict__ mel, unsigned* __restrict__ clipmax,
+                   const FbTables* __restrict__ fbs, const float4* __restrict__ tw2_end,
+                   float* __restrict__ mel, unsigned* __restrict__ clipmax,
                    int ppc /*frame pairs per CTA*/) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   constexpr int NSLOT = pp_slots<T>();
@@ -585,9 +494,9 @@ frontend_pp_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips
       }
 #pragma unroll
       for (int u = 0; u < CH; ++u)
-        x[fe_in(j0 + u)] = pk(fmaf(sa[u], wt[u].x, -(sb[u] * wt[u].y)), fmaf(sa[u], wt[u].y, sb[u] * wt[u].x));
+        x[rev5(j0 + u)] = pk(fmaf(sa[u], wt[u].x, -(sb[u] * wt[u].y)), fmaf(sa[u], wt[u].y, sb[u] * wt[u].x));
     }
-    fft1024_plane(x, scratch + r * kScratchPerWarp, lane, tw2);
+    fft1024_plane(x, scratch + r * kScratchPerWarp, lane, tw2_end);
     __syncthreads();                    // all four planes written (and every warp is past the input stage: the slot is free)
     if (NSLOT == 1 && p + 1 < p1)
       pp_issue_pair<T>(y, a + 2 * cd.hop, span, cd.n_samples, reinterpret_cast<T*>(smem_raw), tid);
@@ -638,7 +547,7 @@ static void launch_frontend_mels(cudaStream_t st, const void* pcm, int fmt_f32, 
                                  int n_clips, int max_pairs, const FbTables* fbs,
                                  const float2* tw, float* mel, unsigned* clipmax, int Q, int max_span, int ppc) {
   const float2* tw1 = tw;               // [3][32][32]
-  const float4* tw2 = reinterpret_cast<const float4*>(tw + 4 * 1024);    // [32][32] (x, y, -y, x)
+  const float4* tw2_end = reinterpret_cast<const float4*>(tw + 4 * 1024);    // end of tw2 [32][32]
   if (Q == 1 && max_span <= kSpanMax) { // the pipelined multi-pair kernel
     static unsigned long long configured = 0;
     if (first_launch_on_device(configured)) {
@@ -648,9 +557,9 @@ static void launch_frontend_mels(cudaStream_t st, const void* pcm, int fmt_f32, 
     if (ppc < 1) ppc = kPairsPerCta;
     const dim3 grid((max_pairs + ppc - 1) / ppc, n_clips);
     if (fmt_f32)
-      frontend_pp_kernel<float, MELS><<<grid, kFeThreads, pp_smem_bytes<float>(), st>>>((const float*)pcm, clips, fbs, tw1, tw2, mel, clipmax, ppc);
+      frontend_pp_kernel<float, MELS><<<grid, kFeThreads, pp_smem_bytes<float>(), st>>>((const float*)pcm, clips, fbs, tw2_end, mel, clipmax, ppc);
     else
-      frontend_pp_kernel<short, MELS><<<grid, kFeThreads, pp_smem_bytes<short>(), st>>>((const short*)pcm, clips, fbs, tw1, tw2, mel, clipmax, ppc);
+      frontend_pp_kernel<short, MELS><<<grid, kFeThreads, pp_smem_bytes<short>(), st>>>((const short*)pcm, clips, fbs, tw2_end, mel, clipmax, ppc);
     return;
   }
   const int smem = frontend_smem_bytes(Q);
@@ -664,10 +573,10 @@ static void launch_frontend_mels(cudaStream_t st, const void* pcm, int fmt_f32, 
   const dim3 grid(max_pairs, n_clips);
   if (fmt_f32) {
     frontend_kernel<float, MELS><<<grid, kFeThreads, smem, st>>>(
-        (const float*)pcm, clips, n_clips, fbs, tw1, tw2, mel, clipmax, Q);
+        (const float*)pcm, clips, n_clips, fbs, tw1, tw2_end, mel, clipmax, Q);
   } else {
     frontend_kernel<short, MELS><<<grid, kFeThreads, smem, st>>>(
-        (const short*)pcm, clips, n_clips, fbs, tw1, tw2, mel, clipmax, Q);
+        (const short*)pcm, clips, n_clips, fbs, tw1, tw2_end, mel, clipmax, Q);
   }
 }
 
@@ -682,10 +591,10 @@ void launch_frontend(cudaStream_t st, int n_mels, const void* pcm, int fmt_f32, 
                      int n_clips, int max_pairs, const FbTables* fbs,
                      const float2* tw, float* mel, unsigned* clipmax, int Q, int max_span, int ppc) {
   switch (n_mels) {       // (nisqa_create accepts these only: frontend_supports_mels)
-#define NISQA_FE_CASE(M) \
+#define FE_MELS_CASE(M) \
     case M: launch_frontend_mels<M>(st, pcm, fmt_f32, clips, n_clips, max_pairs, fbs, tw, mel, clipmax, Q, max_span, ppc); break;
-    NISQA_FE_CASE(32) NISQA_FE_CASE(40) NISQA_FE_CASE(48) NISQA_FE_CASE(64) NISQA_FE_CASE(80) NISQA_FE_CASE(96) NISQA_FE_CASE(128)
-#undef NISQA_FE_CASE
+    FE_MELS_CASE(32) FE_MELS_CASE(40) FE_MELS_CASE(48) FE_MELS_CASE(64) FE_MELS_CASE(80) FE_MELS_CASE(96) FE_MELS_CASE(128)
+#undef FE_MELS_CASE
     default: break;
   }
 }

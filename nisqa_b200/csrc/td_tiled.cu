@@ -22,12 +22,7 @@
 // ones in flight while the current one is multiplied.  fp32 throughout (parity: +-1e-4 on the scores).
 #include "../../include/nisqa_b200.h"
 #include "common.cuh"
-#include "f32x2.cuh"
 #include "launch.cuh"
-
-#ifndef NISQA_TD_PK
-#define NISQA_TD_PK 0        // tile GEMMs with packed FFMA2 (same FMAs in the same order)
-#endif
 
 namespace nisqa {
 
@@ -65,73 +60,6 @@ __device__ __forceinline__ void zero_acc(float (&acc)[4][4]) {
     for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
 }
 
-#if NISQA_TD_PK
-// acc[i][j] += sum_k A[4ty+i][k] * B[k][4tx+j]   (packed FFMA2: the same fp32 FMA per element, in the same k order)
-__device__ __forceinline__ void gemm_nn(float (&acc)[4][4], const float* __restrict__ A, const float* __restrict__ B,
-                                        int ldb, int ty, int tx) {
-  const float* a0 = A + (4 * ty) * kLd;
-  const float* b0 = B + 4 * tx;
-  f2 c[4][2];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { c[i][0] = pk(acc[i][0], acc[i][1]); c[i][1] = pk(acc[i][2], acc[i][3]); }
-#pragma unroll 2
-  for (int k = 0; k < kT; k += 4) {
-    float4 a[4], b[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) a[i] = *reinterpret_cast<const float4*>(a0 + i * kLd + k);
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) b[kk] = *reinterpret_cast<const float4*>(b0 + (k + kk) * ldb);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float av[4] = {a[i].x, a[i].y, a[i].z, a[i].w};
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        c[i][0] = fma2(bc(av[kk]), pk(b[kk].x, b[kk].y), c[i][0]);
-        c[i][1] = fma2(bc(av[kk]), pk(b[kk].z, b[kk].w), c[i][1]);
-      }
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float2 lo = upk(c[i][0]), hi = upk(c[i][1]);
-    acc[i][0] = lo.x; acc[i][1] = lo.y; acc[i][2] = hi.x; acc[i][3] = hi.y;
-  }
-}
-
-// acc[i][j] += sum_k A[4ty+i][k] * B[tx+16j][k]   (columns j, j+1 packed: FFMA2 with the A element broadcast)
-__device__ __forceinline__ void gemm_nt(float (&acc)[4][4], const float* __restrict__ A, const float* __restrict__ B,
-                                        int ty, int tx) {
-  const float* a0 = A + (4 * ty) * kLd;
-  const float* b0 = B + tx * kLd;
-  f2 c[4][2];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { c[i][0] = pk(acc[i][0], acc[i][1]); c[i][1] = pk(acc[i][2], acc[i][3]); }
-#pragma unroll 2
-  for (int k = 0; k < kT; k += 4) {
-    float4 a[4], b[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) a[i] = *reinterpret_cast<const float4*>(a0 + i * kLd + k);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) b[j] = *reinterpret_cast<const float4*>(b0 + (16 * j) * kLd + k);
-    const f2 b01[4] = {pk(b[0].x, b[1].x), pk(b[0].y, b[1].y), pk(b[0].z, b[1].z), pk(b[0].w, b[1].w)};
-    const f2 b23[4] = {pk(b[2].x, b[3].x), pk(b[2].y, b[3].y), pk(b[2].z, b[3].z), pk(b[2].w, b[3].w)};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float av[4] = {a[i].x, a[i].y, a[i].z, a[i].w};
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        c[i][0] = fma2(bc(av[kk]), b01[kk], c[i][0]);
-        c[i][1] = fma2(bc(av[kk]), b23[kk], c[i][1]);
-      }
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float2 lo = upk(c[i][0]), hi = upk(c[i][1]);
-    acc[i][0] = lo.x; acc[i][1] = lo.y; acc[i][2] = hi.x; acc[i][3] = hi.y;
-  }
-}
-#else
 // acc[i][j] += sum_k A[4ty+i][k] * B[k][4tx+j]
 __device__ __forceinline__ void gemm_nn(float (&acc)[4][4], const float* __restrict__ A, const float* __restrict__ B,
                                         int ldb, int ty, int tx) {
@@ -181,7 +109,6 @@ __device__ __forceinline__ void gemm_nt(float (&acc)[4][4], const float* __restr
       }
   }
 }
-#endif
 
 // reductions over the 16 lanes (tx) that share a row
 __device__ __forceinline__ float row_sum(float v) {

@@ -2,7 +2,8 @@
 # GPU-box memory / race / init check of every kernel on the default path (SURVEY.md section 5: the reference has no
 # sanitizer story; this is ours): compute-sanitizer memcheck over __graft_entry__.smoke() (nisqa.tar, two
 # short clips at 48 / 16 kHz: front-end, conv1, the five wgmma conv layers with their bulk copies /
-# mbarriers, self-attention, pooling), over a short nisqa_tts.tar call (StandardCNN, BiLSTM) and over device-batch
+# mbarriers, self-attention, pooling), over a 96 kHz clip (frontend_kernel, the front end for windows over 1024
+# samples), over a short nisqa_tts.tar call (StandardCNN, BiLSTM) and over device-batch
 # calls (the ingest kernel, with and without ms_sr); racecheck over the double-ended alignment's multi-block path.
 #   bash tools/sanitize.sh TAG
 TAG=${1:-rXX}
@@ -16,6 +17,14 @@ import __graft_entry__ as g
 g.smoke()
 from nisqa_b200 import engine as E, synth
 from oracle import nisqa_oracle as O
+args, sd = O.load_checkpoint(os.path.join("weights", "nisqa.tar"))
+eng = E.Engine(E.config_from_args(args), 0); eng.load_state_dict(sd)
+x = synth.synth_speech_pcm16(15, 0.7, 96000)
+sc = eng.predict_pcm([x], [96000])[0]
+ref, _, _ = O.predict_pcm(args, sd, x.astype(np.float32) / 32768.0, 96000)
+assert float(np.abs(sc[0] - ref).max()) <= 1e-4
+print("96 kHz ok", sc.tolist())
+eng.close()
 args, sd = O.load_checkpoint(os.path.join("weights", "nisqa_tts.tar"))
 eng = E.Engine(E.config_from_args(args, max_chunk_segments=64), 0); eng.load_state_dict(sd)   # two passes: shrinking planes
 sc, ns, st = eng.predict_pcm([synth.synth_speech_pcm16(7, 0.6, 16000), synth.synth_speech_pcm16(8, 0.3, 16000)], [16000, 16000])
