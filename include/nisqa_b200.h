@@ -268,6 +268,34 @@ NISQA_API int  nisqa_predict_device_batch(nisqa_engine* e, void* cuda_stream, co
                                           const nisqa_device_batch* ref, int32_t target_sr, float* scores_dev,
                                           int32_t* n_segments_out, int32_t* status_out);
 
+/* Where in a clip the quality drops: the per-segment outputs of nisqa_predict_device_batch_segments.  Row r of both
+ * arrays belongs to one segment; the rows of clip g follow those of the clips before it, one row per segment for every
+ * clip whose status is OK, none for the others and none for NISQA_DE's reference clips (2p + 1).  For pooling head h
+ * (n_out of them) and segment t of a clip:
+ *   scores[r][h]  : the pooling module applied to the one-segment sequence x[t:t+1] (x: the rows NISQA_STAGE_TD_OUT
+ *                   documents), i.e. its last Linear applied to x_t (PoolAttFF linear3, PoolAtt linear2, else linear)
+ *   weights[r][h] : PoolAtt / PoolAttFF: the softmax weight of step t over the clip's segments; PoolAvg: 1 / n_seg;
+ *                   PoolLastStep: 1 at the last segment, 0 elsewhere; PoolMax / PoolLastStepBi: NaN.  Where a weight
+ *                   exists, the clip's score is sum_t weights[t][h] * scores[t][h].
+ * A clip that scores NaN while its status is OK (NISQA_DE: a reference that is too short or too long) has NaN rows.
+ * Segment t spans t*seg_hop*hop / sr .. (t*seg_hop + seg_len - 1)*hop / sr seconds (the centres of its first and last
+ * mel frame; hop = (int)(sr*hop_s), sr the model rate: target_sr when set, else the batch's sample_rate). */
+typedef struct nisqa_segment_out {
+  float*  scores;    /* device [n_rows][n_out] fp32 */
+  float*  weights;   /* device [n_rows][n_out] fp32 */
+  int64_t n_rows;    /* rows the two arrays hold */
+} nisqa_segment_out;
+
+/* nisqa_predict_device_batch that also writes the per-segment scores and weights to seg (not NULL), with the same
+ * stream contract and no host wait of its own.  If seg->n_rows is smaller than the segment count of the call's OK
+ * (non-reference) clips it returns NISQA_ERR_INVALID before anything is enqueued.  scores_dev gets the same values as
+ * nisqa_predict_device_batch would write.  The shipped nisqa_tts.tar shape stores the per-step BiLSTM outputs in such a
+ * call (as "keep_td_out" does, without changing that option). */
+NISQA_API int  nisqa_predict_device_batch_segments(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                                                   const nisqa_device_batch* ref, int32_t target_sr, float* scores_dev,
+                                                   const nisqa_segment_out* seg, int32_t* n_segments_out,
+                                                   int32_t* status_out);
+
 /* Copy an intermediate of the LAST predict call to host memory (parity tests).  Only valid
  * when that call fitted in one internal pass.  Returns the number of floats written (>=0)
  * or a negative status; with out == NULL returns the required count. */

@@ -9,11 +9,16 @@ same precedence of checkpoint args vs. CLI args, but with the torch modules repl
 ``train()`` and ``mode == 'main'`` raise ``NotImplementedError``.  Double-ended checkpoints (NISQA_DE) run in
 ``predict_csv`` mode with ``args['csv_ref']`` naming the reference column, as in the reference (model:846, 951-955).  There is no CPU device: ``tr_device='cpu'``
 or a machine without CUDA raises.
+
+``args['segments']`` (``run_predict.py --segments``) also writes ``NISQA_segments.csv`` into ``output_dir``: one row per
+segment of every file with its time span, its score under each pooling head and the head's pooling weight
+(:meth:`nisqa_b200.scorer.Scorer.segments`).  Single process only.
 """
 import datetime
 import os
 from glob import glob
 
+import numpy as np
 import pandas as pd
 
 pd.options.mode.chained_assignment = None
@@ -31,6 +36,9 @@ class nisqaModel(object):
 
     def __init__(self, args):
         self.args = args
+        if args.get("segments") and nb_dist.env_world()[1] > 1:
+            raise ValueError("segments: NISQA_segments.csv is written by a single process, not under torchrun with %d ranks"
+                             % nb_dist.env_world()[1])
         if "mode" not in self.args:
             self.args["mode"] = "main"
         self.runinfos = {}
@@ -99,7 +107,65 @@ class nisqaModel(object):
                     os.path.join(self.args["output_dir"], "NISQA_results.csv"), index=False)
         if chatty:
             print(self.ds_val.df.to_string(index=False))
+        if self.args.get("segments") and self.args["output_dir"]:
+            self.predict_segments().to_csv(os.path.join(self.args["output_dir"], "NISQA_segments.csv"), index=False)
         return self.ds_val.df
+
+    def predict_segments(self):
+        """-> DataFrame with one row per segment of every file, in file order: the file column, ``segment``,
+        ``t_start`` / ``t_end`` (seconds), each head's segment score (``*_pred``) and pooling weight (``*_weight``).
+        The files are decoded by the dataset's loader and scored in batches of ``tr_bs_val`` clips of one sample rate
+        through :meth:`Scorer.segments`."""
+        from .scorer import Scorer
+        sc = Scorer.__new__(Scorer)
+        sc._configure(self.args, self.dev)
+        sc.engine = self.model
+        ds, bs = self.ds_val, max(1, int(self.args["tr_bs_val"]))
+        de = ds.double_ended
+        col = ds.filename_column
+        files = ds.df[col].tolist()
+        weight_cols = [c[:-len("_pred")] + "_weight" for c in sc.columns]
+        loaded = []
+        for i in range(len(ds)):
+            y, sr = NL.read_wav(ds.file_path(i), ds.ms_channel)
+            ref = NL.read_wav(ds.file_path_ref(i), None) if de else (None, None)
+            loaded.append((y, sr) + ref)
+        groups = {}
+        for i, (_, sr, _, sr_ref) in enumerate(loaded):
+            groups.setdefault((sr, sr_ref), []).append(i)
+        parts = {}
+        for (sr, sr_ref), rows in groups.items():
+            for k in range(0, len(rows), bs):
+                batch = rows[k:k + bs]
+                wave, lens = self._batch_tensor([loaded[i][0] for i in batch])
+                kw = {}
+                if de:
+                    kw["reference"], kw["reference_lengths"] = self._batch_tensor([loaded[i][2] for i in batch])
+                    kw["reference_sample_rate"] = sr_ref
+                res = sc.segments(wave, sr, lengths=lens, **kw)
+                s, w = res.seg_scores.cpu().numpy(), res.seg_weights.cpu().numpy()
+                r0 = 0
+                for j, i in enumerate(batch):
+                    n = res.counts[j]
+                    part = pd.DataFrame({col: [files[i]] * n, "segment": np.arange(n),
+                                         "t_start": res.t_start[r0:r0 + n], "t_end": res.t_end[r0:r0 + n]})
+                    for h, c in enumerate(sc.columns):
+                        part[c] = s[r0:r0 + n, h].astype(float)
+                    for h, c in enumerate(weight_cols):
+                        part[c] = w[r0:r0 + n, h].astype(float)
+                    parts[i] = part
+                    r0 += n
+        return pd.concat([parts[i] for i in range(len(ds))], ignore_index=True)
+
+    def _batch_tensor(self, clips):
+        """host clips -> ([B, T] CUDA tensor, lengths): int16 when every clip is int16, else float32"""
+        if any(c.dtype != np.int16 for c in clips):
+            clips = [c if c.dtype == np.float32 else c.astype(np.float32) / np.float32(32768.0) for c in clips]
+        lens = [c.shape[0] for c in clips]
+        x = np.zeros((len(clips), max(lens)), dtype=clips[0].dtype)
+        for j, c in enumerate(clips):
+            x[j, :lens[j]] = c
+        return torch.from_numpy(x).to(self.dev), lens
 
     # ------------------------------------------------------------------ datasets (model:732-847)
     def _loadDatasets(self):

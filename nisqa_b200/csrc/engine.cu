@@ -122,8 +122,9 @@ struct Stage {
   int lane = 0;
   HostBuf h_tables;
   DevBuf pcm, clips, prefixes, clipmax;
+  DevBuf seg_row;        // segments call: each clip's first output row (int64, < 0: none)
   void release() {
-    DevBuf* all[] = {&pcm, &clips, &prefixes, &clipmax};
+    DevBuf* all[] = {&pcm, &clips, &prefixes, &clipmax, &seg_row};
     for (auto* b : all) b->release();
     h_tables.release();
     if (ev_copied) cudaEventDestroy(ev_copied);
@@ -236,6 +237,10 @@ struct nisqa_engine {
   // call's last pass (the caller's stream waits for it)
   cudaEvent_t ev_in = nullptr, ev_out = nullptr;
   float pool_bias_std = 0.f;
+  // nisqa_predict_device_batch_segments: the call's output rows (nullptr outside such a call) and the first row of each
+  // clip of the call (-1: none)
+  const nisqa_segment_out* seg_out = nullptr;
+  std::vector<long long> seg_row;
   float tc_scale[8] = {1, 1, 1, 1, 1, 1, 1, 1};   // 2^(e_{i-1} - S_i): undoes the activation and weight pre-scales of conv i
   int act_exp[8] = {0, 0, 0, 0, 0, 0, 0, 0};      // e_i: conv i's activations are stored as fp16 planes of v * 2^-e_i
   float act_store(int i) const { return ldexpf(1.f, -act_exp[i]); }
@@ -1121,6 +1126,13 @@ struct Pass {
   int* seg_frame0 = nullptr;                  // segment table (lane, seg_table_kernel)
   float* seg_thr = nullptr;
   int* seg_clip = nullptr;
+  const long long* seg_row = nullptr;         // segments call: the clips' first output rows (staging slot)
+  // the rows the pooling module read (segment_rows): D real columns at a stride of ld, the attention logits the pooling
+  // path wrote (or nullptr), and each head's last Linear (PoolSimpleParams.w3 / b3; a1 / a1b for PoolAtt)
+  const float* pool_x = nullptr;
+  int pool_D = 0, pool_ld = 0;
+  const float* pool_logits = nullptr;
+  PoolSimpleParams pool_P = {};
   Pass(nisqa_engine* e_, const PassInput& in)
       : e(e_), c(e_->cfg), w(e_->w), LN(e_->lanes[in.slot]), SG(e_->stages[in.stage]), st(LN.stream),
         std_mode(e_->std_cnn()), scores(in.scores_dev_out), n(in.n_clips) {}
@@ -1180,10 +1192,17 @@ int upload_inputs(Pass& p, const PassInput& in) {
   SG.lane = in.slot;
   // one pinned block: ClipDesc[n] | the prefix arrays
   const size_t tb_clips = (size_t)n * sizeof(ClipDesc), tb_pref = pre.size() * 4;
-  CK(SG.h_tables.reserve(tb_clips + tb_pref));
+  const size_t tb_rows_at = (tb_clips + tb_pref + 7) / 8 * 8, tb_rows = e->seg_out ? (size_t)n * 8 : 0;
+  CK(SG.h_tables.reserve(tb_rows_at + tb_rows));
   char* ht = SG.h_tables.as<char>();
   memcpy(ht, cl.data(), tb_clips);
   memcpy(ht + tb_clips, pre.data(), tb_pref);
+  if (tb_rows) {      // (a segments call: the rows of the pass's clips)
+    memcpy(ht + tb_rows_at, e->seg_row.data() + in.first_clip, tb_rows);
+    CK(SG.seg_row.reserve(tb_rows));
+    CK(cudaMemcpyAsync(SG.seg_row.p, ht + tb_rows_at, tb_rows, cudaMemcpyHostToDevice, cs));
+    p.seg_row = SG.seg_row.as<long long>();
+  }
   CK(SG.clips.reserve(tb_clips));
   CK(SG.prefixes.reserve(tb_pref));
   CK(SG.clipmax.reserve((size_t)n * 4));
@@ -1456,6 +1475,9 @@ int pool_rows(Pass& p, const float* x, int D, int ld, bool after_lstm) {
   Lane& LN = p.LN;
   const Weights& w = p.w;
   const int n_seg = p.n_seg, nh = c.n_out;
+  p.pool_x = x; p.pool_D = D; p.pool_ld = ld;
+  p.pool_P = w.pool_simple;
+  if (c.pool == NISQA_POOL_ATT_FF) p.pool_P = {nullptr, nullptr, w.pool_head.w3, w.pool_head.b3};
   if (!after_lstm) {
     Scope s(e, "pool");
     if (c.pool == NISQA_POOL_ATT_FF)
@@ -1463,6 +1485,7 @@ int pool_rows(Pass& p, const float* x, int D, int ld, bool after_lstm) {
     else
       launch_pool_simple(p.st, x, D, ld, p.clips, p.n, c.pool, w.pool_simple, nh, p.max_n_seg, p.scores);
     if (c.double_ended) launch_de_finalize(p.st, p.clips, p.n, nh, p.scores);
+    if (c.pool == NISQA_POOL_ATT_FF) p.pool_logits = LN.logits.as<float>();     // (written by the last td_sa layer)
     return 0;
   }
   Scope s(e, "pool", c.pool == NISQA_POOL_ATT_FF ? 3 : 1);
@@ -1472,6 +1495,7 @@ int pool_rows(Pass& p, const float* x, int D, int ld, bool after_lstm) {
     launch_linear_tile(p.st, x, ld, w.lstm_att.wT, w.lstm_att.b, 1, LN.atth.as<float>(), nh * 128, n_seg, ld, nh * 128);
     launch_att_logits(p.st, LN.atth.as<float>(), w.pool_head.w2, w.pool_head.b2, nh, n_seg, LN.logits.as<float>());
     launch_pool_final(p.st, x, D, ld, LN.logits.as<float>(), p.clips, p.n, w.pool_head, nh, p.max_n_seg, p.scores);
+    p.pool_logits = LN.logits.as<float>();      // (taken after the reserve above, which may move the buffer)
   } else {
     launch_pool_simple(p.st, x, D, ld, p.clips, p.n, c.pool, w.pool_simple, nh, p.max_n_seg, p.scores);
   }
@@ -1499,6 +1523,8 @@ int pool_framewise(Pass& p, const float* x, int D, int ld) {
     P.b3 = w.pool_head.b3;
   }
   launch_pool_wide(p.st, x, D, ld, c.pool, P, nh, LN.logits.as<float>(), n_seg, p.clips, p.n, LN.partial.as<float>(), p.scores);
+  p.pool_x = x; p.pool_D = D; p.pool_ld = ld; p.pool_P = P;
+  if (attff || att) p.pool_logits = LN.logits.as<float>();      // (PoolAtt's too: launch_pool_wide wrote them)
   return 0;
 }
 
@@ -1590,7 +1616,8 @@ int lstm_head(Pass& p) {
   CK(LN.partial.reserve((size_t)p.n * 2 * 4));
   { Scope s(e, "fc_out"); launch_fc20(p.st, LN.feats.as<float>(), w.fc.wT, w.fc.b, LN.feats20.as<float>(), n_seg); }
   const bool lastbi = c.pool == NISQA_POOL_LAST_STEP_BI;
-  const bool keep = e->keep_td_out || !lastbi;        // the other pooling modules read every step's output
+  // the other pooling modules read every step's output, and so does a segments call
+  const bool keep = e->keep_td_out || !lastbi || e->seg_out;
   { Scope s(e, "lstm", 2);
     if (e->lstm_batched)
       launch_lstm_batched(p.st, LN.feats20.as<float>(), p.clips, p.by_len, p.n, w.lstm, keep ? LN.tdout.as<float>() : nullptr,
@@ -1608,6 +1635,28 @@ int lstm_head(Pass& p) {
   e->last_td_out = (e->lstm_batched && !keep) ? nullptr : LN.tdout.as<float>();
   e->last_td_out_d = 256;
   e->last_td_out_ld = 256;
+  p.pool_x = LN.tdout.as<float>(); p.pool_D = 256; p.pool_ld = 256; p.pool_P = w.pool_simple;
+  return 0;
+}
+
+// A segments call: every segment's score and pooling weight under each head, from the rows the pooling module read,
+// to the call's output rows.  A clip the call counts rows for but the pass did not run (NISQA_DE: its reference is
+// too short or too long) gets NaN rows, like its score.
+int segment_rows(Pass& p, const PassInput& in) {
+  nisqa_engine* e = p.e;
+  const int nh = p.c.n_out;
+  const nisqa_segment_out& so = *e->seg_out;
+  for (int i = 0; i < p.n; ++i) {
+    const long long r = e->seg_row[in.first_clip + i];
+    if (r < 0 || in.plan[i].run) continue;
+    const size_t off = (size_t)r * nh, bytes = (size_t)in.plan[i].n_seg * nh * 4;
+    CK(cudaMemsetAsync(so.scores + off, 0xFF, bytes, p.st));
+    CK(cudaMemsetAsync(so.weights + off, 0xFF, bytes, p.st));
+  }
+  if (p.n_seg == 0) return 0;
+  Scope s(e, "segments");
+  launch_segment_scores(p.st, p.pool_x, p.pool_D, p.pool_ld, p.pool_logits, p.pool_P, nh, p.c.pool, p.clips, p.n, p.seg_row,
+                        so.scores, so.weights);
   return 0;
 }
 
@@ -1622,6 +1671,10 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
     Rows rows;
     rc = framewise(p, in.fmt, &rows);
     if (!rc) rc = p.w.lstm_shipped ? lstm_head(p) : td_stages(p, rows);
+    if (rc) return rc;
+  }
+  if (e->seg_out) {
+    rc = segment_rows(p, in);
     if (rc) return rc;
   }
   CK(cudaGetLastError());
@@ -2082,9 +2135,10 @@ static int enqueue_device_batch(nisqa_engine* e, cudaStream_t caller, int n_clip
   return 0;
 }
 
-int nisqa_predict_device_batch(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
-                               const nisqa_device_batch* ref, int32_t target_sr, float* scores_dev,
-                               int32_t* n_segments_out, int32_t* status_out) {
+// nisqa_predict_device_batch (seg == nullptr) and nisqa_predict_device_batch_segments
+static int device_batch_call(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg, const nisqa_device_batch* ref,
+                             int32_t target_sr, float* scores_dev, const nisqa_segment_out* seg, int32_t* n_segments_out,
+                             int32_t* status_out) {
   if (!e) return NISQA_ERR_INVALID;
   if (!e->stream) return fail(e, NISQA_ERR_STATE, "engine was not created successfully");
   if (!deg) return fail(e, NISQA_ERR_INVALID, "deg: null argument");
@@ -2122,11 +2176,30 @@ int nisqa_predict_device_batch(nisqa_engine* e, void* cuda_stream, const nisqa_d
   std::vector<int32_t> sr(n_clips);
   for (int g = 0; g < n_clips; ++g) { ns[g] = src[g % n_src]->n_samples[g / n_src]; sr[g] = src[g % n_src]->sample_rate; }
   const int fmt = out_f32 ? NISQA_FMT_F32 : NISQA_FMT_S16;
+  if (seg) {
+    // each OK clip's rows, in clip order (NISQA_DE: the degraded clips only), from the host arithmetic the passes repeat
+    if (n_clips > 0 && (!seg->scores || !seg->weights)) return fail(e, NISQA_ERR_INVALID, "seg: null scores / weights");
+    e->seg_row.assign(n_clips, -1);
+    long long rows = 0;
+    for (int g = 0; g < n_clips; ++g) {
+      const int64_t n = target_sr > 0 ? nisqa_resample_out_len(ns[g], sr[g], target_sr) : ns[g];
+      ClipPlan pl;
+      plan_clip(e->cfg, n, target_sr > 0 ? target_sr : sr[g], &pl);
+      if (pl.status != NISQA_CLIP_OK || (e->cfg.double_ended && (g & 1))) continue;
+      e->seg_row[g] = rows;
+      rows += pl.n_seg;
+    }
+    if (seg->n_rows < rows)
+      return fail(e, NISQA_ERR_INVALID, "seg->n_rows = " + std::to_string(seg->n_rows) + ": the call has " +
+                                            std::to_string(rows) + " segment rows");
+  }
   CK(cudaSetDevice(e->device));
   cudaStream_t caller = static_cast<cudaStream_t>(cuda_stream);
   RsSlot* S = nullptr;
+  e->seg_out = seg;
   const int rc = enqueue_device_batch(e, caller, n_clips, ing, ns.data(), sr.data(), fmt, target_sr, scores_dev,
                                       n_segments_out, status_out, &S);
+  e->seg_out = nullptr;
   if (rc) {
     // whatever was enqueued before the failure may still read the caller's input or the conversion slot: the caller's
     // stream waits for every lane, and the slot stays in use until then (best effort: the error is already reported)
@@ -2135,6 +2208,19 @@ int nisqa_predict_device_batch(nisqa_engine* e, void* cuda_stream, const nisqa_d
     if (S && cudaEventRecord(S->done, caller) == cudaSuccess) S->busy = true;
   }
   return rc;
+}
+
+int nisqa_predict_device_batch(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                               const nisqa_device_batch* ref, int32_t target_sr, float* scores_dev,
+                               int32_t* n_segments_out, int32_t* status_out) {
+  return device_batch_call(e, cuda_stream, deg, ref, target_sr, scores_dev, nullptr, n_segments_out, status_out);
+}
+
+int nisqa_predict_device_batch_segments(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                                        const nisqa_device_batch* ref, int32_t target_sr, float* scores_dev,
+                                        const nisqa_segment_out* seg, int32_t* n_segments_out, int32_t* status_out) {
+  if (e && !seg) return fail(e, NISQA_ERR_INVALID, "seg: null argument");
+  return device_batch_call(e, cuda_stream, deg, ref, target_sr, scores_dev, seg, n_segments_out, status_out);
 }
 
 int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {

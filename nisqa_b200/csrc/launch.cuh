@@ -165,6 +165,14 @@ constexpr int kPoolWideSlab = 128;
 constexpr int pool_wide_slabs(int D) { return (D + kPoolWideSlab - 1) / kPoolWideSlab; }
 void launch_pool_wide(cudaStream_t st, const float* x, int D, int ldx, int mode, const PoolSimpleParams& P, int n_heads,
                       float* logits, int n_seg, const ClipDesc* clips, int n_clips, float* partial, float* scores);
+// Per-segment scores and weights [rows][n_heads] of the rows the pooling module read (x: D real columns at a stride of
+// ldx, D <= 4096).  mode: enum nisqa_pool.  P.w3 / P.b3: each head's last Linear [n_heads][D] (columns in the rows'
+// order).  logits [n_seg][n_heads]: the attention logits the pooling path wrote (PoolAttFF; PoolAtt over wide rows), or
+// nullptr for PoolAtt, whose logits a1 . x + a1b (P.a1 [n_heads][D], P.a1b) are then formed here.  row_off [n_clips]:
+// the clip's first output row, < 0 for a clip that gets none.
+void launch_segment_scores(cudaStream_t st, const float* x, int D, int ldx, const float* logits, const PoolSimpleParams& P,
+                           int n_heads, int mode, const ClipDesc* clips, int n_clips, const long long* row_off,
+                           float* seg_scores, float* seg_weights);
 
 // ---------------------------------------------------------------- td_tiled.cu (self-attention, NISQA_DE, SkipCNN / DFF)
 void launch_td_in(cudaStream_t st, int nc, const float* feats, const float* WT, int nk, const float* b, const float* g,

@@ -801,6 +801,88 @@ __global__ void pool_att_logits_kernel(const float* __restrict__ x, int D, int l
   }
 }
 
+// ---------------------------------------------------------------------------------------
+// Per-segment scores and pooling weights (nisqa_predict_device_batch_segments).  Segment t's score under head h is the
+// pooling module applied to the one-step sequence x[t:t+1]: its last Linear, w3_h . x_t + b3_h, for every module.  Its
+// weight is the module's softmax weight of step t (PoolAtt, PoolAttFF), 1 / S (PoolAvg), [t == S - 1] (PoolLastStep)
+// or NaN (PoolMax, PoolLastStepBi: no weight per step reproduces the clip's score).  One CTA per clip, its warps over
+// the clip's segments, lanes over the columns.  Sweep 1 writes the scores and parks the attention logits in the
+// weight rows while it keeps each warp's running max and rescaled sum; sweep 2 turns the logits into weights.  Clips
+// with row_off < 0 (skipped, or NISQA_DE reference clips) get no rows.  About n_seg n_heads D FMAs and one read of the
+// rows: far too little work for the tensor cores.
+constexpr int kSegWarps = 8;
+
+template <int NH>
+__global__ void __launch_bounds__(kSegWarps * 32)
+segment_scores_kernel(const float* __restrict__ x, int D, int ldx, const float* __restrict__ logits, PoolSimpleParams P,
+                      int mode, const ClipDesc* __restrict__ clips, const long long* __restrict__ row_off,
+                      float* __restrict__ seg_scores, float* seg_weights) {
+  __shared__ float wm[kSegWarps][NH], ws[kSegWarps][NH];
+  __shared__ float mx[NH], sum[NH];
+  const ClipDesc cd = clips[blockIdx.x];
+  const long long r0 = row_off[blockIdx.x];
+  const int S = cd.n_seg;
+  if (S <= 0 || r0 < 0) return;
+  const int lane = threadIdx.x & 31, g = threadIdx.x >> 5;
+  const bool att = mode == 0 || mode == 1, own_logits = mode == 1 && logits == nullptr;
+  float m[NH], s[NH];
+#pragma unroll
+  for (int h = 0; h < NH; ++h) { m[h] = -INFINITY; s[h] = 0.f; }
+  for (int t = g; t < S; t += kSegWarps) {
+    const float* xr = x + (size_t)(cd.seg_off + t) * ldx;
+    float acc[NH], la[NH];
+#pragma unroll
+    for (int h = 0; h < NH; ++h) { acc[h] = 0.f; la[h] = 0.f; }
+    for (int k = lane; k < D; k += 32) {
+      const float v = __ldg(xr + k);
+#pragma unroll
+      for (int h = 0; h < NH; ++h) {
+        acc[h] = fmaf(v, __ldg(P.w3 + (size_t)h * D + k), acc[h]);
+        if (own_logits) la[h] = fmaf(v, __ldg(P.a1 + (size_t)h * D + k), la[h]);
+      }
+    }
+    const long long row = r0 + t;
+#pragma unroll
+    for (int h = 0; h < NH; ++h) {
+      const float sc = warp_sum(acc[h]) + __ldg(P.b3 + h);
+      float l = 0.f;
+      if (own_logits) l = warp_sum(la[h]) + __ldg(P.a1b + h);
+      else if (att) l = __ldg(logits + (size_t)(cd.seg_off + t) * NH + h);
+      if (lane == 0) {
+        seg_scores[row * NH + h] = sc;
+        if (att) seg_weights[row * NH + h] = l;
+      }
+      if (att) {
+        const float nm = fmaxf(m[h], l);
+        s[h] = s[h] * expf(m[h] - nm) + expf(l - nm);
+        m[h] = nm;
+      }
+    }
+  }
+  if (att) {
+    if (lane == 0)
+#pragma unroll
+      for (int h = 0; h < NH; ++h) { wm[g][h] = m[h]; ws[g][h] = s[h]; }
+    __syncthreads();
+    if (threadIdx.x < NH) {
+      const int h = threadIdx.x;
+      float M = wm[0][h];
+      for (int w = 1; w < kSegWarps; ++w) M = fmaxf(M, wm[w][h]);
+      float tot = 0.f;
+      for (int w = 0; w < kSegWarps; ++w) tot += ws[w][h] == 0.f ? 0.f : ws[w][h] * expf(wm[w][h] - M);
+      mx[h] = M;
+      sum[h] = tot;
+    }
+  }
+  __syncthreads();                       // (also makes sweep 1's parked logits visible to the whole CTA)
+  const float nan = __int_as_float(0x7fc00000);
+  for (int i = threadIdx.x; i < S * NH; i += kSegWarps * 32) {
+    const int t = i / NH, h = i - t * NH;
+    float* wp = seg_weights + (r0 + t) * NH + h;
+    *wp = att ? expf(*wp - mx[h]) / sum[h] : mode == 2 ? 1.f / (float)S : mode == 4 ? (t == S - 1 ? 1.f : 0.f) : nan;
+  }
+}
+
 // ------------------------------------------------------------------ host launchers
 constexpr int kRowSmem20 = (kRows * kXS + 64 * 20) * 4;
 
@@ -933,6 +1015,16 @@ void launch_pool_wide(cudaStream_t st, const float* x, int D, int ldx, int mode,
   if (n_clips <= 0) return;
   if (n_heads == 5) pool_wide_instance<5>(st, x, D, ldx, mode, P, logits, n_seg, clips, n_clips, partial, scores);
   else pool_wide_instance<1>(st, x, D, ldx, mode, P, logits, n_seg, clips, n_clips, partial, scores);
+}
+
+void launch_segment_scores(cudaStream_t st, const float* x, int D, int ldx, const float* logits, const PoolSimpleParams& P,
+                           int n_heads, int mode, const ClipDesc* clips, int n_clips, const long long* row_off,
+                           float* seg_scores, float* seg_weights) {
+  if (n_clips <= 0) return;
+  if (n_heads == 5)
+    segment_scores_kernel<5><<<n_clips, kSegWarps * 32, 0, st>>>(x, D, ldx, logits, P, mode, clips, row_off, seg_scores, seg_weights);
+  else
+    segment_scores_kernel<1><<<n_clips, kSegWarps * 32, 0, st>>>(x, D, ldx, logits, P, mode, clips, row_off, seg_scores, seg_weights);
 }
 
 }  // namespace nisqa

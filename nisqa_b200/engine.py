@@ -39,6 +39,7 @@ EXPORTS = [
     "nisqa_wav_probe", "nisqa_wav_decode", "nisqa_wav_probe_batch", "nisqa_wav_decode_batch",
     "nisqa_resample_set_filter", "nisqa_resample_out_len", "nisqa_resample_f32",
     "nisqa_resample_device", "nisqa_predict_pcm_resampled", "nisqa_set_cnn_pools", "nisqa_predict_device_batch",
+    "nisqa_predict_device_batch_segments",
 ]
 
 
@@ -167,6 +168,11 @@ class NisqaDeviceBatch(C.Structure):
                 ("n_samples", C.POINTER(C.c_int64)), ("sample_rate", C.c_int32)]
 
 
+class NisqaSegmentOut(C.Structure):
+    """nisqa_segment_out: device [n_rows][n_out] per-segment scores and pooling weights"""
+    _fields_ = [("scores", C.c_void_p), ("weights", C.c_void_p), ("n_rows", C.c_int64)]
+
+
 class NisqaTensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", C.POINTER(C.c_float)), ("ndim", C.c_int32),
                 ("dims", C.c_int64 * 4)]
@@ -235,6 +241,8 @@ def load_library(path=None):
     dbp = C.POINTER(NisqaDeviceBatch)
     lib.nisqa_predict_device_batch.argtypes = [vp, vp, dbp, dbp, C.c_int32, vp, i32p, i32p]
     lib.nisqa_predict_device_batch.restype = C.c_int
+    lib.nisqa_predict_device_batch_segments.argtypes = [vp, vp, dbp, dbp, C.c_int32, vp, C.POINTER(NisqaSegmentOut), i32p, i32p]
+    lib.nisqa_predict_device_batch_segments.restype = C.c_int
     lib.nisqa_stage_dump.argtypes = [vp, C.c_int, f32p, C.c_int64]
     lib.nisqa_stage_dump.restype = C.c_int64
     lib.nisqa_segment_counts.argtypes = [C.POINTER(NisqaConfig), C.c_int64, C.c_int32, i32p, i32p, i32p]
@@ -692,17 +700,32 @@ class Engine(object):
         the checkpoint's ``ms_sr`` (0: none; every clip is converted to it on the device), the scores
         go to ``scores_dev_ptr`` ([rows, n_out] fp32 device memory; rows = n_clips, NISQA_DE 2 n_clips).  Returns
         (n_segments int32[rows], status int32[rows]), valid on return; the scores are valid in ``stream``'s order."""
+        return self._device_batch(stream, deg, scores_dev_ptr, ref, target_sr, None)
+
+    def predict_device_batch_segments(self, stream, deg, scores_dev_ptr, seg_scores_ptr, seg_weights_ptr, n_rows, ref=None,
+                                      target_sr=0):
+        """:meth:`predict_device_batch` that also writes every segment's score and pooling weight to the device arrays
+        ``seg_scores_ptr`` / ``seg_weights_ptr`` ([n_rows, n_out] fp32 each; one row per segment of every OK clip in
+        clip order, none for NISQA_DE's reference clips; include/nisqa_b200.h nisqa_segment_out).  Raises EngineError,
+        with nothing enqueued, when ``n_rows`` is too small."""
+        seg = NisqaSegmentOut(scores=seg_scores_ptr or None, weights=seg_weights_ptr or None, n_rows=int(n_rows))
+        return self._device_batch(stream, deg, scores_dev_ptr, ref, target_sr, seg)
+
+    def _device_batch(self, stream, deg, scores_dev_ptr, ref, target_sr, seg):
         rows = deg[0].n_clips * (2 if ref is not None else 1)
         if target_sr:
             from . import resample as _rs
             _rs.out_len(1, 1, 1)                                      # the interpolation table is set once
         nseg = np.empty(rows, dtype=np.int32)
         status = np.empty(rows, dtype=np.int32)
-        rc = self.lib.nisqa_predict_device_batch(
-            self.h, C.c_void_p(stream or None), C.byref(deg[0]), C.byref(ref[0]) if ref is not None else None,
-            int(target_sr or 0), C.c_void_p(scores_dev_ptr), nseg.ctypes.data_as(C.POINTER(C.c_int32)),
-            status.ctypes.data_as(C.POINTER(C.c_int32)))
-        self._check(rc, "nisqa_predict_device_batch")
+        args = (self.h, C.c_void_p(stream or None), C.byref(deg[0]), C.byref(ref[0]) if ref is not None else None,
+                int(target_sr or 0), C.c_void_p(scores_dev_ptr))
+        outs = (nseg.ctypes.data_as(C.POINTER(C.c_int32)), status.ctypes.data_as(C.POINTER(C.c_int32)))
+        if seg is None:
+            self._check(self.lib.nisqa_predict_device_batch(*args, *outs), "nisqa_predict_device_batch")
+        else:
+            self._check(self.lib.nisqa_predict_device_batch_segments(*args, C.byref(seg), *outs),
+                        "nisqa_predict_device_batch_segments")
         return nseg, status
 
     # ------------------------------------------------------------------ introspection

@@ -7,7 +7,11 @@
 The audio never leaves the device: the engine packs it with its own ingest kernel (``nisqa_predict_device_batch``)
 and the scores come back as a CUDA tensor, written in the order of ``torch.cuda.current_stream()``.  Nothing waits for
 the GPU: ``wave`` may be freed or reused in stream order as soon as the call returns.
+
+``scorer.segments(wave, 48000)`` also returns where in each clip the quality drops: every segment's score and pooling
+weight (``nisqa_predict_device_batch_segments``) with its time span.
 """
+import collections
 import numbers
 
 import numpy as np
@@ -16,6 +20,11 @@ import torch
 from . import engine as E
 
 DIM_COLUMNS = ["mos_pred", "noi_pred", "dis_pred", "col_pred", "loud_pred"]     # NISQA_DIM's outputs (lib:1461-1465)
+
+
+# Scorer.segments: scores [B, n_cols] (as Scorer.__call__), seg_scores / seg_weights [N, n_cols] CUDA tensors (the rows of
+# clip b follow those of the clips before it, counts[b] of them), t_start / t_end float64 [N] seconds
+Segments = collections.namedtuple("Segments", ["scores", "seg_scores", "seg_weights", "counts", "t_start", "t_end"])
 
 
 class Scorer(object):
@@ -56,6 +65,47 @@ class Scorer(object):
                       ``reference_lengths`` and ``reference_sample_rate`` (default: ``sample_rate``)
         A clip too short or too long for the checkpoint raises the file ingest's ValueError before anything is enqueued.
         """
+        deg, ref, _ = self._arguments(wave, sample_rate, lengths, channel, reference, reference_lengths, reference_sample_rate)
+        out = self._scores_buffer(deg, ref)
+        if out.shape[0]:
+            self.engine.predict_device_batch(self._stream(), deg, out.data_ptr(), ref=ref, target_sr=self.target_sr)
+        return self._clip_rows(out, ref)
+
+    def segments(self, wave, sample_rate, lengths=None, channel=None, reference=None, reference_lengths=None,
+                 reference_sample_rate=None):
+        """Scores of a batch and of every segment of its clips -> :data:`Segments`.  Takes the arguments of
+        ``__call__`` and checks them alike.
+
+        scores      : float32 [B, len(columns)], the values ``__call__`` returns
+        seg_scores  : float32 [N, len(columns)] CUDA tensor: each pooling head applied to the segment alone (its last
+                      Linear of the segment's time-dependency output row)
+        seg_weights : float32 [N, len(columns)] CUDA tensor: the head's pooling weight of the segment (attention: its
+                      softmax weight; avg: 1 / n_seg; last_step: 1 at the last segment; max, last_step_bi: NaN).  Where
+                      defined, a clip's score is the weighted sum of its segments' scores
+        counts      : host list of B ints, the segments of each clip (its rows follow those of the clips before it)
+        t_start, t_end : float64 [N] host arrays, seconds: the centres of the segment's first and last mel frame
+        NISQA_DE: rows for the degraded clips only.
+        """
+        deg, ref, counts = self._arguments(wave, sample_rate, lengths, channel, reference, reference_lengths,
+                                           reference_sample_rate)
+        out = self._scores_buffer(deg, ref)
+        n_rows = int(sum(counts))
+        seg_s = torch.empty((n_rows, len(self.columns)), dtype=torch.float32, device=self.device)
+        seg_w = torch.empty_like(seg_s)
+        if out.shape[0]:
+            self.engine.predict_device_batch_segments(self._stream(), deg, out.data_ptr(), seg_s.data_ptr(), seg_w.data_ptr(),
+                                                      n_rows, ref=ref, target_sr=self.target_sr)
+        rate = self.target_sr or deg[0].sample_rate
+        a = self.args
+        hop = int(rate * a["ms_hop_length"])                  # (int)(sr * hop_s), as the engine's front end
+        t = np.concatenate([np.arange(c, dtype=np.float64) for c in counts]) if counts else np.zeros(0)
+        t_start = t * a["ms_seg_hop_length"] * hop / rate
+        t_end = (t * a["ms_seg_hop_length"] + a["ms_seg_length"] - 1) * hop / rate
+        return Segments(self._clip_rows(out, ref), seg_s, seg_w, list(counts), t_start, t_end)
+
+    # ------------------------------------------------------------------ shared by __call__ and segments
+    def _arguments(self, wave, sample_rate, lengths, channel, reference, reference_lengths, reference_sample_rate):
+        """-> (deg, ref or None, segment counts of wave's clips) after every check, before anything is enqueued"""
         if self.double_ended and reference is None:
             raise ValueError("reference: a double-ended (NISQA_DE) checkpoint scores (wave, reference) pairs")
         if not self.double_ended and reference is not None:
@@ -67,14 +117,20 @@ class Scorer(object):
                               reference_lengths, None)
             if ref[0].n_clips != deg[0].n_clips:
                 raise ValueError("reference: %d clips for %d clips of wave" % (ref[0].n_clips, deg[0].n_clips))
-        for name, b in (("wave", deg), ("reference", ref)):
-            if b is not None:
-                self._check_segments(name, b[1], b[0].sample_rate)
+        counts = self._check_segments("wave", deg[1], deg[0].sample_rate)
+        if ref is not None:
+            self._check_segments("reference", ref[1], ref[0].sample_rate)
+        return deg, ref, counts
+
+    def _scores_buffer(self, deg, ref):
         n = deg[0].n_clips * (2 if ref is not None else 1)
-        out = torch.empty((n, len(self.columns)), dtype=torch.float32, device=self.device)
-        if n:
-            stream = torch.cuda.current_stream(self.device).cuda_stream
-            self.engine.predict_device_batch(stream, deg, out.data_ptr(), ref=ref, target_sr=self.target_sr)
+        return torch.empty((n, len(self.columns)), dtype=torch.float32, device=self.device)
+
+    def _stream(self):
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    @staticmethod
+    def _clip_rows(out, ref):
         # (NISQA_DE: row 2p holds pair p's score, row 2p + 1 is the reference clip's NaN row)
         return out[0::2].contiguous() if ref is not None else out
 
@@ -124,10 +180,12 @@ class Scorer(object):
         return E.device_batch(x3.data_ptr(), fmt, ns, C, ch, T, x3.stride(0), x3.stride(1), int(sample_rate))
 
     def _check_segments(self, name, n_samples, sample_rate):
-        """The file ingest's too-short / too-long errors (NISQA_lib._raise_for_status), on the host, before any launch"""
+        """The file ingest's too-short / too-long errors (NISQA_lib._raise_for_status), on the host, before any launch.
+        Returns each clip's segment count."""
         from . import resample as RS
         rate = self.target_sr or sample_rate
         a = self.args
+        counts = []
         for i, n in enumerate(n_samples):
             n = int(n) if rate == sample_rate else RS.out_len(int(n), sample_rate, rate)
             _, n_seg, status = E.segment_counts(self.cfg, n, rate)
@@ -135,3 +193,5 @@ class Scorer(object):
                                       a["ms_max_segments"])
             if err is not None:
                 raise err
+            counts.append(n_seg)
+        return counts

@@ -7,6 +7,7 @@ and the same option names, so existing invocations keep working:
     python run_predict.py --mode predict_file --pretrained_model weights/nisqa.tar --deg a.wav
     python run_predict.py --mode predict_dir  --pretrained_model weights/nisqa.tar --data_dir d --bs 64
     torchrun --nproc-per-node 8 run_predict.py --mode predict_csv ...   (one rank per GPU)
+    python run_predict.py --mode predict_dir ... --output_dir out --segments   (+ out/NISQA_segments.csv)
 """
 import argparse
 
@@ -40,6 +41,9 @@ def parse_args(argv=None):
     parser = argparse.ArgumentParser(description="NISQA speech quality prediction on H100")
     for name, (typ, default, text) in _OPTIONS.items():
         parser.add_argument("--" + name, type=typ, default=default, required=name in _REQUIRED, help=text)
+    parser.add_argument("--segments", action="store_true",
+                        help="also write NISQA_segments.csv into output_dir: every segment's time span, score and "
+                             "pooling weight (single process only)")
     args = vars(parser.parse_args(argv))
 
     if args["mode"] not in _NEEDS:

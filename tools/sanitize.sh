@@ -4,7 +4,7 @@
 # short clips at 48 / 16 kHz: front-end, conv1, the five wgmma conv layers with their bulk copies /
 # mbarriers, self-attention, pooling), over a 96 kHz clip (frontend_kernel, the front end for windows over 1024
 # samples), over a short nisqa_tts.tar call (StandardCNN, BiLSTM) and over device-batch
-# calls (the ingest kernel, with and without ms_sr); racecheck over the double-ended alignment's multi-block path.
+# calls (the ingest kernel, with and without ms_sr, and one segments call); racecheck over the double-ended alignment's multi-block path.
 #   bash tools/sanitize.sh TAG
 TAG=${1:-rXX}
 OUT=gpurun_out
@@ -63,6 +63,8 @@ from nisqa_b200.scorer import Scorer
 w = torch.from_numpy(np.stack([synth.synth_speech_pcm16(12 + c, 0.7, 48000) for c in range(2)])[None]).cuda()   # [1, 2, T]
 s4 = Scorer(os.path.join("weights", "nisqa.tar"))
 print("ingest", s4(w, 48000, channel=1).tolist(), s4(w.float() / 32768, 48000).tolist())
+seg = s4.segments(w, 48000, channel=0)      # segment_scores_kernel (PoolAttFF logits of the last td_sa layer)
+print("segments", seg.counts, seg.seg_weights.sum(0).tolist())
 s4.close()
 s5 = Scorer(os.path.join("weights", "nisqa_mos_only.tar"), ms_sr=16000)
 print("ingest ms_sr", s5(w[0], 48000, lengths=[30000, w.shape[-1]]).tolist())
