@@ -296,6 +296,28 @@ NISQA_API int  nisqa_predict_device_batch_segments(nisqa_engine* e, void* cuda_s
                                                    const nisqa_segment_out* seg, int32_t* n_segments_out,
                                                    int32_t* status_out);
 
+/* Recordings of any length scored as a timeline of overlapping windows, each window scored exactly as the clip cut out of
+ * the recording would be (its own reflect padding, top_db maximum, segment count and status).  At the model rate sr
+ * (target_sr when set, else the batch's sample_rate; an ms_sr checkpoint converts each WHOLE recording first) a
+ * recording of T samples, hop = (int)(sr*hop_s) and H = hop_frames * hop:
+ *   K = 1 if T <= window, else 1 + ceil((T - window) / H) windows; window k covers samples [k H, min(k H + window, T)).
+ * Only a recording's last window can be shorter than `window`; when it is too short for one segment it scores NaN with
+ * status NISQA_CLIP_TOO_SHORT.  Refused (NISQA_ERR_INVALID): H > window, a window of more than max_segments segments or of
+ * none, a recording of more than 2^31 - 1 samples at the model rate, and double-ended engines.
+ * nisqa_window_counts: pure host arithmetic for one recording: *n_windows = K, and the first min(K, cap) windows' segment
+ * counts and statuses (either array may be NULL). */
+NISQA_API int  nisqa_window_counts(const nisqa_config* cfg, int64_t n_samples, int32_t sample_rate, int64_t window,
+                                   int32_t hop_frames, int64_t* n_windows, int32_t* n_segments, int32_t* status,
+                                   int64_t cap);
+/* nisqa_predict_device_batch for windows of the recordings of `rec` (its channel applies), with the same stream contract
+ * and no host wait of its own.  scores_dev: device [n_rows][n_out], the windows of recording b following those of the
+ * recordings before it; n_segments_out / status_out: host [windows] (may be NULL), valid on return.  A too-small n_rows is
+ * refused before anything is enqueued.  The front end packs each recording's span of a pass once and computes each mel
+ * frame pair that lies inside a window once, whatever the overlap. */
+NISQA_API int  nisqa_predict_device_windows(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* rec,
+                                            int32_t target_sr, int64_t window, int32_t hop_frames, float* scores_dev,
+                                            int64_t n_rows, int32_t* n_segments_out, int32_t* status_out);
+
 /* Copy an intermediate of the LAST predict call to host memory (parity tests).  Only valid
  * when that call fitted in one internal pass.  Returns the number of floats written (>=0)
  * or a negative status; with out == NULL returns the required count. */

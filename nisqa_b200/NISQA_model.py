@@ -13,6 +13,11 @@ or a machine without CUDA raises.
 ``args['segments']`` (``run_predict.py --segments``) also writes ``NISQA_segments.csv`` into ``output_dir``: one row per
 segment of every file with its time span, its score under each pooling head and the head's pooling weight
 (:meth:`nisqa_b200.scorer.Scorer.segments`).  Single process only.
+
+``args['window_s']`` / ``args['window_hop_s']`` (``run_predict.py --window_s S --window_hop_s S``) score every file as a
+timeline of overlapping windows instead (:meth:`nisqa_b200.scorer.Scorer.windows`): ``predict()`` returns, and writes
+to ``output_dir/NISQA_windows.csv``, one row per window with its time span, segment count and scores.  Files longer than
+``ms_max_segments`` are accepted in this mode.  Single process, single-ended checkpoints only.
 """
 import datetime
 import os
@@ -39,11 +44,22 @@ class nisqaModel(object):
         if args.get("segments") and nb_dist.env_world()[1] > 1:
             raise ValueError("segments: NISQA_segments.csv is written by a single process, not under torchrun with %d ranks"
                              % nb_dist.env_world()[1])
+        win = args.get("window_s") is not None or args.get("window_hop_s") is not None
+        if win and nb_dist.env_world()[1] > 1:
+            raise ValueError("window_s: NISQA_windows.csv is written by a single process, not under torchrun with %d ranks"
+                             % nb_dist.env_world()[1])
+        if win and (args.get("window_s") is None or args.get("window_hop_s") is None):
+            raise ValueError("window_s / window_hop_s: windows need both, got window_s=%r, window_hop_s=%r"
+                             % (args.get("window_s"), args.get("window_hop_s")))
+        if win and args.get("segments"):
+            raise ValueError("segments: per-segment rows are not written in windows mode (window_s)")
         if "mode" not in self.args:
             self.args["mode"] = "main"
         self.runinfos = {}
         self._getDevice()
         self._loadModel()
+        if win and self.args["double_ended"]:
+            raise ValueError("window_s: a double-ended (NISQA_DE) checkpoint scores (degraded, reference) pairs, not windows")
         self._loadDatasets()
         self.args["now"] = datetime.datetime.today()
 
@@ -91,6 +107,12 @@ class nisqaModel(object):
         chatty = rank == 0
         if chatty:
             print("---> Predicting ...")
+        if self.args.get("window_s") is not None:
+            df = self.predict_windows()
+            if self.args["output_dir"]:
+                df.to_csv(os.path.join(self.args["output_dir"], "NISQA_windows.csv"), index=False)
+            print(df.to_string(index=False))
+            return df
         if self.args["dim"] == True:  # noqa: E712  (mirrors the reference comparison)
             y_val_hat, y_val = NL.predict_dim(
                 self.model, self.ds_val, self.args["tr_bs_val"], self.dev,
@@ -156,6 +178,30 @@ class nisqaModel(object):
                     parts[i] = part
                     r0 += n
         return pd.concat([parts[i] for i in range(len(ds))], ignore_index=True)
+
+    def predict_windows(self):
+        """-> DataFrame with one row per window of every file, in file order: the file column, ``t_start`` / ``t_end``
+        (seconds), ``n_segments`` and each head's score (``*_pred``).  Each file is decoded by the dataset's loader and
+        scored on its own through :meth:`Scorer.windows`."""
+        from .scorer import Scorer
+        sc = Scorer.__new__(Scorer)
+        sc._configure(self.args, self.dev)
+        sc.engine = self.model
+        ds = self.ds_val
+        col = ds.filename_column
+        files = ds.df[col].tolist()
+        parts = []
+        for i in range(len(ds)):
+            y, sr = NL.read_wav(ds.file_path(i), ds.ms_channel)
+            wave, _ = self._batch_tensor([y])
+            res = sc.windows(wave, sr, self.args["window_s"], self.args["window_hop_s"])
+            s = res.scores.cpu().numpy()
+            part = pd.DataFrame({col: [files[i]] * res.counts[0], "t_start": res.t_start, "t_end": res.t_end,
+                                 "n_segments": res.n_segments})
+            for h, c in enumerate(sc.columns):
+                part[c] = s[:, h].astype(float)
+            parts.append(part)
+        return pd.concat(parts, ignore_index=True)
 
     def _batch_tensor(self, clips):
         """host clips -> ([B, T] CUDA tensor, lengths): int16 when every clip is int16, else float32"""

@@ -21,6 +21,7 @@
 #include "../../include/nisqa_b200.h"
 #include "common.cuh"
 #include "launch.cuh"
+#include "windows.cuh"
 
 using namespace nisqa;
 
@@ -123,8 +124,9 @@ struct Stage {
   HostBuf h_tables;
   DevBuf pcm, clips, prefixes, clipmax;
   DevBuf seg_row;        // segments call: each clip's first output row (int64, < 0: none)
+  DevBuf spans;          // windows call: the pass's recording spans (WinSpan)
   void release() {
-    DevBuf* all[] = {&pcm, &clips, &prefixes, &clipmax, &seg_row};
+    DevBuf* all[] = {&pcm, &clips, &prefixes, &clipmax, &seg_row, &spans};
     for (auto* b : all) b->release();
     h_tables.release();
     if (ev_copied) cudaEventDestroy(ev_copied);
@@ -382,6 +384,33 @@ void plan_clip(const nisqa_config& c, int64_t n_samples, int sr, ClipPlan* p) {
   if (c.max_segments > 0 && n_seg > c.max_segments) { p->status = NISQA_CLIP_TOO_LONG; return; }  // lib:2276-2277
   p->status = NISQA_CLIP_OK;
 }
+
+// Windows of a recording (nisqa_predict_device_windows) at the model rate sr: window `window` samples, hop `hop_frames` mel
+// frames = *H samples, so that every window starts on a mel frame of the recording.  false (the reason in *why) for a
+// geometry the checkpoint cannot score: a hop longer than the window, or a window of more than max_segments segments or
+// of none.
+bool window_geometry(const nisqa_config& c, int sr, int64_t window, int32_t hop_frames, int* H, std::string* why) {
+  if (window < 1 || window > INT32_MAX) { *why = "window = " + std::to_string(window) + ": not within 1 .. 2^31 - 1 samples"; return false; }
+  ClipPlan pl;
+  plan_clip(c, window, sr, &pl);
+  if (pl.hop < 1) { *why = "sample rate " + std::to_string(sr) + ": no mel frame hop"; return false; }
+  if (hop_frames < 1) { *why = "hop_frames = " + std::to_string(hop_frames) + ": at least one mel frame"; return false; }
+  const int64_t h = (int64_t)hop_frames * pl.hop;
+  if (h > window) {
+    *why = "hop_frames = " + std::to_string(hop_frames) + ": a window hop of " + std::to_string(h) +
+           " samples is longer than the window (" + std::to_string(window) + " samples)";
+    return false;
+  }
+  if (pl.status == NISQA_CLIP_TOO_LONG) {
+    *why = "window = " + std::to_string(window) + " samples: " + std::to_string(pl.n_seg) + " segments > max_segments " +
+           std::to_string(c.max_segments);
+    return false;
+  }
+  if (pl.status != NISQA_CLIP_OK) { *why = "window = " + std::to_string(window) + " samples: too short for one segment"; return false; }
+  *H = (int)h;
+  return true;
+}
+int64_t window_count(int64_t T, int64_t W, int64_t H) { return T <= W ? 1 : 1 + (T - W + H - 1) / H; }
 
 // ---------------------------------------------------------------- librosa.filters.mel in double
 double hz_to_mel(double f) {
@@ -1087,6 +1116,23 @@ int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
 }
 
 // ---------------------------------------------------------------- one pass over a run of clips
+// A windows call (nisqa_predict_device_windows): its windows are the clips of predict_common, in recording order
+struct WinLayout {
+  const int* rec;              // [windows] recording of each window
+  const int64_t* start;        // [windows] first sample of each window in its recording (model rate)
+  const int64_t* rec_off;      // [recordings] element offset of each converted recording in dev_pcm (ms_sr), or nullptr:
+                               // the ingest packs each pass's spans from the caller's batch
+  int H, hf, W;                // window hop (samples, mel frames) and length
+};
+// The recording spans of one pass of a windows call and the launch shape of its front end
+struct WinPass {
+  std::vector<WinSpan> spans;
+  std::vector<int64_t> pcm_off;    // each window's first sample in the pass's PCM (ClipDesc.pcm_off)
+  long long pcm_elems = 0;         // ingest: the packed spans
+  long long max_span = 0;          // the longest span
+  int edge = 0, pairs = 0, ncls = 1;
+};
+
 struct PassInput {
   int n_clips;
   const ClipPlan* plan;               // [n_clips]
@@ -1100,6 +1146,7 @@ struct PassInput {
   float* scores_dev_out;              // device destination [n_clips][n_out]
   int slot;                           // compute lane
   int stage;                          // staging slot
+  const WinPass* win;                 // windows call: the pass's spans (else nullptr)
 };
 
 int lane_allgather(nisqa_engine* e, const float* src, float* dst, size_t count, cudaStream_t st);
@@ -1127,6 +1174,7 @@ struct Pass {
   float* seg_thr = nullptr;
   int* seg_clip = nullptr;
   const long long* seg_row = nullptr;         // segments call: the clips' first output rows (staging slot)
+  const WinSpan* spans = nullptr;             // windows call: the recording spans (staging slot)
   // the rows the pooling module read (segment_rows): D real columns at a stride of ld, the attention logits the pooling
   // path wrote (or nullptr), and each head's last Linear (PoolSimpleParams.w3 / b3; a1 / a1b for PoolAtt)
   const float* pool_x = nullptr;
@@ -1167,7 +1215,8 @@ int upload_inputs(Pass& p, const PassInput& in) {
     d.n_frames = ok ? pl.n_frames : 0;
     d.n_seg = ok ? pl.n_seg : 0;
     d.frame_off = p.n_frames; d.seg_off = p.n_seg; d.pair_off = n_pairs;
-    if (in.host_pcm || in.ingest) { d.pcm_off = pcm_elems; pcm_elems += ((long long)in.n_samples[i] + 15) / 16 * 16; }
+    if (in.win) d.pcm_off = in.win->pcm_off[i];
+    else if (in.host_pcm || in.ingest) { d.pcm_off = pcm_elems; pcm_elems += ((long long)in.n_samples[i] + 15) / 16 * 16; }
     else d.pcm_off = in.dev_off[i];
     if (ok) max_run_samples = std::max<long long>(max_run_samples, in.n_samples[i]);
     pair_prefix[i] = n_pairs; seg_prefix[i] = p.n_seg; qt_prefix[i] = n_qt; qt64_prefix[i] = p.n_qt64;
@@ -1180,6 +1229,7 @@ int upload_inputs(Pass& p, const PassInput& in) {
     if (ok) { p.Q = std::max(p.Q, (pl.win + 1023) / 1024); p.max_span = std::max(p.max_span, pl.hop + pl.win); }
   }
   pair_prefix[n] = n_pairs; seg_prefix[n] = p.n_seg; qt_prefix[n] = n_qt; qt64_prefix[n] = p.n_qt64;
+  if (in.win) { pcm_elems = in.win->pcm_elems; max_run_samples = in.win->max_span; }
   for (int i = 0; i < n; ++i) by_len[i] = i;
   std::stable_sort(by_len, by_len + n, [&](int a, int b) { return cl[a].n_seg > cl[b].n_seg; });
   e->last_n_seg = p.n_seg; e->last_n_frames = p.n_frames;
@@ -1193,7 +1243,8 @@ int upload_inputs(Pass& p, const PassInput& in) {
   // one pinned block: ClipDesc[n] | the prefix arrays
   const size_t tb_clips = (size_t)n * sizeof(ClipDesc), tb_pref = pre.size() * 4;
   const size_t tb_rows_at = (tb_clips + tb_pref + 7) / 8 * 8, tb_rows = e->seg_out ? (size_t)n * 8 : 0;
-  CK(SG.h_tables.reserve(tb_rows_at + tb_rows));
+  const size_t tb_spans_at = tb_rows_at + tb_rows, tb_spans = in.win ? in.win->spans.size() * sizeof(WinSpan) : 0;
+  CK(SG.h_tables.reserve(tb_spans_at + tb_spans));
   char* ht = SG.h_tables.as<char>();
   memcpy(ht, cl.data(), tb_clips);
   memcpy(ht + tb_clips, pre.data(), tb_pref);
@@ -1202,6 +1253,12 @@ int upload_inputs(Pass& p, const PassInput& in) {
     CK(SG.seg_row.reserve(tb_rows));
     CK(cudaMemcpyAsync(SG.seg_row.p, ht + tb_rows_at, tb_rows, cudaMemcpyHostToDevice, cs));
     p.seg_row = SG.seg_row.as<long long>();
+  }
+  if (tb_spans) {     // (a windows call: the pass's recording spans)
+    memcpy(ht + tb_spans_at, in.win->spans.data(), tb_spans);
+    CK(SG.spans.reserve(tb_spans));
+    CK(cudaMemcpyAsync(SG.spans.p, ht + tb_spans_at, tb_spans, cudaMemcpyHostToDevice, cs));
+    p.spans = SG.spans.as<WinSpan>();
   }
   CK(SG.clips.reserve(tb_clips));
   CK(SG.prefixes.reserve(tb_pref));
@@ -1246,7 +1303,11 @@ int upload_inputs(Pass& p, const PassInput& in) {
     // the caller's batch -> packed mono PCM in the staging slot, on the lane (behind `ready`: the caller's stream order)
     CK(SG.pcm.reserve((size_t)pcm_elems * (in.fmt == NISQA_FMT_F32 ? 4 : 2)));
     Scope sc(e, "ingest");
-    launch_ingest(p.st, *in.ingest, in.first_clip, p.clips, n, max_run_samples, in.fmt == NISQA_FMT_F32, SG.pcm.p);
+    if (in.win)         // each recording span once, however many windows read it
+      launch_ingest_spans(p.st, in.ingest->s[0], p.spans, (int)in.win->spans.size(), max_run_samples,
+                          in.fmt == NISQA_FMT_F32, SG.pcm.p);
+    else
+      launch_ingest(p.st, *in.ingest, in.first_clip, p.clips, n, max_run_samples, in.fmt == NISQA_FMT_F32, SG.pcm.p);
     p.pcm = SG.pcm.p;
   }
   return 0;
@@ -1322,7 +1383,7 @@ int ff_layers(Pass& p, Rows* out) {
 
 // The framewise model: workspaces, front end, segment table, then the CNN (+ AdaptCNN's Linear or StandardCNN's fc_out)
 // or SkipCNN / DFF.  `out`: the rows that feed the time-dependency block (the shipped LSTM shape reads LN.feats itself).
-int framewise(Pass& p, int fmt, Rows* out) {
+int framewise(Pass& p, int fmt, Rows* out, const WinPass* win) {
   nisqa_engine* e = p.e;
   const nisqa_config& c = p.c;
   Lane& LN = p.LN;
@@ -1355,8 +1416,13 @@ int framewise(Pass& p, int fmt, Rows* out) {
   p.seg_clip = p.seg_frame0 + 2 * (size_t)n_seg;
 
   { Scope s(e, "frontend");
-    launch_frontend(p.st, c.n_mels, p.pcm, fmt == NISQA_FMT_F32, p.clips, p.n, p.max_pairs, e->fb_table.as<FbTables>(),
-                    e->tw4096.as<float2>(), LN.mel.as<float>(), p.clipmax, p.Q, p.max_span, e->fe_ppc); }
+    if (win)            // windows: each interior frame pair of a recording span once, the edge pairs per window
+      launch_frontend_windows(p.st, c.n_mels, p.pcm, fmt == NISQA_FMT_F32, p.clips, p.n, win->edge, p.spans,
+                              (int)win->spans.size(), win->pairs, win->ncls, e->fb_table.as<FbTables>(),
+                              e->tw4096.as<float2>(), LN.mel.as<float>(), p.clipmax, p.Q, p.max_span);
+    else
+      launch_frontend(p.st, c.n_mels, p.pcm, fmt == NISQA_FMT_F32, p.clips, p.n, p.max_pairs, e->fb_table.as<FbTables>(),
+                      e->tw4096.as<float2>(), LN.mel.as<float>(), p.clipmax, p.Q, p.max_span, e->fe_ppc); }
   { Scope s(e, "seg_table");
     launch_seg_table(p.st, p.clips, p.n, p.seg_prefix, p.clipmax, c.seg_hop, n_seg, p.seg_frame0, p.seg_thr, p.seg_clip); }
   e->last_conv12 = e->fused12();
@@ -1669,7 +1735,7 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
     CK(cudaMemsetAsync(p.scores, 0xFF, (size_t)p.n * p.c.n_out * 4, p.st));
   } else {
     Rows rows;
-    rc = framewise(p, in.fmt, &rows);
+    rc = framewise(p, in.fmt, &rows, in.win);
     if (!rc) rc = p.w.lstm_shipped ? lstm_head(p) : td_stages(p, rows);
     if (rc) return rc;
   }
@@ -1683,11 +1749,49 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
   return 0;
 }
 
+// The spans of windows i0 .. i1 - 1 of a windows call (one per run of windows of one recording), each window's offset in
+// the pass's PCM and the launch shape of the windows front end (launch_frontend_windows)
+void win_pass(const nisqa_config& c, const WinLayout& L, const ClipPlan* plan, const int64_t* len, int i0, int i1,
+              WinPass* w) {
+  *w = WinPass();
+  w->pcm_off.resize(i1 - i0);
+  for (int i = i0; i < i1;) {
+    const int b = L.rec[i];
+    int j = i;
+    while (j < i1 && L.rec[j] == b) ++j;
+    WinSpan s = {};
+    s.src = b; s.src_off = L.start[i];
+    s.n_samples = (int)(L.start[j - 1] + len[j - 1] - L.start[i]);
+    if (L.rec_off) s.pcm_off = L.rec_off[b] + L.start[i];
+    else { s.pcm_off = w->pcm_elems; w->pcm_elems += ((long long)s.n_samples + 15) / 16 * 16; }
+    s.clip0 = i - i0;
+    while (i + s.n_win < j && plan[i + s.n_win].run) ++s.n_win;
+    s.H = L.H; s.hf = L.hf; s.W = L.W;
+    for (int k = i; k < j; ++k) w->pcm_off[k - i0] = s.pcm_off + (L.start[k] - L.start[i]);
+    if (s.n_win > 0) {
+      const ClipPlan& pl = plan[i];
+      const int s0 = (c.n_fft - pl.win) / 2 - c.n_fft / 2;
+      const long long last = ((long long)s.n_samples - pl.hop - pl.win - s0) / pl.hop;    // last first frame of a pair
+      if (last >= 0) w->pairs = std::max(w->pairs, (int)(last / 2 + 1));
+      if (s.n_win > 1 && (s.hf & 1)) w->ncls = 2;
+      for (int k = i; k < i + s.n_win; ++k) {
+        int lead, tail;
+        interior_pairs(plan[k].n_frames, (int)len[k], s0, pl.hop, pl.win, &lead, &tail);
+        w->edge = std::max(w->edge, lead + (plan[k].n_frames + 1) / 2 - tail);
+      }
+      w->max_span = std::max<long long>(w->max_span, s.n_samples);
+    }
+    w->spans.push_back(s);
+    i = j;
+  }
+}
+
 int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, const void* dev_pcm,
                    const int64_t* dev_off, const int64_t* n_samples, const int32_t* sample_rate,
                    int fmt, float* scores_host, float* scores_dev, int32_t* n_seg_out,
                    int32_t* status_out, int sync, int64_t* ticket_out = nullptr,
-                   const IngestSources* ingest = nullptr, cudaEvent_t ready = nullptr, cudaStream_t* fin_out = nullptr) {
+                   const IngestSources* ingest = nullptr, cudaEvent_t ready = nullptr, cudaStream_t* fin_out = nullptr,
+                   const WinLayout* win = nullptr) {
   if (!e) return NISQA_ERR_INVALID;
   if (!e->weights_loaded) return fail(e, NISQA_ERR_STATE, "nisqa_load_weights has not been called");
   if (!e->conv_tc && e->conv_net() && !e->w.shipped_channels())
@@ -1738,6 +1842,7 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
   const int64_t first_pass = e->pass_counter;
   int i0 = 0;
   e->last_passes = 0;
+  WinPass wp;
   while (i0 < n_clips) {
     int i1 = i0; long long segs = 0;
     while (i1 < n_clips) {
@@ -1754,6 +1859,11 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
     in.ready = ready;
     in.fmt = fmt;
     in.scores_dev_out = scores_all + (size_t)i0 * e->cfg.n_out;
+    in.win = nullptr;
+    if (win) {
+      win_pass(e->cfg, *win, plan.data(), n_samples, i0, i1, &wp);
+      in.win = &wp;
+    }
     in.slot = e->profiling ? 0 : (int)(e->pass_counter % kLanes);
     in.stage = (int)(e->pass_counter % kStages);
     ++e->pass_counter;
@@ -1768,7 +1878,7 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
   if (n_pass == 0) fin = e->lanes[0].stream;
   for (int k = 0; k < kStages && n_pass > 1; ++k)      // passes of this call that ran on other lanes
     if (e->stages[k].busy && e->stages[k].lane != e->last_lane) CK(cudaStreamWaitEvent(fin, e->stages[k].ev_done, 0));
-  if (e->gather_dst && e->nccl_comm && n_clips == e->gather_rows && (ticket_out || scores_dev)) {
+  if (e->gather_dst && e->nccl_comm && n_clips == e->gather_rows && (ticket_out || scores_dev) && !win) {
     // the path's single exchange step, enqueued behind this call's kernels on its own lane
     int rc = lane_allgather(e, scores_all, e->gather_dst, (size_t)n_clips * e->cfg.n_out, fin);
     if (rc) return rc;
@@ -2135,6 +2245,26 @@ static int enqueue_device_batch(nisqa_engine* e, cudaStream_t caller, int n_clip
   return 0;
 }
 
+// The checks of one nisqa_device_batch argument (nm: its name in messages; ch: the channel it is read with; n_clips: the
+// clip count it must have) -> its ingest source and whether it is mixed to mono
+static int check_device_batch(nisqa_engine* e, const nisqa_device_batch& b, const std::string& nm, int ch, int n_clips,
+                              IngestSrc* src, bool* mix) {
+  if (b.sample_fmt != NISQA_FMT_S16 && b.sample_fmt != NISQA_FMT_F32) return fail(e, NISQA_ERR_INVALID, nm + "sample_fmt");
+  if (b.n_clips < 0 || b.n_clips != n_clips) return fail(e, NISQA_ERR_INVALID, nm + "n_clips");
+  if (b.n_channels < 1) return fail(e, NISQA_ERR_INVALID, nm + "n_channels");
+  if (b.n_channels > 1 && (ch < -1 || ch >= b.n_channels)) return fail(e, NISQA_ERR_INVALID, nm + "channel out of range");
+  if (b.length < 1 || b.clip_stride < 0 || b.channel_stride < 0) return fail(e, NISQA_ERR_INVALID, nm + "length / strides");
+  if (b.sample_rate <= 0) return fail(e, NISQA_ERR_INVALID, nm + "sample_rate");
+  if (b.n_clips > 0 && (!b.data || !b.n_samples)) return fail(e, NISQA_ERR_INVALID, nm + "data / n_samples: null argument");
+  for (int i = 0; i < b.n_clips; ++i)
+    if (b.n_samples[i] < 1 || b.n_samples[i] > b.length)
+      return fail(e, NISQA_ERR_INVALID, nm + "n_samples[" + std::to_string(i) + "] = " + std::to_string(b.n_samples[i]) +
+                                            ": not within 1 .. length (" + std::to_string(b.length) + ")");
+  *mix = b.n_channels > 1 && ch < 0;
+  *src = {b.data, b.clip_stride, b.channel_stride, b.n_channels, ch, b.sample_fmt == NISQA_FMT_F32 ? 1 : 0};
+  return 0;
+}
+
 // nisqa_predict_device_batch (seg == nullptr) and nisqa_predict_device_batch_segments
 static int device_batch_call(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg, const nisqa_device_batch* ref,
                              int32_t target_sr, float* scores_dev, const nisqa_segment_out* seg, int32_t* n_segments_out,
@@ -2154,19 +2284,9 @@ static int device_batch_call(nisqa_engine* e, void* cuda_stream, const nisqa_dev
     const nisqa_device_batch& b = *src[k];
     const std::string nm = k ? "ref." : "deg.";
     const int ch = k ? -1 : b.channel;        // the reference of a pair is always the mono mix
-    if (b.sample_fmt != NISQA_FMT_S16 && b.sample_fmt != NISQA_FMT_F32) return fail(e, NISQA_ERR_INVALID, nm + "sample_fmt");
-    if (b.n_clips < 0 || b.n_clips != deg->n_clips) return fail(e, NISQA_ERR_INVALID, nm + "n_clips");
-    if (b.n_channels < 1) return fail(e, NISQA_ERR_INVALID, nm + "n_channels");
-    if (b.n_channels > 1 && (ch < -1 || ch >= b.n_channels)) return fail(e, NISQA_ERR_INVALID, nm + "channel out of range");
-    if (b.length < 1 || b.clip_stride < 0 || b.channel_stride < 0) return fail(e, NISQA_ERR_INVALID, nm + "length / strides");
-    if (b.sample_rate <= 0) return fail(e, NISQA_ERR_INVALID, nm + "sample_rate");
-    if (b.n_clips > 0 && (!b.data || !b.n_samples)) return fail(e, NISQA_ERR_INVALID, nm + "data / n_samples: null argument");
-    for (int i = 0; i < b.n_clips; ++i)
-      if (b.n_samples[i] < 1 || b.n_samples[i] > b.length)
-        return fail(e, NISQA_ERR_INVALID, nm + "n_samples[" + std::to_string(i) + "] = " + std::to_string(b.n_samples[i]) +
-                                              ": not within 1 .. length (" + std::to_string(b.length) + ")");
-    const bool mix = b.n_channels > 1 && ch < 0;
-    ing.s[k] = {b.data, b.clip_stride, b.channel_stride, b.n_channels, ch, b.sample_fmt == NISQA_FMT_F32 ? 1 : 0};
+    bool mix = false;
+    const int rc = check_device_batch(e, b, nm, ch, deg->n_clips, &ing.s[k], &mix);
+    if (rc) return rc;
     out_f32 = out_f32 || b.sample_fmt == NISQA_FMT_F32 || mix;
   }
   const int n_clips = deg->n_clips * n_src;
@@ -2221,6 +2341,105 @@ int nisqa_predict_device_batch_segments(nisqa_engine* e, void* cuda_stream, cons
                                         const nisqa_segment_out* seg, int32_t* n_segments_out, int32_t* status_out) {
   if (e && !seg) return fail(e, NISQA_ERR_INVALID, "seg: null argument");
   return device_batch_call(e, cuda_stream, deg, ref, target_sr, scores_dev, seg, n_segments_out, status_out);
+}
+
+int nisqa_predict_device_windows(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* rec, int32_t target_sr,
+                                 int64_t window, int32_t hop_frames, float* scores_dev, int64_t n_rows,
+                                 int32_t* n_segments_out, int32_t* status_out) {
+  if (!e) return NISQA_ERR_INVALID;
+  if (!e->stream) return fail(e, NISQA_ERR_STATE, "engine was not created successfully");
+  if (e->cfg.double_ended)
+    return fail(e, NISQA_ERR_INVALID, "a double-ended (NISQA_DE) engine scores (degraded, reference) pairs, not windows of a recording");
+  if (!rec) return fail(e, NISQA_ERR_INVALID, "rec: null argument");
+  if (target_sr < 0) return fail(e, NISQA_ERR_INVALID, "target_sr");
+  IngestSources ing = {};
+  ing.n_src = 1;
+  bool mix = false;
+  int rc = check_device_batch(e, *rec, "rec.", rec->channel, rec->n_clips, &ing.s[0], &mix);
+  if (rc) return rc;
+  const int fmt = rec->sample_fmt == NISQA_FMT_F32 || mix ? NISQA_FMT_F32 : NISQA_FMT_S16;
+  const int rate = target_sr > 0 ? target_sr : rec->sample_rate;
+  std::string why;
+  int H = 0;
+  if (!window_geometry(e->cfg, rate, window, hop_frames, &H, &why)) return fail(e, NISQA_ERR_INVALID, why);
+  const int W = (int)window;
+  // the windows of every recording, in recording order (host arithmetic: nisqa_window_counts)
+  const int n_rec = rec->n_clips;
+  std::vector<int> wrec;
+  std::vector<int64_t> start, len;
+  for (int b = 0; b < n_rec; ++b) {
+    const int64_t T = target_sr > 0 ? nisqa_resample_out_len(rec->n_samples[b], rec->sample_rate, target_sr) : rec->n_samples[b];
+    if (T > (int64_t)INT32_MAX)
+      return fail(e, NISQA_ERR_INVALID, "rec.n_samples[" + std::to_string(b) + "]: " + std::to_string(T) +
+                                            " samples at the model rate, more than 2^31 - 1");
+    const int64_t K = window_count(T, W, H);
+    if ((int64_t)wrec.size() + K > INT32_MAX) return fail(e, NISQA_ERR_INVALID, "rec: more than 2^31 - 1 windows");
+    for (int64_t k = 0; k < K; ++k) {
+      wrec.push_back(b);
+      start.push_back(k * H);
+      len.push_back(std::min<int64_t>(W, T - k * H));
+    }
+  }
+  const int N = (int)wrec.size();
+  if (n_rows < N)
+    return fail(e, NISQA_ERR_INVALID, "n_rows = " + std::to_string(n_rows) + ": the call has " + std::to_string(N) + " windows");
+  if (N > 0 && !scores_dev) return fail(e, NISQA_ERR_INVALID, "scores_dev: null argument");
+  CK(cudaSetDevice(e->device));
+  cudaStream_t caller = static_cast<cudaStream_t>(cuda_stream);
+  std::vector<int32_t> srs(N, rate);
+  const int hop = (int)((double)rate * e->cfg.hop_s);
+  WinLayout L = {wrec.data(), start.data(), nullptr, H, H / hop, W};
+  RsSlot* S = nullptr;
+  cudaStream_t fin = nullptr;
+  CK(cudaEventRecord(e->ev_in, caller));
+  if (target_sr > 0) {
+    // the whole recording converted first (a span converted alone differs at its edges); every pass waits for `ready`
+    cudaStream_t st = e->lanes[e->profiling ? 0 : (int)(e->pass_counter % kLanes)].stream;
+    CK(cudaStreamWaitEvent(st, e->ev_in, 0));
+    std::vector<int32_t> rsr(n_rec, rec->sample_rate);
+    std::vector<int64_t> offs, n_fix;
+    rc = resample_to_device(e, st, n_rec, nullptr, &ing, rec->n_samples, rsr.data(), fmt, target_sr, &offs, &n_fix, &S);
+    if (!rc) {
+      L.rec_off = offs.data();
+      CK(cudaEventRecord(S->ready, st));
+      rc = predict_common(e, N, nullptr, S->out.p, nullptr, len.data(), srs.data(), NISQA_FMT_F32, nullptr, scores_dev,
+                          n_segments_out, status_out, 0, nullptr, nullptr, S->ready, &fin, &L);
+    }
+    if (!rc) {
+      CK(cudaEventRecord(S->done, fin));
+      S->busy = N > 0;
+    }
+  } else {
+    rc = predict_common(e, N, nullptr, nullptr, nullptr, len.data(), srs.data(), fmt, nullptr, scores_dev, n_segments_out,
+                        status_out, 0, nullptr, &ing, e->ev_in, &fin, &L);
+  }
+  if (!rc) {
+    CK(cudaEventRecord(e->ev_out, fin));
+    CK(cudaStreamWaitEvent(caller, e->ev_out, 0));
+    return 0;
+  }
+  // (as device_batch_call: whatever was enqueued may still read the input or the conversion slot)
+  for (auto& l : e->lanes)
+    if (cudaEventRecord(e->ev_out, l.stream) == cudaSuccess) cudaStreamWaitEvent(caller, e->ev_out, 0);
+  if (S && cudaEventRecord(S->done, caller) == cudaSuccess) S->busy = true;
+  return rc;
+}
+
+int nisqa_window_counts(const nisqa_config* cfg, int64_t n_samples, int32_t sample_rate, int64_t window, int32_t hop_frames,
+                        int64_t* n_windows, int32_t* n_segments, int32_t* status, int64_t cap) {
+  if (!cfg || n_samples < 1) return NISQA_ERR_INVALID;
+  std::string why;
+  int H = 0;
+  if (!window_geometry(*cfg, sample_rate, window, hop_frames, &H, &why)) return NISQA_ERR_INVALID;
+  const int64_t K = window_count(n_samples, window, H);
+  if (n_windows) *n_windows = K;
+  for (int64_t k = 0; k < std::min(K, cap); ++k) {
+    ClipPlan p;
+    plan_clip(*cfg, std::min<int64_t>(window, n_samples - k * H), sample_rate, &p);
+    if (n_segments) n_segments[k] = p.n_seg;
+    if (status) status[k] = p.status;
+  }
+  return 0;
 }
 
 int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {

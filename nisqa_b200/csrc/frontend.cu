@@ -14,6 +14,7 @@
 #include "common.cuh"
 #include "f32x2.cuh"
 #include "launch.cuh"
+#include "windows.cuh"
 
 namespace nisqa {
 
@@ -510,6 +511,166 @@ frontend_pp_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips
   if (lane == 0 && wmax > -INFINITY) atomicMax(clipmax + c, f2key(wmax));
 }
 
+// ---- windows of a recording (nisqa_predict_device_windows) -----------------------------------------------------------
+// Every window is a clip of the pass: its own ClipDesc, mel rows and clip max, so everything behind the front end runs
+// as for clips.  A frame pair of a window whose taps all lie inside the window (no reflect padding) reads the same
+// samples, paired the same way, in every window that holds it at an even local frame: it is computed ONCE per recording
+// span (`shared` launch) and its mel rows are stored into each such window, with an atomic max on that window's key.
+// The other pairs - the first and last one or two of each window - are computed per window over its own bounds (edge
+// launch).  Both run the arithmetic of the kernel the clip path picks for the pass (PP: frontend_pp_kernel's input stage,
+// mag_stage and mel_bands_staged; else frontend_kernel's input stage and mel_bands) through the same device functions
+// in the same order, so every row is bit for bit the row of the window cut out and scored as a clip.  (Two real frames
+// share one complex transform, so a frame's row depends on its partner: a pair is shared only between windows whose
+// local frame parity agrees.  Beyond the window the weight of a tap is zero: the clip kernels' values there add zeros.)
+template <typename T, int MELS, bool PP>
+__device__ __forceinline__ float win_pair(const T* __restrict__ y, int n, int a, int hop, int win, bool validB,
+                                          const FbTables& fb, const int* band_meta, const float2* __restrict__ tw1,
+                                          const float4* __restrict__ tw2_end, float2* zin, float2* scratch, int Q,
+                                          float* srow) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, r = warp;
+  if constexpr (PP) {
+    const int hopB = validB ? hop : 0;
+    const float2* wtab = fb.wtab + r * 1024 + lane;
+    f2 x[32];
+    constexpr int CH = 4;
+#pragma unroll
+    for (int j0 = 0; j0 < 32; j0 += CH) {
+      float2 wt[CH];
+      float sa[CH], sb[CH];
+#pragma unroll
+      for (int u = 0; u < CH; ++u) {
+        const int k = lane + 32 * (j0 + u);
+        wt[u] = __ldg(wtab + 32 * (j0 + u));
+        sa[u] = 0.f; sb[u] = 0.f;
+        if (k < win) {
+          sa[u] = (float)y[reflect_index(a + k, n)];
+          sb[u] = (float)y[reflect_index(a + k + hopB, n)];
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < CH; ++u)
+        x[rev5(j0 + u)] = pk(fmaf(sa[u], wt[u].x, -(sb[u] * wt[u].y)), fmaf(sa[u], wt[u].y, sb[u] * wt[u].x));
+    }
+    fft1024_plane(x, scratch + r * kScratchPerWarp, lane, tw2_end);
+    __syncthreads();
+    mag_stage(scratch, fb.n_mag, tid);
+    __syncthreads();
+    return mel_bands_staged<MELS>(scratch, band_meta, fb.weights, warp, lane, validB,
+                                  sizeof(T) == 2 ? 9.313225746154785e-10f : 1.0f, srow);
+  } else {
+    for (int q0 = 0; q0 < Q; ++q0) {
+      float wv[8], sa[8], sb[8];
+      const int ia0 = a + q0 * 1024 + tid;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int k = q0 * 1024 + tid + i * kFeThreads;
+        wv[i] = 0.f; sa[i] = 0.f; sb[i] = 0.f;
+        if (k < win) {
+          wv[i] = __ldg(fb.window + k);
+          const int ia = ia0 + i * kFeThreads;
+          sa[i] = sample_to_float<T>(y[reflect_index(ia, n)]);
+          if (validB) sb[i] = sample_to_float<T>(y[reflect_index(ia + hop, n)]);
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+        zin[q0 * 1024 + tid + i * kFeThreads] = make_float2(wv[i] * sa[i], wv[i] * sb[i]);
+    }
+    __syncthreads();
+    {
+      f2 x[32];
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const int k = lane + 32 * j;
+        float2 v = zin[k];
+        for (int q = 1; q < Q; ++q) {
+          const float2 u = zin[k + 1024 * q];
+          switch ((r * q) & 3) {
+            case 0: v.x += u.x; v.y += u.y; break;
+            case 1: v.x += u.y; v.y -= u.x; break;
+            case 2: v.x -= u.x; v.y -= u.y; break;
+            default: v.x -= u.y; v.y += u.x; break;
+          }
+        }
+        if (r != 0) v = cmul(v, __ldg(tw1 + ((r - 1) * 32 + j) * 32 + lane));
+        x[rev5(j)] = pk(v);
+      }
+      fft1024_plane(x, scratch + r * kScratchPerWarp, lane, tw2_end);
+    }
+    __syncthreads();
+    return mel_bands<MELS>(scratch, band_meta, fb.weights, warp, lane, validB, srow);
+  }
+}
+
+// shared == 0: grid (edge pair slot, window); shared == 1: grid (pair of a span, span * ncls + parity class)
+template <typename T, int MELS, bool PP>
+__global__ void __launch_bounds__(kFeThreads, 4)
+frontend_windows_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips, const WinSpan* __restrict__ spans,
+                        int shared, int ncls, const FbTables* __restrict__ fbs, const float2* __restrict__ tw1,
+                        const float4* __restrict__ tw2_end, float* __restrict__ mel, unsigned* __restrict__ clipmax,
+                        int Q) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  float2* zin = reinterpret_cast<float2*>(smem_raw);                                      // (generic arithmetic only)
+  float2* scratch = reinterpret_cast<float2*>(smem_raw + (PP ? 0 : fe_region0_bytes(Q)));
+  __shared__ int band_meta[2 * MELS + 1];
+  __shared__ __align__(16) float srow[2 * MELS];                                          // the pair's two mel rows
+  __shared__ float wred[kFeThreads / 32];
+  const int tid = threadIdx.x;
+  // the pair: samples y reflected over [0, n), first tap a; its rows go to the windows c0, c0 + cstep, ... (n_dst of
+  // them), at local frame f0, f0 - fstep, ...
+  const T* y;
+  int n, a, c0, n_dst, cstep, f0, fstep;
+  bool validB;
+  ClipDesc cd;
+  if (shared) {
+    const WinSpan sp = spans[blockIdx.y / ncls];
+    const int cls = blockIdx.y % ncls;             // pairs that start at even (0) or odd (1) frames of the span
+    if (sp.n_win <= 0) return;
+    cd = clips[sp.clip0];
+    const int jA = 2 * blockIdx.x + cls, g = cd.s0 + jA * cd.hop, ext = cd.hop + cd.win;
+    if (g < 0 || g + ext > sp.n_samples) return;
+    // window i holds the pair as an interior pair iff i H <= g and g + ext <= i H + W
+    const int i_hi = min(g / sp.H, sp.n_win - 1);
+    int i_lo = g + ext - sp.W <= 0 ? 0 : (g + ext - sp.W + sp.H - 1) / sp.H;
+    cstep = 1;
+    if (sp.hf & 1) {                               // window i pairs the span's frames from parity (i hf) & 1 = i & 1
+      cstep = 2;
+      if ((i_lo & 1) != cls) ++i_lo;
+    }
+    if (i_lo > i_hi) return;
+    n_dst = (i_hi - i_lo) / cstep + 1;
+    c0 = sp.clip0 + i_lo; f0 = jA - i_lo * sp.hf; fstep = cstep * sp.hf;
+    y = pcm + sp.pcm_off; n = sp.n_samples; a = g; validB = true;
+  } else {
+    c0 = blockIdx.y;
+    cd = clips[c0];
+    if (cd.n_frames <= 0) return;
+    int lead, tail;
+    interior_pairs(cd.n_frames, cd.n_samples, cd.s0, cd.hop, cd.win, &lead, &tail);
+    const int s = blockIdx.x, p = s < lead ? s : tail + (s - lead);
+    if (p >= (cd.n_frames + 1) >> 1) return;
+    n_dst = 1; cstep = 0; f0 = 2 * p; fstep = 0;
+    y = pcm + cd.pcm_off; n = cd.n_samples; a = cd.s0 + 2 * p * cd.hop; validB = 2 * p + 1 < cd.n_frames;
+  }
+  const FbTables fb = fbs[cd.fb_id];
+  load_band_meta<MELS>(band_meta, fb, tid);
+  const float v = warp_max(win_pair<T, MELS, PP>(y, n, a, cd.hop, cd.win, validB, fb, band_meta, tw1, tw2_end, zin,
+                                                 scratch, Q, srow));
+  if ((tid & 31) == 0) wred[tid >> 5] = v;
+  __syncthreads();                                 // srow and wred complete
+  const float m = fmaxf(fmaxf(wred[0], wred[1]), fmaxf(wred[2], wred[3]));
+  // fan-out: the pair's rows as 16-byte stores into every window that holds it, then each window's clip max
+  const int q4 = (validB ? 2 : 1) * MELS / 4;
+  const float4* s4 = reinterpret_cast<const float4*>(srow);
+  for (int i = tid; i < n_dst * q4; i += kFeThreads) {
+    const int d = i / q4, u = i - d * q4;
+    float4* dst = reinterpret_cast<float4*>(mel + (size_t)(clips[c0 + d * cstep].frame_off + f0 - d * fstep) * MELS);
+    dst[u] = s4[u];
+  }
+  if (m > -INFINITY)
+    for (int d = tid; d < n_dst; d += kFeThreads) atomicMax(clipmax + c0 + d * cstep, f2key(m));
+}
+
 // Per-segment lookup rows, built once per pass after the front-end:
 //   seg_frame0[s] = first mel row of segment s,  seg_thr[s] = clipmax(clip) - 80  (top_db)
 __global__ void seg_table_kernel(const ClipDesc* __restrict__ clips, int n_clips,
@@ -577,6 +738,52 @@ static void launch_frontend_mels(cudaStream_t st, const void* pcm, int fmt_f32, 
   } else {
     frontend_kernel<short, MELS><<<grid, kFeThreads, smem, st>>>(
         (const short*)pcm, clips, n_clips, fbs, tw1, tw2_end, mel, clipmax, Q);
+  }
+}
+
+template <typename T, int MELS, bool PP>
+static void launch_frontend_windows_t(cudaStream_t st, const T* pcm, const ClipDesc* clips, int n_clips, int edge_pairs,
+                                      const WinSpan* spans, int n_spans, int span_pairs, int ncls, const FbTables* fbs,
+                                      const float2* tw, float* mel, unsigned* clipmax, int Q) {
+  const float4* tw2_end = reinterpret_cast<const float4*>(tw + 4 * 1024);
+  const int smem = PP ? 4 * kScratchPerWarp * 8 : frontend_smem_bytes(Q);
+  if (!PP) {
+    static unsigned long long configured = 0;
+    if (first_launch_on_device(configured))
+      cudaFuncSetAttribute(frontend_windows_kernel<T, MELS, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           frontend_smem_bytes(4));
+  }
+  if (edge_pairs > 0 && n_clips > 0)
+    frontend_windows_kernel<T, MELS, PP><<<dim3(edge_pairs, n_clips), kFeThreads, smem, st>>>(
+        pcm, clips, spans, 0, 1, fbs, tw, tw2_end, mel, clipmax, Q);
+  if (span_pairs > 0 && n_spans > 0)
+    frontend_windows_kernel<T, MELS, PP><<<dim3(span_pairs, n_spans * ncls), kFeThreads, smem, st>>>(
+        pcm, clips, spans, 1, ncls, fbs, tw, tw2_end, mel, clipmax, Q);
+}
+
+template <int MELS>
+static void launch_frontend_windows_mels(cudaStream_t st, const void* pcm, int fmt_f32, const ClipDesc* clips, int n_clips,
+                                         int edge_pairs, const WinSpan* spans, int n_spans, int span_pairs, int ncls,
+                                         const FbTables* fbs, const float2* tw, float* mel, unsigned* clipmax, int Q,
+                                         int max_span) {
+  const bool pp = Q == 1 && max_span <= kSpanMax;        // the clip path's choice (launch_frontend_mels)
+#define FE_WIN(T, PP) launch_frontend_windows_t<T, MELS, PP>(st, (const T*)pcm, clips, n_clips, edge_pairs, spans, n_spans, \
+                                                             span_pairs, ncls, fbs, tw, mel, clipmax, Q)
+  if (fmt_f32) { if (pp) FE_WIN(float, true); else FE_WIN(float, false); }
+  else { if (pp) FE_WIN(short, true); else FE_WIN(short, false); }
+#undef FE_WIN
+}
+
+void launch_frontend_windows(cudaStream_t st, int n_mels, const void* pcm, int fmt_f32, const ClipDesc* clips, int n_clips,
+                             int edge_pairs, const WinSpan* spans, int n_spans, int span_pairs, int ncls,
+                             const FbTables* fbs, const float2* tw, float* mel, unsigned* clipmax, int Q, int max_span) {
+  switch (n_mels) {
+#define FE_MELS_CASE(M) \
+    case M: launch_frontend_windows_mels<M>(st, pcm, fmt_f32, clips, n_clips, edge_pairs, spans, n_spans, span_pairs, ncls, \
+                                            fbs, tw, mel, clipmax, Q, max_span); break;
+    FE_MELS_CASE(32) FE_MELS_CASE(40) FE_MELS_CASE(48) FE_MELS_CASE(64) FE_MELS_CASE(80) FE_MELS_CASE(96) FE_MELS_CASE(128)
+#undef FE_MELS_CASE
+    default: break;
   }
 }
 

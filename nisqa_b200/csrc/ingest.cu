@@ -8,6 +8,7 @@
 
 #include "common.cuh"
 #include "launch.cuh"
+#include "windows.cuh"
 
 namespace nisqa {
 
@@ -71,6 +72,30 @@ static void launch_ingest_rows(cudaStream_t st, const IngestSources& src, int fi
   const long long per_block = (long long)kIngestThreads * kIngestPerThread;
   const dim3 grid((unsigned)std::min<long long>((max_n + per_block - 1) / per_block, 4096), n_clips);
   ingest_kernel<Row><<<grid, kIngestThreads, 0, st>>>(src, first_clip, rows, out_f32, out);
+}
+
+// nisqa_predict_device_windows: each recording span of a pass packed once, however many windows read it; grid (sample
+// blocks, spans)
+__global__ void __launch_bounds__(kIngestThreads)
+ingest_span_kernel(IngestSrc s, const WinSpan* __restrict__ spans, int out_f32, void* __restrict__ out) {
+  const WinSpan sp = spans[blockIdx.y];
+  if (sp.n_win <= 0) return;             // (no window of the span runs)
+  s.data = static_cast<const char*>(s.data) + sp.src_off * (s.f32 ? 4 : 2);
+  if (out_f32) {
+    float* y = static_cast<float*>(out) + sp.pcm_off;
+    if (s.f32) ingest_clip<float, float>(s, sp.src, sp.n_samples, y);
+    else ingest_clip<short, float>(s, sp.src, sp.n_samples, y);
+  } else {
+    ingest_clip<short, short>(s, sp.src, sp.n_samples, static_cast<short*>(out) + sp.pcm_off);
+  }
+}
+
+void launch_ingest_spans(cudaStream_t st, const IngestSrc& src, const WinSpan* spans, int n_spans, long long max_n,
+                         int out_f32, void* out) {
+  if (n_spans <= 0 || max_n <= 0) return;
+  const long long per_block = (long long)kIngestThreads * kIngestPerThread;
+  const dim3 grid((unsigned)std::min<long long>((max_n + per_block - 1) / per_block, 4096), n_spans);
+  ingest_span_kernel<<<grid, kIngestThreads, 0, st>>>(src, spans, out_f32, out);
 }
 
 void launch_ingest(cudaStream_t st, const IngestSources& src, int first_clip, const ClipDesc* clips, int n_clips,

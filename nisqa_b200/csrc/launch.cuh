@@ -12,6 +12,7 @@ namespace nisqa {
 
 struct ClipDesc;
 struct FbTables;
+struct WinSpan;
 
 // AdaptCNN's adaptive max-pool output sizes cnn_pool_1 / 2 / 3 as h1 w1 h2 w2 h3 w3 (lib:586-710), shipped 24 x 7, 12 x 5,
 // 6 x 3.  The tensor-core kernels take any [h, w] with w <= kMaxPoolW and (h + 1) (w + 1) <= kMaxPoolCells (one
@@ -105,6 +106,13 @@ struct ResampleClip {
 bool frontend_supports_mels(int n_mels);
 void launch_frontend(cudaStream_t st, int n_mels, const void* pcm, int fmt_f32, const ClipDesc* clips, int n_clips, int max_pairs,
                      const FbTables* fbs, const float2* tw, float* mel, unsigned* clipmax, int Q, int max_span, int ppc);
+// Windows of recordings (WinSpan rows; every window is also a ClipDesc row): the edge pairs of every window (grid
+// edge_pairs x n_clips) and the interior pairs of every span once (grid span_pairs x n_spans * ncls; ncls 2 when the
+// window hop is an odd number of frames), each stored into every window that holds it.  Rows bit-identical to
+// launch_frontend over the windows as clips.
+void launch_frontend_windows(cudaStream_t st, int n_mels, const void* pcm, int fmt_f32, const ClipDesc* clips, int n_clips,
+                             int edge_pairs, const WinSpan* spans, int n_spans, int span_pairs, int ncls,
+                             const FbTables* fbs, const float2* tw, float* mel, unsigned* clipmax, int Q, int max_span);
 void launch_seg_table(cudaStream_t st, const ClipDesc* clips, int n_clips, const int* seg_prefix, const unsigned* clipmax,
                       int seg_hop, int n_seg, int* seg_frame0, float* seg_thr, int* seg_clip);
 void launch_mel_dump(cudaStream_t st, const float* mel, const ClipDesc* clips, int n_clips, const unsigned* clipmax, int n_mels,
@@ -220,6 +228,10 @@ void launch_ingest(cudaStream_t st, const IngestSources& src, int first_clip, co
                    long long max_n, int out_f32, void* out);
 void launch_ingest(cudaStream_t st, const IngestSources& src, int first_clip, const ResampleClip* clips, int n_clips,
                    long long max_n, int out_f32, void* out);
+// nisqa_predict_device_windows: samples src_off .. src_off + n_samples - 1 of recording `src` of the batch to pcm_off, once
+// per span (max_n: the longest span)
+void launch_ingest_spans(cudaStream_t st, const IngestSrc& src, const WinSpan* spans, int n_spans, long long max_n,
+                         int out_f32, void* out);
 
 // ---------------------------------------------------------------- resample.cpp
 // the interpolation table of the resampler (set by nisqa_resample_set_filter); false before that call

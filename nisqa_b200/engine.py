@@ -39,7 +39,7 @@ EXPORTS = [
     "nisqa_wav_probe", "nisqa_wav_decode", "nisqa_wav_probe_batch", "nisqa_wav_decode_batch",
     "nisqa_resample_set_filter", "nisqa_resample_out_len", "nisqa_resample_f32",
     "nisqa_resample_device", "nisqa_predict_pcm_resampled", "nisqa_set_cnn_pools", "nisqa_predict_device_batch",
-    "nisqa_predict_device_batch_segments",
+    "nisqa_predict_device_batch_segments", "nisqa_window_counts", "nisqa_predict_device_windows",
 ]
 
 
@@ -243,6 +243,11 @@ def load_library(path=None):
     lib.nisqa_predict_device_batch.restype = C.c_int
     lib.nisqa_predict_device_batch_segments.argtypes = [vp, vp, dbp, dbp, C.c_int32, vp, C.POINTER(NisqaSegmentOut), i32p, i32p]
     lib.nisqa_predict_device_batch_segments.restype = C.c_int
+    lib.nisqa_predict_device_windows.argtypes = [vp, vp, dbp, C.c_int32, C.c_int64, C.c_int32, vp, C.c_int64, i32p, i32p]
+    lib.nisqa_predict_device_windows.restype = C.c_int
+    lib.nisqa_window_counts.argtypes = [C.POINTER(NisqaConfig), C.c_int64, C.c_int32, C.c_int64, C.c_int32, i64p, i32p, i32p,
+                                        C.c_int64]
+    lib.nisqa_window_counts.restype = C.c_int
     lib.nisqa_stage_dump.argtypes = [vp, C.c_int, f32p, C.c_int64]
     lib.nisqa_stage_dump.restype = C.c_int64
     lib.nisqa_segment_counts.argtypes = [C.POINTER(NisqaConfig), C.c_int64, C.c_int32, i32p, i32p, i32p]
@@ -480,6 +485,22 @@ def segment_counts(cfg, n_samples, sample_rate):
     return a.value, b.value, c.value
 
 
+def window_counts(cfg, n_samples, sample_rate, window, hop_frames):
+    """(n_segments int32[K], status int32[K]) of the K windows of a recording of ``n_samples`` samples at the model rate
+    ``sample_rate``: ``window`` samples, a hop of ``hop_frames`` mel frames (nisqa_window_counts, host arithmetic)"""
+    lib = load_library()
+    k = C.c_int64()
+    args = (C.byref(cfg), int(n_samples), int(sample_rate), int(window), int(hop_frames), C.byref(k))
+    rc = lib.nisqa_window_counts(*args, None, None, 0)
+    if rc != 0:
+        raise EngineError("nisqa_window_counts failed (%d): window %d, hop_frames %d at %d Hz" % (rc, window, hop_frames,
+                                                                                                  sample_rate))
+    nseg, status = np.empty(k.value, np.int32), np.empty(k.value, np.int32)
+    lib.nisqa_window_counts(*args, nseg.ctypes.data_as(C.POINTER(C.c_int32)), status.ctypes.data_as(C.POINTER(C.c_int32)),
+                            k.value)
+    return nseg, status
+
+
 class Engine(object):
     """One engine per GPU (rank)."""
 
@@ -710,6 +731,22 @@ class Engine(object):
         with nothing enqueued, when ``n_rows`` is too small."""
         seg = NisqaSegmentOut(scores=seg_scores_ptr or None, weights=seg_weights_ptr or None, n_rows=int(n_rows))
         return self._device_batch(stream, deg, scores_dev_ptr, ref, target_sr, seg)
+
+    def predict_device_windows(self, stream, rec, scores_dev_ptr, n_rows, window, hop_frames, target_sr=0):
+        """Windows of the recordings ``rec`` (a :func:`device_batch` tuple) ordered on ``stream``: ``window`` samples and a
+        hop of ``hop_frames`` mel frames at the model rate (``target_sr``, else the batch's rate), the scores of every
+        window to ``scores_dev_ptr`` ([n_rows, n_out] fp32 device memory, recording after recording).  Returns (n_segments,
+        status) int32[windows], valid on return; raises EngineError, with nothing enqueued, for a refused call."""
+        if target_sr:
+            from . import resample as _rs
+            _rs.out_len(1, 1, 1)                                      # the interpolation table is set once
+        n = max(int(n_rows), 0)
+        nseg, status = np.empty(n, dtype=np.int32), np.empty(n, dtype=np.int32)
+        self._check(self.lib.nisqa_predict_device_windows(
+            self.h, C.c_void_p(stream or None), C.byref(rec[0]), int(target_sr or 0), int(window), int(hop_frames),
+            C.c_void_p(scores_dev_ptr), int(n_rows), nseg.ctypes.data_as(C.POINTER(C.c_int32)),
+            status.ctypes.data_as(C.POINTER(C.c_int32))), "nisqa_predict_device_windows")
+        return nseg, status
 
     def _device_batch(self, stream, deg, scores_dev_ptr, ref, target_sr, seg):
         rows = deg[0].n_clips * (2 if ref is not None else 1)

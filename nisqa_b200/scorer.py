@@ -10,6 +10,9 @@ the GPU: ``wave`` may be freed or reused in stream order as soon as the call ret
 
 ``scorer.segments(wave, 48000)`` also returns where in each clip the quality drops: every segment's score and pooling
 weight (``nisqa_predict_device_batch_segments``) with its time span.
+
+``scorer.windows(wave, 48000, 10.0, 1.0)`` scores recordings of any length as a timeline: every 10 s window at a 1 s hop,
+each scored as the clip cut out of the recording would be (``nisqa_predict_device_windows``).
 """
 import collections
 import numbers
@@ -25,6 +28,34 @@ DIM_COLUMNS = ["mos_pred", "noi_pred", "dis_pred", "col_pred", "loud_pred"]     
 # Scorer.segments: scores [B, n_cols] (as Scorer.__call__), seg_scores / seg_weights [N, n_cols] CUDA tensors (the rows of
 # clip b follow those of the clips before it, counts[b] of them), t_start / t_end float64 [N] seconds
 Segments = collections.namedtuple("Segments", ["scores", "seg_scores", "seg_weights", "counts", "t_start", "t_end"])
+# Scorer.windows: scores [N, n_cols] CUDA tensor (the windows of recording b follow those of the recordings before it,
+# counts[b] of them); t_start / t_end float64 [N] seconds, n_segments / status int32 [N] host arrays
+Windows = collections.namedtuple("Windows", ["scores", "counts", "t_start", "t_end", "n_segments", "status"])
+
+
+def window_geometry(args, rate, window_s, window_hop_s):
+    """(W, hop_frames) of windows of ``window_s`` seconds at a hop of ``window_hop_s`` seconds at the model rate ``rate``:
+    W = round(window_s rate) samples, a hop of max(1, round(window_hop_s rate / hop)) mel frames of hop = int(rate
+    ms_hop_length) samples, so that every window starts on a mel frame of the recording"""
+    for name, v in (("window_s", window_s), ("window_hop_s", window_hop_s)):
+        if isinstance(v, bool) or not isinstance(v, numbers.Real) or not np.isfinite(v) or v <= 0:
+            raise ValueError("%s: a positive number of seconds, not %r" % (name, v))
+    hop = int(rate * args["ms_hop_length"])
+    W = int(round(window_s * rate))
+    hop_frames = max(1, int(round(window_hop_s * rate / hop)))
+    if W < 1:
+        raise ValueError("window_s=%r: no sample at %d Hz" % (window_s, rate))
+    if hop_frames * hop > W:
+        raise ValueError("window_hop_s=%r: a hop of %d samples (%d mel frames of %d) is longer than the window of %d samples "
+                         "(window_s=%r) at %d Hz" % (window_hop_s, hop_frames * hop, hop_frames, hop, W, window_s, rate))
+    return W, hop_frames
+
+
+def window_times(T, W, H, rate):
+    """(t_start, t_end) in seconds of the windows of a recording of T samples at the model rate"""
+    K = 1 if T <= W else 1 + -(-(T - W) // H)
+    k = np.arange(K, dtype=np.int64)
+    return k * H / rate, np.minimum(k * H + W, T) / rate
 
 
 class Scorer(object):
@@ -102,6 +133,49 @@ class Scorer(object):
         t_start = t * a["ms_seg_hop_length"] * hop / rate
         t_end = (t * a["ms_seg_hop_length"] + a["ms_seg_length"] - 1) * hop / rate
         return Segments(self._clip_rows(out, ref), seg_s, seg_w, list(counts), t_start, t_end)
+
+    def windows(self, wave, sample_rate, window_s, window_hop_s, lengths=None, channel=None):
+        """Every recording of a batch scored as a timeline of overlapping windows -> :data:`Windows`.  Takes the
+        arguments of ``__call__`` (single-ended checkpoints only) and checks them alike, but accepts recordings of any
+        length.
+
+        window_s     : window length in seconds at the model rate (``ms_sr`` when set, else ``sample_rate``):
+                       W = round(window_s rate) samples; its segment count must fit ``ms_max_segments``
+        window_hop_s : hop between window starts, rounded to whole mel frames (at least one); at most the window
+        Window k of a recording of T samples covers samples [k H, min(k H + W, T)) and scores exactly what that cut-out
+        clip scores through ``__call__``.  Only the last window can be shorter than W; if it is too short for the
+        checkpoint its scores are NaN and its status is CLIP_TOO_SHORT.
+        scores       : float32 [N, len(columns)] CUDA tensor, the windows of recording b after those of the ones before it
+        counts       : host list of B ints, windows per recording
+        t_start, t_end : float64 [N] host arrays, seconds at the model rate
+        n_segments, status : int32 [N] host arrays
+        """
+        from . import resample as RS
+        if self.double_ended:
+            raise ValueError("windows: a double-ended (NISQA_DE) checkpoint scores (wave, reference) pairs, not windows")
+        deg = self._batch("wave", wave, sample_rate, lengths, channel)
+        sr = deg[0].sample_rate
+        rate = self.target_sr or sr
+        W, hop_frames = window_geometry(self.args, rate, window_s, window_hop_s)
+        H = hop_frames * int(rate * self.args["ms_hop_length"])
+        _, n_seg, status = E.segment_counts(self.cfg, W, rate)
+        if status != E.CLIP_OK:
+            a = self.args
+            err = E.clip_status_error(status, "window_s=%r (%d samples at %d Hz)" % (window_s, W, rate), W, rate, n_seg,
+                                      a["ms_hop_length"], a["ms_seg_length"], a["ms_max_segments"])
+            raise ValueError("window_s: " + str(err))
+        counts, t0, t1, nseg, st = [], [], [], [], []
+        for n in deg[1]:
+            T = int(n) if rate == sr else RS.out_len(int(n), sr, rate)
+            s, z = E.window_counts(self.cfg, T, rate, W, hop_frames)
+            a, b = window_times(T, W, H, rate)
+            counts.append(len(s)); nseg.append(s); st.append(z); t0.append(a); t1.append(b)
+        N = int(sum(counts))
+        out = torch.empty((N, len(self.columns)), dtype=torch.float32, device=self.device)
+        if N:
+            self.engine.predict_device_windows(self._stream(), deg, out.data_ptr(), N, W, hop_frames, target_sr=self.target_sr)
+        cat = lambda parts, dt: np.concatenate(parts).astype(dt) if parts else np.zeros(0, dt)      # noqa: E731
+        return Windows(out, counts, cat(t0, np.float64), cat(t1, np.float64), cat(nseg, np.int32), cat(st, np.int32))
 
     # ------------------------------------------------------------------ shared by __call__ and segments
     def _arguments(self, wave, sample_rate, lengths, channel, reference, reference_lengths, reference_sample_rate):

@@ -8,6 +8,7 @@ and the same option names, so existing invocations keep working:
     python run_predict.py --mode predict_dir  --pretrained_model weights/nisqa.tar --data_dir d --bs 64
     torchrun --nproc-per-node 8 run_predict.py --mode predict_csv ...   (one rank per GPU)
     python run_predict.py --mode predict_dir ... --output_dir out --segments   (+ out/NISQA_segments.csv)
+    python run_predict.py --mode predict_dir ... --output_dir out --window_s 10 --window_hop_s 1   (out/NISQA_windows.csv)
 """
 import argparse
 
@@ -44,7 +45,17 @@ def parse_args(argv=None):
     parser.add_argument("--segments", action="store_true",
                         help="also write NISQA_segments.csv into output_dir: every segment's time span, score and "
                              "pooling weight (single process only)")
+    parser.add_argument("--window_s", type=float, default=None,
+                        help="score every file as a timeline of windows of this many seconds (with --window_hop_s) and "
+                             "write NISQA_windows.csv into output_dir; files of any length (single process only)")
+    parser.add_argument("--window_hop_s", type=float, default=None, help="hop between window starts in seconds")
     args = vars(parser.parse_args(argv))
+    if (args["window_s"] is None) != (args["window_hop_s"] is None):
+        missing = "window_hop_s" if args["window_hop_s"] is None else "window_s"
+        raise ValueError("--%s argument needed: --window_s and --window_hop_s go together" % missing)
+    for key in ("window_s", "window_hop_s"):
+        if args[key] is not None and not args[key] > 0:
+            raise ValueError("--%s argument must be a positive number of seconds, not %r" % (key, args[key]))
 
     if args["mode"] not in _NEEDS:
         raise NotImplementedError("--mode given not available")

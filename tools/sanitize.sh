@@ -4,7 +4,7 @@
 # short clips at 48 / 16 kHz: front-end, conv1, the five wgmma conv layers with their bulk copies /
 # mbarriers, self-attention, pooling), over a 96 kHz clip (frontend_kernel, the front end for windows over 1024
 # samples), over a short nisqa_tts.tar call (StandardCNN, BiLSTM) and over device-batch
-# calls (the ingest kernel, with and without ms_sr, and one segments call); racecheck over the double-ended alignment's multi-block path.
+# calls (the ingest kernel, with and without ms_sr, one segments call and two windows calls); racecheck over the double-ended alignment's multi-block path.
 #   bash tools/sanitize.sh TAG
 TAG=${1:-rXX}
 OUT=gpurun_out
@@ -69,6 +69,13 @@ s4.close()
 s5 = Scorer(os.path.join("weights", "nisqa_mos_only.tar"), ms_sr=16000)
 print("ingest ms_sr", s5(w[0], 48000, lengths=[30000, w.shape[-1]]).tolist())
 s5.close()
+# windows of a recording (ingest_span_kernel, frontend_windows_kernel: shared and edge pairs, both pairings): 25 s at a
+# 3.33 s hop (an odd number of frames), and 96 kHz windows (the generic front-end arithmetic)
+s6 = Scorer(os.path.join("weights", "nisqa.tar"))
+r = torch.from_numpy(synth.synth_speech_pcm16(16, 25.0, 48000)).cuda()
+print("windows", s6.windows(r, 48000, 10.0, 3.33).scores.tolist())
+print("windows 96 kHz", s6.windows(torch.from_numpy(synth.synth_speech_pcm16(17, 12.0, 96000)).cuda(), 96000, 10.0, 1.0).scores.tolist())
+s6.close()
 PY
 timeout 400 compute-sanitizer --tool memcheck --error-exitcode 7 --log-file $OUT/${TAG}_memcheck.log python /tmp/san_run.py > $OUT/${TAG}_memcheck_stdout.log 2>&1
 echo "memcheck exit $?"
