@@ -318,6 +318,42 @@ NISQA_API int  nisqa_predict_device_windows(nisqa_engine* e, void* cuda_stream, 
                                             int32_t target_sr, int64_t window, int32_t hop_frames, float* scores_dev,
                                             int64_t n_rows, int32_t* n_segments_out, int32_t* status_out);
 
+/* Live feeds: n_feeds independent recordings that arrive chunk by chunk (calls, conference bridges, broadcast and TTS
+ * monitoring), scored as the windows of nisqa_predict_device_windows as soon as each window is complete.  A feed object
+ * runs at one rate (the model rate: checkpoints with ms_sr take feeds at ms_sr only), with the window geometry of
+ * nisqa_window_counts; window k of a feed covers samples [k H, min(k H + window, T)) of its current recording and scores
+ * bit for bit what nisqa_predict_device_windows gives on the concatenated recording (and so what the cut-out clip gives).
+ *   nisqa_feed_create : n_feeds 1 .. 65535, sample_rate, window / hop_frames as nisqa_predict_device_windows (the same
+ *                       refusals; double-ended engines are refused), max_push: the most samples one push may append to
+ *                       one feed.  Device memory: nisqa_feed_device_bytes.  Destroy a feed object before its engine.
+ *   nisqa_feed_rows   : pure host arithmetic.  For feeds that hold held[b] samples of their current recording, the rows
+ *                       a push of n_samples[b] samples (0 allowed) with end[b] (NULL: none) emits, in feed then window
+ *                       order: window k of feed b once the feed holds k H + window samples; with end[b] every remaining
+ *                       window of the final length T (1 if T <= window, else 1 + ceil((T - window) / H) in all; a
+ *                       feed that ends with no sample has none).  *n_rows, and for the first min(rows, cap) rows their
+ *                       feed, window index k, segment count and status (any array may be NULL).
+ *   nisqa_feed_push   : appends chunk's clip b (n_samples[b] samples, 0 .. max_push, of a [n_feeds][C][length] int16 /
+ *                       float32 device batch at the feed rate; its channel applies) to feed b and scores the windows it
+ *                       completes into scores_dev (device [n_rows][n_out]); feed_out, index_out, n_segments_out,
+ *                       status_out: host [rows], valid on return (may be NULL).  A window too short for one segment
+ *                       scores NaN with NISQA_CLIP_TOO_SHORT.  After end[b], feed b starts a new recording at sample 0.
+ *                       The stream contract of nisqa_predict_device_windows: no host wait of its own, nothing enqueued
+ *                       when it refuses (n_rows too small, a chunk of other n_clips / sample_rate, more than max_push
+ *                       samples, or another sample format - int16 mono vs float32 or mixed - while a feed holds samples).
+ *                       Pushes of one feed object run in push order, on any streams. */
+typedef struct nisqa_feed nisqa_feed;
+NISQA_API int     nisqa_feed_create(nisqa_engine* e, nisqa_feed** out, int32_t n_feeds, int32_t sample_rate, int64_t window,
+                                    int32_t hop_frames, int64_t max_push);
+NISQA_API int     nisqa_feed_rows(const nisqa_config* cfg, int32_t sample_rate, int64_t window, int32_t hop_frames,
+                                  int32_t n_feeds, const int64_t* held, const int64_t* n_samples, const uint8_t* end,
+                                  int64_t* n_rows, int32_t* feed, int64_t* index, int32_t* n_segments, int32_t* status,
+                                  int64_t cap);
+NISQA_API int     nisqa_feed_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch* chunk, const uint8_t* end,
+                                  float* scores_dev, int64_t n_rows, int32_t* feed_out, int64_t* index_out,
+                                  int32_t* n_segments_out, int32_t* status_out);
+NISQA_API int64_t nisqa_feed_device_bytes(const nisqa_feed* f);
+NISQA_API void    nisqa_feed_destroy(nisqa_feed* f);
+
 /* Copy an intermediate of the LAST predict call to host memory (parity tests).  Only valid
  * when that call fitted in one internal pass.  Returns the number of floats written (>=0)
  * or a negative status; with out == NULL returns the required count. */

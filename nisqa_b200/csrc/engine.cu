@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <cmath>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -125,8 +126,9 @@ struct Stage {
   DevBuf pcm, clips, prefixes, clipmax;
   DevBuf seg_row;        // segments call: each clip's first output row (int64, < 0: none)
   DevBuf spans;          // windows call: the pass's recording spans (WinSpan)
+  DevBuf fwins;          // feed push: the pass's windows (FeedWin)
   void release() {
-    DevBuf* all[] = {&pcm, &clips, &prefixes, &clipmax, &seg_row, &spans};
+    DevBuf* all[] = {&pcm, &clips, &prefixes, &clipmax, &seg_row, &spans, &fwins};
     for (auto* b : all) b->release();
     h_tables.release();
     if (ev_copied) cudaEventDestroy(ev_copied);
@@ -325,6 +327,37 @@ struct nisqa_engine {
   }
 };
 
+// A feed object (nisqa_feed_create): n_feeds live recordings at one rate, their rings (windows.cuh) and the host state
+// of each feed.  Its pushes run in push order: a push's ingest waits for the last push's passes (done), so one ring
+// holds what any push reads (R = W + max_push samples; P pair slots for the frames of W + max_push samples).
+constexpr int kFeedSlots = 4;      // push tables in flight (pinned -> device)
+struct nisqa_feed {
+  nisqa_engine* e = nullptr;
+  int n_feeds = 0, rate = 0;
+  int64_t max_push = 0;
+  FeedGeom g = {};
+  int fmt = -1;                            // the rings' sample format (NISQA_FMT_*) while a feed holds samples
+  std::vector<int64_t> held;               // samples of each feed's current recording
+  std::vector<int64_t> j_next;             // each feed's first frame whose pair is not computed yet
+  void* ring = nullptr;                    // [n_feeds][stride] samples (4 bytes each reserved)
+  float* frames = nullptr;                 // [n_feeds][P][2 n_mels]
+  size_t ring_bytes = 0, frame_bytes = 0;
+  struct Slot { HostBuf h; DevBuf d; cudaEvent_t copied = nullptr; bool busy = false; } slots[kFeedSlots];
+  int64_t n_push = 0;
+  cudaEvent_t ready = nullptr;             // this push's samples and pairs are in the rings
+  cudaEvent_t done = nullptr;              // the last push's passes are done
+  bool pending = false;
+  ~nisqa_feed() {         // (nisqa_feed_destroy first waits for the work in flight)
+    for (auto& sl : slots) {
+      sl.h.release(); sl.d.release();
+      if (sl.copied) cudaEventDestroy(sl.copied);
+    }
+    if (ring) cudaFree(ring);
+    if (frames) cudaFree(frames);
+    for (cudaEvent_t ev : {ready, done}) if (ev) cudaEventDestroy(ev);
+  }
+};
+
 namespace {
 
 int fail(nisqa_engine* e, int code, const std::string& msg) {
@@ -411,6 +444,18 @@ bool window_geometry(const nisqa_config& c, int sr, int64_t window, int32_t hop_
   return true;
 }
 int64_t window_count(int64_t T, int64_t W, int64_t H) { return T <= W ? 1 : 1 + (T - W + H - 1) / H; }
+// The windows a push of n[b] samples to feeds that held held[b] completes, as emit(feed, k, length) in feed then window
+// order: window k once the feed holds k H + W samples; with end[b], every remaining window of the final length T
+// (window_count: the last may be short; a feed that ended with no sample has none).
+template <class Emit>
+void feed_windows(int n_feeds, int64_t W, int64_t H, const int64_t* held, const int64_t* n, const uint8_t* end, Emit emit) {
+  auto complete = [&](int64_t T) { return T >= W ? (T - W) / H + 1 : 0; };
+  for (int b = 0; b < n_feeds; ++b) {
+    const int64_t T = held[b] + n[b];
+    const int64_t k1 = end && end[b] && T > 0 ? window_count(T, W, H) : complete(T);
+    for (int64_t k = complete(held[b]); k < k1; ++k) emit(b, k, std::min(W, T - k * H));
+  }
+}
 
 // ---------------------------------------------------------------- librosa.filters.mel in double
 double hz_to_mel(double f) {
@@ -1116,6 +1161,12 @@ int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
 }
 
 // ---------------------------------------------------------------- one pass over a run of clips
+// The rings of a feed object (nisqa_feed_push), as its passes read them
+struct FeedRings {
+  const void* ring;            // sample rings (int16 or float32, the push's format)
+  const float* frames;         // frame-pair rings
+  FeedGeom g;
+};
 // A windows call (nisqa_predict_device_windows): its windows are the clips of predict_common, in recording order
 struct WinLayout {
   const int* rec;              // [windows] recording of each window
@@ -1123,6 +1174,7 @@ struct WinLayout {
   const int64_t* rec_off;      // [recordings] element offset of each converted recording in dev_pcm (ms_sr), or nullptr:
                                // the ingest packs each pass's spans from the caller's batch
   int H, hf, W;                // window hop (samples, mel frames) and length
+  const FeedRings* feed = nullptr;    // a feed push: the windows read the feeds' rings (rec: the feed)
 };
 // The recording spans of one pass of a windows call and the launch shape of its front end
 struct WinPass {
@@ -1131,6 +1183,9 @@ struct WinPass {
   long long pcm_elems = 0;         // ingest: the packed spans
   long long max_span = 0;          // the longest span
   int edge = 0, pairs = 0, ncls = 1;
+  const FeedRings* feed = nullptr;   // a feed push: each window's FeedWin row and the most interior pairs of one
+  std::vector<FeedWin> fwins;
+  int interior = 0;
 };
 
 struct PassInput {
@@ -1175,6 +1230,7 @@ struct Pass {
   int* seg_clip = nullptr;
   const long long* seg_row = nullptr;         // segments call: the clips' first output rows (staging slot)
   const WinSpan* spans = nullptr;             // windows call: the recording spans (staging slot)
+  const FeedWin* fwins = nullptr;             // feed push: the windows' rows (staging slot)
   // the rows the pooling module read (segment_rows): D real columns at a stride of ld, the attention logits the pooling
   // path wrote (or nullptr), and each head's last Linear (PoolSimpleParams.w3 / b3; a1 / a1b for PoolAtt)
   const float* pool_x = nullptr;
@@ -1244,7 +1300,8 @@ int upload_inputs(Pass& p, const PassInput& in) {
   const size_t tb_clips = (size_t)n * sizeof(ClipDesc), tb_pref = pre.size() * 4;
   const size_t tb_rows_at = (tb_clips + tb_pref + 7) / 8 * 8, tb_rows = e->seg_out ? (size_t)n * 8 : 0;
   const size_t tb_spans_at = tb_rows_at + tb_rows, tb_spans = in.win ? in.win->spans.size() * sizeof(WinSpan) : 0;
-  CK(SG.h_tables.reserve(tb_spans_at + tb_spans));
+  const size_t tb_fwins_at = (tb_spans_at + tb_spans + 15) / 16 * 16, tb_fwins = in.win ? in.win->fwins.size() * sizeof(FeedWin) : 0;
+  CK(SG.h_tables.reserve(tb_fwins_at + tb_fwins));
   char* ht = SG.h_tables.as<char>();
   memcpy(ht, cl.data(), tb_clips);
   memcpy(ht + tb_clips, pre.data(), tb_pref);
@@ -1259,6 +1316,12 @@ int upload_inputs(Pass& p, const PassInput& in) {
     CK(SG.spans.reserve(tb_spans));
     CK(cudaMemcpyAsync(SG.spans.p, ht + tb_spans_at, tb_spans, cudaMemcpyHostToDevice, cs));
     p.spans = SG.spans.as<WinSpan>();
+  }
+  if (tb_fwins) {     // (a feed push: the pass's windows in the feeds' rings)
+    memcpy(ht + tb_fwins_at, in.win->fwins.data(), tb_fwins);
+    CK(SG.fwins.reserve(tb_fwins));
+    CK(cudaMemcpyAsync(SG.fwins.p, ht + tb_fwins_at, tb_fwins, cudaMemcpyHostToDevice, cs));
+    p.fwins = SG.fwins.as<FeedWin>();
   }
   CK(SG.clips.reserve(tb_clips));
   CK(SG.prefixes.reserve(tb_pref));
@@ -1416,13 +1479,17 @@ int framewise(Pass& p, int fmt, Rows* out, const WinPass* win) {
   p.seg_clip = p.seg_frame0 + 2 * (size_t)n_seg;
 
   { Scope s(e, "frontend");
-    if (win)            // windows: each interior frame pair of a recording span once, the edge pairs per window
+    if (win) {          // windows: each interior frame pair of a recording span once, the edge pairs per window
       launch_frontend_windows(p.st, c.n_mels, p.pcm, fmt == NISQA_FMT_F32, p.clips, p.n, win->edge, p.spans,
                               (int)win->spans.size(), win->pairs, win->ncls, e->fb_table.as<FbTables>(),
                               e->tw4096.as<float2>(), LN.mel.as<float>(), p.clipmax, p.Q, p.max_span);
-    else
+      if (win->feed)    // a feed push (no spans): the interior rows, computed as their samples arrived, from the rings
+        launch_feed_rows(p.st, c.n_mels, p.clips, p.fwins, p.n, win->interior, win->feed->g, win->feed->frames,
+                         LN.mel.as<float>(), p.clipmax);
+    } else {
       launch_frontend(p.st, c.n_mels, p.pcm, fmt == NISQA_FMT_F32, p.clips, p.n, p.max_pairs, e->fb_table.as<FbTables>(),
-                      e->tw4096.as<float2>(), LN.mel.as<float>(), p.clipmax, p.Q, p.max_span, e->fe_ppc); }
+                      e->tw4096.as<float2>(), LN.mel.as<float>(), p.clipmax, p.Q, p.max_span, e->fe_ppc);
+    } }
   { Scope s(e, "seg_table");
     launch_seg_table(p.st, p.clips, p.n, p.seg_prefix, p.clipmax, c.seg_hop, n_seg, p.seg_frame0, p.seg_thr, p.seg_clip); }
   e->last_conv12 = e->fused12();
@@ -1786,6 +1853,26 @@ void win_pass(const nisqa_config& c, const WinLayout& L, const ClipPlan* plan, c
   }
 }
 
+// The windows i0 .. i1 - 1 of a feed push: each window's offset in the sample rings and FeedWin row, and the launch shape
+// of its edge pairs and interior rows (nothing to ingest: the push appended its samples to the rings)
+void feed_pass(const WinLayout& L, const ClipPlan* plan, const int64_t* len, int i0, int i1, WinPass* w) {
+  *w = WinPass();
+  const FeedGeom& g = L.feed->g;
+  w->feed = L.feed;
+  w->pcm_off.resize(i1 - i0);
+  w->fwins.resize(i1 - i0);
+  for (int i = i0; i < i1; ++i) {
+    const int b = L.rec[i];
+    w->pcm_off[i - i0] = b * g.stride + L.start[i] % g.R;
+    w->fwins[i - i0] = {L.start[i] / g.hop, b, 0};
+    if (!plan[i].run) continue;
+    int lead, tail;
+    interior_pairs(plan[i].n_frames, (int)len[i], g.s0, g.hop, g.win, &lead, &tail);
+    w->edge = std::max(w->edge, lead + (plan[i].n_frames + 1) / 2 - tail);
+    w->interior = std::max(w->interior, tail - lead);
+  }
+}
+
 int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, const void* dev_pcm,
                    const int64_t* dev_off, const int64_t* n_samples, const int32_t* sample_rate,
                    int fmt, float* scores_host, float* scores_dev, int32_t* n_seg_out,
@@ -1861,7 +1948,8 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
     in.scores_dev_out = scores_all + (size_t)i0 * e->cfg.n_out;
     in.win = nullptr;
     if (win) {
-      win_pass(e->cfg, *win, plan.data(), n_samples, i0, i1, &wp);
+      if (win->feed) feed_pass(*win, plan.data(), n_samples, i0, i1, &wp);
+      else win_pass(e->cfg, *win, plan.data(), n_samples, i0, i1, &wp);
       in.win = &wp;
     }
     in.slot = e->profiling ? 0 : (int)(e->pass_counter % kLanes);
@@ -2246,9 +2334,10 @@ static int enqueue_device_batch(nisqa_engine* e, cudaStream_t caller, int n_clip
 }
 
 // The checks of one nisqa_device_batch argument (nm: its name in messages; ch: the channel it is read with; n_clips: the
-// clip count it must have) -> its ingest source and whether it is mixed to mono
+// clip count it must have; min_n: the fewest samples a clip may have, 0 for a feed push) -> its ingest source and whether
+// it is mixed to mono
 static int check_device_batch(nisqa_engine* e, const nisqa_device_batch& b, const std::string& nm, int ch, int n_clips,
-                              IngestSrc* src, bool* mix) {
+                              IngestSrc* src, bool* mix, int min_n = 1) {
   if (b.sample_fmt != NISQA_FMT_S16 && b.sample_fmt != NISQA_FMT_F32) return fail(e, NISQA_ERR_INVALID, nm + "sample_fmt");
   if (b.n_clips < 0 || b.n_clips != n_clips) return fail(e, NISQA_ERR_INVALID, nm + "n_clips");
   if (b.n_channels < 1) return fail(e, NISQA_ERR_INVALID, nm + "n_channels");
@@ -2257,9 +2346,10 @@ static int check_device_batch(nisqa_engine* e, const nisqa_device_batch& b, cons
   if (b.sample_rate <= 0) return fail(e, NISQA_ERR_INVALID, nm + "sample_rate");
   if (b.n_clips > 0 && (!b.data || !b.n_samples)) return fail(e, NISQA_ERR_INVALID, nm + "data / n_samples: null argument");
   for (int i = 0; i < b.n_clips; ++i)
-    if (b.n_samples[i] < 1 || b.n_samples[i] > b.length)
+    if (b.n_samples[i] < min_n || b.n_samples[i] > b.length)
       return fail(e, NISQA_ERR_INVALID, nm + "n_samples[" + std::to_string(i) + "] = " + std::to_string(b.n_samples[i]) +
-                                            ": not within 1 .. length (" + std::to_string(b.length) + ")");
+                                            ": not within " + std::to_string(min_n) + " .. length (" +
+                                            std::to_string(b.length) + ")");
   *mix = b.n_channels > 1 && ch < 0;
   *src = {b.data, b.clip_stride, b.channel_stride, b.n_channels, ch, b.sample_fmt == NISQA_FMT_F32 ? 1 : 0};
   return 0;
@@ -2440,6 +2530,221 @@ int nisqa_window_counts(const nisqa_config* cfg, int64_t n_samples, int32_t samp
     if (status) status[k] = p.status;
   }
   return 0;
+}
+
+// ---- live feeds
+int nisqa_feed_rows(const nisqa_config* cfg, int32_t sample_rate, int64_t window, int32_t hop_frames, int32_t n_feeds,
+                    const int64_t* held, const int64_t* n_samples, const uint8_t* end, int64_t* n_rows, int32_t* feed,
+                    int64_t* index, int32_t* n_segments, int32_t* status, int64_t cap) {
+  if (!cfg || n_feeds < 0 || (n_feeds > 0 && (!held || !n_samples)) || !n_rows) return NISQA_ERR_INVALID;
+  std::string why;
+  int H = 0;
+  if (!window_geometry(*cfg, sample_rate, window, hop_frames, &H, &why)) return NISQA_ERR_INVALID;
+  for (int b = 0; b < n_feeds; ++b)
+    if (held[b] < 0 || n_samples[b] < 0) return NISQA_ERR_INVALID;
+  int64_t r = 0;
+  feed_windows(n_feeds, window, H, held, n_samples, end, [&](int b, int64_t k, int64_t len) {
+    if (r < cap) {
+      ClipPlan p;
+      plan_clip(*cfg, len, sample_rate, &p);
+      if (feed) feed[r] = b;
+      if (index) index[r] = k;
+      if (n_segments) n_segments[r] = p.n_seg;
+      if (status) status[r] = p.status;
+    }
+    ++r;
+  });
+  *n_rows = r;
+  return 0;
+}
+
+int nisqa_feed_create(nisqa_engine* e, nisqa_feed** out, int32_t n_feeds, int32_t sample_rate, int64_t window,
+                      int32_t hop_frames, int64_t max_push) {
+  if (!e) return NISQA_ERR_INVALID;
+  if (!out) return fail(e, NISQA_ERR_INVALID, "out: null argument");
+  *out = nullptr;
+  if (!e->stream) return fail(e, NISQA_ERR_STATE, "engine was not created successfully");
+  if (e->cfg.double_ended)
+    return fail(e, NISQA_ERR_INVALID, "a double-ended (NISQA_DE) engine scores (degraded, reference) pairs, not live feeds");
+  if (n_feeds < 1 || n_feeds > 65535)
+    return fail(e, NISQA_ERR_INVALID, "n_feeds = " + std::to_string(n_feeds) + ": not within 1 .. 65535");
+  if (sample_rate <= 0) return fail(e, NISQA_ERR_INVALID, "sample_rate = " + std::to_string(sample_rate));
+  std::string why;
+  int H = 0;
+  if (!window_geometry(e->cfg, sample_rate, window, hop_frames, &H, &why)) return fail(e, NISQA_ERR_INVALID, why);
+  if (max_push < 1 || max_push > (int64_t)INT32_MAX - 2 * window)
+    return fail(e, NISQA_ERR_INVALID, "max_push = " + std::to_string(max_push) + ": not within 1 .. 2^31 - 1 - 2 window samples");
+  CK(cudaSetDevice(e->device));
+  ClipPlan pl;
+  plan_clip(e->cfg, window, sample_rate, &pl);
+  int fb_id = -1;
+  int rc = build_fb(e, sample_rate, pl.hop, pl.win, &fb_id);
+  if (rc) return rc;
+  std::unique_ptr<nisqa_feed> f(new nisqa_feed());
+  f->e = e;
+  f->n_feeds = n_feeds; f->rate = sample_rate; f->max_push = max_push;
+  FeedGeom& g = f->g;
+  g = {};
+  g.W = (int)window; g.H = H; g.hf = hop_frames;
+  g.R = (int)(window + max_push);
+  g.stride = ((long long)g.R + g.W + 15) / 16 * 16;
+  g.hop = pl.hop; g.win = pl.win; g.s0 = (e->cfg.n_fft - pl.win) / 2 - e->cfg.n_fft / 2;
+  g.ncls = (hop_frames & 1) ? 2 : 1;
+  const int frames_live = (int)((window + max_push) / pl.hop) + 2;       // frames whose pairs one push may touch
+  g.P = g.ncls == 2 ? frames_live : frames_live / 2 + 2;
+  g.fb_id = fb_id;
+  f->held.assign(n_feeds, 0);
+  f->j_next.assign(n_feeds, 0);
+  const size_t ring_bytes = (size_t)n_feeds * g.stride * 4;             // (int16 rings use half)
+  const size_t frame_bytes = (size_t)n_feeds * g.P * 2 * e->cfg.n_mels * 4;
+  CK(cudaMalloc(&f->ring, ring_bytes));
+  f->ring_bytes = ring_bytes;
+  CK(cudaMalloc(&f->frames, frame_bytes));
+  f->frame_bytes = frame_bytes;
+  CK(cudaMemset(f->ring, 0, ring_bytes));
+  CK(cudaMemset(f->frames, 0, frame_bytes));
+  CK(cudaEventCreateWithFlags(&f->ready, cudaEventDisableTiming));
+  CK(cudaEventCreateWithFlags(&f->done, cudaEventDisableTiming));
+  for (auto& sl : f->slots) CK(cudaEventCreateWithFlags(&sl.copied, cudaEventDisableTiming));
+  *out = f.release();
+  return 0;
+}
+
+int64_t nisqa_feed_device_bytes(const nisqa_feed* f) {
+  if (!f) return NISQA_ERR_INVALID;
+  int64_t n = (int64_t)(f->ring_bytes + f->frame_bytes);
+  for (const auto& sl : f->slots) n += (int64_t)sl.d.cap;
+  return n;
+}
+
+int nisqa_feed_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch* chunk, const uint8_t* end, float* scores_dev,
+                    int64_t n_rows, int32_t* feed_out, int64_t* index_out, int32_t* n_segments_out, int32_t* status_out) {
+  if (!f) return NISQA_ERR_INVALID;
+  nisqa_engine* e = f->e;
+  if (!e->weights_loaded) return fail(e, NISQA_ERR_STATE, "nisqa_load_weights has not been called");
+  if (!chunk) return fail(e, NISQA_ERR_INVALID, "chunk: null argument");
+  if (chunk->n_clips != f->n_feeds)
+    return fail(e, NISQA_ERR_INVALID, "chunk.n_clips = " + std::to_string(chunk->n_clips) + ": the feed object has " +
+                                          std::to_string(f->n_feeds) + " feeds");
+  if (chunk->sample_rate != f->rate)
+    return fail(e, NISQA_ERR_INVALID, "chunk.sample_rate = " + std::to_string(chunk->sample_rate) + ": the feeds run at " +
+                                          std::to_string(f->rate) + " Hz");
+  IngestSources ing = {};
+  ing.n_src = 1;
+  bool mix = false;
+  int rc = check_device_batch(e, *chunk, "chunk.", chunk->channel, f->n_feeds, &ing.s[0], &mix, 0);
+  if (rc) return rc;
+  const FeedGeom& g = f->g;
+  const int B = f->n_feeds;
+  long long max_in = 0;
+  bool holds = false;
+  for (int b = 0; b < B; ++b) {
+    if (chunk->n_samples[b] > f->max_push)
+      return fail(e, NISQA_ERR_INVALID, "chunk.n_samples[" + std::to_string(b) + "] = " + std::to_string(chunk->n_samples[b]) +
+                                            ": more than max_push (" + std::to_string(f->max_push) + " samples)");
+    max_in = std::max<long long>(max_in, chunk->n_samples[b]);
+    holds = holds || f->held[b] > 0;
+  }
+  const int fmt = chunk->sample_fmt == NISQA_FMT_F32 || mix ? NISQA_FMT_F32 : NISQA_FMT_S16;
+  if (max_in > 0 && holds && f->fmt != fmt)
+    return fail(e, NISQA_ERR_INVALID, std::string("chunk.sample_fmt: the feeds hold ") +
+                                          (f->fmt == NISQA_FMT_F32 ? "float32" : "int16") + " samples and this push " +
+                                          (fmt == NISQA_FMT_F32 ? "float32 (or mixed) ones" : "mono int16 ones") +
+                                          "; a format holds until every feed has ended");
+  // the windows the push completes (host arithmetic: nisqa_feed_rows)
+  std::vector<int> wfeed;
+  std::vector<int64_t> wstart, wlen, widx;
+  feed_windows(B, g.W, g.H, f->held.data(), chunk->n_samples, end, [&](int b, int64_t k, int64_t len) {
+    wfeed.push_back(b); widx.push_back(k); wstart.push_back(k * g.H); wlen.push_back(len);
+  });
+  const int N = (int)wfeed.size();
+  if (n_rows < N)
+    return fail(e, NISQA_ERR_INVALID, "n_rows = " + std::to_string(n_rows) + ": the push completes " + std::to_string(N) + " windows");
+  if (N > 0 && !scores_dev) return fail(e, NISQA_ERR_INVALID, "scores_dev: null argument");
+
+  // each feed's new samples and the interior pairs whose last tap they bring
+  CK(cudaSetDevice(e->device));
+  for (auto& t : e->timers) { t.ms = 0.0; t.launches = 0; }
+  cudaStream_t caller = static_cast<cudaStream_t>(cuda_stream);
+  auto& sl = f->slots[f->n_push % kFeedSlots];
+  if (sl.busy) { CK(cudaEventSynchronize(sl.copied)); sl.busy = false; }
+  CK(sl.h.reserve((size_t)B * sizeof(FeedPush)));
+  FeedPush* tab = sl.h.as<FeedPush>();
+  const int step = 3 - g.ncls, ext = g.hop + g.win;
+  const long long j_min = (-g.s0 + g.hop - 1) / g.hop;       // the first frame whose taps start at or after sample 0
+  int max_pairs = 0;
+  for (int b = 0; b < B; ++b) {
+    const long long t1 = f->held[b] + chunk->n_samples[b], num = t1 - ext - g.s0;
+    const long long j_end = num < 0 ? 0 : num / g.hop + 1;     // frames whose pair's taps have all arrived
+    long long j0 = std::max<long long>(f->j_next[b], j_min);
+    if (j0 % step) ++j0;
+    const long long np = j_end > j0 ? (j_end - j0 + step - 1) / step : 0;
+    tab[b] = {f->held[b], j0, (int)chunk->n_samples[b], (int)np};
+    max_pairs = std::max(max_pairs, (int)np);
+    f->j_next[b] = std::max<long long>(f->j_next[b], j_end);
+  }
+  CK(cudaEventRecord(e->ev_in, caller));
+  cudaStream_t st = e->lanes[e->profiling ? 0 : (int)(e->pass_counter % kLanes)].stream;
+  CK(cudaStreamWaitEvent(st, e->ev_in, 0));
+  if (f->pending) CK(cudaStreamWaitEvent(st, f->done, 0));  // push order: the last push's passes are done with the rings
+  if (max_in > 0) {
+    CK(sl.d.reserve((size_t)B * sizeof(FeedPush)));
+    CK(cudaMemcpyAsync(sl.d.p, tab, (size_t)B * sizeof(FeedPush), cudaMemcpyHostToDevice, st));
+    CK(cudaEventRecord(sl.copied, st));
+    sl.busy = true;
+    ++f->n_push;
+    e->cur_stream = st;
+    { Scope s(e, "ingest");
+      launch_ingest_feed(st, ing.s[0], sl.d.as<FeedPush>(), B, max_in, g, fmt == NISQA_FMT_F32, f->ring); }
+    if (max_pairs > 0) {
+      Scope s(e, "frontend");
+      launch_frontend_feed_pairs(st, e->cfg.n_mels, f->ring, fmt == NISQA_FMT_F32, sl.d.as<FeedPush>(), B, max_pairs, g,
+                                 e->fb_table.as<FbTables>(), e->tw4096.as<float2>(), f->frames);
+    }
+    CK(cudaGetLastError());
+    f->fmt = fmt;
+  }
+  for (int b = 0; b < B; ++b) {
+    f->held[b] += chunk->n_samples[b];
+    if (end && end[b]) { f->held[b] = 0; f->j_next[b] = 0; }
+  }
+  CK(cudaEventRecord(f->ready, st));
+  // the completed windows, each a clip of a pass that reads the rings
+  cudaStream_t fin = st;
+  if (N > 0) {
+    FeedRings rings = {f->ring, f->frames, g};
+    WinLayout L = {wfeed.data(), wstart.data(), nullptr, g.H, g.hf, g.W, &rings};
+    std::vector<int32_t> srs(N, f->rate);
+    rc = predict_common(e, N, nullptr, f->ring, nullptr, wlen.data(), srs.data(), f->fmt, nullptr, scores_dev,
+                        n_segments_out, status_out, 0, nullptr, nullptr, f->ready, &fin, &L);
+    if (rc) {
+      for (auto& l : e->lanes)
+        if (cudaEventRecord(e->ev_out, l.stream) == cudaSuccess) cudaStreamWaitEvent(caller, e->ev_out, 0);
+      if (cudaEventRecord(f->done, caller) == cudaSuccess) f->pending = true;
+      return rc;
+    }
+  } else if (e->profiling) {
+    CK(cudaStreamSynchronize(st));
+    collect_timers(e);
+  }
+  for (int r = 0; r < N; ++r) {
+    if (feed_out) feed_out[r] = wfeed[r];
+    if (index_out) index_out[r] = widx[r];
+  }
+  CK(cudaEventRecord(f->done, fin));
+  f->pending = true;
+  CK(cudaEventRecord(e->ev_out, fin));
+  CK(cudaStreamWaitEvent(caller, e->ev_out, 0));
+  return 0;
+}
+
+void nisqa_feed_destroy(nisqa_feed* f) {
+  if (!f) return;
+  cudaSetDevice(f->e->device);
+  if (f->pending) cudaEventSynchronize(f->done);
+  for (auto& sl : f->slots)
+    if (sl.busy) cudaEventSynchronize(sl.copied);
+  delete f;
 }
 
 int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {

@@ -671,6 +671,73 @@ frontend_windows_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ 
     for (int d = tid; d < n_dst; d += kFeThreads) atomicMax(clipmax + c0 + d * cstep, f2key(m));
 }
 
+// ---- live feeds (nisqa_feed_push) ------------------------------------------------------------------------------------
+// The interior pairs of one push: grid (pair of the push, feed).  A pair whose taps have all arrived and that some window
+// holds as an interior pair (k H <= a, a + hop + win <= k H + W, k of the pair's class) is computed once with win_pair
+// - the arithmetic of frontend_windows_kernel's shared pairs - over the W contiguous ring samples from its first tap,
+// and its two rows go to the feed's frame ring.  Windows take them from there when they complete (feed_rows_kernel).
+template <typename T, int MELS, bool PP>
+__global__ void __launch_bounds__(kFeThreads, 4)
+frontend_feed_kernel(const T* __restrict__ ring, const FeedPush* __restrict__ push, FeedGeom g,
+                     const FbTables* __restrict__ fbs, const float2* __restrict__ tw1, const float4* __restrict__ tw2_end,
+                     float* __restrict__ frames, int Q) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  float2* zin = reinterpret_cast<float2*>(smem_raw);                                      // (generic arithmetic only)
+  float2* scratch = reinterpret_cast<float2*>(smem_raw + (PP ? 0 : fe_region0_bytes(Q)));
+  __shared__ int band_meta[2 * MELS + 1];
+  __shared__ __align__(16) float srow[2 * MELS];
+  const int tid = threadIdx.x, b = blockIdx.y;
+  const FeedPush fp = push[b];
+  if ((int)blockIdx.x >= fp.n_pairs) return;
+  const long long j = fp.j0 + (long long)blockIdx.x * (3 - g.ncls);
+  const long long a = g.s0 + j * g.hop, ext = g.hop + g.win;                   // first tap (>= 0: the host's range)
+  const long long k_hi = a / g.H;
+  long long k_lo = a + ext - g.W <= 0 ? 0 : (a + ext - g.W + g.H - 1) / g.H;
+  if (g.ncls == 2 && ((k_lo ^ j) & 1)) ++k_lo;      // (odd hf: window k pairs the frames from parity k & 1)
+  if (k_lo > k_hi) return;
+  const FbTables fb = fbs[g.fb_id];
+  load_band_meta<MELS>(band_meta, fb, tid);
+  win_pair<T, MELS, PP>(ring + b * g.stride + a % g.R, (int)ext, 0, g.hop, g.win, true, fb, band_meta, tw1, tw2_end, zin,
+                        scratch, Q, srow);
+  __syncthreads();                                  // srow complete
+  float4* dst = reinterpret_cast<float4*>(frames + ((size_t)b * g.P + (size_t)((j / (3 - g.ncls)) % g.P)) * 2 * MELS);
+  const float4* s4 = reinterpret_cast<const float4*>(srow);
+  for (int u = tid; u < MELS / 2; u += kFeThreads) dst[u] = s4[u];
+}
+
+// The interior rows of a pass's feed windows from the frame ring: grid (block of kFeedRowPairs interior pairs, window).
+// Each window's clip-max key is the max over the rows it holds (order-independent: the same key as computing them).
+__global__ void __launch_bounds__(256)
+feed_rows_kernel(const ClipDesc* __restrict__ clips, const FeedWin* __restrict__ wins, FeedGeom g, int n_mels,
+                 const float* __restrict__ frames, float* __restrict__ mel, unsigned* __restrict__ clipmax) {
+  __shared__ float wred[8];
+  const int c = blockIdx.y;
+  const ClipDesc cd = clips[c];
+  if (cd.n_frames <= 0) return;
+  int lead, tail;
+  interior_pairs(cd.n_frames, cd.n_samples, cd.s0, cd.hop, cd.win, &lead, &tail);
+  const int p0 = lead + blockIdx.x * kFeedRowPairs, p1 = min(tail, p0 + kFeedRowPairs);
+  if (p0 >= p1) return;
+  const FeedWin fw = wins[c];
+  const int q4 = n_mels / 2;                        // float4 per pair (two rows)
+  const float* src = frames + (size_t)fw.feed * g.P * 2 * n_mels;
+  float m = -INFINITY;
+  for (int i = threadIdx.x; i < (p1 - p0) * q4; i += blockDim.x) {
+    const int p = p0 + i / q4, u = i - (i / q4) * q4;
+    const long long slot = ((fw.j0 + 2 * p) / (3 - g.ncls)) % g.P;
+    const float4 v = reinterpret_cast<const float4*>(src + (size_t)slot * 2 * n_mels)[u];
+    reinterpret_cast<float4*>(mel + (size_t)(cd.frame_off + 2 * p) * n_mels)[u] = v;
+    m = fmaxf(m, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
+  }
+  m = warp_max(m);
+  if ((threadIdx.x & 31) == 0) wred[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) m = fmaxf(m, wred[w]);
+    if (m > -INFINITY) atomicMax(clipmax + c, f2key(m));
+  }
+}
+
 // Per-segment lookup rows, built once per pass after the front-end:
 //   seg_frame0[s] = first mel row of segment s,  seg_thr[s] = clipmax(clip) - 80  (top_db)
 __global__ void seg_table_kernel(const ClipDesc* __restrict__ clips, int n_clips,
@@ -785,6 +852,52 @@ void launch_frontend_windows(cudaStream_t st, int n_mels, const void* pcm, int f
 #undef FE_MELS_CASE
     default: break;
   }
+}
+
+template <typename T, int MELS, bool PP>
+static void launch_frontend_feed_t(cudaStream_t st, const T* ring, const FeedPush* push, int n_feeds, int max_pairs,
+                                   const FeedGeom& g, const FbTables* fbs, const float2* tw, float* frames, int Q) {
+  const float4* tw2_end = reinterpret_cast<const float4*>(tw + 4 * 1024);
+  const int smem = PP ? 4 * kScratchPerWarp * 8 : frontend_smem_bytes(Q);
+  if (!PP) {
+    static unsigned long long configured = 0;
+    if (first_launch_on_device(configured))
+      cudaFuncSetAttribute(frontend_feed_kernel<T, MELS, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           frontend_smem_bytes(4));
+  }
+  frontend_feed_kernel<T, MELS, PP><<<dim3(max_pairs, n_feeds), kFeThreads, smem, st>>>(ring, push, g, fbs, tw, tw2_end,
+                                                                                         frames, Q);
+}
+
+template <int MELS>
+static void launch_frontend_feed_mels(cudaStream_t st, const void* ring, int fmt_f32, const FeedPush* push, int n_feeds,
+                                      int max_pairs, const FeedGeom& g, const FbTables* fbs, const float2* tw,
+                                      float* frames) {
+  const int Q = (g.win + 1023) / 1024;
+  const bool pp = Q == 1 && g.hop + g.win <= kSpanMax;    // the clip path's choice (launch_frontend_mels)
+#define FE_FEED(T, PP) launch_frontend_feed_t<T, MELS, PP>(st, (const T*)ring, push, n_feeds, max_pairs, g, fbs, tw, frames, Q)
+  if (fmt_f32) { if (pp) FE_FEED(float, true); else FE_FEED(float, false); }
+  else { if (pp) FE_FEED(short, true); else FE_FEED(short, false); }
+#undef FE_FEED
+}
+
+void launch_frontend_feed_pairs(cudaStream_t st, int n_mels, const void* ring, int fmt_f32, const FeedPush* push, int n_feeds,
+                                int max_pairs, const FeedGeom& g, const FbTables* fbs, const float2* tw, float* frames) {
+  if (max_pairs <= 0 || n_feeds <= 0) return;
+  switch (n_mels) {
+#define FE_MELS_CASE(M) \
+    case M: launch_frontend_feed_mels<M>(st, ring, fmt_f32, push, n_feeds, max_pairs, g, fbs, tw, frames); break;
+    FE_MELS_CASE(32) FE_MELS_CASE(40) FE_MELS_CASE(48) FE_MELS_CASE(64) FE_MELS_CASE(80) FE_MELS_CASE(96) FE_MELS_CASE(128)
+#undef FE_MELS_CASE
+    default: break;
+  }
+}
+
+void launch_feed_rows(cudaStream_t st, int n_mels, const ClipDesc* clips, const FeedWin* wins, int n_clips, int max_interior,
+                      const FeedGeom& g, const float* frames, float* mel, unsigned* clipmax) {
+  if (n_clips <= 0 || max_interior <= 0) return;
+  const dim3 grid((max_interior + kFeedRowPairs - 1) / kFeedRowPairs, n_clips);
+  feed_rows_kernel<<<grid, 256, 0, st>>>(clips, wins, g, n_mels, frames, mel, clipmax);
 }
 
 bool frontend_supports_mels(int n_mels) {

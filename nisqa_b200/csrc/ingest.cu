@@ -98,6 +98,48 @@ void launch_ingest_spans(cudaStream_t st, const IngestSrc& src, const WinSpan* s
   ingest_span_kernel<<<grid, kIngestThreads, 0, st>>>(src, spans, out_f32, out);
 }
 
+// Live feeds: feed b's chunk (clip b of the push) appended to its sample ring, samples t0 .. t0 + n_in - 1 at ring
+// positions t mod R, and again at R + (t mod R) where that is below W (the mirror); grid (sample blocks, feeds).  Up to
+// four contiguous runs, each converted by ingest_clip, so a ring sample is the sample the span ingest would pack.
+template <class Tin, class Tout>
+__device__ __forceinline__ void ingest_feed_runs(const IngestSrc& s, int b, const FeedPush& fp, const FeedGeom& g,
+                                                 Tout* __restrict__ y) {
+  const long long n = fp.n_in, u = fp.t0 % g.R, nA = min(n, (long long)g.R - u);
+  auto run = [&](long long i0, long long len, long long at) {
+    if (len <= 0) return;
+    IngestSrc r = s;
+    r.data = static_cast<const Tin*>(s.data) + i0;
+    ingest_clip<Tin, Tout>(r, b, (int)len, y + at);
+  };
+  run(0, nA, u);                                       // up to the end of the ring
+  run(nA, n - nA, 0);                                  // wrapped to its start
+  run(0, min(nA, (long long)g.W - u), g.R + u);        // the mirror of positions below W
+  run(nA, min(n - nA, (long long)g.W), g.R);
+}
+
+__global__ void __launch_bounds__(kIngestThreads)
+ingest_feed_kernel(IngestSrc s, const FeedPush* __restrict__ push, FeedGeom g, int out_f32, void* __restrict__ ring) {
+  const int b = blockIdx.y;
+  const FeedPush fp = push[b];
+  if (fp.n_in <= 0) return;
+  const long long at = (long long)b * g.stride;
+  if (out_f32) {
+    float* y = static_cast<float*>(ring) + at;
+    if (s.f32) ingest_feed_runs<float, float>(s, b, fp, g, y);
+    else ingest_feed_runs<short, float>(s, b, fp, g, y);
+  } else {
+    ingest_feed_runs<short, short>(s, b, fp, g, static_cast<short*>(ring) + at);
+  }
+}
+
+void launch_ingest_feed(cudaStream_t st, const IngestSrc& src, const FeedPush* push, int n_feeds, long long max_n,
+                        const FeedGeom& g, int out_f32, void* ring) {
+  if (n_feeds <= 0 || max_n <= 0) return;
+  const long long per_block = (long long)kIngestThreads * kIngestPerThread;
+  const dim3 grid((unsigned)std::min<long long>((max_n + per_block - 1) / per_block, 4096), n_feeds);
+  ingest_feed_kernel<<<grid, kIngestThreads, 0, st>>>(src, push, g, out_f32, ring);
+}
+
 void launch_ingest(cudaStream_t st, const IngestSources& src, int first_clip, const ClipDesc* clips, int n_clips,
                    long long max_n, int out_f32, void* out) {
   launch_ingest_rows(st, src, first_clip, clips, n_clips, max_n, out_f32, out);

@@ -13,6 +13,9 @@ namespace nisqa {
 struct ClipDesc;
 struct FbTables;
 struct WinSpan;
+struct FeedGeom;
+struct FeedPush;
+struct FeedWin;
 
 // AdaptCNN's adaptive max-pool output sizes cnn_pool_1 / 2 / 3 as h1 w1 h2 w2 h3 w3 (lib:586-710), shipped 24 x 7, 12 x 5,
 // 6 x 3.  The tensor-core kernels take any [h, w] with w <= kMaxPoolW and (h + 1) (w + 1) <= kMaxPoolCells (one
@@ -113,6 +116,15 @@ void launch_frontend(cudaStream_t st, int n_mels, const void* pcm, int fmt_f32, 
 void launch_frontend_windows(cudaStream_t st, int n_mels, const void* pcm, int fmt_f32, const ClipDesc* clips, int n_clips,
                              int edge_pairs, const WinSpan* spans, int n_spans, int span_pairs, int ncls,
                              const FbTables* fbs, const float2* tw, float* mel, unsigned* clipmax, int Q, int max_span);
+// Live feeds (FeedGeom): the interior frame pairs of a push into the frame ring, once (grid max n_pairs x n_feeds), with
+// the arithmetic the clip path picks for the feed's rate; then, in each pass, the interior rows of the pass's windows
+// from the frame ring into their mel rows, with each window's clip-max key (grid pair blocks x n_clips; the edge pairs
+// come from launch_frontend_windows without spans).  Rows bit-identical to launch_frontend over the windows as clips.
+void launch_frontend_feed_pairs(cudaStream_t st, int n_mels, const void* ring, int fmt_f32, const FeedPush* push, int n_feeds,
+                                int max_pairs, const FeedGeom& g, const FbTables* fbs, const float2* tw, float* frames);
+constexpr int kFeedRowPairs = 32;    // interior pairs per CTA of the row copy
+void launch_feed_rows(cudaStream_t st, int n_mels, const ClipDesc* clips, const FeedWin* wins, int n_clips, int max_interior,
+                      const FeedGeom& g, const float* frames, float* mel, unsigned* clipmax);
 void launch_seg_table(cudaStream_t st, const ClipDesc* clips, int n_clips, const int* seg_prefix, const unsigned* clipmax,
                       int seg_hop, int n_seg, int* seg_frame0, float* seg_thr, int* seg_clip);
 void launch_mel_dump(cudaStream_t st, const float* mel, const ClipDesc* clips, int n_clips, const unsigned* clipmax, int n_mels,
@@ -232,6 +244,9 @@ void launch_ingest(cudaStream_t st, const IngestSources& src, int first_clip, co
 // per span (max_n: the longest span)
 void launch_ingest_spans(cudaStream_t st, const IngestSrc& src, const WinSpan* spans, int n_spans, long long max_n,
                          int out_f32, void* out);
+// Live feeds: the n_in samples of feed b's chunk (clip b of src) appended to its sample ring at t0 (and its mirror)
+void launch_ingest_feed(cudaStream_t st, const IngestSrc& src, const FeedPush* push, int n_feeds, long long max_n,
+                        const FeedGeom& g, int out_f32, void* ring);
 
 // ---------------------------------------------------------------- resample.cpp
 // the interpolation table of the resampler (set by nisqa_resample_set_filter); false before that call

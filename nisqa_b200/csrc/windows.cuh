@@ -1,5 +1,5 @@
-// windows.cuh - the recording spans of nisqa_predict_device_windows, shared by the host runtime (engine.cu), the windows
-// front end (frontend.cu) and the span ingest (ingest.cu).
+// windows.cuh - the recording spans of nisqa_predict_device_windows and the rings of the live feeds (nisqa_feed_*), shared
+// by the host runtime (engine.cu), the windows front end (frontend.cu) and the span and feed ingest (ingest.cu).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -17,6 +17,34 @@ struct WinSpan {
   int n_win;           // leading windows the pass runs (only a recording's last window can be too short)
   int H, hf;           // window hop in samples and in mel frames (H = hf * hop)
   int W;               // window length in samples
+  int pad_;
+};
+
+// Live feeds (nisqa_feed_*): n_feeds recordings that grow push by push.  Feed b's samples live in a ring of R >= W +
+// max_push samples at element b * stride of the sample ring, sample t at t mod R; the first W ring positions are mirrored
+// at R .. R + W - 1 (stride = R + W), so that any W consecutive samples of the recording are contiguous.  Its interior
+// frame pairs (taps inside every window that holds them) are computed once, as soon as their last tap arrives, into a
+// ring of P pair slots of 2 n_mels floats at (b P + slot) 2 n_mels of the frame ring: the pair of global first frame j
+// at slot (j / (3 - ncls)) mod P (ncls 1: windows pair even frames only; 2: the window hop is an odd number of frames,
+// both pairings are kept).
+struct FeedGeom {
+  long long stride;    // elements per feed in the sample ring (R + W)
+  int R, W, H, hf;     // ring length; window length and hop (samples, mel frames)
+  int hop, win, s0;    // the model rate's mel frame hop, window and first tap of frame 0 (ClipDesc)
+  int P, ncls, fb_id;  // pair slots per feed, pairing classes, front-end tables
+  int pad_;
+};
+// One feed in one push (uploaded per push)
+struct FeedPush {
+  long long t0;        // samples of the feed's recording before this push (the ring position of the chunk's first sample)
+  long long j0;        // global first frame of the first pair computed in this push (then j0 + (3 - ncls) x)
+  int n_in;            // samples appended
+  int n_pairs;         // pairs computed
+};
+// One window of a feed in a pass (one per ClipDesc row of the pass)
+struct FeedWin {
+  long long j0;        // global frame of the window's frame 0 (k hf)
+  int feed;
   int pad_;
 };
 

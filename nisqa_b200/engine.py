@@ -40,6 +40,7 @@ EXPORTS = [
     "nisqa_resample_set_filter", "nisqa_resample_out_len", "nisqa_resample_f32",
     "nisqa_resample_device", "nisqa_predict_pcm_resampled", "nisqa_set_cnn_pools", "nisqa_predict_device_batch",
     "nisqa_predict_device_batch_segments", "nisqa_window_counts", "nisqa_predict_device_windows",
+    "nisqa_feed_create", "nisqa_feed_rows", "nisqa_feed_push", "nisqa_feed_device_bytes", "nisqa_feed_destroy",
 ]
 
 
@@ -248,6 +249,18 @@ def load_library(path=None):
     lib.nisqa_window_counts.argtypes = [C.POINTER(NisqaConfig), C.c_int64, C.c_int32, C.c_int64, C.c_int32, i64p, i32p, i32p,
                                         C.c_int64]
     lib.nisqa_window_counts.restype = C.c_int
+    u8p = C.POINTER(C.c_uint8)
+    lib.nisqa_feed_create.argtypes = [vp, C.POINTER(vp), C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int64]
+    lib.nisqa_feed_create.restype = C.c_int
+    lib.nisqa_feed_rows.argtypes = [C.POINTER(NisqaConfig), C.c_int32, C.c_int64, C.c_int32, C.c_int32, i64p, i64p, u8p,
+                                    i64p, i32p, i64p, i32p, i32p, C.c_int64]
+    lib.nisqa_feed_rows.restype = C.c_int
+    lib.nisqa_feed_push.argtypes = [vp, vp, dbp, u8p, vp, C.c_int64, i32p, i64p, i32p, i32p]
+    lib.nisqa_feed_push.restype = C.c_int
+    lib.nisqa_feed_device_bytes.argtypes = [vp]
+    lib.nisqa_feed_device_bytes.restype = C.c_int64
+    lib.nisqa_feed_destroy.argtypes = [vp]
+    lib.nisqa_feed_destroy.restype = None
     lib.nisqa_stage_dump.argtypes = [vp, C.c_int, f32p, C.c_int64]
     lib.nisqa_stage_dump.restype = C.c_int64
     lib.nisqa_segment_counts.argtypes = [C.POINTER(NisqaConfig), C.c_int64, C.c_int32, i32p, i32p, i32p]
@@ -501,6 +514,32 @@ def window_counts(cfg, n_samples, sample_rate, window, hop_frames):
     return nseg, status
 
 
+def _ptr(a, ct):
+    return a.ctypes.data_as(C.POINTER(ct))
+
+
+def feed_rows(cfg, sample_rate, window, hop_frames, held, n_samples, end=None):
+    """(feed int32[N], index int64[N], n_segments int32[N], status int32[N]) of the windows a push of ``n_samples`` samples
+    (and ``end`` flags) to feeds that hold ``held`` samples emits, in feed then window order (nisqa_feed_rows, host
+    arithmetic)"""
+    lib = load_library()
+    held = np.ascontiguousarray(held, dtype=np.int64)
+    ns = np.ascontiguousarray(n_samples, dtype=np.int64)
+    e = None if end is None else np.ascontiguousarray(end, dtype=np.uint8)
+    n = C.c_int64()
+    args = (C.byref(cfg), int(sample_rate), int(window), int(hop_frames), len(held), _ptr(held, C.c_int64),
+            _ptr(ns, C.c_int64), None if e is None else _ptr(e, C.c_uint8), C.byref(n))
+    rc = lib.nisqa_feed_rows(*args, None, None, None, None, 0)
+    if rc != 0:
+        raise EngineError("nisqa_feed_rows failed (%d): window %d, hop_frames %d at %d Hz" % (rc, window, hop_frames,
+                                                                                              sample_rate))
+    feed, index = np.empty(n.value, np.int32), np.empty(n.value, np.int64)
+    nseg, status = np.empty(n.value, np.int32), np.empty(n.value, np.int32)
+    lib.nisqa_feed_rows(*args, _ptr(feed, C.c_int32), _ptr(index, C.c_int64), _ptr(nseg, C.c_int32),
+                        _ptr(status, C.c_int32), n.value)
+    return feed, index, nseg, status
+
+
 class Engine(object):
     """One engine per GPU (rank)."""
 
@@ -517,6 +556,7 @@ class Engine(object):
                 self.h = C.c_void_p()
             raise EngineError("nisqa_create failed (%d): %s" % (rc, msg))
         self.device = int(device)
+        self._feeds = set()                 # nisqa_feed handles, destroyed before the engine
         pools = getattr(cfg, "cnn_pools", None)
         if pools is not None:
             self.set_cnn_pools(pools)
@@ -536,6 +576,8 @@ class Engine(object):
 
     def close(self):
         if getattr(self, "h", None):
+            for f in list(getattr(self, "_feeds", ())):
+                self.feed_destroy(f)
             self.lib.nisqa_drain(self.h)
             self.lib.nisqa_destroy(self.h)
             self.h = C.c_void_p()
@@ -747,6 +789,42 @@ class Engine(object):
             C.c_void_p(scores_dev_ptr), int(n_rows), nseg.ctypes.data_as(C.POINTER(C.c_int32)),
             status.ctypes.data_as(C.POINTER(C.c_int32))), "nisqa_predict_device_windows")
         return nseg, status
+
+    def feed_create(self, n_feeds, sample_rate, window, hop_frames, max_push):
+        """A feed object (nisqa_feed_create) -> its handle (an int)"""
+        h = C.c_void_p()
+        self._check(self.lib.nisqa_feed_create(self.h, C.byref(h), int(n_feeds), int(sample_rate), int(window),
+                                               int(hop_frames), int(max_push)), "nisqa_feed_create")
+        self._feeds.add(h.value)
+        return h.value
+
+    def feed_push(self, feed, stream, chunk, end, scores_dev_ptr, n_rows):
+        """nisqa_feed_push of ``chunk`` (a :func:`device_batch` tuple, 0 samples allowed) and ``end`` (uint8[n_feeds] or
+        None) ordered on ``stream``; the scores of the completed windows to ``scores_dev_ptr`` ([n_rows, n_out] fp32 device
+        memory).  Returns (feed, index, n_segments, status) arrays of n_rows entries, the push's windows first (size
+        n_rows with :func:`feed_rows`), valid on return; raises EngineError, with nothing enqueued, for a refused push."""
+        n = max(int(n_rows), 0)
+        fo, index = np.empty(n, np.int32), np.empty(n, np.int64)
+        nseg, status = np.empty(n, np.int32), np.empty(n, np.int32)
+        e = None if end is None else np.ascontiguousarray(end, dtype=np.uint8)
+        self._check(self.lib.nisqa_feed_push(
+            C.c_void_p(self._feed(feed)), C.c_void_p(stream or None), C.byref(chunk[0]),
+            None if e is None else _ptr(e, C.c_uint8), C.c_void_p(scores_dev_ptr), int(n_rows), _ptr(fo, C.c_int32),
+            _ptr(index, C.c_int64), _ptr(nseg, C.c_int32), _ptr(status, C.c_int32)), "nisqa_feed_push")
+        return fo, index, nseg, status
+
+    def _feed(self, feed):
+        if feed not in self._feeds:
+            raise EngineError("the feed object is closed")
+        return feed
+
+    def feed_device_bytes(self, feed):
+        return int(self.lib.nisqa_feed_device_bytes(C.c_void_p(self._feed(feed))))
+
+    def feed_destroy(self, feed):
+        if feed in self._feeds:
+            self._feeds.discard(feed)
+            self.lib.nisqa_feed_destroy(C.c_void_p(feed))
 
     def _device_batch(self, stream, deg, scores_dev_ptr, ref, target_sr, seg):
         rows = deg[0].n_clips * (2 if ref is not None else 1)

@@ -13,6 +13,10 @@ weight (``nisqa_predict_device_batch_segments``) with its time span.
 
 ``scorer.windows(wave, 48000, 10.0, 1.0)`` scores recordings of any length as a timeline: every 10 s window at a 1 s hop,
 each scored as the clip cut out of the recording would be (``nisqa_predict_device_windows``).
+
+``scorer.feed(256, 48000, 10.0, 1.0)`` scores live sources as their audio arrives: ``feed.push(chunk)`` appends a chunk to
+every source and returns the windows it completed, with the scores ``windows`` gives on the whole recording
+(``nisqa_feed_push``).
 """
 import collections
 import numbers
@@ -31,6 +35,10 @@ Segments = collections.namedtuple("Segments", ["scores", "seg_scores", "seg_weig
 # Scorer.windows: scores [N, n_cols] CUDA tensor (the windows of recording b follow those of the recordings before it,
 # counts[b] of them); t_start / t_end float64 [N] seconds, n_segments / status int32 [N] host arrays
 Windows = collections.namedtuple("Windows", ["scores", "counts", "t_start", "t_end", "n_segments", "status"])
+# Feed.push: scores [N, n_cols] CUDA tensor of the windows the push completed, by feed then window index; feed int32 [N],
+# index int64 [N] (window k of the feed's current recording), t_start / t_end float64 [N] seconds, n_segments / status
+# int32 [N] host arrays
+FeedRows = collections.namedtuple("FeedRows", ["scores", "feed", "index", "t_start", "t_end", "n_segments", "status"])
 
 
 def window_geometry(args, rate, window_s, window_hop_s):
@@ -177,6 +185,36 @@ class Scorer(object):
         cat = lambda parts, dt: np.concatenate(parts).astype(dt) if parts else np.zeros(0, dt)      # noqa: E731
         return Windows(out, counts, cat(t0, np.float64), cat(t1, np.float64), cat(nseg, np.int32), cat(st, np.int32))
 
+    def feed(self, n_feeds, sample_rate, window_s, window_hop_s, channel=None, max_push_s=None):
+        """A :class:`Feed` of ``n_feeds`` live recordings at ``sample_rate``, scored as the windows of :meth:`windows`
+        (``window_s``, ``window_hop_s``, checked alike) as soon as each window is complete.  ``channel`` applies to every
+        push (None: the mono mix); ``max_push_s`` (default ``window_s``) is the longest chunk one push may append to one
+        feed, which sizes the feed's device rings.  A checkpoint with ``ms_sr`` takes feeds at that rate only."""
+        if self.double_ended:
+            raise ValueError("feed: a double-ended (NISQA_DE) checkpoint scores (wave, reference) pairs, not live feeds")
+        if isinstance(n_feeds, bool) or not isinstance(n_feeds, numbers.Integral) or not 1 <= n_feeds <= 65535:
+            raise ValueError("n_feeds: an int within 1 .. 65535, not %r" % (n_feeds,))
+        if isinstance(sample_rate, bool) or not isinstance(sample_rate, numbers.Integral) or sample_rate <= 0:
+            raise ValueError("sample_rate must be a positive int, not %r" % (sample_rate,))
+        if self.target_sr and sample_rate != self.target_sr:
+            raise ValueError("sample_rate: %d Hz, but the checkpoint resamples to ms_sr=%d; a feed takes audio at ms_sr"
+                             % (sample_rate, self.target_sr))
+        if channel is not None and (isinstance(channel, bool) or not isinstance(channel, numbers.Integral) or channel < 0):
+            raise TypeError("channel: a non-negative int or None, not %r" % (channel,))
+        W, hop_frames = window_geometry(self.args, sample_rate, window_s, window_hop_s)
+        _, n_seg, status = E.segment_counts(self.cfg, W, sample_rate)
+        if status != E.CLIP_OK:
+            a = self.args
+            err = E.clip_status_error(status, "window_s=%r (%d samples at %d Hz)" % (window_s, W, sample_rate), W,
+                                      sample_rate, n_seg, a["ms_hop_length"], a["ms_seg_length"], a["ms_max_segments"])
+            raise ValueError("window_s: " + str(err))
+        if max_push_s is None:
+            max_push_s = window_s
+        if isinstance(max_push_s, bool) or not isinstance(max_push_s, numbers.Real) or not np.isfinite(max_push_s) \
+                or max_push_s <= 0 or int(round(max_push_s * sample_rate)) < 1:
+            raise ValueError("max_push_s: a positive number of seconds (at least one sample), not %r" % (max_push_s,))
+        return Feed(self, int(n_feeds), int(sample_rate), W, hop_frames, channel, int(round(max_push_s * sample_rate)))
+
     # ------------------------------------------------------------------ shared by __call__ and segments
     def _arguments(self, wave, sample_rate, lengths, channel, reference, reference_lengths, reference_sample_rate):
         """-> (deg, ref or None, segment counts of wave's clips) after every check, before anything is enqueued"""
@@ -209,8 +247,8 @@ class Scorer(object):
         return out[0::2].contiguous() if ref is not None else out
 
     # ------------------------------------------------------------------ arguments
-    def _batch(self, name, x, sample_rate, lengths, channel):
-        """-> engine.device_batch(...) of one batch argument, after the argument checks"""
+    def _batch(self, name, x, sample_rate, lengths, channel, min_len=1):
+        """-> engine.device_batch(...) of one batch argument, after the argument checks (lengths >= min_len)"""
         if not isinstance(x, torch.Tensor):
             raise TypeError("%s: a torch.Tensor on the GPU, not %s" % (name, type(x).__name__))
         if x.dtype not in (torch.int16, torch.float32):
@@ -247,9 +285,9 @@ class Scorer(object):
             ns = ns.astype(np.int64)
             if ns.shape[0] != B:
                 raise ValueError("%s: %d entries for %d clips" % (what, ns.shape[0], B))
-            bad = np.nonzero((ns < 1) | (ns > T))[0]
+            bad = np.nonzero((ns < min_len) | (ns > T))[0]
             if bad.size:
-                raise ValueError("%s[%d] = %d: not within 1 .. %d samples" % (what, bad[0], ns[bad[0]], T))
+                raise ValueError("%s[%d] = %d: not within %d .. %d samples" % (what, bad[0], ns[bad[0]], min_len, T))
         fmt = E.FMT_S16 if x.dtype == torch.int16 else E.FMT_F32
         return E.device_batch(x3.data_ptr(), fmt, ns, C, ch, T, x3.stride(0), x3.stride(1), int(sample_rate))
 
@@ -269,3 +307,82 @@ class Scorer(object):
                 raise err
             counts.append(n_seg)
         return counts
+
+
+class Feed(object):
+    """Live recordings scored window by window as their samples arrive (``Scorer.feed``).  Holds device rings of
+    ``device_bytes`` bytes until ``close()``.  Pushes are ordered on ``torch.cuda.current_stream()`` at each call; the
+    feed runs them in push order whatever streams they come from."""
+
+    def __init__(self, scorer, n_feeds, sample_rate, W, hop_frames, channel, max_push):
+        self.scorer, self.n_feeds, self.sample_rate, self.channel, self.max_push = scorer, n_feeds, sample_rate, channel, max_push
+        self.window, self.hop_frames = W, hop_frames
+        self.hop = hop_frames * int(sample_rate * scorer.args["ms_hop_length"])
+        self.held = np.zeros(n_feeds, np.int64)          # samples of each feed's current recording
+        self._fmt = None                                  # the format the feeds' samples are held in
+        self._h = scorer.engine.feed_create(n_feeds, sample_rate, W, hop_frames, max_push)
+
+    @property
+    def device_bytes(self):
+        return self.scorer.engine.feed_device_bytes(self._h)
+
+    def close(self):
+        if self._h is not None:
+            self.scorer.engine.feed_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def push(self, wave, lengths=None, end=None):
+        """Append a chunk to every feed and score the windows it completes -> :data:`FeedRows`.
+
+        wave    : [B, T] or [B, C, T] int16 / float32 CUDA tensor, B = n_feeds (a [T] tensor for one feed), T >= 0
+        lengths : host ints, the samples of each feed's chunk, 0 .. T and at most max_push_s (default T)
+        end     : host bools, one per feed: the feed's recording ends after this chunk; its remaining windows are scored
+                  as ``Scorer.windows`` scores the last ones (the last may be short: NaN, CLIP_TOO_SHORT) and the next
+                  sample pushed to it starts a new recording
+        Window k of a feed is emitted by the first push after which the feed holds k H + W samples of its recording,
+        with the scores ``Scorer.windows`` gives that window of the whole recording, bit for bit.
+        """
+        if self._h is None:
+            raise ValueError("push: the feed is closed")
+        if isinstance(wave, torch.Tensor) and wave.shape[-1] == 0:
+            if lengths is not None and np.any(np.asarray(lengths) != 0):
+                raise ValueError("lengths: a chunk of 0 samples holds no sample")
+            wave = torch.zeros(tuple(wave.shape[:-1]) + (1,), dtype=wave.dtype, device=wave.device)
+            lengths = [0] * (wave.shape[0] if wave.dim() > 1 else 1)
+        deg = self.scorer._batch("wave", wave, self.sample_rate, lengths, self.channel, min_len=0)
+        b, ns = deg
+        if b.n_clips != self.n_feeds:
+            raise ValueError("wave: %d feeds (clips) in the chunk for a feed object of %d feeds" % (b.n_clips, self.n_feeds))
+        over = np.nonzero(ns > self.max_push)[0]
+        if over.size:
+            raise ValueError("lengths[%d] = %d: more than max_push_s (%d samples)" % (over[0], ns[over[0]], self.max_push))
+        if end is None:
+            ends = np.zeros(self.n_feeds, np.uint8)
+        else:
+            ends = np.asarray(end.tolist() if isinstance(end, torch.Tensor) else end)
+            if ends.shape != (self.n_feeds,) or not (ends.dtype == np.bool_ or np.issubdtype(ends.dtype, np.integer)):
+                raise ValueError("end: one bool per feed (%d), not %r" % (self.n_feeds, end))
+            ends = ends.astype(bool).astype(np.uint8)
+        fmt = E.FMT_S16 if b.sample_fmt == E.FMT_S16 and (b.n_channels == 1 or b.channel >= 0) else E.FMT_F32
+        if ns.sum() > 0 and self.held.sum() > 0 and fmt != self._fmt:
+            raise ValueError("wave: %s samples, but the feeds hold %s ones until every feed has ended" % (
+                "mono int16" if fmt == E.FMT_S16 else "float32 (or mixed)",
+                "mono int16" if self._fmt == E.FMT_S16 else "float32 (or mixed)"))
+        eng = self.scorer.engine
+        feed, index, _, _ = E.feed_rows(self.scorer.cfg, self.sample_rate, self.window, self.hop_frames, self.held, ns, ends)
+        N = feed.shape[0]
+        out = torch.empty((N, len(self.scorer.columns)), dtype=torch.float32, device=self.scorer.device)
+        f2, i2, nseg, status = eng.feed_push(self._h, self.scorer._stream(), deg, ends, out.data_ptr(), N)
+        T = self.held + ns
+        t_start = index * self.hop / self.sample_rate
+        t_end = np.minimum(index * self.hop + self.window, T[feed]) / self.sample_rate
+        if ns.sum() > 0:
+            self._fmt = fmt
+        self.held = np.where(ends.astype(bool), 0, T)
+        return FeedRows(out, f2, i2, t_start, t_end, nseg, status)

@@ -4,7 +4,7 @@
 # short clips at 48 / 16 kHz: front-end, conv1, the five wgmma conv layers with their bulk copies /
 # mbarriers, self-attention, pooling), over a 96 kHz clip (frontend_kernel, the front end for windows over 1024
 # samples), over a short nisqa_tts.tar call (StandardCNN, BiLSTM) and over device-batch
-# calls (the ingest kernel, with and without ms_sr, one segments call and two windows calls); racecheck over the double-ended alignment's multi-block path.
+# calls (the ingest kernel, with and without ms_sr, one segments call, two windows calls and a live feed); racecheck over the double-ended alignment's multi-block path.
 #   bash tools/sanitize.sh TAG
 TAG=${1:-rXX}
 OUT=gpurun_out
@@ -75,6 +75,15 @@ s6 = Scorer(os.path.join("weights", "nisqa.tar"))
 r = torch.from_numpy(synth.synth_speech_pcm16(16, 25.0, 48000)).cuda()
 print("windows", s6.windows(r, 48000, 10.0, 3.33).scores.tolist())
 print("windows 96 kHz", s6.windows(torch.from_numpy(synth.synth_speech_pcm16(17, 12.0, 96000)).cuda(), 96000, 10.0, 1.0).scores.tolist())
+# live feeds (ingest_feed_kernel, frontend_feed_kernel, feed_rows_kernel, and frontend_windows_kernel's edge pairs over
+# the rings): two feeds of 12.5 s and 3 s at a 3.33 s hop (both pairings) in 0.7 s pushes, ring wrap and mirror included
+fd = s6.feed(2, 48000, 10.0, 3.33, max_push_s=0.7)
+n, T = 33600, 600000
+for t in range(0, T, n):
+    m = [min(n, T - t), min(n, max(0, 144000 - t))]
+    out = fd.push(torch.stack([r[t:t + n], r[t:t + n]]), lengths=m, end=[t + n >= T, t < 144000 <= t + n])
+    print("feed", out.scores.tolist())
+fd.close()
 s6.close()
 PY
 timeout 400 compute-sanitizer --tool memcheck --error-exitcode 7 --log-file $OUT/${TAG}_memcheck.log python /tmp/san_run.py > $OUT/${TAG}_memcheck_stdout.log 2>&1
