@@ -37,8 +37,8 @@
 //   wgmmas run.  Where the staging tile does not alias the A tile, the A tile is double-buffered (conv_split_kernel).
 //
 // The fused kernel (conv12_kernel) also computes conv1 + BN + ReLU + pool1 of the tile's segment straight into the A
-// tile, so pool1 never reaches HBM; two warpgroups run the GEMM while the other two compute conv1 of the next tile
-// and the epilogue of the previous one.
+// tile, so pool1 never reaches HBM; two warpgroups take alternate tiles, GEMM and epilogue, so that one's epilogue runs
+// under the other's GEMM, while the other two compute conv1 of the tiles ahead.
 #include <cuda_fp16.h>
 
 #include <algorithm>
@@ -63,8 +63,8 @@ struct TapUnits {
                        N = C::NTAP * PER_TAP;
 };
 
-// A fragments of K steps k0 .. k0 + UK - 1 of one tap (row offset tapoff) for this warpgroup's NB m64 blocks: block b
-// reads tile row row[b] + tapoff
+// A fragments of K steps k0 .. k0 + UK - 1 of one tap (row offset tapoff) for NB m64 blocks: block b reads tile row
+// row[b] + tapoff
 template <class C, int NB>
 __device__ __forceinline__ void load_unit(uint32_t a_hi, uint32_t a_lo, const int (&row)[NB], int tapoff, int k0, int lchunk,
                                           uint32_t (&ah)[NB][TapUnits<C>::UK][4], uint32_t (&al)[NB][TapUnits<C>::UK][4]) {
@@ -117,19 +117,26 @@ __device__ __forceinline__ void tile_gemm(float (&acc_m)[NB][C::COUT / 2], float
   for (int b = 0; b < NB; ++b)
 #pragma unroll
     for (int i = 0; i < C::COUT / 2; ++i) { acc_m[b][i] = 0.f; acc_s[b][i] = 0.f; }
-  // one unit in flight: unit u + 1's fragments load into the other register set while unit u's wgmmas run
-  uint32_t ah[2][NB][UK][4], al[2][NB][UK][4];
-  load_unit<C, NB>(a_hi, a_lo, row, -P - C::PADX, 0, lchunk, ah[0], al[0]);
+  // one step (unit u of block b, in the order u, then b) in flight: step v + 1's fragments load into the other register
+  // set while step v's wgmmas run.  Each accumulator still sees its taps in order.
+  using Acc1 = float[1][C::COUT / 2];
+  constexpr int NS = U::N * NB;
+  uint32_t ah[2][1][UK][4], al[2][1][UK][4];
+  const int row0[1] = {row[0]};
+  load_unit<C, 1>(a_hi, a_lo, row0, -P - C::PADX, 0, lchunk, ah[0], al[0]);
 #pragma unroll
-  for (int u = 0; u < U::N; ++u) {
+  for (int v = 0; v < NS; ++v) {
+    const int u = v / NB, b = v % NB;
     wgmma_fence();
-    mma_unit<C, NB>(acc_m, acc_s, ah[u & 1], al[u & 1], b_base + (u / PT) * C::B_STAGE, (u % PT) * UK);
+    mma_unit<C, 1>(reinterpret_cast<Acc1&>(acc_m[b]), reinterpret_cast<Acc1&>(acc_s[b]), ah[v & 1], al[v & 1],
+                   b_base + (u / PT) * C::B_STAGE, (u % PT) * UK);
     wgmma_commit();
-    if (u + 1 < U::N) {
-      wgmma_wait<1>();                           // unit u - 1 is done with the set that unit u + 1 loads into
-      const int v = u + 1, t = v / PT;
-      load_unit<C, NB>(a_hi, a_lo, row, (t / C::KX - 1) * P + (t % C::KX - C::PADX), (v % PT) * UK, lchunk, ah[v & 1],
-                       al[v & 1]);
+    if (v + 1 < NS) {
+      wgmma_wait<1>();                           // step v - 1 is done with the set that step v + 1 loads into
+      const int nu = (v + 1) / NB, t = nu / PT;
+      const int rown[1] = {row[(v + 1) % NB]};
+      load_unit<C, 1>(a_hi, a_lo, rown, (t / C::KX - 1) * P + (t % C::KX - C::PADX), (nu % PT) * UK, lchunk,
+                      ah[(v + 1) & 1], al[(v + 1) & 1]);
     }
   }
   wgmma_wait<0>();
@@ -367,18 +374,20 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
 // ---- conv1 + pool1 + conv2 + pool2 ----
 // conv1 + BN + ReLU + pool1 (conv1_cell.cuh, the same fp32 arithmetic as conv1_pool1_kernel) of one segment per tile
 // goes straight into the A tile; the conv2 GEMM and epilogue are the same code on the same values as conv_split_kernel,
-// so results are bit-identical to the separate kernels.  The persistent CTA splits into two roles:
-//   warpgroups 0, 1 (MMA):   wait A full[i & 1]; GEMM of m64 blocks 0, 1 (warpgroup 0) or block 2 (warpgroup 1);
-//                            arrive A empty[i & 1]; bias + ReLU into staging tile i & 1; named barrier of the 256 MMA
-//                            threads; max-pool / split / store of tile i
-//   warpgroups 2, 3 (conv1): one thread copies the mel block of tile i + 3 into the mel ring; wait mel full[(i + 1) % 4]
-//                            and A empty[(i + 1) & 1]; conv1 of tile i + 1 from the ring into A buffer (i + 1) & 1;
-//                            arrive mel empty and A full
-// so conv1 of the next tile runs while the tensor cores work on this one, and its mel reads never wait for global
-// memory.  The A and mel empty barriers count the 256 threads of the role that arrives on them (mel full: the copying
-// thread, plus the copy's bytes); a barrier's k-th use waits on parity k & 1 (full) or (k & 1) ^ 1 (empty: a fresh
-// barrier's "previous phase" counts as complete).  Staging tile i & 1 is next written at tile i + 2, after the named
-// barrier of tile i + 1, which every MMA thread reaches only after its part of tile i's store.
+// so results are bit-identical to the separate kernels.  The persistent CTA splits into two roles, and the CTA's i-th
+// tile goes to MMA warpgroup i & 1 (ping-pong):
+//   warpgroup w = i & 1 (MMA): wait A full[i % 3]; GEMM of m64 blocks 0, 1, 2; arrive A empty[i % 3]; named barrier
+//                            of its 128 threads; bias + ReLU into its staging tile w; named barrier; max-pool / split /
+//                            store of tile i
+//   warpgroups 2, 3 (conv1): one thread copies the mel block of tile i + 2 into the mel ring; wait A empty[i % 3] and
+//                            mel full[i % 4]; conv1 of tile i from the ring into A buffer i % 3; arrive mel empty and
+//                            A full
+// so one MMA warpgroup's epilogue runs under the other's GEMM, conv1 fills tile i + 2 while tiles i and i + 1 are read,
+// and conv1's mel reads never wait for global memory (the copy is issued two conv1 tiles ahead however far conv1 runs
+// ahead of the GEMMs).  A full and mel empty count the 256 conv1 threads, A empty the 128 threads of the tile's MMA
+// warpgroup (mel full: the copying thread, plus the copy's bytes); a barrier's k-th use waits on parity k & 1 (full) or
+// (k & 1) ^ 1 (empty: a fresh barrier's "previous phase" counts as complete).  A warpgroup writes its staging tile only
+// after the first named barrier of its next tile, which each of its threads reaches after its part of the store.
 template <class C, int MODE>
 __global__ void __launch_bounds__(C::NT, 1)
 conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, float out_scale, float store_scale,
@@ -388,25 +397,28 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
               float c1_scale /*2^-e1: conv1's activation scale*/) {
   using L = SpFused<C>;
   constexpr C g{};
-  constexpr int W = C::W, P = C::P, HALO = C::HALO, ROWB = C::ROWB, NT = C::NT, NR = NT / 2;
+  constexpr int W = C::W, P = C::P, HALO = C::HALO, ROWB = C::ROWB, NT = C::NT, NR = NT / 2, AB = L::A_BUFS;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const uint32_t sbase = smem_u32(smem);
   const uint32_t b_base = sbase + L::OFF_B;
-  const uint32_t bar_w = sbase + L::OFF_BAR, a_full = bar_w + 8 * 9, a_empty = a_full + 16;
-  const uint32_t mel_full = a_empty + 16, mel_empty = mel_full + 8 * L::MEL_R;
+  const uint32_t bar_w = sbase + L::OFF_BAR, a_full = bar_w + 8 * 9, a_empty = a_full + 8 * AB;
+  const uint32_t mel_full = a_empty + 8 * AB, mel_empty = mel_full + 8 * L::MEL_R;
   float* ws = reinterpret_cast<float*>(smem + L::OFF_W1);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);   // warp-uniform as far as ptxas can tell: the role branch
                                                            // below must not count as divergent around the wgmmas
   const int n_tiles = n_seg;                     // G == 1
 
-  // the zero row / zero column / halo rows of both A buffers are never written again
-  for (int i = tid; i < 2 * C::A_BUF / 16; i += NT) reinterpret_cast<uint4*>(smem + L::OFF_A)[i] = make_uint4(0u, 0u, 0u, 0u);
+  // the zero row / zero column / halo rows of the A buffers are never written again
+  for (int i = tid; i < AB * C::A_BUF / 16; i += NT) reinterpret_cast<uint4*>(smem + L::OFF_A)[i] = make_uint4(0u, 0u, 0u, 0u);
   for (int i = tid; i < 9 * 16 + 16; i += NT) ws[i] = (i < 144) ? __ldg(w1 + i) : __ldg(b1 + i - 144);
   if (tid == 0) {
     for (int t = 0; t < 9; ++t) mbar_init(bar_w + 8 * t, 1);
-    for (int b = 0; b < 4; ++b) mbar_init(a_full + 8 * b, NR);
+    for (int b = 0; b < AB; ++b) {
+      mbar_init(a_full + 8 * b, NR);
+      mbar_init(a_empty + 8 * b, 128);
+    }
     for (int s = 0; s < L::MEL_R; ++s) {
       mbar_init(mel_full + 8 * s, 1);
       mbar_init(mel_empty + 8 * s, NR);
@@ -419,47 +431,41 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
   }
   __syncthreads();
 
-  // registers: 64 accumulators and two fragment sets per MMA thread; 2 x 128 x (160 + 96) = the whole register file
+  // registers: 96 accumulators and two fragment sets per MMA thread (at 160, ptxas spills in the AdaptCNN instance), the
+  // conv1 role spill-free in 88; 2 x 128 x (168 + 88) = the whole register file
   if (wg < 2) {
-    // ===== MMA warpgroups: warpgroup 0 runs m64 blocks 0 and 1 (GEMM rows 0 .. 127), warpgroup 1 block 2 (rows
-    // 128 .. 191); block 3 would hold only rows m >= KEPT, which are never staged =====
-    setmaxnreg_inc<160>();
+    // ===== MMA warpgroups: warpgroup wg runs the CTA's tiles wg, wg + 2, ..., all three m64 blocks (GEMM rows
+    // 0 .. 191) of each; block 3 would hold only rows m >= KEPT, which are never staged =====
+    setmaxnreg_inc<168>();
     const int lm = (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;   // ldmatrix row within an m64 block
     const int am = (warp & 3) * 16 + (lane >> 2);                          // accumulator row within an m64 block
     const int lchunk = lane >> 4;
     const int acol = 2 * (lane & 3);
-    // the whole tile loop of a warpgroup that owns NB blocks from block b0 on: the branch between the two instances is
-    // taken once, outside the loop, on the warp-uniform wg
     float2 bb[C::COUT / 8];
     load_bias<C>(bias, acol, bb);
     wait_weights<C>(bar_w);
-    auto mma_role = [&](auto nb, int b0) {
-      constexpr int NB = decltype(nb)::value;
-      int lrow[NB];
+    int lrow[3];
 #pragma unroll
-      for (int b = 0; b < NB; ++b) lrow[b] = HALO + gemm_row(g, lm + 64 * (b0 + b));
-      int it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-        const int ab = it & 1;
-        const uint32_t par = (uint32_t)(it >> 1) & 1u;
-        mbar_wait(a_full + 8 * ab, par);
-        const uint32_t a_hi = sbase + L::OFF_A + ab * C::A_BUF, a_lo = a_hi + C::A_BYTES;
-        float acc_m[NB][C::COUT / 2], acc_s[NB][C::COUT / 2];
-        tile_gemm<C, NB>(acc_m, acc_s, a_hi, a_lo, b_base, lrow, lchunk, P);
-        mbar_arrive(a_empty + 8 * ab);
-        float* stg = reinterpret_cast<float*>(smem + L::OFF_STG + ab * C::STG_BYTES);
+    for (int b = 0; b < 3; ++b) lrow[b] = HALO + gemm_row(g, lm + 64 * b);
+    float* stg = reinterpret_cast<float*>(smem + L::OFF_STG + wg * C::STG_BYTES);
+    const uint32_t own_bar = 1 + wg;             // named barrier of this warpgroup's 128 threads
+    int it = wg;
+    for (int tile = blockIdx.x + wg * gridDim.x; tile < n_tiles; tile += 2 * gridDim.x, it += 2) {
+      const int ab = it % AB;
+      mbar_wait(a_full + 8 * ab, (uint32_t)(it / AB) & 1u);
+      const uint32_t a_hi = sbase + L::OFF_A + ab * C::A_BUF, a_lo = a_hi + C::A_BYTES;
+      float acc_m[3][C::COUT / 2], acc_s[3][C::COUT / 2];
+      tile_gemm<C, 3>(acc_m, acc_s, a_hi, a_lo, b_base, lrow, lchunk, P);
+      mbar_arrive(a_empty + 8 * ab);
+      named_bar_sync<128>(own_bar);              // this warpgroup's store of tile i - 2 is done with the staging tile
 #pragma unroll
-        for (int b = 0; b < NB; ++b)
-          stage_rows<C>(g, acc_m[b], acc_s[b], am + 64 * (b0 + b), acol, tile, n_seg, bb, out_scale, stg);
-        named_bar_sync<1, NR>();
-        store_tile<C>(g, stg, tile, 1, tid, NR, store_scale, out_hi, out_lo, nullptr);
-      }
-    };
-    if (wg == 0) mma_role(std::integral_constant<int, 2>(), 0);
-    else mma_role(std::integral_constant<int, 1>(), 2);
+      for (int b = 0; b < 3; ++b) stage_rows<C>(g, acc_m[b], acc_s[b], am + 64 * b, acol, tile, n_seg, bb, out_scale, stg);
+      named_bar_sync<128>(own_bar);
+      store_tile<C>(g, stg, tile, 1, tid - 128 * wg, 128, store_scale, out_hi, out_lo, nullptr);
+    }
   } else {
     // ===== worker warpgroups =====
-    setmaxnreg_dec<96>();
+    setmaxnreg_dec<88>();
     const int wt = tid - NR;
     constexpr int R = L::MEL_R, MEL_FLOATS = L::MEL_BYTES / 4;
     const float* ring = reinterpret_cast<const float*>(smem + L::OFF_MEL);
@@ -488,14 +494,17 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
       prefetch_seg(0);
       for (int k = 0; k < R - 2; ++k) issue_mel(k);
     }
-    // conv1 + BN + ReLU + pool1 of the CTA's j-th segment (mel ring slot j % R) into A buffer j & 1.  Thread wt < 192
-    // owns one strip for the kernel's life: pooled row ph, channel quad cq, and the left (pw < W / 2) or right half of
-    // the pooled cells (warp-uniform: 96 strips = 3 warps per half); conv1_strip computes each conv1 output position
-    // of the strip once.  The quad's weights and biases stay in registers.  A warp's lanes run over cq, then ph: its 8
-    // distinct mel addresses are rows 2 apart, on distinct banks.  Each cell -> one 8-byte half of a 16-byte chunk.
-    constexpr int NSTRIP = 2 * 4 * 24;
-    const int cq = wt & 3, ph = (wt >> 2) % 24;
-    const bool right = __shfl_sync(0xffffffffu, wt >= NSTRIP / 2, 0);
+    // conv1 + BN + ReLU + pool1 of the CTA's j-th segment (mel ring slot j % R) into A buffer j % AB.  Lane < 24 of
+    // each of the 8 conv1 warps owns one strip for the kernel's life: pooled row ph, channel quad cq, and the left
+    // (pw < W / 2) or right half of the pooled cells (warp-uniform: 96 strips = 4 warps per half); conv1_strip computes
+    // each conv1 output position of the strip once.  24 strips in each warp rather than 32 in each of 6 give each of the
+    // four SM sub-partitions (warp w on sub-partition w % 4) two conv1 warps and the same share of the conv1 work.  The
+    // quad's weights and biases stay in registers.  A warp's lanes run over cq, then ph: its 6 distinct mel addresses
+    // are rows 2 apart, on distinct banks.  Each cell -> one 8-byte half of a 16-byte chunk.
+    constexpr int NSTRIP = 2 * 4 * 24, SPW = NSTRIP / (NR / 32);
+    const int strip = (wt >> 5) * SPW + lane;
+    const int cq = strip & 3, ph = (strip >> 2) % 24;
+    const bool right = __shfl_sync(0xffffffffu, strip >= NSTRIP / 2, 0);
     float wq[9][4], bq[4];
 #pragma unroll
     for (int t = 0; t < 9; ++t)
@@ -504,9 +513,9 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
 #pragma unroll
     for (int c = 0; c < 4; ++c) bq[c] = ws[144 + cq * 4 + c];
     auto fill = [&](int j) {
-      const int b = j & 1, s = j % R;
+      const int b = j % AB, s = j % R;
       if (wt == 0) issue_mel(j + R - 2);         // its slot held segment j - 2
-      mbar_wait(a_empty + 8 * b, ((uint32_t)(j >> 1) & 1u) ^ 1u);
+      mbar_wait(a_empty + 8 * b, ((uint32_t)(j / AB) & 1u) ^ 1u);
       mbar_wait(mel_full + 8 * s, (uint32_t)(j / R) & 1u);
       unsigned char* a = smem + L::OFF_A + b * C::A_BUF;
       const float* slot = ring + s * MEL_FLOATS;
@@ -518,7 +527,7 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
         *reinterpret_cast<uint2*>(a + o) = hi;
         *reinterpret_cast<uint2*>(a + C::A_BYTES + o) = lo;
       };
-      if (wt < NSTRIP) {
+      if (lane < SPW) {
         if (right) conv1_strip<MODE, W / 2, W, kMels>(slot, thr, wq, bq, ph, emit);
         else conv1_strip<MODE, 0, W / 2, kMels>(slot, thr, wq, bq, ph, emit);
       }

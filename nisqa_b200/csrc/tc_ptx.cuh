@@ -51,6 +51,8 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 // barrier ID among the first N threads that reach it (N a multiple of 32; ID 0 is __syncthreads)
 template <int ID, int N> __device__ __forceinline__ void named_bar_sync() { asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(N) : "memory"); }
+// the same with a warp-uniform run-time ID
+template <int N> __device__ __forceinline__ void named_bar_sync(uint32_t id) { asm volatile("bar.sync %0, %1;" ::"r"(id), "n"(N) : "memory"); }
 
 // per-thread register budget of the calling warpgroup, raised (waits for registers released by others) or lowered
 template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
