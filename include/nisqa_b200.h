@@ -296,6 +296,38 @@ NISQA_API int  nisqa_predict_device_batch_segments(nisqa_engine* e, void* cuda_s
                                                    const nisqa_segment_out* seg, int32_t* n_segments_out,
                                                    int32_t* status_out);
 
+/* Quality embeddings: the representation behind the scores, as nisqa_predict_device_batch_embeddings writes it.  x are
+ * the rows the pooling module reads (the rows NISQA_STAGE_TD_OUT documents, in the reference's column order; NISQA_DE:
+ * td_2's rows of the degraded clip), S of them per clip, `width` columns each (nisqa_embedding_width).  For pooling
+ * head h (n_out of them):
+ *   pooled[g][h] : the input of the head's last Linear (PoolAttFF linear3, PoolAtt linear2, else linear), so that its
+ *                  score is pooled[g][h] . w + b: PoolAtt / PoolAttFF sum_t a_t x_t with the head's softmax weights (the
+ *                  weights nisqa_predict_device_batch_segments reports); PoolAvg (sum_t x_t) / S; PoolMax the column-wise
+ *                  max; PoolLastStep x_{S-1}; PoolLastStepBi the forward half of x_{S-1} and the backward half of x_0.
+ *                  Modules without parameters give every head the same vector.  Rows g as scores_dev (NISQA_DE: 2p + 1
+ *                  is the reference clip's row); clips whose status is not OK, reference clips, and clips that score
+ *                  NaN while their status is OK (NISQA_DE: a reference that is too short or too long) get NaN.
+ *   rows         : x itself, one row per segment of every OK clip in clip order, none for the others and none for
+ *                  NISQA_DE's reference clips (the row table of nisqa_segment_out); NaN rows where pooled is NaN. */
+typedef struct nisqa_embedding_out {
+  float*  pooled;    /* device [rows][n_out][width] fp32 (rows as scores_dev) */
+  float*  rows;      /* device [n_rows][width] fp32, or NULL: no per-segment rows */
+  int64_t n_rows;    /* rows `rows` holds (ignored when rows == NULL) */
+} nisqa_embedding_out;
+
+/* The width of the embedding rows of the loaded checkpoint (NISQA_ERR_STATE before nisqa_load_weights). */
+NISQA_API int  nisqa_embedding_width(const nisqa_engine* e, int32_t* width);
+
+/* nisqa_predict_device_batch that also writes the embeddings to emb, with the same stream contract and no host wait of
+ * its own.  NISQA_ERR_INVALID before anything is enqueued when emb or emb->pooled is NULL, or when emb->rows is given
+ * and emb->n_rows is smaller than the segment count of the call's OK (non-reference) clips.  scores_dev gets the same
+ * values as nisqa_predict_device_batch would write.  The shipped nisqa_tts.tar shape stores the per-step BiLSTM outputs
+ * in such a call (as "keep_td_out" does, without changing that option). */
+NISQA_API int  nisqa_predict_device_batch_embeddings(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                                                     const nisqa_device_batch* ref, int32_t target_sr, float* scores_dev,
+                                                     const nisqa_embedding_out* emb, int32_t* n_segments_out,
+                                                     int32_t* status_out);
+
 /* Recordings of any length scored as a timeline of overlapping windows, each window scored exactly as the clip cut out of
  * the recording would be (its own reflect padding, top_db maximum, segment count and status).  At the model rate sr
  * (target_sr when set, else the batch's sample_rate; an ms_sr checkpoint converts each WHOLE recording first) a

@@ -14,6 +14,11 @@ or a machine without CUDA raises.
 segment of every file with its time span, its score under each pooling head and the head's pooling weight
 (:meth:`nisqa_b200.scorer.Scorer.segments`).  Single process only.
 
+``args['embeddings']`` (``run_predict.py --embeddings``) also writes ``NISQA_embeddings.npz`` into ``output_dir``: the
+file column (``files``; NISQA_DE also ``references``), the head names (``heads``, the ``*_pred`` columns) and each file's
+pooled vector under every head (``pooled`` float32 [files, heads, width], :meth:`nisqa_b200.scorer.Scorer.embed`).
+Single process only.
+
 ``args['window_s']`` / ``args['window_hop_s']`` (``run_predict.py --window_s S --window_hop_s S``) score every file as a
 timeline of overlapping windows instead (:meth:`nisqa_b200.scorer.Scorer.windows`): ``predict()`` returns, and writes
 to ``output_dir/NISQA_windows.csv``, one row per window with its time span, segment count and scores.  Files longer than
@@ -51,8 +56,13 @@ class nisqaModel(object):
         if win and (args.get("window_s") is None or args.get("window_hop_s") is None):
             raise ValueError("window_s / window_hop_s: windows need both, got window_s=%r, window_hop_s=%r"
                              % (args.get("window_s"), args.get("window_hop_s")))
+        if args.get("embeddings") and nb_dist.env_world()[1] > 1:
+            raise ValueError("embeddings: NISQA_embeddings.npz is written by a single process, not under torchrun with %d "
+                             "ranks" % nb_dist.env_world()[1])
         if win and args.get("segments"):
             raise ValueError("segments: per-segment rows are not written in windows mode (window_s)")
+        if win and args.get("embeddings"):
+            raise ValueError("embeddings: pooled vectors are not written in windows mode (window_s)")
         if "mode" not in self.args:
             self.args["mode"] = "main"
         self.runinfos = {}
@@ -131,6 +141,8 @@ class nisqaModel(object):
             print(self.ds_val.df.to_string(index=False))
         if self.args.get("segments") and self.args["output_dir"]:
             self.predict_segments().to_csv(os.path.join(self.args["output_dir"], "NISQA_segments.csv"), index=False)
+        if self.args.get("embeddings") and self.args["output_dir"]:
+            np.savez(os.path.join(self.args["output_dir"], "NISQA_embeddings.npz"), **self.predict_embeddings())
         return self.ds_val.df
 
     def predict_segments(self):
@@ -138,15 +150,55 @@ class nisqaModel(object):
         ``t_start`` / ``t_end`` (seconds), each head's segment score (``*_pred``) and pooling weight (``*_weight``).
         The files are decoded by the dataset's loader and scored in batches of ``tr_bs_val`` clips of one sample rate
         through :meth:`Scorer.segments`."""
+        sc = self._scorer()
+        ds = self.ds_val
+        col = ds.filename_column
+        files = ds.df[col].tolist()
+        weight_cols = [c[:-len("_pred")] + "_weight" for c in sc.columns]
+        parts = {}
+        for batch, call in self._file_batches():
+            res = call(sc.segments)
+            s, w = res.seg_scores.cpu().numpy(), res.seg_weights.cpu().numpy()
+            r0 = 0
+            for j, i in enumerate(batch):
+                n = res.counts[j]
+                part = pd.DataFrame({col: [files[i]] * n, "segment": np.arange(n),
+                                     "t_start": res.t_start[r0:r0 + n], "t_end": res.t_end[r0:r0 + n]})
+                for h, c in enumerate(sc.columns):
+                    part[c] = s[r0:r0 + n, h].astype(float)
+                for h, c in enumerate(weight_cols):
+                    part[c] = w[r0:r0 + n, h].astype(float)
+                parts[i] = part
+                r0 += n
+        return pd.concat([parts[i] for i in range(len(ds))], ignore_index=True)
+
+    def predict_embeddings(self):
+        """-> dict of the arrays of ``NISQA_embeddings.npz``: ``files`` (the file column; NISQA_DE also ``references``,
+        the reference column), ``heads`` (the ``*_pred`` names) and ``pooled`` float32 [files, heads, width], each
+        file's pooled vector under every head (:meth:`Scorer.embed`), batched and decoded as :meth:`predict_segments`."""
+        sc = self._scorer()
+        ds = self.ds_val
+        pooled = np.empty((len(ds), len(sc.columns), self.model.embedding_width()), dtype=np.float32)
+        for batch, call in self._file_batches():
+            pooled[batch] = call(sc.embed).pooled.cpu().numpy()
+        out = {"files": np.array(ds.df[ds.filename_column].tolist()), "heads": np.array(sc.columns), "pooled": pooled}
+        if ds.double_ended:
+            out["references"] = np.array(ds.df[ds.filename_column_ref].tolist())
+        return out
+
+    def _scorer(self):
+        """a Scorer over the loaded engine"""
         from .scorer import Scorer
         sc = Scorer.__new__(Scorer)
         sc._configure(self.args, self.dev)
         sc.engine = self.model
+        return sc
+
+    def _file_batches(self):
+        """The files decoded by the dataset's loader, in batches of ``tr_bs_val`` clips of one sample rate (NISQA_DE: one
+        pair of rates) -> (file indices, call), call(f) = f(wave, sr, lengths=..., reference...) on the batch"""
         ds, bs = self.ds_val, max(1, int(self.args["tr_bs_val"]))
         de = ds.double_ended
-        col = ds.filename_column
-        files = ds.df[col].tolist()
-        weight_cols = [c[:-len("_pred")] + "_weight" for c in sc.columns]
         loaded = []
         for i in range(len(ds)):
             y, sr = NL.read_wav(ds.file_path(i), ds.ms_channel)
@@ -155,7 +207,6 @@ class nisqaModel(object):
         groups = {}
         for i, (_, sr, _, sr_ref) in enumerate(loaded):
             groups.setdefault((sr, sr_ref), []).append(i)
-        parts = {}
         for (sr, sr_ref), rows in groups.items():
             for k in range(0, len(rows), bs):
                 batch = rows[k:k + bs]
@@ -164,29 +215,13 @@ class nisqaModel(object):
                 if de:
                     kw["reference"], kw["reference_lengths"] = self._batch_tensor([loaded[i][2] for i in batch])
                     kw["reference_sample_rate"] = sr_ref
-                res = sc.segments(wave, sr, lengths=lens, **kw)
-                s, w = res.seg_scores.cpu().numpy(), res.seg_weights.cpu().numpy()
-                r0 = 0
-                for j, i in enumerate(batch):
-                    n = res.counts[j]
-                    part = pd.DataFrame({col: [files[i]] * n, "segment": np.arange(n),
-                                         "t_start": res.t_start[r0:r0 + n], "t_end": res.t_end[r0:r0 + n]})
-                    for h, c in enumerate(sc.columns):
-                        part[c] = s[r0:r0 + n, h].astype(float)
-                    for h, c in enumerate(weight_cols):
-                        part[c] = w[r0:r0 + n, h].astype(float)
-                    parts[i] = part
-                    r0 += n
-        return pd.concat([parts[i] for i in range(len(ds))], ignore_index=True)
+                yield batch, lambda f, wave=wave, sr=sr, lens=lens, kw=kw: f(wave, sr, lengths=lens, **kw)
 
     def predict_windows(self):
         """-> DataFrame with one row per window of every file, in file order: the file column, ``t_start`` / ``t_end``
         (seconds), ``n_segments`` and each head's score (``*_pred``).  Each file is decoded by the dataset's loader and
         scored on its own through :meth:`Scorer.windows`."""
-        from .scorer import Scorer
-        sc = Scorer.__new__(Scorer)
-        sc._configure(self.args, self.dev)
-        sc.engine = self.model
+        sc = self._scorer()
         ds = self.ds_val
         col = ds.filename_column
         files = ds.df[col].tolist()

@@ -208,6 +208,10 @@ struct Weights {
   struct LstmStack { LstmShape s; Linear ih[4]; const float* hh[4] = {}; };
   LstmStack lstm_st[2];          // time_dependency, time_dependency_2
   Linear lstm_att;               // PoolAttFF behind an LSTM: linear1 of every head, k-major [D pad 64][n_heads 128]
+  // the rows the pooling module reads: their width, and the engine column of each reference column (td = 'skip' conv6
+  // features; empty: the reference's order)
+  int pool_width = 0;
+  std::vector<int> pool_src;
 };
 
 }  // namespace
@@ -245,6 +249,10 @@ struct nisqa_engine {
   // clip of the call (-1: none)
   const nisqa_segment_out* seg_out = nullptr;
   std::vector<long long> seg_row;
+  // nisqa_predict_device_batch_embeddings: the call's outputs (nullptr outside such a call; its rows use seg_row), and
+  // Weights.pool_src on the device (unset when the rows are in the reference's order)
+  const nisqa_embedding_out* emb_out = nullptr;
+  DevBuf emb_src;
   float tc_scale[8] = {1, 1, 1, 1, 1, 1, 1, 1};   // 2^(e_{i-1} - S_i): undoes the activation and weight pre-scales of conv i
   int act_exp[8] = {0, 0, 0, 0, 0, 0, 0, 0};      // e_i: conv i's activations are stored as fp16 planes of v * 2^-e_i
   float act_store(int i) const { return ldexpf(1.f, -act_exp[i]); }
@@ -313,7 +321,7 @@ struct nisqa_engine {
 
   ~nisqa_engine() {
     for (auto* f : fbs) { f->window.release(); f->band_start.release(); f->band_k0.release(); f->weights.release(); f->wtab.release(); delete f; }
-    DevBuf* all[] = {&warena, &fb_table, &tw4096, &scores, &dump, &rs_win};
+    DevBuf* all[] = {&warena, &fb_table, &tw4096, &scores, &dump, &rs_win, &emb_src};
     for (auto& r : rs) r.release();
     for (auto* b : all) b->release();
     h_scores.release();
@@ -896,6 +904,12 @@ bool pack_de_align(Packer& P, const nisqa_config& c, int W) {
 // framewise model - k-major [Dp padded to 64][head 128] for the tile GEMM (lstm_att), zero in the padding rows
 bool pack_pool_heads(Packer& P, const nisqa_config& c, InRows in, bool gemm = false) {
   const int nh = c.n_out, Dp = in.dim;
+  P.w.pool_width = Dp;
+  P.w.pool_src.clear();
+  if (in.order != IN_PLAIN) {
+    P.w.pool_src.assign(Dp, 0);
+    for (int k = 0; k < Dp; ++k) P.w.pool_src[in_col(in, k)] = k;
+  }
   auto prefix = [&](int h) { return nh == 1 ? std::string("pool.model.") : "pool_layers." + std::to_string(h) + ".model."; };
   auto put_row = [&](size_t o, const TensorView* v) {          // one [1, Dp] weight in the rows' column order
     for (int k = 0; k < Dp; ++k) P.arena[o + k] = v->d[in_col(in, k)];
@@ -955,6 +969,7 @@ bool pack_bilstm128(Packer& P, nisqa_engine* e) {
   const TensorView* fw = P.get("cnn.model.fc_out.weight", {20, 768});
   const TensorView* fb = P.get("cnn.model.fc_out.bias", {20});
   if (!fw || !fb) return false;
+  P.w.pool_width = 256;                   // (fwd || bwd)
   const size_t o = P.alloc(P.w.fc.wT, 768 * 20);
   // engine order k' = (h*2 + w)*64 + c  <->  reference view order c*12 + h*2 + w (lib:830)
   for (int hw = 0; hw < 12; ++hw)
@@ -1156,6 +1171,10 @@ int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
   CK(e->warena.reserve(P.arena.size() * 4));
   CK(cudaMemcpy(e->warena.p, P.arena.data(), P.arena.size() * 4, cudaMemcpyHostToDevice));
   for (auto& s : P.slots) *s.first = e->warena.as<float>() + s.second;
+  if (!P.w.pool_src.empty()) {
+    CK(e->emb_src.reserve(P.w.pool_src.size() * 4));
+    CK(cudaMemcpy(e->emb_src.p, P.w.pool_src.data(), P.w.pool_src.size() * 4, cudaMemcpyHostToDevice));
+  }
   e->w = P.w;
   return 0;
 }
@@ -1228,7 +1247,7 @@ struct Pass {
   int* seg_frame0 = nullptr;                  // segment table (lane, seg_table_kernel)
   float* seg_thr = nullptr;
   int* seg_clip = nullptr;
-  const long long* seg_row = nullptr;         // segments call: the clips' first output rows (staging slot)
+  const long long* seg_row = nullptr;         // segments / embeddings call: the clips' first output rows (staging slot)
   const WinSpan* spans = nullptr;             // windows call: the recording spans (staging slot)
   const FeedWin* fwins = nullptr;             // feed push: the windows' rows (staging slot)
   // the rows the pooling module read (segment_rows): D real columns at a stride of ld, the attention logits the pooling
@@ -1298,14 +1317,14 @@ int upload_inputs(Pass& p, const PassInput& in) {
   SG.lane = in.slot;
   // one pinned block: ClipDesc[n] | the prefix arrays
   const size_t tb_clips = (size_t)n * sizeof(ClipDesc), tb_pref = pre.size() * 4;
-  const size_t tb_rows_at = (tb_clips + tb_pref + 7) / 8 * 8, tb_rows = e->seg_out ? (size_t)n * 8 : 0;
+  const size_t tb_rows_at = (tb_clips + tb_pref + 7) / 8 * 8, tb_rows = e->seg_out || e->emb_out ? (size_t)n * 8 : 0;
   const size_t tb_spans_at = tb_rows_at + tb_rows, tb_spans = in.win ? in.win->spans.size() * sizeof(WinSpan) : 0;
   const size_t tb_fwins_at = (tb_spans_at + tb_spans + 15) / 16 * 16, tb_fwins = in.win ? in.win->fwins.size() * sizeof(FeedWin) : 0;
   CK(SG.h_tables.reserve(tb_fwins_at + tb_fwins));
   char* ht = SG.h_tables.as<char>();
   memcpy(ht, cl.data(), tb_clips);
   memcpy(ht + tb_clips, pre.data(), tb_pref);
-  if (tb_rows) {      // (a segments call: the rows of the pass's clips)
+  if (tb_rows) {      // (a segments or embeddings call: the rows of the pass's clips)
     memcpy(ht + tb_rows_at, e->seg_row.data() + in.first_clip, tb_rows);
     CK(SG.seg_row.reserve(tb_rows));
     CK(cudaMemcpyAsync(SG.seg_row.p, ht + tb_rows_at, tb_rows, cudaMemcpyHostToDevice, cs));
@@ -1749,8 +1768,8 @@ int lstm_head(Pass& p) {
   CK(LN.partial.reserve((size_t)p.n * 2 * 4));
   { Scope s(e, "fc_out"); launch_fc20(p.st, LN.feats.as<float>(), w.fc.wT, w.fc.b, LN.feats20.as<float>(), n_seg); }
   const bool lastbi = c.pool == NISQA_POOL_LAST_STEP_BI;
-  // the other pooling modules read every step's output, and so does a segments call
-  const bool keep = e->keep_td_out || !lastbi || e->seg_out;
+  // the other pooling modules read every step's output, and so do segments and embeddings calls
+  const bool keep = e->keep_td_out || !lastbi || e->seg_out || e->emb_out;
   { Scope s(e, "lstm", 2);
     if (e->lstm_batched)
       launch_lstm_batched(p.st, LN.feats20.as<float>(), p.clips, p.by_len, p.n, w.lstm, keep ? LN.tdout.as<float>() : nullptr,
@@ -1772,24 +1791,40 @@ int lstm_head(Pass& p) {
   return 0;
 }
 
-// A segments call: every segment's score and pooling weight under each head, from the rows the pooling module read,
-// to the call's output rows.  A clip the call counts rows for but the pass did not run (NISQA_DE: its reference is
-// too short or too long) gets NaN rows, like its score.
+// A segments call: every segment's score and pooling weight under each head; an embeddings call: each head's pooled
+// vector and optionally the segments' rows - from the rows the pooling module read, to the call's outputs.  A clip the
+// call counts rows for but the pass did not run (NISQA_DE: its reference is too short or too long) gets NaN rows, like
+// its score.
 int segment_rows(Pass& p, const PassInput& in) {
   nisqa_engine* e = p.e;
-  const int nh = p.c.n_out;
-  const nisqa_segment_out& so = *e->seg_out;
+  const int nh = p.c.n_out, W = p.w.pool_width;
+  const nisqa_segment_out* so = e->seg_out;
+  const nisqa_embedding_out* eo = e->emb_out;
   for (int i = 0; i < p.n; ++i) {
     const long long r = e->seg_row[in.first_clip + i];
     if (r < 0 || in.plan[i].run) continue;
-    const size_t off = (size_t)r * nh, bytes = (size_t)in.plan[i].n_seg * nh * 4;
-    CK(cudaMemsetAsync(so.scores + off, 0xFF, bytes, p.st));
-    CK(cudaMemsetAsync(so.weights + off, 0xFF, bytes, p.st));
+    const size_t n = in.plan[i].n_seg;
+    if (so) {
+      CK(cudaMemsetAsync(so->scores + (size_t)r * nh, 0xFF, n * nh * 4, p.st));
+      CK(cudaMemsetAsync(so->weights + (size_t)r * nh, 0xFF, n * nh * 4, p.st));
+    }
+    if (eo && eo->rows) CK(cudaMemsetAsync(eo->rows + (size_t)r * W, 0xFF, n * W * 4, p.st));
   }
-  if (p.n_seg == 0) return 0;
-  Scope s(e, "segments");
-  launch_segment_scores(p.st, p.pool_x, p.pool_D, p.pool_ld, p.pool_logits, p.pool_P, nh, p.c.pool, p.clips, p.n, p.seg_row,
-                        so.scores, so.weights);
+  float* pooled = eo ? eo->pooled + (size_t)in.first_clip * nh * W : nullptr;
+  if (p.n_seg == 0) {     // (nothing ran: NaN vectors, like the scores)
+    if (eo) CK(cudaMemsetAsync(pooled, 0xFF, (size_t)p.n * nh * W * 4, p.st));
+    return 0;
+  }
+  if (so) {
+    Scope s(e, "segments");
+    launch_segment_scores(p.st, p.pool_x, p.pool_D, p.pool_ld, p.pool_logits, p.pool_P, nh, p.c.pool, p.clips, p.n, p.seg_row,
+                          so->scores, so->weights);
+  }
+  if (eo) {
+    Scope s(e, "embed");
+    launch_pool_embed(p.st, p.pool_x, W, p.pool_ld, p.w.pool_src.empty() ? nullptr : e->emb_src.as<int>(), p.pool_logits,
+                      p.pool_P, nh, p.c.pool, p.c.double_ended, p.clips, p.n, p.seg_row, pooled, eo->rows);
+  }
   return 0;
 }
 
@@ -1806,7 +1841,7 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
     if (!rc) rc = p.w.lstm_shipped ? lstm_head(p) : td_stages(p, rows);
     if (rc) return rc;
   }
-  if (e->seg_out) {
+  if (e->seg_out || e->emb_out) {
     rc = segment_rows(p, in);
     if (rc) return rc;
   }
@@ -2355,10 +2390,11 @@ static int check_device_batch(nisqa_engine* e, const nisqa_device_batch& b, cons
   return 0;
 }
 
-// nisqa_predict_device_batch (seg == nullptr) and nisqa_predict_device_batch_segments
+// nisqa_predict_device_batch (seg == emb == nullptr), nisqa_predict_device_batch_segments and
+// nisqa_predict_device_batch_embeddings
 static int device_batch_call(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg, const nisqa_device_batch* ref,
-                             int32_t target_sr, float* scores_dev, const nisqa_segment_out* seg, int32_t* n_segments_out,
-                             int32_t* status_out) {
+                             int32_t target_sr, float* scores_dev, const nisqa_segment_out* seg,
+                             const nisqa_embedding_out* emb, int32_t* n_segments_out, int32_t* status_out) {
   if (!e) return NISQA_ERR_INVALID;
   if (!e->stream) return fail(e, NISQA_ERR_STATE, "engine was not created successfully");
   if (!deg) return fail(e, NISQA_ERR_INVALID, "deg: null argument");
@@ -2386,9 +2422,10 @@ static int device_batch_call(nisqa_engine* e, void* cuda_stream, const nisqa_dev
   std::vector<int32_t> sr(n_clips);
   for (int g = 0; g < n_clips; ++g) { ns[g] = src[g % n_src]->n_samples[g / n_src]; sr[g] = src[g % n_src]->sample_rate; }
   const int fmt = out_f32 ? NISQA_FMT_F32 : NISQA_FMT_S16;
-  if (seg) {
+  if (seg && n_clips > 0 && (!seg->scores || !seg->weights)) return fail(e, NISQA_ERR_INVALID, "seg: null scores / weights");
+  if (emb && !e->weights_loaded) return fail(e, NISQA_ERR_STATE, "nisqa_load_weights has not been called");
+  if (seg || emb) {
     // each OK clip's rows, in clip order (NISQA_DE: the degraded clips only), from the host arithmetic the passes repeat
-    if (n_clips > 0 && (!seg->scores || !seg->weights)) return fail(e, NISQA_ERR_INVALID, "seg: null scores / weights");
     e->seg_row.assign(n_clips, -1);
     long long rows = 0;
     for (int g = 0; g < n_clips; ++g) {
@@ -2399,17 +2436,22 @@ static int device_batch_call(nisqa_engine* e, void* cuda_stream, const nisqa_dev
       e->seg_row[g] = rows;
       rows += pl.n_seg;
     }
-    if (seg->n_rows < rows)
+    if (seg && seg->n_rows < rows)
       return fail(e, NISQA_ERR_INVALID, "seg->n_rows = " + std::to_string(seg->n_rows) + ": the call has " +
+                                            std::to_string(rows) + " segment rows");
+    if (emb && emb->rows && emb->n_rows < rows)
+      return fail(e, NISQA_ERR_INVALID, "emb->n_rows = " + std::to_string(emb->n_rows) + ": the call has " +
                                             std::to_string(rows) + " segment rows");
   }
   CK(cudaSetDevice(e->device));
   cudaStream_t caller = static_cast<cudaStream_t>(cuda_stream);
   RsSlot* S = nullptr;
   e->seg_out = seg;
+  e->emb_out = emb;
   const int rc = enqueue_device_batch(e, caller, n_clips, ing, ns.data(), sr.data(), fmt, target_sr, scores_dev,
                                       n_segments_out, status_out, &S);
   e->seg_out = nullptr;
+  e->emb_out = nullptr;
   if (rc) {
     // whatever was enqueued before the failure may still read the caller's input or the conversion slot: the caller's
     // stream waits for every lane, and the slot stays in use until then (best effort: the error is already reported)
@@ -2423,14 +2465,29 @@ static int device_batch_call(nisqa_engine* e, void* cuda_stream, const nisqa_dev
 int nisqa_predict_device_batch(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
                                const nisqa_device_batch* ref, int32_t target_sr, float* scores_dev,
                                int32_t* n_segments_out, int32_t* status_out) {
-  return device_batch_call(e, cuda_stream, deg, ref, target_sr, scores_dev, nullptr, n_segments_out, status_out);
+  return device_batch_call(e, cuda_stream, deg, ref, target_sr, scores_dev, nullptr, nullptr, n_segments_out, status_out);
 }
 
 int nisqa_predict_device_batch_segments(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
                                         const nisqa_device_batch* ref, int32_t target_sr, float* scores_dev,
                                         const nisqa_segment_out* seg, int32_t* n_segments_out, int32_t* status_out) {
   if (e && !seg) return fail(e, NISQA_ERR_INVALID, "seg: null argument");
-  return device_batch_call(e, cuda_stream, deg, ref, target_sr, scores_dev, seg, n_segments_out, status_out);
+  return device_batch_call(e, cuda_stream, deg, ref, target_sr, scores_dev, seg, nullptr, n_segments_out, status_out);
+}
+
+int nisqa_embedding_width(const nisqa_engine* e, int32_t* width) {
+  if (!e || !width) return NISQA_ERR_INVALID;
+  if (!e->weights_loaded) return NISQA_ERR_STATE;
+  *width = e->w.pool_width;
+  return 0;
+}
+
+int nisqa_predict_device_batch_embeddings(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                                          const nisqa_device_batch* ref, int32_t target_sr, float* scores_dev,
+                                          const nisqa_embedding_out* emb, int32_t* n_segments_out, int32_t* status_out) {
+  if (e && !emb) return fail(e, NISQA_ERR_INVALID, "emb: null argument");
+  if (e && !emb->pooled) return fail(e, NISQA_ERR_INVALID, "emb->pooled: null argument");
+  return device_batch_call(e, cuda_stream, deg, ref, target_sr, scores_dev, nullptr, emb, n_segments_out, status_out);
 }
 
 int nisqa_predict_device_windows(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* rec, int32_t target_sr,

@@ -193,6 +193,13 @@ void launch_pool_wide(cudaStream_t st, const float* x, int D, int ldx, int mode,
 void launch_segment_scores(cudaStream_t st, const float* x, int D, int ldx, const float* logits, const PoolSimpleParams& P,
                            int n_heads, int mode, const ClipDesc* clips, int n_clips, const long long* row_off,
                            float* seg_scores, float* seg_weights);
+// Each head's pooled vector [n_clips][n_heads][W] (the input of its last Linear) and, when rows != nullptr, the rows
+// themselves [.][W] at row_off (< 0: none), both in the reference's column order: reference column j is x's column
+// src_col[j] (nullptr: the same order; W <= 4096).  x, ldx, logits, P.a1 / P.a1b, mode as launch_segment_scores.  de:
+// odd clips are NISQA_DE reference clips.  Clips with n_seg == 0 and reference clips get NaN vectors.
+void launch_pool_embed(cudaStream_t st, const float* x, int W, int ldx, const int* src_col, const float* logits,
+                       const PoolSimpleParams& P, int n_heads, int mode, int de, const ClipDesc* clips, int n_clips,
+                       const long long* row_off, float* pooled, float* rows);
 
 // ---------------------------------------------------------------- td_tiled.cu (self-attention, NISQA_DE, SkipCNN / DFF)
 void launch_td_in(cudaStream_t st, int nc, const float* feats, const float* WT, int nk, const float* b, const float* g,

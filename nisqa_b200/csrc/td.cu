@@ -812,6 +812,30 @@ __global__ void pool_att_logits_kernel(const float* __restrict__ x, int D, int l
 // rows: far too little work for the tensor cores.
 constexpr int kSegWarps = 8;
 
+// The attention softmax of a clip's steps as a running max m and a sum s rescaled to it: warp g folds the logits of
+// steps g, g + kSegWarps, ... in order (softmax_fold), then softmax_merge combines the warps' (m, s) [kSegWarps][NH] in
+// warp order into the clip's max and sum.  The segments and the embeddings kernels both use this arithmetic, so they
+// agree on every weight.  softmax_fold returns the max before the fold: s was rescaled by exp(that - m).
+__device__ __forceinline__ float softmax_fold(float& m, float& s, float l) {
+  const float m0 = m, nm = fmaxf(m, l);
+  s = s * expf(m - nm) + expf(l - nm);
+  m = nm;
+  return m0;
+}
+// thread h < NH: mx[h], sum[h] from the warps' wm / ws (a warp without steps has ws == 0 and adds nothing)
+template <int NH>
+__device__ __forceinline__ void softmax_merge(const float (*wm)[NH], const float (*ws)[NH], float* mx, float* sum) {
+  if (threadIdx.x < NH) {
+    const int h = threadIdx.x;
+    float M = wm[0][h];
+    for (int w = 1; w < kSegWarps; ++w) M = fmaxf(M, wm[w][h]);
+    float tot = 0.f;
+    for (int w = 0; w < kSegWarps; ++w) tot += ws[w][h] == 0.f ? 0.f : ws[w][h] * expf(wm[w][h] - M);
+    mx[h] = M;
+    sum[h] = tot;
+  }
+}
+
 template <int NH>
 __global__ void __launch_bounds__(kSegWarps * 32)
 segment_scores_kernel(const float* __restrict__ x, int D, int ldx, const float* __restrict__ logits, PoolSimpleParams P,
@@ -852,11 +876,7 @@ segment_scores_kernel(const float* __restrict__ x, int D, int ldx, const float* 
         seg_scores[row * NH + h] = sc;
         if (att) seg_weights[row * NH + h] = l;
       }
-      if (att) {
-        const float nm = fmaxf(m[h], l);
-        s[h] = s[h] * expf(m[h] - nm) + expf(l - nm);
-        m[h] = nm;
-      }
+      if (att) softmax_fold(m[h], s[h], l);
     }
   }
   if (att) {
@@ -864,15 +884,7 @@ segment_scores_kernel(const float* __restrict__ x, int D, int ldx, const float* 
 #pragma unroll
       for (int h = 0; h < NH; ++h) { wm[g][h] = m[h]; ws[g][h] = s[h]; }
     __syncthreads();
-    if (threadIdx.x < NH) {
-      const int h = threadIdx.x;
-      float M = wm[0][h];
-      for (int w = 1; w < kSegWarps; ++w) M = fmaxf(M, wm[w][h]);
-      float tot = 0.f;
-      for (int w = 0; w < kSegWarps; ++w) tot += ws[w][h] == 0.f ? 0.f : ws[w][h] * expf(wm[w][h] - M);
-      mx[h] = M;
-      sum[h] = tot;
-    }
+    softmax_merge<NH>(wm, ws, mx, sum);
   }
   __syncthreads();                       // (also makes sweep 1's parked logits visible to the whole CTA)
   const float nan = __int_as_float(0x7fc00000);
@@ -880,6 +892,139 @@ segment_scores_kernel(const float* __restrict__ x, int D, int ldx, const float* 
     const int t = i / NH, h = i - t * NH;
     float* wp = seg_weights + (r0 + t) * NH + h;
     *wp = att ? expf(*wp - mx[h]) / sum[h] : mode == 2 ? 1.f / (float)S : mode == 4 ? (t == S - 1 ? 1.f : 0.f) : nan;
+  }
+}
+
+// ---------------------------------------------------------------------------------------
+// Quality embeddings (nisqa_predict_device_batch_embeddings): each pooling head's pooled vector - the input of its last
+// Linear - and optionally the rows the module read, both in the reference's column order (src_col[j]: the column of
+// x that holds reference column j; nullptr: the same order).  PoolAtt / PoolAttFF: sum_t a_t[h] x_t with the softmax
+// weights of segment_scores_kernel, formed on the fly: each warp folds its steps into a running max and rescaled sum
+// (softmax_fold) and rescales its accumulators with the sum, then the warps merge (softmax_merge).  The logits are the
+// ones the pooling path wrote, or a1 . x_t + a1b, formed here as the segments kernel forms them (PoolAtt over rows of
+// at most 512 columns, which one CTA row covers).  PoolAvg: (sum_t x_t) / S; PoolMax: the column-wise max; PoolLastStep:
+// x_{S-1}; PoolLastStepBi: the forward half of x_{S-1} and the backward half of x_0 (copies of the rows).  The modules
+// without parameters write the same vector for every head.  One CTA per (clip, block of kEmbCols columns), its warps
+// over the clip's steps, lanes over the columns; rows with row_off >= 0 are written as they are read.  Clips that did
+// not run and NISQA_DE's reference clips (odd clips when de) get NaN vectors.  About S n_heads W FMAs and one read of
+// the rows: memory-bound, plain fp32.
+constexpr int kEmbCols = 128;
+constexpr int kEmbPer = kEmbCols / 32;
+
+template <int NH>
+__global__ void __launch_bounds__(kSegWarps * 32)
+pool_embed_kernel(const float* __restrict__ x, int W, int ldx, const int* __restrict__ src_col,
+                  const float* __restrict__ logits, PoolSimpleParams P, int mode, int de, const ClipDesc* __restrict__ clips,
+                  const long long* __restrict__ row_off, float* __restrict__ pooled, float* __restrict__ rows) {
+  __shared__ float wm[kSegWarps][NH], ws[kSegWarps][NH];
+  __shared__ float mx[NH], sum[NH];
+  __shared__ float part[kSegWarps][NH][kEmbCols];
+  const int clip = blockIdx.x, j0 = blockIdx.y * kEmbCols;
+  const ClipDesc cd = clips[clip];
+  const int S = cd.n_seg;
+  const int lane = threadIdx.x & 31, g = threadIdx.x >> 5;
+  float* out = pooled + (size_t)clip * NH * W;
+  if (S <= 0 || (de && (clip & 1))) {
+    for (int i = threadIdx.x; i < NH * kEmbCols; i += kSegWarps * 32) {
+      const int h = i / kEmbCols, j = j0 + i % kEmbCols;
+      if (j < W) out[(size_t)h * W + j] = __int_as_float(0x7fc00000);
+    }
+    return;
+  }
+  const long long r0 = rows ? row_off[clip] : -1;
+  const bool att = mode == 0 || mode == 1, own_logits = mode == 1 && logits == nullptr, last = mode >= 4;
+  int col[kEmbPer];
+#pragma unroll
+  for (int i = 0; i < kEmbPer; ++i) {
+    const int j = j0 + lane + 32 * i;
+    col[i] = j >= W ? -1 : src_col ? __ldg(src_col + j) : j;
+  }
+  float m[NH], s[NH], acc[NH][kEmbPer];
+#pragma unroll
+  for (int h = 0; h < NH; ++h) {
+    m[h] = -INFINITY; s[h] = 0.f;
+#pragma unroll
+    for (int i = 0; i < kEmbPer; ++i) acc[h][i] = mode == 3 ? -INFINITY : 0.f;
+  }
+  for (int t = g; t < S; t += kSegWarps) {
+    if (last && r0 < 0 && t != S - 1 && t != 0) continue;     // (the last-step modules read one or two rows)
+    const float* xr = x + (size_t)(cd.seg_off + t) * ldx;
+    float v[kEmbPer];
+#pragma unroll
+    for (int i = 0; i < kEmbPer; ++i) v[i] = col[i] >= 0 ? __ldg(xr + col[i]) : 0.f;
+    if (r0 >= 0) {
+      float* rr = rows + (size_t)(r0 + t) * W;
+#pragma unroll
+      for (int i = 0; i < kEmbPer; ++i)
+        if (col[i] >= 0) rr[j0 + lane + 32 * i] = v[i];
+    }
+    if (att) {
+      float la[NH];
+#pragma unroll
+      for (int h = 0; h < NH; ++h) la[h] = 0.f;
+      if (own_logits)
+        for (int k = lane; k < W; k += 32) {
+          const float xv = __ldg(xr + k);
+#pragma unroll
+          for (int h = 0; h < NH; ++h) la[h] = fmaf(xv, __ldg(P.a1 + (size_t)h * W + k), la[h]);
+        }
+#pragma unroll
+      for (int h = 0; h < NH; ++h) {
+        const float l = own_logits ? warp_sum(la[h]) + __ldg(P.a1b + h) : __ldg(logits + (size_t)(cd.seg_off + t) * NH + h);
+        const float m0 = softmax_fold(m[h], s[h], l);
+        const float r = expf(m0 - m[h]), e = expf(l - m[h]);
+#pragma unroll
+        for (int i = 0; i < kEmbPer; ++i) acc[h][i] = fmaf(e, v[i], acc[h][i] * r);
+      }
+    } else if (mode == 2) {
+#pragma unroll
+      for (int i = 0; i < kEmbPer; ++i) acc[0][i] += v[i];
+    } else if (mode == 3) {
+#pragma unroll
+      for (int i = 0; i < kEmbPer; ++i) acc[0][i] = fmaxf(acc[0][i], v[i]);
+    } else {
+#pragma unroll
+      for (int i = 0; i < kEmbPer; ++i) {
+        const int j = j0 + lane + 32 * i;
+        const bool fwd = mode == 4 || j < W / 2;
+        if (col[i] >= 0 && ((fwd && t == S - 1) || (!fwd && t == 0)))
+#pragma unroll
+          for (int h = 0; h < NH; ++h) out[(size_t)h * W + j] = v[i];
+      }
+    }
+  }
+  if (last) return;
+#pragma unroll
+  for (int h = 0; h < NH; ++h)
+    if (att || h == 0)
+#pragma unroll
+      for (int i = 0; i < kEmbPer; ++i) part[g][h][lane + 32 * i] = acc[h][i];
+  if (att && lane == 0)
+#pragma unroll
+    for (int h = 0; h < NH; ++h) { wm[g][h] = m[h]; ws[g][h] = s[h]; }
+  __syncthreads();
+  if (att) {
+    softmax_merge<NH>(wm, ws, mx, sum);
+    __syncthreads();
+  }
+  for (int i = threadIdx.x; i < NH * kEmbCols; i += kSegWarps * 32) {
+    const int h = i / kEmbCols, c = i % kEmbCols, j = j0 + c;
+    if (j >= W) continue;
+    float o;
+    if (att) {
+      o = 0.f;
+      for (int w = 0; w < kSegWarps; ++w)
+        if (ws[w][h] != 0.f) o = fmaf(part[w][h][c], expf(wm[w][h] - mx[h]), o);
+      o /= sum[h];
+    } else if (mode == 2) {
+      o = 0.f;
+      for (int w = 0; w < kSegWarps; ++w) o += part[w][0][c];
+      o /= (float)S;
+    } else {
+      o = part[0][0][c];
+      for (int w = 1; w < kSegWarps; ++w) o = fmaxf(o, part[w][0][c]);
+    }
+    out[(size_t)h * W + j] = o;
   }
 }
 
@@ -1025,6 +1170,17 @@ void launch_segment_scores(cudaStream_t st, const float* x, int D, int ldx, cons
     segment_scores_kernel<5><<<n_clips, kSegWarps * 32, 0, st>>>(x, D, ldx, logits, P, mode, clips, row_off, seg_scores, seg_weights);
   else
     segment_scores_kernel<1><<<n_clips, kSegWarps * 32, 0, st>>>(x, D, ldx, logits, P, mode, clips, row_off, seg_scores, seg_weights);
+}
+
+void launch_pool_embed(cudaStream_t st, const float* x, int W, int ldx, const int* src_col, const float* logits,
+                       const PoolSimpleParams& P, int n_heads, int mode, int de, const ClipDesc* clips, int n_clips,
+                       const long long* row_off, float* pooled, float* rows) {
+  if (n_clips <= 0) return;
+  const dim3 grid(n_clips, (W + kEmbCols - 1) / kEmbCols);
+  if (n_heads == 5)
+    pool_embed_kernel<5><<<grid, kSegWarps * 32, 0, st>>>(x, W, ldx, src_col, logits, P, mode, de, clips, row_off, pooled, rows);
+  else
+    pool_embed_kernel<1><<<grid, kSegWarps * 32, 0, st>>>(x, W, ldx, src_col, logits, P, mode, de, clips, row_off, pooled, rows);
 }
 
 }  // namespace nisqa

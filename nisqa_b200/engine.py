@@ -41,6 +41,7 @@ EXPORTS = [
     "nisqa_resample_device", "nisqa_predict_pcm_resampled", "nisqa_set_cnn_pools", "nisqa_predict_device_batch",
     "nisqa_predict_device_batch_segments", "nisqa_window_counts", "nisqa_predict_device_windows",
     "nisqa_feed_create", "nisqa_feed_rows", "nisqa_feed_push", "nisqa_feed_device_bytes", "nisqa_feed_destroy",
+    "nisqa_embedding_width", "nisqa_predict_device_batch_embeddings",
 ]
 
 
@@ -169,6 +170,11 @@ class NisqaDeviceBatch(C.Structure):
                 ("n_samples", C.POINTER(C.c_int64)), ("sample_rate", C.c_int32)]
 
 
+class NisqaEmbeddingOut(C.Structure):
+    """nisqa_embedding_out: device [rows][n_out][width] pooled vectors and optional [n_rows][width] segment rows"""
+    _fields_ = [("pooled", C.c_void_p), ("rows", C.c_void_p), ("n_rows", C.c_int64)]
+
+
 class NisqaSegmentOut(C.Structure):
     """nisqa_segment_out: device [n_rows][n_out] per-segment scores and pooling weights"""
     _fields_ = [("scores", C.c_void_p), ("weights", C.c_void_p), ("n_rows", C.c_int64)]
@@ -244,6 +250,11 @@ def load_library(path=None):
     lib.nisqa_predict_device_batch.restype = C.c_int
     lib.nisqa_predict_device_batch_segments.argtypes = [vp, vp, dbp, dbp, C.c_int32, vp, C.POINTER(NisqaSegmentOut), i32p, i32p]
     lib.nisqa_predict_device_batch_segments.restype = C.c_int
+    lib.nisqa_embedding_width.argtypes = [vp, i32p]
+    lib.nisqa_embedding_width.restype = C.c_int
+    lib.nisqa_predict_device_batch_embeddings.argtypes = [vp, vp, dbp, dbp, C.c_int32, vp, C.POINTER(NisqaEmbeddingOut),
+                                                          i32p, i32p]
+    lib.nisqa_predict_device_batch_embeddings.restype = C.c_int
     lib.nisqa_predict_device_windows.argtypes = [vp, vp, dbp, C.c_int32, C.c_int64, C.c_int32, vp, C.c_int64, i32p, i32p]
     lib.nisqa_predict_device_windows.restype = C.c_int
     lib.nisqa_window_counts.argtypes = [C.POINTER(NisqaConfig), C.c_int64, C.c_int32, C.c_int64, C.c_int32, i64p, i32p, i32p,
@@ -774,6 +785,22 @@ class Engine(object):
         seg = NisqaSegmentOut(scores=seg_scores_ptr or None, weights=seg_weights_ptr or None, n_rows=int(n_rows))
         return self._device_batch(stream, deg, scores_dev_ptr, ref, target_sr, seg)
 
+    def embedding_width(self):
+        """The width of the embedding rows of the loaded checkpoint (nisqa_embedding_width)"""
+        w = C.c_int32()
+        self._check(self.lib.nisqa_embedding_width(self.h, C.byref(w)), "nisqa_embedding_width")
+        return int(w.value)
+
+    def predict_device_batch_embeddings(self, stream, deg, scores_dev_ptr, pooled_ptr, rows_ptr, n_rows, ref=None,
+                                        target_sr=0):
+        """:meth:`predict_device_batch` that also writes each pooling head's pooled vector to ``pooled_ptr`` ([rows,
+        n_out, width] fp32 device memory, rows as the scores) and, unless ``rows_ptr`` is 0, every segment's row to
+        ``rows_ptr`` ([n_rows, width] fp32; the row table of :meth:`predict_device_batch_segments`;
+        include/nisqa_b200.h nisqa_embedding_out).  Raises EngineError, with nothing enqueued, when ``n_rows`` is too
+        small."""
+        emb = NisqaEmbeddingOut(pooled=pooled_ptr or None, rows=rows_ptr or None, n_rows=int(n_rows))
+        return self._device_batch(stream, deg, scores_dev_ptr, ref, target_sr, emb)
+
     def predict_device_windows(self, stream, rec, scores_dev_ptr, n_rows, window, hop_frames, target_sr=0):
         """Windows of the recordings ``rec`` (a :func:`device_batch` tuple) ordered on ``stream``: ``window`` samples and a
         hop of ``hop_frames`` mel frames at the model rate (``target_sr``, else the batch's rate), the scores of every
@@ -826,7 +853,7 @@ class Engine(object):
             self._feeds.discard(feed)
             self.lib.nisqa_feed_destroy(C.c_void_p(feed))
 
-    def _device_batch(self, stream, deg, scores_dev_ptr, ref, target_sr, seg):
+    def _device_batch(self, stream, deg, scores_dev_ptr, ref, target_sr, out):
         rows = deg[0].n_clips * (2 if ref is not None else 1)
         if target_sr:
             from . import resample as _rs
@@ -836,11 +863,14 @@ class Engine(object):
         args = (self.h, C.c_void_p(stream or None), C.byref(deg[0]), C.byref(ref[0]) if ref is not None else None,
                 int(target_sr or 0), C.c_void_p(scores_dev_ptr))
         outs = (nseg.ctypes.data_as(C.POINTER(C.c_int32)), status.ctypes.data_as(C.POINTER(C.c_int32)))
-        if seg is None:
+        if out is None:
             self._check(self.lib.nisqa_predict_device_batch(*args, *outs), "nisqa_predict_device_batch")
-        else:
-            self._check(self.lib.nisqa_predict_device_batch_segments(*args, C.byref(seg), *outs),
+        elif isinstance(out, NisqaSegmentOut):
+            self._check(self.lib.nisqa_predict_device_batch_segments(*args, C.byref(out), *outs),
                         "nisqa_predict_device_batch_segments")
+        else:
+            self._check(self.lib.nisqa_predict_device_batch_embeddings(*args, C.byref(out), *outs),
+                        "nisqa_predict_device_batch_embeddings")
         return nseg, status
 
     # ------------------------------------------------------------------ introspection

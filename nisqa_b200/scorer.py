@@ -11,6 +11,9 @@ the GPU: ``wave`` may be freed or reused in stream order as soon as the call ret
 ``scorer.segments(wave, 48000)`` also returns where in each clip the quality drops: every segment's score and pooling
 weight (``nisqa_predict_device_batch_segments``) with its time span.
 
+``scorer.embed(wave, 48000)`` returns the representation behind the scores: each pooling head's pooled vector, the
+input of its last Linear, and optionally every segment's row (``nisqa_predict_device_batch_embeddings``).
+
 ``scorer.windows(wave, 48000, 10.0, 1.0)`` scores recordings of any length as a timeline: every 10 s window at a 1 s hop,
 each scored as the clip cut out of the recording would be (``nisqa_predict_device_windows``).
 
@@ -32,6 +35,9 @@ DIM_COLUMNS = ["mos_pred", "noi_pred", "dis_pred", "col_pred", "loud_pred"]     
 # Scorer.segments: scores [B, n_cols] (as Scorer.__call__), seg_scores / seg_weights [N, n_cols] CUDA tensors (the rows of
 # clip b follow those of the clips before it, counts[b] of them), t_start / t_end float64 [N] seconds
 Segments = collections.namedtuple("Segments", ["scores", "seg_scores", "seg_weights", "counts", "t_start", "t_end"])
+# Scorer.embed: scores [B, n_cols] (as Scorer.__call__), pooled [B, n_cols, width] CUDA tensor (head h's pooled vector),
+# rows [N, width] CUDA tensor or None (the rows of clip b follow those of the clips before it, counts[b] of them)
+Embeddings = collections.namedtuple("Embeddings", ["scores", "pooled", "rows", "counts"])
 # Scorer.windows: scores [N, n_cols] CUDA tensor (the windows of recording b follow those of the recordings before it,
 # counts[b] of them); t_start / t_end float64 [N] seconds, n_segments / status int32 [N] host arrays
 Windows = collections.namedtuple("Windows", ["scores", "counts", "t_start", "t_end", "n_segments", "status"])
@@ -215,7 +221,35 @@ class Scorer(object):
             raise ValueError("max_push_s: a positive number of seconds (at least one sample), not %r" % (max_push_s,))
         return Feed(self, int(n_feeds), int(sample_rate), W, hop_frames, channel, int(round(max_push_s * sample_rate)))
 
-    # ------------------------------------------------------------------ shared by __call__ and segments
+    def embed(self, wave, sample_rate, lengths=None, channel=None, reference=None, reference_lengths=None,
+              reference_sample_rate=None, rows=False):
+        """Scores of a batch and the representation behind them -> :data:`Embeddings`.  Takes the arguments of
+        ``__call__`` and checks them alike.
+
+        scores : float32 [B, len(columns)], the values ``__call__`` returns
+        pooled : float32 [B, len(columns), width] CUDA tensor: the input of each pooling head's last Linear (attention:
+                 the softmax-weighted sum of the rows; avg: their mean; max: their column-wise max; last_step: the last
+                 row; last_step_bi: the last row's forward half and the first row's backward half), so that a head's
+                 score is pooled[b, h] @ w + b of that Linear.  NaN for a clip whose score is NaN
+        rows   : float32 [N, width] CUDA tensor of every segment's row the pooling module reads, in the reference's
+                 column order (``rows=True``), else None
+        counts : host list of B ints, the segments of each clip (its rows follow those of the clips before it)
+        NISQA_DE: one pooled vector per pair, rows for the degraded clips only.
+        """
+        deg, ref, counts = self._arguments(wave, sample_rate, lengths, channel, reference, reference_lengths,
+                                           reference_sample_rate)
+        out = self._scores_buffer(deg, ref)
+        width = self.engine.embedding_width()
+        pooled = torch.empty((out.shape[0], len(self.columns), width), dtype=torch.float32, device=self.device)
+        n_rows = int(sum(counts))
+        seg_rows = torch.empty((n_rows, width), dtype=torch.float32, device=self.device) if rows else None
+        if out.shape[0]:
+            self.engine.predict_device_batch_embeddings(self._stream(), deg, out.data_ptr(), pooled.data_ptr(),
+                                                        seg_rows.data_ptr() if rows else 0, n_rows, ref=ref,
+                                                        target_sr=self.target_sr)
+        return Embeddings(self._clip_rows(out, ref), self._clip_rows(pooled, ref), seg_rows, list(counts))
+
+    # ------------------------------------------------------------------ shared by __call__, segments and embed
     def _arguments(self, wave, sample_rate, lengths, channel, reference, reference_lengths, reference_sample_rate):
         """-> (deg, ref or None, segment counts of wave's clips) after every check, before anything is enqueued"""
         if self.double_ended and reference is None:

@@ -8,6 +8,7 @@ and the same option names, so existing invocations keep working:
     python run_predict.py --mode predict_dir  --pretrained_model weights/nisqa.tar --data_dir d --bs 64
     torchrun --nproc-per-node 8 run_predict.py --mode predict_csv ...   (one rank per GPU)
     python run_predict.py --mode predict_dir ... --output_dir out --segments   (+ out/NISQA_segments.csv)
+    python run_predict.py --mode predict_dir ... --output_dir out --embeddings   (+ out/NISQA_embeddings.npz)
     python run_predict.py --mode predict_dir ... --output_dir out --window_s 10 --window_hop_s 1   (out/NISQA_windows.csv)
 """
 import argparse
@@ -45,6 +46,9 @@ def parse_args(argv=None):
     parser.add_argument("--segments", action="store_true",
                         help="also write NISQA_segments.csv into output_dir: every segment's time span, score and "
                              "pooling weight (single process only)")
+    parser.add_argument("--embeddings", action="store_true",
+                        help="also write NISQA_embeddings.npz into output_dir: each file's pooled vector under every "
+                             "pooling head, the input of its last Linear (single process only)")
     parser.add_argument("--window_s", type=float, default=None,
                         help="score every file as a timeline of windows of this many seconds (with --window_hop_s) and "
                              "write NISQA_windows.csv into output_dir; files of any length (single process only)")

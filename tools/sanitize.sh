@@ -4,7 +4,7 @@
 # short clips at 48 / 16 kHz: front-end, conv1, the five wgmma conv layers with their bulk copies /
 # mbarriers, self-attention, pooling), over a 96 kHz clip (frontend_kernel, the front end for windows over 1024
 # samples), over a short nisqa_tts.tar call (StandardCNN, BiLSTM) and over device-batch
-# calls (the ingest kernel, with and without ms_sr, one segments call, two windows calls and a live feed); racecheck over the double-ended alignment's multi-block path.
+# calls (the ingest kernel, with and without ms_sr, one segments call, one embeddings call, two windows calls and a live feed); racecheck over the double-ended alignment's multi-block path.
 #   bash tools/sanitize.sh TAG
 TAG=${1:-rXX}
 OUT=gpurun_out
@@ -65,6 +65,8 @@ s4 = Scorer(os.path.join("weights", "nisqa.tar"))
 print("ingest", s4(w, 48000, channel=1).tolist(), s4(w.float() / 32768, 48000).tolist())
 seg = s4.segments(w, 48000, channel=0)      # segment_scores_kernel (PoolAttFF logits of the last td_sa layer)
 print("segments", seg.counts, seg.seg_weights.sum(0).tolist())
+emb = s4.embed(w, 48000, channel=0, rows=True)    # pool_embed_kernel (rows in the reference's order)
+print("embeddings", emb.counts, emb.pooled.shape, emb.rows.shape)
 s4.close()
 s5 = Scorer(os.path.join("weights", "nisqa_mos_only.tar"), ms_sr=16000)
 print("ingest ms_sr", s5(w[0], 48000, lengths=[30000, w.shape[-1]]).tolist())
