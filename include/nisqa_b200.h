@@ -350,6 +350,32 @@ NISQA_API int  nisqa_predict_device_windows(nisqa_engine* e, void* cuda_stream, 
                                             int32_t target_sr, int64_t window, int32_t hop_frames, float* scores_dev,
                                             int64_t n_rows, int32_t* n_segments_out, int32_t* status_out);
 
+/* Double-ended (NISQA_DE) recordings of any length scored as a timeline of window pairs.  The degraded recording of T
+ * samples gets the windows of nisqa_window_counts; pair k's reference window, with a margin of M = margin_frames * hop
+ * samples, covers samples [max(0, k H - M), min(T_ref, k H + window + M)) of its reference recording of T_ref samples
+ * (any length; empty once k H - M >= T_ref).  Each pair scores bit for bit what nisqa_predict_device_batch gives the two
+ * cut-out clips.  A pair whose degraded window (only the last can be) or reference window is too short or empty scores
+ * NaN; both statuses are reported.  Refused (NISQA_ERR_INVALID): what nisqa_predict_device_windows refuses (single-ended
+ * instead of double-ended engines), a negative margin, a reference window of window + 2M samples with more than
+ * max_segments segments, a reference batch of another clip count, and, without target_sr, a ref.sample_rate other than
+ * deg.sample_rate (with target_sr both recordings are converted whole first).  The reference is always the mono mix.
+ * nisqa_window_pair_counts: pure host arithmetic for one pair of recordings: *n_windows = K, and the first min(K, cap)
+ * pairs' segment counts and statuses of both windows (any array may be NULL). */
+NISQA_API int  nisqa_window_pair_counts(const nisqa_config* cfg, int64_t n_samples, int64_t ref_n_samples,
+                                        int32_t sample_rate, int64_t window, int32_t hop_frames, int32_t margin_frames,
+                                        int64_t* n_windows, int32_t* n_segments, int32_t* status, int32_t* ref_n_segments,
+                                        int32_t* ref_status, int64_t cap);
+/* The stream contract of nisqa_predict_device_windows.  scores_dev: device [n_rows][n_out], compact: pair k of recording
+ * b after the pairs of the recordings before it (not the (degraded, reference) row pairs of nisqa_predict_device_batch);
+ * n_segments_out / status_out (degraded windows) and ref_n_segments_out / ref_status_out (reference windows): host
+ * [pairs] (may be NULL), valid on return.  Each recording span is packed once and each mel frame pair inside a window
+ * computed once, for the degraded and the reference recording alike. */
+NISQA_API int  nisqa_predict_device_window_pairs(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                                                 const nisqa_device_batch* ref, int32_t target_sr, int64_t window,
+                                                 int32_t hop_frames, int32_t margin_frames, float* scores_dev,
+                                                 int64_t n_rows, int32_t* n_segments_out, int32_t* status_out,
+                                                 int32_t* ref_n_segments_out, int32_t* ref_status_out);
+
 /* Live feeds: n_feeds independent recordings that arrive chunk by chunk (calls, conference bridges, broadcast and TTS
  * monitoring), scored as the windows of nisqa_predict_device_windows as soon as each window is complete.  A feed object
  * runs at one rate (the model rate: checkpoints with ms_sr take feeds at ms_sr only), with the window geometry of

@@ -22,7 +22,10 @@ Single process only.
 ``args['window_s']`` / ``args['window_hop_s']`` (``run_predict.py --window_s S --window_hop_s S``) score every file as a
 timeline of overlapping windows instead (:meth:`nisqa_b200.scorer.Scorer.windows`): ``predict()`` returns, and writes
 to ``output_dir/NISQA_windows.csv``, one row per window with its time span, segment count and scores.  Files longer than
-``ms_max_segments`` are accepted in this mode.  Single process, single-ended checkpoints only.
+``ms_max_segments`` are accepted in this mode.  Single process only.  A double-ended checkpoint (``predict_csv`` with
+``csv_ref``) scores window pairs of each file and its reference, the reference windows widened by
+``args['reference_margin_s']`` seconds on either side (default 0): each row also has the reference file and the
+reference window's time span and segment count.
 """
 import datetime
 import os
@@ -63,13 +66,15 @@ class nisqaModel(object):
             raise ValueError("segments: per-segment rows are not written in windows mode (window_s)")
         if win and args.get("embeddings"):
             raise ValueError("embeddings: pooled vectors are not written in windows mode (window_s)")
+        if args.get("reference_margin_s") is not None and not win:
+            raise ValueError("reference_margin_s: a margin of the reference windows needs windows mode (window_s)")
         if "mode" not in self.args:
             self.args["mode"] = "main"
         self.runinfos = {}
         self._getDevice()
         self._loadModel()
-        if win and self.args["double_ended"]:
-            raise ValueError("window_s: a double-ended (NISQA_DE) checkpoint scores (degraded, reference) pairs, not windows")
+        if self.args.get("reference_margin_s") is not None and not self.args["double_ended"]:
+            raise ValueError("reference_margin_s: a single-ended checkpoint reads no reference (NISQA_DE only)")
         self._loadDatasets()
         self.args["now"] = datetime.datetime.today()
 
@@ -220,19 +225,34 @@ class nisqaModel(object):
     def predict_windows(self):
         """-> DataFrame with one row per window of every file, in file order: the file column, ``t_start`` / ``t_end``
         (seconds), ``n_segments`` and each head's score (``*_pred``).  Each file is decoded by the dataset's loader and
-        scored on its own through :meth:`Scorer.windows`."""
+        scored on its own through :meth:`Scorer.windows`.  NISQA_DE: one row per window pair, with the reference column
+        after the file column and ``ref_t_start`` / ``ref_t_end`` / ``ref_n_segments`` of the reference window; the
+        reference is read as the loader's mono mix."""
         sc = self._scorer()
         ds = self.ds_val
         col = ds.filename_column
         files = ds.df[col].tolist()
+        de = ds.double_ended
         parts = []
         for i in range(len(ds)):
             y, sr = NL.read_wav(ds.file_path(i), ds.ms_channel)
             wave, _ = self._batch_tensor([y])
-            res = sc.windows(wave, sr, self.args["window_s"], self.args["window_hop_s"])
+            kw = {}
+            if de:
+                y_ref, sr_ref = NL.read_wav(ds.file_path_ref(i), None)
+                kw = {"reference": self._batch_tensor([y_ref])[0], "reference_sample_rate": sr_ref,
+                      "reference_margin_s": self.args.get("reference_margin_s") or 0.0}
+            res = sc.windows(wave, sr, self.args["window_s"], self.args["window_hop_s"], **kw)
             s = res.scores.cpu().numpy()
-            part = pd.DataFrame({col: [files[i]] * res.counts[0], "t_start": res.t_start, "t_end": res.t_end,
-                                 "n_segments": res.n_segments})
+            part = pd.DataFrame({col: [files[i]] * res.counts[0]})
+            if de:
+                part[ds.filename_column_ref] = ds.df[ds.filename_column_ref].iloc[i]
+            part["t_start"], part["t_end"] = res.t_start, res.t_end
+            if de:
+                part["ref_t_start"], part["ref_t_end"] = res.ref_t_start, res.ref_t_end
+            part["n_segments"] = res.n_segments
+            if de:
+                part["ref_n_segments"] = res.ref_n_segments
             for h, c in enumerate(sc.columns):
                 part[c] = s[:, h].astype(float)
             parts.append(part)

@@ -127,8 +127,9 @@ struct Stage {
   DevBuf seg_row;        // segments call: each clip's first output row (int64, < 0: none)
   DevBuf spans;          // windows call: the pass's recording spans (WinSpan)
   DevBuf fwins;          // feed push: the pass's windows (FeedWin)
+  DevBuf pair_scores;    // window-pairs call: the pass's (degraded, reference) score rows, before the compact copy
   void release() {
-    DevBuf* all[] = {&pcm, &clips, &prefixes, &clipmax, &seg_row, &spans, &fwins};
+    DevBuf* all[] = {&pcm, &clips, &prefixes, &clipmax, &seg_row, &spans, &fwins, &pair_scores};
     for (auto* b : all) b->release();
     h_tables.release();
     if (ev_copied) cudaEventDestroy(ev_copied);
@@ -452,6 +453,29 @@ bool window_geometry(const nisqa_config& c, int sr, int64_t window, int32_t hop_
   return true;
 }
 int64_t window_count(int64_t T, int64_t W, int64_t H) { return T <= W ? 1 : 1 + (T - W + H - 1) / H; }
+// Window pairs (nisqa_predict_device_window_pairs): the degraded windows of window_geometry and a reference margin of
+// margin_frames mel frames = *M samples on either side.  false (the reason in *why) for what window_geometry refuses, a
+// negative margin, or a reference window of W + 2M samples with more than max_segments segments.
+bool window_pair_geometry(const nisqa_config& c, int sr, int64_t window, int32_t hop_frames, int32_t margin_frames, int* H,
+                          int64_t* M, std::string* why) {
+  if (!window_geometry(c, sr, window, hop_frames, H, why)) return false;
+  if (margin_frames < 0) { *why = "margin_frames = " + std::to_string(margin_frames) + ": a margin cannot be negative"; return false; }
+  *M = (int64_t)margin_frames * (*H / hop_frames);
+  ClipPlan pl;
+  plan_clip(c, window + 2 * *M, sr, &pl);
+  if (window + 2 * *M > INT32_MAX || pl.status == NISQA_CLIP_TOO_LONG) {
+    *why = "margin_frames = " + std::to_string(margin_frames) + ": a reference window of " + std::to_string(window + 2 * *M) +
+           " samples has " + std::to_string(pl.n_seg) + " segments > max_segments " + std::to_string(c.max_segments);
+    return false;
+  }
+  return true;
+}
+// Pair k of a degraded recording of T samples and its reference of T_ref: the reference window [max(0, kH - M),
+// min(T_ref, kH + W + M)), empty (length 0) once kH - M >= T_ref
+void ref_window(int64_t k, int64_t T_ref, int64_t W, int64_t H, int64_t M, int64_t* start, int64_t* n) {
+  *start = std::max<int64_t>(0, k * H - M);
+  *n = std::max<int64_t>(0, std::min(T_ref, k * H + W + M) - *start);
+}
 // The windows a push of n[b] samples to feeds that held held[b] completes, as emit(feed, k, length) in feed then window
 // order: window k once the feed holds k H + W samples; with end[b], every remaining window of the final length T
 // (window_count: the last may be short; a feed that ended with no sample has none).
@@ -1186,18 +1210,23 @@ struct FeedRings {
   const float* frames;         // frame-pair rings
   FeedGeom g;
 };
-// A windows call (nisqa_predict_device_windows): its windows are the clips of predict_common, in recording order
+// A windows call (nisqa_predict_device_windows): its windows are the clips of predict_common, in recording order.  A
+// window-pairs call (nisqa_predict_device_window_pairs, n_src 2): clip 2p is pair p's degraded window, clip 2p + 1 its
+// reference window, and the scores are compact, one row per pair.
 struct WinLayout {
-  const int* rec;              // [windows] recording of each window
-  const int64_t* start;        // [windows] first sample of each window in its recording (model rate)
-  const int64_t* rec_off;      // [recordings] element offset of each converted recording in dev_pcm (ms_sr), or nullptr:
-                               // the ingest packs each pass's spans from the caller's batch
+  const int* rec;              // [clips] recording of each window
+  const int64_t* start;        // [clips] first sample of each window in its recording (model rate)
+  const int64_t* rec_off;      // [recordings * n_src] element offset of each converted recording (clip order: recording
+                               // b's source s at b * n_src + s) in dev_pcm (ms_sr), or nullptr: the ingest packs each
+                               // pass's spans from the caller's batch
   int H, hf, W;                // window hop (samples, mel frames) and length
   const FeedRings* feed = nullptr;    // a feed push: the windows read the feeds' rings (rec: the feed)
+  int n_src = 1;               // clips alternate over n_src sources (IngestSources order)
 };
 // The recording spans of one pass of a windows call and the launch shape of its front end
 struct WinPass {
-  std::vector<WinSpan> spans;
+  std::vector<WinSpan> spans;      // source 0's spans, then source 1's
+  int n_spans[2] = {0, 0};         // spans per source
   std::vector<int64_t> pcm_off;    // each window's first sample in the pass's PCM (ClipDesc.pcm_off)
   long long pcm_elems = 0;         // ingest: the packed spans
   long long max_span = 0;          // the longest span
@@ -1221,6 +1250,7 @@ struct PassInput {
   int slot;                           // compute lane
   int stage;                          // staging slot
   const WinPass* win;                 // windows call: the pass's spans (else nullptr)
+  bool pair_rows = false;             // window-pairs call: scores_dev_out is compact, [n_clips / 2][n_out]
 };
 
 int lane_allgather(nisqa_engine* e, const float* src, float* dst, size_t count, cudaStream_t st);
@@ -1385,10 +1415,11 @@ int upload_inputs(Pass& p, const PassInput& in) {
     // the caller's batch -> packed mono PCM in the staging slot, on the lane (behind `ready`: the caller's stream order)
     CK(SG.pcm.reserve((size_t)pcm_elems * (in.fmt == NISQA_FMT_F32 ? 4 : 2)));
     Scope sc(e, "ingest");
-    if (in.win)         // each recording span once, however many windows read it
-      launch_ingest_spans(p.st, in.ingest->s[0], p.spans, (int)in.win->spans.size(), max_run_samples,
-                          in.fmt == NISQA_FMT_F32, SG.pcm.p);
-    else
+    if (in.win) {       // each recording span once, however many windows read it (window pairs: the reference mixed)
+      for (int k = 0, s0 = 0; k < in.ingest->n_src; s0 += in.win->n_spans[k++])
+        launch_ingest_spans(p.st, in.ingest->s[k], p.spans + s0, in.win->n_spans[k], max_run_samples,
+                            in.fmt == NISQA_FMT_F32, SG.pcm.p);
+    } else
       launch_ingest(p.st, *in.ingest, in.first_clip, p.clips, n, max_run_samples, in.fmt == NISQA_FMT_F32, SG.pcm.p);
     p.pcm = SG.pcm.p;
   }
@@ -1833,6 +1864,10 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
   e->cur_stream = p.st;
   int rc = upload_inputs(p, in);
   if (rc) return rc;
+  if (in.pair_rows) {   // the pass's interleaved pair rows in its staging slot (free once upload_inputs returns)
+    CK(p.SG.pair_scores.reserve((size_t)p.n * p.c.n_out * 4));
+    p.scores = p.SG.pair_scores.as<float>();
+  }
   if (p.n_seg == 0) {   // nothing valid in this pass: NaN scores
     CK(cudaMemsetAsync(p.scores, 0xFF, (size_t)p.n * p.c.n_out * 4, p.st));
   } else {
@@ -1845,46 +1880,60 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
     rc = segment_rows(p, in);
     if (rc) return rc;
   }
+  if (in.pair_rows) {   // row 2p (pair p's score) of each pair to row p of the caller's compact output
+    const size_t row = (size_t)p.c.n_out * 4;
+    CK(cudaMemcpy2DAsync(in.scores_dev_out, row, p.scores, 2 * row, row, p.n / 2, cudaMemcpyDeviceToDevice, p.st));
+  }
   CK(cudaGetLastError());
   CK(cudaEventRecord(p.SG.ev_done, p.st));
   p.SG.busy = true;
   return 0;
 }
 
-// The spans of windows i0 .. i1 - 1 of a windows call (one per run of windows of one recording), each window's offset in
-// the pass's PCM and the launch shape of the windows front end (launch_frontend_windows)
+// The spans of windows i0 .. i1 - 1 of a windows call, each window's offset in the pass's PCM and the launch shape of the
+// windows front end (launch_frontend_windows).  A span is a run of windows of one source and recording, every L.n_src-th
+// clip, that all run and share one geometry: window m starts m H after the first and covers the first's length or ends
+// where the span ends (a recording's short last window; the reference windows that the end of the reference clips).  A
+// window that does not run is in no span: no sample of it is packed and no row of it computed.
 void win_pass(const nisqa_config& c, const WinLayout& L, const ClipPlan* plan, const int64_t* len, int i0, int i1,
               WinPass* w) {
   *w = WinPass();
-  w->pcm_off.resize(i1 - i0);
-  for (int i = i0; i < i1;) {
-    const int b = L.rec[i];
-    int j = i;
-    while (j < i1 && L.rec[j] == b) ++j;
-    WinSpan s = {};
-    s.src = b; s.src_off = L.start[i];
-    s.n_samples = (int)(L.start[j - 1] + len[j - 1] - L.start[i]);
-    if (L.rec_off) s.pcm_off = L.rec_off[b] + L.start[i];
-    else { s.pcm_off = w->pcm_elems; w->pcm_elems += ((long long)s.n_samples + 15) / 16 * 16; }
-    s.clip0 = i - i0;
-    while (i + s.n_win < j && plan[i + s.n_win].run) ++s.n_win;
-    s.H = L.H; s.hf = L.hf; s.W = L.W;
-    for (int k = i; k < j; ++k) w->pcm_off[k - i0] = s.pcm_off + (L.start[k] - L.start[i]);
-    if (s.n_win > 0) {
+  w->pcm_off.assign(i1 - i0, 0);
+  const int u = L.n_src;
+  for (int src = 0; src < u; ++src) {
+    for (int i = i0 + src; i < i1;) {
+      if (!plan[i].run) { i += u; continue; }
+      const int b = L.rec[i];
+      int j = i + u;
+      for (; j < i1 && L.rec[j] == b && plan[j].run; j += u) {
+        const int64_t pe = L.start[j - u] + len[j - u], e = L.start[j] + len[j];
+        const bool full = len[j - u] == len[i];
+        if (L.start[j] != L.start[j - u] + L.H || len[j] > len[i] || (full ? e < pe : e != pe)) break;
+      }
+      WinSpan s = {};
+      s.src = b; s.src_off = L.start[i];
+      s.n_samples = (int)(L.start[j - u] + len[j - u] - L.start[i]);
+      if (L.rec_off) s.pcm_off = L.rec_off[(int64_t)b * u + src] + L.start[i];
+      else { s.pcm_off = w->pcm_elems; w->pcm_elems += ((long long)s.n_samples + 15) / 16 * 16; }
+      s.clip0 = i - i0; s.cstride = u;
+      s.n_win = (j - i) / u;
+      s.H = L.H; s.hf = L.hf; s.W = (int)len[i];
       const ClipPlan& pl = plan[i];
       const int s0 = (c.n_fft - pl.win) / 2 - c.n_fft / 2;
       const long long last = ((long long)s.n_samples - pl.hop - pl.win - s0) / pl.hop;    // last first frame of a pair
       if (last >= 0) w->pairs = std::max(w->pairs, (int)(last / 2 + 1));
       if (s.n_win > 1 && (s.hf & 1)) w->ncls = 2;
-      for (int k = i; k < i + s.n_win; ++k) {
+      for (int k = i; k < j; k += u) {
+        w->pcm_off[k - i0] = s.pcm_off + (L.start[k] - L.start[i]);
         int lead, tail;
         interior_pairs(plan[k].n_frames, (int)len[k], s0, pl.hop, pl.win, &lead, &tail);
         w->edge = std::max(w->edge, lead + (plan[k].n_frames + 1) / 2 - tail);
       }
       w->max_span = std::max<long long>(w->max_span, s.n_samples);
+      w->spans.push_back(s);
+      ++w->n_spans[src];
+      i = j;
     }
-    w->spans.push_back(s);
-    i = j;
   }
 }
 
@@ -1980,7 +2029,8 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
     in.ingest = ingest; in.first_clip = i0;
     in.ready = ready;
     in.fmt = fmt;
-    in.scores_dev_out = scores_all + (size_t)i0 * e->cfg.n_out;
+    in.pair_rows = win && win->n_src == 2;
+    in.scores_dev_out = scores_all + (size_t)(in.pair_rows ? i0 / 2 : i0) * e->cfg.n_out;
     in.win = nullptr;
     if (win) {
       if (win->feed) feed_pass(*win, plan.data(), n_samples, i0, i1, &wp);
@@ -2490,6 +2540,52 @@ int nisqa_predict_device_batch_embeddings(nisqa_engine* e, void* cuda_stream, co
   return device_batch_call(e, cuda_stream, deg, ref, target_sr, scores_dev, nullptr, emb, n_segments_out, status_out);
 }
 
+// The device work of a windows or window-pairs call once its arguments are checked and its windows laid out (L: N clips
+// of lengths len at `rate`; rs_n / rs_sr: the n_rs recordings of the caller's batch in IngestSources order, which an
+// ms_sr checkpoint converts whole first, as a span converted alone differs at its edges), with the stream contract of
+// nisqa_predict_device_batch
+static int enqueue_windows(nisqa_engine* e, void* cuda_stream, const IngestSources& ing, int fmt, int32_t target_sr,
+                           int rate, int N, const int64_t* len, WinLayout* L, int n_rs, const int64_t* rs_n,
+                           const int32_t* rs_sr, float* scores_dev, int32_t* n_segments_out, int32_t* status_out) {
+  CK(cudaSetDevice(e->device));
+  cudaStream_t caller = static_cast<cudaStream_t>(cuda_stream);
+  std::vector<int32_t> srs(N, rate);
+  RsSlot* S = nullptr;
+  cudaStream_t fin = nullptr;
+  int rc = 0;
+  CK(cudaEventRecord(e->ev_in, caller));
+  if (target_sr > 0) {
+    // the whole recordings converted first; every pass waits for `ready`
+    cudaStream_t st = e->lanes[e->profiling ? 0 : (int)(e->pass_counter % kLanes)].stream;
+    CK(cudaStreamWaitEvent(st, e->ev_in, 0));
+    std::vector<int64_t> offs, n_fix;
+    rc = resample_to_device(e, st, n_rs, nullptr, &ing, rs_n, rs_sr, fmt, target_sr, &offs, &n_fix, &S);
+    if (!rc) {
+      L->rec_off = offs.data();
+      CK(cudaEventRecord(S->ready, st));
+      rc = predict_common(e, N, nullptr, S->out.p, nullptr, len, srs.data(), NISQA_FMT_F32, nullptr, scores_dev,
+                          n_segments_out, status_out, 0, nullptr, nullptr, S->ready, &fin, L);
+    }
+    if (!rc) {
+      CK(cudaEventRecord(S->done, fin));
+      S->busy = N > 0;
+    }
+  } else {
+    rc = predict_common(e, N, nullptr, nullptr, nullptr, len, srs.data(), fmt, nullptr, scores_dev, n_segments_out,
+                        status_out, 0, nullptr, &ing, e->ev_in, &fin, L);
+  }
+  if (!rc) {
+    CK(cudaEventRecord(e->ev_out, fin));
+    CK(cudaStreamWaitEvent(caller, e->ev_out, 0));
+    return 0;
+  }
+  // (as device_batch_call: whatever was enqueued may still read the input or the conversion slot)
+  for (auto& l : e->lanes)
+    if (cudaEventRecord(e->ev_out, l.stream) == cudaSuccess) cudaStreamWaitEvent(caller, e->ev_out, 0);
+  if (S && cudaEventRecord(S->done, caller) == cudaSuccess) S->busy = true;
+  return rc;
+}
+
 int nisqa_predict_device_windows(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* rec, int32_t target_sr,
                                  int64_t window, int32_t hop_frames, float* scores_dev, int64_t n_rows,
                                  int32_t* n_segments_out, int32_t* status_out) {
@@ -2531,44 +2627,85 @@ int nisqa_predict_device_windows(nisqa_engine* e, void* cuda_stream, const nisqa
   if (n_rows < N)
     return fail(e, NISQA_ERR_INVALID, "n_rows = " + std::to_string(n_rows) + ": the call has " + std::to_string(N) + " windows");
   if (N > 0 && !scores_dev) return fail(e, NISQA_ERR_INVALID, "scores_dev: null argument");
-  CK(cudaSetDevice(e->device));
-  cudaStream_t caller = static_cast<cudaStream_t>(cuda_stream);
-  std::vector<int32_t> srs(N, rate);
   const int hop = (int)((double)rate * e->cfg.hop_s);
   WinLayout L = {wrec.data(), start.data(), nullptr, H, H / hop, W};
-  RsSlot* S = nullptr;
-  cudaStream_t fin = nullptr;
-  CK(cudaEventRecord(e->ev_in, caller));
-  if (target_sr > 0) {
-    // the whole recording converted first (a span converted alone differs at its edges); every pass waits for `ready`
-    cudaStream_t st = e->lanes[e->profiling ? 0 : (int)(e->pass_counter % kLanes)].stream;
-    CK(cudaStreamWaitEvent(st, e->ev_in, 0));
-    std::vector<int32_t> rsr(n_rec, rec->sample_rate);
-    std::vector<int64_t> offs, n_fix;
-    rc = resample_to_device(e, st, n_rec, nullptr, &ing, rec->n_samples, rsr.data(), fmt, target_sr, &offs, &n_fix, &S);
-    if (!rc) {
-      L.rec_off = offs.data();
-      CK(cudaEventRecord(S->ready, st));
-      rc = predict_common(e, N, nullptr, S->out.p, nullptr, len.data(), srs.data(), NISQA_FMT_F32, nullptr, scores_dev,
-                          n_segments_out, status_out, 0, nullptr, nullptr, S->ready, &fin, &L);
+  std::vector<int32_t> rsr(n_rec, rec->sample_rate);
+  return enqueue_windows(e, cuda_stream, ing, fmt, target_sr, rate, N, len.data(), &L, n_rec, rec->n_samples, rsr.data(),
+                         scores_dev, n_segments_out, status_out);
+}
+
+int nisqa_predict_device_window_pairs(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                                      const nisqa_device_batch* ref, int32_t target_sr, int64_t window, int32_t hop_frames,
+                                      int32_t margin_frames, float* scores_dev, int64_t n_rows, int32_t* n_segments_out,
+                                      int32_t* status_out, int32_t* ref_n_segments_out, int32_t* ref_status_out) {
+  if (!e) return NISQA_ERR_INVALID;
+  if (!e->stream) return fail(e, NISQA_ERR_STATE, "engine was not created successfully");
+  if (!e->cfg.double_ended)
+    return fail(e, NISQA_ERR_INVALID, "ref: only a double-ended (NISQA_DE) engine scores window pairs");
+  if (!deg) return fail(e, NISQA_ERR_INVALID, "deg: null argument");
+  if (!ref) return fail(e, NISQA_ERR_INVALID, "ref: null argument");
+  if (target_sr < 0) return fail(e, NISQA_ERR_INVALID, "target_sr");
+  IngestSources ing = {};
+  ing.n_src = 2;
+  bool mix[2] = {false, false};
+  int rc = check_device_batch(e, *deg, "deg.", deg->channel, deg->n_clips, &ing.s[0], &mix[0]);
+  if (!rc) rc = check_device_batch(e, *ref, "ref.", -1, deg->n_clips, &ing.s[1], &mix[1]);     // always the mono mix
+  if (rc) return rc;
+  if (target_sr == 0 && ref->sample_rate != deg->sample_rate)
+    return fail(e, NISQA_ERR_INVALID, "ref.sample_rate = " + std::to_string(ref->sample_rate) + ": the windows of both recordings "
+                                      "run at one rate, deg.sample_rate = " + std::to_string(deg->sample_rate));
+  const bool f32 = deg->sample_fmt == NISQA_FMT_F32 || ref->sample_fmt == NISQA_FMT_F32 || mix[0] || mix[1];
+  const int fmt = f32 ? NISQA_FMT_F32 : NISQA_FMT_S16;
+  const int rate = target_sr > 0 ? target_sr : deg->sample_rate;
+  std::string why;
+  int H = 0;
+  int64_t M = 0;
+  if (!window_pair_geometry(e->cfg, rate, window, hop_frames, margin_frames, &H, &M, &why))
+    return fail(e, NISQA_ERR_INVALID, why);
+  const int W = (int)window;
+  // window pair k of recording b: clips 2p (degraded window) and 2p + 1 (reference window), in recording order (host
+  // arithmetic: nisqa_window_pair_counts)
+  const int n_rec = deg->n_clips;
+  std::vector<int> wrec;
+  std::vector<int64_t> start, len, rs_n(2 * (size_t)n_rec);
+  std::vector<int32_t> rs_sr(2 * (size_t)n_rec);
+  for (int b = 0; b < n_rec; ++b) {
+    int64_t T[2];
+    for (int k = 0; k < 2; ++k) {
+      const nisqa_device_batch* x = k ? ref : deg;
+      rs_n[2 * b + k] = x->n_samples[b]; rs_sr[2 * b + k] = x->sample_rate;
+      T[k] = target_sr > 0 ? nisqa_resample_out_len(x->n_samples[b], x->sample_rate, target_sr) : x->n_samples[b];
+      if (T[k] > (int64_t)INT32_MAX)
+        return fail(e, NISQA_ERR_INVALID, std::string(k ? "ref" : "deg") + ".n_samples[" + std::to_string(b) + "]: " +
+                                              std::to_string(T[k]) + " samples at the model rate, more than 2^31 - 1");
     }
-    if (!rc) {
-      CK(cudaEventRecord(S->done, fin));
-      S->busy = N > 0;
+    const int64_t K = window_count(T[0], W, H);
+    if ((int64_t)wrec.size() + 2 * K > INT32_MAX) return fail(e, NISQA_ERR_INVALID, "deg: more than 2^30 - 1 window pairs");
+    for (int64_t k = 0; k < K; ++k) {
+      int64_t r0, rn;
+      ref_window(k, T[1], W, H, M, &r0, &rn);
+      wrec.insert(wrec.end(), {b, b});
+      start.insert(start.end(), {k * H, r0});
+      len.insert(len.end(), {std::min<int64_t>(W, T[0] - k * H), rn});
     }
-  } else {
-    rc = predict_common(e, N, nullptr, nullptr, nullptr, len.data(), srs.data(), fmt, nullptr, scores_dev, n_segments_out,
-                        status_out, 0, nullptr, &ing, e->ev_in, &fin, &L);
   }
-  if (!rc) {
-    CK(cudaEventRecord(e->ev_out, fin));
-    CK(cudaStreamWaitEvent(caller, e->ev_out, 0));
-    return 0;
+  const int N = (int)wrec.size();
+  if (n_rows < N / 2)
+    return fail(e, NISQA_ERR_INVALID, "n_rows = " + std::to_string(n_rows) + ": the call has " + std::to_string(N / 2) +
+                                          " window pairs");
+  if (N > 0 && !scores_dev) return fail(e, NISQA_ERR_INVALID, "scores_dev: null argument");
+  const int hop = (int)((double)rate * e->cfg.hop_s);
+  WinLayout L = {wrec.data(), start.data(), nullptr, H, H / hop, W};
+  L.n_src = 2;
+  std::vector<int32_t> nseg(N), status(N);
+  rc = enqueue_windows(e, cuda_stream, ing, fmt, target_sr, rate, N, len.data(), &L, 2 * n_rec, rs_n.data(), rs_sr.data(),
+                       scores_dev, nseg.data(), status.data());
+  for (int p = 0; p < N / 2; ++p) {
+    if (n_segments_out) n_segments_out[p] = nseg[2 * p];
+    if (status_out) status_out[p] = status[2 * p];
+    if (ref_n_segments_out) ref_n_segments_out[p] = nseg[2 * p + 1];
+    if (ref_status_out) ref_status_out[p] = status[2 * p + 1];
   }
-  // (as device_batch_call: whatever was enqueued may still read the input or the conversion slot)
-  for (auto& l : e->lanes)
-    if (cudaEventRecord(e->ev_out, l.stream) == cudaSuccess) cudaStreamWaitEvent(caller, e->ev_out, 0);
-  if (S && cudaEventRecord(S->done, caller) == cudaSuccess) S->busy = true;
   return rc;
 }
 
@@ -2585,6 +2722,30 @@ int nisqa_window_counts(const nisqa_config* cfg, int64_t n_samples, int32_t samp
     plan_clip(*cfg, std::min<int64_t>(window, n_samples - k * H), sample_rate, &p);
     if (n_segments) n_segments[k] = p.n_seg;
     if (status) status[k] = p.status;
+  }
+  return 0;
+}
+
+int nisqa_window_pair_counts(const nisqa_config* cfg, int64_t n_samples, int64_t ref_n_samples, int32_t sample_rate,
+                             int64_t window, int32_t hop_frames, int32_t margin_frames, int64_t* n_windows,
+                             int32_t* n_segments, int32_t* status, int32_t* ref_n_segments, int32_t* ref_status, int64_t cap) {
+  if (!cfg || n_samples < 1 || ref_n_samples < 1) return NISQA_ERR_INVALID;
+  std::string why;
+  int H = 0;
+  int64_t M = 0;
+  if (!window_pair_geometry(*cfg, sample_rate, window, hop_frames, margin_frames, &H, &M, &why)) return NISQA_ERR_INVALID;
+  const int64_t K = window_count(n_samples, window, H);
+  if (n_windows) *n_windows = K;
+  for (int64_t k = 0; k < std::min(K, cap); ++k) {
+    ClipPlan p, q;
+    int64_t r0, rn;
+    ref_window(k, ref_n_samples, window, H, M, &r0, &rn);
+    plan_clip(*cfg, std::min<int64_t>(window, n_samples - k * H), sample_rate, &p);
+    plan_clip(*cfg, rn, sample_rate, &q);
+    if (n_segments) n_segments[k] = p.n_seg;
+    if (status) status[k] = p.status;
+    if (ref_n_segments) ref_n_segments[k] = q.n_seg;
+    if (ref_status) ref_status[k] = q.status;
   }
   return 0;
 }

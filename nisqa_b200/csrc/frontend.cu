@@ -639,7 +639,8 @@ frontend_windows_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ 
     }
     if (i_lo > i_hi) return;
     n_dst = (i_hi - i_lo) / cstep + 1;
-    c0 = sp.clip0 + i_lo; f0 = jA - i_lo * sp.hf; fstep = cstep * sp.hf;
+    c0 = sp.clip0 + i_lo * sp.cstride; f0 = jA - i_lo * sp.hf; fstep = cstep * sp.hf;
+    cstep *= sp.cstride;
     y = pcm + sp.pcm_off; n = sp.n_samples; a = g; validB = true;
   } else {
     c0 = blockIdx.y;

@@ -5,19 +5,20 @@
 
 namespace nisqa {
 
-// Windows of a recording (nisqa_predict_device_windows): one row per run of consecutive windows of one recording in a
-// pass.  Every window is also a ClipDesc row of the pass (its own bounds, mel rows and clip max); the span is the PCM
-// those windows read, packed once.
+// Windows of a recording (nisqa_predict_device_windows, nisqa_predict_device_window_pairs): one row per run of
+// consecutive windows of one recording in a pass that all run, window i starting at sample i * H of the span and
+// covering W samples or up to the span's end.  Every window is also a ClipDesc row of the pass (its own bounds, mel rows
+// and clip max); the span is the PCM those windows read, packed once.
 struct WinSpan {
   long long pcm_off;   // element offset of the span's first sample (its first window's start) in the pass's PCM
   long long src_off;   // first sample of the span in its recording (model rate; the ingest reads from there)
   int src;             // the recording's index in the caller's batch (ingest)
   int n_samples;       // first window's start .. last window's end
-  int clip0;           // the span's windows are ClipDesc rows clip0 .. ; window i starts at sample i * H of the span
-  int n_win;           // leading windows the pass runs (only a recording's last window can be too short)
+  int clip0;           // window i of the span is ClipDesc row clip0 + i * cstride
+  int n_win;           // windows of the span
   int H, hf;           // window hop in samples and in mel frames (H = hf * hop)
   int W;               // window length in samples
-  int pad_;
+  int cstride;         // 1; window pairs: 2 (the clips of a pass alternate degraded and reference windows)
 };
 
 // Live feeds (nisqa_feed_*): n_feeds recordings that grow push by push.  Feed b's samples live in a ring of R >= W +

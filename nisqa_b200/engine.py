@@ -41,7 +41,8 @@ EXPORTS = [
     "nisqa_resample_device", "nisqa_predict_pcm_resampled", "nisqa_set_cnn_pools", "nisqa_predict_device_batch",
     "nisqa_predict_device_batch_segments", "nisqa_window_counts", "nisqa_predict_device_windows",
     "nisqa_feed_create", "nisqa_feed_rows", "nisqa_feed_push", "nisqa_feed_device_bytes", "nisqa_feed_destroy",
-    "nisqa_embedding_width", "nisqa_predict_device_batch_embeddings",
+    "nisqa_embedding_width", "nisqa_predict_device_batch_embeddings", "nisqa_window_pair_counts",
+    "nisqa_predict_device_window_pairs",
 ]
 
 
@@ -260,6 +261,12 @@ def load_library(path=None):
     lib.nisqa_window_counts.argtypes = [C.POINTER(NisqaConfig), C.c_int64, C.c_int32, C.c_int64, C.c_int32, i64p, i32p, i32p,
                                         C.c_int64]
     lib.nisqa_window_counts.restype = C.c_int
+    lib.nisqa_predict_device_window_pairs.argtypes = [vp, vp, dbp, dbp, C.c_int32, C.c_int64, C.c_int32, C.c_int32, vp,
+                                                      C.c_int64, i32p, i32p, i32p, i32p]
+    lib.nisqa_predict_device_window_pairs.restype = C.c_int
+    lib.nisqa_window_pair_counts.argtypes = [C.POINTER(NisqaConfig), C.c_int64, C.c_int64, C.c_int32, C.c_int64, C.c_int32,
+                                             C.c_int32, i64p, i32p, i32p, i32p, i32p, C.c_int64]
+    lib.nisqa_window_pair_counts.restype = C.c_int
     u8p = C.POINTER(C.c_uint8)
     lib.nisqa_feed_create.argtypes = [vp, C.POINTER(vp), C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int64]
     lib.nisqa_feed_create.restype = C.c_int
@@ -523,6 +530,24 @@ def window_counts(cfg, n_samples, sample_rate, window, hop_frames):
     lib.nisqa_window_counts(*args, nseg.ctypes.data_as(C.POINTER(C.c_int32)), status.ctypes.data_as(C.POINTER(C.c_int32)),
                             k.value)
     return nseg, status
+
+
+def window_pair_counts(cfg, n_samples, ref_n_samples, sample_rate, window, hop_frames, margin_frames):
+    """(n_segments, status, ref_n_segments, ref_status), int32[K] each, of the K window pairs of a degraded recording of
+    ``n_samples`` samples and its reference of ``ref_n_samples`` at the model rate ``sample_rate``: the windows of
+    :func:`window_counts` and reference windows ``margin_frames`` mel frames wider on either side
+    (nisqa_window_pair_counts, host arithmetic)"""
+    lib = load_library()
+    k = C.c_int64()
+    args = (C.byref(cfg), int(n_samples), int(ref_n_samples), int(sample_rate), int(window), int(hop_frames),
+            int(margin_frames), C.byref(k))
+    rc = lib.nisqa_window_pair_counts(*args, None, None, None, None, 0)
+    if rc != 0:
+        raise EngineError("nisqa_window_pair_counts failed (%d): window %d, hop_frames %d, margin_frames %d at %d Hz"
+                          % (rc, window, hop_frames, margin_frames, sample_rate))
+    out = [np.empty(k.value, np.int32) for _ in range(4)]
+    lib.nisqa_window_pair_counts(*args, *[_ptr(a, C.c_int32) for a in out], k.value)
+    return tuple(out)
 
 
 def _ptr(a, ct):
@@ -816,6 +841,24 @@ class Engine(object):
             C.c_void_p(scores_dev_ptr), int(n_rows), nseg.ctypes.data_as(C.POINTER(C.c_int32)),
             status.ctypes.data_as(C.POINTER(C.c_int32))), "nisqa_predict_device_windows")
         return nseg, status
+
+    def predict_device_window_pairs(self, stream, deg, ref, scores_dev_ptr, n_rows, window, hop_frames, margin_frames,
+                                    target_sr=0):
+        """Window pairs of the degraded recordings ``deg`` and their references ``ref`` (:func:`device_batch` tuples)
+        ordered on ``stream``: the windows of :meth:`predict_device_windows` and reference windows ``margin_frames`` mel
+        frames wider on either side; each pair's score to ``scores_dev_ptr`` ([n_rows, n_out] fp32 device memory, one row
+        per pair, recording after recording).  Returns (n_segments, status, ref_n_segments, ref_status) int32[pairs],
+        valid on return; raises EngineError, with nothing enqueued, for a refused call."""
+        if target_sr:
+            from . import resample as _rs
+            _rs.out_len(1, 1, 1)                                      # the interpolation table is set once
+        n = max(int(n_rows), 0)
+        out = [np.empty(n, dtype=np.int32) for _ in range(4)]
+        self._check(self.lib.nisqa_predict_device_window_pairs(
+            self.h, C.c_void_p(stream or None), C.byref(deg[0]), C.byref(ref[0]), int(target_sr or 0), int(window),
+            int(hop_frames), int(margin_frames), C.c_void_p(scores_dev_ptr), int(n_rows),
+            *[_ptr(a, C.c_int32) for a in out]), "nisqa_predict_device_window_pairs")
+        return tuple(out)
 
     def feed_create(self, n_feeds, sample_rate, window, hop_frames, max_push):
         """A feed object (nisqa_feed_create) -> its handle (an int)"""

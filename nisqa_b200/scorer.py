@@ -15,7 +15,9 @@ weight (``nisqa_predict_device_batch_segments``) with its time span.
 input of its last Linear, and optionally every segment's row (``nisqa_predict_device_batch_embeddings``).
 
 ``scorer.windows(wave, 48000, 10.0, 1.0)`` scores recordings of any length as a timeline: every 10 s window at a 1 s hop,
-each scored as the clip cut out of the recording would be (``nisqa_predict_device_windows``).
+each scored as the clip cut out of the recording would be (``nisqa_predict_device_windows``).  A NISQA_DE checkpoint
+scores window pairs of a recording and its reference: ``scorer.windows(wave, 48000, 10.0, 1.0, reference=ref)``
+(``nisqa_predict_device_window_pairs``).
 
 ``scorer.feed(256, 48000, 10.0, 1.0)`` scores live sources as their audio arrives: ``feed.push(chunk)`` appends a chunk to
 every source and returns the windows it completed, with the scores ``windows`` gives on the whole recording
@@ -41,6 +43,11 @@ Embeddings = collections.namedtuple("Embeddings", ["scores", "pooled", "rows", "
 # Scorer.windows: scores [N, n_cols] CUDA tensor (the windows of recording b follow those of the recordings before it,
 # counts[b] of them); t_start / t_end float64 [N] seconds, n_segments / status int32 [N] host arrays
 Windows = collections.namedtuple("Windows", ["scores", "counts", "t_start", "t_end", "n_segments", "status"])
+# Scorer.windows with a reference (NISQA_DE): scores [N, n_cols] CUDA tensor, one row per window pair (the pairs of
+# recording b follow those of the recordings before it, counts[b] of them); the degraded windows' t_start / t_end float64
+# [N] seconds and n_segments / status int32 [N], and the same of the reference windows (ref_*), host arrays
+WindowPairs = collections.namedtuple("WindowPairs", ["scores", "counts", "t_start", "t_end", "n_segments", "status",
+                                                     "ref_t_start", "ref_t_end", "ref_n_segments", "ref_status"])
 # Feed.push: scores [N, n_cols] CUDA tensor of the windows the push completed, by feed then window index; feed int32 [N],
 # index int64 [N] (window k of the feed's current recording), t_start / t_end float64 [N] seconds, n_segments / status
 # int32 [N] host arrays
@@ -148,10 +155,11 @@ class Scorer(object):
         t_end = (t * a["ms_seg_hop_length"] + a["ms_seg_length"] - 1) * hop / rate
         return Segments(self._clip_rows(out, ref), seg_s, seg_w, list(counts), t_start, t_end)
 
-    def windows(self, wave, sample_rate, window_s, window_hop_s, lengths=None, channel=None):
-        """Every recording of a batch scored as a timeline of overlapping windows -> :data:`Windows`.  Takes the
-        arguments of ``__call__`` (single-ended checkpoints only) and checks them alike, but accepts recordings of any
-        length.
+    def windows(self, wave, sample_rate, window_s, window_hop_s, lengths=None, channel=None, reference=None,
+                reference_lengths=None, reference_sample_rate=None, reference_margin_s=0.0):
+        """Every recording of a batch scored as a timeline of overlapping windows -> :data:`Windows`, or with a
+        ``reference`` (NISQA_DE) as a timeline of window pairs -> :data:`WindowPairs`.  Takes the arguments of
+        ``__call__`` and checks them alike, but accepts recordings of any length.
 
         window_s     : window length in seconds at the model rate (``ms_sr`` when set, else ``sample_rate``):
                        W = round(window_s rate) samples; its segment count must fit ``ms_max_segments``
@@ -163,33 +171,82 @@ class Scorer(object):
         counts       : host list of B ints, windows per recording
         t_start, t_end : float64 [N] host arrays, seconds at the model rate
         n_segments, status : int32 [N] host arrays
+
+        reference          : NISQA_DE only: one reference recording per recording of ``wave``, of any length, always
+                             mixed to mono; with its own ``reference_lengths`` and ``reference_sample_rate`` (default
+                             ``sample_rate``; without ``ms_sr`` it must equal ``sample_rate``)
+        reference_margin_s : widens each reference window by M = round(reference_margin_s rate / hop) hop samples on
+                             either side (default 0), so that the alignment finds delayed content near a window's edge
+        Pair k scores exactly what ``__call__`` gives the degraded window k and the reference window [max(0, k H - M),
+        min(T_ref, k H + W + M)) cut out as clips.  A pair whose degraded or reference window is too short (or empty:
+        k H - M >= T_ref) scores NaN; ``status`` and ``ref_status`` tell which.
         """
         from . import resample as RS
-        if self.double_ended:
-            raise ValueError("windows: a double-ended (NISQA_DE) checkpoint scores (wave, reference) pairs, not windows")
+        m = reference_margin_s
+        if isinstance(m, bool) or not isinstance(m, numbers.Real) or not np.isfinite(m) or m < 0:
+            raise ValueError("reference_margin_s: a non-negative number of seconds, not %r" % (m,))
+        if reference is None:
+            if m != 0:
+                raise ValueError("reference_margin_s=%r: a margin widens reference windows; pass reference= (NISQA_DE)" % (m,))
+            if self.double_ended:
+                raise ValueError("windows: a double-ended (NISQA_DE) checkpoint scores window pairs of a recording and its "
+                                 "reference: pass reference=")
+        elif not self.double_ended:
+            raise ValueError("reference: only a double-ended (NISQA_DE) checkpoint takes reference clips")
         deg = self._batch("wave", wave, sample_rate, lengths, channel)
         sr = deg[0].sample_rate
+        ref = None
+        if reference is not None:
+            ref = self._batch("reference", reference, sample_rate if reference_sample_rate is None else reference_sample_rate,
+                              reference_lengths, None)
+            if ref[0].n_clips != deg[0].n_clips:
+                raise ValueError("reference: %d recordings for %d recordings of wave" % (ref[0].n_clips, deg[0].n_clips))
+            if not self.target_sr and ref[0].sample_rate != sr:
+                raise ValueError("reference_sample_rate: %d Hz for wave at %d Hz; without ms_sr both recordings' windows "
+                                 "run at one rate" % (ref[0].sample_rate, sr))
         rate = self.target_sr or sr
         W, hop_frames = window_geometry(self.args, rate, window_s, window_hop_s)
-        H = hop_frames * int(rate * self.args["ms_hop_length"])
+        hop = int(rate * self.args["ms_hop_length"])
+        H = hop_frames * hop
+        a = self.args
         _, n_seg, status = E.segment_counts(self.cfg, W, rate)
         if status != E.CLIP_OK:
-            a = self.args
             err = E.clip_status_error(status, "window_s=%r (%d samples at %d Hz)" % (window_s, W, rate), W, rate, n_seg,
                                       a["ms_hop_length"], a["ms_seg_length"], a["ms_max_segments"])
             raise ValueError("window_s: " + str(err))
-        counts, t0, t1, nseg, st = [], [], [], [], []
-        for n in deg[1]:
-            T = int(n) if rate == sr else RS.out_len(int(n), sr, rate)
-            s, z = E.window_counts(self.cfg, T, rate, W, hop_frames)
-            a, b = window_times(T, W, H, rate)
-            counts.append(len(s)); nseg.append(s); st.append(z); t0.append(a); t1.append(b)
+        margin_frames = int(round(m * rate / hop))
+        M = margin_frames * hop
+        if ref is not None:
+            _, n_seg, status = E.segment_counts(self.cfg, W + 2 * M, rate)
+            if status != E.CLIP_OK:
+                raise ValueError("reference_margin_s=%r: reference windows of %d samples (W + 2 x %d) have %d segments > "
+                                 "ms_max_segments %d" % (m, W + 2 * M, M, n_seg, a["ms_max_segments"]))
+        model_len = lambda n, r: int(n) if rate == r else RS.out_len(int(n), r, rate)      # noqa: E731
+        counts, parts = [], []
+        for b, n in enumerate(deg[1]):
+            T = model_len(n, sr)
+            t0, t1 = window_times(T, W, H, rate)
+            if ref is None:
+                cols = E.window_counts(self.cfg, T, rate, W, hop_frames)
+            else:
+                T_ref = model_len(ref[1][b], ref[0].sample_rate)
+                cols = E.window_pair_counts(self.cfg, T, T_ref, rate, W, hop_frames, margin_frames)
+                k = np.arange(len(t0), dtype=np.int64)
+                r0 = np.maximum(0, k * H - M)
+                r1 = np.maximum(r0, np.minimum(T_ref, k * H + W + M))
+                cols = cols[:2] + (r0 / rate, r1 / rate) + cols[2:]
+            counts.append(len(t0))
+            parts.append((t0, t1) + tuple(cols))
         N = int(sum(counts))
         out = torch.empty((N, len(self.columns)), dtype=torch.float32, device=self.device)
-        if N:
+        if N and ref is None:
             self.engine.predict_device_windows(self._stream(), deg, out.data_ptr(), N, W, hop_frames, target_sr=self.target_sr)
-        cat = lambda parts, dt: np.concatenate(parts).astype(dt) if parts else np.zeros(0, dt)      # noqa: E731
-        return Windows(out, counts, cat(t0, np.float64), cat(t1, np.float64), cat(nseg, np.int32), cat(st, np.int32))
+        elif N:
+            self.engine.predict_device_window_pairs(self._stream(), deg, ref, out.data_ptr(), N, W, hop_frames, margin_frames,
+                                                    target_sr=self.target_sr)
+        types = (np.float64, np.float64, np.int32, np.int32) * (1 if ref is None else 2)
+        cols = [np.concatenate([p[i] for p in parts]).astype(t) if parts else np.zeros(0, t) for i, t in enumerate(types)]
+        return Windows(out, counts, *cols) if ref is None else WindowPairs(out, counts, *cols)
 
     def feed(self, n_feeds, sample_rate, window_s, window_hop_s, channel=None, max_push_s=None):
         """A :class:`Feed` of ``n_feeds`` live recordings at ``sample_rate``, scored as the windows of :meth:`windows`

@@ -10,6 +10,8 @@ and the same option names, so existing invocations keep working:
     python run_predict.py --mode predict_dir ... --output_dir out --segments   (+ out/NISQA_segments.csv)
     python run_predict.py --mode predict_dir ... --output_dir out --embeddings   (+ out/NISQA_embeddings.npz)
     python run_predict.py --mode predict_dir ... --output_dir out --window_s 10 --window_hop_s 1   (out/NISQA_windows.csv)
+    python run_predict.py --mode predict_csv --pretrained_model de.tar --csv_file t.csv --csv_deg deg --csv_ref ref \
+        --output_dir out --window_s 10 --window_hop_s 1 --reference_margin_s 0.5   (NISQA_DE window pairs)
 """
 import argparse
 
@@ -24,6 +26,7 @@ _OPTIONS = {
     "output_dir": (str, None, "if given, NISQA_results.csv is written here"),
     "csv_file": (str, None, "table of files to score (predict_csv)"),
     "csv_deg": (str, None, "name of the csv column with the file paths"),
+    "csv_ref": (str, None, "NISQA_DE: name of the csv column with the reference file paths (default: the checkpoint's)"),
     "num_workers": (int, 0, "native wav-decode threads per batch"),
     "bs": (int, 1, "clips per engine call"),
     "ms_channel": (int, None, "channel to use for multi-channel files (default: mono mix)"),
@@ -53,7 +56,20 @@ def parse_args(argv=None):
                         help="score every file as a timeline of windows of this many seconds (with --window_hop_s) and "
                              "write NISQA_windows.csv into output_dir; files of any length (single process only)")
     parser.add_argument("--window_hop_s", type=float, default=None, help="hop between window starts in seconds")
+    parser.add_argument("--reference_margin_s", type=float, default=None,
+                        help="NISQA_DE windows: widen each reference window by this many seconds on either side, so "
+                             "that delayed content near a window's edge is found (default 0)")
     args = vars(parser.parse_args(argv))
+    if args["csv_ref"] is None:
+        del args["csv_ref"]                       # (the checkpoint's column stays)
+    if args["reference_margin_s"] is not None:
+        if args["window_s"] is None:
+            raise ValueError("--reference_margin_s argument needs --window_s and --window_hop_s")
+        if not args["reference_margin_s"] >= 0:
+            raise ValueError("--reference_margin_s argument must be a non-negative number of seconds, not %r"
+                             % args["reference_margin_s"])
+    else:
+        del args["reference_margin_s"]
     if (args["window_s"] is None) != (args["window_hop_s"] is None):
         missing = "window_hop_s" if args["window_hop_s"] is None else "window_s"
         raise ValueError("--%s argument needed: --window_s and --window_hop_s go together" % missing)
