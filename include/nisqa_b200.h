@@ -412,6 +412,50 @@ NISQA_API int     nisqa_feed_push(nisqa_feed* f, void* cuda_stream, const nisqa_
 NISQA_API int64_t nisqa_feed_device_bytes(const nisqa_feed* f);
 NISQA_API void    nisqa_feed_destroy(nisqa_feed* f);
 
+/* Live double-ended feeds: n_feeds (degraded, reference) recording pairs that arrive chunk by chunk (a media gateway with
+ * its ingress and egress tapped, a conference bridge, a known source played through a network), scored as the window
+ * pairs of nisqa_predict_device_window_pairs as soon as both windows of a pair are complete.  Pair k of a feed is the
+ * degraded window [k H, min(k H + window, T)) and the reference window [max(0, k H - M), min(T_ref, k H + window + M)),
+ * M = margin_frames mel hops, and scores bit for bit what nisqa_predict_device_window_pairs gives on the concatenated
+ * recordings.  nisqa_feed_device_bytes and nisqa_feed_destroy serve pair feed objects too.
+ *   nisqa_feed_pair_create : a double-ended engine only (nisqa_feed_create keeps refusing them); n_feeds, sample_rate,
+ *                            window, hop_frames and max_push as nisqa_feed_create, margin_frames as
+ *                            nisqa_predict_device_window_pairs (the same refusals).  max_skew (>= 0): the largest
+ *                            difference between a feed's degraded and reference lengths after any push (for an ending
+ *                            push, before it resets them); pairs wait for the slower side, so the rings hold the faster
+ *                            side's backlog: window + max_push + M + max_skew samples per feed for the degraded side and
+ *                            window + max_push + M + max(M, max_skew) for the reference.  Two recordings that end more
+ *                            than max_skew samples apart need a larger max_skew.
+ *   nisqa_feed_pair_rows   : pure host arithmetic.  For feeds that hold held[b] degraded and ref_held[b] reference samples,
+ *                            the pairs a push of n_samples[b] and ref_n_samples[b] samples (0 allowed on either side)
+ *                            with end[b] (NULL: none) emits, in feed then pair order: pair k of feed b once the feed holds
+ *                            k H + window degraded and k H + window + M reference samples; with end[b] (which ends both
+ *                            sides) every remaining pair of the final degraded length T (as nisqa_feed_rows; a reference
+ *                            window that is empty, k H - M >= T_ref, scores NaN with NISQA_CLIP_TOO_SHORT).  *n_rows, and
+ *                            for the first min(rows, cap) rows their feed, pair index k, and the segment count and status
+ *                            of both windows (any array may be NULL).
+ *   nisqa_feed_pair_push   : appends deg's clip b (its channel applies) and ref's clip b (always the mono mix), each 0 ..
+ *                            max_push samples of a device batch at the feed rate, to feed b and scores the pairs it
+ *                            completes into scores_dev (device [n_rows][n_out], one row per pair); the host arrays [rows]
+ *                            are valid on return (may be NULL).  Both rings hold float32 if either side is float32 or
+ *                            mixed, else int16; a push in the other format is refused while a feed holds samples on
+ *                            either side.  After end[b], feed b starts a new pair of recordings at sample 0.  The stream
+ *                            contract of nisqa_feed_push; refused with nothing enqueued: what nisqa_feed_push refuses, for
+ *                            either batch, and a push after which a feed's two lengths differ by more than max_skew.
+ * nisqa_feed_push on a pair feed object and nisqa_feed_pair_push on a single-ended one are refused. */
+NISQA_API int     nisqa_feed_pair_create(nisqa_engine* e, nisqa_feed** out, int32_t n_feeds, int32_t sample_rate,
+                                         int64_t window, int32_t hop_frames, int32_t margin_frames, int64_t max_push,
+                                         int64_t max_skew);
+NISQA_API int     nisqa_feed_pair_rows(const nisqa_config* cfg, int32_t sample_rate, int64_t window, int32_t hop_frames,
+                                       int32_t margin_frames, int32_t n_feeds, const int64_t* held, const int64_t* ref_held,
+                                       const int64_t* n_samples, const int64_t* ref_n_samples, const uint8_t* end,
+                                       int64_t* n_rows, int32_t* feed, int64_t* index, int32_t* n_segments, int32_t* status,
+                                       int32_t* ref_n_segments, int32_t* ref_status, int64_t cap);
+NISQA_API int     nisqa_feed_pair_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch* deg,
+                                       const nisqa_device_batch* ref, const uint8_t* end, float* scores_dev, int64_t n_rows,
+                                       int32_t* feed_out, int64_t* index_out, int32_t* n_segments_out, int32_t* status_out,
+                                       int32_t* ref_n_segments_out, int32_t* ref_status_out);
+
 /* Copy an intermediate of the LAST predict call to host memory (parity tests).  Only valid
  * when that call fitted in one internal pass.  Returns the number of floats written (>=0)
  * or a negative status; with out == NULL returns the required count. */

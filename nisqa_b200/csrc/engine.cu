@@ -336,20 +336,24 @@ struct nisqa_engine {
   }
 };
 
-// A feed object (nisqa_feed_create): n_feeds live recordings at one rate, their rings (windows.cuh) and the host state
-// of each feed.  Its pushes run in push order: a push's ingest waits for the last push's passes (done), so one ring
-// holds what any push reads (R = W + max_push samples; P pair slots for the frames of W + max_push samples).
+// A feed object (nisqa_feed_create, nisqa_feed_pair_create): n_feeds live recordings at one rate from n_src sources (1;
+// pair feeds: 2, degraded and reference), their rings (windows.cuh: one sample allocation and one frame allocation, each
+// source's region at ring_at[s] elements / frames_at[s] floats) and the host state of each feed and source.  Its pushes
+// run in push order: a push's ingest waits for the last push's passes (done), so one ring holds what any push reads
+// (feed_create derives the ring lengths).
 constexpr int kFeedSlots = 4;      // push tables in flight (pinned -> device)
 struct nisqa_feed {
   nisqa_engine* e = nullptr;
-  int n_feeds = 0, rate = 0;
-  int64_t max_push = 0;
-  FeedGeom g = {};
+  int n_feeds = 0, rate = 0, n_src = 1;
+  int64_t max_push = 0, max_skew = 0;
+  FeedGeom g[2] = {};                      // per source
   int fmt = -1;                            // the rings' sample format (NISQA_FMT_*) while a feed holds samples
-  std::vector<int64_t> held;               // samples of each feed's current recording
-  std::vector<int64_t> j_next;             // each feed's first frame whose pair is not computed yet
-  void* ring = nullptr;                    // [n_feeds][stride] samples (4 bytes each reserved)
-  float* frames = nullptr;                 // [n_feeds][P][2 n_mels]
+  std::vector<int64_t> held[2];            // samples of each feed's current recording, per source
+  std::vector<int64_t> j_next[2];          // each feed's first frame whose pair is not computed yet, per source
+  long long ring_at[2] = {0, 0};           // each source's first element in the sample ring
+  size_t frames_at[2] = {0, 0};            // each source's first float in the frame ring
+  void* ring = nullptr;                    // [n_src][n_feeds][stride] samples (4 bytes each reserved)
+  float* frames = nullptr;                 // [n_src][n_feeds][P][2 n_mels]
   size_t ring_bytes = 0, frame_bytes = 0;
   struct Slot { HostBuf h; DevBuf d; cudaEvent_t copied = nullptr; bool busy = false; } slots[kFeedSlots];
   int64_t n_push = 0;
@@ -476,16 +480,21 @@ void ref_window(int64_t k, int64_t T_ref, int64_t W, int64_t H, int64_t M, int64
   *start = std::max<int64_t>(0, k * H - M);
   *n = std::max<int64_t>(0, std::min(T_ref, k * H + W + M) - *start);
 }
-// The windows a push of n[b] samples to feeds that held held[b] completes, as emit(feed, k, length) in feed then window
-// order: window k once the feed holds k H + W samples; with end[b], every remaining window of the final length T
-// (window_count: the last may be short; a feed that ended with no sample has none).
+// The windows a push of n[b] samples to feeds that held held[b] completes, as emit(feed, k, T, T_ref) in feed then
+// window order (T, T_ref: the feed's lengths after the push): window k once the feed holds k H + W samples; with end[b],
+// every remaining window of the final length T (window_count: the last may be short; a feed that ended with no sample has
+// none).  Pair feeds (ref_held / ref_n not null; margin M): pair k once the feed also holds k H + W + M reference
+// samples; with end[b], every remaining pair of the final degraded length.  Both conditions are monotone in k, so a push
+// emits a contiguous range of pairs per feed, a function of the held counts alone.
 template <class Emit>
-void feed_windows(int n_feeds, int64_t W, int64_t H, const int64_t* held, const int64_t* n, const uint8_t* end, Emit emit) {
-  auto complete = [&](int64_t T) { return T >= W ? (T - W) / H + 1 : 0; };
+void feed_windows(int n_feeds, int64_t W, int64_t H, int64_t M, const int64_t* held, const int64_t* n,
+                  const int64_t* ref_held, const int64_t* ref_n, const uint8_t* end, Emit emit) {
+  auto complete = [&](int64_t T, int64_t w) { return T >= w ? (T - w) / H + 1 : 0; };
+  auto both = [&](int64_t T, int64_t T_ref) { return ref_held ? std::min(complete(T, W), complete(T_ref, W + M)) : complete(T, W); };
   for (int b = 0; b < n_feeds; ++b) {
-    const int64_t T = held[b] + n[b];
-    const int64_t k1 = end && end[b] && T > 0 ? window_count(T, W, H) : complete(T);
-    for (int64_t k = complete(held[b]); k < k1; ++k) emit(b, k, std::min(W, T - k * H));
+    const int64_t T = held[b] + n[b], T_ref = ref_held ? ref_held[b] + ref_n[b] : 0;
+    const int64_t k1 = end && end[b] && T > 0 ? window_count(T, W, H) : both(T, T_ref);
+    for (int64_t k = both(held[b], ref_held ? ref_held[b] : 0); k < k1; ++k) emit(b, k, T, T_ref);
   }
 }
 
@@ -1204,11 +1213,12 @@ int pack_weights(nisqa_engine* e, const nisqa_tensor* tensors, int n) {
 }
 
 // ---------------------------------------------------------------- one pass over a run of clips
-// The rings of a feed object (nisqa_feed_push), as its passes read them
+// The rings of a feed object (nisqa_feed_push, nisqa_feed_pair_push), as its passes read them: per source (clip i of a
+// pass reads source i % n_src) its geometry, its first element in the sample rings and its frame-pair rings
 struct FeedRings {
-  const void* ring;            // sample rings (int16 or float32, the push's format)
-  const float* frames;         // frame-pair rings
-  FeedGeom g;
+  FeedGeom g[2];
+  long long ring_at[2];
+  const float* frames[2];
 };
 // A windows call (nisqa_predict_device_windows): its windows are the clips of predict_common, in recording order.  A
 // window-pairs call (nisqa_predict_device_window_pairs, n_src 2): clip 2p is pair p's degraded window, clip 2p + 1 its
@@ -1533,9 +1543,9 @@ int framewise(Pass& p, int fmt, Rows* out, const WinPass* win) {
       launch_frontend_windows(p.st, c.n_mels, p.pcm, fmt == NISQA_FMT_F32, p.clips, p.n, win->edge, p.spans,
                               (int)win->spans.size(), win->pairs, win->ncls, e->fb_table.as<FbTables>(),
                               e->tw4096.as<float2>(), LN.mel.as<float>(), p.clipmax, p.Q, p.max_span);
-      if (win->feed)    // a feed push (no spans): the interior rows, computed as their samples arrived, from the rings
-        launch_feed_rows(p.st, c.n_mels, p.clips, p.fwins, p.n, win->interior, win->feed->g, win->feed->frames,
-                         LN.mel.as<float>(), p.clipmax);
+      if (win->feed)    // a feed push: the interior rows, computed as their samples arrived, from the rings
+        launch_feed_rows(p.st, c.n_mels, p.clips, p.fwins, p.n, win->interior, win->feed->g[0], win->feed->g[1],
+                         win->feed->frames[0], win->feed->frames[1], LN.mel.as<float>(), p.clipmax);
     } else {
       launch_frontend(p.st, c.n_mels, p.pcm, fmt == NISQA_FMT_F32, p.clips, p.n, p.max_pairs, e->fb_table.as<FbTables>(),
                       e->tw4096.as<float2>(), LN.mel.as<float>(), p.clipmax, p.Q, p.max_span, e->fe_ppc);
@@ -1938,22 +1948,35 @@ void win_pass(const nisqa_config& c, const WinLayout& L, const ClipPlan* plan, c
 }
 
 // The windows i0 .. i1 - 1 of a feed push: each window's offset in the sample rings and FeedWin row, and the launch shape
-// of its edge pairs and interior rows (nothing to ingest: the push appended its samples to the rings)
+// of its edge pairs and interior rows (nothing to ingest: the push appended its samples to the rings).  A front-clipped
+// reference window (pair k with k H < M: it starts at sample 0, off the uniform windows' frame grid) is a one-window
+// span, as in win_pass: the span launch computes its interior pairs from the ring, and feed_rows_kernel skips it.
 void feed_pass(const WinLayout& L, const ClipPlan* plan, const int64_t* len, int i0, int i1, WinPass* w) {
   *w = WinPass();
-  const FeedGeom& g = L.feed->g;
   w->feed = L.feed;
   w->pcm_off.resize(i1 - i0);
   w->fwins.resize(i1 - i0);
   for (int i = i0; i < i1; ++i) {
-    const int b = L.rec[i];
-    w->pcm_off[i - i0] = b * g.stride + L.start[i] % g.R;
-    w->fwins[i - i0] = {L.start[i] / g.hop, b, 0};
+    const int b = L.rec[i], src = i % L.n_src;
+    const FeedGeom& g = L.feed->g[src];
+    const bool clipped = src == 1 && L.start[i - 1] < g.off;      // (clip i - 1: the pair's degraded window, at k H)
+    w->pcm_off[i - i0] = L.feed->ring_at[src] + b * g.stride + L.start[i] % g.R;
+    w->fwins[i - i0] = {clipped ? -1 : (L.start[i] / g.hop), b, src};
     if (!plan[i].run) continue;
     int lead, tail;
     interior_pairs(plan[i].n_frames, (int)len[i], g.s0, g.hop, g.win, &lead, &tail);
     w->edge = std::max(w->edge, lead + (plan[i].n_frames + 1) / 2 - tail);
-    w->interior = std::max(w->interior, tail - lead);
+    if (!clipped) { w->interior = std::max(w->interior, tail - lead); continue; }
+    WinSpan s = {};
+    s.pcm_off = w->pcm_off[i - i0]; s.src = b;
+    s.n_samples = (int)len[i];
+    s.clip0 = i - i0; s.cstride = L.n_src; s.n_win = 1;
+    s.H = L.H; s.hf = L.hf; s.W = (int)len[i];
+    const long long last = ((long long)s.n_samples - g.hop - g.win - g.s0) / g.hop;    // last first frame of a pair
+    if (last >= 0) w->pairs = std::max(w->pairs, (int)(last / 2 + 1));
+    w->max_span = std::max<long long>(w->max_span, s.n_samples);
+    w->spans.push_back(s);
+    ++w->n_spans[src];
   }
 }
 
@@ -2761,10 +2784,10 @@ int nisqa_feed_rows(const nisqa_config* cfg, int32_t sample_rate, int64_t window
   for (int b = 0; b < n_feeds; ++b)
     if (held[b] < 0 || n_samples[b] < 0) return NISQA_ERR_INVALID;
   int64_t r = 0;
-  feed_windows(n_feeds, window, H, held, n_samples, end, [&](int b, int64_t k, int64_t len) {
+  feed_windows(n_feeds, window, H, 0, held, n_samples, nullptr, nullptr, end, [&](int b, int64_t k, int64_t T, int64_t) {
     if (r < cap) {
       ClipPlan p;
-      plan_clip(*cfg, len, sample_rate, &p);
+      plan_clip(*cfg, std::min(window, T - k * H), sample_rate, &p);
       if (feed) feed[r] = b;
       if (index) index[r] = k;
       if (n_segments) n_segments[r] = p.n_seg;
@@ -2776,22 +2799,80 @@ int nisqa_feed_rows(const nisqa_config* cfg, int32_t sample_rate, int64_t window
   return 0;
 }
 
-int nisqa_feed_create(nisqa_engine* e, nisqa_feed** out, int32_t n_feeds, int32_t sample_rate, int64_t window,
-                      int32_t hop_frames, int64_t max_push) {
+int nisqa_feed_pair_rows(const nisqa_config* cfg, int32_t sample_rate, int64_t window, int32_t hop_frames,
+                         int32_t margin_frames, int32_t n_feeds, const int64_t* held, const int64_t* ref_held,
+                         const int64_t* n_samples, const int64_t* ref_n_samples, const uint8_t* end, int64_t* n_rows,
+                         int32_t* feed, int64_t* index, int32_t* n_segments, int32_t* status, int32_t* ref_n_segments,
+                         int32_t* ref_status, int64_t cap) {
+  if (!cfg || n_feeds < 0 || (n_feeds > 0 && (!held || !ref_held || !n_samples || !ref_n_samples)) || !n_rows)
+    return NISQA_ERR_INVALID;
+  std::string why;
+  int H = 0;
+  int64_t M = 0;
+  if (!window_pair_geometry(*cfg, sample_rate, window, hop_frames, margin_frames, &H, &M, &why)) return NISQA_ERR_INVALID;
+  for (int b = 0; b < n_feeds; ++b)
+    if (held[b] < 0 || n_samples[b] < 0 || ref_held[b] < 0 || ref_n_samples[b] < 0) return NISQA_ERR_INVALID;
+  int64_t r = 0;
+  feed_windows(n_feeds, window, H, M, held, n_samples, ref_held, ref_n_samples, end,
+               [&](int b, int64_t k, int64_t T, int64_t T_ref) {
+    if (r < cap) {
+      ClipPlan p, q;
+      int64_t r0, rn;
+      ref_window(k, T_ref, window, H, M, &r0, &rn);
+      plan_clip(*cfg, std::min(window, T - k * H), sample_rate, &p);
+      plan_clip(*cfg, rn, sample_rate, &q);
+      if (feed) feed[r] = b;
+      if (index) index[r] = k;
+      if (n_segments) n_segments[r] = p.n_seg;
+      if (status) status[r] = p.status;
+      if (ref_n_segments) ref_n_segments[r] = q.n_seg;
+      if (ref_status) ref_status[r] = q.status;
+    }
+    ++r;
+  });
+  *n_rows = r;
+  return 0;
+}
+
+// nisqa_feed_create (n_src 1: margin_frames = max_skew = 0) and nisqa_feed_pair_create (n_src 2)
+static int feed_create(nisqa_engine* e, nisqa_feed** out, int32_t n_feeds, int32_t sample_rate, int64_t window,
+                       int32_t hop_frames, int32_t margin_frames, int64_t max_push, int64_t max_skew, int n_src) {
   if (!e) return NISQA_ERR_INVALID;
   if (!out) return fail(e, NISQA_ERR_INVALID, "out: null argument");
   *out = nullptr;
   if (!e->stream) return fail(e, NISQA_ERR_STATE, "engine was not created successfully");
-  if (e->cfg.double_ended)
-    return fail(e, NISQA_ERR_INVALID, "a double-ended (NISQA_DE) engine scores (degraded, reference) pairs, not live feeds");
+  if (n_src == 1 && e->cfg.double_ended)
+    return fail(e, NISQA_ERR_INVALID, "a double-ended (NISQA_DE) engine scores (degraded, reference) pairs, not live feeds: "
+                                      "nisqa_feed_pair_create scores live pairs");
+  if (n_src == 2 && !e->cfg.double_ended)
+    return fail(e, NISQA_ERR_INVALID, "nisqa_feed_pair_create: only a double-ended (NISQA_DE) engine scores live pairs; "
+                                      "nisqa_feed_create scores live feeds");
   if (n_feeds < 1 || n_feeds > 65535)
     return fail(e, NISQA_ERR_INVALID, "n_feeds = " + std::to_string(n_feeds) + ": not within 1 .. 65535");
   if (sample_rate <= 0) return fail(e, NISQA_ERR_INVALID, "sample_rate = " + std::to_string(sample_rate));
   std::string why;
   int H = 0;
-  if (!window_geometry(e->cfg, sample_rate, window, hop_frames, &H, &why)) return fail(e, NISQA_ERR_INVALID, why);
+  int64_t M = 0;
+  if (!window_pair_geometry(e->cfg, sample_rate, window, hop_frames, margin_frames, &H, &M, &why))
+    return fail(e, NISQA_ERR_INVALID, why);
   if (max_push < 1 || max_push > (int64_t)INT32_MAX - 2 * window)
     return fail(e, NISQA_ERR_INVALID, "max_push = " + std::to_string(max_push) + ": not within 1 .. 2^31 - 1 - 2 window samples");
+  // The ring of each source must keep every sample that a pair emitted by a push reads while that push appends its
+  // samples: no position may alias modulo R.  With E_old = min(cd(Td_old), cr(Tr_old)) the first pair a push emits
+  // (cd(T) = T >= W ? (T - W) / H + 1 : 0, cr(T) = T >= W + M ? (T - W - M) / H + 1 : 0, so cd(T) H >= T - W + 1 and
+  // cr(T) H >= T - W - M + 1), the push reads degraded samples from E_old H and reference samples from max(0, E_old H -
+  // M), and writes up to Td_old + max_push - 1 and Tr_old + max_push - 1, where |Td_old - Tr_old| <= max_skew (the bound
+  // held after the last push):
+  //   degraded:  Td_new - E_old H <= W + max_push - 1 (E_old = cd) or W + M + max_push + max_skew - 1 (E_old = cr)
+  //              -> R_d = W + max_push + M + max_skew
+  //   reference: Tr_new - E_old H + M <= W + 2M + max_push - 1 (E_old = cr) or W + M + max_push + max_skew - 1 (E_old = cd)
+  //              -> R_r = W + max_push + M + max(M, max_skew)
+  // (a single-ended feed: M = max_skew = 0, R = W + max_push).  The mirror of a source is its window length (reference:
+  // W + 2M), so that any of its windows is contiguous.  The frame-pair ring of a source covers the frames of R samples,
+  // which bound those a push writes and the pairs its emitted windows read alike.
+  if (max_skew < 0 || window + max_push + M + std::max(M, max_skew) > (int64_t)INT32_MAX)
+    return fail(e, NISQA_ERR_INVALID, "max_skew = " + std::to_string(max_skew) + ": not within 0 .. 2^31 - 1 - window - "
+                                          "max_push - margin samples (with a margin, the reference ring must fit 2^31 - 1)");
   CK(cudaSetDevice(e->device));
   ClipPlan pl;
   plan_clip(e->cfg, window, sample_rate, &pl);
@@ -2800,21 +2881,32 @@ int nisqa_feed_create(nisqa_engine* e, nisqa_feed** out, int32_t n_feeds, int32_
   if (rc) return rc;
   std::unique_ptr<nisqa_feed> f(new nisqa_feed());
   f->e = e;
-  f->n_feeds = n_feeds; f->rate = sample_rate; f->max_push = max_push;
-  FeedGeom& g = f->g;
-  g = {};
-  g.W = (int)window; g.H = H; g.hf = hop_frames;
-  g.R = (int)(window + max_push);
-  g.stride = ((long long)g.R + g.W + 15) / 16 * 16;
-  g.hop = pl.hop; g.win = pl.win; g.s0 = (e->cfg.n_fft - pl.win) / 2 - e->cfg.n_fft / 2;
-  g.ncls = (hop_frames & 1) ? 2 : 1;
-  const int frames_live = (int)((window + max_push) / pl.hop) + 2;       // frames whose pairs one push may touch
-  g.P = g.ncls == 2 ? frames_live : frames_live / 2 + 2;
-  g.fb_id = fb_id;
-  f->held.assign(n_feeds, 0);
-  f->j_next.assign(n_feeds, 0);
-  const size_t ring_bytes = (size_t)n_feeds * g.stride * 4;             // (int16 rings use half)
-  const size_t frame_bytes = (size_t)n_feeds * g.P * 2 * e->cfg.n_mels * 4;
+  f->n_feeds = n_feeds; f->rate = sample_rate; f->n_src = n_src;
+  f->max_push = max_push; f->max_skew = max_skew;
+  long long ring_elems = 0;
+  size_t frame_floats = 0;
+  for (int s = 0; s < n_src; ++s) {
+    const int64_t m = s ? M : 0;
+    FeedGeom& g = f->g[s];
+    g = {};
+    g.W = (int)(window + 2 * m); g.H = H; g.hf = hop_frames;
+    g.R = (int)(window + max_push + M + (s ? std::max(M, max_skew) : max_skew));
+    g.stride = ((long long)g.R + g.W + 15) / 16 * 16;
+    g.hop = pl.hop; g.win = pl.win; g.s0 = (e->cfg.n_fft - pl.win) / 2 - e->cfg.n_fft / 2;
+    g.ncls = (hop_frames & 1) ? 2 : 1;
+    const int frames_live = g.R / pl.hop + 2;             // frames whose pairs one push may touch
+    g.P = g.ncls == 2 ? frames_live : frames_live / 2 + 2;
+    g.fb_id = fb_id;
+    g.off = (int)m; g.par = (int)((m / pl.hop) & 1);
+    f->held[s].assign(n_feeds, 0);
+    f->j_next[s].assign(n_feeds, 0);
+    f->ring_at[s] = ring_elems;
+    ring_elems += (long long)n_feeds * g.stride;
+    f->frames_at[s] = frame_floats;
+    frame_floats += (size_t)n_feeds * g.P * 2 * e->cfg.n_mels;
+  }
+  const size_t ring_bytes = (size_t)ring_elems * 4;                     // (int16 rings use half)
+  const size_t frame_bytes = frame_floats * 4;
   CK(cudaMalloc(&f->ring, ring_bytes));
   f->ring_bytes = ring_bytes;
   CK(cudaMalloc(&f->frames, frame_bytes));
@@ -2828,6 +2920,16 @@ int nisqa_feed_create(nisqa_engine* e, nisqa_feed** out, int32_t n_feeds, int32_
   return 0;
 }
 
+int nisqa_feed_create(nisqa_engine* e, nisqa_feed** out, int32_t n_feeds, int32_t sample_rate, int64_t window,
+                      int32_t hop_frames, int64_t max_push) {
+  return feed_create(e, out, n_feeds, sample_rate, window, hop_frames, 0, max_push, 0, 1);
+}
+
+int nisqa_feed_pair_create(nisqa_engine* e, nisqa_feed** out, int32_t n_feeds, int32_t sample_rate, int64_t window,
+                           int32_t hop_frames, int32_t margin_frames, int64_t max_push, int64_t max_skew) {
+  return feed_create(e, out, n_feeds, sample_rate, window, hop_frames, margin_frames, max_push, max_skew, 2);
+}
+
 int64_t nisqa_feed_device_bytes(const nisqa_feed* f) {
   if (!f) return NISQA_ERR_INVALID;
   int64_t n = (int64_t)(f->ring_bytes + f->frame_bytes);
@@ -2835,106 +2937,155 @@ int64_t nisqa_feed_device_bytes(const nisqa_feed* f) {
   return n;
 }
 
-int nisqa_feed_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch* chunk, const uint8_t* end, float* scores_dev,
-                    int64_t n_rows, int32_t* feed_out, int64_t* index_out, int32_t* n_segments_out, int32_t* status_out) {
-  if (!f) return NISQA_ERR_INVALID;
+// nisqa_feed_push (ref == nullptr) and nisqa_feed_pair_push: the chunk of each source appended to its rings, the
+// interior pairs whose last tap it brings computed into its frame rings, then the windows (pairs) the push completes
+// scored as the clips of predict_common, reading the rings
+static int feed_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch* deg, const nisqa_device_batch* ref,
+                     const uint8_t* end, float* scores_dev, int64_t n_rows, int32_t* feed_out, int64_t* index_out,
+                     int32_t* n_segments_out, int32_t* status_out, int32_t* ref_n_segments_out, int32_t* ref_status_out) {
   nisqa_engine* e = f->e;
   if (!e->weights_loaded) return fail(e, NISQA_ERR_STATE, "nisqa_load_weights has not been called");
-  if (!chunk) return fail(e, NISQA_ERR_INVALID, "chunk: null argument");
-  if (chunk->n_clips != f->n_feeds)
-    return fail(e, NISQA_ERR_INVALID, "chunk.n_clips = " + std::to_string(chunk->n_clips) + ": the feed object has " +
-                                          std::to_string(f->n_feeds) + " feeds");
-  if (chunk->sample_rate != f->rate)
-    return fail(e, NISQA_ERR_INVALID, "chunk.sample_rate = " + std::to_string(chunk->sample_rate) + ": the feeds run at " +
-                                          std::to_string(f->rate) + " Hz");
+  const int S = f->n_src, B = f->n_feeds;
+  const nisqa_device_batch* src[2] = {deg, ref};
+  const std::string nm[2] = {S == 2 ? "deg" : "chunk", "ref"};
   IngestSources ing = {};
-  ing.n_src = 1;
-  bool mix = false;
-  int rc = check_device_batch(e, *chunk, "chunk.", chunk->channel, f->n_feeds, &ing.s[0], &mix, 0);
-  if (rc) return rc;
-  const FeedGeom& g = f->g;
-  const int B = f->n_feeds;
-  long long max_in = 0;
-  bool holds = false;
-  for (int b = 0; b < B; ++b) {
-    if (chunk->n_samples[b] > f->max_push)
-      return fail(e, NISQA_ERR_INVALID, "chunk.n_samples[" + std::to_string(b) + "] = " + std::to_string(chunk->n_samples[b]) +
-                                            ": more than max_push (" + std::to_string(f->max_push) + " samples)");
-    max_in = std::max<long long>(max_in, chunk->n_samples[b]);
-    holds = holds || f->held[b] > 0;
+  ing.n_src = S;
+  bool f32 = false;
+  for (int s = 0; s < S; ++s) {
+    const nisqa_device_batch* c = src[s];
+    if (!c) return fail(e, NISQA_ERR_INVALID, nm[s] + ": null argument");
+    if (c->n_clips != B)
+      return fail(e, NISQA_ERR_INVALID, nm[s] + ".n_clips = " + std::to_string(c->n_clips) + ": the feed object has " +
+                                            std::to_string(B) + " feeds");
+    if (c->sample_rate != f->rate)
+      return fail(e, NISQA_ERR_INVALID, nm[s] + ".sample_rate = " + std::to_string(c->sample_rate) + ": the feeds run at " +
+                                            std::to_string(f->rate) + " Hz");
+    bool mix = false;
+    const int rc = check_device_batch(e, *c, nm[s] + ".", s ? -1 : c->channel, B, &ing.s[s], &mix, 0);  // (ref: mono mix)
+    if (rc) return rc;
+    f32 = f32 || c->sample_fmt == NISQA_FMT_F32 || mix;
   }
-  const int fmt = chunk->sample_fmt == NISQA_FMT_F32 || mix ? NISQA_FMT_F32 : NISQA_FMT_S16;
-  if (max_in > 0 && holds && f->fmt != fmt)
-    return fail(e, NISQA_ERR_INVALID, std::string("chunk.sample_fmt: the feeds hold ") +
-                                          (f->fmt == NISQA_FMT_F32 ? "float32" : "int16") + " samples and this push " +
+  long long max_in[2] = {0, 0};
+  bool holds = false;
+  for (int s = 0; s < S; ++s)
+    for (int b = 0; b < B; ++b) {
+      const int64_t n = src[s]->n_samples[b];
+      if (n > f->max_push)
+        return fail(e, NISQA_ERR_INVALID, nm[s] + ".n_samples[" + std::to_string(b) + "] = " + std::to_string(n) +
+                                              ": more than max_push (" + std::to_string(f->max_push) + " samples)");
+      max_in[s] = std::max<long long>(max_in[s], n);
+      holds = holds || f->held[s][b] > 0;
+    }
+  if (S == 2)       // (the rings hold the faster side's backlog: measured before an end resets the feed)
+    for (int b = 0; b < B; ++b) {
+      const int64_t Td = f->held[0][b] + deg->n_samples[b], Tr = f->held[1][b] + ref->n_samples[b];
+      if ((Td > Tr ? Td - Tr : Tr - Td) > f->max_skew)
+        return fail(e, NISQA_ERR_INVALID, "deg.n_samples[" + std::to_string(b) + "] / ref.n_samples[" + std::to_string(b) +
+                                              "]: feed " + std::to_string(b) + " would hold " + std::to_string(Td) +
+                                              " degraded and " + std::to_string(Tr) + " reference samples, more than "
+                                              "max_skew (" + std::to_string(f->max_skew) + " samples) apart");
+    }
+  // one format for both sources (as nisqa_predict_device_window_pairs): float32 if either is float32 or mixed
+  const int fmt = f32 ? NISQA_FMT_F32 : NISQA_FMT_S16;
+  if (std::max(max_in[0], max_in[1]) > 0 && holds && f->fmt != fmt)
+    return fail(e, NISQA_ERR_INVALID, (S == 2 ? std::string("deg.sample_fmt / ref.sample_fmt") : std::string("chunk.sample_fmt")) +
+                                          ": the feeds hold " + (f->fmt == NISQA_FMT_F32 ? "float32" : "int16") +
+                                          " samples and this push " +
                                           (fmt == NISQA_FMT_F32 ? "float32 (or mixed) ones" : "mono int16 ones") +
                                           "; a format holds until every feed has ended");
-  // the windows the push completes (host arithmetic: nisqa_feed_rows)
+  // the windows (pairs: clips 2p and 2p + 1) the push completes (host arithmetic: nisqa_feed_rows, nisqa_feed_pair_rows)
+  const FeedGeom& g = f->g[0];
+  const int64_t M = S == 2 ? f->g[1].off : 0;
   std::vector<int> wfeed;
   std::vector<int64_t> wstart, wlen, widx;
-  feed_windows(B, g.W, g.H, f->held.data(), chunk->n_samples, end, [&](int b, int64_t k, int64_t len) {
-    wfeed.push_back(b); widx.push_back(k); wstart.push_back(k * g.H); wlen.push_back(len);
+  feed_windows(B, g.W, g.H, M, f->held[0].data(), deg->n_samples, S == 2 ? f->held[1].data() : nullptr,
+               S == 2 ? ref->n_samples : nullptr, end, [&](int b, int64_t k, int64_t T, int64_t T_ref) {
+    widx.push_back(k);
+    wfeed.push_back(b); wstart.push_back(k * g.H); wlen.push_back(std::min<int64_t>(g.W, T - k * g.H));
+    if (S == 2) {
+      int64_t r0, rn;
+      ref_window(k, T_ref, g.W, g.H, M, &r0, &rn);
+      wfeed.push_back(b); wstart.push_back(r0); wlen.push_back(rn);
+    }
   });
-  const int N = (int)wfeed.size();
-  if (n_rows < N)
-    return fail(e, NISQA_ERR_INVALID, "n_rows = " + std::to_string(n_rows) + ": the push completes " + std::to_string(N) + " windows");
+  const int N = (int)wfeed.size(), rows = N / S;
+  if (n_rows < rows)
+    return fail(e, NISQA_ERR_INVALID, "n_rows = " + std::to_string(n_rows) + ": the push completes " + std::to_string(rows) +
+                                          (S == 2 ? " window pairs" : " windows"));
   if (N > 0 && !scores_dev) return fail(e, NISQA_ERR_INVALID, "scores_dev: null argument");
 
-  // each feed's new samples and the interior pairs whose last tap they bring
+  // each source's new samples and the interior pairs whose last tap they bring
   CK(cudaSetDevice(e->device));
   for (auto& t : e->timers) { t.ms = 0.0; t.launches = 0; }
   cudaStream_t caller = static_cast<cudaStream_t>(cuda_stream);
   auto& sl = f->slots[f->n_push % kFeedSlots];
   if (sl.busy) { CK(cudaEventSynchronize(sl.copied)); sl.busy = false; }
-  CK(sl.h.reserve((size_t)B * sizeof(FeedPush)));
+  CK(sl.h.reserve((size_t)S * B * sizeof(FeedPush)));
   FeedPush* tab = sl.h.as<FeedPush>();
-  const int step = 3 - g.ncls, ext = g.hop + g.win;
-  const long long j_min = (-g.s0 + g.hop - 1) / g.hop;       // the first frame whose taps start at or after sample 0
-  int max_pairs = 0;
-  for (int b = 0; b < B; ++b) {
-    const long long t1 = f->held[b] + chunk->n_samples[b], num = t1 - ext - g.s0;
-    const long long j_end = num < 0 ? 0 : num / g.hop + 1;     // frames whose pair's taps have all arrived
-    long long j0 = std::max<long long>(f->j_next[b], j_min);
-    if (j0 % step) ++j0;
-    const long long np = j_end > j0 ? (j_end - j0 + step - 1) / step : 0;
-    tab[b] = {f->held[b], j0, (int)chunk->n_samples[b], (int)np};
-    max_pairs = std::max(max_pairs, (int)np);
-    f->j_next[b] = std::max<long long>(f->j_next[b], j_end);
+  int max_pairs[2] = {0, 0};
+  for (int s = 0; s < S; ++s) {
+    const FeedGeom& gs = f->g[s];
+    const int step = 3 - gs.ncls, ext = gs.hop + gs.win;
+    const long long j_min = (-gs.s0 + gs.hop - 1) / gs.hop;     // the first frame whose taps start at or after sample 0
+    for (int b = 0; b < B; ++b) {
+      const long long t1 = f->held[s][b] + src[s]->n_samples[b], num = t1 - ext - gs.s0;
+      const long long j_end = num < 0 ? 0 : num / gs.hop + 1;     // frames whose pair's taps have all arrived
+      long long j0 = std::max<long long>(f->j_next[s][b], j_min);
+      if ((j0 - gs.par) % step) ++j0;                              // (ncls 1: the windows' pairing parity)
+      const long long np = j_end > j0 ? (j_end - j0 + step - 1) / step : 0;
+      tab[s * B + b] = {f->held[s][b], j0, (int)src[s]->n_samples[b], (int)np};
+      max_pairs[s] = std::max(max_pairs[s], (int)np);
+      f->j_next[s][b] = std::max<long long>(f->j_next[s][b], j_end);
+    }
   }
   CK(cudaEventRecord(e->ev_in, caller));
   cudaStream_t st = e->lanes[e->profiling ? 0 : (int)(e->pass_counter % kLanes)].stream;
   CK(cudaStreamWaitEvent(st, e->ev_in, 0));
   if (f->pending) CK(cudaStreamWaitEvent(st, f->done, 0));  // push order: the last push's passes are done with the rings
-  if (max_in > 0) {
-    CK(sl.d.reserve((size_t)B * sizeof(FeedPush)));
-    CK(cudaMemcpyAsync(sl.d.p, tab, (size_t)B * sizeof(FeedPush), cudaMemcpyHostToDevice, st));
+  if (std::max(max_in[0], max_in[1]) > 0) {
+    CK(sl.d.reserve((size_t)S * B * sizeof(FeedPush)));
+    CK(cudaMemcpyAsync(sl.d.p, tab, (size_t)S * B * sizeof(FeedPush), cudaMemcpyHostToDevice, st));
     CK(cudaEventRecord(sl.copied, st));
     sl.busy = true;
     ++f->n_push;
     e->cur_stream = st;
-    { Scope s(e, "ingest");
-      launch_ingest_feed(st, ing.s[0], sl.d.as<FeedPush>(), B, max_in, g, fmt == NISQA_FMT_F32, f->ring); }
-    if (max_pairs > 0) {
-      Scope s(e, "frontend");
-      launch_frontend_feed_pairs(st, e->cfg.n_mels, f->ring, fmt == NISQA_FMT_F32, sl.d.as<FeedPush>(), B, max_pairs, g,
-                                 e->fb_table.as<FbTables>(), e->tw4096.as<float2>(), f->frames);
+    const size_t esz = fmt == NISQA_FMT_F32 ? 4 : 2;
+    for (int s = 0; s < S; ++s) {
+      void* ring = static_cast<char*>(f->ring) + f->ring_at[s] * esz;
+      const FeedPush* push = sl.d.as<FeedPush>() + s * B;
+      if (max_in[s] > 0) {
+        Scope sc(e, "ingest");
+        launch_ingest_feed(st, ing.s[s], push, B, max_in[s], f->g[s], fmt == NISQA_FMT_F32, ring);
+      }
+      if (max_pairs[s] > 0) {
+        Scope sc(e, "frontend");
+        launch_frontend_feed_pairs(st, e->cfg.n_mels, ring, fmt == NISQA_FMT_F32, push, B, max_pairs[s], f->g[s],
+                                   e->fb_table.as<FbTables>(), e->tw4096.as<float2>(), f->frames + f->frames_at[s]);
+      }
     }
     CK(cudaGetLastError());
     f->fmt = fmt;
   }
   for (int b = 0; b < B; ++b) {
-    f->held[b] += chunk->n_samples[b];
-    if (end && end[b]) { f->held[b] = 0; f->j_next[b] = 0; }
+    for (int s = 0; s < S; ++s) f->held[s][b] += src[s]->n_samples[b];
+    if (end && end[b])
+      for (int s = 0; s < S; ++s) { f->held[s][b] = 0; f->j_next[s][b] = 0; }
   }
   CK(cudaEventRecord(f->ready, st));
   // the completed windows, each a clip of a pass that reads the rings
   cudaStream_t fin = st;
+  std::vector<int32_t> nseg(N), status(N);
   if (N > 0) {
-    FeedRings rings = {f->ring, f->frames, g};
+    FeedRings rings = {};
+    for (int s = 0; s < 2; ++s) {
+      const int u = s < S ? s : 0;        // (single-ended: both entries are the one source)
+      rings.g[s] = f->g[u]; rings.ring_at[s] = f->ring_at[u]; rings.frames[s] = f->frames + f->frames_at[u];
+    }
     WinLayout L = {wfeed.data(), wstart.data(), nullptr, g.H, g.hf, g.W, &rings};
+    L.n_src = S;
     std::vector<int32_t> srs(N, f->rate);
-    rc = predict_common(e, N, nullptr, f->ring, nullptr, wlen.data(), srs.data(), f->fmt, nullptr, scores_dev,
-                        n_segments_out, status_out, 0, nullptr, nullptr, f->ready, &fin, &L);
+    const int rc = predict_common(e, N, nullptr, f->ring, nullptr, wlen.data(), srs.data(), f->fmt, nullptr, scores_dev,
+                                  nseg.data(), status.data(), 0, nullptr, nullptr, f->ready, &fin, &L);
     if (rc) {
       for (auto& l : e->lanes)
         if (cudaEventRecord(e->ev_out, l.stream) == cudaSuccess) cudaStreamWaitEvent(caller, e->ev_out, 0);
@@ -2945,15 +3096,41 @@ int nisqa_feed_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch* 
     CK(cudaStreamSynchronize(st));
     collect_timers(e);
   }
-  for (int r = 0; r < N; ++r) {
-    if (feed_out) feed_out[r] = wfeed[r];
+  for (int r = 0; r < rows; ++r) {
+    if (feed_out) feed_out[r] = wfeed[S * r];
     if (index_out) index_out[r] = widx[r];
+    if (n_segments_out) n_segments_out[r] = nseg[S * r];
+    if (status_out) status_out[r] = status[S * r];
+    if (S == 2 && ref_n_segments_out) ref_n_segments_out[r] = nseg[2 * r + 1];
+    if (S == 2 && ref_status_out) ref_status_out[r] = status[2 * r + 1];
   }
   CK(cudaEventRecord(f->done, fin));
   f->pending = true;
   CK(cudaEventRecord(e->ev_out, fin));
   CK(cudaStreamWaitEvent(caller, e->ev_out, 0));
   return 0;
+}
+
+int nisqa_feed_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch* chunk, const uint8_t* end, float* scores_dev,
+                    int64_t n_rows, int32_t* feed_out, int64_t* index_out, int32_t* n_segments_out, int32_t* status_out) {
+  if (!f) return NISQA_ERR_INVALID;
+  if (f->n_src == 2)
+    return fail(f->e, NISQA_ERR_INVALID, "nisqa_feed_push: a pair feed object (nisqa_feed_pair_create) takes its pushes "
+                                         "through nisqa_feed_pair_push");
+  return feed_push(f, cuda_stream, chunk, nullptr, end, scores_dev, n_rows, feed_out, index_out, n_segments_out, status_out,
+                   nullptr, nullptr);
+}
+
+int nisqa_feed_pair_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch* deg, const nisqa_device_batch* ref,
+                         const uint8_t* end, float* scores_dev, int64_t n_rows, int32_t* feed_out, int64_t* index_out,
+                         int32_t* n_segments_out, int32_t* status_out, int32_t* ref_n_segments_out,
+                         int32_t* ref_status_out) {
+  if (!f) return NISQA_ERR_INVALID;
+  if (f->n_src != 2)
+    return fail(f->e, NISQA_ERR_INVALID, "nisqa_feed_pair_push: a single-ended feed object (nisqa_feed_create) takes its "
+                                         "pushes through nisqa_feed_push");
+  return feed_push(f, cuda_stream, deg, ref, end, scores_dev, n_rows, feed_out, index_out, n_segments_out, status_out,
+                   ref_n_segments_out, ref_status_out);
 }
 
 void nisqa_feed_destroy(nisqa_feed* f) {

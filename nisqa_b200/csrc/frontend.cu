@@ -672,11 +672,12 @@ frontend_windows_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ 
     for (int d = tid; d < n_dst; d += kFeThreads) atomicMax(clipmax + c0 + d * cstep, f2key(m));
 }
 
-// ---- live feeds (nisqa_feed_push) ------------------------------------------------------------------------------------
-// The interior pairs of one push: grid (pair of the push, feed).  A pair whose taps have all arrived and that some window
-// holds as an interior pair (k H <= a, a + hop + win <= k H + W, k of the pair's class) is computed once with win_pair
-// - the arithmetic of frontend_windows_kernel's shared pairs - over the W contiguous ring samples from its first tap,
-// and its two rows go to the feed's frame ring.  Windows take them from there when they complete (feed_rows_kernel).
+// ---- live feeds (nisqa_feed_push, nisqa_feed_pair_push) --------------------------------------------------------------
+// The interior pairs of one push of one source: grid (pair of the push, feed).  A pair whose taps have all arrived and
+// that some uniform window holds as an interior pair (k H - off <= a, a + hop + win <= k H - off + W, k >= ceil(off / H),
+// k of the pair's class) is computed once with win_pair - the arithmetic of frontend_windows_kernel's shared pairs - over
+// the W contiguous ring samples from its first tap, and its two rows go to the feed's frame ring.  Windows take them from
+// there when they complete (feed_rows_kernel).
 template <typename T, int MELS, bool PP>
 __global__ void __launch_bounds__(kFeThreads, 4)
 frontend_feed_kernel(const T* __restrict__ ring, const FeedPush* __restrict__ push, FeedGeom g,
@@ -692,9 +693,10 @@ frontend_feed_kernel(const T* __restrict__ ring, const FeedPush* __restrict__ pu
   if ((int)blockIdx.x >= fp.n_pairs) return;
   const long long j = fp.j0 + (long long)blockIdx.x * (3 - g.ncls);
   const long long a = g.s0 + j * g.hop, ext = g.hop + g.win;                   // first tap (>= 0: the host's range)
-  const long long k_hi = a / g.H;
-  long long k_lo = a + ext - g.W <= 0 ? 0 : (a + ext - g.W + g.H - 1) / g.H;
-  if (g.ncls == 2 && ((k_lo ^ j) & 1)) ++k_lo;      // (odd hf: window k pairs the frames from parity k & 1)
+  const long long k_hi = (a + g.off) / g.H;
+  long long k_lo = a + ext - g.W + g.off <= 0 ? 0 : (a + ext - g.W + g.off + g.H - 1) / g.H;
+  k_lo = max(k_lo, (long long)((g.off + g.H - 1) / g.H));     // (the front-clipped windows are computed per window)
+  if (g.ncls == 2 && ((k_lo ^ j ^ g.par) & 1)) ++k_lo;       // (odd hf: window k pairs the frames of parity k ^ par)
   if (k_lo > k_hi) return;
   const FbTables fb = fbs[g.fb_id];
   load_band_meta<MELS>(band_meta, fb, tid);
@@ -706,11 +708,14 @@ frontend_feed_kernel(const T* __restrict__ ring, const FeedPush* __restrict__ pu
   for (int u = tid; u < MELS / 2; u += kFeThreads) dst[u] = s4[u];
 }
 
-// The interior rows of a pass's feed windows from the frame ring: grid (block of kFeedRowPairs interior pairs, window).
-// Each window's clip-max key is the max over the rows it holds (order-independent: the same key as computing them).
+// The interior rows of a pass's feed windows from the frame ring of their source (g0 / frames0: degraded or single-ended,
+// g1 / frames1: reference): grid (block of kFeedRowPairs interior pairs, window).  Front-clipped reference windows (j0 <
+// 0) are skipped: the pass's spans compute them.  Each window's clip-max key is the max over the rows it holds
+// (order-independent: the same key as computing them).
 __global__ void __launch_bounds__(256)
-feed_rows_kernel(const ClipDesc* __restrict__ clips, const FeedWin* __restrict__ wins, FeedGeom g, int n_mels,
-                 const float* __restrict__ frames, float* __restrict__ mel, unsigned* __restrict__ clipmax) {
+feed_rows_kernel(const ClipDesc* __restrict__ clips, const FeedWin* __restrict__ wins, FeedGeom g0, FeedGeom g1, int n_mels,
+                 const float* __restrict__ frames0, const float* __restrict__ frames1, float* __restrict__ mel,
+                 unsigned* __restrict__ clipmax) {
   __shared__ float wred[8];
   const int c = blockIdx.y;
   const ClipDesc cd = clips[c];
@@ -720,12 +725,14 @@ feed_rows_kernel(const ClipDesc* __restrict__ clips, const FeedWin* __restrict__
   const int p0 = lead + blockIdx.x * kFeedRowPairs, p1 = min(tail, p0 + kFeedRowPairs);
   if (p0 >= p1) return;
   const FeedWin fw = wins[c];
+  if (fw.j0 < 0) return;
+  const int P = fw.src ? g1.P : g0.P, step = 3 - (fw.src ? g1.ncls : g0.ncls);
   const int q4 = n_mels / 2;                        // float4 per pair (two rows)
-  const float* src = frames + (size_t)fw.feed * g.P * 2 * n_mels;
+  const float* src = (fw.src ? frames1 : frames0) + (size_t)fw.feed * P * 2 * n_mels;
   float m = -INFINITY;
   for (int i = threadIdx.x; i < (p1 - p0) * q4; i += blockDim.x) {
     const int p = p0 + i / q4, u = i - (i / q4) * q4;
-    const long long slot = ((fw.j0 + 2 * p) / (3 - g.ncls)) % g.P;
+    const long long slot = ((fw.j0 + 2 * p) / step) % P;
     const float4 v = reinterpret_cast<const float4*>(src + (size_t)slot * 2 * n_mels)[u];
     reinterpret_cast<float4*>(mel + (size_t)(cd.frame_off + 2 * p) * n_mels)[u] = v;
     m = fmaxf(m, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
@@ -895,10 +902,11 @@ void launch_frontend_feed_pairs(cudaStream_t st, int n_mels, const void* ring, i
 }
 
 void launch_feed_rows(cudaStream_t st, int n_mels, const ClipDesc* clips, const FeedWin* wins, int n_clips, int max_interior,
-                      const FeedGeom& g, const float* frames, float* mel, unsigned* clipmax) {
+                      const FeedGeom& g0, const FeedGeom& g1, const float* frames0, const float* frames1, float* mel,
+                      unsigned* clipmax) {
   if (n_clips <= 0 || max_interior <= 0) return;
   const dim3 grid((max_interior + kFeedRowPairs - 1) / kFeedRowPairs, n_clips);
-  feed_rows_kernel<<<grid, 256, 0, st>>>(clips, wins, g, n_mels, frames, mel, clipmax);
+  feed_rows_kernel<<<grid, 256, 0, st>>>(clips, wins, g0, g1, n_mels, frames0, frames1, mel, clipmax);
 }
 
 bool frontend_supports_mels(int n_mels) {

@@ -116,15 +116,18 @@ void launch_frontend(cudaStream_t st, int n_mels, const void* pcm, int fmt_f32, 
 void launch_frontend_windows(cudaStream_t st, int n_mels, const void* pcm, int fmt_f32, const ClipDesc* clips, int n_clips,
                              int edge_pairs, const WinSpan* spans, int n_spans, int span_pairs, int ncls,
                              const FbTables* fbs, const float2* tw, float* mel, unsigned* clipmax, int Q, int max_span);
-// Live feeds (FeedGeom): the interior frame pairs of a push into the frame ring, once (grid max n_pairs x n_feeds), with
-// the arithmetic the clip path picks for the feed's rate; then, in each pass, the interior rows of the pass's windows
-// from the frame ring into their mel rows, with each window's clip-max key (grid pair blocks x n_clips; the edge pairs
-// come from launch_frontend_windows without spans).  Rows bit-identical to launch_frontend over the windows as clips.
+// Live feeds (FeedGeom): the interior frame pairs of a push of one source into its frame ring, once (grid max n_pairs x
+// n_feeds), with the arithmetic the clip path picks for the feed's rate; then, in each pass, the interior rows of the
+// pass's windows from their source's frame ring (g0 / frames0: degraded or single-ended, g1 / frames1: reference) into
+// their mel rows, with each window's clip-max key (grid pair blocks x n_clips; the edge pairs, and every pair of a
+// front-clipped reference window as a one-window span, come from launch_frontend_windows).  Rows bit-identical to
+// launch_frontend over the windows as clips.
 void launch_frontend_feed_pairs(cudaStream_t st, int n_mels, const void* ring, int fmt_f32, const FeedPush* push, int n_feeds,
                                 int max_pairs, const FeedGeom& g, const FbTables* fbs, const float2* tw, float* frames);
 constexpr int kFeedRowPairs = 32;    // interior pairs per CTA of the row copy
 void launch_feed_rows(cudaStream_t st, int n_mels, const ClipDesc* clips, const FeedWin* wins, int n_clips, int max_interior,
-                      const FeedGeom& g, const float* frames, float* mel, unsigned* clipmax);
+                      const FeedGeom& g0, const FeedGeom& g1, const float* frames0, const float* frames1, float* mel,
+                      unsigned* clipmax);
 void launch_seg_table(cudaStream_t st, const ClipDesc* clips, int n_clips, const int* seg_prefix, const unsigned* clipmax,
                       int seg_hop, int n_seg, int* seg_frame0, float* seg_thr, int* seg_clip);
 void launch_mel_dump(cudaStream_t st, const float* mel, const ClipDesc* clips, int n_clips, const unsigned* clipmax, int n_mels,

@@ -21,19 +21,23 @@ struct WinSpan {
   int cstride;         // 1; window pairs: 2 (the clips of a pass alternate degraded and reference windows)
 };
 
-// Live feeds (nisqa_feed_*): n_feeds recordings that grow push by push.  Feed b's samples live in a ring of R >= W +
-// max_push samples at element b * stride of the sample ring, sample t at t mod R; the first W ring positions are mirrored
-// at R .. R + W - 1 (stride = R + W), so that any W consecutive samples of the recording are contiguous.  Its interior
-// frame pairs (taps inside every window that holds them) are computed once, as soon as their last tap arrives, into a
-// ring of P pair slots of 2 n_mels floats at (b P + slot) 2 n_mels of the frame ring: the pair of global first frame j
-// at slot (j / (3 - ncls)) mod P (ncls 1: windows pair even frames only; 2: the window hop is an odd number of frames,
-// both pairings are kept).
+// Live feeds (nisqa_feed_*): n_feeds recordings that grow push by push, from one source (nisqa_feed_create) or two
+// (nisqa_feed_pair_create: degraded, reference), each source with its own FeedGeom and its own region of the object's
+// sample ring and frame ring.  Window k of a source covers [k H - off, k H - off + W) (clipped to the recording); feed
+// b's samples live in a ring of R samples at element b * stride of the source's region, sample t at t mod R; the first W
+// ring positions are mirrored at R .. R + W - 1 (stride = R + W), so that any W consecutive samples of the recording are
+// contiguous.  Its interior frame pairs (taps inside every window k >= ceil(off / H) that holds them) are computed once,
+// as soon as their last tap arrives, into a ring of P pair slots of 2 n_mels floats at (b P + slot) 2 n_mels of the
+// source's frame region: the pair of global first frame j at slot (j / (3 - ncls)) mod P (ncls 1: window k pairs the
+// frames from k hf - off / hop, all of parity par; 2: the window hop is an odd number of frames, both pairings are kept).
+// The windows k < ceil(off / H) start at sample 0 (front-clipped reference windows) and are computed per window.
 struct FeedGeom {
   long long stride;    // elements per feed in the sample ring (R + W)
-  int R, W, H, hf;     // ring length; window length and hop (samples, mel frames)
+  int R, W, H, hf;     // ring length; window length (reference: window + 2 margin) and hop (samples, mel frames)
   int hop, win, s0;    // the model rate's mel frame hop, window and first tap of frame 0 (ClipDesc)
   int P, ncls, fb_id;  // pair slots per feed, pairing classes, front-end tables
-  int pad_;
+  int off, par;        // window k starts at k H - off (the reference margin M; 0 for degraded and single-ended
+                       // feeds); the parity of the frames its pairs start at when ncls is 1 ((off / hop) & 1)
 };
 // One feed in one push (uploaded per push)
 struct FeedPush {
@@ -44,9 +48,10 @@ struct FeedPush {
 };
 // One window of a feed in a pass (one per ClipDesc row of the pass)
 struct FeedWin {
-  long long j0;        // global frame of the window's frame 0 (k hf)
+  long long j0;        // global frame of the window's frame 0 (k hf - off / hop); -1: a front-clipped reference window,
+                       // whose rows come from the pass's spans rather than the frame ring
   int feed;
-  int pad_;
+  int src;             // 0: degraded (or single-ended), 1: reference - the FeedGeom and frame ring it reads
 };
 
 // Frame pairs p = 0 .. (n_frames + 1) / 2 - 1 of a clip whose taps (s0 + 2 p hop .. + hop + win - 1) all lie inside

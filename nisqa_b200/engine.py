@@ -42,7 +42,7 @@ EXPORTS = [
     "nisqa_predict_device_batch_segments", "nisqa_window_counts", "nisqa_predict_device_windows",
     "nisqa_feed_create", "nisqa_feed_rows", "nisqa_feed_push", "nisqa_feed_device_bytes", "nisqa_feed_destroy",
     "nisqa_embedding_width", "nisqa_predict_device_batch_embeddings", "nisqa_window_pair_counts",
-    "nisqa_predict_device_window_pairs",
+    "nisqa_predict_device_window_pairs", "nisqa_feed_pair_create", "nisqa_feed_pair_rows", "nisqa_feed_pair_push",
 ]
 
 
@@ -279,6 +279,14 @@ def load_library(path=None):
     lib.nisqa_feed_device_bytes.restype = C.c_int64
     lib.nisqa_feed_destroy.argtypes = [vp]
     lib.nisqa_feed_destroy.restype = None
+    lib.nisqa_feed_pair_create.argtypes = [vp, C.POINTER(vp), C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32,
+                                           C.c_int64, C.c_int64]
+    lib.nisqa_feed_pair_create.restype = C.c_int
+    lib.nisqa_feed_pair_rows.argtypes = [C.POINTER(NisqaConfig), C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+                                         i64p, i64p, i64p, i64p, u8p, i64p, i32p, i64p, i32p, i32p, i32p, i32p, C.c_int64]
+    lib.nisqa_feed_pair_rows.restype = C.c_int
+    lib.nisqa_feed_pair_push.argtypes = [vp, vp, dbp, dbp, u8p, vp, C.c_int64, i32p, i64p, i32p, i32p, i32p, i32p]
+    lib.nisqa_feed_pair_push.restype = C.c_int
     lib.nisqa_stage_dump.argtypes = [vp, C.c_int, f32p, C.c_int64]
     lib.nisqa_stage_dump.restype = C.c_int64
     lib.nisqa_segment_counts.argtypes = [C.POINTER(NisqaConfig), C.c_int64, C.c_int32, i32p, i32p, i32p]
@@ -574,6 +582,28 @@ def feed_rows(cfg, sample_rate, window, hop_frames, held, n_samples, end=None):
     lib.nisqa_feed_rows(*args, _ptr(feed, C.c_int32), _ptr(index, C.c_int64), _ptr(nseg, C.c_int32),
                         _ptr(status, C.c_int32), n.value)
     return feed, index, nseg, status
+
+
+def feed_pair_rows(cfg, sample_rate, window, hop_frames, margin_frames, held, ref_held, n_samples, ref_n_samples,
+                   end=None):
+    """(feed int32[N], index int64[N], n_segments, status, ref_n_segments, ref_status int32[N]) of the window pairs a push
+    of ``n_samples`` degraded and ``ref_n_samples`` reference samples (and ``end`` flags) to pair feeds that hold
+    ``held`` / ``ref_held`` samples emits, in feed then pair order (nisqa_feed_pair_rows, host arithmetic)"""
+    lib = load_library()
+    arrs = [np.ascontiguousarray(a, dtype=np.int64) for a in (held, ref_held, n_samples, ref_n_samples)]
+    e = None if end is None else np.ascontiguousarray(end, dtype=np.uint8)
+    n = C.c_int64()
+    args = (C.byref(cfg), int(sample_rate), int(window), int(hop_frames), int(margin_frames), len(arrs[0]),
+            *[_ptr(a, C.c_int64) for a in arrs], None if e is None else _ptr(e, C.c_uint8), C.byref(n))
+    rc = lib.nisqa_feed_pair_rows(*args, None, None, None, None, None, None, 0)
+    if rc != 0:
+        raise EngineError("nisqa_feed_pair_rows failed (%d): window %d, hop_frames %d, margin_frames %d at %d Hz"
+                          % (rc, window, hop_frames, margin_frames, sample_rate))
+    feed, index = np.empty(n.value, np.int32), np.empty(n.value, np.int64)
+    out = [np.empty(n.value, np.int32) for _ in range(4)]
+    lib.nisqa_feed_pair_rows(*args, _ptr(feed, C.c_int32), _ptr(index, C.c_int64), *[_ptr(a, C.c_int32) for a in out],
+                             n.value)
+    return (feed, index) + tuple(out)
 
 
 class Engine(object):
@@ -882,6 +912,31 @@ class Engine(object):
             None if e is None else _ptr(e, C.c_uint8), C.c_void_p(scores_dev_ptr), int(n_rows), _ptr(fo, C.c_int32),
             _ptr(index, C.c_int64), _ptr(nseg, C.c_int32), _ptr(status, C.c_int32)), "nisqa_feed_push")
         return fo, index, nseg, status
+
+    def feed_pair_create(self, n_feeds, sample_rate, window, hop_frames, margin_frames, max_push, max_skew):
+        """A pair feed object (nisqa_feed_pair_create) -> its handle (an int)"""
+        h = C.c_void_p()
+        self._check(self.lib.nisqa_feed_pair_create(self.h, C.byref(h), int(n_feeds), int(sample_rate), int(window),
+                                                    int(hop_frames), int(margin_frames), int(max_push), int(max_skew)),
+                    "nisqa_feed_pair_create")
+        self._feeds.add(h.value)
+        return h.value
+
+    def feed_pair_push(self, feed, stream, deg, ref, end, scores_dev_ptr, n_rows):
+        """nisqa_feed_pair_push of ``deg`` and ``ref`` (:func:`device_batch` tuples, 0 samples allowed) and ``end``
+        (uint8[n_feeds] or None) ordered on ``stream``; the scores of the completed pairs to ``scores_dev_ptr`` ([n_rows,
+        n_out] fp32 device memory).  Returns (feed, index, n_segments, status, ref_n_segments, ref_status) arrays of
+        n_rows entries (size n_rows with :func:`feed_pair_rows`), valid on return; raises EngineError, with nothing
+        enqueued, for a refused push."""
+        n = max(int(n_rows), 0)
+        fo, index = np.empty(n, np.int32), np.empty(n, np.int64)
+        out = [np.empty(n, np.int32) for _ in range(4)]
+        e = None if end is None else np.ascontiguousarray(end, dtype=np.uint8)
+        self._check(self.lib.nisqa_feed_pair_push(
+            C.c_void_p(self._feed(feed)), C.c_void_p(stream or None), C.byref(deg[0]), C.byref(ref[0]),
+            None if e is None else _ptr(e, C.c_uint8), C.c_void_p(scores_dev_ptr), int(n_rows), _ptr(fo, C.c_int32),
+            _ptr(index, C.c_int64), *[_ptr(a, C.c_int32) for a in out]), "nisqa_feed_pair_push")
+        return (fo, index) + tuple(out)
 
     def _feed(self, feed):
         if feed not in self._feeds:

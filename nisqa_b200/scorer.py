@@ -21,7 +21,8 @@ scores window pairs of a recording and its reference: ``scorer.windows(wave, 480
 
 ``scorer.feed(256, 48000, 10.0, 1.0)`` scores live sources as their audio arrives: ``feed.push(chunk)`` appends a chunk to
 every source and returns the windows it completed, with the scores ``windows`` gives on the whole recording
-(``nisqa_feed_push``).
+(``nisqa_feed_push``).  A NISQA_DE checkpoint scores live (degraded, reference) pairs:
+``scorer.feed(256, 48000, 10.0, 1.0, reference=True)`` and ``feed.push(chunk, ref_chunk)`` (``nisqa_feed_pair_push``).
 """
 import collections
 import numbers
@@ -52,6 +53,11 @@ WindowPairs = collections.namedtuple("WindowPairs", ["scores", "counts", "t_star
 # index int64 [N] (window k of the feed's current recording), t_start / t_end float64 [N] seconds, n_segments / status
 # int32 [N] host arrays
 FeedRows = collections.namedtuple("FeedRows", ["scores", "feed", "index", "t_start", "t_end", "n_segments", "status"])
+# FeedPairs.push: the fields of FeedRows for the window pairs the push completed (one score row per pair; t_start / t_end,
+# n_segments / status of the degraded windows), and ref_t_start / ref_t_end float64 [N] seconds, ref_n_segments /
+# ref_status int32 [N] of the reference windows, host arrays
+FeedPairRows = collections.namedtuple("FeedPairRows", FeedRows._fields + ("ref_t_start", "ref_t_end", "ref_n_segments",
+                                                                          "ref_status"))
 
 
 def window_geometry(args, rate, window_s, window_hop_s):
@@ -248,13 +254,36 @@ class Scorer(object):
         cols = [np.concatenate([p[i] for p in parts]).astype(t) if parts else np.zeros(0, t) for i, t in enumerate(types)]
         return Windows(out, counts, *cols) if ref is None else WindowPairs(out, counts, *cols)
 
-    def feed(self, n_feeds, sample_rate, window_s, window_hop_s, channel=None, max_push_s=None):
+    def feed(self, n_feeds, sample_rate, window_s, window_hop_s, channel=None, max_push_s=None, reference=None,
+             reference_margin_s=0.0, max_skew_s=None):
         """A :class:`Feed` of ``n_feeds`` live recordings at ``sample_rate``, scored as the windows of :meth:`windows`
         (``window_s``, ``window_hop_s``, checked alike) as soon as each window is complete.  ``channel`` applies to every
         push (None: the mono mix); ``max_push_s`` (default ``window_s``) is the longest chunk one push may append to one
-        feed, which sizes the feed's device rings.  A checkpoint with ``ms_sr`` takes feeds at that rate only."""
-        if self.double_ended:
-            raise ValueError("feed: a double-ended (NISQA_DE) checkpoint scores (wave, reference) pairs, not live feeds")
+        feed, which sizes the feed's device rings.  A checkpoint with ``ms_sr`` takes feeds at that rate only.
+
+        NISQA_DE: ``reference=True`` returns :class:`FeedPairs`, ``n_feeds`` live (degraded, reference) recording pairs
+        scored as the window pairs of ``windows(..., reference=, reference_margin_s=)`` as soon as both windows of a pair
+        are complete; ``channel`` applies to the degraded side, the reference is always the mono mix.  ``max_skew_s``
+        (default ``max_push_s``) is the most a feed's two sides may differ in length after any push: pairs wait for the
+        slower side, so the rings hold the faster side's backlog (device memory grows with it).  Recordings whose two
+        sides end further apart than that need a larger ``max_skew_s``."""
+        m = reference_margin_s
+        if reference is not None and not isinstance(reference, bool):
+            raise TypeError("reference: True (NISQA_DE: live (degraded, reference) pairs) or None, not %r" % (reference,))
+        if isinstance(m, bool) or not isinstance(m, numbers.Real) or not np.isfinite(m) or m < 0:
+            raise ValueError("reference_margin_s: a non-negative number of seconds, not %r" % (m,))
+        if not reference:
+            if m != 0:
+                raise ValueError("reference_margin_s=%r: a margin widens reference windows; pass reference=True "
+                                 "(NISQA_DE)" % (m,))
+            if max_skew_s is not None:
+                raise ValueError("max_skew_s=%r: the skew of a feed's two sides; pass reference=True (NISQA_DE)"
+                                 % (max_skew_s,))
+            if self.double_ended:
+                raise ValueError("feed: a double-ended (NISQA_DE) checkpoint scores (wave, reference) pairs, not live "
+                                 "feeds; pass reference=True")
+        elif not self.double_ended:
+            raise ValueError("reference: only a double-ended (NISQA_DE) checkpoint scores live (degraded, reference) pairs")
         if isinstance(n_feeds, bool) or not isinstance(n_feeds, numbers.Integral) or not 1 <= n_feeds <= 65535:
             raise ValueError("n_feeds: an int within 1 .. 65535, not %r" % (n_feeds,))
         if isinstance(sample_rate, bool) or not isinstance(sample_rate, numbers.Integral) or sample_rate <= 0:
@@ -265,9 +294,9 @@ class Scorer(object):
         if channel is not None and (isinstance(channel, bool) or not isinstance(channel, numbers.Integral) or channel < 0):
             raise TypeError("channel: a non-negative int or None, not %r" % (channel,))
         W, hop_frames = window_geometry(self.args, sample_rate, window_s, window_hop_s)
+        a = self.args
         _, n_seg, status = E.segment_counts(self.cfg, W, sample_rate)
         if status != E.CLIP_OK:
-            a = self.args
             err = E.clip_status_error(status, "window_s=%r (%d samples at %d Hz)" % (window_s, W, sample_rate), W,
                                       sample_rate, n_seg, a["ms_hop_length"], a["ms_seg_length"], a["ms_max_segments"])
             raise ValueError("window_s: " + str(err))
@@ -276,7 +305,24 @@ class Scorer(object):
         if isinstance(max_push_s, bool) or not isinstance(max_push_s, numbers.Real) or not np.isfinite(max_push_s) \
                 or max_push_s <= 0 or int(round(max_push_s * sample_rate)) < 1:
             raise ValueError("max_push_s: a positive number of seconds (at least one sample), not %r" % (max_push_s,))
-        return Feed(self, int(n_feeds), int(sample_rate), W, hop_frames, channel, int(round(max_push_s * sample_rate)))
+        max_push = int(round(max_push_s * sample_rate))
+        if not reference:
+            return Feed(self, int(n_feeds), int(sample_rate), W, hop_frames, channel, max_push)
+        hop = int(sample_rate * a["ms_hop_length"])
+        margin_frames = int(round(m * sample_rate / hop))
+        M = margin_frames * hop
+        _, n_seg, status = E.segment_counts(self.cfg, W + 2 * M, sample_rate)
+        if status != E.CLIP_OK:
+            raise ValueError("reference_margin_s=%r: reference windows of %d samples (W + 2 x %d) have %d segments > "
+                             "ms_max_segments %d" % (m, W + 2 * M, M, n_seg, a["ms_max_segments"]))
+        if max_skew_s is None:
+            max_skew = max_push
+        elif isinstance(max_skew_s, bool) or not isinstance(max_skew_s, numbers.Real) or not np.isfinite(max_skew_s) \
+                or max_skew_s < 0:
+            raise ValueError("max_skew_s: a non-negative number of seconds, not %r" % (max_skew_s,))
+        else:
+            max_skew = int(round(max_skew_s * sample_rate))
+        return FeedPairs(self, int(n_feeds), int(sample_rate), W, hop_frames, channel, max_push, margin_frames, max_skew)
 
     def embed(self, wave, sample_rate, lengths=None, channel=None, reference=None, reference_lengths=None,
               reference_sample_rate=None, rows=False):
@@ -411,7 +457,10 @@ class Feed(object):
         self.hop = hop_frames * int(sample_rate * scorer.args["ms_hop_length"])
         self.held = np.zeros(n_feeds, np.int64)          # samples of each feed's current recording
         self._fmt = None                                  # the format the feeds' samples are held in
-        self._h = scorer.engine.feed_create(n_feeds, sample_rate, W, hop_frames, max_push)
+        self._h = self._create()
+
+    def _create(self):
+        return self.scorer.engine.feed_create(self.n_feeds, self.sample_rate, self.window, self.hop_frames, self.max_push)
 
     @property
     def device_bytes(self):
@@ -439,32 +488,10 @@ class Feed(object):
         Window k of a feed is emitted by the first push after which the feed holds k H + W samples of its recording,
         with the scores ``Scorer.windows`` gives that window of the whole recording, bit for bit.
         """
-        if self._h is None:
-            raise ValueError("push: the feed is closed")
-        if isinstance(wave, torch.Tensor) and wave.shape[-1] == 0:
-            if lengths is not None and np.any(np.asarray(lengths) != 0):
-                raise ValueError("lengths: a chunk of 0 samples holds no sample")
-            wave = torch.zeros(tuple(wave.shape[:-1]) + (1,), dtype=wave.dtype, device=wave.device)
-            lengths = [0] * (wave.shape[0] if wave.dim() > 1 else 1)
-        deg = self.scorer._batch("wave", wave, self.sample_rate, lengths, self.channel, min_len=0)
+        deg = self._chunk("wave", wave, lengths, self.channel)
+        ends = self._ends(end)
         b, ns = deg
-        if b.n_clips != self.n_feeds:
-            raise ValueError("wave: %d feeds (clips) in the chunk for a feed object of %d feeds" % (b.n_clips, self.n_feeds))
-        over = np.nonzero(ns > self.max_push)[0]
-        if over.size:
-            raise ValueError("lengths[%d] = %d: more than max_push_s (%d samples)" % (over[0], ns[over[0]], self.max_push))
-        if end is None:
-            ends = np.zeros(self.n_feeds, np.uint8)
-        else:
-            ends = np.asarray(end.tolist() if isinstance(end, torch.Tensor) else end)
-            if ends.shape != (self.n_feeds,) or not (ends.dtype == np.bool_ or np.issubdtype(ends.dtype, np.integer)):
-                raise ValueError("end: one bool per feed (%d), not %r" % (self.n_feeds, end))
-            ends = ends.astype(bool).astype(np.uint8)
-        fmt = E.FMT_S16 if b.sample_fmt == E.FMT_S16 and (b.n_channels == 1 or b.channel >= 0) else E.FMT_F32
-        if ns.sum() > 0 and self.held.sum() > 0 and fmt != self._fmt:
-            raise ValueError("wave: %s samples, but the feeds hold %s ones until every feed has ended" % (
-                "mono int16" if fmt == E.FMT_S16 else "float32 (or mixed)",
-                "mono int16" if self._fmt == E.FMT_S16 else "float32 (or mixed)"))
+        self._check_format(self._format(b), ns.sum() > 0, self.held.sum() > 0, "wave")
         eng = self.scorer.engine
         feed, index, _, _ = E.feed_rows(self.scorer.cfg, self.sample_rate, self.window, self.hop_frames, self.held, ns, ends)
         N = feed.shape[0]
@@ -474,6 +501,106 @@ class Feed(object):
         t_start = index * self.hop / self.sample_rate
         t_end = np.minimum(index * self.hop + self.window, T[feed]) / self.sample_rate
         if ns.sum() > 0:
-            self._fmt = fmt
+            self._fmt = self._format(b)
         self.held = np.where(ends.astype(bool), 0, T)
         return FeedRows(out, f2, i2, t_start, t_end, nseg, status)
+
+    # ------------------------------------------------------------------ shared by Feed.push and FeedPairs.push
+    def _chunk(self, name, wave, lengths, channel):
+        """-> engine.device_batch(...) of one chunk argument (``wave`` or ``reference``), after its checks"""
+        if self._h is None:
+            raise ValueError("push: the feed is closed")
+        what = "reference_lengths" if name == "reference" else "lengths"
+        if isinstance(wave, torch.Tensor) and wave.shape[-1] == 0:
+            if lengths is not None and np.any(np.asarray(lengths) != 0):
+                raise ValueError("%s: a chunk of 0 samples holds no sample" % what)
+            wave = torch.zeros(tuple(wave.shape[:-1]) + (1,), dtype=wave.dtype, device=wave.device)
+            lengths = [0] * (wave.shape[0] if wave.dim() > 1 else 1)
+        batch = self.scorer._batch(name, wave, self.sample_rate, lengths, channel, min_len=0)
+        b, ns = batch
+        if b.n_clips != self.n_feeds:
+            raise ValueError("%s: %d feeds (clips) in the chunk for a feed object of %d feeds" % (name, b.n_clips, self.n_feeds))
+        over = np.nonzero(ns > self.max_push)[0]
+        if over.size:
+            raise ValueError("%s[%d] = %d: more than max_push_s (%d samples)" % (what, over[0], ns[over[0]], self.max_push))
+        return batch
+
+    def _ends(self, end):
+        if end is None:
+            return np.zeros(self.n_feeds, np.uint8)
+        ends = np.asarray(end.tolist() if isinstance(end, torch.Tensor) else end)
+        if ends.shape != (self.n_feeds,) or not (ends.dtype == np.bool_ or np.issubdtype(ends.dtype, np.integer)):
+            raise ValueError("end: one bool per feed (%d), not %r" % (self.n_feeds, end))
+        return ends.astype(bool).astype(np.uint8)
+
+    @staticmethod
+    def _format(b):
+        """the ring format of a chunk: mono int16 (one channel, or one picked) or float32 (float32 or mixed)"""
+        return E.FMT_S16 if b.sample_fmt == E.FMT_S16 and (b.n_channels == 1 or b.channel >= 0) else E.FMT_F32
+
+    def _check_format(self, fmt, pushes, holds, name):
+        if pushes and holds and fmt != self._fmt:
+            raise ValueError("%s: %s samples, but the feeds hold %s ones until every feed has ended" % (
+                name, "mono int16" if fmt == E.FMT_S16 else "float32 (or mixed)",
+                "mono int16" if self._fmt == E.FMT_S16 else "float32 (or mixed)"))
+
+
+class FeedPairs(Feed):
+    """Live (degraded, reference) recording pairs of a NISQA_DE checkpoint scored window pair by window pair as both
+    sides' samples arrive (``Scorer.feed(..., reference=True)``).  Closes, reports ``device_bytes`` and orders its pushes
+    as :class:`Feed`."""
+
+    def __init__(self, scorer, n_feeds, sample_rate, W, hop_frames, channel, max_push, margin_frames, max_skew):
+        self.margin_frames, self.max_skew = margin_frames, max_skew
+        self.margin = margin_frames * int(sample_rate * scorer.args["ms_hop_length"])
+        self.ref_held = np.zeros(n_feeds, np.int64)      # reference samples of each feed's current recording pair
+        super(FeedPairs, self).__init__(scorer, n_feeds, sample_rate, W, hop_frames, channel, max_push)
+
+    def _create(self):
+        return self.scorer.engine.feed_pair_create(self.n_feeds, self.sample_rate, self.window, self.hop_frames,
+                                                   self.margin_frames, self.max_push, self.max_skew)
+
+    def push(self, wave, reference, lengths=None, reference_lengths=None, end=None):
+        """Append a degraded and a reference chunk to every feed and score the window pairs they complete ->
+        :data:`FeedPairRows`.
+
+        wave, lengths      : the degraded chunks, as :meth:`Feed.push` (the feed's ``channel`` applies)
+        reference          : the reference chunks, [B, T] or [B, C, T] int16 / float32 CUDA tensor (always mixed to mono),
+                             with their own ``reference_lengths``; either side may bring 0 samples
+        end                : host bools, one per feed: both recordings of the feed end after this push; its remaining
+                             pairs are scored as ``Scorer.windows(..., reference=)`` scores the last ones of the final
+                             lengths (a reference window that is empty scores NaN with ``ref_status`` CLIP_TOO_SHORT), and
+                             the next sample on either side starts a new pair of recordings
+        Pair k of a feed is emitted by the first push after which the feed holds k H + W degraded and k H + W + M
+        reference samples, with the scores ``Scorer.windows(..., reference=, reference_margin_s=)`` gives that pair of
+        the whole recordings, bit for bit.  Both sides share one sample format (float32 if either is float32 or mixed),
+        which holds until every feed has ended; after a push, a feed's two lengths may differ by at most max_skew_s.
+        """
+        deg = self._chunk("wave", wave, lengths, self.channel)
+        ref = self._chunk("reference", reference, reference_lengths, None)
+        ends = self._ends(end)
+        (b, ns), (rb, rns) = deg, ref
+        T, T_ref = self.held + ns, self.ref_held + rns
+        skew = np.nonzero(np.abs(T - T_ref) > self.max_skew)[0]
+        if skew.size:
+            i = skew[0]
+            raise ValueError("lengths / reference_lengths: feed %d would hold %d degraded and %d reference samples, more "
+                             "than max_skew_s (%d samples) apart" % (i, T[i], T_ref[i], self.max_skew))
+        fmt = E.FMT_F32 if E.FMT_F32 in (self._format(b), self._format(rb)) else E.FMT_S16
+        pushes = ns.sum() + rns.sum() > 0
+        self._check_format(fmt, pushes, self.held.sum() + self.ref_held.sum() > 0, "wave / reference")
+        eng = self.scorer.engine
+        feed, index = E.feed_pair_rows(self.scorer.cfg, self.sample_rate, self.window, self.hop_frames, self.margin_frames,
+                                       self.held, self.ref_held, ns, rns, ends)[:2]
+        N = feed.shape[0]
+        out = torch.empty((N, len(self.scorer.columns)), dtype=torch.float32, device=self.scorer.device)
+        rows = eng.feed_pair_push(self._h, self.scorer._stream(), deg, ref, ends, out.data_ptr(), N)
+        kH, W, M, rate = index * self.hop, self.window, self.margin, self.sample_rate
+        r0 = np.maximum(0, kH - M)
+        r1 = np.maximum(r0, np.minimum(T_ref[feed], kH + W + M))
+        if pushes:
+            self._fmt = fmt
+        self.held = np.where(ends.astype(bool), 0, T)
+        self.ref_held = np.where(ends.astype(bool), 0, T_ref)
+        return FeedPairRows(out, rows[0], rows[1], kH / rate, np.minimum(kH + W, T[feed]) / rate, rows[2], rows[3],
+                            r0 / rate, r1 / rate, rows[4], rows[5])

@@ -4,7 +4,7 @@
 # short clips at 48 / 16 kHz: front-end, conv1, the five wgmma conv layers with their bulk copies /
 # mbarriers, self-attention, pooling), over a 96 kHz clip (frontend_kernel, the front end for windows over 1024
 # samples), over a short nisqa_tts.tar call (StandardCNN, BiLSTM) and over device-batch
-# calls (the ingest kernel, with and without ms_sr, one segments call, one embeddings call, two windows calls and a live feed); racecheck over the double-ended alignment's multi-block path.
+# calls (the ingest kernel, with and without ms_sr, one segments call, one embeddings call, two windows calls, a live feed and a live pair feed); racecheck over the double-ended alignment's multi-block path.
 #   bash tools/sanitize.sh TAG
 TAG=${1:-rXX}
 OUT=gpurun_out
@@ -87,6 +87,25 @@ for t in range(0, T, n):
     print("feed", out.scores.tolist())
 fd.close()
 s6.close()
+# live pair feeds (both sources' rings in one allocation, the reference's offset geometry and mirror of W + 2M, the
+# front-clipped reference windows as one-window spans over the ring): one pair of 16 s / 15.5 s at 16 kHz with a 1.5 s
+# margin (two front-clipped windows), 0.5 s pushes and the reference 1 s behind (the maximal skew), so both rings wrap;
+# the ending push emits end-clipped reference windows
+import tempfile
+a7, s7 = V.de_checkpoint("de_cosine_hard", bargs, bsd)
+p7 = os.path.join(tempfile.mkdtemp(), "de.tar")
+torch.save({"args": a7, "model_state_dict": s7}, p7)
+s8 = Scorer(p7)
+d8 = torch.from_numpy(synth.synth_speech_pcm16(18, 16.0, 16000)).cuda()
+fp = s8.feed(1, 16000, 5.0, 1.0, max_push_s=0.5, reference=True, reference_margin_s=1.5, max_skew_s=1.0)
+n, Td, Tr = 8000, 256000, 248000
+for t in range(0, Td + n, n):
+    a, b = min(n, max(0, Td - t)), min(n, max(0, Tr - (t - 16000))) if t >= 16000 else 0
+    out = fp.push(d8[None, t:t + n], d8[None, max(0, t - 16000):max(0, t - 16000) + n], lengths=[a], reference_lengths=[b],
+                  end=[t + n >= Td + n])
+    print("pair feed", out.scores.tolist())
+fp.close()
+s8.close()
 PY
 timeout 400 compute-sanitizer --tool memcheck --error-exitcode 7 --log-file $OUT/${TAG}_memcheck.log python /tmp/san_run.py > $OUT/${TAG}_memcheck_stdout.log 2>&1
 echo "memcheck exit $?"
