@@ -14,6 +14,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <functional>
 #include <map>
 #include <memory>
 #include <string>
@@ -246,13 +247,8 @@ struct nisqa_engine {
   // call's last pass (the caller's stream waits for it)
   cudaEvent_t ev_in = nullptr, ev_out = nullptr;
   float pool_bias_std = 0.f;
-  // nisqa_predict_device_batch_segments: the call's output rows (nullptr outside such a call) and the first row of each
-  // clip of the call (-1: none)
-  const nisqa_segment_out* seg_out = nullptr;
-  std::vector<long long> seg_row;
-  // nisqa_predict_device_batch_embeddings: the call's outputs (nullptr outside such a call; its rows use seg_row), and
-  // Weights.pool_src on the device (unset when the rows are in the reference's order)
-  const nisqa_embedding_out* emb_out = nullptr;
+  // nisqa_predict_device_batch_embeddings: Weights.pool_src on the device (unset when the rows are in the reference's
+  // order)
   DevBuf emb_src;
   float tc_scale[8] = {1, 1, 1, 1, 1, 1, 1, 1};   // 2^(e_{i-1} - S_i): undoes the activation and weight pre-scales of conv i
   int act_exp[8] = {0, 0, 0, 0, 0, 0, 0, 0};      // e_i: conv i's activations are stored as fp16 planes of v * 2^-e_i
@@ -1220,7 +1216,7 @@ struct FeedRings {
   long long ring_at[2];
   const float* frames[2];
 };
-// A windows call (nisqa_predict_device_windows): its windows are the clips of predict_common, in recording order.  A
+// A windows call (nisqa_predict_device_windows): its windows are the clips of the call, in recording order.  A
 // window-pairs call (nisqa_predict_device_window_pairs, n_src 2): clip 2p is pair p's degraded window, clip 2p + 1 its
 // reference window, and the scores are compact, one row per pair.
 struct WinLayout {
@@ -1246,6 +1242,46 @@ struct WinPass {
   int interior = 0;
 };
 
+// One scoring call, as its entry point describes it: the clips, exactly one input, the outputs and how the call
+// completes.  plan_call fills `plan` and `seg_row`.
+struct Call {
+  int n_clips;
+  const int64_t* n_samples;           // [n_clips] at the rate the clips are scored at
+  const int32_t* sample_rate;         // [n_clips]
+  int fmt;                            // NISQA_FMT_* of the input
+  // the input, exactly one of: per-clip host pointers; a packed device buffer and each clip's element offset (a windows
+  // call or feed push: dev_off nullptr, `win` places the windows); the caller's strided device batch
+  const void* const* host_pcm = nullptr;
+  const void* dev_pcm = nullptr;
+  const int64_t* dev_off = nullptr;
+  const IngestSources* ingest = nullptr;
+  // target_sr > 0 (ms_sr): the caller's batch holds n_rec recordings of rec_n samples at rec_sr (IngestSources order),
+  // converted whole to target_sr before the passes, as a span converted alone differs at its edges
+  int32_t target_sr = 0;
+  int n_rec = 0;
+  const int64_t* rec_n = nullptr;
+  const int32_t* rec_sr = nullptr;
+  // outputs: host or device scores [n_clips][n_out] (a window-pairs call: one row per pair), each clip's segment count
+  // and status, and a segments or embeddings call's outputs
+  float* scores_host = nullptr;
+  float* scores_dev = nullptr;
+  int32_t* n_segments;
+  int32_t* status;
+  const nisqa_segment_out* seg = nullptr;
+  const nisqa_embedding_out* emb = nullptr;
+  // completion: synchronous, a ticket, or in stream order (the lanes wait for `ready` before they read the input or
+  // write outputs)
+  bool sync = false;
+  int64_t* ticket = nullptr;
+  cudaEvent_t ready = nullptr;
+  WinLayout* win = nullptr;           // a windows call or feed push
+  std::vector<ClipPlan> plan;         // [n_clips]
+  std::vector<long long> seg_row;     // segments / embeddings call: each clip's first output row (-1: none)
+  Call(int n, const int64_t* ns, const int32_t* sr, int fmt_, int32_t* n_seg, int32_t* st)
+      : n_clips(n), n_samples(ns), sample_rate(sr), fmt(fmt_), n_segments(n_seg), status(st) {}
+};
+
+// What one pass reads of its call: clips first_clip .. first_clip + n_clips - 1
 struct PassInput {
   int n_clips;
   const ClipPlan* plan;               // [n_clips]
@@ -1261,6 +1297,9 @@ struct PassInput {
   int stage;                          // staging slot
   const WinPass* win;                 // windows call: the pass's spans (else nullptr)
   bool pair_rows = false;             // window-pairs call: scores_dev_out is compact, [n_clips / 2][n_out]
+  const nisqa_segment_out* seg;       // segments call: its outputs (else nullptr)
+  const nisqa_embedding_out* emb;     // embeddings call: its outputs (else nullptr)
+  const long long* seg_row;           // either: the first output row of each clip (-1: none)
 };
 
 int lane_allgather(nisqa_engine* e, const float* src, float* dst, size_t count, cudaStream_t st);
@@ -1357,7 +1396,7 @@ int upload_inputs(Pass& p, const PassInput& in) {
   SG.lane = in.slot;
   // one pinned block: ClipDesc[n] | the prefix arrays
   const size_t tb_clips = (size_t)n * sizeof(ClipDesc), tb_pref = pre.size() * 4;
-  const size_t tb_rows_at = (tb_clips + tb_pref + 7) / 8 * 8, tb_rows = e->seg_out || e->emb_out ? (size_t)n * 8 : 0;
+  const size_t tb_rows_at = (tb_clips + tb_pref + 7) / 8 * 8, tb_rows = in.seg || in.emb ? (size_t)n * 8 : 0;
   const size_t tb_spans_at = tb_rows_at + tb_rows, tb_spans = in.win ? in.win->spans.size() * sizeof(WinSpan) : 0;
   const size_t tb_fwins_at = (tb_spans_at + tb_spans + 15) / 16 * 16, tb_fwins = in.win ? in.win->fwins.size() * sizeof(FeedWin) : 0;
   CK(SG.h_tables.reserve(tb_fwins_at + tb_fwins));
@@ -1365,7 +1404,7 @@ int upload_inputs(Pass& p, const PassInput& in) {
   memcpy(ht, cl.data(), tb_clips);
   memcpy(ht + tb_clips, pre.data(), tb_pref);
   if (tb_rows) {      // (a segments or embeddings call: the rows of the pass's clips)
-    memcpy(ht + tb_rows_at, e->seg_row.data() + in.first_clip, tb_rows);
+    memcpy(ht + tb_rows_at, in.seg_row, tb_rows);
     CK(SG.seg_row.reserve(tb_rows));
     CK(cudaMemcpyAsync(SG.seg_row.p, ht + tb_rows_at, tb_rows, cudaMemcpyHostToDevice, cs));
     p.seg_row = SG.seg_row.as<long long>();
@@ -1798,7 +1837,7 @@ int td_stages(Pass& p, Rows rows) {
 }
 
 // The shipped shape's fc_out 768 -> 20, BiLSTM and pooling (PoolLastStepBi fused into the BiLSTM launch)
-int lstm_head(Pass& p) {
+int lstm_head(Pass& p, const PassInput& in) {
   nisqa_engine* e = p.e;
   const nisqa_config& c = p.c;
   Lane& LN = p.LN;
@@ -1810,7 +1849,7 @@ int lstm_head(Pass& p) {
   { Scope s(e, "fc_out"); launch_fc20(p.st, LN.feats.as<float>(), w.fc.wT, w.fc.b, LN.feats20.as<float>(), n_seg); }
   const bool lastbi = c.pool == NISQA_POOL_LAST_STEP_BI;
   // the other pooling modules read every step's output, and so do segments and embeddings calls
-  const bool keep = e->keep_td_out || !lastbi || e->seg_out || e->emb_out;
+  const bool keep = e->keep_td_out || !lastbi || in.seg || in.emb;
   { Scope s(e, "lstm", 2);
     if (e->lstm_batched)
       launch_lstm_batched(p.st, LN.feats20.as<float>(), p.clips, p.by_len, p.n, w.lstm, keep ? LN.tdout.as<float>() : nullptr,
@@ -1839,10 +1878,10 @@ int lstm_head(Pass& p) {
 int segment_rows(Pass& p, const PassInput& in) {
   nisqa_engine* e = p.e;
   const int nh = p.c.n_out, W = p.w.pool_width;
-  const nisqa_segment_out* so = e->seg_out;
-  const nisqa_embedding_out* eo = e->emb_out;
+  const nisqa_segment_out* so = in.seg;
+  const nisqa_embedding_out* eo = in.emb;
   for (int i = 0; i < p.n; ++i) {
-    const long long r = e->seg_row[in.first_clip + i];
+    const long long r = in.seg_row[i];
     if (r < 0 || in.plan[i].run) continue;
     const size_t n = in.plan[i].n_seg;
     if (so) {
@@ -1883,10 +1922,10 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
   } else {
     Rows rows;
     rc = framewise(p, in.fmt, &rows, in.win);
-    if (!rc) rc = p.w.lstm_shipped ? lstm_head(p) : td_stages(p, rows);
+    if (!rc) rc = p.w.lstm_shipped ? lstm_head(p, in) : td_stages(p, rows);
     if (rc) return rc;
   }
-  if (e->seg_out || e->emb_out) {
+  if (in.seg || in.emb) {
     rc = segment_rows(p, in);
     if (rc) return rc;
   }
@@ -1980,12 +2019,13 @@ void feed_pass(const WinLayout& L, const ClipPlan* plan, const int64_t* len, int
   }
 }
 
-int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, const void* dev_pcm,
-                   const int64_t* dev_off, const int64_t* n_samples, const int32_t* sample_rate,
-                   int fmt, float* scores_host, float* scores_dev, int32_t* n_seg_out,
-                   int32_t* status_out, int sync, int64_t* ticket_out = nullptr,
-                   const IngestSources* ingest = nullptr, cudaEvent_t ready = nullptr, cudaStream_t* fin_out = nullptr,
-                   const WinLayout* win = nullptr) {
+// The lane of the next pass
+int next_lane(const nisqa_engine* e) { return e->profiling ? 0 : (int)(e->pass_counter % kLanes); }
+
+// The checks and the plan of a call, all before anything is enqueued: each clip's ClipPlan (its front-end tables built),
+// segment count and status, and for a segments or embeddings call each OK clip's first output row, in clip order
+// (NISQA_DE: the degraded clips only)
+int plan_call(nisqa_engine* e, Call& c) {
   if (!e) return NISQA_ERR_INVALID;
   if (!e->weights_loaded) return fail(e, NISQA_ERR_STATE, "nisqa_load_weights has not been called");
   if (!e->conv_tc && e->conv_net() && !e->w.shipped_channels())
@@ -1999,37 +2039,63 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
     return fail(e, NISQA_ERR_STATE, std::string("conv_tc=0: the fp32 FFMA convolutions run the AdaptCNN pools [24, 7] [12, 5] [6, 3] "
                                                 "only, this checkpoint has ") + buf + " (nisqa_set_option(\"conv_tc\", 1))");
   }
-  if (n_clips < 0 || (n_clips > 0 && (!n_samples || !sample_rate)))
+  const int n_clips = c.n_clips;
+  if (n_clips < 0 || (n_clips > 0 && (!c.n_samples || !c.sample_rate)))
     return fail(e, NISQA_ERR_INVALID, "null argument");
-  if (fmt != NISQA_FMT_S16 && fmt != NISQA_FMT_F32) return fail(e, NISQA_ERR_INVALID, "sample_fmt");
+  if (c.fmt != NISQA_FMT_S16 && c.fmt != NISQA_FMT_F32) return fail(e, NISQA_ERR_INVALID, "sample_fmt");
   CK(cudaSetDevice(e->device));
   for (auto& t : e->timers) { t.ms = 0.0; t.launches = 0; }
-  std::vector<ClipPlan> plan(n_clips);
+  std::vector<ClipPlan>& plan = c.plan;
+  plan.assign(n_clips, ClipPlan());
   for (int i = 0; i < n_clips; ++i) {
-    if (n_samples[i] > (int64_t)INT32_MAX) return fail(e, NISQA_ERR_INVALID, "clip longer than 2^31 samples");
-    plan_clip(e->cfg, n_samples[i], sample_rate[i], &plan[i]);
+    if (c.n_samples[i] > (int64_t)INT32_MAX) return fail(e, NISQA_ERR_INVALID, "clip longer than 2^31 samples");
+    plan_clip(e->cfg, c.n_samples[i], c.sample_rate[i], &plan[i]);
     if (plan[i].status == NISQA_CLIP_OK) {
-      int rc = build_fb(e, sample_rate[i], plan[i].hop, plan[i].win, &plan[i].fb_id);
+      int rc = build_fb(e, c.sample_rate[i], plan[i].hop, plan[i].win, &plan[i].fb_id);
       if (rc) return rc;
     }
     plan[i].run = plan[i].status == NISQA_CLIP_OK;
-    if (n_seg_out) n_seg_out[i] = plan[i].n_seg;
-    if (status_out) status_out[i] = plan[i].status;
+    if (c.n_segments) c.n_segments[i] = plan[i].n_seg;
+    if (c.status) c.status[i] = plan[i].status;
   }
-  const int unit = e->cfg.double_ended ? 2 : 1;      // clips travel in (degraded, reference) pairs through a double-ended engine
   if (e->cfg.double_ended) {
     if (n_clips & 1) return fail(e, NISQA_ERR_INVALID, "a double-ended engine takes clips in (degraded, reference) pairs: n_clips must be even");
     for (int i = 0; i < n_clips; i += 2)
       if (!plan[i].run || !plan[i + 1].run) plan[i].run = plan[i + 1].run = 0;      // the pair scores NaN
   }
+  if (c.seg || c.emb) {
+    c.seg_row.assign(n_clips, -1);
+    long long rows = 0;
+    for (int g = 0; g < n_clips; ++g) {
+      if (plan[g].status != NISQA_CLIP_OK || (e->cfg.double_ended && (g & 1))) continue;
+      c.seg_row[g] = rows;
+      rows += plan[g].n_seg;
+    }
+    if (c.seg && c.seg->n_rows < rows)
+      return fail(e, NISQA_ERR_INVALID, "seg->n_rows = " + std::to_string(c.seg->n_rows) + ": the call has " +
+                                            std::to_string(rows) + " segment rows");
+    if (c.emb && c.emb->rows && c.emb->n_rows < rows)
+      return fail(e, NISQA_ERR_INVALID, "emb->n_rows = " + std::to_string(c.emb->n_rows) + ": the call has " +
+                                            std::to_string(rows) + " segment rows");
+  }
+  return 0;
+}
+
+// The passes of a planned call - runs of whole clips (NISQA_DE: pairs) over the lanes and staging slots in turn - and
+// its completion.  *fin_out: the stream the call ends on, the last pass's lane once it has waited for the call's other
+// lanes (no pass: the lane the first pass would have run on).
+int run_call(nisqa_engine* e, const Call& c, cudaStream_t* fin_out) {
+  const int n_clips = c.n_clips;
+  const std::vector<ClipPlan>& plan = c.plan;
+  const int unit = e->cfg.double_ended ? 2 : 1;      // clips travel in (degraded, reference) pairs through a double-ended engine
   // segments per internal pass: 131072 segments keep ~8 GB of activation planes per compute lane (three lanes stay
   // well inside the 80 GB of an H100) and give the BiLSTM >= 128 clips per launch at configs[3]; one 64-clip batch is 15 808
   // (scaled down for self-attention stacks wider than 64: their activation rows grow with d_model)
   const int d_max = std::max(e->sa_d(), e->cfg.td2_layers > 0 ? e->td2_d() : 64);
   const int max_seg = e->cfg.max_chunk_segments > 0 ? e->cfg.max_chunk_segments : 131072 / (d_max / 64);
-  float* scores_all = scores_dev;
+  float* scores_all = c.scores_dev;
   if (!scores_all) {
-    DevBuf& sb = ticket_out ? e->tickets[e->next_ticket % kStages].scores : e->scores;
+    DevBuf& sb = c.ticket ? e->tickets[e->next_ticket % kStages].scores : e->scores;
     CK(sb.reserve((size_t)std::max(n_clips, 1) * e->cfg.n_out * 4));
     scores_all = sb.as<float>();
   }
@@ -2046,21 +2112,23 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
       segs += s; i1 += unit;
     }
     PassInput in;
-    in.n_clips = i1 - i0; in.plan = plan.data() + i0; in.n_samples = n_samples + i0;
-    in.host_pcm = host_pcm ? host_pcm + i0 : nullptr;
-    in.dev_pcm = dev_pcm; in.dev_off = dev_off ? dev_off + i0 : nullptr;
-    in.ingest = ingest; in.first_clip = i0;
-    in.ready = ready;
-    in.fmt = fmt;
-    in.pair_rows = win && win->n_src == 2;
+    in.n_clips = i1 - i0; in.plan = plan.data() + i0; in.n_samples = c.n_samples + i0;
+    in.host_pcm = c.host_pcm ? c.host_pcm + i0 : nullptr;
+    in.dev_pcm = c.dev_pcm; in.dev_off = c.dev_off ? c.dev_off + i0 : nullptr;
+    in.ingest = c.ingest; in.first_clip = i0;
+    in.ready = c.ready;
+    in.fmt = c.fmt;
+    in.pair_rows = c.win && c.win->n_src == 2;
     in.scores_dev_out = scores_all + (size_t)(in.pair_rows ? i0 / 2 : i0) * e->cfg.n_out;
+    in.seg = c.seg; in.emb = c.emb;
+    in.seg_row = c.seg_row.empty() ? nullptr : c.seg_row.data() + i0;
     in.win = nullptr;
-    if (win) {
-      if (win->feed) feed_pass(*win, plan.data(), n_samples, i0, i1, &wp);
-      else win_pass(e->cfg, *win, plan.data(), n_samples, i0, i1, &wp);
+    if (c.win) {
+      if (c.win->feed) feed_pass(*c.win, plan.data(), c.n_samples, i0, i1, &wp);
+      else win_pass(e->cfg, *c.win, plan.data(), c.n_samples, i0, i1, &wp);
       in.win = &wp;
     }
-    in.slot = e->profiling ? 0 : (int)(e->pass_counter % kLanes);
+    in.slot = next_lane(e);
     in.stage = (int)(e->pass_counter % kStages);
     ++e->pass_counter;
     int rc = run_pass(e, in);
@@ -2070,41 +2138,46 @@ int predict_common(nisqa_engine* e, int n_clips, const void* const* host_pcm, co
   }
   // the lane of the last pass collects: it waits for the other lanes this call used
   const int n_pass = (int)(e->pass_counter - first_pass);
-  cudaStream_t fin = e->lanes[e->last_lane].stream;
-  if (n_pass == 0) fin = e->lanes[0].stream;
+  const cudaStream_t fin = e->lanes[n_pass ? e->last_lane : next_lane(e)].stream;
   for (int k = 0; k < kStages && n_pass > 1; ++k)      // passes of this call that ran on other lanes
     if (e->stages[k].busy && e->stages[k].lane != e->last_lane) CK(cudaStreamWaitEvent(fin, e->stages[k].ev_done, 0));
-  if (e->gather_dst && e->nccl_comm && n_clips == e->gather_rows && (ticket_out || scores_dev) && !win) {
+  if (e->gather_dst && e->nccl_comm && n_clips == e->gather_rows && (c.ticket || c.scores_dev) && !c.win) {
     // the path's single exchange step, enqueued behind this call's kernels on its own lane
     int rc = lane_allgather(e, scores_all, e->gather_dst, (size_t)n_clips * e->cfg.n_out, fin);
     if (rc) return rc;
     CK(cudaEventRecord(e->stages[e->last_stage].ev_done, fin));
   }
   if (fin_out) *fin_out = fin;
-  if (ticket_out) {
+  if (c.ticket) {
     // asynchronous completion: scores land in the ticket's pinned block; nisqa_wait hands them over
     Ticket& tk = e->tickets[e->next_ticket % kStages];
     tk.bytes = (size_t)n_clips * e->cfg.n_out * 4;
-    tk.user_scores = scores_host;
+    tk.user_scores = c.scores_host;
     CK(tk.pinned.reserve(std::max<size_t>(tk.bytes, 16)));
     if (tk.bytes) CK(cudaMemcpyAsync(tk.pinned.p, scores_all, tk.bytes, cudaMemcpyDeviceToHost, fin));
     if (!tk.done) CK(cudaEventCreateWithFlags(&tk.done, cudaEventDisableTiming));
     CK(cudaEventRecord(tk.done, fin));
     tk.active = true;
     tk.id = e->next_ticket++;
-    *ticket_out = tk.id;
+    *c.ticket = tk.id;
     return 0;
   }
-  if (scores_host && n_clips > 0) {
+  if (c.scores_host && n_clips > 0) {
     const size_t bytes = (size_t)n_clips * e->cfg.n_out * 4;
     CK(e->h_scores.reserve(bytes));
     CK(cudaMemcpyAsync(e->h_scores.p, scores_all, bytes, cudaMemcpyDeviceToHost, fin));
     CK(cudaStreamSynchronize(fin));
-    memcpy(scores_host, e->h_scores.p, bytes);
+    memcpy(c.scores_host, e->h_scores.p, bytes);
   }
-  if (sync || scores_host || e->profiling) CK(cudaStreamSynchronize(fin));
+  if (c.sync || c.scores_host || e->profiling) CK(cudaStreamSynchronize(fin));
   if (e->profiling) collect_timers(e);
   return 0;
+}
+
+// A call of the host entry points: planned, then run
+int score(nisqa_engine* e, Call& c) {
+  const int rc = plan_call(e, c);
+  return rc ? rc : run_call(e, c, nullptr);
 }
 
 int finish_ticket(nisqa_engine* e, Ticket& tk) {
@@ -2259,8 +2332,9 @@ int nisqa_predict_pcm(nisqa_engine* e, int n_clips, const void* const* pcm, cons
   if (!e) return NISQA_ERR_INVALID;
   if (n_clips > 0 && (!pcm || !scores_out)) return fail(e, NISQA_ERR_INVALID, "null argument");
   for (auto& tk : e->tickets) { int rc = finish_ticket(e, tk); if (rc) return rc; }
-  return predict_common(e, n_clips, pcm, nullptr, nullptr, n_samples, sample_rate, sample_fmt,
-                        scores_out, nullptr, n_segments_out, status_out, 1);
+  Call c(n_clips, n_samples, sample_rate, sample_fmt, n_segments_out, status_out);
+  c.host_pcm = pcm; c.scores_host = scores_out; c.sync = true;
+  return score(e, c);
 }
 
 int nisqa_submit_pcm(nisqa_engine* e, int n_clips, const void* const* pcm, const int64_t* n_samples,
@@ -2271,8 +2345,9 @@ int nisqa_submit_pcm(nisqa_engine* e, int n_clips, const void* const* pcm, const
   if (e->profiling) return fail(e, NISQA_ERR_STATE, "profiling needs the synchronous entry points");
   int rc = finish_ticket(e, e->tickets[e->next_ticket % kStages]);      // at most kStages submissions in flight
   if (rc) return rc;
-  return predict_common(e, n_clips, pcm, nullptr, nullptr, n_samples, sample_rate, sample_fmt,
-                        scores_out, nullptr, n_segments_out, status_out, 0, ticket);
+  Call c(n_clips, n_samples, sample_rate, sample_fmt, n_segments_out, status_out);
+  c.host_pcm = pcm; c.scores_host = scores_out; c.ticket = ticket;
+  return score(e, c);
 }
 
 int nisqa_wait(nisqa_engine* e, int64_t ticket) {
@@ -2303,8 +2378,9 @@ int nisqa_predict_pcm_device(nisqa_engine* e, int n_clips, const void* pcm_dev, 
                              float* scores_dev, int32_t* n_segments_out, int32_t* status_out, int sync) {
   if (!e) return NISQA_ERR_INVALID;
   if (n_clips > 0 && (!pcm_dev || !pcm_offsets || !scores_dev)) return fail(e, NISQA_ERR_INVALID, "null argument");
-  return predict_common(e, n_clips, nullptr, pcm_dev, pcm_offsets, n_samples, sample_rate, sample_fmt,
-                        nullptr, scores_dev, n_segments_out, status_out, sync);
+  Call c(n_clips, n_samples, sample_rate, sample_fmt, n_segments_out, status_out);
+  c.dev_pcm = pcm_dev; c.dev_off = pcm_offsets; c.scores_dev = scores_dev; c.sync = sync != 0;
+  return score(e, c);
 }
 
 
@@ -2403,63 +2479,94 @@ int nisqa_predict_pcm_resampled(nisqa_engine* e, int n_clips, const void* const*
   if (rc) return rc;
   std::vector<int32_t> srs(n_clips, target_sr);
   // the converted clips are ordinary float32 PCM resident in HBM: the device entry of the predict path takes over
-  return predict_common(e, n_clips, nullptr, S->out.p, offs.data(), n_fix.data(), srs.data(), NISQA_FMT_F32,
-                        scores_out, nullptr, n_segments_out, status_out, 1);
+  Call c(n_clips, n_fix.data(), srs.data(), NISQA_FMT_F32, n_segments_out, status_out);
+  c.dev_pcm = S->out.p; c.dev_off = offs.data(); c.scores_host = scores_out; c.sync = true;
+  return score(e, c);
 }
 
-// The device work of nisqa_predict_device_batch once its arguments are checked: the lanes wait for the caller's stream,
-// the clips are packed (and converted to target_sr), the passes run, and the caller's stream waits for the last pass.
-// *slot_out: the conversion slot the call uses (ms_sr), also when it fails.
-static int enqueue_device_batch(nisqa_engine* e, cudaStream_t caller, int n_clips, const IngestSources& ing,
-                                const int64_t* ns, const int32_t* sr, int fmt, int32_t target_sr, float* scores_dev,
-                                int32_t* n_segments_out, int32_t* status_out, RsSlot** slot_out) {
-  CK(cudaEventRecord(e->ev_in, caller));
-  cudaStream_t fin = nullptr;
-  if (target_sr > 0) {
-    // convert on the lane of the call's first pass; every pass waits for the slot's `ready`
-    cudaStream_t st = e->lanes[e->profiling ? 0 : (int)(e->pass_counter % kLanes)].stream;
-    CK(cudaStreamWaitEvent(st, e->ev_in, 0));
-    std::vector<int64_t> offs, n_fix;
-    int rc = resample_to_device(e, st, n_clips, nullptr, &ing, ns, sr, fmt, target_sr, &offs, &n_fix, slot_out);
+// The stream contract of the device calls (device batch, windows, feed pushes), for a planned call: ev_in is recorded on
+// the caller's stream.  A call that prepares its input first does so on the lane of its first pass, behind ev_in - an
+// ms_sr call converts the whole recordings of the caller's batch (a span converted alone differs at its edges), a feed
+// push (f) runs feed_ingest, which appends its samples to the rings - and its passes wait for that; the others' passes
+// wait for ev_in.  The caller's stream continues behind the last pass's lane, which has joined the call's other lanes
+// (ev_out); the conversion slot and the feed stay in use until then.  On a failure, whatever was enqueued may still read
+// the caller's input, the slot or the rings: the caller's stream waits for every lane, and the slot and the feed stay in
+// use until then (best effort: the error is already reported).
+static int enqueue_call(nisqa_engine* e, void* cuda_stream, Call& c, nisqa_feed* f = nullptr,
+                        const std::function<int(cudaStream_t)>& feed_ingest = nullptr) {
+  cudaStream_t caller = static_cast<cudaStream_t>(cuda_stream);
+  RsSlot* S = nullptr;
+  std::vector<int64_t> offs, n_fix;
+  const int err = [&]() -> int {
+    CK(cudaEventRecord(e->ev_in, caller));
+    c.ready = e->ev_in;
+    if (c.target_sr > 0 || f) {
+      cudaStream_t st = e->lanes[next_lane(e)].stream;
+      CK(cudaStreamWaitEvent(st, e->ev_in, 0));
+      const int rc = f ? feed_ingest(st) : resample_to_device(e, st, c.n_rec, nullptr, c.ingest, c.rec_n, c.rec_sr, c.fmt,
+                                                              c.target_sr, &offs, &n_fix, &S);
+      if (rc) return rc;
+      if (S) {
+        CK(cudaEventRecord(S->ready, st));
+        c.dev_pcm = S->out.p; c.ingest = nullptr; c.fmt = NISQA_FMT_F32; c.ready = S->ready;
+        if (c.win) c.win->rec_off = offs.data();
+        else c.dev_off = offs.data();
+      }
+    }
+    cudaStream_t fin = nullptr;
+    const int rc = run_call(e, c, &fin);
     if (rc) return rc;
-    RsSlot& S = **slot_out;
-    CK(cudaEventRecord(S.ready, st));
-    std::vector<int32_t> srs(n_clips, target_sr);
-    rc = predict_common(e, n_clips, nullptr, S.out.p, offs.data(), n_fix.data(), srs.data(), NISQA_FMT_F32, nullptr,
-                        scores_dev, n_segments_out, status_out, 0, nullptr, nullptr, S.ready, &fin);
-    if (rc) return rc;
-    CK(cudaEventRecord(S.done, fin));
-    S.busy = n_clips > 0;
-  } else {
-    int rc = predict_common(e, n_clips, nullptr, nullptr, nullptr, ns, sr, fmt, nullptr, scores_dev, n_segments_out,
-                            status_out, 0, nullptr, &ing, e->ev_in, &fin);
-    if (rc) return rc;
+    if (S) {
+      CK(cudaEventRecord(S->done, fin));
+      S->busy = c.n_clips > 0;
+    }
+    if (f) {
+      CK(cudaEventRecord(f->done, fin));
+      f->pending = true;
+    }
+    CK(cudaEventRecord(e->ev_out, fin));
+    CK(cudaStreamWaitEvent(caller, e->ev_out, 0));
+    return 0;
+  }();
+  if (err) {
+    for (auto& l : e->lanes)
+      if (cudaEventRecord(e->ev_out, l.stream) == cudaSuccess) cudaStreamWaitEvent(caller, e->ev_out, 0);
+    if (S && cudaEventRecord(S->done, caller) == cudaSuccess) S->busy = true;
+    if (f && cudaEventRecord(f->done, caller) == cudaSuccess) f->pending = true;
   }
-  // the last pass's lane has joined the call's other lanes: the caller's stream continues behind all of them
-  CK(cudaEventRecord(e->ev_out, fin));
-  CK(cudaStreamWaitEvent(caller, e->ev_out, 0));
-  return 0;
+  return err;
 }
 
-// The checks of one nisqa_device_batch argument (nm: its name in messages; ch: the channel it is read with; n_clips: the
-// clip count it must have; min_n: the fewest samples a clip may have, 0 for a feed push) -> its ingest source and whether
-// it is mixed to mono
-static int check_device_batch(nisqa_engine* e, const nisqa_device_batch& b, const std::string& nm, int ch, int n_clips,
-                              IngestSrc* src, bool* mix, int min_n = 1) {
-  if (b.sample_fmt != NISQA_FMT_S16 && b.sample_fmt != NISQA_FMT_F32) return fail(e, NISQA_ERR_INVALID, nm + "sample_fmt");
-  if (b.n_clips < 0 || b.n_clips != n_clips) return fail(e, NISQA_ERR_INVALID, nm + "n_clips");
-  if (b.n_channels < 1) return fail(e, NISQA_ERR_INVALID, nm + "n_channels");
-  if (b.n_channels > 1 && (ch < -1 || ch >= b.n_channels)) return fail(e, NISQA_ERR_INVALID, nm + "channel out of range");
-  if (b.length < 1 || b.clip_stride < 0 || b.channel_stride < 0) return fail(e, NISQA_ERR_INVALID, nm + "length / strides");
-  if (b.sample_rate <= 0) return fail(e, NISQA_ERR_INVALID, nm + "sample_rate");
-  if (b.n_clips > 0 && (!b.data || !b.n_samples)) return fail(e, NISQA_ERR_INVALID, nm + "data / n_samples: null argument");
-  for (int i = 0; i < b.n_clips; ++i)
-    if (b.n_samples[i] < min_n || b.n_samples[i] > b.length)
-      return fail(e, NISQA_ERR_INVALID, nm + "n_samples[" + std::to_string(i) + "] = " + std::to_string(b.n_samples[i]) +
-                                            ": not within " + std::to_string(min_n) + " .. length (" +
-                                            std::to_string(b.length) + ")");
-  *mix = b.n_channels > 1 && ch < 0;
-  *src = {b.data, b.clip_stride, b.channel_stride, b.n_channels, ch, b.sample_fmt == NISQA_FMT_F32 ? 1 : 0};
+// The sources of a device call: deg, read with its channel (or mixed to mono), and ref when given, always the mono mix.
+// Each must be a batch of n_clips clips of min_n .. length samples (0 for a feed push); messages name deg by deg_nm and
+// ref by "ref.".  -> their ingest sources and the call's format: float32 if either is float32 or mixed, else int16.
+static int check_sources(nisqa_engine* e, const std::string& deg_nm, const nisqa_device_batch& deg, const nisqa_device_batch* ref,
+                         int n_clips, int min_n, IngestSources* ing, int* fmt) {
+  const nisqa_device_batch* src[2] = {&deg, ref};
+  *ing = {};
+  ing->n_src = ref ? 2 : 1;
+  bool f32 = false;
+  for (int k = 0; k < ing->n_src; ++k) {
+    const nisqa_device_batch& b = *src[k];
+    const std::string nm = k ? "ref." : deg_nm;
+    const int ch = k ? -1 : b.channel;
+    if (b.sample_fmt != NISQA_FMT_S16 && b.sample_fmt != NISQA_FMT_F32) return fail(e, NISQA_ERR_INVALID, nm + "sample_fmt");
+    if (b.n_clips < 0 || b.n_clips != n_clips) return fail(e, NISQA_ERR_INVALID, nm + "n_clips");
+    if (b.n_channels < 1) return fail(e, NISQA_ERR_INVALID, nm + "n_channels");
+    if (b.n_channels > 1 && (ch < -1 || ch >= b.n_channels)) return fail(e, NISQA_ERR_INVALID, nm + "channel out of range");
+    if (b.length < 1 || b.clip_stride < 0 || b.channel_stride < 0) return fail(e, NISQA_ERR_INVALID, nm + "length / strides");
+    if (b.sample_rate <= 0) return fail(e, NISQA_ERR_INVALID, nm + "sample_rate");
+    if (b.n_clips > 0 && (!b.data || !b.n_samples)) return fail(e, NISQA_ERR_INVALID, nm + "data / n_samples: null argument");
+    for (int i = 0; i < b.n_clips; ++i)
+      if (b.n_samples[i] < min_n || b.n_samples[i] > b.length)
+        return fail(e, NISQA_ERR_INVALID, nm + "n_samples[" + std::to_string(i) + "] = " + std::to_string(b.n_samples[i]) +
+                                              ": not within " + std::to_string(min_n) + " .. length (" +
+                                              std::to_string(b.length) + ")");
+    const bool mix = b.n_channels > 1 && ch < 0;
+    ing->s[k] = {b.data, b.clip_stride, b.channel_stride, b.n_channels, ch, b.sample_fmt == NISQA_FMT_F32 ? 1 : 0};
+    f32 = f32 || b.sample_fmt == NISQA_FMT_F32 || mix;
+  }
+  *fmt = f32 ? NISQA_FMT_F32 : NISQA_FMT_S16;
   return 0;
 }
 
@@ -2474,65 +2581,28 @@ static int device_batch_call(nisqa_engine* e, void* cuda_stream, const nisqa_dev
   if (e->cfg.double_ended && !ref) return fail(e, NISQA_ERR_INVALID, "ref: a double-ended engine needs the reference batch");
   if (!e->cfg.double_ended && ref) return fail(e, NISQA_ERR_INVALID, "ref: only a double-ended engine takes a reference batch");
   if (target_sr < 0) return fail(e, NISQA_ERR_INVALID, "target_sr");
-  const nisqa_device_batch* src[2] = {deg, ref};
-  const int n_src = ref ? 2 : 1;
-  IngestSources ing = {};
-  ing.n_src = n_src;
-  bool out_f32 = false;
-  for (int k = 0; k < n_src; ++k) {
-    const nisqa_device_batch& b = *src[k];
-    const std::string nm = k ? "ref." : "deg.";
-    const int ch = k ? -1 : b.channel;        // the reference of a pair is always the mono mix
-    bool mix = false;
-    const int rc = check_device_batch(e, b, nm, ch, deg->n_clips, &ing.s[k], &mix);
-    if (rc) return rc;
-    out_f32 = out_f32 || b.sample_fmt == NISQA_FMT_F32 || mix;
-  }
+  IngestSources ing;
+  int fmt;
+  int rc = check_sources(e, "deg.", *deg, ref, deg->n_clips, 1, &ing, &fmt);
+  if (rc) return rc;
+  const int n_src = ing.n_src;
   const int n_clips = deg->n_clips * n_src;
   if (n_clips > 0 && !scores_dev) return fail(e, NISQA_ERR_INVALID, "scores_dev: null argument");
-  // the engine's clip order: clip g is clip g / n_src of source g % n_src (NISQA_DE: degraded, reference pairs)
-  std::vector<int64_t> ns(n_clips);
-  std::vector<int32_t> sr(n_clips);
-  for (int g = 0; g < n_clips; ++g) { ns[g] = src[g % n_src]->n_samples[g / n_src]; sr[g] = src[g % n_src]->sample_rate; }
-  const int fmt = out_f32 ? NISQA_FMT_F32 : NISQA_FMT_S16;
   if (seg && n_clips > 0 && (!seg->scores || !seg->weights)) return fail(e, NISQA_ERR_INVALID, "seg: null scores / weights");
-  if (emb && !e->weights_loaded) return fail(e, NISQA_ERR_STATE, "nisqa_load_weights has not been called");
-  if (seg || emb) {
-    // each OK clip's rows, in clip order (NISQA_DE: the degraded clips only), from the host arithmetic the passes repeat
-    e->seg_row.assign(n_clips, -1);
-    long long rows = 0;
-    for (int g = 0; g < n_clips; ++g) {
-      const int64_t n = target_sr > 0 ? nisqa_resample_out_len(ns[g], sr[g], target_sr) : ns[g];
-      ClipPlan pl;
-      plan_clip(e->cfg, n, target_sr > 0 ? target_sr : sr[g], &pl);
-      if (pl.status != NISQA_CLIP_OK || (e->cfg.double_ended && (g & 1))) continue;
-      e->seg_row[g] = rows;
-      rows += pl.n_seg;
-    }
-    if (seg && seg->n_rows < rows)
-      return fail(e, NISQA_ERR_INVALID, "seg->n_rows = " + std::to_string(seg->n_rows) + ": the call has " +
-                                            std::to_string(rows) + " segment rows");
-    if (emb && emb->rows && emb->n_rows < rows)
-      return fail(e, NISQA_ERR_INVALID, "emb->n_rows = " + std::to_string(emb->n_rows) + ": the call has " +
-                                            std::to_string(rows) + " segment rows");
+  // the engine's clip order: clip g is clip g / n_src of source g % n_src (NISQA_DE: degraded, reference pairs), at its
+  // own rate and, with ms_sr, at target_sr
+  const nisqa_device_batch* src[2] = {deg, ref};
+  std::vector<int64_t> ns(n_clips), n_model(n_clips);
+  std::vector<int32_t> sr(n_clips), sr_model(n_clips, target_sr);
+  for (int g = 0; g < n_clips; ++g) {
+    ns[g] = src[g % n_src]->n_samples[g / n_src]; sr[g] = src[g % n_src]->sample_rate;
+    n_model[g] = target_sr > 0 ? nisqa_resample_out_len(ns[g], sr[g], target_sr) : ns[g];
   }
-  CK(cudaSetDevice(e->device));
-  cudaStream_t caller = static_cast<cudaStream_t>(cuda_stream);
-  RsSlot* S = nullptr;
-  e->seg_out = seg;
-  e->emb_out = emb;
-  const int rc = enqueue_device_batch(e, caller, n_clips, ing, ns.data(), sr.data(), fmt, target_sr, scores_dev,
-                                      n_segments_out, status_out, &S);
-  e->seg_out = nullptr;
-  e->emb_out = nullptr;
-  if (rc) {
-    // whatever was enqueued before the failure may still read the caller's input or the conversion slot: the caller's
-    // stream waits for every lane, and the slot stays in use until then (best effort: the error is already reported)
-    for (auto& l : e->lanes)
-      if (cudaEventRecord(e->ev_out, l.stream) == cudaSuccess) cudaStreamWaitEvent(caller, e->ev_out, 0);
-    if (S && cudaEventRecord(S->done, caller) == cudaSuccess) S->busy = true;
-  }
-  return rc;
+  Call c(n_clips, n_model.data(), target_sr > 0 ? sr_model.data() : sr.data(), fmt, n_segments_out, status_out);
+  c.ingest = &ing; c.scores_dev = scores_dev; c.seg = seg; c.emb = emb;
+  c.target_sr = target_sr; c.n_rec = n_clips; c.rec_n = ns.data(); c.rec_sr = sr.data();
+  rc = plan_call(e, c);
+  return rc ? rc : enqueue_call(e, cuda_stream, c);
 }
 
 int nisqa_predict_device_batch(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
@@ -2563,49 +2633,103 @@ int nisqa_predict_device_batch_embeddings(nisqa_engine* e, void* cuda_stream, co
   return device_batch_call(e, cuda_stream, deg, ref, target_sr, scores_dev, nullptr, emb, n_segments_out, status_out);
 }
 
-// The device work of a windows or window-pairs call once its arguments are checked and its windows laid out (L: N clips
-// of lengths len at `rate`; rs_n / rs_sr: the n_rs recordings of the caller's batch in IngestSources order, which an
-// ms_sr checkpoint converts whole first, as a span converted alone differs at its edges), with the stream contract of
-// nisqa_predict_device_batch
-static int enqueue_windows(nisqa_engine* e, void* cuda_stream, const IngestSources& ing, int fmt, int32_t target_sr,
-                           int rate, int N, const int64_t* len, WinLayout* L, int n_rs, const int64_t* rs_n,
-                           const int32_t* rs_sr, float* scores_dev, int32_t* n_segments_out, int32_t* status_out) {
-  CK(cudaSetDevice(e->device));
-  cudaStream_t caller = static_cast<cudaStream_t>(cuda_stream);
-  std::vector<int32_t> srs(N, rate);
-  RsSlot* S = nullptr;
-  cudaStream_t fin = nullptr;
-  int rc = 0;
-  CK(cudaEventRecord(e->ev_in, caller));
-  if (target_sr > 0) {
-    // the whole recordings converted first; every pass waits for `ready`
-    cudaStream_t st = e->lanes[e->profiling ? 0 : (int)(e->pass_counter % kLanes)].stream;
-    CK(cudaStreamWaitEvent(st, e->ev_in, 0));
-    std::vector<int64_t> offs, n_fix;
-    rc = resample_to_device(e, st, n_rs, nullptr, &ing, rs_n, rs_sr, fmt, target_sr, &offs, &n_fix, &S);
-    if (!rc) {
-      L->rec_off = offs.data();
-      CK(cudaEventRecord(S->ready, st));
-      rc = predict_common(e, N, nullptr, S->out.p, nullptr, len, srs.data(), NISQA_FMT_F32, nullptr, scores_dev,
-                          n_segments_out, status_out, 0, nullptr, nullptr, S->ready, &fin, L);
-    }
-    if (!rc) {
-      CK(cudaEventRecord(S->done, fin));
-      S->busy = N > 0;
-    }
-  } else {
-    rc = predict_common(e, N, nullptr, nullptr, nullptr, len, srs.data(), fmt, nullptr, scores_dev, n_segments_out,
-                        status_out, 0, nullptr, &ing, e->ev_in, &fin, L);
+// The window list of a windows call or feed push, in recording order
+struct WinList {
+  std::vector<int> rec;
+  std::vector<int64_t> start, len;
+};
+// Window k of recording b (T samples at the model rate) appended to the list, followed, when the call has a reference
+// (n_src 2: T_ref samples, margin M), by its reference window
+void add_window(WinList* w, int n_src, int b, int64_t k, int64_t T, int64_t T_ref, int64_t W, int64_t H, int64_t M) {
+  w->rec.push_back(b); w->start.push_back(k * H); w->len.push_back(std::min(W, T - k * H));
+  if (n_src == 2) {
+    int64_t r0, rn;
+    ref_window(k, T_ref, W, H, M, &r0, &rn);
+    w->rec.push_back(b); w->start.push_back(r0); w->len.push_back(rn);
   }
-  if (!rc) {
-    CK(cudaEventRecord(e->ev_out, fin));
-    CK(cudaStreamWaitEvent(caller, e->ev_out, 0));
-    return 0;
+}
+// The per-clip segment counts and statuses of a window list as per-row outputs (each may be nullptr): row r is clip r,
+// or with a reference (n_src 2) clips 2r (the degraded window) and 2r + 1 (the reference window)
+void split_rows(int n_src, int64_t rows, const int32_t* nseg, const int32_t* status, int32_t* n_seg_out, int32_t* status_out,
+                int32_t* ref_n_seg_out, int32_t* ref_status_out) {
+  for (int64_t r = 0; r < rows; ++r) {
+    if (n_seg_out) n_seg_out[r] = nseg[n_src * r];
+    if (status_out) status_out[r] = status[n_src * r];
+    if (n_src == 2 && ref_n_seg_out) ref_n_seg_out[r] = nseg[2 * r + 1];
+    if (n_src == 2 && ref_status_out) ref_status_out[r] = status[2 * r + 1];
   }
-  // (as device_batch_call: whatever was enqueued may still read the input or the conversion slot)
-  for (auto& l : e->lanes)
-    if (cudaEventRecord(e->ev_out, l.stream) == cudaSuccess) cudaStreamWaitEvent(caller, e->ev_out, 0);
-  if (S && cudaEventRecord(S->done, caller) == cudaSuccess) S->busy = true;
+}
+// The rows of a window list planned at `rate` (host arithmetic: the counts a call reports)
+void plan_rows(const nisqa_config& c, int rate, int n_src, const WinList& w, int32_t* n_seg_out, int32_t* status_out,
+               int32_t* ref_n_seg_out, int32_t* ref_status_out) {
+  const size_t n = w.len.size();
+  std::vector<int32_t> nseg(n), status(n);
+  for (size_t i = 0; i < n; ++i) {
+    ClipPlan p;
+    plan_clip(c, w.len[i], rate, &p);
+    nseg[i] = p.n_seg; status[i] = p.status;
+  }
+  split_rows(n_src, n / n_src, nseg.data(), status.data(), n_seg_out, status_out, ref_n_seg_out, ref_status_out);
+}
+
+// nisqa_predict_device_windows (ref == nullptr, margin_frames 0; the recordings deg named `nm` "rec") and
+// nisqa_predict_device_window_pairs (nm "deg")
+static int windows_call(nisqa_engine* e, void* cuda_stream, const char* nm, const nisqa_device_batch* deg,
+                        const nisqa_device_batch* ref, int32_t target_sr, int64_t window, int32_t hop_frames,
+                        int32_t margin_frames, float* scores_dev, int64_t n_rows, int32_t* n_segments_out,
+                        int32_t* status_out, int32_t* ref_n_segments_out, int32_t* ref_status_out) {
+  if (target_sr < 0) return fail(e, NISQA_ERR_INVALID, "target_sr");
+  IngestSources ing;
+  int fmt;
+  int rc = check_sources(e, std::string(nm) + ".", *deg, ref, deg->n_clips, 1, &ing, &fmt);
+  if (rc) return rc;
+  const int S = ing.n_src;
+  if (ref && target_sr == 0 && ref->sample_rate != deg->sample_rate)
+    return fail(e, NISQA_ERR_INVALID, "ref.sample_rate = " + std::to_string(ref->sample_rate) + ": the windows of both recordings "
+                                      "run at one rate, deg.sample_rate = " + std::to_string(deg->sample_rate));
+  const int rate = target_sr > 0 ? target_sr : deg->sample_rate;
+  std::string why;
+  int H = 0;
+  int64_t M = 0;
+  if (!window_pair_geometry(e->cfg, rate, window, hop_frames, margin_frames, &H, &M, &why))
+    return fail(e, NISQA_ERR_INVALID, why);
+  const int W = (int)window;
+  // the windows (pairs) of every recording, in recording order (host arithmetic: nisqa_window_counts,
+  // nisqa_window_pair_counts), and the recordings in IngestSources order for an ms_sr conversion
+  const int n_rec = deg->n_clips;
+  WinList wl;
+  std::vector<int64_t> rs_n(S * (size_t)n_rec);
+  std::vector<int32_t> rs_sr(S * (size_t)n_rec);
+  for (int b = 0; b < n_rec; ++b) {
+    int64_t T[2] = {0, 0};
+    for (int k = 0; k < S; ++k) {
+      const nisqa_device_batch* x = k ? ref : deg;
+      rs_n[S * b + k] = x->n_samples[b]; rs_sr[S * b + k] = x->sample_rate;
+      T[k] = target_sr > 0 ? nisqa_resample_out_len(x->n_samples[b], x->sample_rate, target_sr) : x->n_samples[b];
+      if (T[k] > (int64_t)INT32_MAX)
+        return fail(e, NISQA_ERR_INVALID, std::string(k ? "ref" : nm) + ".n_samples[" + std::to_string(b) + "]: " +
+                                              std::to_string(T[k]) + " samples at the model rate, more than 2^31 - 1");
+    }
+    const int64_t K = window_count(T[0], W, H);
+    if ((int64_t)wl.rec.size() + S * K > INT32_MAX)
+      return fail(e, NISQA_ERR_INVALID, S == 2 ? "deg: more than 2^30 - 1 window pairs" : "rec: more than 2^31 - 1 windows");
+    for (int64_t k = 0; k < K; ++k) add_window(&wl, S, b, k, T[0], T[1], W, H, M);
+  }
+  const int N = (int)wl.rec.size(), rows = N / S;
+  if (n_rows < rows)
+    return fail(e, NISQA_ERR_INVALID, "n_rows = " + std::to_string(n_rows) + ": the call has " + std::to_string(rows) +
+                                          (S == 2 ? " window pairs" : " windows"));
+  if (N > 0 && !scores_dev) return fail(e, NISQA_ERR_INVALID, "scores_dev: null argument");
+  const int hop = (int)((double)rate * e->cfg.hop_s);
+  WinLayout L = {wl.rec.data(), wl.start.data(), nullptr, H, H / hop, W};
+  L.n_src = S;
+  std::vector<int32_t> srs(N, rate), nseg(N), status(N);
+  Call c(N, wl.len.data(), srs.data(), fmt, nseg.data(), status.data());
+  c.ingest = &ing; c.scores_dev = scores_dev; c.win = &L;
+  c.target_sr = target_sr; c.n_rec = S * n_rec; c.rec_n = rs_n.data(); c.rec_sr = rs_sr.data();
+  rc = plan_call(e, c);
+  if (!rc) rc = enqueue_call(e, cuda_stream, c);
+  split_rows(S, rows, nseg.data(), status.data(), n_segments_out, status_out, ref_n_segments_out, ref_status_out);
   return rc;
 }
 
@@ -2617,44 +2741,8 @@ int nisqa_predict_device_windows(nisqa_engine* e, void* cuda_stream, const nisqa
   if (e->cfg.double_ended)
     return fail(e, NISQA_ERR_INVALID, "a double-ended (NISQA_DE) engine scores (degraded, reference) pairs, not windows of a recording");
   if (!rec) return fail(e, NISQA_ERR_INVALID, "rec: null argument");
-  if (target_sr < 0) return fail(e, NISQA_ERR_INVALID, "target_sr");
-  IngestSources ing = {};
-  ing.n_src = 1;
-  bool mix = false;
-  int rc = check_device_batch(e, *rec, "rec.", rec->channel, rec->n_clips, &ing.s[0], &mix);
-  if (rc) return rc;
-  const int fmt = rec->sample_fmt == NISQA_FMT_F32 || mix ? NISQA_FMT_F32 : NISQA_FMT_S16;
-  const int rate = target_sr > 0 ? target_sr : rec->sample_rate;
-  std::string why;
-  int H = 0;
-  if (!window_geometry(e->cfg, rate, window, hop_frames, &H, &why)) return fail(e, NISQA_ERR_INVALID, why);
-  const int W = (int)window;
-  // the windows of every recording, in recording order (host arithmetic: nisqa_window_counts)
-  const int n_rec = rec->n_clips;
-  std::vector<int> wrec;
-  std::vector<int64_t> start, len;
-  for (int b = 0; b < n_rec; ++b) {
-    const int64_t T = target_sr > 0 ? nisqa_resample_out_len(rec->n_samples[b], rec->sample_rate, target_sr) : rec->n_samples[b];
-    if (T > (int64_t)INT32_MAX)
-      return fail(e, NISQA_ERR_INVALID, "rec.n_samples[" + std::to_string(b) + "]: " + std::to_string(T) +
-                                            " samples at the model rate, more than 2^31 - 1");
-    const int64_t K = window_count(T, W, H);
-    if ((int64_t)wrec.size() + K > INT32_MAX) return fail(e, NISQA_ERR_INVALID, "rec: more than 2^31 - 1 windows");
-    for (int64_t k = 0; k < K; ++k) {
-      wrec.push_back(b);
-      start.push_back(k * H);
-      len.push_back(std::min<int64_t>(W, T - k * H));
-    }
-  }
-  const int N = (int)wrec.size();
-  if (n_rows < N)
-    return fail(e, NISQA_ERR_INVALID, "n_rows = " + std::to_string(n_rows) + ": the call has " + std::to_string(N) + " windows");
-  if (N > 0 && !scores_dev) return fail(e, NISQA_ERR_INVALID, "scores_dev: null argument");
-  const int hop = (int)((double)rate * e->cfg.hop_s);
-  WinLayout L = {wrec.data(), start.data(), nullptr, H, H / hop, W};
-  std::vector<int32_t> rsr(n_rec, rec->sample_rate);
-  return enqueue_windows(e, cuda_stream, ing, fmt, target_sr, rate, N, len.data(), &L, n_rec, rec->n_samples, rsr.data(),
-                         scores_dev, n_segments_out, status_out);
+  return windows_call(e, cuda_stream, "rec", rec, nullptr, target_sr, window, hop_frames, 0, scores_dev, n_rows, n_segments_out,
+                      status_out, nullptr, nullptr);
 }
 
 int nisqa_predict_device_window_pairs(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
@@ -2667,136 +2755,77 @@ int nisqa_predict_device_window_pairs(nisqa_engine* e, void* cuda_stream, const 
     return fail(e, NISQA_ERR_INVALID, "ref: only a double-ended (NISQA_DE) engine scores window pairs");
   if (!deg) return fail(e, NISQA_ERR_INVALID, "deg: null argument");
   if (!ref) return fail(e, NISQA_ERR_INVALID, "ref: null argument");
-  if (target_sr < 0) return fail(e, NISQA_ERR_INVALID, "target_sr");
-  IngestSources ing = {};
-  ing.n_src = 2;
-  bool mix[2] = {false, false};
-  int rc = check_device_batch(e, *deg, "deg.", deg->channel, deg->n_clips, &ing.s[0], &mix[0]);
-  if (!rc) rc = check_device_batch(e, *ref, "ref.", -1, deg->n_clips, &ing.s[1], &mix[1]);     // always the mono mix
-  if (rc) return rc;
-  if (target_sr == 0 && ref->sample_rate != deg->sample_rate)
-    return fail(e, NISQA_ERR_INVALID, "ref.sample_rate = " + std::to_string(ref->sample_rate) + ": the windows of both recordings "
-                                      "run at one rate, deg.sample_rate = " + std::to_string(deg->sample_rate));
-  const bool f32 = deg->sample_fmt == NISQA_FMT_F32 || ref->sample_fmt == NISQA_FMT_F32 || mix[0] || mix[1];
-  const int fmt = f32 ? NISQA_FMT_F32 : NISQA_FMT_S16;
-  const int rate = target_sr > 0 ? target_sr : deg->sample_rate;
-  std::string why;
-  int H = 0;
-  int64_t M = 0;
-  if (!window_pair_geometry(e->cfg, rate, window, hop_frames, margin_frames, &H, &M, &why))
-    return fail(e, NISQA_ERR_INVALID, why);
-  const int W = (int)window;
-  // window pair k of recording b: clips 2p (degraded window) and 2p + 1 (reference window), in recording order (host
-  // arithmetic: nisqa_window_pair_counts)
-  const int n_rec = deg->n_clips;
-  std::vector<int> wrec;
-  std::vector<int64_t> start, len, rs_n(2 * (size_t)n_rec);
-  std::vector<int32_t> rs_sr(2 * (size_t)n_rec);
-  for (int b = 0; b < n_rec; ++b) {
-    int64_t T[2];
-    for (int k = 0; k < 2; ++k) {
-      const nisqa_device_batch* x = k ? ref : deg;
-      rs_n[2 * b + k] = x->n_samples[b]; rs_sr[2 * b + k] = x->sample_rate;
-      T[k] = target_sr > 0 ? nisqa_resample_out_len(x->n_samples[b], x->sample_rate, target_sr) : x->n_samples[b];
-      if (T[k] > (int64_t)INT32_MAX)
-        return fail(e, NISQA_ERR_INVALID, std::string(k ? "ref" : "deg") + ".n_samples[" + std::to_string(b) + "]: " +
-                                              std::to_string(T[k]) + " samples at the model rate, more than 2^31 - 1");
-    }
-    const int64_t K = window_count(T[0], W, H);
-    if ((int64_t)wrec.size() + 2 * K > INT32_MAX) return fail(e, NISQA_ERR_INVALID, "deg: more than 2^30 - 1 window pairs");
-    for (int64_t k = 0; k < K; ++k) {
-      int64_t r0, rn;
-      ref_window(k, T[1], W, H, M, &r0, &rn);
-      wrec.insert(wrec.end(), {b, b});
-      start.insert(start.end(), {k * H, r0});
-      len.insert(len.end(), {std::min<int64_t>(W, T[0] - k * H), rn});
-    }
-  }
-  const int N = (int)wrec.size();
-  if (n_rows < N / 2)
-    return fail(e, NISQA_ERR_INVALID, "n_rows = " + std::to_string(n_rows) + ": the call has " + std::to_string(N / 2) +
-                                          " window pairs");
-  if (N > 0 && !scores_dev) return fail(e, NISQA_ERR_INVALID, "scores_dev: null argument");
-  const int hop = (int)((double)rate * e->cfg.hop_s);
-  WinLayout L = {wrec.data(), start.data(), nullptr, H, H / hop, W};
-  L.n_src = 2;
-  std::vector<int32_t> nseg(N), status(N);
-  rc = enqueue_windows(e, cuda_stream, ing, fmt, target_sr, rate, N, len.data(), &L, 2 * n_rec, rs_n.data(), rs_sr.data(),
-                       scores_dev, nseg.data(), status.data());
-  for (int p = 0; p < N / 2; ++p) {
-    if (n_segments_out) n_segments_out[p] = nseg[2 * p];
-    if (status_out) status_out[p] = status[2 * p];
-    if (ref_n_segments_out) ref_n_segments_out[p] = nseg[2 * p + 1];
-    if (ref_status_out) ref_status_out[p] = status[2 * p + 1];
-  }
-  return rc;
+  return windows_call(e, cuda_stream, "deg", deg, ref, target_sr, window, hop_frames, margin_frames, scores_dev, n_rows,
+                      n_segments_out, status_out, ref_n_segments_out, ref_status_out);
 }
 
-int nisqa_window_counts(const nisqa_config* cfg, int64_t n_samples, int32_t sample_rate, int64_t window, int32_t hop_frames,
-                        int64_t* n_windows, int32_t* n_segments, int32_t* status, int64_t cap) {
-  if (!cfg || n_samples < 1) return NISQA_ERR_INVALID;
-  std::string why;
-  int H = 0;
-  if (!window_geometry(*cfg, sample_rate, window, hop_frames, &H, &why)) return NISQA_ERR_INVALID;
-  const int64_t K = window_count(n_samples, window, H);
-  if (n_windows) *n_windows = K;
-  for (int64_t k = 0; k < std::min(K, cap); ++k) {
-    ClipPlan p;
-    plan_clip(*cfg, std::min<int64_t>(window, n_samples - k * H), sample_rate, &p);
-    if (n_segments) n_segments[k] = p.n_seg;
-    if (status) status[k] = p.status;
-  }
-  return 0;
-}
-
-int nisqa_window_pair_counts(const nisqa_config* cfg, int64_t n_samples, int64_t ref_n_samples, int32_t sample_rate,
-                             int64_t window, int32_t hop_frames, int32_t margin_frames, int64_t* n_windows,
-                             int32_t* n_segments, int32_t* status, int32_t* ref_n_segments, int32_t* ref_status, int64_t cap) {
-  if (!cfg || n_samples < 1 || ref_n_samples < 1) return NISQA_ERR_INVALID;
+// nisqa_window_counts (n_src 1, margin_frames 0) and nisqa_window_pair_counts (n_src 2)
+static int window_counts(const nisqa_config* cfg, int n_src, int64_t n_samples, int64_t ref_n_samples, int32_t sample_rate,
+                         int64_t window, int32_t hop_frames, int32_t margin_frames, int64_t* n_windows, int32_t* n_segments,
+                         int32_t* status, int32_t* ref_n_segments, int32_t* ref_status, int64_t cap) {
+  if (!cfg || n_samples < 1 || (n_src == 2 && ref_n_samples < 1)) return NISQA_ERR_INVALID;
   std::string why;
   int H = 0;
   int64_t M = 0;
   if (!window_pair_geometry(*cfg, sample_rate, window, hop_frames, margin_frames, &H, &M, &why)) return NISQA_ERR_INVALID;
   const int64_t K = window_count(n_samples, window, H);
   if (n_windows) *n_windows = K;
-  for (int64_t k = 0; k < std::min(K, cap); ++k) {
-    ClipPlan p, q;
-    int64_t r0, rn;
-    ref_window(k, ref_n_samples, window, H, M, &r0, &rn);
-    plan_clip(*cfg, std::min<int64_t>(window, n_samples - k * H), sample_rate, &p);
-    plan_clip(*cfg, rn, sample_rate, &q);
-    if (n_segments) n_segments[k] = p.n_seg;
-    if (status) status[k] = p.status;
-    if (ref_n_segments) ref_n_segments[k] = q.n_seg;
-    if (ref_status) ref_status[k] = q.status;
-  }
+  WinList w;
+  for (int64_t k = 0; k < std::min(K, cap); ++k) add_window(&w, n_src, 0, k, n_samples, ref_n_samples, window, H, M);
+  plan_rows(*cfg, sample_rate, n_src, w, n_segments, status, ref_n_segments, ref_status);
   return 0;
 }
 
+int nisqa_window_counts(const nisqa_config* cfg, int64_t n_samples, int32_t sample_rate, int64_t window, int32_t hop_frames,
+                        int64_t* n_windows, int32_t* n_segments, int32_t* status, int64_t cap) {
+  return window_counts(cfg, 1, n_samples, 0, sample_rate, window, hop_frames, 0, n_windows, n_segments, status, nullptr,
+                       nullptr, cap);
+}
+
+int nisqa_window_pair_counts(const nisqa_config* cfg, int64_t n_samples, int64_t ref_n_samples, int32_t sample_rate,
+                             int64_t window, int32_t hop_frames, int32_t margin_frames, int64_t* n_windows,
+                             int32_t* n_segments, int32_t* status, int32_t* ref_n_segments, int32_t* ref_status, int64_t cap) {
+  return window_counts(cfg, 2, n_samples, ref_n_samples, sample_rate, window, hop_frames, margin_frames, n_windows, n_segments,
+                       status, ref_n_segments, ref_status, cap);
+}
+
 // ---- live feeds
-int nisqa_feed_rows(const nisqa_config* cfg, int32_t sample_rate, int64_t window, int32_t hop_frames, int32_t n_feeds,
-                    const int64_t* held, const int64_t* n_samples, const uint8_t* end, int64_t* n_rows, int32_t* feed,
-                    int64_t* index, int32_t* n_segments, int32_t* status, int64_t cap) {
-  if (!cfg || n_feeds < 0 || (n_feeds > 0 && (!held || !n_samples)) || !n_rows) return NISQA_ERR_INVALID;
+// nisqa_feed_rows (n_src 1, margin_frames 0) and nisqa_feed_pair_rows (n_src 2)
+static int feed_rows(const nisqa_config* cfg, int n_src, int32_t sample_rate, int64_t window, int32_t hop_frames,
+                     int32_t margin_frames, int32_t n_feeds, const int64_t* held, const int64_t* ref_held,
+                     const int64_t* n_samples, const int64_t* ref_n_samples, const uint8_t* end, int64_t* n_rows,
+                     int32_t* feed, int64_t* index, int32_t* n_segments, int32_t* status, int32_t* ref_n_segments,
+                     int32_t* ref_status, int64_t cap) {
+  const bool pair = n_src == 2;
+  if (!cfg || n_feeds < 0 || (n_feeds > 0 && (!held || !n_samples || (pair && (!ref_held || !ref_n_samples)))) || !n_rows)
+    return NISQA_ERR_INVALID;
   std::string why;
   int H = 0;
-  if (!window_geometry(*cfg, sample_rate, window, hop_frames, &H, &why)) return NISQA_ERR_INVALID;
+  int64_t M = 0;
+  if (!window_pair_geometry(*cfg, sample_rate, window, hop_frames, margin_frames, &H, &M, &why)) return NISQA_ERR_INVALID;
   for (int b = 0; b < n_feeds; ++b)
-    if (held[b] < 0 || n_samples[b] < 0) return NISQA_ERR_INVALID;
+    if (held[b] < 0 || n_samples[b] < 0 || (pair && (ref_held[b] < 0 || ref_n_samples[b] < 0))) return NISQA_ERR_INVALID;
   int64_t r = 0;
-  feed_windows(n_feeds, window, H, 0, held, n_samples, nullptr, nullptr, end, [&](int b, int64_t k, int64_t T, int64_t) {
+  WinList w;
+  feed_windows(n_feeds, window, H, M, held, n_samples, pair ? ref_held : nullptr, pair ? ref_n_samples : nullptr, end,
+               [&](int b, int64_t k, int64_t T, int64_t T_ref) {
     if (r < cap) {
-      ClipPlan p;
-      plan_clip(*cfg, std::min(window, T - k * H), sample_rate, &p);
       if (feed) feed[r] = b;
       if (index) index[r] = k;
-      if (n_segments) n_segments[r] = p.n_seg;
-      if (status) status[r] = p.status;
+      add_window(&w, n_src, b, k, T, T_ref, window, H, M);
     }
     ++r;
   });
   *n_rows = r;
+  plan_rows(*cfg, sample_rate, n_src, w, n_segments, status, ref_n_segments, ref_status);
   return 0;
+}
+
+int nisqa_feed_rows(const nisqa_config* cfg, int32_t sample_rate, int64_t window, int32_t hop_frames, int32_t n_feeds,
+                    const int64_t* held, const int64_t* n_samples, const uint8_t* end, int64_t* n_rows, int32_t* feed,
+                    int64_t* index, int32_t* n_segments, int32_t* status, int64_t cap) {
+  return feed_rows(cfg, 1, sample_rate, window, hop_frames, 0, n_feeds, held, nullptr, n_samples, nullptr, end, n_rows, feed,
+                   index, n_segments, status, nullptr, nullptr, cap);
 }
 
 int nisqa_feed_pair_rows(const nisqa_config* cfg, int32_t sample_rate, int64_t window, int32_t hop_frames,
@@ -2804,34 +2833,8 @@ int nisqa_feed_pair_rows(const nisqa_config* cfg, int32_t sample_rate, int64_t w
                          const int64_t* n_samples, const int64_t* ref_n_samples, const uint8_t* end, int64_t* n_rows,
                          int32_t* feed, int64_t* index, int32_t* n_segments, int32_t* status, int32_t* ref_n_segments,
                          int32_t* ref_status, int64_t cap) {
-  if (!cfg || n_feeds < 0 || (n_feeds > 0 && (!held || !ref_held || !n_samples || !ref_n_samples)) || !n_rows)
-    return NISQA_ERR_INVALID;
-  std::string why;
-  int H = 0;
-  int64_t M = 0;
-  if (!window_pair_geometry(*cfg, sample_rate, window, hop_frames, margin_frames, &H, &M, &why)) return NISQA_ERR_INVALID;
-  for (int b = 0; b < n_feeds; ++b)
-    if (held[b] < 0 || n_samples[b] < 0 || ref_held[b] < 0 || ref_n_samples[b] < 0) return NISQA_ERR_INVALID;
-  int64_t r = 0;
-  feed_windows(n_feeds, window, H, M, held, n_samples, ref_held, ref_n_samples, end,
-               [&](int b, int64_t k, int64_t T, int64_t T_ref) {
-    if (r < cap) {
-      ClipPlan p, q;
-      int64_t r0, rn;
-      ref_window(k, T_ref, window, H, M, &r0, &rn);
-      plan_clip(*cfg, std::min(window, T - k * H), sample_rate, &p);
-      plan_clip(*cfg, rn, sample_rate, &q);
-      if (feed) feed[r] = b;
-      if (index) index[r] = k;
-      if (n_segments) n_segments[r] = p.n_seg;
-      if (status) status[r] = p.status;
-      if (ref_n_segments) ref_n_segments[r] = q.n_seg;
-      if (ref_status) ref_status[r] = q.status;
-    }
-    ++r;
-  });
-  *n_rows = r;
-  return 0;
+  return feed_rows(cfg, 2, sample_rate, window, hop_frames, margin_frames, n_feeds, held, ref_held, n_samples, ref_n_samples,
+                   end, n_rows, feed, index, n_segments, status, ref_n_segments, ref_status, cap);
 }
 
 // nisqa_feed_create (n_src 1: margin_frames = max_skew = 0) and nisqa_feed_pair_create (n_src 2)
@@ -2939,7 +2942,7 @@ int64_t nisqa_feed_device_bytes(const nisqa_feed* f) {
 
 // nisqa_feed_push (ref == nullptr) and nisqa_feed_pair_push: the chunk of each source appended to its rings, the
 // interior pairs whose last tap it brings computed into its frame rings, then the windows (pairs) the push completes
-// scored as the clips of predict_common, reading the rings
+// scored as the clips of a call that reads the rings
 static int feed_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch* deg, const nisqa_device_batch* ref,
                      const uint8_t* end, float* scores_dev, int64_t n_rows, int32_t* feed_out, int64_t* index_out,
                      int32_t* n_segments_out, int32_t* status_out, int32_t* ref_n_segments_out, int32_t* ref_status_out) {
@@ -2948,9 +2951,6 @@ static int feed_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch*
   const int S = f->n_src, B = f->n_feeds;
   const nisqa_device_batch* src[2] = {deg, ref};
   const std::string nm[2] = {S == 2 ? "deg" : "chunk", "ref"};
-  IngestSources ing = {};
-  ing.n_src = S;
-  bool f32 = false;
   for (int s = 0; s < S; ++s) {
     const nisqa_device_batch* c = src[s];
     if (!c) return fail(e, NISQA_ERR_INVALID, nm[s] + ": null argument");
@@ -2960,11 +2960,11 @@ static int feed_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch*
     if (c->sample_rate != f->rate)
       return fail(e, NISQA_ERR_INVALID, nm[s] + ".sample_rate = " + std::to_string(c->sample_rate) + ": the feeds run at " +
                                             std::to_string(f->rate) + " Hz");
-    bool mix = false;
-    const int rc = check_device_batch(e, *c, nm[s] + ".", s ? -1 : c->channel, B, &ing.s[s], &mix, 0);  // (ref: mono mix)
-    if (rc) return rc;
-    f32 = f32 || c->sample_fmt == NISQA_FMT_F32 || mix;
   }
+  IngestSources ing;
+  int fmt;
+  int rc = check_sources(e, nm[0] + ".", *deg, ref, B, 0, &ing, &fmt);
+  if (rc) return rc;
   long long max_in[2] = {0, 0};
   bool holds = false;
   for (int s = 0; s < S; ++s)
@@ -2985,8 +2985,7 @@ static int feed_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch*
                                               " degraded and " + std::to_string(Tr) + " reference samples, more than "
                                               "max_skew (" + std::to_string(f->max_skew) + " samples) apart");
     }
-  // one format for both sources (as nisqa_predict_device_window_pairs): float32 if either is float32 or mixed
-  const int fmt = f32 ? NISQA_FMT_F32 : NISQA_FMT_S16;
+  // one format for both sources (as nisqa_predict_device_window_pairs)
   if (std::max(max_in[0], max_in[1]) > 0 && holds && f->fmt != fmt)
     return fail(e, NISQA_ERR_INVALID, (S == 2 ? std::string("deg.sample_fmt / ref.sample_fmt") : std::string("chunk.sample_fmt")) +
                                           ": the feeds hold " + (f->fmt == NISQA_FMT_F32 ? "float32" : "int16") +
@@ -2996,28 +2995,33 @@ static int feed_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch*
   // the windows (pairs: clips 2p and 2p + 1) the push completes (host arithmetic: nisqa_feed_rows, nisqa_feed_pair_rows)
   const FeedGeom& g = f->g[0];
   const int64_t M = S == 2 ? f->g[1].off : 0;
-  std::vector<int> wfeed;
-  std::vector<int64_t> wstart, wlen, widx;
+  WinList wl;
+  std::vector<int64_t> widx;
   feed_windows(B, g.W, g.H, M, f->held[0].data(), deg->n_samples, S == 2 ? f->held[1].data() : nullptr,
                S == 2 ? ref->n_samples : nullptr, end, [&](int b, int64_t k, int64_t T, int64_t T_ref) {
     widx.push_back(k);
-    wfeed.push_back(b); wstart.push_back(k * g.H); wlen.push_back(std::min<int64_t>(g.W, T - k * g.H));
-    if (S == 2) {
-      int64_t r0, rn;
-      ref_window(k, T_ref, g.W, g.H, M, &r0, &rn);
-      wfeed.push_back(b); wstart.push_back(r0); wlen.push_back(rn);
-    }
+    add_window(&wl, S, b, k, T, T_ref, g.W, g.H, M);
   });
-  const int N = (int)wfeed.size(), rows = N / S;
+  const int N = (int)wl.rec.size(), rows = N / S;
   if (n_rows < rows)
     return fail(e, NISQA_ERR_INVALID, "n_rows = " + std::to_string(n_rows) + ": the push completes " + std::to_string(rows) +
                                           (S == 2 ? " window pairs" : " windows"));
   if (N > 0 && !scores_dev) return fail(e, NISQA_ERR_INVALID, "scores_dev: null argument");
+  // the completed windows, each a clip of a pass that reads the rings
+  FeedRings rings = {};
+  for (int s = 0; s < 2; ++s) {
+    const int u = s < S ? s : 0;        // (single-ended: both entries are the one source)
+    rings.g[s] = f->g[u]; rings.ring_at[s] = f->ring_at[u]; rings.frames[s] = f->frames + f->frames_at[u];
+  }
+  WinLayout L = {wl.rec.data(), wl.start.data(), nullptr, g.H, g.hf, g.W, &rings};
+  L.n_src = S;
+  std::vector<int32_t> srs(N, f->rate), nseg(N), status(N);
+  Call c(N, wl.len.data(), srs.data(), fmt, nseg.data(), status.data());
+  c.dev_pcm = f->ring; c.scores_dev = scores_dev; c.win = &L;
+  rc = plan_call(e, c);
+  if (rc) return rc;
 
   // each source's new samples and the interior pairs whose last tap they bring
-  CK(cudaSetDevice(e->device));
-  for (auto& t : e->timers) { t.ms = 0.0; t.launches = 0; }
-  cudaStream_t caller = static_cast<cudaStream_t>(cuda_stream);
   auto& sl = f->slots[f->n_push % kFeedSlots];
   if (sl.busy) { CK(cudaEventSynchronize(sl.copied)); sl.busy = false; }
   CK(sl.h.reserve((size_t)S * B * sizeof(FeedPush)));
@@ -3038,76 +3042,48 @@ static int feed_push(nisqa_feed* f, void* cuda_stream, const nisqa_device_batch*
       f->j_next[s][b] = std::max<long long>(f->j_next[s][b], j_end);
     }
   }
-  CK(cudaEventRecord(e->ev_in, caller));
-  cudaStream_t st = e->lanes[e->profiling ? 0 : (int)(e->pass_counter % kLanes)].stream;
-  CK(cudaStreamWaitEvent(st, e->ev_in, 0));
-  if (f->pending) CK(cudaStreamWaitEvent(st, f->done, 0));  // push order: the last push's passes are done with the rings
-  if (std::max(max_in[0], max_in[1]) > 0) {
-    CK(sl.d.reserve((size_t)S * B * sizeof(FeedPush)));
-    CK(cudaMemcpyAsync(sl.d.p, tab, (size_t)S * B * sizeof(FeedPush), cudaMemcpyHostToDevice, st));
-    CK(cudaEventRecord(sl.copied, st));
-    sl.busy = true;
-    ++f->n_push;
-    e->cur_stream = st;
-    const size_t esz = fmt == NISQA_FMT_F32 ? 4 : 2;
-    for (int s = 0; s < S; ++s) {
-      void* ring = static_cast<char*>(f->ring) + f->ring_at[s] * esz;
-      const FeedPush* push = sl.d.as<FeedPush>() + s * B;
-      if (max_in[s] > 0) {
-        Scope sc(e, "ingest");
-        launch_ingest_feed(st, ing.s[s], push, B, max_in[s], f->g[s], fmt == NISQA_FMT_F32, ring);
+  rc = enqueue_call(e, cuda_stream, c, f, [&](cudaStream_t st) -> int {
+    if (f->pending) CK(cudaStreamWaitEvent(st, f->done, 0));  // push order: the last push's passes are done with the rings
+    if (std::max(max_in[0], max_in[1]) > 0) {
+      CK(sl.d.reserve((size_t)S * B * sizeof(FeedPush)));
+      CK(cudaMemcpyAsync(sl.d.p, tab, (size_t)S * B * sizeof(FeedPush), cudaMemcpyHostToDevice, st));
+      CK(cudaEventRecord(sl.copied, st));
+      sl.busy = true;
+      ++f->n_push;
+      e->cur_stream = st;
+      const size_t esz = fmt == NISQA_FMT_F32 ? 4 : 2;
+      for (int s = 0; s < S; ++s) {
+        void* ring = static_cast<char*>(f->ring) + f->ring_at[s] * esz;
+        const FeedPush* push = sl.d.as<FeedPush>() + s * B;
+        if (max_in[s] > 0) {
+          Scope sc(e, "ingest");
+          launch_ingest_feed(st, ing.s[s], push, B, max_in[s], f->g[s], fmt == NISQA_FMT_F32, ring);
+        }
+        if (max_pairs[s] > 0) {
+          Scope sc(e, "frontend");
+          launch_frontend_feed_pairs(st, e->cfg.n_mels, ring, fmt == NISQA_FMT_F32, push, B, max_pairs[s], f->g[s],
+                                     e->fb_table.as<FbTables>(), e->tw4096.as<float2>(), f->frames + f->frames_at[s]);
+        }
       }
-      if (max_pairs[s] > 0) {
-        Scope sc(e, "frontend");
-        launch_frontend_feed_pairs(st, e->cfg.n_mels, ring, fmt == NISQA_FMT_F32, push, B, max_pairs[s], f->g[s],
-                                   e->fb_table.as<FbTables>(), e->tw4096.as<float2>(), f->frames + f->frames_at[s]);
-      }
+      CK(cudaGetLastError());
+      f->fmt = fmt;
     }
-    CK(cudaGetLastError());
-    f->fmt = fmt;
-  }
-  for (int b = 0; b < B; ++b) {
-    for (int s = 0; s < S; ++s) f->held[s][b] += src[s]->n_samples[b];
-    if (end && end[b])
-      for (int s = 0; s < S; ++s) { f->held[s][b] = 0; f->j_next[s][b] = 0; }
-  }
-  CK(cudaEventRecord(f->ready, st));
-  // the completed windows, each a clip of a pass that reads the rings
-  cudaStream_t fin = st;
-  std::vector<int32_t> nseg(N), status(N);
-  if (N > 0) {
-    FeedRings rings = {};
-    for (int s = 0; s < 2; ++s) {
-      const int u = s < S ? s : 0;        // (single-ended: both entries are the one source)
-      rings.g[s] = f->g[u]; rings.ring_at[s] = f->ring_at[u]; rings.frames[s] = f->frames + f->frames_at[u];
+    for (int b = 0; b < B; ++b) {
+      for (int s = 0; s < S; ++s) f->held[s][b] += src[s]->n_samples[b];
+      if (end && end[b])
+        for (int s = 0; s < S; ++s) { f->held[s][b] = 0; f->j_next[s][b] = 0; }
     }
-    WinLayout L = {wfeed.data(), wstart.data(), nullptr, g.H, g.hf, g.W, &rings};
-    L.n_src = S;
-    std::vector<int32_t> srs(N, f->rate);
-    const int rc = predict_common(e, N, nullptr, f->ring, nullptr, wlen.data(), srs.data(), f->fmt, nullptr, scores_dev,
-                                  nseg.data(), status.data(), 0, nullptr, nullptr, f->ready, &fin, &L);
-    if (rc) {
-      for (auto& l : e->lanes)
-        if (cudaEventRecord(e->ev_out, l.stream) == cudaSuccess) cudaStreamWaitEvent(caller, e->ev_out, 0);
-      if (cudaEventRecord(f->done, caller) == cudaSuccess) f->pending = true;
-      return rc;
-    }
-  } else if (e->profiling) {
-    CK(cudaStreamSynchronize(st));
-    collect_timers(e);
-  }
+    CK(cudaEventRecord(f->ready, st));
+    c.fmt = f->fmt;                     // (the passes read the rings, in the format they hold)
+    c.ready = f->ready;
+    return 0;
+  });
+  if (rc) return rc;
   for (int r = 0; r < rows; ++r) {
-    if (feed_out) feed_out[r] = wfeed[S * r];
+    if (feed_out) feed_out[r] = wl.rec[S * r];
     if (index_out) index_out[r] = widx[r];
-    if (n_segments_out) n_segments_out[r] = nseg[S * r];
-    if (status_out) status_out[r] = status[S * r];
-    if (S == 2 && ref_n_segments_out) ref_n_segments_out[r] = nseg[2 * r + 1];
-    if (S == 2 && ref_status_out) ref_status_out[r] = status[2 * r + 1];
   }
-  CK(cudaEventRecord(f->done, fin));
-  f->pending = true;
-  CK(cudaEventRecord(e->ev_out, fin));
-  CK(cudaStreamWaitEvent(caller, e->ev_out, 0));
+  split_rows(S, rows, nseg.data(), status.data(), n_segments_out, status_out, ref_n_segments_out, ref_status_out);
   return 0;
 }
 
