@@ -328,6 +328,34 @@ NISQA_API int  nisqa_predict_device_batch_embeddings(nisqa_engine* e, void* cuda
                                                      const nisqa_embedding_out* emb, int32_t* n_segments_out,
                                                      int32_t* status_out);
 
+/* NISQA_DE's time alignment: where in the reference each degraded segment came from, as the model's Alignment module
+ * (AttDot / AttCosine / AttDistance / AttLuong / AttBahdanau) sees it, from the rows NISQA_STAGE_TD1_OUT documents.  For
+ * degraded segment i of a pair and reference segments j = 0 .. Sy - 1 with alignment scores s_ij and a_ij = softmax_j(s_ij):
+ *   ref_seg[r]  : the first j with the maximal s_ij (under hard application: the reference row the fusion copied)
+ *   weight[r]   : a_i,ref_seg = 1 / sum_j exp(s_ij - s_i,ref_seg): how sharp the match is
+ *   centroid[r] : sum_j a_ij j, the attention-weighted reference segment (what soft application reads)
+ *   peak[r]     : s_i,ref_seg as the module computes it (AttCosine: the cosine similarity; AttBahdanau: with v's bias)
+ * Rows as in nisqa_segment_out: one per segment of every OK degraded clip in clip order, none for the others and none for
+ * the reference clips (2p + 1).  A pair that scores NaN while its degraded status is OK (a reference that is too short,
+ * too long or, for window pairs, empty) has ref_seg -1 and NaN values.  Segment i starts at i*seg_hop*hop / sr seconds
+ * of its clip, each clip at its own model rate and hop (see nisqa_segment_out). */
+typedef struct nisqa_alignment_out {
+  int32_t* ref_seg;    /* device [n_rows] int32 */
+  float*   weight;     /* device [n_rows] fp32 */
+  float*   centroid;   /* device [n_rows] fp32 */
+  float*   peak;       /* device [n_rows] fp32 */
+  int64_t  n_rows;     /* rows each array holds */
+} nisqa_alignment_out;
+
+/* nisqa_predict_device_batch of a double-ended engine that also writes the alignment to al, with the same stream contract
+ * and no host wait of its own.  NISQA_ERR_INVALID before anything is enqueued for a single-ended engine, a NULL al or
+ * array, or an al->n_rows smaller than the segment count of the call's OK degraded clips.  scores_dev gets the same
+ * values as nisqa_predict_device_batch would write. */
+NISQA_API int  nisqa_predict_device_batch_alignment(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                                                    const nisqa_device_batch* ref, int32_t target_sr, float* scores_dev,
+                                                    const nisqa_alignment_out* al, int32_t* n_segments_out,
+                                                    int32_t* status_out);
+
 /* Recordings of any length scored as a timeline of overlapping windows, each window scored exactly as the clip cut out of
  * the recording would be (its own reflect padding, top_db maximum, segment count and status).  At the model rate sr
  * (target_sr when set, else the batch's sample_rate; an ms_sr checkpoint converts each WHOLE recording first) a
@@ -375,6 +403,18 @@ NISQA_API int  nisqa_predict_device_window_pairs(nisqa_engine* e, void* cuda_str
                                                  int32_t hop_frames, int32_t margin_frames, float* scores_dev,
                                                  int64_t n_rows, int32_t* n_segments_out, int32_t* status_out,
                                                  int32_t* ref_n_segments_out, int32_t* ref_status_out);
+/* nisqa_predict_device_window_pairs that also writes each pair's alignment to al (nisqa_alignment_out), with the same
+ * stream contract and no host wait of its own: the rows of each pair's degraded window in pair order, segment i of pair k
+ * starting i*seg_hop*hop / sr seconds into its degraded window (k H samples into the recording) and ref_seg counted from
+ * its reference window's start (max(0, k H - M) samples into the reference).  The refusals of
+ * nisqa_predict_device_batch_alignment, with al->n_rows counting the degraded windows' segments; scores_dev gets what
+ * nisqa_predict_device_window_pairs would write. */
+NISQA_API int  nisqa_predict_device_window_pairs_alignment(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                                                           const nisqa_device_batch* ref, int32_t target_sr, int64_t window,
+                                                           int32_t hop_frames, int32_t margin_frames, float* scores_dev,
+                                                           int64_t n_rows, const nisqa_alignment_out* al,
+                                                           int32_t* n_segments_out, int32_t* status_out,
+                                                           int32_t* ref_n_segments_out, int32_t* ref_status_out);
 
 /* Live feeds: n_feeds independent recordings that arrive chunk by chunk (calls, conference bridges, broadcast and TTS
  * monitoring), scored as the windows of nisqa_predict_device_windows as soon as each window is complete.  A feed object

@@ -26,6 +26,12 @@ to ``output_dir/NISQA_windows.csv``, one row per window with its time span, segm
 ``csv_ref``) scores window pairs of each file and its reference, the reference windows widened by
 ``args['reference_margin_s']`` seconds on either side (default 0): each row also has the reference file and the
 reference window's time span and segment count.
+
+``args['alignment']`` (``run_predict.py --alignment``, NISQA_DE in ``predict_csv`` mode with ``csv_ref``) also writes
+``NISQA_alignment.csv`` into ``output_dir``: one row per degraded segment (in windows mode: per segment of every window
+pair's degraded window) with the file and reference columns, ``seg``, ``t_start``, ``ref_seg``, ``ref_t_start``,
+``delay_s``, ``weight``, ``centroid_delay_s`` and ``peak`` (:meth:`nisqa_b200.scorer.Scorer.align`).  Single process
+only.
 """
 import datetime
 import os
@@ -66,6 +72,9 @@ class nisqaModel(object):
             raise ValueError("segments: per-segment rows are not written in windows mode (window_s)")
         if win and args.get("embeddings"):
             raise ValueError("embeddings: pooled vectors are not written in windows mode (window_s)")
+        if args.get("alignment") and nb_dist.env_world()[1] > 1:
+            raise ValueError("alignment: NISQA_alignment.csv is written by a single process, not under torchrun with %d "
+                             "ranks" % nb_dist.env_world()[1])
         if args.get("reference_margin_s") is not None and not win:
             raise ValueError("reference_margin_s: a margin of the reference windows needs windows mode (window_s)")
         if "mode" not in self.args:
@@ -75,6 +84,8 @@ class nisqaModel(object):
         self._loadModel()
         if self.args.get("reference_margin_s") is not None and not self.args["double_ended"]:
             raise ValueError("reference_margin_s: a single-ended checkpoint reads no reference (NISQA_DE only)")
+        if self.args.get("alignment") and not self.args["double_ended"]:
+            raise ValueError("alignment: a single-ended checkpoint aligns no reference (NISQA_DE only)")
         self._loadDatasets()
         self.args["now"] = datetime.datetime.today()
 
@@ -126,6 +137,8 @@ class nisqaModel(object):
             df = self.predict_windows()
             if self.args["output_dir"]:
                 df.to_csv(os.path.join(self.args["output_dir"], "NISQA_windows.csv"), index=False)
+                if self.args.get("alignment"):
+                    self.predict_alignment().to_csv(os.path.join(self.args["output_dir"], "NISQA_alignment.csv"), index=False)
             print(df.to_string(index=False))
             return df
         if self.args["dim"] == True:  # noqa: E712  (mirrors the reference comparison)
@@ -148,7 +161,52 @@ class nisqaModel(object):
             self.predict_segments().to_csv(os.path.join(self.args["output_dir"], "NISQA_segments.csv"), index=False)
         if self.args.get("embeddings") and self.args["output_dir"]:
             np.savez(os.path.join(self.args["output_dir"], "NISQA_embeddings.npz"), **self.predict_embeddings())
+        if self.args.get("alignment") and self.args["output_dir"]:
+            self.predict_alignment().to_csv(os.path.join(self.args["output_dir"], "NISQA_alignment.csv"), index=False)
         return self.ds_val.df
+
+    def predict_alignment(self):
+        """-> DataFrame of ``NISQA_alignment.csv``: one row per degraded segment of every file pair, in file order (in
+        windows mode: per segment of every window pair's degraded window, with the pair's ``window`` index and its
+        ``win_t_start`` / ``win_ref_t_start`` after the file columns), from :meth:`Scorer.align`.  Pairs are batched and
+        decoded as :meth:`predict_segments` (windows mode: one file pair per call, as :meth:`predict_windows`)."""
+        sc = self._scorer()
+        ds = self.ds_val
+        col, col_ref = ds.filename_column, ds.filename_column_ref
+        files, refs = ds.df[col].tolist(), ds.df[col_ref].tolist()
+        win = self.args.get("window_s") is not None
+        parts = {}
+
+        def part(i, res, r0, n, extra):
+            d = pd.DataFrame({col: [files[i]] * n, col_ref: [refs[i]] * n})
+            for k, v in extra.items():
+                d[k] = v
+            d["seg"] = np.arange(n) if not win else np.concatenate([np.arange(c) for c in res.counts]) if n else []
+            sl = slice(r0, r0 + n)
+            d["t_start"], d["ref_seg"] = res.t_start[sl], res.ref_seg[sl].cpu().numpy()
+            d["ref_t_start"], d["delay_s"] = res.ref_t_start[sl], res.delay_s[sl]
+            d["weight"] = res.weight[sl].cpu().numpy().astype(float)
+            d["centroid_delay_s"] = res.centroid_delay_s[sl]
+            d["peak"] = res.peak[sl].cpu().numpy().astype(float)
+            return d
+        if win:
+            for i in range(len(ds)):
+                y, sr = NL.read_wav(ds.file_path(i), ds.ms_channel)
+                y_ref, sr_ref = NL.read_wav(ds.file_path_ref(i), None)
+                res = sc.align(self._batch_tensor([y])[0], sr, self._batch_tensor([y_ref])[0], reference_sample_rate=sr_ref,
+                               window_s=self.args["window_s"], window_hop_s=self.args["window_hop_s"],
+                               reference_margin_s=self.args.get("reference_margin_s") or 0.0)
+                n = int(sum(res.counts))
+                parts[i] = part(i, res, 0, n, {"window": res.window, "win_t_start": res.pair_t_start[res.window],
+                                               "win_ref_t_start": res.pair_ref_t_start[res.window]})
+        else:
+            for batch, call in self._file_batches():
+                res = call(sc.align)
+                r0 = 0
+                for j, i in enumerate(batch):
+                    parts[i] = part(i, res, r0, res.counts[j], {})
+                    r0 += res.counts[j]
+        return pd.concat([parts[i] for i in range(len(ds))], ignore_index=True)
 
     def predict_segments(self):
         """-> DataFrame with one row per segment of every file, in file order: the file column, ``segment``,

@@ -921,6 +921,8 @@ bool pack_de_align(Packer& P, const nisqa_config& c, int W) {
     memcpy(&P.arena[ob], bq->d, 512);
     memcpy(&P.arena[ob + 128], by->d, 512);
     P.copy(A.v, v->d, 128);
+    auto vb = P.t.find("align.att.v.bias");     // (only the peak an alignment call reports reads it: softmax drops it)
+    A.vb = vb != P.t.end() && vb->second.numel == 1 ? vb->second.d[0] : 0.f;
   }
   return true;
 }
@@ -1269,6 +1271,7 @@ struct Call {
   int32_t* status;
   const nisqa_segment_out* seg = nullptr;
   const nisqa_embedding_out* emb = nullptr;
+  const nisqa_alignment_out* al = nullptr;
   // completion: synchronous, a ticket, or in stream order (the lanes wait for `ready` before they read the input or
   // write outputs)
   bool sync = false;
@@ -1276,7 +1279,7 @@ struct Call {
   cudaEvent_t ready = nullptr;
   WinLayout* win = nullptr;           // a windows call or feed push
   std::vector<ClipPlan> plan;         // [n_clips]
-  std::vector<long long> seg_row;     // segments / embeddings call: each clip's first output row (-1: none)
+  std::vector<long long> seg_row;     // segments / embeddings / alignment call: each clip's first output row (-1: none)
   Call(int n, const int64_t* ns, const int32_t* sr, int fmt_, int32_t* n_seg, int32_t* st)
       : n_clips(n), n_samples(ns), sample_rate(sr), fmt(fmt_), n_segments(n_seg), status(st) {}
 };
@@ -1299,7 +1302,8 @@ struct PassInput {
   bool pair_rows = false;             // window-pairs call: scores_dev_out is compact, [n_clips / 2][n_out]
   const nisqa_segment_out* seg;       // segments call: its outputs (else nullptr)
   const nisqa_embedding_out* emb;     // embeddings call: its outputs (else nullptr)
-  const long long* seg_row;           // either: the first output row of each clip (-1: none)
+  const nisqa_alignment_out* al;      // alignment call: its outputs (else nullptr)
+  const long long* seg_row;           // any of them: the first output row of each clip (-1: none)
 };
 
 int lane_allgather(nisqa_engine* e, const float* src, float* dst, size_t count, cudaStream_t st);
@@ -1326,7 +1330,8 @@ struct Pass {
   int* seg_frame0 = nullptr;                  // segment table (lane, seg_table_kernel)
   float* seg_thr = nullptr;
   int* seg_clip = nullptr;
-  const long long* seg_row = nullptr;         // segments / embeddings call: the clips' first output rows (staging slot)
+  const long long* seg_row = nullptr;         // segments / embeddings / alignment call: the clips' first output rows (staging slot)
+  const nisqa_alignment_out* al = nullptr;    // alignment call: its outputs
   const WinSpan* spans = nullptr;             // windows call: the recording spans (staging slot)
   const FeedWin* fwins = nullptr;             // feed push: the windows' rows (staging slot)
   // the rows the pooling module read (segment_rows): D real columns at a stride of ld, the attention logits the pooling
@@ -1337,7 +1342,7 @@ struct Pass {
   PoolSimpleParams pool_P = {};
   Pass(nisqa_engine* e_, const PassInput& in)
       : e(e_), c(e_->cfg), w(e_->w), LN(e_->lanes[in.slot]), SG(e_->stages[in.stage]), st(LN.stream),
-        std_mode(e_->std_cnn()), scores(in.scores_dev_out), n(in.n_clips) {}
+        std_mode(e_->std_cnn()), scores(in.scores_dev_out), n(in.n_clips), al(in.al) {}
 };
 
 // [n_seg][64 nk] rows that feed a time-dependency block
@@ -1396,14 +1401,14 @@ int upload_inputs(Pass& p, const PassInput& in) {
   SG.lane = in.slot;
   // one pinned block: ClipDesc[n] | the prefix arrays
   const size_t tb_clips = (size_t)n * sizeof(ClipDesc), tb_pref = pre.size() * 4;
-  const size_t tb_rows_at = (tb_clips + tb_pref + 7) / 8 * 8, tb_rows = in.seg || in.emb ? (size_t)n * 8 : 0;
+  const size_t tb_rows_at = (tb_clips + tb_pref + 7) / 8 * 8, tb_rows = in.seg || in.emb || in.al ? (size_t)n * 8 : 0;
   const size_t tb_spans_at = tb_rows_at + tb_rows, tb_spans = in.win ? in.win->spans.size() * sizeof(WinSpan) : 0;
   const size_t tb_fwins_at = (tb_spans_at + tb_spans + 15) / 16 * 16, tb_fwins = in.win ? in.win->fwins.size() * sizeof(FeedWin) : 0;
   CK(SG.h_tables.reserve(tb_fwins_at + tb_fwins));
   char* ht = SG.h_tables.as<char>();
   memcpy(ht, cl.data(), tb_clips);
   memcpy(ht + tb_clips, pre.data(), tb_pref);
-  if (tb_rows) {      // (a segments or embeddings call: the rows of the pass's clips)
+  if (tb_rows) {      // (a segments, embeddings or alignment call: the rows of the pass's clips)
     memcpy(ht + tb_rows_at, in.seg_row, tb_rows);
     CK(SG.seg_row.reserve(tb_rows));
     CK(cudaMemcpyAsync(SG.seg_row.p, ht + tb_rows_at, tb_rows, cudaMemcpyHostToDevice, cs));
@@ -1658,8 +1663,11 @@ int de_fuse(Pass& p, const float* td_rows, int W, Rows* out) {
   if (work) CK(LN.dework.reserve(work * 4));
   CK(cudaMemsetAsync(LN.fused.p, 0, (size_t)n_seg * fd * 4, p.st));      // rows of the reference clips stay zero
   { Scope s(e, "de_align", de_align_launches(c.de_align));
+    DeAlignOut al = {};
+    if (p.al) al = {p.seg_row, p.al->ref_seg, p.al->weight, p.al->centroid, p.al->peak, 0.f};
     launch_de_align(p.st, td_rows, W, n_seg, p.clips, p.n, p.qt64_prefix, p.n_qt64, c.de_align,
-                    c.de_align_apply == NISQA_DE_APPLY_SOFT, c.de_fuse, p.w.de, LN.dework.as<float>(), LN.fused.as<float>()); }
+                    c.de_align_apply == NISQA_DE_APPLY_SOFT, c.de_fuse, p.w.de, LN.dework.as<float>(), LN.fused.as<float>(),
+                    p.al ? &al : nullptr); }
   *out = {LN.fused.as<float>(), fd / 64};
   e->last_de_fused = LN.fused.as<float>();      // (nothing behind the alignment writes fused: lin_fusion writes ffa, td_2 its own buffers)
   e->last_de_fused_d = fd;
@@ -1874,7 +1882,7 @@ int lstm_head(Pass& p, const PassInput& in) {
 // A segments call: every segment's score and pooling weight under each head; an embeddings call: each head's pooled
 // vector and optionally the segments' rows - from the rows the pooling module read, to the call's outputs.  A clip the
 // call counts rows for but the pass did not run (NISQA_DE: its reference is too short or too long) gets NaN rows, like
-// its score.
+// its score; in an alignment call (whose rows de_fuse wrote) ref_seg -1 and NaN values.
 int segment_rows(Pass& p, const PassInput& in) {
   nisqa_engine* e = p.e;
   const int nh = p.c.n_out, W = p.w.pool_width;
@@ -1889,6 +1897,12 @@ int segment_rows(Pass& p, const PassInput& in) {
       CK(cudaMemsetAsync(so->weights + (size_t)r * nh, 0xFF, n * nh * 4, p.st));
     }
     if (eo && eo->rows) CK(cudaMemsetAsync(eo->rows + (size_t)r * W, 0xFF, n * W * 4, p.st));
+    if (const nisqa_alignment_out* ao = in.al) {        // (0xFFFFFFFF: int32 -1, a float NaN)
+      CK(cudaMemsetAsync(ao->ref_seg + r, 0xFF, n * 4, p.st));
+      CK(cudaMemsetAsync(ao->weight + r, 0xFF, n * 4, p.st));
+      CK(cudaMemsetAsync(ao->centroid + r, 0xFF, n * 4, p.st));
+      CK(cudaMemsetAsync(ao->peak + r, 0xFF, n * 4, p.st));
+    }
   }
   float* pooled = eo ? eo->pooled + (size_t)in.first_clip * nh * W : nullptr;
   if (p.n_seg == 0) {     // (nothing ran: NaN vectors, like the scores)
@@ -1925,7 +1939,7 @@ int run_pass(nisqa_engine* e, const PassInput& in) {
     if (!rc) rc = p.w.lstm_shipped ? lstm_head(p, in) : td_stages(p, rows);
     if (rc) return rc;
   }
-  if (in.seg || in.emb) {
+  if (in.seg || in.emb || in.al) {
     rc = segment_rows(p, in);
     if (rc) return rc;
   }
@@ -2023,8 +2037,8 @@ void feed_pass(const WinLayout& L, const ClipPlan* plan, const int64_t* len, int
 int next_lane(const nisqa_engine* e) { return e->profiling ? 0 : (int)(e->pass_counter % kLanes); }
 
 // The checks and the plan of a call, all before anything is enqueued: each clip's ClipPlan (its front-end tables built),
-// segment count and status, and for a segments or embeddings call each OK clip's first output row, in clip order
-// (NISQA_DE: the degraded clips only)
+// segment count and status, and for a segments, embeddings or alignment call each OK clip's first output row, in clip
+// order (NISQA_DE: the degraded clips only)
 int plan_call(nisqa_engine* e, Call& c) {
   if (!e) return NISQA_ERR_INVALID;
   if (!e->weights_loaded) return fail(e, NISQA_ERR_STATE, "nisqa_load_weights has not been called");
@@ -2063,7 +2077,7 @@ int plan_call(nisqa_engine* e, Call& c) {
     for (int i = 0; i < n_clips; i += 2)
       if (!plan[i].run || !plan[i + 1].run) plan[i].run = plan[i + 1].run = 0;      // the pair scores NaN
   }
-  if (c.seg || c.emb) {
+  if (c.seg || c.emb || c.al) {
     c.seg_row.assign(n_clips, -1);
     long long rows = 0;
     for (int g = 0; g < n_clips; ++g) {
@@ -2077,6 +2091,9 @@ int plan_call(nisqa_engine* e, Call& c) {
     if (c.emb && c.emb->rows && c.emb->n_rows < rows)
       return fail(e, NISQA_ERR_INVALID, "emb->n_rows = " + std::to_string(c.emb->n_rows) + ": the call has " +
                                             std::to_string(rows) + " segment rows");
+    if (c.al && c.al->n_rows < rows)
+      return fail(e, NISQA_ERR_INVALID, "al->n_rows = " + std::to_string(c.al->n_rows) + ": the call has " +
+                                            std::to_string(rows) + " degraded segment rows");
   }
   return 0;
 }
@@ -2120,7 +2137,7 @@ int run_call(nisqa_engine* e, const Call& c, cudaStream_t* fin_out) {
     in.fmt = c.fmt;
     in.pair_rows = c.win && c.win->n_src == 2;
     in.scores_dev_out = scores_all + (size_t)(in.pair_rows ? i0 / 2 : i0) * e->cfg.n_out;
-    in.seg = c.seg; in.emb = c.emb;
+    in.seg = c.seg; in.emb = c.emb; in.al = c.al;
     in.seg_row = c.seg_row.empty() ? nullptr : c.seg_row.data() + i0;
     in.win = nullptr;
     if (c.win) {
@@ -2570,11 +2587,12 @@ static int check_sources(nisqa_engine* e, const std::string& deg_nm, const nisqa
   return 0;
 }
 
-// nisqa_predict_device_batch (seg == emb == nullptr), nisqa_predict_device_batch_segments and
-// nisqa_predict_device_batch_embeddings
+// nisqa_predict_device_batch (seg == emb == al == nullptr), nisqa_predict_device_batch_segments,
+// nisqa_predict_device_batch_embeddings and nisqa_predict_device_batch_alignment
 static int device_batch_call(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg, const nisqa_device_batch* ref,
                              int32_t target_sr, float* scores_dev, const nisqa_segment_out* seg,
-                             const nisqa_embedding_out* emb, int32_t* n_segments_out, int32_t* status_out) {
+                             const nisqa_embedding_out* emb, int32_t* n_segments_out, int32_t* status_out,
+                             const nisqa_alignment_out* al = nullptr) {
   if (!e) return NISQA_ERR_INVALID;
   if (!e->stream) return fail(e, NISQA_ERR_STATE, "engine was not created successfully");
   if (!deg) return fail(e, NISQA_ERR_INVALID, "deg: null argument");
@@ -2599,7 +2617,7 @@ static int device_batch_call(nisqa_engine* e, void* cuda_stream, const nisqa_dev
     n_model[g] = target_sr > 0 ? nisqa_resample_out_len(ns[g], sr[g], target_sr) : ns[g];
   }
   Call c(n_clips, n_model.data(), target_sr > 0 ? sr_model.data() : sr.data(), fmt, n_segments_out, status_out);
-  c.ingest = &ing; c.scores_dev = scores_dev; c.seg = seg; c.emb = emb;
+  c.ingest = &ing; c.scores_dev = scores_dev; c.seg = seg; c.emb = emb; c.al = al;
   c.target_sr = target_sr; c.n_rec = n_clips; c.rec_n = ns.data(); c.rec_sr = sr.data();
   rc = plan_call(e, c);
   return rc ? rc : enqueue_call(e, cuda_stream, c);
@@ -2616,6 +2634,26 @@ int nisqa_predict_device_batch_segments(nisqa_engine* e, void* cuda_stream, cons
                                         const nisqa_segment_out* seg, int32_t* n_segments_out, int32_t* status_out) {
   if (e && !seg) return fail(e, NISQA_ERR_INVALID, "seg: null argument");
   return device_batch_call(e, cuda_stream, deg, ref, target_sr, scores_dev, seg, nullptr, n_segments_out, status_out);
+}
+
+// The refusals of an alignment call that precede its argument checks: a single-ended engine, a null struct or array
+static int check_alignment_out(nisqa_engine* e, const nisqa_alignment_out* al) {
+  if (!e) return NISQA_ERR_INVALID;
+  if (!e->cfg.double_ended)
+    return fail(e, NISQA_ERR_INVALID, "al: only a double-ended (NISQA_DE) engine aligns a reference to the degraded clip");
+  if (!al) return fail(e, NISQA_ERR_INVALID, "al: null argument");
+  if (!al->ref_seg || !al->weight || !al->centroid || !al->peak)
+    return fail(e, NISQA_ERR_INVALID, "al: null ref_seg / weight / centroid / peak");
+  return 0;
+}
+
+int nisqa_predict_device_batch_alignment(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                                         const nisqa_device_batch* ref, int32_t target_sr, float* scores_dev,
+                                         const nisqa_alignment_out* al, int32_t* n_segments_out, int32_t* status_out) {
+  if (e && !e->stream) return fail(e, NISQA_ERR_STATE, "engine was not created successfully");
+  const int rc = check_alignment_out(e, al);
+  return rc ? rc : device_batch_call(e, cuda_stream, deg, ref, target_sr, scores_dev, nullptr, nullptr, n_segments_out,
+                                     status_out, al);
 }
 
 int nisqa_embedding_width(const nisqa_engine* e, int32_t* width) {
@@ -2677,7 +2715,8 @@ void plan_rows(const nisqa_config& c, int rate, int n_src, const WinList& w, int
 static int windows_call(nisqa_engine* e, void* cuda_stream, const char* nm, const nisqa_device_batch* deg,
                         const nisqa_device_batch* ref, int32_t target_sr, int64_t window, int32_t hop_frames,
                         int32_t margin_frames, float* scores_dev, int64_t n_rows, int32_t* n_segments_out,
-                        int32_t* status_out, int32_t* ref_n_segments_out, int32_t* ref_status_out) {
+                        int32_t* status_out, int32_t* ref_n_segments_out, int32_t* ref_status_out,
+                        const nisqa_alignment_out* al = nullptr) {
   if (target_sr < 0) return fail(e, NISQA_ERR_INVALID, "target_sr");
   IngestSources ing;
   int fmt;
@@ -2725,7 +2764,7 @@ static int windows_call(nisqa_engine* e, void* cuda_stream, const char* nm, cons
   L.n_src = S;
   std::vector<int32_t> srs(N, rate), nseg(N), status(N);
   Call c(N, wl.len.data(), srs.data(), fmt, nseg.data(), status.data());
-  c.ingest = &ing; c.scores_dev = scores_dev; c.win = &L;
+  c.ingest = &ing; c.scores_dev = scores_dev; c.win = &L; c.al = al;
   c.target_sr = target_sr; c.n_rec = S * n_rec; c.rec_n = rs_n.data(); c.rec_sr = rs_sr.data();
   rc = plan_call(e, c);
   if (!rc) rc = enqueue_call(e, cuda_stream, c);
@@ -2757,6 +2796,20 @@ int nisqa_predict_device_window_pairs(nisqa_engine* e, void* cuda_stream, const 
   if (!ref) return fail(e, NISQA_ERR_INVALID, "ref: null argument");
   return windows_call(e, cuda_stream, "deg", deg, ref, target_sr, window, hop_frames, margin_frames, scores_dev, n_rows,
                       n_segments_out, status_out, ref_n_segments_out, ref_status_out);
+}
+
+int nisqa_predict_device_window_pairs_alignment(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                                                const nisqa_device_batch* ref, int32_t target_sr, int64_t window,
+                                                int32_t hop_frames, int32_t margin_frames, float* scores_dev, int64_t n_rows,
+                                                const nisqa_alignment_out* al, int32_t* n_segments_out, int32_t* status_out,
+                                                int32_t* ref_n_segments_out, int32_t* ref_status_out) {
+  if (e && !e->stream) return fail(e, NISQA_ERR_STATE, "engine was not created successfully");
+  const int rc = check_alignment_out(e, al);
+  if (rc) return rc;
+  if (!deg) return fail(e, NISQA_ERR_INVALID, "deg: null argument");
+  if (!ref) return fail(e, NISQA_ERR_INVALID, "ref: null argument");
+  return windows_call(e, cuda_stream, "deg", deg, ref, target_sr, window, hop_frames, margin_frames, scores_dev, n_rows,
+                      n_segments_out, status_out, ref_n_segments_out, ref_status_out, al);
 }
 
 // nisqa_window_counts (n_src 1, margin_frames 0) and nisqa_window_pair_counts (n_src 2)

@@ -92,7 +92,10 @@ struct LstmLayerParams {
 };
 // learned weights of the alignment at td's fan_out W, rows padded to ld = 64 NC with zero rows / columns: AttLuong
 // (wT [ld][ld] k-major, b [ld]) / AttBahdanau (wqyT [ld][256] k-major = Wq^T | Wy^T, bqy [256] = bq | by, v [128])
-struct DeAlignParams { const float* wT; const float* b; const float* wqyT; const float* bqy; const float* v; };
+struct DeAlignParams { const float* wT; const float* b; const float* wqyT; const float* bqy; const float* v; float vb; };
+// An alignment call's outputs (nisqa_alignment_out): degraded row i of clip c at row_off[c] + i; pbias is added to peak
+// (launch_de_align sets it)
+struct DeAlignOut { const long long* row_off; int* ref_seg; float* weight; float* centroid; float* peak; float pbias; };
 struct ResampleClip {
   long long in_off;      // element offset of the clip in the raw input buffer (float32, or int16 scaled by 1/32768)
   long long out_off;     // element offset in the packed float32 output buffer
@@ -215,11 +218,13 @@ void launch_td_sa(cudaStream_t st, int nc, const float* x_in, const float* qkv, 
 // NISQA_DE alignment + fusion over td's rows x_td (W real columns, W <= 512, at a pitch of ld = 64 NC, pad columns zero)
 // into fused [n_rows][nf ld] (part p at column p ld; rows of reference clips untouched).  work: de_align_work_floats(W,
 // align, n_rows) floats (AttLuong / AttBahdanau projections, AttCosine norms); de_align_launches(align) kernels.
+// al (an alignment call, else nullptr): each degraded row's first maximal score, its softmax weight, the softmax-weighted
+// key position and the score (+ AttBahdanau's v bias) to al's arrays
 size_t de_align_work_floats(int W, int align, int n_rows);
 int de_align_launches(int align);
 void launch_de_align(cudaStream_t st, const float* x_td, int W, int n_rows, const ClipDesc* clips, int n_clips,
                      const int* qtile64_prefix, int n_qtiles, int align, int soft, int fuse, const DeAlignParams& A,
-                     float* work, float* fused);
+                     float* work, float* fused, const DeAlignOut* al = nullptr);
 void launch_de_finalize(cudaStream_t st, const ClipDesc* clips, int n_clips, int n_out, float* scores);
 // SkipCNN / DFF rows: n_mels * seg_len features at index m * seg_len + t, zero up to the row stride ld (a multiple of 64)
 void launch_seg_feats(cudaStream_t st, const float* mel, int n_mels, int seg_len, int ld, const int* seg_frame0,

@@ -521,6 +521,10 @@ td_sa_kernel(const float* __restrict__ x_in, const float* __restrict__ qkv, cons
 // resident; per key block the n_sc score chunks of the keys (row-major, pitch 68) and - soft - the value chunks of y the
 // CTA outputs (k-major, pitch 64) stream through one TileStream.  A soft CTA outputs a group of at most G column chunks
 // (blockIdx.y: the group) and recomputes the scores for it, so at most 4 output chunks sit in registers.
+// AL (alignment calls): also the online softmax sum l and position sum c = sum_j exp(s_ij - m) j of every row, rescaled
+// per key block like the soft path's (hard application: besides its running first maximum), and - the blockIdx.y == 0
+// CTA only, the others recompute the same scores - ref_seg = the first maximal key, weight = 1 / l, centroid = c / l,
+// peak = m + pbias (AttBahdanau's v bias, which the softmax drops) at al.row_off[c] + row.
 
 // s[i][j] -= sum_k |A[4ty+i][k] - B[tx+16j][k]|
 __device__ __forceinline__ void absdiff_nt(float (&s)[4][4], const float* __restrict__ A, const float* __restrict__ B, int ty, int tx) {
@@ -584,13 +588,17 @@ constexpr int kDeRing = 3;              // de_align_kernel ring slots
 // shared memory of de_align_kernel: Qs [n_sc][64][68] | Ps [64][68] | ring [kDeRing][64][68]; n_sc <= 8: 204 KB
 constexpr int de_smem_bytes(int n_sc) { return (n_sc + 1 + kDeRing) * kTileF * 4; }
 
-// G: output chunks per soft CTA (hard application runs G = 1 and writes every chunk of y[best])
-template <int G>
+// G: output chunks per soft CTA (hard application runs G = 1 and writes every chunk of y[best]).  Al: empty (the plain
+// instances, whose parameter list stays that of the kernel without alignment outputs) or one DeAlignOut (AL).
+template <typename T> __device__ __forceinline__ const T& first_arg(const T& t) { return t; }
+template <int G, typename... Al>
 __global__ void __launch_bounds__(kNT, G <= 2 ? 2 : 1)
 de_align_kernel(const float* __restrict__ x_td /*[n_seg][ld]*/, int ld, int W, const ClipDesc* __restrict__ clips, int n_clips,
                 const int* __restrict__ qtile_prefix /*64-row tiles*/, int align, int soft, int fuse,
                 const float* __restrict__ qsrc, const float* __restrict__ ksrc, int pld, int n_sc,
-                const float* __restrict__ rnorm, const float* __restrict__ v, float* __restrict__ fused /*[n_seg][nf ld]*/) {
+                const float* __restrict__ rnorm, const float* __restrict__ v, float* __restrict__ fused /*[n_seg][nf ld]*/,
+                Al... al_arg) {
+  constexpr bool AL = sizeof...(Al) > 0;
   extern __shared__ __align__(16) float sm[];
   float* Qs = sm;                          // [n_sc][64][68] query operand of the CTA's degraded steps
   float* Ps = sm + n_sc * kTileF;          // [64][68] softmax numerators (soft attention)
@@ -623,10 +631,14 @@ de_align_kernel(const float* __restrict__ x_td /*[n_seg][ld]*/, int ld, int W, c
   float o[G][4][4];
 #pragma unroll
   for (int n = 0; n < G; ++n) zero_acc(o[n]);
-  float m[4], l[4];
+  float m[4], l[4], cpos[4];
   int best[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) { m[i] = -INFINITY; l[i] = 0.f; best[i] = 0; }
+  if constexpr (AL) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) cpos[i] = 0.f;
+  }
 #pragma unroll 1
   for (int kb = 0; kb < n_kb; ++kb) {
     const int j0 = kb * kT, nkeys = Sy - j0;            // keys >= nkeys of this block do not exist
@@ -670,25 +682,54 @@ de_align_kernel(const float* __restrict__ x_td /*[n_seg][ld]*/, int ld, int W, c
           const int oi = __shfl_xor_sync(0xffffffffu, bi, of);
           if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
         }
+        if constexpr (AL) {                              // (bv: the block's maximum, on all 16 lanes of the row)
+          const float mn = fmaxf(m[i], bv);
+          const float sc = expf(m[i] - mn);
+          float ps = 0.f, pc = 0.f;
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+            if (tx + 16 * j < nkeys) {
+              const float p = expf(s[i][j] - mn);
+              ps += p;
+              pc = fmaf(p, (float)(j0 + tx + 16 * j), pc);
+            }
+          l[i] = l[i] * sc + row_sum(ps);
+          cpos[i] = cpos[i] * sc + row_sum(pc);
+        }
         if (bv > m[i]) { m[i] = bv; best[i] = bi; }       // (strictly greater: an earlier block keeps a tie)
       }
     } else {
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
+        if constexpr (AL) {                              // the first maximal key, as the hard path finds it
+          float bv = -INFINITY; int bi = 0x7fffffff;
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+            if (tx + 16 * j < nkeys && s[i][j] > bv) { bv = s[i][j]; bi = j0 + tx + 16 * j; }
+#pragma unroll
+          for (int of = 8; of > 0; of >>= 1) {
+            const float ov = __shfl_xor_sync(0xffffffffu, bv, of);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, of);
+            if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+          }
+          if (bv > m[i]) best[i] = bi;
+        }
         float bm = -INFINITY;
 #pragma unroll
         for (int j = 0; j < 4; ++j) { if (tx + 16 * j >= nkeys) s[i][j] = -INFINITY; bm = fmaxf(bm, s[i][j]); }
         bm = row_max(bm);
         const float mn = fmaxf(m[i], bm);
         const float sc = expf(m[i] - mn);
-        float ps = 0.f;
+        float ps = 0.f, pc = 0.f;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const float p = expf(s[i][j] - mn);
           ps += p;
+          if constexpr (AL) pc = fmaf(p, (float)(j0 + tx + 16 * j), pc);
           Ps[(4 * ty + i) * kLd + tx + 16 * j] = p;
         }
         l[i] = l[i] * sc + row_sum(ps);
+        if constexpr (AL) cpos[i] = cpos[i] * sc + row_sum(pc);
         m[i] = mn;
 #pragma unroll
         for (int n = 0; n < G; ++n) { o[n][i][0] *= sc; o[n][i][1] *= sc; o[n][i][2] *= sc; o[n][i][3] *= sc; }
@@ -697,6 +738,21 @@ de_align_kernel(const float* __restrict__ x_td /*[n_seg][ld]*/, int ld, int W, c
 #pragma unroll
       for (int n = 0; n < G; ++n)
         if (n < ng) gemm_nn(o[n], Ps, st.acquire(), 64, ty, tx);   // o[n][i][d] += sum_j p[i][j] y[j][64 (c0 + n) + d]
+    }
+  }
+  if constexpr (AL) {
+    const DeAlignOut al = first_arg(al_arg...);
+    if (blockIdx.y == 0 && tx == 0) {
+      const long long r0 = al.row_off[c] + q0 + 4 * ty;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        if (4 * ty + i >= rows_valid) continue;
+        const float inv = 1.0f / l[i];
+        al.ref_seg[r0 + i] = best[i];
+        al.weight[r0 + i] = inv;
+        al.centroid[r0 + i] = cpos[i] * inv;
+        al.peak[r0 + i] = m[i] + al.pbias;
+      }
     }
   }
   // ---- fusion (lib:1402-1417): x from the td rows, y_al from y[best] (hard) or the accumulators (soft)
@@ -838,15 +894,30 @@ void launch_td_in(cudaStream_t st, int nc, const float* feats, const float* WT, 
   }
 }
 
-template <int G>
+template <int G, typename... Al>
 void de_align_instance(cudaStream_t st, dim3 grid, int smem, const float* x_td, int ld, int W, const ClipDesc* clips,
                        int n_clips, const int* qtile64_prefix, int align, int soft, int fuse, const float* q, const float* k,
-                       int pld, int n_sc, const float* rnorm, const float* v, float* fused) {
+                       int pld, int n_sc, const float* rnorm, const float* v, float* fused, Al... al) {
   static unsigned long long cfg = 0;
   if (first_launch_on_device(cfg))
-    cudaFuncSetAttribute(de_align_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, de_smem_bytes(8));
-  de_align_kernel<G><<<grid, kNT, smem, st>>>(x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc,
-                                              rnorm, v, fused);
+    cudaFuncSetAttribute(de_align_kernel<G, Al...>, cudaFuncAttributeMaxDynamicSharedMemorySize, de_smem_bytes(8));
+  de_align_kernel<G, Al...><<<grid, kNT, smem, st>>>(x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k,
+                                                     pld, n_sc, rnorm, v, fused, al...);
+}
+template <int G>
+void de_align_select(const DeAlignOut* al, cudaStream_t st, dim3 grid, int smem, const float* x_td, int ld, int W,
+                     const ClipDesc* clips, int n_clips, const int* qtile64_prefix, int align, int soft, int fuse,
+                     const float* q, const float* k, int pld, int n_sc, const float* rnorm, const float* v, float vb,
+                     float* fused) {
+  if (!al) {
+    de_align_instance<G>(st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, rnorm,
+                         v, fused);
+    return;
+  }
+  DeAlignOut o = *al;
+  o.pbias = align == NISQA_DE_ALIGN_BAHDANAU ? vb : 0.f;
+  de_align_instance<G>(st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, rnorm,
+                       v, fused, o);
 }
 
 size_t de_align_work_floats(int W, int align, int n_rows) {
@@ -860,7 +931,7 @@ int de_align_launches(int align) {
 
 void launch_de_align(cudaStream_t st, const float* x_td, int W, int n_rows, const ClipDesc* clips, int n_clips,
                      const int* qtile64_prefix, int n_qtiles, int align, int soft, int fuse, const DeAlignParams& A,
-                     float* work, float* fused) {
+                     float* work, float* fused, const DeAlignOut* al) {
   const int NC = (W + 63) / 64, ld = 64 * NC;
   const float *q = x_td, *k = x_td;
   int pld = ld, n_sc = NC;
@@ -878,10 +949,10 @@ void launch_de_align(cudaStream_t st, const float* x_td, int W, int n_rows, cons
   const dim3 grid(n_qtiles, soft ? (NC + G - 1) / G : 1);
   const int smem = de_smem_bytes(n_sc);
   switch (G) {
-    case 1: de_align_instance<1>(st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, work, A.v, fused); break;
-    case 2: de_align_instance<2>(st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, work, A.v, fused); break;
-    case 3: de_align_instance<3>(st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, work, A.v, fused); break;
-    default: de_align_instance<4>(st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, work, A.v, fused); break;
+    case 1: de_align_select<1>(al, st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, work, A.v, A.vb, fused); break;
+    case 2: de_align_select<2>(al, st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, work, A.v, A.vb, fused); break;
+    case 3: de_align_select<3>(al, st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, work, A.v, A.vb, fused); break;
+    default: de_align_select<4>(al, st, grid, smem, x_td, ld, W, clips, n_clips, qtile64_prefix, align, soft, fuse, q, k, pld, n_sc, work, A.v, A.vb, fused); break;
   }
 }
 

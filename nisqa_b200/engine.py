@@ -43,6 +43,7 @@ EXPORTS = [
     "nisqa_feed_create", "nisqa_feed_rows", "nisqa_feed_push", "nisqa_feed_device_bytes", "nisqa_feed_destroy",
     "nisqa_embedding_width", "nisqa_predict_device_batch_embeddings", "nisqa_window_pair_counts",
     "nisqa_predict_device_window_pairs", "nisqa_feed_pair_create", "nisqa_feed_pair_rows", "nisqa_feed_pair_push",
+    "nisqa_predict_device_batch_alignment", "nisqa_predict_device_window_pairs_alignment",
 ]
 
 
@@ -181,6 +182,12 @@ class NisqaSegmentOut(C.Structure):
     _fields_ = [("scores", C.c_void_p), ("weights", C.c_void_p), ("n_rows", C.c_int64)]
 
 
+class NisqaAlignmentOut(C.Structure):
+    """nisqa_alignment_out: device [n_rows] ref_seg (int32), weight, centroid and peak (fp32) of NISQA_DE's alignment"""
+    _fields_ = [("ref_seg", C.c_void_p), ("weight", C.c_void_p), ("centroid", C.c_void_p), ("peak", C.c_void_p),
+                ("n_rows", C.c_int64)]
+
+
 class NisqaTensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", C.POINTER(C.c_float)), ("ndim", C.c_int32),
                 ("dims", C.c_int64 * 4)]
@@ -264,6 +271,13 @@ def load_library(path=None):
     lib.nisqa_predict_device_window_pairs.argtypes = [vp, vp, dbp, dbp, C.c_int32, C.c_int64, C.c_int32, C.c_int32, vp,
                                                       C.c_int64, i32p, i32p, i32p, i32p]
     lib.nisqa_predict_device_window_pairs.restype = C.c_int
+    lib.nisqa_predict_device_batch_alignment.argtypes = [vp, vp, dbp, dbp, C.c_int32, vp, C.POINTER(NisqaAlignmentOut),
+                                                         i32p, i32p]
+    lib.nisqa_predict_device_batch_alignment.restype = C.c_int
+    lib.nisqa_predict_device_window_pairs_alignment.argtypes = [vp, vp, dbp, dbp, C.c_int32, C.c_int64, C.c_int32, C.c_int32,
+                                                                vp, C.c_int64, C.POINTER(NisqaAlignmentOut), i32p, i32p,
+                                                                i32p, i32p]
+    lib.nisqa_predict_device_window_pairs_alignment.restype = C.c_int
     lib.nisqa_window_pair_counts.argtypes = [C.POINTER(NisqaConfig), C.c_int64, C.c_int64, C.c_int32, C.c_int64, C.c_int32,
                                              C.c_int32, i64p, i32p, i32p, i32p, i32p, C.c_int64]
     lib.nisqa_window_pair_counts.restype = C.c_int
@@ -856,6 +870,13 @@ class Engine(object):
         emb = NisqaEmbeddingOut(pooled=pooled_ptr or None, rows=rows_ptr or None, n_rows=int(n_rows))
         return self._device_batch(stream, deg, scores_dev_ptr, ref, target_sr, emb)
 
+    def predict_device_batch_alignment(self, stream, deg, ref, scores_dev_ptr, al, target_sr=0):
+        """:meth:`predict_device_batch` of a NISQA_DE engine that also writes the alignment of every degraded segment to
+        ``al``, a :class:`NisqaAlignmentOut` of device arrays (one row per segment of every OK degraded clip in clip
+        order; include/nisqa_b200.h nisqa_alignment_out).  Raises EngineError, with nothing enqueued, for a refused call
+        (a single-ended engine, a null array, a too-small ``al.n_rows``)."""
+        return self._device_batch(stream, deg, scores_dev_ptr, ref, target_sr, al)
+
     def predict_device_windows(self, stream, rec, scores_dev_ptr, n_rows, window, hop_frames, target_sr=0):
         """Windows of the recordings ``rec`` (a :func:`device_batch` tuple) ordered on ``stream``: ``window`` samples and a
         hop of ``hop_frames`` mel frames at the model rate (``target_sr``, else the batch's rate), the scores of every
@@ -888,6 +909,22 @@ class Engine(object):
             self.h, C.c_void_p(stream or None), C.byref(deg[0]), C.byref(ref[0]), int(target_sr or 0), int(window),
             int(hop_frames), int(margin_frames), C.c_void_p(scores_dev_ptr), int(n_rows),
             *[_ptr(a, C.c_int32) for a in out]), "nisqa_predict_device_window_pairs")
+        return tuple(out)
+
+    def predict_device_window_pairs_alignment(self, stream, deg, ref, scores_dev_ptr, n_rows, window, hop_frames,
+                                              margin_frames, al, target_sr=0):
+        """:meth:`predict_device_window_pairs` that also writes the alignment of every segment of each pair's degraded
+        window to ``al`` (:class:`NisqaAlignmentOut`; the pairs in order, include/nisqa_b200.h
+        nisqa_predict_device_window_pairs_alignment).  Returns what :meth:`predict_device_window_pairs` returns."""
+        if target_sr:
+            from . import resample as _rs
+            _rs.out_len(1, 1, 1)                                      # the interpolation table is set once
+        n = max(int(n_rows), 0)
+        out = [np.empty(n, dtype=np.int32) for _ in range(4)]
+        self._check(self.lib.nisqa_predict_device_window_pairs_alignment(
+            self.h, C.c_void_p(stream or None), C.byref(deg[0]), C.byref(ref[0]), int(target_sr or 0), int(window),
+            int(hop_frames), int(margin_frames), C.c_void_p(scores_dev_ptr), int(n_rows), C.byref(al),
+            *[_ptr(a, C.c_int32) for a in out]), "nisqa_predict_device_window_pairs_alignment")
         return tuple(out)
 
     def feed_create(self, n_feeds, sample_rate, window, hop_frames, max_push):
@@ -963,6 +1000,9 @@ class Engine(object):
         outs = (nseg.ctypes.data_as(C.POINTER(C.c_int32)), status.ctypes.data_as(C.POINTER(C.c_int32)))
         if out is None:
             self._check(self.lib.nisqa_predict_device_batch(*args, *outs), "nisqa_predict_device_batch")
+        elif isinstance(out, NisqaAlignmentOut):
+            self._check(self.lib.nisqa_predict_device_batch_alignment(*args, C.byref(out), *outs),
+                        "nisqa_predict_device_batch_alignment")
         elif isinstance(out, NisqaSegmentOut):
             self._check(self.lib.nisqa_predict_device_batch_segments(*args, C.byref(out), *outs),
                         "nisqa_predict_device_batch_segments")

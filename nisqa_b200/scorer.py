@@ -19,6 +19,10 @@ each scored as the clip cut out of the recording would be (``nisqa_predict_devic
 scores window pairs of a recording and its reference: ``scorer.windows(wave, 48000, 10.0, 1.0, reference=ref)``
 (``nisqa_predict_device_window_pairs``).
 
+``scorer.align(wave, 48000, ref)`` reports a NISQA_DE checkpoint's time alignment: for every degraded segment the
+reference segment it matched, how sharp the match is, and the delay in seconds (``nisqa_predict_device_batch_alignment``;
+with ``window_s`` of window pairs, ``nisqa_predict_device_window_pairs_alignment``).
+
 ``scorer.feed(256, 48000, 10.0, 1.0)`` scores live sources as their audio arrives: ``feed.push(chunk)`` appends a chunk to
 every source and returns the windows it completed, with the scores ``windows`` gives on the whole recording
 (``nisqa_feed_push``).  A NISQA_DE checkpoint scores live (degraded, reference) pairs:
@@ -49,6 +53,16 @@ Windows = collections.namedtuple("Windows", ["scores", "counts", "t_start", "t_e
 # [N] seconds and n_segments / status int32 [N], and the same of the reference windows (ref_*), host arrays
 WindowPairs = collections.namedtuple("WindowPairs", ["scores", "counts", "t_start", "t_end", "n_segments", "status",
                                                      "ref_t_start", "ref_t_end", "ref_n_segments", "ref_status"])
+# Scorer.align: scores [B, n_cols] (as Scorer.__call__); ref_seg int32, weight / centroid / peak float32 [N] CUDA tensors
+# (the rows of clip b follow those of the clips before it, counts[b] of them); t_start / ref_t_start / delay_s /
+# centroid_delay_s float64 [N] host arrays, seconds
+Alignment = collections.namedtuple("Alignment", ["scores", "ref_seg", "weight", "centroid", "peak", "counts", "t_start",
+                                                 "ref_t_start", "delay_s", "centroid_delay_s"])
+# Scorer.align with window_s: the fields of Alignment (scores, counts: of the window pairs, counts[k] rows of pair k),
+# window int64 [N] (the row's pair), and the pair columns of WindowPairs, one entry per pair, as pair_* (pair_counts:
+# pairs per recording)
+AlignmentWindows = collections.namedtuple("AlignmentWindows", Alignment._fields + ("window",) + tuple(
+    "pair_" + f for f in WindowPairs._fields[1:]))
 # Feed.push: scores [N, n_cols] CUDA tensor of the windows the push completed, by feed then window index; feed int32 [N],
 # index int64 [N] (window k of the feed's current recording), t_start / t_end float64 [N] seconds, n_segments / status
 # int32 [N] host arrays
@@ -187,6 +201,13 @@ class Scorer(object):
         min(T_ref, k H + W + M)) cut out as clips.  A pair whose degraded or reference window is too short (or empty:
         k H - M >= T_ref) scores NaN; ``status`` and ``ref_status`` tell which.
         """
+        return self._windows(wave, sample_rate, window_s, window_hop_s, lengths, channel, reference, reference_lengths,
+                             reference_sample_rate, reference_margin_s, None)
+
+    def _windows(self, wave, sample_rate, window_s, window_hop_s, lengths, channel, reference, reference_lengths,
+                 reference_sample_rate, reference_margin_s, alignment):
+        """windows(); alignment (window pairs only): None, or alignment(n_segments, status) of the pairs -> the
+        NisqaAlignmentOut the call also writes"""
         from . import resample as RS
         m = reference_margin_s
         if isinstance(m, bool) or not isinstance(m, numbers.Real) or not np.isfinite(m) or m < 0:
@@ -245,14 +266,99 @@ class Scorer(object):
             parts.append((t0, t1) + tuple(cols))
         N = int(sum(counts))
         out = torch.empty((N, len(self.columns)), dtype=torch.float32, device=self.device)
-        if N and ref is None:
-            self.engine.predict_device_windows(self._stream(), deg, out.data_ptr(), N, W, hop_frames, target_sr=self.target_sr)
-        elif N:
-            self.engine.predict_device_window_pairs(self._stream(), deg, ref, out.data_ptr(), N, W, hop_frames, margin_frames,
-                                                    target_sr=self.target_sr)
         types = (np.float64, np.float64, np.int32, np.int32) * (1 if ref is None else 2)
         cols = [np.concatenate([p[i] for p in parts]).astype(t) if parts else np.zeros(0, t) for i, t in enumerate(types)]
+        if N and ref is None:
+            self.engine.predict_device_windows(self._stream(), deg, out.data_ptr(), N, W, hop_frames, target_sr=self.target_sr)
+        elif N and alignment is None:
+            self.engine.predict_device_window_pairs(self._stream(), deg, ref, out.data_ptr(), N, W, hop_frames, margin_frames,
+                                                    target_sr=self.target_sr)
+        elif N:
+            self.engine.predict_device_window_pairs_alignment(self._stream(), deg, ref, out.data_ptr(), N, W, hop_frames,
+                                                              margin_frames, alignment(cols[2], cols[3]),
+                                                              target_sr=self.target_sr)
         return Windows(out, counts, *cols) if ref is None else WindowPairs(out, counts, *cols)
+
+    def align(self, wave, sample_rate, reference, lengths=None, channel=None, reference_lengths=None,
+              reference_sample_rate=None, window_s=None, window_hop_s=None, reference_margin_s=0.0):
+        """NISQA_DE's time alignment of every degraded segment -> :data:`Alignment`, or with ``window_s`` of every segment
+        of each window pair's degraded window -> :data:`AlignmentWindows`.  Takes the arguments of ``__call__`` (of
+        ``windows`` with a ``window_s``) and checks them alike; a single-ended checkpoint raises ValueError.
+
+        scores        : the values ``__call__`` (``windows(..., reference=)``) returns
+        ref_seg       : int32 [N] CUDA tensor, the reference segment with the first maximal alignment score (under hard
+                        application: the one the model fused); -1 where the pair scores NaN
+        weight        : float32 [N] CUDA tensor, that segment's softmax weight: how sharp the match is
+        centroid      : float32 [N] CUDA tensor, the softmax-weighted reference segment position
+        peak          : float32 [N] CUDA tensor, the maximal score as the alignment module computes it (cosine: the
+                        cosine similarity)
+        counts        : host list, the rows of each clip (window mode: of each pair)
+        t_start       : float64 [N] seconds, the degraded segment's start in its recording
+        ref_t_start   : float64 [N] seconds, the start of reference segment ref_seg in the reference recording
+        delay_s       : ref_t_start - t_start;  centroid_delay_s: the centroid's position in seconds minus t_start
+        Segment i starts i * ms_seg_hop_length * hop / rate seconds into its clip, each side at its own model rate and hop;
+        window mode adds k H / rate on the degraded side and max(0, k H - M) / rate on the reference side of pair k.
+        """
+        if not self.double_ended:
+            raise ValueError("align: only a double-ended (NISQA_DE) checkpoint aligns a reference to the degraded signal")
+        if window_s is not None or window_hop_s is not None:
+            return self._align_windows(wave, sample_rate, reference, lengths, channel, reference_lengths,
+                                       reference_sample_rate, window_s, window_hop_s, reference_margin_s)
+        if reference_margin_s != 0:
+            raise ValueError("reference_margin_s=%r: a margin widens reference windows; pass window_s and window_hop_s"
+                             % (reference_margin_s,))
+        deg, ref, counts = self._arguments(wave, sample_rate, lengths, channel, reference, reference_lengths,
+                                           reference_sample_rate)
+        out = self._scores_buffer(deg, ref)
+        n_rows = int(sum(counts))
+        al, outs = self._alignment_buffers(n_rows)
+        if out.shape[0]:
+            self.engine.predict_device_batch_alignment(self._stream(), deg, ref, out.data_ptr(), al, target_sr=self.target_sr)
+        i = np.concatenate([np.arange(c, dtype=np.float64) for c in counts]) if counts else np.zeros(0)
+        z = np.zeros(n_rows)
+        cols = self._alignment_times(outs, i, deg[0].sample_rate, ref[0].sample_rate, z, z)
+        return Alignment(self._clip_rows(out, ref), *outs, list(counts), *cols)
+
+    def _align_windows(self, wave, sample_rate, reference, lengths, channel, reference_lengths, reference_sample_rate,
+                       window_s, window_hop_s, reference_margin_s):
+        made = []
+
+        def buffers(n_segments, status):            # the rows: every segment of each pair's OK degraded window
+            counts = np.where(status == E.CLIP_OK, n_segments, 0).astype(np.int64)
+            made.append((counts,) + self._alignment_buffers(int(counts.sum())))
+            return made[0][1]
+        pairs = self._windows(wave, sample_rate, window_s, window_hop_s, lengths, channel, reference, reference_lengths,
+                              reference_sample_rate, reference_margin_s, buffers)
+        if not made:                                 # (no pair: nothing was enqueued)
+            buffers(pairs.n_segments, pairs.status)
+        counts, _, outs = made[0]
+        n_rows = int(counts.sum())
+        window = np.repeat(np.arange(len(counts), dtype=np.int64), counts)
+        i = np.concatenate([np.arange(c, dtype=np.float64) for c in counts]) if n_rows else np.zeros(0)
+        rate = self.target_sr or int(sample_rate)
+        cols = self._alignment_times(outs, i, rate, rate, pairs.t_start[window], pairs.ref_t_start[window])
+        return AlignmentWindows(pairs.scores, *outs, counts.tolist(), *cols, window, *pairs[1:])
+
+    def _alignment_buffers(self, n_rows):
+        outs = (torch.empty(n_rows, dtype=torch.int32, device=self.device),) + tuple(
+            torch.empty(n_rows, dtype=torch.float32, device=self.device) for _ in range(3))
+        al = E.NisqaAlignmentOut(*[t.data_ptr() or None for t in outs], n_rows)
+        return al, outs
+
+    def _alignment_times(self, outs, i, sr, ref_sr, off, ref_off):
+        """-> (t_start, ref_t_start, delay_s, centroid_delay_s) of the rows: segment i of the degraded side starts at
+        off + i seg_hop hop / rate, reference segment j at ref_off + j seg_hop ref_hop / ref_rate (each side at its own
+        model rate and hop).  Waits for the alignment (a device-to-host copy of ref_seg and centroid)."""
+        a = self.args
+        rate, ref_rate = self.target_sr or int(sr), self.target_sr or int(ref_sr)
+        step = a["ms_seg_hop_length"] * int(rate * a["ms_hop_length"]) / rate
+        ref_step = a["ms_seg_hop_length"] * int(ref_rate * a["ms_hop_length"]) / ref_rate
+        j = outs[0].cpu().numpy().astype(np.float64)
+        j[j < 0] = np.nan
+        cen = outs[2].cpu().numpy().astype(np.float64)
+        t_start = off + i * step
+        ref_t_start = ref_off + j * ref_step
+        return t_start, ref_t_start, ref_t_start - t_start, ref_off + cen * ref_step - t_start
 
     def feed(self, n_feeds, sample_rate, window_s, window_hop_s, channel=None, max_push_s=None, reference=None,
              reference_margin_s=0.0, max_skew_s=None):

@@ -12,6 +12,8 @@ and the same option names, so existing invocations keep working:
     python run_predict.py --mode predict_dir ... --output_dir out --window_s 10 --window_hop_s 1   (out/NISQA_windows.csv)
     python run_predict.py --mode predict_csv --pretrained_model de.tar --csv_file t.csv --csv_deg deg --csv_ref ref \
         --output_dir out --window_s 10 --window_hop_s 1 --reference_margin_s 0.5   (NISQA_DE window pairs)
+    python run_predict.py --mode predict_csv --pretrained_model de.tar --csv_file t.csv --csv_deg deg --csv_ref ref \
+        --output_dir out --alignment   (+ out/NISQA_alignment.csv: each degraded segment's reference segment and delay)
 """
 import argparse
 
@@ -52,6 +54,10 @@ def parse_args(argv=None):
     parser.add_argument("--embeddings", action="store_true",
                         help="also write NISQA_embeddings.npz into output_dir: each file's pooled vector under every "
                              "pooling head, the input of its last Linear (single process only)")
+    parser.add_argument("--alignment", action="store_true",
+                        help="NISQA_DE: also write NISQA_alignment.csv into output_dir: for every degraded segment (of "
+                             "every window pair with --window_s) the reference segment it matched, the delay in seconds "
+                             "and the match's weight and score (single process only)")
     parser.add_argument("--window_s", type=float, default=None,
                         help="score every file as a timeline of windows of this many seconds (with --window_hop_s) and "
                              "write NISQA_windows.csv into output_dir; files of any length (single process only)")
