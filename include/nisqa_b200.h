@@ -356,6 +356,40 @@ NISQA_API int  nisqa_predict_device_batch_alignment(nisqa_engine* e, void* cuda_
                                                     const nisqa_alignment_out* al, int32_t* n_segments_out,
                                                     int32_t* status_out);
 
+/* NISQA_DE pairs whose references repeat (a codec, bitrate or network sweep scoring one source under many conditions):
+ * pair p is deg clip p and ref clip ref_index[p] (host [deg->n_clips], each in 0 .. ref->n_clips - 1).  Each reference a
+ * pass needs is computed once in that pass - ingest, ms_sr conversion (once per call), front end, framewise model, td and
+ * td_2 - and every pair that names it reads those rows; every pair scores bit for bit what nisqa_predict_device_batch
+ * gives the replicated (deg, ref[ref_index]) batch.  A reference that no pair names is neither ingested nor computed.
+ * Outputs are compact, one row per pair: scores_dev [deg->n_clips][n_out]; seg / emb / al optional (NULL), with the row
+ * tables of the nisqa_predict_device_batch_{segments,embeddings,alignment} calls (degraded segments only),
+ * emb->pooled [deg->n_clips][n_out][width].  n_segments_out / status_out host [deg->n_clips] (the degraded clips);
+ * ref_n_segments_out / ref_status_out host [ref->n_clips] (may be NULL), host arithmetic for every reference.  A pair
+ * whose degraded clip or reference is too short or too long scores NaN.  The stream contract of
+ * nisqa_predict_device_batch.  NISQA_ERR_INVALID, naming the argument, before anything is enqueued for: a single-ended
+ * engine, no reference, a NULL or out-of-range ref_index, an output's n_rows too small, and whatever
+ * nisqa_predict_device_batch refuses except that ref->n_clips may differ from deg->n_clips.
+ * nisqa_stage_dump after a one-pass call: the rows in pass slot order, i.e. pair p's degraded rows followed, when p is
+ * the first pair of the pass that names its reference, by that reference's rows; each reference's rows appear once. */
+NISQA_API int  nisqa_predict_device_batch_shared_ref(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                                                     const nisqa_device_batch* ref, const int32_t* ref_index,
+                                                     int32_t target_sr, float* scores_dev, const nisqa_segment_out* seg,
+                                                     const nisqa_embedding_out* emb, const nisqa_alignment_out* al,
+                                                     int32_t* n_segments_out, int32_t* status_out,
+                                                     int32_t* ref_n_segments_out, int32_t* ref_status_out);
+
+/* nisqa_submit_pcm for pairs with shared references from HOST memory (predict_csv): n_pairs degraded clips, n_refs
+ * references, ref_index host [n_pairs]; each reference a pass needs is uploaded and computed once in that pass.
+ * scores_out [n_pairs][n_out]; n_segments_out / status_out [n_pairs], ref_n_segments_out / ref_status_out [n_refs] (may
+ * be NULL), valid on return.  Waited with nisqa_wait, abandoned with nisqa_drain, the same staging / in-flight rules as
+ * nisqa_submit_pcm.  The refusals of nisqa_predict_device_batch_shared_ref's pairing. */
+NISQA_API int  nisqa_submit_pcm_pairs(nisqa_engine* e, int n_pairs, const void* const* pcm, const int64_t* n_samples,
+                                      const int32_t* sample_rate, int n_refs, const void* const* ref_pcm,
+                                      const int64_t* ref_n_samples, const int32_t* ref_sample_rate,
+                                      const int32_t* ref_index, int sample_fmt, float* scores_out,
+                                      int32_t* n_segments_out, int32_t* status_out, int32_t* ref_n_segments_out,
+                                      int32_t* ref_status_out, int64_t* ticket);
+
 /* Recordings of any length scored as a timeline of overlapping windows, each window scored exactly as the clip cut out of
  * the recording would be (its own reflect padding, top_db maximum, segment count and status).  At the model rate sr
  * (target_sr when set, else the batch's sample_rate; an ms_sr checkpoint converts each WHOLE recording first) a

@@ -170,24 +170,34 @@ def _load_batch_resampled(ds, paths, sr, nf, target, pool, slot, n_threads):
 
 
 def _load_batch_de(ds, batch):
-    """Double-ended rows (lib:2132-2156): clip 2j = degraded file (``ms_channel`` applies), clip 2j + 1 = its reference
-    (always the mono mix: the reference call passes no ``ms_channel``, lib:2146-2154); the engine takes the pairs in
-    this order.  Mixed sample formats / ``ms_sr`` go through float32."""
-    clips, srs = [], []
+    """Double-ended rows (lib:2132-2156): the degraded files (``ms_channel`` applies) and each distinct reference file of
+    the batch once (always the mono mix: the reference call passes no ``ms_channel``, lib:2146-2154), in the order the
+    rows first name them; ``ms_sr`` converts each decoded file once.  -> (degraded clips, their rates, reference clips,
+    their rates, ref_index: each row's reference).  Mixed sample formats go through float32 (submit_pcm_pairs)."""
     target = ds.target_sr()
+
+    def load(path, ch):
+        y, sr = read_wav(path, ch)
+        if target is not None and sr != target:
+            try:
+                y, sr = nb_resample.resample(y, sr, target), target
+            except Exception:
+                raise ValueError("Could not load file {}".format(path))
+        return np.ascontiguousarray(y), int(sr)
+
+    clips, srs, refs, ref_srs, ref_index, seen = [], [], [], [], [], {}
     for i in batch:
-        for path, ch in ((ds.file_path(int(i)), ds.ms_channel), (ds.file_path_ref(int(i)), None)):
-            y, sr = read_wav(path, ch)
-            if target is not None and sr != target:
-                try:
-                    y, sr = nb_resample.resample(y, sr, target), target
-                except Exception:
-                    raise ValueError("Could not load file {}".format(path))
-            clips.append(np.ascontiguousarray(y))
-            srs.append(int(sr))
-    if any(c.dtype != clips[0].dtype for c in clips):
-        clips = [c if c.dtype == np.float32 else c.astype(np.float32) / np.float32(32768.0) for c in clips]
-    return clips, srs
+        y, sr = load(ds.file_path(int(i)), ds.ms_channel)
+        clips.append(y)
+        srs.append(sr)
+        path = ds.file_path_ref(int(i))
+        if path not in seen:
+            seen[path] = len(refs)
+            y, sr = load(path, None)
+            refs.append(y)
+            ref_srs.append(sr)
+        ref_index.append(seen[path])
+    return clips, srs, refs, ref_srs, ref_index
 
 
 def _predict_rows(engine, ds, rows, bs, num_workers):
@@ -203,15 +213,35 @@ def _predict_rows(engine, ds, rows, bs, num_workers):
     n_threads = max(1, min(int(num_workers) if num_workers else 1, max(1, nb_dist.usable_cpus() // 2)))
 
     de = getattr(ds, "double_ended", False)
-    per_row = 2 if de else 1          # a double-ended row is a (degraded, reference) pair of clips
+    order = np.arange(len(rows))
+    if de:
+        # a double-ended row is a (degraded, reference) pair; rows that share a reference file (a condition sweep) are
+        # submitted next to each other, so that a batch decodes, uploads and computes that reference once.  The stable
+        # sort keeps CSV order among them; the scores go back to the given row order.
+        order = np.argsort(np.array([ds.file_path_ref(int(i)) for i in rows], dtype=object), kind="stable")
+        batches = [np.asarray(rows)[order[i:i + bs]] for i in range(0, len(rows), bs)]
 
     def finish(job):
-        handle, batch, clips, srs, pos = job
+        handle, batch, clips, srs, pos, shared = job
         scores, nseg, status = engine.wait(handle)
+        # (the reference names the degraded file for either signal, lib:2187-2192)
+        if shared:      # one score per pair; the references' statuses come apart
+            refs, ref_srs, ref_index = shared
+            ref_nseg, ref_status = handle[4], handle[5]
+            for j, st in enumerate(status):
+                u = ref_index[j]
+                if st != nb_engine.CLIP_OK:
+                    _raise_for_status(ds, engine, int(batch[j]), clips[j].shape[0], srs[j], int(nseg[j]), int(st))
+                if ref_status[u] != nb_engine.CLIP_OK:
+                    _raise_for_status(ds, engine, int(batch[j]), refs[u].shape[0], ref_srs[u], int(ref_nseg[u]),
+                                      int(ref_status[u]))
+            out[order[pos:pos + len(batch)]] = scores
+            return
+        per_row = 2 if de else 1          # (a double-ended row: the clips of its (degraded, reference) pair)
         for j, st in enumerate(status):
-            if st != nb_engine.CLIP_OK:      # (the reference names the degraded file for either signal, lib:2187-2192)
+            if st != nb_engine.CLIP_OK:
                 _raise_for_status(ds, engine, int(batch[j // per_row]), clips[j].shape[0], srs[j], int(nseg[j]), int(st))
-        out[pos:pos + len(batch)] = scores[::per_row]
+        out[order[pos:pos + len(batch)]] = scores[::per_row]
 
     DEPTH = 3                         # batches being decoded ahead of the GPU
     FLIGHT = 5                        # submissions kept in flight on the engine (it has 6 staging slots)
@@ -234,16 +264,30 @@ def _predict_rows(engine, ds, rows, bs, num_workers):
             top_up()
             pos = 0
             for b, batch in enumerate(batches):
-                clips, srs = pending.pop(0).result()
+                shared = None
+                if de:
+                    clips, srs, refs, ref_srs, ref_index = pending.pop(0).result()
+                    if len(refs) < len(clips):      # a reference repeats: computed once per engine pass
+                        shared = (refs, ref_srs, ref_index)
+                    else:                           # every reference once: the (degraded, reference) clip pairs
+                        clips = [c for j, u in enumerate(ref_index) for c in (clips[j], refs[u])]
+                        srs = [r for j, u in enumerate(ref_index) for r in (srs[j], ref_srs[u])]
+                        if any(c.dtype != clips[0].dtype for c in clips):
+                            clips = [c if c.dtype == np.float32 else c.astype(np.float32) / np.float32(32768.0)
+                                     for c in clips]
+                else:
+                    clips, srs = pending.pop(0).result()
                 target = ds.target_sr()
-                if target is not None and not de and any(sr != target for sr in srs):
+                if shared:
+                    handle = engine.submit_pcm_pairs(clips, srs, refs, ref_srs, ref_index)
+                elif target is not None and not de and any(sr != target for sr in srs):
                     # ms_sr checkpoint (lib:2300-2304): the clips travel at their native rates and are converted on
                     # the device (csrc/resample_gpu.cu), where the predict path picks them up - one synchronous call
                     handle = (None,) + tuple(engine.predict_pcm_resampled(clips, srs, target))
                     srs = [target] * len(srs)
                 else:
                     handle = engine.submit_pcm(clips, srs)      # asynchronous: H2D + kernels enqueued
-                in_flight.append((handle, batch, clips, srs, pos))
+                in_flight.append((handle, batch, clips, srs, pos, shared))
                 pos += len(batch)
                 if len(in_flight) >= FLIGHT:
                     finish(in_flight.pop(0))

@@ -25,8 +25,12 @@ struct ClipDesc {
   int pair_off;        // first frame-pair work item of this clip
   int n_seg;           // segments ("n_wins" after seg_hop, lib:2271-2273)
   int seg_off;         // first segment row of this clip in the segment-major buffers
-  int pad_;
+  int ref_clip;        // NISQA_DE, degraded clip c: the pass slot whose rows are its pair's reference (c + 1, or in a
+                       // shared-reference call the slot of that reference's first pair in the pass)
+  int src_clip;        // device ingest: the clip's position in IngestSources order (clip src_clip / n_src of source
+                       // src_clip % n_src); in the struct's tail padding
 };
+static_assert(sizeof(ClipDesc) == 56, "ClipDesc: ref_clip and src_clip fill the layout of the former padding");
 
 // Per-sample-rate front-end tables (device pointers).
 struct FbTables {

@@ -129,8 +129,9 @@ struct Stage {
   DevBuf spans;          // windows call: the pass's recording spans (WinSpan)
   DevBuf fwins;          // feed push: the pass's windows (FeedWin)
   DevBuf pair_scores;    // window-pairs call: the pass's (degraded, reference) score rows, before the compact copy
+  DevBuf pair_pooled;    // shared-reference embeddings call: the pass's pooled vectors, before the compact copy
   void release() {
-    DevBuf* all[] = {&pcm, &clips, &prefixes, &clipmax, &seg_row, &spans, &fwins, &pair_scores};
+    DevBuf* all[] = {&pcm, &clips, &prefixes, &clipmax, &seg_row, &spans, &fwins, &pair_scores, &pair_pooled};
     for (auto* b : all) b->release();
     h_tables.release();
     if (ev_copied) cudaEventDestroy(ev_copied);
@@ -1278,6 +1279,14 @@ struct Call {
   int64_t* ticket = nullptr;
   cudaEvent_t ready = nullptr;
   WinLayout* win = nullptr;           // a windows call or feed push
+  // a shared-reference call (NISQA_DE): clip 2p + 1 is a slot of pair p's reference ref_index[p] (of n_refs).  Each pass
+  // computes a reference once, in the slot of its first running pair there; the pass's other pairs of that reference get
+  // alias slots (nothing computed, ClipDesc.ref_clip names the real slot).  The scores are compact, one row per pair.
+  const int32_t* ref_index = nullptr;
+  int n_refs = 0;
+  const int* src_clip = nullptr;      // the caller's batch: [n_clips] each clip's position in IngestSources order (nullptr: g)
+  const int* rec_src = nullptr;       // ms_sr: [n_rec] each recording's position in IngestSources order (nullptr: its index)
+  const int* clip_rec = nullptr;      // ms_sr: [n_clips] the converted recording each clip reads (nullptr: recording g)
   std::vector<ClipPlan> plan;         // [n_clips]
   std::vector<long long> seg_row;     // segments / embeddings / alignment call: each clip's first output row (-1: none)
   Call(int n, const int64_t* ns, const int32_t* sr, int fmt_, int32_t* n_seg, int32_t* st)
@@ -1293,13 +1302,17 @@ struct PassInput {
   const void* const* host_pcm;        // per-clip host pointers, or
   const void* dev_pcm; const int64_t* dev_off;   // packed device buffer + element offsets, or
   const IngestSources* ingest; int first_clip;   // the caller's strided device batch (clips first_clip.. of the call)
+  const int* src_clip = nullptr;      // [n_clips] the clips' positions in IngestSources order (nullptr: first_clip + i)
+  const int* ref_clip = nullptr;      // NISQA_DE: [n_clips] ClipDesc.ref_clip (nullptr: i + 1); an odd slot that its pair
+                                      // does not name is an alias slot (a shared-reference call)
   cudaEvent_t ready;                  // when set, the lane waits for it before it reads the input or writes scores
   int fmt;
   float* scores_dev_out;              // device destination [n_clips][n_out]
   int slot;                           // compute lane
   int stage;                          // staging slot
   const WinPass* win;                 // windows call: the pass's spans (else nullptr)
-  bool pair_rows = false;             // window-pairs call: scores_dev_out is compact, [n_clips / 2][n_out]
+  bool pair_rows = false;             // window-pairs or shared-reference call: scores_dev_out (and an embeddings call's
+                                      // pooled vectors) compact, [n_clips / 2][n_out]
   const nisqa_segment_out* seg;       // segments call: its outputs (else nullptr)
   const nisqa_embedding_out* emb;     // embeddings call: its outputs (else nullptr)
   const nisqa_alignment_out* al;      // alignment call: its outputs (else nullptr)
@@ -1374,8 +1387,11 @@ int upload_inputs(Pass& p, const PassInput& in) {
     d.n_frames = ok ? pl.n_frames : 0;
     d.n_seg = ok ? pl.n_seg : 0;
     d.frame_off = p.n_frames; d.seg_off = p.n_seg; d.pair_off = n_pairs;
+    d.ref_clip = in.ref_clip ? in.ref_clip[i] : i + 1;
+    d.src_clip = in.src_clip ? in.src_clip[i] : in.first_clip + i;
+    const bool alias = in.ref_clip && (i & 1) && in.ref_clip[i - 1] != i;       // (no PCM: it is never read)
     if (in.win) d.pcm_off = in.win->pcm_off[i];
-    else if (in.host_pcm || in.ingest) { d.pcm_off = pcm_elems; pcm_elems += ((long long)in.n_samples[i] + 15) / 16 * 16; }
+    else if (in.host_pcm || in.ingest) { d.pcm_off = pcm_elems; if (!alias) pcm_elems += ((long long)in.n_samples[i] + 15) / 16 * 16; }
     else d.pcm_off = in.dev_off[i];
     if (ok) max_run_samples = std::max<long long>(max_run_samples, in.n_samples[i]);
     pair_prefix[i] = n_pairs; seg_prefix[i] = p.n_seg; qt_prefix[i] = n_qt; qt64_prefix[i] = p.n_qt64;
@@ -1474,7 +1490,7 @@ int upload_inputs(Pass& p, const PassInput& in) {
         launch_ingest_spans(p.st, in.ingest->s[k], p.spans + s0, in.win->n_spans[k], max_run_samples,
                             in.fmt == NISQA_FMT_F32, SG.pcm.p);
     } else
-      launch_ingest(p.st, *in.ingest, in.first_clip, p.clips, n, max_run_samples, in.fmt == NISQA_FMT_F32, SG.pcm.p);
+      launch_ingest(p.st, *in.ingest, p.clips, n, max_run_samples, in.fmt == NISQA_FMT_F32, SG.pcm.p);
     p.pcm = SG.pcm.p;
   }
   return 0;
@@ -1904,9 +1920,10 @@ int segment_rows(Pass& p, const PassInput& in) {
       CK(cudaMemsetAsync(ao->peak + r, 0xFF, n * 4, p.st));
     }
   }
-  float* pooled = eo ? eo->pooled + (size_t)in.first_clip * nh * W : nullptr;
+  const int n_pooled = in.pair_rows ? p.n / 2 : p.n;          // (compact: one vector per pair)
+  float* pooled = eo ? eo->pooled + (size_t)(in.pair_rows ? in.first_clip / 2 : in.first_clip) * nh * W : nullptr;
   if (p.n_seg == 0) {     // (nothing ran: NaN vectors, like the scores)
-    if (eo) CK(cudaMemsetAsync(pooled, 0xFF, (size_t)p.n * nh * W * 4, p.st));
+    if (eo) CK(cudaMemsetAsync(pooled, 0xFF, (size_t)n_pooled * nh * W * 4, p.st));
     return 0;
   }
   if (so) {
@@ -1916,8 +1933,17 @@ int segment_rows(Pass& p, const PassInput& in) {
   }
   if (eo) {
     Scope s(e, "embed");
+    float* dst = pooled;
+    if (in.pair_rows) {   // the pass's interleaved vectors in its staging slot, then row 2p to row p
+      CK(p.SG.pair_pooled.reserve((size_t)p.n * nh * W * 4));
+      dst = p.SG.pair_pooled.as<float>();
+    }
     launch_pool_embed(p.st, p.pool_x, W, p.pool_ld, p.w.pool_src.empty() ? nullptr : e->emb_src.as<int>(), p.pool_logits,
-                      p.pool_P, nh, p.c.pool, p.c.double_ended, p.clips, p.n, p.seg_row, pooled, eo->rows);
+                      p.pool_P, nh, p.c.pool, p.c.double_ended, p.clips, p.n, p.seg_row, dst, eo->rows);
+    if (in.pair_rows) {
+      const size_t row = (size_t)nh * W * 4;
+      CK(cudaMemcpy2DAsync(pooled, row, dst, 2 * row, row, n_pooled, cudaMemcpyDeviceToDevice, p.st));
+    }
   }
   return 0;
 }
@@ -2110,6 +2136,9 @@ int run_call(nisqa_engine* e, const Call& c, cudaStream_t* fin_out) {
   // (scaled down for self-attention stacks wider than 64: their activation rows grow with d_model)
   const int d_max = std::max(e->sa_d(), e->cfg.td2_layers > 0 ? e->td2_d() : 64);
   const int max_seg = e->cfg.max_chunk_segments > 0 ? e->cfg.max_chunk_segments : 131072 / (d_max / 64);
+  const bool shared = c.ref_index != nullptr;
+  const bool pair_rows = shared || (c.win && c.win->n_src == 2);     // compact scores, one row per pair
+  const int n_rows = pair_rows ? n_clips / 2 : n_clips;
   float* scores_all = c.scores_dev;
   if (!scores_all) {
     DevBuf& sb = c.ticket ? e->tickets[e->next_ticket % kStages].scores : e->scores;
@@ -2120,22 +2149,44 @@ int run_call(nisqa_engine* e, const Call& c, cudaStream_t* fin_out) {
   int i0 = 0;
   e->last_passes = 0;
   WinPass wp;
+  // a shared-reference call: each reference's slot in the current pass (-1: none yet), the pass's ClipDesc.ref_clip and
+  // its plans with alias slots not run
+  std::vector<int> ref_slot(shared ? c.n_refs : 0, -1), ref_clip, named;
+  std::vector<ClipPlan> pass_plan;
   while (i0 < n_clips) {
     int i1 = i0; long long segs = 0;
     while (i1 < n_clips) {
       long long s = 0;
       for (int u = 0; u < unit; ++u) s += plan[i1 + u].run ? plan[i1 + u].n_seg : 0;
+      const int ru = shared && plan[i1].run ? c.ref_index[i1 / 2] : -1;     // (a pair that runs: its reference runs too)
+      if (ru >= 0 && ref_slot[ru] >= 0) s -= plan[i1 + 1].n_seg;            // (its reference is in the pass already)
       if (i1 > i0 && (segs + s > max_seg || i1 - i0 >= 32768)) break;      // (clips ride in grid.y of the front-end: < 65536)
+      if (ru >= 0 && ref_slot[ru] < 0) { ref_slot[ru] = i1 + 1 - i0; named.push_back(ru); }
       segs += s; i1 += unit;
     }
     PassInput in;
     in.n_clips = i1 - i0; in.plan = plan.data() + i0; in.n_samples = c.n_samples + i0;
+    if (shared) {
+      pass_plan.assign(plan.begin() + i0, plan.begin() + i1);
+      ref_clip.resize(i1 - i0);
+      for (int i = 0; i < i1 - i0; i += 2) {
+        ref_clip[i] = ref_clip[i + 1] = i + 1;
+        if (!pass_plan[i].run) continue;
+        ref_clip[i] = ref_slot[c.ref_index[(i0 + i) / 2]];
+        if (ref_clip[i] != i + 1) pass_plan[i + 1].run = 0;        // an alias slot: the front end, CNN and td skip it
+      }
+      for (int u : named) ref_slot[u] = -1;
+      named.clear();
+      in.plan = pass_plan.data();
+      in.ref_clip = ref_clip.data();
+    }
     in.host_pcm = c.host_pcm ? c.host_pcm + i0 : nullptr;
     in.dev_pcm = c.dev_pcm; in.dev_off = c.dev_off ? c.dev_off + i0 : nullptr;
     in.ingest = c.ingest; in.first_clip = i0;
+    in.src_clip = c.src_clip ? c.src_clip + i0 : nullptr;
     in.ready = c.ready;
     in.fmt = c.fmt;
-    in.pair_rows = c.win && c.win->n_src == 2;
+    in.pair_rows = pair_rows;
     in.scores_dev_out = scores_all + (size_t)(in.pair_rows ? i0 / 2 : i0) * e->cfg.n_out;
     in.seg = c.seg; in.emb = c.emb; in.al = c.al;
     in.seg_row = c.seg_row.empty() ? nullptr : c.seg_row.data() + i0;
@@ -2158,7 +2209,7 @@ int run_call(nisqa_engine* e, const Call& c, cudaStream_t* fin_out) {
   const cudaStream_t fin = e->lanes[n_pass ? e->last_lane : next_lane(e)].stream;
   for (int k = 0; k < kStages && n_pass > 1; ++k)      // passes of this call that ran on other lanes
     if (e->stages[k].busy && e->stages[k].lane != e->last_lane) CK(cudaStreamWaitEvent(fin, e->stages[k].ev_done, 0));
-  if (e->gather_dst && e->nccl_comm && n_clips == e->gather_rows && (c.ticket || c.scores_dev) && !c.win) {
+  if (e->gather_dst && e->nccl_comm && n_clips == e->gather_rows && (c.ticket || c.scores_dev) && !c.win && !shared) {
     // the path's single exchange step, enqueued behind this call's kernels on its own lane
     int rc = lane_allgather(e, scores_all, e->gather_dst, (size_t)n_clips * e->cfg.n_out, fin);
     if (rc) return rc;
@@ -2168,7 +2219,7 @@ int run_call(nisqa_engine* e, const Call& c, cudaStream_t* fin_out) {
   if (c.ticket) {
     // asynchronous completion: scores land in the ticket's pinned block; nisqa_wait hands them over
     Ticket& tk = e->tickets[e->next_ticket % kStages];
-    tk.bytes = (size_t)n_clips * e->cfg.n_out * 4;
+    tk.bytes = (size_t)n_rows * e->cfg.n_out * 4;
     tk.user_scores = c.scores_host;
     CK(tk.pinned.reserve(std::max<size_t>(tk.bytes, 16)));
     if (tk.bytes) CK(cudaMemcpyAsync(tk.pinned.p, scores_all, tk.bytes, cudaMemcpyDeviceToHost, fin));
@@ -2179,8 +2230,8 @@ int run_call(nisqa_engine* e, const Call& c, cudaStream_t* fin_out) {
     *c.ticket = tk.id;
     return 0;
   }
-  if (c.scores_host && n_clips > 0) {
-    const size_t bytes = (size_t)n_clips * e->cfg.n_out * 4;
+  if (c.scores_host && n_rows > 0) {
+    const size_t bytes = (size_t)n_rows * e->cfg.n_out * 4;
     CK(e->h_scores.reserve(bytes));
     CK(cudaMemcpyAsync(e->h_scores.p, scores_all, bytes, cudaMemcpyDeviceToHost, fin));
     CK(cudaStreamSynchronize(fin));
@@ -2408,7 +2459,8 @@ int nisqa_predict_pcm_device(nisqa_engine* e, int n_clips, const void* pcm_dev, 
 // `done` behind its last use of the slot and marks it busy).  A busy slot is waited for before it is reused.
 static int resample_to_device(nisqa_engine* e, cudaStream_t st, int n_clips, const void* const* pcm,
                               const IngestSources* ingest, const int64_t* n_samples, const int32_t* sample_rate, int fmt,
-                              int32_t target, std::vector<int64_t>* offs, std::vector<int64_t>* n_fix, RsSlot** slot_out) {
+                              int32_t target, std::vector<int64_t>* offs, std::vector<int64_t>* n_fix, RsSlot** slot_out,
+                              const int* src_clip = nullptr) {
   if (fmt != NISQA_FMT_S16 && fmt != NISQA_FMT_F32) return fail(e, NISQA_ERR_INVALID, "sample_fmt");
   if (target <= 0) return fail(e, NISQA_ERR_INVALID, "target sample rate");
   CK(cudaSetDevice(e->device));
@@ -2431,6 +2483,7 @@ static int resample_to_device(nisqa_engine* e, cudaStream_t st, int n_clips, con
       return fail(e, NISQA_ERR_INVALID, "resample: clip length / sample rate");
     ResampleClip& c = rc[i];
     c.n_in = (int)n_samples[i];
+    c.src_clip = src_clip ? src_clip[i] : i;
     c.copy = sample_rate[i] == target;
     c.ratio = (double)target / (double)sample_rate[i];
     c.n_out = c.copy ? c.n_in : (int)((double)c.n_in * c.ratio);                      // resampy: int(shape * ratio)
@@ -2457,7 +2510,7 @@ static int resample_to_device(nisqa_engine* e, cudaStream_t st, int n_clips, con
     long long max_in = 0;
     for (const ResampleClip& c : rc) max_in = std::max<long long>(max_in, c.n_in);
     e->launches += 1;
-    launch_ingest(st, *ingest, 0, S.clips.as<ResampleClip>(), n_clips, max_in, fmt == NISQA_FMT_F32, S.raw.p);
+    launch_ingest(st, *ingest, S.clips.as<ResampleClip>(), n_clips, max_in, fmt == NISQA_FMT_F32, S.raw.p);
   } else {
     for (int i = 0; i < n_clips; ++i)
       if (rc[i].n_in > 0)
@@ -2513,7 +2566,7 @@ static int enqueue_call(nisqa_engine* e, void* cuda_stream, Call& c, nisqa_feed*
                         const std::function<int(cudaStream_t)>& feed_ingest = nullptr) {
   cudaStream_t caller = static_cast<cudaStream_t>(cuda_stream);
   RsSlot* S = nullptr;
-  std::vector<int64_t> offs, n_fix;
+  std::vector<int64_t> offs, n_fix, clip_off;
   const int err = [&]() -> int {
     CK(cudaEventRecord(e->ev_in, caller));
     c.ready = e->ev_in;
@@ -2521,13 +2574,18 @@ static int enqueue_call(nisqa_engine* e, void* cuda_stream, Call& c, nisqa_feed*
       cudaStream_t st = e->lanes[next_lane(e)].stream;
       CK(cudaStreamWaitEvent(st, e->ev_in, 0));
       const int rc = f ? feed_ingest(st) : resample_to_device(e, st, c.n_rec, nullptr, c.ingest, c.rec_n, c.rec_sr, c.fmt,
-                                                              c.target_sr, &offs, &n_fix, &S);
+                                                              c.target_sr, &offs, &n_fix, &S, c.rec_src);
       if (rc) return rc;
       if (S) {
         CK(cudaEventRecord(S->ready, st));
         c.dev_pcm = S->out.p; c.ingest = nullptr; c.fmt = NISQA_FMT_F32; c.ready = S->ready;
         if (c.win) c.win->rec_off = offs.data();
-        else c.dev_off = offs.data();
+        else if (!c.clip_rec) c.dev_off = offs.data();
+        else {            // (a shared-reference call: each reference was converted once, its slots read that recording)
+          clip_off.resize(c.n_clips);
+          for (int g = 0; g < c.n_clips; ++g) clip_off[g] = offs[c.clip_rec[g]];
+          c.dev_off = clip_off.data();
+        }
       }
     }
     cudaStream_t fin = nullptr;
@@ -2555,10 +2613,11 @@ static int enqueue_call(nisqa_engine* e, void* cuda_stream, Call& c, nisqa_feed*
 }
 
 // The sources of a device call: deg, read with its channel (or mixed to mono), and ref when given, always the mono mix.
-// Each must be a batch of n_clips clips of min_n .. length samples (0 for a feed push); messages name deg by deg_nm and
-// ref by "ref.".  -> their ingest sources and the call's format: float32 if either is float32 or mixed, else int16.
+// Each must be a batch of n_clips clips (ref: ref_n_clips when >= 0, a shared-reference call) of min_n .. length samples
+// (0 for a feed push); messages name deg by deg_nm and ref by "ref.".  -> their ingest sources and the call's format:
+// float32 if either is float32 or mixed, else int16.
 static int check_sources(nisqa_engine* e, const std::string& deg_nm, const nisqa_device_batch& deg, const nisqa_device_batch* ref,
-                         int n_clips, int min_n, IngestSources* ing, int* fmt) {
+                         int n_clips, int min_n, IngestSources* ing, int* fmt, int ref_n_clips = -1) {
   const nisqa_device_batch* src[2] = {&deg, ref};
   *ing = {};
   ing->n_src = ref ? 2 : 1;
@@ -2568,7 +2627,7 @@ static int check_sources(nisqa_engine* e, const std::string& deg_nm, const nisqa
     const std::string nm = k ? "ref." : deg_nm;
     const int ch = k ? -1 : b.channel;
     if (b.sample_fmt != NISQA_FMT_S16 && b.sample_fmt != NISQA_FMT_F32) return fail(e, NISQA_ERR_INVALID, nm + "sample_fmt");
-    if (b.n_clips < 0 || b.n_clips != n_clips) return fail(e, NISQA_ERR_INVALID, nm + "n_clips");
+    if (b.n_clips < 0 || b.n_clips != (k && ref_n_clips >= 0 ? ref_n_clips : n_clips)) return fail(e, NISQA_ERR_INVALID, nm + "n_clips");
     if (b.n_channels < 1) return fail(e, NISQA_ERR_INVALID, nm + "n_channels");
     if (b.n_channels > 1 && (ch < -1 || ch >= b.n_channels)) return fail(e, NISQA_ERR_INVALID, nm + "channel out of range");
     if (b.length < 1 || b.clip_stride < 0 || b.channel_stride < 0) return fail(e, NISQA_ERR_INVALID, nm + "length / strides");
@@ -2669,6 +2728,127 @@ int nisqa_predict_device_batch_embeddings(nisqa_engine* e, void* cuda_stream, co
   if (e && !emb) return fail(e, NISQA_ERR_INVALID, "emb: null argument");
   if (e && !emb->pooled) return fail(e, NISQA_ERR_INVALID, "emb->pooled: null argument");
   return device_batch_call(e, cuda_stream, deg, ref, target_sr, scores_dev, nullptr, emb, n_segments_out, status_out);
+}
+
+// The refusals of a shared-reference call that concern its pairing: a single-ended engine, no reference, a null or out
+// of range ref_index
+static int check_ref_index(nisqa_engine* e, int n_pairs, int n_refs, const int32_t* ref_index) {
+  if (!e->cfg.double_ended)
+    return fail(e, NISQA_ERR_INVALID, "ref_index: only a double-ended (NISQA_DE) engine pairs degraded clips with references");
+  if (n_refs < 1) return fail(e, NISQA_ERR_INVALID, "ref: no reference clip (a shared-reference call needs at least one)");
+  if (!ref_index) return fail(e, NISQA_ERR_INVALID, "ref_index: null argument");
+  for (int p = 0; p < n_pairs; ++p)
+    if (ref_index[p] < 0 || ref_index[p] >= n_refs)
+      return fail(e, NISQA_ERR_INVALID, "ref_index[" + std::to_string(p) + "] = " + std::to_string(ref_index[p]) +
+                                            ": not within 0 .. " + std::to_string(n_refs - 1));
+  return 0;
+}
+
+// A planned shared-reference call's statuses split into its pairs' (the degraded clips') and its references' (each
+// planned alone at the model rate: host arithmetic, reported for references no pair names too)
+static void shared_ref_rows(const nisqa_engine* e, const Call& c, int n_refs, const int64_t* ref_n, int32_t ref_sr,
+                            int32_t target_sr, int32_t* n_segments_out, int32_t* status_out, int32_t* ref_n_segments_out,
+                            int32_t* ref_status_out) {
+  for (int p = 0; p < c.n_clips / 2; ++p) {
+    if (n_segments_out) n_segments_out[p] = c.plan[2 * p].n_seg;
+    if (status_out) status_out[p] = c.plan[2 * p].status;
+  }
+  for (int u = 0; u < n_refs; ++u) {
+    ClipPlan pl;
+    plan_clip(e->cfg, target_sr > 0 ? nisqa_resample_out_len(ref_n[u], ref_sr, target_sr) : ref_n[u],
+              target_sr > 0 ? target_sr : ref_sr, &pl);
+    if (ref_n_segments_out) ref_n_segments_out[u] = pl.n_seg;
+    if (ref_status_out) ref_status_out[u] = pl.status;
+  }
+}
+
+int nisqa_predict_device_batch_shared_ref(nisqa_engine* e, void* cuda_stream, const nisqa_device_batch* deg,
+                                          const nisqa_device_batch* ref, const int32_t* ref_index, int32_t target_sr,
+                                          float* scores_dev, const nisqa_segment_out* seg, const nisqa_embedding_out* emb,
+                                          const nisqa_alignment_out* al, int32_t* n_segments_out, int32_t* status_out,
+                                          int32_t* ref_n_segments_out, int32_t* ref_status_out) {
+  if (!e) return NISQA_ERR_INVALID;
+  if (!e->stream) return fail(e, NISQA_ERR_STATE, "engine was not created successfully");
+  if (!deg) return fail(e, NISQA_ERR_INVALID, "deg: null argument");
+  if (!ref) return fail(e, NISQA_ERR_INVALID, "ref: null argument");
+  int rc = check_ref_index(e, std::max(deg->n_clips, 0), ref->n_clips, ref_index);
+  if (rc) return rc;
+  if (target_sr < 0) return fail(e, NISQA_ERR_INVALID, "target_sr");
+  if (al && (rc = check_alignment_out(e, al))) return rc;
+  IngestSources ing;
+  int fmt;
+  if ((rc = check_sources(e, "deg.", *deg, ref, deg->n_clips, 1, &ing, &fmt, ref->n_clips))) return rc;
+  const int B = deg->n_clips, n_clips = 2 * B;
+  if (B > 0 && !scores_dev) return fail(e, NISQA_ERR_INVALID, "scores_dev: null argument");
+  if (seg && B > 0 && (!seg->scores || !seg->weights)) return fail(e, NISQA_ERR_INVALID, "seg: null scores / weights");
+  if (emb && !emb->pooled) return fail(e, NISQA_ERR_INVALID, "emb->pooled: null argument");
+  // the engine's clips: pair p's degraded clip, then a slot of its reference (IngestSources position 2 u + 1); with ms_sr
+  // the degraded clips and each named reference once are converted, in that order
+  std::vector<int64_t> ns(n_clips), n_model(n_clips), rec_n;
+  std::vector<int32_t> sr(n_clips), sr_model(n_clips, target_sr), rec_sr, nseg(n_clips), status(n_clips);
+  std::vector<int> src(n_clips), rec_src, clip_rec(n_clips), rec_of(ref->n_clips, -1);
+  for (int g = 0; g < n_clips; ++g) {
+    const int u = ref_index[g / 2];
+    const nisqa_device_batch& b = (g & 1) ? *ref : *deg;
+    const int k = (g & 1) ? u : g / 2;
+    ns[g] = b.n_samples[k]; sr[g] = b.sample_rate; src[g] = (g & 1) ? 2 * u + 1 : g;
+    n_model[g] = target_sr > 0 ? nisqa_resample_out_len(ns[g], sr[g], target_sr) : ns[g];
+    if (!(g & 1)) { clip_rec[g] = g / 2; rec_src.push_back(g); rec_n.push_back(ns[g]); rec_sr.push_back(sr[g]); }
+  }
+  for (int p = 0; p < B; ++p) {
+    int& r = rec_of[ref_index[p]];
+    if (r < 0) { r = (int)rec_src.size(); rec_src.push_back(src[2 * p + 1]); rec_n.push_back(ns[2 * p + 1]); rec_sr.push_back(ref->sample_rate); }
+    clip_rec[2 * p + 1] = r;
+  }
+  Call c(n_clips, n_model.data(), target_sr > 0 ? sr_model.data() : sr.data(), fmt, nseg.data(), status.data());
+  c.ingest = &ing; c.src_clip = src.data(); c.scores_dev = scores_dev; c.seg = seg; c.emb = emb; c.al = al;
+  c.ref_index = ref_index; c.n_refs = ref->n_clips;
+  c.target_sr = target_sr; c.n_rec = (int)rec_src.size(); c.rec_n = rec_n.data(); c.rec_sr = rec_sr.data();
+  c.rec_src = rec_src.data(); c.clip_rec = clip_rec.data();
+  if ((rc = plan_call(e, c))) return rc;
+  shared_ref_rows(e, c, ref->n_clips, ref->n_samples, ref->sample_rate, target_sr, n_segments_out, status_out,
+                  ref_n_segments_out, ref_status_out);
+  return enqueue_call(e, cuda_stream, c);
+}
+
+int nisqa_submit_pcm_pairs(nisqa_engine* e, int n_pairs, const void* const* pcm, const int64_t* n_samples,
+                           const int32_t* sample_rate, int n_refs, const void* const* ref_pcm, const int64_t* ref_n_samples,
+                           const int32_t* ref_sample_rate, const int32_t* ref_index, int sample_fmt, float* scores_out,
+                           int32_t* n_segments_out, int32_t* status_out, int32_t* ref_n_segments_out,
+                           int32_t* ref_status_out, int64_t* ticket) {
+  if (!e || !ticket) return NISQA_ERR_INVALID;
+  if (n_pairs < 0) return fail(e, NISQA_ERR_INVALID, "n_pairs");
+  int rc = check_ref_index(e, n_pairs, n_refs, ref_index);
+  if (rc) return rc;
+  if (n_pairs > 0 && (!pcm || !n_samples || !sample_rate || !scores_out)) return fail(e, NISQA_ERR_INVALID, "null argument");
+  if (!ref_pcm || !ref_n_samples || !ref_sample_rate)
+    return fail(e, NISQA_ERR_INVALID, "ref_pcm / ref_n_samples / ref_sample_rate: null argument");
+  if (e->profiling) return fail(e, NISQA_ERR_STATE, "profiling needs the synchronous entry points");
+  if ((rc = finish_ticket(e, e->tickets[e->next_ticket % kStages]))) return rc;      // at most kStages submissions in flight
+  const int n_clips = 2 * n_pairs;
+  std::vector<const void*> ptr(n_clips);
+  std::vector<int64_t> ns(n_clips);
+  std::vector<int32_t> sr(n_clips), nseg(n_clips), status(n_clips);
+  for (int p = 0; p < n_pairs; ++p) {
+    const int u = ref_index[p];
+    ptr[2 * p] = pcm[p]; ns[2 * p] = n_samples[p]; sr[2 * p] = sample_rate[p];
+    ptr[2 * p + 1] = ref_pcm[u]; ns[2 * p + 1] = ref_n_samples[u]; sr[2 * p + 1] = ref_sample_rate[u];
+  }
+  Call c(n_clips, ns.data(), sr.data(), sample_fmt, nseg.data(), status.data());
+  c.host_pcm = ptr.data(); c.scores_host = scores_out; c.ticket = ticket;
+  c.ref_index = ref_index; c.n_refs = n_refs;
+  if ((rc = plan_call(e, c))) return rc;
+  for (int p = 0; p < n_pairs; ++p) {
+    if (n_segments_out) n_segments_out[p] = c.plan[2 * p].n_seg;
+    if (status_out) status_out[p] = c.plan[2 * p].status;
+  }
+  for (int u = 0; u < n_refs; ++u) {
+    ClipPlan pl;
+    plan_clip(e->cfg, ref_n_samples[u], ref_sample_rate[u], &pl);
+    if (ref_n_segments_out) ref_n_segments_out[u] = pl.n_seg;
+    if (ref_status_out) ref_status_out[u] = pl.status;
+  }
+  return run_call(e, c, nullptr);
 }
 
 // The window list of a windows call or feed push, in recording order

@@ -18,12 +18,12 @@ constexpr int kIngestPerThread = 4;      // samples per thread and grid-stride s
 __device__ __forceinline__ float ingest_f32(const short* x, long long i) { return __fmul_rn((float)x[i], 1.0f / 32768.0f); }
 __device__ __forceinline__ float ingest_f32(const float* x, long long i) { return x[i]; }
 
-__device__ __forceinline__ bool ingest_row(const ClipDesc& c, long long* off, int* n) {
-  *off = c.pcm_off; *n = c.n_samples;
+__device__ __forceinline__ bool ingest_row(const ClipDesc& c, long long* off, int* n, int* g) {
+  *off = c.pcm_off; *n = c.n_samples; *g = c.src_clip;
   return c.n_frames > 0;                 // a skipped clip (too short / too long, or its pair's) is never read
 }
-__device__ __forceinline__ bool ingest_row(const ResampleClip& c, long long* off, int* n) {
-  *off = c.in_off; *n = c.n_in;
+__device__ __forceinline__ bool ingest_row(const ResampleClip& c, long long* off, int* n, int* g) {
+  *off = c.in_off; *n = c.n_in; *g = c.src_clip;
   return c.n_in > 0;
 }
 
@@ -46,14 +46,13 @@ __device__ __forceinline__ void ingest_clip(const IngestSrc& s, long long b, int
   }
 }
 
-// grid (sample blocks, clips)
+// grid (sample blocks, clips); each row names the clip of the sources it packs (src_clip, IngestSources order)
 template <class Row>
 __global__ void __launch_bounds__(kIngestThreads)
-ingest_kernel(IngestSources src, int first_clip, const Row* __restrict__ rows, int out_f32, void* __restrict__ out) {
+ingest_kernel(IngestSources src, const Row* __restrict__ rows, int out_f32, void* __restrict__ out) {
   long long off;
-  int n;
-  if (!ingest_row(rows[blockIdx.y], &off, &n)) return;
-  const int g = first_clip + (int)blockIdx.y;
+  int n, g;
+  if (!ingest_row(rows[blockIdx.y], &off, &n, &g)) return;
   const IngestSrc s = g % src.n_src ? src.s[1] : src.s[0];     // (no dynamic index into the parameter struct: no stack)
   const long long b = g / src.n_src;
   if (out_f32) {
@@ -66,12 +65,12 @@ ingest_kernel(IngestSources src, int first_clip, const Row* __restrict__ rows, i
 }
 
 template <class Row>
-static void launch_ingest_rows(cudaStream_t st, const IngestSources& src, int first_clip, const Row* rows, int n_clips,
+static void launch_ingest_rows(cudaStream_t st, const IngestSources& src, const Row* rows, int n_clips,
                                long long max_n, int out_f32, void* out) {
   if (n_clips <= 0 || max_n <= 0) return;
   const long long per_block = (long long)kIngestThreads * kIngestPerThread;
   const dim3 grid((unsigned)std::min<long long>((max_n + per_block - 1) / per_block, 4096), n_clips);
-  ingest_kernel<Row><<<grid, kIngestThreads, 0, st>>>(src, first_clip, rows, out_f32, out);
+  ingest_kernel<Row><<<grid, kIngestThreads, 0, st>>>(src, rows, out_f32, out);
 }
 
 // nisqa_predict_device_windows: each recording span of a pass packed once, however many windows read it; grid (sample
@@ -140,13 +139,13 @@ void launch_ingest_feed(cudaStream_t st, const IngestSrc& src, const FeedPush* p
   ingest_feed_kernel<<<grid, kIngestThreads, 0, st>>>(src, push, g, out_f32, ring);
 }
 
-void launch_ingest(cudaStream_t st, const IngestSources& src, int first_clip, const ClipDesc* clips, int n_clips,
-                   long long max_n, int out_f32, void* out) {
-  launch_ingest_rows(st, src, first_clip, clips, n_clips, max_n, out_f32, out);
+void launch_ingest(cudaStream_t st, const IngestSources& src, const ClipDesc* clips, int n_clips, long long max_n,
+                   int out_f32, void* out) {
+  launch_ingest_rows(st, src, clips, n_clips, max_n, out_f32, out);
 }
-void launch_ingest(cudaStream_t st, const IngestSources& src, int first_clip, const ResampleClip* clips, int n_clips,
-                   long long max_n, int out_f32, void* out) {
-  launch_ingest_rows(st, src, first_clip, clips, n_clips, max_n, out_f32, out);
+void launch_ingest(cudaStream_t st, const IngestSources& src, const ResampleClip* clips, int n_clips, long long max_n,
+                   int out_f32, void* out) {
+  launch_ingest_rows(st, src, clips, n_clips, max_n, out_f32, out);
 }
 
 }  // namespace nisqa

@@ -105,6 +105,7 @@ struct ResampleClip {
   int n_fix;             // librosa fix_length: ceil(n_in * ratio) (zero padded / trimmed)
   int copy;              // 1: sr_orig == sr_new, plain conversion / copy
   double ratio;          // sr_new / sr_orig
+  int src_clip;          // device ingest: the clip's position in IngestSources order
 };
 
 // ---------------------------------------------------------------- frontend.cu
@@ -248,13 +249,13 @@ struct IngestSrc {
 // The clips of a call in the engine's order: clip g (of the whole call) is clip g / n_src of source g % n_src (NISQA_DE:
 // source 0 the degraded batch, source 1 the reference batch)
 struct IngestSources { IngestSrc s[2]; int n_src; };
-// Packed mono PCM of clips first_clip .. first_clip + n_clips - 1 of the call, written where the table says: the pass's
-// ClipDesc rows (pcm_off, n_samples; skipped clips are not read) or the resampler's ResampleClip rows (in_off, n_in).
+// Packed mono PCM of the clips a table names (src_clip of each row), written where the table says: the pass's ClipDesc
+// rows (pcm_off, n_samples; skipped clips are not read) or the resampler's ResampleClip rows (in_off, n_in).
 // out_f32 0: int16 out (every source int16 and mono or picked); 1: float32 out (int16 scaled by 1/32768).
-void launch_ingest(cudaStream_t st, const IngestSources& src, int first_clip, const ClipDesc* clips, int n_clips,
-                   long long max_n, int out_f32, void* out);
-void launch_ingest(cudaStream_t st, const IngestSources& src, int first_clip, const ResampleClip* clips, int n_clips,
-                   long long max_n, int out_f32, void* out);
+void launch_ingest(cudaStream_t st, const IngestSources& src, const ClipDesc* clips, int n_clips, long long max_n,
+                   int out_f32, void* out);
+void launch_ingest(cudaStream_t st, const IngestSources& src, const ResampleClip* clips, int n_clips, long long max_n,
+                   int out_f32, void* out);
 // nisqa_predict_device_windows: samples src_off .. src_off + n_samples - 1 of recording `src` of the batch to pcm_off, once
 // per span (max_n: the longest span)
 void launch_ingest_spans(cudaStream_t st, const IngestSrc& src, const WinSpan* spans, int n_spans, long long max_n,

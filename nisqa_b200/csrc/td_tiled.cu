@@ -606,7 +606,7 @@ de_align_kernel(const float* __restrict__ x_td /*[n_seg][ld]*/, int ld, int W, c
   const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
   const int c = upper_slot(qtile_prefix, n_clips, blockIdx.x);
   if (c & 1) return;                       // reference clips are keys only
-  const ClipDesc cd = clips[c], cr = clips[c + 1];
+  const ClipDesc cd = clips[c], cr = clips[cd.ref_clip];
   const int Sx = cd.n_seg, Sy = cr.n_seg;
   if (Sx <= 0 || Sy <= 0) return;
   const int q0 = (blockIdx.x - __ldg(qtile_prefix + c)) * kT;
@@ -797,7 +797,7 @@ __global__ void row_rnorm_kernel(const float* __restrict__ x, int ld, int W, int
 __global__ void de_finalize_kernel(const ClipDesc* __restrict__ clips, int n_clips, int n_out, float* __restrict__ scores) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= n_clips) return;
-  const bool bad = (c & 1) || clips[c].n_seg <= 0 || clips[c + 1].n_seg <= 0;
+  const bool bad = (c & 1) || clips[c].n_seg <= 0 || clips[clips[c].ref_clip].n_seg <= 0;
   if (bad) for (int h = 0; h < n_out; ++h) scores[c * n_out + h] = __int_as_float(0x7fc00000);
 }
 

@@ -44,6 +44,7 @@ EXPORTS = [
     "nisqa_embedding_width", "nisqa_predict_device_batch_embeddings", "nisqa_window_pair_counts",
     "nisqa_predict_device_window_pairs", "nisqa_feed_pair_create", "nisqa_feed_pair_rows", "nisqa_feed_pair_push",
     "nisqa_predict_device_batch_alignment", "nisqa_predict_device_window_pairs_alignment",
+    "nisqa_predict_device_batch_shared_ref", "nisqa_submit_pcm_pairs",
 ]
 
 
@@ -274,6 +275,13 @@ def load_library(path=None):
     lib.nisqa_predict_device_batch_alignment.argtypes = [vp, vp, dbp, dbp, C.c_int32, vp, C.POINTER(NisqaAlignmentOut),
                                                          i32p, i32p]
     lib.nisqa_predict_device_batch_alignment.restype = C.c_int
+    lib.nisqa_predict_device_batch_shared_ref.argtypes = [vp, vp, dbp, dbp, i32p, C.c_int32, vp, C.POINTER(NisqaSegmentOut),
+                                                          C.POINTER(NisqaEmbeddingOut), C.POINTER(NisqaAlignmentOut),
+                                                          i32p, i32p, i32p, i32p]
+    lib.nisqa_predict_device_batch_shared_ref.restype = C.c_int
+    lib.nisqa_submit_pcm_pairs.argtypes = [vp, C.c_int, C.POINTER(vp), i64p, i32p, C.c_int, C.POINTER(vp), i64p, i32p, i32p,
+                                           C.c_int, f32p, i32p, i32p, i32p, i32p, i64p]
+    lib.nisqa_submit_pcm_pairs.restype = C.c_int
     lib.nisqa_predict_device_window_pairs_alignment.argtypes = [vp, vp, dbp, dbp, C.c_int32, C.c_int64, C.c_int32, C.c_int32,
                                                                 vp, C.c_int64, C.POINTER(NisqaAlignmentOut), i32p, i32p,
                                                                 i32p, i32p]
@@ -789,6 +797,39 @@ class Engine(object):
         self._check(rc, "nisqa_submit_pcm")
         return (ticket.value, scores, nseg, status, clips, ptrs, ns, sr)      # keeps the buffers alive
 
+    def submit_pcm_pairs(self, clips, sample_rates, refs, ref_sample_rates, ref_index):
+        """:meth:`submit_pcm` for NISQA_DE pairs whose references repeat: pair p is ``clips[p]`` and ``refs[ref_index[p]]``;
+        each reference is uploaded and computed once per engine pass.  Returns a handle; ``wait(handle)`` -> (scores
+        [n_pairs, n_out], n_segments [n_pairs], status [n_pairs]); ``handle[4]`` / ``handle[5]`` are the references'
+        n_segments / status [n_refs]."""
+        n, u = len(clips), len(refs)
+        every = list(clips) + list(refs)
+        if every and any(c.dtype != every[0].dtype for c in every):
+            every = [c if c.dtype == np.float32 else c.astype(np.float32) / np.float32(32768.0) for c in every]
+        dt = every[0].dtype if every else np.dtype(np.int16)
+        if dt not in (np.dtype(np.int16), np.dtype(np.float32)):
+            raise ValueError("clips must be int16 or float32")
+        every = [np.ascontiguousarray(c) for c in every]
+        ptrs = (C.c_void_p * max(n, 1))(*[c.ctypes.data for c in every[:n]])
+        ref_ptrs = (C.c_void_p * max(u, 1))(*[c.ctypes.data for c in every[n:]])
+        ns = np.array([c.shape[0] for c in every[:n]], dtype=np.int64)
+        ref_ns = np.array([c.shape[0] for c in every[n:]], dtype=np.int64)
+        sr = np.ascontiguousarray(sample_rates, dtype=np.int32)
+        ref_sr = np.ascontiguousarray(ref_sample_rates, dtype=np.int32)
+        idx = np.ascontiguousarray(ref_index, dtype=np.int32)
+        scores = np.empty((n, self.n_out), dtype=np.float32)
+        nseg, status = np.empty(n, dtype=np.int32), np.empty(n, dtype=np.int32)
+        ref_nseg, ref_status = np.empty(u, dtype=np.int32), np.empty(u, dtype=np.int32)
+        ticket = C.c_int64(0)
+        p32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32))      # noqa: E731
+        rc = self.lib.nisqa_submit_pcm_pairs(
+            self.h, n, ptrs, ns.ctypes.data_as(C.POINTER(C.c_int64)), p32(sr), u, ref_ptrs,
+            ref_ns.ctypes.data_as(C.POINTER(C.c_int64)), p32(ref_sr), p32(idx), FMT_S16 if dt == np.int16 else FMT_F32,
+            scores.ctypes.data_as(C.POINTER(C.c_float)), p32(nseg), p32(status), p32(ref_nseg), p32(ref_status),
+            C.byref(ticket))
+        self._check(rc, "nisqa_submit_pcm_pairs")
+        return (ticket.value, scores, nseg, status, ref_nseg, ref_status, every, ptrs, ref_ptrs, ns, ref_ns, sr, ref_sr, idx)
+
     def wait(self, handle):
         if handle[0] is not None:             # (None: a synchronous call's results wrapped as a handle)
             self._check(self.lib.nisqa_wait(self.h, handle[0]), "nisqa_wait")
@@ -876,6 +917,30 @@ class Engine(object):
         order; include/nisqa_b200.h nisqa_alignment_out).  Raises EngineError, with nothing enqueued, for a refused call
         (a single-ended engine, a null array, a too-small ``al.n_rows``)."""
         return self._device_batch(stream, deg, scores_dev_ptr, ref, target_sr, al)
+
+    def predict_device_batch_shared_ref(self, stream, deg, ref, ref_index, scores_dev_ptr, out=None, target_sr=0):
+        """:meth:`predict_device_batch` of a NISQA_DE engine whose pairs share references: pair p is clip p of ``deg`` and
+        clip ``ref_index[p]`` of ``ref`` (host ints); each reference is computed once per engine pass.  The scores go to
+        ``scores_dev_ptr`` ([n_pairs, n_out], one row per pair); ``out``: None or a :class:`NisqaSegmentOut`,
+        :class:`NisqaEmbeddingOut` (pooled [n_pairs, n_out, width]) or :class:`NisqaAlignmentOut`.  Returns (n_segments,
+        status) int32[n_pairs] and (ref_n_segments, ref_status) int32[n_refs], valid on return."""
+        if target_sr:
+            from . import resample as _rs
+            _rs.out_len(1, 1, 1)                                      # the interpolation table is set once
+        n, u = deg[0].n_clips, ref[0].n_clips
+        idx = None if ref_index is None else np.ascontiguousarray(ref_index, dtype=np.int32)
+        nseg, status = np.empty(n, dtype=np.int32), np.empty(n, dtype=np.int32)
+        ref_nseg, ref_status = np.empty(max(u, 0), dtype=np.int32), np.empty(max(u, 0), dtype=np.int32)
+        outs = [None, None, None]
+        for k, t in enumerate((NisqaSegmentOut, NisqaEmbeddingOut, NisqaAlignmentOut)):
+            if isinstance(out, t):
+                outs[k] = C.byref(out)
+        p32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32))      # noqa: E731
+        self._check(self.lib.nisqa_predict_device_batch_shared_ref(
+            self.h, C.c_void_p(stream or None), C.byref(deg[0]), C.byref(ref[0]),
+            p32(idx) if idx is not None else None, int(target_sr or 0), C.c_void_p(scores_dev_ptr), *outs,
+            p32(nseg), p32(status), p32(ref_nseg), p32(ref_status)), "nisqa_predict_device_batch_shared_ref")
+        return nseg, status, ref_nseg, ref_status
 
     def predict_device_windows(self, stream, rec, scores_dev_ptr, n_rows, window, hop_frames, target_sr=0):
         """Windows of the recordings ``rec`` (a :func:`device_batch` tuple) ordered on ``stream``: ``window`` samples and a

@@ -125,7 +125,7 @@ class Scorer(object):
         self.engine.close()
 
     def __call__(self, wave, sample_rate, lengths=None, channel=None, reference=None, reference_lengths=None,
-                 reference_sample_rate=None):
+                 reference_sample_rate=None, reference_index=None):
         """Scores of a batch -> float32 [B, len(columns)] on ``wave.device``.
 
         wave        : [T], [B, T] or [B, C, T] int16 / float32 CUDA tensor on the scorer's device, any batch and channel
@@ -135,16 +135,23 @@ class Scorer(object):
         channel     : None = the mono mix (mean over channels, as the file ingest), else that channel
         reference   : NISQA_DE only: the reference clips, one per clip of ``wave``, always mixed to mono; with their own
                       ``reference_lengths`` and ``reference_sample_rate`` (default: ``sample_rate``)
+        reference_index : NISQA_DE only, references shared by several clips (a sweep of conditions over one source):
+                      host ints, one per clip of ``wave``, naming its clip of ``reference``, which then holds any number
+                      U >= 1 of clips.  Each reference is computed once per engine pass and every pair scores bit for
+                      bit what ``reference[reference_index]`` gives; a reference no clip names is not read.
         A clip too short or too long for the checkpoint raises the file ingest's ValueError before anything is enqueued.
         """
-        deg, ref, _ = self._arguments(wave, sample_rate, lengths, channel, reference, reference_lengths, reference_sample_rate)
-        out = self._scores_buffer(deg, ref)
-        if out.shape[0]:
+        deg, ref, _, idx = self._arguments(wave, sample_rate, lengths, channel, reference, reference_lengths,
+                                           reference_sample_rate, reference_index)
+        out = self._scores_buffer(deg, ref, idx)
+        if out.shape[0] and idx is not None:
+            self.engine.predict_device_batch_shared_ref(self._stream(), deg, ref, idx, out.data_ptr(), target_sr=self.target_sr)
+        elif out.shape[0]:
             self.engine.predict_device_batch(self._stream(), deg, out.data_ptr(), ref=ref, target_sr=self.target_sr)
-        return self._clip_rows(out, ref)
+        return self._clip_rows(out, ref, idx)
 
     def segments(self, wave, sample_rate, lengths=None, channel=None, reference=None, reference_lengths=None,
-                 reference_sample_rate=None):
+                 reference_sample_rate=None, reference_index=None):
         """Scores of a batch and of every segment of its clips -> :data:`Segments`.  Takes the arguments of
         ``__call__`` and checks them alike.
 
@@ -158,13 +165,17 @@ class Scorer(object):
         t_start, t_end : float64 [N] host arrays, seconds: the centres of the segment's first and last mel frame
         NISQA_DE: rows for the degraded clips only.
         """
-        deg, ref, counts = self._arguments(wave, sample_rate, lengths, channel, reference, reference_lengths,
-                                           reference_sample_rate)
-        out = self._scores_buffer(deg, ref)
+        deg, ref, counts, idx = self._arguments(wave, sample_rate, lengths, channel, reference, reference_lengths,
+                                                reference_sample_rate, reference_index)
+        out = self._scores_buffer(deg, ref, idx)
         n_rows = int(sum(counts))
         seg_s = torch.empty((n_rows, len(self.columns)), dtype=torch.float32, device=self.device)
         seg_w = torch.empty_like(seg_s)
-        if out.shape[0]:
+        if out.shape[0] and idx is not None:
+            so = E.NisqaSegmentOut(scores=seg_s.data_ptr() or None, weights=seg_w.data_ptr() or None, n_rows=n_rows)
+            self.engine.predict_device_batch_shared_ref(self._stream(), deg, ref, idx, out.data_ptr(), so,
+                                                        target_sr=self.target_sr)
+        elif out.shape[0]:
             self.engine.predict_device_batch_segments(self._stream(), deg, out.data_ptr(), seg_s.data_ptr(), seg_w.data_ptr(),
                                                       n_rows, ref=ref, target_sr=self.target_sr)
         rate = self.target_sr or deg[0].sample_rate
@@ -173,10 +184,10 @@ class Scorer(object):
         t = np.concatenate([np.arange(c, dtype=np.float64) for c in counts]) if counts else np.zeros(0)
         t_start = t * a["ms_seg_hop_length"] * hop / rate
         t_end = (t * a["ms_seg_hop_length"] + a["ms_seg_length"] - 1) * hop / rate
-        return Segments(self._clip_rows(out, ref), seg_s, seg_w, list(counts), t_start, t_end)
+        return Segments(self._clip_rows(out, ref, idx), seg_s, seg_w, list(counts), t_start, t_end)
 
     def windows(self, wave, sample_rate, window_s, window_hop_s, lengths=None, channel=None, reference=None,
-                reference_lengths=None, reference_sample_rate=None, reference_margin_s=0.0):
+                reference_lengths=None, reference_sample_rate=None, reference_margin_s=0.0, reference_index=None):
         """Every recording of a batch scored as a timeline of overlapping windows -> :data:`Windows`, or with a
         ``reference`` (NISQA_DE) as a timeline of window pairs -> :data:`WindowPairs`.  Takes the arguments of
         ``__call__`` and checks them alike, but accepts recordings of any length.
@@ -200,7 +211,9 @@ class Scorer(object):
         Pair k scores exactly what ``__call__`` gives the degraded window k and the reference window [max(0, k H - M),
         min(T_ref, k H + W + M)) cut out as clips.  A pair whose degraded or reference window is too short (or empty:
         k H - M >= T_ref) scores NaN; ``status`` and ``ref_status`` tell which.
+        ``reference_index`` (shared references) is refused: window pairs take one reference recording per recording.
         """
+        _refuse_reference_index(reference_index, "windows")
         return self._windows(wave, sample_rate, window_s, window_hop_s, lengths, channel, reference, reference_lengths,
                              reference_sample_rate, reference_margin_s, None)
 
@@ -280,7 +293,7 @@ class Scorer(object):
         return Windows(out, counts, *cols) if ref is None else WindowPairs(out, counts, *cols)
 
     def align(self, wave, sample_rate, reference, lengths=None, channel=None, reference_lengths=None,
-              reference_sample_rate=None, window_s=None, window_hop_s=None, reference_margin_s=0.0):
+              reference_sample_rate=None, window_s=None, window_hop_s=None, reference_margin_s=0.0, reference_index=None):
         """NISQA_DE's time alignment of every degraded segment -> :data:`Alignment`, or with ``window_s`` of every segment
         of each window pair's degraded window -> :data:`AlignmentWindows`.  Takes the arguments of ``__call__`` (of
         ``windows`` with a ``window_s``) and checks them alike; a single-ended checkpoint raises ValueError.
@@ -298,26 +311,31 @@ class Scorer(object):
         delay_s       : ref_t_start - t_start;  centroid_delay_s: the centroid's position in seconds minus t_start
         Segment i starts i * ms_seg_hop_length * hop / rate seconds into its clip, each side at its own model rate and hop;
         window mode adds k H / rate on the degraded side and max(0, k H - M) / rate on the reference side of pair k.
+        reference_index : clip mode only, as in ``__call__`` (shared references)
         """
         if not self.double_ended:
             raise ValueError("align: only a double-ended (NISQA_DE) checkpoint aligns a reference to the degraded signal")
         if window_s is not None or window_hop_s is not None:
+            _refuse_reference_index(reference_index, "align(window_s=...)")
             return self._align_windows(wave, sample_rate, reference, lengths, channel, reference_lengths,
                                        reference_sample_rate, window_s, window_hop_s, reference_margin_s)
         if reference_margin_s != 0:
             raise ValueError("reference_margin_s=%r: a margin widens reference windows; pass window_s and window_hop_s"
                              % (reference_margin_s,))
-        deg, ref, counts = self._arguments(wave, sample_rate, lengths, channel, reference, reference_lengths,
-                                           reference_sample_rate)
-        out = self._scores_buffer(deg, ref)
+        deg, ref, counts, idx = self._arguments(wave, sample_rate, lengths, channel, reference, reference_lengths,
+                                                reference_sample_rate, reference_index)
+        out = self._scores_buffer(deg, ref, idx)
         n_rows = int(sum(counts))
         al, outs = self._alignment_buffers(n_rows)
-        if out.shape[0]:
+        if out.shape[0] and idx is not None:
+            self.engine.predict_device_batch_shared_ref(self._stream(), deg, ref, idx, out.data_ptr(), al,
+                                                        target_sr=self.target_sr)
+        elif out.shape[0]:
             self.engine.predict_device_batch_alignment(self._stream(), deg, ref, out.data_ptr(), al, target_sr=self.target_sr)
         i = np.concatenate([np.arange(c, dtype=np.float64) for c in counts]) if counts else np.zeros(0)
         z = np.zeros(n_rows)
         cols = self._alignment_times(outs, i, deg[0].sample_rate, ref[0].sample_rate, z, z)
-        return Alignment(self._clip_rows(out, ref), *outs, list(counts), *cols)
+        return Alignment(self._clip_rows(out, ref, idx), *outs, list(counts), *cols)
 
     def _align_windows(self, wave, sample_rate, reference, lengths, channel, reference_lengths, reference_sample_rate,
                        window_s, window_hop_s, reference_margin_s):
@@ -361,7 +379,7 @@ class Scorer(object):
         return t_start, ref_t_start, ref_t_start - t_start, ref_off + cen * ref_step - t_start
 
     def feed(self, n_feeds, sample_rate, window_s, window_hop_s, channel=None, max_push_s=None, reference=None,
-             reference_margin_s=0.0, max_skew_s=None):
+             reference_margin_s=0.0, max_skew_s=None, reference_index=None):
         """A :class:`Feed` of ``n_feeds`` live recordings at ``sample_rate``, scored as the windows of :meth:`windows`
         (``window_s``, ``window_hop_s``, checked alike) as soon as each window is complete.  ``channel`` applies to every
         push (None: the mono mix); ``max_push_s`` (default ``window_s``) is the longest chunk one push may append to one
@@ -374,6 +392,7 @@ class Scorer(object):
         slower side, so the rings hold the faster side's backlog (device memory grows with it).  Recordings whose two
         sides end further apart than that need a larger ``max_skew_s``."""
         m = reference_margin_s
+        _refuse_reference_index(reference_index, "feed")
         if reference is not None and not isinstance(reference, bool):
             raise TypeError("reference: True (NISQA_DE: live (degraded, reference) pairs) or None, not %r" % (reference,))
         if isinstance(m, bool) or not isinstance(m, numbers.Real) or not np.isfinite(m) or m < 0:
@@ -431,7 +450,7 @@ class Scorer(object):
         return FeedPairs(self, int(n_feeds), int(sample_rate), W, hop_frames, channel, max_push, margin_frames, max_skew)
 
     def embed(self, wave, sample_rate, lengths=None, channel=None, reference=None, reference_lengths=None,
-              reference_sample_rate=None, rows=False):
+              reference_sample_rate=None, rows=False, reference_index=None):
         """Scores of a batch and the representation behind them -> :data:`Embeddings`.  Takes the arguments of
         ``__call__`` and checks them alike.
 
@@ -445,22 +464,31 @@ class Scorer(object):
         counts : host list of B ints, the segments of each clip (its rows follow those of the clips before it)
         NISQA_DE: one pooled vector per pair, rows for the degraded clips only.
         """
-        deg, ref, counts = self._arguments(wave, sample_rate, lengths, channel, reference, reference_lengths,
-                                           reference_sample_rate)
-        out = self._scores_buffer(deg, ref)
+        deg, ref, counts, idx = self._arguments(wave, sample_rate, lengths, channel, reference, reference_lengths,
+                                                reference_sample_rate, reference_index)
+        out = self._scores_buffer(deg, ref, idx)
         width = self.engine.embedding_width()
         pooled = torch.empty((out.shape[0], len(self.columns), width), dtype=torch.float32, device=self.device)
         n_rows = int(sum(counts))
         seg_rows = torch.empty((n_rows, width), dtype=torch.float32, device=self.device) if rows else None
-        if out.shape[0]:
+        if out.shape[0] and idx is not None:
+            eo = E.NisqaEmbeddingOut(pooled=pooled.data_ptr() or None, rows=seg_rows.data_ptr() if rows else None,
+                                     n_rows=n_rows)
+            self.engine.predict_device_batch_shared_ref(self._stream(), deg, ref, idx, out.data_ptr(), eo,
+                                                        target_sr=self.target_sr)
+        elif out.shape[0]:
             self.engine.predict_device_batch_embeddings(self._stream(), deg, out.data_ptr(), pooled.data_ptr(),
                                                         seg_rows.data_ptr() if rows else 0, n_rows, ref=ref,
                                                         target_sr=self.target_sr)
-        return Embeddings(self._clip_rows(out, ref), self._clip_rows(pooled, ref), seg_rows, list(counts))
+        return Embeddings(self._clip_rows(out, ref, idx), self._clip_rows(pooled, ref, idx), seg_rows, list(counts))
 
     # ------------------------------------------------------------------ shared by __call__, segments and embed
-    def _arguments(self, wave, sample_rate, lengths, channel, reference, reference_lengths, reference_sample_rate):
-        """-> (deg, ref or None, segment counts of wave's clips) after every check, before anything is enqueued"""
+    def _arguments(self, wave, sample_rate, lengths, channel, reference, reference_lengths, reference_sample_rate,
+                   reference_index=None):
+        """-> (deg, ref or None, segment counts of wave's clips, reference_index as int32 or None) after every check,
+        before anything is enqueued"""
+        if reference_index is not None and not self.double_ended:
+            raise ValueError("reference_index: only a double-ended (NISQA_DE) checkpoint pairs clips with references")
         if self.double_ended and reference is None:
             raise ValueError("reference: a double-ended (NISQA_DE) checkpoint scores (wave, reference) pairs")
         if not self.double_ended and reference is not None:
@@ -470,24 +498,32 @@ class Scorer(object):
         if reference is not None:
             ref = self._batch("reference", reference, sample_rate if reference_sample_rate is None else reference_sample_rate,
                               reference_lengths, None)
-            if ref[0].n_clips != deg[0].n_clips:
+            if reference_index is None and ref[0].n_clips != deg[0].n_clips:
                 raise ValueError("reference: %d clips for %d clips of wave" % (ref[0].n_clips, deg[0].n_clips))
+        idx = None
+        if reference_index is not None:
+            idx = _host_ints("reference_index", reference_index, deg[0].n_clips)
+            bad = np.nonzero((idx < 0) | (idx >= ref[0].n_clips))[0]
+            if bad.size:
+                raise ValueError("reference_index[%d] = %d: not within 0 .. %d (the clips of reference)"
+                                 % (bad[0], idx[bad[0]], ref[0].n_clips - 1))
+            idx = idx.astype(np.int32)
         counts = self._check_segments("wave", deg[1], deg[0].sample_rate)
-        if ref is not None:
-            self._check_segments("reference", ref[1], ref[0].sample_rate)
-        return deg, ref, counts
+        if ref is not None:      # (shared references: the ones some clip names)
+            self._check_segments("reference", ref[1], ref[0].sample_rate, None if idx is None else np.unique(idx))
+        return deg, ref, counts, idx
 
-    def _scores_buffer(self, deg, ref):
-        n = deg[0].n_clips * (2 if ref is not None else 1)
+    def _scores_buffer(self, deg, ref, idx=None):
+        n = deg[0].n_clips * (2 if ref is not None and idx is None else 1)
         return torch.empty((n, len(self.columns)), dtype=torch.float32, device=self.device)
 
     def _stream(self):
         return torch.cuda.current_stream(self.device).cuda_stream
 
     @staticmethod
-    def _clip_rows(out, ref):
-        # (NISQA_DE: row 2p holds pair p's score, row 2p + 1 is the reference clip's NaN row)
-        return out[0::2].contiguous() if ref is not None else out
+    def _clip_rows(out, ref, idx=None):
+        # (NISQA_DE: row 2p holds pair p's score, row 2p + 1 is the reference clip's NaN row; shared references: compact)
+        return out[0::2].contiguous() if ref is not None and idx is None else out
 
     # ------------------------------------------------------------------ arguments
     def _batch(self, name, x, sample_rate, lengths, channel, min_len=1):
@@ -520,28 +556,24 @@ class Scorer(object):
         if lengths is None:
             ns = np.full(B, T, dtype=np.int64)
         else:
-            if isinstance(lengths, torch.Tensor) and lengths.device.type != "cpu":
-                raise TypeError("%s: host integers (a list, NumPy array or CPU tensor), not a CUDA tensor" % what)
-            ns = np.asarray(lengths.tolist() if isinstance(lengths, torch.Tensor) else lengths)
-            if ns.ndim != 1 or (ns.size and not np.issubdtype(ns.dtype, np.integer)):
-                raise TypeError("%s: one int per clip" % what)
-            ns = ns.astype(np.int64)
-            if ns.shape[0] != B:
-                raise ValueError("%s: %d entries for %d clips" % (what, ns.shape[0], B))
+            ns = _host_ints(what, lengths, B)
             bad = np.nonzero((ns < min_len) | (ns > T))[0]
             if bad.size:
                 raise ValueError("%s[%d] = %d: not within %d .. %d samples" % (what, bad[0], ns[bad[0]], min_len, T))
         fmt = E.FMT_S16 if x.dtype == torch.int16 else E.FMT_F32
         return E.device_batch(x3.data_ptr(), fmt, ns, C, ch, T, x3.stride(0), x3.stride(1), int(sample_rate))
 
-    def _check_segments(self, name, n_samples, sample_rate):
-        """The file ingest's too-short / too-long errors (NISQA_lib._raise_for_status), on the host, before any launch.
-        Returns each clip's segment count."""
+    def _check_segments(self, name, n_samples, sample_rate, which=None):
+        """The file ingest's too-short / too-long errors (NISQA_lib._raise_for_status), on the host, before any launch,
+        for every clip or the clips ``which`` names.  Returns each clip's segment count."""
         from . import resample as RS
         rate = self.target_sr or sample_rate
         a = self.args
         counts = []
         for i, n in enumerate(n_samples):
+            if which is not None and i not in which:
+                counts.append(0)
+                continue
             n = int(n) if rate == sample_rate else RS.out_len(int(n), sample_rate, rate)
             _, n_seg, status = E.segment_counts(self.cfg, n, rate)
             err = E.clip_status_error(status, "%s[%d]" % (name, i), n, rate, n_seg, a["ms_hop_length"], a["ms_seg_length"],
@@ -550,6 +582,25 @@ class Scorer(object):
                 raise err
             counts.append(n_seg)
         return counts
+
+
+def _host_ints(what, x, B):
+    """-> int64 [B] of a host-integer argument (a list, NumPy array or CPU tensor; ``lengths``, ``reference_index``)"""
+    if isinstance(x, torch.Tensor) and x.device.type != "cpu":
+        raise TypeError("%s: host integers (a list, NumPy array or CPU tensor), not a CUDA tensor" % what)
+    a = np.asarray(x.tolist() if isinstance(x, torch.Tensor) else x)
+    if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)):
+        raise TypeError("%s: one int per clip" % what)
+    a = a.astype(np.int64)
+    if a.shape[0] != B:
+        raise ValueError("%s: %d entries for %d clips" % (what, a.shape[0], B))
+    return a
+
+
+def _refuse_reference_index(reference_index, where):
+    if reference_index is not None:
+        raise ValueError("reference_index: %s takes one reference recording per recording; shared references are for "
+                         "clip pairs (__call__, segments, embed, align)" % where)
 
 
 class Feed(object):
