@@ -477,9 +477,11 @@ frontend_pp_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips
     f2 x[32];
     const int hopB = validB ? cd.hop : 0;
     const float2* wtab = fb.wtab + r * 1024 + lane;
-    // PCM16: 1023 + hop + shift < the slot's 1544 elements (hop <= 512 whenever win <= 1024), unfilled elements are
-    // finite integers under a zero window weight; float input could hold non-finite garbage there: clamped
-    const int nmax = sizeof(T) == 2 ? 4096 : cd.win - 1;
+    // the taps n >= win carry a zero weight: their index is clamped to win - 1, so that every read stays among the
+    // hop + win samples the slot was filled with (win - 1 + hop + shift < the slot's elements).  Unclamped, a hop over
+    // 512 (hop = win = 640: 20 ms at 32 kHz) would read past the slot into the FFT planes while other warps write them,
+    // and float input past the span could be non-finite.
+    const int nmax = cd.win - 1;
     constexpr int CH = 4;
 #pragma unroll
     for (int j0 = 0; j0 < 32; j0 += CH) {
@@ -488,7 +490,7 @@ frontend_pp_kernel(const T* __restrict__ pcm, const ClipDesc* __restrict__ clips
 #pragma unroll
       for (int u = 0; u < CH; ++u) {
         const int n = lane + 32 * (j0 + u);
-        const int ni = sizeof(T) == 2 ? n : min(n, nmax);
+        const int ni = min(n, nmax);
         wt[u] = __ldg(wtab + 32 * (j0 + u));
         sa[u] = (float)src[ni];
         sb[u] = (float)src[ni + hopB];

@@ -128,6 +128,24 @@ PY
 timeout 300 compute-sanitizer --tool racecheck --error-exitcode 7 --log-file $OUT/${TAG}_de_racecheck.log python /tmp/san_de.py > $OUT/${TAG}_de_racecheck_stdout.log 2>&1
 echo "de racecheck exit $?"
 tail -4 $OUT/${TAG}_de_racecheck.log; tail -2 $OUT/${TAG}_de_racecheck_stdout.log
+# frontend_pp_kernel with a hop over 512 (ms_hop_length = ms_win_length = 20 ms at 32 kHz: hop = win = 640): the input
+# stage's reads must stay inside the sample slot, clear of the FFT planes the other warps write; PCM16 and float32
+cat > /tmp/san_fe.py <<'PY'
+import os, sys
+sys.path.insert(0, os.getcwd())
+from nisqa_b200 import engine as E, synth
+from oracle import nisqa_oracle as O
+args, sd = O.load_checkpoint(os.path.join("weights", "nisqa_mos_only.tar"))
+e = E.Engine(E.config_from_args(dict(args, ms_hop_length=0.02, ms_win_length=0.02)), 0); e.load_state_dict(sd)
+x = synth.synth_speech_pcm16(19, 1.3, 32000)
+print("hop 640", e.predict_pcm([x], [32000])[0].tolist(), e.predict_pcm([x.astype("float32") / 32768], [32000])[0].tolist())
+e.close()
+PY
+for tool in racecheck memcheck; do
+  timeout 300 compute-sanitizer --tool $tool --error-exitcode 7 --log-file $OUT/${TAG}_fe_hop640_$tool.log python /tmp/san_fe.py > $OUT/${TAG}_fe_hop640_${tool}_stdout.log 2>&1
+  echo "fe hop 640 $tool exit $?"
+  tail -4 $OUT/${TAG}_fe_hop640_$tool.log; tail -1 $OUT/${TAG}_fe_hop640_${tool}_stdout.log
+done
 # shared-memory hazards (racecheck) and uninitialised device reads (initcheck) of the whole run (RACE=1)
 [ -z "$RACE" ] && exit 0
 timeout 400 compute-sanitizer --tool racecheck --error-exitcode 7 --log-file $OUT/${TAG}_racecheck.log python /tmp/san_run.py > $OUT/${TAG}_racecheck_stdout.log 2>&1
