@@ -34,8 +34,7 @@ __global__ void __launch_bounds__(256, 2)
 conv1_pool1_kernel(const float* __restrict__ mel, int n_mels, int seg_len, const int* __restrict__ seg_frame0,
                    const float* __restrict__ seg_thr, const float* __restrict__ w1 /*[9][C1]*/,
                    const float* __restrict__ b1 /*[C1]*/, float* __restrict__ out,
-                   unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo,
-                   float store_scale /*2^-e1*/, int n_seg, int PH, int PW) {
+                   unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo, int n_seg, int PH, int PW) {
   static_assert(C1 == 16 || (MODE == 0 && SPLIT), "StandardCNN and the fp32 output: 16 channels");
   __shared__ __align__(16) float ws[9 * C1 + C1];
   for (int i = threadIdx.x; i < 9 * C1 + C1; i += blockDim.x)
@@ -57,7 +56,7 @@ conv1_pool1_kernel(const float* __restrict__ mel, int n_mels, int seg_len, const
     for (int c = 0; c < 2; ++c) {
       uint4 hi, lo;
       split8(make_float4(res[8 * c], res[8 * c + 1], res[8 * c + 2], res[8 * c + 3]),
-             make_float4(res[8 * c + 4], res[8 * c + 5], res[8 * c + 6], res[8 * c + 7]), store_scale, hi, lo);
+             make_float4(res[8 * c + 4], res[8 * c + 5], res[8 * c + 6], res[8 * c + 7]), hi, lo);
       const size_t o = split_off<2 * C1>(g, 2 * cg + c);
       *reinterpret_cast<uint4*>(out_hi + o) = hi;
       *reinterpret_cast<uint4*>(out_lo + o) = lo;
@@ -285,23 +284,22 @@ static void launch_conv(cudaStream_t st, const float* in, const float* w, const 
 
 bool launch_conv1(cudaStream_t st, int std_mode, int c1, const float* mel, int n_mels, int seg_len, const int* seg_frame0,
                   const float* seg_thr, const float* w1, const float* b1, float* out, int n_seg, void* out_hi, void* out_lo,
-                  float store_scale, int ph, int pw) {
+                  int ph, int pw) {
   if (c1 != 16 && (std_mode || !out_hi || (c1 != 32 && c1 != 64))) return false;
   if (std_mode) { ph = 24; pw = 8; }
   const long long total = (long long)n_seg * ph * pw;
   const int grid = (int)((total + 255) / 256);
   unsigned char* oh = static_cast<unsigned char*>(out_hi);
   unsigned char* ol = static_cast<unsigned char*>(out_lo);
-  const float s = store_scale;
   const int H = n_mels, W = seg_len;
   if (out_hi) {
-    if (std_mode) conv1_pool1_kernel<1, true><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg, ph, pw);
-    else if (c1 == 32) conv1_pool1_kernel<0, true, 32><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg, ph, pw);
-    else if (c1 == 64) conv1_pool1_kernel<0, true, 64><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg, ph, pw);
-    else conv1_pool1_kernel<0, true><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg, ph, pw);
+    if (std_mode) conv1_pool1_kernel<1, true><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, n_seg, ph, pw);
+    else if (c1 == 32) conv1_pool1_kernel<0, true, 32><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, n_seg, ph, pw);
+    else if (c1 == 64) conv1_pool1_kernel<0, true, 64><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, n_seg, ph, pw);
+    else conv1_pool1_kernel<0, true><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, n_seg, ph, pw);
   } else {
-    if (std_mode) conv1_pool1_kernel<1, false><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg, ph, pw);
-    else conv1_pool1_kernel<0, false><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, s, n_seg, ph, pw);
+    if (std_mode) conv1_pool1_kernel<1, false><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, n_seg, ph, pw);
+    else conv1_pool1_kernel<0, false><<<grid, 256, 0, st>>>(mel, H, W, seg_frame0, seg_thr, w1, b1, out, oh, ol, n_seg, ph, pw);
   }
   return true;
 }

@@ -6,10 +6,13 @@
 //      a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi          (dropped a_lo*b_lo ~ 2^-22 |a b|)
 // The main accumulator only ever sees the hi*hi products; hi*lo and lo*hi go to a second, small accumulator, and the
 // epilogue adds the two.  The weights are pre-scaled by 2^S on the host (S chosen per layer so that max|w| 2^S <= 1024)
-// to keep b_lo out of the fp16 subnormal range; the epilogue multiplies by 2^-S (exact).  Activations are stored
-// multiplied by 2^-e (e per layer, from its folded BatchNorm) for the same reason; the consuming layer's epilogue
-// multiplies by 2^(e_in - S).  Every stored fp16 value is therefore unchanged when a checkpoint is rescaled by
-// powers of two (BatchNorm i times 2^k, conv i+1 times 2^-k), and so is every score.
+// to keep b_lo out of the fp16 subnormal range; the epilogue multiplies by 2^-S (exact).  Activations are stored as
+// v 2^-e_c for the same reason, with one exponent e_c per channel, from that channel's folded BatchNorm: the producing
+// layer's weights and bias carry 2^-e_c for output channel c and the consuming layer's weights 2^e_c for input channel
+// c (pack_weights), so a channel whose range lies far below the layer's largest keeps its 22 bits.  Every stored fp16
+// value, packed weight and scale is therefore unchanged when a checkpoint is rescaled by powers of two, per layer or
+// per channel (BatchNorm i channel c times 2^k_c, input channel c of conv i+1 times 2^-k_c), and so is every score.
+// conv6 writes fp32 features: its epilogue multiplies channel c back by 2^e_c (exact).
 //
 // The activations travel BETWEEN the layers already in the form the GEMM consumes: two fp16 planes (hi, lo), laid out
 // in HBM as the exact shared-memory image of the A tile:
@@ -176,7 +179,7 @@ __device__ __forceinline__ void stage_rows(const Geo& g, const float (&acc_m)[C:
 // epilogue part 2 (threads t0, t0 + nthr, ...): staging tile -> max-pool / split / store of the tile's nvalid segments
 template <class C, class Geo>
 __device__ __forceinline__ void store_tile(const Geo& g, const float* stg, int seg0, int nvalid, int t0, int nthr,
-                                           float store_scale, unsigned char* __restrict__ out_hi,
+                                           const float* __restrict__ out_unit, unsigned char* __restrict__ out_hi,
                                            unsigned char* __restrict__ out_lo, float* __restrict__ out_f32) {
   constexpr int COUT = C::COUT, SS = C::STG_STRIDE;
   const int H = g.H, W = g.W, P = g.P, BLK = g.BLK;
@@ -206,7 +209,7 @@ __device__ __forceinline__ void store_tile(const Geo& g, const float* stg, int s
           mb.x = fmaxf(mb.x, tb.x); mb.y = fmaxf(mb.y, tb.y); mb.z = fmaxf(mb.z, tb.z); mb.w = fmaxf(mb.w, tb.w);
         }
       uint4 hi, lo;
-      split8(ma, mb, store_scale, hi, lo);
+      split8(ma, mb, hi, lo);
       const int gr = kSplitLead + (seg0 + s) * g.OBLK + (ph + 1) * g.OP + (pw + 1);
       const size_t o = split_off<C::OROWB>(gr, c8);
       *reinterpret_cast<uint4*>(out_hi + o) = hi;
@@ -221,21 +224,29 @@ __device__ __forceinline__ void store_tile(const Geo& g, const float* stg, int s
       uint4 hi = make_uint4(0u, 0u, 0u, 0u), lo = hi;
       if (hh >= 1 && ww >= 1) {
         const float4* tp = reinterpret_cast<const float4*>(stg + r * SS + c8 * 8);
-        split8(tp[0], tp[1], store_scale, hi, lo);
+        split8(tp[0], tp[1], hi, lo);
       }
       const size_t o = split_off<C::OROWB>(kSplitLead + seg0 * BLK + r, c8);
       *reinterpret_cast<uint4*>(out_hi + o) = hi;
       *reinterpret_cast<uint4*>(out_lo + o) = lo;
     }
   } else {
-    // fp32 CNN features, channels-last [seg][HO][WO][COUT] in rows of OUT_LD floats (the last layer does not pool)
+    // fp32 CNN features, channels-last [seg][HO][WO][COUT] in rows of OUT_LD floats (the last layer does not pool), channel
+    // c times out_unit[c] = 2^e_c.  nthr (conv_split_kernel's NT) is a multiple of C4: every item of this thread has
+    // c4 = t0 % C4
     constexpr int C4 = COUT / 4;
+    static_assert(C::NT % C4 == 0, "a thread's fp32 feature items must share their channel quad");
+    const float4 u = __ldg(reinterpret_cast<const float4*>(out_unit) + t0 % C4);
+    auto feat = [&](int r, int c4) {
+      const float4 v = *reinterpret_cast<const float4*>(stg + r * SS + c4 * 4);
+      return make_float4(v.x * u.x, v.y * u.y, v.z * u.z, v.w * u.w);
+    };
     if constexpr (C::RT) {
       // conv6 of a run-time geometry: one column, [seg][H][COUT]
       for (int i = t0; i < nvalid * H * C4; i += nthr) {
         const int c4 = i % C4, rest = i / C4, h = rest % H, s = rest / H;
         *reinterpret_cast<float4*>(out_f32 + (size_t)(seg0 + s) * g.OUT_LD + h * COUT + c4 * 4) =
-            *reinterpret_cast<const float4*>(stg + (s * BLK + (h + 1) * P + g.X0) * SS + c4 * 4);
+            feat(s * BLK + (h + 1) * P + g.X0, c4);
       }
     } else {
       constexpr int HO = C::HO, WO = C::WO;
@@ -248,7 +259,7 @@ __device__ __forceinline__ void store_tile(const Geo& g, const float* stg, int s
         const int r = s * BLK + (h + 1) * P + (w + g.X0);
         float* dst = g.OUT_LD == g.OUT_COLS ? out_f32 + ((size_t)(seg0 + s) * (HO * WO) + h * WO + w) * COUT + c4 * 4
                                             : out_f32 + (size_t)(seg0 + s) * g.OUT_LD + (h * WO + w) * COUT + c4 * 4;
-        *reinterpret_cast<float4*>(dst) = *reinterpret_cast<const float4*>(stg + r * SS + c4 * 4);
+        *reinterpret_cast<float4*>(dst) = feat(r, c4);
       }
     }
     // the padding columns are written as zeros: the Linear behind reads them (against zero weights)
@@ -272,9 +283,10 @@ template <class C>
 __global__ void __launch_bounds__(C::NT, 1)
 conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* __restrict__ in_lo,
                   const __half* __restrict__ wtc /*[NTAP][CIN/8][hi co | lo co][8] fp16, scaled by 2^S*/,
-                  const float* __restrict__ bias, float out_scale /*2^(e_in - S)*/, float store_scale /*2^-e_out*/,
-                  unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo,
-                  float* __restrict__ out_f32 /*last layer only*/, int n_seg, const SpGeom geo) {
+                  const float* __restrict__ bias, float out_scale /*2^-S*/,
+                  const float* __restrict__ out_unit /*[COUT] 2^e_c, last layer only*/, unsigned char* __restrict__ out_hi,
+                  unsigned char* __restrict__ out_lo, float* __restrict__ out_f32 /*last layer only*/, int n_seg,
+                  const SpGeom geo) {
   constexpr int ROWB = C::ROWB, NT = C::NT, NTAP = C::NTAP;
   const auto g = C::geom(geo);
   const int G = g.G, BLK = g.BLK, HALO = g.HALO;
@@ -363,7 +375,7 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
     __syncthreads();
 
     // ===== epilogue part 2 (all threads): max-pool / split / store =====
-    store_tile<C>(g, stg, seg0, min(G, n_seg - seg0), tid, NT, store_scale, out_hi, out_lo, out_f32);
+    store_tile<C>(g, stg, seg0, min(G, n_seg - seg0), tid, NT, out_unit, out_hi, out_lo, out_f32);
     if constexpr (C::ALIAS) {
       fence_proxy_async();                       // staging stores (generic proxy) before the next tile's bulk copy
       __syncthreads();
@@ -390,11 +402,10 @@ conv_split_kernel(const unsigned char* __restrict__ in_hi, const unsigned char* 
 // after the first named barrier of its next tile, which each of its threads reaches after its part of the store.
 template <class C, int MODE>
 __global__ void __launch_bounds__(C::NT, 1)
-conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, float out_scale, float store_scale,
+conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, float out_scale,
               unsigned char* __restrict__ out_hi, unsigned char* __restrict__ out_lo, int n_seg,
               const float* __restrict__ mel, const int* __restrict__ seg_frame0, const float* __restrict__ seg_thr,
-              const float* __restrict__ w1 /*[9][16]*/, const float* __restrict__ b1 /*[16]*/,
-              float c1_scale /*2^-e1: conv1's activation scale*/) {
+              const float* __restrict__ w1 /*[9][16], channel c times 2^-e_c*/, const float* __restrict__ b1 /*[16]*/) {
   using L = SpFused<C>;
   constexpr C g{};
   constexpr int W = C::W, P = C::P, HALO = C::HALO, ROWB = C::ROWB, NT = C::NT, NR = NT / 2, AB = L::A_BUFS;
@@ -461,7 +472,7 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
 #pragma unroll
       for (int b = 0; b < 3; ++b) stage_rows<C>(g, acc_m[b], acc_s[b], am + 64 * b, acol, tile, n_seg, bb, out_scale, stg);
       named_bar_sync<128>(own_bar);
-      store_tile<C>(g, stg, tile, 1, tid - 128 * wg, 128, store_scale, out_hi, out_lo, nullptr);
+      store_tile<C>(g, stg, tile, 1, tid - 128 * wg, 128, nullptr, out_hi, out_lo, nullptr);
     }
   } else {
     // ===== worker warpgroups =====
@@ -522,7 +533,7 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
       const float thr = ring_thr[s];
       auto emit = [&](int pw, const float (&res)[4]) {
         uint2 hi, lo;
-        split4(make_float4(res[0], res[1], res[2], res[3]), c1_scale, hi, lo);
+        split4(make_float4(res[0], res[1], res[2], res[3]), hi, lo);
         const uint32_t o = (uint32_t)split_off<ROWB>(HALO + (ph + 1) * P + (pw + 1), cq >> 1) + 8 * (cq & 1);
         *reinterpret_cast<uint2*>(a + o) = hi;
         *reinterpret_cast<uint2*>(a + C::A_BYTES + o) = lo;
@@ -539,11 +550,11 @@ conv12_kernel(const __half* __restrict__ wtc, const float* __restrict__ bias, fl
   }
 }
 
-// planes -> fp32 channels-last [seg][H][W][C] (stage dumps for the parity tests; x_hi + x_lo == x 2^-e to 2^-22,
-// unit = 2^e undoes the activation scale exactly)
+// planes -> fp32 channels-last [seg][H][W][C] (stage dumps for the parity tests; x_hi + x_lo == x 2^-e_c to 2^-22,
+// unit[c] = 2^e_c undoes the activation scale of channel c exactly)
 template <int ROWB>
 __global__ void unsplit_kernel(const unsigned char* __restrict__ hi, const unsigned char* __restrict__ lo,
-                               float* __restrict__ out, long long n_items, int H, int W, float unit) {
+                               float* __restrict__ out, long long n_items, int H, int W, const float* __restrict__ unit) {
   constexpr int C8 = ROWB / 16;
   const int P = W + 1, BLK = (H + 1) * P;
   for (long long it = (long long)blockIdx.x * blockDim.x + threadIdx.x; it < n_items; it += (long long)gridDim.x * blockDim.x) {
@@ -561,7 +572,7 @@ __global__ void unsplit_kernel(const unsigned char* __restrict__ hi, const unsig
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const float2 x = __half22float2(ah[i]), y = __half22float2(bh[i]);
-      r[2 * i] = (x.x + y.x) * unit; r[2 * i + 1] = (x.y + y.y) * unit;
+      r[2 * i] = (x.x + y.x) * __ldg(unit + 8 * c8 + 2 * i); r[2 * i + 1] = (x.y + y.y) * __ldg(unit + 8 * c8 + 2 * i + 1);
     }
     float4* dst = reinterpret_cast<float4*>(out + it * 8);
     dst[0] = make_float4(r[0], r[1], r[2], r[3]);
@@ -579,7 +590,7 @@ static int device_sms() {
 // geo: a run-time geometry type's geometry (compile-time types have theirs)
 template <class C>
 static void launch_sp(cudaStream_t st, const unsigned char* in_hi, const unsigned char* in_lo, const __half* wtc,
-                      const float* b, float scale, float store_scale, unsigned char* out_hi, unsigned char* out_lo,
+                      const float* b, float scale, const float* out_unit, unsigned char* out_hi, unsigned char* out_lo,
                       float* out_f32, int n_seg, const SpGeom& geo = SpGeom{}) {
   static unsigned long long configured = 0;
   static int n_sm = 0;
@@ -589,14 +600,14 @@ static void launch_sp(cudaStream_t st, const unsigned char* in_hi, const unsigne
   }
   const int n_tiles = (n_seg + C::geom(geo).G - 1) / C::geom(geo).G;
   const int grid = std::min(n_tiles, n_sm);              // one persistent CTA per SM
-  conv_split_kernel<C><<<grid, C::NT, C::SMEM_BYTES, st>>>(in_hi, in_lo, wtc, b, scale, store_scale, out_hi, out_lo,
+  conv_split_kernel<C><<<grid, C::NT, C::SMEM_BYTES, st>>>(in_hi, in_lo, wtc, b, scale, out_unit, out_hi, out_lo,
                                                            out_f32, n_seg, geo);
 }
 
 template <class C, int MODE>
-static void launch_c12(cudaStream_t st, const __half* wtc, const float* b, float scale, float store_scale,
-                       unsigned char* out_hi, unsigned char* out_lo, int n_seg, const float* mel, const int* seg_frame0,
-                       const float* seg_thr, const float* w1, const float* b1, float c1_scale) {
+static void launch_c12(cudaStream_t st, const __half* wtc, const float* b, float scale, unsigned char* out_hi,
+                       unsigned char* out_lo, int n_seg, const float* mel, const int* seg_frame0, const float* seg_thr,
+                       const float* w1, const float* b1) {
   static unsigned long long configured = 0;
   static int n_sm = 0;
   if (first_launch_on_device(configured)) {
@@ -604,8 +615,8 @@ static void launch_c12(cudaStream_t st, const __half* wtc, const float* b, float
     n_sm = device_sms();
   }
   const int grid = std::min(n_seg, n_sm);                // one persistent CTA per SM, one segment per tile
-  conv12_kernel<C, MODE><<<grid, C::NT, SpFused<C>::SMEM_BYTES, st>>>(wtc, b, scale, store_scale, out_hi, out_lo, n_seg,
-                                                                      mel, seg_frame0, seg_thr, w1, b1, c1_scale);
+  conv12_kernel<C, MODE><<<grid, C::NT, SpFused<C>::SMEM_BYTES, st>>>(wtc, b, scale, out_hi, out_lo, n_seg, mel, seg_frame0,
+                                                                      seg_thr, w1, b1);
 }
 
 #define NISQA_SP_GEOM(L, CI, CO) static_assert(input_is<SpAdapt<L, CI, CO>>(0, L), "SpCfg geometry differs from split_geometry");
@@ -633,7 +644,7 @@ bool conv_split_supported(int cin, int cout) {
 // AdaptCNN layers whose input map and output pooling are the shipped ones run the compile-time instances, every other
 // one a run-time geometry instance.  false: no instance for the shape.
 bool launch_conv_split(cudaStream_t st, int std_mode, int layer, int cin, int cout, const void* in_hi, const void* in_lo,
-                       const void* wtc, const float* b, float out_scale, float store_scale, void* out_hi,
+                       const void* wtc, const float* b, float out_scale, const float* out_unit, void* out_hi,
                        void* out_lo, float* out_f32, int n_seg, const CnnPools& pools) {
   const __half* w = reinterpret_cast<const __half*>(wtc);
   const unsigned char* ih = static_cast<const unsigned char*>(in_hi);
@@ -643,18 +654,18 @@ bool launch_conv_split(cudaStream_t st, int std_mode, int layer, int cin, int co
   if (std_mode) {
     if (cin != split_geometry(1, layer, 0).C || cout != (layer == 2 ? 32 : 64)) return false;
     switch (layer) {
-      case 2: launch_sp<SpConv2S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 3: launch_sp<SpConv3S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 4: launch_sp<SpConv4S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      case 5: launch_sp<SpConv5S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
-      default: launch_sp<SpConv6S>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg); break;
+      case 2: launch_sp<SpConv2S>(st, ih, il, w, b, out_scale, out_unit, oh, ol, out_f32, n_seg); break;
+      case 3: launch_sp<SpConv3S>(st, ih, il, w, b, out_scale, out_unit, oh, ol, out_f32, n_seg); break;
+      case 4: launch_sp<SpConv4S>(st, ih, il, w, b, out_scale, out_unit, oh, ol, out_f32, n_seg); break;
+      case 5: launch_sp<SpConv5S>(st, ih, il, w, b, out_scale, out_unit, oh, ol, out_f32, n_seg); break;
+      default: launch_sp<SpConv6S>(st, ih, il, w, b, out_scale, out_unit, oh, ol, out_f32, n_seg); break;
     }
     return true;
   }
   if (shipped_layer_geometry(layer, pools)) {
 #define NISQA_SP_LAUNCH(L, CI, CO)                                                                           \
     if (layer == L && cin == CI && cout == CO) {                                                              \
-      launch_sp<SpAdapt<L, CI, CO>>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg);        \
+      launch_sp<SpAdapt<L, CI, CO>>(st, ih, il, w, b, out_scale, out_unit, oh, ol, out_f32, n_seg);        \
       return true;                                                                                            \
     }
     NISQA_SP_ADAPT_LAYERS(NISQA_SP_LAUNCH)
@@ -668,7 +679,7 @@ bool launch_conv_split(cudaStream_t st, int std_mode, int layer, int cin, int co
   const int ntap = layer == 6 ? 3 * in.W : 9;
 #define NISQA_SP_RT_LAUNCH(L, CI, CO, NT)                                                                    \
   if (layer == L && cin == CI && cout == CO && ntap == NT) {                                                  \
-    launch_sp<SpRt<L, CI, CO, NT>>(st, ih, il, w, b, out_scale, store_scale, oh, ol, out_f32, n_seg, g);      \
+    launch_sp<SpRt<L, CI, CO, NT>>(st, ih, il, w, b, out_scale, out_unit, oh, ol, out_f32, n_seg, g);      \
     return true;                                                                                              \
   }
   NISQA_SP_RT_LAYERS(NISQA_SP_RT_LAUNCH)
@@ -680,20 +691,20 @@ bool conv12_supported(int std_mode, int c1, int c2) { return c1 == 16 && (c2 == 
 
 // conv1 + pool1 + conv2 + pool2 in one kernel: mel segments -> the plane pair feeding conv3 (conv12_supported shapes)
 void launch_conv12(cudaStream_t st, int std_mode, int c2, const float* mel, const int* seg_frame0, const float* seg_thr,
-                   const float* w1, const float* b1, float c1_scale, const void* wtc2, const float* bias2,
-                   float scale2, float store_scale, void* out_hi, void* out_lo, int n_seg) {
+                   const float* w1, const float* b1, const void* wtc2, const float* bias2, float scale2, void* out_hi,
+                   void* out_lo, int n_seg) {
   const __half* w = reinterpret_cast<const __half*>(wtc2);
   unsigned char* oh = static_cast<unsigned char*>(out_hi);
   unsigned char* ol = static_cast<unsigned char*>(out_lo);
   if (std_mode)
-    launch_c12<SpConv2S, 1>(st, w, bias2, scale2, store_scale, oh, ol, n_seg, mel, seg_frame0, seg_thr, w1, b1, c1_scale);
+    launch_c12<SpConv2S, 1>(st, w, bias2, scale2, oh, ol, n_seg, mel, seg_frame0, seg_thr, w1, b1);
   else if (c2 == 16)
-    launch_c12<SpAdapt<2, 16, 16>, 0>(st, w, bias2, scale2, store_scale, oh, ol, n_seg, mel, seg_frame0, seg_thr, w1, b1, c1_scale);
+    launch_c12<SpAdapt<2, 16, 16>, 0>(st, w, bias2, scale2, oh, ol, n_seg, mel, seg_frame0, seg_thr, w1, b1);
   else
-    launch_c12<SpConv2A, 0>(st, w, bias2, scale2, store_scale, oh, ol, n_seg, mel, seg_frame0, seg_thr, w1, b1, c1_scale);
+    launch_c12<SpConv2A, 0>(st, w, bias2, scale2, oh, ol, n_seg, mel, seg_frame0, seg_thr, w1, b1);
 }
 
-void launch_unsplit(cudaStream_t st, int std_mode, int layer, int C, const void* hi, const void* lo, float unit, float* out,
+void launch_unsplit(cudaStream_t st, int std_mode, int layer, int C, const void* hi, const void* lo, const float* unit, float* out,
                     int n_seg, const CnnPools& pools) {
   const ConvGeom g = split_geometry(std_mode, layer, C, pools);
   const long long items = (long long)n_seg * g.H * g.W * (g.C / 8);

@@ -171,7 +171,11 @@ struct Linear { const float* wT = nullptr; const float* b = nullptr; };    // k-
 struct ConvWeights {
   const float* w = nullptr;      // [ci][tap][co] fp32, BatchNorm folded in (conv1, and conv2..6 on the FFMA path)
   const float* b = nullptr;      // [co]
-  const float* wtc = nullptr;    // conv2..6 on the tensor cores: fp16 hi / lo split (pack_conv_tc)
+  // The tensor-core path stores output channel c as v 2^-e_c (pack_conv): its weights and bias carry that factor
+  const float* w_split = nullptr;  // conv1: w, channel c times 2^-e_c
+  const float* b_split = nullptr;  // [co] b 2^-e_c
+  const float* wtc = nullptr;      // conv2..6: fp16 hi / lo split (pack_conv_tc)
+  const float* unit = nullptr;     // [co] 2^e_c: channel c's value from what the path stores (stage dumps, conv6 features)
 };
 constexpr int kMaxSaLayers = 8;  // nisqa_create's limit on sa_layers / td2_layers
 struct SaStackWeights {
@@ -251,9 +255,7 @@ struct nisqa_engine {
   // nisqa_predict_device_batch_embeddings: Weights.pool_src on the device (unset when the rows are in the reference's
   // order)
   DevBuf emb_src;
-  float tc_scale[8] = {1, 1, 1, 1, 1, 1, 1, 1};   // 2^(e_{i-1} - S_i): undoes the activation and weight pre-scales of conv i
-  int act_exp[8] = {0, 0, 0, 0, 0, 0, 0, 0};      // e_i: conv i's activations are stored as fp16 planes of v * 2^-e_i
-  float act_store(int i) const { return ldexpf(1.f, -act_exp[i]); }
+  float tc_scale[8] = {1, 1, 1, 1, 1, 1, 1, 1};   // 2^-S_i: undoes the weight pre-scale of conv i on the tensor cores
   // widths of the self-attention stacks (0 in the config = 64) and of the rows the pooling module reads
   int sa_d() const { return cfg.sa_d_model ? cfg.sa_d_model : 64; }
   int sa_f() const { return cfg.sa_ff ? cfg.sa_ff : 64; }
@@ -626,9 +628,30 @@ struct Packer {
   void copy(const float*& dst, const float* src, size_t n) { memcpy(&arena[alloc(dst, n)], src, n * 4); }
 };
 
+// Activation exponents of conv<idx>'s output channels (BatchNorm tensors g, be): e_c = ilogb(E_c sqrt(2) / 4) of the
+// channel's BN output estimate E_c = |beta_c| + 3 |gamma_c| (three standard deviations), so that the stored v 2^-e_c
+// lies in [2.8, 5.7) at E_c.  e_c moves by exactly k when channel c's BatchNorm weight and bias are multiplied by 2^k.
+// It is kept at most kExpWindow binades below the layer's largest: a dead channel (E_c zero or denormal) must not push a
+// folded weight out of fp32 range.
+constexpr int kExpWindow = 64;
+std::vector<int> act_exponents(const TensorView* g, const TensorView* be, int cout) {
+  std::vector<double> E(cout);
+  double emax = 0.0;
+  for (int co = 0; co < cout; ++co) {
+    E[co] = fabs((double)be->d[co]) + 3.0 * fabs((double)g->d[co]);
+    if (std::isfinite(E[co])) emax = std::max(emax, E[co]);
+  }
+  const int top = emax > 0.0 ? ilogb(emax * sqrt(2.0) / 4.0) : 0, floor = top - kExpWindow;
+  std::vector<int> e(cout, floor);
+  for (int co = 0; co < cout; ++co)
+    if (E[co] > 0.0 && std::isfinite(E[co])) e[co] = std::max(floor, ilogb(E[co] * sqrt(2.0) / 4.0));
+  return e;
+}
+
 // conv<idx> (kernel 3 x kw: AdaptCNN's conv6 is 3 x pool_3[1]) with bn<idx> folded in, as [ci][tap][co] (conv1: [tap][16]),
-// tap = ky kw + kx; *w_off: the offset of the weights in the arena
-bool pack_conv(Packer& P, int idx, int cin, int cout, int* act_exp, size_t* w_off, int kw = 3) {
+// for the FFMA path; the tensor-core path's bias (and conv1's weights) with 2^-e_c folded into output channel c, and 2^e_c.
+// *e: the activation exponents of the output channels; *w_off: the offset of the fp32 weights in the arena
+bool pack_conv(Packer& P, int idx, int cin, int cout, std::vector<int>* e, size_t* w_off, int kw = 3) {
   const std::string cv = "cnn.model.conv" + std::to_string(idx) + ".", bn = "cnn.model.bn" + std::to_string(idx) + ".";
   const int ntap = 3 * kw;
   const TensorView* w = P.get(cv + "weight", {cout, cin, 3, kw});
@@ -638,13 +661,11 @@ bool pack_conv(Packer& P, int idx, int cin, int cout, int* act_exp, size_t* w_of
   const TensorView* mu = P.get(bn + "running_mean", {cout});
   const TensorView* var = P.get(bn + "running_var", {cout});
   if (!w || !b || !g || !be || !mu || !var) return false;
-  // activation exponent: max_c |beta_c| + 3 |gamma_c| (the BN output at three standard deviations) -> [2.8, 5.7) 2^e.
-  // It moves by exactly k when BatchNorm's weight and bias are multiplied by 2^k.
-  double E = 0.0;
-  for (int co = 0; co < cout; ++co) E = std::max(E, fabs((double)be->d[co]) + 3.0 * fabs((double)g->d[co]));
-  *act_exp = (E > 0.0 && std::isfinite(E)) ? ilogb(E * sqrt(2.0) / 4.0) : 0;
-  const size_t wo = P.alloc(P.w.conv[idx].w, (size_t)cin * ntap * cout);
-  const size_t bo = P.alloc(P.w.conv[idx].b, cout);
+  *e = act_exponents(g, be, cout);
+  ConvWeights& cw = P.w.conv[idx];
+  const size_t wo = P.alloc(cw.w, (size_t)cin * ntap * cout);
+  const size_t bo = P.alloc(cw.b, cout), bso = P.alloc(cw.b_split, cout), uo = P.alloc(cw.unit, cout);
+  const size_t wso = idx == 1 ? P.alloc(cw.w_split, (size_t)ntap * cout) : 0;
   for (int co = 0; co < cout; ++co) {
     // eval-mode BatchNorm2d (eps 1e-5) folded into the convolution (SURVEY.md Appendix A)
     const double s = (double)g->d[co] / sqrt((double)var->d[co] + 1e-5);
@@ -653,29 +674,44 @@ bool pack_conv(Packer& P, int idx, int cin, int cout, int* act_exp, size_t* w_of
       for (int tap = 0; tap < ntap; ++tap)
         P.arena[wo + ((size_t)ci * ntap + tap) * cout + co] =
             (float)((double)w->d[((size_t)co * cin + ci) * ntap + tap] * s);
+    // powers of two of the fp32 values: exact
+    P.arena[bso + co] = (float)ldexp((double)P.arena[bo + co], -(*e)[co]);
+    P.arena[uo + co] = (float)ldexp(1.0, (*e)[co]);
+    if (idx == 1)
+      for (int tap = 0; tap < ntap; ++tap)
+        P.arena[wso + (size_t)tap * cout + co] = (float)ldexp((double)P.arena[wo + (size_t)tap * cout + co], -(*e)[co]);
   }
   *w_off = wo;
   return true;
 }
 
 // conv2..conv6 for the tensor-core path, from the folded fp32 weights at `src` (ntap taps): [tap][ci/8][hi co | lo co][8]
-// fp16 two-term split of w * 2^S, S chosen so that max|w| 2^S lies in (512, 1024] whatever the weights' range (b_lo stays
-// out of the fp16 subnormals)
-void pack_conv_tc(Packer& P, int idx, int ci_n, int co_n, size_t src, int act_exp_in, float* tc_scale, int ntap = 9) {
+// fp16 two-term split of w 2^(e_in[ci] - e_out[co] + S): input channel ci stored at 2^-e_in[ci], output channel co to be
+// stored at 2^-e_out[co] (pack_conv), and S chosen so that the largest of these lies in (512, 1024] whatever the weights'
+// range (b_lo stays out of the fp16 subnormals)
+void pack_conv_tc(Packer& P, int idx, int ci_n, int co_n, size_t src, const std::vector<int>& e_in,
+                  const std::vector<int>& e_out, float* tc_scale, int ntap = 9) {
+  std::vector<float> ws((size_t)ci_n * ntap * co_n);
   float wmax = 0.f;
-  for (size_t j = 0; j < (size_t)ci_n * ntap * co_n; ++j) wmax = std::max(wmax, fabsf(P.arena[src + j]));
+  for (int ci = 0; ci < ci_n; ++ci)
+    for (int tap = 0; tap < ntap; ++tap)
+      for (int co = 0; co < co_n; ++co) {
+        const size_t j = ((size_t)ci * ntap + tap) * co_n + co;
+        ws[j] = (float)ldexp((double)P.arena[src + j], e_in[ci] - e_out[co]);
+        wmax = std::max(wmax, fabsf(ws[j]));
+      }
   int S = 0;
   if (wmax > 0.f && std::isfinite(wmax)) {
     S = 9 - ilogbf(wmax);                                         // max|w| 2^S in [512, 1024)
     if (ldexpf(wmax, S) == 512.f) ++S;                            // a power of two: 1024 itself
   }
-  *tc_scale = ldexpf(1.f, act_exp_in - S);
+  *tc_scale = ldexpf(1.f, -S);
   const size_t n_half = (size_t)ntap * 2 * ci_n * co_n;
   const size_t dst = P.alloc(P.w.conv[idx].wtc, (n_half + 1) / 2);   // fp16 payload inside the float arena
   for (int tap = 0; tap < ntap; ++tap)
     for (int ci = 0; ci < ci_n; ++ci)
       for (int co = 0; co < co_n; ++co) {
-        const float w = ldexpf(P.arena[src + ((size_t)ci * ntap + tap) * co_n + co], S);
+        const float w = ldexpf(ws[((size_t)ci * ntap + tap) * co_n + co], S);
         const __half hi = __float2half_rn(w);
         const __half lo = __float2half_rn(w - __half2float(hi));
         __half* base = reinterpret_cast<__half*>(&P.arena[dst]) + (size_t)tap * 2 * ci_n * co_n;
@@ -789,11 +825,12 @@ bool pack_framewise(Packer& P, nisqa_engine* e) {
     return P.fail("tensor cnn.model.conv6.weight: " + std::to_string(cc[6]) + " channels x pool_3 height " + std::to_string(h3) +
                   " = " + std::to_string(h3 * cc[6]) + " features (cnn_c_out_3 x cnn_pool_3[0]): the engine runs up to " +
                   std::to_string(kMaxCnnFeatures));
+  std::vector<int> ex[7];                  // ex[i][c]: the activation exponent of conv i's output channel c
   for (int i = 1; i <= 6; ++i) {
     size_t w_off = 0;
     const int kw = i == 6 ? w3 : 3;        // conv6: kernel (3, pool_3[1]), padding (1, 0) (lib:674-678)
-    if (!pack_conv(P, i, cc[i - 1], cc[i], &e->act_exp[i], &w_off, kw)) return false;
-    if (i >= 2) pack_conv_tc(P, i, cc[i - 1], cc[i], w_off, e->act_exp[i - 1], &e->tc_scale[i], 3 * kw);
+    if (!pack_conv(P, i, cc[i - 1], cc[i], &ex[i], &w_off, kw)) return false;
+    if (i >= 2) pack_conv_tc(P, i, cc[i - 1], cc[i], w_off, ex[i - 1], ex[i], &e->tc_scale[i], 3 * kw);
   }
   if (c.cnn_fc > 0) {
     // AdaptCNN's optional Linear (lib:682-684, 708-709): k-major, rows in the engine's feature order h*c3 + c, zero rows
@@ -1512,23 +1549,22 @@ int conv_layers(Pass& p) {
   };
   if (fused12) {
     Scope s(e, "conv12");
-    launch_conv12(p.st, p.std_mode, cc[2], LN.mel.as<float>(), p.seg_frame0, p.seg_thr, w.conv[1].w, w.conv[1].b,
-                  e->act_store(1), w.conv[2].wtc, w.conv[2].b, e->tc_scale[2], e->act_store(2),
-                  plane_hi(3), plane_lo(3), p.n_seg);
+    launch_conv12(p.st, p.std_mode, cc[2], LN.mel.as<float>(), p.seg_frame0, p.seg_thr, w.conv[1].w_split,
+                  w.conv[1].b_split, w.conv[2].wtc, w.conv[2].b_split, e->tc_scale[2], plane_hi(3), plane_lo(3), p.n_seg);
   } else {
     Scope s(e, "conv1");
     if (!launch_conv1(p.st, p.std_mode, cc[1], LN.mel.as<float>(), p.c.n_mels, p.c.seg_len, p.seg_frame0, p.seg_thr,
-                      w.conv[1].w, w.conv[1].b, split ? nullptr : LN.act[2].as<float>(), p.n_seg,
-                      split ? plane_hi(2) : nullptr, split ? plane_lo(2) : nullptr, e->act_store(1), w.pools.p[0],
-                      w.pools.p[1]))
+                      split ? w.conv[1].w_split : w.conv[1].w, split ? w.conv[1].b_split : w.conv[1].b,
+                      split ? nullptr : LN.act[2].as<float>(), p.n_seg, split ? plane_hi(2) : nullptr,
+                      split ? plane_lo(2) : nullptr, w.pools.p[0], w.pools.p[1]))
       return no_kernel(1);
   }
   static const char* const names[7] = {"", "", "conv2", "conv3", "conv4", "conv5", "conv6"};
   for (int l = fused12 ? 3 : 2; l <= 6; ++l) {
     Scope s(e, names[l]);
     if (split) {
-      if (!launch_conv_split(p.st, p.std_mode, l, cc[l - 1], cc[l], plane_hi(l), plane_lo(l), w.conv[l].wtc, w.conv[l].b,
-                             e->tc_scale[l], e->act_store(l), l < 6 ? plane_hi(l + 1) : nullptr,
+      if (!launch_conv_split(p.st, p.std_mode, l, cc[l - 1], cc[l], plane_hi(l), plane_lo(l), w.conv[l].wtc, w.conv[l].b_split,
+                             e->tc_scale[l], w.conv[l].unit, l < 6 ? plane_hi(l + 1) : nullptr,
                              l < 6 ? plane_lo(l + 1) : nullptr, l == 6 ? LN.feats.as<float>() : nullptr, p.n_seg, w.pools))
         return no_kernel(l);
     } else {
@@ -3420,7 +3456,7 @@ int64_t nisqa_stage_dump(nisqa_engine* e, int stage, float* out, int64_t cap) {
     if (from_planes) {
       CK(LN.act[layer].reserve((size_t)count * 4));
       launch_unsplit(st, std_mode, layer, ch, LN.planes[layer].as<char>(), LN.planes[layer].as<char>() + LN.plane_bytes[layer],
-                     ldexpf(1.f, e->act_exp[layer - 1]), LN.act[layer].as<float>(), (int)ns, e->w.pools);
+                     e->w.conv[layer - 1].unit, LN.act[layer].as<float>(), (int)ns, e->w.pools);
       src = LN.act[layer].as<float>();
     }
     CK(e->dump.reserve((size_t)count * 4));

@@ -140,10 +140,11 @@ void launch_mel_dump(cudaStream_t st, const float* mel, const ClipDesc* clips, i
 // ---------------------------------------------------------------- cnn.cu (fp32 FFMA convolutions)
 // conv1 + pool1 of segments of n_mels x seg_len mel cells (rows n_mels floats apart): AdaptCNN any accepted shape ->
 // ph x pw (cnn_pool_1), StandardCNN 48 x 15 only -> 24 x 8.  c1 output channels: 16, 32 or 64 into the planes (out_hi),
-// 16 into fp32 `out`.  false: no instance for the shape.
+// 16 into fp32 `out`.  The planes hold what w1, b1 give (the tensor-core path passes them with 2^-e_c folded into
+// channel c).  false: no instance for the shape.
 bool launch_conv1(cudaStream_t st, int std_mode, int c1, const float* mel, int n_mels, int seg_len, const int* seg_frame0,
                   const float* seg_thr, const float* w1, const float* b1, float* out, int n_seg, void* out_hi, void* out_lo,
-                  float store_scale, int ph, int pw);
+                  int ph, int pw);
 void launch_conv_layer(cudaStream_t st, int std_mode, int layer, const float* in, const float* w, const float* b, float* out,
                        int n_seg);
 // rows of `ld` floats (>= hw * ch)
@@ -153,18 +154,19 @@ void launch_nhwc_to_nchw(cudaStream_t st, const float* in, int ld, float* out, l
 size_t split_plane_bytes(int std_mode, int layer, int C, int n_seg, const CnnPools& pools);
 // AdaptCNN conv2..conv6 take cin, cout in {16, 32, 64} (the pairs cnn_c_out_1/2/3 reach) and any accepted pools;
 // StandardCNN its shipped ones.  The fp32 features of conv6 go out in rows of (h3 cout + 63) / 64 * 64 floats (AdaptCNN),
-// zero-padded.
+// zero-padded, channel c times out_unit[c] (2^e_c: the activation scale folded into conv6's weights and bias).
 bool conv_split_supported(int cin, int cout);
 bool launch_conv_split(cudaStream_t st, int std_mode, int layer, int cin, int cout, const void* in_hi, const void* in_lo,
-                       const void* wtc, const float* b, float out_scale, float store_scale, void* out_hi, void* out_lo,
+                       const void* wtc, const float* b, float out_scale, const float* out_unit, void* out_hi, void* out_lo,
                        float* out_f32, int n_seg, const CnnPools& pools);
 // the fused conv1 + conv2 kernel: 48 x 15 segments, c1 = 16, c2 = 32 (AdaptCNN also 16)
 bool conv12_supported(int std_mode, int c1, int c2);
 void launch_conv12(cudaStream_t st, int std_mode, int c2, const float* mel, const int* seg_frame0, const float* seg_thr,
-                   const float* w1, const float* b1, float c1_scale, const void* wtc2, const float* bias2, float scale2,
-                   float store_scale, void* out_hi, void* out_lo, int n_seg);
-void launch_unsplit(cudaStream_t st, int std_mode, int layer, int C, const void* hi, const void* lo, float unit, float* out,
-                    int n_seg, const CnnPools& pools);
+                   const float* w1, const float* b1, const void* wtc2, const float* bias2, float scale2, void* out_hi,
+                   void* out_lo, int n_seg);
+// planes -> fp32 channels-last, channel c times unit[c] (2^e_c)
+void launch_unsplit(cudaStream_t st, int std_mode, int layer, int C, const void* hi, const void* lo, const float* unit,
+                    float* out, int n_seg, const CnnPools& pools);
 
 // ---------------------------------------------------------------- td.cu (fc_out, BiLSTM, pooling)
 void launch_fc20(cudaStream_t st, const float* feats, const float* WT, const float* b, float* out, int n_rows);

@@ -108,18 +108,19 @@ template <> __device__ __forceinline__ void wgmma_rs<64>(float* d, const uint32_
 }
 
 
-// two-term fp16 split of 8 consecutive channels, each multiplied by s = 2^-e (the layer's activation scale,
-// pack_weights) -> two 16-byte rows.  hi + lo keeps 22 significant bits of x s while 2^-3 <= x s <= 60000; below
-// 2^-3 lo is subnormal (absolute error <= 2^-25), above 60000 the value is clamped.  With e chosen from the folded
-// BatchNorm (E = max_c |beta_c| + 3 |gamma_c| maps to [2.8, 5.7)) that is 1e4 times the BN output estimate.
+// two-term fp16 split of 8 consecutive channels -> two 16-byte rows.  hi + lo keeps 22 significant bits of x while
+// 2^-3 <= x <= 60000; below 2^-3 lo is subnormal (absolute error <= 2^-25), above 60000 the value is clamped.  The
+// producing layer's weights and bias carry 2^-e_c for each output channel c (pack_weights), with e_c chosen from that
+// channel's folded BatchNorm (E_c = |beta_c| + 3 |gamma_c| maps to [2.8, 5.7)), so x is the channel's value times 2^-e_c
+// and the window is 1e4 times the channel's own BN output estimate, whatever the other channels' ranges.
 // split4: the same for 4 consecutive channels (one 8-byte half of a row chunk); split8 is two of them.
-__device__ __forceinline__ void split4(const float4& a, float s, uint2& hi, uint2& lo) {
+__device__ __forceinline__ void split4(const float4& a, uint2& hi, uint2& lo) {
   const float x[4] = {a.x, a.y, a.z, a.w};
   uint32_t h[2], l[2];
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
-    // post-ReLU inputs (>= 0); x * 2^-e is exact
-    const float x0 = fminf(x[2 * i] * s, 60000.f), x1 = fminf(x[2 * i + 1] * s, 60000.f);
+    // post-ReLU inputs (>= 0)
+    const float x0 = fminf(x[2 * i], 60000.f), x1 = fminf(x[2 * i + 1], 60000.f);
     const __half h0 = __float2half_rn(x0), h1 = __float2half_rn(x1);
     const __half l0 = __float2half_rn(x0 - __half2float(h0)), l1 = __float2half_rn(x1 - __half2float(h1));
     h[i] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
@@ -128,10 +129,10 @@ __device__ __forceinline__ void split4(const float4& a, float s, uint2& hi, uint
   hi = make_uint2(h[0], h[1]);
   lo = make_uint2(l[0], l[1]);
 }
-__device__ __forceinline__ void split8(const float4& a, const float4& b, float s, uint4& hi, uint4& lo) {
+__device__ __forceinline__ void split8(const float4& a, const float4& b, uint4& hi, uint4& lo) {
   uint2 ha, la, hb, lb;
-  split4(a, s, ha, la);
-  split4(b, s, hb, lb);
+  split4(a, ha, la);
+  split4(b, hb, lb);
   hi = make_uint4(ha.x, ha.y, hb.x, hb.y);
   lo = make_uint4(la.x, la.y, lb.x, lb.y);
 }

@@ -12,7 +12,8 @@ against torch's conv2d on the CPU:
 No GPU and no library call: this pins the layout contract the CUDA kernels implement (their numerical parity is
 tests/test_gpu_parity.py's and tests/test_gpu_layers.py's job).  The last tests run the per-stage float64 checker of
 tests/test_gpu_layers.py on this emulation: it passes the correct three-term split and catches each of three
-plausible kernel faults.
+plausible kernel faults; and it fails a split with one activation exponent per layer on a checkpoint whose channels
+lie far apart, which one exponent per channel stores exactly as the unscaled checkpoint.
 """
 import numpy as np
 import pytest
@@ -42,8 +43,9 @@ def swz(off, rowb):
 
 
 def split(x, e=0):
-    """split8 of csrc/tc_ptx.cuh with the layer's activation exponent e: x >= 0 -> (hi, lo) fp16 with
-    hi + lo == x 2^-e to 2^-22 (values of x 2^-e in [2^-3, 60000]; the product with 2^-e is exact)."""
+    """split8 of csrc/tc_ptx.cuh of x 2^-e: x >= 0 -> (hi, lo) fp16 with hi + lo == x 2^-e to 2^-22 (values of x 2^-e
+    in [2^-3, 60000]; the product with 2^-e is exact).  e is one exponent, or one per channel (the last axis of x): the
+    engine folds each channel's 2^-e into the producing layer's weights, so the kernels split x 2^-e as it comes."""
     x = np.minimum(np.ldexp(x.astype(np.float32), -e).astype(np.float32), np.float32(60000.0))
     hi = x.astype(np.float16)
     lo = (x - hi.astype(np.float32)).astype(np.float16)
@@ -224,6 +226,51 @@ def test_split_is_invariant_under_power_of_two_rescaling():
         back = np.ldexp(h2.astype(np.float64) + l2.astype(np.float64), k)
         big = x >= 0.125
         assert np.all(np.abs(back - np.ldexp(x, k).astype(np.float64))[big] <= 2.0 ** -22 * np.ldexp(x, k)[big])
+
+
+def _exponent(E):
+    """pack_conv's activation exponent ilogb(E sqrt(2) / 4) of the BatchNorm estimate E = |beta| + 3 |gamma|"""
+    return np.frexp(np.asarray(E, np.float64) * np.sqrt(2.0) / 4.0)[1] - 1
+
+
+def test_one_exponent_per_channel_keeps_a_rescaled_channel_that_one_per_layer_loses():
+    """pool2 of nisqa.tar with three channels of BatchNorm 2 scaled by 2^-k (conv3's inputs by 2^k: the same network),
+    split and read back, against tests/stage_ref.py's bound of that stage.  With one exponent per layer, taken from the
+    layer's largest channel, the scaled channels sit below 2^-3 where lo is subnormal, and at k = 12 the stored values
+    are outside the bound.  With one exponent per channel the planes are the unscaled planes bit for bit."""
+    import os
+
+    import stage_ref as R
+    from conftest import WEIGHTS
+    from nisqa_b200 import synth
+    from oracle import nisqa_oracle as O
+    from rescale import rescale_channels
+    args, sd = O.load_checkpoint(os.path.join(WEIGHTS, "nisqa.tar"))
+    taps = {}
+    O.forward_from_mel(args, sd, O.mel_db(synth.synth_speech_f32(77, 2.0, 16000), 16000, args), taps)
+    pool1 = taps["pool1"].double()
+
+    def planes(sdk, per_channel):
+        y, bound = R.conv_layer(sdk, args, 2, pool1)
+        E = (sdk["cnn.model.bn2.bias"].double().abs() + 3 * sdk["cnn.model.bn2.weight"].double().abs()).numpy()
+        e = _exponent(E) if per_channel else _exponent(E.max())
+        hi, lo = split(y.permute(0, 2, 3, 1).float().numpy(), e)
+        back = np.ldexp(hi.astype(np.float32) + lo.astype(np.float32), e)         # the sum and the scale are exact
+        return hi, lo, R.ratio(torch.from_numpy(back).permute(0, 3, 1, 2), y, bound)
+
+    hi0, lo0, r0 = planes(sd, True)
+    ratios = {}
+    for k in (0, 6, 12):
+        ks = np.zeros(32, np.int64)
+        ks[[3, 11, 27]] = -k
+        sdk = rescale_channels(sd, 2, ks)
+        _, _, ratios[k] = planes(sdk, False)
+        hi, lo, r = planes(sdk, True)
+        np.testing.assert_array_equal(hi.view(np.uint16), hi0.view(np.uint16), err_msg=str(k))
+        np.testing.assert_array_equal(lo.view(np.uint16), lo0.view(np.uint16), err_msg=str(k))
+        assert r == r0 <= 1.0
+    print("one exponent per layer, max |got - ref| / bound at 2^-k:", ratios, "; one per channel:", r0)
+    assert ratios[0] <= 1.0 and ratios[12] > 1.0, ratios
 
 
 def _plane_conv(x, wgt, bias, g, fault=None):

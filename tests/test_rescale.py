@@ -1,9 +1,10 @@
 """Checkpoints rescaled by powers of two (tests/rescale.py) compute the same function.
 
 The oracle pins the premise on the CPU: its scores are bit-identical for every conv layer and k = +-12, +-24.  The
-engine stores activations and weights as fp16 pairs with a per-layer power-of-two scale chosen from the folded
-BatchNorm and the weights (pack_weights), so its scores must be bit-identical too - on every conv path - and within
-the usual 1e-4 of the oracle.  A fixed fp16 range would clamp or lose the lo half instead.
+engine stores activations as fp16 pairs with a power-of-two scale per channel, chosen from that channel's folded
+BatchNorm, and weights with one per layer, chosen from the weights (pack_weights), so its scores must be bit-identical
+too - on every conv path - and within the usual 1e-4 of the oracle.  A fixed fp16 range would clamp or lose the lo half
+instead.  tests/test_channel_rescale.py rescales channel by channel.
 """
 import os
 
